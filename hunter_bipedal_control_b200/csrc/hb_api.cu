@@ -1033,34 +1033,31 @@ struct hb_ctx {
   hb_wbc_settings wbc;       // WBC gains / limits / weights in force (task.info values by default; hb_wbc_set_settings, hb_load_task_info)
   int device;
   cudaStream_t stream;
-  cudaStream_t stream_main, stream_aux;   // the host-pointer control step pipelines two half-batches over these
+  cudaStream_t stream_main, stream_aux;   // the chunked host-pointer calls pipeline their chunks over these
   int base;                               // instance offset into the per-instance scratch (chunked calls)
   int64_t launches;
   // MPC scratch
   double *dxt, *dut, *perf;
   double *lin, *proj, *rk;   // node records of the SQP pipeline (K0 -> K1 -> K2/K3)
   int32_t* flags;
-  // WBC scratch
-  double *xdes, *udes, *wsol;
+  // WBC scratch: the control step's desired state / input / mode, the fused WBC's status and iterations when the caller passes none
+  double *xdes, *udes;
   int32_t *wstatus, *witers, *wmode;
-  // staging for host-pointer calls
-  double *s_x0, *s_xref, *s_swing, *s_xt, *s_ut, *s_rbd, *s_xd, *s_ud, *s_sol, *s_tau, *s_t0, *s_misc;
-  double *res_xt = nullptr, *res_ut = nullptr, *res_t0 = nullptr;   // resident primal solution (hb_resident_cycle_batch)
-  double *s_tk = nullptr, *res_tk = nullptr; int32_t *s_nn = nullptr, *res_nn = nullptr;   // node times / interval counts (event-node grids)
-  unsigned long long* h_refstat = nullptr; unsigned long long* d_refstat = nullptr; int refstat_cap = 0;   // per chunk: {invalid structs, words read} of the pinned gather
-  double* h_pack = nullptr; double* d_pack = nullptr; size_t pack_cap = 0;   // packed reference stream: pinned host staging + device copy (words)
-  double* hoqp_scratch = nullptr; hb_hoqp_problem* hoqp_prob = nullptr;   // hierarchical WBC (allocated by its first call)
-  int32_t* res_mode = nullptr;                                      // node modes of the resident solution (policy evaluation between MPC solves)
-  int res_valid = 0;                                                // number of instances holding a previous solution
-  hb_plan_input* s_plan = nullptr; double* res_stance = nullptr; int32_t* s_pstatus = nullptr;   // device planner (row N1)
-  double* res_sol = nullptr; int res_sol_valid = 0;   // last good WBC solution per instance (WeightedWbc fallback, W5)
-  hb_kf_state* s_kf = nullptr;                                                                  // estimator staging (row N3)
-  int32_t *s_mode, *s_imode, *s_status, *s_iters;
-  uint8_t* s_stance;
-  hb_solve_info* s_info;
-  hb_reference* s_refs;
-  double *s_qpH, *s_qpA;   // generic QP staging (sized on demand)
-  size_t s_qp_cap;
+  double* hoqp_scratch; hb_hoqp_problem* hoqp_prob;   // hierarchical WBC (allocated by its first call)
+  // hb_resident_cycle_batch_dev: references expanded over the horizon and, with event_nodes, the node grid they are expanded on
+  double *cyc_xref, *cyc_swing, *cyc_tk;
+  int32_t *cyc_mode, *cyc_nn;
+  // resident primal solution (hb_resident_cycle_batch): solve time, trajectories, node modes (policy evaluation between MPC solves),
+  // node times / interval counts (event-node grids)
+  double *res_t0, *res_xt, *res_ut, *res_tk;
+  int32_t *res_mode, *res_nn;
+  int res_valid;                      // number of instances holding a previous solution
+  double* res_sol; int res_sol_valid;   // last good WBC solution per instance (WeightedWbc fallback, W5)
+  double* res_stance;                 // the device planner's latest stance positions (row N1)
+  // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
+  // hb_resident_cycle_batch's packed references / reference verdicts
+  void* arena; size_t arena_cap;
+  void* pinned; size_t pinned_cap;
   int last_cuda;
   size_t last_h2d_bytes;     // bytes of packed references uploaded by the last hb_resident_cycle_batch
   // optional per-kernel event timing (hb_profile_enable / hb_profile_read)
@@ -1080,9 +1077,7 @@ enum { HB_OK = 0, HB_EINVAL = -1, HB_ECUDA = -2, HB_ENOMEM = -3, HB_ECAP = -4, H
   } while (0)
 
 constexpr int PROF_MAX = 4096;
-enum { K_BACKWARD = 0, K_FORWARD_LS = 1, K_WBC_ASSEMBLE = 2, K_QP = 3, K_OTHER = 4, K_LIN = 5, K_LQ = 6, K_NKINDS = 7 };
-inline void prof_begin(hb_ctx* ctx, int kind);
-inline void prof_end(hb_ctx* ctx);
+enum { K_UNPROFILED = -1, K_BACKWARD = 0, K_FORWARD_LS = 1, K_WBC_ASSEMBLE = 2, K_QP = 3, K_OTHER = 4, K_LIN = 5, K_LQ = 6, K_NKINDS = 7 };
 
 template <class T> cudaError_t dalloc(T** p, size_t n) { return cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)); }
 
@@ -1093,7 +1088,131 @@ inline void prof_end(hb_ctx* ctx) {
   if (ctx->prof_on && ctx->prof_n < PROF_MAX) { cudaEventRecord(ctx->prof_ev[2 * ctx->prof_n + 1], ctx->stream); ctx->prof_n++; }
 }
 
+// One kernel launch on ctx->stream: counted (hb_launch_count), timed under `kind` when profiling is on (K_UNPROFILED: never), launch
+// error checked.
+template <class... P, class... A>
+int launch(hb_ctx* ctx, int kind, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, A&&... args) {
+  if (kind != K_UNPROFILED) prof_begin(ctx, kind);
+  kernel<<<grid, block, smem, ctx->stream>>>(std::forward<A>(args)...);
+  if (kind != K_UNPROFILED) prof_end(ctx);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  return HB_OK;
+}
+
 int set_device(hb_ctx* ctx) { return cudaSetDevice(ctx->device) == cudaSuccess ? HB_OK : HB_ECUDA; }
+
+// The growth policy of the context's on-demand buffers (the staging arena, the pinned host buffer): grow only, to 5/4 of the request so
+// that a packed reference stream a little longer than the last one does not reallocate, contents not kept. Every host-pointer call waits
+// for its copies before it returns, so no copy still reads the buffer that is freed.
+int grow(hb_ctx* ctx, void** buf, size_t* cap, size_t bytes, bool pinned_host) {
+  if (bytes <= *cap) return HB_OK;
+  if (*buf) { if (pinned_host) cudaFreeHost(*buf); else cudaFree(*buf); }
+  *buf = nullptr; *cap = 0;
+  const size_t want = bytes + bytes / 4;
+  const cudaError_t e = pinned_host ? cudaHostAlloc(buf, want, cudaHostAllocDefault) : cudaMalloc(buf, want);
+  if (e != cudaSuccess) { *buf = nullptr; ctx->last_cuda = (int)e; cudaGetLastError(); return HB_ENOMEM; }
+  *cap = want;
+  return HB_OK;
+}
+
+// Device side of one staged argument. Converts to its device pointer once Staging::reserve has placed it (null for a null pass-through
+// argument); at(i) points at instance i (element i of a buf slice).
+template <class T> struct Dev {
+  void* const* p;
+  size_t per;
+  operator T*() const { return static_cast<T*>(*p); }
+  T* at(size_t i) const { return static_cast<T*>(*p) + i * per; }
+};
+
+// Staging of one host-pointer call. The call declares its host arguments with their elements per instance; reserve() then places all of
+// them in the context's device arena (grown on demand, freed by hb_destroy) before any copy is enqueued, and h2d / d2h copy instances
+// [lo, hi) of every argument on ctx->stream. Slices start on 256-byte boundaries, as separate cudaMalloc's would.
+//   in / inout   copied in (inout: and back)
+//   out          the device always gets a buffer; copied back only when the caller passed a host pointer
+//   *_or_null    a null host pointer stays a null device pointer
+//   tmp / buf    device only: per instance (tmp) or n elements for the whole call (buf)
+class Staging {
+ public:
+  Staging(hb_ctx* ctx, int B) : ctx_(ctx), B_((size_t)B) {}
+  template <class T> Dev<const T> in(const T* h, size_t per) { return add<const T>(h, nullptr, per, B_, true); }
+  template <class T> Dev<T> inout(T* h, size_t per) { return add<T>(h, h, per, B_, true); }
+  template <class T> Dev<T> out(T* h, size_t per) { return add<T>(nullptr, h, per, B_, true); }
+  template <class T> Dev<const T> in_or_null(const T* h, size_t per) { return add<const T>(h, nullptr, per, B_, h != nullptr); }
+  template <class T> Dev<T> inout_or_null(T* h, size_t per) { return add<T>(h, h, per, B_, h != nullptr); }
+  template <class T> Dev<T> tmp(size_t per) { return add<T>(nullptr, nullptr, per, B_, true); }
+  template <class T> Dev<T> buf(size_t n) { Dev<T> d = add<T>(nullptr, nullptr, n, 1, true); d.per = 1; return d; }
+
+  int reserve() {
+    size_t total = 0;
+    for (int k = 0; k < n_; ++k) if (s_[k].used) { s_[k].off = total; total += (s_[k].bytes * s_[k].count + 255) & ~(size_t)255; }
+    const int rc = grow(ctx_, &ctx_->arena, &ctx_->arena_cap, total, false);
+    if (rc) return rc;
+    for (int k = 0; k < n_; ++k) if (s_[k].used) s_[k].dev = static_cast<char*>(ctx_->arena) + s_[k].off;
+    return HB_OK;
+  }
+  int h2d(size_t lo, size_t hi) { return copy(lo, hi, true); }
+  int d2h(size_t lo, size_t hi) { return copy(lo, hi, false); }
+  // the whole batch in one piece: reserve, copy in, call(), copy out, wait
+  template <class F> int run(F&& call) {
+    int rc = reserve();
+    if (!rc) rc = h2d(0, B_);
+    if (!rc) rc = call();
+    if (!rc) rc = d2h(0, B_);
+    if (rc) return rc;
+    hb_ctx* ctx = ctx_;
+    CK(cudaStreamSynchronize(ctx->stream));
+    return HB_OK;
+  }
+
+ private:
+  struct Slot { const void* src; void* dst; size_t bytes, count, off; void* dev; bool used; };
+  template <class T> Dev<T> add(const void* src, void* dst, size_t per, size_t count, bool used) {
+    Slot& s = s_[n_++];
+    s = Slot{src, dst, per * sizeof(T), count, 0, nullptr, used};
+    return Dev<T>{&s.dev, per};
+  }
+  int copy(size_t lo, size_t hi, bool to_dev) {
+    hb_ctx* ctx = ctx_;
+    for (int k = 0; k < n_; ++k) {
+      const Slot& s = s_[k];
+      const size_t off = lo * s.bytes, n = (hi - lo) * s.bytes;
+      if (to_dev && s.src) CK(cudaMemcpyAsync(static_cast<char*>(s.dev) + off, static_cast<const char*>(s.src) + off, n, cudaMemcpyHostToDevice, ctx->stream));
+      if (!to_dev && s.dst) CK(cudaMemcpyAsync(static_cast<char*>(s.dst) + off, static_cast<char*>(s.dev) + off, n, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    return HB_OK;
+  }
+  hb_ctx* ctx_;
+  size_t B_;
+  Slot s_[16];   // the largest call (hb_resident_plan_cycle_batch) declares 11
+  int n_ = 0;
+};
+
+// The pipelined host-pointer calls: chunk c of nchunk covers instances [B c / nchunk, B (c + 1) / nchunk) on stream_main (even c) or
+// stream_aux (odd c), so the copies of one chunk overlap the kernels of the other. ctx->stream / ctx->base point at the chunk while
+// body(c, lo, hi) runs and are restored after the last one; both streams are drained before the first error is returned.
+template <class F> int chunked(hb_ctx* ctx, int B, int nchunk, F&& body) {
+  int rc = HB_OK;
+  for (int c = 0; c < nchunk && rc == HB_OK; ++c) {
+    const size_t lo = (size_t)B * c / nchunk, hi = (size_t)B * (c + 1) / nchunk;
+    ctx->stream = (c % 2 == 0) ? ctx->stream_main : ctx->stream_aux;
+    ctx->base = (int)lo;
+    rc = body(c, lo, hi);
+  }
+  ctx->stream = ctx->stream_main;
+  ctx->base = 0;
+  cudaError_t e1 = cudaStreamSynchronize(ctx->stream_aux), e0 = cudaStreamSynchronize(ctx->stream_main);
+  if (rc) return rc;
+  if (e0 != cudaSuccess || e1 != cudaSuccess) { ctx->last_cuda = (int)(e0 != cudaSuccess ? e0 : e1); return HB_ECUDA; }
+  return HB_OK;
+}
+
+// chunk count of the host-pointer cycles: cfg.e2e_chunks when set (one chunk below 64 instances per chunk), otherwise two from 4096
+// instances on when the call has host work and copies to hide behind the other chunk's kernels (`overlap`)
+int cycle_chunks(const hb_ctx* ctx, int B, bool overlap) {
+  const int c = ctx->cfg.e2e_chunks;
+  return c > 0 ? (B >= 64 * c ? c : 1) : ((overlap && B >= 4096) ? 2 : 1);
+}
 
 // Caller-supplied hb_reference structs (host-pointer entry points): counts within the capacities, monotone times, positive segment
 // lengths, modes in 0..3. The device expansion indexes with these counts, so a malformed struct is rejected here with HB_EINVAL.
@@ -1206,19 +1325,14 @@ int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
   // WBC / QP / planner / estimator entry points never pay for them
   ok = ok && dalloc(&ctx->dxt, B * (N + 1) * NX) == cudaSuccess && dalloc(&ctx->dut, B * N * NU) == cudaSuccess;
   ok = ok && dalloc(&ctx->perf, B * 4) == cudaSuccess && dalloc(&ctx->flags, B) == cudaSuccess;
-  ok = ok && dalloc(&ctx->xdes, B * NX) == cudaSuccess && dalloc(&ctx->udes, B * NU) == cudaSuccess && dalloc(&ctx->wsol, B * NWBC) == cudaSuccess;
+  ok = ok && dalloc(&ctx->xdes, B * NX) == cudaSuccess && dalloc(&ctx->udes, B * NU) == cudaSuccess;
   ok = ok && dalloc(&ctx->wstatus, B) == cudaSuccess && dalloc(&ctx->witers, B) == cudaSuccess && dalloc(&ctx->wmode, B) == cudaSuccess;
-  ok = ok && dalloc(&ctx->s_x0, B * NX) == cudaSuccess && dalloc(&ctx->s_xref, B * (N + 1) * NX) == cudaSuccess && dalloc(&ctx->s_swing, B * (N + 1) * 24) == cudaSuccess;
-  ok = ok && dalloc(&ctx->s_kf, B) == cudaSuccess && dalloc(&ctx->res_sol, B * NWBC) == cudaSuccess;
-  ok = ok && dalloc(&ctx->s_plan, B) == cudaSuccess && dalloc(&ctx->res_stance, B * 12) == cudaSuccess && dalloc(&ctx->s_pstatus, B) == cudaSuccess;
+  ok = ok && dalloc(&ctx->cyc_xref, B * (N + 1) * NX) == cudaSuccess && dalloc(&ctx->cyc_swing, B * (N + 1) * 24) == cudaSuccess;
+  ok = ok && dalloc(&ctx->cyc_mode, B * (N + 1)) == cudaSuccess && dalloc(&ctx->cyc_tk, B * (N + 1)) == cudaSuccess && dalloc(&ctx->cyc_nn, B) == cudaSuccess;
   ok = ok && dalloc(&ctx->res_xt, B * (N + 1) * NX) == cudaSuccess && dalloc(&ctx->res_ut, B * N * NU) == cudaSuccess && dalloc(&ctx->res_t0, B) == cudaSuccess;
-  ok = ok && dalloc(&ctx->res_mode, B * (N + 1)) == cudaSuccess;
-  ok = ok && dalloc(&ctx->s_tk, B * (N + 1)) == cudaSuccess && dalloc(&ctx->res_tk, B * (N + 1)) == cudaSuccess && dalloc(&ctx->s_nn, B) == cudaSuccess && dalloc(&ctx->res_nn, B) == cudaSuccess;
-  ok = ok && dalloc(&ctx->s_xt, B * (N + 1) * NX) == cudaSuccess && dalloc(&ctx->s_ut, B * N * NU) == cudaSuccess && dalloc(&ctx->s_rbd, B * 32) == cudaSuccess;
-  ok = ok && dalloc(&ctx->s_xd, B * NX) == cudaSuccess && dalloc(&ctx->s_ud, B * NU) == cudaSuccess && dalloc(&ctx->s_sol, B * NWBC) == cudaSuccess;
-  ok = ok && dalloc(&ctx->s_tau, B * NJ) == cudaSuccess && dalloc(&ctx->s_t0, B) == cudaSuccess && dalloc(&ctx->s_misc, B * (size_t)(NX + 2 * TS + 24 + 36 * NX)) == cudaSuccess;
-  ok = ok && dalloc(&ctx->s_mode, B * (N + 1)) == cudaSuccess && dalloc(&ctx->s_imode, B) == cudaSuccess && dalloc(&ctx->s_status, B) == cudaSuccess && dalloc(&ctx->s_iters, B) == cudaSuccess;
-  ok = ok && dalloc(&ctx->s_stance, B) == cudaSuccess && dalloc(&ctx->s_info, B) == cudaSuccess && dalloc(&ctx->s_refs, B) == cudaSuccess;
+  ok = ok && dalloc(&ctx->res_mode, B * (N + 1)) == cudaSuccess && dalloc(&ctx->res_tk, B * (N + 1)) == cudaSuccess && dalloc(&ctx->res_nn, B) == cudaSuccess;
+  ok = ok && dalloc(&ctx->res_sol, B * NWBC) == cudaSuccess && dalloc(&ctx->res_stance, B * 12) == cudaSuccess;
+  // host-pointer calls stage through ctx->arena, which the first such call sizes: contexts driven through device pointers never pay for it
   if (!ok) { hb_destroy(ctx); return HB_ENOMEM; }
   {
     cudaError_t fe = cudaSuccess;
@@ -1241,16 +1355,12 @@ int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
 int hb_destroy(hb_ctx* ctx) {
   if (!ctx) return HB_EINVAL;
   cudaSetDevice(ctx->device);
-  void* ptrs[] = {ctx->lin, ctx->proj, ctx->rk, ctx->dxt, ctx->dut, ctx->perf, ctx->flags, ctx->xdes, ctx->udes,
-                  ctx->wsol, ctx->wstatus, ctx->witers, ctx->wmode, ctx->s_x0, ctx->s_xref, ctx->s_swing, ctx->s_xt, ctx->s_ut, ctx->s_rbd, ctx->s_xd,
-                  ctx->s_ud, ctx->s_sol, ctx->s_tau, ctx->s_t0, ctx->s_misc, ctx->s_mode, ctx->s_imode, ctx->s_status, ctx->s_iters, ctx->s_stance,
-                  ctx->s_info, ctx->s_refs, ctx->s_qpH, ctx->s_qpA, ctx->res_xt, ctx->res_ut, ctx->res_t0, ctx->s_plan, ctx->res_stance, ctx->s_pstatus, ctx->s_kf, ctx->res_sol, ctx->s_tk, ctx->res_tk, ctx->s_nn, ctx->res_nn, ctx->res_mode, ctx->hoqp_scratch, ctx->hoqp_prob};
+  void* ptrs[] = {ctx->lin, ctx->proj, ctx->rk, ctx->dxt, ctx->dut, ctx->perf, ctx->flags, ctx->xdes, ctx->udes, ctx->wstatus, ctx->witers, ctx->wmode,
+                  ctx->hoqp_scratch, ctx->hoqp_prob, ctx->cyc_xref, ctx->cyc_swing, ctx->cyc_tk, ctx->cyc_mode, ctx->cyc_nn, ctx->res_t0, ctx->res_xt,
+                  ctx->res_ut, ctx->res_tk, ctx->res_mode, ctx->res_nn, ctx->res_sol, ctx->res_stance, ctx->arena};
   for (void* p : ptrs) if (p) cudaFree(p);
+  if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
-  if (ctx->h_refstat) cudaFreeHost(ctx->h_refstat);
-  if (ctx->d_refstat) cudaFree(ctx->d_refstat);
-  if (ctx->h_pack) cudaFreeHost(ctx->h_pack);
-  if (ctx->d_pack) cudaFree(ctx->d_pack);
   if (ctx->stream_aux) cudaStreamDestroy(ctx->stream_aux);
   if (ctx->stream_main) cudaStreamDestroy(ctx->stream_main);
   else if (ctx->stream) cudaStreamDestroy(ctx->stream);
@@ -1307,13 +1417,8 @@ static int launch_qp(hb_ctx* ctx, int B, int n, int m, const double* H, const do
   if (wpb < 1) return HB_EINVAL;
   if (wpb > 1) wpb = 1;   // one warp per CTA: the shared-memory footprint, not the thread count, bounds residency
   const int blocks = (B + wpb - 1) / wpb;
-  prof_begin(ctx, K_QP);
-  qp_batch_kernel<<<blocks, 32 * wpb, per_warp * wpb, ctx->stream>>>(B, n, m, H, g, A, lbA, ubA, sH, sA, sB, m_per, ctx->cfg.wbc_rho,
-                                                                     ctx->cfg.qp_max_iter, x, status, iters);
-  prof_end(ctx);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_QP, qp_batch_kernel, blocks, 32 * wpb, per_warp * wpb, B, n, m, H, g, A, lbA, ubA, sH, sA, sB, m_per, ctx->cfg.wbc_rho,
+                ctx->cfg.qp_max_iter, x, status, iters);
 }
 
 int hb_wbc_qp_batch_dev(hb_ctx* ctx, int B, int n, int m, const double* H, const double* g, const double* A, const double* lbA,
@@ -1330,14 +1435,8 @@ int hb_wbc_solve_batch_dev(hb_ctx* ctx, int B, const double* x_des, const double
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  const size_t per_warp = wbc_fused_doubles() * sizeof(double);
-  prof_begin(ctx, K_QP);
-  wbc_fused_kernel<<<B, 32, per_warp, ctx->stream>>>(B, ctx->wbc, x_des, u_des, rbd, mode, stance_mode, ctx->cfg.wbc_rho, ctx->cfg.qp_max_iter, sol,
-                                                      status ? status : ctx->wstatus + ctx->base, ctx->witers + ctx->base);
-  prof_end(ctx);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_QP, wbc_fused_kernel, B, 32, wbc_fused_doubles() * sizeof(double), B, ctx->wbc, x_des, u_des, rbd, mode, stance_mode,
+                ctx->cfg.wbc_rho, ctx->cfg.qp_max_iter, sol, status ? status : ctx->wstatus + ctx->base, ctx->witers + ctx->base);
 }
 
 int hb_wbc_assemble_batch_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
@@ -1346,12 +1445,8 @@ int hb_wbc_assemble_batch_dev(hb_ctx* ctx, int B, const double* x_des, const dou
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
   const int wpb = 4;
-  prof_begin(ctx, K_WBC_ASSEMBLE);
-  wbc_assemble_kernel<<<(B + wpb - 1) / wpb, 32 * wpb, sizeof(WbcShared) * wpb, ctx->stream>>>(B, ctx->wbc, x_des, u_des, rbd, mode, stance_mode, H, g, A, lbA, ubA, m_rows);
-  prof_end(ctx);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_WBC_ASSEMBLE, wbc_assemble_kernel, (B + wpb - 1) / wpb, 32 * wpb, sizeof(WbcShared) * wpb, B, ctx->wbc, x_des, u_des, rbd, mode,
+                stance_mode, H, g, A, lbA, ubA, m_rows);
 }
 
 int hb_wbc_qp_rows_batch_dev(hb_ctx* ctx, int B, int n, int m_alloc, const int32_t* m_rows, const double* H, const double* g, const double* A,
@@ -1379,23 +1474,13 @@ int hb_hoqp_solve_batch_dev(hb_ctx* ctx, int B, const hb_hoqp_problem* problems,
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  int rc = hoqp_reserve(ctx);
+  const int rc = hoqp_reserve(ctx);
   if (rc) return rc;
-  prof_begin(ctx, K_QP);
-  hoqp_kernel<<<B, 32, hoqp_smem_bytes(), ctx->stream>>>(B, problems, ctx->hoqp_scratch, 2 * ctx->cfg.qp_max_iter, x, slack, status);
-  prof_end(ctx);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_QP, hoqp_kernel, B, 32, hoqp_smem_bytes(), B, problems, ctx->hoqp_scratch, 2 * ctx->cfg.qp_max_iter, x, slack, status);
 }
 
 static int hwbc_tasks_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, hb_hoqp_problem* problems) {
-  prof_begin(ctx, K_WBC_ASSEMBLE);
-  hwbc_tasks_kernel<<<B, 32, 0, ctx->stream>>>(B, ctx->wbc, x_des, u_des, rbd, mode, problems);
-  prof_end(ctx);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_WBC_ASSEMBLE, hwbc_tasks_kernel, B, 32, 0, B, ctx->wbc, x_des, u_des, rbd, mode, problems);
 }
 
 int hb_hierarchical_wbc_solve_batch_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, double* sol,
@@ -1415,10 +1500,7 @@ int hb_mpc_cold_start_batch_dev(hb_ctx* ctx, int B, const double* x0, const int3
   if (!ctx || B < 0 || !x0 || !mode || !x_traj || !u_traj) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
-  cold_start_kernel<<<B, 128, 0, ctx->stream>>>(B, ctx->cfg.horizon_N, x0, mode, x_traj, u_traj);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, cold_start_kernel, B, 128, 0, B, ctx->cfg.horizon_N, x0, mode, x_traj, u_traj);
 }
 
 static int mpc_solve_impl(hb_ctx* ctx, int B, const double* x0, const double* x_ref, const double* swing_ref, const int32_t* mode,
@@ -1447,27 +1529,11 @@ static int mpc_solve_impl(hb_ctx* ctx, int B, const double* x0, const double* x_
   }
   const int N = a.N, NP = (N + 1) / 2;
   const long long nw = (long long)B * NP;
-  prof_begin(ctx, K_LIN);
-  lin_kernel<<<(unsigned)((nw + 1) / 2), 64, 4 * sizeof(LinHalf) + sizeof(ChainModel), ctx->stream>>>(a);
-  prof_end(ctx);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  prof_begin(ctx, K_LQ);
-  lq_kernel<<<(unsigned)((long long)B * N), 32, sizeof(LqShared), ctx->stream>>>(a);
-  prof_end(ctx);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  prof_begin(ctx, K_BACKWARD);
-  riccati_kernel<<<B, 64, sizeof(RicShared), ctx->stream>>>(a);
-  prof_end(ctx);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  prof_begin(ctx, K_FORWARD_LS);
-  forward_linesearch2_kernel<<<B, 32, sizeof(Fw2Shared), ctx->stream>>>(a, ctx->cfg.line_search_max_trials, info);
-  prof_end(ctx);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  int rc = launch(ctx, K_LIN, lin_kernel, (unsigned)((nw + 1) / 2), 64, 4 * sizeof(LinHalf) + sizeof(ChainModel), a);
+  if (!rc) rc = launch(ctx, K_LQ, lq_kernel, (unsigned)((long long)B * N), 32, sizeof(LqShared), a);
+  if (!rc) rc = launch(ctx, K_BACKWARD, riccati_kernel, B, 64, sizeof(RicShared), a);
+  if (!rc) rc = launch(ctx, K_FORWARD_LS, forward_linesearch2_kernel, B, 32, sizeof(Fw2Shared), a, ctx->cfg.line_search_max_trials, info);
+  return rc;
 }
 
 int hb_mpc_solve_batch_dev(hb_ctx* ctx, int B, const double* x0, const double* x_ref, const double* swing_ref, const int32_t* mode,
@@ -1487,11 +1553,8 @@ static int policy_eval_impl(hb_ctx* ctx, int B, double t_rel, const double* x_tr
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
   const int wpb = 4;
-  policy_eval_kernel<<<(B + wpb - 1) / wpb, 32 * wpb, 0, ctx->stream>>>(B, ctx->cfg.horizon_N, ctx->cfg.dt, t_rel, x_traj, u_traj, mode, x_des, u_des, mode_out,
-                                                                         tk, nn, nullptr, nullptr);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, policy_eval_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, ctx->cfg.horizon_N, ctx->cfg.dt, t_rel, x_traj, u_traj, mode,
+                x_des, u_des, mode_out, tk, nn, nullptr, nullptr);
 }
 
 int hb_policy_eval_batch_dev(hb_ctx* ctx, int B, double t_rel, const double* x_traj, const double* u_traj, const int32_t* mode, double* x_des,
@@ -1510,10 +1573,7 @@ int hb_time_grid_batch_dev(hb_ctx* ctx, int B, const double* t0, const hb_refere
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
   const double T = ctx->cfg.time_horizon > 0.0 ? ctx->cfg.time_horizon : ctx->cfg.horizon_N * ctx->cfg.dt;
-  time_grid_kernel<<<(B + 127) / 128, 128, 0, ctx->stream>>>(B, ctx->cfg.horizon_N, ctx->cfg.dt, T, t0, refs, node_times, n_intervals, status);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, time_grid_kernel, (B + 127) / 128, 128, 0, B, ctx->cfg.horizon_N, ctx->cfg.dt, T, t0, refs, node_times, n_intervals, status);
 }
 
 static int control_step_impl(hb_ctx* ctx, int B, double t_rel, const double* x0, const double* x_ref, const double* swing_ref, const int32_t* mode,
@@ -1527,13 +1587,8 @@ static int control_step_impl(hb_ctx* ctx, int B, double t_rel, const double* x0,
   rc = policy_eval_impl(ctx, B, t_rel, x_traj, u_traj, mode, xdes, udes, wmode, tk, nn);
   if (rc) return rc;
   rc = hb_wbc_solve_batch_dev(ctx, B, xdes, udes, rbd, wmode, nullptr, wbc_sol, wbc_status);
-  if (rc) return rc;
-  if (torque) {
-    torque_kernel<<<(B * NJ + 127) / 128, 128, 0, ctx->stream>>>(B, wbc_sol, torque);
-    ctx->launches++;
-    CK(cudaGetLastError());
-  }
-  return HB_OK;
+  if (!rc && torque) rc = launch(ctx, K_UNPROFILED, torque_kernel, (B * NJ + 127) / 128, 128, 0, B, wbc_sol, torque);
+  return rc;
 }
 
 int hb_control_step_batch_dev(hb_ctx* ctx, int B, double t_rel, const double* x0, const double* x_ref, const double* swing_ref, const int32_t* mode,
@@ -1577,11 +1632,11 @@ int hb_resident_cycle_batch_dev(hb_ctx* ctx, int B, int cold_start, double t_rel
   if (!cold_start && ctx->res_valid < ctx->base + B) return HB_EINVAL;     // no previous solution to shift
   if (set_device(ctx)) return HB_ECUDA;
   const size_t N = ctx->cfg.horizon_N, o = (size_t)ctx->base;
-  double* xref = ctx->s_xref + o * (N + 1) * NX; double* swing = ctx->s_swing + o * (N + 1) * 24; int32_t* mode = ctx->s_mode + o * (N + 1);
+  double* xref = ctx->cyc_xref + o * (N + 1) * NX; double* swing = ctx->cyc_swing + o * (N + 1) * 24; int32_t* mode = ctx->cyc_mode + o * (N + 1);
   double* xt = ctx->res_xt + o * (N + 1) * NX; double* ut = ctx->res_ut + o * N * NU; double* tres = ctx->res_t0 + o;
   // event-node grids (cfg.event_nodes): per-instance node times, kept resident beside the primal solution
   const bool grid = ctx->cfg.event_nodes != 0;
-  double* tk = grid ? ctx->s_tk + o * (N + 1) : nullptr; int32_t* nn = grid ? ctx->s_nn + o : nullptr;
+  double* tk = grid ? ctx->cyc_tk + o * (N + 1) : nullptr; int32_t* nn = grid ? ctx->cyc_nn + o : nullptr;
   double* tkres = grid ? ctx->res_tk + o * (N + 1) : nullptr; int32_t* nnres = grid ? ctx->res_nn + o : nullptr;
   int rc = HB_OK;
   if (grid) {
@@ -1594,23 +1649,20 @@ int hb_resident_cycle_batch_dev(hb_ctx* ctx, int B, int cold_start, double t_rel
   if (rc) return rc;
   if (cold_start) {
     rc = hb_mpc_cold_start_batch_dev(ctx, B, x0, mode, xt, ut);
-    if (rc) return rc;
-    set_times_kernel<<<(B + 127) / 128, 128, 0, ctx->stream>>>(B, (int)N, t0, tres, tk, nn, tkres, nnres);
+    if (!rc) rc = launch(ctx, K_UNPROFILED, set_times_kernel, (B + 127) / 128, 128, 0, B, (int)N, t0, tres, tk, nn, tkres, nnres);
   } else {
     const size_t smem = sizeof(double) * ((N + 1) * NX + N * NU);     // opted in at hb_create
-    warm_shift_kernel<<<B, 128, smem, ctx->stream>>>(B, (int)N, ctx->cfg.dt, t0, tres, x0, mode, xt, ut, tk, nn, tkres, nnres);
+    rc = launch(ctx, K_UNPROFILED, warm_shift_kernel, B, 128, smem, B, (int)N, ctx->cfg.dt, t0, tres, x0, mode, xt, ut, tk, nn, tkres, nnres);
   }
-  ctx->launches++;
-  CK(cudaGetLastError());
+  if (rc) return rc;
   CK(cudaMemcpyAsync(ctx->res_mode + o * (N + 1), mode, sizeof(int32_t) * B * (N + 1), cudaMemcpyDeviceToDevice, ctx->stream));
   if (ctx->res_valid < ctx->base + B) ctx->res_valid = ctx->base + B;
   rc = control_step_impl(ctx, B, t_rel, x0, xref, swing, mode, rbd, xt, ut, info, wbc_sol, torque, wbc_status, tk, nn);
   if (rc) return rc;
   if (wbc_status) {
     const int have_prev = (!cold_start && ctx->res_sol_valid >= ctx->base + B) ? 1 : 0;
-    wbc_fallback_kernel<<<(B * NWBC + 127) / 128, 128, 0, ctx->stream>>>(B, have_prev, wbc_status, wbc_sol, ctx->res_sol + o * NWBC, torque);
-    ctx->launches++;
-    CK(cudaGetLastError());
+    rc = launch(ctx, K_UNPROFILED, wbc_fallback_kernel, (B * NWBC + 127) / 128, 128, 0, B, have_prev, wbc_status, wbc_sol, ctx->res_sol + o * NWBC, torque);
+    if (rc) return rc;
     if (ctx->res_sol_valid < ctx->base + B) ctx->res_sol_valid = ctx->base + B;
   }
   return HB_OK;
@@ -1622,10 +1674,7 @@ int hb_plan_references_batch_dev(hb_ctx* ctx, int B, const hb_plan_input* in, co
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
   static const hbplan::PlanConsts pc = hbplan::make_consts();
-  plan_references_coop_kernel<<<(B + 7) / 8, 32, 0, ctx->stream>>>(B, in, feet, latest_stance, out, status, pc);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, plan_references_coop_kernel, (B + 7) / 8, 32, 0, B, in, feet, latest_stance, out, status, pc);
 }
 
 int hb_default_kf_params(hb_kf_params* p) {
@@ -1650,11 +1699,8 @@ int hb_estimator_update_batch_dev(hb_ctx* ctx, int B, const hb_kf_params* params
   if (!ctx || B < 0 || !params || !state || !quat || !ang_vel_local || !lin_acc_local || !joint_pos || !joint_vel || !contact_flag || !rbd_out) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
-  kf_update_kernel<<<B, 32, sizeof(KfShared), ctx->stream>>>(B, *params, dt, state, quat, ang_vel_local, lin_acc_local, joint_pos, joint_vel, contact_flag,
-                                                            rbd_out);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, kf_update_kernel, B, 32, sizeof(KfShared), B, *params, dt, state, quat, ang_vel_local, lin_acc_local, joint_pos,
+                joint_vel, contact_flag, rbd_out);
 }
 
 int hb_default_wbc_settings(hb_wbc_settings* s) {
@@ -1805,20 +1851,14 @@ int hb_actuation_batch_dev(hb_ctx* ctx, int B, double delay, const double* time,
   if (!ctx || B < 0 || !time || !state || !command || !rbd || !tau || delay < 0.0) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
-  actuation_kernel<<<(B + 63) / 64, 64, 0, ctx->stream>>>(B, delay, time, state, command, rbd, tau);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, actuation_kernel, (B + 63) / 64, 64, 0, B, delay, time, state, command, rbd, tau);
 }
 
 int hb_sim_step_batch_dev(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {
   if (!ctx || B < 0 || !params || !rbd || !tau || !(params->dt > 0.0) || params->substeps < 1 || params->substeps > 1000) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
-  sim_step_kernel<<<B, 32, 0, ctx->stream>>>(B, *params, rbd, tau, contact_force, contact_flag);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, *params, rbd, tau, contact_force, contact_flag);
 }
 
 int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
@@ -1830,23 +1870,16 @@ int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const dou
   const size_t N = ctx->cfg.horizon_N, o = (size_t)ctx->base;
   const bool grid = ctx->cfg.event_nodes != 0;
   const int wpb = 4;
-  policy_eval_kernel<<<(B + wpb - 1) / wpb, 32 * wpb, 0, ctx->stream>>>(B, (int)N, ctx->cfg.dt, 0.0, ctx->res_xt + o * (N + 1) * NX, ctx->res_ut + o * N * NU,
-                                                                         ctx->res_mode + o * (N + 1), x_des, u_des, mode_out, grid ? ctx->res_tk + o * (N + 1) : nullptr,
-                                                                         grid ? ctx->res_nn + o : nullptr, t_now, ctx->res_t0 + o);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  int rc = hb_wbc_solve_batch_dev(ctx, B, x_des, u_des, rbd, mode_out, stance_mode, wbc_sol, wbc_status);
+  int rc = launch(ctx, K_UNPROFILED, policy_eval_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, (int)N, ctx->cfg.dt, 0.0, ctx->res_xt + o * (N + 1) * NX,
+                  ctx->res_ut + o * N * NU, ctx->res_mode + o * (N + 1), x_des, u_des, mode_out, grid ? ctx->res_tk + o * (N + 1) : nullptr,
+                  grid ? ctx->res_nn + o : nullptr, t_now, ctx->res_t0 + o);
+  if (!rc) rc = hb_wbc_solve_batch_dev(ctx, B, x_des, u_des, rbd, mode_out, stance_mode, wbc_sol, wbc_status);
+  if (!rc && torque) rc = launch(ctx, K_UNPROFILED, torque_kernel, (B * NJ + 127) / 128, 128, 0, B, wbc_sol, torque);
   if (rc) return rc;
-  if (torque) {
-    torque_kernel<<<(B * NJ + 127) / 128, 128, 0, ctx->stream>>>(B, wbc_sol, torque);
-    ctx->launches++;
-    CK(cudaGetLastError());
-  }
   if (wbc_status) {
     const int have_prev = (ctx->res_sol_valid >= ctx->base + B) ? 1 : 0;
-    wbc_fallback_kernel<<<(B * NWBC + 127) / 128, 128, 0, ctx->stream>>>(B, have_prev, wbc_status, wbc_sol, ctx->res_sol + o * NWBC, torque);
-    ctx->launches++;
-    CK(cudaGetLastError());
+    rc = launch(ctx, K_UNPROFILED, wbc_fallback_kernel, (B * NWBC + 127) / 128, 128, 0, B, have_prev, wbc_status, wbc_sol, ctx->res_sol + o * NWBC, torque);
+    if (rc) return rc;
     if (ctx->res_sol_valid < ctx->base + B) ctx->res_sol_valid = ctx->base + B;
   }
   return HB_OK;
@@ -1863,10 +1896,7 @@ int hb_contact_force_estimate_batch_dev(hb_ctx* ctx, int B, double cutoff_freque
   if (!ctx || B < 0 || !state || !rbd || !tau_cmd || !est_contact_force || !(cutoff_frequency > 0.0) || !(dt > 0.0)) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
-  contact_force_kernel<<<B, 32, 0, ctx->stream>>>(B, cutoff_frequency, dt, state, rbd, tau_cmd, est_contact_force, disturbance_torque);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, contact_force_kernel, B, 32, 0, B, cutoff_frequency, dt, state, rbd, tau_cmd, est_contact_force, disturbance_torque);
 }
 
 int hb_default_pd_gains(hb_pd_gains* g) {
@@ -1884,31 +1914,22 @@ int hb_joint_command_batch_dev(hb_ctx* ctx, int B, const hb_pd_gains* gains, dou
   if (!ctx || B < 0 || !gains || !x_des || !u_des || !wbc_sol || !mode_cmd || !rbd || !command || !output_torque) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
-  joint_command_kernel<<<(B + 63) / 64, 64, 0, ctx->stream>>>(B, *gains, period, x_des, u_des, wbc_sol, mode_cmd, rbd, loaded, estop, command,
-                                                             output_torque);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, joint_command_kernel, (B + 63) / 64, 64, 0, B, *gains, period, x_des, u_des, wbc_sol, mode_cmd, rbd, loaded, estop,
+                command, output_torque);
 }
 
 int hb_rbd_to_centroidal_batch_dev(hb_ctx* ctx, int B, const double* rbd, double* x) {
   if (!ctx || B < 0 || !rbd || !x) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
-  rbd_to_centroidal_kernel<<<(B + 63) / 64, 64, 0, ctx->stream>>>(B, rbd, x);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, rbd_to_centroidal_kernel, (B + 63) / 64, 64, 0, B, rbd, x);
 }
 
 int hb_reference_expand_batch_dev(hb_ctx* ctx, int B, const double* t0, const hb_reference* refs, double* x_ref, double* swing_ref, int32_t* mode) {
   if (!ctx || B < 0 || !t0 || !refs || !x_ref || !swing_ref || !mode) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
-  reference_expand_kernel<<<B, 128, 0, ctx->stream>>>(B, ctx->cfg.horizon_N, ctx->cfg.dt, t0, refs, x_ref, swing_ref, mode, nullptr);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, reference_expand_kernel, B, 128, 0, B, ctx->cfg.horizon_N, ctx->cfg.dt, t0, refs, x_ref, swing_ref, mode, nullptr);
 }
 
 int hb_reference_expand_grid_batch_dev(hb_ctx* ctx, int B, const double* node_times, const hb_reference* refs, double* x_ref, double* swing_ref,
@@ -1916,45 +1937,28 @@ int hb_reference_expand_grid_batch_dev(hb_ctx* ctx, int B, const double* node_ti
   if (!ctx || B < 0 || !node_times || !refs || !x_ref || !swing_ref || !mode) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
-  reference_expand_kernel<<<B, 128, 0, ctx->stream>>>(B, ctx->cfg.horizon_N, ctx->cfg.dt, nullptr, refs, x_ref, swing_ref, mode, node_times);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, reference_expand_kernel, B, 128, 0, B, ctx->cfg.horizon_N, ctx->cfg.dt, nullptr, refs, x_ref, swing_ref, mode, node_times);
 }
 
 int hb_contact_positions_batch_dev(hb_ctx* ctx, int B, const double* x, double* pos) {
   if (!ctx || B < 0 || !x || !pos) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
-  contact_positions_kernel<<<(B + 63) / 64, 64, 0, ctx->stream>>>(B, x, pos);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, contact_positions_kernel, (B + 63) / 64, 64, 0, B, x, pos);
 }
 
 int hb_probe_flow_map_dev(hb_ctx* ctx, int B, const double* x, const double* u, double* f, double* A, double* Bm, double* ee) {
   if (!ctx || B < 0 || !x || !u || !f || !A || !Bm) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
-  probe_flow_map_kernel<<<B, 32, sizeof(ProbeShared), ctx->stream>>>(B, x, u, f, A, Bm, ee);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return HB_OK;
+  return launch(ctx, K_UNPROFILED, probe_flow_map_kernel, B, 32, sizeof(ProbeShared), B, x, u, f, A, Bm, ee);
 }
 
 // ------------------------------------------------------------------------------------------ host-pointer entry points
+// Each call checks its arguments, declares its host inputs and outputs to a Staging (per-instance element counts) and runs the
+// device-pointer entry point on the staged slices.
 #define H2D(dst, src, n) CK(cudaMemcpyAsync(dst, src, (n), cudaMemcpyHostToDevice, ctx->stream))
 #define D2H(dst, src, n) CK(cudaMemcpyAsync(dst, src, (n), cudaMemcpyDeviceToHost, ctx->stream))
-
-static int qp_staging_reserve(hb_ctx* ctx, size_t need) {
-  if (need > ctx->s_qp_cap) {
-    if (ctx->s_qpH) cudaFree(ctx->s_qpH);
-    ctx->s_qpH = nullptr; ctx->s_qp_cap = 0;
-    CK(dalloc(&ctx->s_qpH, need));
-    ctx->s_qp_cap = need;
-  }
-  return HB_OK;
-}
 
 int hb_wbc_qp_batch(hb_ctx* ctx, int B, int n, int m, const double* H, const double* g, const double* A, const double* lbA, const double* ubA,
                     double* x, int32_t* status, int32_t* iters) {
@@ -1962,18 +1966,10 @@ int hb_wbc_qp_batch(hb_ctx* ctx, int B, int n, int m, const double* H, const dou
   if (B == 0) return HB_OK;
   if (n < 1 || n > QP_MAX_N || m < 0 || m > QP_MAX_M) return HB_EINVAL;
   if (set_device(ctx)) return HB_ECUDA;
-  const size_t need = (size_t)B * ((size_t)n * n + (size_t)m * n + 3 * (size_t)n + 2 * (size_t)m + 2);
-  { const int rc0 = qp_staging_reserve(ctx, need); if (rc0) return rc0; }
-  double* dH = ctx->s_qpH; double* dA = dH + (size_t)B * n * n; double* dg = dA + (size_t)B * m * n; double* dlb = dg + (size_t)B * n;
-  double* dub = dlb + (size_t)B * m; double* dx = dub + (size_t)B * m; int32_t* dst = reinterpret_cast<int32_t*>(dx + (size_t)B * n); int32_t* dit = dst + B;
-  H2D(dH, H, sizeof(double) * B * n * n); H2D(dA, A, sizeof(double) * B * m * n); H2D(dg, g, sizeof(double) * B * n);
-  H2D(dlb, lbA, sizeof(double) * B * m); H2D(dub, ubA, sizeof(double) * B * m);
-  int rc = hb_wbc_qp_batch_dev(ctx, B, n, m, dH, dg, dA, dlb, dub, dx, dst, dit);
-  if (rc) return rc;
-  D2H(x, dx, sizeof(double) * B * n);
-  if (status) D2H(status, dst, sizeof(int32_t) * B);
-  if (iters) D2H(iters, dit, sizeof(int32_t) * B);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto dH = s.in(H, (size_t)n * n); auto dA = s.in(A, (size_t)m * n); auto dg = s.in(g, n); auto dlb = s.in(lbA, m); auto dub = s.in(ubA, m);
+  auto dx = s.out(x, n); auto dst = s.out(status, 1); auto dit = s.out(iters, 1);
+  return s.run([&] { return hb_wbc_qp_batch_dev(ctx, B, n, m, dH, dg, dA, dlb, dub, dx, dst, dit); });
 }
 
 int hb_wbc_assemble_batch(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
@@ -1982,19 +1978,11 @@ int hb_wbc_assemble_batch(hb_ctx* ctx, int B, const double* x_des, const double*
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  const size_t per = (size_t)QP_STRIDE_H + QP_STRIDE_A + NWBC + 2 * WBC_ROWS + 1;
-  int rc = qp_staging_reserve(ctx, (size_t)B * per);
-  if (rc) return rc;
-  double* dH = ctx->s_qpH; double* dA = dH + (size_t)B * QP_STRIDE_H; double* dg = dA + (size_t)B * QP_STRIDE_A; double* dlb = dg + (size_t)B * NWBC;
-  double* dub = dlb + (size_t)B * WBC_ROWS; int32_t* dm = reinterpret_cast<int32_t*>(dub + (size_t)B * WBC_ROWS);
-  H2D(ctx->s_xd, x_des, sizeof(double) * B * NX); H2D(ctx->s_ud, u_des, sizeof(double) * B * NU); H2D(ctx->s_rbd, rbd, sizeof(double) * B * 32);
-  H2D(ctx->s_imode, mode, sizeof(int32_t) * B);
-  if (stance_mode) H2D(ctx->s_stance, stance_mode, B);
-  rc = hb_wbc_assemble_batch_dev(ctx, B, ctx->s_xd, ctx->s_ud, ctx->s_rbd, ctx->s_imode, stance_mode ? ctx->s_stance : nullptr, dH, dg, dA, dlb, dub, dm);
-  if (rc) return rc;
-  D2H(H, dH, sizeof(double) * B * QP_STRIDE_H); D2H(A, dA, sizeof(double) * B * QP_STRIDE_A); D2H(g, dg, sizeof(double) * B * NWBC);
-  D2H(lbA, dlb, sizeof(double) * B * WBC_ROWS); D2H(ubA, dub, sizeof(double) * B * WBC_ROWS); D2H(m_rows, dm, sizeof(int32_t) * B);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto xd = s.in(x_des, NX); auto ud = s.in(u_des, NU); auto r = s.in(rbd, 32); auto md = s.in(mode, 1); auto sm = s.in_or_null(stance_mode, 1);
+  auto dH = s.out(H, QP_STRIDE_H); auto dA = s.out(A, QP_STRIDE_A); auto dg = s.out(g, NWBC); auto dlb = s.out(lbA, WBC_ROWS);
+  auto dub = s.out(ubA, WBC_ROWS); auto dm = s.out(m_rows, 1);
+  return s.run([&] { return hb_wbc_assemble_batch_dev(ctx, B, xd, ud, r, md, sm, dH, dg, dA, dlb, dub, dm); });
 }
 
 int hb_wbc_solve_batch(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
@@ -2003,14 +1991,10 @@ int hb_wbc_solve_batch(hb_ctx* ctx, int B, const double* x_des, const double* u_
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  H2D(ctx->s_xd, x_des, sizeof(double) * B * NX); H2D(ctx->s_ud, u_des, sizeof(double) * B * NU); H2D(ctx->s_rbd, rbd, sizeof(double) * B * 32);
-  H2D(ctx->s_imode, mode, sizeof(int32_t) * B);
-  if (stance_mode) H2D(ctx->s_stance, stance_mode, B);
-  int rc = hb_wbc_solve_batch_dev(ctx, B, ctx->s_xd, ctx->s_ud, ctx->s_rbd, ctx->s_imode, stance_mode ? ctx->s_stance : nullptr, ctx->s_sol, ctx->s_status);
-  if (rc) return rc;
-  D2H(sol, ctx->s_sol, sizeof(double) * B * NWBC);
-  if (status) D2H(status, ctx->s_status, sizeof(int32_t) * B);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto xd = s.in(x_des, NX); auto ud = s.in(u_des, NU); auto r = s.in(rbd, 32); auto md = s.in(mode, 1); auto sm = s.in_or_null(stance_mode, 1);
+  auto dsol = s.out(sol, NWBC); auto dst = s.out(status, 1);
+  return s.run([&] { return hb_wbc_solve_batch_dev(ctx, B, xd, ud, r, md, sm, dsol, dst); });
 }
 
 int hb_hoqp_solve_batch(hb_ctx* ctx, int B, const hb_hoqp_problem* problems, double* x, double* slack, int32_t* status) {
@@ -2025,18 +2009,9 @@ int hb_hoqp_solve_batch(hb_ctx* ctx, int B, const hb_hoqp_problem* problems, dou
     if (stk > HB_HOQP_MAX_STACKED) return HB_EINVAL;
   }
   if (set_device(ctx)) return HB_ECUDA;
-  int rc = hoqp_reserve(ctx);
-  if (rc) return rc;
-  rc = qp_staging_reserve(ctx, (size_t)B * (HQ_N + HQ_STK + 1));
-  if (rc) return rc;
-  double* dx = ctx->s_qpH; double* dsl = dx + (size_t)B * HQ_N; int32_t* dst = reinterpret_cast<int32_t*>(dsl + (size_t)B * HQ_STK);
-  H2D(ctx->hoqp_prob, problems, sizeof(hb_hoqp_problem) * B);
-  rc = hb_hoqp_solve_batch_dev(ctx, B, ctx->hoqp_prob, dx, dsl, dst);
-  if (rc) return rc;
-  D2H(x, dx, sizeof(double) * B * HQ_N);
-  if (slack) D2H(slack, dsl, sizeof(double) * B * HQ_STK);
-  if (status) D2H(status, dst, sizeof(int32_t) * B);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto pb = s.in(problems, 1); auto dx = s.out(x, HQ_N); auto dsl = s.out(slack, HQ_STK); auto dst = s.out(status, 1);
+  return s.run([&] { return hb_hoqp_solve_batch_dev(ctx, B, pb, dx, dsl, dst); });
 }
 
 int hb_hierarchical_wbc_tasks_batch(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
@@ -2045,14 +2020,9 @@ int hb_hierarchical_wbc_tasks_batch(hb_ctx* ctx, int B, const double* x_des, con
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  int rc = hoqp_reserve(ctx);
-  if (rc) return rc;
-  H2D(ctx->s_xd, x_des, sizeof(double) * B * NX); H2D(ctx->s_ud, u_des, sizeof(double) * B * NU); H2D(ctx->s_rbd, rbd, sizeof(double) * B * 32);
-  H2D(ctx->s_imode, mode, sizeof(int32_t) * B);
-  rc = hwbc_tasks_dev(ctx, B, ctx->s_xd, ctx->s_ud, ctx->s_rbd, ctx->s_imode, ctx->hoqp_prob);
-  if (rc) return rc;
-  D2H(problems, ctx->hoqp_prob, sizeof(hb_hoqp_problem) * B);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto xd = s.in(x_des, NX); auto ud = s.in(u_des, NU); auto r = s.in(rbd, 32); auto md = s.in(mode, 1); auto pb = s.out(problems, 1);
+  return s.run([&] { return hwbc_tasks_dev(ctx, B, xd, ud, r, md, pb); });
 }
 
 int hb_hierarchical_wbc_solve_batch(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, double* sol,
@@ -2061,13 +2031,10 @@ int hb_hierarchical_wbc_solve_batch(hb_ctx* ctx, int B, const double* x_des, con
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  H2D(ctx->s_xd, x_des, sizeof(double) * B * NX); H2D(ctx->s_ud, u_des, sizeof(double) * B * NU); H2D(ctx->s_rbd, rbd, sizeof(double) * B * 32);
-  H2D(ctx->s_imode, mode, sizeof(int32_t) * B);
-  int rc = hb_hierarchical_wbc_solve_batch_dev(ctx, B, ctx->s_xd, ctx->s_ud, ctx->s_rbd, ctx->s_imode, ctx->s_sol, ctx->s_status);
-  if (rc) return rc;
-  D2H(sol, ctx->s_sol, sizeof(double) * B * NWBC);
-  if (status) D2H(status, ctx->s_status, sizeof(int32_t) * B);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto xd = s.in(x_des, NX); auto ud = s.in(u_des, NU); auto r = s.in(rbd, 32); auto md = s.in(mode, 1);
+  auto dsol = s.out(sol, NWBC); auto dst = s.out(status, 1);
+  return s.run([&] { return hb_hierarchical_wbc_solve_batch_dev(ctx, B, xd, ud, r, md, dsol, dst); });
 }
 
 int hb_mpc_cold_start_batch(hb_ctx* ctx, int B, const double* x0, const int32_t* mode, double* x_traj, double* u_traj) {
@@ -2076,11 +2043,9 @@ int hb_mpc_cold_start_batch(hb_ctx* ctx, int B, const double* x0, const int32_t*
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
   const size_t N = ctx->cfg.horizon_N;
-  H2D(ctx->s_x0, x0, sizeof(double) * B * NX); H2D(ctx->s_mode, mode, sizeof(int32_t) * B * (N + 1));
-  int rc = hb_mpc_cold_start_batch_dev(ctx, B, ctx->s_x0, ctx->s_mode, ctx->s_xt, ctx->s_ut);
-  if (rc) return rc;
-  D2H(x_traj, ctx->s_xt, sizeof(double) * B * (N + 1) * NX); D2H(u_traj, ctx->s_ut, sizeof(double) * B * N * NU);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto d0 = s.in(x0, NX); auto md = s.in(mode, N + 1); auto xt = s.out(x_traj, (N + 1) * NX); auto ut = s.out(u_traj, N * NU);
+  return s.run([&] { return hb_mpc_cold_start_batch_dev(ctx, B, d0, md, xt, ut); });
 }
 
 int hb_mpc_solve_batch(hb_ctx* ctx, int B, const double* x0, const double* x_ref, const double* swing_ref, const int32_t* mode, double* x_traj,
@@ -2090,14 +2055,10 @@ int hb_mpc_solve_batch(hb_ctx* ctx, int B, const double* x0, const double* x_ref
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
   const size_t N = ctx->cfg.horizon_N;
-  H2D(ctx->s_x0, x0, sizeof(double) * B * NX); H2D(ctx->s_xref, x_ref, sizeof(double) * B * (N + 1) * NX);
-  H2D(ctx->s_swing, swing_ref, sizeof(double) * B * (N + 1) * 24); H2D(ctx->s_mode, mode, sizeof(int32_t) * B * (N + 1));
-  H2D(ctx->s_xt, x_traj, sizeof(double) * B * (N + 1) * NX); H2D(ctx->s_ut, u_traj, sizeof(double) * B * N * NU);
-  int rc = hb_mpc_solve_batch_dev(ctx, B, ctx->s_x0, ctx->s_xref, ctx->s_swing, ctx->s_mode, ctx->s_xt, ctx->s_ut, ctx->s_info);
-  if (rc) return rc;
-  D2H(x_traj, ctx->s_xt, sizeof(double) * B * (N + 1) * NX); D2H(u_traj, ctx->s_ut, sizeof(double) * B * N * NU);
-  if (info) D2H(info, ctx->s_info, sizeof(hb_solve_info) * B);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto d0 = s.in(x0, NX); auto xr = s.in(x_ref, (N + 1) * NX); auto sw = s.in(swing_ref, (N + 1) * 24); auto md = s.in(mode, N + 1);
+  auto xt = s.inout(x_traj, (N + 1) * NX); auto ut = s.inout(u_traj, N * NU); auto inf = s.out(info, 1);
+  return s.run([&] { return hb_mpc_solve_batch_dev(ctx, B, d0, xr, sw, md, xt, ut, inf); });
 }
 
 int hb_mpc_solve_grid_batch(hb_ctx* ctx, int B, const double* x0, const double* node_times, const int32_t* n_intervals, const double* x_ref,
@@ -2111,15 +2072,11 @@ int hb_mpc_solve_grid_batch(hb_ctx* ctx, int B, const double* x0, const double* 
     for (int k = 0; k < n_intervals[i]; ++k) if (!(node_times[(size_t)i * (N + 1) + k + 1] > node_times[(size_t)i * (N + 1) + k])) return HB_EINVAL;
   }
   if (set_device(ctx)) return HB_ECUDA;
-  H2D(ctx->s_x0, x0, sizeof(double) * B * NX); H2D(ctx->s_xref, x_ref, sizeof(double) * B * (N + 1) * NX);
-  H2D(ctx->s_swing, swing_ref, sizeof(double) * B * (N + 1) * 24); H2D(ctx->s_mode, mode, sizeof(int32_t) * B * (N + 1));
-  H2D(ctx->s_xt, x_traj, sizeof(double) * B * (N + 1) * NX); H2D(ctx->s_ut, u_traj, sizeof(double) * B * N * NU);
-  H2D(ctx->s_tk, node_times, sizeof(double) * B * (N + 1)); H2D(ctx->s_nn, n_intervals, sizeof(int32_t) * B);
-  int rc = hb_mpc_solve_grid_batch_dev(ctx, B, ctx->s_x0, ctx->s_tk, ctx->s_nn, ctx->s_xref, ctx->s_swing, ctx->s_mode, ctx->s_xt, ctx->s_ut, ctx->s_info);
-  if (rc) return rc;
-  D2H(x_traj, ctx->s_xt, sizeof(double) * B * (N + 1) * NX); D2H(u_traj, ctx->s_ut, sizeof(double) * B * N * NU);
-  if (info) D2H(info, ctx->s_info, sizeof(hb_solve_info) * B);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto d0 = s.in(x0, NX); auto xr = s.in(x_ref, (N + 1) * NX); auto sw = s.in(swing_ref, (N + 1) * 24); auto md = s.in(mode, N + 1);
+  auto xt = s.inout(x_traj, (N + 1) * NX); auto ut = s.inout(u_traj, N * NU); auto tk = s.in(node_times, N + 1); auto nn = s.in(n_intervals, 1);
+  auto inf = s.out(info, 1);
+  return s.run([&] { return hb_mpc_solve_grid_batch_dev(ctx, B, d0, tk, nn, xr, sw, md, xt, ut, inf); });
 }
 
 int hb_time_grid_batch(hb_ctx* ctx, int B, const double* t0, const hb_reference* refs, double* node_times, int32_t* n_intervals, int32_t* status) {
@@ -2129,12 +2086,9 @@ int hb_time_grid_batch(hb_ctx* ctx, int B, const double* t0, const hb_reference*
   if (!references_valid(B, refs)) return HB_EINVAL;
   if (set_device(ctx)) return HB_ECUDA;
   const size_t N = ctx->cfg.horizon_N;
-  H2D(ctx->s_t0, t0, sizeof(double) * B); H2D(ctx->s_refs, refs, sizeof(hb_reference) * B);
-  int rc = hb_time_grid_batch_dev(ctx, B, ctx->s_t0, ctx->s_refs, ctx->s_tk, ctx->s_nn, ctx->s_pstatus);
-  if (rc) return rc;
-  D2H(node_times, ctx->s_tk, sizeof(double) * B * (N + 1)); D2H(n_intervals, ctx->s_nn, sizeof(int32_t) * B);
-  if (status) D2H(status, ctx->s_pstatus, sizeof(int32_t) * B);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto d0 = s.in(t0, 1); auto rf = s.in(refs, 1); auto tk = s.out(node_times, N + 1); auto nn = s.out(n_intervals, 1); auto st = s.out(status, 1);
+  return s.run([&] { return hb_time_grid_batch_dev(ctx, B, d0, rf, tk, nn, st); });
 }
 
 int hb_reference_expand_grid_batch(hb_ctx* ctx, int B, const double* node_times, const hb_reference* refs, double* x_ref, double* swing_ref,
@@ -2145,12 +2099,10 @@ int hb_reference_expand_grid_batch(hb_ctx* ctx, int B, const double* node_times,
   if (!references_valid(B, refs)) return HB_EINVAL;
   if (set_device(ctx)) return HB_ECUDA;
   const size_t N = ctx->cfg.horizon_N;
-  H2D(ctx->s_tk, node_times, sizeof(double) * B * (N + 1)); H2D(ctx->s_refs, refs, sizeof(hb_reference) * B);
-  int rc = hb_reference_expand_grid_batch_dev(ctx, B, ctx->s_tk, ctx->s_refs, ctx->s_xref, ctx->s_swing, ctx->s_mode);
-  if (rc) return rc;
-  D2H(x_ref, ctx->s_xref, sizeof(double) * B * (N + 1) * NX); D2H(swing_ref, ctx->s_swing, sizeof(double) * B * (N + 1) * 24);
-  D2H(mode, ctx->s_mode, sizeof(int32_t) * B * (N + 1));
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto tk = s.in(node_times, N + 1); auto rf = s.in(refs, 1);
+  auto xr = s.out(x_ref, (N + 1) * NX); auto sw = s.out(swing_ref, (N + 1) * 24); auto md = s.out(mode, N + 1);
+  return s.run([&] { return hb_reference_expand_grid_batch_dev(ctx, B, tk, rf, xr, sw, md); });
 }
 
 int hb_resident_write_batch(hb_ctx* ctx, int B, const double* t0, const double* x_traj, const double* u_traj, const int32_t* mode, const double* node_times,
@@ -2190,42 +2142,19 @@ int hb_control_step_batch(hb_ctx* ctx, int B, double t_rel, const double* x0, co
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
   const size_t N = ctx->cfg.horizon_N;
-  // Two half-batches on two streams: the copies of one half overlap the kernels of the other (pinned host memory assumed).
-  const int nchunk = (B >= 256) ? 2 : 1;
-  int rc = HB_OK;
-  for (int c = 0; c < nchunk && rc == HB_OK; ++c) {
-    const size_t lo = (size_t)B * c / nchunk, hi = (size_t)B * (c + 1) / nchunk, n = hi - lo;
-    ctx->stream = (c == 0) ? ctx->stream_main : ctx->stream_aux;
-    ctx->base = (int)lo;
-    cudaError_t e = cudaSuccess;
-    auto h2d = [&](void* d, const void* h, size_t bytes) { if (e == cudaSuccess) e = cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, ctx->stream); };
-    auto d2h = [&](void* h, const void* d, size_t bytes) { if (e == cudaSuccess) e = cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, ctx->stream); };
-    h2d(ctx->s_x0 + lo * NX, x0 + lo * NX, sizeof(double) * n * NX);
-    h2d(ctx->s_xref + lo * (N + 1) * NX, x_ref + lo * (N + 1) * NX, sizeof(double) * n * (N + 1) * NX);
-    h2d(ctx->s_swing + lo * (N + 1) * 24, swing_ref + lo * (N + 1) * 24, sizeof(double) * n * (N + 1) * 24);
-    h2d(ctx->s_mode + lo * (N + 1), mode + lo * (N + 1), sizeof(int32_t) * n * (N + 1));
-    h2d(ctx->s_xt + lo * (N + 1) * NX, x_traj + lo * (N + 1) * NX, sizeof(double) * n * (N + 1) * NX);
-    h2d(ctx->s_ut + lo * N * NU, u_traj + lo * N * NU, sizeof(double) * n * N * NU);
-    h2d(ctx->s_rbd + lo * 32, rbd + lo * 32, sizeof(double) * n * 32);
-    if (e != cudaSuccess) { ctx->last_cuda = (int)e; rc = HB_ECUDA; break; }
-    rc = hb_control_step_batch_dev(ctx, (int)n, t_rel, ctx->s_x0 + lo * NX, ctx->s_xref + lo * (N + 1) * NX, ctx->s_swing + lo * (N + 1) * 24,
-                                   ctx->s_mode + lo * (N + 1), ctx->s_rbd + lo * 32, ctx->s_xt + lo * (N + 1) * NX, ctx->s_ut + lo * N * NU,
-                                   ctx->s_info + lo, ctx->s_sol + lo * NWBC, ctx->s_tau + lo * NJ, ctx->s_status + lo);
-    if (rc) break;
-    d2h(x_traj + lo * (N + 1) * NX, ctx->s_xt + lo * (N + 1) * NX, sizeof(double) * n * (N + 1) * NX);
-    d2h(u_traj + lo * N * NU, ctx->s_ut + lo * N * NU, sizeof(double) * n * N * NU);
-    if (info) d2h(info + lo, ctx->s_info + lo, sizeof(hb_solve_info) * n);
-    if (wbc_sol) d2h(wbc_sol + lo * NWBC, ctx->s_sol + lo * NWBC, sizeof(double) * n * NWBC);
-    if (torque) d2h(torque + lo * NJ, ctx->s_tau + lo * NJ, sizeof(double) * n * NJ);
-    if (wbc_status) d2h(wbc_status + lo, ctx->s_status + lo, sizeof(int32_t) * n);
-    if (e != cudaSuccess) { ctx->last_cuda = (int)e; rc = HB_ECUDA; }
-  }
-  ctx->stream = ctx->stream_main;
-  ctx->base = 0;
-  cudaError_t e1 = cudaStreamSynchronize(ctx->stream_aux), e0 = cudaStreamSynchronize(ctx->stream_main);
+  Staging s(ctx, B);
+  auto d0 = s.in(x0, NX); auto xr = s.in(x_ref, (N + 1) * NX); auto sw = s.in(swing_ref, (N + 1) * 24); auto md = s.in(mode, N + 1);
+  auto xt = s.inout(x_traj, (N + 1) * NX); auto ut = s.inout(u_traj, N * NU); auto r = s.in(rbd, 32);
+  auto inf = s.out(info, 1); auto sol = s.out(wbc_sol, NWBC); auto tau = s.out(torque, NJ); auto st = s.out(wbc_status, 1);
+  const int rc = s.reserve();
   if (rc) return rc;
-  if (e0 != cudaSuccess || e1 != cudaSuccess) { ctx->last_cuda = (int)(e0 != cudaSuccess ? e0 : e1); return HB_ECUDA; }
-  return HB_OK;
+  // Two half-batches on two streams: the copies of one half overlap the kernels of the other (pinned host memory assumed).
+  return chunked(ctx, B, B >= 256 ? 2 : 1, [&](int, size_t lo, size_t hi) -> int {
+    int r2 = s.h2d(lo, hi);
+    if (!r2) r2 = hb_control_step_batch_dev(ctx, (int)(hi - lo), t_rel, d0.at(lo), xr.at(lo), sw.at(lo), md.at(lo), r.at(lo), xt.at(lo), ut.at(lo),
+                                            inf.at(lo), sol.at(lo), tau.at(lo), st.at(lo));
+    return r2 ? r2 : s.d2h(lo, hi);
+  });
 }
 
 // words (8 bytes) one packed instance needs
@@ -2282,92 +2211,52 @@ int hb_resident_cycle_batch(hb_ctx* ctx, int B, int cold_start, double t_rel, co
   // Automatic choice: with a pageable reference array the host packs the used entries, and from 4096 instances on two chunks hide that pass
   // and the copies behind the other chunk's kernels; below, the half-batch kernels of the sequential stages run no faster than the full
   // batch. With a pinned array there is no host pass to hide and one chunk is used at every size.
-  const int nchunk = ctx->cfg.e2e_chunks > 0 ? ((B >= 64 * ctx->cfg.e2e_chunks) ? ctx->cfg.e2e_chunks : 1) : ((!refs_dev && B >= 4096) ? 2 : 1);
-  if (refs_dev) {
-    // validation and byte count happen on the device while it copies (no per-instance host work at all); the verdict comes back with the results
-    if (ctx->refstat_cap < 2 * nchunk) {
-      if (ctx->h_refstat) cudaFreeHost(ctx->h_refstat);
-      if (ctx->d_refstat) cudaFree(ctx->d_refstat);
-      ctx->h_refstat = nullptr; ctx->d_refstat = nullptr; ctx->refstat_cap = 0;
-      if (cudaHostAlloc(reinterpret_cast<void**>(&ctx->h_refstat), sizeof(unsigned long long) * 2 * nchunk, cudaHostAllocDefault) != cudaSuccess ||
-          cudaMalloc(reinterpret_cast<void**>(&ctx->d_refstat), sizeof(unsigned long long) * 2 * nchunk) != cudaSuccess) {
-        cudaGetLastError();
-        if (ctx->h_refstat) { cudaFreeHost(ctx->h_refstat); ctx->h_refstat = nullptr; }
-        return HB_ENOMEM;
-      }
-      ctx->refstat_cap = 2 * nchunk;
-    }
-  } else {
+  const int nchunk = cycle_chunks(ctx, B, !refs_dev);
+  // pinned path: validation and byte count happen on the device while it copies (no per-instance host work at all); the verdict, two words
+  // per chunk {invalid structs, words read}, comes back with the results. Pageable path: the used entries are packed into the context's
+  // pinned host buffer, copied, and unpacked on the device.
+  size_t pack_words = 0;
+  if (!refs_dev) {
     if (!references_valid(B, refs)) return HB_EINVAL;
-    size_t need = 0;
-    for (int i = 0; i < B; ++i) need += ref_pack_words(refs[i]);
-    need += (size_t)B + 2 * (size_t)nchunk + 8;
-    if (need > ctx->pack_cap) {
-      if (ctx->h_pack) cudaFreeHost(ctx->h_pack);
-      if (ctx->d_pack) cudaFree(ctx->d_pack);
-      ctx->h_pack = nullptr; ctx->d_pack = nullptr; ctx->pack_cap = 0;
-      const size_t cap = need + need / 4;
-      if (cudaHostAlloc(reinterpret_cast<void**>(&ctx->h_pack), cap * sizeof(double), cudaHostAllocDefault) != cudaSuccess || dalloc(&ctx->d_pack, cap) != cudaSuccess) {
-        cudaGetLastError();
-        if (ctx->h_pack) { cudaFreeHost(ctx->h_pack); ctx->h_pack = nullptr; }
-        return HB_ENOMEM;
-      }
-      ctx->pack_cap = cap;
-    }
+    for (int i = 0; i < B; ++i) pack_words += ref_pack_words(refs[i]);
+    pack_words += (size_t)B + 2 * (size_t)nchunk + 8;
   }
+  const size_t stat_words = refs_dev ? 2 * (size_t)nchunk : 0;
+  Staging s(ctx, B);
+  auto d0 = s.in(t0, 1); auto dx0 = s.in(x0, NX); auto r = s.in(rbd, 32); auto rf = s.tmp<hb_reference>(1);
+  auto d_pack = s.buf<double>(pack_words); auto d_stat = s.buf<unsigned long long>(stat_words);
+  auto inf = s.out(info, 1); auto sol = s.out(wbc_sol, NWBC); auto tau = s.out(torque, NJ); auto st = s.out(wbc_status, 1);
+  int rc = s.reserve();
+  if (!rc) rc = grow(ctx, &ctx->pinned, &ctx->pinned_cap, refs_dev ? sizeof(unsigned long long) * stat_words : sizeof(double) * pack_words, true);
+  if (rc) return rc;
+  double* h_pack = static_cast<double*>(ctx->pinned);
+  unsigned long long* h_stat = static_cast<unsigned long long*>(ctx->pinned);
   size_t pack_base = 0;
   ctx->last_h2d_bytes = 0;
-  int rc = HB_OK;
-  for (int c = 0; c < nchunk && rc == HB_OK; ++c) {
-    const size_t lo = (size_t)B * c / nchunk, hi = (size_t)B * (c + 1) / nchunk, n = hi - lo;
-    ctx->stream = (c % 2 == 0) ? ctx->stream_main : ctx->stream_aux;
-    ctx->base = (int)lo;
-    cudaError_t e = cudaSuccess;
-    auto h2d = [&](void* d, const void* h, size_t bytes) { if (e == cudaSuccess) e = cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, ctx->stream); };
-    auto d2h = [&](void* h, const void* d, size_t bytes) { if (e == cudaSuccess) e = cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, ctx->stream); };
-    h2d(ctx->s_t0 + lo, t0 + lo, sizeof(double) * n);
-    h2d(ctx->s_x0 + lo * NX, x0 + lo * NX, sizeof(double) * n * NX);
+  rc = chunked(ctx, B, nchunk, [&](int c, size_t lo, size_t hi) -> int {
+    const int n = (int)(hi - lo);
+    int r2 = s.h2d(lo, hi);
+    if (r2) return r2;
     if (refs_dev) {
-      // pinned caller array: the device gathers the used entries itself (no host pass, no staging copy)
-      if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_refstat + 2 * c, 0, 2 * sizeof(unsigned long long), ctx->stream);
-      if (e == cudaSuccess) {
-        reference_gather_pinned_kernel<<<(unsigned)n, 128, 0, ctx->stream>>>((int)n, refs_dev + lo, ctx->s_refs + lo, ctx->d_refstat + 2 * c);
-        ctx->launches++;
-        e = cudaGetLastError();
-      }
-      d2h(ctx->h_refstat + 2 * c, ctx->d_refstat + 2 * c, 2 * sizeof(unsigned long long));
+      CK(cudaMemsetAsync(d_stat.at(2 * c), 0, 2 * sizeof(unsigned long long), ctx->stream));
+      r2 = launch(ctx, K_UNPROFILED, reference_gather_pinned_kernel, n, 128, 0, n, refs_dev + lo, rf.at(lo), d_stat.at(2 * c));
+      if (r2) return r2;
+      D2H(h_stat + 2 * c, d_stat.at(2 * c), 2 * sizeof(unsigned long long));
     } else {
-      // references: only the used entries cross PCIe (packed into the context's pinned staging area, unpacked into s_refs on the device)
-      const size_t words = ref_pack(refs, lo, hi, ctx->h_pack + pack_base);
-      h2d(ctx->d_pack + pack_base, ctx->h_pack + pack_base, sizeof(double) * words);
-      if (e == cudaSuccess) {
-        reference_unpack_kernel<<<(unsigned)n, 128, 0, ctx->stream>>>((int)n, reinterpret_cast<const long long*>(ctx->d_pack + pack_base), ctx->d_pack + pack_base,
-                                                                        ctx->s_refs + lo);
-        ctx->launches++;
-        e = cudaGetLastError();
-      }
+      const size_t words = ref_pack(refs, lo, hi, h_pack + pack_base);
+      H2D(d_pack.at(pack_base), h_pack + pack_base, sizeof(double) * words);
+      r2 = launch(ctx, K_UNPROFILED, reference_unpack_kernel, n, 128, 0, n, reinterpret_cast<const long long*>(d_pack.at(pack_base)), d_pack.at(pack_base), rf.at(lo));
+      if (r2) return r2;
       pack_base += words;
       ctx->last_h2d_bytes += sizeof(double) * words;
     }
-    h2d(ctx->s_rbd + lo * 32, rbd + lo * 32, sizeof(double) * n * 32);
-    if (e != cudaSuccess) { ctx->last_cuda = (int)e; rc = HB_ECUDA; break; }
-    rc = hb_resident_cycle_batch_dev(ctx, (int)n, cold_start, t_rel, ctx->s_t0 + lo, ctx->s_x0 + lo * NX, ctx->s_refs + lo, ctx->s_rbd + lo * 32,
-                                     ctx->s_info + lo, ctx->s_sol + lo * NWBC, ctx->s_tau + lo * NJ, ctx->s_status + lo);
-    if (rc) break;
-    if (info) d2h(info + lo, ctx->s_info + lo, sizeof(hb_solve_info) * n);
-    if (wbc_sol) d2h(wbc_sol + lo * NWBC, ctx->s_sol + lo * NWBC, sizeof(double) * n * NWBC);
-    if (torque) d2h(torque + lo * NJ, ctx->s_tau + lo * NJ, sizeof(double) * n * NJ);
-    if (wbc_status) d2h(wbc_status + lo, ctx->s_status + lo, sizeof(int32_t) * n);
-    if (e != cudaSuccess) { ctx->last_cuda = (int)e; rc = HB_ECUDA; }
-  }
-  ctx->stream = ctx->stream_main;
-  ctx->base = 0;
-  cudaError_t e1 = cudaStreamSynchronize(ctx->stream_aux), e0 = cudaStreamSynchronize(ctx->stream_main);
+    r2 = hb_resident_cycle_batch_dev(ctx, n, cold_start, t_rel, d0.at(lo), dx0.at(lo), rf.at(lo), r.at(lo), inf.at(lo), sol.at(lo), tau.at(lo), st.at(lo));
+    return r2 ? r2 : s.d2h(lo, hi);
+  });
   if (rc) return rc;
-  if (e0 != cudaSuccess || e1 != cudaSuccess) { ctx->last_cuda = (int)(e0 != cudaSuccess ? e0 : e1); return HB_ECUDA; }
   if (refs_dev) {
     unsigned long long invalid = 0, words = 0;
-    for (int c = 0; c < nchunk; ++c) { invalid += ctx->h_refstat[2 * c]; words += ctx->h_refstat[2 * c + 1]; }
+    for (int c = 0; c < nchunk; ++c) { invalid += h_stat[2 * c]; words += h_stat[2 * c + 1]; }
     ctx->last_h2d_bytes = sizeof(double) * (size_t)words;
     if (invalid) { ctx->res_valid = 0; return HB_EINVAL; }      // malformed structs: counts were clamped on the device, the outputs are not meaningful
   }
@@ -2379,14 +2268,9 @@ int hb_plan_references_gpu(hb_ctx* ctx, int B, const hb_plan_input* in, double* 
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  H2D(ctx->s_plan, in, sizeof(hb_plan_input) * B);
-  H2D(ctx->s_misc, latest_stance, sizeof(double) * B * 12);
-  int rc = hb_plan_references_batch_dev(ctx, B, ctx->s_plan, nullptr, ctx->s_misc, ctx->s_refs, ctx->s_pstatus);
-  if (rc) return rc;
-  D2H(out, ctx->s_refs, sizeof(hb_reference) * B);
-  D2H(latest_stance, ctx->s_misc, sizeof(double) * B * 12);
-  if (status) D2H(status, ctx->s_pstatus, sizeof(int32_t) * B);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto din = s.in(in, 1); auto ls = s.inout(latest_stance, 12); auto dout = s.out(out, 1); auto st = s.out(status, 1);
+  return s.run([&] { return hb_plan_references_batch_dev(ctx, B, din, nullptr, ls, dout, st); });
 }
 
 int hb_resident_plan_cycle_batch(hb_ctx* ctx, int B, int cold_start, double t_rel, const hb_plan_input* in, const double* rbd, hb_solve_info* info,
@@ -2396,40 +2280,23 @@ int hb_resident_plan_cycle_batch(hb_ctx* ctx, int B, int cold_start, double t_re
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (!cold_start && ctx->res_valid < B) return HB_EINVAL;
   if (set_device(ctx)) return HB_ECUDA;
-  const int nchunk = ctx->cfg.e2e_chunks > 0 ? ((B >= 64 * ctx->cfg.e2e_chunks) ? ctx->cfg.e2e_chunks : 1) : ((B >= 4096) ? 2 : 1);
-  int rc = HB_OK;
-  for (int c = 0; c < nchunk && rc == HB_OK; ++c) {
-    const size_t lo = (size_t)B * c / nchunk, hi = (size_t)B * (c + 1) / nchunk, n = hi - lo;
-    ctx->stream = (c % 2 == 0) ? ctx->stream_main : ctx->stream_aux;
-    ctx->base = (int)lo;
-    cudaError_t e = cudaSuccess;
-    auto h2d = [&](void* d, const void* h, size_t bytes) { if (e == cudaSuccess) e = cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, ctx->stream); };
-    auto d2h = [&](void* h, const void* d, size_t bytes) { if (e == cudaSuccess) e = cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, ctx->stream); };
-    h2d(ctx->s_plan + lo, in + lo, sizeof(hb_plan_input) * n);
-    h2d(ctx->s_rbd + lo * 32, rbd + lo * 32, sizeof(double) * n * 32);
-    if (cold_start && e == cudaSuccess) e = cudaMemsetAsync(ctx->res_stance + lo * 12, 0, sizeof(double) * n * 12, ctx->stream);   // latestStanceposition_ starts at zero
-    if (e != cudaSuccess) { ctx->last_cuda = (int)e; rc = HB_ECUDA; break; }
-    double* feet = ctx->s_misc + lo * 12;
-    plan_prepare_kernel<<<((int)n + 63) / 64, 64, 0, ctx->stream>>>((int)n, ctx->s_plan + lo, ctx->s_t0 + lo, ctx->s_x0 + lo * NX, feet);
-    ctx->launches++;
-    rc = hb_plan_references_batch_dev(ctx, (int)n, ctx->s_plan + lo, feet, ctx->res_stance + lo * 12, ctx->s_refs + lo, ctx->s_pstatus + lo);
-    if (rc) break;
-    rc = hb_resident_cycle_batch_dev(ctx, (int)n, cold_start, t_rel, ctx->s_t0 + lo, ctx->s_x0 + lo * NX, ctx->s_refs + lo, ctx->s_rbd + lo * 32,
-                                     ctx->s_info + lo, ctx->s_sol + lo * NWBC, ctx->s_tau + lo * NJ, ctx->s_status + lo);
-    if (rc) break;
-    if (info) d2h(info + lo, ctx->s_info + lo, sizeof(hb_solve_info) * n);
-    if (wbc_sol) d2h(wbc_sol + lo * NWBC, ctx->s_sol + lo * NWBC, sizeof(double) * n * NWBC);
-    if (torque) d2h(torque + lo * NJ, ctx->s_tau + lo * NJ, sizeof(double) * n * NJ);
-    if (wbc_status) d2h(wbc_status + lo, ctx->s_status + lo, sizeof(int32_t) * n);
-    if (plan_status) d2h(plan_status + lo, ctx->s_pstatus + lo, sizeof(int32_t) * n);
-    if (e != cudaSuccess) { ctx->last_cuda = (int)e; rc = HB_ECUDA; }
-  }
-  ctx->stream = ctx->stream_main;
-  ctx->base = 0;
-  cudaError_t e1 = cudaStreamSynchronize(ctx->stream_aux), e0 = cudaStreamSynchronize(ctx->stream_main);
+  const int nchunk = cycle_chunks(ctx, B, true);
+  Staging s(ctx, B);
+  auto din = s.in(in, 1); auto r = s.in(rbd, 32);
+  auto d0 = s.tmp<double>(1); auto dx0 = s.tmp<double>(NX); auto feet = s.tmp<double>(12); auto rf = s.tmp<hb_reference>(1);   // planner -> cycle
+  auto inf = s.out(info, 1); auto sol = s.out(wbc_sol, NWBC); auto tau = s.out(torque, NJ); auto st = s.out(wbc_status, 1); auto pst = s.out(plan_status, 1);
+  const int rc = s.reserve();
   if (rc) return rc;
-  if (e0 != cudaSuccess || e1 != cudaSuccess) { ctx->last_cuda = (int)(e0 != cudaSuccess ? e0 : e1); return HB_ECUDA; }
-  return HB_OK;
+  return chunked(ctx, B, nchunk, [&](int, size_t lo, size_t hi) -> int {
+    const int n = (int)(hi - lo);
+    int r2 = s.h2d(lo, hi);
+    if (r2) return r2;
+    if (cold_start) CK(cudaMemsetAsync(ctx->res_stance + lo * 12, 0, sizeof(double) * n * 12, ctx->stream));   // latestStanceposition_ starts at zero
+    r2 = launch(ctx, K_UNPROFILED, plan_prepare_kernel, (n + 63) / 64, 64, 0, n, din.at(lo), d0.at(lo), dx0.at(lo), feet.at(lo));
+    if (!r2) r2 = hb_plan_references_batch_dev(ctx, n, din.at(lo), feet.at(lo), ctx->res_stance + lo * 12, rf.at(lo), pst.at(lo));
+    if (!r2) r2 = hb_resident_cycle_batch_dev(ctx, n, cold_start, t_rel, d0.at(lo), dx0.at(lo), rf.at(lo), r.at(lo), inf.at(lo), sol.at(lo), tau.at(lo), st.at(lo));
+    return r2 ? r2 : s.d2h(lo, hi);
+  });
 }
 
 int hb_resident_read_batch(hb_ctx* ctx, int B, double* t0, double* x_traj, double* u_traj) {
@@ -2451,18 +2318,10 @@ int hb_joint_command_batch(hb_ctx* ctx, int B, const hb_pd_gains* gains, double 
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  H2D(ctx->s_xd, x_des, sizeof(double) * B * NX); H2D(ctx->s_ud, u_des, sizeof(double) * B * NU); H2D(ctx->s_rbd, rbd, sizeof(double) * B * 32);
-  H2D(ctx->s_sol, wbc_sol, sizeof(double) * B * NWBC); H2D(ctx->s_imode, mode_cmd, sizeof(int32_t) * B);
-  uint8_t* d_loaded = (uint8_t*)ctx->s_status;      // B int32 words: room for two B-byte flag arrays
-  uint8_t* d_estop = d_loaded + B;
-  if (loaded) H2D(d_loaded, loaded, B);
-  if (estop) H2D(d_estop, estop, B);
-  int rc = hb_joint_command_batch_dev(ctx, B, gains, period, ctx->s_xd, ctx->s_ud, ctx->s_sol, ctx->s_imode, ctx->s_rbd, loaded ? d_loaded : nullptr,
-                                      estop ? d_estop : nullptr, ctx->s_misc, ctx->s_tau);
-  if (rc) return rc;
-  D2H(command, ctx->s_misc, sizeof(double) * B * NJ * 5); D2H(output_torque, ctx->s_tau, sizeof(double) * B * NJ);
-  if (estop) D2H(estop, d_estop, B);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto xd = s.in(x_des, NX); auto ud = s.in(u_des, NU); auto r = s.in(rbd, 32); auto sol = s.in(wbc_sol, NWBC); auto md = s.in(mode_cmd, 1);
+  auto ld = s.in_or_null(loaded, 1); auto es = s.inout_or_null(estop, 1); auto cmd = s.out(command, NJ * 5); auto tau = s.out(output_torque, NJ);
+  return s.run([&] { return hb_joint_command_batch_dev(ctx, B, gains, period, xd, ud, sol, md, r, ld, es, cmd, tau); });
 }
 
 int hb_estimator_update_batch(hb_ctx* ctx, int B, const hb_kf_params* params, double dt, hb_kf_state* state, const double* quat,
@@ -2472,17 +2331,10 @@ int hb_estimator_update_batch(hb_ctx* ctx, int B, const hb_kf_params* params, do
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  double* d_quat = ctx->s_misc; double* d_w = d_quat + (size_t)B * 4; double* d_a = d_w + (size_t)B * 3; double* d_jp = d_a + (size_t)B * 3;
-  double* d_jv = d_jp + (size_t)B * NJ;
-  uint8_t* d_flag = (uint8_t*)ctx->s_status;      // B int32 words hold B x 4 flags
-  H2D(ctx->s_kf, state, sizeof(hb_kf_state) * B);
-  H2D(d_quat, quat, sizeof(double) * B * 4); H2D(d_w, ang_vel_local, sizeof(double) * B * 3); H2D(d_a, lin_acc_local, sizeof(double) * B * 3);
-  H2D(d_jp, joint_pos, sizeof(double) * B * NJ); H2D(d_jv, joint_vel, sizeof(double) * B * NJ); H2D(d_flag, contact_flag, (size_t)B * 4);
-  int rc = hb_estimator_update_batch_dev(ctx, B, params, dt, ctx->s_kf, d_quat, d_w, d_a, d_jp, d_jv, d_flag, ctx->s_rbd);
-  if (rc) return rc;
-  D2H(state, ctx->s_kf, sizeof(hb_kf_state) * B);
-  D2H(rbd_out, ctx->s_rbd, sizeof(double) * B * 32);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto kf = s.inout(state, 1); auto q = s.in(quat, 4); auto w = s.in(ang_vel_local, 3); auto a = s.in(lin_acc_local, 3);
+  auto jp = s.in(joint_pos, NJ); auto jv = s.in(joint_vel, NJ); auto fl = s.in(contact_flag, 4); auto ro = s.out(rbd_out, 32);
+  return s.run([&] { return hb_estimator_update_batch_dev(ctx, B, params, dt, kf, q, w, a, jp, jv, fl, ro); });
 }
 
 int hb_actuation_batch(hb_ctx* ctx, int B, double delay, const double* time, hb_actuation_state* state, const double* command, const double* rbd,
@@ -2491,16 +2343,9 @@ int hb_actuation_batch(hb_ctx* ctx, int B, double delay, const double* time, hb_
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  const size_t need = ((size_t)B * sizeof(hb_actuation_state) + 7) / 8;
-  int rc = qp_staging_reserve(ctx, need);
-  if (rc) return rc;
-  hb_actuation_state* d_state = reinterpret_cast<hb_actuation_state*>(ctx->s_qpH);
-  H2D(d_state, state, sizeof(hb_actuation_state) * B); H2D(ctx->s_t0, time, sizeof(double) * B);
-  H2D(ctx->s_misc, command, sizeof(double) * B * NJ * 5); H2D(ctx->s_rbd, rbd, sizeof(double) * B * 32);
-  rc = hb_actuation_batch_dev(ctx, B, delay, ctx->s_t0, d_state, ctx->s_misc, ctx->s_rbd, ctx->s_tau);
-  if (rc) return rc;
-  D2H(state, d_state, sizeof(hb_actuation_state) * B); D2H(tau, ctx->s_tau, sizeof(double) * B * NJ);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto st = s.inout(state, 1); auto tm = s.in(time, 1); auto cmd = s.in(command, NJ * 5); auto r = s.in(rbd, 32); auto t = s.out(tau, NJ);
+  return s.run([&] { return hb_actuation_batch_dev(ctx, B, delay, tm, st, cmd, r, t); });
 }
 
 int hb_sim_step_batch(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {
@@ -2508,14 +2353,9 @@ int hb_sim_step_batch(hb_ctx* ctx, int B, const hb_sim_params* params, double* r
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  uint8_t* d_flag = (uint8_t*)ctx->s_status;      // B int32 words hold B x 4 flags
-  H2D(ctx->s_rbd, rbd, sizeof(double) * B * 32); H2D(ctx->s_tau, tau, sizeof(double) * B * NJ);
-  int rc = hb_sim_step_batch_dev(ctx, B, params, ctx->s_rbd, ctx->s_tau, ctx->s_misc, d_flag);
-  if (rc) return rc;
-  D2H(rbd, ctx->s_rbd, sizeof(double) * B * 32);
-  if (contact_force) D2H(contact_force, ctx->s_misc, sizeof(double) * B * 12);
-  if (contact_flag) D2H(contact_flag, d_flag, (size_t)B * 4);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
+  return s.run([&] { return hb_sim_step_batch_dev(ctx, B, params, r, t, cf, fl); });
 }
 
 int hb_resident_wbc_batch(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
@@ -2525,16 +2365,11 @@ int hb_resident_wbc_batch(hb_ctx* ctx, int B, const double* t_now, const double*
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (B > ctx->res_valid) return HB_EINVAL;
   if (set_device(ctx)) return HB_ECUDA;
-  H2D(ctx->s_t0, t_now, sizeof(double) * B); H2D(ctx->s_rbd, rbd, sizeof(double) * B * 32);
-  if (stance_mode) H2D(ctx->s_stance, stance_mode, B);
-  int rc = hb_resident_wbc_batch_dev(ctx, B, ctx->s_t0, ctx->s_rbd, stance_mode ? ctx->s_stance : nullptr, ctx->s_xd, ctx->s_ud, ctx->s_imode, ctx->s_sol, ctx->s_tau,
-                                     ctx->s_status);
-  if (rc) return rc;
-  D2H(x_des, ctx->s_xd, sizeof(double) * B * NX); D2H(u_des, ctx->s_ud, sizeof(double) * B * NU); D2H(mode_out, ctx->s_imode, sizeof(int32_t) * B);
-  D2H(wbc_sol, ctx->s_sol, sizeof(double) * B * NWBC);
-  if (torque) D2H(torque, ctx->s_tau, sizeof(double) * B * NJ);
-  if (wbc_status) D2H(wbc_status, ctx->s_status, sizeof(int32_t) * B);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto tn = s.in(t_now, 1); auto r = s.in(rbd, 32); auto sm = s.in_or_null(stance_mode, 1);
+  auto xd = s.out(x_des, NX); auto ud = s.out(u_des, NU); auto md = s.out(mode_out, 1); auto sol = s.out(wbc_sol, NWBC);
+  auto tau = s.out(torque, NJ); auto st = s.out(wbc_status, 1);    // always passed: the fallback and its bookkeeping run on every call
+  return s.run([&] { return hb_resident_wbc_batch_dev(ctx, B, tn, r, sm, xd, ud, md, sol, tau, st); });
 }
 
 int hb_contact_force_estimate_batch(hb_ctx* ctx, int B, double cutoff_frequency, double dt, hb_observer_state* state, const double* rbd,
@@ -2543,15 +2378,10 @@ int hb_contact_force_estimate_batch(hb_ctx* ctx, int B, double cutoff_frequency,
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  // staging: s_misc holds the observer states (16 doubles), the estimates (16) and the disturbance torques (16) of the batch
-  hb_observer_state* d_state = reinterpret_cast<hb_observer_state*>(ctx->s_misc);
-  double* d_est = ctx->s_misc + (size_t)B * 16; double* d_dist = d_est + (size_t)B * 16;
-  H2D(d_state, state, sizeof(hb_observer_state) * B); H2D(ctx->s_rbd, rbd, sizeof(double) * B * 32); H2D(ctx->s_tau, tau_cmd, sizeof(double) * B * NJ);
-  int rc = hb_contact_force_estimate_batch_dev(ctx, B, cutoff_frequency, dt, d_state, ctx->s_rbd, ctx->s_tau, d_est, d_dist);
-  if (rc) return rc;
-  D2H(state, d_state, sizeof(hb_observer_state) * B); D2H(est_contact_force, d_est, sizeof(double) * B * 16);
-  if (disturbance_torque) D2H(disturbance_torque, d_dist, sizeof(double) * B * NQ);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto st = s.inout(state, 1); auto r = s.in(rbd, 32); auto t = s.in(tau_cmd, NJ); auto est = s.out(est_contact_force, 16);
+  auto dist = s.out(disturbance_torque, NQ);
+  return s.run([&] { return hb_contact_force_estimate_batch_dev(ctx, B, cutoff_frequency, dt, st, r, t, est, dist); });
 }
 
 int hb_rbd_to_centroidal_batch(hb_ctx* ctx, int B, const double* rbd, double* x) {
@@ -2559,11 +2389,9 @@ int hb_rbd_to_centroidal_batch(hb_ctx* ctx, int B, const double* rbd, double* x)
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  H2D(ctx->s_rbd, rbd, sizeof(double) * B * 32);
-  int rc = hb_rbd_to_centroidal_batch_dev(ctx, B, ctx->s_rbd, ctx->s_xd);
-  if (rc) return rc;
-  D2H(x, ctx->s_xd, sizeof(double) * B * NX);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto r = s.in(rbd, 32); auto dx = s.out(x, NX);
+  return s.run([&] { return hb_rbd_to_centroidal_batch_dev(ctx, B, r, dx); });
 }
 
 int hb_reference_expand_batch(hb_ctx* ctx, int B, const double* t0, const hb_reference* refs, double* x_ref, double* swing_ref, int32_t* mode) {
@@ -2573,12 +2401,10 @@ int hb_reference_expand_batch(hb_ctx* ctx, int B, const double* t0, const hb_ref
   if (!references_valid(B, refs)) return HB_EINVAL;
   if (set_device(ctx)) return HB_ECUDA;
   const size_t N = ctx->cfg.horizon_N;
-  H2D(ctx->s_t0, t0, sizeof(double) * B); H2D(ctx->s_refs, refs, sizeof(hb_reference) * B);
-  int rc = hb_reference_expand_batch_dev(ctx, B, ctx->s_t0, ctx->s_refs, ctx->s_xref, ctx->s_swing, ctx->s_mode);
-  if (rc) return rc;
-  D2H(x_ref, ctx->s_xref, sizeof(double) * B * (N + 1) * NX); D2H(swing_ref, ctx->s_swing, sizeof(double) * B * (N + 1) * 24);
-  D2H(mode, ctx->s_mode, sizeof(int32_t) * B * (N + 1));
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto d0 = s.in(t0, 1); auto rf = s.in(refs, 1);
+  auto xr = s.out(x_ref, (N + 1) * NX); auto sw = s.out(swing_ref, (N + 1) * 24); auto md = s.out(mode, N + 1);
+  return s.run([&] { return hb_reference_expand_batch_dev(ctx, B, d0, rf, xr, sw, md); });
 }
 
 int hb_contact_positions_batch(hb_ctx* ctx, int B, const double* x, double* pos) {
@@ -2586,11 +2412,9 @@ int hb_contact_positions_batch(hb_ctx* ctx, int B, const double* x, double* pos)
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  H2D(ctx->s_xd, x, sizeof(double) * B * NX);
-  int rc = hb_contact_positions_batch_dev(ctx, B, ctx->s_xd, ctx->s_misc);
-  if (rc) return rc;
-  D2H(pos, ctx->s_misc, sizeof(double) * B * 12);
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto dx = s.in(x, NX); auto dp = s.out(pos, 12);
+  return s.run([&] { return hb_contact_positions_batch_dev(ctx, B, dx, dp); });
 }
 
 static std::atomic<int> g_plan_threads{0};   // 0 = hardware_concurrency (hb_plan_set_threads)
@@ -2644,15 +2468,10 @@ int hb_probe_flow_map(hb_ctx* ctx, int B, const double* x, const double* u, doub
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   if (set_device(ctx)) return HB_ECUDA;
-  const size_t per = NX + 2 * TS + 24 + 36 * NX;
-  H2D(ctx->s_xd, x, sizeof(double) * B * NX); H2D(ctx->s_ud, u, sizeof(double) * B * NU);
-  double* df = ctx->s_misc; double* dA = df + (size_t)B * NX; double* dB = dA + (size_t)B * TS; double* dee = dB + (size_t)B * TS;
-  (void)per;
-  int rc = hb_probe_flow_map_dev(ctx, B, ctx->s_xd, ctx->s_ud, df, dA, dB, dee);
-  if (rc) return rc;
-  D2H(f, df, sizeof(double) * B * NX); D2H(A, dA, sizeof(double) * B * TS); D2H(Bm, dB, sizeof(double) * B * TS);
-  if (ee) D2H(ee, dee, sizeof(double) * B * (24 + 36 * NX));
-  return hb_sync(ctx);
+  Staging s(ctx, B);
+  auto dx = s.in(x, NX); auto du = s.in(u, NU);
+  auto df = s.out(f, NX); auto dA = s.out(A, TS); auto dB = s.out(Bm, TS); auto dee = s.out(ee, 24 + 36 * NX);
+  return s.run([&] { return hb_probe_flow_map_dev(ctx, B, dx, du, df, dA, dB, dee); });
 }
 
 }  // extern "C"
