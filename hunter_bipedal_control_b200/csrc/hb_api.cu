@@ -90,12 +90,15 @@ __global__ void wbc_assemble_kernel(int B, hb_wbc_settings ws, const double* x_d
 }
 
 // Fused WeightedWbc step (K5+K6): assembly terms, reduced QP (tau and swing forces eliminated), interior point, expansion to
-// the reference's 38-vector [qdd, F, tau]. Shared memory per warp: QP workspace for n<=28 (the assembly scratch aliases the
-// factorisation area, which is dead until the first Newton step) + the reduced constraint matrix.
+// the reference's 38-vector [qdd, F, tau]. Shared memory per warp: QP workspace for n<=28 with the Hessian as a packed triangle (the
+// assembly scratch aliases the factorisation area, which is dead until the first Newton step) + the reduced constraint matrix.
 constexpr int WZ_N = 28, WZ_ME = 6, WZ_MI = 40, WZ_ROWS = 36;
-__host__ __device__ inline size_t wbc_fused_doubles() { return qp_workspace_doubles(WZ_N, WZ_ME, WZ_MI) + WZ_ROWS * WZ_N + 2 * WZ_ROWS + 3 * WZ_N + 16 + 8; }
+__host__ __device__ constexpr size_t wbc_fused_doubles() { return qp_workspace_doubles(WZ_N, WZ_ME, WZ_MI, true) + WZ_ROWS * WZ_N + 2 * WZ_ROWS + 3 * WZ_N + 16 + 8; }
+// One warp per block and one block per instance: 8 blocks per SM put a 1024-instance batch in one wave on 132 SMs (8 x 132 >= 1024;
+// at 7 a tail wave of 100 blocks costs almost as much as the full one). The runtime reserves 1 KB of shared memory per block.
+static_assert(8 * (wbc_fused_doubles() * sizeof(double) + 1024) <= 228 * 1024, "wbc_fused_kernel must fit 8 blocks per SM");
 
-__global__ void wbc_fused_kernel(int B, hb_wbc_settings ws, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const uint8_t* stance_mode,
+__global__ void __launch_bounds__(32, 8) wbc_fused_kernel(int B, hb_wbc_settings ws, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const uint8_t* stance_mode,
                                  double rho, int max_iter, double* sol, int32_t* status, int32_t* iters) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, wpb = blockDim.x >> 5, lane = threadIdx.x & 31;
@@ -103,8 +106,8 @@ __global__ void wbc_fused_kernel(int B, hb_wbc_settings ws, const double* x_des,
   if (inst >= B) return;
   double* base = reinterpret_cast<double*>(smem_raw) + (size_t)warp * wbc_fused_doubles();
   QpWorkspace w;
-  qp_carve(base, WZ_N, w, WZ_ME, WZ_MI);
-  double* p = base + qp_workspace_doubles(WZ_N, WZ_ME, WZ_MI);
+  qp_carve(base, WZ_N, w, WZ_ME, WZ_MI, true);
+  double* p = base + qp_workspace_doubles(WZ_N, WZ_ME, WZ_MI, true);
   double* Az = p; p += WZ_ROWS * WZ_N;
   double* lbz = p; p += WZ_ROWS;
   double* ubz = p; p += WZ_ROWS;
@@ -119,11 +122,11 @@ __global__ void wbc_fused_kernel(int B, hb_wbc_settings ws, const double* x_des,
   wbc_assemble_warp(x_des + (size_t)inst * NX, u_des + (size_t)inst * NU, rbd + (size_t)inst * 32, md, stance_mode ? stance_mode[inst] != 0 : false, ws, sh,
                     nullptr, nullptr, nullptr, nullptr, nullptr, &nw);
   int m = 0;
-  const int nz = wbc_reduced_build(sh, md, nw, stance_mode ? stance_mode[inst] != 0 : false, rho, ws, u_des + (size_t)inst * NU, w.H, qp_ld(WZ_N), gz, Az, lbz, ubz, stcol, m);
+  const int nz = wbc_reduced_build(sh, md, nw, stance_mode ? stance_mode[inst] != 0 : false, rho, ws, u_des + (size_t)inst * NU, w.H, gz, Az, lbz, ubz, stcol, m);
   if (lane < NJ) nlej[lane] = sh.nle[6 + lane];
   __syncwarp();
   // the workspace is carved for n = 28 (leading dimension 29); smaller problems (nz = 22, 16) use the same leading dimension
-  QpResult r = qp_solve_warp(nz, m, nullptr, gz, Az, lbz, ubz, 0.0, max_iter, xz, w);
+  QpResult r = qp_solve_warp<true>(nz, m, nullptr, gz, Az, lbz, ubz, 0.0, max_iter, xz, w);
   __syncwarp();
   double* out = sol + (size_t)inst * NWBC;
   if (lane < NQ) out[lane] = xz[lane];
@@ -1346,6 +1349,9 @@ int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
     attr((const void*)riccati_kernel, sizeof(RicShared));
     attr((const void*)forward_linesearch2_kernel, sizeof(Fw2Shared));
     attr((const void*)warm_shift_kernel, sizeof(double) * ((N + 1) * NX + N * NU));
+    // the one-block-per-instance kernels fit 8 blocks per SM only with the full shared-memory carveout; do not leave it to the driver
+    for (const void* fn : {(const void*)wbc_fused_kernel, (const void*)riccati_kernel})
+      if (fe == cudaSuccess) fe = cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
     if (fe != cudaSuccess) { ctx->last_cuda = (int)fe; hb_destroy(ctx); return HB_ECUDA; }
   }
   *out = ctx;

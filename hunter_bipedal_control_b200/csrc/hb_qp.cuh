@@ -30,13 +30,17 @@ struct QpWorkspace {
   int me_cap, mi_cap;   // capacity of the equality / one-sided inequality lists
 };
 
-__host__ __device__ inline int qp_ld(int n) { return n | 1; }
+__host__ __device__ constexpr int qp_ld(int n) { return n | 1; }
 
-// doubles needed by one warp for problems with n variables, <= me_cap equalities and <= mi_cap one-sided inequality entries
-__host__ __device__ inline size_t qp_workspace_doubles(int n, int me_cap = QP_MAX_EQ, int mi_cap = QP_MAX_IN) {
+// Lower triangle of a symmetric n x n matrix, row by row: entry (i, c), c <= i, at tri_row(i) + c
+__host__ __device__ constexpr int tri_row(int i) { return i * (i + 1) / 2; }
+
+// doubles needed by one warp for problems with n variables, <= me_cap equalities and <= mi_cap one-sided inequality entries;
+// packed_h: H is kept as its packed lower triangle (see qp_solve_warp)
+__host__ __device__ constexpr size_t qp_workspace_doubles(int n, int me_cap = QP_MAX_EQ, int mi_cap = QP_MAX_IN, bool packed_h = false) {
   const int ldn = qp_ld(n), lde = me_cap | 1;
   size_t d = 0;
-  d += (size_t)n * ldn;            // H
+  d += packed_h ? (size_t)tri_row(n) : (size_t)n * ldn;   // H
   d += (size_t)me_cap * ldn;       // Aeq
   d += (size_t)n * ldn;            // K
   d += (size_t)n * lde;            // V
@@ -49,11 +53,11 @@ __host__ __device__ inline size_t qp_workspace_doubles(int n, int me_cap = QP_MA
   return d;
 }
 
-__device__ inline void qp_carve(double* base, int n, QpWorkspace& w, int me_cap = QP_MAX_EQ, int mi_cap = QP_MAX_IN) {
+__device__ inline void qp_carve(double* base, int n, QpWorkspace& w, int me_cap = QP_MAX_EQ, int mi_cap = QP_MAX_IN, bool packed_h = false) {
   const int ldn = qp_ld(n), lde = me_cap | 1;
   w.ldn = ldn; w.ldv = lde; w.lds = lde; w.me_cap = me_cap; w.mi_cap = mi_cap;
   double* p = base;
-  w.H = p; p += n * ldn;
+  w.H = p; p += packed_h ? tri_row(n) : n * ldn;
   w.Aeq = p; p += me_cap * ldn;
   w.K = p; p += n * ldn;
   w.V = p; p += n * lde;
@@ -217,6 +221,9 @@ __device__ inline void warp_lit_mv(const double* M, int n, int ld, const double*
 struct QpResult { int status; int iters; };
 
 // A, lbA, ubA, H, g may live in global or shared memory (generic pointers). x_out: n doubles (generic).
+// PACKED_H: the caller assembled H in w.H as its packed lower triangle (tri_row) and passes H == nullptr; H must be exactly symmetric.
+// The products read the same values in the same order as with the full matrix, so the iterates are bit-identical.
+template <bool PACKED_H = false>
 __device__ inline QpResult qp_solve_warp(int n, int m, const double* __restrict__ H, const double* __restrict__ g,
                                          const double* __restrict__ A, const double* __restrict__ lbA,
                                          const double* __restrict__ ubA, double rho, int max_iter, double* x_out,
@@ -327,8 +334,14 @@ __device__ inline QpResult qp_solve_warp(int n, int m, const double* __restrict_
     __syncwarp();
     for (int i = lane; i < n; i += 32) {
       double a = w.g[i] + rho * w.x[i];
-      const double* hr = w.H + i * ldn;
-      for (int c = 0; c < n; ++c) a += hr[c] * w.x[c];
+      if (PACKED_H) {
+        const double* hr = w.H + tri_row(i);
+        for (int c = 0; c <= i; ++c) a += hr[c] * w.x[c];
+        for (int c = i + 1; c < n; ++c) a += w.H[tri_row(c) + i] * w.x[c];
+      } else {
+        const double* hr = w.H + i * ldn;
+        for (int c = 0; c < n; ++c) a += hr[c] * w.x[c];
+      }
       for (int e = 0; e < me; ++e) a += w.Aeq[e * ldn + i] * w.y[e];
       w.rd[i] = at_mul(i, a);
     }
@@ -355,7 +368,12 @@ __device__ inline QpResult qp_solve_warp(int n, int m, const double* __restrict_
     if (!(rdn == rdn) || !(rpn == rpn) || !(mu == mu) || rdn > 1e300 || rpn > 1e300) { res.status = 3; break; }
     if (rdn < 1e-10 * gs && rpn < 1e-10 * bs && mu < 1e-12) { res.status = 0; break; }
     // ---------------- K = H + rho I + D' W D
-    for (int idx = lane; idx < n * ldn; idx += 32) { const int i = idx / ldn, c = idx - i * ldn; w.K[idx] = w.H[idx] + ((i == c) ? rho : 0.0); }
+    // (only the lower triangle of K is read before the factorisation overwrites the upper one with L^-1)
+    if (PACKED_H) {
+      for (int idx = lane; idx < n * ldn; idx += 32) { const int i = idx / ldn, c = idx - i * ldn; if (c <= i) w.K[idx] = w.H[tri_row(i) + c] + ((i == c) ? rho : 0.0); }
+    } else {
+      for (int idx = lane; idx < n * ldn; idx += 32) { const int i = idx / ldn, c = idx - i * ldn; w.K[idx] = w.H[idx] + ((i == c) ? rho : 0.0); }
+    }
     __syncwarp();
     // lower triangle only; a two-sided row contributes once with the sum of its two weights
     for (int j = lane; j < mi; j += 32) {

@@ -29,7 +29,7 @@ constexpr int NTMAX = 16;   // free inputs after projection: 3 n_stance + (10 - 
 constexpr int NVMAX = 8;    // null-space columns kept for the velocity rows
 constexpr int PJ_AT = 0, PJ_BT = 484, PJ_BTV = 836, PJ_QT = 858, PJ_PT = 1342, PJ_RT = 1694, PJ_QV = 1950, PJ_RV = 1972,
               PJ_PXV = 1988, PJ_NV = 2208, PJ_PEV = 2288, PJ_META = 2298, PJ_STRIDE = 2320;
-// META: [0] nt, [1] n_stance_force_dims, [2] nv, [3] dt cost, [4] dt defect^2, [5] dt eq^2, [6] overflow flag
+// META: [0] nt, [1] n_stance_force_dims, [2] nv, [3] dt cost, [4] dt defect^2, [5] dt eq^2, [6] overflow flag, [7] dt
 constexpr int RK_STRIDE = NTMAX * NX + NTMAX;  // K (nt x 22, ld 22) + kff
 __host__ __device__ inline int ntp_of(int nt) { return nt <= 6 ? 6 : (nt <= 10 ? 10 : (nt <= 12 ? 12 : 16)); }
 
@@ -826,7 +826,7 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
     }
     out[PJ_BTV + lane] = s;
   }
-  if (lane == 0) { out[PJ_META] = nt; out[PJ_META + 1] = NF; out[PJ_META + 2] = nv; out[PJ_META + 3] = dt * cost; out[PJ_META + 4] = dt * d2; out[PJ_META + 5] = dt * e2; out[PJ_META + 6] = overflow ? 1.0 : 0.0; }
+  if (lane == 0) { out[PJ_META] = nt; out[PJ_META + 1] = NF; out[PJ_META + 2] = nv; out[PJ_META + 3] = dt * cost; out[PJ_META + 4] = dt * d2; out[PJ_META + 5] = dt * e2; out[PJ_META + 6] = overflow ? 1.0 : 0.0; out[PJ_META + 7] = dt; }
 }
 
 // Minimum resident warps per SM. 8 lets ptxas keep the kernel in 232 registers without spills; on H100 that beats 12 warps at 168
@@ -874,55 +874,109 @@ __global__ void __launch_bounds__(32, HB_LQ_MINB) lq_kernel(SqpArgs a) {
 // are zero (identity on the diagonal of R~), so the padded gains are zero.
 // TC: the result is stored transposed (C[j * ldc + i]): lanes then touch consecutive addresses -- the layout of choice whenever the
 // row-major leading dimension would be a multiple of 16 doubles (every lane in the same bank).
-template <int N, bool TA, int MODE, bool TC = false>
-__device__ __forceinline__ void rowmm(double* __restrict__ C, int ldc, const double* __restrict__ A, int lda,
-                                      const double* __restrict__ B, int ldb, int m, int kdim) {
+
+// acc_rows: c[j] = fma(a(k), B[k * ldb + j], c[j]) for k = 0 .. kn-1 in ascending order; a(k) is the lane's entry of the left operand.
+template <int N, class AF>
+__device__ __forceinline__ void acc_rows(double (&c)[N], AF a, const double* __restrict__ B, int ldb, int kn) {
+#pragma unroll 2
+  for (int k = 0; k < kn; ++k) {
+    const double ak = a(k);
+    const double* br = B + k * ldb;
+#pragma unroll
+    for (int j = 0; j < N; j += 2) {
+      const double2 b2 = *reinterpret_cast<const double2*>(br + j);
+      c[j] = fma(ak, b2.x, c[j]);
+      c[j + 1] = fma(ak, b2.y, c[j + 1]);
+    }
+  }
+}
+
+// the same for KN rows of the right operand given in closed form: c[j] = fma(a(k), b(k, j), c[j])
+template <int N, int KN, class AF, class BF>
+__device__ __forceinline__ void acc_rows_gen(double (&c)[N], AF a, BF b) {
+#pragma unroll 2
+  for (int k = 0; k < KN; ++k) {
+    const double ak = a(k);
+#pragma unroll
+    for (int j = 0; j < N; ++j) c[j] = fma(ak, b(k, j), c[j]);
+  }
+}
+
+// Row-owner shell: lane i < m owns row i of C (N columns): c starts at 0 (MODE 0) or at C (MODE 1), body(c, i) accumulates, c is stored.
+template <int N, int MODE, bool TC = false, class Body>
+__device__ __forceinline__ void rowmm_by(double* __restrict__ C, int ldc, int m, Body body) {
   const int i = lane_id();
   if (i < m) {
     double c[N];
 #pragma unroll
     for (int j = 0; j < N; ++j) c[j] = (MODE == 1) ? (TC ? C[j * ldc + i] : C[i * ldc + j]) : 0.0;
-#pragma unroll 2
-    for (int k = 0; k < kdim; ++k) {
-      const double a = TA ? A[k * lda + i] : A[i * lda + k];
-      const double* br = B + k * ldb;
-#pragma unroll
-      for (int j = 0; j < N; j += 2) {
-        const double2 b2 = *reinterpret_cast<const double2*>(br + j);
-        c[j] = fma(a, b2.x, c[j]);
-        c[j + 1] = fma(a, b2.y, c[j + 1]);
-      }
-    }
+    body(c, i);
 #pragma unroll
     for (int j = 0; j < N; ++j) { if (TC) C[j * ldc + i] = c[j]; else C[i * ldc + j] = c[j]; }
   }
   __syncwarp();
 }
 
+template <int N, bool TA, int MODE, bool TC = false>
+__device__ __forceinline__ void rowmm(double* __restrict__ C, int ldc, const double* __restrict__ A, int lda,
+                                      const double* __restrict__ B, int ldb, int m, int kdim) {
+  rowmm_by<N, MODE, TC>(C, ldc, m, [&](double (&c)[N], int i) { acc_rows(c, [&](int k) { return TA ? A[k * lda + i] : A[i * lda + k]; }, B, ldb, kdim); });
+}
+
 
 constexpr int SB_LD = 18;
-struct RicNodeIn { double At[TS], Bt[NX * NTMAX], bt[NX], qt[NX], rt[NTMAX], meta[8]; };
+// Node inputs as staged in shared memory. Of A~ (22 x 22) and B~ (22 x NTMAX) only the rows that carry data are staged: A~ rows 3..21
+// and B~ rows 3..11, plus N_v. The other rows are closed-form values that lq_node writes, regenerated here as the same doubles and
+// consumed by the same fma in the same order, so the recursion is bit-identical to one that stages the full matrices:
+//   A~ rows 0..2   the identity rows
+//   B~ rows 0..2   dt/m (dt * (1/m)) at row c % 3 of each stance-force column c < NF, zero elsewhere
+//   B~ rows 12..21 dt N_v on the null-space columns NF .. NF+nv-1, zero on the others
+struct RicNodeIn { double At3[19 * NX], Bt9[9 * NTMAX], Nv[NJ * NVMAX], bt[NX], qt[NX], rt[NTMAX], meta[8]; };
+struct BtGen {                                    // per-node data of the closed-form rows of B~, from the staged META
+  double dt, dtim; int nf, nv;
+  __device__ explicit BtGen(const double* meta) : dt(meta[7]), dtim(meta[7] * (1.0 / c_model.total_mass)), nf((int)meta[1]), nv((int)meta[2]) {}
+};
+__device__ __forceinline__ double bt_top(const BtGen& g, int k, int c) { return (c < g.nf && c % 3 == k) ? g.dtim : 0.0; }
+__device__ __forceinline__ double bt_null(const RicNodeIn& in, const BtGen& g, int r, int c) {
+  return (c >= g.nf && c - g.nf < g.nv) ? g.dt * in.Nv[r * NVMAX + c - g.nf] : 0.0;
+}
+// entry (k, c) of B~ and of A~ for a lane-owned column c; k is a compile-time index wherever these are called (unrolled loops)
+__device__ __forceinline__ double bt_entry(const RicNodeIn& in, const BtGen& g, int k, int c) {
+  return k < 3 ? bt_top(g, k, c) : (k < 12 ? in.Bt9[(k - 3) * NTMAX + c] : bt_null(in, g, k - 12, c));
+}
+__device__ __forceinline__ double at_entry(const RicNodeIn& in, int k, int c) { return k < 3 ? ((k == c) ? 1.0 : 0.0) : in.At3[(k - 3) * NX + c]; }
+// c[j] += sum_k a(k) B~[k][j] (B~ as the right operand), k = 0..21 in order
+template <int NTP, class AF>
+__device__ __forceinline__ void acc_bt(double (&c)[NTP], const RicNodeIn& in, const BtGen& g, AF a) {
+  acc_rows_gen<NTP, 3>(c, a, [&](int k, int j) { return bt_top(g, k, j); });
+  acc_rows(c, [&](int k) { return a(k + 3); }, in.Bt9, NTMAX, 9);
+  acc_rows_gen<NTP, NJ>(c, [&](int k) { return a(k + 12); }, [&](int k, int j) { return bt_null(in, g, k, j); });
+}
+
 struct RicShared {
   double S[TS], SA[TS];
-  RicNodeIn in[2];                                   // node data, staged one node ahead with cp.async
+  RicNodeIn in[2];                                   // node data, staged one node ahead by TMA
   double SBK[NX * SB_LD];                            // SB (22 x NTP, leading dimension 18: 2-way instead of 16-way bank conflicts on the row-owner stores), later K (NTMAX x 22)
   double Hux[NTMAX * NX], Huu[NTMAX * 18];           // Hux input-major (NTMAX x 22): lanes = state index touch consecutive addresses
-  double sv[NX], sb[NX], hu[NTMAX], kff[NTMAX], idg[NTMAX];
+  double sv[NX], sb[NX], hu[NTMAX], kff[NTMAX];
   unsigned long long bar[4];                         // mbarriers of the TMA staging: node inputs (two buffers), Pt / Rt, Qt
-  unsigned short pair[NX * (NX - 1) / 2];            // (i << 8 | j), j > i: the strict upper triangle of S, one entry per symmetrisation task
 };
 static_assert(sizeof(RicNodeIn) % 16 == 0 && (TS * sizeof(double)) % 16 == 0 && (NX * NTMAX * sizeof(double)) % 16 == 0, "bulk copies need 16-byte multiples");
+// One block per instance: 8 blocks per SM put a 1024-instance batch in one wave on 132 SMs (8 x 132 >= 1024; at 7 a tail wave of 100
+// blocks costs almost as much as the full one). The runtime reserves 1 KB of shared memory per block.
+static_assert(8 * (sizeof(RicShared) + 1024) <= 228 * 1024, "riccati_kernel must fit 8 blocks per SM");
 
-// node inputs by TMA: one elected lane arms the buffer's mbarrier with the byte count and issues six bulk copies (At, Bt, bt, qt, rt, meta)
+// node inputs by TMA: one elected lane arms the buffer's mbarrier with the byte count and issues the bulk copies
 __device__ __forceinline__ void ric_prefetch_tma(RicNodeIn& n, const double* __restrict__ rec, unsigned long long* bar) {
   fence_proxy_async();
   mbar_expect_tx(bar, (unsigned)sizeof(RicNodeIn));
-  bulk_g2s(n.At, rec + PJ_AT, TS * sizeof(double), bar);
-  bulk_g2s(n.Bt, rec + PJ_BT, NX * NTMAX * sizeof(double), bar);
-  bulk_g2s(n.bt, rec + PJ_BTV, NX * sizeof(double), bar);
-  bulk_g2s(n.qt, rec + PJ_QV, NX * sizeof(double), bar);
-  bulk_g2s(n.rt, rec + PJ_RV, NTMAX * sizeof(double), bar);
-  bulk_g2s(n.meta, rec + PJ_META, 8 * sizeof(double), bar);
+  bulk_g2s(n.At3, rec + PJ_AT + 3 * NX, sizeof(n.At3), bar);
+  bulk_g2s(n.Bt9, rec + PJ_BT + 3 * NTMAX, sizeof(n.Bt9), bar);
+  bulk_g2s(n.Nv, rec + PJ_NV, sizeof(n.Nv), bar);
+  bulk_g2s(n.bt, rec + PJ_BTV, sizeof(n.bt), bar);
+  bulk_g2s(n.qt, rec + PJ_QV, sizeof(n.qt), bar);
+  bulk_g2s(n.rt, rec + PJ_RV, sizeof(n.rt), bar);
+  bulk_g2s(n.meta, rec + PJ_META, sizeof(n.meta), bar);
 }
 
 // One node of the recursion, executed by the TWO warps of the block. The products that do not depend on each other are split
@@ -932,15 +986,23 @@ template <int NTP>
 __device__ __noinline__ void riccati_node(RicShared& sh, const RicNodeIn& in, const double* __restrict__ rec, double* __restrict__ rk, bool& fail,
                                           int warp, unsigned ph) {
   const int lane = lane_id();
+  const BtGen g(in.meta);
   double* SB = sh.SBK; double* K = sh.SBK;
   // ---- phase A: [SA | SB | sb] = S [At | Bt | bt] (+ s): 22 + NTP + 1 result columns, split 16 / rest. S is exactly symmetric (both halves
   // are written with the same value at the end of every node), so lane i reads its row as column i: consecutive addresses, no bank conflicts
+  // (S^T: lane i reads S[k][i]; the identity rows of At contribute through fma with 1.0 / 0.0 as in the full product)
   if (warp == 0) {
-    rowmm<16, true, 0>(sh.SA, NX, sh.S, NX, in.At, NX, NX, NX);
+    rowmm_by<16, 0>(sh.SA, NX, NX, [&](double (&c)[16], int i) {
+      acc_rows_gen<16, 3>(c, [&](int k) { return sh.S[k * NX + i]; }, [](int k, int j) { return (k == j) ? 1.0 : 0.0; });
+      acc_rows(c, [&](int k) { return sh.S[(k + 3) * NX + i]; }, in.At3, NX, 19);
+    });
     mbar_wait(&sh.bar[2], ph);                // Pt / Rt staged by this warp at the top of the node
   } else {
-    rowmm<6, true, 0>(sh.SA + 16, NX, sh.S, NX, in.At + 16, NX, NX, NX);
-    rowmm<NTP, true, 0>(SB, SB_LD, sh.S, NX, in.Bt, NTMAX, NX, NX);
+    rowmm_by<6, 0>(sh.SA + 16, NX, NX, [&](double (&c)[6], int i) {
+      acc_rows_gen<6, 3>(c, [&](int k) { return sh.S[k * NX + i]; }, [](int, int) { return 0.0; });
+      acc_rows(c, [&](int k) { return sh.S[(k + 3) * NX + i]; }, in.At3 + 16, NX, 19);
+    });
+    rowmm_by<NTP, 0>(SB, SB_LD, NX, [&](double (&c)[NTP], int i) { acc_bt(c, in, g, [&](int k) { return sh.S[k * NX + i]; }); });
     if (lane < NX) {
       double s0 = sh.sv[lane], s1 = 0.0;
 #pragma unroll
@@ -951,22 +1013,27 @@ __device__ __noinline__ void riccati_node(RicShared& sh, const RicNodeIn& in, co
   __syncthreads();
   // ---- phase B: Hux (NTP x 22, stored input-major) = Pt + Bt^T SA (warp 0: row-owner over the state index, transposed store) ; Huu = Rt + Bt^T SB, hu = rt + Bt^T sb (warp 1)
   if (warp == 0) {
-    rowmm<NTP, true, 1, true>(sh.Hux, NX, sh.SA, NX, in.Bt, NTMAX, NX, NX);
+    rowmm_by<NTP, 1, true>(sh.Hux, NX, NX, [&](double (&c)[NTP], int i) { acc_bt(c, in, g, [&](int k) { return sh.SA[k * NX + i]; }); });
   } else {
     // S is dead until phase C: stage Qt into it now (arrives while Huu is formed)
     if (lane == 0) { fence_proxy_async(); mbar_expect_tx(&sh.bar[3], TS * sizeof(double)); bulk_g2s(sh.S, rec + PJ_QT, TS * sizeof(double), &sh.bar[3]); }
-    rowmm<NTP, true, 1>(sh.Huu, 18, in.Bt, NTMAX, SB, SB_LD, NTP, NX);
+    rowmm_by<NTP, 1>(sh.Huu, 18, NTP, [&](double (&c)[NTP], int i) {      // Bt^T: lane i owns column i of Bt
+      acc_rows(c, [&](int k) { return bt_top(g, k, i); }, SB, SB_LD, 3);
+      acc_rows(c, [&](int k) { return in.Bt9[k * NTMAX + i]; }, SB + 3 * SB_LD, SB_LD, 9);
+      acc_rows(c, [&](int k) { return bt_null(in, g, k, i); }, SB + 12 * SB_LD, SB_LD, NJ);
+    });
     if (lane < NTP) {
       double s0 = in.rt[lane];
 #pragma unroll
-      for (int k = 0; k < NX; ++k) s0 = fma(in.Bt[k * NTMAX + lane], sh.sb[k], s0);
+      for (int k = 0; k < NX; ++k) s0 = fma(bt_entry(in, g, k, lane), sh.sb[k], s0);
       sh.hu[lane] = s0;
     }
   }
   __syncthreads();
   // ---- phase C: gains (warp 0) || S = Qt + At' SA (warp 1)
   // (Measured and rejected: factorising Huu in warp 1's phase-B slack and keeping the factor in registers across the barrier -- the
-  // kernel needs 255 registers then, and capped at 7 blocks/SM the factor lives in local memory, which is slower.)
+  // kernel needs 255 registers then, and capped for occupancy the factor lives in local memory, which is slower. 8 blocks/SM, which
+  // puts 1024 instances in one wave, leave 128 registers per thread.)
   if (warp == 0) {
     // Cholesky of the symmetrised Huu entirely in registers: lane i owns row i (right-looking, column by column, the pivot column is
     // broadcast with shuffles), then forward / backward substitution of the 22 + 1 right-hand sides, one per lane, with the factor
@@ -1016,7 +1083,7 @@ __device__ __noinline__ void riccati_node(RicShared& sh, const RicNodeIn& in, co
     if (lane < NX) {
       double s0 = in.qt[lane], s1 = 0.0;
 #pragma unroll
-      for (int k = 0; k < NX; k += 2) { s0 = fma(in.At[k * NX + lane], sh.sb[k], s0); s1 = fma(in.At[(k + 1) * NX + lane], sh.sb[k + 1], s1); }
+      for (int k = 0; k < NX; k += 2) { s0 = fma(at_entry(in, k, lane), sh.sb[k], s0); s1 = fma(at_entry(in, k + 1, lane), sh.sb[k + 1], s1); }
 #pragma unroll
       for (int c = 0; c < NTP; ++c) s0 = fma(sh.Hux[c * NX + lane], sh.kff[c], s0);
       sh.sv[lane] = s0 + s1;
@@ -1024,22 +1091,28 @@ __device__ __noinline__ void riccati_node(RicShared& sh, const RicNodeIn& in, co
   } else {
     mbar_wait(&sh.bar[3], ph);   // Qt has landed in S
     __syncwarp();
-    rowmm<NX, true, 1>(sh.S, NX, in.At, NX, sh.SA, NX, NX, NX);
+    rowmm_by<NX, 1>(sh.S, NX, NX, [&](double (&c)[NX], int i) {          // At^T: lane i owns column i of At
+      acc_rows(c, [&](int k) { return (k == i) ? 1.0 : 0.0; }, sh.SA, NX, 3);
+      acc_rows(c, [&](int k) { return in.At3[k * NX + i]; }, sh.SA + 3 * NX, NX, 19);
+    });
   }
   __syncthreads();
   // ---- phase D: S += Hux' K, result columns split 12 / 10
   if (warp == 0) rowmm<12, true, 1>(sh.S, NX, sh.Hux, NX, K, NX, NX, NTP);
   else rowmm<10, true, 1>(sh.S + 12, NX, sh.Hux, NX, K + 12, NX, NX, NTP);
   __syncthreads();
-  // S <- (S + S') / 2: one (i, j) pair per thread and round, 231 pairs = 4 rounds of 64 threads
+  // S <- (S + S') / 2: one (i, j) pair per thread and round, 231 pairs = 4 rounds of 64 threads. Pair t is (i, (i + d) mod 22) with
+  // i = t mod 22, d = t / 22 + 1: d = 1..10 gives every pair at cyclic distance 1..10 once, d = 11 (t = 220..230) the 11 pairs (i, i + 11)
   for (int t = threadIdx.x; t < NX * (NX - 1) / 2; t += 64) {
-    const int pr = sh.pair[t], i = pr >> 8, j = pr & 255;
+    const int d = t / NX + 1, i = t - (d - 1) * NX, j = (i + d) % NX;
     const double v = 0.5 * (sh.S[i * NX + j] + sh.S[j * NX + i]);
     sh.S[i * NX + j] = v; sh.S[j * NX + i] = v;
   }
   __syncthreads();
 }
 
+// 128 registers x 64 threads also allow 8 blocks per SM. ptxas reaches 128 without spills on its own; a minimum-blocks bound of 8 (or
+// __maxnreg__(128)) makes it spill 40 B around the riccati_node calls at the same register count, so the bound is left out.
 __global__ void __launch_bounds__(64) riccati_kernel(SqpArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   RicShared& sh = *reinterpret_cast<RicShared*>(smem_raw);
@@ -1052,10 +1125,6 @@ __global__ void __launch_bounds__(64) riccati_kernel(SqpArgs a) {
   if (warp == 1 && lane == 0) ric_prefetch_tma(sh.in[(N - 1) & 1], proj + (size_t)(N - 1) * PJ_STRIDE, &sh.bar[(N - 1) & 1]);
   unsigned ph_in0 = 0u, ph_in1 = 0u;
   for (int idx = threadIdx.x; idx < TS; idx += 64) sh.S[idx] = 0.0;   // no terminal cost (SURVEY App. B)
-  for (int idx = threadIdx.x; idx < TS; idx += 64) {
-    const int i = idx / NX, j = idx - i * NX;
-    if (j > i) sh.pair[i * NX - i * (i + 1) / 2 + (j - i - 1)] = (unsigned short)((i << 8) | j);
-  }
   if (threadIdx.x < NX) sh.sv[threadIdx.x] = 0.0;
   bool fail = false;
   double merit = 0.0, dyn = 0.0, eqs = 0.0;

@@ -8,6 +8,7 @@
 // The QP (H, g, A, lbA, ubA) is written in the reference's own layout (qpOASES row-major, WeightedWbc.cpp:27-41).
 #pragma once
 #include "hb_common.cuh"
+#include "hb_qp.cuh"
 #include "hb_rbd.cuh"
 #include "../../include/hunter_b200.h"
 
@@ -246,9 +247,10 @@ __device__ inline int wbc_assemble_warp(const double* __restrict__ x_des, const 
 // Reduced WeightedWbc QP for the fused path: tau = M_j qdd - J_j' F + nle_j and F_swing = 0 are substituted, leaving
 //   z = [qdd(16), F_stance(3 n_st)],  6 equalities (base rows of the EoM), 10 two-sided torque rows, 5 friction rows per
 // stance contact. The Tikhonov term rho ||[qdd, F, tau]||^2 of the full problem is carried over exactly (rho I + rho T'T).
-// Hz is written into `Hw` (leading dimension ldh), rows of Az have stride nz. Returns nz; m_out = number of rows.
+// Hz is written into `Hw` as its packed lower triangle (tri_row; Hz is exactly symmetric: entry (i, j) and (j, i) are the same products
+// summed in the same order), rows of Az have stride nz. Returns nz; m_out = number of rows.
 __device__ inline int wbc_reduced_build(const WbcShared& sh, int mode, int nw, bool stance_mode, double rho, const hb_wbc_settings& ws, const double* __restrict__ u_des,
-                                        double* Hw, int ldh, double* gz, double* Az, double* lbz, double* ubz, int* stcol /*12*/, int& m_out) {
+                                        double* Hw, double* gz, double* Az, double* lbz, double* ubz, int* stcol /*12*/, int& m_out) {
   const int lane = lane_id();
   int nst = 0;
   for (int j = 0; j < 12; ++j) if (contact_flag(mode, j / 3)) { if (lane == 0) stcol[nst] = j; ++nst; }
@@ -282,12 +284,13 @@ __device__ inline int wbc_reduced_build(const WbcShared& sh, int mode, int nw, b
   const double wf2 = stance_mode ? 0.0 : ws.weight_contact_force * ws.weight_contact_force;
   for (int idx = lane; idx < nz * nz; idx += 32) {
     const int i = idx / nz, j = idx - i * nz;
+    if (j > i) continue;
     double s = (i == j) ? rho : 0.0;
     if (i == j && i >= NQ) s += wf2;                      // contact-force task on the stance forces (swing forces are eliminated at zero)
     if (i < NQ && j < NQ) for (int r = 0; r < nw; ++r) s += sh.Aw[r * 16 + i] * sh.Aw[r * 16 + j];
     double t = 0.0;
     for (int r = 0; r < NJ; ++r) t += Tm[r * nz + i] * Tm[r * nz + j];
-    Hw[i * ldh + j] = s + rho * t;
+    Hw[tri_row(i) + j] = s + rho * t;
   }
   for (int i = lane; i < nz; i += 32) {
     double s = 0.0;
