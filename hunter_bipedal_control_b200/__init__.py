@@ -4,7 +4,9 @@ Only what the path needs: ``csrc/`` (sm_90a CUDA kernels + the C ABI of include/
 host-side mirrors of the reference's WbcBase / MPC_MRT_Interface calls). No CPU fallback exists.
 """
 from .api import (HbWbcSettings, HbTaskInfo, parse_task_info, Context, WeightedWbc, HierarchicalWbc, HbHoqpProblem, make_hoqp_problems, hoqp_tasks, SqpMpc, HbReference, HbSolveInfo, HbConfig, HunterB200Error, load_library, EXPORTED_SYMBOLS,
-                  NX, NU, NQ, NJ, NWBC, INFO_DTYPE, HbPlanInput, plan_references, plan_set_threads, make_plan_inputs, GAIT_IDS, GaitSelector, HbPdGains, default_pd_gains, HbKfState, HbKfParams, default_kf_params, kf_states, HbObserverState, observer_states, HbActuationState, HbSimParams, default_sim_params, actuation_states)
+                  NX, NU, NQ, NJ, NWBC, INFO_DTYPE, HbPlanInput, plan_references, plan_set_threads, make_plan_inputs, GAIT_IDS, GaitSelector, HbPdGains, default_pd_gains, HbKfState, HbKfParams, default_kf_params, kf_states, HbObserverState, observer_states, HbActuationState, HbSimParams, default_sim_params, actuation_states,
+                  HbRolloutCommand, HbRolloutParams, ROLLOUT_STATS_DTYPE, ROLLOUT_FAIL, default_rollout_params, rollout_stats, make_rollout_commands)
 
 __all__ = ["HbWbcSettings", "HbTaskInfo", "parse_task_info", "Context", "WeightedWbc", "HierarchicalWbc", "HbHoqpProblem", "make_hoqp_problems", "hoqp_tasks", "SqpMpc", "HbReference", "HbSolveInfo", "HbConfig", "HunterB200Error", "load_library",
-           "EXPORTED_SYMBOLS", "NX", "NU", "NQ", "NJ", "NWBC", "INFO_DTYPE", "HbPlanInput", "plan_references", "plan_set_threads", "make_plan_inputs", "GAIT_IDS", "GaitSelector", "HbPdGains", "default_pd_gains", "HbKfState", "HbKfParams", "default_kf_params", "kf_states", "HbObserverState", "observer_states", "HbActuationState", "HbSimParams", "default_sim_params", "actuation_states"]
+           "EXPORTED_SYMBOLS", "NX", "NU", "NQ", "NJ", "NWBC", "INFO_DTYPE", "HbPlanInput", "plan_references", "plan_set_threads", "make_plan_inputs", "GAIT_IDS", "GaitSelector", "HbPdGains", "default_pd_gains", "HbKfState", "HbKfParams", "default_kf_params", "kf_states", "HbObserverState", "observer_states", "HbActuationState", "HbSimParams", "default_sim_params", "actuation_states",
+           "HbRolloutCommand", "HbRolloutParams", "ROLLOUT_STATS_DTYPE", "ROLLOUT_FAIL", "default_rollout_params", "rollout_stats", "make_rollout_commands"]

@@ -36,6 +36,7 @@ EXPORTED_SYMBOLS = [
     "hb_resident_wbc_batch_dev", "hb_resident_wbc_batch",
     "hb_time_grid_batch_dev", "hb_reference_expand_grid_batch_dev", "hb_mpc_solve_grid_batch_dev", "hb_policy_eval_grid_batch_dev",
     "hb_time_grid_batch", "hb_reference_expand_grid_batch", "hb_mpc_solve_grid_batch", "hb_resident_read_grid_batch", "hb_resident_write_batch",
+    "hb_default_rollout_params", "hb_rollout_batch_dev",
 ]
 
 
@@ -162,6 +163,62 @@ def actuation_states(B):
     st = (HbActuationState * B)()
     _check(load_library().hb_actuation_reset(B, st), "hb_actuation_reset")
     return st
+
+
+HB_ROLLOUT_MAX_CMDS = 8
+ROLLOUT_FAIL = {"estop": 1, "orientation": 2, "height": 4, "nonfinite": 8}     # hb_rollout_stats.fail_reason bits
+
+
+class HbRolloutCommand(C.Structure):
+    _fields_ = [("gait", C.c_int32), ("gait_start", C.c_double), ("n_cmd", C.c_int32), ("cmd_time", C.c_double * HB_ROLLOUT_MAX_CMDS),
+                ("cmd_vel", (C.c_double * 4) * HB_ROLLOUT_MAX_CMDS)]
+
+
+class HbRolloutParams(C.Structure):
+    _fields_ = [("period", C.c_double), ("mpc_every", C.c_int32), ("actuation_delay", C.c_double), ("sim", HbSimParams), ("gains", HbPdGains),
+                ("torque_limit", C.c_double * 10), ("min_base_height", C.c_double), ("log_every", C.c_int32)]
+
+
+ROLLOUT_STATS_DTYPE = np.dtype([("fail_tick", "i4"), ("fail_reason", "i4"), ("mpc_bad", "i4"), ("wbc_fallbacks", "i4"), ("plan_rejects", "i4"),
+                                ("max_abs_torque", "f8")], align=True)
+
+
+def default_rollout_params():
+    p = HbRolloutParams()
+    _check(load_library().hb_default_rollout_params(C.byref(p)), "hb_default_rollout_params")
+    return p
+
+
+def rollout_stats(B):
+    """Stats of B fresh episodes: zeros, fail_tick = -1."""
+    st = np.zeros(B, dtype=ROLLOUT_STATS_DTYPE)
+    st["fail_tick"] = -1
+    return st
+
+
+def make_rollout_commands(gait, gait_start, cmd_times, cmd_vels):
+    """ctypes array of HbRolloutCommand. cmd_vels: [n, 4] (one schedule for the batch) or [B, n, 4]; cmd_times: [n] or [B, n], ascending;
+    gait (name or id) and gait_start: one for the batch or one per instance. cmd_vels[.., j, :] holds from cmd_times[.., j] on."""
+    vel = _f64(cmd_vels)
+    tim = _f64(cmd_times)
+    sizes = [vel.shape[0] if vel.ndim == 3 else 1, tim.shape[0] if tim.ndim == 2 else 1, np.size(gait_start)]
+    if not isinstance(gait, str) and np.ndim(gait) > 0:
+        sizes.append(len(gait))
+    B = max(sizes)
+    n = vel.shape[-2]
+    if not 1 <= n <= HB_ROLLOUT_MAX_CMDS or tim.shape[-1] != n:
+        raise ValueError("cmd_times / cmd_vels: 1..%d segments of the same count expected" % HB_ROLLOUT_MAX_CMDS)
+    vel = np.broadcast_to(vel, (B, n, 4)); tim = np.broadcast_to(tim, (B, n))
+    gids = _gait_ids(gait, B); start = np.broadcast_to(_f64(gait_start), (B,))
+    cmds = (HbRolloutCommand * B)()
+    for i in range(B):
+        c = cmds[i]
+        c.gait = gids[i]; c.gait_start = start[i]; c.n_cmd = n
+        for j in range(n):
+            c.cmd_time[j] = tim[i, j]
+            for k in range(4):
+                c.cmd_vel[j][k] = vel[i, j, k]
+    return cmds
 
 
 class HbObserverState(C.Structure):
@@ -630,6 +687,30 @@ class Context:
     def resident_cycle_dev(self, cold_start, t_rel, t0, x0, refs_dev_ptr, rbd, info, sol, tau, status=None):
         _check(self._lib.hb_resident_cycle_batch_dev(self._h, x0.shape[0], 1 if cold_start else 0, C.c_double(t_rel), _ptr(t0), _ptr(x0), C.c_void_p(refs_dev_ptr),
                                                      _ptr(rbd), _ptr(info), _ptr(sol), _ptr(tau), _ptr(status)), "hb_resident_cycle_batch_dev", self._h)
+
+    def rollout(self, rbd, commands, n_ticks, tick0=0, params=None, act=None, estop=None, stats=None, log_every=0):
+        """n_ticks ticks of closed-loop episodes on the device (hb_rollout_batch_dev). rbd: cuda float64 tensor [B, 32], advanced in place;
+        commands: ctypes array of HbRolloutCommand (make_rollout_commands); act: cuda uint8 tensor of B hb_actuation_state (None: fresh, in
+        place); estop: cuda uint8 tensor [B] (None: zeros, in place); stats: ROLLOUT_STATS_DTYPE array (None: rollout_stats(B)).
+        Returns (rbd, act, estop, stats, log): stats as a new structured array, log a cuda tensor [B, ceil(n_ticks / log_every), 32] or None.
+        Waits for the episode to finish (the stats are read back)."""
+        import torch
+        B = rbd.shape[0]
+        dev = rbd.device
+        params = params or default_rollout_params()
+        params.log_every = int(log_every)
+        if act is None:
+            act = torch.zeros(B * C.sizeof(HbActuationState), dtype=torch.uint8, device=dev)
+        if estop is None:
+            estop = torch.zeros(B, dtype=torch.uint8, device=dev)
+        st = rollout_stats(B) if stats is None else np.ascontiguousarray(stats, dtype=ROLLOUT_STATS_DTYPE)
+        d_st = torch.from_numpy(st.view(np.uint8).copy()).to(dev)
+        log = torch.zeros((B, -(-n_ticks // log_every), 32), dtype=torch.float64, device=dev) if log_every > 0 else None
+        torch.cuda.current_stream(dev).synchronize()          # the context's stream does not order itself after torch's
+        _check(self._lib.hb_rollout_batch_dev(self._h, B, C.c_int64(tick0), int(n_ticks), C.byref(params), commands, _ptr(rbd), _ptr(act), _ptr(estop),
+                                              _ptr(d_st), _ptr(log)), "hb_rollout_batch_dev", self._h)
+        self.sync()
+        return rbd, act, estop, d_st.cpu().numpy().view(ROLLOUT_STATS_DTYPE), log
 
     def control_step_dev(self, t_rel, x0, x_ref, swing, mode, rbd, xt, ut, info, sol, tau, status=None):
         _check(self._lib.hb_control_step_batch_dev(self._h, x0.shape[0], C.c_double(t_rel), _ptr(x0), _ptr(x_ref), _ptr(swing), _ptr(mode), _ptr(rbd), _ptr(xt),

@@ -24,6 +24,7 @@
 #include "hb_sqp.cuh"
 #include "hb_wbc.cuh"
 #include "hb_hoqp.cuh"
+#include "hb_rollout.cuh"
 
 using namespace hb;
 
@@ -721,18 +722,7 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
 __global__ void rbd_to_centroidal_kernel(int B, const double* rbd, double* x) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
-  const double* r = rbd + (size_t)inst * 32;
-  double q[NQ], v[NQ];
-  for (int i = 0; i < 3; ++i) { q[i] = r[3 + i]; q[3 + i] = r[i]; v[i] = r[NQ + 3 + i]; }
-  for (int j = 0; j < NJ; ++j) { q[6 + j] = r[6 + j]; v[6 + j] = r[NQ + 6 + j]; }
-  double sz, cz, sy, cy;
-  sincos(q[3], &sz, &cz); sincos(q[4], &sy, &cy);
-  const double dxr = (cz * r[NQ] + sz * r[NQ + 1]) / cy;
-  v[5] = dxr; v[4] = -sz * r[NQ] + cz * r[NQ + 1]; v[3] = r[NQ + 2] + sy * dxr;
-  KinOut<double> o;
-  kin_pass<double>(q, v, o);
-  for (int i = 0; i < 6; ++i) x[(size_t)inst * NX + i] = o.h[i] / c_model.total_mass;
-  for (int i = 0; i < NQ; ++i) x[(size_t)inst * NX + 6 + i] = q[i];
+  rbd_to_centroidal(rbd + (size_t)inst * 32, x + (size_t)inst * NX);
 }
 
 // Expansion of the compact reference description onto the node grid (SwitchedModelReferenceManager::modifyReferences
@@ -1057,6 +1047,11 @@ struct hb_ctx {
   int res_valid;                      // number of instances holding a previous solution
   double* res_sol; int res_sol_valid;   // last good WBC solution per instance (WeightedWbc fallback, W5)
   double* res_stance;                 // the device planner's latest stance positions (row N1)
+  // hb_rollout_batch_dev's scratch, allocated at max_batch by its first call: commands, plan inputs -> planner -> cycle, the tick's WBC
+  // solution / joint command / torques, the states held instances are put back to, the tick time
+  void* ro_mem;
+  hb_rollout_command* ro_cmd; hb_plan_input* ro_in; hb_reference* ro_refs; hb_solve_info* ro_info; int32_t* ro_pstat;
+  double *ro_t0, *ro_x0, *ro_feet, *ro_sol, *ro_jcmd, *ro_jtau, *ro_tau, *ro_held, *ro_tnow;
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
   // hb_resident_cycle_batch's packed references / reference verdicts
   void* arena; size_t arena_cap;
@@ -1363,7 +1358,7 @@ int hb_destroy(hb_ctx* ctx) {
   cudaSetDevice(ctx->device);
   void* ptrs[] = {ctx->lin, ctx->proj, ctx->rk, ctx->dxt, ctx->dut, ctx->perf, ctx->flags, ctx->xdes, ctx->udes, ctx->wstatus, ctx->witers, ctx->wmode,
                   ctx->hoqp_scratch, ctx->hoqp_prob, ctx->cyc_xref, ctx->cyc_swing, ctx->cyc_tk, ctx->cyc_mode, ctx->cyc_nn, ctx->res_t0, ctx->res_xt,
-                  ctx->res_ut, ctx->res_tk, ctx->res_mode, ctx->res_nn, ctx->res_sol, ctx->res_stance, ctx->arena};
+                  ctx->res_ut, ctx->res_tk, ctx->res_mode, ctx->res_nn, ctx->res_sol, ctx->res_stance, ctx->arena, ctx->ro_mem};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -1630,9 +1625,11 @@ __global__ void set_times_kernel(int B, int N, const double* t0_new, double* t0_
   }
 }
 
-int hb_resident_cycle_batch_dev(hb_ctx* ctx, int B, int cold_start, double t_rel, const double* t0, const double* x0, const hb_reference* refs,
-                                const double* rbd, hb_solve_info* info, double* wbc_sol, double* torque, int32_t* wbc_status) {
-  if (!ctx || B < 0 || !t0 || !x0 || !refs || !rbd || !wbc_sol) return HB_EINVAL;
+// hb_resident_cycle_batch_dev; with run_wbc = false the cycle ends after the SQP iteration (hb_rollout_batch_dev: the 500 Hz tick at the
+// same time is the WBC of that cycle, so the cycle's own would be thrown away)
+static int resident_cycle_impl(hb_ctx* ctx, int B, int cold_start, double t_rel, const double* t0, const double* x0, const hb_reference* refs,
+                               const double* rbd, hb_solve_info* info, double* wbc_sol, double* torque, int32_t* wbc_status, bool run_wbc) {
+  if (!ctx || B < 0 || !t0 || !x0 || !refs || !rbd) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (ctx->base + B > ctx->cfg.max_batch) return HB_ECAP;
   if (!cold_start && ctx->res_valid < ctx->base + B) return HB_EINVAL;     // no previous solution to shift
@@ -1663,6 +1660,7 @@ int hb_resident_cycle_batch_dev(hb_ctx* ctx, int B, int cold_start, double t_rel
   if (rc) return rc;
   CK(cudaMemcpyAsync(ctx->res_mode + o * (N + 1), mode, sizeof(int32_t) * B * (N + 1), cudaMemcpyDeviceToDevice, ctx->stream));
   if (ctx->res_valid < ctx->base + B) ctx->res_valid = ctx->base + B;
+  if (!run_wbc) return mpc_solve_impl(ctx, B, x0, xref, swing, mode, xt, ut, info, tk, nn);
   rc = control_step_impl(ctx, B, t_rel, x0, xref, swing, mode, rbd, xt, ut, info, wbc_sol, torque, wbc_status, tk, nn);
   if (rc) return rc;
   if (wbc_status) {
@@ -1672,6 +1670,12 @@ int hb_resident_cycle_batch_dev(hb_ctx* ctx, int B, int cold_start, double t_rel
     if (ctx->res_sol_valid < ctx->base + B) ctx->res_sol_valid = ctx->base + B;
   }
   return HB_OK;
+}
+
+int hb_resident_cycle_batch_dev(hb_ctx* ctx, int B, int cold_start, double t_rel, const double* t0, const double* x0, const hb_reference* refs,
+                                const double* rbd, hb_solve_info* info, double* wbc_sol, double* torque, int32_t* wbc_status) {
+  if (!wbc_sol) return HB_EINVAL;
+  return resident_cycle_impl(ctx, B, cold_start, t_rel, t0, x0, refs, rbd, info, wbc_sol, torque, wbc_status, true);
 }
 
 int hb_plan_references_batch_dev(hb_ctx* ctx, int B, const hb_plan_input* in, const double* feet, double* latest_stance, hb_reference* out,
@@ -1867,8 +1871,9 @@ int hb_sim_step_batch_dev(hb_ctx* ctx, int B, const hb_sim_params* params, doubl
   return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, *params, rbd, tau, contact_force, contact_flag);
 }
 
-int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
-                              int32_t* mode_out, double* wbc_sol, double* torque, int32_t* wbc_status) {
+// hb_resident_wbc_batch_dev; no_prev = true: the fallback has no previous solution yet (first tick after a cold start whose cycle ran no WBC)
+static int resident_wbc_impl(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
+                             int32_t* mode_out, double* wbc_sol, double* torque, int32_t* wbc_status, bool no_prev) {
   if (!ctx || B < 0 || !t_now || !rbd || !x_des || !u_des || !mode_out || !wbc_sol) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (ctx->base + B > ctx->res_valid) return HB_EINVAL;             // no resident solution to evaluate
@@ -1883,12 +1888,97 @@ int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const dou
   if (!rc && torque) rc = launch(ctx, K_UNPROFILED, torque_kernel, (B * NJ + 127) / 128, 128, 0, B, wbc_sol, torque);
   if (rc) return rc;
   if (wbc_status) {
-    const int have_prev = (ctx->res_sol_valid >= ctx->base + B) ? 1 : 0;
+    const int have_prev = (!no_prev && ctx->res_sol_valid >= ctx->base + B) ? 1 : 0;
     rc = launch(ctx, K_UNPROFILED, wbc_fallback_kernel, (B * NWBC + 127) / 128, 128, 0, B, have_prev, wbc_status, wbc_sol, ctx->res_sol + o * NWBC, torque);
     if (rc) return rc;
     if (ctx->res_sol_valid < ctx->base + B) ctx->res_sol_valid = ctx->base + B;
   }
   return HB_OK;
+}
+
+int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
+                              int32_t* mode_out, double* wbc_sol, double* torque, int32_t* wbc_status) {
+  return resident_wbc_impl(ctx, B, t_now, rbd, stance_mode, x_des, u_des, mode_out, wbc_sol, torque, wbc_status, false);
+}
+
+int hb_default_rollout_params(hb_rollout_params* p) {
+  if (!p) return HB_EINVAL;
+  memset(p, 0, sizeof(*p));
+  p->period = 0.002; p->mpc_every = 5; p->actuation_delay = 0.009;
+  hb_default_sim_params(&p->sim);
+  hb_default_pd_gains(&p->gains);
+  for (int j = 0; j < NJ; ++j) p->torque_limit[j] = HB_WBC_TORQUE_LIMITS[j % 5];
+  return HB_OK;
+}
+
+// hb_rollout_batch_dev's scratch: one allocation at max_batch, carved into 256-byte aligned slices
+static int rollout_reserve(hb_ctx* ctx) {
+  if (ctx->ro_mem) return HB_OK;
+  const size_t Bc = ctx->cfg.max_batch;
+  size_t total = 0;
+  auto slice = [&](size_t per) { const size_t o = total; total += (per * Bc + 255) & ~(size_t)255; return o; };
+  const size_t o_cmd = slice(sizeof(hb_rollout_command)), o_in = slice(sizeof(hb_plan_input)), o_refs = slice(sizeof(hb_reference));
+  const size_t o_info = slice(sizeof(hb_solve_info)), o_pstat = slice(sizeof(int32_t)), o_t0 = slice(sizeof(double)), o_x0 = slice(sizeof(double) * NX);
+  const size_t o_feet = slice(sizeof(double) * 12), o_sol = slice(sizeof(double) * NWBC), o_jcmd = slice(sizeof(double) * NJ * 5);
+  const size_t o_jtau = slice(sizeof(double) * NJ), o_tau = slice(sizeof(double) * NJ), o_held = slice(sizeof(double) * 32), o_tnow = slice(sizeof(double));
+  if (cudaMalloc(&ctx->ro_mem, total) != cudaSuccess) { cudaGetLastError(); ctx->ro_mem = nullptr; return HB_ENOMEM; }
+  char* b = static_cast<char*>(ctx->ro_mem);
+  ctx->ro_cmd = reinterpret_cast<hb_rollout_command*>(b + o_cmd); ctx->ro_in = reinterpret_cast<hb_plan_input*>(b + o_in);
+  ctx->ro_refs = reinterpret_cast<hb_reference*>(b + o_refs); ctx->ro_info = reinterpret_cast<hb_solve_info*>(b + o_info);
+  ctx->ro_pstat = reinterpret_cast<int32_t*>(b + o_pstat);
+  double** dp[] = {&ctx->ro_t0, &ctx->ro_x0, &ctx->ro_feet, &ctx->ro_sol, &ctx->ro_jcmd, &ctx->ro_jtau, &ctx->ro_tau, &ctx->ro_held, &ctx->ro_tnow};
+  const size_t offs[] = {o_t0, o_x0, o_feet, o_sol, o_jcmd, o_jtau, o_tau, o_held, o_tnow};
+  for (int k = 0; k < 9; ++k) *dp[k] = reinterpret_cast<double*>(b + offs[k]);
+  return HB_OK;
+}
+
+int hb_rollout_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb_rollout_params* p, const hb_rollout_command* cmd, double* rbd,
+                         hb_actuation_state* act, uint8_t* estop, hb_rollout_stats* stats, double* log) {
+  if (!ctx || B < 0 || n_ticks < 0 || tick0 < 0 || !p || !cmd || !rbd || !act || !estop || !stats) return HB_EINVAL;
+  if (p->mpc_every < 1 || !(p->period > 0.0) || p->log_every < 0 || !(p->actuation_delay >= 0.0) || !(p->sim.dt > 0.0) || p->sim.substeps < 1 ||
+      p->sim.substeps > 1000 || tick0 + n_ticks > INT32_MAX)
+    return HB_EINVAL;
+  if (B == 0) return HB_OK;
+  if (B > ctx->cfg.max_batch) return HB_ECAP;
+  for (int i = 0; i < B; ++i) {
+    const hb_rollout_command& c = cmd[i];
+    if (c.gait < 0 || c.gait > 3 || c.n_cmd < 1 || c.n_cmd > HB_ROLLOUT_MAX_CMDS || !(c.gait_start == c.gait_start)) return HB_EINVAL;
+    for (int k = 0; k < c.n_cmd; ++k) if (!(c.cmd_time[k] == c.cmd_time[k]) || (k > 0 && c.cmd_time[k] < c.cmd_time[k - 1])) return HB_EINVAL;
+  }
+  const bool cold = tick0 == 0;
+  if (!cold && ctx->res_valid < B) return HB_EINVAL;       // no resident solution to continue from
+  if (n_ticks == 0) return HB_OK;
+  if (set_device(ctx)) return HB_ECUDA;
+  int rc = rollout_reserve(ctx);
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(ctx->ro_cmd, cmd, sizeof(hb_rollout_command) * B, cudaMemcpyHostToDevice, ctx->stream));
+  const double horizon = (ctx->cfg.event_nodes && ctx->cfg.time_horizon > 0.0) ? ctx->cfg.time_horizon : ctx->cfg.horizon_N * ctx->cfg.dt;
+  const int n_log = (log && p->log_every > 0) ? (n_ticks + p->log_every - 1) / p->log_every : 0;
+  const unsigned grid = (B + 63) / 64;
+  for (int k = 0; k < n_ticks && !rc; ++k) {
+    const int64_t a = tick0 + k;
+    const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
+    const bool mpc = a % p->mpc_every == 0, first_cold = cold && k == 0;
+    double* log_row = (n_log && k % p->log_every == 0) ? log + (size_t)(k / p->log_every) * 32 : nullptr;
+    rc = launch(ctx, K_UNPROFILED, rollout_tick_begin_kernel, grid, 64, 0, B, (int)a, t, p->min_base_height, rbd, ctx->ro_held, stats, ctx->ro_tnow,
+                log_row, (size_t)n_log * 32);
+    if (!rc && mpc) {
+      if (first_cold) CK(cudaMemsetAsync(ctx->res_stance, 0, sizeof(double) * B * 12, ctx->stream));   // latestStanceposition_ starts at zero
+      rc = launch(ctx, K_UNPROFILED, rollout_plan_inputs_kernel, grid, 64, 0, B, t, horizon, ctx->ro_cmd, rbd, ctx->ro_in);
+      if (!rc) rc = launch(ctx, K_UNPROFILED, plan_prepare_kernel, grid, 64, 0, B, ctx->ro_in, ctx->ro_t0, ctx->ro_x0, ctx->ro_feet);
+      if (!rc) rc = hb_plan_references_batch_dev(ctx, B, ctx->ro_in, ctx->ro_feet, ctx->res_stance, ctx->ro_refs, ctx->ro_pstat);
+      if (!rc) rc = resident_cycle_impl(ctx, B, first_cold, 0.0, ctx->ro_t0, ctx->ro_x0, ctx->ro_refs, rbd, ctx->ro_info, nullptr, nullptr, nullptr, false);
+    }
+    // the cycle ran no WBC, so after a cold start the first tick's fallback has no previous solution, as the cycle's own would not have
+    if (!rc) rc = resident_wbc_impl(ctx, B, ctx->ro_tnow, rbd, nullptr, ctx->xdes, ctx->udes, ctx->wmode, ctx->ro_sol, nullptr, ctx->wstatus, first_cold);
+    if (!rc) rc = hb_joint_command_batch_dev(ctx, B, &p->gains, p->period, ctx->xdes, ctx->udes, ctx->ro_sol, ctx->wmode, rbd, nullptr, estop, ctx->ro_jcmd,
+                                             ctx->ro_jtau);
+    if (!rc) rc = hb_actuation_batch_dev(ctx, B, p->actuation_delay, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau);
+    if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, ctx->ro_tau);
+    if (!rc) rc = hb_sim_step_batch_dev(ctx, B, &p->sim, rbd, ctx->ro_tau, nullptr, nullptr);
+    if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_tick_end_kernel, grid, 64, 0, B, (int)a, mpc ? 1 : 0, ctx->ro_info, ctx->ro_pstat, ctx->wstatus, estop, ctx->ro_tau, ctx->ro_held, rbd, stats);
+  }
+  return rc;
 }
 
 int hb_observer_reset(int B, hb_observer_state* state) {

@@ -335,6 +335,21 @@ __device__ void kin_pass(const T* q, const T* v, KinOut<T>& o) {
                 [&](int k, T& s, T& c) { sincos_t(q[3 + k], s, c); }, sink);
 }
 
+// computeCentroidalStateFromRbdModel (LeggedController.cpp:336): rbd [zyx, p, q_j, omega_world, v, qd_j] -> x [h_lin/m, h_ang/m, p, zyx, q_j]
+__device__ __forceinline__ void rbd_to_centroidal(const double* r, double* x) {
+  double q[NQ], v[NQ];
+  for (int i = 0; i < 3; ++i) { q[i] = r[3 + i]; q[3 + i] = r[i]; v[i] = r[NQ + 3 + i]; }
+  for (int j = 0; j < NJ; ++j) { q[6 + j] = r[6 + j]; v[6 + j] = r[NQ + 6 + j]; }
+  double sz, cz, sy, cy;
+  sincos(q[3], &sz, &cz); sincos(q[4], &sy, &cy);
+  const double dxr = (cz * r[NQ] + sz * r[NQ + 1]) / cy;
+  v[5] = dxr; v[4] = -sz * r[NQ] + cz * r[NQ + 1]; v[3] = r[NQ + 2] + sy * dxr;
+  KinOut<double> o;
+  kin_pass<double>(q, v, o);
+  for (int i = 0; i < 6; ++i) x[i] = o.h[i] / c_model.total_mass;
+  for (int i = 0; i < NQ; ++i) x[6 + i] = q[i];
+}
+
 // Recursive Newton-Euler in the coordinates above: tau = M(q) a + C(q,v) v + g(q)   (float64, per lane).
 // Also returns the classical acceleration of the four contact points (= J_c a + dJ_c/dt v).
 __device__ void rnea_pass(const double* q, const double* v, const double* a, bool gravity, double* tau, double* cacc) {

@@ -200,6 +200,38 @@ typedef struct {
 int hb_default_sim_params(hb_sim_params* p);
 int hb_actuation_reset(int B, hb_actuation_state* state);   /* host only */
 
+/* ---- closed-loop episodes (hb_rollout_batch_dev): planner + MPC cycle at mpc_every ticks, 500 Hz WBC tick, joint command law, actuation
+ * delay, saturation and plant, for a batch of robots in one call ---- */
+#define HB_ROLLOUT_MAX_CMDS 8
+typedef struct {                 /* the command of one instance: gait and a piecewise-constant cmd_vel                            */
+  int32_t gait;                  /* 0..3 as hb_plan_input.gait                                                                    */
+  double gait_start;             /* as hb_plan_input.gait_start                                                                   */
+  int32_t n_cmd;                 /* 1..HB_ROLLOUT_MAX_CMDS                                                                        */
+  double cmd_time[HB_ROLLOUT_MAX_CMDS];      /* ascending; cmd_vel[j] holds from cmd_time[j] on (cmd_vel[0] also before cmd_time[0]) */
+  double cmd_vel[HB_ROLLOUT_MAX_CMDS][4];
+} hb_rollout_command;
+typedef struct {
+  double period;                 /* one WBC tick [s] (0.002); tick k of a call runs at t = (tick0 + k) * period                   */
+  int32_t mpc_every;             /* an MPC cycle on every tick with (tick0 + k) % mpc_every == 0 (5: 100 Hz, task.info mpcDesiredFrequency) */
+  double actuation_delay;        /* command delay of the actuation model [s] (legged_gazebo/config/default.yaml:2, 0.009)         */
+  hb_sim_params sim;             /* the plant; sim.dt is the time it advances per tick                                            */
+  hb_pd_gains gains;             /* joint command law                                                                             */
+  double torque_limit[10];       /* actuator saturation of the applied torques (default: HB_WBC_TORQUE_LIMITS per leg)             */
+  double min_base_height;        /* failure when the base z falls below it; 0 disables the check                                  */
+  int32_t log_every;             /* 0: no log                                                                                     */
+} hb_rollout_params;
+#define HB_ROLLOUT_FAIL_ESTOP 1        /* the joint command law raised the emergency stop                                       */
+#define HB_ROLLOUT_FAIL_ORIENTATION 2  /* |roll| > pi/2 (SafetyChecker::checkOrientation, SafetyChecker.h:34-43)                 */
+#define HB_ROLLOUT_FAIL_HEIGHT 4       /* base z < min_base_height                                                             */
+#define HB_ROLLOUT_FAIL_NONFINITE 8    /* an rbd entry is not finite                                                           */
+typedef struct {                 /* per-instance outcome, in/out: start an episode with zeros and fail_tick = -1                  */
+  int32_t fail_tick;             /* absolute tick of the first failure, -1: never failed                                          */
+  int32_t fail_reason;           /* HB_ROLLOUT_FAIL_* bits of that tick                                                           */
+  int32_t mpc_bad, wbc_fallbacks, plan_rejects;   /* counts of info.status != 0, wbc_status != 0, plan_status != 0                */
+  double max_abs_torque;         /* over the applied (saturated) torques                                                          */
+} hb_rollout_stats;
+int hb_default_rollout_params(hb_rollout_params* p);       /* host only */
+
 int hb_default_kf_params(hb_kf_params* p);
 /* x_hat = 0, P = 100 I, heights = 0 (KalmanFilterEstimate constructor, LinearKalmanFilter.cpp:24-63); host only */
 int hb_kf_reset(int B, hb_kf_state* state);
@@ -313,6 +345,20 @@ int hb_sim_step_batch_dev(hb_ctx* ctx, int B, const hb_sim_params* params, doubl
  * (inputs of hb_joint_command_batch). */
 int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode /*nullable*/, double* x_des,
                               double* u_des, int32_t* mode_out, double* wbc_sol, double* torque /*nullable*/, int32_t* wbc_status /*nullable*/);
+/* n_ticks ticks of B closed-loop episodes (LeggedController::update on the batched plant). On a tick with (tick0 + k) % mpc_every == 0 an MPC
+ * cycle runs first: plan inputs built on the device from rbd (x0 = hb_rbd_to_centroidal, t0 = t, cmd_vel of the command segment in force,
+ * horizon = time_to_target = horizon_N * dt or, for event_nodes contexts, the time horizon, prev_event = min(t, gait_start) - 0.5, IK
+ * joint references), device planner, resident cycle without its WBC (cold start iff tick0 == 0). Every tick then runs
+ * hb_resident_wbc_batch's policy + WeightedWbc at t, the joint command law (loaded, walking branch), the actuation model, saturation to
+ * +-torque_limit and one plant step. Failure checks run on the state entering each tick (finite, |roll| <= pi/2, base height) and on the
+ * emergency stop the joint command raises; from its first failure on an instance is held (rbd put back to its last finite state after
+ * every plant step; a non-finite state entering the first tick of a call is replaced by the nominal standing pose) and its outputs no
+ * longer count in stats. rbd (B x 32), act, estop (B) and stats are device memory, in/out. cmd (B) is a host array, validated and copied
+ * to the context once per call; p is read on the host. log (device, nullable): rbd at the start of every log_every-th tick of the call,
+ * B x ceil(n_ticks / log_every) x 32. Asynchronous: launches only, on the context's stream; per-call scratch is allocated at max_batch by
+ * the first call and freed by hb_destroy. */
+int hb_rollout_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb_rollout_params* p, const hb_rollout_command* cmd, double* rbd,
+                         hb_actuation_state* act, uint8_t* estop, hb_rollout_stats* stats, double* log /*nullable*/);
 int hb_rbd_to_centroidal_batch_dev(hb_ctx* ctx, int B, const double* rbd, double* x);
 int hb_reference_expand_batch_dev(hb_ctx* ctx, int B, const double* t0, const hb_reference* refs, double* x_ref, double* swing_ref,
                                   int32_t* mode);
