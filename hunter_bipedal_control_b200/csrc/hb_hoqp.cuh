@@ -171,3 +171,71 @@ __device__ inline int hoqp_solve_warp(const hb_hoqp_problem& pb, HoqpShared& sh,
 }
 
 }  // namespace hb
+
+namespace {  // the kernels: internal linkage, the library exports only the hb_* entry points
+using namespace hb;
+__global__ void __launch_bounds__(32) hoqp_kernel(int B, const hb_hoqp_problem* problems, double* scratch, int max_iter, double* x, double* slack, int32_t* status) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int inst = blockIdx.x;
+  if (inst >= B) return;
+  HoqpShared& sh = *reinterpret_cast<HoqpShared*>(smem_raw);
+  QpWorkspace w;
+  qp_carve(reinterpret_cast<double*>(smem_raw + sizeof(HoqpShared)), HQ_NQ, w, 1, HQ_ROWS);
+  const int st = hoqp_solve_warp(problems[inst], sh, w, scratch + (size_t)inst * HQ_SCRATCH, max_iter, x + (size_t)inst * HQ_N, slack ? slack + (size_t)inst * HQ_STK : nullptr);
+  if (status && threadIdx.x == 0) status[inst] = st;
+}
+
+// The three tasks of HierarchicalWbc::update from the WBC terms of one instance (decision vector [qdd(16), F(12), tau(10)]):
+//   task0 = formulateFloatingBaseEomTask + formulateTorqueLimitsTask + formulateFrictionConeTask + formulateNoContactMotionTask
+//   task1 = formulateBaseAccelTask          task2 = formulateContactForceTask * 0.1 + formulateSwingLegTask * 1     (WbcBase.cpp:138-338)
+__global__ void __launch_bounds__(32) hwbc_tasks_kernel(int B, hb_wbc_settings ws, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
+                                                        hb_hoqp_problem* problems) {
+  __shared__ WbcShared sh;
+  const int inst = blockIdx.x, lane = threadIdx.x;
+  if (inst >= B) return;
+  const int md_ = mode[inst];
+  int nw = 0;
+  wbc_assemble_warp(x_des + (size_t)inst * NX, u_des + (size_t)inst * NU, rbd + (size_t)inst * 32, md_, false, ws, sh, nullptr, nullptr, nullptr, nullptr, nullptr, &nw);
+  hb_hoqp_problem& pb = problems[inst];
+  bool fl[4]; int nc = 0;
+  for (int c = 0; c < 4; ++c) { fl[c] = contact_flag(md_, c); nc += fl[c]; }
+  const int nsw = 4 - nc;
+  const int ma0 = 16 + 3 * nsw + 3 * nc, md0 = 20 + 5 * nc, ma1 = 6, ma2 = 12 + 3 * nsw;
+  if (lane == 0) { pb.n = NWBC; pb.levels = 3; pb.ma[0] = ma0; pb.md[0] = md0; pb.ma[1] = ma1; pb.md[1] = 0; pb.ma[2] = ma2; pb.md[2] = 0; }
+  for (int idx = lane; idx < HB_HOQP_MAX_EQ * NWBC; idx += 32) { (&pb.a[0][0][0])[idx] = 0.0; (&pb.a[1][0][0])[idx] = 0.0; (&pb.a[2][0][0])[idx] = 0.0; }
+  for (int idx = lane; idx < HB_HOQP_MAX_IN * NWBC; idx += 32) (&pb.d[0][0][0])[idx] = 0.0;
+  __syncwarp();
+  // task0 equalities: EoM rows [M | -J' | -S'] x = -nle
+  for (int idx = lane; idx < 16 * NWBC; idx += 32) {
+    const int i = idx / NWBC, j = idx - i * NWBC;
+    double a;
+    if (j < NQ) a = sh.M[i * 16 + j];
+    else if (j < NQ + 12) a = -sh.J[(j - NQ) * 16 + i];
+    else a = (i >= 6 && j - NQ - 12 == i - 6) ? -1.0 : 0.0;
+    pb.a[0][i][j] = a;
+  }
+  if (lane < 16) pb.b[0][lane] = -sh.nle[lane];
+  if (lane == 0) {
+    int r = 16;
+    for (int c = 0; c < 4; ++c) if (!fl[c]) for (int a = 0; a < 3; ++a) { pb.a[0][r][NQ + 3 * c + a] = 1.0; pb.b[0][r] = 0.0; ++r; }      // zero swing force
+    for (int c = 0; c < 4; ++c) if (fl[c]) for (int a = 0; a < 3; ++a) {                                                                  // no contact motion
+      for (int j = 0; j < NQ; ++j) pb.a[0][r][j] = sh.J[(3 * c + a) * 16 + j];
+      pb.b[0][r] = -sh.dJv[3 * c + a]; ++r;
+    }
+    // task0 inequalities: torque limits, friction pyramid
+    int q = 0;
+    for (int sgn = 0; sgn < 2; ++sgn) for (int j = 0; j < NJ; ++j) { pb.d[0][q][NQ + 12 + j] = sgn == 0 ? 1.0 : -1.0; pb.f[0][q] = ws.torque_limits[j % 5]; ++q; }
+    const double mu = ws.friction_coefficient;
+    const double pyr[5][3] = {{0, 0, -1}, {1, 0, -mu}, {-1, 0, -mu}, {0, 1, -mu}, {0, -1, -mu}};
+    for (int c = 0; c < 4; ++c) if (fl[c]) for (int k = 0; k < 5; ++k) { for (int a = 0; a < 3; ++a) pb.d[0][q][NQ + 3 * c + a] = pyr[k][a]; pb.f[0][q] = 0.0; ++q; }
+    // task2 first part: 0.1 * (F = F_des)
+    for (int j = 0; j < 12; ++j) { pb.a[2][j][NQ + j] = 0.1; pb.b[2][j] = 0.1 * u_des[(size_t)inst * NU + j]; }
+  }
+  // task1: base acceleration rows (the weighted formulation's base rows with the weight divided out); task2 second part: swing rows
+  const int nswr = 3 * nsw;
+  for (int idx = lane; idx < 6 * NQ; idx += 32) { const int i = idx / NQ, j = idx - i * NQ; pb.a[1][i][j] = sh.Aw[(nswr + i) * 16 + j] / ws.weight_base_accel; }
+  if (lane < 6) pb.b[1][lane] = sh.bw[nswr + lane] / ws.weight_base_accel;
+  for (int idx = lane; idx < nswr * NQ; idx += 32) { const int i = idx / NQ, j = idx - i * NQ; pb.a[2][12 + i][j] = sh.Aw[i * 16 + j] / ws.weight_swing_leg; }
+  if (lane < nswr) pb.b[2][12 + lane] = sh.bw[lane] / ws.weight_swing_leg;
+}
+}  // namespace

@@ -242,3 +242,34 @@ __device__ inline void node_values_lane(const double* x, const double* u, const 
 
 
 }  // namespace hb
+
+namespace {  // the kernels: internal linkage, the library exports only the hb_* entry points
+using namespace hb;
+// input cost R = blkdiag(R_f, J0' R_v J0) with J0 the contact Jacobian at initialState (LeggedInterface.cpp:263-288)
+__global__ void init_input_cost_kernel(double* Rout) {
+  __shared__ double J0[12 * 16];
+  const int lane = threadIdx.x;
+  if (lane < 16) {
+    double q[NQ], e[NQ];
+    const double q0[NQ] = {HB_INITIAL_STATE[6], HB_INITIAL_STATE[7], HB_INITIAL_STATE[8], HB_INITIAL_STATE[9], HB_INITIAL_STATE[10], HB_INITIAL_STATE[11],
+                           HB_INITIAL_STATE[12], HB_INITIAL_STATE[13], HB_INITIAL_STATE[14], HB_INITIAL_STATE[15], HB_INITIAL_STATE[16], HB_INITIAL_STATE[17],
+                           HB_INITIAL_STATE[18], HB_INITIAL_STATE[19], HB_INITIAL_STATE[20], HB_INITIAL_STATE[21]};
+    for (int i = 0; i < NQ; ++i) { q[i] = q0[i]; e[i] = (i == lane) ? 1.0 : 0.0; }
+    KinOut<double> o;
+    kin_pass<double>(q, e, o);
+    for (int r = 0; r < 12; ++r) J0[r * 16 + lane] = o.cvel[r];
+  }
+  __syncthreads();
+  const double rts[24] = {HB_R_TASKSPACE_DIAG[0], HB_R_TASKSPACE_DIAG[1], HB_R_TASKSPACE_DIAG[2], HB_R_TASKSPACE_DIAG[3], HB_R_TASKSPACE_DIAG[4], HB_R_TASKSPACE_DIAG[5],
+                          HB_R_TASKSPACE_DIAG[6], HB_R_TASKSPACE_DIAG[7], HB_R_TASKSPACE_DIAG[8], HB_R_TASKSPACE_DIAG[9], HB_R_TASKSPACE_DIAG[10], HB_R_TASKSPACE_DIAG[11],
+                          HB_R_TASKSPACE_DIAG[12], HB_R_TASKSPACE_DIAG[13], HB_R_TASKSPACE_DIAG[14], HB_R_TASKSPACE_DIAG[15], HB_R_TASKSPACE_DIAG[16], HB_R_TASKSPACE_DIAG[17],
+                          HB_R_TASKSPACE_DIAG[18], HB_R_TASKSPACE_DIAG[19], HB_R_TASKSPACE_DIAG[20], HB_R_TASKSPACE_DIAG[21], HB_R_TASKSPACE_DIAG[22], HB_R_TASKSPACE_DIAG[23]};
+  for (int idx = lane; idx < NU * NU; idx += 32) {
+    const int i = idx / NU, j = idx - i * NU;
+    double v = 0.0;
+    if (i < 12 && i == j) v = rts[i];
+    if (i >= 12 && j >= 12) for (int r = 0; r < 12; ++r) v += J0[r * 16 + 6 + i - 12] * rts[12 + r] * J0[r * 16 + 6 + j - 12];
+    Rout[idx] = v;
+  }
+}
+}  // namespace

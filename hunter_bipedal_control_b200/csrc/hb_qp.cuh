@@ -543,3 +543,22 @@ __device__ inline QpResult qp_solve_warp(int n, int m, const double* __restrict_
 }
 
 }  // namespace hb
+
+namespace {  // the kernels: internal linkage, the library exports only the hb_* entry points
+using namespace hb;
+__global__ void qp_batch_kernel(int B, int n, int m, const double* H, const double* g, const double* A, const double* lbA, const double* ubA,
+                                size_t strideH, size_t strideA, size_t strideB, const int32_t* m_per, double rho, int max_iter, double* x,
+                                int32_t* status, int32_t* iters) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
+  const int inst = blockIdx.x * wpb + warp;
+  if (inst >= B) return;
+  double* base = reinterpret_cast<double*>(smem_raw) + (size_t)warp * qp_workspace_doubles(n);
+  QpWorkspace w;
+  qp_carve(base, n, w);
+  const int mi = m_per ? m_per[inst] : m;
+  QpResult r = qp_solve_warp(n, mi, H + inst * strideH, g + (size_t)inst * n, A + inst * strideA, lbA + inst * strideB, ubA + inst * strideB,
+                             rho, max_iter, x + (size_t)inst * n, w);
+  if (lane_id() == 0) { if (status) status[inst] = r.status; if (iters) iters[inst] = r.iters; }
+}
+}  // namespace

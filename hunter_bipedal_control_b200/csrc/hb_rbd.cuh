@@ -446,3 +446,24 @@ __device__ __forceinline__ void solve6_cmm(const double* A, const double* r, dou
 }
 
 }  // namespace hb
+
+namespace {  // the kernels: internal linkage, the library exports only the hb_* entry points
+using namespace hb;
+// computeCentroidalStateFromRbdModel (LeggedController.cpp:336)
+__global__ void rbd_to_centroidal_kernel(int B, const double* rbd, double* x) {
+  const int inst = blockIdx.x * blockDim.x + threadIdx.x;
+  if (inst >= B) return;
+  rbd_to_centroidal(rbd + (size_t)inst * 32, x + (size_t)inst * NX);
+}
+
+// InverseKinematics::computeFootPos: contact frame positions at the configuration of x (one thread per instance)
+__global__ void contact_positions_kernel(int B, const double* x, double* pos) {
+  const int inst = blockIdx.x * blockDim.x + threadIdx.x;
+  if (inst >= B) return;
+  double q[NQ], v[NQ];
+  for (int i = 0; i < NQ; ++i) { q[i] = x[(size_t)inst * NX + 6 + i]; v[i] = 0.0; }
+  KinOut<double> o;
+  kin_pass<double>(q, v, o);
+  for (int i = 0; i < 12; ++i) pos[(size_t)inst * 12 + i] = o.cpos[i];
+}
+}  // namespace

@@ -1,8 +1,10 @@
-// Closed-loop episodes (hb_rollout_batch_dev, SURVEY 8f row N2): the per-instance kernels the episode loop adds around the device planner,
-// the resident cycle, the 500 Hz WBC tick, the joint command law, the actuation model and the plant. One thread per instance.
+// Closed-loop episodes (hb_rollout_batch_dev, SURVEY 8f row N2): the joint command law, the actuation model and the plant, and the
+// per-instance kernels the episode loop adds around them, the device planner, the resident cycle and the 500 Hz WBC tick.
 #pragma once
 #include "hb_common.cuh"
+#include "hb_qp.cuh"
 #include "hb_rbd.cuh"
+#include "../../include/hunter_b200.h"
 
 namespace hb {
 
@@ -91,3 +93,142 @@ __global__ void rollout_tick_end_kernel(int B, int tick, int mpc_tick, const hb_
 }
 
 }  // namespace hb
+
+namespace {  // the kernels: internal linkage, the library exports only the hb_* entry points
+using namespace hb;
+// joint command law (LeggedController.cpp:186-257), one thread per instance; joints are visited in order because the limit
+// protection of joint j only affects the commands of joints >= j within the same cycle
+__global__ void joint_command_kernel(int B, hb_pd_gains g, double dt, const double* x_des, const double* u_des, const double* sol,
+                                     const int32_t* mode_cmd, const double* rbd, const uint8_t* loaded, uint8_t* estop, double* command,
+                                     double* out_tau) {
+  const int inst = blockIdx.x * blockDim.x + threadIdx.x;
+  if (inst >= B) return;
+  const double* xd = x_des + (size_t)inst * NX; const double* ud = u_des + (size_t)inst * NU;
+  const double* ws = sol + (size_t)inst * NWBC; const double* r = rbd + (size_t)inst * 32;
+  const bool is_loaded = loaded ? loaded[inst] != 0 : true;
+  bool stop = estop ? estop[inst] != 0 : false;
+  const int mode = mode_cmd[inst];
+  for (int j = 0; j < NJ; ++j) {
+    const double q = r[6 + j], qd = r[NQ + 6 + j];
+    if (!stop && is_loaded && (q > c_model.joint_upper[j] + 0.02 || q < c_model.joint_lower[j] - 0.02)) stop = true;
+    double pd, vd, kp, kd, ff;
+    if (!is_loaded) {
+      pd = xd[12 + j]; vd = ud[12 + j]; kp = g.kp_position; kd = (j == 4 || j == 9) ? g.kd_feet : g.kd_position; ff = 0.0;
+    } else {
+      const double qdd = ws[6 + j];
+      pd = xd[12 + j] + 0.5 * qdd * dt * dt; vd = ud[12 + j] + qdd * dt; ff = ws[28 + j];
+      const bool contact = contact_flag(mode, j / 5);
+      if (j == 0 || j == 1 || j == 5 || j == 6) { kp = contact ? g.kp_small_stance : g.kp_small_swing; kd = g.kd_small; }
+      else if (j == 4 || j == 9) { kp = contact ? g.kp_small_stance : g.kp_small_swing; kd = g.kd_feet; }
+      else { kp = contact ? g.kp_big_stance : g.kp_big_swing; kd = g.kd_big; }
+    }
+    if (stop) { pd = 0.0; vd = 0.0; kp = 0.0; kd = 1.0; ff = 0.0; }
+    double* c = command + ((size_t)inst * NJ + j) * 5;
+    c[0] = pd; c[1] = vd; c[2] = kp; c[3] = kd; c[4] = ff;
+    out_tau[(size_t)inst * NJ + j] = ff + kp * (pd - q) + kd * (vd - qd);
+  }
+  if (estop) estop[inst] = stop ? 1 : 0;
+}
+
+// Actuation model of the simulated hardware (legged_gazebo/src/LeggedHWSim.cpp:166-192): every write pushes the hybrid joint command
+// (posDes, velDes, kp, kd, ff) with its time stamp on a buffer, drops the entries older than `delay` from the far end, and applies the
+// OLDEST remaining one: tau = kp (posDes - q) + kd (velDes - qd) + ff with the CURRENT joint state. One thread per instance; the deque is a
+// ring of HB_ACT_CAPACITY entries (a full ring drops its oldest entry first).
+__global__ void actuation_kernel(int B, double delay, const double* time, hb_actuation_state* state, const double* command, const double* rbd, double* tau) {
+  const int inst = blockIdx.x * blockDim.x + threadIdx.x;
+  if (inst >= B) return;
+  hb_actuation_state& st = state[inst];
+  const double t = time[inst];
+  int cnt = st.count, head = st.head;             // head = newest entry; entries head, head+1, ... (mod capacity) are older and older
+  while (cnt > 0 && st.stamp[(head + cnt - 1) % HB_ACT_CAPACITY] + delay < t) --cnt;
+  if (cnt == HB_ACT_CAPACITY) --cnt;
+  head = (head + HB_ACT_CAPACITY - 1) % HB_ACT_CAPACITY;
+  st.stamp[head] = t;
+  for (int k = 0; k < NJ * 5; ++k) st.cmd[head][k] = command[(size_t)inst * NJ * 5 + k];
+  ++cnt;
+  st.count = cnt; st.head = head;
+  const double* c = st.cmd[(head + cnt - 1) % HB_ACT_CAPACITY];
+  const double* r = rbd + (size_t)inst * 32;
+  for (int j = 0; j < NJ; ++j) tau[(size_t)inst * NJ + j] = c[5 * j + 2] * (c[5 * j] - r[6 + j]) + c[5 * j + 3] * (c[5 * j + 1] - r[NQ + 6 + j]) + c[5 * j + 4];
+}
+
+// One step of a batched rigid-body simulation of the robot on flat ground (stands in for the Gazebo / MuJoCo plant of the reference's
+// closed loop, legged_gazebo / legged_mujoco): forward dynamics M(q) qdd = S' tau + J_c' F_c - nle with compliant point contacts at the four
+// contact frames (normal spring-damper, viscous tangential friction clipped to the cone), semi-implicit Euler over `substeps` substeps.
+// Same rigid-body passes as the WBC assembly: lanes 0-15 unit-velocity sweeps -> J_c columns, lanes 0-15 RNEA with unit accelerations ->
+// M columns, lane 16 -> nle; 16 x 16 Cholesky in shared memory. One warp per instance.
+struct SimShared { double q[NQ], v[NQ], J[12 * NQ], M[NQ * 17], nle[NQ], rhs[NQ], t1[NQ], t2[NQ], kdi[NQ], F[12], cpos[12], cvel[12]; };
+__global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, double* rbd_io, const double* tau, double* contact_force, uint8_t* contact_flag) {
+  __shared__ SimShared sh;
+  const int inst = blockIdx.x, lane = threadIdx.x;
+  double* r = rbd_io + (size_t)inst * 32;
+  if (lane == 0) {
+    for (int i = 0; i < 3; ++i) { sh.q[i] = r[3 + i]; sh.q[3 + i] = r[i]; sh.v[i] = r[NQ + 3 + i]; }
+    for (int j = 0; j < NJ; ++j) { sh.q[6 + j] = r[6 + j]; sh.v[6 + j] = r[NQ + 6 + j]; }
+    double sz, cz, sy, cy;
+    sincos(sh.q[3], &sz, &cz); sincos(sh.q[4], &sy, &cy);
+    const double dxr = (cz * r[NQ] + sz * r[NQ + 1]) / cy;
+    sh.v[5] = dxr; sh.v[4] = -sz * r[NQ] + cz * r[NQ + 1]; sh.v[3] = r[NQ + 2] + sy * dxr;
+  }
+  __syncwarp();
+  const double h = prm.dt / (prm.substeps > 0 ? prm.substeps : 1);
+  for (int sub = 0; sub < (prm.substeps > 0 ? prm.substeps : 1); ++sub) {
+    if (lane < NQ) {
+      double q[NQ], e[NQ];
+      for (int i = 0; i < NQ; ++i) { q[i] = sh.q[i]; e[i] = (i == lane) ? 1.0 : 0.0; }
+      KinOut<double> o;
+      kin_pass<double>(q, e, o);
+      for (int rr = 0; rr < 12; ++rr) sh.J[rr * NQ + lane] = o.cvel[rr];
+      if (lane == 0) for (int rr = 0; rr < 12; ++rr) sh.cpos[rr] = o.cpos[rr];
+    }
+    __syncwarp();
+    if (lane < 12) { double s = 0.0; for (int i = 0; i < NQ; ++i) s += sh.J[lane * NQ + i] * sh.v[i]; sh.cvel[lane] = s; }
+    __syncwarp();
+    if (lane < 4) {
+      const double depth = prm.ground_height - sh.cpos[3 * lane + 2];
+      double fz = 0.0, fx = 0.0, fy = 0.0;
+      if (depth > 0.0) {
+        fz = prm.ground_stiffness * depth - prm.ground_damping * sh.cvel[3 * lane + 2];
+        if (fz < 0.0) fz = 0.0;
+        fx = -prm.tangential_damping * sh.cvel[3 * lane]; fy = -prm.tangential_damping * sh.cvel[3 * lane + 1];
+        const double ft = sqrt(fx * fx + fy * fy), fmax_ = prm.friction_mu * fz;
+        if (ft > fmax_) { const double sc = ft > 0.0 ? fmax_ / ft : 0.0; fx *= sc; fy *= sc; }
+      }
+      sh.F[3 * lane] = fx; sh.F[3 * lane + 1] = fy; sh.F[3 * lane + 2] = fz;
+    }
+    if (lane < 17) {
+      double q[NQ], v[NQ], a[NQ], tq[NQ];
+      for (int i = 0; i < NQ; ++i) { q[i] = sh.q[i]; v[i] = lane == 16 ? sh.v[i] : 0.0; a[i] = (i == lane) ? 1.0 : 0.0; }
+      rnea_pass(q, v, a, lane == 16, tq, nullptr);
+      if (lane < 16) { for (int rr = 0; rr < NQ; ++rr) sh.M[rr * 17 + lane] = tq[rr]; }
+      else { for (int rr = 0; rr < NQ; ++rr) sh.nle[rr] = tq[rr]; }
+    }
+    __syncwarp();
+    if (lane < NQ) {
+      // joint side of the plant as in the reference's MuJoCo model (mujoco/model/hunter/hunter.xml:6): rotor armature on the diagonal of M,
+      // viscous joint damping
+      double s = -sh.nle[lane] + (lane >= 6 ? tau[(size_t)inst * NJ + lane - 6] - prm.joint_damping * sh.v[lane] : 0.0);
+      for (int rr = 0; rr < 12; ++rr) s += sh.J[rr * NQ + lane] * sh.F[rr];
+      sh.rhs[lane] = s;
+      if (lane >= 6) sh.M[lane * 17 + lane] += prm.joint_armature;
+      for (int j = lane + 1; j < NQ; ++j) { const double a = 0.5 * (sh.M[lane * 17 + j] + sh.M[j * 17 + lane]); sh.M[j * 17 + lane] = a; }   // lower triangle, symmetrised
+    }
+    __syncwarp();
+    warp_chol_inv(sh.M, NQ, 17, sh.kdi, lane);
+    warp_li_mv(sh.M, NQ, 17, sh.kdi, sh.rhs, sh.t1, lane);
+    warp_lit_mv(sh.M, NQ, 17, sh.kdi, sh.t1, sh.t2, lane);      // t2 = qdd
+    if (lane < NQ) { const double vn = sh.v[lane] + h * sh.t2[lane]; sh.v[lane] = vn; sh.q[lane] += h * vn; }
+    __syncwarp();
+  }
+  if (lane == 0) {
+    for (int i = 0; i < 3; ++i) { r[3 + i] = sh.q[i]; r[i] = sh.q[3 + i]; r[NQ + 3 + i] = sh.v[i]; }
+    for (int j = 0; j < NJ; ++j) { r[6 + j] = sh.q[6 + j]; r[NQ + 6 + j] = sh.v[6 + j]; }
+    double sz, cz, sy, cy;
+    sincos(sh.q[3], &sz, &cz); sincos(sh.q[4], &sy, &cy);
+    const double d0 = sh.v[3], d1 = sh.v[4], d2 = sh.v[5];      // yaw, pitch, roll rates -> world angular velocity
+    r[NQ] = -sz * d1 + cz * cy * d2; r[NQ + 1] = cz * d1 + sz * cy * d2; r[NQ + 2] = d0 - sy * d2;
+  }
+  if (lane < 12 && contact_force) contact_force[(size_t)inst * 12 + lane] = sh.F[lane];
+  if (lane < 4 && contact_flag) contact_flag[(size_t)inst * 4 + lane] = sh.F[3 * lane + 2] > 0.0 ? 1 : 0;
+}
+}  // namespace

@@ -329,6 +329,58 @@ __global__ void __launch_bounds__(64, HB_LIN_MINB) lin_kernel(SqpArgs a) {
   lin_half(sh, cm, sh.x2, hl, act, rec + LIN_F2, rec + LIN_A2, rec + LIN_BF2, rec + LIN_BV2, false, rec);
 }
 
+}  // namespace hb
+
+namespace {  // internal linkage: the library exports only the hb_* entry points
+using namespace hb;
+// parity probe of the SHIPPING linearisation (lin_half of K0): flow map value, the full Jacobian tiles rebuilt from the compact
+// record (rows 3..11 of df/dx, the force / joint-velocity blocks of df/du) and the contact kinematics with their Jacobians.
+struct ProbeShared { LinHalf h[2]; ChainModel cm; double rec[LIN_STRIDE]; double dummy[LIN_STRIDE]; };
+__global__ void __launch_bounds__(32) probe_flow_map_kernel(int B, const double* x, const double* u, double* f, double* A, double* Bm, double* ee) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  ProbeShared& ps = *reinterpret_cast<ProbeShared*>(smem_raw);
+  const int inst = blockIdx.x, lane = threadIdx.x, half = lane >> 4, hl = lane & 15;
+  chain_model_load(ps.cm, threadIdx.x, blockDim.x);
+  LinHalf& sh = ps.h[half];
+  for (int i = hl; i < NX; i += 16) { sh.x[i] = x[(size_t)inst * NX + i]; sh.u[i] = u[(size_t)inst * NU + i]; }
+  __syncwarp();
+  // both halves linearise the same node; only half 0 writes the record (half 1 runs with act = false into a dummy record)
+  double* rec = half == 0 ? ps.rec : ps.dummy;
+  lin_half(sh, ps.cm, sh.x, hl, half == 0, rec + LIN_F1, rec + LIN_A1, rec + LIN_BF1, rec + LIN_BV1, true, rec);
+  __syncwarp();
+  const double im = 1.0 / c_model.total_mass;
+  if (lane < NX) f[(size_t)inst * NX + lane] = ps.rec[LIN_F1 + lane];
+  for (int idx = lane; idx < TS; idx += 32) {
+    const int i = idx / NX, j = idx - i * NX;
+    double a = 0.0, b = 0.0;
+    if (i >= 3 && i < 12) a = ps.rec[LIN_A1 + (i - 3) * NX + j];
+    if (j < 12) {
+      if (i < 3) b = (j % 3 == i) ? im : 0.0;
+      else if (i < 6) b = ps.rec[LIN_BF1 + (i - 3) * 12 + j];
+    } else {
+      if (i >= 6 && i < 12) b = ps.rec[LIN_BV1 + (i - 6) * NJ + j - 12];
+      else if (i >= 12) b = (i == j) ? 1.0 : 0.0;
+    }
+    A[(size_t)inst * TS + idx] = a; Bm[(size_t)inst * TS + idx] = b;
+  }
+  if (ee) {
+    double* o = ee + (size_t)inst * (24 + 3 * 12 * NX);
+    if (lane < 12) { o[lane] = ps.rec[LIN_EPOS + lane]; o[12 + lane] = ps.rec[LIN_EVEL + lane]; }
+    for (int idx = lane; idx < 12 * NX; idx += 32) {
+      const int r = idx / NX, j = idx - r * NX;
+      double dp = 0.0;
+      if (j >= 6 && j < 9) dp = (j - 6 == r % 3) ? 1.0 : 0.0;
+      else if (j >= 9) dp = ps.rec[LIN_DPQ + r * NDIR + j - 9];
+      o[24 + idx] = dp;
+      o[24 + 12 * NX + idx] = ps.rec[LIN_DVX + idx];
+      o[24 + 24 * NX + idx] = (j >= 12) ? ps.rec[LIN_DVV + r * NJ + j - 12] : 0.0;
+    }
+  }
+}
+}  // namespace
+
+namespace hb {
+
 // ---------------------------------------------------------------- K1
 // TMA bulk copies (1-D, cp.async.bulk) completing on an mbarrier: one elected lane arms the barrier with the byte count and issues the
 // copies, every lane waits on the phase bit. Addresses and sizes must be multiples of 16 bytes (the node records are).

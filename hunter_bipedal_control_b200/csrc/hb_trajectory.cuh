@@ -1,0 +1,138 @@
+// The resident primal solution on the device: the initializer (cold start), the warm shift of the previous solution onto the next
+// solve's grid, and the policy evaluation between MPC solves.
+#pragma once
+#include "hb_common.cuh"
+
+namespace {  // the kernels: internal linkage, the library exports only the hb_* entry points
+using namespace hb;
+// Input j of the initializer at a node of mode md (LeggedRobotInitializer::compute, LeggedRobotInitializer.cpp:67-77): the stance feet
+// share the robot's weight in z, everything else is zero.
+__device__ __forceinline__ double initializer_input(int md, int j) {
+  int ns = 0;
+  for (int c = 0; c < 4; ++c) ns += contact_flag(md, c);
+  return (j < 12 && (j % 3) == 2 && contact_flag(md, j / 3)) ? c_model.total_mass * HB_GRAVITY / ns : 0.0;
+}
+
+// LeggedRobotInitializer::compute (initialization/LeggedRobotInitializer.cpp:67-77)
+__global__ void cold_start_kernel(int B, int N, const double* x0, const int32_t* mode, double* xt, double* ut) {
+  const int inst = blockIdx.x;
+  const double* x = x0 + (size_t)inst * NX;
+  for (int idx = threadIdx.x; idx < (N + 1) * NX; idx += blockDim.x) xt[(size_t)inst * (N + 1) * NX + idx] = x[idx % NX];
+  for (int idx = threadIdx.x; idx < N * NU; idx += blockDim.x) {
+    const int k = idx / NU, j = idx - k * NU;
+    ut[(size_t)inst * N * NU + idx] = initializer_input(mode[(size_t)inst * (N + 1) + k], j);
+  }
+}
+
+// index k of the interval [tk[k], tk[k+1]) of a grid with n intervals that holds t (clamped to 0 .. n-1), and the interpolation weight
+__device__ __forceinline__ int grid_interval(const double* tk, int n, double t, double& al) {
+  int lo = 0, hi = n;                     // invariant: tk[lo] <= t (or lo == 0), tk[hi] > t (or hi == n)
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (tk[mid] <= t) lo = mid; else hi = mid; }
+  const double d = tk[lo + 1] - tk[lo];
+  double a = d > 0.0 ? (t - tk[lo]) / d : 0.0;
+  al = a < 0.0 ? 0.0 : (a > 1.0 ? 1.0 : a);
+  return lo;
+}
+
+// The same on the uniform grid of n intervals, with s = (t - t_0) / dt the caller computes: s clamped to [0, n], k = floor(s) capped at
+// n - 1, weight s - k
+__device__ __forceinline__ int uniform_interval(double s, int n, double& al) {
+  if (s < 0.0) s = 0.0;
+  if (s > (double)n) s = (double)n;
+  int k = (int)floor(s);
+  if (k >= n) k = n - 1;
+  al = s - k;
+  return k;
+}
+
+// Warm start of the next solve from the resident primal solution (ocs2::SqpSolver::initializeStateInputTrajectories; mpc.coldStart
+// false, task.info:146): x[0] = measured state; interval i takes u[i] = previous input at t_i and x[i+1] = previous state at t_{i+1}
+// while t_{i+1} lies inside the previous horizon, otherwise the initializer (weight-compensating input, state kept,
+// LeggedRobotInitializer.cpp:67-77). One block per instance; the previous trajectories are staged in shared memory so that the
+// update can be done in place. With event-node grids (tk_new != null) both the previous and the new node times are arbitrary:
+// tk_res / nn_res hold the previous grid and are replaced by the new one at the end.
+__global__ void __launch_bounds__(128) warm_shift_kernel(int B, int N, double dt, const double* t0_new, double* t0_res, const double* x0,
+                                                          const int32_t* mode, double* xt, double* ut, const double* tk_new, const int32_t* nn_new,
+                                                          double* tk_res, int32_t* nn_res) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  double* px = reinterpret_cast<double*>(smem_raw);
+  double* pu = px + (size_t)(N + 1) * NX;
+  __shared__ double ptk[HB_MAX_HORIZON + 1];
+  const int inst = blockIdx.x;
+  const bool grid = tk_new != nullptr;
+  double* x = xt + (size_t)inst * (N + 1) * NX; double* u = ut + (size_t)inst * N * NU;
+  for (int i = threadIdx.x; i < (N + 1) * NX; i += blockDim.x) px[i] = x[i];
+  for (int i = threadIdx.x; i < N * NU; i += blockDim.x) pu[i] = u[i];
+  const int np = grid ? nn_res[inst] : N;                        // intervals of the previous grid
+  const int nw = grid ? nn_new[inst] : N;                        // intervals of the new grid
+  const double* tn_ = grid ? tk_new + (size_t)inst * (N + 1) : nullptr;
+  if (grid) for (int i = threadIdx.x; i <= N; i += blockDim.x) ptk[i] = tk_res[(size_t)inst * (N + 1) + i];
+  __syncthreads();
+  const double tp = grid ? ptk[0] : t0_res[inst], tn = t0_new[inst], t_end = grid ? ptk[np] : tp + N * dt;
+  auto new_time = [&](int k) { return grid ? tn_[k < nw ? k : nw] : tn + k * dt; };
+  auto locate = [&](double t, double& al) {
+    if (grid) return grid_interval(ptk, np, t, al);
+    return uniform_interval((t - tp) / dt, N, al);
+  };
+  auto prev_state = [&](double t, int j) { double al; const int k = locate(t, al); return (1.0 - al) * px[k * NX + j] + al * px[(k + 1) * NX + j]; };
+  auto prev_input = [&](double t, int j) {
+    double al; const int k = locate(t, al);
+    const int k1 = (k + 1 < np) ? k + 1 : np - 1;
+    return (1.0 - al) * pu[k * NU + j] + al * pu[k1 * NU + j];
+  };
+  // first interval that falls back to the initializer: smallest i with t_{i+1} > t_end (1e-9 guards the grid-aligned case)
+  int istar = nw;
+  for (int i = 0; i < nw; ++i) if (new_time(i + 1) > t_end + 1e-9) { istar = i; break; }
+  for (int idx = threadIdx.x; idx < (N + 1) * NX; idx += blockDim.x) {
+    const int k = idx / NX, j = idx - k * NX;
+    const int ks = k <= istar ? k : istar;                 // the initializer keeps the state of node istar
+    x[idx] = (ks == 0) ? x0[(size_t)inst * NX + j] : prev_state(new_time(ks), j);
+  }
+  for (int idx = threadIdx.x; idx < N * NU; idx += blockDim.x) {
+    const int k = idx / NU, j = idx - k * NU;
+    u[idx] = k < istar ? prev_input(new_time(k), j) : initializer_input(mode[(size_t)inst * (N + 1) + k], j);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) { t0_res[inst] = tn; if (grid) nn_res[inst] = nw; }
+  if (grid) for (int i = threadIdx.x; i <= N; i += blockDim.x) tk_res[(size_t)inst * (N + 1) + i] = tn_[i];
+}
+
+// MPC_MRT_Interface::evaluatePolicy with the feed-forward policy (LeggedController.cpp:154-156, task.info:93):
+// linear interpolation of the state / input trajectories at t0 + t_rel; mode = mode in force at that time.
+__global__ void policy_eval_kernel(int B, int N, double dt, double t_rel, const double* xt, const double* ut, const int32_t* mode, double* x_des,
+                                   double* u_des, int32_t* mode_out, const double* tk, const int32_t* nn, const double* t_abs, const double* t0res) {
+  const int inst = blockIdx.x * blockDim.x / 32 + (threadIdx.x >> 5);
+  if (inst >= B) return;
+  const int lane = threadIdx.x & 31;
+  if (t_abs) t_rel = t_abs[inst] - t0res[inst];        // evaluation at an absolute time per instance (500 Hz WBC ticks between MPC updates)
+  int k, na = N;
+  double al;
+  if (tk) {      // event-node grid: node times of this instance
+    const double* t = tk + (size_t)inst * (N + 1);
+    na = nn[inst];
+    k = grid_interval(t, na, t[0] + t_rel, al);
+  } else {
+    k = uniform_interval(t_rel / dt, N, al);
+  }
+  const double* x = xt + (size_t)inst * (N + 1) * NX;
+  const double* u = ut + (size_t)inst * N * NU;
+  if (lane < NX) {
+    x_des[(size_t)inst * NX + lane] = (1.0 - al) * x[k * NX + lane] + al * x[(k + 1) * NX + lane];
+    const int k1 = (k + 1 < na) ? k + 1 : na - 1;   // the input trajectory repeats its last sample at the final node
+    u_des[(size_t)inst * NU + lane] = (1.0 - al) * u[k * NU + lane] + al * u[k1 * NU + lane];
+  }
+  if (lane == 0 && mode_out) mode_out[inst] = mode[(size_t)inst * (N + 1) + k];
+}
+
+// store the solve time of a cold-started resident solution
+__global__ void set_times_kernel(int B, int N, const double* t0_new, double* t0_res, const double* tk_new, const int32_t* nn_new, double* tk_res,
+                                 int32_t* nn_res) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B) return;
+  t0_res[i] = t0_new[i];
+  if (tk_new) {
+    nn_res[i] = nn_new[i];
+    for (int k = 0; k <= N; ++k) tk_res[(size_t)i * (N + 1) + k] = tk_new[(size_t)i * (N + 1) + k];
+  }
+}
+}  // namespace

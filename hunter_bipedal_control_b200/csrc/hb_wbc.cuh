@@ -306,3 +306,96 @@ __device__ inline int wbc_reduced_build(const WbcShared& sh, int mode, int nw, b
 }
 
 }  // namespace hb
+
+namespace {  // the kernels: internal linkage, the library exports only the hb_* entry points
+using namespace hb;
+constexpr int QP_STRIDE_H = NWBC * NWBC, QP_STRIDE_A = WBC_ROWS * NWBC;
+
+__global__ void wbc_assemble_kernel(int B, hb_wbc_settings ws, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
+                                    const uint8_t* stance_mode, double* H, double* g, double* A, double* lbA, double* ubA, int32_t* m_out) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
+  const int inst = blockIdx.x * wpb + warp;
+  if (inst >= B) return;
+  WbcShared& sh = reinterpret_cast<WbcShared*>(smem_raw)[warp];
+  const int m = wbc_assemble_warp(x_des + (size_t)inst * NX, u_des + (size_t)inst * NU, rbd + (size_t)inst * 32, mode[inst],
+                                  stance_mode ? stance_mode[inst] != 0 : false, ws, sh, H + (size_t)inst * QP_STRIDE_H, g + (size_t)inst * NWBC,
+                                  A + (size_t)inst * QP_STRIDE_A, lbA + (size_t)inst * WBC_ROWS, ubA + (size_t)inst * WBC_ROWS);
+  if (lane_id() == 0) m_out[inst] = m;
+}
+
+// Fused WeightedWbc step (K5+K6): assembly terms, reduced QP (tau and swing forces eliminated), interior point, expansion to
+// the reference's 38-vector [qdd, F, tau]. Shared memory per warp: QP workspace for n<=28 with the Hessian as a packed triangle (the
+// assembly scratch aliases the factorisation area, which is dead until the first Newton step) + the reduced constraint matrix.
+constexpr int WZ_N = 28, WZ_ME = 6, WZ_MI = 40, WZ_ROWS = 36;
+__host__ __device__ constexpr size_t wbc_fused_doubles() { return qp_workspace_doubles(WZ_N, WZ_ME, WZ_MI, true) + WZ_ROWS * WZ_N + 2 * WZ_ROWS + 3 * WZ_N + 16 + 8; }
+// One warp per block and one block per instance: 8 blocks per SM put a 1024-instance batch in one wave on 132 SMs (8 x 132 >= 1024;
+// at 7 a tail wave of 100 blocks costs almost as much as the full one). The runtime reserves 1 KB of shared memory per block.
+static_assert(8 * (wbc_fused_doubles() * sizeof(double) + 1024) <= 228 * 1024, "wbc_fused_kernel must fit 8 blocks per SM");
+
+__global__ void __launch_bounds__(32, 8) wbc_fused_kernel(int B, hb_wbc_settings ws, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const uint8_t* stance_mode,
+                                 double rho, int max_iter, double* sol, int32_t* status, int32_t* iters) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int warp = threadIdx.x >> 5, wpb = blockDim.x >> 5, lane = threadIdx.x & 31;
+  const int inst = blockIdx.x * wpb + warp;
+  if (inst >= B) return;
+  double* base = reinterpret_cast<double*>(smem_raw) + (size_t)warp * wbc_fused_doubles();
+  QpWorkspace w;
+  qp_carve(base, WZ_N, w, WZ_ME, WZ_MI, true);
+  double* p = base + qp_workspace_doubles(WZ_N, WZ_ME, WZ_MI, true);
+  double* Az = p; p += WZ_ROWS * WZ_N;
+  double* lbz = p; p += WZ_ROWS;
+  double* ubz = p; p += WZ_ROWS;
+  double* gz = p; p += WZ_N;
+  double* xz = p; p += WZ_N;
+  double* nlej = p; p += WZ_N;
+  int* stcol = reinterpret_cast<int*>(p);
+  static_assert(sizeof(WbcShared) <= sizeof(double) * (WZ_N * 29 + WZ_N * 7 + WZ_ME * 7 + WZ_N + WZ_ME + 6 * WZ_N + 5 * WZ_ME + 8 * WZ_MI), "assembly scratch must fit in the aliased area");
+  WbcShared& sh = *reinterpret_cast<WbcShared*>(w.K);   // K, V, S, vectors: dead until the QP starts
+  const int md = mode[inst];
+  int nw = 0;
+  wbc_assemble_warp(x_des + (size_t)inst * NX, u_des + (size_t)inst * NU, rbd + (size_t)inst * 32, md, stance_mode ? stance_mode[inst] != 0 : false, ws, sh,
+                    nullptr, nullptr, nullptr, nullptr, nullptr, &nw);
+  int m = 0;
+  const int nz = wbc_reduced_build(sh, md, nw, stance_mode ? stance_mode[inst] != 0 : false, rho, ws, u_des + (size_t)inst * NU, w.H, gz, Az, lbz, ubz, stcol, m);
+  if (lane < NJ) nlej[lane] = sh.nle[6 + lane];
+  __syncwarp();
+  // the workspace is carved for n = 28 (leading dimension 29); smaller problems (nz = 22, 16) use the same leading dimension
+  QpResult r = qp_solve_warp<true>(nz, m, nullptr, gz, Az, lbz, ubz, 0.0, max_iter, xz, w);
+  __syncwarp();
+  double* out = sol + (size_t)inst * NWBC;
+  if (lane < NQ) out[lane] = xz[lane];
+  if (lane < 12) {
+    double f = 0.0;
+    for (int c = 0; c < nz - NQ; ++c) if (stcol[c] == lane) f = xz[NQ + c];
+    out[NQ + lane] = f;
+  }
+  if (lane < NJ) {
+    double t = nlej[lane];
+    for (int c = 0; c < nz; ++c) t += Az[(6 + lane) * nz + c] * xz[c];
+    out[NQ + 12 + lane] = t;
+  }
+  if (lane == 0) { if (status) status[inst] = r.status; if (iters) iters[inst] = r.iters; }
+}
+
+// torque law (LeggedController.cpp:181-184): feed-forward joint torques = tail(10) of the WBC solution
+__global__ void torque_kernel(int B, const double* sol, double* torque) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx < B * NJ) { const int i = idx / NJ, j = idx - i * NJ; torque[idx] = sol[(size_t)i * NWBC + 28 + j]; }
+}
+
+// WeightedWbc::update fallback (WeightedWbc.cpp:57-64): a QP that did not solve returns the previous solution of that instance; a solved
+// one becomes the new "previous". `have_prev` is 0 on the first cycle after a cold start (the reference then returns the unsolved iterate).
+__global__ void wbc_fallback_kernel(int B, int have_prev, const int32_t* status, double* sol, double* prev, double* torque) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= B * NWBC) return;
+  const int i = idx / NWBC, j = idx - i * NWBC;
+  if (status[i] != 0 && have_prev) {
+    const double v = prev[idx];
+    sol[idx] = v;
+    if (torque && j >= 28) torque[(size_t)i * NJ + j - 28] = v;
+  } else {
+    prev[idx] = sol[idx];
+  }
+}
+}  // namespace
