@@ -37,6 +37,7 @@ EXPORTED_SYMBOLS = [
     "hb_time_grid_batch_dev", "hb_reference_expand_grid_batch_dev", "hb_mpc_solve_grid_batch_dev", "hb_policy_eval_grid_batch_dev",
     "hb_time_grid_batch", "hb_reference_expand_grid_batch", "hb_mpc_solve_grid_batch", "hb_resident_read_grid_batch", "hb_resident_write_batch",
     "hb_default_rollout_params", "hb_rollout_batch_dev",
+    "hb_default_estimation_params", "hb_estimation_reset", "hb_sim_read_sensors_batch_dev", "hb_sim_read_sensors", "hb_rollout_estimated_batch_dev",
 ]
 
 
@@ -243,6 +244,43 @@ def kf_states(B):
     st = (HbKfState * B)()
     _check(load_library().hb_kf_reset(B, st), "hb_kf_reset")
     return st
+
+
+class HbSensorNoise(C.Structure):
+    _fields_ = [("seed", C.c_uint64)] + [(k, C.c_double) for k in ("orientation", "angular_velocity", "linear_acceleration", "joint_position",
+                                                                   "joint_velocity")]
+
+
+class HbEstimationParams(C.Structure):
+    _fields_ = [("kf", HbKfParams), ("noise", HbSensorNoise)]
+
+
+class HbEstimationState(C.Structure):
+    _fields_ = [("kf", HbKfState), ("noise_stream", C.c_uint64), ("base_vel_prev", C.c_double * 3), ("primed", C.c_int32), ("yaw_obs", C.c_double),
+                ("has_plan", C.c_int32), ("n_events", C.c_int32), ("event_times", C.c_double * HB_MAX_EVENTS), ("modes", C.c_int32 * (HB_MAX_EVENTS + 1))]
+
+
+ESTIMATION_STATS_DTYPE = np.dtype([("max_vel_err", "f8"), ("max_height_err", "f8"), ("sum_sq_vel_err", "f8"), ("sum_sq_height_err", "f8"),
+                                   ("count", "i4")], align=True)
+
+
+def default_estimation_params():
+    """Default filter (hb_default_kf_params), no sensor noise, seed 0."""
+    p = HbEstimationParams()
+    _check(load_library().hb_default_estimation_params(C.byref(p)), "hb_default_estimation_params")
+    return p
+
+
+def estimation_states(B, first_stream=0):
+    """Fresh estimation states (filter reset, noise stream first_stream + i, unprimed accelerometer, no plan, yaw_obs = 0)."""
+    st = (HbEstimationState * B)()
+    _check(load_library().hb_estimation_reset(B, C.c_uint64(first_stream), st), "hb_estimation_reset")
+    return st
+
+
+def estimation_stats(B):
+    """Estimation stats of B fresh episodes: zeros."""
+    return np.zeros(B, dtype=ESTIMATION_STATS_DTYPE)
 
 
 class HbGaitSelector(C.Structure):
@@ -593,6 +631,17 @@ class Context:
                                                    _ptr(joint_pos), _ptr(joint_vel), _ptr(flags), _ptr(rbd)), "hb_estimator_update_batch", self._h)
         return rbd
 
+    def read_sensors(self, rbd, est, tick, noise=None, accel_dt=0.002):
+        """Sensors of the simulated robot at absolute tick `tick` from the true rbd [B,32] (hb_sim_read_sensors); `est` (ctypes array of
+        HbEstimationState) gives the noise streams and the accelerometer's previous velocity and is updated in place. noise: HbSensorNoise
+        (None: exact). Returns (quat [B,4], ang_vel_local [B,3], lin_acc_local [B,3], joint_pos [B,10], joint_vel [B,10])."""
+        rbd = _f64(rbd); B = rbd.shape[0]
+        noise = noise or HbSensorNoise()
+        quat = np.zeros((B, 4)); w = np.zeros((B, 3)); a = np.zeros((B, 3)); jp = np.zeros((B, NJ)); jv = np.zeros((B, NJ))
+        _check(self._lib.hb_sim_read_sensors(self._h, B, C.byref(noise), C.c_int64(tick), C.c_double(accel_dt), _ptr(rbd), est, _ptr(quat), _ptr(w), _ptr(a),
+                                             _ptr(jp), _ptr(jv)), "hb_sim_read_sensors", self._h)
+        return quat, w, a, jp, jv
+
     def actuation(self, time, state, command, rbd, delay=0.009):
         """LeggedHWSim::writeSim: delayed hybrid joint command -> applied joint torques [B,10]; `state` (ctypes array of HbActuationState) in place."""
         command, rbd = _f64(command), _f64(rbd); B = rbd.shape[0]
@@ -711,6 +760,38 @@ class Context:
                                               _ptr(d_st), _ptr(log)), "hb_rollout_batch_dev", self._h)
         self.sync()
         return rbd, act, estop, d_st.cpu().numpy().view(ROLLOUT_STATS_DTYPE), log
+
+    def rollout_estimated(self, rbd, commands, n_ticks, tick0=0, params=None, est_params=None, est=None, act=None, estop=None, stats=None, est_stats=None,
+                          log_every=0):
+        """rollout() with the controllers on the Kalman filter's estimate from noisy sensors (hb_rollout_estimated_batch_dev). est_params:
+        HbEstimationParams (None: default_estimation_params(), no noise); est: cuda uint8 tensor of B hb_estimation_state (None: fresh
+        estimation_states(B), in place); est_stats: ESTIMATION_STATS_DTYPE array (None: zeros). Returns rollout()'s tuple followed by
+        (est, est_stats, est_log): est_log the estimated rbd in log's layout, or None."""
+        import torch
+        B = rbd.shape[0]
+        dev = rbd.device
+        params = params or default_rollout_params()
+        params.log_every = int(log_every)
+        est_params = est_params or default_estimation_params()
+        if act is None:
+            act = torch.zeros(B * C.sizeof(HbActuationState), dtype=torch.uint8, device=dev)
+        if estop is None:
+            estop = torch.zeros(B, dtype=torch.uint8, device=dev)
+        if est is None:
+            est = torch.from_numpy(np.frombuffer(bytes(estimation_states(B)), dtype=np.uint8).copy()).to(dev)
+        st = rollout_stats(B) if stats is None else np.ascontiguousarray(stats, dtype=ROLLOUT_STATS_DTYPE)
+        d_st = torch.from_numpy(st.view(np.uint8).copy()).to(dev)
+        es = estimation_stats(B) if est_stats is None else np.ascontiguousarray(est_stats, dtype=ESTIMATION_STATS_DTYPE)
+        d_es = torch.from_numpy(es.view(np.uint8).copy()).to(dev)
+        rows = -(-n_ticks // log_every) if log_every > 0 else 0
+        log = torch.zeros((B, rows, 32), dtype=torch.float64, device=dev) if log_every > 0 else None
+        est_log = torch.zeros((B, rows, 32), dtype=torch.float64, device=dev) if log_every > 0 else None
+        torch.cuda.current_stream(dev).synchronize()          # the context's stream does not order itself after torch's
+        _check(self._lib.hb_rollout_estimated_batch_dev(self._h, B, C.c_int64(tick0), int(n_ticks), C.byref(params), C.byref(est_params), commands, _ptr(rbd),
+                                                        _ptr(act), _ptr(estop), _ptr(d_st), _ptr(est), _ptr(d_es), _ptr(log), _ptr(est_log)),
+               "hb_rollout_estimated_batch_dev", self._h)
+        self.sync()
+        return (rbd, act, estop, d_st.cpu().numpy().view(ROLLOUT_STATS_DTYPE), log, est, d_es.cpu().numpy().view(ESTIMATION_STATS_DTYPE), est_log)
 
     def control_step_dev(self, t_rel, x0, x_ref, swing, mode, rbd, xt, ut, info, sol, tau, status=None):
         _check(self._lib.hb_control_step_batch_dev(self._h, x0.shape[0], C.c_double(t_rel), _ptr(x0), _ptr(x_ref), _ptr(swing), _ptr(mode), _ptr(rbd), _ptr(xt),

@@ -64,6 +64,10 @@ struct hb_ctx {
   void* ro_mem;
   hb_rollout_command* ro_cmd; hb_plan_input* ro_in; hb_reference* ro_refs; hb_solve_info* ro_info; int32_t* ro_pstat;
   double *ro_t0, *ro_x0, *ro_feet, *ro_sol, *ro_jcmd, *ro_jtau, *ro_tau, *ro_held, *ro_tnow;
+  // hb_rollout_estimated_batch_dev's own scratch (first such call, at max_batch): the tick's sensor readings, contact flags, estimated rbd
+  void* re_mem;
+  double *re_quat, *re_gyro, *re_acc, *re_jpos, *re_jvel, *re_rbd;
+  uint8_t* re_flag;
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
   // hb_resident_cycle_batch's packed references / reference verdicts
   void* arena; size_t arena_cap;
@@ -373,7 +377,7 @@ int hb_destroy(hb_ctx* ctx) {
   cudaSetDevice(ctx->device);
   void* ptrs[] = {ctx->sqp_mem, ctx->dxt, ctx->dut, ctx->perf, ctx->flags, ctx->xdes, ctx->udes, ctx->wstatus, ctx->witers, ctx->wmode,
                   ctx->hoqp_mem, ctx->cyc_xref, ctx->cyc_swing, ctx->cyc_tk, ctx->cyc_mode, ctx->cyc_nn, ctx->res_t0, ctx->res_xt,
-                  ctx->res_ut, ctx->res_tk, ctx->res_mode, ctx->res_nn, ctx->res_sol, ctx->res_stance, ctx->arena, ctx->ro_mem};
+                  ctx->res_ut, ctx->res_tk, ctx->res_mode, ctx->res_nn, ctx->res_sol, ctx->res_stance, ctx->arena, ctx->ro_mem, ctx->re_mem};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -697,8 +701,8 @@ int hb_estimator_update_batch_dev(hb_ctx* ctx, int B, const hb_kf_params* params
   if (!ctx || B < 0 || !params || !state || !quat || !ang_vel_local || !lin_acc_local || !joint_pos || !joint_vel || !contact_flag || !rbd_out) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
-  return launch(ctx, K_UNPROFILED, kf_update_kernel, B, 32, sizeof(KfShared), B, *params, dt, state, quat, ang_vel_local, lin_acc_local, joint_pos,
-                joint_vel, contact_flag, rbd_out);
+  return launch(ctx, K_UNPROFILED, kf_update_kernel<hb_kf_state>, B, 32, sizeof(KfShared), B, *params, dt, state, quat, ang_vel_local, lin_acc_local,
+                joint_pos, joint_vel, contact_flag, rbd_out);
 }
 
 int hb_default_wbc_settings(hb_wbc_settings* s) {
@@ -906,12 +910,40 @@ static int rollout_reserve(hb_ctx* ctx) {
   });
 }
 
-int hb_rollout_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb_rollout_params* p, const hb_rollout_command* cmd, double* rbd,
-                         hb_actuation_state* act, uint8_t* estop, hb_rollout_stats* stats, double* log) {
+// hb_rollout_estimated_batch_dev's scratch, at max_batch
+static int estimation_reserve(hb_ctx* ctx) {
+  const size_t Bc = ctx->cfg.max_batch;
+  return reserve_group(&ctx->re_mem, [&](void* m) {
+    size_t off = 0;
+    ctx->re_quat = carve<double>(m, off, Bc * 4); ctx->re_gyro = carve<double>(m, off, Bc * 3); ctx->re_acc = carve<double>(m, off, Bc * 3);
+    ctx->re_jpos = carve<double>(m, off, Bc * NJ); ctx->re_jvel = carve<double>(m, off, Bc * NJ); ctx->re_rbd = carve<double>(m, off, Bc * 32);
+    ctx->re_flag = carve<uint8_t>(m, off, Bc * 4);
+    return off;
+  });
+}
+
+static bool sensor_noise_ok(const hb_sensor_noise& n) {
+  for (double s : {n.orientation, n.angular_velocity, n.linear_acceleration, n.joint_position, n.joint_velocity})
+    if (!(s >= 0.0) || !isfinite(s)) return false;
+  return true;
+}
+
+// the estimation arguments of an estimated episode; a null pointer to them is hb_rollout_batch_dev
+struct EstimationArgs {
+  const hb_estimation_params* ep;
+  hb_estimation_state* est;
+  hb_estimation_stats* stats;   // nullable
+  double* log;                  // nullable
+};
+
+// The episode loop of hb_rollout_batch_dev (e == nullptr: exactly its launches) and hb_rollout_estimated_batch_dev
+static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb_rollout_params* p, const hb_rollout_command* cmd, double* rbd,
+                        hb_actuation_state* act, uint8_t* estop, hb_rollout_stats* stats, double* log, const EstimationArgs* e) {
   if (!ctx || B < 0 || n_ticks < 0 || tick0 < 0 || !p || !cmd || !rbd || !act || !estop || !stats) return HB_EINVAL;
   if (p->mpc_every < 1 || !(p->period > 0.0) || p->log_every < 0 || !(p->actuation_delay >= 0.0) || !(p->sim.dt > 0.0) || p->sim.substeps < 1 ||
       p->sim.substeps > 1000 || tick0 + n_ticks > INT32_MAX)
     return HB_EINVAL;
+  if (e && (!e->ep || !e->est || !sensor_noise_ok(e->ep->noise))) return HB_EINVAL;
   if (B == 0) return HB_OK;
   if (B > ctx->cfg.max_batch) return HB_ECAP;
   for (int i = 0; i < B; ++i) {
@@ -924,11 +956,15 @@ int hb_rollout_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const h
   if (n_ticks == 0) return HB_OK;
   if (set_device(ctx)) return HB_ECUDA;
   int rc = rollout_reserve(ctx);
+  if (!rc && e) rc = estimation_reserve(ctx);
   if (rc) return rc;
   CK(cudaMemcpyAsync(ctx->ro_cmd, cmd, sizeof(hb_rollout_command) * B, cudaMemcpyHostToDevice, ctx->stream));
   const double horizon = (ctx->cfg.event_nodes && ctx->cfg.time_horizon > 0.0) ? ctx->cfg.time_horizon : ctx->cfg.horizon_N * ctx->cfg.dt;
   const int n_log = (log && p->log_every > 0) ? (n_ticks + p->log_every - 1) / p->log_every : 0;
+  const int n_est_log = (e && e->log && p->log_every > 0) ? (n_ticks + p->log_every - 1) / p->log_every : 0;
   const unsigned grid = (B + 63) / 64;
+  // what the controllers measure: the true state, or the filter's estimate
+  double* meas = e ? ctx->re_rbd : rbd;
   for (int k = 0; k < n_ticks && !rc; ++k) {
     const int64_t a = tick0 + k;
     const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
@@ -936,16 +972,26 @@ int hb_rollout_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const h
     double* log_row = (n_log && k % p->log_every == 0) ? log + (size_t)(k / p->log_every) * 32 : nullptr;
     rc = launch(ctx, K_UNPROFILED, rollout_tick_begin_kernel, grid, 64, 0, B, (int)a, t, p->min_base_height, rbd, ctx->ro_held, stats, ctx->ro_tnow,
                 log_row, (size_t)n_log * 32);
+    if (!rc && e) {
+      // LeggedController::updateStateEstimation: sensors and contact flags at the previous observation's time, filter, observation step
+      double* est_row = (n_est_log && k % p->log_every == 0) ? e->log + (size_t)(k / p->log_every) * 32 : nullptr;
+      rc = launch(ctx, K_UNPROFILED, sensor_read_kernel, grid, 64, 0, B, e->ep->noise, (uint32_t)a, p->sim.dt, (double)(a - 1) * p->period, rbd, e->est,
+                  ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag);
+      if (!rc) rc = launch(ctx, K_UNPROFILED, kf_update_kernel<hb_estimation_state>, B, 32, sizeof(KfShared), B, e->ep->kf, p->period, e->est, ctx->re_quat,
+                           ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag, meas);
+      if (!rc) rc = launch(ctx, K_UNPROFILED, est_observe_kernel, grid, 64, 0, B, rbd, meas, stats, e->est, e->stats, est_row, (size_t)n_est_log * 32);
+    }
     if (!rc && mpc) {
       if (first_cold) CK(cudaMemsetAsync(ctx->res_stance, 0, sizeof(double) * B * 12, ctx->stream));   // latestStanceposition_ starts at zero
-      rc = launch(ctx, K_UNPROFILED, rollout_plan_inputs_kernel, grid, 64, 0, B, t, horizon, ctx->ro_cmd, rbd, ctx->ro_in);
+      rc = launch(ctx, K_UNPROFILED, rollout_plan_inputs_kernel, grid, 64, 0, B, t, horizon, ctx->ro_cmd, meas, e ? e->est : nullptr, ctx->ro_in);
       if (!rc) rc = launch(ctx, K_UNPROFILED, plan_prepare_kernel, grid, 64, 0, B, ctx->ro_in, ctx->ro_t0, ctx->ro_x0, ctx->ro_feet);
       if (!rc) rc = hb_plan_references_batch_dev(ctx, B, ctx->ro_in, ctx->ro_feet, ctx->res_stance, ctx->ro_refs, ctx->ro_pstat);
-      if (!rc) rc = resident_cycle_impl(ctx, B, first_cold, 0.0, ctx->ro_t0, ctx->ro_x0, ctx->ro_refs, rbd, ctx->ro_info, nullptr, nullptr, nullptr, false);
+      if (!rc) rc = resident_cycle_impl(ctx, B, first_cold, 0.0, ctx->ro_t0, ctx->ro_x0, ctx->ro_refs, meas, ctx->ro_info, nullptr, nullptr, nullptr, false);
+      if (!rc && e) rc = launch(ctx, K_UNPROFILED, est_schedule_kernel, grid, 64, 0, B, ctx->ro_refs, e->est);
     }
     // the cycle ran no WBC, so after a cold start the first tick's fallback has no previous solution, as the cycle's own would not have
-    if (!rc) rc = resident_wbc_impl(ctx, B, ctx->ro_tnow, rbd, nullptr, ctx->xdes, ctx->udes, ctx->wmode, ctx->ro_sol, nullptr, ctx->wstatus, first_cold);
-    if (!rc) rc = hb_joint_command_batch_dev(ctx, B, &p->gains, p->period, ctx->xdes, ctx->udes, ctx->ro_sol, ctx->wmode, rbd, nullptr, estop, ctx->ro_jcmd,
+    if (!rc) rc = resident_wbc_impl(ctx, B, ctx->ro_tnow, meas, nullptr, ctx->xdes, ctx->udes, ctx->wmode, ctx->ro_sol, nullptr, ctx->wstatus, first_cold);
+    if (!rc) rc = hb_joint_command_batch_dev(ctx, B, &p->gains, p->period, ctx->xdes, ctx->udes, ctx->ro_sol, ctx->wmode, meas, nullptr, estop, ctx->ro_jcmd,
                                              ctx->ro_jtau);
     if (!rc) rc = hb_actuation_batch_dev(ctx, B, p->actuation_delay, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, ctx->ro_tau);
@@ -953,6 +999,46 @@ int hb_rollout_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const h
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_tick_end_kernel, grid, 64, 0, B, (int)a, mpc ? 1 : 0, ctx->ro_info, ctx->ro_pstat, ctx->wstatus, estop, ctx->ro_tau, ctx->ro_held, rbd, stats);
   }
   return rc;
+}
+
+int hb_rollout_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb_rollout_params* p, const hb_rollout_command* cmd, double* rbd,
+                         hb_actuation_state* act, uint8_t* estop, hb_rollout_stats* stats, double* log) {
+  return rollout_impl(ctx, B, tick0, n_ticks, p, cmd, rbd, act, estop, stats, log, nullptr);
+}
+
+int hb_rollout_estimated_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb_rollout_params* p, const hb_estimation_params* ep,
+                                   const hb_rollout_command* cmd, double* rbd, hb_actuation_state* act, uint8_t* estop, hb_rollout_stats* stats,
+                                   hb_estimation_state* est, hb_estimation_stats* est_stats, double* log, double* est_log) {
+  const EstimationArgs e{ep, est, est_stats, est_log};
+  return rollout_impl(ctx, B, tick0, n_ticks, p, cmd, rbd, act, estop, stats, log, &e);
+}
+
+int hb_default_estimation_params(hb_estimation_params* p) {
+  if (!p) return HB_EINVAL;
+  memset(p, 0, sizeof(*p));
+  return hb_default_kf_params(&p->kf);
+}
+
+int hb_estimation_reset(int B, uint64_t first_stream, hb_estimation_state* state) {
+  if (B < 0 || !state) return HB_EINVAL;
+  for (int i = 0; i < B; ++i) {
+    memset(&state[i], 0, sizeof(hb_estimation_state));
+    hb_kf_reset(1, &state[i].kf);
+    state[i].noise_stream = first_stream + (uint64_t)i;
+  }
+  return HB_OK;
+}
+
+int hb_sim_read_sensors_batch_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, double accel_dt, const double* rbd,
+                                  hb_estimation_state* est, double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos,
+                                  double* joint_vel) {
+  if (!ctx || B < 0 || !noise || !rbd || !est || !quat || !ang_vel_local || !lin_acc_local || !joint_pos || !joint_vel) return HB_EINVAL;
+  if (!sensor_noise_ok(*noise) || !(accel_dt > 0.0) || tick < 0 || tick > UINT32_MAX) return HB_EINVAL;
+  if (B == 0) return HB_OK;
+  if (B > ctx->cfg.max_batch) return HB_ECAP;
+  if (set_device(ctx)) return HB_ECUDA;
+  return launch(ctx, K_UNPROFILED, sensor_read_kernel, (B + 63) / 64, 64, 0, B, *noise, (uint32_t)tick, accel_dt, 0.0, rbd, est, quat, ang_vel_local,
+                lin_acc_local, joint_pos, joint_vel, (uint8_t*)nullptr);
 }
 
 int hb_observer_reset(int B, hb_observer_state* state) {
@@ -1369,6 +1455,19 @@ int hb_estimator_update_batch(hb_ctx* ctx, int B, const hb_kf_params* params, do
   auto kf = s.inout(state, 1); auto q = s.in(quat, 4); auto w = s.in(ang_vel_local, 3); auto a = s.in(lin_acc_local, 3);
   auto jp = s.in(joint_pos, NJ); auto jv = s.in(joint_vel, NJ); auto fl = s.in(contact_flag, 4); auto ro = s.out(rbd_out, 32);
   return s.run([&] { return hb_estimator_update_batch_dev(ctx, B, params, dt, kf, q, w, a, jp, jv, fl, ro); });
+}
+
+int hb_sim_read_sensors(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, double accel_dt, const double* rbd, hb_estimation_state* est,
+                        double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos, double* joint_vel) {
+  if (!ctx || B < 0 || !noise || !rbd || !est || !quat || !ang_vel_local || !lin_acc_local || !joint_pos || !joint_vel) return HB_EINVAL;
+  if (!sensor_noise_ok(*noise) || !(accel_dt > 0.0) || tick < 0 || tick > UINT32_MAX) return HB_EINVAL;
+  if (B == 0) return HB_OK;
+  if (B > ctx->cfg.max_batch) return HB_ECAP;
+  if (set_device(ctx)) return HB_ECUDA;
+  Staging s(ctx, B);
+  auto r = s.in(rbd, 32); auto es = s.inout(est, 1); auto q = s.out(quat, 4); auto w = s.out(ang_vel_local, 3); auto a = s.out(lin_acc_local, 3);
+  auto jp = s.out(joint_pos, NJ); auto jv = s.out(joint_vel, NJ);
+  return s.run([&] { return hb_sim_read_sensors_batch_dev(ctx, B, noise, tick, accel_dt, r, es, q, w, a, jp, jv); });
 }
 
 int hb_actuation_batch(hb_ctx* ctx, int B, double delay, const double* time, hb_actuation_state* state, const double* command, const double* rbd,

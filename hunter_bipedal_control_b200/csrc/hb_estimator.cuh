@@ -22,12 +22,16 @@ __device__ __forceinline__ double kf_c_row(const double* M, int ld, int r, int c
   if (r < 24) return M[(3 + (r % 3)) * ld + c];
   return M[(8 + 3 * (r - 24)) * ld + c];
 }
-__global__ void __launch_bounds__(32) kf_update_kernel(int B, hb_kf_params prm, double dt, hb_kf_state* state, const double* quat, const double* angl,
+// the filter state of one instance: hb_estimator_update_batch passes hb_kf_state[], the estimated episodes their hb_estimation_state[]
+__device__ __forceinline__ hb_kf_state& kf_of(hb_kf_state& s) { return s; }
+__device__ __forceinline__ hb_kf_state& kf_of(hb_estimation_state& s) { return s.kf; }
+template <class State>
+__global__ void __launch_bounds__(32) kf_update_kernel(int B, hb_kf_params prm, double dt, State* state, const double* quat, const double* angl,
                                                        const double* accl, const double* jpos, const double* jvel, const uint8_t* cflag, double* rbd_out) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   KfShared& sh = *reinterpret_cast<KfShared*>(smem_raw);
   const int inst = blockIdx.x, lane = threadIdx.x;
-  hb_kf_state& st = state[inst];
+  hb_kf_state& st = kf_of(state[inst]);
   // ---- updateImu: quaternion -> ZYX angles, local angular velocity -> Euler rates -> global angular velocity (every lane, registers)
   const double qx = quat[4 * inst], qy = quat[4 * inst + 1], qz = quat[4 * inst + 2], qw = quat[4 * inst + 3];
   double zyx[3];

@@ -100,10 +100,13 @@ HBP_HD inline bool tile_gait(int gait, double prev_event, double start, double t
 }
 
 // ModeSchedule::modeAtTime: lower_bound on the event times (an event time itself belongs to the earlier mode)
-HBP_HD inline int mode_at(const ModeSchedule& ms, double t) {
+HBP_HD inline int mode_at(int n_events, const double* events, const int* modes, double t) {
   int idx = 0;
-  while (idx < ms.n_events && ms.events[idx] < t) ++idx;
-  return ms.modes[idx];
+  while (idx < n_events && events[idx] < t) ++idx;
+  return modes[idx];
+}
+HBP_HD inline int mode_at(const ModeSchedule& ms, double t) {
+  return mode_at(ms.n_events, ms.events, ms.modes, t);
 }
 
 struct Target { int n; double t[HB_MAX_TARGETS]; double x[HB_MAX_TARGETS][22]; };

@@ -2,6 +2,7 @@
 // per-instance kernels the episode loop adds around them, the device planner, the resident cycle and the 500 Hz WBC tick.
 #pragma once
 #include "hb_common.cuh"
+#include "hb_planner.h"
 #include "hb_qp.cuh"
 #include "hb_rbd.cuh"
 #include "../../include/hunter_b200.h"
@@ -10,8 +11,10 @@ namespace hb {
 
 // Plan inputs of the MPC cycle at time t, with the defaults of api.make_plan_inputs: x0 = the centroidal restatement of the measured rbd,
 // cmd_vel of the last command segment that has started (the first one before that), prev_event = min(t, gait_start) - 0.5, IK joint
-// references. feet_pos is left zero: plan_prepare_kernel computes the feet from x0.
-__global__ void rollout_plan_inputs_kernel(int B, double t, double horizon, const hb_rollout_command* cmd, const double* rbd, hb_plan_input* in) {
+// references. feet_pos is left zero: plan_prepare_kernel computes the feet from x0. With est (estimated episodes) x0[9] is the unwrapped
+// observation yaw (LeggedController.cpp:335-337).
+__global__ void rollout_plan_inputs_kernel(int B, double t, double horizon, const hb_rollout_command* cmd, const double* rbd, const hb_estimation_state* est,
+                                           hb_plan_input* in) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
   const hb_rollout_command& c = cmd[inst];
@@ -22,6 +25,7 @@ __global__ void rollout_plan_inputs_kernel(int B, double t, double horizon, cons
   for (int k = 1; k < c.n_cmd; ++k) if (c.cmd_time[k] <= t) j = k;
   for (int i = 0; i < 4; ++i) p.cmd_vel[i] = c.cmd_vel[j][i];
   rbd_to_centroidal(rbd + (size_t)inst * 32, p.x0);
+  if (est) p.x0[9] = est[inst].yaw_obs;
   for (int i = 0; i < 12; ++i) p.feet_pos[i] = 0.0;
   p.gait = c.gait; p.joint_ik = 1;
 }
@@ -90,6 +94,138 @@ __global__ void rollout_tick_end_kernel(int B, int tick, int mpc_tick, const hb_
     if (restore) { s.fail_tick = tick + 1; s.fail_reason = HB_ROLLOUT_FAIL_NONFINITE; }
   }
   if (restore) for (int i = 0; i < 32; ++i) r[i] = held[(size_t)inst * 32 + i];
+}
+
+// ---- estimated episodes (hb_rollout_estimated_batch_dev, hb_sim_read_sensors_batch_dev)
+
+// Philox4x32-10 (Salmon et al., SC'11): counter c encrypted under key (k0, k1), in place. Written out rather than taken from curand so that
+// the noise is a documented function a test can restate.
+__device__ __forceinline__ void philox4x32_10(uint32_t k0, uint32_t k1, uint32_t c[4]) {
+  for (int round = 0; round < 10; ++round) {
+    if (round) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+    const uint64_t p0 = (uint64_t)0xD2511F53u * c[0], p1 = (uint64_t)0xCD9E8D57u * c[2];
+    const uint32_t n0 = (uint32_t)(p1 >> 32) ^ c[1] ^ k0, n2 = (uint32_t)(p0 >> 32) ^ c[3] ^ k1;
+    c[0] = n0; c[1] = (uint32_t)p1; c[2] = n2; c[3] = (uint32_t)p0;
+  }
+}
+
+// Noise block numbers: each sensor channel owns fixed blocks of 4 normals, so a channel with sigma 0 draws nothing and shifts no other one.
+enum { NOISE_BLOCK_ORIENTATION = 0, NOISE_BLOCK_GYRO = 1, NOISE_BLOCK_ACCEL = 2, NOISE_BLOCK_JOINT_POS = 3, NOISE_BLOCK_JOINT_VEL = 6 };
+
+// v[0..m) += sigma x normals of blocks block0, block0 + 1, ...: counter (block, tick, stream_lo, stream_hi), key (seed_lo, seed_hi); the 4 words
+// w of a block are u = (w + 0.5) 2^-32 and Box-Muller turns (u0, u1) and (u2, u3) into normals 0, 1 and 2, 3.
+__device__ __forceinline__ void add_sensor_noise(double sigma, uint64_t seed, int block0, uint32_t tick, uint64_t stream, double* v, int m) {
+  if (!(sigma > 0.0)) return;
+  double n[4];
+  for (int j = 0; j < m; ++j) {
+    if (j % 4 == 0) {
+      uint32_t c[4] = {(uint32_t)(block0 + j / 4), tick, (uint32_t)stream, (uint32_t)(stream >> 32)};
+      philox4x32_10((uint32_t)seed, (uint32_t)(seed >> 32), c);
+      for (int h = 0; h < 2; ++h) {
+        const double u0 = ((double)c[2 * h] + 0.5) * 0x1p-32, u1 = ((double)c[2 * h + 1] + 0.5) * 0x1p-32;
+        const double r = sqrt(-2.0 * log(u0));
+        double s, co;
+        sincos(2.0 * M_PI * u1, &s, &co);
+        n[2 * h] = r * co; n[2 * h + 1] = r * s;
+      }
+    }
+    v[j] += sigma * n[j % 4];
+  }
+}
+
+// The simulated robot's sensors at absolute tick `tick` from the true rbd r (LeggedHWSim::readSim, LeggedHWSim.cpp:116-130, and the joint
+// encoders). The accelerometer differences the world base velocity over the last plant step (accel_dt) where Gazebo reads the instantaneous
+// acceleration; unprimed, it reads gravity only. Updates base_vel_prev / primed.
+__device__ __forceinline__ void read_sensors(const hb_sensor_noise& nz, uint32_t tick, double accel_dt, const double* r, hb_estimation_state& e,
+                                             double* quat, double* gyro, double* acc, double* jp, double* jv) {
+  double sz, cz, sy, cy, sx, cx;
+  sincos(r[0], &sz, &cz); sincos(r[1], &sy, &cy); sincos(r[2], &sx, &cx);
+  const double R[9] = {cz * cy, cz * sy * sx - sz * cx, cz * sy * cx + sz * sx, sz * cy, sz * sy * sx + cz * cx, sz * sy * cx - cz * sx, -sy, cy * sx, cy * cx};
+  double aw[3] = {0.0, 0.0, 0.0};
+  if (e.primed) for (int i = 0; i < 3; ++i) aw[i] = (r[NQ + 3 + i] - e.base_vel_prev[i]) / accel_dt;
+  aw[2] += 9.81;
+  double ang[3] = {r[0], r[1], r[2]}, g[3], a[3], q[NJ], qd[NJ];
+  for (int i = 0; i < 3; ++i) {
+    g[i] = R[i] * r[NQ] + R[3 + i] * r[NQ + 1] + R[6 + i] * r[NQ + 2];           // R' omega_world: RelativeAngularVel
+    a[i] = R[i] * aw[0] + R[3 + i] * aw[1] + R[6 + i] * aw[2];
+  }
+  for (int j = 0; j < NJ; ++j) { q[j] = r[6 + j]; qd[j] = r[NQ + 6 + j]; }
+  for (int i = 0; i < 3; ++i) { e.base_vel_prev[i] = r[NQ + 3 + i]; }
+  e.primed = 1;
+  const uint64_t st = e.noise_stream;
+  add_sensor_noise(nz.orientation, nz.seed, NOISE_BLOCK_ORIENTATION, tick, st, ang, 3);
+  add_sensor_noise(nz.angular_velocity, nz.seed, NOISE_BLOCK_GYRO, tick, st, g, 3);
+  add_sensor_noise(nz.linear_acceleration, nz.seed, NOISE_BLOCK_ACCEL, tick, st, a, 3);
+  add_sensor_noise(nz.joint_position, nz.seed, NOISE_BLOCK_JOINT_POS, tick, st, q, NJ);
+  add_sensor_noise(nz.joint_velocity, nz.seed, NOISE_BLOCK_JOINT_VEL, tick, st, qd, NJ);
+  // quaternion (x, y, z, w) of R = Rz(yaw) Ry(pitch) Rx(roll)
+  double hsz, hcz, hsy, hcy, hsx, hcx;
+  sincos(0.5 * ang[0], &hsz, &hcz); sincos(0.5 * ang[1], &hsy, &hcy); sincos(0.5 * ang[2], &hsx, &hcx);
+  quat[0] = hcz * hcy * hsx - hsz * hsy * hcx; quat[1] = hcz * hsy * hcx + hsz * hcy * hsx;
+  quat[2] = hsz * hcy * hcx - hcz * hsy * hsx; quat[3] = hcz * hcy * hcx + hsz * hsy * hsx;
+  for (int i = 0; i < 3; ++i) { gyro[i] = g[i]; acc[i] = a[i]; }
+  for (int j = 0; j < NJ; ++j) { jp[j] = q[j]; jv[j] = qd[j]; }
+}
+
+// Sensor read of B instances, one thread each. With cflag (the episode tick) the filter's contact flags come from the stored schedule of the
+// latest plan at flag_time, the previous observation's time (LeggedController.cpp:296-297), all 1 before the first plan (:298-304).
+__global__ void sensor_read_kernel(int B, hb_sensor_noise nz, uint32_t tick, double accel_dt, double flag_time, const double* rbd, hb_estimation_state* est,
+                                   double* quat, double* gyro, double* acc, double* jp, double* jv, uint8_t* cflag) {
+  const int inst = blockIdx.x * blockDim.x + threadIdx.x;
+  if (inst >= B) return;
+  hb_estimation_state& e = est[inst];
+  read_sensors(nz, tick, accel_dt, rbd + (size_t)inst * 32, e, quat + (size_t)inst * 4, gyro + (size_t)inst * 3, acc + (size_t)inst * 3,
+               jp + (size_t)inst * NJ, jv + (size_t)inst * NJ);
+  if (cflag) {
+    const int mode = e.has_plan ? hbplan::mode_at(e.n_events, e.event_times, e.modes, flag_time) : 3;
+    for (int c = 0; c < 4; ++c) cflag[(size_t)inst * 4 + c] = contact_flag(mode, c) ? 1 : 0;
+  }
+}
+
+// angles::normalize_angle_positive / normalize_angle / shortest_angular_distance (ROS angles): fmod and one subtraction, all exact
+__device__ __forceinline__ double shortest_angular_distance(double from, double to) {
+  const double two_pi = 2.0 * M_PI;
+  double a = fmod(fmod(to - from, two_pi) + two_pi, two_pi);
+  if (a > M_PI) a -= two_pi;
+  return a;
+}
+
+// The observation step after the filter (LeggedController.cpp:334-337): yaw_obs follows the filter's wrapped yaw by the shortest angular
+// distance. Errors of the estimate against the true state entering the tick count while the instance has not failed; est_log takes the
+// estimated rbd. The squares and sums are rounded one operation at a time (no contraction) so that a restatement reproduces them.
+__global__ void est_observe_kernel(int B, const double* rbd, const double* est_rbd, const hb_rollout_stats* stats, hb_estimation_state* est,
+                                   hb_estimation_stats* est_stats, double* log_row, size_t log_stride) {
+  const int inst = blockIdx.x * blockDim.x + threadIdx.x;
+  if (inst >= B) return;
+  const double* r = rbd + (size_t)inst * 32;
+  const double* e = est_rbd + (size_t)inst * 32;
+  hb_estimation_state& s = est[inst];
+  s.yaw_obs = s.yaw_obs + shortest_angular_distance(s.yaw_obs, e[0]);
+  if (est_stats && stats[inst].fail_tick < 0) {
+    hb_estimation_stats& es = est_stats[inst];
+    const double d0 = e[NQ + 3] - r[NQ + 3], d1 = e[NQ + 4] - r[NQ + 4], d2 = e[NQ + 5] - r[NQ + 5], dz = fabs(e[5] - r[5]);
+    const double sq = __dadd_rn(__dadd_rn(__dmul_rn(d0, d0), __dmul_rn(d1, d1)), __dmul_rn(d2, d2)), ve = sqrt(sq);
+    if (ve > es.max_vel_err) es.max_vel_err = ve;
+    if (dz > es.max_height_err) es.max_height_err = dz;
+    es.sum_sq_vel_err = __dadd_rn(es.sum_sq_vel_err, sq);
+    es.sum_sq_height_err = __dadd_rn(es.sum_sq_height_err, __dmul_rn(dz, dz));
+    es.count += 1;
+  }
+  if (log_row) for (int i = 0; i < 32; ++i) log_row[inst * log_stride + i] = e[i];
+}
+
+// After an MPC cycle of an estimated episode: the mode schedule the cycle used becomes the instance's own, so that the filter's contact
+// flags survive the end of the call (the next call reads no context scratch of this one)
+__global__ void est_schedule_kernel(int B, const hb_reference* refs, hb_estimation_state* est) {
+  const int inst = blockIdx.x * blockDim.x + threadIdx.x;
+  if (inst >= B) return;
+  const hb_reference& f = refs[inst];
+  hb_estimation_state& s = est[inst];
+  const int n = f.n_events < HB_MAX_EVENTS ? f.n_events : HB_MAX_EVENTS;
+  s.n_events = n;
+  for (int i = 0; i < n; ++i) s.event_times[i] = f.event_times[i];
+  for (int i = 0; i <= n; ++i) s.modes[i] = f.modes[i];
+  s.has_plan = 1;
 }
 
 }  // namespace hb

@@ -232,6 +232,38 @@ typedef struct {                 /* per-instance outcome, in/out: start an episo
 } hb_rollout_stats;
 int hb_default_rollout_params(hb_rollout_params* p);       /* host only */
 
+/* ---- estimated episodes (hb_rollout_estimated_batch_dev): the controllers read the Kalman filter's estimate from synthesised, noisy
+ * sensors instead of the plant's true state (LeggedController::updateStateEstimation, LeggedController.cpp:280-349) ---- */
+typedef struct {                 /* standard deviations of additive Gaussian sensor noise; 0 = that channel is exact and draws nothing */
+  uint64_t seed;                 /* Philox4x32-10 key                                                                              */
+  double orientation;            /* on each ZYX angle before the quaternion [rad]                                                  */
+  double angular_velocity;       /* gyro, body frame [rad/s]                                                                       */
+  double linear_acceleration;    /* accelerometer, body frame [m/s^2]                                                              */
+  double joint_position, joint_velocity;   /* encoders [rad], [rad/s]                                                             */
+} hb_sensor_noise;
+typedef struct {
+  hb_kf_params kf;               /* hb_default_kf_params, or hb_parse_task_info(...).kalman                                        */
+  hb_sensor_noise noise;
+} hb_estimation_params;
+typedef struct {                 /* per instance, in/out, device memory for the episode call; hb_estimation_reset starts it       */
+  hb_kf_state kf;
+  uint64_t noise_stream;         /* Philox counter words 2-3: the instance's noise stream, independent of its batch position       */
+  double base_vel_prev[3];       /* world base velocity at the last sensor read (accelerometer finite difference)                  */
+  int32_t primed;                /* 0: no previous read, the accelerometer reads gravity only                                      */
+  double yaw_obs;                /* unwrapped yaw handed to the MPC (currentObservation_.state(9))                                 */
+  int32_t has_plan, n_events;    /* mode schedule of the latest plan (contact flags of the filter); has_plan = 0: all feet trusted */
+  double event_times[HB_MAX_EVENTS];
+  int32_t modes[HB_MAX_EVENTS + 1];
+} hb_estimation_state;
+typedef struct {                 /* per instance, in/out; counts while the instance has not failed (as hb_rollout_stats)            */
+  double max_vel_err, max_height_err;          /* |v_hat - v| (world base linear velocity), |z_hat - z|, against the true state entering the tick */
+  double sum_sq_vel_err, sum_sq_height_err;
+  int32_t count;                               /* ticks counted                                                                  */
+} hb_estimation_stats;
+int hb_default_estimation_params(hb_estimation_params* p);  /* host only: default filter, no noise, seed 0 */
+/* host only: x_hat = 0, P = 100 I, feet heights 0 (hb_kf_reset), noise_stream = first_stream + i, primed = has_plan = 0, yaw_obs = 0 */
+int hb_estimation_reset(int B, uint64_t first_stream, hb_estimation_state* state);
+
 int hb_default_kf_params(hb_kf_params* p);
 /* x_hat = 0, P = 100 I, heights = 0 (KalmanFilterEstimate constructor, LinearKalmanFilter.cpp:24-63); host only */
 int hb_kf_reset(int B, hb_kf_state* state);
@@ -359,6 +391,25 @@ int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const dou
  * the first call and freed by hb_destroy. */
 int hb_rollout_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb_rollout_params* p, const hb_rollout_command* cmd, double* rbd,
                          hb_actuation_state* act, uint8_t* estop, hb_rollout_stats* stats, double* log /*nullable*/);
+/* The sensors of the simulated robot (LeggedHWSim::readSim, legged_gazebo/src/LeggedHWSim.cpp:116-130, and the joint encoders) read from the
+ * true rbd at absolute tick `tick`, in the inputs hb_estimator_update_batch takes: quat (B x 4, x y z w) of the ZYX angles after noise on
+ * the angles; ang_vel_local (B x 3) = R' omega_world; lin_acc_local (B x 3) = R' (a_world + (0, 0, 9.81)) with a_world = (v - base_vel_prev)
+ * / accel_dt, or 0 on an unprimed instance; joint_pos / joint_vel (B x 10) = q_j, qd_j; each plus sigma x its Philox normals. est (B) is
+ * read for noise_stream / base_vel_prev / primed and gets base_vel_prev = v, primed = 1. Device pointers, asynchronous. */
+int hb_sim_read_sensors_batch_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, double accel_dt, const double* rbd,
+                                  hb_estimation_state* est, double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos,
+                                  double* joint_vel);
+/* hb_rollout_batch_dev with the controllers on the estimated state. Every tick, after the start-of-tick checks: sensors from the true rbd
+ * (hb_sim_read_sensors_batch_dev, accel_dt = p->sim.dt) and the filter's contact flags from the stored mode schedule at (tick - 1) * period
+ * (all 1 before the first plan), hb_estimator_update at dt = period, yaw_obs += the shortest angular distance to the filter's yaw, est_stats
+ * and est_log. On MPC ticks the plan inputs come from the estimated rbd with x0[9] = yaw_obs, the planner and the cycle see the estimate,
+ * and the schedule of the new plan is copied into est. The policy, the WeightedWbc and the joint command law see the estimated rbd;
+ * actuation, saturation, the plant and the failure checks the true one. est (B) is in/out; est_stats (B, nullable) in/out; est_log
+ * (nullable) the estimated rbd in log's layout. Arguments are checked before any launch (sigmas finite and >= 0). */
+int hb_rollout_estimated_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb_rollout_params* p, const hb_estimation_params* ep,
+                                   const hb_rollout_command* cmd, double* rbd, hb_actuation_state* act, uint8_t* estop, hb_rollout_stats* stats,
+                                   hb_estimation_state* est, hb_estimation_stats* est_stats /*nullable*/, double* log /*nullable*/,
+                                   double* est_log /*nullable*/);
 int hb_rbd_to_centroidal_batch_dev(hb_ctx* ctx, int B, const double* rbd, double* x);
 int hb_reference_expand_batch_dev(hb_ctx* ctx, int B, const double* t0, const hb_reference* refs, double* x_ref, double* swing_ref,
                                   int32_t* mode);
@@ -420,6 +471,9 @@ int hb_resident_plan_cycle_batch(hb_ctx* ctx, int B, int cold_start, double t_re
 int hb_estimator_update_batch(hb_ctx* ctx, int B, const hb_kf_params* params, double dt, hb_kf_state* state, const double* quat,
                               const double* ang_vel_local, const double* lin_acc_local, const double* joint_pos, const double* joint_vel,
                               const uint8_t* contact_flag, double* rbd_out);
+/* hb_sim_read_sensors_batch_dev with host pointers (est in/out) */
+int hb_sim_read_sensors(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, double accel_dt, const double* rbd, hb_estimation_state* est,
+                        double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos, double* joint_vel);
 int hb_contact_force_estimate_batch(hb_ctx* ctx, int B, double cutoff_frequency, double dt, hb_observer_state* state, const double* rbd,
                                     const double* tau_cmd, double* est_contact_force, double* disturbance_torque /*nullable*/);
 int hb_actuation_batch(hb_ctx* ctx, int B, double delay, const double* time, hb_actuation_state* state, const double* command, const double* rbd,
