@@ -363,8 +363,9 @@ int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
     attr((const void*)riccati_kernel, sizeof(RicShared));
     attr((const void*)forward_linesearch2_kernel, sizeof(Fw2Shared));
     attr((const void*)warm_shift_kernel, sizeof(double) * ((N + 1) * NX + N * NU));
-    // the one-block-per-instance kernels fit 8 blocks per SM only with the full shared-memory carveout; do not leave it to the driver
-    for (const void* fn : {(const void*)wbc_fused_kernel, (const void*)riccati_kernel})
+    // these kernels reach their blocks per SM (8 for the one-block-per-instance kernels, HB_LQ_MINB for lq_kernel) only with the full
+    // shared-memory carveout; do not leave it to the driver
+    for (const void* fn : {(const void*)wbc_fused_kernel, (const void*)riccati_kernel, (const void*)lq_kernel})
       if (fe == cudaSuccess) fe = cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
     if (fe != cudaSuccess) { ctx->last_cuda = (int)fe; hb_destroy(ctx); return HB_ECUDA; }
   }

@@ -412,7 +412,7 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned phas
       : "memory");
 }
 
-// Shared memory of the node LQ kernel (14.2 KB -> 14 CTAs per SM by shared memory). `rec` receives the linearisation record by one TMA bulk
+// Shared memory of the node LQ kernel (14 312 B: 15 CTAs per SM with the 1 KB per-block reserve). `rec` receives the linearisation record by one TMA bulk
 // copy; its regions are re-used as soon as they are dead:
 //   A1 (9x22)            -> Ad  : rows 3..11 of the discrete A                     (after the RK2 sensitivities)
 //   A2 (9x22)            -> BdF (9x12), Bdv (9x10): rows 3..11 of the discrete B
@@ -432,44 +432,32 @@ static_assert(LQ_BDV + 9 * NJ <= LIN_BF1, "discrete B must fit in the A2 region"
 static_assert(LQ_T + NJ * LQ_TL <= LIN_STRIDE && LQ_GV + 8 * NJ <= NJ * LQ_GL, "aliased areas overflow");
 static_assert((LQ_T % 2) == 0 && (sizeof(double) * LIN_STRIDE) % 16 == 0, "T is read with 128-bit loads");
 
-// One node of the LQ approximation. NSW = number of swing contacts (0 stance, 2 single support, 4 flight): 3 (4 - NSW) stance-force inputs,
-// 12 - 2 NSW contact-velocity rows, 2 NSW soft swing rows.
-//
-// Every quadratic term in the joint velocities v is reduced through the affine map v = T (dx, w, 1) of the projection:
-//   stage cost  1/2 v' Rb v + r_v' v        ->  T' Rb T  (blocks: Qt, Pt, Rt_nn and the vectors qt, rt_n)
-//   soft swing  1/2 w_s (h + gx' dx + gv' v)^2  ->  rank one in YZ_p = [gx_p | 0 | h_p] + gv_p' T
-// so the projected model is M = T' Rb T + w_s YZ' YZ evaluated once, lane = column, rows streamed from shared memory.
-template <int NSW>
-__device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst, int k, int lane, int mode, double xn_l, double xref_l) {
-  constexpr int MR = 12 - 2 * NSW, NP = 2 * NSW, NF = 3 * (4 - NSW), GL = LQ_GL, TL = LQ_TL;
-  const int N = a.N;
-  const double dt = sqp_dt(a, inst, k);
+// RK2 sensitivities (S2) and the stage cost (M2, M6, M8) of one node: the part of the LQ approximation that does not depend on the number
+// of swing contacts, so one copy of its code serves every lq_node<NSW>. Leaves the discrete A / B rows 3..11 in the record and q, Qd, r,
+// b, RFF, dvd in shared memory; returns this lane's share of the cost and the warp's squared dynamics defect.
+__device__ __forceinline__ void lq_model(LqShared& sh, int lane, unsigned flm, int nsw, double dt, double xn_l, double xref_l, double& cost_l, double& d2_w) {
   const Model& md = c_model;
   const double im = 1.0 / md.total_mass;
-  double* out = a.proj + ((size_t)inst * N + k) * PJ_STRIDE;
-  const unsigned flm = (contact_flag(mode, 0) ? 1u : 0u) | (contact_flag(mode, 1) ? 2u : 0u) | (contact_flag(mode, 2) ? 4u : 0u) | (contact_flag(mode, 3) ? 8u : 0u);
   const double* A1c = sh.rec + LIN_A1; const double* A2c = sh.rec + LIN_A2;
   const double* Bf1 = sh.rec + LIN_BF1; const double* Bf2 = sh.rec + LIN_BF2;
   const double* Bv1 = sh.rec + LIN_BV1; const double* Bv2 = sh.rec + LIN_BV2;
   const double* f1 = sh.rec + LIN_F1; const double* f2 = sh.rec + LIN_F2;
-  const double* epos = sh.rec + LIN_EPOS; const double* evel = sh.rec + LIN_EVEL;
-  const double* dpq = sh.rec + LIN_DPQ; const double* dvx = sh.rec + LIN_DVX; const double* dvv = sh.rec + LIN_DVV;
-  double* Ad = sh.rec + LQ_AD; double* BdF = sh.rec + LQ_BDF; double* Bdv = sh.rec + LQ_BDV; double* T = sh.rec + LQ_T;
-  double* G = sh.G; double* YZ = sh.G + LQ_YZ; double* GV = sh.G + LQ_GV;
-  // ---- RK2 sensitivities (S2) on the non-trivial rows 3..11, lane = column; results stay in registers until every lane has read A2
-  double ad[9], bd[9];
+  double* Ad = sh.rec + LQ_AD; double* BdF = sh.rec + LQ_BDF; double* Bdv = sh.rec + LQ_BDV;
+  // ---- RK2 sensitivities (S2) on the non-trivial rows 3..11, lane = column. Column j of A1 is read by lane j alone, so Ad replaces it
+  // at once; B stays in registers until every lane has read A2.
+  double bd[9];
   double d2 = 0.0;
   if (lane < NX) {
     const int j = lane;
     double c1[9];
 #pragma unroll
     for (int kk = 0; kk < 9; ++kk) c1[kk] = A1c[kk * NX + j];
-#pragma unroll
+#pragma unroll 1
     for (int i = 0; i < 9; ++i) {
       double s = 0.0;
 #pragma unroll
       for (int kk = 0; kk < 9; ++kk) s = fma(A2c[i * NX + 3 + kk], c1[kk], s);
-      ad[i] = 0.5 * dt * (c1[i] + A2c[i * NX + j] + dt * s) + ((3 + i == j) ? 1.0 : 0.0);
+      Ad[i * NX + j] = 0.5 * dt * (A1c[i * NX + j] + A2c[i * NX + j] + dt * s) + ((3 + i == j) ? 1.0 : 0.0);
     }
     if (j < 12) {
       // B1 force column j = [e_a / m ; Bf1[:, j] ; 0]: (A2 B1)[i][j] = A2c[i][a] / m + A2c[i][3:6] Bf1[:, j]
@@ -499,11 +487,9 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
     sh.b[lane] = bb; d2 = bb * bb;
   }
   d2 = warp_sum(d2);
-  __syncwarp();          // every lane has read A1 / A2: their storage takes the discrete model
+  __syncwarp();          // every lane has read A2: its storage takes the discrete B
   if (lane < NX) {
     const int j = lane;
-#pragma unroll
-    for (int i = 0; i < 9; ++i) Ad[i * NX + j] = ad[i];
     if (j < 12) {
 #pragma unroll
       for (int i = 0; i < 9; ++i) BdF[i * 12 + j] = bd[i];
@@ -514,7 +500,7 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
   }
   // ---- cost (M2, M6, M8), scaled by dt at the end
   const double* __restrict__ ltab = g_lq_lane + lane * LQ_LANE_TAB;     // this lane's constants (global memory: see hb_common.cuh)
-  const double fz = (NSW < 4) ? md.total_mass * HB_GRAVITY / (4 - NSW) : 0.0;
+  const double fz = (nsw < 4) ? md.total_mass * HB_GRAVITY / (4 - nsw) : 0.0;
   double cost = 0.0;
   if (lane < NX) {
     const double d = sh.x[lane] - xref_l;
@@ -584,6 +570,27 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
   if (lane < NX) sh.Qd[lane] += shiftsum;
   if (lane < 12) sh.RFF[(lane / 3) * 9 + (lane % 3) * 4] += shiftsum;
   else if (lane >= 16 && lane < 16 + NJ) sh.dvd[lane - 16] += shiftsum;
+  cost_l = cost; d2_w = d2;
+}
+
+// One node of the LQ approximation. NSW = number of swing contacts (0 stance, 2 single support, 4 flight): 3 (4 - NSW) stance-force inputs,
+// 12 - 2 NSW contact-velocity rows, 2 NSW soft swing rows.
+//
+// Every quadratic term in the joint velocities v is reduced through the affine map v = T (dx, w, 1) of the projection:
+//   stage cost  1/2 v' Rb v + r_v' v        ->  T' Rb T  (blocks: Qt, Pt, Rt_nn and the vectors qt, rt_n)
+//   soft swing  1/2 w_s (h + gx' dx + gv' v)^2  ->  rank one in YZ_p = [gx_p | 0 | h_p] + gv_p' T
+// so the projected model is M = T' Rb T + w_s YZ' YZ evaluated once, lane = column, rows streamed from shared memory.
+template <int NSW>
+__device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst, int k, int lane, unsigned flm, double dt, double cost, double d2) {
+  constexpr int MR = 12 - 2 * NSW, NP = 2 * NSW, NF = 3 * (4 - NSW), GL = LQ_GL, TL = LQ_TL;
+  const int N = a.N;
+  const Model& md = c_model;
+  const double im = 1.0 / md.total_mass;
+  double* out = a.proj + ((size_t)inst * N + k) * PJ_STRIDE;
+  const double* epos = sh.rec + LIN_EPOS; const double* evel = sh.rec + LIN_EVEL;
+  const double* dpq = sh.rec + LIN_DPQ; const double* dvx = sh.rec + LIN_DVX; const double* dvv = sh.rec + LIN_DVV;
+  double* Ad = sh.rec + LQ_AD; double* BdF = sh.rec + LQ_BDF; double* Bdv = sh.rec + LQ_BDV; double* T = sh.rec + LQ_T;
+  double* G = sh.G; double* YZ = sh.G + LQ_YZ; double* GV = sh.G + LQ_GV;
   // ---- contact-velocity equality rows (M4, M5); swing forces handled separately (M3). Row r -> contact-kinematics row rowi[r] = 3c + axis.
   if (lane == 0) {
     int mr = 0;
@@ -625,7 +632,7 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
       }
       xr[r] = v;
     }
-#pragma unroll
+#pragma unroll 1
     for (int i = 0; i < NJ; ++i) {
       double s = 0.0;
 #pragma unroll
@@ -725,17 +732,24 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
   __syncwarp();       // every read of the contact-kinematics part of the record is done: T takes its place
 #pragma unroll
   for (int i = 0; i < NJ; ++i) T[i * TL + lane] = tc[i];
+  const double* tl = T + lane;      // column `lane` of T from here on: read back where it is used rather than held in registers
   double wyz[NP > 0 ? NP : 1];
   if (NP > 0) {
     if (lane < NP) { const double g = YZ[lane * TL + 30]; cost += 0.5 * HB_SOFT_SWING_WEIGHT * g * g; }
     __syncwarp();       // the unreduced h_p are read before lane 30 replaces them
+    double yz[NP > 0 ? NP : 1];
+#pragma unroll
+    for (int p = 0; p < NP; ++p) yz[p] = YZ[p * TL + lane];
+#pragma unroll 1
+    for (int kk = 0; kk < NJ; ++kk) {
+      const double t = tl[kk * TL];
+#pragma unroll
+      for (int p = 0; p < NP; ++p) yz[p] = fma(GV[p * NJ + kk], t, yz[p]);
+    }
 #pragma unroll
     for (int p = 0; p < NP; ++p) {
-      double s = YZ[p * TL + lane];
-#pragma unroll
-      for (int kk = 0; kk < NJ; ++kk) s = fma(GV[p * NJ + kk], tc[kk], s);
-      wyz[p] = HB_SOFT_SWING_WEIGHT * s;
-      YZ[p * TL + lane] = s;
+      wyz[p] = HB_SOFT_SWING_WEIGHT * yz[p];
+      YZ[p * TL + lane] = yz[p];
     }
   }
   cost = warp_sum(cost);
@@ -743,12 +757,13 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
   double rb[NJ];
   double lin = 0.0;
 #pragma unroll
-  for (int i = 0; i < NJ; ++i) {
-    double s = sh.dvd[i] * tc[i];
+  for (int i = 0; i < NJ; ++i) rb[i] = sh.dvd[i] * tl[i * TL];
+#pragma unroll 1
+  for (int kk = 0; kk < NJ; ++kk) {
+    const double t = tl[kk * TL];
 #pragma unroll
-    for (int kk = 0; kk < NJ; ++kk) s = fma(md.R[(12 + i) * NU + 12 + kk], tc[kk], s);
-    rb[i] = s;
-    lin = fma(sh.r[12 + i], tc[i], lin);
+    for (int i = 0; i < NJ; ++i) rb[i] = fma(md.R[(12 + i) * NU + 12 + kk], t, rb[i]);
+    lin = fma(sh.r[12 + kk], t, lin);
   }
   __syncwarp();
   // ---- M = T' Rb T + YZ' (w YZ), row by row (rows come in pairs with 128-bit broadcast loads); lane = column:
@@ -765,7 +780,7 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
       else if (nlane) out[PJ_RV + NF + cc] = dt * (s + lin);
     }
   };
-#pragma unroll
+#pragma unroll 1
   for (int i = 0; i < 30; i += 2) {
     double s0 = 0.0, s1 = 0.0;
 #pragma unroll
@@ -791,17 +806,18 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
   // ---- dynamics through T: Bdv T (rows 3..11) -> At (lanes 0..21, + Ad), Bt null columns (lanes 22..29), bt (lane 30); rows 12..21 are dt T
   double at9[9];
 #pragma unroll
-  for (int i = 0; i < 9; ++i) {
-    double s = (lane < NX) ? Ad[i * NX + lane] : 0.0;
+  for (int i = 0; i < 9; ++i) at9[i] = (lane < NX) ? Ad[i * NX + lane] : 0.0;
+#pragma unroll 1
+  for (int kk = 0; kk < NJ; ++kk) {
+    const double t = tl[kk * TL];
 #pragma unroll
-    for (int kk = 0; kk < NJ; ++kk) s = fma(Bdv[i * NJ + kk], tc[kk], s);
-    at9[i] = s;
+    for (int i = 0; i < 9; ++i) at9[i] = fma(Bdv[i * NJ + kk], t, at9[i]);
   }
   if (lane == 30) {
 #pragma unroll
     for (int i = 0; i < 9; ++i) sh.b[3 + i] += at9[i];
 #pragma unroll
-    for (int kk = 0; kk < NJ; ++kk) sh.b[12 + kk] += dt * tc[kk];
+    for (int kk = 0; kk < NJ; ++kk) sh.b[12 + kk] += dt * tl[kk * TL];
   }
   // role of the lane in the input-column writes: lanes 0..15 own the stance-force columns c < NF and the padded columns c >= nt,
   // lanes 22..29 own the null-space columns NF + cc
@@ -820,15 +836,15 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
 #pragma unroll
     for (int i = 0; i < 9; ++i) out[PJ_AT + (3 + i) * NX + lane] = at9[i];
 #pragma unroll
-    for (int i = 0; i < NJ; ++i) out[PJ_AT + (12 + i) * NX + lane] = ((12 + i == lane) ? 1.0 : 0.0) + dt * tc[i];
+    for (int i = 0; i < NJ; ++i) out[PJ_AT + (12 + i) * NX + lane] = ((12 + i == lane) ? 1.0 : 0.0) + dt * tl[i * TL];
 #pragma unroll
-    for (int i = 0; i < NJ; ++i) out[PJ_PXV + i * NX + lane] = tc[i];
+    for (int i = 0; i < NJ; ++i) out[PJ_PXV + i * NX + lane] = tl[i * TL];
   } else if (cc >= 0 && cc < NVMAX) {
 #pragma unroll
-    for (int i = 0; i < NJ; ++i) out[PJ_NV + i * NVMAX + cc] = nlane ? tc[i] : 0.0;
+    for (int i = 0; i < NJ; ++i) out[PJ_NV + i * NVMAX + cc] = nlane ? tl[i * TL] : 0.0;
   } else if (lane == 30) {
 #pragma unroll
-    for (int i = 0; i < NJ; ++i) out[PJ_PEV + i] = tc[i];
+    for (int i = 0; i < NJ; ++i) out[PJ_PEV + i] = tl[i * TL];
   }
   if (wcol) {
     const int sa = sj % 3;
@@ -837,7 +853,7 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
 #pragma unroll
     for (int i = 0; i < 9; ++i) out[PJ_BT + (3 + i) * NTMAX + col] = fcol ? BdF[i * 12 + sj] : (nlane ? at9[i] : 0.0);
 #pragma unroll
-    for (int i = 0; i < NJ; ++i) out[PJ_BT + (12 + i) * NTMAX + col] = nlane ? dt * tc[i] : 0.0;
+    for (int i = 0; i < NJ; ++i) out[PJ_BT + (12 + i) * NTMAX + col] = nlane ? dt * tl[i * TL] : 0.0;
     if (!nlane) {
 #pragma unroll
       for (int i = 0; i < NX; ++i) out[PJ_PT + col * NX + i] = 0.0;
@@ -881,11 +897,15 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
   if (lane == 0) { out[PJ_META] = nt; out[PJ_META + 1] = NF; out[PJ_META + 2] = nv; out[PJ_META + 3] = dt * cost; out[PJ_META + 4] = dt * d2; out[PJ_META + 5] = dt * e2; out[PJ_META + 6] = overflow ? 1.0 : 0.0; out[PJ_META + 7] = dt; }
 }
 
-// Minimum resident warps per SM. 8 lets ptxas keep the kernel in 232 registers without spills; on H100 that beats 12 warps at 168
-// registers with ~650 B of spill traffic per lane (K1 2.88 vs 3.97 ms per 1024-instance step) and 14 warps at 128 registers (4.07 ms).
+// Minimum resident warps per SM: 15 is what shared memory allows, with the full carveout hb_create requests. A warp lives on one of the
+// SM's four 16 K-register sub-partitions, so 13..16 warps cap a thread at 128 registers; the kernel fits in that without spills because
+// Ad and the column of T go to shared memory instead of waiting in registers. The extra warps pay only with compact code, since warps
+// out of phase each stream it through the instruction cache: hence lq_model as one copy and the rolled inner-product loops. On H100
+// (configs[1]) K1 takes 1.74 ms per step, against 2.88 ms at 8 warps and 3.04 ms at 15 warps with every loop unrolled.
 #ifndef HB_LQ_MINB
-#define HB_LQ_MINB 8
+#define HB_LQ_MINB 15
 #endif
+static_assert(HB_LQ_MINB * (sizeof(LqShared) + 1024) <= 228 * 1024, "lq_kernel must fit HB_LQ_MINB blocks per SM");
 __global__ void __launch_bounds__(32, HB_LQ_MINB) lq_kernel(SqpArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   LqShared& sh = *reinterpret_cast<LqShared*>(smem_raw);
@@ -914,9 +934,13 @@ __global__ void __launch_bounds__(32, HB_LQ_MINB) lq_kernel(SqpArgs a) {
 #pragma unroll
   for (int c = 0; c < 4; ++c) nsw += contact_flag(mode, c) ? 0 : 1;
   mbar_wait(&sh.bar, 0);
-  if (nsw == 2) lq_node<2>(sh, a, inst, k, lane, mode, xn_l, xref_l);
-  else if (nsw == 0) lq_node<0>(sh, a, inst, k, lane, mode, xn_l, xref_l);
-  else lq_node<4>(sh, a, inst, k, lane, mode, xn_l, xref_l);
+  const double dt = sqp_dt(a, inst, k);
+  const unsigned flm = (contact_flag(mode, 0) ? 1u : 0u) | (contact_flag(mode, 1) ? 2u : 0u) | (contact_flag(mode, 2) ? 4u : 0u) | (contact_flag(mode, 3) ? 8u : 0u);
+  double cost, d2;
+  lq_model(sh, lane, flm, nsw, dt, xn_l, xref_l, cost, d2);
+  if (nsw == 2) lq_node<2>(sh, a, inst, k, lane, flm, dt, cost, d2);
+  else if (nsw == 0) lq_node<0>(sh, a, inst, k, lane, flm, dt, cost, d2);
+  else lq_node<4>(sh, a, inst, k, lane, flm, dt, cost, d2);
 }
 
 // ---------------------------------------------------------------- K2: value-function recursion
