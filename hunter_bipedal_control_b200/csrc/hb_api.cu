@@ -116,6 +116,47 @@ int launch(hb_ctx* ctx, int kind, void (*kernel)(P...), dim3 grid, dim3 block, s
 
 int set_device(hb_ctx* ctx) { return cudaSetDevice(ctx->device) == cudaSuccess ? HB_OK : HB_ECUDA; }
 
+// The checks an entry point that takes (ctx, B) opens with, in this order: the context, B >= 0 and `args` (its required pointers and the
+// scalars it checks up front) -> HB_EINVAL; an empty batch -> EMPTY; with CAPPED, instances beyond the context's capacity -> HB_ECAP;
+// host_ok() (host data the call reads, the resident solution it needs) -> HB_EINVAL; then the switch to the context's device. The
+// capacity test counts ctx->base: 0 outside a chunked call, and inside one the offset of the chunk's instances in the per-instance scratch.
+enum Cap : bool { UNCAPPED = false, CAPPED = true };
+constexpr int EMPTY = 1;
+inline bool no_host_check() { return true; }
+template <class F = bool (*)()> int enter(hb_ctx* ctx, int B, bool args, Cap cap, const F& host_ok = no_host_check) {
+  if (!ctx || B < 0 || !args) return HB_EINVAL;
+  if (B == 0) return EMPTY;
+  if (cap && ctx->base + B > ctx->cfg.max_batch) return HB_ECAP;
+  if (!host_ok()) return HB_EINVAL;
+  return set_device(ctx);
+}
+// returns from the entry point unless enter() passed, with HB_OK for an empty batch (EMPTY never crosses the ABI)
+#define ENTER(...)                                                   \
+  do {                                                               \
+    const int rc__ = enter(__VA_ARGS__);                             \
+    if (rc__) return rc__ == EMPTY ? HB_OK : rc__;                   \
+  } while (0)
+
+// The validity of each kind of scalar parameter, shared by every entry point that takes it (NaN fails every test)
+bool sim_params_ok(const hb_sim_params& p) { return p.dt > 0.0 && p.substeps >= 1 && p.substeps <= 1000; }
+bool delay_ok(double delay) { return delay >= 0.0; }
+bool cutoff_ok(double cutoff_frequency, double dt) { return cutoff_frequency > 0.0 && dt > 0.0; }
+bool qp_shape_ok(int n, int m) { return n >= 1 && n <= QP_MAX_N && m >= 0 && m <= QP_MAX_M; }
+bool sensor_noise_ok(const hb_sensor_noise& n) {
+  for (double s : {n.orientation, n.angular_velocity, n.linear_acceleration, n.joint_position, n.joint_velocity})
+    if (!(s >= 0.0) || !isfinite(s)) return false;
+  return true;
+}
+
+// Waits for both streams of the context and returns rc, or the first failed wait when rc is HB_OK. Every host-pointer call ends here
+// once it has queued a copy, on every exit: no copy is left reading or writing the caller's buffers, or the arena the next call may free.
+int drain(hb_ctx* ctx, int rc) {
+  const cudaError_t e1 = cudaStreamSynchronize(ctx->stream_aux), e0 = cudaStreamSynchronize(ctx->stream_main);
+  if (rc) return rc;
+  if (e0 != cudaSuccess || e1 != cudaSuccess) { ctx->last_cuda = (int)(e0 != cudaSuccess ? e0 : e1); return HB_ECUDA; }
+  return HB_OK;
+}
+
 // The growth policy of the context's on-demand buffers (the staging arena, the pinned host buffer): grow only, to 5/4 of the request so
 // that a packed reference stream a little longer than the last one does not reallocate, contents not kept. Every host-pointer call waits
 // for its copies before it returns, so no copy still reads the buffer that is freed.
@@ -157,9 +198,12 @@ template <class T> struct Dev {
   T* at(size_t i) const { return static_cast<T*>(*p) + i * per; }
 };
 
-// Staging of one host-pointer call. The call declares its host arguments with their elements per instance; reserve() then places all of
-// them in the context's device arena (grown on demand, freed by hb_destroy) before any copy is enqueued, and h2d / d2h copy instances
-// [lo, hi) of every argument on ctx->stream. Slices start on 256-byte boundaries, as separate cudaMalloc's would.
+// Instances [lo, hi) of a staged call, its chunk c
+struct Chunk { int c; size_t lo, hi; int n; };
+
+// Staging of one host-pointer call. The call declares its host arguments with their elements per instance; run() then places all of
+// them in the context's device arena (grown on demand, freed by hb_destroy) before any copy is enqueued. Slices start on 256-byte
+// boundaries, as separate cudaMalloc's would.
 //   in / inout   copied in (inout: and back)
 //   out          the device always gets a buffer; copied back only when the caller passed a host pointer
 //   *_or_null    a null host pointer stays a null device pointer
@@ -175,24 +219,25 @@ class Staging {
   template <class T> Dev<T> tmp(size_t per) { return add<T>(nullptr, nullptr, per, B_, true); }
   template <class T> Dev<T> buf(size_t n) { Dev<T> d = add<T>(nullptr, nullptr, n, 1, true); d.per = 1; return d; }
 
-  int reserve() {
-    const int rc = grow(ctx_, &ctx_->arena, &ctx_->arena_cap, place(nullptr), false);
+  // Places the arguments, then runs the call in nchunk chunks: chunk c covers instances [B c / nchunk, B (c + 1) / nchunk) on
+  // stream_main (even c) or stream_aux (odd c), so the copies of one chunk overlap the kernels of the other. Per chunk: copy in, body(k)
+  // with ctx->stream / ctx->base pointing at the chunk, copy out. The first error ends the loop; ctx->stream / ctx->base are restored and
+  // both streams drained before it is returned. One chunk is the whole batch on stream_main.
+  template <class F> int run(int nchunk, F&& body) {
+    int rc = grow(ctx_, &ctx_->arena, &ctx_->arena_cap, place(nullptr), false);
     if (rc) return rc;
     place(ctx_->arena);
-    return HB_OK;
-  }
-  int h2d(size_t lo, size_t hi) { return copy(lo, hi, true); }
-  int d2h(size_t lo, size_t hi) { return copy(lo, hi, false); }
-  // the whole batch in one piece: reserve, copy in, call(), copy out, wait
-  template <class F> int run(F&& call) {
-    int rc = reserve();
-    if (!rc) rc = h2d(0, B_);
-    if (!rc) rc = call();
-    if (!rc) rc = d2h(0, B_);
-    if (rc) return rc;
-    hb_ctx* ctx = ctx_;
-    CK(cudaStreamSynchronize(ctx->stream));
-    return HB_OK;
+    for (int c = 0; c < nchunk && rc == HB_OK; ++c) {
+      const size_t lo = B_ * c / nchunk, hi = B_ * (c + 1) / nchunk;
+      ctx_->stream = (c % 2 == 0) ? ctx_->stream_main : ctx_->stream_aux;
+      ctx_->base = (int)lo;
+      rc = copy(lo, hi, true);
+      if (!rc) rc = body(Chunk{c, lo, hi, (int)(hi - lo)});
+      if (!rc) rc = copy(lo, hi, false);
+    }
+    ctx_->stream = ctx_->stream_main;
+    ctx_->base = 0;
+    return drain(ctx_, rc);
   }
 
  private:
@@ -223,25 +268,6 @@ class Staging {
   Slot s_[16];   // the largest call (hb_resident_plan_cycle_batch) declares 11
   int n_ = 0;
 };
-
-// The pipelined host-pointer calls: chunk c of nchunk covers instances [B c / nchunk, B (c + 1) / nchunk) on stream_main (even c) or
-// stream_aux (odd c), so the copies of one chunk overlap the kernels of the other. ctx->stream / ctx->base point at the chunk while
-// body(c, lo, hi) runs and are restored after the last one; both streams are drained before the first error is returned.
-template <class F> int chunked(hb_ctx* ctx, int B, int nchunk, F&& body) {
-  int rc = HB_OK;
-  for (int c = 0; c < nchunk && rc == HB_OK; ++c) {
-    const size_t lo = (size_t)B * c / nchunk, hi = (size_t)B * (c + 1) / nchunk;
-    ctx->stream = (c % 2 == 0) ? ctx->stream_main : ctx->stream_aux;
-    ctx->base = (int)lo;
-    rc = body(c, lo, hi);
-  }
-  ctx->stream = ctx->stream_main;
-  ctx->base = 0;
-  cudaError_t e1 = cudaStreamSynchronize(ctx->stream_aux), e0 = cudaStreamSynchronize(ctx->stream_main);
-  if (rc) return rc;
-  if (e0 != cudaSuccess || e1 != cudaSuccess) { ctx->last_cuda = (int)(e0 != cudaSuccess ? e0 : e1); return HB_ECUDA; }
-  return HB_OK;
-}
 
 // chunk count of the host-pointer cycles: cfg.e2e_chunks when set (one chunk below 64 instances per chunk), otherwise two from 4096
 // instances on when the call has host work and copies to hide behind the other chunk's kernels (`overlap`)
@@ -432,7 +458,7 @@ void* hb_stream(hb_ctx* ctx) { return ctx ? (void*)ctx->stream : nullptr; }
 // ------------------------------------------------------------------------------------------ device-pointer entry points
 static int launch_qp(hb_ctx* ctx, int B, int n, int m, const double* H, const double* g, const double* A, const double* lbA, const double* ubA,
                      size_t sH, size_t sA, size_t sB, const int32_t* m_per, double* x, int32_t* status, int32_t* iters) {
-  if (n < 1 || n > QP_MAX_N || m < 0 || m > QP_MAX_M) return HB_EINVAL;
+  if (!qp_shape_ok(n, m)) return HB_EINVAL;
   const size_t per_warp = qp_workspace_doubles(n) * sizeof(double);
   int wpb = (int)((200 * 1024) / per_warp);
   if (wpb < 1) return HB_EINVAL;
@@ -444,27 +470,20 @@ static int launch_qp(hb_ctx* ctx, int B, int n, int m, const double* H, const do
 
 int hb_wbc_qp_batch_dev(hb_ctx* ctx, int B, int n, int m, const double* H, const double* g, const double* A, const double* lbA,
                         const double* ubA, double* x, int32_t* status, int32_t* iters) {
-  if (!ctx || B < 0 || !H || !g || !A || !lbA || !ubA || !x) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, H && g && A && lbA && ubA && x, UNCAPPED);
   return launch_qp(ctx, B, n, m, H, g, A, lbA, ubA, (size_t)n * n, (size_t)m * n, (size_t)m, nullptr, x, status, iters);
 }
 
 int hb_wbc_solve_batch_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
                            const uint8_t* stance_mode, double* sol, int32_t* status) {
-  if (!ctx || B < 0 || !x_des || !u_des || !rbd || !mode || !sol) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x_des && u_des && rbd && mode && sol, CAPPED);
   return launch(ctx, K_QP, wbc_fused_kernel, B, 32, wbc_fused_doubles() * sizeof(double), B, ctx->wbc, x_des, u_des, rbd, mode, stance_mode,
                 ctx->cfg.wbc_rho, ctx->cfg.qp_max_iter, sol, status ? status : ctx->wstatus + ctx->base, ctx->witers + ctx->base);
 }
 
 int hb_wbc_assemble_batch_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
                               const uint8_t* stance_mode, double* H, double* g, double* A, double* lbA, double* ubA, int32_t* m_rows) {
-  if (!ctx || B < 0 || !x_des || !u_des || !rbd || !mode || !H || !g || !A || !lbA || !ubA || !m_rows) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x_des && u_des && rbd && mode && H && g && A && lbA && ubA && m_rows, UNCAPPED);
   const int wpb = 4;
   return launch(ctx, K_WBC_ASSEMBLE, wbc_assemble_kernel, (B + wpb - 1) / wpb, 32 * wpb, sizeof(WbcShared) * wpb, B, ctx->wbc, x_des, u_des, rbd, mode,
                 stance_mode, H, g, A, lbA, ubA, m_rows);
@@ -472,9 +491,7 @@ int hb_wbc_assemble_batch_dev(hb_ctx* ctx, int B, const double* x_des, const dou
 
 int hb_wbc_qp_rows_batch_dev(hb_ctx* ctx, int B, int n, int m_alloc, const int32_t* m_rows, const double* H, const double* g, const double* A,
                              const double* lbA, const double* ubA, double* x, int32_t* status, int32_t* iters) {
-  if (!ctx || B < 0 || !m_rows || !H || !g || !A || !lbA || !ubA || !x) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, m_rows && H && g && A && lbA && ubA && x, UNCAPPED);
   return launch_qp(ctx, B, n, m_alloc, H, g, A, lbA, ubA, (size_t)n * n, (size_t)m_alloc * n, (size_t)m_alloc, m_rows, x, status, iters);
 }
 
@@ -488,10 +505,7 @@ static int hoqp_reserve(hb_ctx* ctx) {
 }
 
 int hb_hoqp_solve_batch_dev(hb_ctx* ctx, int B, const hb_hoqp_problem* problems, double* x, double* slack, int32_t* status) {
-  if (!ctx || B < 0 || !problems || !x) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, problems && x, CAPPED);
   const int rc = hoqp_reserve(ctx);
   if (rc) return rc;
   return launch(ctx, K_QP, hoqp_kernel, B, 32, hoqp_smem_bytes(), B, problems, ctx->hoqp_scratch, 2 * ctx->cfg.qp_max_iter, x, slack, status);
@@ -503,10 +517,7 @@ static int hwbc_tasks_dev(hb_ctx* ctx, int B, const double* x_des, const double*
 
 int hb_hierarchical_wbc_solve_batch_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, double* sol,
                                         int32_t* status) {
-  if (!ctx || B < 0 || !x_des || !u_des || !rbd || !mode || !sol) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x_des && u_des && rbd && mode && sol, CAPPED);
   int rc = hoqp_reserve(ctx);
   if (rc) return rc;
   rc = hwbc_tasks_dev(ctx, B, x_des, u_des, rbd, mode, ctx->hoqp_prob);
@@ -515,18 +526,13 @@ int hb_hierarchical_wbc_solve_batch_dev(hb_ctx* ctx, int B, const double* x_des,
 }
 
 int hb_mpc_cold_start_batch_dev(hb_ctx* ctx, int B, const double* x0, const int32_t* mode, double* x_traj, double* u_traj) {
-  if (!ctx || B < 0 || !x0 || !mode || !x_traj || !u_traj) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x0 && mode && x_traj && u_traj, UNCAPPED);
   return launch(ctx, K_UNPROFILED, cold_start_kernel, B, 128, 0, B, ctx->cfg.horizon_N, x0, mode, x_traj, u_traj);
 }
 
 static int mpc_solve_impl(hb_ctx* ctx, int B, const double* x0, const double* x_ref, const double* swing_ref, const int32_t* mode,
                           double* x_traj, double* u_traj, hb_solve_info* info, const double* tk, const int32_t* nn) {
-  if (!ctx || B < 0 || !x0 || !x_ref || !swing_ref || !mode || !x_traj || !u_traj || ((tk == nullptr) != (nn == nullptr))) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x0 && x_ref && swing_ref && mode && x_traj && u_traj && (tk == nullptr) == (nn == nullptr), CAPPED);
   const size_t Bc = ctx->cfg.max_batch, Nc = ctx->cfg.horizon_N;
   int rc = reserve_group(&ctx->sqp_mem, [&](void* m) {
     size_t off = 0;
@@ -565,9 +571,7 @@ int hb_mpc_solve_grid_batch_dev(hb_ctx* ctx, int B, const double* x0, const doub
 
 static int policy_eval_impl(hb_ctx* ctx, int B, double t_rel, const double* x_traj, const double* u_traj, const int32_t* mode, double* x_des,
                             double* u_des, int32_t* mode_out, const double* tk, const int32_t* nn) {
-  if (!ctx || B < 0 || !x_traj || !u_traj || !mode || !x_des || !u_des || ((tk == nullptr) != (nn == nullptr))) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x_traj && u_traj && mode && x_des && u_des && (tk == nullptr) == (nn == nullptr), UNCAPPED);
   const int wpb = 4;
   return launch(ctx, K_UNPROFILED, policy_eval_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, ctx->cfg.horizon_N, ctx->cfg.dt, t_rel, x_traj, u_traj, mode,
                 x_des, u_des, mode_out, tk, nn, nullptr, nullptr);
@@ -585,9 +589,7 @@ int hb_policy_eval_grid_batch_dev(hb_ctx* ctx, int B, double t_rel, const double
 }
 
 int hb_time_grid_batch_dev(hb_ctx* ctx, int B, const double* t0, const hb_reference* refs, double* node_times, int32_t* n_intervals, int32_t* status) {
-  if (!ctx || B < 0 || !t0 || !refs || !node_times || !n_intervals) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, t0 && refs && node_times && n_intervals, UNCAPPED);
   const double T = ctx->cfg.time_horizon > 0.0 ? ctx->cfg.time_horizon : ctx->cfg.horizon_N * ctx->cfg.dt;
   return launch(ctx, K_UNPROFILED, time_grid_kernel, (B + 127) / 128, 128, 0, B, ctx->cfg.horizon_N, ctx->cfg.dt, T, t0, refs, node_times, n_intervals, status);
 }
@@ -595,10 +597,9 @@ int hb_time_grid_batch_dev(hb_ctx* ctx, int B, const double* t0, const hb_refere
 static int control_step_impl(hb_ctx* ctx, int B, double t_rel, const double* x0, const double* x_ref, const double* swing_ref, const int32_t* mode,
                              const double* rbd, double* x_traj, double* u_traj, hb_solve_info* info, double* wbc_sol, double* torque,
                              int32_t* wbc_status, const double* tk, const int32_t* nn) {
-  if (!ctx || !rbd || !wbc_sol) return HB_EINVAL;
+  ENTER(ctx, B, x0 && x_ref && swing_ref && mode && rbd && x_traj && u_traj && wbc_sol && (tk == nullptr) == (nn == nullptr), CAPPED);
   int rc = mpc_solve_impl(ctx, B, x0, x_ref, swing_ref, mode, x_traj, u_traj, info, tk, nn);
   if (rc) return rc;
-  if (B == 0) return HB_OK;
   double* xdes = ctx->xdes + (size_t)ctx->base * NX; double* udes = ctx->udes + (size_t)ctx->base * NU; int32_t* wmode = ctx->wmode + ctx->base;
   rc = policy_eval_impl(ctx, B, t_rel, x_traj, u_traj, mode, xdes, udes, wmode, tk, nn);
   if (rc) return rc;
@@ -629,11 +630,7 @@ static int wbc_fallback(hb_ctx* ctx, int B, bool no_prev, const int32_t* wbc_sta
 // same time is the WBC of that cycle, so the cycle's own would be thrown away)
 static int resident_cycle_impl(hb_ctx* ctx, int B, int cold_start, double t_rel, const double* t0, const double* x0, const hb_reference* refs,
                                const double* rbd, hb_solve_info* info, double* wbc_sol, double* torque, int32_t* wbc_status, bool run_wbc) {
-  if (!ctx || B < 0 || !t0 || !x0 || !refs || !rbd) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (ctx->base + B > ctx->cfg.max_batch) return HB_ECAP;
-  if (!cold_start && ctx->res_valid < ctx->base + B) return HB_EINVAL;     // no previous solution to shift
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, t0 && x0 && refs && rbd, CAPPED, [&] { return cold_start || ctx->res_valid >= ctx->base + B; });   // a warm start shifts the previous solution
   const size_t N = ctx->cfg.horizon_N, o = (size_t)ctx->base;
   double* xref = ctx->cyc_xref + o * (N + 1) * NX; double* swing = ctx->cyc_swing + o * (N + 1) * 24; int32_t* mode = ctx->cyc_mode + o * (N + 1);
   double* xt = ctx->res_xt + o * (N + 1) * NX; double* ut = ctx->res_ut + o * N * NU; double* tres = ctx->res_t0 + o;
@@ -673,9 +670,7 @@ int hb_resident_cycle_batch_dev(hb_ctx* ctx, int B, int cold_start, double t_rel
 
 int hb_plan_references_batch_dev(hb_ctx* ctx, int B, const hb_plan_input* in, const double* feet, double* latest_stance, hb_reference* out,
                                  int32_t* status) {
-  if (!ctx || B < 0 || !in || !latest_stance || !out) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, in && latest_stance && out, UNCAPPED);
   static const hbplan::PlanConsts pc = hbplan::make_consts();
   return launch(ctx, K_UNPROFILED, plan_references_coop_kernel, (B + 7) / 8, 32, 0, B, in, feet, latest_stance, out, status, pc);
 }
@@ -699,9 +694,7 @@ int hb_kf_reset(int B, hb_kf_state* state) {
 int hb_estimator_update_batch_dev(hb_ctx* ctx, int B, const hb_kf_params* params, double dt, hb_kf_state* state, const double* quat,
                                   const double* ang_vel_local, const double* lin_acc_local, const double* joint_pos, const double* joint_vel,
                                   const uint8_t* contact_flag, double* rbd_out) {
-  if (!ctx || B < 0 || !params || !state || !quat || !ang_vel_local || !lin_acc_local || !joint_pos || !joint_vel || !contact_flag || !rbd_out) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, params && state && quat && ang_vel_local && lin_acc_local && joint_pos && joint_vel && contact_flag && rbd_out, UNCAPPED);
   return launch(ctx, K_UNPROFILED, kf_update_kernel<hb_kf_state>, B, 32, sizeof(KfShared), B, *params, dt, state, quat, ang_vel_local, lin_acc_local,
                 joint_pos, joint_vel, contact_flag, rbd_out);
 }
@@ -851,26 +844,20 @@ int hb_actuation_reset(int B, hb_actuation_state* state) {
 
 int hb_actuation_batch_dev(hb_ctx* ctx, int B, double delay, const double* time, hb_actuation_state* state, const double* command, const double* rbd,
                            double* tau) {
-  if (!ctx || B < 0 || !time || !state || !command || !rbd || !tau || delay < 0.0) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, time && state && command && rbd && tau && delay_ok(delay), UNCAPPED);
   return launch(ctx, K_UNPROFILED, actuation_kernel, (B + 63) / 64, 64, 0, B, delay, time, state, command, rbd, tau);
 }
 
 int hb_sim_step_batch_dev(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {
-  if (!ctx || B < 0 || !params || !rbd || !tau || !(params->dt > 0.0) || params->substeps < 1 || params->substeps > 1000) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, params && rbd && tau && sim_params_ok(*params), UNCAPPED);
   return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, *params, rbd, tau, contact_force, contact_flag);
 }
 
 // hb_resident_wbc_batch_dev; no_prev = true: the fallback has no previous solution yet (first tick after a cold start whose cycle ran no WBC)
 static int resident_wbc_impl(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
                              int32_t* mode_out, double* wbc_sol, double* torque, int32_t* wbc_status, bool no_prev) {
-  if (!ctx || B < 0 || !t_now || !rbd || !x_des || !u_des || !mode_out || !wbc_sol) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (ctx->base + B > ctx->res_valid) return HB_EINVAL;             // no resident solution to evaluate
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, t_now && rbd && x_des && u_des && mode_out && wbc_sol, UNCAPPED,
+        [&] { return ctx->base + B <= ctx->res_valid; });             // a resident solution to evaluate
   const size_t N = ctx->cfg.horizon_N, o = (size_t)ctx->base;
   const bool grid = ctx->cfg.event_nodes != 0;
   const int wpb = 4;
@@ -923,12 +910,6 @@ static int estimation_reserve(hb_ctx* ctx) {
   });
 }
 
-static bool sensor_noise_ok(const hb_sensor_noise& n) {
-  for (double s : {n.orientation, n.angular_velocity, n.linear_acceleration, n.joint_position, n.joint_velocity})
-    if (!(s >= 0.0) || !isfinite(s)) return false;
-  return true;
-}
-
 // the estimation arguments of an estimated episode; a null pointer to them is hb_rollout_batch_dev
 struct EstimationArgs {
   const hb_estimation_params* ep;
@@ -940,22 +921,18 @@ struct EstimationArgs {
 // The episode loop of hb_rollout_batch_dev (e == nullptr: exactly its launches) and hb_rollout_estimated_batch_dev
 static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb_rollout_params* p, const hb_rollout_command* cmd, double* rbd,
                         hb_actuation_state* act, uint8_t* estop, hb_rollout_stats* stats, double* log, const EstimationArgs* e) {
-  if (!ctx || B < 0 || n_ticks < 0 || tick0 < 0 || !p || !cmd || !rbd || !act || !estop || !stats) return HB_EINVAL;
-  if (p->mpc_every < 1 || !(p->period > 0.0) || p->log_every < 0 || !(p->actuation_delay >= 0.0) || !(p->sim.dt > 0.0) || p->sim.substeps < 1 ||
-      p->sim.substeps > 1000 || tick0 + n_ticks > INT32_MAX)
-    return HB_EINVAL;
-  if (e && (!e->ep || !e->est || !sensor_noise_ok(e->ep->noise))) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  for (int i = 0; i < B; ++i) {
-    const hb_rollout_command& c = cmd[i];
-    if (c.gait < 0 || c.gait > 3 || c.n_cmd < 1 || c.n_cmd > HB_ROLLOUT_MAX_CMDS || !(c.gait_start == c.gait_start)) return HB_EINVAL;
-    for (int k = 0; k < c.n_cmd; ++k) if (!(c.cmd_time[k] == c.cmd_time[k]) || (k > 0 && c.cmd_time[k] < c.cmd_time[k - 1])) return HB_EINVAL;
-  }
+  const bool params_ok = p && p->mpc_every >= 1 && p->period > 0.0 && p->log_every >= 0 && delay_ok(p->actuation_delay) && sim_params_ok(p->sim) &&
+                         tick0 + n_ticks <= INT32_MAX && (!e || (e->ep && e->est && sensor_noise_ok(e->ep->noise)));
   const bool cold = tick0 == 0;
-  if (!cold && ctx->res_valid < B) return HB_EINVAL;       // no resident solution to continue from
+  ENTER(ctx, B, n_ticks >= 0 && tick0 >= 0 && cmd && rbd && act && estop && stats && params_ok, CAPPED, [&] {
+    for (int i = 0; i < B; ++i) {
+      const hb_rollout_command& c = cmd[i];
+      if (c.gait < 0 || c.gait > 3 || c.n_cmd < 1 || c.n_cmd > HB_ROLLOUT_MAX_CMDS || !(c.gait_start == c.gait_start)) return false;
+      for (int k = 0; k < c.n_cmd; ++k) if (!(c.cmd_time[k] == c.cmd_time[k]) || (k > 0 && c.cmd_time[k] < c.cmd_time[k - 1])) return false;
+    }
+    return cold || ctx->res_valid >= B;       // a warm start continues from the resident solution
+  });
   if (n_ticks == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
   int rc = rollout_reserve(ctx);
   if (!rc && e) rc = estimation_reserve(ctx);
   if (rc) return rc;
@@ -1033,11 +1010,8 @@ int hb_estimation_reset(int B, uint64_t first_stream, hb_estimation_state* state
 int hb_sim_read_sensors_batch_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, double accel_dt, const double* rbd,
                                   hb_estimation_state* est, double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos,
                                   double* joint_vel) {
-  if (!ctx || B < 0 || !noise || !rbd || !est || !quat || !ang_vel_local || !lin_acc_local || !joint_pos || !joint_vel) return HB_EINVAL;
-  if (!sensor_noise_ok(*noise) || !(accel_dt > 0.0) || tick < 0 || tick > UINT32_MAX) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, noise && rbd && est && quat && ang_vel_local && lin_acc_local && joint_pos && joint_vel && sensor_noise_ok(*noise) && accel_dt > 0.0 &&
+        tick >= 0 && tick <= UINT32_MAX, CAPPED);
   return launch(ctx, K_UNPROFILED, sensor_read_kernel, (B + 63) / 64, 64, 0, B, *noise, (uint32_t)tick, accel_dt, 0.0, rbd, est, quat, ang_vel_local,
                 lin_acc_local, joint_pos, joint_vel, (uint8_t*)nullptr);
 }
@@ -1050,9 +1024,7 @@ int hb_observer_reset(int B, hb_observer_state* state) {
 
 int hb_contact_force_estimate_batch_dev(hb_ctx* ctx, int B, double cutoff_frequency, double dt, hb_observer_state* state, const double* rbd,
                                         const double* tau_cmd, double* est_contact_force, double* disturbance_torque) {
-  if (!ctx || B < 0 || !state || !rbd || !tau_cmd || !est_contact_force || !(cutoff_frequency > 0.0) || !(dt > 0.0)) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, state && rbd && tau_cmd && est_contact_force && cutoff_ok(cutoff_frequency, dt), UNCAPPED);
   return launch(ctx, K_UNPROFILED, contact_force_kernel, B, 32, 0, B, cutoff_frequency, dt, state, rbd, tau_cmd, est_contact_force, disturbance_torque);
 }
 
@@ -1068,46 +1040,34 @@ int hb_default_pd_gains(hb_pd_gains* g) {
 int hb_joint_command_batch_dev(hb_ctx* ctx, int B, const hb_pd_gains* gains, double period, const double* x_des, const double* u_des,
                                const double* wbc_sol, const int32_t* mode_cmd, const double* rbd, const uint8_t* loaded, uint8_t* estop,
                                double* command, double* output_torque) {
-  if (!ctx || B < 0 || !gains || !x_des || !u_des || !wbc_sol || !mode_cmd || !rbd || !command || !output_torque) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, gains && x_des && u_des && wbc_sol && mode_cmd && rbd && command && output_torque, UNCAPPED);
   return launch(ctx, K_UNPROFILED, joint_command_kernel, (B + 63) / 64, 64, 0, B, *gains, period, x_des, u_des, wbc_sol, mode_cmd, rbd, loaded, estop,
                 command, output_torque);
 }
 
 int hb_rbd_to_centroidal_batch_dev(hb_ctx* ctx, int B, const double* rbd, double* x) {
-  if (!ctx || B < 0 || !rbd || !x) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, rbd && x, UNCAPPED);
   return launch(ctx, K_UNPROFILED, rbd_to_centroidal_kernel, (B + 63) / 64, 64, 0, B, rbd, x);
 }
 
 int hb_reference_expand_batch_dev(hb_ctx* ctx, int B, const double* t0, const hb_reference* refs, double* x_ref, double* swing_ref, int32_t* mode) {
-  if (!ctx || B < 0 || !t0 || !refs || !x_ref || !swing_ref || !mode) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, t0 && refs && x_ref && swing_ref && mode, UNCAPPED);
   return launch(ctx, K_UNPROFILED, reference_expand_kernel, B, 128, 0, B, ctx->cfg.horizon_N, ctx->cfg.dt, t0, refs, x_ref, swing_ref, mode, nullptr);
 }
 
 int hb_reference_expand_grid_batch_dev(hb_ctx* ctx, int B, const double* node_times, const hb_reference* refs, double* x_ref, double* swing_ref,
                                        int32_t* mode) {
-  if (!ctx || B < 0 || !node_times || !refs || !x_ref || !swing_ref || !mode) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, node_times && refs && x_ref && swing_ref && mode, UNCAPPED);
   return launch(ctx, K_UNPROFILED, reference_expand_kernel, B, 128, 0, B, ctx->cfg.horizon_N, ctx->cfg.dt, nullptr, refs, x_ref, swing_ref, mode, node_times);
 }
 
 int hb_contact_positions_batch_dev(hb_ctx* ctx, int B, const double* x, double* pos) {
-  if (!ctx || B < 0 || !x || !pos) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x && pos, UNCAPPED);
   return launch(ctx, K_UNPROFILED, contact_positions_kernel, (B + 63) / 64, 64, 0, B, x, pos);
 }
 
 int hb_probe_flow_map_dev(hb_ctx* ctx, int B, const double* x, const double* u, double* f, double* A, double* Bm, double* ee) {
-  if (!ctx || B < 0 || !x || !u || !f || !A || !Bm) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x && u && f && A && Bm, UNCAPPED);
   return launch(ctx, K_UNPROFILED, probe_flow_map_kernel, B, 32, sizeof(ProbeShared), B, x, u, f, A, Bm, ee);
 }
 
@@ -1119,208 +1079,168 @@ int hb_probe_flow_map_dev(hb_ctx* ctx, int B, const double* x, const double* u, 
 
 int hb_wbc_qp_batch(hb_ctx* ctx, int B, int n, int m, const double* H, const double* g, const double* A, const double* lbA, const double* ubA,
                     double* x, int32_t* status, int32_t* iters) {
-  if (!ctx || B < 0 || !H || !g || !A || !lbA || !ubA || !x) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (n < 1 || n > QP_MAX_N || m < 0 || m > QP_MAX_M) return HB_EINVAL;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, H && g && A && lbA && ubA && x, UNCAPPED, [&] { return qp_shape_ok(n, m); });
   Staging s(ctx, B);
   auto dH = s.in(H, (size_t)n * n); auto dA = s.in(A, (size_t)m * n); auto dg = s.in(g, n); auto dlb = s.in(lbA, m); auto dub = s.in(ubA, m);
   auto dx = s.out(x, n); auto dst = s.out(status, 1); auto dit = s.out(iters, 1);
-  return s.run([&] { return hb_wbc_qp_batch_dev(ctx, B, n, m, dH, dg, dA, dlb, dub, dx, dst, dit); });
+  return s.run(1, [&](Chunk) { return hb_wbc_qp_batch_dev(ctx, B, n, m, dH, dg, dA, dlb, dub, dx, dst, dit); });
 }
 
 int hb_wbc_assemble_batch(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
                           const uint8_t* stance_mode, double* H, double* g, double* A, double* lbA, double* ubA, int32_t* m_rows) {
-  if (!ctx || B < 0 || !x_des || !u_des || !rbd || !mode || !H || !g || !A || !lbA || !ubA || !m_rows) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x_des && u_des && rbd && mode && H && g && A && lbA && ubA && m_rows, CAPPED);
   Staging s(ctx, B);
   auto xd = s.in(x_des, NX); auto ud = s.in(u_des, NU); auto r = s.in(rbd, 32); auto md = s.in(mode, 1); auto sm = s.in_or_null(stance_mode, 1);
   auto dH = s.out(H, QP_STRIDE_H); auto dA = s.out(A, QP_STRIDE_A); auto dg = s.out(g, NWBC); auto dlb = s.out(lbA, WBC_ROWS);
   auto dub = s.out(ubA, WBC_ROWS); auto dm = s.out(m_rows, 1);
-  return s.run([&] { return hb_wbc_assemble_batch_dev(ctx, B, xd, ud, r, md, sm, dH, dg, dA, dlb, dub, dm); });
+  return s.run(1, [&](Chunk) { return hb_wbc_assemble_batch_dev(ctx, B, xd, ud, r, md, sm, dH, dg, dA, dlb, dub, dm); });
 }
 
 int hb_wbc_solve_batch(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
                        const uint8_t* stance_mode, double* sol, int32_t* status) {
-  if (!ctx || B < 0 || !x_des || !u_des || !rbd || !mode || !sol) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x_des && u_des && rbd && mode && sol, CAPPED);
   Staging s(ctx, B);
   auto xd = s.in(x_des, NX); auto ud = s.in(u_des, NU); auto r = s.in(rbd, 32); auto md = s.in(mode, 1); auto sm = s.in_or_null(stance_mode, 1);
   auto dsol = s.out(sol, NWBC); auto dst = s.out(status, 1);
-  return s.run([&] { return hb_wbc_solve_batch_dev(ctx, B, xd, ud, r, md, sm, dsol, dst); });
+  return s.run(1, [&](Chunk) { return hb_wbc_solve_batch_dev(ctx, B, xd, ud, r, md, sm, dsol, dst); });
 }
 
 int hb_hoqp_solve_batch(hb_ctx* ctx, int B, const hb_hoqp_problem* problems, double* x, double* slack, int32_t* status) {
-  if (!ctx || B < 0 || !problems || !x) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  for (int i = 0; i < B; ++i) {
-    const hb_hoqp_problem& p = problems[i];
-    if (p.n < 1 || p.n > HB_HOQP_N || p.levels < 1 || p.levels > HB_HOQP_MAX_LEVELS) return HB_EINVAL;
-    int stk = 0;
-    for (int l = 0; l < p.levels; ++l) { if (p.ma[l] < 0 || p.ma[l] > HB_HOQP_MAX_EQ || p.md[l] < 0 || p.md[l] > HB_HOQP_MAX_IN) return HB_EINVAL; stk += p.md[l]; }
-    if (stk > HB_HOQP_MAX_STACKED) return HB_EINVAL;
-  }
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, problems && x, CAPPED, [&] {
+    for (int i = 0; i < B; ++i) {
+      const hb_hoqp_problem& p = problems[i];
+      if (p.n < 1 || p.n > HB_HOQP_N || p.levels < 1 || p.levels > HB_HOQP_MAX_LEVELS) return false;
+      int stk = 0;
+      for (int l = 0; l < p.levels; ++l) { if (p.ma[l] < 0 || p.ma[l] > HB_HOQP_MAX_EQ || p.md[l] < 0 || p.md[l] > HB_HOQP_MAX_IN) return false; stk += p.md[l]; }
+      if (stk > HB_HOQP_MAX_STACKED) return false;
+    }
+    return true;
+  });
   Staging s(ctx, B);
   auto pb = s.in(problems, 1); auto dx = s.out(x, HQ_N); auto dsl = s.out(slack, HQ_STK); auto dst = s.out(status, 1);
-  return s.run([&] { return hb_hoqp_solve_batch_dev(ctx, B, pb, dx, dsl, dst); });
+  return s.run(1, [&](Chunk) { return hb_hoqp_solve_batch_dev(ctx, B, pb, dx, dsl, dst); });
 }
 
 int hb_hierarchical_wbc_tasks_batch(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
                                     hb_hoqp_problem* problems) {
-  if (!ctx || B < 0 || !x_des || !u_des || !rbd || !mode || !problems) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x_des && u_des && rbd && mode && problems, CAPPED);
   Staging s(ctx, B);
   auto xd = s.in(x_des, NX); auto ud = s.in(u_des, NU); auto r = s.in(rbd, 32); auto md = s.in(mode, 1); auto pb = s.out(problems, 1);
-  return s.run([&] { return hwbc_tasks_dev(ctx, B, xd, ud, r, md, pb); });
+  return s.run(1, [&](Chunk) { return hwbc_tasks_dev(ctx, B, xd, ud, r, md, pb); });
 }
 
 int hb_hierarchical_wbc_solve_batch(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, double* sol,
                                     int32_t* status) {
-  if (!ctx || B < 0 || !x_des || !u_des || !rbd || !mode || !sol) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x_des && u_des && rbd && mode && sol, CAPPED);
   Staging s(ctx, B);
   auto xd = s.in(x_des, NX); auto ud = s.in(u_des, NU); auto r = s.in(rbd, 32); auto md = s.in(mode, 1);
   auto dsol = s.out(sol, NWBC); auto dst = s.out(status, 1);
-  return s.run([&] { return hb_hierarchical_wbc_solve_batch_dev(ctx, B, xd, ud, r, md, dsol, dst); });
+  return s.run(1, [&](Chunk) { return hb_hierarchical_wbc_solve_batch_dev(ctx, B, xd, ud, r, md, dsol, dst); });
 }
 
 int hb_mpc_cold_start_batch(hb_ctx* ctx, int B, const double* x0, const int32_t* mode, double* x_traj, double* u_traj) {
-  if (!ctx || B < 0 || !x0 || !mode || !x_traj || !u_traj) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x0 && mode && x_traj && u_traj, CAPPED);
   const size_t N = ctx->cfg.horizon_N;
   Staging s(ctx, B);
   auto d0 = s.in(x0, NX); auto md = s.in(mode, N + 1); auto xt = s.out(x_traj, (N + 1) * NX); auto ut = s.out(u_traj, N * NU);
-  return s.run([&] { return hb_mpc_cold_start_batch_dev(ctx, B, d0, md, xt, ut); });
+  return s.run(1, [&](Chunk) { return hb_mpc_cold_start_batch_dev(ctx, B, d0, md, xt, ut); });
 }
 
 int hb_mpc_solve_batch(hb_ctx* ctx, int B, const double* x0, const double* x_ref, const double* swing_ref, const int32_t* mode, double* x_traj,
                        double* u_traj, hb_solve_info* info) {
-  if (!ctx || B < 0 || !x0 || !x_ref || !swing_ref || !mode || !x_traj || !u_traj) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x0 && x_ref && swing_ref && mode && x_traj && u_traj, CAPPED);
   const size_t N = ctx->cfg.horizon_N;
   Staging s(ctx, B);
   auto d0 = s.in(x0, NX); auto xr = s.in(x_ref, (N + 1) * NX); auto sw = s.in(swing_ref, (N + 1) * 24); auto md = s.in(mode, N + 1);
   auto xt = s.inout(x_traj, (N + 1) * NX); auto ut = s.inout(u_traj, N * NU); auto inf = s.out(info, 1);
-  return s.run([&] { return hb_mpc_solve_batch_dev(ctx, B, d0, xr, sw, md, xt, ut, inf); });
+  return s.run(1, [&](Chunk) { return hb_mpc_solve_batch_dev(ctx, B, d0, xr, sw, md, xt, ut, inf); });
 }
 
 int hb_mpc_solve_grid_batch(hb_ctx* ctx, int B, const double* x0, const double* node_times, const int32_t* n_intervals, const double* x_ref,
                             const double* swing_ref, const int32_t* mode, double* x_traj, double* u_traj, hb_solve_info* info) {
-  if (!ctx || B < 0 || !x0 || !node_times || !n_intervals || !x_ref || !swing_ref || !mode || !x_traj || !u_traj) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
+  ENTER(ctx, B, x0 && node_times && n_intervals && x_ref && swing_ref && mode && x_traj && u_traj, CAPPED, [&] {
+    const size_t N = ctx->cfg.horizon_N;
+    for (int i = 0; i < B; ++i) {      // a grid the kernels can walk: 1 <= n <= N intervals of positive length
+      if (n_intervals[i] < 1 || n_intervals[i] > (int)N) return false;
+      for (int k = 0; k < n_intervals[i]; ++k) if (!(node_times[(size_t)i * (N + 1) + k + 1] > node_times[(size_t)i * (N + 1) + k])) return false;
+    }
+    return true;
+  });
   const size_t N = ctx->cfg.horizon_N;
-  for (int i = 0; i < B; ++i) {      // a grid the kernels can walk: 1 <= n <= N intervals of positive length
-    if (n_intervals[i] < 1 || n_intervals[i] > (int)N) return HB_EINVAL;
-    for (int k = 0; k < n_intervals[i]; ++k) if (!(node_times[(size_t)i * (N + 1) + k + 1] > node_times[(size_t)i * (N + 1) + k])) return HB_EINVAL;
-  }
-  if (set_device(ctx)) return HB_ECUDA;
   Staging s(ctx, B);
   auto d0 = s.in(x0, NX); auto xr = s.in(x_ref, (N + 1) * NX); auto sw = s.in(swing_ref, (N + 1) * 24); auto md = s.in(mode, N + 1);
   auto xt = s.inout(x_traj, (N + 1) * NX); auto ut = s.inout(u_traj, N * NU); auto tk = s.in(node_times, N + 1); auto nn = s.in(n_intervals, 1);
   auto inf = s.out(info, 1);
-  return s.run([&] { return hb_mpc_solve_grid_batch_dev(ctx, B, d0, tk, nn, xr, sw, md, xt, ut, inf); });
+  return s.run(1, [&](Chunk) { return hb_mpc_solve_grid_batch_dev(ctx, B, d0, tk, nn, xr, sw, md, xt, ut, inf); });
 }
 
 int hb_time_grid_batch(hb_ctx* ctx, int B, const double* t0, const hb_reference* refs, double* node_times, int32_t* n_intervals, int32_t* status) {
-  if (!ctx || B < 0 || !t0 || !refs || !node_times || !n_intervals) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (!references_valid(B, refs)) return HB_EINVAL;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, t0 && refs && node_times && n_intervals, CAPPED, [&] { return references_valid(B, refs); });
   const size_t N = ctx->cfg.horizon_N;
   Staging s(ctx, B);
   auto d0 = s.in(t0, 1); auto rf = s.in(refs, 1); auto tk = s.out(node_times, N + 1); auto nn = s.out(n_intervals, 1); auto st = s.out(status, 1);
-  return s.run([&] { return hb_time_grid_batch_dev(ctx, B, d0, rf, tk, nn, st); });
+  return s.run(1, [&](Chunk) { return hb_time_grid_batch_dev(ctx, B, d0, rf, tk, nn, st); });
 }
 
 int hb_reference_expand_grid_batch(hb_ctx* ctx, int B, const double* node_times, const hb_reference* refs, double* x_ref, double* swing_ref,
                                    int32_t* mode) {
-  if (!ctx || B < 0 || !node_times || !refs || !x_ref || !swing_ref || !mode) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (!references_valid(B, refs)) return HB_EINVAL;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, node_times && refs && x_ref && swing_ref && mode, CAPPED, [&] { return references_valid(B, refs); });
   const size_t N = ctx->cfg.horizon_N;
   Staging s(ctx, B);
   auto tk = s.in(node_times, N + 1); auto rf = s.in(refs, 1);
   auto xr = s.out(x_ref, (N + 1) * NX); auto sw = s.out(swing_ref, (N + 1) * 24); auto md = s.out(mode, N + 1);
-  return s.run([&] { return hb_reference_expand_grid_batch_dev(ctx, B, tk, rf, xr, sw, md); });
+  return s.run(1, [&](Chunk) { return hb_reference_expand_grid_batch_dev(ctx, B, tk, rf, xr, sw, md); });
 }
 
 int hb_resident_write_batch(hb_ctx* ctx, int B, const double* t0, const double* x_traj, const double* u_traj, const int32_t* mode, const double* node_times,
                             const int32_t* n_intervals) {
-  if (!ctx || B < 0 || !t0 || !x_traj || !u_traj) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
+  ENTER(ctx, B, t0 && x_traj && u_traj, CAPPED, [&] {
+    if (!ctx->cfg.event_nodes) return true;
+    if (!node_times || !n_intervals) return false;      // an event-node context shifts between grids: the snapshot needs its grid
+    for (int i = 0; i < B; ++i) if (n_intervals[i] < 1 || n_intervals[i] > ctx->cfg.horizon_N) return false;
+    return true;
+  });
   const bool grid = ctx->cfg.event_nodes != 0;
-  if (grid && (!node_times || !n_intervals)) return HB_EINVAL;      // an event-node context shifts between grids: the snapshot needs its grid
   const size_t N = ctx->cfg.horizon_N;
-  if (grid) for (int i = 0; i < B; ++i) if (n_intervals[i] < 1 || n_intervals[i] > (int)N) return HB_EINVAL;
-  if (set_device(ctx)) return HB_ECUDA;
-  H2D(ctx->res_t0, t0, sizeof(double) * B); H2D(ctx->res_xt, x_traj, sizeof(double) * B * (N + 1) * NX); H2D(ctx->res_ut, u_traj, sizeof(double) * B * N * NU);
-  if (mode) H2D(ctx->res_mode, mode, sizeof(int32_t) * B * (N + 1));
-  if (grid) { H2D(ctx->res_tk, node_times, sizeof(double) * B * (N + 1)); H2D(ctx->res_nn, n_intervals, sizeof(int32_t) * B); }
-  int rc = hb_sync(ctx);
+  const int rc = drain(ctx, [&]() -> int {
+    H2D(ctx->res_t0, t0, sizeof(double) * B); H2D(ctx->res_xt, x_traj, sizeof(double) * B * (N + 1) * NX); H2D(ctx->res_ut, u_traj, sizeof(double) * B * N * NU);
+    if (mode) H2D(ctx->res_mode, mode, sizeof(int32_t) * B * (N + 1));
+    if (grid) { H2D(ctx->res_tk, node_times, sizeof(double) * B * (N + 1)); H2D(ctx->res_nn, n_intervals, sizeof(int32_t) * B); }
+    return HB_OK;
+  }());
   if (rc) return rc;
   if (ctx->res_valid < B) ctx->res_valid = B;
   return HB_OK;
 }
 
 int hb_resident_read_grid_batch(hb_ctx* ctx, int B, double* node_times, int32_t* n_intervals) {
-  if (!ctx || B < 0 || !node_times || !n_intervals) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->res_valid || !ctx->cfg.event_nodes) return HB_EINVAL;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, node_times && n_intervals, UNCAPPED, [&] { return B <= ctx->res_valid && ctx->cfg.event_nodes; });
   const size_t N = ctx->cfg.horizon_N;
-  D2H(node_times, ctx->res_tk, sizeof(double) * B * (N + 1)); D2H(n_intervals, ctx->res_nn, sizeof(int32_t) * B);
-  return hb_sync(ctx);
+  return drain(ctx, [&]() -> int {
+    D2H(node_times, ctx->res_tk, sizeof(double) * B * (N + 1)); D2H(n_intervals, ctx->res_nn, sizeof(int32_t) * B);
+    return HB_OK;
+  }());
 }
 
 int hb_control_step_batch(hb_ctx* ctx, int B, double t_rel, const double* x0, const double* x_ref, const double* swing_ref, const int32_t* mode,
                           const double* rbd, double* x_traj, double* u_traj, hb_solve_info* info, double* wbc_sol, double* torque,
                           int32_t* wbc_status) {
-  if (!ctx || B < 0 || !x0 || !x_ref || !swing_ref || !mode || !rbd || !x_traj || !u_traj) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x0 && x_ref && swing_ref && mode && rbd && x_traj && u_traj, CAPPED);
   const size_t N = ctx->cfg.horizon_N;
   Staging s(ctx, B);
   auto d0 = s.in(x0, NX); auto xr = s.in(x_ref, (N + 1) * NX); auto sw = s.in(swing_ref, (N + 1) * 24); auto md = s.in(mode, N + 1);
   auto xt = s.inout(x_traj, (N + 1) * NX); auto ut = s.inout(u_traj, N * NU); auto r = s.in(rbd, 32);
   auto inf = s.out(info, 1); auto sol = s.out(wbc_sol, NWBC); auto tau = s.out(torque, NJ); auto st = s.out(wbc_status, 1);
-  const int rc = s.reserve();
-  if (rc) return rc;
   // Two half-batches on two streams: the copies of one half overlap the kernels of the other (pinned host memory assumed).
-  return chunked(ctx, B, B >= 256 ? 2 : 1, [&](int, size_t lo, size_t hi) -> int {
-    int r2 = s.h2d(lo, hi);
-    if (!r2) r2 = hb_control_step_batch_dev(ctx, (int)(hi - lo), t_rel, d0.at(lo), xr.at(lo), sw.at(lo), md.at(lo), r.at(lo), xt.at(lo), ut.at(lo),
-                                            inf.at(lo), sol.at(lo), tau.at(lo), st.at(lo));
-    return r2 ? r2 : s.d2h(lo, hi);
+  return s.run(B >= 256 ? 2 : 1, [&](Chunk k) {
+    return hb_control_step_batch_dev(ctx, k.n, t_rel, d0.at(k.lo), xr.at(k.lo), sw.at(k.lo), md.at(k.lo), r.at(k.lo), xt.at(k.lo), ut.at(k.lo),
+                                     inf.at(k.lo), sol.at(k.lo), tau.at(k.lo), st.at(k.lo));
   });
 }
 
 int hb_resident_cycle_batch(hb_ctx* ctx, int B, int cold_start, double t_rel, const double* t0, const double* x0, const hb_reference* refs,
                             const double* rbd, hb_solve_info* info, double* wbc_sol, double* torque, int32_t* wbc_status) {
-  if (!ctx || B < 0 || !t0 || !x0 || !refs || !rbd) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (!cold_start && ctx->res_valid < B) return HB_EINVAL;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, t0 && x0 && refs && rbd, CAPPED, [&] { return cold_start || ctx->res_valid >= B; });
   // a pinned (page-locked, mapped) reference array is read by the device directly
   const hb_reference* refs_dev = nullptr;
   {
@@ -1347,32 +1267,29 @@ int hb_resident_cycle_batch(hb_ctx* ctx, int B, int cold_start, double t_rel, co
   auto d0 = s.in(t0, 1); auto dx0 = s.in(x0, NX); auto r = s.in(rbd, 32); auto rf = s.tmp<hb_reference>(1);
   auto d_pack = s.buf<double>(pack_words); auto d_stat = s.buf<unsigned long long>(stat_words);
   auto inf = s.out(info, 1); auto sol = s.out(wbc_sol, NWBC); auto tau = s.out(torque, NJ); auto st = s.out(wbc_status, 1);
-  int rc = s.reserve();
-  if (!rc) rc = grow(ctx, &ctx->pinned, &ctx->pinned_cap, refs_dev ? sizeof(unsigned long long) * stat_words : sizeof(double) * pack_words, true);
+  int rc = grow(ctx, &ctx->pinned, &ctx->pinned_cap, refs_dev ? sizeof(unsigned long long) * stat_words : sizeof(double) * pack_words, true);
   if (rc) return rc;
   double* h_pack = static_cast<double*>(ctx->pinned);
   unsigned long long* h_stat = static_cast<unsigned long long*>(ctx->pinned);
   size_t pack_base = 0;
   ctx->last_h2d_bytes = 0;
-  rc = chunked(ctx, B, nchunk, [&](int c, size_t lo, size_t hi) -> int {
-    const int n = (int)(hi - lo);
-    int r2 = s.h2d(lo, hi);
-    if (r2) return r2;
+  rc = s.run(nchunk, [&](Chunk k) -> int {
     if (refs_dev) {
-      CK(cudaMemsetAsync(d_stat.at(2 * c), 0, 2 * sizeof(unsigned long long), ctx->stream));
-      r2 = launch(ctx, K_UNPROFILED, reference_gather_pinned_kernel, n, 128, 0, n, refs_dev + lo, rf.at(lo), d_stat.at(2 * c));
+      CK(cudaMemsetAsync(d_stat.at(2 * k.c), 0, 2 * sizeof(unsigned long long), ctx->stream));
+      const int r2 = launch(ctx, K_UNPROFILED, reference_gather_pinned_kernel, k.n, 128, 0, k.n, refs_dev + k.lo, rf.at(k.lo), d_stat.at(2 * k.c));
       if (r2) return r2;
-      D2H(h_stat + 2 * c, d_stat.at(2 * c), 2 * sizeof(unsigned long long));
+      D2H(h_stat + 2 * k.c, d_stat.at(2 * k.c), 2 * sizeof(unsigned long long));
     } else {
-      const size_t words = ref_pack(refs, lo, hi, h_pack + pack_base);
+      const size_t words = ref_pack(refs, k.lo, k.hi, h_pack + pack_base);
       H2D(d_pack.at(pack_base), h_pack + pack_base, sizeof(double) * words);
-      r2 = launch(ctx, K_UNPROFILED, reference_unpack_kernel, n, 128, 0, n, reinterpret_cast<const long long*>(d_pack.at(pack_base)), d_pack.at(pack_base), rf.at(lo));
+      const int r2 = launch(ctx, K_UNPROFILED, reference_unpack_kernel, k.n, 128, 0, k.n, reinterpret_cast<const long long*>(d_pack.at(pack_base)),
+                            d_pack.at(pack_base), rf.at(k.lo));
       if (r2) return r2;
       pack_base += words;
       ctx->last_h2d_bytes += sizeof(double) * words;
     }
-    r2 = hb_resident_cycle_batch_dev(ctx, n, cold_start, t_rel, d0.at(lo), dx0.at(lo), rf.at(lo), r.at(lo), inf.at(lo), sol.at(lo), tau.at(lo), st.at(lo));
-    return r2 ? r2 : s.d2h(lo, hi);
+    return hb_resident_cycle_batch_dev(ctx, k.n, cold_start, t_rel, d0.at(k.lo), dx0.at(k.lo), rf.at(k.lo), r.at(k.lo), inf.at(k.lo), sol.at(k.lo),
+                                       tau.at(k.lo), st.at(k.lo));
   });
   if (rc) return rc;
   if (refs_dev) {
@@ -1385,170 +1302,127 @@ int hb_resident_cycle_batch(hb_ctx* ctx, int B, int cold_start, double t_rel, co
 }
 
 int hb_plan_references_gpu(hb_ctx* ctx, int B, const hb_plan_input* in, double* latest_stance, hb_reference* out, int32_t* status) {
-  if (!ctx || B < 0 || !in || !latest_stance || !out) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, in && latest_stance && out, CAPPED);
   Staging s(ctx, B);
   auto din = s.in(in, 1); auto ls = s.inout(latest_stance, 12); auto dout = s.out(out, 1); auto st = s.out(status, 1);
-  return s.run([&] { return hb_plan_references_batch_dev(ctx, B, din, nullptr, ls, dout, st); });
+  return s.run(1, [&](Chunk) { return hb_plan_references_batch_dev(ctx, B, din, nullptr, ls, dout, st); });
 }
 
 int hb_resident_plan_cycle_batch(hb_ctx* ctx, int B, int cold_start, double t_rel, const hb_plan_input* in, const double* rbd, hb_solve_info* info,
                                  double* wbc_sol, double* torque, int32_t* wbc_status, int32_t* plan_status) {
-  if (!ctx || B < 0 || !in || !rbd) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (!cold_start && ctx->res_valid < B) return HB_EINVAL;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, in && rbd, CAPPED, [&] { return cold_start || ctx->res_valid >= B; });
   const int nchunk = cycle_chunks(ctx, B, true);
   Staging s(ctx, B);
   auto din = s.in(in, 1); auto r = s.in(rbd, 32);
   auto d0 = s.tmp<double>(1); auto dx0 = s.tmp<double>(NX); auto feet = s.tmp<double>(12); auto rf = s.tmp<hb_reference>(1);   // planner -> cycle
   auto inf = s.out(info, 1); auto sol = s.out(wbc_sol, NWBC); auto tau = s.out(torque, NJ); auto st = s.out(wbc_status, 1); auto pst = s.out(plan_status, 1);
-  const int rc = s.reserve();
-  if (rc) return rc;
-  return chunked(ctx, B, nchunk, [&](int, size_t lo, size_t hi) -> int {
-    const int n = (int)(hi - lo);
-    int r2 = s.h2d(lo, hi);
-    if (r2) return r2;
+  return s.run(nchunk, [&](Chunk k) -> int {
+    const size_t lo = k.lo;
+    const int n = k.n;
     if (cold_start) CK(cudaMemsetAsync(ctx->res_stance + lo * 12, 0, sizeof(double) * n * 12, ctx->stream));   // latestStanceposition_ starts at zero
-    r2 = launch(ctx, K_UNPROFILED, plan_prepare_kernel, (n + 63) / 64, 64, 0, n, din.at(lo), d0.at(lo), dx0.at(lo), feet.at(lo));
+    int r2 = launch(ctx, K_UNPROFILED, plan_prepare_kernel, (n + 63) / 64, 64, 0, n, din.at(lo), d0.at(lo), dx0.at(lo), feet.at(lo));
     if (!r2) r2 = hb_plan_references_batch_dev(ctx, n, din.at(lo), feet.at(lo), ctx->res_stance + lo * 12, rf.at(lo), pst.at(lo));
     if (!r2) r2 = hb_resident_cycle_batch_dev(ctx, n, cold_start, t_rel, d0.at(lo), dx0.at(lo), rf.at(lo), r.at(lo), inf.at(lo), sol.at(lo), tau.at(lo), st.at(lo));
-    return r2 ? r2 : s.d2h(lo, hi);
+    return r2;
   });
 }
 
 int hb_resident_read_batch(hb_ctx* ctx, int B, double* t0, double* x_traj, double* u_traj) {
-  if (!ctx || B < 0) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->res_valid) return HB_EINVAL;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, true, UNCAPPED, [&] { return B <= ctx->res_valid; });
   const size_t N = ctx->cfg.horizon_N;
-  if (t0) D2H(t0, ctx->res_t0, sizeof(double) * B);
-  if (x_traj) D2H(x_traj, ctx->res_xt, sizeof(double) * B * (N + 1) * NX);
-  if (u_traj) D2H(u_traj, ctx->res_ut, sizeof(double) * B * N * NU);
-  return hb_sync(ctx);
+  return drain(ctx, [&]() -> int {
+    if (t0) D2H(t0, ctx->res_t0, sizeof(double) * B);
+    if (x_traj) D2H(x_traj, ctx->res_xt, sizeof(double) * B * (N + 1) * NX);
+    if (u_traj) D2H(u_traj, ctx->res_ut, sizeof(double) * B * N * NU);
+    return HB_OK;
+  }());
 }
 
 int hb_joint_command_batch(hb_ctx* ctx, int B, const hb_pd_gains* gains, double period, const double* x_des, const double* u_des,
                            const double* wbc_sol, const int32_t* mode_cmd, const double* rbd, const uint8_t* loaded, uint8_t* estop,
                            double* command, double* output_torque) {
-  if (!ctx || B < 0 || !gains || !x_des || !u_des || !wbc_sol || !mode_cmd || !rbd || !command || !output_torque) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, gains && x_des && u_des && wbc_sol && mode_cmd && rbd && command && output_torque, CAPPED);
   Staging s(ctx, B);
   auto xd = s.in(x_des, NX); auto ud = s.in(u_des, NU); auto r = s.in(rbd, 32); auto sol = s.in(wbc_sol, NWBC); auto md = s.in(mode_cmd, 1);
   auto ld = s.in_or_null(loaded, 1); auto es = s.inout_or_null(estop, 1); auto cmd = s.out(command, NJ * 5); auto tau = s.out(output_torque, NJ);
-  return s.run([&] { return hb_joint_command_batch_dev(ctx, B, gains, period, xd, ud, sol, md, r, ld, es, cmd, tau); });
+  return s.run(1, [&](Chunk) { return hb_joint_command_batch_dev(ctx, B, gains, period, xd, ud, sol, md, r, ld, es, cmd, tau); });
 }
 
 int hb_estimator_update_batch(hb_ctx* ctx, int B, const hb_kf_params* params, double dt, hb_kf_state* state, const double* quat,
                               const double* ang_vel_local, const double* lin_acc_local, const double* joint_pos, const double* joint_vel,
                               const uint8_t* contact_flag, double* rbd_out) {
-  if (!ctx || B < 0 || !params || !state || !quat || !ang_vel_local || !lin_acc_local || !joint_pos || !joint_vel || !contact_flag || !rbd_out) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, params && state && quat && ang_vel_local && lin_acc_local && joint_pos && joint_vel && contact_flag && rbd_out, CAPPED);
   Staging s(ctx, B);
   auto kf = s.inout(state, 1); auto q = s.in(quat, 4); auto w = s.in(ang_vel_local, 3); auto a = s.in(lin_acc_local, 3);
   auto jp = s.in(joint_pos, NJ); auto jv = s.in(joint_vel, NJ); auto fl = s.in(contact_flag, 4); auto ro = s.out(rbd_out, 32);
-  return s.run([&] { return hb_estimator_update_batch_dev(ctx, B, params, dt, kf, q, w, a, jp, jv, fl, ro); });
+  return s.run(1, [&](Chunk) { return hb_estimator_update_batch_dev(ctx, B, params, dt, kf, q, w, a, jp, jv, fl, ro); });
 }
 
 int hb_sim_read_sensors(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, double accel_dt, const double* rbd, hb_estimation_state* est,
                         double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos, double* joint_vel) {
-  if (!ctx || B < 0 || !noise || !rbd || !est || !quat || !ang_vel_local || !lin_acc_local || !joint_pos || !joint_vel) return HB_EINVAL;
-  if (!sensor_noise_ok(*noise) || !(accel_dt > 0.0) || tick < 0 || tick > UINT32_MAX) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, noise && rbd && est && quat && ang_vel_local && lin_acc_local && joint_pos && joint_vel && sensor_noise_ok(*noise) && accel_dt > 0.0 &&
+        tick >= 0 && tick <= UINT32_MAX, CAPPED);
   Staging s(ctx, B);
   auto r = s.in(rbd, 32); auto es = s.inout(est, 1); auto q = s.out(quat, 4); auto w = s.out(ang_vel_local, 3); auto a = s.out(lin_acc_local, 3);
   auto jp = s.out(joint_pos, NJ); auto jv = s.out(joint_vel, NJ);
-  return s.run([&] { return hb_sim_read_sensors_batch_dev(ctx, B, noise, tick, accel_dt, r, es, q, w, a, jp, jv); });
+  return s.run(1, [&](Chunk) { return hb_sim_read_sensors_batch_dev(ctx, B, noise, tick, accel_dt, r, es, q, w, a, jp, jv); });
 }
 
 int hb_actuation_batch(hb_ctx* ctx, int B, double delay, const double* time, hb_actuation_state* state, const double* command, const double* rbd,
                        double* tau) {
-  if (!ctx || B < 0 || !time || !state || !command || !rbd || !tau) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, time && state && command && rbd && tau, CAPPED, [&] { return delay_ok(delay); });
   Staging s(ctx, B);
   auto st = s.inout(state, 1); auto tm = s.in(time, 1); auto cmd = s.in(command, NJ * 5); auto r = s.in(rbd, 32); auto t = s.out(tau, NJ);
-  return s.run([&] { return hb_actuation_batch_dev(ctx, B, delay, tm, st, cmd, r, t); });
+  return s.run(1, [&](Chunk) { return hb_actuation_batch_dev(ctx, B, delay, tm, st, cmd, r, t); });
 }
 
 int hb_sim_step_batch(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {
-  if (!ctx || B < 0 || !params || !rbd || !tau) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, params && rbd && tau, CAPPED, [&] { return sim_params_ok(*params); });
   Staging s(ctx, B);
   auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
-  return s.run([&] { return hb_sim_step_batch_dev(ctx, B, params, r, t, cf, fl); });
+  return s.run(1, [&](Chunk) { return hb_sim_step_batch_dev(ctx, B, params, r, t, cf, fl); });
 }
 
 int hb_resident_wbc_batch(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
                           int32_t* mode_out, double* wbc_sol, double* torque, int32_t* wbc_status) {
-  if (!ctx || B < 0 || !t_now || !rbd || !x_des || !u_des || !mode_out || !wbc_sol) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (B > ctx->res_valid) return HB_EINVAL;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, t_now && rbd && x_des && u_des && mode_out && wbc_sol, CAPPED, [&] { return B <= ctx->res_valid; });
   Staging s(ctx, B);
   auto tn = s.in(t_now, 1); auto r = s.in(rbd, 32); auto sm = s.in_or_null(stance_mode, 1);
   auto xd = s.out(x_des, NX); auto ud = s.out(u_des, NU); auto md = s.out(mode_out, 1); auto sol = s.out(wbc_sol, NWBC);
   auto tau = s.out(torque, NJ); auto st = s.out(wbc_status, 1);    // always passed: the fallback and its bookkeeping run on every call
-  return s.run([&] { return hb_resident_wbc_batch_dev(ctx, B, tn, r, sm, xd, ud, md, sol, tau, st); });
+  return s.run(1, [&](Chunk) { return hb_resident_wbc_batch_dev(ctx, B, tn, r, sm, xd, ud, md, sol, tau, st); });
 }
 
 int hb_contact_force_estimate_batch(hb_ctx* ctx, int B, double cutoff_frequency, double dt, hb_observer_state* state, const double* rbd,
                                     const double* tau_cmd, double* est_contact_force, double* disturbance_torque) {
-  if (!ctx || B < 0 || !state || !rbd || !tau_cmd || !est_contact_force) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, state && rbd && tau_cmd && est_contact_force, CAPPED, [&] { return cutoff_ok(cutoff_frequency, dt); });
   Staging s(ctx, B);
   auto st = s.inout(state, 1); auto r = s.in(rbd, 32); auto t = s.in(tau_cmd, NJ); auto est = s.out(est_contact_force, 16);
   auto dist = s.out(disturbance_torque, NQ);
-  return s.run([&] { return hb_contact_force_estimate_batch_dev(ctx, B, cutoff_frequency, dt, st, r, t, est, dist); });
+  return s.run(1, [&](Chunk) { return hb_contact_force_estimate_batch_dev(ctx, B, cutoff_frequency, dt, st, r, t, est, dist); });
 }
 
 int hb_rbd_to_centroidal_batch(hb_ctx* ctx, int B, const double* rbd, double* x) {
-  if (!ctx || B < 0 || !rbd || !x) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, rbd && x, CAPPED);
   Staging s(ctx, B);
   auto r = s.in(rbd, 32); auto dx = s.out(x, NX);
-  return s.run([&] { return hb_rbd_to_centroidal_batch_dev(ctx, B, r, dx); });
+  return s.run(1, [&](Chunk) { return hb_rbd_to_centroidal_batch_dev(ctx, B, r, dx); });
 }
 
 int hb_reference_expand_batch(hb_ctx* ctx, int B, const double* t0, const hb_reference* refs, double* x_ref, double* swing_ref, int32_t* mode) {
-  if (!ctx || B < 0 || !t0 || !refs || !x_ref || !swing_ref || !mode) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (!references_valid(B, refs)) return HB_EINVAL;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, t0 && refs && x_ref && swing_ref && mode, CAPPED, [&] { return references_valid(B, refs); });
   const size_t N = ctx->cfg.horizon_N;
   Staging s(ctx, B);
   auto d0 = s.in(t0, 1); auto rf = s.in(refs, 1);
   auto xr = s.out(x_ref, (N + 1) * NX); auto sw = s.out(swing_ref, (N + 1) * 24); auto md = s.out(mode, N + 1);
-  return s.run([&] { return hb_reference_expand_batch_dev(ctx, B, d0, rf, xr, sw, md); });
+  return s.run(1, [&](Chunk) { return hb_reference_expand_batch_dev(ctx, B, d0, rf, xr, sw, md); });
 }
 
 int hb_contact_positions_batch(hb_ctx* ctx, int B, const double* x, double* pos) {
-  if (!ctx || B < 0 || !x || !pos) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x && pos, CAPPED);
   Staging s(ctx, B);
   auto dx = s.in(x, NX); auto dp = s.out(pos, 12);
-  return s.run([&] { return hb_contact_positions_batch_dev(ctx, B, dx, dp); });
+  return s.run(1, [&](Chunk) { return hb_contact_positions_batch_dev(ctx, B, dx, dp); });
 }
 
 static std::atomic<int> g_plan_threads{0};   // 0 = hardware_concurrency (hb_plan_set_threads)
@@ -1598,14 +1472,11 @@ int hb_gait_select(int B, hb_gait_selector* state, const int32_t* gait_type, con
 }
 
 int hb_probe_flow_map(hb_ctx* ctx, int B, const double* x, const double* u, double* f, double* A, double* Bm, double* ee) {
-  if (!ctx || B < 0 || !x || !u || !f || !A || !Bm) return HB_EINVAL;
-  if (B == 0) return HB_OK;
-  if (B > ctx->cfg.max_batch) return HB_ECAP;
-  if (set_device(ctx)) return HB_ECUDA;
+  ENTER(ctx, B, x && u && f && A && Bm, CAPPED);
   Staging s(ctx, B);
   auto dx = s.in(x, NX); auto du = s.in(u, NU);
   auto df = s.out(f, NX); auto dA = s.out(A, TS); auto dB = s.out(Bm, TS); auto dee = s.out(ee, 24 + 36 * NX);
-  return s.run([&] { return hb_probe_flow_map_dev(ctx, B, dx, du, df, dA, dB, dee); });
+  return s.run(1, [&](Chunk) { return hb_probe_flow_map_dev(ctx, B, dx, du, df, dA, dB, dee); });
 }
 
 }  // extern "C"
