@@ -36,7 +36,7 @@ EXPORTED_SYMBOLS = [
     "hb_resident_wbc_batch_dev", "hb_resident_wbc_batch",
     "hb_time_grid_batch_dev", "hb_reference_expand_grid_batch_dev", "hb_mpc_solve_grid_batch_dev", "hb_policy_eval_grid_batch_dev",
     "hb_time_grid_batch", "hb_reference_expand_grid_batch", "hb_mpc_solve_grid_batch", "hb_resident_read_grid_batch", "hb_resident_write_batch",
-    "hb_default_rollout_params", "hb_rollout_batch_dev",
+    "hb_default_rollout_params", "hb_rollout_batch_dev", "hb_rollout_set_pushes", "hb_sim_step_wrench",
     "hb_default_estimation_params", "hb_estimation_reset", "hb_sim_read_sensors_batch_dev", "hb_sim_read_sensors", "hb_rollout_estimated_batch_dev",
 ]
 
@@ -220,6 +220,44 @@ def make_rollout_commands(gait, gait_start, cmd_times, cmd_vels):
             for k in range(4):
                 c.cmd_vel[j][k] = vel[i, j, k]
     return cmds
+
+
+HB_MAX_PUSHES = 4
+
+
+class HbPushSchedule(C.Structure):
+    _fields_ = [("n_push", C.c_int32), ("t_start", C.c_double * HB_MAX_PUSHES), ("duration", C.c_double * HB_MAX_PUSHES),
+                ("force", (C.c_double * 3) * HB_MAX_PUSHES), ("torque", (C.c_double * 3) * HB_MAX_PUSHES)]
+
+
+def make_push_schedules(B, t_start, duration, force, torque=None):
+    """ctypes array of B HbPushSchedule (Context.set_pushes). Push j of instance i acts on the plant steps of the ticks with
+    t_start[i, j] <= t < t_start[i, j] + duration[i, j]: a world force[i, j] [N] at the base origin plus a world couple torque[i, j] [N m]
+    (None: zero). t_start / duration: (B, n), (n,) or scalars; force / torque: (B, n, 3), (n, 3) or (3,); n <= HB_MAX_PUSHES."""
+    tim, dur, frc = _f64(t_start), _f64(duration), _f64(force)
+    trq = np.zeros(3) if torque is None else _f64(torque)
+    dims = [a.shape[-1] for a in (tim, dur) if a.ndim >= 1] + [a.shape[-2] for a in (frc, trq) if a.ndim >= 2]
+    n = max(dims) if dims else 1
+    if not 0 <= n <= HB_MAX_PUSHES:
+        raise ValueError("push schedules: at most %d pushes per instance, got %d" % (HB_MAX_PUSHES, n))
+    try:
+        tim = np.broadcast_to(tim, (B, n)); dur = np.broadcast_to(dur, (B, n))
+        frc = np.broadcast_to(frc, (B, n, 3)); trq = np.broadcast_to(trq, (B, n, 3))
+    except ValueError as e:
+        raise ValueError("push schedules: t_start / duration (B, n), force / torque (B, n, 3) expected: %s" % e)
+    if not (np.isfinite(tim).all() and np.isfinite(frc).all() and np.isfinite(trq).all()):
+        raise ValueError("push schedules: t_start, force and torque must be finite")
+    if not (np.isfinite(dur).all() and (dur >= 0).all()):
+        raise ValueError("push schedules: durations must be finite and >= 0")
+    out = (HbPushSchedule * B)()
+    for i in range(B):
+        s = out[i]
+        s.n_push = n
+        for j in range(n):
+            s.t_start[j] = tim[i, j]; s.duration[j] = dur[i, j]
+            for k in range(3):
+                s.force[j][k] = frc[i, j, k]; s.torque[j][k] = trq[i, j, k]
+    return out
 
 
 class HbObserverState(C.Structure):
@@ -650,13 +688,26 @@ class Context:
         _check(self._lib.hb_actuation_batch(self._h, B, C.c_double(delay), _ptr(time), state, _ptr(command), _ptr(rbd), _ptr(tau)), "hb_actuation_batch", self._h)
         return tau
 
-    def sim_step(self, rbd, tau, params=None):
-        """One control period of the batched rigid-body plant: returns (rbd_next [B,32], contact_force [B,12], contact_flag [B,4])."""
+    def sim_step(self, rbd, tau, params=None, wrench=None):
+        """One control period of the batched rigid-body plant: returns (rbd_next [B,32], contact_force [B,12], contact_flag [B,4]).
+        wrench [B,6] (hb_sim_step_wrench): an external world force at the base origin, then a world couple, held over the period."""
         rbd = _f64(rbd).copy(); tau = _f64(tau); B = rbd.shape[0]
         params = params or default_sim_params()
         cf = np.zeros((B, 12)); fl = np.zeros((B, 4), dtype=np.uint8)
-        _check(self._lib.hb_sim_step_batch(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(cf), _ptr(fl)), "hb_sim_step_batch", self._h)
+        if wrench is None:
+            _check(self._lib.hb_sim_step_batch(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(cf), _ptr(fl)), "hb_sim_step_batch", self._h)
+        else:
+            w = _f64(wrench).reshape(B, 6)
+            _check(self._lib.hb_sim_step_wrench(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), _ptr(cf), _ptr(fl)), "hb_sim_step_wrench", self._h)
         return rbd, cf, fl
+
+    def set_pushes(self, schedules):
+        """Push schedules of this context's episodes (hb_rollout_set_pushes): schedules[i] (make_push_schedules) acts on instance i of every
+        later rollout / rollout_estimated call, instances beyond len(schedules) are not pushed; None clears them."""
+        if schedules is None:
+            _check(self._lib.hb_rollout_set_pushes(self._h, 0, None), "hb_rollout_set_pushes", self._h)
+        else:
+            _check(self._lib.hb_rollout_set_pushes(self._h, len(schedules), schedules), "hb_rollout_set_pushes", self._h)
 
     def resident_wbc(self, t_now, rbd, stance_mode=None):
         """Policy of the resident solution at absolute time t_now + WeightedWbc: returns (x_des, u_des, mode, sol, torque, status)."""

@@ -68,6 +68,12 @@ struct hb_ctx {
   void* re_mem;
   double *re_quat, *re_gyro, *re_acc, *re_jpos, *re_jvel, *re_rbd;
   uint8_t* re_flag;
+  // push schedules of the episodes (hb_rollout_set_pushes): the first push_n instances have one, the device copy and the tick's wrench
+  // (B x 6) are allocated at max_batch by the first call that sets them; push_host keeps the validated array the copy reads
+  void* push_mem;
+  hb_push_schedule* push_sched; double* push_wrench;
+  int push_n;
+  std::vector<hb_push_schedule> push_host;
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
   // hb_resident_cycle_batch's packed references / reference verdicts
   void* arena; size_t arena_cap;
@@ -404,7 +410,8 @@ int hb_destroy(hb_ctx* ctx) {
   cudaSetDevice(ctx->device);
   void* ptrs[] = {ctx->sqp_mem, ctx->dxt, ctx->dut, ctx->perf, ctx->flags, ctx->xdes, ctx->udes, ctx->wstatus, ctx->witers, ctx->wmode,
                   ctx->hoqp_mem, ctx->cyc_xref, ctx->cyc_swing, ctx->cyc_tk, ctx->cyc_mode, ctx->cyc_nn, ctx->res_t0, ctx->res_xt,
-                  ctx->res_ut, ctx->res_tk, ctx->res_mode, ctx->res_nn, ctx->res_sol, ctx->res_stance, ctx->arena, ctx->ro_mem, ctx->re_mem};
+                  ctx->res_ut, ctx->res_tk, ctx->res_mode, ctx->res_nn, ctx->res_sol, ctx->res_stance, ctx->arena, ctx->ro_mem, ctx->re_mem,
+                  ctx->push_mem};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -848,9 +855,15 @@ int hb_actuation_batch_dev(hb_ctx* ctx, int B, double delay, const double* time,
   return launch(ctx, K_UNPROFILED, actuation_kernel, (B + 63) / 64, 64, 0, B, delay, time, state, command, rbd, tau);
 }
 
+// the plant step after the entry checks; wrench (B x 6) nullable
+static int sim_step(hb_ctx* ctx, int B, const hb_sim_params& params, double* rbd, const double* tau, const double* wrench, double* contact_force,
+                    uint8_t* contact_flag) {
+  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, params, rbd, tau, wrench, contact_force, contact_flag);
+}
+
 int hb_sim_step_batch_dev(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {
   ENTER(ctx, B, params && rbd && tau && sim_params_ok(*params), UNCAPPED);
-  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, *params, rbd, tau, contact_force, contact_flag);
+  return sim_step(ctx, B, *params, rbd, tau, nullptr, contact_force, contact_flag);
 }
 
 // hb_resident_wbc_batch_dev; no_prev = true: the fallback has no previous solution yet (first tick after a cold start whose cycle ran no WBC)
@@ -910,6 +923,40 @@ static int estimation_reserve(hb_ctx* ctx) {
   });
 }
 
+// the episodes' push schedules and the tick's wrench, at max_batch
+static int push_reserve(hb_ctx* ctx) {
+  const size_t Bc = ctx->cfg.max_batch;
+  return reserve_group(&ctx->push_mem, [&](void* m) {
+    size_t off = 0;
+    ctx->push_sched = carve<hb_push_schedule>(m, off, Bc); ctx->push_wrench = carve<double>(m, off, Bc * 6);
+    return off;
+  });
+}
+
+static bool push_schedule_ok(const hb_push_schedule& s) {
+  if (s.n_push < 0 || s.n_push > HB_MAX_PUSHES) return false;
+  for (int j = 0; j < s.n_push; ++j) {
+    if (!isfinite(s.t_start[j]) || !isfinite(s.duration[j]) || !(s.duration[j] >= 0.0)) return false;
+    for (int c = 0; c < 3; ++c) if (!isfinite(s.force[j][c]) || !isfinite(s.torque[j][c])) return false;
+  }
+  return true;
+}
+
+int hb_rollout_set_pushes(hb_ctx* ctx, int B, const hb_push_schedule* pushes) {
+  const int rc = enter(ctx, B, B == 0 || pushes, CAPPED, [&] {
+    for (int i = 0; i < B; ++i) if (!push_schedule_ok(pushes[i])) return false;
+    return true;
+  });
+  if (rc == EMPTY) { ctx->push_n = 0; return HB_OK; }     // cleared: the episodes run without a wrench
+  if (rc) return rc;
+  if (int e = push_reserve(ctx)) return e;
+  // a pageable copy the context owns: cudaMemcpyAsync has consumed it when it returns, whatever memory the caller's array is in
+  try { ctx->push_host.assign(pushes, pushes + B); } catch (const std::bad_alloc&) { return HB_ENOMEM; }
+  CK(cudaMemcpyAsync(ctx->push_sched, ctx->push_host.data(), sizeof(hb_push_schedule) * B, cudaMemcpyHostToDevice, ctx->stream));
+  ctx->push_n = B;
+  return HB_OK;
+}
+
 // the estimation arguments of an estimated episode; a null pointer to them is hb_rollout_batch_dev
 struct EstimationArgs {
   const hb_estimation_params* ep;
@@ -943,13 +990,15 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   const unsigned grid = (B + 63) / 64;
   // what the controllers measure: the true state, or the filter's estimate
   double* meas = e ? ctx->re_rbd : rbd;
+  // the push wrench the begin kernel writes and the plant applies; none without schedules
+  double* wrench = ctx->push_n > 0 ? ctx->push_wrench : nullptr;
   for (int k = 0; k < n_ticks && !rc; ++k) {
     const int64_t a = tick0 + k;
     const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
     const bool mpc = a % p->mpc_every == 0, first_cold = cold && k == 0;
     double* log_row = (n_log && k % p->log_every == 0) ? log + (size_t)(k / p->log_every) * 32 : nullptr;
     rc = launch(ctx, K_UNPROFILED, rollout_tick_begin_kernel, grid, 64, 0, B, (int)a, t, p->min_base_height, rbd, ctx->ro_held, stats, ctx->ro_tnow,
-                log_row, (size_t)n_log * 32);
+                log_row, (size_t)n_log * 32, ctx->push_sched, ctx->push_n, wrench);
     if (!rc && e) {
       // LeggedController::updateStateEstimation: sensors and contact flags at the previous observation's time, filter, observation step
       double* est_row = (n_est_log && k % p->log_every == 0) ? e->log + (size_t)(k / p->log_every) * 32 : nullptr;
@@ -973,7 +1022,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
                                              ctx->ro_jtau);
     if (!rc) rc = hb_actuation_batch_dev(ctx, B, p->actuation_delay, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, ctx->ro_tau);
-    if (!rc) rc = hb_sim_step_batch_dev(ctx, B, &p->sim, rbd, ctx->ro_tau, nullptr, nullptr);
+    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, nullptr, nullptr);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_tick_end_kernel, grid, 64, 0, B, (int)a, mpc ? 1 : 0, ctx->ro_info, ctx->ro_pstat, ctx->wstatus, estop, ctx->ro_tau, ctx->ro_held, rbd, stats);
   }
   return rc;
@@ -1381,6 +1430,14 @@ int hb_sim_step_batch(hb_ctx* ctx, int B, const hb_sim_params* params, double* r
   Staging s(ctx, B);
   auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
   return s.run(1, [&](Chunk) { return hb_sim_step_batch_dev(ctx, B, params, r, t, cf, fl); });
+}
+
+int hb_sim_step_wrench(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench, double* contact_force,
+                       uint8_t* contact_flag) {
+  ENTER(ctx, B, params && rbd && tau, CAPPED, [&] { return sim_params_ok(*params); });
+  Staging s(ctx, B);
+  auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto w = s.in_or_null(wrench, 6); auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
+  return s.run(1, [&](Chunk) { return sim_step(ctx, B, *params, r, t, w, cf, fl); });
 }
 
 int hb_resident_wbc_batch(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,

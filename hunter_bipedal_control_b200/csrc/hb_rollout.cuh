@@ -39,12 +39,24 @@ __device__ __forceinline__ int rollout_state_check(const double* r, double min_b
   return why;
 }
 
+// The world wrench (force, couple) the push schedule s puts on the plant step of the tick at time t: the active pushes added in ascending j
+// to zeros, so that a host restatement reproduces it bit for bit
+__device__ __forceinline__ void push_wrench(const hb_push_schedule& s, double t, double* w) {
+  for (int c = 0; c < 6; ++c) w[c] = 0.0;
+  for (int j = 0; j < s.n_push; ++j) {
+    if (!(s.t_start[j] <= t && t < s.t_start[j] + s.duration[j])) continue;
+    for (int c = 0; c < 3; ++c) { w[c] += s.force[j][c]; w[3 + c] += s.torque[j][c]; }
+  }
+}
+
 // Start of tick `tick` (absolute): the state entering it is checked (an instance that fails is held from this tick on), `held` takes the
 // state every held instance is put back to, the tick time goes to every instance (policy evaluation, actuation stamp), and the state is
 // logged when log_row is set. A non-finite state can only enter the first tick of a call (the end kernel never leaves one behind); with no
-// finite state of that instance known, the nominal standing pose replaces it.
+// finite state of that instance known, the nominal standing pose replaces it. With wrench set, the tick's push wrench (B x 6) is written
+// for the plant step: from pushes[inst] for inst < n_pushes, zeros for the others.
 __global__ void rollout_tick_begin_kernel(int B, int tick, double t, double min_base_height, double* rbd, double* held, hb_rollout_stats* stats,
-                                          double* t_now, double* log_row, size_t log_stride) {
+                                          double* t_now, double* log_row, size_t log_stride, const hb_push_schedule* pushes, int n_pushes,
+                                          double* wrench) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
   double* r = rbd + (size_t)inst * 32;
@@ -61,6 +73,11 @@ __global__ void rollout_tick_begin_kernel(int B, int tick, double t, double min_
   for (int i = 0; i < 32; ++i) h[i] = r[i];
   t_now[inst] = t;
   if (log_row) for (int i = 0; i < 32; ++i) log_row[inst * log_stride + i] = r[i];
+  if (wrench) {
+    double* w = wrench + (size_t)inst * 6;
+    if (inst < n_pushes) push_wrench(pushes[inst], t, w);
+    else for (int c = 0; c < 6; ++c) w[c] = 0.0;
+  }
 }
 
 // actuator saturation of the applied torques (B x 10); NaN passes through as in numpy.clip
@@ -292,9 +309,12 @@ __global__ void actuation_kernel(int B, double delay, const double* time, hb_act
 // closed loop, legged_gazebo / legged_mujoco): forward dynamics M(q) qdd = S' tau + J_c' F_c - nle with compliant point contacts at the four
 // contact frames (normal spring-damper, viscous tangential friction clipped to the cone), semi-implicit Euler over `substeps` substeps.
 // Same rigid-body passes as the WBC assembly: lanes 0-15 unit-velocity sweeps -> J_c columns, lanes 0-15 RNEA with unit accelerations ->
-// M columns, lane 16 -> nle; 16 x 16 Cholesky in shared memory. One warp per instance.
+// M columns, lane 16 -> nle; 16 x 16 Cholesky in shared memory. One warp per instance. wrench (B x 6, nullable): an external world force at
+// the base origin and a world couple, which enter as the generalised forces Q_p = f, Q_zyx = T' tau with omega_world = T(zyx) zyx_dot (the
+// map of the world angular velocity written back below); null adds nothing.
 struct SimShared { double q[NQ], v[NQ], J[12 * NQ], M[NQ * 17], nle[NQ], rhs[NQ], t1[NQ], t2[NQ], kdi[NQ], F[12], cpos[12], cvel[12]; };
-__global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, double* rbd_io, const double* tau, double* contact_force, uint8_t* contact_flag) {
+__global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, double* rbd_io, const double* tau, const double* wrench, double* contact_force,
+                                                      uint8_t* contact_flag) {
   __shared__ SimShared sh;
   const int inst = blockIdx.x, lane = threadIdx.x;
   double* r = rbd_io + (size_t)inst * 32;
@@ -345,6 +365,15 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
       // viscous joint damping
       double s = -sh.nle[lane] + (lane >= 6 ? tau[(size_t)inst * NJ + lane - 6] - prm.joint_damping * sh.v[lane] : 0.0);
       for (int rr = 0; rr < 12; ++rr) s += sh.J[rr * NQ + lane] * sh.F[rr];
+      if (wrench && lane < 6) {
+        const double* w = wrench + (size_t)inst * 6;
+        if (lane < 3) s += w[lane];
+        else {
+          double sz, cz, sy, cy;
+          sincos(sh.q[3], &sz, &cz); sincos(sh.q[4], &sy, &cy);
+          s += lane == 3 ? w[5] : (lane == 4 ? -sz * w[3] + cz * w[4] : cz * cy * w[3] + sz * cy * w[4] - sy * w[5]);   // yaw, pitch, roll
+        }
+      }
       sh.rhs[lane] = s;
       if (lane >= 6) sh.M[lane * 17 + lane] += prm.joint_armature;
       for (int j = lane + 1; j < NQ; ++j) { const double a = 0.5 * (sh.M[lane * 17 + j] + sh.M[j * 17 + lane]); sh.M[j * 17 + lane] = a; }   // lower triangle, symmetrised

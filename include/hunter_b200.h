@@ -232,6 +232,30 @@ typedef struct {                 /* per-instance outcome, in/out: start an episo
 } hb_rollout_stats;
 int hb_default_rollout_params(hb_rollout_params* p);       /* host only */
 
+/* ---- pushed episodes: scheduled external wrenches on the base, applied by the plant of both episode calls ----
+ * Push j acts on the plant step of absolute tick a iff t_start[j] <= t && t < t_start[j] + duration[j], with t = (double)a * period (the
+ * episode's tick time). During that step the wrench is constant over all substeps, so a push is quantised to whole ticks. Overlapping
+ * pushes add up: each of the 6 wrench components starts from 0.0 and the active pushes are added in ascending j. A world force f at the
+ * base frame origin (rbd[3:6]) and a world couple tau enter the plant as generalised forces on the base coordinates (p, zyx): Q_p = f and
+ * Q_zyx = T' tau, where omega_world = T(zyx) (dyaw, dpitch, droll) is the map behind rbd[16:19], i.e. Q_yaw = tau_z,
+ * Q_pitch = -sz tau_x + cz tau_y, Q_roll = cz cy tau_x + sz cy tau_y - sy tau_z, evaluated at each substep's orientation. A push on
+ * another point r of the body is the force f plus the couple r x f. The controllers are not told about the push. */
+#define HB_MAX_PUSHES 4
+typedef struct {                      /* external pushes on one robot's base                                                  */
+  int32_t n_push;                     /* 0..HB_MAX_PUSHES; 0 = undisturbed                                                    */
+  double t_start[HB_MAX_PUSHES];      /* absolute time [s]                                                                    */
+  double duration[HB_MAX_PUSHES];     /* [s], >= 0                                                                            */
+  double force[HB_MAX_PUSHES][3];     /* world frame [N], applied at the base frame origin (rbd[3:6])                         */
+  double torque[HB_MAX_PUSHES][3];    /* world frame couple [N m]                                                             */
+} hb_push_schedule;
+/* Sets the push schedules of the context's episodes: from then on both episode calls apply pushes[i] to instance i of their batch for i < B;
+ * instances at or beyond B get no push. B == 0 clears them (pushes may be NULL). pushes is a host array, validated on the host and copied
+ * to the context in stream order on the context's stream; the caller may free it when the call returns. -1: B < 0, NULL pushes with B > 0,
+ * n_push outside 0..HB_MAX_PUSHES, a non-finite t_start / force / torque, a negative or non-finite duration; -4: B > max_batch. A rejected
+ * call keeps the previous setting and enqueues nothing. The device copy is allocated at max_batch by the first call that sets pushes and
+ * freed by hb_destroy. Pushes add no launch to an episode. */
+int hb_rollout_set_pushes(hb_ctx* ctx, int B, const hb_push_schedule* pushes);
+
 /* ---- estimated episodes (hb_rollout_estimated_batch_dev): the controllers read the Kalman filter's estimate from synthesised, noisy
  * sensors instead of the plant's true state (LeggedController::updateStateEstimation, LeggedController.cpp:280-349) ---- */
 typedef struct {                 /* standard deviations of additive Gaussian sensor noise; 0 = that channel is exact and draws nothing */
@@ -382,7 +406,7 @@ int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const dou
  * horizon = time_to_target = horizon_N * dt or, for event_nodes contexts, the time horizon, prev_event = min(t, gait_start) - 0.5, IK
  * joint references), device planner, resident cycle without its WBC (cold start iff tick0 == 0). Every tick then runs
  * hb_resident_wbc_batch's policy + WeightedWbc at t, the joint command law (loaded, walking branch), the actuation model, saturation to
- * +-torque_limit and one plant step. Failure checks run on the state entering each tick (finite, |roll| <= pi/2, base height) and on the
+ * +-torque_limit and one plant step (with the tick's push wrench when hb_rollout_set_pushes has set schedules). Failure checks run on the state entering each tick (finite, |roll| <= pi/2, base height) and on the
  * emergency stop the joint command raises; from its first failure on an instance is held (rbd put back to its last finite state after
  * every plant step; a non-finite state entering the first tick of a call is replaced by the nominal standing pose) and its outputs no
  * longer count in stats. rbd (B x 32), act, estop (B) and stats are device memory, in/out. cmd (B) is a host array, validated and copied
@@ -480,6 +504,11 @@ int hb_actuation_batch(hb_ctx* ctx, int B, double delay, const double* time, hb_
                        double* tau);
 int hb_sim_step_batch(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force /*nullable*/,
                       uint8_t* contact_flag /*nullable*/);
+/* hb_sim_step_batch with an external world wrench on each robot's base: wrench (B x 6) = force [N] at the base frame origin, then a couple
+ * [N m], both in the world frame and constant over the step (generalised forces as for pushed episodes, above). NULL wrench is exactly
+ * hb_sim_step_batch. */
+int hb_sim_step_wrench(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench /*nullable*/,
+                       double* contact_force /*nullable*/, uint8_t* contact_flag /*nullable*/);
 int hb_resident_wbc_batch(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode /*nullable*/, double* x_des, double* u_des,
                           int32_t* mode_out, double* wbc_sol, double* torque /*nullable*/, int32_t* wbc_status /*nullable*/);
 int hb_rbd_to_centroidal_batch(hb_ctx* ctx, int B, const double* rbd, double* x);

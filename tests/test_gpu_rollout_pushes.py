@@ -1,0 +1,471 @@
+"""Pushed episodes (hb_rollout_set_pushes, hb_sim_step_wrench): scheduled external wrenches on the base, applied by the plant of both episode
+calls. The plant step with a wrench is checked against a numpy restatement and against momentum balance in free flight; the pushed episode
+bit for bit against the loop of public calls with the documented wrench restated in numpy, and against the unpushed episode: causality,
+null schedules, continuation, independence, permutation, instances beyond the schedules, estimated episodes; then the argument checks."""
+import ctypes as C
+
+import numpy as np
+import pytest
+
+import hunter_bipedal_control_b200 as hb
+from hunter_bipedal_control_b200 import scenarios as sc
+from test_gpu_rollout_episodes import (CMD_TIMES, GAIT_START, GAITS, _assert_stats_equal, _cmd_vels, _context, _device, _params, _start_states,
+                                       _stepwise)
+from test_gpu_rollout_estimation import _assert_est_equal, _assert_est_stats_equal, _est_params
+from test_gpu_rollout_estimation import _device as _est_device
+from test_gpu_rollout_estimation import _stepwise as _est_stepwise
+
+pytestmark = pytest.mark.gpu
+
+
+def _torch():
+    import torch
+    return torch
+
+
+def _T(zyx):
+    """omega_world = T(zyx) (yaw, pitch, roll rates): the columns are the world axes of the three rotations."""
+    sz, cz, sy, cy = np.sin(zyx[0]), np.cos(zyx[0]), np.sin(zyx[1]), np.cos(zyx[1])
+    return np.array([[0.0, -sz, cz * cy], [0.0, cz, sz * cy], [1.0, 0.0, -sy]])
+
+
+def _plant_numpy(oracle, rbd, tau, prm, wrench):
+    """test_gpu_rollout._plant_numpy with the external wrench: Q_p = f, Q_zyx = T' tau at each substep's orientation."""
+    from oracle import refs
+    q = np.concatenate([rbd[3:6], rbd[0:3], rbd[6:16]])
+    v = np.concatenate([rbd[19:22], refs.euler_rates_from_global(rbd[0:3], rbd[16:19]), rbd[22:32]])
+    h = prm.dt / prm.substeps
+    F = np.zeros(12)
+    for _ in range(prm.substeps):
+        r = oracle.rbd(q, v)
+        cvel = r["J"] @ v
+        F = np.zeros(12)
+        for c in range(4):
+            depth = prm.ground_height - r["cpos"][3 * c + 2]
+            if depth > 0:
+                fz = max(0.0, prm.ground_stiffness * depth - prm.ground_damping * cvel[3 * c + 2])
+                ft = -prm.tangential_damping * cvel[3 * c:3 * c + 2]
+                n = np.linalg.norm(ft)
+                if n > prm.friction_mu * fz:
+                    ft = ft * (prm.friction_mu * fz / n if n > 0 else 0.0)
+                F[3 * c:3 * c + 3] = [ft[0], ft[1], fz]
+        Q = np.concatenate([wrench[:3], _T(q[3:6]).T @ wrench[3:], np.zeros(10)])
+        rhs = np.concatenate([np.zeros(6), tau - prm.joint_damping * v[6:]]) + r["J"].T @ F - r["nle"] + Q
+        qdd = np.linalg.solve(r["M"] + np.diag(np.r_[np.zeros(6), np.full(10, prm.joint_armature)]), rhs)
+        v = v + h * qdd
+        q = q + h * v
+    out = np.zeros(32)
+    out[0:3] = q[3:6]; out[3:6] = q[0:3]; out[6:16] = q[6:]
+    out[16:19] = refs.global_from_euler_rates(q[3:6], v[3:6]); out[19:22] = v[0:3]; out[22:32] = v[6:]
+    return out, F
+
+
+def _wrench_numpy(pushes, t, B):
+    """The documented wrench of the tick at time t: zeros, plus every active push in ascending j (B x 6; instances without a schedule: 0)."""
+    w = np.zeros((B, 6))
+    for i in range(min(B, len(pushes))):
+        s = pushes[i]
+        for j in range(s.n_push):
+            if s.t_start[j] <= t and t < s.t_start[j] + s.duration[j]:
+                for c in range(3):
+                    w[i, c] += s.force[j][c]; w[i, 3 + c] += s.torque[j][c]
+    return w
+
+
+class _PushedPlant:
+    """A context for the stepwise loops of the episode tests whose plant step applies the push wrench of the tick it advances: those loops
+    call sim_step once per tick, in tick order from tick0."""
+
+    def __init__(self, ctx, pushes, period, tick0=0):
+        self._ctx, self._pushes, self._period, self._tick = ctx, pushes, period, tick0
+        self.steps = 0
+
+    def __getattr__(self, name):
+        return getattr(self._ctx, name)
+
+    def sim_step(self, rbd, tau, params=None):
+        t = self._tick * self._period
+        self._tick += 1
+        self.steps += 1
+        return self._ctx.sim_step(rbd, tau, params, wrench=_wrench_numpy(self._pushes, t, rbd.shape[0]))
+
+
+def _schedules():
+    """Six instances: one push; two overlapping pushes; a push starting between ticks in mid-episode, with a couple; none; one after the
+    episode; three pushes (from t = 0, one of zero duration, a couple only)."""
+    S = (hb.HbPushSchedule * 6)()
+    spec = [
+        [(0.05, 0.1, (60.0, 0.0, 0.0), (0.0, 0.0, 0.0))],
+        [(0.1, 0.08, (0.0, -50.0, 0.0), (0.0, 0.0, 0.0)), (0.14, 0.1, (20.0, 10.0, 0.0), (0.0, 0.0, 5.0))],
+        [(0.2031, 0.05, (-40.0, 30.0, 10.0), (2.0, -3.0, 1.0))],
+        [],
+        [(1.0, 0.1, (100.0, 0.0, 0.0), (0.0, 0.0, 0.0))],
+        [(0.0, 0.02, (0.0, 40.0, 0.0), (0.0, 0.0, 0.0)), (0.1, 0.0, (500.0, 0.0, 0.0), (0.0, 0.0, 0.0)), (0.3, 0.05, (0.0, 0.0, 0.0), (-3.0, 4.0, 0.0))],
+    ]
+    for s, pushes in zip(S, spec):
+        s.n_push = len(pushes)
+        for j, (t0, d, f, tq) in enumerate(pushes):
+            s.t_start[j] = t0; s.duration[j] = d
+            for c in range(3):
+                s.force[j][c] = f[c]; s.torque[j][c] = tq[c]
+    return S
+
+
+def _one_push(B, i, t_start, duration, force, torque=(0.0, 0.0, 0.0)):
+    """B schedules, only instance i pushed."""
+    return hb.make_push_schedules(B, np.where(np.arange(B) == i, t_start, 0.0)[:, None], np.where(np.arange(B) == i, duration, 0.0)[:, None],
+                                  np.where((np.arange(B) == i)[:, None, None], np.array(force, dtype=float)[None, None], 0.0),
+                                  np.where((np.arange(B) == i)[:, None, None], np.array(torque, dtype=float)[None, None], 0.0))
+
+
+def _np(out):
+    return [o.cpu().numpy() if hasattr(o, "cpu") else o for o in out]
+
+
+def _assert_episode_equal(a, b, estimated=False, B=None):
+    a, b = _np(a), _np(b)
+    for k in (0, 1, 2, 4):
+        assert np.array_equal(a[k], b[k]), k
+    _assert_stats_equal(a[3], b[3])
+    if estimated:
+        _assert_est_equal(a[5], b[5], B)
+        _assert_est_stats_equal(a[6], b[6])
+        assert np.array_equal(a[7], b[7])
+
+
+# ---------------------------------------------------------------------------------------------------------------- the plant step
+def test_plant_step_with_wrench_matches_numpy_restatement(gpu_ctx, oracle):
+    B = 10
+    rng = np.random.default_rng(8)
+    x = sc.random_initial_states(B, seed=50)
+    rbd = sc.consistent_rbd(x, rng, 0.02)
+    rbd[:, 5] = rng.uniform(0.60, 0.64, B)               # some feet in the ground, some above it
+    rbd[:, 1] = rng.uniform(-0.3, 0.3, B); rbd[:, 2] = rng.uniform(-0.3, 0.3, B)    # pitch and roll, so that T is not a permutation
+    tau = rng.uniform(-15, 15, (B, 10))
+    W = np.c_[rng.uniform(-300, 300, (B, 3)), rng.uniform(-60, 60, (B, 3))]
+    prm = hb.default_sim_params()
+    nxt, cf, fl = gpu_ctx.sim_step(rbd, tau, prm, wrench=W)
+    base = gpu_ctx.sim_step(rbd, tau, prm)
+    touched = 0
+    for i in range(B):
+        ref, F = _plant_numpy(oracle, rbd[i], tau[i], prm, W[i])
+        assert np.abs(nxt[i] - ref).max() < 1e-9 * max(1.0, np.abs(ref).max()), i
+        assert np.abs(cf[i] - F).max() < 1e-7 * max(1.0, np.abs(F).max())
+        assert np.array_equal(fl[i] != 0, F[2::3] > 0)
+        touched += int((F[2::3] > 0).sum())
+        assert np.abs(nxt[i] - base[0][i]).max() > 1e-6          # the wrench acts
+    assert 0 < touched < 4 * B
+    # no wrench and an all-zero wrench are the plant step of hb_sim_step_batch, bit for bit
+    zero = gpu_ctx.sim_step(rbd, tau, prm, wrench=np.zeros((B, 6)))
+    r = rbd.copy(); cfn = np.zeros((B, 12)); fln = np.zeros((B, 4), dtype=np.uint8)
+    assert gpu_ctx._lib.hb_sim_step_wrench(gpu_ctx._h, B, C.byref(prm), C.c_void_p(r.ctypes.data), C.c_void_p(tau.ctypes.data), None,
+                                           C.c_void_p(cfn.ctypes.data), C.c_void_p(fln.ctypes.data)) == 0
+    for got in (zero, (r, cfn, fln)):
+        for a, b in zip(got, base):
+            assert np.array_equal(a, b)
+
+
+@pytest.mark.parametrize("kind", ["force", "couple"])
+def test_free_flight_momentum_balance(gpu_ctx, kind):
+    """Free flight (ground far below), zero joint torques, armature and joint damping: over T = 50 ticks the centroidal momentum
+    (rbd_to_centroidal, normalised momentum x TOTAL_MASS) changes by (F + m g) T for a force at the base origin and by (m g T, tau T) for a
+    pure couple tau. Independent of the numpy restatement: a wrong sign or a transposed T fails here.
+    Tolerance: semi-implicit Euler updates v with M(q_n) and then moves q, so each substep changes the momentum A(q) v by h Q_ext + O(h^2),
+    and over T / h substeps the error is O(h T). With the legs swinging freely (joint rates reach ~ 17 rad/s) it is ~ 0.08 N s at
+    4 substeps, so the test runs 4 and 16 substeps: the error must shrink about 4x (first order), and the Richardson extrapolation
+    (4 e_16 - e_4) / 3, which cancels the O(h) term, must be below 2e-3 N s (N m s), against changes of 0.4 .. 8 N s. A wrong sign or a
+    transposed T leaves an O(1) error that does not shrink with h."""
+    B = 3
+    rng = np.random.default_rng(21)
+    rbd = sc.consistent_rbd(sc.random_initial_states(B, seed=7))
+    rbd[:, 0:3] = [[0.7, 0.3, -0.2], [-1.2, -0.25, 0.35], [2.5, 0.1, 0.5]]   # yaw, pitch, roll away from the identity
+    rbd[:, 16:] = 0.0
+    m, g = sc.TOTAL_MASS, np.array([0.0, 0.0, -9.81])
+    if kind == "force":
+        W = np.c_[rng.uniform(-80, 80, (B, 3)), np.zeros((B, 3))]
+    else:
+        W = np.c_[np.zeros((B, 3)), rng.uniform(-8, 8, (B, 3))]
+    n = 50
+    err = {}
+    for substeps in (4, 16):
+        prm = hb.default_sim_params()
+        prm.ground_height = -100.0; prm.joint_armature = 0.0; prm.joint_damping = 0.0; prm.substeps = substeps
+        T = n * prm.dt
+        h0 = gpu_ctx.rbd_to_centroidal(rbd)[:, :6] * m
+        r = rbd.copy()
+        for _ in range(n):
+            r, _, fl = gpu_ctx.sim_step(r, np.zeros((B, 10)), prm, wrench=W)
+            assert (fl == 0).all()
+        dh = gpu_ctx.rbd_to_centroidal(r)[:, :6] * m - h0
+        want = np.c_[W[:, :3] * T + m * g * T, W[:, 3:] * T]
+        # a force at the base origin also has a moment about the CoM: only the linear momentum is checked then
+        err[substeps] = (dh - want)[:, :3] if kind == "force" else dh - want
+    e4, e16 = np.abs(err[4]).max(), np.abs(err[16]).max()
+    assert e16 < 0.3 * e4 + 1e-6, (e4, e16)
+    rich = (4 * err[16] - err[4]) / 3
+    assert np.abs(rich).max() < 2e-3, (rich, err)
+    assert np.abs(W).max() * T > 0.4
+
+
+# ---------------------------------------------------------------------------------------------------------------- pushed episodes
+@pytest.mark.parametrize("event_nodes", [False, True], ids=["uniform", "event_nodes"])
+def test_pushed_episode_equals_the_stepwise_loop_bitwise(event_nodes):
+    ctx = _context(event_nodes)
+    B, n_ticks, log_every = 6, 200, 10
+    rbd0 = _start_states(ctx, B, seed=11)
+    vels = _cmd_vels(B)
+    prm = _params(log_every)
+    S = _schedules()
+    ctx.set_pushes(S)
+    d = _device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
+    plant = _PushedPlant(ctx, S, prm.period)
+    r = _stepwise(plant, rbd0, GAITS, vels, n_ticks, prm, log_every)
+    assert plant.steps == n_ticks
+    _assert_episode_equal(d, r)
+    ctx.set_pushes(None)
+    u = _device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
+    moved = [not np.array_equal(a, b) for a, b in zip(d[0].cpu().numpy(), u[0].cpu().numpy())]
+    assert moved == [True, True, True, False, False, True], moved
+    ctx.close()
+
+
+def test_state_before_the_push_is_unchanged_and_the_state_after_it_moves():
+    ctx = _context()
+    B, n_ticks = 6, 80
+    rbd0 = _start_states(ctx, B, seed=12)
+    vels = _cmd_vels(B)
+    prm = _params(1)
+    u = _np(_device(ctx, rbd0, GAITS, vels, n_ticks, prm, 1))
+    k = 50
+    ctx.set_pushes(_one_push(B, 0, k * prm.period, 0.02, (0.0, 80.0, 0.0)))
+    p = _np(_device(ctx, rbd0, GAITS, vels, n_ticks, prm, 1))
+    assert np.array_equal(p[4][:, :k + 1], u[4][:, :k + 1])          # log row k: the state entering the tick the push starts
+    assert not np.array_equal(p[4][0, k + 1], u[4][0, k + 1])
+    assert np.array_equal(p[4][1:], u[4][1:]) and np.array_equal(p[0][1:], u[0][1:])
+    ctx.close()
+
+
+def _null_schedule_checks(ctx, run, B, n_ticks, horizon_t):
+    """Every null setting reproduces the unset episode bit for bit with the same launches; a rejected set keeps the previous setting."""
+    def counted():
+        c0 = ctx.launch_count
+        out = run()
+        return out, ctx.launch_count - c0
+
+    ctx.set_pushes(None)
+    ref, launches = counted()
+    nothing = hb.make_push_schedules(B, np.zeros((B, 0)), np.zeros((B, 0)), np.zeros((B, 0, 3)))
+    later = hb.make_push_schedules(B, [horizon_t, horizon_t + 0.5], [0.1, 1.0], [[500.0, 0, 0], [0, 500.0, 0]], [[0, 0, 50.0], [0, 0, 0]])
+    for setting in (nothing, later, "clear"):
+        if setting == "clear":
+            ctx.set_pushes(_schedules()); ctx.set_pushes(None)
+        else:
+            ctx.set_pushes(setting)
+        out, n = counted()
+        assert n == launches, (setting, n, launches)
+        yield ref, out
+    pushed = _one_push(B, 1, 0.02, 0.06, (0.0, -70.0, 0.0), (0.0, 0.0, 4.0))
+    ctx.set_pushes(pushed)
+    want, n = counted()
+    assert n == launches
+    bad = _one_push(B, 1, 0.02, 0.06, (0.0, -70.0, 0.0))
+    bad[0].force[0][0] = float("nan")
+    with pytest.raises(hb.HunterB200Error):
+        ctx.set_pushes(bad)
+    assert ctx._lib.hb_rollout_set_pushes(ctx._h, ctx.max_batch + 1, _schedules()) == -4
+    got, _ = counted()
+    yield want, got
+    assert not np.array_equal(_np(want)[0], _np(ref)[0])
+
+
+def test_null_schedules_change_nothing():
+    ctx = _context()
+    B, n_ticks = 6, 100
+    rbd0 = _start_states(ctx, B, seed=13)
+    vels = _cmd_vels(B)
+    prm = _params(5)
+    for a, b in _null_schedule_checks(ctx, lambda: _device(ctx, rbd0, GAITS, vels, n_ticks, prm, 5), B, n_ticks, n_ticks * prm.period):
+        _assert_episode_equal(a, b)
+    ctx.close()
+
+
+def test_continuation_independence_permutation_and_unscheduled_instances():
+    ctx = _context()
+    B = 6
+    rbd0 = _start_states(ctx, B, seed=14)
+    vels = _cmd_vels(B)
+    prm = _params(10)
+    cmds = hb.make_rollout_commands(GAITS, GAIT_START, CMD_TIMES, vels)
+    # two calls split inside a push window (ticks 75..124, split at tick 100) equal one call
+    ctx.set_pushes(hb.make_push_schedules(B, 0.15, 0.1, np.linspace(-60, 60, B)[:, None, None] * np.array([1.0, 0.5, 0.0]), [0.0, 0.0, 3.0]))
+    one = _device(ctx, rbd0, GAITS, vels, 200, prm, 10)
+    h = _device(ctx, rbd0, GAITS, vels, 100, prm, 10)
+    two = ctx.rollout(h[0], cmds, 100, tick0=100, params=prm, act=h[1], estop=h[2], stats=h[3], log_every=10)
+    for k in (0, 1, 2):
+        assert np.array_equal(one[k].cpu().numpy(), two[k].cpu().numpy()), k
+    _assert_stats_equal(one[3], two[3])
+    assert np.array_equal(one[4].cpu().numpy(), np.concatenate([h[4].cpu().numpy(), two[4].cpu().numpy()], axis=1))
+    # pushing instance 0 only leaves every other instance as in the unpushed run
+    ctx.set_pushes(None)
+    u = _np(_device(ctx, rbd0, GAITS, vels, 200, prm, 10))
+    ctx.set_pushes(_one_push(B, 0, 0.1, 0.1, (70.0, -30.0, 0.0), (0.0, 2.0, 0.0)))
+    p = _np(_device(ctx, rbd0, GAITS, vels, 200, prm, 10))
+    assert not np.array_equal(p[0][0], u[0][0])
+    size = C.sizeof(hb.HbActuationState)
+    assert np.array_equal(p[0][1:], u[0][1:]) and np.array_equal(p[4][1:], u[4][1:])
+    assert np.array_equal(p[1].reshape(B, size)[1:], u[1].reshape(B, size)[1:]) and np.array_equal(p[2][1:], u[2][1:])
+    _assert_stats_equal(p[3][1:], u[3][1:])
+    # a permuted batch with permuted schedules gives the permuted result
+    S = _schedules()
+    ctx.set_pushes(S)
+    full = _np(_device(ctx, rbd0, GAITS, vels, 200, prm, 10))
+    perm = [4, 0, 5, 2, 1, 3]
+    Sp = (hb.HbPushSchedule * B)(*[S[i] for i in perm])
+    ctx.set_pushes(Sp)
+    q = _np(_device(ctx, rbd0[perm], [GAITS[i] for i in perm], vels[perm], 200, prm, 10))
+    assert np.array_equal(full[0][perm], q[0]) and np.array_equal(full[4][perm], q[4]) and np.array_equal(full[2][perm], q[2])
+    assert np.array_equal(full[1].reshape(B, size)[perm], q[1].reshape(B, size))
+    _assert_stats_equal(full[3][perm], q[3])
+    # schedules for the first 3 instances only: the others run unpushed, the first 3 as with the full setting
+    ctx.set_pushes(hb.make_push_schedules(3, 0.05, 0.2, [40.0, 40.0, 0.0]))
+    part = _np(_device(ctx, rbd0, GAITS, vels, 200, prm, 10))
+    padded = hb.make_push_schedules(B, 0.05, 0.2, [40.0, 40.0, 0.0])
+    for i in range(3, B):
+        padded[i].n_push = 0
+    ctx.set_pushes(padded)
+    full6 = _np(_device(ctx, rbd0, GAITS, vels, 200, prm, 10))
+    assert np.array_equal(part[0][3:], u[0][3:]) and np.array_equal(part[4][3:], u[4][3:])
+    assert np.array_equal(part[0], full6[0]) and np.array_equal(part[4], full6[4])
+    assert not np.array_equal(part[0][:3], u[0][:3])
+    ctx.close()
+
+
+# ---------------------------------------------------------------------------------------------------------------- estimated episodes
+def test_pushed_estimated_episode_equals_the_stepwise_loop_bitwise():
+    ctx = _context()
+    B, n_ticks, log_every = 6, 120, 10
+    rbd0 = _start_states(ctx, B, seed=11)
+    vels = _cmd_vels(B)
+    prm = _params(log_every)
+    ep = _est_params(seed=2024)
+    S = _schedules()
+    ctx.set_pushes(S)
+    d = _est_device(ctx, rbd0, GAITS, vels, n_ticks, prm, ep, hb.estimation_states(B, 40), log_every)
+    plant = _PushedPlant(ctx, S, prm.period)
+    r = _est_stepwise(plant, rbd0, GAITS, vels, n_ticks, prm, ep, hb.estimation_states(B, 40), log_every)
+    assert plant.steps == n_ticks
+    _assert_episode_equal(d, r, estimated=True, B=B)
+    ctx.close()
+
+
+def test_estimated_episodes_null_schedules_independence_and_continuation():
+    ctx = _context()
+    B, n_ticks = 6, 100
+    rbd0 = _start_states(ctx, B, seed=15)
+    vels = _cmd_vels(B)
+    prm = _params(5)
+    ep = _est_params(seed=77)
+
+    def run(n=n_ticks, rbd=rbd0, gaits=GAITS, v=vels, est=None):
+        return _est_device(ctx, rbd, gaits, v, n, prm, ep, hb.estimation_states(B) if est is None else est, 5)
+
+    for a, b in _null_schedule_checks(ctx, run, B, n_ticks, n_ticks * prm.period):
+        _assert_episode_equal(a, b, estimated=True, B=B)
+    # only instance 2 pushed: its estimation stats change, every other instance is the unpushed run
+    ctx.set_pushes(None)
+    u = _np(run())
+    ctx.set_pushes(_one_push(B, 2, 0.06, 0.08, (-60.0, 50.0, 0.0), (0.0, 0.0, -3.0)))
+    p = _np(run())
+    assert not np.array_equal(p[6][2], u[6][2]) and not np.array_equal(p[0][2], u[0][2])
+    keep = [0, 1, 3, 4, 5]
+    for k in (0, 2, 4, 7):
+        assert np.array_equal(p[k][keep], u[k][keep]), k
+    _assert_stats_equal(p[3][keep], u[3][keep])
+    _assert_est_stats_equal(p[6][keep], u[6][keep])
+    size = C.sizeof(hb.HbEstimationState)
+    assert np.array_equal(p[5].reshape(B, size)[keep], u[5].reshape(B, size)[keep])
+    # two calls split inside the push window equal one call
+    one = _np(run())
+    h = run(n=50)
+    two = ctx.rollout_estimated(h[0], hb.make_rollout_commands(GAITS, GAIT_START, CMD_TIMES, vels), 50, tick0=50, params=prm, est_params=ep, est=h[5],
+                                act=h[1], estop=h[2], stats=h[3], est_stats=h[6], log_every=5)
+    two = _np(two); h = _np(h)
+    for k in (0, 1, 2, 5):
+        assert np.array_equal(one[k], two[k]), k
+    _assert_stats_equal(one[3], two[3]); _assert_est_stats_equal(one[6], two[6])
+    for k in (4, 7):
+        assert np.array_equal(one[k], np.concatenate([h[k], two[k]], axis=1)), k
+    # a permuted batch, with its schedules and noise streams permuted, gives the permuted result
+    perm = [3, 5, 0, 1, 4, 2]
+    S = _schedules()
+    ctx.set_pushes(S)
+    full = _np(run())
+    ctx.set_pushes((hb.HbPushSchedule * B)(*[S[i] for i in perm]))
+    est_p = hb.estimation_states(B)
+    for j, i in enumerate(perm):
+        est_p[j].noise_stream = i
+    q = _np(run(rbd=rbd0[perm], gaits=[GAITS[i] for i in perm], v=vels[perm], est=est_p))
+    for k in (0, 2, 4, 7):
+        assert np.array_equal(full[k][perm], q[k]), k
+    _assert_stats_equal(full[3][perm], q[3]); _assert_est_stats_equal(full[6][perm], q[6])
+    assert np.array_equal(full[5].reshape(B, size)[perm], q[5].reshape(B, size))
+    # schedules for the first 2 instances only: the others run unpushed
+    ctx.set_pushes(None)
+    u = _np(run())
+    ctx.set_pushes(hb.make_push_schedules(2, 0.04, 0.1, [0.0, 60.0, 0.0]))
+    part = _np(run())
+    assert np.array_equal(part[0][2:], u[0][2:]) and np.array_equal(part[7][2:], u[7][2:])
+    _assert_est_stats_equal(part[6][2:], u[6][2:])
+    assert not np.array_equal(part[0][:2], u[0][:2])
+    ctx.close()
+
+
+# ---------------------------------------------------------------------------------------------------------------- argument checks
+def test_argument_checks_return_before_any_launch():
+    ctx = hb.Context(horizon_N=4, dt=0.01, max_batch=2, device=0)
+    lib = ctx._lib
+    assert C.sizeof(hb.HbPushSchedule) == 264
+    c0 = ctx.launch_count
+
+    def sched(n=3, **change):
+        S = hb.make_push_schedules(n, [0.1, 0.2], [0.05, 0.05], [[10.0, 0, 0], [0, 10.0, 0]])
+        for field, (j, value) in change.items():
+            if field in ("force", "torque"):
+                getattr(S[1], field)[j][2] = value
+            elif field == "n_push":
+                S[1].n_push = value
+            else:
+                getattr(S[1], field)[j] = value
+        return S
+
+    assert lib.hb_rollout_set_pushes(None, 1, sched()) == -1
+    assert lib.hb_rollout_set_pushes(ctx._h, -1, sched()) == -1
+    assert lib.hb_rollout_set_pushes(ctx._h, 1, None) == -1
+    nan, inf = float("nan"), float("inf")
+    for field, j, value in (("n_push", 0, -1), ("n_push", 0, hb.HB_MAX_PUSHES + 1), ("t_start", 1, nan), ("t_start", 0, -inf), ("force", 0, nan),
+                            ("force", 1, inf), ("torque", 1, nan), ("torque", 0, -inf), ("duration", 0, -0.01), ("duration", 1, nan),
+                            ("duration", 0, inf)):
+        assert lib.hb_rollout_set_pushes(ctx._h, 2, sched(**{field: (j, value)})) == -1, (field, j, value)
+    assert lib.hb_rollout_set_pushes(ctx._h, 3, sched()) == -4
+    assert lib.hb_rollout_set_pushes(ctx._h, 0, None) == 0 and lib.hb_rollout_set_pushes(ctx._h, 0, sched()) == 0
+    # a push beyond the used count is not read: n_push = 1 with a NaN in the second slot is valid
+    ok = sched(t_start=(1, nan)); ok[1].n_push = 1
+    assert lib.hb_rollout_set_pushes(ctx._h, 2, ok) == 0
+    assert lib.hb_rollout_set_pushes(ctx._h, 0, None) == 0
+
+    prm = hb.default_sim_params()
+    rbd = np.zeros((3, 32)); tau = np.zeros((3, 10)); w = np.zeros((3, 6))
+    P = lambda a: C.c_void_p(a.ctypes.data)
+
+    def step(h=ctx._h, B=1, p=prm, r=rbd, t=tau):
+        return lib.hb_sim_step_wrench(h, B, None if p is None else C.byref(p), None if r is None else P(r), None if t is None else P(t), P(w), None, None)
+
+    assert step(h=None) == -1 and step(B=-1) == -1 and step(p=None) == -1 and step(r=None) == -1 and step(t=None) == -1
+    for field, value in (("dt", 0.0), ("dt", nan), ("substeps", 0), ("substeps", 1001)):
+        bad = hb.default_sim_params()
+        setattr(bad, field, value)
+        assert step(p=bad) == -1, field
+    assert step(B=3) == -4
+    assert step(B=0) == 0
+    assert ctx.launch_count == c0
+    ctx.close()
