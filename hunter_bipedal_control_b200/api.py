@@ -51,6 +51,9 @@ class HbSolveInfo(C.Structure):
                 ("armijo", C.c_double), ("status", C.c_int32), ("n_trials", C.c_int32)]
 
 
+INFO_DTYPE = np.dtype(HbSolveInfo)
+
+
 class HbReference(C.Structure):
     _fields_ = [("n_events", C.c_int32), ("event_times", C.c_double * HB_MAX_EVENTS), ("modes", C.c_int32 * (HB_MAX_EVENTS + 1)),
                 ("n_targets", C.c_int32), ("target_times", C.c_double * HB_MAX_TARGETS), ("target_states", (C.c_double * 22) * HB_MAX_TARGETS),
@@ -116,33 +119,31 @@ class HbHoqpProblem(C.Structure):
 def make_hoqp_problems(hierarchies):
     """hierarchies: list (one per instance) of lists of tasks (a, b, d, f) by decreasing priority -> ctypes array of HbHoqpProblem."""
     pbs = (HbHoqpProblem * len(hierarchies))()
-    for pb, levels in zip(pbs, hierarchies):
-        pb.levels = len(levels)
-        n = 0
+    for pb, levels in zip(np.ctypeslib.as_array(pbs), hierarchies):
+        pb["levels"] = len(levels)
         for l, (a, b, d, f) in enumerate(levels):
-            a = np.zeros((0, 0)) if a is None else np.atleast_2d(np.asarray(a, dtype=float)); d = np.zeros((0, 0)) if d is None else np.atleast_2d(np.asarray(d, dtype=float))
-            n = max(n, a.shape[1] if a.size else 0, d.shape[1] if d.size else 0)
-            pb.ma[l] = a.shape[0] if a.size else 0; pb.md[l] = d.shape[0] if d.size else 0
-            for i in range(pb.ma[l]):
-                pb.b[l][i] = float(b[i])
-                for j in range(a.shape[1]):
-                    pb.a[l][i][j] = a[i, j]
-            for i in range(pb.md[l]):
-                pb.f[l][i] = float(f[i])
-                for j in range(d.shape[1]):
-                    pb.d[l][i][j] = d[i, j]
-        pb.n = n
+            a, d = _task_matrix(a), _task_matrix(d)
+            pb["ma"][l], pb["md"][l] = len(a), len(d)
+            pb["n"] = max(pb["n"], a.shape[1], d.shape[1])
+            if len(a):
+                pb["a"][l, :len(a), :a.shape[1]] = a; pb["b"][l, :len(a)] = b[:len(a)]
+            if len(d):
+                pb["d"][l, :len(d), :d.shape[1]] = d; pb["f"][l, :len(d)] = f[:len(d)]
     return pbs
+
+
+def _task_matrix(m):
+    """a or d of a task as a float matrix; None or an empty matrix has no rows and no columns."""
+    m = np.zeros((0, 0)) if m is None else np.atleast_2d(np.asarray(m, dtype=float))
+    return m if m.size else np.zeros((0, 0))
 
 
 def hoqp_tasks(pb):
     """HbHoqpProblem -> list of (a, b, d, f) numpy tasks."""
-    out = []
-    for l in range(pb.levels):
-        a = np.array([[pb.a[l][i][j] for j in range(pb.n)] for i in range(pb.ma[l])]).reshape(pb.ma[l], pb.n)
-        d = np.array([[pb.d[l][i][j] for j in range(pb.n)] for i in range(pb.md[l])]).reshape(pb.md[l], pb.n)
-        out.append((a, np.array([pb.b[l][i] for i in range(pb.ma[l])]), d, np.array([pb.f[l][i] for i in range(pb.md[l])])))
-    return out
+    p = np.ctypeslib.as_array(pb)
+    n, levels = int(p["n"]), int(p["levels"])
+    return [(p["a"][l, :ma, :n].copy(), p["b"][l, :ma].copy(), p["d"][l, :md, :n].copy(), p["f"][l, :md].copy())
+            for l, (ma, md) in enumerate(zip(p["ma"][:levels], p["md"][:levels]))]
 
 
 class HbActuationState(C.Structure):
@@ -180,8 +181,11 @@ class HbRolloutParams(C.Structure):
                 ("torque_limit", C.c_double * 10), ("min_base_height", C.c_double), ("log_every", C.c_int32)]
 
 
-ROLLOUT_STATS_DTYPE = np.dtype([("fail_tick", "i4"), ("fail_reason", "i4"), ("mpc_bad", "i4"), ("wbc_fallbacks", "i4"), ("plan_rejects", "i4"),
-                                ("max_abs_torque", "f8")], align=True)
+class HbRolloutStats(C.Structure):
+    _fields_ = [(k, C.c_int32) for k in ("fail_tick", "fail_reason", "mpc_bad", "wbc_fallbacks", "plan_rejects")] + [("max_abs_torque", C.c_double)]
+
+
+ROLLOUT_STATS_DTYPE = np.dtype(HbRolloutStats)
 
 
 def default_rollout_params():
@@ -212,13 +216,9 @@ def make_rollout_commands(gait, gait_start, cmd_times, cmd_vels):
     vel = np.broadcast_to(vel, (B, n, 4)); tim = np.broadcast_to(tim, (B, n))
     gids = _gait_ids(gait, B); start = np.broadcast_to(_f64(gait_start), (B,))
     cmds = (HbRolloutCommand * B)()
-    for i in range(B):
-        c = cmds[i]
-        c.gait = gids[i]; c.gait_start = start[i]; c.n_cmd = n
-        for j in range(n):
-            c.cmd_time[j] = tim[i, j]
-            for k in range(4):
-                c.cmd_vel[j][k] = vel[i, j, k]
+    v = np.ctypeslib.as_array(cmds)
+    v["gait"] = gids; v["gait_start"] = start; v["n_cmd"] = n
+    v["cmd_time"][:, :n] = tim; v["cmd_vel"][:, :n] = vel
     return cmds
 
 
@@ -250,13 +250,9 @@ def make_push_schedules(B, t_start, duration, force, torque=None):
     if not (np.isfinite(dur).all() and (dur >= 0).all()):
         raise ValueError("push schedules: durations must be finite and >= 0")
     out = (HbPushSchedule * B)()
-    for i in range(B):
-        s = out[i]
-        s.n_push = n
-        for j in range(n):
-            s.t_start[j] = tim[i, j]; s.duration[j] = dur[i, j]
-            for k in range(3):
-                s.force[j][k] = frc[i, j, k]; s.torque[j][k] = trq[i, j, k]
+    v = np.ctypeslib.as_array(out)
+    v["n_push"] = n
+    v["t_start"][:, :n] = tim; v["duration"][:, :n] = dur; v["force"][:, :n] = frc; v["torque"][:, :n] = trq
     return out
 
 
@@ -298,8 +294,11 @@ class HbEstimationState(C.Structure):
                 ("has_plan", C.c_int32), ("n_events", C.c_int32), ("event_times", C.c_double * HB_MAX_EVENTS), ("modes", C.c_int32 * (HB_MAX_EVENTS + 1))]
 
 
-ESTIMATION_STATS_DTYPE = np.dtype([("max_vel_err", "f8"), ("max_height_err", "f8"), ("sum_sq_vel_err", "f8"), ("sum_sq_height_err", "f8"),
-                                   ("count", "i4")], align=True)
+class HbEstimationStats(C.Structure):
+    _fields_ = [(k, C.c_double) for k in ("max_vel_err", "max_height_err", "sum_sq_vel_err", "sum_sq_height_err")] + [("count", C.c_int32)]
+
+
+ESTIMATION_STATS_DTYPE = np.dtype(HbEstimationStats)
 
 
 def default_estimation_params():
@@ -332,8 +331,7 @@ class GaitSelector:
     def __init__(self, B, gait_level=-1):
         self.B = B
         self.state = (HbGaitSelector * B)()
-        for i in range(B):
-            self.state[i].gait_level = gait_level
+        np.ctypeslib.as_array(self.state)["gait_level"] = gait_level
 
     def update(self, cmd_vel, target_state0, gait_type=0):
         lib = load_library()
@@ -345,7 +343,7 @@ class GaitSelector:
 
     @property
     def vel_avg(self):
-        return np.array([self.state[i].vel_avg for i in range(self.B)])
+        return np.ctypeslib.as_array(self.state)["vel_avg"].copy()
 
 
 GAIT_IDS = {"stance": 0, "trot": 1, "standing_trot": 2, "flying_trot": 3}
@@ -371,15 +369,12 @@ def make_plan_inputs(t0, horizon, x0, cmd_vel, feet_pos, gait, gait_start, prev_
     feet_pos = np.zeros((B, 12)) if feet_pos is None else _f64(feet_pos).reshape(B, 12)
     t0 = np.broadcast_to(_f64(t0), (B,)); gait_start = np.broadcast_to(_f64(gait_start), (B,))
     ins = (HbPlanInput * B)()
-    for i in range(B):
-        p = ins[i]
-        p.t0 = t0[i]; p.horizon = horizon; p.time_to_target = horizon if time_to_target is None else time_to_target
-        p.gait_start = gait_start[i]; p.prev_event = (min(t0[i], gait_start[i]) - 0.5) if prev_event is None else prev_event
-        p.gait = gids[i]
-        p.joint_ik = 1 if joint_ik else 0
-        for j in range(22): p.x0[j] = x0[i, j]
-        for j in range(4): p.cmd_vel[j] = cmd_vel[i, j]
-        for j in range(12): p.feet_pos[j] = feet_pos[i, j]
+    v = np.ctypeslib.as_array(ins)
+    v["t0"] = t0; v["horizon"] = horizon; v["time_to_target"] = horizon if time_to_target is None else time_to_target
+    v["gait_start"] = gait_start; v["prev_event"] = (np.minimum(t0, gait_start) - 0.5) if prev_event is None else prev_event
+    v["gait"] = gids
+    v["joint_ik"] = 1 if joint_ik else 0
+    v["x0"] = x0.reshape(B, 22); v["cmd_vel"] = cmd_vel; v["feet_pos"] = feet_pos
     return ins
 
 
@@ -397,11 +392,6 @@ def plan_references(t0, horizon, x0, cmd_vel, feet_pos, gait, gait_start, prev_e
     refs = (HbReference * B)()
     _check(lib.hb_plan_references(B, ins, _ptr(ls), refs), "hb_plan_references")
     return refs, ls
-
-
-INFO_DTYPE = np.dtype([("alpha", "f8"), ("merit0", "f8"), ("merit1", "f8"), ("viol0", "f8"), ("viol1", "f8"), ("armijo", "f8"),
-                       ("status", "i4"), ("n_trials", "i4")], align=True)
-assert INFO_DTYPE.itemsize == C.sizeof(HbSolveInfo)
 
 
 class HunterB200Error(RuntimeError):
@@ -794,23 +784,7 @@ class Context:
         place); estop: cuda uint8 tensor [B] (None: zeros, in place); stats: ROLLOUT_STATS_DTYPE array (None: rollout_stats(B)).
         Returns (rbd, act, estop, stats, log): stats as a new structured array, log a cuda tensor [B, ceil(n_ticks / log_every), 32] or None.
         Waits for the episode to finish (the stats are read back)."""
-        import torch
-        B = rbd.shape[0]
-        dev = rbd.device
-        params = params or default_rollout_params()
-        params.log_every = int(log_every)
-        if act is None:
-            act = torch.zeros(B * C.sizeof(HbActuationState), dtype=torch.uint8, device=dev)
-        if estop is None:
-            estop = torch.zeros(B, dtype=torch.uint8, device=dev)
-        st = rollout_stats(B) if stats is None else np.ascontiguousarray(stats, dtype=ROLLOUT_STATS_DTYPE)
-        d_st = torch.from_numpy(st.view(np.uint8).copy()).to(dev)
-        log = torch.zeros((B, -(-n_ticks // log_every), 32), dtype=torch.float64, device=dev) if log_every > 0 else None
-        torch.cuda.current_stream(dev).synchronize()          # the context's stream does not order itself after torch's
-        _check(self._lib.hb_rollout_batch_dev(self._h, B, C.c_int64(tick0), int(n_ticks), C.byref(params), commands, _ptr(rbd), _ptr(act), _ptr(estop),
-                                              _ptr(d_st), _ptr(log)), "hb_rollout_batch_dev", self._h)
-        self.sync()
-        return rbd, act, estop, d_st.cpu().numpy().view(ROLLOUT_STATS_DTYPE), log
+        return self._episodes(rbd, commands, n_ticks, tick0, params, act, estop, stats, log_every)
 
     def rollout_estimated(self, rbd, commands, n_ticks, tick0=0, params=None, est_params=None, est=None, act=None, estop=None, stats=None, est_stats=None,
                           log_every=0):
@@ -818,31 +792,44 @@ class Context:
         HbEstimationParams (None: default_estimation_params(), no noise); est: cuda uint8 tensor of B hb_estimation_state (None: fresh
         estimation_states(B), in place); est_stats: ESTIMATION_STATS_DTYPE array (None: zeros). Returns rollout()'s tuple followed by
         (est, est_stats, est_log): est_log the estimated rbd in log's layout, or None."""
+        return self._episodes(rbd, commands, n_ticks, tick0, params, act, estop, stats, log_every, True, est_params, est, est_stats)
+
+    def _episodes(self, rbd, commands, n_ticks, tick0, params, act, estop, stats, log_every, estimated=False, est_params=None, est=None, est_stats=None):
+        """The body of rollout() and, with estimated = True, of rollout_estimated()."""
         import torch
         B = rbd.shape[0]
         dev = rbd.device
         params = params or default_rollout_params()
         params.log_every = int(log_every)
-        est_params = est_params or default_estimation_params()
         if act is None:
             act = torch.zeros(B * C.sizeof(HbActuationState), dtype=torch.uint8, device=dev)
         if estop is None:
             estop = torch.zeros(B, dtype=torch.uint8, device=dev)
-        if est is None:
-            est = torch.from_numpy(np.frombuffer(bytes(estimation_states(B)), dtype=np.uint8).copy()).to(dev)
-        st = rollout_stats(B) if stats is None else np.ascontiguousarray(stats, dtype=ROLLOUT_STATS_DTYPE)
-        d_st = torch.from_numpy(st.view(np.uint8).copy()).to(dev)
-        es = estimation_stats(B) if est_stats is None else np.ascontiguousarray(est_stats, dtype=ESTIMATION_STATS_DTYPE)
-        d_es = torch.from_numpy(es.view(np.uint8).copy()).to(dev)
-        rows = -(-n_ticks // log_every) if log_every > 0 else 0
-        log = torch.zeros((B, rows, 32), dtype=torch.float64, device=dev) if log_every > 0 else None
-        est_log = torch.zeros((B, rows, 32), dtype=torch.float64, device=dev) if log_every > 0 else None
+
+        def records(a, dtype):
+            return torch.from_numpy(np.ascontiguousarray(a, dtype=dtype).view(np.uint8).copy()).to(dev)
+
+        def new_log():
+            return torch.zeros((B, -(-n_ticks // log_every), 32), dtype=torch.float64, device=dev) if log_every > 0 else None
+
+        d_st = records(rollout_stats(B) if stats is None else stats, ROLLOUT_STATS_DTYPE)
+        log = new_log()
+        if estimated:
+            est_params = est_params or default_estimation_params()
+            if est is None:
+                est = torch.from_numpy(np.frombuffer(bytes(estimation_states(B)), dtype=np.uint8).copy()).to(dev)
+            d_es = records(estimation_stats(B) if est_stats is None else est_stats, ESTIMATION_STATS_DTYPE)
+            est_log = new_log()
         torch.cuda.current_stream(dev).synchronize()          # the context's stream does not order itself after torch's
-        _check(self._lib.hb_rollout_estimated_batch_dev(self._h, B, C.c_int64(tick0), int(n_ticks), C.byref(params), C.byref(est_params), commands, _ptr(rbd),
-                                                        _ptr(act), _ptr(estop), _ptr(d_st), _ptr(est), _ptr(d_es), _ptr(log), _ptr(est_log)),
-               "hb_rollout_estimated_batch_dev", self._h)
+        head = (self._h, B, C.c_int64(tick0), int(n_ticks), C.byref(params))
+        if estimated:
+            _check(self._lib.hb_rollout_estimated_batch_dev(*head, C.byref(est_params), commands, _ptr(rbd), _ptr(act), _ptr(estop), _ptr(d_st), _ptr(est),
+                                                            _ptr(d_es), _ptr(log), _ptr(est_log)), "hb_rollout_estimated_batch_dev", self._h)
+        else:
+            _check(self._lib.hb_rollout_batch_dev(*head, commands, _ptr(rbd), _ptr(act), _ptr(estop), _ptr(d_st), _ptr(log)), "hb_rollout_batch_dev", self._h)
         self.sync()
-        return (rbd, act, estop, d_st.cpu().numpy().view(ROLLOUT_STATS_DTYPE), log, est, d_es.cpu().numpy().view(ESTIMATION_STATS_DTYPE), est_log)
+        out = (rbd, act, estop, d_st.cpu().numpy().view(ROLLOUT_STATS_DTYPE), log)
+        return out + (est, d_es.cpu().numpy().view(ESTIMATION_STATS_DTYPE), est_log) if estimated else out
 
     def control_step_dev(self, t_rel, x0, x_ref, swing, mode, rbd, xt, ut, info, sol, tau, status=None):
         _check(self._lib.hb_control_step_batch_dev(self._h, x0.shape[0], C.c_double(t_rel), _ptr(x0), _ptr(x_ref), _ptr(swing), _ptr(mode), _ptr(rbd), _ptr(xt),

@@ -241,24 +241,15 @@ def pack_references(compacts, horizon):
     """Compact descriptions returned by make_reference (4th value) -> ctypes array of HbReference for the device expansion."""
     from .api import HbReference, HB_MAX_SEGMENTS
     refs = (HbReference * len(compacts))()
-    for r, c in zip(refs, compacts):
-        r.n_events = len(c["events"])
-        for k, t in enumerate(c["events"]):
-            r.event_times[k] = t
-        for k, m in enumerate(c["modes"]):
-            r.modes[k] = m
-        r.n_targets = len(c["target_times"])
-        for k in range(r.n_targets):
-            r.target_times[k] = c["target_times"][k]
-            for j in range(22):
-                r.target_states[k][j] = c["target_states"][k][j]
+    for r, c in zip(np.ctypeslib.as_array(refs), compacts):
+        ne, nm, nt = len(c["events"]), len(c["modes"]), len(c["target_times"])
+        r["n_events"] = ne; r["event_times"][:ne] = c["events"]; r["modes"][:nm] = c["modes"]
+        r["n_targets"] = nt; r["target_times"][:nt] = c["target_times"]; r["target_states"][:nt] = c["target_states"]
         for cc in range(4):
             for a in range(3):
                 segs = [sg for sg in c["segments"][cc][a] if sg[0] <= horizon + 1e-9]      # only what the horizon can see
                 if len(segs) > HB_MAX_SEGMENTS:
                     raise ValueError("too many swing segments for hb_reference")
-                r.n_segments[cc][a] = len(segs)
-                for si, sg in enumerate(segs):
-                    for j in range(6):
-                        r.segments[cc][a][si][j] = sg[j]
+                r["n_segments"][cc, a] = len(segs)
+                r["segments"][cc, a, :len(segs)] = np.reshape(segs, (-1, 6))
     return refs
