@@ -9,23 +9,22 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = os.path.join(ROOT, "hunter_bipedal_control_b200")
-EXE = os.path.join(ROOT, "tests", "adapters_main")
 INC = ["-I" + os.path.join(ROOT, "adapters"), "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(ROOT, "tests", "adapter_stubs")]
 
 
-def build_driver():
+def build_driver(out_dir):
+    """The driver program, built in out_dir: the repository tree may be read-only."""
+    exe = os.path.join(out_dir, "adapters_main")
     src = os.path.join(ROOT, "tests", "adapters_main.cpp")
-    deps = [src, os.path.join(ROOT, "adapters", "B200Wbc.h"), os.path.join(ROOT, "adapters", "B200Mpc.h"), os.path.join(ROOT, "include", "hunter_b200.h")]
-    if not os.path.exists(EXE) or any(os.path.getmtime(d) > os.path.getmtime(EXE) for d in deps):
-        subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-Werror"] + INC + ["-o", EXE, src, "-L" + PKG, "-l:libhunter_b200.so", "-Wl,-rpath," + PKG])
-    return EXE
+    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-Werror"] + INC + ["-o", exe, src, "-L" + PKG, "-l:libhunter_b200.so", "-Wl,-rpath," + PKG])
+    return exe
 
 
-def test_adapters_compile_and_link_against_the_c_abi():
+def test_adapters_compile_and_link_against_the_c_abi(tmp_path):
     """Each header on its own (self-contained includes), then the driver program linked with the shared library."""
     for h in ("B200Wbc.h", "B200Mpc.h"):
         subprocess.run(["g++", "-std=c++17", "-fsyntax-only", "-Wall", "-Werror"] + INC + ["-x", "c++", "-"], input=('#include "%s"\n' % h).encode(), check=True)
-    assert os.path.exists(build_driver())
+    assert os.path.exists(build_driver(tmp_path))
 
 
 @pytest.mark.gpu
@@ -33,7 +32,7 @@ def test_adapters_drive_the_gpu_path_like_the_controller(tmp_path):
     import hunter_bipedal_control_b200 as hb
     from hunter_bipedal_control_b200 import scenarios as sc
     from test_gpu_event_nodes import _shift_numpy
-    exe = build_driver()
+    exe = build_driver(tmp_path)
     task = os.path.join(ROOT, "tests", "golden", "task_wbc_variant.info")
     rng = np.random.default_rng(17)
     # ---- WBC cases: (mode, stance flag, setKpKd or not)

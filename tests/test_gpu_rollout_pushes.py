@@ -9,85 +9,10 @@ import pytest
 
 import hunter_bipedal_control_b200 as hb
 from hunter_bipedal_control_b200 import scenarios as sc
-from test_gpu_rollout_episodes import (CMD_TIMES, GAIT_START, GAITS, _assert_stats_equal, _cmd_vels, _context, _device, _params, _start_states,
-                                       _stepwise)
-from test_gpu_rollout_estimation import _assert_est_equal, _assert_est_stats_equal, _est_params
-from test_gpu_rollout_estimation import _device as _est_device
-from test_gpu_rollout_estimation import _stepwise as _est_stepwise
+from episode_ref import (GAITS, assert_continues, assert_episode_equal, cmd_vels, context, device, est_params, outputs, params, plant_numpy,
+                         start_states, stepwise)
 
 pytestmark = pytest.mark.gpu
-
-
-def _torch():
-    import torch
-    return torch
-
-
-def _T(zyx):
-    """omega_world = T(zyx) (yaw, pitch, roll rates): the columns are the world axes of the three rotations."""
-    sz, cz, sy, cy = np.sin(zyx[0]), np.cos(zyx[0]), np.sin(zyx[1]), np.cos(zyx[1])
-    return np.array([[0.0, -sz, cz * cy], [0.0, cz, sz * cy], [1.0, 0.0, -sy]])
-
-
-def _plant_numpy(oracle, rbd, tau, prm, wrench):
-    """test_gpu_rollout._plant_numpy with the external wrench: Q_p = f, Q_zyx = T' tau at each substep's orientation."""
-    from oracle import refs
-    q = np.concatenate([rbd[3:6], rbd[0:3], rbd[6:16]])
-    v = np.concatenate([rbd[19:22], refs.euler_rates_from_global(rbd[0:3], rbd[16:19]), rbd[22:32]])
-    h = prm.dt / prm.substeps
-    F = np.zeros(12)
-    for _ in range(prm.substeps):
-        r = oracle.rbd(q, v)
-        cvel = r["J"] @ v
-        F = np.zeros(12)
-        for c in range(4):
-            depth = prm.ground_height - r["cpos"][3 * c + 2]
-            if depth > 0:
-                fz = max(0.0, prm.ground_stiffness * depth - prm.ground_damping * cvel[3 * c + 2])
-                ft = -prm.tangential_damping * cvel[3 * c:3 * c + 2]
-                n = np.linalg.norm(ft)
-                if n > prm.friction_mu * fz:
-                    ft = ft * (prm.friction_mu * fz / n if n > 0 else 0.0)
-                F[3 * c:3 * c + 3] = [ft[0], ft[1], fz]
-        Q = np.concatenate([wrench[:3], _T(q[3:6]).T @ wrench[3:], np.zeros(10)])
-        rhs = np.concatenate([np.zeros(6), tau - prm.joint_damping * v[6:]]) + r["J"].T @ F - r["nle"] + Q
-        qdd = np.linalg.solve(r["M"] + np.diag(np.r_[np.zeros(6), np.full(10, prm.joint_armature)]), rhs)
-        v = v + h * qdd
-        q = q + h * v
-    out = np.zeros(32)
-    out[0:3] = q[3:6]; out[3:6] = q[0:3]; out[6:16] = q[6:]
-    out[16:19] = refs.global_from_euler_rates(q[3:6], v[3:6]); out[19:22] = v[0:3]; out[22:32] = v[6:]
-    return out, F
-
-
-def _wrench_numpy(pushes, t, B):
-    """The documented wrench of the tick at time t: zeros, plus every active push in ascending j (B x 6; instances without a schedule: 0)."""
-    w = np.zeros((B, 6))
-    for i in range(min(B, len(pushes))):
-        s = pushes[i]
-        for j in range(s.n_push):
-            if s.t_start[j] <= t and t < s.t_start[j] + s.duration[j]:
-                for c in range(3):
-                    w[i, c] += s.force[j][c]; w[i, 3 + c] += s.torque[j][c]
-    return w
-
-
-class _PushedPlant:
-    """A context for the stepwise loops of the episode tests whose plant step applies the push wrench of the tick it advances: those loops
-    call sim_step once per tick, in tick order from tick0."""
-
-    def __init__(self, ctx, pushes, period, tick0=0):
-        self._ctx, self._pushes, self._period, self._tick = ctx, pushes, period, tick0
-        self.steps = 0
-
-    def __getattr__(self, name):
-        return getattr(self._ctx, name)
-
-    def sim_step(self, rbd, tau, params=None):
-        t = self._tick * self._period
-        self._tick += 1
-        self.steps += 1
-        return self._ctx.sim_step(rbd, tau, params, wrench=_wrench_numpy(self._pushes, t, rbd.shape[0]))
 
 
 def _schedules():
@@ -118,21 +43,6 @@ def _one_push(B, i, t_start, duration, force, torque=(0.0, 0.0, 0.0)):
                                   np.where((np.arange(B) == i)[:, None, None], np.array(torque, dtype=float)[None, None], 0.0))
 
 
-def _np(out):
-    return [o.cpu().numpy() if hasattr(o, "cpu") else o for o in out]
-
-
-def _assert_episode_equal(a, b, estimated=False, B=None):
-    a, b = _np(a), _np(b)
-    for k in (0, 1, 2, 4):
-        assert np.array_equal(a[k], b[k]), k
-    _assert_stats_equal(a[3], b[3])
-    if estimated:
-        _assert_est_equal(a[5], b[5], B)
-        _assert_est_stats_equal(a[6], b[6])
-        assert np.array_equal(a[7], b[7])
-
-
 # ---------------------------------------------------------------------------------------------------------------- the plant step
 def test_plant_step_with_wrench_matches_numpy_restatement(gpu_ctx, oracle):
     B = 10
@@ -148,7 +58,7 @@ def test_plant_step_with_wrench_matches_numpy_restatement(gpu_ctx, oracle):
     base = gpu_ctx.sim_step(rbd, tau, prm)
     touched = 0
     for i in range(B):
-        ref, F = _plant_numpy(oracle, rbd[i], tau[i], prm, W[i])
+        ref, F = plant_numpy(oracle, rbd[i], tau[i], prm, W[i])
         assert np.abs(nxt[i] - ref).max() < 1e-9 * max(1.0, np.abs(ref).max()), i
         assert np.abs(cf[i] - F).max() < 1e-7 * max(1.0, np.abs(F).max())
         assert np.array_equal(fl[i] != 0, F[2::3] > 0)
@@ -210,35 +120,33 @@ def test_free_flight_momentum_balance(gpu_ctx, kind):
 # ---------------------------------------------------------------------------------------------------------------- pushed episodes
 @pytest.mark.parametrize("event_nodes", [False, True], ids=["uniform", "event_nodes"])
 def test_pushed_episode_equals_the_stepwise_loop_bitwise(event_nodes):
-    ctx = _context(event_nodes)
+    ctx = context(event_nodes)
     B, n_ticks, log_every = 6, 200, 10
-    rbd0 = _start_states(ctx, B, seed=11)
-    vels = _cmd_vels(B)
-    prm = _params(log_every)
+    rbd0 = start_states(ctx, B, seed=11)
+    vels = cmd_vels(B)
+    prm = params(log_every)
     S = _schedules()
     ctx.set_pushes(S)
-    d = _device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
-    plant = _PushedPlant(ctx, S, prm.period)
-    r = _stepwise(plant, rbd0, GAITS, vels, n_ticks, prm, log_every)
-    assert plant.steps == n_ticks
-    _assert_episode_equal(d, r)
+    d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, pushes=S)
+    assert_episode_equal(d, r)
     ctx.set_pushes(None)
-    u = _device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
+    u = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
     moved = [not np.array_equal(a, b) for a, b in zip(d[0].cpu().numpy(), u[0].cpu().numpy())]
     assert moved == [True, True, True, False, False, True], moved
     ctx.close()
 
 
 def test_state_before_the_push_is_unchanged_and_the_state_after_it_moves():
-    ctx = _context()
+    ctx = context()
     B, n_ticks = 6, 80
-    rbd0 = _start_states(ctx, B, seed=12)
-    vels = _cmd_vels(B)
-    prm = _params(1)
-    u = _np(_device(ctx, rbd0, GAITS, vels, n_ticks, prm, 1))
+    rbd0 = start_states(ctx, B, seed=12)
+    vels = cmd_vels(B)
+    prm = params(1)
+    u = outputs(device(ctx, rbd0, GAITS, vels, n_ticks, prm, 1))
     k = 50
     ctx.set_pushes(_one_push(B, 0, k * prm.period, 0.02, (0.0, 80.0, 0.0)))
-    p = _np(_device(ctx, rbd0, GAITS, vels, n_ticks, prm, 1))
+    p = outputs(device(ctx, rbd0, GAITS, vels, n_ticks, prm, 1))
     assert np.array_equal(p[4][:, :k + 1], u[4][:, :k + 1])          # log row k: the state entering the tick the push starts
     assert not np.array_equal(p[4][0, k + 1], u[4][0, k + 1])
     assert np.array_equal(p[4][1:], u[4][1:]) and np.array_equal(p[0][1:], u[0][1:])
@@ -275,147 +183,115 @@ def _null_schedule_checks(ctx, run, B, n_ticks, horizon_t):
     assert ctx._lib.hb_rollout_set_pushes(ctx._h, ctx.max_batch + 1, _schedules()) == -4
     got, _ = counted()
     yield want, got
-    assert not np.array_equal(_np(want)[0], _np(ref)[0])
+    assert not np.array_equal(outputs(want)[0], outputs(ref)[0])
 
 
 def test_null_schedules_change_nothing():
-    ctx = _context()
+    ctx = context()
     B, n_ticks = 6, 100
-    rbd0 = _start_states(ctx, B, seed=13)
-    vels = _cmd_vels(B)
-    prm = _params(5)
-    for a, b in _null_schedule_checks(ctx, lambda: _device(ctx, rbd0, GAITS, vels, n_ticks, prm, 5), B, n_ticks, n_ticks * prm.period):
-        _assert_episode_equal(a, b)
+    rbd0 = start_states(ctx, B, seed=13)
+    vels = cmd_vels(B)
+    prm = params(5)
+    for a, b in _null_schedule_checks(ctx, lambda: device(ctx, rbd0, GAITS, vels, n_ticks, prm, 5), B, n_ticks, n_ticks * prm.period):
+        assert_episode_equal(a, b)
     ctx.close()
 
 
 def test_continuation_independence_permutation_and_unscheduled_instances():
-    ctx = _context()
+    ctx = context()
     B = 6
-    rbd0 = _start_states(ctx, B, seed=14)
-    vels = _cmd_vels(B)
-    prm = _params(10)
-    cmds = hb.make_rollout_commands(GAITS, GAIT_START, CMD_TIMES, vels)
+    rbd0 = start_states(ctx, B, seed=14)
+    vels = cmd_vels(B)
+    prm = params(10)
     # two calls split inside a push window (ticks 75..124, split at tick 100) equal one call
     ctx.set_pushes(hb.make_push_schedules(B, 0.15, 0.1, np.linspace(-60, 60, B)[:, None, None] * np.array([1.0, 0.5, 0.0]), [0.0, 0.0, 3.0]))
-    one = _device(ctx, rbd0, GAITS, vels, 200, prm, 10)
-    h = _device(ctx, rbd0, GAITS, vels, 100, prm, 10)
-    two = ctx.rollout(h[0], cmds, 100, tick0=100, params=prm, act=h[1], estop=h[2], stats=h[3], log_every=10)
-    for k in (0, 1, 2):
-        assert np.array_equal(one[k].cpu().numpy(), two[k].cpu().numpy()), k
-    _assert_stats_equal(one[3], two[3])
-    assert np.array_equal(one[4].cpu().numpy(), np.concatenate([h[4].cpu().numpy(), two[4].cpu().numpy()], axis=1))
+    assert_continues(ctx, rbd0, GAITS, vels, 200, 100, prm, 10)
     # pushing instance 0 only leaves every other instance as in the unpushed run
     ctx.set_pushes(None)
-    u = _np(_device(ctx, rbd0, GAITS, vels, 200, prm, 10))
+    u = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
     ctx.set_pushes(_one_push(B, 0, 0.1, 0.1, (70.0, -30.0, 0.0), (0.0, 2.0, 0.0)))
-    p = _np(_device(ctx, rbd0, GAITS, vels, 200, prm, 10))
+    p = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
     assert not np.array_equal(p[0][0], u[0][0])
-    size = C.sizeof(hb.HbActuationState)
-    assert np.array_equal(p[0][1:], u[0][1:]) and np.array_equal(p[4][1:], u[4][1:])
-    assert np.array_equal(p[1].reshape(B, size)[1:], u[1].reshape(B, size)[1:]) and np.array_equal(p[2][1:], u[2][1:])
-    _assert_stats_equal(p[3][1:], u[3][1:])
+    assert_episode_equal(p, u, rows_a=slice(1, None), rows_b=slice(1, None))
     # a permuted batch with permuted schedules gives the permuted result
     S = _schedules()
     ctx.set_pushes(S)
-    full = _np(_device(ctx, rbd0, GAITS, vels, 200, prm, 10))
+    full = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
     perm = [4, 0, 5, 2, 1, 3]
     Sp = (hb.HbPushSchedule * B)(*[S[i] for i in perm])
     ctx.set_pushes(Sp)
-    q = _np(_device(ctx, rbd0[perm], [GAITS[i] for i in perm], vels[perm], 200, prm, 10))
-    assert np.array_equal(full[0][perm], q[0]) and np.array_equal(full[4][perm], q[4]) and np.array_equal(full[2][perm], q[2])
-    assert np.array_equal(full[1].reshape(B, size)[perm], q[1].reshape(B, size))
-    _assert_stats_equal(full[3][perm], q[3])
+    q = outputs(device(ctx, rbd0[perm], [GAITS[i] for i in perm], vels[perm], 200, prm, 10))
+    assert_episode_equal(full, q, rows_a=perm)
     # schedules for the first 3 instances only: the others run unpushed, the first 3 as with the full setting
     ctx.set_pushes(hb.make_push_schedules(3, 0.05, 0.2, [40.0, 40.0, 0.0]))
-    part = _np(_device(ctx, rbd0, GAITS, vels, 200, prm, 10))
+    part = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
     padded = hb.make_push_schedules(B, 0.05, 0.2, [40.0, 40.0, 0.0])
     for i in range(3, B):
         padded[i].n_push = 0
     ctx.set_pushes(padded)
-    full6 = _np(_device(ctx, rbd0, GAITS, vels, 200, prm, 10))
-    assert np.array_equal(part[0][3:], u[0][3:]) and np.array_equal(part[4][3:], u[4][3:])
-    assert np.array_equal(part[0], full6[0]) and np.array_equal(part[4], full6[4])
+    full6 = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
+    assert_episode_equal(part, u, rows_a=slice(3, None), rows_b=slice(3, None))
+    assert_episode_equal(part, full6)
     assert not np.array_equal(part[0][:3], u[0][:3])
     ctx.close()
 
 
 # ---------------------------------------------------------------------------------------------------------------- estimated episodes
 def test_pushed_estimated_episode_equals_the_stepwise_loop_bitwise():
-    ctx = _context()
+    ctx = context()
     B, n_ticks, log_every = 6, 120, 10
-    rbd0 = _start_states(ctx, B, seed=11)
-    vels = _cmd_vels(B)
-    prm = _params(log_every)
-    ep = _est_params(seed=2024)
+    rbd0 = start_states(ctx, B, seed=11)
+    vels = cmd_vels(B)
+    prm = params(log_every)
+    ep = est_params(seed=2024)
     S = _schedules()
     ctx.set_pushes(S)
-    d = _est_device(ctx, rbd0, GAITS, vels, n_ticks, prm, ep, hb.estimation_states(B, 40), log_every)
-    plant = _PushedPlant(ctx, S, prm.period)
-    r = _est_stepwise(plant, rbd0, GAITS, vels, n_ticks, prm, ep, hb.estimation_states(B, 40), log_every)
-    assert plant.steps == n_ticks
-    _assert_episode_equal(d, r, estimated=True, B=B)
+    d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40))
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40), pushes=S)
+    assert_episode_equal(d, r)
     ctx.close()
 
 
 def test_estimated_episodes_null_schedules_independence_and_continuation():
-    ctx = _context()
+    ctx = context()
     B, n_ticks = 6, 100
-    rbd0 = _start_states(ctx, B, seed=15)
-    vels = _cmd_vels(B)
-    prm = _params(5)
-    ep = _est_params(seed=77)
+    rbd0 = start_states(ctx, B, seed=15)
+    vels = cmd_vels(B)
+    prm = params(5)
+    ep = est_params(seed=77)
 
-    def run(n=n_ticks, rbd=rbd0, gaits=GAITS, v=vels, est=None):
-        return _est_device(ctx, rbd, gaits, v, n, prm, ep, hb.estimation_states(B) if est is None else est, 5)
+    def run(rbd=rbd0, gaits=GAITS, v=vels, est=None):
+        return device(ctx, rbd, gaits, v, n_ticks, prm, 5, ep, est)
 
     for a, b in _null_schedule_checks(ctx, run, B, n_ticks, n_ticks * prm.period):
-        _assert_episode_equal(a, b, estimated=True, B=B)
+        assert_episode_equal(a, b)
     # only instance 2 pushed: its estimation stats change, every other instance is the unpushed run
     ctx.set_pushes(None)
-    u = _np(run())
+    u = outputs(run())
     ctx.set_pushes(_one_push(B, 2, 0.06, 0.08, (-60.0, 50.0, 0.0), (0.0, 0.0, -3.0)))
-    p = _np(run())
+    p = outputs(run())
     assert not np.array_equal(p[6][2], u[6][2]) and not np.array_equal(p[0][2], u[0][2])
     keep = [0, 1, 3, 4, 5]
-    for k in (0, 2, 4, 7):
-        assert np.array_equal(p[k][keep], u[k][keep]), k
-    _assert_stats_equal(p[3][keep], u[3][keep])
-    _assert_est_stats_equal(p[6][keep], u[6][keep])
-    size = C.sizeof(hb.HbEstimationState)
-    assert np.array_equal(p[5].reshape(B, size)[keep], u[5].reshape(B, size)[keep])
+    assert_episode_equal(p, u, rows_a=keep, rows_b=keep)
     # two calls split inside the push window equal one call
-    one = _np(run())
-    h = run(n=50)
-    two = ctx.rollout_estimated(h[0], hb.make_rollout_commands(GAITS, GAIT_START, CMD_TIMES, vels), 50, tick0=50, params=prm, est_params=ep, est=h[5],
-                                act=h[1], estop=h[2], stats=h[3], est_stats=h[6], log_every=5)
-    two = _np(two); h = _np(h)
-    for k in (0, 1, 2, 5):
-        assert np.array_equal(one[k], two[k]), k
-    _assert_stats_equal(one[3], two[3]); _assert_est_stats_equal(one[6], two[6])
-    for k in (4, 7):
-        assert np.array_equal(one[k], np.concatenate([h[k], two[k]], axis=1)), k
+    assert_continues(ctx, rbd0, GAITS, vels, n_ticks, 50, prm, 5, ep)
     # a permuted batch, with its schedules and noise streams permuted, gives the permuted result
     perm = [3, 5, 0, 1, 4, 2]
     S = _schedules()
     ctx.set_pushes(S)
-    full = _np(run())
+    full = outputs(run())
     ctx.set_pushes((hb.HbPushSchedule * B)(*[S[i] for i in perm]))
     est_p = hb.estimation_states(B)
     for j, i in enumerate(perm):
         est_p[j].noise_stream = i
-    q = _np(run(rbd=rbd0[perm], gaits=[GAITS[i] for i in perm], v=vels[perm], est=est_p))
-    for k in (0, 2, 4, 7):
-        assert np.array_equal(full[k][perm], q[k]), k
-    _assert_stats_equal(full[3][perm], q[3]); _assert_est_stats_equal(full[6][perm], q[6])
-    assert np.array_equal(full[5].reshape(B, size)[perm], q[5].reshape(B, size))
+    q = outputs(run(rbd=rbd0[perm], gaits=[GAITS[i] for i in perm], v=vels[perm], est=est_p))
+    assert_episode_equal(full, q, rows_a=perm)
     # schedules for the first 2 instances only: the others run unpushed
     ctx.set_pushes(None)
-    u = _np(run())
+    u = outputs(run())
     ctx.set_pushes(hb.make_push_schedules(2, 0.04, 0.1, [0.0, 60.0, 0.0]))
-    part = _np(run())
-    assert np.array_equal(part[0][2:], u[0][2:]) and np.array_equal(part[7][2:], u[7][2:])
-    _assert_est_stats_equal(part[6][2:], u[6][2:])
+    part = outputs(run())
+    assert_episode_equal(part, u, rows_a=slice(2, None), rows_b=slice(2, None))
     assert not np.array_equal(part[0][:2], u[0][:2])
     ctx.close()
 
