@@ -27,11 +27,23 @@ constexpr int LIN_F1 = 0, LIN_F2 = 22, LIN_A1 = 44, LIN_A2 = 242, LIN_BF1 = 440,
               LIN_EPOS = 632, LIN_EVEL = 644, LIN_DPQ = 656, LIN_DVX = 812, LIN_DVV = 1076, LIN_STRIDE = 1200;
 constexpr int NTMAX = 16;   // free inputs after projection: 3 n_stance + (10 - rank of the velocity rows); 12 / 9 / 6 in regular poses
 constexpr int NVMAX = 8;    // null-space columns kept for the velocity rows
-constexpr int PJ_AT = 0, PJ_BT = 484, PJ_BTV = 836, PJ_QT = 858, PJ_PT = 1342, PJ_RT = 1694, PJ_QV = 1950, PJ_RV = 1972,
-              PJ_PXV = 1988, PJ_NV = 2208, PJ_PEV = 2288, PJ_META = 2298, PJ_STRIDE = 2320;
+// Projected record: only the entries that carry data. Each reader stages one contiguous span of it:
+//   [B~ rows 3..11 (9 x NTMAX) | A~ rows 3..11 (9 x 22) | P_xv (10 x 22) | N_v (10 x NVMAX) | b~ | q~ | r~ | META]  K2 (one bulk copy)
+//   ... followed by p_ev                                                                                           K3 (one bulk copy)
+//   Q~ (22 x 22, full: its two halves are not bitwise symmetric)                                                   K2
+//   P~ null-space rows (nv x 22 of NVMAX x 22; the stance-force rows of P~ are zero)                               K2
+//   R~ packed: one 3x3 block per stance contact (force columns 3b..3b+2), then the nv x nv null block (ld NVMAX)   K2
+// The closed-form parts are not stored: A~ rows 0..2 = [I 0], A~ rows 12..21 = [0 I] + dt P_xv, B~ rows 0..2 = dt/m at row c % 3 of
+// the force columns c < NF, B~ rows 12..21 = dt N_v on the null-space columns, R~ = I on the padded diagonal and 0 between the blocks.
+// Columns of B~, entries of r~ and N_v beyond nt / nv, R~ blocks of swing contacts and P~ / R~ null rows beyond nv are not written.
+// The bulk copies still stage those bytes (uninitialised); every reader gates them out by nf / nt / nv, so no value depends on them.
+constexpr int PJ_BT = 0, PJ_AT = 144, PJ_PXV = 342, PJ_NV = 562, PJ_BTV = 642, PJ_QV = 664, PJ_RV = 686, PJ_META = 702, PJ_PEV = 710,
+              PJ_QT = 720, PJ_PT = 1204, PJ_RF = 1380, PJ_RN = 1416, PJ_STRIDE = 1480;
+constexpr int PJ_RT_PACKED = PJ_STRIDE - PJ_RF;   // 4 force blocks (36) + the null block (NVMAX x NVMAX)
+static_assert(PJ_AT + 9 * NX == PJ_PXV && PJ_RN + NVMAX * NVMAX == PJ_STRIDE && PJ_PEV + NJ == PJ_QT, "projected record blocks are contiguous");
+static_assert(PJ_QT % 2 == 0 && PJ_PT % 2 == 0 && PJ_RF % 2 == 0 && PJ_STRIDE % 2 == 0, "bulk-copied blocks start on 16 bytes");
 // META: [0] nt, [1] n_stance_force_dims, [2] nv, [3] dt cost, [4] dt defect^2, [5] dt eq^2, [6] overflow flag, [7] dt
 constexpr int RK_STRIDE = NTMAX * NX + NTMAX;  // K (nt x 22, ld 22) + kff
-__host__ __device__ inline int ntp_of(int nt) { return nt <= 6 ? 6 : (nt <= 10 ? 10 : (nt <= 12 ? 12 : 16)); }
 
 // ---------------------------------------------------------------- K0
 struct LinHalf {
@@ -772,9 +784,9 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
   auto m_store = [&](int i, double s) {
     if (i < NX) {
       if (lane < NX) out[PJ_QT + i * NX + lane] = dt * (s + ((i == lane) ? Qd_l : 0.0));
-      else if (nlane) out[PJ_PT + (NF + cc) * NX + i] = dt * s;
+      else if (nlane) out[PJ_PT + cc * NX + i] = dt * s;
     } else if (i < NX + NVMAX) {
-      if (nlane && i - NX < nv) out[PJ_RT + (NF + i - NX) * NTMAX + NF + cc] = dt * s;
+      if (nlane && i - NX < nv) out[PJ_RN + (i - NX) * NVMAX + cc] = dt * s;
     } else {
       if (lane < NX) out[PJ_QV + lane] = dt * (sh.q[lane] + s + lin);
       else if (nlane) out[PJ_RV + NF + cc] = dt * (s + lin);
@@ -819,10 +831,8 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
 #pragma unroll
     for (int kk = 0; kk < NJ; ++kk) sh.b[12 + kk] += dt * tl[kk * TL];
   }
-  // role of the lane in the input-column writes: lanes 0..15 own the stance-force columns c < NF and the padded columns c >= nt,
-  // lanes 22..29 own the null-space columns NF + cc
-  const bool fcol = lane < NF, pcol = lane >= nt && lane < NTMAX;
-  const bool wcol = fcol || pcol || nlane;
+  // role of the lane in the input-column writes: lanes 0..NF-1 own the stance-force columns, lanes 22..29 the null-space columns NF + cc
+  const bool fcol = lane < NF;
   const int col = nlane ? NF + cc : lane;
   int sj = 0;           // input index of stance-force column `lane`
   if (fcol) {
@@ -832,53 +842,27 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
   }
   if (lane < NX) {
 #pragma unroll
-    for (int i = 0; i < 3; ++i) out[PJ_AT + i * NX + lane] = (i == lane) ? 1.0 : 0.0;
-#pragma unroll
-    for (int i = 0; i < 9; ++i) out[PJ_AT + (3 + i) * NX + lane] = at9[i];
-#pragma unroll
-    for (int i = 0; i < NJ; ++i) out[PJ_AT + (12 + i) * NX + lane] = ((12 + i == lane) ? 1.0 : 0.0) + dt * tl[i * TL];
+    for (int i = 0; i < 9; ++i) out[PJ_AT + i * NX + lane] = at9[i];
 #pragma unroll
     for (int i = 0; i < NJ; ++i) out[PJ_PXV + i * NX + lane] = tl[i * TL];
-  } else if (cc >= 0 && cc < NVMAX) {
+  } else if (nlane) {
 #pragma unroll
-    for (int i = 0; i < NJ; ++i) out[PJ_NV + i * NVMAX + cc] = nlane ? tl[i * TL] : 0.0;
+    for (int i = 0; i < NJ; ++i) out[PJ_NV + i * NVMAX + cc] = tl[i * TL];
   } else if (lane == 30) {
 #pragma unroll
     for (int i = 0; i < NJ; ++i) out[PJ_PEV + i] = tl[i * TL];
   }
-  if (wcol) {
-    const int sa = sj % 3;
+  if (fcol || nlane) {
 #pragma unroll
-    for (int i = 0; i < 3; ++i) out[PJ_BT + i * NTMAX + col] = (fcol && i == sa) ? dt * im : 0.0;
-#pragma unroll
-    for (int i = 0; i < 9; ++i) out[PJ_BT + (3 + i) * NTMAX + col] = fcol ? BdF[i * 12 + sj] : (nlane ? at9[i] : 0.0);
-#pragma unroll
-    for (int i = 0; i < NJ; ++i) out[PJ_BT + (12 + i) * NTMAX + col] = nlane ? dt * tl[i * TL] : 0.0;
-    if (!nlane) {
-#pragma unroll
-      for (int i = 0; i < NX; ++i) out[PJ_PT + col * NX + i] = 0.0;
-      out[PJ_RV + col] = fcol ? dt * sh.r[sj] : 0.0;
-    }
-    // Rt column: stance-force block (3x3 per contact), identity on the padded diagonal, zeros between the blocks
-    int cnt = 0;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      if (!((flm >> c) & 1u)) continue;
-#pragma unroll
-      for (int ax = 0; ax < 3; ++ax) {
-        double v = 0.0;
-        if (fcol && sj / 3 == c) v = dt * sh.RFF[c * 9 + ax * 3 + sa];
-        if (cnt < NF) out[PJ_RT + cnt * NTMAX + col] = v;
-        ++cnt;
-      }
-    }
-#pragma unroll
-    for (int i = NF; i < NTMAX; ++i) {
-      if (nlane) { if (i >= nt) out[PJ_RT + i * NTMAX + col] = 0.0; }
-      else out[PJ_RT + i * NTMAX + col] = (pcol && i == col) ? 1.0 : 0.0;
-    }
+    for (int i = 0; i < 9; ++i) out[PJ_BT + i * NTMAX + col] = fcol ? BdF[i * 12 + sj] : at9[i];
   }
-  // a null lane's Rt rows NF..nt-1 with cc2 >= nv do not exist (nv rows); rows of inactive null columns are padded columns (lanes >= nt)
+  if (fcol) {
+    // column sa of the 3x3 R~ block of this lane's contact, stored as block lane / 3 (the contact's rank among the stance contacts)
+    const int sa = sj % 3;
+    out[PJ_RV + col] = dt * sh.r[sj];
+#pragma unroll
+    for (int ax = 0; ax < 3; ++ax) out[PJ_RF + 9 * (lane / 3) + ax * 3 + sa] = dt * sh.RFF[(sj / 3) * 9 + ax * 3 + sa];
+  }
   __syncwarp();
   // bt = b + Bd_v pev + dt pev - Bd_F[:, swing] F_swing
   if (lane < NX) {
@@ -967,17 +951,6 @@ __device__ __forceinline__ void acc_rows(double (&c)[N], AF a, const double* __r
   }
 }
 
-// the same for KN rows of the right operand given in closed form: c[j] = fma(a(k), b(k, j), c[j])
-template <int N, int KN, class AF, class BF>
-__device__ __forceinline__ void acc_rows_gen(double (&c)[N], AF a, BF b) {
-#pragma unroll 2
-  for (int k = 0; k < KN; ++k) {
-    const double ak = a(k);
-#pragma unroll
-    for (int j = 0; j < N; ++j) c[j] = fma(ak, b(k, j), c[j]);
-  }
-}
-
 // Row-owner shell: lane i < m owns row i of C (N columns): c starts at 0 (MODE 0) or at C (MODE 1), body(c, i) accumulates, c is stored.
 template <int N, int MODE, bool TC = false, class Body>
 __device__ __forceinline__ void rowmm_by(double* __restrict__ C, int ldc, int m, Body body) {
@@ -1001,32 +974,60 @@ __device__ __forceinline__ void rowmm(double* __restrict__ C, int ldc, const dou
 
 
 constexpr int SB_LD = 18;
-// Node inputs as staged in shared memory. Of A~ (22 x 22) and B~ (22 x NTMAX) only the rows that carry data are staged: A~ rows 3..21
-// and B~ rows 3..11, plus N_v. The other rows are closed-form values that lq_node writes, regenerated here as the same doubles and
-// consumed by the same fma in the same order, so the recursion is bit-identical to one that stages the full matrices:
-//   A~ rows 0..2   the identity rows
-//   B~ rows 0..2   dt/m (dt * (1/m)) at row c % 3 of each stance-force column c < NF, zero elsewhere
-//   B~ rows 12..21 dt N_v on the null-space columns NF .. NF+nv-1, zero on the others
-struct RicNodeIn { double At3[19 * NX], Bt9[9 * NTMAX], Nv[NJ * NVMAX], bt[NX], qt[NX], rt[NTMAX], meta[8]; };
-struct BtGen {                                    // per-node data of the closed-form rows of B~, from the staged META
-  double dt, dtim; int nf, nv;
-  __device__ explicit BtGen(const double* meta) : dt(meta[7]), dtim(meta[7] * (1.0 / c_model.total_mass)), nf((int)meta[1]), nv((int)meta[2]) {}
+// Node inputs as staged in shared memory: the leading span of the projected record, one bulk copy. The rows of A~ and B~ that the record
+// does not store are closed-form values; the recursion multiplies only the support of each row and column of A~ and B~:
+//   A~ rows 0..2    the identity rows: adds (fma(a, 1.0, c) rounds as a + c), except in Qt + At' SA, where a lane-owned row would
+//                   cost registers below the 8-blocks/SM budget
+//   A~ rows 12..21  [0 I] + dt P_xv, regenerated in place of the staged P_xv with the fma lq_node used for them
+//   B~ rows 0..2    dt/m (dt * (1/m)) at row c % 3 of each stance-force column c < nf
+//   B~ rows 12..21  dt N_v on the null-space columns nf .. nt-1
+//   padded columns  nt .. NTP-1 of B~ are zero: no rows at all
+// Skipping fma(a, 0.0, c) leaves c as it was, and the remaining terms keep their order, so every value is the one the full products
+// give (the sign of an exact zero aside).
+struct RicNodeIn { double Bt9[9 * NTMAX], At3[19 * NX], Nv[NJ * NVMAX], bt[NX], qt[NX], rt[NTMAX], meta[8]; };
+static_assert(offsetof(RicNodeIn, At3) == PJ_AT * sizeof(double) && offsetof(RicNodeIn, Nv) == PJ_NV * sizeof(double) &&
+              offsetof(RicNodeIn, meta) == PJ_META * sizeof(double) && sizeof(RicNodeIn) == PJ_PEV * sizeof(double), "RicNodeIn mirrors the record");
+// Column classes of a node: nf stance-force columns, then the null-space columns up to nt, then padding up to NTP. NF >= 0: the regular
+// class of a stance (12), single-support (6) or flight (0) node, with NF and NT known at compile time; NF < 0: any other node (rank
+// loss of the contact-velocity rows), classes read from META.
+__host__ __device__ constexpr int nt_regular(int nf) { return nf == 12 ? 12 : (nf == 6 ? 9 : 6); }
+template <int NF>
+struct NodeCols {
+  double dt, dtim; int nf, nt;
+  __device__ explicit NodeCols(const double* meta)
+      : dt(meta[7]), dtim(meta[7] * (1.0 / c_model.total_mass)), nf(NF >= 0 ? NF : (int)meta[1]), nt(NF >= 0 ? nt_regular(NF) : (int)meta[1] + (int)meta[2]) {}
+  __device__ bool force(int c) const { return c < nf; }
+  __device__ bool null(int c) const { return c >= nf && c < nt; }
+  __device__ bool data(int c) const { return c < nt; }
 };
-__device__ __forceinline__ double bt_top(const BtGen& g, int k, int c) { return (c < g.nf && c % 3 == k) ? g.dtim : 0.0; }
-__device__ __forceinline__ double bt_null(const RicNodeIn& in, const BtGen& g, int r, int c) {
-  return (c >= g.nf && c - g.nf < g.nv) ? g.dt * in.Nv[r * NVMAX + c - g.nf] : 0.0;
-}
-// entry (k, c) of B~ and of A~ for a lane-owned column c; k is a compile-time index wherever these are called (unrolled loops)
-__device__ __forceinline__ double bt_entry(const RicNodeIn& in, const BtGen& g, int k, int c) {
-  return k < 3 ? bt_top(g, k, c) : (k < 12 ? in.Bt9[(k - 3) * NTMAX + c] : bt_null(in, g, k - 12, c));
-}
-__device__ __forceinline__ double at_entry(const RicNodeIn& in, int k, int c) { return k < 3 ? ((k == c) ? 1.0 : 0.0) : in.At3[(k - 3) * NX + c]; }
-// c[j] += sum_k a(k) B~[k][j] (B~ as the right operand), k = 0..21 in order
-template <int NTP, class AF>
-__device__ __forceinline__ void acc_bt(double (&c)[NTP], const RicNodeIn& in, const BtGen& g, AF a) {
-  acc_rows_gen<NTP, 3>(c, a, [&](int k, int j) { return bt_top(g, k, j); });
-  acc_rows(c, [&](int k) { return a(k + 3); }, in.Bt9, NTMAX, 9);
-  acc_rows_gen<NTP, NJ>(c, [&](int k) { return a(k + 12); }, [&](int k, int j) { return bt_null(in, g, k, j); });
+// c[j] += sum_k a(k) B~[k][j] (B~ as the right operand), k = 0..21 in order, over the support of each column j
+template <int NTP, int NF, class AF>
+__device__ __forceinline__ void acc_bt(double (&c)[NTP], const RicNodeIn& in, const NodeCols<NF>& g, AF a) {
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const double ak = a(k);
+#pragma unroll
+    for (int j = k; j < NTP; j += 3) if (g.force(j)) c[j] = fma(ak, g.dtim, c[j]);
+  }
+#pragma unroll 2
+  for (int k = 0; k < 9; ++k) {
+    const double ak = a(k + 3);
+    const double* br = in.Bt9 + k * NTMAX;
+#pragma unroll
+    for (int j = 0; j < NTP; j += 2) {
+      if (g.data(j)) {
+        const double2 b2 = *reinterpret_cast<const double2*>(br + j);
+        c[j] = fma(ak, b2.x, c[j]);
+        if (g.data(j + 1)) c[j + 1] = fma(ak, b2.y, c[j + 1]);
+      }
+    }
+  }
+#pragma unroll 2
+  for (int k = 0; k < NJ; ++k) {
+    const double ak = a(k + 12);
+#pragma unroll
+    for (int j = 0; j < NTP; ++j) if (g.null(j)) c[j] = fma(ak, g.dt * in.Nv[k * NVMAX + j - g.nf], c[j]);
+  }
 }
 
 struct RicShared {
@@ -1035,9 +1036,13 @@ struct RicShared {
   double SBK[NX * SB_LD];                            // SB (22 x NTP, leading dimension 18: 2-way instead of 16-way bank conflicts on the row-owner stores), later K (NTMAX x 22)
   double Hux[NTMAX * NX], Huu[NTMAX * 18];           // Hux input-major (NTMAX x 22): lanes = state index touch consecutive addresses
   double sv[NX], sb[NX], hu[NTMAX], kff[NTMAX];
-  unsigned long long bar[4];                         // mbarriers of the TMA staging: node inputs (two buffers), Pt / Rt, Qt
+  unsigned long long bar[4];                         // mbarriers of the TMA staging: node inputs (two buffers), P~ / R~, Q~
 };
-static_assert(sizeof(RicNodeIn) % 16 == 0 && (TS * sizeof(double)) % 16 == 0 && (NX * NTMAX * sizeof(double)) % 16 == 0, "bulk copies need 16-byte multiples");
+// The packed R~ lands at the end of Huu and is expanded from there (every entry read before any is written)
+constexpr int HUU_RP = NTMAX * 18 - PJ_RT_PACKED;
+constexpr int SA_SPLIT = 14;                         // phase A: columns 0..13 of SA on warp 0, 14..21 (with SB, sb) on warp 1
+static_assert(sizeof(RicNodeIn) % 16 == 0 && (TS * sizeof(double)) % 16 == 0 && (NX * sizeof(double)) % 16 == 0 && HUU_RP % 2 == 0 &&
+              (PJ_RT_PACKED * sizeof(double)) % 16 == 0 && SA_SPLIT % 2 == 0, "bulk copies and 128-bit loads need 16-byte multiples");
 // One block per instance: 8 blocks per SM put a 1024-instance batch in one wave on 132 SMs (8 x 132 >= 1024; at 7 a tail wave of 100
 // blocks costs almost as much as the full one). The runtime reserves 1 KB of shared memory per block.
 static_assert(8 * (sizeof(RicShared) + 1024) <= 228 * 1024, "riccati_kernel must fit 8 blocks per SM");
@@ -1046,37 +1051,41 @@ static_assert(8 * (sizeof(RicShared) + 1024) <= 228 * 1024, "riccati_kernel must
 __device__ __forceinline__ void ric_prefetch_tma(RicNodeIn& n, const double* __restrict__ rec, unsigned long long* bar) {
   fence_proxy_async();
   mbar_expect_tx(bar, (unsigned)sizeof(RicNodeIn));
-  bulk_g2s(n.At3, rec + PJ_AT + 3 * NX, sizeof(n.At3), bar);
-  bulk_g2s(n.Bt9, rec + PJ_BT + 3 * NTMAX, sizeof(n.Bt9), bar);
-  bulk_g2s(n.Nv, rec + PJ_NV, sizeof(n.Nv), bar);
-  bulk_g2s(n.bt, rec + PJ_BTV, sizeof(n.bt), bar);
-  bulk_g2s(n.qt, rec + PJ_QV, sizeof(n.qt), bar);
-  bulk_g2s(n.rt, rec + PJ_RV, sizeof(n.rt), bar);
-  bulk_g2s(n.meta, rec + PJ_META, sizeof(n.meta), bar);
+  bulk_g2s(&n, rec, sizeof(RicNodeIn), bar);
 }
 
 // One node of the recursion, executed by the TWO warps of the block. The products that do not depend on each other are split
 // between the warps (by result columns, so that every row-owner product keeps its full lane utilisation); the Cholesky of Huu and
 // the gain solve (one warp, latency bound) overlap with the largest product At' S At of the other warp.
-template <int NTP>
-__device__ __noinline__ void riccati_node(RicShared& sh, const RicNodeIn& in, const double* __restrict__ rec, double* __restrict__ rk, bool& fail,
+template <int NTP, int NF>
+__device__ __noinline__ void riccati_node(RicShared& sh, RicNodeIn& in, const double* __restrict__ rec, double* __restrict__ rk, bool& fail,
                                           int warp, unsigned ph) {
   const int lane = lane_id();
-  const BtGen g(in.meta);
+  const NodeCols<NF> g(in.meta);
   double* SB = sh.SBK; double* K = sh.SBK;
-  // ---- phase A: [SA | SB | sb] = S [At | Bt | bt] (+ s): 22 + NTP + 1 result columns, split 16 / rest. S is exactly symmetric (both halves
-  // are written with the same value at the end of every node), so lane i reads its row as column i: consecutive addresses, no bank conflicts
-  // (S^T: lane i reads S[k][i]; the identity rows of At contribute through fma with 1.0 / 0.0 as in the full product)
+  {
+    // A~ rows 12..21 over this warp's phase-A columns, in place of the staged P_xv: fma(P_xv, dt, 1 or 0) as lq_node formed them
+    const int c0 = warp == 0 ? 0 : SA_SPLIT, w = warp == 0 ? SA_SPLIT : NX - SA_SPLIT;
+    for (int idx = lane; idx < NJ * w; idx += 32) {
+      const int r = idx / w, j = c0 + idx - r * w;
+      double& v = in.At3[(9 + r) * NX + j];
+      v = __fma_rn(v, g.dt, (12 + r == j) ? 1.0 : 0.0);
+    }
+    __syncwarp();
+  }
+  // ---- phase A: [SA | SB | sb] = S [At | Bt | bt] (+ s): 22 + NTP + 1 result columns, split SA_SPLIT / rest. S is exactly symmetric (both
+  // halves are written with the same value at the end of every node), so lane i reads its row as column i: consecutive addresses, no
+  // bank conflicts (S^T: lane i reads S[k][i])
   if (warp == 0) {
-    rowmm_by<16, 0>(sh.SA, NX, NX, [&](double (&c)[16], int i) {
-      acc_rows_gen<16, 3>(c, [&](int k) { return sh.S[k * NX + i]; }, [](int k, int j) { return (k == j) ? 1.0 : 0.0; });
+    rowmm_by<SA_SPLIT, 0>(sh.SA, NX, NX, [&](double (&c)[SA_SPLIT], int i) {
+#pragma unroll
+      for (int j = 0; j < 3; ++j) c[j] = c[j] + sh.S[j * NX + i];
       acc_rows(c, [&](int k) { return sh.S[(k + 3) * NX + i]; }, in.At3, NX, 19);
     });
-    mbar_wait(&sh.bar[2], ph);                // Pt / Rt staged by this warp at the top of the node
+    mbar_wait(&sh.bar[2], ph);                // P~ / R~ staged by this warp at the top of the node
   } else {
-    rowmm_by<6, 0>(sh.SA + 16, NX, NX, [&](double (&c)[6], int i) {
-      acc_rows_gen<6, 3>(c, [&](int k) { return sh.S[k * NX + i]; }, [](int, int) { return 0.0; });
-      acc_rows(c, [&](int k) { return sh.S[(k + 3) * NX + i]; }, in.At3 + 16, NX, 19);
+    rowmm_by<NX - SA_SPLIT, 0>(sh.SA + SA_SPLIT, NX, NX, [&](double (&c)[NX - SA_SPLIT], int i) {
+      acc_rows(c, [&](int k) { return sh.S[(k + 3) * NX + i]; }, in.At3 + SA_SPLIT, NX, 19);
     });
     rowmm_by<NTP, 0>(SB, SB_LD, NX, [&](double (&c)[NTP], int i) { acc_bt(c, in, g, [&](int k) { return sh.S[k * NX + i]; }); });
     if (lane < NX) {
@@ -1089,19 +1098,40 @@ __device__ __noinline__ void riccati_node(RicShared& sh, const RicNodeIn& in, co
   __syncthreads();
   // ---- phase B: Hux (NTP x 22, stored input-major) = Pt + Bt^T SA (warp 0: row-owner over the state index, transposed store) ; Huu = Rt + Bt^T SB, hu = rt + Bt^T sb (warp 1)
   if (warp == 0) {
-    rowmm_by<NTP, 1, true>(sh.Hux, NX, NX, [&](double (&c)[NTP], int i) { acc_bt(c, in, g, [&](int k) { return sh.SA[k * NX + i]; }); });
+    rowmm_by<NTP, 0, true>(sh.Hux, NX, NX, [&](double (&c)[NTP], int i) {     // P~ is zero outside the null-space rows
+#pragma unroll
+      for (int j = 0; j < NTP; ++j) if (g.null(j)) c[j] = sh.Hux[j * NX + i];
+      acc_bt(c, in, g, [&](int k) { return sh.SA[k * NX + i]; });
+    });
   } else {
     // S is dead until phase C: stage Qt into it now (arrives while Huu is formed)
     if (lane == 0) { fence_proxy_async(); mbar_expect_tx(&sh.bar[3], TS * sizeof(double)); bulk_g2s(sh.S, rec + PJ_QT, TS * sizeof(double), &sh.bar[3]); }
-    rowmm_by<NTP, 1>(sh.Huu, 18, NTP, [&](double (&c)[NTP], int i) {      // Bt^T: lane i owns column i of Bt
-      acc_rows(c, [&](int k) { return bt_top(g, k, i); }, SB, SB_LD, 3);
-      acc_rows(c, [&](int k) { return in.Bt9[k * NTMAX + i]; }, SB + 3 * SB_LD, SB_LD, 9);
-      acc_rows(c, [&](int k) { return bt_null(in, g, k, i); }, SB + 12 * SB_LD, SB_LD, NJ);
+    rowmm_by<NTP, 0>(sh.Huu, 18, NTP, [&](double (&c)[NTP], int i) {      // Bt^T: lane i owns column i of Bt
+      // row i of R~ from its packed blocks at Huu + HUU_RP: 3x3 force blocks, the null block, I on the padded diagonal. Every lane
+      // reads its row before any lane stores one over the packed blocks.
+      const double* rp = sh.Huu + HUU_RP;
+#pragma unroll
+      for (int j = 0; j < NTP; ++j) {
+        if (g.force(i) && g.force(j) && i / 3 == j / 3) c[j] = rp[9 * (i / 3) + (i % 3) * 3 + j % 3];
+        else if (g.null(i) && g.null(j)) c[j] = rp[PJ_RN - PJ_RF + (i - g.nf) * NVMAX + j - g.nf];
+        else if (i == j && !g.data(i)) c[j] = 1.0;
+      }
+      __syncwarp((1u << NTP) - 1u);
+      if (g.force(i)) acc_rows(c, [&](int) { return g.dtim; }, SB + (i % 3) * SB_LD, SB_LD, 1);
+      if (g.data(i)) acc_rows(c, [&](int k) { return in.Bt9[k * NTMAX + i]; }, SB + 3 * SB_LD, SB_LD, 9);
+      if (g.null(i)) acc_rows(c, [&](int k) { return g.dt * in.Nv[k * NVMAX + i - g.nf]; }, SB + 12 * SB_LD, SB_LD, NJ);
     });
     if (lane < NTP) {
-      double s0 = in.rt[lane];
+      double s0 = g.data(lane) ? in.rt[lane] : 0.0;
+      if (g.force(lane)) s0 = fma(g.dtim, sh.sb[lane % 3], s0);
+      if (g.data(lane)) {
 #pragma unroll
-      for (int k = 0; k < NX; ++k) s0 = fma(bt_entry(in, g, k, lane), sh.sb[k], s0);
+        for (int k = 0; k < 9; ++k) s0 = fma(in.Bt9[k * NTMAX + lane], sh.sb[3 + k], s0);
+      }
+      if (g.null(lane)) {
+#pragma unroll
+        for (int k = 0; k < NJ; ++k) s0 = fma(g.dt * in.Nv[k * NVMAX + lane - g.nf], sh.sb[12 + k], s0);
+      }
       sh.hu[lane] = s0;
     }
   }
@@ -1131,10 +1161,8 @@ __device__ __noinline__ void riccati_node(RicShared& sh, const RicNodeIn& in, co
       }
       double col[NTP], y[NTP];
 #pragma unroll
-      for (int c = 0; c < NTP; ++c) col[c] = (lane < NX) ? sh.Hux[c * NX + lane] : ((lane == NX) ? sh.hu[c] : 0.0);
-#pragma unroll
       for (int c = 0; c < NTP; ++c) {
-        double sacc = col[c];
+        double sacc = (lane < NX) ? sh.Hux[c * NX + lane] : ((lane == NX) ? sh.hu[c] : 0.0);
 #pragma unroll
         for (int kk = 0; kk < c; ++kk) sacc = fma(-__shfl_sync(HB_FULL_MASK, a[kk], c), y[kk], sacc);
         y[c] = sacc * rinv[c];
@@ -1158,8 +1186,13 @@ __device__ __noinline__ void riccati_node(RicShared& sh, const RicNodeIn& in, co
     // s <- qt + At' sb + Hux' kff
     if (lane < NX) {
       double s0 = in.qt[lane], s1 = 0.0;
+      if (lane == 1) s1 = s1 + sh.sb[1];                    // rows 0..2 of A~ (identity), even rows on s0 and odd rows on s1
+      else if (lane < 3) s0 = s0 + sh.sb[lane];
 #pragma unroll
-      for (int k = 0; k < NX; k += 2) { s0 = fma(at_entry(in, k, lane), sh.sb[k], s0); s1 = fma(at_entry(in, k + 1, lane), sh.sb[k + 1], s1); }
+      for (int k = 3; k < NX; ++k) {
+        if (k & 1) s1 = fma(in.At3[(k - 3) * NX + lane], sh.sb[k], s1);
+        else s0 = fma(in.At3[(k - 3) * NX + lane], sh.sb[k], s0);
+      }
 #pragma unroll
       for (int c = 0; c < NTP; ++c) s0 = fma(sh.Hux[c * NX + lane], sh.kff[c], s0);
       sh.sv[lane] = s0 + s1;
@@ -1212,26 +1245,25 @@ __global__ void __launch_bounds__(64) riccati_kernel(SqpArgs a) {
     // every thread waits for the inputs of node k (prefetched one node ahead); the two block barriers that end the previous node already
     // order the re-use of Hux / Huu / the other input buffer, so no barrier is needed here
     if (k & 1) { mbar_wait(&sh.bar[1], ph_in1); ph_in1 ^= 1u; } else { mbar_wait(&sh.bar[0], ph_in0); ph_in0 ^= 1u; }
+    RicNodeIn& in = sh.in[k & 1];
+    const int nt = (int)in.meta[0], nf = (int)in.meta[1], nv = (int)in.meta[2];
     if (warp == 0) {
       if (lane == 0) {
-        // Pt -> Hux (16 x 22, contiguous) and Rt -> Huu (16 rows of 16 doubles, leading dimension 18): 1 + 16 bulk copies on one mbarrier
+        // P~ null rows -> rows nf .. nt-1 of Hux (input-major, contiguous) and the packed R~ -> the end of Huu: 2 bulk copies on one mbarrier
         fence_proxy_async();
-        mbar_expect_tx(&sh.bar[2], (unsigned)((NX * NTMAX + NTMAX * NTMAX) * sizeof(double)));
-        bulk_g2s(sh.Hux, rec + PJ_PT, NX * NTMAX * sizeof(double), &sh.bar[2]);
-        for (int r = 0; r < NTMAX; ++r) bulk_g2s(sh.Huu + r * 18, rec + PJ_RT + r * NTMAX, NTMAX * sizeof(double), &sh.bar[2]);
+        mbar_expect_tx(&sh.bar[2], (unsigned)((nv * NX + PJ_RT_PACKED) * sizeof(double)));
+        if (nv > 0) bulk_g2s(sh.Hux + nf * NX, rec + PJ_PT, nv * NX * sizeof(double), &sh.bar[2]);
+        bulk_g2s(sh.Huu + HUU_RP, rec + PJ_RF, PJ_RT_PACKED * sizeof(double), &sh.bar[2]);
       }
     } else if (k > 0 && lane == 0) {
       ric_prefetch_tma(sh.in[(k - 1) & 1], proj + (size_t)(k - 1) * PJ_STRIDE, &sh.bar[(k - 1) & 1]);
     }
-    const RicNodeIn& in = sh.in[k & 1];
-    const int nt = (int)in.meta[0];
     merit += in.meta[3]; dyn += in.meta[4]; eqs += in.meta[5];
     if (in.meta[6] != 0.0) fail = true;
-    const int ntp = ntp_of(nt);
-    if (ntp == 12) riccati_node<12>(sh, in, rec, rk, fail, warp, ph);
-    else if (ntp == 10) riccati_node<10>(sh, in, rec, rk, fail, warp, ph);
-    else if (ntp == 6) riccati_node<6>(sh, in, rec, rk, fail, warp, ph);
-    else riccati_node<16>(sh, in, rec, rk, fail, warp, ph);
+    if (nf == 12 && nt == nt_regular(12)) riccati_node<12, 12>(sh, in, rec, rk, fail, warp, ph);
+    else if (nf == 6 && nt == nt_regular(6)) riccati_node<10, 6>(sh, in, rec, rk, fail, warp, ph);
+    else if (nf == 0 && nt == nt_regular(0)) riccati_node<6, 0>(sh, in, rec, rk, fail, warp, ph);
+    else riccati_node<NTMAX, -1>(sh, in, rec, rk, fail, warp, ph);
   }
   if (threadIdx.x == 0) {
     double* pf = a.perf + (size_t)inst * 4;
@@ -1242,12 +1274,16 @@ __global__ void __launch_bounds__(64) riccati_kernel(SqpArgs a) {
 
 // ---------------------------------------------------------------- K3: forward pass + filter line search
 // per-node data of the forward pass, double-buffered and filled with cp.async (16-byte LDGSTS) one node ahead
-// Of A~ and B~ the forward pass loads rows 3..11 only: rows 0..2 are the identity plus dt/m on the stance-force coordinates, rows 12..21 are
-// I + dt P_xv and dt N_v, and P_xv / N_v are loaded anyway for the input step (8.9 KB per node instead of 12.8 KB; this kernel runs at half of HBM).
+// The record stores rows 3..11 of A~ and B~ only: rows 0..2 are the identity plus dt/m on the stance-force coordinates, rows 12..21 are
+// I + dt P_xv and dt N_v, and P_xv / N_v are loaded anyway for the input step. Three bulk copies: the leading span of the projected
+// record, the gains (K then kff) and the input.
 struct FwNode {
-  double At9[9 * NX], Bt9[9 * NTMAX], K[NTMAX * NX], Pxv[NJ * NX], Nv[NJ * NVMAX];
-  double bt[NX], qt[NX], kff[NTMAX], rt[NTMAX], pev[NJ], meta[8], u[NU];
+  double Bt9[9 * NTMAX], At9[9 * NX], Pxv[NJ * NX], Nv[NJ * NVMAX], bt[NX], qt[NX], rt[NTMAX], meta[8], pev[NJ];
+  double K[NTMAX * NX], kff[NTMAX], u[NU];
 };
+static_assert(offsetof(FwNode, At9) == PJ_AT * sizeof(double) && offsetof(FwNode, pev) == PJ_PEV * sizeof(double) &&
+              offsetof(FwNode, K) == PJ_QT * sizeof(double) && offsetof(FwNode, u) == offsetof(FwNode, K) + RK_STRIDE * sizeof(double),
+              "FwNode mirrors the record and the gains");
 struct Fw2Shared {
   FwNode nd[2];
   double dx[NX], dxn[NX], w[NTMAX];
@@ -1259,17 +1295,8 @@ __device__ __forceinline__ void fw_prefetch_tma(FwNode& n, const double* __restr
                                                 unsigned long long* bar) {
   fence_proxy_async();
   mbar_expect_tx(bar, (unsigned)sizeof(FwNode));
-  bulk_g2s(n.At9, rec + PJ_AT + 3 * NX, sizeof(n.At9), bar);
-  bulk_g2s(n.Bt9, rec + PJ_BT + 3 * NTMAX, sizeof(n.Bt9), bar);
-  bulk_g2s(n.K, rk, sizeof(n.K), bar);
-  bulk_g2s(n.Pxv, rec + PJ_PXV, sizeof(n.Pxv), bar);
-  bulk_g2s(n.Nv, rec + PJ_NV, sizeof(n.Nv), bar);
-  bulk_g2s(n.bt, rec + PJ_BTV, sizeof(n.bt), bar);
-  bulk_g2s(n.qt, rec + PJ_QV, sizeof(n.qt), bar);
-  bulk_g2s(n.kff, rk + NTMAX * NX, sizeof(n.kff), bar);
-  bulk_g2s(n.rt, rec + PJ_RV, sizeof(n.rt), bar);
-  bulk_g2s(n.pev, rec + PJ_PEV, sizeof(n.pev), bar);
-  bulk_g2s(n.meta, rec + PJ_META, sizeof(n.meta), bar);
+  bulk_g2s(n.Bt9, rec, PJ_QT * sizeof(double), bar);
+  bulk_g2s(n.K, rk, RK_STRIDE * sizeof(double), bar);
   bulk_g2s(n.u, uk, sizeof(n.u), bar);
 }
 
