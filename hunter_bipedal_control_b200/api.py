@@ -37,6 +37,7 @@ EXPORTED_SYMBOLS = [
     "hb_time_grid_batch_dev", "hb_reference_expand_grid_batch_dev", "hb_mpc_solve_grid_batch_dev", "hb_policy_eval_grid_batch_dev",
     "hb_time_grid_batch", "hb_reference_expand_grid_batch", "hb_mpc_solve_grid_batch", "hb_resident_read_grid_batch", "hb_resident_write_batch",
     "hb_default_rollout_params", "hb_rollout_batch_dev", "hb_rollout_set_pushes", "hb_sim_step_wrench",
+    "hb_default_plant_variation", "hb_rollout_set_plant_variations", "hb_sim_step_varied",
     "hb_default_estimation_params", "hb_estimation_reset", "hb_sim_read_sensors_batch_dev", "hb_sim_read_sensors", "hb_rollout_estimated_batch_dev",
 ]
 
@@ -253,6 +254,60 @@ def make_push_schedules(B, t_start, duration, force, torque=None):
     v = np.ctypeslib.as_array(out)
     v["n_push"] = n
     v["t_start"][:, :n] = tim; v["duration"][:, :n] = dur; v["force"][:, :n] = frc; v["torque"][:, :n] = trq
+    return out
+
+
+class HbPlantVariation(C.Structure):
+    _fields_ = [("payload_mass", C.c_double), ("payload_com", C.c_double * 3), ("payload_inertia", C.c_double * 9), ("friction_scale", C.c_double),
+                ("stiffness_scale", C.c_double), ("damping_scale", C.c_double), ("motor_strength", C.c_double * NJ)]
+
+
+def default_plant_variation():
+    """hb_default_plant_variation: the nominal plant (no payload, every scale 1)."""
+    v = HbPlantVariation()
+    _check(load_library().hb_default_plant_variation(C.byref(v)), "hb_default_plant_variation")
+    return v
+
+
+def _psd_by_minors(I):
+    """Sylvester's criterion for semidefiniteness of the symmetric 3 x 3 matrices I (..., 3, 3): no negative principal minor."""
+    d = [I[..., 0, 0], I[..., 1, 1], I[..., 2, 2],
+         I[..., 0, 0] * I[..., 1, 1] - I[..., 0, 1] * I[..., 1, 0], I[..., 0, 0] * I[..., 2, 2] - I[..., 0, 2] * I[..., 2, 0],
+         I[..., 1, 1] * I[..., 2, 2] - I[..., 1, 2] * I[..., 2, 1],
+         I[..., 0, 0] * (I[..., 1, 1] * I[..., 2, 2] - I[..., 1, 2] * I[..., 2, 1]) - I[..., 0, 1] * (I[..., 1, 0] * I[..., 2, 2] - I[..., 1, 2] * I[..., 2, 0])
+         + I[..., 0, 2] * (I[..., 1, 0] * I[..., 2, 1] - I[..., 1, 1] * I[..., 2, 0])]
+    return np.all([m >= 0 for m in d], axis=0)
+
+
+def make_plant_variations(B, payload_mass=0.0, payload_com=(0.0, 0.0, 0.0), payload_inertia=None, friction_scale=1.0, stiffness_scale=1.0,
+                          damping_scale=1.0, motor_strength=1.0):
+    """ctypes array of B HbPlantVariation (Context.set_plant_variations, Context.sim_step). Instance i carries a payload of payload_mass[i]
+    [kg] with its CoM at payload_com[i] (base frame, from the base origin) and inertia payload_inertia[i] (3 x 3 about the CoM, base frame;
+    None: zero), on ground of friction_scale[i] * mu, stiffness_scale[i] * k and damping_scale[i] * d, with motor_strength[i, j] scaling the
+    torque of joint j. Scalars and per-instance arrays broadcast: masses and scales () or (B,), payload_com (3,) or (B, 3), payload_inertia
+    (3, 3) or (B, 3, 3), motor_strength (), (10,) or (B, 10) (per instance only: (B, 1)). Raises ValueError for what
+    hb_rollout_set_plant_variations rejects. The defaults give the nominal plant."""
+    try:
+        m = np.broadcast_to(_f64(payload_mass), (B,)); c = np.broadcast_to(_f64(payload_com), (B, 3))
+        I = np.broadcast_to(np.zeros((3, 3)) if payload_inertia is None else _f64(payload_inertia), (B, 3, 3))
+        fs, ks, ds = (np.broadcast_to(_f64(x), (B,)) for x in (friction_scale, stiffness_scale, damping_scale))
+        ms = np.broadcast_to(_f64(motor_strength), (B, NJ))
+    except ValueError as e:
+        raise ValueError("plant variations: masses / scales (B,), payload_com (B, 3), payload_inertia (B, 3, 3), motor_strength (B, 10) expected: %s"
+                         % e)
+    if not all(np.isfinite(a).all() for a in (m, c, I, fs, ks, ds, ms)):
+        raise ValueError("plant variations: every value must be finite")
+    if not ((m >= 0).all() and (fs >= 0).all() and (ks > 0).all() and (ds >= 0).all() and (ms >= 0).all()):
+        raise ValueError("plant variations: payload_mass, friction_scale, damping_scale and motor_strength must be >= 0, stiffness_scale > 0")
+    if not (np.array_equal(I, np.swapaxes(I, 1, 2)) and _psd_by_minors(I).all()):
+        raise ValueError("plant variations: payload_inertia must be exactly symmetric and positive semidefinite")
+    none = m == 0
+    if (c[none] != 0).any() or (I[none] != 0).any():
+        raise ValueError("plant variations: a zero payload_mass needs a zero payload_com and payload_inertia")
+    out = (HbPlantVariation * B)()
+    v = np.ctypeslib.as_array(out)
+    v["payload_mass"] = m; v["payload_com"] = c; v["payload_inertia"] = I.reshape(B, 9)
+    v["friction_scale"] = fs; v["stiffness_scale"] = ks; v["damping_scale"] = ds; v["motor_strength"] = ms
     return out
 
 
@@ -678,18 +733,31 @@ class Context:
         _check(self._lib.hb_actuation_batch(self._h, B, C.c_double(delay), _ptr(time), state, _ptr(command), _ptr(rbd), _ptr(tau)), "hb_actuation_batch", self._h)
         return tau
 
-    def sim_step(self, rbd, tau, params=None, wrench=None):
+    def sim_step(self, rbd, tau, params=None, wrench=None, variation=None):
         """One control period of the batched rigid-body plant: returns (rbd_next [B,32], contact_force [B,12], contact_flag [B,4]).
-        wrench [B,6] (hb_sim_step_wrench): an external world force at the base origin, then a world couple, held over the period."""
+        wrench [B,6]: an external world force at the base origin, then a world couple, held over the period. variation: B HbPlantVariation
+        (make_plant_variations), the plant of each robot. With either, the step is hb_sim_step_varied."""
         rbd = _f64(rbd).copy(); tau = _f64(tau); B = rbd.shape[0]
         params = params or default_sim_params()
         cf = np.zeros((B, 12)); fl = np.zeros((B, 4), dtype=np.uint8)
-        if wrench is None:
+        if wrench is None and variation is None:
             _check(self._lib.hb_sim_step_batch(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(cf), _ptr(fl)), "hb_sim_step_batch", self._h)
         else:
-            w = _f64(wrench).reshape(B, 6)
-            _check(self._lib.hb_sim_step_wrench(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), _ptr(cf), _ptr(fl)), "hb_sim_step_wrench", self._h)
+            w = None if wrench is None else _f64(wrench).reshape(B, 6)
+            if variation is not None and len(variation) != B:
+                raise ValueError("sim_step: %d plant variations for %d robots" % (len(variation), B))
+            _check(self._lib.hb_sim_step_varied(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), variation, _ptr(cf), _ptr(fl)),
+                   "hb_sim_step_varied", self._h)
         return rbd, cf, fl
+
+    def set_plant_variations(self, variations):
+        """Plant variations of this context's episodes (hb_rollout_set_plant_variations): variations[i] (make_plant_variations) is the plant
+        of instance i of every later rollout / rollout_estimated call, instances beyond len(variations) run the nominal plant; None clears
+        them."""
+        if variations is None:
+            _check(self._lib.hb_rollout_set_plant_variations(self._h, 0, None), "hb_rollout_set_plant_variations", self._h)
+        else:
+            _check(self._lib.hb_rollout_set_plant_variations(self._h, len(variations), variations), "hb_rollout_set_plant_variations", self._h)
 
     def set_pushes(self, schedules):
         """Push schedules of this context's episodes (hb_rollout_set_pushes): schedules[i] (make_push_schedules) acts on instance i of every

@@ -74,6 +74,11 @@ struct hb_ctx {
   hb_push_schedule* push_sched; double* push_wrench;
   int push_n;
   std::vector<hb_push_schedule> push_host;
+  // plant variations of the episodes (hb_rollout_set_plant_variations): the first var_n instances have one; the device copy is allocated
+  // at max_batch by the first call that sets them, var_host keeps the validated array the copy reads
+  hb_plant_variation* var_dev;
+  int var_n;
+  std::vector<hb_plant_variation> var_host;
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
   // hb_resident_cycle_batch's packed references / reference verdicts
   void* arena; size_t arena_cap;
@@ -411,7 +416,7 @@ int hb_destroy(hb_ctx* ctx) {
   void* ptrs[] = {ctx->sqp_mem, ctx->dxt, ctx->dut, ctx->perf, ctx->flags, ctx->xdes, ctx->udes, ctx->wstatus, ctx->witers, ctx->wmode,
                   ctx->hoqp_mem, ctx->cyc_xref, ctx->cyc_swing, ctx->cyc_tk, ctx->cyc_mode, ctx->cyc_nn, ctx->res_t0, ctx->res_xt,
                   ctx->res_ut, ctx->res_tk, ctx->res_mode, ctx->res_nn, ctx->res_sol, ctx->res_stance, ctx->arena, ctx->ro_mem, ctx->re_mem,
-                  ctx->push_mem};
+                  ctx->push_mem, ctx->var_dev};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -855,15 +860,62 @@ int hb_actuation_batch_dev(hb_ctx* ctx, int B, double delay, const double* time,
   return launch(ctx, K_UNPROFILED, actuation_kernel, (B + 63) / 64, 64, 0, B, delay, time, state, command, rbd, tau);
 }
 
-// the plant step after the entry checks; wrench (B x 6) nullable
-static int sim_step(hb_ctx* ctx, int B, const hb_sim_params& params, double* rbd, const double* tau, const double* wrench, double* contact_force,
-                    uint8_t* contact_flag) {
-  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, params, rbd, tau, wrench, contact_force, contact_flag);
+// the plant step after the entry checks; wrench (B x 6) nullable; var (nullable): the plants of instances 0 .. n_var - 1
+static int sim_step(hb_ctx* ctx, int B, const hb_sim_params& params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* var,
+                    int n_var, double* contact_force, uint8_t* contact_flag) {
+  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, params, rbd, tau, wrench, var, n_var, contact_force, contact_flag);
 }
 
 int hb_sim_step_batch_dev(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {
   ENTER(ctx, B, params && rbd && tau && sim_params_ok(*params), UNCAPPED);
-  return sim_step(ctx, B, *params, rbd, tau, nullptr, contact_force, contact_flag);
+  return sim_step(ctx, B, *params, rbd, tau, nullptr, nullptr, 0, contact_force, contact_flag);
+}
+
+int hb_default_plant_variation(hb_plant_variation* v) {
+  if (!v) return HB_EINVAL;
+  memset(v, 0, sizeof(*v));
+  v->friction_scale = 1.0; v->stiffness_scale = 1.0; v->damping_scale = 1.0;
+  for (int j = 0; j < NJ; ++j) v->motor_strength[j] = 1.0;
+  return HB_OK;
+}
+
+// The ranges of hunter_b200.h's hb_plant_variation. The payload inertia is checked for exact symmetry and, by Sylvester's criterion for
+// semidefiniteness, for no negative principal minor (the three diagonal entries, the three 2 x 2 minors and the determinant).
+static bool plant_variation_ok(const hb_plant_variation& v) {
+  const double* I = v.payload_inertia;
+  auto finite = [](const double* x, int n) { for (int i = 0; i < n; ++i) if (!isfinite(x[i])) return false; return true; };
+  if (!finite(&v.payload_mass, 1) || !finite(v.payload_com, 3) || !finite(I, 9) || !finite(&v.friction_scale, 1) || !finite(&v.stiffness_scale, 1) ||
+      !finite(&v.damping_scale, 1) || !finite(v.motor_strength, NJ))
+    return false;
+  if (!(v.payload_mass >= 0.0) || !(v.friction_scale >= 0.0) || !(v.stiffness_scale > 0.0) || !(v.damping_scale >= 0.0)) return false;
+  for (int j = 0; j < NJ; ++j) if (!(v.motor_strength[j] >= 0.0)) return false;
+  if (I[1] != I[3] || I[2] != I[6] || I[5] != I[7]) return false;
+  if (I[0] < 0.0 || I[4] < 0.0 || I[8] < 0.0) return false;
+  if (I[0] * I[4] - I[1] * I[3] < 0.0 || I[0] * I[8] - I[2] * I[6] < 0.0 || I[4] * I[8] - I[5] * I[7] < 0.0) return false;
+  const double det = I[0] * (I[4] * I[8] - I[5] * I[7]) - I[1] * (I[3] * I[8] - I[5] * I[6]) + I[2] * (I[3] * I[7] - I[4] * I[6]);
+  if (det < 0.0) return false;
+  if (v.payload_mass == 0.0) {
+    for (int i = 0; i < 3; ++i) if (v.payload_com[i] != 0.0) return false;
+    for (int i = 0; i < 9; ++i) if (I[i] != 0.0) return false;
+  }
+  return true;
+}
+
+int hb_rollout_set_plant_variations(hb_ctx* ctx, int B, const hb_plant_variation* v) {
+  const int rc = enter(ctx, B, B == 0 || v, CAPPED, [&] {
+    for (int i = 0; i < B; ++i) if (!plant_variation_ok(v[i])) return false;
+    return true;
+  });
+  if (rc == EMPTY) { ctx->var_n = 0; return HB_OK; }      // cleared: the episodes run the nominal plant
+  if (rc) return rc;
+  if (!ctx->var_dev && dalloc(&ctx->var_dev, (size_t)ctx->cfg.max_batch) != cudaSuccess) {
+    cudaGetLastError(); ctx->var_dev = nullptr; return HB_ENOMEM;
+  }
+  // a pageable copy the context owns: cudaMemcpyAsync has consumed it when it returns, whatever memory the caller's array is in
+  try { ctx->var_host.assign(v, v + B); } catch (const std::bad_alloc&) { return HB_ENOMEM; }
+  CK(cudaMemcpyAsync(ctx->var_dev, ctx->var_host.data(), sizeof(hb_plant_variation) * B, cudaMemcpyHostToDevice, ctx->stream));
+  ctx->var_n = B;
+  return HB_OK;
 }
 
 // hb_resident_wbc_batch_dev; no_prev = true: the fallback has no previous solution yet (first tick after a cold start whose cycle ran no WBC)
@@ -992,6 +1044,8 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   double* meas = e ? ctx->re_rbd : rbd;
   // the push wrench the begin kernel writes and the plant applies; none without schedules
   double* wrench = ctx->push_n > 0 ? ctx->push_wrench : nullptr;
+  // the instances' plants; the nominal one for all without variations
+  const hb_plant_variation* var = ctx->var_n > 0 ? ctx->var_dev : nullptr;
   for (int k = 0; k < n_ticks && !rc; ++k) {
     const int64_t a = tick0 + k;
     const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
@@ -1022,7 +1076,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
                                              ctx->ro_jtau);
     if (!rc) rc = hb_actuation_batch_dev(ctx, B, p->actuation_delay, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, ctx->ro_tau);
-    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, nullptr, nullptr);
+    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, var, ctx->var_n, nullptr, nullptr);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_tick_end_kernel, grid, 64, 0, B, (int)a, mpc ? 1 : 0, ctx->ro_info, ctx->ro_pstat, ctx->wstatus, estop, ctx->ro_tau, ctx->ro_held, rbd, stats);
   }
   return rc;
@@ -1437,7 +1491,20 @@ int hb_sim_step_wrench(hb_ctx* ctx, int B, const hb_sim_params* params, double* 
   ENTER(ctx, B, params && rbd && tau, CAPPED, [&] { return sim_params_ok(*params); });
   Staging s(ctx, B);
   auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto w = s.in_or_null(wrench, 6); auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
-  return s.run(1, [&](Chunk) { return sim_step(ctx, B, *params, r, t, w, cf, fl); });
+  return s.run(1, [&](Chunk) { return sim_step(ctx, B, *params, r, t, w, nullptr, 0, cf, fl); });
+}
+
+int hb_sim_step_varied(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* v,
+                       double* contact_force, uint8_t* contact_flag) {
+  ENTER(ctx, B, params && rbd && tau, CAPPED, [&] {
+    if (!sim_params_ok(*params)) return false;
+    if (v) for (int i = 0; i < B; ++i) if (!plant_variation_ok(v[i])) return false;
+    return true;
+  });
+  Staging s(ctx, B);
+  auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto w = s.in_or_null(wrench, 6); auto pv = s.in_or_null(v, 1); auto cf = s.out(contact_force, 12);
+  auto fl = s.out(contact_flag, 4);
+  return s.run(1, [&](Chunk) { return sim_step(ctx, B, *params, r, t, w, pv, v ? B : 0, cf, fl); });
 }
 
 int hb_resident_wbc_batch(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,

@@ -350,42 +350,52 @@ __device__ __forceinline__ void rbd_to_centroidal(const double* r, double* x) {
   for (int i = 0; i < NQ; ++i) x[6 + i] = q[i];
 }
 
+// The base of rnea_pass for the coordinates q, v, a: its orientation R0, the world axes of its yaw / pitch / roll rotations ax0 (rows), its
+// world angular velocity w0 and acceleration wd0, and the acceleration pd0 of its origin.
+__device__ __forceinline__ void rnea_base_motion(const double* q, const double* v, const double* a, double* R0, double* ax0, double* w0, double* wd0,
+                                                 double* pd0) {
+  base_frame(q, R0, ax0);
+  double w1[3], w2[3], t1[3], t2[3];
+  for (int i = 0; i < 3; ++i) { w1[i] = ax0[i] * v[3]; w2[i] = w1[i] + ax0[3 + i] * v[4]; }
+  cross(w1, &ax0[3], t1);
+  cross(w2, &ax0[6], t2);
+  for (int i = 0; i < 3; ++i) {
+    w0[i] = w2[i] + ax0[6 + i] * v[5];
+    wd0[i] = ax0[i] * a[3] + ax0[3 + i] * a[4] + ax0[6 + i] * a[5] + t1[i] * v[4] + t2[i] * v[5];
+    pd0[i] = a[i];
+  }
+}
+
+// Newton-Euler wrench of one rigid body, world frame: orientation R, angular velocity w and acceleration wd, acceleration pd of its frame
+// origin; mass mb, CoM com and inertia I about the CoM (both in the body frame, I row-major). F = mb (pd + wd x r + w x (w x r)) (+ mb g e_z
+// with gravity) and the moment about the frame origin n = R (I wd_l + w_l x I w_l) + r x F, with r = R com and w_l, wd_l = R' w, R' wd.
+__device__ __forceinline__ void rigid_body_wrench(const double* R, const double* w, const double* wd, const double* pd, double mb, const double* com,
+                                                  const double* I, bool gravity, double* F, double* n) {
+  double r[3], t[3], t2[3], t3[3], wl[3], wdl[3], Iw[3], Iwd[3], Nl[3], N[3], rxF[3];
+  rot_const(R, com, r);
+  cross(wd, r, t); cross(w, r, t2); cross(w, t2, t3);
+  for (int i = 0; i < 3; ++i) F[i] = (pd[i] + t[i] + t3[i]) * mb;
+  if (gravity) F[2] += mb * HB_GRAVITY;
+  rotT(R, w, wl); rotT(R, wd, wdl);
+  for (int i = 0; i < 3; ++i) {
+    Iw[i] = wl[0] * I[3 * i] + wl[1] * I[3 * i + 1] + wl[2] * I[3 * i + 2];
+    Iwd[i] = wdl[0] * I[3 * i] + wdl[1] * I[3 * i + 1] + wdl[2] * I[3 * i + 2];
+  }
+  cross(wl, Iw, Nl);
+  for (int i = 0; i < 3; ++i) Nl[i] += Iwd[i];
+  rot(R, Nl, N);
+  cross(r, F, rxF);
+  for (int i = 0; i < 3; ++i) n[i] = N[i] + rxF[i];
+}
+
 // Recursive Newton-Euler in the coordinates above: tau = M(q) a + C(q,v) v + g(q)   (float64, per lane).
 // Also returns the classical acceleration of the four contact points (= J_c a + dJ_c/dt v).
 __device__ void rnea_pass(const double* q, const double* v, const double* a, bool gravity, double* tau, double* cacc) {
   const Model& md = c_model;
-  double R0[9], ax0[9];
-  base_frame(q, R0, ax0);
-  double w0[3], wd0[3], pd0[3];
-  {
-    double w1[3], w2[3], t1[3], t2[3];
-    for (int i = 0; i < 3; ++i) { w1[i] = ax0[i] * v[3]; w2[i] = w1[i] + ax0[3 + i] * v[4]; }
-    cross(w1, &ax0[3], t1);
-    cross(w2, &ax0[6], t2);
-    for (int i = 0; i < 3; ++i) {
-      w0[i] = w2[i] + ax0[6 + i] * v[5];
-      wd0[i] = ax0[i] * a[3] + ax0[3 + i] * a[4] + ax0[6 + i] * a[5] + t1[i] * v[4] + t2[i] * v[5];
-      pd0[i] = a[i];
-    }
-  }
+  double R0[9], ax0[9], w0[3], wd0[3], pd0[3];
+  rnea_base_motion(q, v, a, R0, ax0, w0, wd0, pd0);
   auto body_wrench = [&](int b, const double* R, const double* w, const double* wd, const double* pd, double* F, double* n) {
-    double r[3], t[3], t2[3], t3[3], wl[3], wdl[3], Iw[3], Iwd[3], Nl[3], N[3], rxF[3];
-    rot_const(R, &md.com[3 * b], r);
-    cross(wd, r, t); cross(w, r, t2); cross(w, t2, t3);
-    const double mb = md.mass[b];
-    for (int i = 0; i < 3; ++i) F[i] = (pd[i] + t[i] + t3[i]) * mb;
-    if (gravity) F[2] += mb * HB_GRAVITY;
-    rotT(R, w, wl); rotT(R, wd, wdl);
-    const double* I = &md.inertia[9 * b];
-    for (int i = 0; i < 3; ++i) {
-      Iw[i] = wl[0] * I[3 * i] + wl[1] * I[3 * i + 1] + wl[2] * I[3 * i + 2];
-      Iwd[i] = wdl[0] * I[3 * i] + wdl[1] * I[3 * i + 1] + wdl[2] * I[3 * i + 2];
-    }
-    cross(wl, Iw, Nl);
-    for (int i = 0; i < 3; ++i) Nl[i] += Iwd[i];
-    rot(R, Nl, N);
-    cross(r, F, rxF);
-    for (int i = 0; i < 3; ++i) n[i] = N[i] + rxF[i];
+    rigid_body_wrench(R, w, wd, pd, md.mass[b], &md.com[3 * b], &md.inertia[9 * b], gravity, F, n);
   };
   double f0[3], n0[3];
   body_wrench(0, R0, w0, wd0, pd0, f0, n0);

@@ -311,12 +311,29 @@ __global__ void actuation_kernel(int B, double delay, const double* time, hb_act
 // Same rigid-body passes as the WBC assembly: lanes 0-15 unit-velocity sweeps -> J_c columns, lanes 0-15 RNEA with unit accelerations ->
 // M columns, lane 16 -> nle; 16 x 16 Cholesky in shared memory. One warp per instance. wrench (B x 6, nullable): an external world force at
 // the base origin and a world couple, which enter as the generalised forces Q_p = f, Q_zyx = T' tau with omega_world = T(zyx) zyx_dot (the
-// map of the world angular velocity written back below); null adds nothing.
+// map of the world angular velocity written back below); null adds nothing. var (nullable): the plants of instances 0 .. n_var - 1 (varied
+// plants, hunter_b200.h); the others, and every instance with a null var, run the nominal plant.
 struct SimShared { double q[NQ], v[NQ], J[12 * NQ], M[NQ * 17], nle[NQ], rhs[NQ], t1[NQ], t2[NQ], kdi[NQ], F[12], cpos[12], cvel[12]; };
-__global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, double* rbd_io, const double* tau, const double* wrench, double* contact_force,
-                                                      uint8_t* contact_flag) {
+
+// The payload of a varied plant in one RNEA lane: rnea_pass's base-body wrench for a rigid body fixed to the base with mass m, CoM c and
+// inertia I (base frame), added to the base rows of tau (the joint rows get nothing from a body on the base). Not inlined: inlined after
+// rnea_pass it keeps q, v, a live across that pass and sim_step_kernel spills (255 registers); called, the kernel stays without spills.
+__device__ __noinline__ void payload_rnea(const double* q, const double* v, const double* a, bool gravity, double m, const double* c, const double* I,
+                                             double* tau) {
+  double R0[9], ax0[9], w0[3], wd0[3], pd0[3], F[3], n[3];
+  rnea_base_motion(q, v, a, R0, ax0, w0, wd0, pd0);
+  rigid_body_wrench(R0, w0, wd0, pd0, m, c, I, gravity, F, n);
+  for (int i = 0; i < 3; ++i) {
+    tau[i] += F[i];
+    tau[3 + i] += ax0[3 * i] * n[0] + ax0[3 * i + 1] * n[1] + ax0[3 * i + 2] * n[2];
+  }
+}
+
+__global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, double* rbd_io, const double* tau, const double* wrench,
+                                                      const hb_plant_variation* var, int n_var, double* contact_force, uint8_t* contact_flag) {
   __shared__ SimShared sh;
   const int inst = blockIdx.x, lane = threadIdx.x;
+  const hb_plant_variation* pv = (var && inst < n_var) ? var + inst : nullptr;      // null: the nominal plant
   double* r = rbd_io + (size_t)inst * 32;
   if (lane == 0) {
     for (int i = 0; i < 3; ++i) { sh.q[i] = r[3 + i]; sh.q[3 + i] = r[i]; sh.v[i] = r[NQ + 3 + i]; }
@@ -344,10 +361,12 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
       const double depth = prm.ground_height - sh.cpos[3 * lane + 2];
       double fz = 0.0, fx = 0.0, fy = 0.0;
       if (depth > 0.0) {
-        fz = prm.ground_stiffness * depth - prm.ground_damping * sh.cvel[3 * lane + 2];
+        double kg = prm.ground_stiffness, dg = prm.ground_damping, mu = prm.friction_mu;
+        if (pv) { kg *= pv->stiffness_scale; dg *= pv->damping_scale; mu *= pv->friction_scale; }
+        fz = kg * depth - dg * sh.cvel[3 * lane + 2];
         if (fz < 0.0) fz = 0.0;
         fx = -prm.tangential_damping * sh.cvel[3 * lane]; fy = -prm.tangential_damping * sh.cvel[3 * lane + 1];
-        const double ft = sqrt(fx * fx + fy * fy), fmax_ = prm.friction_mu * fz;
+        const double ft = sqrt(fx * fx + fy * fy), fmax_ = mu * fz;
         if (ft > fmax_) { const double sc = ft > 0.0 ? fmax_ / ft : 0.0; fx *= sc; fy *= sc; }
       }
       sh.F[3 * lane] = fx; sh.F[3 * lane + 1] = fy; sh.F[3 * lane + 2] = fz;
@@ -356,14 +375,19 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
       double q[NQ], v[NQ], a[NQ], tq[NQ];
       for (int i = 0; i < NQ; ++i) { q[i] = sh.q[i]; v[i] = lane == 16 ? sh.v[i] : 0.0; a[i] = (i == lane) ? 1.0 : 0.0; }
       rnea_pass(q, v, a, lane == 16, tq, nullptr);
+      if (pv && (lane < 6 || lane == 16) && pv->payload_mass > 0.0)
+        payload_rnea(q, v, a, lane == 16, pv->payload_mass, pv->payload_com, pv->payload_inertia, tq);
       if (lane < 16) { for (int rr = 0; rr < NQ; ++rr) sh.M[rr * 17 + lane] = tq[rr]; }
       else { for (int rr = 0; rr < NQ; ++rr) sh.nle[rr] = tq[rr]; }
     }
     __syncwarp();
     if (lane < NQ) {
       // joint side of the plant as in the reference's MuJoCo model (mujoco/model/hunter/hunter.xml:6): rotor armature on the diagonal of M,
-      // viscous joint damping
-      double s = -sh.nle[lane] + (lane >= 6 ? tau[(size_t)inst * NJ + lane - 6] - prm.joint_damping * sh.v[lane] : 0.0);
+      // viscous joint damping. A varied plant's motor strength scales the torque first, as one rounded product (never contracted into
+      // the damping term), so that strength s on tau is strength 1 on s * tau.
+      double tj = lane >= 6 ? tau[(size_t)inst * NJ + lane - 6] : 0.0;
+      if (pv && lane >= 6) tj = __dmul_rn(pv->motor_strength[lane - 6], tj);
+      double s = -sh.nle[lane] + (lane >= 6 ? tj - prm.joint_damping * sh.v[lane] : 0.0);
       for (int rr = 0; rr < 12; ++rr) s += sh.J[rr * NQ + lane] * sh.F[rr];
       if (wrench && lane < 6) {
         const double* w = wrench + (size_t)inst * 6;

@@ -228,7 +228,7 @@ typedef struct {                 /* per-instance outcome, in/out: start an episo
   int32_t fail_tick;             /* absolute tick of the first failure, -1: never failed                                          */
   int32_t fail_reason;           /* HB_ROLLOUT_FAIL_* bits of that tick                                                           */
   int32_t mpc_bad, wbc_fallbacks, plan_rejects;   /* counts of info.status != 0, wbc_status != 0, plan_status != 0                */
-  double max_abs_torque;         /* over the applied (saturated) torques                                                          */
+  double max_abs_torque;         /* over the applied (saturated) torques, before a plant variation's motor_strength scales them  */
 } hb_rollout_stats;
 int hb_default_rollout_params(hb_rollout_params* p);       /* host only */
 
@@ -255,6 +255,41 @@ typedef struct {                      /* external pushes on one robot's base    
  * call keeps the previous setting and enqueues nothing. The device copy is allocated at max_batch by the first call that sets pushes and
  * freed by hb_destroy. Pushes add no launch to an episode. */
 int hb_rollout_set_pushes(hb_ctx* ctx, int B, const hb_push_schedule* pushes);
+
+/* ---- varied plants: a plant of its own for each robot of the episodes (payload on the base, ground contact, motor strength) ----
+ * The variation acts on the simulated plant only; the planner, MPC, WBC, joint command law, actuation model and estimator keep the nominal
+ * model and are not told about it. With s the variation of an instance, its plant step differs from hb_sim_step_batch in:
+ *  - ground contact: k = sim.ground_stiffness * s.stiffness_scale, d = sim.ground_damping * s.damping_scale and
+ *    mu = sim.friction_mu * s.friction_scale, each product formed once and used where the unvaried step uses the parameter (tangential
+ *    damping is not varied);
+ *  - motors: joint j receives the generalised force s.motor_strength[j] * tau[j], after the episode's saturation (hb_rollout_stats'
+ *    max_abs_torque counts the saturated command, before this scaling);
+ *  - payload (when payload_mass > 0): a rigid body fixed to the base, mass m, CoM c and inertia I_c (base frame). With the base coordinates
+ *    (p, zyx), omega = T(zyx) zyx_dot, r = R(zyx) c and I_w = R I_c R': column k < 6 of M gains [F; T' n], the payload wrench about the
+ *    base origin for a unit acceleration of coordinate k with v = 0 and no gravity (F = m (pdd + omega_dot x r), n = I_w omega_dot + r x F);
+ *    nle gains the same for the actual velocity with no acceleration and gravity on: omega_dot0 = (omega_1 x a_pitch) dpitch +
+ *    (omega_2 x a_roll) droll (the velocity-product term of the base's angular acceleration), F = m (omega_dot0 x r + omega x (omega x r))
+ *    + m g e_z, n = I_w omega_dot0 + omega x I_w omega + r x F. Joint columns are unchanged.
+ * The default variation (hb_default_plant_variation: no payload, every scale 1) is the unvaried plant bit for bit, as is an instance with no
+ * variation set. */
+typedef struct {                 /* the plant of one robot, relative to hb_sim_params and the nominal model            */
+  double payload_mass;           /* [kg], >= 0; 0 = no payload (then payload_com and payload_inertia must be all zero) */
+  double payload_com[3];         /* payload CoM in the base frame [m], relative to the base frame origin (rbd[3:6])  */
+  double payload_inertia[9];     /* about the payload CoM, base frame, row-major, symmetric positive semidefinite     */
+  double friction_scale;         /* mu = friction_scale * sim.friction_mu, >= 0                                       */
+  double stiffness_scale;        /* ground_stiffness scaled, > 0                                                      */
+  double damping_scale;          /* ground_damping scaled, >= 0                                                       */
+  double motor_strength[10];     /* joint j receives motor_strength[j] * tau[j], >= 0 (0 = a dead motor)              */
+} hb_plant_variation;            /* 208 B */
+int hb_default_plant_variation(hb_plant_variation* v);      /* host only: no payload, every scale 1 */
+/* Sets the plant variations of the context's episodes: from then on both episode calls run instance i of their batch on the plant v[i] for
+ * i < B; instances at or beyond B get the nominal plant. B == 0 clears them (v may be NULL). v is a host array, validated on the host and
+ * copied to the context in stream order on the context's stream; the caller may free it when the call returns. -1: B < 0, NULL v with
+ * B > 0, or a field outside its range above: any non-finite value, an inertia that is not exactly symmetric or has a negative principal
+ * minor (Sylvester's criterion, in double), a zero mass with a nonzero CoM or inertia; -4: B > max_batch. A rejected call keeps the previous
+ * setting and enqueues nothing. The device copy is allocated at max_batch by the first call that sets variations and freed by hb_destroy.
+ * Variations add no launch to an episode. */
+int hb_rollout_set_plant_variations(hb_ctx* ctx, int B, const hb_plant_variation* v);
 
 /* ---- estimated episodes (hb_rollout_estimated_batch_dev): the controllers read the Kalman filter's estimate from synthesised, noisy
  * sensors instead of the plant's true state (LeggedController::updateStateEstimation, LeggedController.cpp:280-349) ---- */
@@ -406,7 +441,8 @@ int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const dou
  * horizon = time_to_target = horizon_N * dt or, for event_nodes contexts, the time horizon, prev_event = min(t, gait_start) - 0.5, IK
  * joint references), device planner, resident cycle without its WBC (cold start iff tick0 == 0). Every tick then runs
  * hb_resident_wbc_batch's policy + WeightedWbc at t, the joint command law (loaded, walking branch), the actuation model, saturation to
- * +-torque_limit and one plant step (with the tick's push wrench when hb_rollout_set_pushes has set schedules). Failure checks run on the state entering each tick (finite, |roll| <= pi/2, base height) and on the
+ * +-torque_limit and one plant step (with the tick's push wrench when hb_rollout_set_pushes has set schedules, on the instance's plant
+ * when hb_rollout_set_plant_variations has set variations). Failure checks run on the state entering each tick (finite, |roll| <= pi/2, base height) and on the
  * emergency stop the joint command raises; from its first failure on an instance is held (rbd put back to its last finite state after
  * every plant step; a non-finite state entering the first tick of a call is replaced by the nominal standing pose) and its outputs no
  * longer count in stats. rbd (B x 32), act, estop (B) and stats are device memory, in/out. cmd (B) is a host array, validated and copied
@@ -509,6 +545,10 @@ int hb_sim_step_batch(hb_ctx* ctx, int B, const hb_sim_params* params, double* r
  * hb_sim_step_batch. */
 int hb_sim_step_wrench(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench /*nullable*/,
                        double* contact_force /*nullable*/, uint8_t* contact_flag /*nullable*/);
+/* hb_sim_step_wrench on varied plants: v (B, nullable) = the plant of each robot (varied plants, above), validated as by
+ * hb_rollout_set_plant_variations (-1). NULL v is exactly hb_sim_step_wrench. */
+int hb_sim_step_varied(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench /*nullable*/,
+                       const hb_plant_variation* v /*nullable*/, double* contact_force /*nullable*/, uint8_t* contact_flag /*nullable*/);
 int hb_resident_wbc_batch(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode /*nullable*/, double* x_des, double* u_des,
                           int32_t* mode_out, double* wbc_sol, double* torque /*nullable*/, int32_t* wbc_status /*nullable*/);
 int hb_rbd_to_centroidal_batch(hb_ctx* ctx, int B, const double* rbd, double* x);
