@@ -37,7 +37,7 @@ EXPORTED_SYMBOLS = [
     "hb_time_grid_batch_dev", "hb_reference_expand_grid_batch_dev", "hb_mpc_solve_grid_batch_dev", "hb_policy_eval_grid_batch_dev",
     "hb_time_grid_batch", "hb_reference_expand_grid_batch", "hb_mpc_solve_grid_batch", "hb_resident_read_grid_batch", "hb_resident_write_batch",
     "hb_default_rollout_params", "hb_rollout_batch_dev", "hb_rollout_set_pushes", "hb_sim_step_wrench",
-    "hb_default_plant_variation", "hb_rollout_set_plant_variations", "hb_sim_step_varied",
+    "hb_default_plant_variation", "hb_rollout_set_plant_variations", "hb_sim_step_varied", "hb_rollout_set_terrains", "hb_sim_step_terrain",
     "hb_default_estimation_params", "hb_estimation_reset", "hb_sim_read_sensors_batch_dev", "hb_sim_read_sensors", "hb_rollout_estimated_batch_dev",
 ]
 
@@ -308,6 +308,40 @@ def make_plant_variations(B, payload_mass=0.0, payload_com=(0.0, 0.0, 0.0), payl
     v = np.ctypeslib.as_array(out)
     v["payload_mass"] = m; v["payload_com"] = c; v["payload_inertia"] = I.reshape(B, 9)
     v["friction_scale"] = fs; v["stiffness_scale"] = ks; v["damping_scale"] = ds; v["motor_strength"] = ms
+    return out
+
+
+HB_TERRAIN_MAX = 64
+
+
+class HbTerrain(C.Structure):
+    _fields_ = [("nx", C.c_int32), ("ny", C.c_int32), ("origin", C.c_double * 2), ("spacing", C.c_double),
+                ("height", (C.c_double * HB_TERRAIN_MAX) * HB_TERRAIN_MAX)]
+
+
+def make_terrains(B, heights, spacing, origin=(0.0, 0.0)):
+    """ctypes array of B HbTerrain (Context.set_terrains, Context.sim_step). Instance i stands on the height field heights[i] (ny x nx,
+    2..HB_TERRAIN_MAX each): heights[i][j, k] is the ground z at world (origin[i][0] + k spacing[i], origin[i][1] + j spacing[i]),
+    interpolated bilinearly between the samples and continued flat beyond the grid's edges. heights (ny, nx) or (B, ny, nx), spacing () or
+    (B,), origin (2,) or (B, 2). Raises ValueError for what hb_rollout_set_terrains rejects."""
+    h = _f64(heights)
+    if h.ndim not in (2, 3):
+        raise ValueError("terrains: heights (ny, nx) or (B, ny, nx) expected, got shape %s" % (h.shape,))
+    ny, nx = h.shape[-2:]
+    if not (2 <= nx <= HB_TERRAIN_MAX and 2 <= ny <= HB_TERRAIN_MAX):
+        raise ValueError("terrains: 2..%d samples along x and y, got %d x %d" % (HB_TERRAIN_MAX, ny, nx))
+    try:
+        h = np.broadcast_to(h, (B, ny, nx)); s = np.broadcast_to(_f64(spacing), (B,)); o = np.broadcast_to(_f64(origin), (B, 2))
+    except ValueError as e:
+        raise ValueError("terrains: heights (B, ny, nx), spacing (B,), origin (B, 2) expected: %s" % e)
+    if not (np.isfinite(h).all() and np.isfinite(o).all()):
+        raise ValueError("terrains: heights and origins must be finite")
+    if not (np.isfinite(s).all() and (s > 0).all()):
+        raise ValueError("terrains: spacings must be finite and > 0")
+    out = (HbTerrain * B)()
+    v = np.ctypeslib.as_array(out)
+    v["nx"] = nx; v["ny"] = ny; v["origin"] = o; v["spacing"] = s
+    v["height"][:, :ny, :nx] = h
     return out
 
 
@@ -733,22 +767,38 @@ class Context:
         _check(self._lib.hb_actuation_batch(self._h, B, C.c_double(delay), _ptr(time), state, _ptr(command), _ptr(rbd), _ptr(tau)), "hb_actuation_batch", self._h)
         return tau
 
-    def sim_step(self, rbd, tau, params=None, wrench=None, variation=None):
+    def sim_step(self, rbd, tau, params=None, wrench=None, variation=None, terrain=None):
         """One control period of the batched rigid-body plant: returns (rbd_next [B,32], contact_force [B,12], contact_flag [B,4]).
         wrench [B,6]: an external world force at the base origin, then a world couple, held over the period. variation: B HbPlantVariation
-        (make_plant_variations), the plant of each robot. With either, the step is hb_sim_step_varied."""
+        (make_plant_variations), the plant of each robot. With either, the step is hb_sim_step_varied. terrain: B HbTerrain (make_terrains),
+        the ground under each robot; with it, the step is hb_sim_step_terrain."""
         rbd = _f64(rbd).copy(); tau = _f64(tau); B = rbd.shape[0]
         params = params or default_sim_params()
         cf = np.zeros((B, 12)); fl = np.zeros((B, 4), dtype=np.uint8)
-        if wrench is None and variation is None:
+        if wrench is None and variation is None and terrain is None:
             _check(self._lib.hb_sim_step_batch(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(cf), _ptr(fl)), "hb_sim_step_batch", self._h)
-        else:
-            w = None if wrench is None else _f64(wrench).reshape(B, 6)
-            if variation is not None and len(variation) != B:
-                raise ValueError("sim_step: %d plant variations for %d robots" % (len(variation), B))
+            return rbd, cf, fl
+        w = None if wrench is None else _f64(wrench).reshape(B, 6)
+        if variation is not None and len(variation) != B:
+            raise ValueError("sim_step: %d plant variations for %d robots" % (len(variation), B))
+        if terrain is None:
             _check(self._lib.hb_sim_step_varied(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), variation, _ptr(cf), _ptr(fl)),
                    "hb_sim_step_varied", self._h)
+        else:
+            if len(terrain) != B:
+                raise ValueError("sim_step: %d terrains for %d robots" % (len(terrain), B))
+            _check(self._lib.hb_sim_step_terrain(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), variation, terrain, _ptr(cf), _ptr(fl)),
+                   "hb_sim_step_terrain", self._h)
         return rbd, cf, fl
+
+    def set_terrains(self, terrains):
+        """Terrains of this context's episodes (hb_rollout_set_terrains): terrains[i] (make_terrains) is the ground under instance i of every
+        later rollout / rollout_estimated call, for the plant and the base-height check; instances beyond len(terrains) stand on the flat
+        ground of params.sim.ground_height; None clears them."""
+        if terrains is None:
+            _check(self._lib.hb_rollout_set_terrains(self._h, 0, None), "hb_rollout_set_terrains", self._h)
+        else:
+            _check(self._lib.hb_rollout_set_terrains(self._h, len(terrains), terrains), "hb_rollout_set_terrains", self._h)
 
     def set_plant_variations(self, variations):
         """Plant variations of this context's episodes (hb_rollout_set_plant_variations): variations[i] (make_plant_variations) is the plant

@@ -79,6 +79,10 @@ struct hb_ctx {
   hb_plant_variation* var_dev;
   int var_n;
   std::vector<hb_plant_variation> var_host;
+  // terrains of the episodes (hb_rollout_set_terrains): the first ter_n instances have one; allocated and kept as var_dev / var_host
+  hb_terrain* ter_dev;
+  int ter_n;
+  std::vector<hb_terrain> ter_host;
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
   // hb_resident_cycle_batch's packed references / reference verdicts
   void* arena; size_t arena_cap;
@@ -416,7 +420,7 @@ int hb_destroy(hb_ctx* ctx) {
   void* ptrs[] = {ctx->sqp_mem, ctx->dxt, ctx->dut, ctx->perf, ctx->flags, ctx->xdes, ctx->udes, ctx->wstatus, ctx->witers, ctx->wmode,
                   ctx->hoqp_mem, ctx->cyc_xref, ctx->cyc_swing, ctx->cyc_tk, ctx->cyc_mode, ctx->cyc_nn, ctx->res_t0, ctx->res_xt,
                   ctx->res_ut, ctx->res_tk, ctx->res_mode, ctx->res_nn, ctx->res_sol, ctx->res_stance, ctx->arena, ctx->ro_mem, ctx->re_mem,
-                  ctx->push_mem, ctx->var_dev};
+                  ctx->push_mem, ctx->var_dev, ctx->ter_dev};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -860,15 +864,16 @@ int hb_actuation_batch_dev(hb_ctx* ctx, int B, double delay, const double* time,
   return launch(ctx, K_UNPROFILED, actuation_kernel, (B + 63) / 64, 64, 0, B, delay, time, state, command, rbd, tau);
 }
 
-// the plant step after the entry checks; wrench (B x 6) nullable; var (nullable): the plants of instances 0 .. n_var - 1
+// the plant step after the entry checks; wrench (B x 6) nullable; var (nullable): the plants of instances 0 .. n_var - 1; ter (nullable):
+// the ground under instances 0 .. n_ter - 1
 static int sim_step(hb_ctx* ctx, int B, const hb_sim_params& params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* var,
-                    int n_var, double* contact_force, uint8_t* contact_flag) {
-  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, params, rbd, tau, wrench, var, n_var, contact_force, contact_flag);
+                    int n_var, const hb_terrain* ter, int n_ter, double* contact_force, uint8_t* contact_flag) {
+  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, params, rbd, tau, wrench, var, n_var, ter, n_ter, contact_force, contact_flag);
 }
 
 int hb_sim_step_batch_dev(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {
   ENTER(ctx, B, params && rbd && tau && sim_params_ok(*params), UNCAPPED);
-  return sim_step(ctx, B, *params, rbd, tau, nullptr, nullptr, 0, contact_force, contact_flag);
+  return sim_step(ctx, B, *params, rbd, tau, nullptr, nullptr, 0, nullptr, 0, contact_force, contact_flag);
 }
 
 int hb_default_plant_variation(hb_plant_variation* v) {
@@ -915,6 +920,32 @@ int hb_rollout_set_plant_variations(hb_ctx* ctx, int B, const hb_plant_variation
   try { ctx->var_host.assign(v, v + B); } catch (const std::bad_alloc&) { return HB_ENOMEM; }
   CK(cudaMemcpyAsync(ctx->var_dev, ctx->var_host.data(), sizeof(hb_plant_variation) * B, cudaMemcpyHostToDevice, ctx->stream));
   ctx->var_n = B;
+  return HB_OK;
+}
+
+// The ranges of hunter_b200.h's hb_terrain: grid sizes, a finite origin, a finite positive spacing, finite heights where they are read
+static bool terrain_ok(const hb_terrain& t) {
+  if (t.nx < 2 || t.nx > HB_TERRAIN_MAX || t.ny < 2 || t.ny > HB_TERRAIN_MAX) return false;
+  if (!isfinite(t.origin[0]) || !isfinite(t.origin[1]) || !isfinite(t.spacing) || !(t.spacing > 0.0)) return false;
+  for (int j = 0; j < t.ny; ++j)
+    for (int i = 0; i < t.nx; ++i) if (!isfinite(t.height[j][i])) return false;
+  return true;
+}
+
+int hb_rollout_set_terrains(hb_ctx* ctx, int B, const hb_terrain* t) {
+  const int rc = enter(ctx, B, B == 0 || t, CAPPED, [&] {
+    for (int i = 0; i < B; ++i) if (!terrain_ok(t[i])) return false;
+    return true;
+  });
+  if (rc == EMPTY) { ctx->ter_n = 0; return HB_OK; }      // cleared: the episodes run on flat ground
+  if (rc) return rc;
+  if (!ctx->ter_dev && dalloc(&ctx->ter_dev, (size_t)ctx->cfg.max_batch) != cudaSuccess) {
+    cudaGetLastError(); ctx->ter_dev = nullptr; return HB_ENOMEM;
+  }
+  // a pageable copy the context owns: cudaMemcpyAsync has consumed it when it returns, whatever memory the caller's array is in
+  try { ctx->ter_host.assign(t, t + B); } catch (const std::bad_alloc&) { return HB_ENOMEM; }
+  CK(cudaMemcpyAsync(ctx->ter_dev, ctx->ter_host.data(), sizeof(hb_terrain) * B, cudaMemcpyHostToDevice, ctx->stream));
+  ctx->ter_n = B;
   return HB_OK;
 }
 
@@ -1046,13 +1077,15 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   double* wrench = ctx->push_n > 0 ? ctx->push_wrench : nullptr;
   // the instances' plants; the nominal one for all without variations
   const hb_plant_variation* var = ctx->var_n > 0 ? ctx->var_dev : nullptr;
+  // the ground under the instances, for the plant and the height check; flat ground for all without terrains
+  const hb_terrain* ter = ctx->ter_n > 0 ? ctx->ter_dev : nullptr;
   for (int k = 0; k < n_ticks && !rc; ++k) {
     const int64_t a = tick0 + k;
     const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
     const bool mpc = a % p->mpc_every == 0, first_cold = cold && k == 0;
     double* log_row = (n_log && k % p->log_every == 0) ? log + (size_t)(k / p->log_every) * 32 : nullptr;
     rc = launch(ctx, K_UNPROFILED, rollout_tick_begin_kernel, grid, 64, 0, B, (int)a, t, p->min_base_height, rbd, ctx->ro_held, stats, ctx->ro_tnow,
-                log_row, (size_t)n_log * 32, ctx->push_sched, ctx->push_n, wrench);
+                log_row, (size_t)n_log * 32, ctx->push_sched, ctx->push_n, wrench, ter, ctx->ter_n);
     if (!rc && e) {
       // LeggedController::updateStateEstimation: sensors and contact flags at the previous observation's time, filter, observation step
       double* est_row = (n_est_log && k % p->log_every == 0) ? e->log + (size_t)(k / p->log_every) * 32 : nullptr;
@@ -1076,7 +1109,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
                                              ctx->ro_jtau);
     if (!rc) rc = hb_actuation_batch_dev(ctx, B, p->actuation_delay, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, ctx->ro_tau);
-    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, var, ctx->var_n, nullptr, nullptr);
+    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, var, ctx->var_n, ter, ctx->ter_n, nullptr, nullptr);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_tick_end_kernel, grid, 64, 0, B, (int)a, mpc ? 1 : 0, ctx->ro_info, ctx->ro_pstat, ctx->wstatus, estop, ctx->ro_tau, ctx->ro_held, rbd, stats);
   }
   return rc;
@@ -1491,20 +1524,26 @@ int hb_sim_step_wrench(hb_ctx* ctx, int B, const hb_sim_params* params, double* 
   ENTER(ctx, B, params && rbd && tau, CAPPED, [&] { return sim_params_ok(*params); });
   Staging s(ctx, B);
   auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto w = s.in_or_null(wrench, 6); auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
-  return s.run(1, [&](Chunk) { return sim_step(ctx, B, *params, r, t, w, nullptr, 0, cf, fl); });
+  return s.run(1, [&](Chunk) { return sim_step(ctx, B, *params, r, t, w, nullptr, 0, nullptr, 0, cf, fl); });
 }
 
 int hb_sim_step_varied(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* v,
                        double* contact_force, uint8_t* contact_flag) {
+  return hb_sim_step_terrain(ctx, B, params, rbd, tau, wrench, v, nullptr, contact_force, contact_flag);
+}
+
+int hb_sim_step_terrain(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* v,
+                        const hb_terrain* ter, double* contact_force, uint8_t* contact_flag) {
   ENTER(ctx, B, params && rbd && tau, CAPPED, [&] {
     if (!sim_params_ok(*params)) return false;
     if (v) for (int i = 0; i < B; ++i) if (!plant_variation_ok(v[i])) return false;
+    if (ter) for (int i = 0; i < B; ++i) if (!terrain_ok(ter[i])) return false;
     return true;
   });
   Staging s(ctx, B);
-  auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto w = s.in_or_null(wrench, 6); auto pv = s.in_or_null(v, 1); auto cf = s.out(contact_force, 12);
-  auto fl = s.out(contact_flag, 4);
-  return s.run(1, [&](Chunk) { return sim_step(ctx, B, *params, r, t, w, pv, v ? B : 0, cf, fl); });
+  auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto w = s.in_or_null(wrench, 6); auto pv = s.in_or_null(v, 1); auto pt = s.in_or_null(ter, 1);
+  auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
+  return s.run(1, [&](Chunk) { return sim_step(ctx, B, *params, r, t, w, pv, v ? B : 0, pt, ter ? B : 0, cf, fl); });
 }
 
 int hb_resident_wbc_batch(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,

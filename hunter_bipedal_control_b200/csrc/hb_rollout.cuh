@@ -30,12 +30,44 @@ __global__ void rollout_plan_inputs_kernel(int B, double t, double horizon, cons
   p.gait = c.gait; p.joint_ik = 1;
 }
 
-// failure bits of a state entering a tick; the orientation and height checks are only meaningful on a finite state
-__device__ __forceinline__ int rollout_state_check(const double* r, double min_base_height) {
+// One axis of a terrain lookup (terrain, hunter_b200.h): the grid coordinate of the world coordinate x, clamped to [0, n - 1], split into
+// the cell index i <= n - 2 and the fraction a of the cell. Returns whether x was clamped (off the grid, where the gradient along this
+// axis is zero). A NaN coordinate clamps to 0, so no index leaves the grid.
+__device__ __forceinline__ bool terrain_axis(double x, double origin, double spacing, int n, int* i, double* a) {
+  double u = (x - origin) / spacing;
+  bool clamped = false;
+  if (!(u >= 0.0)) { u = 0.0; clamped = true; }
+  else if (u > (double)(n - 1)) { u = (double)(n - 1); clamped = true; }
+  int c = (int)floor(u);
+  if (c > n - 2) c = n - 2;
+  *i = c; *a = u - (double)c;
+  return clamped;
+}
+
+// Height h of the terrain at world (x, y) and its gradient (gx, gy), bilinear on the cell, as hunter_b200.h documents it
+__device__ __forceinline__ double terrain_height(const hb_terrain& t, double x, double y, double* gx, double* gy) {
+  int i, j;
+  double a, b;
+  const bool cx = terrain_axis(x, t.origin[0], t.spacing, t.nx, &i, &a), cy = terrain_axis(y, t.origin[1], t.spacing, t.ny, &j, &b);
+  const double h00 = t.height[j][i], h01 = t.height[j][i + 1], h10 = t.height[j + 1][i], h11 = t.height[j + 1][i + 1];
+  const double h0 = h00 + a * (h01 - h00), h1 = h10 + a * (h11 - h10);
+  const double d0 = h01 - h00, d1 = h11 - h10;
+  *gx = cx ? 0.0 : (d0 + b * (d1 - d0)) / t.spacing;
+  *gy = cy ? 0.0 : (h1 - h0) / t.spacing;
+  return h0 + b * (h1 - h0);
+}
+
+// failure bits of a state entering a tick; the orientation and height checks are only meaningful on a finite state. ter (nullable): the
+// terrain of the instance, above which the base height is measured; null measures it from z = 0.
+__device__ __forceinline__ int rollout_state_check(const double* r, double min_base_height, const hb_terrain* ter) {
   for (int i = 0; i < 32; ++i) if (!isfinite(r[i])) return HB_ROLLOUT_FAIL_NONFINITE;
   int why = 0;
   if (r[2] > M_PI_2 || r[2] < -M_PI_2) why |= HB_ROLLOUT_FAIL_ORIENTATION;     // zyx[2] = roll: SafetyChecker::checkOrientation
-  if (min_base_height != 0.0 && r[5] < min_base_height) why |= HB_ROLLOUT_FAIL_HEIGHT;
+  if (min_base_height != 0.0) {
+    double z = r[5];
+    if (ter) { double gx, gy; z -= terrain_height(*ter, r[3], r[4], &gx, &gy); }
+    if (z < min_base_height) why |= HB_ROLLOUT_FAIL_HEIGHT;
+  }
   return why;
 }
 
@@ -53,16 +85,17 @@ __device__ __forceinline__ void push_wrench(const hb_push_schedule& s, double t,
 // state every held instance is put back to, the tick time goes to every instance (policy evaluation, actuation stamp), and the state is
 // logged when log_row is set. A non-finite state can only enter the first tick of a call (the end kernel never leaves one behind); with no
 // finite state of that instance known, the nominal standing pose replaces it. With wrench set, the tick's push wrench (B x 6) is written
-// for the plant step: from pushes[inst] for inst < n_pushes, zeros for the others.
+// for the plant step: from pushes[inst] for inst < n_pushes, zeros for the others. The base height of instances inst < n_terrain is
+// measured above terrain[inst].
 __global__ void rollout_tick_begin_kernel(int B, int tick, double t, double min_base_height, double* rbd, double* held, hb_rollout_stats* stats,
                                           double* t_now, double* log_row, size_t log_stride, const hb_push_schedule* pushes, int n_pushes,
-                                          double* wrench) {
+                                          double* wrench, const hb_terrain* terrain, int n_terrain) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
   double* r = rbd + (size_t)inst * 32;
   double* h = held + (size_t)inst * 32;
   hb_rollout_stats& s = stats[inst];
-  const int why = rollout_state_check(r, min_base_height);
+  const int why = rollout_state_check(r, min_base_height, (terrain && inst < n_terrain) ? terrain + inst : nullptr);
   if (why && s.fail_tick < 0) { s.fail_tick = tick; s.fail_reason = why; }
   if (why & HB_ROLLOUT_FAIL_NONFINITE) {
     const double nominal[NQ] = {0.0, 0.0, 0.0, 0.0, 0.0, HB_INITIAL_STATE[8], HB_INITIAL_STATE[12], HB_INITIAL_STATE[13], HB_INITIAL_STATE[14],
@@ -305,14 +338,15 @@ __global__ void actuation_kernel(int B, double delay, const double* time, hb_act
   for (int j = 0; j < NJ; ++j) tau[(size_t)inst * NJ + j] = c[5 * j + 2] * (c[5 * j] - r[6 + j]) + c[5 * j + 3] * (c[5 * j + 1] - r[NQ + 6 + j]) + c[5 * j + 4];
 }
 
-// One step of a batched rigid-body simulation of the robot on flat ground (stands in for the Gazebo / MuJoCo plant of the reference's
+// One step of a batched rigid-body simulation of the robot on the ground (stands in for the Gazebo / MuJoCo plant of the reference's
 // closed loop, legged_gazebo / legged_mujoco): forward dynamics M(q) qdd = S' tau + J_c' F_c - nle with compliant point contacts at the four
 // contact frames (normal spring-damper, viscous tangential friction clipped to the cone), semi-implicit Euler over `substeps` substeps.
 // Same rigid-body passes as the WBC assembly: lanes 0-15 unit-velocity sweeps -> J_c columns, lanes 0-15 RNEA with unit accelerations ->
 // M columns, lane 16 -> nle; 16 x 16 Cholesky in shared memory. One warp per instance. wrench (B x 6, nullable): an external world force at
 // the base origin and a world couple, which enter as the generalised forces Q_p = f, Q_zyx = T' tau with omega_world = T(zyx) zyx_dot (the
 // map of the world angular velocity written back below); null adds nothing. var (nullable): the plants of instances 0 .. n_var - 1 (varied
-// plants, hunter_b200.h); the others, and every instance with a null var, run the nominal plant.
+// plants, hunter_b200.h); the others, and every instance with a null var, run the nominal plant. terrain (nullable): the ground under
+// instances 0 .. n_terrain - 1 (terrain, hunter_b200.h); the others stand on flat ground at prm.ground_height.
 struct SimShared { double q[NQ], v[NQ], J[12 * NQ], M[NQ * 17], nle[NQ], rhs[NQ], t1[NQ], t2[NQ], kdi[NQ], F[12], cpos[12], cvel[12]; };
 
 // The payload of a varied plant in one RNEA lane: rnea_pass's base-body wrench for a rigid body fixed to the base with mass m, CoM c and
@@ -329,11 +363,35 @@ __device__ __noinline__ void payload_rnea(const double* q, const double* v, cons
   }
 }
 
+// The contact force F (3) of one contact point at position p, velocity v on a slope of the terrain with height h and gradient (gx, gy)
+// at p (the sloped path of terrain, hunter_b200.h): normal spring-damper along the surface normal, viscous tangential friction in the
+// tangent plane clipped to mu times the normal force. Returns the normal force.
+__device__ __forceinline__ double sloped_contact(const double* p, const double* v, double h, double gx, double gy, double kg, double dg, double ct,
+                                                 double mu, double* F) {
+  const double L = sqrt(1.0 + gx * gx + gy * gy);
+  const double n[3] = {-gx / L, -gy / L, 1.0 / L};
+  const double depth = (h - p[2]) / L;
+  F[0] = F[1] = F[2] = 0.0;
+  if (!(depth > 0.0)) return 0.0;
+  const double vn = v[0] * n[0] + v[1] * n[1] + v[2] * n[2];
+  double fn = kg * depth - dg * vn;
+  if (fn < 0.0) fn = 0.0;
+  double ft[3];
+  for (int c = 0; c < 3; ++c) ft[c] = -ct * (v[c] - vn * n[c]);
+  const double tl = sqrt(ft[0] * ft[0] + ft[1] * ft[1] + ft[2] * ft[2]), fmax_ = mu * fn;
+  if (tl > fmax_) { const double sc = tl > 0.0 ? fmax_ / tl : 0.0; for (int c = 0; c < 3; ++c) ft[c] *= sc; }
+  for (int c = 0; c < 3; ++c) F[c] = fn * n[c] + ft[c];
+  return fn;
+}
+
 __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, double* rbd_io, const double* tau, const double* wrench,
-                                                      const hb_plant_variation* var, int n_var, double* contact_force, uint8_t* contact_flag) {
+                                                      const hb_plant_variation* var, int n_var, const hb_terrain* terrain, int n_terrain,
+                                                      double* contact_force, uint8_t* contact_flag) {
   __shared__ SimShared sh;
   const int inst = blockIdx.x, lane = threadIdx.x;
   const hb_plant_variation* pv = (var && inst < n_var) ? var + inst : nullptr;      // null: the nominal plant
+  const hb_terrain* ter = (terrain && inst < n_terrain) ? terrain + inst : nullptr;  // null: flat ground at prm.ground_height
+  bool touch = false;                    // lanes 0-3: the normal force of their contact in the last substep is positive
   double* r = rbd_io + (size_t)inst * 32;
   if (lane == 0) {
     for (int i = 0; i < 3; ++i) { sh.q[i] = r[3 + i]; sh.q[3 + i] = r[i]; sh.v[i] = r[NQ + 3 + i]; }
@@ -358,18 +416,27 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
     if (lane < 12) { double s = 0.0; for (int i = 0; i < NQ; ++i) s += sh.J[lane * NQ + i] * sh.v[i]; sh.cvel[lane] = s; }
     __syncwarp();
     if (lane < 4) {
-      const double depth = prm.ground_height - sh.cpos[3 * lane + 2];
-      double fz = 0.0, fx = 0.0, fy = 0.0;
-      if (depth > 0.0) {
+      double gh = prm.ground_height, gx = 0.0, gy = 0.0;
+      if (ter) gh = terrain_height(*ter, sh.cpos[3 * lane], sh.cpos[3 * lane + 1], &gx, &gy);
+      if (gx == 0.0 && gy == 0.0) {      // flat ground, or a level patch of the terrain: the flat contact at its height
+        const double depth = gh - sh.cpos[3 * lane + 2];
+        double fz = 0.0, fx = 0.0, fy = 0.0;
+        if (depth > 0.0) {
+          double kg = prm.ground_stiffness, dg = prm.ground_damping, mu = prm.friction_mu;
+          if (pv) { kg *= pv->stiffness_scale; dg *= pv->damping_scale; mu *= pv->friction_scale; }
+          fz = kg * depth - dg * sh.cvel[3 * lane + 2];
+          if (fz < 0.0) fz = 0.0;
+          fx = -prm.tangential_damping * sh.cvel[3 * lane]; fy = -prm.tangential_damping * sh.cvel[3 * lane + 1];
+          const double ft = sqrt(fx * fx + fy * fy), fmax_ = mu * fz;
+          if (ft > fmax_) { const double sc = ft > 0.0 ? fmax_ / ft : 0.0; fx *= sc; fy *= sc; }
+        }
+        sh.F[3 * lane] = fx; sh.F[3 * lane + 1] = fy; sh.F[3 * lane + 2] = fz;
+        touch = fz > 0.0;
+      } else {
         double kg = prm.ground_stiffness, dg = prm.ground_damping, mu = prm.friction_mu;
         if (pv) { kg *= pv->stiffness_scale; dg *= pv->damping_scale; mu *= pv->friction_scale; }
-        fz = kg * depth - dg * sh.cvel[3 * lane + 2];
-        if (fz < 0.0) fz = 0.0;
-        fx = -prm.tangential_damping * sh.cvel[3 * lane]; fy = -prm.tangential_damping * sh.cvel[3 * lane + 1];
-        const double ft = sqrt(fx * fx + fy * fy), fmax_ = mu * fz;
-        if (ft > fmax_) { const double sc = ft > 0.0 ? fmax_ / ft : 0.0; fx *= sc; fy *= sc; }
+        touch = sloped_contact(&sh.cpos[3 * lane], &sh.cvel[3 * lane], gh, gx, gy, kg, dg, prm.tangential_damping, mu, &sh.F[3 * lane]) > 0.0;
       }
-      sh.F[3 * lane] = fx; sh.F[3 * lane + 1] = fy; sh.F[3 * lane + 2] = fz;
     }
     if (lane < 17) {
       double q[NQ], v[NQ], a[NQ], tq[NQ];
@@ -418,6 +485,6 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
     r[NQ] = -sz * d1 + cz * cy * d2; r[NQ + 1] = cz * d1 + sz * cy * d2; r[NQ + 2] = d0 - sy * d2;
   }
   if (lane < 12 && contact_force) contact_force[(size_t)inst * 12 + lane] = sh.F[lane];
-  if (lane < 4 && contact_flag) contact_flag[(size_t)inst * 4 + lane] = sh.F[3 * lane + 2] > 0.0 ? 1 : 0;
+  if (lane < 4 && contact_flag) contact_flag[(size_t)inst * 4 + lane] = touch ? 1 : 0;
 }
 }  // namespace

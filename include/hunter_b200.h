@@ -222,7 +222,7 @@ typedef struct {
 } hb_rollout_params;
 #define HB_ROLLOUT_FAIL_ESTOP 1        /* the joint command law raised the emergency stop                                       */
 #define HB_ROLLOUT_FAIL_ORIENTATION 2  /* |roll| > pi/2 (SafetyChecker::checkOrientation, SafetyChecker.h:34-43)                 */
-#define HB_ROLLOUT_FAIL_HEIGHT 4       /* base z < min_base_height                                                             */
+#define HB_ROLLOUT_FAIL_HEIGHT 4       /* base z < min_base_height (base z above the terrain for an instance with one)         */
 #define HB_ROLLOUT_FAIL_NONFINITE 8    /* an rbd entry is not finite                                                           */
 typedef struct {                 /* per-instance outcome, in/out: start an episode with zeros and fail_tick = -1                  */
   int32_t fail_tick;             /* absolute tick of the first failure, -1: never failed                                          */
@@ -290,6 +290,39 @@ int hb_default_plant_variation(hb_plant_variation* v);      /* host only: no pay
  * setting and enqueues nothing. The device copy is allocated at max_batch by the first call that sets variations and freed by hb_destroy.
  * Variations add no launch to an episode. */
 int hb_rollout_set_plant_variations(hb_ctx* ctx, int B, const hb_plant_variation* v);
+
+/* ---- terrain: the ground under each robot of the episodes, a height field on a regular world-frame grid ----
+ * The terrain acts on the simulated plant and on the height failure check only; the planner, MPC, WBC, joint command law, actuation
+ * model and estimator keep assuming flat ground at z = 0 and are not told about it (the estimator's feet_heights included).
+ * Height and gradient at a world point (x, y): u = (x - origin[0]) / spacing clamped to [0, nx - 1], i = min(floor(u), nx - 2),
+ * a = u - i; the same for y gives w, j and b. With lerp(p, q, s) = p + s (q - p): h0 = lerp(h[j][i], h[j][i+1], a),
+ * h1 = lerp(h[j+1][i], h[j+1][i+1], a), h = lerp(h0, h1, b); g_x = lerp(h[j][i+1] - h[j][i], h[j+1][i+1] - h[j+1][i], b) / spacing,
+ * g_y = (h1 - h0) / spacing. A coordinate that was clamped (u < 0 or u > nx - 1, likewise for y) has a zero gradient component, so the
+ * edge heights continue outward as flat ground. A plateau (four equal corners) gives its height exactly.
+ * Contact of each contact point p (velocity v) in each substep, with k, d and mu those of the instance (scaled by its plant variation):
+ *  - flat path, g_x = g_y = 0 exactly: the flat-ground contact with h in place of sim.ground_height, the same expressions bit for bit;
+ *  - sloped path otherwise: n = (-g_x, -g_y, 1) / L, L = sqrt(1 + g_x^2 + g_y^2), depth = (h - p_z) / L, active iff depth > 0;
+ *    v_n = v.n, f_n = max(0, k depth - d v_n), v_t = v - v_n n, f_t = -sim.tangential_damping v_t scaled down to length mu f_n when it
+ *    is longer, F = f_n n + f_t.
+ *  contact_flag is 1 iff f_n > 0 (on the flat path: F_z > 0, as without a terrain).
+ * Failure check: for an instance with a terrain, HB_ROLLOUT_FAIL_HEIGHT tests base z - h(base x, base y) < min_base_height on a finite
+ * state; instances without one keep the absolute test. Friction is viscous only: on a slope of angle theta a standing robot creeps at
+ * about m g sin(theta) / (n_contacts tangential_damping). Terrains add no launch to an episode. */
+#define HB_TERRAIN_MAX 64
+typedef struct {                      /* the ground under one robot: a height field on a regular world-frame grid                 */
+  int32_t nx, ny;                     /* samples along world x and y, 2..HB_TERRAIN_MAX each                                       */
+  double origin[2];                   /* world (x, y) of sample (0, 0) [m]                                                         */
+  double spacing;                     /* sample spacing [m], > 0                                                                   */
+  double height[HB_TERRAIN_MAX][HB_TERRAIN_MAX];  /* height[j][i] = ground z at (origin[0] + i spacing, origin[1] + j spacing);
+                                         only j < ny, i < nx are read                                                              */
+} hb_terrain;                         /* 32 800 B */
+/* Sets the terrains of the context's episodes: from then on both episode calls run instance i of their batch on the ground t[i] for
+ * i < B; instances at or beyond B stand on the flat ground of sim.ground_height. B == 0 clears them (t may be NULL). t is a host array,
+ * validated on the host and copied to the context in stream order on the context's stream; the caller may free it when the call returns.
+ * -1: B < 0, NULL t with B > 0, nx or ny outside 2..HB_TERRAIN_MAX, a non-finite origin, a spacing that is not finite and > 0, a
+ * non-finite height among the used samples; -4: B > max_batch. A rejected call keeps the previous setting and enqueues nothing. The
+ * device copy is allocated at max_batch by the first call that sets terrains (33.6 MB at 1024) and freed by hb_destroy. */
+int hb_rollout_set_terrains(hb_ctx* ctx, int B, const hb_terrain* t);
 
 /* ---- estimated episodes (hb_rollout_estimated_batch_dev): the controllers read the Kalman filter's estimate from synthesised, noisy
  * sensors instead of the plant's true state (LeggedController::updateStateEstimation, LeggedController.cpp:280-349) ---- */
@@ -442,7 +475,7 @@ int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const dou
  * joint references), device planner, resident cycle without its WBC (cold start iff tick0 == 0). Every tick then runs
  * hb_resident_wbc_batch's policy + WeightedWbc at t, the joint command law (loaded, walking branch), the actuation model, saturation to
  * +-torque_limit and one plant step (with the tick's push wrench when hb_rollout_set_pushes has set schedules, on the instance's plant
- * when hb_rollout_set_plant_variations has set variations). Failure checks run on the state entering each tick (finite, |roll| <= pi/2, base height) and on the
+ * when hb_rollout_set_plant_variations has set variations, on its ground when hb_rollout_set_terrains has set terrains). Failure checks run on the state entering each tick (finite, |roll| <= pi/2, base height) and on the
  * emergency stop the joint command raises; from its first failure on an instance is held (rbd put back to its last finite state after
  * every plant step; a non-finite state entering the first tick of a call is replaced by the nominal standing pose) and its outputs no
  * longer count in stats. rbd (B x 32), act, estop (B) and stats are device memory, in/out. cmd (B) is a host array, validated and copied
@@ -549,6 +582,11 @@ int hb_sim_step_wrench(hb_ctx* ctx, int B, const hb_sim_params* params, double* 
  * hb_rollout_set_plant_variations (-1). NULL v is exactly hb_sim_step_wrench. */
 int hb_sim_step_varied(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench /*nullable*/,
                        const hb_plant_variation* v /*nullable*/, double* contact_force /*nullable*/, uint8_t* contact_flag /*nullable*/);
+/* hb_sim_step_varied on terrains: t (B, nullable) = the ground under each robot (terrain, above), validated as by hb_rollout_set_terrains
+ * (-1). NULL t is exactly hb_sim_step_varied. */
+int hb_sim_step_terrain(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench /*nullable*/,
+                        const hb_plant_variation* v /*nullable*/, const hb_terrain* t /*nullable*/, double* contact_force /*nullable*/,
+                        uint8_t* contact_flag /*nullable*/);
 int hb_resident_wbc_batch(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode /*nullable*/, double* x_des, double* u_des,
                           int32_t* mode_out, double* wbc_sol, double* torque /*nullable*/, int32_t* wbc_status /*nullable*/);
 int hb_rbd_to_centroidal_batch(hb_ctx* ctx, int B, const double* rbd, double* x);
