@@ -770,52 +770,41 @@ class Context:
     def sim_step(self, rbd, tau, params=None, wrench=None, variation=None, terrain=None):
         """One control period of the batched rigid-body plant: returns (rbd_next [B,32], contact_force [B,12], contact_flag [B,4]).
         wrench [B,6]: an external world force at the base origin, then a world couple, held over the period. variation: B HbPlantVariation
-        (make_plant_variations), the plant of each robot. With either, the step is hb_sim_step_varied. terrain: B HbTerrain (make_terrains),
-        the ground under each robot; with it, the step is hb_sim_step_terrain."""
+        (make_plant_variations), the plant of each robot. terrain: B HbTerrain (make_terrains), the ground under each robot. Every step is
+        hb_sim_step_terrain; without any of the three it is the plain plant step of hb_sim_step_batch."""
         rbd = _f64(rbd).copy(); tau = _f64(tau); B = rbd.shape[0]
         params = params or default_sim_params()
         cf = np.zeros((B, 12)); fl = np.zeros((B, 4), dtype=np.uint8)
-        if wrench is None and variation is None and terrain is None:
-            _check(self._lib.hb_sim_step_batch(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(cf), _ptr(fl)), "hb_sim_step_batch", self._h)
-            return rbd, cf, fl
         w = None if wrench is None else _f64(wrench).reshape(B, 6)
         if variation is not None and len(variation) != B:
             raise ValueError("sim_step: %d plant variations for %d robots" % (len(variation), B))
-        if terrain is None:
-            _check(self._lib.hb_sim_step_varied(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), variation, _ptr(cf), _ptr(fl)),
-                   "hb_sim_step_varied", self._h)
-        else:
-            if len(terrain) != B:
-                raise ValueError("sim_step: %d terrains for %d robots" % (len(terrain), B))
-            _check(self._lib.hb_sim_step_terrain(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), variation, terrain, _ptr(cf), _ptr(fl)),
-                   "hb_sim_step_terrain", self._h)
+        if terrain is not None and len(terrain) != B:
+            raise ValueError("sim_step: %d terrains for %d robots" % (len(terrain), B))
+        _check(self._lib.hb_sim_step_terrain(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), variation, terrain, _ptr(cf), _ptr(fl)),
+               "hb_sim_step_terrain", self._h)
         return rbd, cf, fl
+
+    def _set_instances(self, symbol, items):
+        """One per-robot episode setting (hb_rollout_set_*): items[i] for instance i, None clears the setting."""
+        n = 0 if items is None else len(items)
+        _check(getattr(self._lib, symbol)(self._h, n, items), symbol, self._h)
 
     def set_terrains(self, terrains):
         """Terrains of this context's episodes (hb_rollout_set_terrains): terrains[i] (make_terrains) is the ground under instance i of every
         later rollout / rollout_estimated call, for the plant and the base-height check; instances beyond len(terrains) stand on the flat
         ground of params.sim.ground_height; None clears them."""
-        if terrains is None:
-            _check(self._lib.hb_rollout_set_terrains(self._h, 0, None), "hb_rollout_set_terrains", self._h)
-        else:
-            _check(self._lib.hb_rollout_set_terrains(self._h, len(terrains), terrains), "hb_rollout_set_terrains", self._h)
+        self._set_instances("hb_rollout_set_terrains", terrains)
 
     def set_plant_variations(self, variations):
         """Plant variations of this context's episodes (hb_rollout_set_plant_variations): variations[i] (make_plant_variations) is the plant
         of instance i of every later rollout / rollout_estimated call, instances beyond len(variations) run the nominal plant; None clears
         them."""
-        if variations is None:
-            _check(self._lib.hb_rollout_set_plant_variations(self._h, 0, None), "hb_rollout_set_plant_variations", self._h)
-        else:
-            _check(self._lib.hb_rollout_set_plant_variations(self._h, len(variations), variations), "hb_rollout_set_plant_variations", self._h)
+        self._set_instances("hb_rollout_set_plant_variations", variations)
 
     def set_pushes(self, schedules):
         """Push schedules of this context's episodes (hb_rollout_set_pushes): schedules[i] (make_push_schedules) acts on instance i of every
         later rollout / rollout_estimated call, instances beyond len(schedules) are not pushed; None clears them."""
-        if schedules is None:
-            _check(self._lib.hb_rollout_set_pushes(self._h, 0, None), "hb_rollout_set_pushes", self._h)
-        else:
-            _check(self._lib.hb_rollout_set_pushes(self._h, len(schedules), schedules), "hb_rollout_set_pushes", self._h)
+        self._set_instances("hb_rollout_set_pushes", schedules)
 
     def resident_wbc(self, t_now, rbd, stance_mode=None):
         """Policy of the resident solution at absolute time t_now + WeightedWbc: returns (x_des, u_des, mode, sol, torque, status)."""

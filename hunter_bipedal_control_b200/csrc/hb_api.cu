@@ -33,6 +33,15 @@
 using namespace hb;
 
 // ---------------------------------------------------------------------------------------------- context
+// A per-robot setting of the context's episodes: the first n instances have one. The device copy is allocated at max_batch by the first
+// call that sets it; host keeps the validated array the copy reads.
+template <class T> struct InstanceSetting {
+  T* dev;
+  int n;
+  std::vector<T> host;
+  const T* get() const { return n > 0 ? dev : nullptr; }   // what the kernels read: null while unset
+};
+
 struct hb_ctx {
   hb_config cfg;
   hb_wbc_settings wbc;       // WBC gains / limits / weights in force (task.info values by default; hb_wbc_set_settings, hb_load_task_info)
@@ -60,29 +69,18 @@ struct hb_ctx {
   double* res_sol; int res_sol_valid;   // last good WBC solution per instance (WeightedWbc fallback, W5)
   double* res_stance;                 // the device planner's latest stance positions (row N1)
   // hb_rollout_batch_dev's scratch, allocated at max_batch by its first call: commands, plan inputs -> planner -> cycle, the tick's WBC
-  // solution / joint command / torques, the states held instances are put back to, the tick time
+  // solution / joint command / torques, the states held instances are put back to, the tick time, the tick's push wrench (B x 6)
   void* ro_mem;
   hb_rollout_command* ro_cmd; hb_plan_input* ro_in; hb_reference* ro_refs; hb_solve_info* ro_info; int32_t* ro_pstat;
-  double *ro_t0, *ro_x0, *ro_feet, *ro_sol, *ro_jcmd, *ro_jtau, *ro_tau, *ro_held, *ro_tnow;
+  double *ro_t0, *ro_x0, *ro_feet, *ro_sol, *ro_jcmd, *ro_jtau, *ro_tau, *ro_held, *ro_tnow, *ro_wrench;
   // hb_rollout_estimated_batch_dev's own scratch (first such call, at max_batch): the tick's sensor readings, contact flags, estimated rbd
   void* re_mem;
   double *re_quat, *re_gyro, *re_acc, *re_jpos, *re_jvel, *re_rbd;
   uint8_t* re_flag;
-  // push schedules of the episodes (hb_rollout_set_pushes): the first push_n instances have one, the device copy and the tick's wrench
-  // (B x 6) are allocated at max_batch by the first call that sets them; push_host keeps the validated array the copy reads
-  void* push_mem;
-  hb_push_schedule* push_sched; double* push_wrench;
-  int push_n;
-  std::vector<hb_push_schedule> push_host;
-  // plant variations of the episodes (hb_rollout_set_plant_variations): the first var_n instances have one; the device copy is allocated
-  // at max_batch by the first call that sets them, var_host keeps the validated array the copy reads
-  hb_plant_variation* var_dev;
-  int var_n;
-  std::vector<hb_plant_variation> var_host;
-  // terrains of the episodes (hb_rollout_set_terrains): the first ter_n instances have one; allocated and kept as var_dev / var_host
-  hb_terrain* ter_dev;
-  int ter_n;
-  std::vector<hb_terrain> ter_host;
+  // the per-robot settings of the episodes (hb_rollout_set_pushes / _plant_variations / _terrains), set by set_instances
+  InstanceSetting<hb_push_schedule> pushes;
+  InstanceSetting<hb_plant_variation> variations;
+  InstanceSetting<hb_terrain> terrains;
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
   // hb_resident_cycle_batch's packed references / reference verdicts
   void* arena; size_t arena_cap;
@@ -151,6 +149,27 @@ template <class F = bool (*)()> int enter(hb_ctx* ctx, int B, bool args, Cap cap
     const int rc__ = enter(__VA_ARGS__);                             \
     if (rc__) return rc__ == EMPTY ? HB_OK : rc__;                   \
   } while (0)
+
+// true when every one of the B records passes ok (a null array holds none)
+template <class T> bool all_ok(int B, const T* src, bool (*ok)(const T&)) {
+  if (src) for (int i = 0; i < B; ++i) if (!ok(src[i])) return false;
+  return true;
+}
+
+// The body of the per-robot setting calls (hunter_b200.h, "per-robot episode settings"): the records are validated on the host, B == 0
+// clears the setting, a rejected call keeps the previous one and enqueues nothing, the copy goes in stream order on the context's stream.
+template <class T> int set_instances(hb_ctx* ctx, int B, const T* src, bool (*ok)(const T&), InstanceSetting<T> hb_ctx::*setting) {
+  const int rc = enter(ctx, B, B == 0 || src, CAPPED, [&] { return all_ok(B, src, ok); });
+  if (rc == EMPTY) { (ctx->*setting).n = 0; return HB_OK; }
+  if (rc) return rc;
+  InstanceSetting<T>& s = ctx->*setting;
+  if (!s.dev && dalloc(&s.dev, (size_t)ctx->cfg.max_batch) != cudaSuccess) { cudaGetLastError(); s.dev = nullptr; return HB_ENOMEM; }
+  // a pageable copy the context owns: cudaMemcpyAsync has consumed it when it returns, whatever memory the caller's array is in
+  try { s.host.assign(src, src + B); } catch (const std::bad_alloc&) { return HB_ENOMEM; }
+  CK(cudaMemcpyAsync(s.dev, s.host.data(), sizeof(T) * B, cudaMemcpyHostToDevice, ctx->stream));
+  s.n = B;
+  return HB_OK;
+}
 
 // The validity of each kind of scalar parameter, shared by every entry point that takes it (NaN fails every test)
 bool sim_params_ok(const hb_sim_params& p) { return p.dt > 0.0 && p.substeps >= 1 && p.substeps <= 1000; }
@@ -420,7 +439,7 @@ int hb_destroy(hb_ctx* ctx) {
   void* ptrs[] = {ctx->sqp_mem, ctx->dxt, ctx->dut, ctx->perf, ctx->flags, ctx->xdes, ctx->udes, ctx->wstatus, ctx->witers, ctx->wmode,
                   ctx->hoqp_mem, ctx->cyc_xref, ctx->cyc_swing, ctx->cyc_tk, ctx->cyc_mode, ctx->cyc_nn, ctx->res_t0, ctx->res_xt,
                   ctx->res_ut, ctx->res_tk, ctx->res_mode, ctx->res_nn, ctx->res_sol, ctx->res_stance, ctx->arena, ctx->ro_mem, ctx->re_mem,
-                  ctx->push_mem, ctx->var_dev, ctx->ter_dev};
+                  ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -906,23 +925,6 @@ static bool plant_variation_ok(const hb_plant_variation& v) {
   return true;
 }
 
-int hb_rollout_set_plant_variations(hb_ctx* ctx, int B, const hb_plant_variation* v) {
-  const int rc = enter(ctx, B, B == 0 || v, CAPPED, [&] {
-    for (int i = 0; i < B; ++i) if (!plant_variation_ok(v[i])) return false;
-    return true;
-  });
-  if (rc == EMPTY) { ctx->var_n = 0; return HB_OK; }      // cleared: the episodes run the nominal plant
-  if (rc) return rc;
-  if (!ctx->var_dev && dalloc(&ctx->var_dev, (size_t)ctx->cfg.max_batch) != cudaSuccess) {
-    cudaGetLastError(); ctx->var_dev = nullptr; return HB_ENOMEM;
-  }
-  // a pageable copy the context owns: cudaMemcpyAsync has consumed it when it returns, whatever memory the caller's array is in
-  try { ctx->var_host.assign(v, v + B); } catch (const std::bad_alloc&) { return HB_ENOMEM; }
-  CK(cudaMemcpyAsync(ctx->var_dev, ctx->var_host.data(), sizeof(hb_plant_variation) * B, cudaMemcpyHostToDevice, ctx->stream));
-  ctx->var_n = B;
-  return HB_OK;
-}
-
 // The ranges of hunter_b200.h's hb_terrain: grid sizes, a finite origin, a finite positive spacing, finite heights where they are read
 static bool terrain_ok(const hb_terrain& t) {
   if (t.nx < 2 || t.nx > HB_TERRAIN_MAX || t.ny < 2 || t.ny > HB_TERRAIN_MAX) return false;
@@ -932,22 +934,20 @@ static bool terrain_ok(const hb_terrain& t) {
   return true;
 }
 
-int hb_rollout_set_terrains(hb_ctx* ctx, int B, const hb_terrain* t) {
-  const int rc = enter(ctx, B, B == 0 || t, CAPPED, [&] {
-    for (int i = 0; i < B; ++i) if (!terrain_ok(t[i])) return false;
-    return true;
-  });
-  if (rc == EMPTY) { ctx->ter_n = 0; return HB_OK; }      // cleared: the episodes run on flat ground
-  if (rc) return rc;
-  if (!ctx->ter_dev && dalloc(&ctx->ter_dev, (size_t)ctx->cfg.max_batch) != cudaSuccess) {
-    cudaGetLastError(); ctx->ter_dev = nullptr; return HB_ENOMEM;
+static bool push_schedule_ok(const hb_push_schedule& s) {
+  if (s.n_push < 0 || s.n_push > HB_MAX_PUSHES) return false;
+  for (int j = 0; j < s.n_push; ++j) {
+    if (!isfinite(s.t_start[j]) || !isfinite(s.duration[j]) || !(s.duration[j] >= 0.0)) return false;
+    for (int c = 0; c < 3; ++c) if (!isfinite(s.force[j][c]) || !isfinite(s.torque[j][c])) return false;
   }
-  // a pageable copy the context owns: cudaMemcpyAsync has consumed it when it returns, whatever memory the caller's array is in
-  try { ctx->ter_host.assign(t, t + B); } catch (const std::bad_alloc&) { return HB_ENOMEM; }
-  CK(cudaMemcpyAsync(ctx->ter_dev, ctx->ter_host.data(), sizeof(hb_terrain) * B, cudaMemcpyHostToDevice, ctx->stream));
-  ctx->ter_n = B;
-  return HB_OK;
+  return true;
 }
+
+int hb_rollout_set_pushes(hb_ctx* ctx, int B, const hb_push_schedule* p) { return set_instances(ctx, B, p, push_schedule_ok, &hb_ctx::pushes); }
+int hb_rollout_set_plant_variations(hb_ctx* ctx, int B, const hb_plant_variation* v) {
+  return set_instances(ctx, B, v, plant_variation_ok, &hb_ctx::variations);
+}
+int hb_rollout_set_terrains(hb_ctx* ctx, int B, const hb_terrain* t) { return set_instances(ctx, B, t, terrain_ok, &hb_ctx::terrains); }
 
 // hb_resident_wbc_batch_dev; no_prev = true: the fallback has no previous solution yet (first tick after a cold start whose cycle ran no WBC)
 static int resident_wbc_impl(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
@@ -989,7 +989,7 @@ static int rollout_reserve(hb_ctx* ctx) {
     ctx->ro_info = carve<hb_solve_info>(m, off, Bc); ctx->ro_pstat = carve<int32_t>(m, off, Bc); ctx->ro_t0 = carve<double>(m, off, Bc);
     ctx->ro_x0 = carve<double>(m, off, Bc * NX); ctx->ro_feet = carve<double>(m, off, Bc * 12); ctx->ro_sol = carve<double>(m, off, Bc * NWBC);
     ctx->ro_jcmd = carve<double>(m, off, Bc * NJ * 5); ctx->ro_jtau = carve<double>(m, off, Bc * NJ); ctx->ro_tau = carve<double>(m, off, Bc * NJ);
-    ctx->ro_held = carve<double>(m, off, Bc * 32); ctx->ro_tnow = carve<double>(m, off, Bc);
+    ctx->ro_held = carve<double>(m, off, Bc * 32); ctx->ro_tnow = carve<double>(m, off, Bc); ctx->ro_wrench = carve<double>(m, off, Bc * 6);
     return off;
   });
 }
@@ -1004,40 +1004,6 @@ static int estimation_reserve(hb_ctx* ctx) {
     ctx->re_flag = carve<uint8_t>(m, off, Bc * 4);
     return off;
   });
-}
-
-// the episodes' push schedules and the tick's wrench, at max_batch
-static int push_reserve(hb_ctx* ctx) {
-  const size_t Bc = ctx->cfg.max_batch;
-  return reserve_group(&ctx->push_mem, [&](void* m) {
-    size_t off = 0;
-    ctx->push_sched = carve<hb_push_schedule>(m, off, Bc); ctx->push_wrench = carve<double>(m, off, Bc * 6);
-    return off;
-  });
-}
-
-static bool push_schedule_ok(const hb_push_schedule& s) {
-  if (s.n_push < 0 || s.n_push > HB_MAX_PUSHES) return false;
-  for (int j = 0; j < s.n_push; ++j) {
-    if (!isfinite(s.t_start[j]) || !isfinite(s.duration[j]) || !(s.duration[j] >= 0.0)) return false;
-    for (int c = 0; c < 3; ++c) if (!isfinite(s.force[j][c]) || !isfinite(s.torque[j][c])) return false;
-  }
-  return true;
-}
-
-int hb_rollout_set_pushes(hb_ctx* ctx, int B, const hb_push_schedule* pushes) {
-  const int rc = enter(ctx, B, B == 0 || pushes, CAPPED, [&] {
-    for (int i = 0; i < B; ++i) if (!push_schedule_ok(pushes[i])) return false;
-    return true;
-  });
-  if (rc == EMPTY) { ctx->push_n = 0; return HB_OK; }     // cleared: the episodes run without a wrench
-  if (rc) return rc;
-  if (int e = push_reserve(ctx)) return e;
-  // a pageable copy the context owns: cudaMemcpyAsync has consumed it when it returns, whatever memory the caller's array is in
-  try { ctx->push_host.assign(pushes, pushes + B); } catch (const std::bad_alloc&) { return HB_ENOMEM; }
-  CK(cudaMemcpyAsync(ctx->push_sched, ctx->push_host.data(), sizeof(hb_push_schedule) * B, cudaMemcpyHostToDevice, ctx->stream));
-  ctx->push_n = B;
-  return HB_OK;
 }
 
 // the estimation arguments of an estimated episode; a null pointer to them is hb_rollout_batch_dev
@@ -1073,19 +1039,18 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   const unsigned grid = (B + 63) / 64;
   // what the controllers measure: the true state, or the filter's estimate
   double* meas = e ? ctx->re_rbd : rbd;
-  // the push wrench the begin kernel writes and the plant applies; none without schedules
-  double* wrench = ctx->push_n > 0 ? ctx->push_wrench : nullptr;
-  // the instances' plants; the nominal one for all without variations
-  const hb_plant_variation* var = ctx->var_n > 0 ? ctx->var_dev : nullptr;
-  // the ground under the instances, for the plant and the height check; flat ground for all without terrains
-  const hb_terrain* ter = ctx->ter_n > 0 ? ctx->ter_dev : nullptr;
+  // the episode settings (null while unset); the push wrench the begin kernel writes and the plant applies, none without schedules
+  const hb_push_schedule* push = ctx->pushes.get();
+  const hb_plant_variation* var = ctx->variations.get();
+  const hb_terrain* ter = ctx->terrains.get();
+  double* wrench = push ? ctx->ro_wrench : nullptr;
   for (int k = 0; k < n_ticks && !rc; ++k) {
     const int64_t a = tick0 + k;
     const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
     const bool mpc = a % p->mpc_every == 0, first_cold = cold && k == 0;
     double* log_row = (n_log && k % p->log_every == 0) ? log + (size_t)(k / p->log_every) * 32 : nullptr;
     rc = launch(ctx, K_UNPROFILED, rollout_tick_begin_kernel, grid, 64, 0, B, (int)a, t, p->min_base_height, rbd, ctx->ro_held, stats, ctx->ro_tnow,
-                log_row, (size_t)n_log * 32, ctx->push_sched, ctx->push_n, wrench, ter, ctx->ter_n);
+                log_row, (size_t)n_log * 32, push, ctx->pushes.n, wrench, ter, ctx->terrains.n);
     if (!rc && e) {
       // LeggedController::updateStateEstimation: sensors and contact flags at the previous observation's time, filter, observation step
       double* est_row = (n_est_log && k % p->log_every == 0) ? e->log + (size_t)(k / p->log_every) * 32 : nullptr;
@@ -1109,7 +1074,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
                                              ctx->ro_jtau);
     if (!rc) rc = hb_actuation_batch_dev(ctx, B, p->actuation_delay, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, ctx->ro_tau);
-    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, var, ctx->var_n, ter, ctx->ter_n, nullptr, nullptr);
+    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, var, ctx->variations.n, ter, ctx->terrains.n, nullptr, nullptr);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_tick_end_kernel, grid, 64, 0, B, (int)a, mpc ? 1 : 0, ctx->ro_info, ctx->ro_pstat, ctx->wstatus, estop, ctx->ro_tau, ctx->ro_held, rbd, stats);
   }
   return rc;
@@ -1513,18 +1478,12 @@ int hb_actuation_batch(hb_ctx* ctx, int B, double delay, const double* time, hb_
 }
 
 int hb_sim_step_batch(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {
-  ENTER(ctx, B, params && rbd && tau, CAPPED, [&] { return sim_params_ok(*params); });
-  Staging s(ctx, B);
-  auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
-  return s.run(1, [&](Chunk) { return hb_sim_step_batch_dev(ctx, B, params, r, t, cf, fl); });
+  return hb_sim_step_terrain(ctx, B, params, rbd, tau, nullptr, nullptr, nullptr, contact_force, contact_flag);
 }
 
 int hb_sim_step_wrench(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench, double* contact_force,
                        uint8_t* contact_flag) {
-  ENTER(ctx, B, params && rbd && tau, CAPPED, [&] { return sim_params_ok(*params); });
-  Staging s(ctx, B);
-  auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto w = s.in_or_null(wrench, 6); auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
-  return s.run(1, [&](Chunk) { return sim_step(ctx, B, *params, r, t, w, nullptr, 0, nullptr, 0, cf, fl); });
+  return hb_sim_step_terrain(ctx, B, params, rbd, tau, wrench, nullptr, nullptr, contact_force, contact_flag);
 }
 
 int hb_sim_step_varied(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* v,
@@ -1532,14 +1491,11 @@ int hb_sim_step_varied(hb_ctx* ctx, int B, const hb_sim_params* params, double* 
   return hb_sim_step_terrain(ctx, B, params, rbd, tau, wrench, v, nullptr, contact_force, contact_flag);
 }
 
+// the one host-pointer plant step: the three above are it with null terrains, variations and wrench
 int hb_sim_step_terrain(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* v,
                         const hb_terrain* ter, double* contact_force, uint8_t* contact_flag) {
-  ENTER(ctx, B, params && rbd && tau, CAPPED, [&] {
-    if (!sim_params_ok(*params)) return false;
-    if (v) for (int i = 0; i < B; ++i) if (!plant_variation_ok(v[i])) return false;
-    if (ter) for (int i = 0; i < B; ++i) if (!terrain_ok(ter[i])) return false;
-    return true;
-  });
+  ENTER(ctx, B, params && rbd && tau, CAPPED,
+        [&] { return sim_params_ok(*params) && all_ok(B, v, plant_variation_ok) && all_ok(B, ter, terrain_ok); });
   Staging s(ctx, B);
   auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto w = s.in_or_null(wrench, 6); auto pv = s.in_or_null(v, 1); auto pt = s.in_or_null(ter, 1);
   auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);

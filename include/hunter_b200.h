@@ -232,6 +232,14 @@ typedef struct {                 /* per-instance outcome, in/out: start an episo
 } hb_rollout_stats;
 int hb_default_rollout_params(hb_rollout_params* p);       /* host only */
 
+/* ---- per-robot episode settings: pushes, plant variations and terrains (hb_rollout_set_pushes / _plant_variations / _terrains) ----
+ * Each sets one record per robot on the context: from then on both episode calls apply record i to instance i of their batch for i < B.
+ * The records are a host array, validated on the host and copied to the context in stream order on the context's stream; the caller may
+ * free it when the call returns. B == 0 clears the setting (the array may be NULL). -1: B < 0, a NULL array with B > 0, or a record
+ * outside its documented range; -4: B > max_batch. A rejected call keeps the previous setting and enqueues nothing. Instances at or beyond
+ * B run the nominal plant (no push, no variation) on the flat ground of sim.ground_height. The device copy is allocated at max_batch by
+ * the first call that sets records and freed by hb_destroy. Settings add no launch to an episode. */
+
 /* ---- pushed episodes: scheduled external wrenches on the base, applied by the plant of both episode calls ----
  * Push j acts on the plant step of absolute tick a iff t_start[j] <= t && t < t_start[j] + duration[j], with t = (double)a * period (the
  * episode's tick time). During that step the wrench is constant over all substeps, so a push is quantised to whole ticks. Overlapping
@@ -248,12 +256,8 @@ typedef struct {                      /* external pushes on one robot's base    
   double force[HB_MAX_PUSHES][3];     /* world frame [N], applied at the base frame origin (rbd[3:6])                         */
   double torque[HB_MAX_PUSHES][3];    /* world frame couple [N m]                                                             */
 } hb_push_schedule;
-/* Sets the push schedules of the context's episodes: from then on both episode calls apply pushes[i] to instance i of their batch for i < B;
- * instances at or beyond B get no push. B == 0 clears them (pushes may be NULL). pushes is a host array, validated on the host and copied
- * to the context in stream order on the context's stream; the caller may free it when the call returns. -1: B < 0, NULL pushes with B > 0,
- * n_push outside 0..HB_MAX_PUSHES, a non-finite t_start / force / torque, a negative or non-finite duration; -4: B > max_batch. A rejected
- * call keeps the previous setting and enqueues nothing. The device copy is allocated at max_batch by the first call that sets pushes and
- * freed by hb_destroy. Pushes add no launch to an episode. */
+/* Sets the push schedules of the context's episodes (a per-robot episode setting, above). -1 also for n_push outside 0..HB_MAX_PUSHES, a
+ * non-finite t_start / force / torque, a negative or non-finite duration. */
 int hb_rollout_set_pushes(hb_ctx* ctx, int B, const hb_push_schedule* pushes);
 
 /* ---- varied plants: a plant of its own for each robot of the episodes (payload on the base, ground contact, motor strength) ----
@@ -282,13 +286,9 @@ typedef struct {                 /* the plant of one robot, relative to hb_sim_p
   double motor_strength[10];     /* joint j receives motor_strength[j] * tau[j], >= 0 (0 = a dead motor)              */
 } hb_plant_variation;            /* 208 B */
 int hb_default_plant_variation(hb_plant_variation* v);      /* host only: no payload, every scale 1 */
-/* Sets the plant variations of the context's episodes: from then on both episode calls run instance i of their batch on the plant v[i] for
- * i < B; instances at or beyond B get the nominal plant. B == 0 clears them (v may be NULL). v is a host array, validated on the host and
- * copied to the context in stream order on the context's stream; the caller may free it when the call returns. -1: B < 0, NULL v with
- * B > 0, or a field outside its range above: any non-finite value, an inertia that is not exactly symmetric or has a negative principal
- * minor (Sylvester's criterion, in double), a zero mass with a nonzero CoM or inertia; -4: B > max_batch. A rejected call keeps the previous
- * setting and enqueues nothing. The device copy is allocated at max_batch by the first call that sets variations and freed by hb_destroy.
- * Variations add no launch to an episode. */
+/* Sets the plant variations of the context's episodes (a per-robot episode setting, above). -1 also for a field outside its range above:
+ * any non-finite value, an inertia that is not exactly symmetric or has a negative principal minor (Sylvester's criterion, in double), a
+ * zero mass with a nonzero CoM or inertia. */
 int hb_rollout_set_plant_variations(hb_ctx* ctx, int B, const hb_plant_variation* v);
 
 /* ---- terrain: the ground under each robot of the episodes, a height field on a regular world-frame grid ----
@@ -316,12 +316,9 @@ typedef struct {                      /* the ground under one robot: a height fi
   double height[HB_TERRAIN_MAX][HB_TERRAIN_MAX];  /* height[j][i] = ground z at (origin[0] + i spacing, origin[1] + j spacing);
                                          only j < ny, i < nx are read                                                              */
 } hb_terrain;                         /* 32 800 B */
-/* Sets the terrains of the context's episodes: from then on both episode calls run instance i of their batch on the ground t[i] for
- * i < B; instances at or beyond B stand on the flat ground of sim.ground_height. B == 0 clears them (t may be NULL). t is a host array,
- * validated on the host and copied to the context in stream order on the context's stream; the caller may free it when the call returns.
- * -1: B < 0, NULL t with B > 0, nx or ny outside 2..HB_TERRAIN_MAX, a non-finite origin, a spacing that is not finite and > 0, a
- * non-finite height among the used samples; -4: B > max_batch. A rejected call keeps the previous setting and enqueues nothing. The
- * device copy is allocated at max_batch by the first call that sets terrains (33.6 MB at 1024) and freed by hb_destroy. */
+/* Sets the terrains of the context's episodes (a per-robot episode setting, above; the device copy takes 33.6 MB at 1024). -1 also for
+ * nx or ny outside 2..HB_TERRAIN_MAX, a non-finite origin, a spacing that is not finite and > 0, a non-finite height among the used
+ * samples. */
 int hb_rollout_set_terrains(hb_ctx* ctx, int B, const hb_terrain* t);
 
 /* ---- estimated episodes (hb_rollout_estimated_batch_dev): the controllers read the Kalman filter's estimate from synthesised, noisy
@@ -583,7 +580,8 @@ int hb_sim_step_wrench(hb_ctx* ctx, int B, const hb_sim_params* params, double* 
 int hb_sim_step_varied(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench /*nullable*/,
                        const hb_plant_variation* v /*nullable*/, double* contact_force /*nullable*/, uint8_t* contact_flag /*nullable*/);
 /* hb_sim_step_varied on terrains: t (B, nullable) = the ground under each robot (terrain, above), validated as by hb_rollout_set_terrains
- * (-1). NULL t is exactly hb_sim_step_varied. */
+ * (-1). NULL t is exactly hb_sim_step_varied. This is the one host-pointer plant step: hb_sim_step_batch, hb_sim_step_wrench and
+ * hb_sim_step_varied are it with the arguments they lack passed as NULL. */
 int hb_sim_step_terrain(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench /*nullable*/,
                         const hb_plant_variation* v /*nullable*/, const hb_terrain* t /*nullable*/, double* contact_force /*nullable*/,
                         uint8_t* contact_flag /*nullable*/);

@@ -5,6 +5,7 @@ import ctypes as C
 import math
 
 import numpy as np
+import pytest
 
 import hunter_bipedal_control_b200 as hb
 from hunter_bipedal_control_b200 import scenarios as sc
@@ -17,6 +18,7 @@ GAIT_START = 0.1
 CMD_TIMES = [0.0, 0.2]             # the command changes half way through a 200-tick episode
 SIGMAS = dict(orientation=0.002, angular_velocity=0.01, linear_acceleration=0.05, joint_position=0.001, joint_velocity=0.01)
 OUTPUTS = ("rbd", "act", "estop", "stats", "log", "est", "est_stats", "est_log")      # Context.rollout_estimated's tuple; rollout's: the first 5
+G = 9.81
 
 
 # ---------------------------------------------------------------------------------------------------------------- setup
@@ -77,37 +79,127 @@ def T(zyx):
     return np.array([[0.0, -sz, cz * cy], [0.0, cz, sz * cy], [1.0, 0.0, -sy]])
 
 
-def plant_numpy(oracle, rbd, tau, prm, wrench=None):
-    """One plant step of one robot: returns (rbd_next, contact forces of the last substep). wrench (6,): an external world force at the base
-    origin and a world couple, Q_p = f, Q_zyx = T' tau at each substep's orientation; None adds no generalised force."""
+def payload_terms(q, v, variation):
+    """The payload of a plant variation in the base coordinates (p, zyx) of q, v: (M_p, nle_p), the 6 x 6 base block it adds to M and the 6
+    entries it adds to nle, from the documented formulas: with omega = T zyx_dot, r = R c and I_w = R I_c R', column k of M_p is
+    [F; T' n] for F = m (pdd + omega_dot x r), n = I_w omega_dot + r x F at a unit acceleration of coordinate k and v = 0; nle_p is the
+    same with omega_dot0 = (omega_1 x a_pitch) dpitch + (omega_2 x a_roll) droll, F = m (omega_dot0 x r + omega x (omega x r)) + m g e_z,
+    n = I_w omega_dot0 + omega x I_w omega + r x F."""
+    from oracle import refs
+    m = variation.payload_mass
+    c = np.array(variation.payload_com[:]); Ic = np.array(variation.payload_inertia[:]).reshape(3, 3)
+    R, Tm = refs.rot_zyx(q[3:6]), T(q[3:6])
+    r, Iw = R @ c, R @ Ic @ R.T
+    M = np.zeros((6, 6))
+    for k in range(6):
+        a = np.zeros(6); a[k] = 1.0
+        wd = Tm @ a[3:]
+        F = m * (a[:3] + np.cross(wd, r))
+        M[:, k] = np.r_[F, Tm.T @ (Iw @ wd + np.cross(r, F))]
+    dz = v[3:6]
+    w1 = Tm[:, 0] * dz[0]; w2 = w1 + Tm[:, 1] * dz[1]; w = Tm @ dz
+    wd0 = np.cross(w1, Tm[:, 1]) * dz[1] + np.cross(w2, Tm[:, 2]) * dz[2]
+    F = m * (np.cross(wd0, r) + np.cross(w, np.cross(w, r))) + m * G * np.array([0.0, 0.0, 1.0])
+    n = Iw @ wd0 + np.cross(w, Iw @ w) + np.cross(r, F)
+    return M, np.r_[F, Tm.T @ n]
+
+
+def _axis(x, origin, spacing, n):
+    """(cell index, fraction, clamped) of world coordinate x along one grid axis; NaN clamps to 0 as the kernel does."""
+    u = (x - origin) / spacing
+    clamped = False
+    if not u >= 0.0:
+        u, clamped = 0.0, True
+    elif u > n - 1:
+        u, clamped = float(n - 1), True
+    i = min(int(math.floor(u)), n - 2)
+    return i, u - i, clamped
+
+
+def terrain_height(t, x, y):
+    """(h, g_x, g_y) of the HbTerrain t at world (x, y), as hunter_b200.h documents it."""
+    i, a, cx = _axis(x, t.origin[0], t.spacing, t.nx)
+    j, b, cy = _axis(y, t.origin[1], t.spacing, t.ny)
+    h00, h01, h10, h11 = t.height[j][i], t.height[j][i + 1], t.height[j + 1][i], t.height[j + 1][i + 1]
+    h0 = h00 + a * (h01 - h00)
+    h1 = h10 + a * (h11 - h10)
+    d0, d1 = h01 - h00, h11 - h10
+    gx = 0.0 if cx else (d0 + b * (d1 - d0)) / t.spacing
+    gy = 0.0 if cy else (h1 - h0) / t.spacing
+    return h0 + b * (h1 - h0), gx, gy
+
+
+def contact_numpy(p, v, ground, k, d, ct, mu):
+    """(force (3,), normal force) of one contact point at p with velocity v on the ground (h, g_x, g_y) under it, with ground stiffness k,
+    damping d, tangential damping ct and friction coefficient mu: the flat path where the gradient is zero, the sloped path elsewhere."""
+    h, gx, gy = ground
+    if gx == 0.0 and gy == 0.0:
+        depth = h - p[2]
+        if not depth > 0:
+            return np.zeros(3), 0.0
+        fz = max(0.0, k * depth - d * v[2])
+        ft = -ct * v[:2]
+        n = np.linalg.norm(ft)
+        if n > mu * fz:
+            ft = ft * (mu * fz / n if n > 0 else 0.0)
+        return np.array([ft[0], ft[1], fz]), fz
+    L = math.sqrt(1.0 + gx * gx + gy * gy)
+    n = np.array([-gx, -gy, 1.0]) / L
+    depth = (h - p[2]) / L
+    if not depth > 0:
+        return np.zeros(3), 0.0
+    vn = float(v @ n)
+    fn = max(0.0, k * depth - d * vn)
+    ft = -ct * (v - vn * n)
+    tl = np.linalg.norm(ft)
+    if tl > mu * fn:
+        ft = ft * (mu * fn / tl if tl > 0 else 0.0)
+    return fn * n + ft, fn
+
+
+def plant_numpy(oracle, rbd, tau, prm, wrench=None, variation=None, terrain=None):
+    """One plant step of one robot: returns (rbd_next, contact forces of the last substep (12,), contact flags of the last substep (4,)).
+    wrench (6,): an external world force at the base origin and a world couple, Q_p = f, Q_zyx = T' tau at each substep's orientation.
+    variation (an HbPlantVariation): the ground stiffness, damping and friction scaled, the joint torques scaled by the motor strengths and,
+    with a payload, payload_terms added to M and nle. terrain (an HbTerrain): each contact on the ground terrain_height gives under it.
+    None is no wrench, the nominal plant, and flat ground at prm.ground_height."""
     from oracle import refs
     q = np.concatenate([rbd[3:6], rbd[0:3], rbd[6:16]])
     v = np.concatenate([rbd[19:22], refs.euler_rates_from_global(rbd[0:3], rbd[16:19]), rbd[22:32]])
     h = prm.dt / prm.substeps
-    F = np.zeros(12)
+    k_g, d_g, mu = prm.ground_stiffness, prm.ground_damping, prm.friction_mu
+    if variation is not None:
+        k_g, d_g, mu = k_g * variation.stiffness_scale, d_g * variation.damping_scale, mu * variation.friction_scale
+        tau = np.array(variation.motor_strength[:]) * tau
+    F, flags = np.zeros(12), np.zeros(4, dtype=bool)
     for _ in range(prm.substeps):
         r = oracle.rbd(q, v)
+        M, nle = r["M"].copy(), r["nle"].copy()
+        if variation is not None and variation.payload_mass > 0:
+            Mp, nlep = payload_terms(q, v, variation)
+            M[:6, :6] += Mp; nle[:6] += nlep
         cvel = r["J"] @ v
         F = np.zeros(12)
         for c in range(4):
-            depth = prm.ground_height - r["cpos"][3 * c + 2]
-            if depth > 0:
-                fz = max(0.0, prm.ground_stiffness * depth - prm.ground_damping * cvel[3 * c + 2])
-                ft = -prm.tangential_damping * cvel[3 * c:3 * c + 2]
-                n = np.linalg.norm(ft)
-                if n > prm.friction_mu * fz:
-                    ft = ft * (prm.friction_mu * fz / n if n > 0 else 0.0)
-                F[3 * c:3 * c + 3] = [ft[0], ft[1], fz]
-        rhs = np.concatenate([np.zeros(6), tau - prm.joint_damping * v[6:]]) + r["J"].T @ F - r["nle"]
+            p = r["cpos"][3 * c:3 * c + 3]
+            ground = (prm.ground_height, 0.0, 0.0) if terrain is None else terrain_height(terrain, p[0], p[1])
+            F[3 * c:3 * c + 3], fn = contact_numpy(p, cvel[3 * c:3 * c + 3], ground, k_g, d_g, prm.tangential_damping, mu)
+            flags[c] = fn > 0
+        rhs = np.concatenate([np.zeros(6), tau - prm.joint_damping * v[6:]]) + r["J"].T @ F - nle
         if wrench is not None:
             rhs = rhs + np.concatenate([wrench[:3], T(q[3:6]).T @ wrench[3:], np.zeros(10)])
-        qdd = np.linalg.solve(r["M"] + np.diag(np.r_[np.zeros(6), np.full(10, prm.joint_armature)]), rhs)
+        qdd = np.linalg.solve(M + np.diag(np.r_[np.zeros(6), np.full(10, prm.joint_armature)]), rhs)
         v = v + h * qdd
         q = q + h * v
     out = np.zeros(32)
     out[0:3] = q[3:6]; out[3:6] = q[0:3]; out[6:16] = q[6:]
     out[16:19] = refs.global_from_euler_rates(q[3:6], v[3:6]); out[19:22] = v[0:3]; out[22:32] = v[6:]
-    return out, F
+    return out, F, flags
+
+
+def flat_terrain(height, center=(0.0, 0.0), spacing=0.5):
+    """One flat HbTerrain at `height`: a 2 x 2 grid around `center`."""
+    return hb.make_terrains(1, np.full((2, 2), height), spacing, np.asarray(center) - 0.5 * spacing)[0]
 
 
 def wrench_numpy(pushes, t, B):
@@ -130,12 +222,21 @@ def _mode_at(st, t):
     return st.modes[idx]
 
 
-def stepwise(ctx, rbd0, gaits, cmd_vels, n_ticks, prm, log_every, ep=None, est=None, pushes=None):
+def stepwise(ctx, rbd0, gaits, cmd_vels, n_ticks, prm, log_every, ep=None, est=None, pushes=None, variations=None, terrains=None):
     """The episode as a Python loop of public calls from tick 0, with the checks, holding and stats restated in numpy. It is the device
     loop (rollout_impl) tick for tick: with ep and est (fresh estimation states, advanced in place) it is the estimated episode, whose
-    controllers read the filter's estimate, and the estimation steps sit where the device loop's estimation branches sit. pushes: the
-    schedules set on ctx, applied as each tick's wrench. Returns the tuple of Context.rollout, or of Context.rollout_estimated with ep."""
+    controllers read the filter's estimate, and the estimation steps sit where the device loop's estimation branches sit. pushes,
+    variations, terrains: the settings on ctx. Each tick's wrench comes from the pushes; every plant step runs on the variations and
+    terrains, padded as the setting is documented: the default variation, and flat ground at prm.sim.ground_height, beyond them. The
+    height check here is the absolute one, so with terrains it restates the episode only for prm.min_base_height = 0 (params()). Returns
+    the tuple of Context.rollout, or of Context.rollout_estimated with ep."""
     B = rbd0.shape[0]
+    var = None if variations is None else (hb.HbPlantVariation * B)(
+        *[variations[i] if i < len(variations) else hb.default_plant_variation() for i in range(B)])
+    ter = None
+    if terrains is not None:
+        assert prm.min_base_height == 0
+        ter = (hb.HbTerrain * B)(*[terrains[i] if i < len(terrains) else flat_terrain(prm.sim.ground_height) for i in range(B)])
     rbd = rbd0.copy()
     act = hb.actuation_states(B)
     estop = np.zeros(B, dtype=np.uint8)
@@ -207,7 +308,7 @@ def stepwise(ctx, rbd0, gaits, cmd_vels, n_ticks, prm, log_every, ep=None, est=N
         jcmd, _, estop = ctx.joint_command(prm.period, xd, ud, sol, md, meas, estop=estop, gains=prm.gains)
         tau = ctx.actuation(t, act, jcmd, rbd, prm.actuation_delay)
         tau = np.clip(tau, -lim, lim)
-        rbd, _, _ = ctx.sim_step(rbd, tau, prm.sim, wrench=None if pushes is None else wrench_numpy(pushes, t, B))
+        rbd, _, _ = ctx.sim_step(rbd, tau, prm.sim, wrench=None if pushes is None else wrench_numpy(pushes, t, B), variation=var, terrain=ter)
         for i in range(B):                               # after the plant step
             if st["fail_tick"][i] < 0:
                 if mpc:
@@ -313,3 +414,90 @@ def launch_coefficients(ctx, rbd0, gaits, cmd_vels, prm, ep=None):
     for c, n, d in rows:
         assert d == a * c + b * n, (rows, a, b)
     return a, b
+
+
+# ---------------------------------------------------------------------------------------------------------------- per-robot settings
+# Pushes, plant variations and terrains are per-robot settings of the episodes (Context.set_pushes / set_plant_variations / set_terrains,
+# hb_rollout_set_*), with one contract. The checks below take the setting's name and each test file's own data.
+def _counted(ctx, run):
+    c0 = ctx.launch_count
+    out = run()
+    return out, ctx.launch_count - c0
+
+
+def assert_setting_episodes(ctx, name, rbd0, prm, full, one, other, row, part, padded, cont=None):
+    """The setting on 200-tick episodes of the six instances rbd0, with log_every = 10: set to `cont` (default `full`), two calls split at
+    tick 100 equal one; `one` (only instance 0 differs from the unset episode) moves instance 0 and leaves the others as unset; instance
+    `row` of `other` equals instance `row` of `full`, whatever the other instances have; a permuted batch with the permuted setting gives the
+    permuted result; `part`, a setting of the first k instances, moves them, leaves the others as unset and equals `padded`, the full
+    setting it is documented to be; B = 0 clears the setting."""
+    set_ = getattr(ctx, "set_" + name)
+    B = rbd0.shape[0]
+    vels = cmd_vels(B)
+
+    def run(rbd=rbd0, gaits=GAITS, v=vels):
+        return outputs(device(ctx, rbd, gaits, v, 200, prm, 10))
+
+    set_(full if cont is None else cont)
+    assert_continues(ctx, rbd0, GAITS, vels, 200, 100, prm, 10)
+    set_(None)
+    u = run()
+    set_(one)
+    p = run()
+    assert not np.array_equal(p[0][0], u[0][0])
+    assert_episode_equal(p, u, rows_a=slice(1, None), rows_b=slice(1, None))
+    set_(full)
+    f = run()
+    set_(other)
+    assert_episode_equal(f, run(), rows_a=[row], rows_b=[row])
+    perm = [4, 0, 5, 2, 1, 3]
+    set_((type(full[0]) * B)(*[full[i] for i in perm]))
+    assert_episode_equal(f, run(rbd0[perm], [GAITS[i] for i in perm], vels[perm]), rows_a=perm)
+    k = len(part)
+    set_(part)
+    pt = run()
+    set_(padded)
+    assert_episode_equal(pt, run())
+    assert_episode_equal(pt, u, rows_a=slice(k, None), rows_b=slice(k, None))
+    assert not np.array_equal(pt[0][:k], u[0][:k])
+    assert getattr(ctx._lib, "hb_rollout_set_" + name)(ctx._h, 0, None) == 0
+    assert_episode_equal(run(), u)
+
+
+def assert_null_settings(ctx, name, run, nulls, some):
+    """Each setting of `nulls`, and `some` set and then cleared, reproduce the unset episode `run()` bit for bit with the same launches.
+    Returns the unset episode and its launch count."""
+    set_ = getattr(ctx, "set_" + name)
+    set_(None)
+    ref, launches = _counted(ctx, run)
+    for setting in list(nulls) + [None]:
+        if setting is None:
+            set_(some)
+        set_(setting)
+        out, n = _counted(ctx, run)
+        assert n == launches, (n, launches)
+        assert_episode_equal(ref, out)
+    return ref, launches
+
+
+def assert_rejected_settings(ctx, name, run, setting, bad, big):
+    """With `setting` in force, every rejected call returns before any launch, -1 for each setting of `bad`, a null context, B < 0 and a NULL
+    array, -4 for `big` (max_batch + 1 records), and keeps `setting`: run() is as before, with the same launches. Returns that episode and
+    its launch count."""
+    set_, call = getattr(ctx, "set_" + name), getattr(ctx._lib, "hb_rollout_set_" + name)
+    set_(setting)
+    want, launches = _counted(ctx, run)
+    c0 = ctx.launch_count
+    for b in bad:
+        assert call(ctx._h, len(b), b) == -1
+    assert call(None, 1, setting) == -1
+    assert call(ctx._h, -1, setting) == -1
+    assert call(ctx._h, 1, None) == -1
+    assert len(big) == ctx.max_batch + 1 and call(ctx._h, len(big), big) == -4
+    with pytest.raises(hb.HunterB200Error):
+        set_(bad[0])
+    assert ctx.launch_count == c0
+    got, n = _counted(ctx, run)
+    assert n == launches
+    assert_episode_equal(want, got)
+    return want, launches

@@ -46,7 +46,7 @@ def test_plant_step_matches_numpy_restatement(gpu_ctx, oracle):
     nxt, cf, fl = gpu_ctx.sim_step(rbd, tau, prm)
     touched = 0
     for i in range(B):
-        ref, F = plant_numpy(oracle, rbd[i], tau[i], prm)
+        ref, F, _ = plant_numpy(oracle, rbd[i], tau[i], prm)
         assert np.abs(nxt[i] - ref).max() < 1e-9 * max(1.0, np.abs(ref).max()), i
         assert np.abs(cf[i] - F).max() < 1e-7 * max(1.0, np.abs(F).max())
         assert np.array_equal(fl[i] != 0, F[2::3] > 0)

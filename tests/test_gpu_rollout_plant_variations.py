@@ -9,10 +9,9 @@ import pytest
 
 import hunter_bipedal_control_b200 as hb
 from hunter_bipedal_control_b200 import scenarios as sc
-from episode_ref import (GAITS, assert_continues, assert_episode_equal, cmd_vels, context, device, est_params, launch_coefficients, outputs,
-                         params, start_states)
+from episode_ref import (GAITS, assert_episode_equal, assert_null_settings, assert_rejected_settings, assert_setting_episodes, cmd_vels, context,
+                         device, est_params, launch_coefficients, params, plant_numpy, start_states, stepwise)
 from oracle import refs
-from plant_variation_ref import plant_numpy_varied, stepwise_varied
 
 pytestmark = pytest.mark.gpu
 
@@ -70,7 +69,7 @@ def test_varied_plant_step_matches_numpy_restatement(gpu_ctx, oracle):
     base = gpu_ctx.sim_step(rbd, tau, prm, wrench=W)
     touched = 0
     for i in range(B):
-        ref, F = plant_numpy_varied(oracle, rbd[i], tau[i], prm, V[i], W[i])
+        ref, F, _ = plant_numpy(oracle, rbd[i], tau[i], prm, W[i], V[i])
         assert np.abs(nxt[i] - ref).max() < 1e-9 * max(1.0, np.abs(ref).max()), (i, np.abs(nxt[i] - ref).max())
         assert np.abs(cf[i] - F).max() < 1e-7 * max(1.0, np.abs(F).max()), i
         assert np.array_equal(fl[i] != 0, F[2::3] > 0)
@@ -81,7 +80,7 @@ def test_varied_plant_step_matches_numpy_restatement(gpu_ctx, oracle):
     P = hb.make_plant_variations(B, 4.0, [0.05, 0.02, 0.12], _full_inertia(rng, 0.01))
     nxt, cf, _ = gpu_ctx.sim_step(rbd, tau, prm, variation=P)
     for i in range(B):
-        ref, F = plant_numpy_varied(oracle, rbd[i], tau[i], prm, P[i])
+        ref, F, _ = plant_numpy(oracle, rbd[i], tau[i], prm, variation=P[i])
         assert np.abs(nxt[i] - ref).max() < 1e-9 * max(1.0, np.abs(ref).max()), i
         assert np.abs(cf[i] - F).max() < 1e-7 * max(1.0, np.abs(F).max()), i
 
@@ -243,7 +242,7 @@ def test_varied_episode_equals_the_stepwise_loop_bitwise(event_nodes):
     pushes = hb.make_push_schedules(B, 0.15, 0.05, [[30.0, -20.0, 0.0]])
     ctx.set_plant_variations(V); ctx.set_pushes(pushes)
     d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
-    r = stepwise_varied(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, V, pushes=pushes)
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, pushes=pushes, variations=V)
     assert_episode_equal(d, r)
     ctx.set_plant_variations(None)
     u = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
@@ -263,7 +262,7 @@ def test_varied_estimated_episode_equals_the_stepwise_loop_bitwise():
     pushes = hb.make_push_schedules(B, 0.1, 0.04, [[0.0, 40.0, 0.0]])
     ctx.set_plant_variations(V); ctx.set_pushes(pushes)
     d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40))
-    r = stepwise_varied(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, V, ep, hb.estimation_states(B, 40), pushes=pushes)
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40), pushes=pushes, variations=V)
     assert_episode_equal(d, r)
     ctx.close()
 
@@ -276,21 +275,8 @@ def test_default_variations_change_nothing(estimated):
     vels = cmd_vels(B)
     prm = params(5)
     ep = est_params(seed=77) if estimated else None
-
-    def run():
-        c0 = ctx.launch_count
-        out = device(ctx, rbd0, GAITS, vels, n_ticks, prm, 5, ep)
-        return out, ctx.launch_count - c0
-
-    ref, launches = run()
-    for setting in (hb.make_plant_variations(B), hb.make_plant_variations(3), "clear"):
-        if setting == "clear":
-            ctx.set_plant_variations(_variations()); ctx.set_plant_variations(None)
-        else:
-            ctx.set_plant_variations(setting)
-        out, n = run()
-        assert n == launches
-        assert_episode_equal(ref, out)
+    assert_null_settings(ctx, "plant_variations", lambda: device(ctx, rbd0, GAITS, vels, n_ticks, prm, 5, ep),
+                         (hb.make_plant_variations(B), hb.make_plant_variations(3)), _variations())
     ctx.close()
 
 
@@ -298,45 +284,15 @@ def test_continuation_independence_permutation_and_instances_beyond_the_setting(
     ctx = context()
     B = 6
     rbd0 = start_states(ctx, B, seed=14)
-    vels = cmd_vels(B)
-    prm = params(10)
     V = _variations()
-    # two calls equal one
-    ctx.set_plant_variations(V)
-    assert_continues(ctx, rbd0, GAITS, vels, 200, 100, prm, 10)
-    # varying instance 0 only leaves every other instance as in the unvaried run
-    ctx.set_plant_variations(None)
-    u = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
-    ctx.set_plant_variations(_one_varied(B, 0, payload_mass=4.0, payload_com=[0.02, 0.0, 0.1], payload_inertia=4.0 * BOX, friction_scale=0.5))
-    p = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
-    assert not np.array_equal(p[0][0], u[0][0])
-    assert_episode_equal(p, u, rows_a=slice(1, None), rows_b=slice(1, None))
-    # instance i's outputs do not depend on the other instances' variations
+    one = _one_varied(B, 0, payload_mass=4.0, payload_com=[0.02, 0.0, 0.1], payload_inertia=4.0 * BOX, friction_scale=0.5)
     W = _variations()
     for i in range(B):
         if i != 2:
             W[i] = hb.make_plant_variations(1, 1.0 + i, [0.0, 0.01 * i, 0.1], (1.0 + i) * BOX, stiffness_scale=0.8)[0]
-    ctx.set_plant_variations(V)
-    full = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
-    ctx.set_plant_variations(W)
-    other = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
-    assert_episode_equal(full, other, rows_a=[2], rows_b=[2])
-    # a permuted batch with permuted variations gives the permuted result
-    perm = [4, 0, 5, 2, 1, 3]
-    ctx.set_plant_variations((hb.HbPlantVariation * B)(*[V[i] for i in perm]))
-    q = outputs(device(ctx, rbd0[perm], [GAITS[i] for i in perm], vels[perm], 200, prm, 10))
-    assert_episode_equal(full, q, rows_a=perm)
-    # variations for the first 3 instances only: the others run the nominal plant, the first 3 as with the full setting
-    ctx.set_plant_variations((hb.HbPlantVariation * 3)(*[V[i] for i in range(3)]))
-    part = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
+    part = (hb.HbPlantVariation * 3)(*[V[i] for i in range(3)])
     padded = (hb.HbPlantVariation * B)(*[V[i] if i < 3 else hb.default_plant_variation() for i in range(B)])
-    ctx.set_plant_variations(padded)
-    full6 = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
-    assert_episode_equal(part, u, rows_a=slice(3, None), rows_b=slice(3, None))
-    assert_episode_equal(part, full6)
-    # B = 0 clears the setting
-    assert ctx._lib.hb_rollout_set_plant_variations(ctx._h, 0, None) == 0
-    assert_episode_equal(outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10)), u)
+    assert_setting_episodes(ctx, "plant_variations", rbd0, params(10), V, one, W, 2, part, padded)
     ctx.close()
 
 
@@ -363,8 +319,6 @@ def test_argument_checks_return_before_any_launch_and_keep_the_setting():
     vels = cmd_vels(B)
     prm = params(10)
     V = _variations()
-    ctx.set_plant_variations(V)
-    want = outputs(device(ctx, rbd0, GAITS, vels, 60, prm, 10))
     assert C.sizeof(hb.HbPlantVariation) == 208
     nan, inf = float("nan"), float("inf")
 
@@ -383,31 +337,21 @@ def test_argument_checks_return_before_any_launch_and_keep_the_setting():
              ("friction_scale", None, -0.1), ("friction_scale", None, nan), ("stiffness_scale", None, 0.0), ("stiffness_scale", None, -1.0),
              ("stiffness_scale", None, inf), ("damping_scale", None, -0.1), ("damping_scale", None, nan), ("motor_strength", 3, -0.2),
              ("motor_strength", 9, nan), ("motor_strength", 0, inf)]
-    c0 = ctx.launch_count
-    for field, index, value in cases:
-        assert lib.hb_rollout_set_plant_variations(ctx._h, B, bad(field, index, value)) == -1, (field, index, value)
+    rejected = [bad(field, index, value) for field, index, value in cases]
     # a negative 2 x 2 principal minor, and a negative determinant with every 2 x 2 minor >= 0
     for M in ([[0.01, 0.02, 0.0], [0.02, 0.01, 0.0], [0.0, 0.0, 0.01]], [[1.0, 1.0, 0.0], [1.0, 1.0, 1.0], [0.0, 1.0, 1.0]]):
         W = (hb.HbPlantVariation * B)(*V)
         for k in range(9):
             W[1].payload_inertia[k] = np.ravel(M)[k]
-        assert lib.hb_rollout_set_plant_variations(ctx._h, B, W) == -1
+        rejected.append(W)
     # a zero mass with a CoM or an inertia
     for field, index in (("payload_com", 0), ("payload_inertia", 0)):
         W = (hb.HbPlantVariation * B)(*V)
         W[0].payload_mass = 0.0
         getattr(W[0], field)[index] = 0.01
-        assert lib.hb_rollout_set_plant_variations(ctx._h, B, W) == -1, field
-    assert lib.hb_rollout_set_plant_variations(None, 1, V) == -1
-    assert lib.hb_rollout_set_plant_variations(ctx._h, -1, V) == -1
-    assert lib.hb_rollout_set_plant_variations(ctx._h, 1, None) == -1
+        rejected.append(W)
     big = (hb.HbPlantVariation * (B + 1))(*([V[0]] * (B + 1)))
-    assert lib.hb_rollout_set_plant_variations(ctx._h, B + 1, big) == -4
-    with pytest.raises(hb.HunterB200Error):
-        ctx.set_plant_variations(bad("payload_mass", None, nan))
-    assert ctx.launch_count == c0
-    # the previous setting is still in force
-    assert_episode_equal(outputs(device(ctx, rbd0, GAITS, vels, 60, prm, 10)), want)
+    assert_rejected_settings(ctx, "plant_variations", lambda: device(ctx, rbd0, GAITS, vels, 60, prm, 10), V, rejected, big)
     # the host plant step checks its variations as the setting does
     sp = hb.default_sim_params()
     r = np.zeros((B, 32)); t = np.zeros((B, 10))

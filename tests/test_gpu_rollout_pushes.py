@@ -9,8 +9,8 @@ import pytest
 
 import hunter_bipedal_control_b200 as hb
 from hunter_bipedal_control_b200 import scenarios as sc
-from episode_ref import (GAITS, assert_continues, assert_episode_equal, cmd_vels, context, device, est_params, outputs, params, plant_numpy,
-                         start_states, stepwise)
+from episode_ref import (GAITS, assert_continues, assert_episode_equal, assert_null_settings, assert_rejected_settings, assert_setting_episodes,
+                         cmd_vels, context, device, est_params, outputs, params, plant_numpy, start_states, stepwise)
 
 pytestmark = pytest.mark.gpu
 
@@ -58,7 +58,7 @@ def test_plant_step_with_wrench_matches_numpy_restatement(gpu_ctx, oracle):
     base = gpu_ctx.sim_step(rbd, tau, prm)
     touched = 0
     for i in range(B):
-        ref, F = plant_numpy(oracle, rbd[i], tau[i], prm, W[i])
+        ref, F, _ = plant_numpy(oracle, rbd[i], tau[i], prm, W[i])
         assert np.abs(nxt[i] - ref).max() < 1e-9 * max(1.0, np.abs(ref).max()), i
         assert np.abs(cf[i] - F).max() < 1e-7 * max(1.0, np.abs(F).max())
         assert np.array_equal(fl[i] != 0, F[2::3] > 0)
@@ -153,36 +153,16 @@ def test_state_before_the_push_is_unchanged_and_the_state_after_it_moves():
     ctx.close()
 
 
-def _null_schedule_checks(ctx, run, B, n_ticks, horizon_t):
-    """Every null setting reproduces the unset episode bit for bit with the same launches; a rejected set keeps the previous setting."""
-    def counted():
-        c0 = ctx.launch_count
-        out = run()
-        return out, ctx.launch_count - c0
-
-    ctx.set_pushes(None)
-    ref, launches = counted()
+def _null_schedule_checks(ctx, run, B, horizon_t):
+    """Null schedules (none, or pushes after the episode) change nothing; a rejected set keeps the previous, pushing setting."""
     nothing = hb.make_push_schedules(B, np.zeros((B, 0)), np.zeros((B, 0)), np.zeros((B, 0, 3)))
     later = hb.make_push_schedules(B, [horizon_t, horizon_t + 0.5], [0.1, 1.0], [[500.0, 0, 0], [0, 500.0, 0]], [[0, 0, 50.0], [0, 0, 0]])
-    for setting in (nothing, later, "clear"):
-        if setting == "clear":
-            ctx.set_pushes(_schedules()); ctx.set_pushes(None)
-        else:
-            ctx.set_pushes(setting)
-        out, n = counted()
-        assert n == launches, (setting, n, launches)
-        yield ref, out
-    pushed = _one_push(B, 1, 0.02, 0.06, (0.0, -70.0, 0.0), (0.0, 0.0, 4.0))
-    ctx.set_pushes(pushed)
-    want, n = counted()
-    assert n == launches
+    ref, launches = assert_null_settings(ctx, "pushes", run, (nothing, later), _schedules())
     bad = _one_push(B, 1, 0.02, 0.06, (0.0, -70.0, 0.0))
     bad[0].force[0][0] = float("nan")
-    with pytest.raises(hb.HunterB200Error):
-        ctx.set_pushes(bad)
-    assert ctx._lib.hb_rollout_set_pushes(ctx._h, ctx.max_batch + 1, _schedules()) == -4
-    got, _ = counted()
-    yield want, got
+    pushed = _one_push(B, 1, 0.02, 0.06, (0.0, -70.0, 0.0), (0.0, 0.0, 4.0))
+    want, n = assert_rejected_settings(ctx, "pushes", run, pushed, [bad], (hb.HbPushSchedule * (ctx.max_batch + 1))())
+    assert n == launches
     assert not np.array_equal(outputs(want)[0], outputs(ref)[0])
 
 
@@ -192,8 +172,7 @@ def test_null_schedules_change_nothing():
     rbd0 = start_states(ctx, B, seed=13)
     vels = cmd_vels(B)
     prm = params(5)
-    for a, b in _null_schedule_checks(ctx, lambda: device(ctx, rbd0, GAITS, vels, n_ticks, prm, 5), B, n_ticks, n_ticks * prm.period):
-        assert_episode_equal(a, b)
+    _null_schedule_checks(ctx, lambda: device(ctx, rbd0, GAITS, vels, n_ticks, prm, 5), B, n_ticks * prm.period)
     ctx.close()
 
 
@@ -201,38 +180,17 @@ def test_continuation_independence_permutation_and_unscheduled_instances():
     ctx = context()
     B = 6
     rbd0 = start_states(ctx, B, seed=14)
-    vels = cmd_vels(B)
-    prm = params(10)
-    # two calls split inside a push window (ticks 75..124, split at tick 100) equal one call
-    ctx.set_pushes(hb.make_push_schedules(B, 0.15, 0.1, np.linspace(-60, 60, B)[:, None, None] * np.array([1.0, 0.5, 0.0]), [0.0, 0.0, 3.0]))
-    assert_continues(ctx, rbd0, GAITS, vels, 200, 100, prm, 10)
-    # pushing instance 0 only leaves every other instance as in the unpushed run
-    ctx.set_pushes(None)
-    u = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
-    ctx.set_pushes(_one_push(B, 0, 0.1, 0.1, (70.0, -30.0, 0.0), (0.0, 2.0, 0.0)))
-    p = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
-    assert not np.array_equal(p[0][0], u[0][0])
-    assert_episode_equal(p, u, rows_a=slice(1, None), rows_b=slice(1, None))
-    # a permuted batch with permuted schedules gives the permuted result
     S = _schedules()
-    ctx.set_pushes(S)
-    full = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
-    perm = [4, 0, 5, 2, 1, 3]
-    Sp = (hb.HbPushSchedule * B)(*[S[i] for i in perm])
-    ctx.set_pushes(Sp)
-    q = outputs(device(ctx, rbd0[perm], [GAITS[i] for i in perm], vels[perm], 200, prm, 10))
-    assert_episode_equal(full, q, rows_a=perm)
-    # schedules for the first 3 instances only: the others run unpushed, the first 3 as with the full setting
-    ctx.set_pushes(hb.make_push_schedules(3, 0.05, 0.2, [40.0, 40.0, 0.0]))
-    part = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
+    other = hb.make_push_schedules(B, 0.08, 0.1, [[0.0, 50.0, 0.0]])
+    other[2] = S[2]
     padded = hb.make_push_schedules(B, 0.05, 0.2, [40.0, 40.0, 0.0])
     for i in range(3, B):
         padded[i].n_push = 0
-    ctx.set_pushes(padded)
-    full6 = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
-    assert_episode_equal(part, u, rows_a=slice(3, None), rows_b=slice(3, None))
-    assert_episode_equal(part, full6)
-    assert not np.array_equal(part[0][:3], u[0][:3])
+    # continuation split inside a push window (ticks 75..124, split at tick 100); first 3 instances pushed as in `padded`
+    assert_setting_episodes(ctx, "pushes", rbd0, params(10), S, _one_push(B, 0, 0.1, 0.1, (70.0, -30.0, 0.0), (0.0, 2.0, 0.0)), other, 2,
+                            hb.make_push_schedules(3, 0.05, 0.2, [40.0, 40.0, 0.0]), padded,
+                            cont=hb.make_push_schedules(B, 0.15, 0.1, np.linspace(-60, 60, B)[:, None, None] * np.array([1.0, 0.5, 0.0]),
+                                                        [0.0, 0.0, 3.0]))
     ctx.close()
 
 
@@ -263,8 +221,7 @@ def test_estimated_episodes_null_schedules_independence_and_continuation():
     def run(rbd=rbd0, gaits=GAITS, v=vels, est=None):
         return device(ctx, rbd, gaits, v, n_ticks, prm, 5, ep, est)
 
-    for a, b in _null_schedule_checks(ctx, run, B, n_ticks, n_ticks * prm.period):
-        assert_episode_equal(a, b)
+    _null_schedule_checks(ctx, run, B, n_ticks * prm.period)
     # only instance 2 pushed: its estimation stats change, every other instance is the unpushed run
     ctx.set_pushes(None)
     u = outputs(run())

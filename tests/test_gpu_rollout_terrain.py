@@ -11,9 +11,8 @@ import pytest
 
 import hunter_bipedal_control_b200 as hb
 from hunter_bipedal_control_b200 import scenarios as sc
-from episode_ref import (GAITS, GROUND, assert_continues, assert_episode_equal, cmd_vels, context, device, est_params, launch_coefficients,
-                         outputs, params, start_states)
-from terrain_ref import plant_numpy_terrain, stepwise_terrain, terrain_height
+from episode_ref import (GAITS, GROUND, assert_episode_equal, assert_null_settings, assert_rejected_settings, assert_setting_episodes, cmd_vels,
+                         context, device, est_params, launch_coefficients, outputs, params, plant_numpy, start_states, stepwise, terrain_height)
 
 pytestmark = pytest.mark.gpu
 
@@ -118,7 +117,7 @@ def test_terrain_plant_step_matches_numpy_restatement(gpu_ctx, oracle):
     for var, wr in ((None, None), (V, W)):
         nxt, cf, fl = gpu_ctx.sim_step(rbd, tau, prm, wrench=wr, variation=var, terrain=T)
         for i in range(B):
-            ref, F, flags = plant_numpy_terrain(oracle, rbd[i], tau[i], prm, T[i], None if var is None else var[i], None if wr is None else wr[i])
+            ref, F, flags = plant_numpy(oracle, rbd[i], tau[i], prm, None if wr is None else wr[i], None if var is None else var[i], T[i])
             assert np.abs(nxt[i] - ref).max() < 1e-9 * max(1.0, np.abs(ref).max()), (i, np.abs(nxt[i] - ref).max())
             assert np.abs(cf[i] - F).max() < 1e-7 * max(1.0, np.abs(F).max()), (i, cf[i], F)
             assert np.array_equal(fl[i] != 0, flags), (i, fl[i], flags)
@@ -311,7 +310,7 @@ def test_terrain_episode_equals_the_stepwise_loop_bitwise(event_nodes):
     pushes = hb.make_push_schedules(B, 0.15, 0.05, [[25.0, -15.0, 0.0]])
     ctx.set_terrains(T); ctx.set_plant_variations(V); ctx.set_pushes(pushes)
     d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
-    r = stepwise_terrain(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, T, V, pushes=pushes)
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, pushes=pushes, variations=V, terrains=T)
     assert_episode_equal(d, r)
     ctx.set_terrains(None)
     u = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
@@ -332,7 +331,7 @@ def test_terrain_estimated_episode_equals_the_stepwise_loop_bitwise():
     pushes = hb.make_push_schedules(B, 0.1, 0.04, [[0.0, 30.0, 0.0]])
     ctx.set_terrains(T); ctx.set_plant_variations(V); ctx.set_pushes(pushes)
     d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40))
-    r = stepwise_terrain(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, T, V, ep, hb.estimation_states(B, 40), pushes=pushes)
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40), pushes=pushes, variations=V, terrains=T)
     assert_episode_equal(d, r)
     ctx.close()
 
@@ -369,22 +368,9 @@ def test_flat_terrains_at_the_ground_height_change_nothing(estimated):
     vels = cmd_vels(B)
     prm = params(5)
     ep = est_params(seed=78) if estimated else None
-
-    def run():
-        c0 = ctx.launch_count
-        out = device(ctx, rbd0, GAITS, vels, n_ticks, prm, 5, ep)
-        return out, ctx.launch_count - c0
-
-    ref, launches = run()
     flat = _profile_terrains(rbd0, ["flat"] * B)
-    for setting in (flat, (hb.HbTerrain * 3)(*flat[:3]), "clear"):
-        if setting == "clear":
-            ctx.set_terrains(_profile_terrains(rbd0, PROFILES, np.random.default_rng(0))); ctx.set_terrains(None)
-        else:
-            ctx.set_terrains(setting)
-        out, n = run()
-        assert n == launches
-        assert_episode_equal(ref, out)
+    assert_null_settings(ctx, "terrains", lambda: device(ctx, rbd0, GAITS, vels, n_ticks, prm, 5, ep), (flat, (hb.HbTerrain * 3)(*flat[:3])),
+                         _profile_terrains(rbd0, PROFILES, np.random.default_rng(0)))
     ctx.close()
 
 
@@ -392,45 +378,15 @@ def test_continuation_independence_permutation_and_instances_beyond_the_setting(
     ctx = context()
     B = 6
     rbd0 = start_states(ctx, B, seed=55)
-    vels = cmd_vels(B)
-    prm = params(10)
     T = _profile_terrains(rbd0, PROFILES + ["ramp"], np.random.default_rng(55))
-    # two calls equal one
-    ctx.set_terrains(T)
-    assert_continues(ctx, rbd0, GAITS, vels, 200, 100, prm, 10)
-    # a terrain under instance 0 only leaves every other instance as in the unset run
-    ctx.set_terrains(None)
-    u = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
     only0 = _profile_terrains(rbd0, ["flat"] * B)
     only0[0] = _profile_terrains(rbd0, ["ramp"])[0]
-    ctx.set_terrains(only0)
-    p = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
-    assert not np.array_equal(p[0][0], u[0][0])
-    assert_episode_equal(p, u, rows_a=slice(1, None), rows_b=slice(1, None))
-    # instance i's outputs do not depend on the other instances' terrains
-    ctx.set_terrains(T)
-    full = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
     other = _profile_terrains(rbd0, ["rough", "step_up", "ramp", "ramp", "rough", "step_down"], np.random.default_rng(9))
     other[3] = T[3]
-    ctx.set_terrains(other)
-    assert_episode_equal(full, outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10)), rows_a=[3], rows_b=[3])
-    # a permuted batch with permuted terrains gives the permuted result
-    perm = [4, 0, 5, 2, 1, 3]
-    ctx.set_terrains((hb.HbTerrain * B)(*[T[i] for i in perm]))
-    q = outputs(device(ctx, rbd0[perm], [GAITS[i] for i in perm], vels[perm], 200, prm, 10))
-    assert_episode_equal(full, q, rows_a=perm)
-    # terrains for the first 3 instances only: the others stand on flat ground, the first 3 as with the full setting
-    ctx.set_terrains((hb.HbTerrain * 3)(*[T[i] for i in range(3)]))
-    part = outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10))
     padded = _profile_terrains(rbd0, ["flat"] * B)
     for i in range(3):
         padded[i] = T[i]
-    ctx.set_terrains(padded)
-    assert_episode_equal(part, outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10)))
-    assert_episode_equal(part, u, rows_a=slice(3, None), rows_b=slice(3, None))
-    # B = 0 clears the setting
-    assert ctx._lib.hb_rollout_set_terrains(ctx._h, 0, None) == 0
-    assert_episode_equal(outputs(device(ctx, rbd0, GAITS, vels, 200, prm, 10)), u)
+    assert_setting_episodes(ctx, "terrains", rbd0, params(10), T, only0, other, 3, (hb.HbTerrain * 3)(*[T[i] for i in range(3)]), padded)
     ctx.close()
 
 
@@ -457,8 +413,6 @@ def test_argument_checks_return_before_any_launch_and_keep_the_setting():
     vels = cmd_vels(B)
     prm = params(10)
     T = _profile_terrains(rbd0, PROFILES + ["ramp"], np.random.default_rng(57))
-    ctx.set_terrains(T)
-    want = outputs(device(ctx, rbd0, GAITS, vels, 60, prm, 10))
     assert C.sizeof(hb.HbTerrain) == 32800
     nan, inf = float("nan"), float("inf")
 
@@ -476,19 +430,8 @@ def test_argument_checks_return_before_any_launch_and_keep_the_setting():
     cases = [("nx", 1), ("nx", 0), ("nx", -3), ("nx", 65), ("ny", 1), ("ny", 65), ("origin", nan, 0), ("origin", inf, 1),
              ("origin", -inf, 0), ("spacing", 0.0), ("spacing", -0.025), ("spacing", nan), ("spacing", inf), ("height", nan, (0, 0)),
              ("height", inf, (63, 63)), ("height", -inf, (10, 40))]
-    c0 = ctx.launch_count
-    for case in cases:
-        assert lib.hb_rollout_set_terrains(ctx._h, B, bad(*case)) == -1, case
-    assert lib.hb_rollout_set_terrains(None, 1, T) == -1
-    assert lib.hb_rollout_set_terrains(ctx._h, -1, T) == -1
-    assert lib.hb_rollout_set_terrains(ctx._h, 1, None) == -1
     big = (hb.HbTerrain * (B + 1))(*([T[0]] * (B + 1)))
-    assert lib.hb_rollout_set_terrains(ctx._h, B + 1, big) == -4
-    with pytest.raises(hb.HunterB200Error):
-        ctx.set_terrains(bad("spacing", nan))
-    assert ctx.launch_count == c0
-    # the previous setting is still in force
-    assert_episode_equal(outputs(device(ctx, rbd0, GAITS, vels, 60, prm, 10)), want)
+    assert_rejected_settings(ctx, "terrains", lambda: device(ctx, rbd0, GAITS, vels, 60, prm, 10), T, [bad(*case) for case in cases], big)
     # samples beyond nx / ny are not read, so they are not checked either
     small = hb.make_terrains(B, np.full((3, 4), GROUND), 0.3, rbd0[:, 3:5] - 0.45)
     small[1].height[3][0] = nan; small[1].height[0][4] = inf

@@ -3,7 +3,7 @@ import numpy as np
 import pytest
 
 import hunter_bipedal_control_b200 as hb
-from terrain_ref import terrain_height
+from episode_ref import terrain_height
 
 
 def _view(T):

@@ -16,21 +16,18 @@ alternately, with device events around the episode call, and reports the launch 
 name and power limit and the clocks sampled during the timed episodes.
 
 --estimator runs everything through hb_rollout_estimated_batch_dev (controllers on the Kalman filter's estimate from simulated sensors,
-noise = SCALE x bench_rollout's NOISE_SIGMAS).
+noise = SCALE x episode_harness's NOISE_SIGMAS).
 """
-import argparse
-import ctypes as C
 import json
 import os
 import sys
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from bench_rollout import GROUND, MIN_HEIGHT, NOISE_SIGMAS, gpu_identity  # noqa: E402
-from bench import DT, HORIZON_N, SEED, ClockSampler  # noqa: E402  (bench_rollout put the repository root on the path)
+from episode_harness import MIN_HEIGHT, NOISE_SIGMAS, Episodes, cells, gpu_identity, sweep_args  # noqa: E402
+from bench import DT, HORIZON_N, SEED  # noqa: E402  (episode_harness put the repository root on the path)
 
 TICKS, PUSH_T, PUSH_DURATION = 750, 0.5, 0.1
 DIRECTIONS = {"+x": (1.0, 0.0, 0.0), "-x": (-1.0, 0.0, 0.0), "+y": (0.0, 1.0, 0.0), "-y": (0.0, -1.0, 0.0)}
@@ -38,70 +35,18 @@ STEP_N, BLOCK, MAX_FORCE, SURVIVE = 10.0, 16, 1000.0, 0.9
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--repeats", type=int, default=4, help="episodes per grid block (the robot -> cell assignment shifts between them)")
-    ap.add_argument("--timed", type=int, default=3, help="timed pushed / unpushed episode pairs")
-    ap.add_argument("--batch", type=int, default=1024, help="robots per episode (a multiple of 64)")
-    ap.add_argument("--device", type=int, default=0)
-    ap.add_argument("--estimator", action="store_true", help="run the episodes through the state estimator")
-    ap.add_argument("--sensor-noise", type=float, default=0.0, metavar="SCALE", help="with --estimator: sensor noise, SCALE x NOISE_SIGMAS")
-    args = ap.parse_args()
-    ncell = len(DIRECTIONS) * BLOCK
-    if args.batch < ncell or args.batch % ncell or args.repeats < 1 or args.sensor_noise < 0 or (args.sensor_noise and not args.estimator):
-        raise SystemExit("push_sweep.py: --batch a multiple of %d, --repeats >= 1, --sensor-noise takes a scale >= 0 and needs --estimator" % ncell)
-    import torch
-    import hunter_bipedal_control_b200 as hb
-    from hunter_bipedal_control_b200 import scenarios as S
-    if not torch.cuda.is_available():
-        raise SystemExit("push_sweep.py: no CUDA device visible; the product path has no CPU fallback")
-    dev = torch.device("cuda", args.device)
-    torch.cuda.set_device(dev)
-    B = args.batch
-    ctx = hb.Context(horizon_N=HORIZON_N, dt=DT, max_batch=B, device=args.device)
-    x0 = S.random_initial_states(B, SEED)
-    rbd0 = S.consistent_rbd(x0)
-    rbd0[:, 5] -= ctx.contact_positions(x0).reshape(B, 4, 3)[:, :, 2].min(axis=1) - (GROUND - 0.001)
-    prm = hb.default_rollout_params()
-    prm.sim.ground_height = GROUND
-    prm.min_base_height = MIN_HEIGHT
-    cmds = hb.make_rollout_commands("trot", np.full(B, 0.1), [0.0], [[0.3, 0.0, 0.0, 0.0]])
-    ep = hb.default_estimation_params()
-    ep.noise.seed = SEED
-    for k, v in NOISE_SIGMAS.items():
-        setattr(ep.noise, k, args.sensor_noise * v)
-    stream = torch.cuda.ExternalStream(ctx.stream_handle, device=dev)
-    lib = hb.load_library()
-    P = lambda t: C.c_void_p(t.data_ptr())
+    args = sweep_args("push_sweep.py", "timed pushed / zero-force / unpushed episode triples", len(DIRECTIONS) * BLOCK)
+    h = Episodes("push_sweep.py", args, TICKS)
+    hb, ctx, prm, B = h.hb, h.ctx, h.prm, h.B
     push_tick = int(round(PUSH_T / prm.period))
 
-    def episode():
-        d_rbd = torch.from_numpy(rbd0).to(dev)
-        d_act = torch.zeros(B * C.sizeof(hb.HbActuationState), dtype=torch.uint8, device=dev)
-        d_estop = torch.zeros(B, dtype=torch.uint8, device=dev)
-        d_st = torch.from_numpy(hb.rollout_stats(B).view(np.uint8).copy()).to(dev)
-        if args.estimator:
-            d_est = torch.from_numpy(np.frombuffer(bytes(hb.estimation_states(B)), dtype=np.uint8).copy()).to(dev)
-        torch.cuda.synchronize(dev)
-        e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
-        l0 = ctx.launch_count
-        e0.record(stream)
-        if args.estimator:
-            rc = lib.hb_rollout_estimated_batch_dev(ctx._h, B, C.c_int64(0), TICKS, C.byref(prm), C.byref(ep), cmds, P(d_rbd), P(d_act), P(d_estop), P(d_st),
-                                                    P(d_est), None, None, None)
-        else:
-            rc = lib.hb_rollout_batch_dev(ctx._h, B, C.c_int64(0), TICKS, C.byref(prm), cmds, P(d_rbd), P(d_act), P(d_estop), P(d_st), None)
-        e1.record(stream)
-        assert rc == 0, rc
-        ctx.sync()
-        return e0.elapsed_time(e1), ctx.launch_count - l0, d_st.cpu().numpy().view(hb.ROLLOUT_STATS_DTYPE)
-
-    def cells(block, shift):
+    def push_cells(block, shift):
         """(direction index, magnitude) of every robot for grid block `block`, assignment shifted by `shift`."""
-        c = (np.arange(B) + shift) % ncell
-        return c // BLOCK, (block * BLOCK + c % BLOCK) * STEP_N
+        c, d = cells(B, BLOCK, len(DIRECTIONS), shift)
+        return d, (block * BLOCK + c) * STEP_N
 
     def schedules(block, shift):
-        d, mag = cells(block, shift)
+        d, mag = push_cells(block, shift)
         dirs = np.array(list(DIRECTIONS.values()))
         return hb.make_push_schedules(B, PUSH_T, PUSH_DURATION, (dirs[d] * mag[:, None])[:, None, :])
 
@@ -110,13 +55,13 @@ def main():
     survived = {n: {} for n in names}
     reasons = {name: 0 for name in hb.ROLLOUT_FAIL}
     ctx.set_pushes(schedules(0, 0))
-    episode()                                   # warm-up episode
+    h.episode()                                 # warm-up episode
     block = 0
     while True:
         for r in range(args.repeats):
             ctx.set_pushes(schedules(block, r))
-            _, _, st = episode()
-            d, mag = cells(block, r)
+            st = h.episode().stats
+            d, mag = push_cells(block, r)
             was_up = (st["fail_tick"] < 0) | (st["fail_tick"] > push_tick)
             ok = st["fail_tick"] < 0
             for i in np.nonzero(was_up)[0]:
@@ -139,31 +84,14 @@ def main():
     # pushed, zero-force (schedules set, the trajectories of the unpushed batch: the cost of the wrench path alone) and unpushed episodes
     # alternate
     zero = hb.make_push_schedules(B, PUSH_T, PUSH_DURATION, [0.0, 0.0, 0.0])
-    sampler = ClockSampler(args.device); sampler.start()
-    pushed, zeroed, unpushed = [], [], []
-    for _ in range(max(1, args.timed)):
-        ctx.set_pushes(schedules(0, 0))
-        pushed.append(episode())
-        ctx.set_pushes(zero)
-        zeroed.append(episode())
-        ctx.set_pushes(None)
-        unpushed.append(episode())
-    clocks = sampler.stop()
-    pm, zm, um = [r[0] for r in pushed], [r[0] for r in zeroed], [r[0] for r in unpushed]
-    lp, lu = pushed[-1][1], unpushed[-1][1]
+    runs, clocks, timing = h.alternate(ctx.set_pushes, [("pushed", schedules(0, 0)), ("zero_force", zero), ("unpushed", None)], args.timed)
+    timing.update(launches_pushed=int(runs["pushed"][-1].launches), launches_unpushed=int(runs["unpushed"][-1].launches))
     known = [v for v in largest.values() if v is not None]
     line = {"metric": "push recovery: the largest %.1f s world-frame push at the base, over the four horizontal directions, that >= 90 %% of the "
                       "trotting robots survive" % PUSH_DURATION, "value": min(known) if len(known) == len(names) else None, "unit": "N",
             "n_gpus": 1, "dtype": "f64", "data": "synthetic", "estimator": bool(args.estimator),
             "largest_force_90pct": largest, "survival": survival, "robots_up_at_push": up, "fail_reasons_after_push": reasons,
-            "upright_fraction_unpushed": float((unpushed[-1][2]["fail_tick"] < 0).mean()),
-            "timing": {"ms_per_episode_pushed": float(np.median(pm)), "ms_per_episode_pushed_range": [min(pm), max(pm)],
-                       "ms_per_episode_unpushed": float(np.median(um)), "ms_per_episode_unpushed_range": [min(um), max(um)],
-                       "pushed_minus_unpushed_ms": float(np.median(pm) - np.median(um)),
-                       "ms_per_episode_zero_force": float(np.median(zm)), "ms_per_episode_zero_force_range": [min(zm), max(zm)],
-                       "zero_force_minus_unpushed_ms": float(np.median(zm) - np.median(um)),
-                       "zero_force_same_outcome_as_unpushed": all(np.array_equal(z[2], u[2]) for z, u in zip(zeroed, unpushed)), "episodes": len(pm),
-                       "launches_pushed": int(lp), "launches_unpushed": int(lu), "launches_equal": lp == lu == zeroed[-1][1]},
+            "upright_fraction_unpushed": float((runs["unpushed"][-1].stats["fail_tick"] < 0).mean()), "timing": timing,
             "config": {"workload": "%d robots, %.1f s simulated (%d ticks of %.0f ms), trot at 0.3 m/s from t = 0.1 s, initial poses of "
                                    "scenarios.random_initial_states(seed %d), N=%d dt=%.0f ms; one push per robot at t = %.1f s for %.1f s, %d "
                                    "episodes per grid block of %d magnitudes x 4 directions" % (B, TICKS * prm.period, TICKS, 1e3 * prm.period, SEED,

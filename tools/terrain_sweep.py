@@ -25,21 +25,18 @@ alternately, with device events around the episode call, and reports the launch 
 flat and unset give the same outcome, and the card's name and power limit and the clocks sampled during the timed episodes.
 
 --estimator runs everything through hb_rollout_estimated_batch_dev (controllers on the Kalman filter's estimate from simulated sensors,
-noise = SCALE x bench_rollout's NOISE_SIGMAS).
+noise = SCALE x episode_harness's NOISE_SIGMAS).
 """
-import argparse
-import ctypes as C
 import json
 import os
 import sys
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from bench_rollout import GROUND, MIN_HEIGHT, NOISE_SIGMAS, gpu_identity  # noqa: E402
-from bench import DT, HORIZON_N, SEED, ClockSampler  # noqa: E402  (bench_rollout put the repository root on the path)
+from episode_harness import GROUND, MIN_HEIGHT, NOISE_SIGMAS, Episodes, cells, gpu_identity, sweep_args  # noqa: E402
+from bench import DT, HORIZON_N, SEED  # noqa: E402  (episode_harness put the repository root on the path)
 
 TICKS = 750
 KINDS = ["step_up", "step_down", "incline", "decline"]
@@ -72,72 +69,14 @@ def terrain_heights(rbd0, kind, magnitude, step_ahead, ramp_ahead):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--repeats", type=int, default=4, help="episodes of the grid (the robot -> cell assignment shifts between them)")
-    ap.add_argument("--timed", type=int, default=3, help="timed terrain / flat / unset episode triples")
-    ap.add_argument("--batch", type=int, default=1024, help="robots per episode (a multiple of 64)")
-    ap.add_argument("--device", type=int, default=0)
-    ap.add_argument("--estimator", action="store_true", help="run the episodes through the state estimator")
-    ap.add_argument("--sensor-noise", type=float, default=0.0, metavar="SCALE", help="with --estimator: sensor noise, SCALE x NOISE_SIGMAS")
-    args = ap.parse_args()
-    ncell = len(KINDS) * len(MAGNITUDES)
-    if args.batch < ncell or args.batch % ncell or args.repeats < 1 or args.sensor_noise < 0 or (args.sensor_noise and not args.estimator):
-        raise SystemExit("terrain_sweep.py: --batch a multiple of %d, --repeats >= 1, --sensor-noise takes a scale >= 0 and needs --estimator" % ncell)
-    import torch
-    import hunter_bipedal_control_b200 as hb
-    from hunter_bipedal_control_b200 import scenarios as S
-    if not torch.cuda.is_available():
-        raise SystemExit("terrain_sweep.py: no CUDA device visible; the product path has no CPU fallback")
-    dev = torch.device("cuda", args.device)
-    torch.cuda.set_device(dev)
-    B = args.batch
-    ctx = hb.Context(horizon_N=HORIZON_N, dt=DT, max_batch=B, device=args.device)
-    x0 = S.random_initial_states(B, SEED)
-    rbd0 = S.consistent_rbd(x0)
-    feet = ctx.contact_positions(x0).reshape(B, 4, 3)
-    rbd0[:, 5] -= feet[:, :, 2].min(axis=1) - (GROUND - 0.001)
-    step_ahead, ramp_ahead = feature_distances(rbd0, feet)
-    prm = hb.default_rollout_params()
-    prm.sim.ground_height = GROUND
-    prm.min_base_height = MIN_HEIGHT
-    cmds = hb.make_rollout_commands("trot", np.full(B, 0.1), [0.0], [[0.3, 0.0, 0.0, 0.0]])
-    ep = hb.default_estimation_params()
-    ep.noise.seed = SEED
-    for k, v in NOISE_SIGMAS.items():
-        setattr(ep.noise, k, args.sensor_noise * v)
-    stream = torch.cuda.ExternalStream(ctx.stream_handle, device=dev)
-    lib = hb.load_library()
-    P = lambda t: C.c_void_p(t.data_ptr())
+    args = sweep_args("terrain_sweep.py", "timed terrain / flat / unset episode triples", len(KINDS) * len(MAGNITUDES))
+    h = Episodes("terrain_sweep.py", args, TICKS)
+    hb, ctx, prm, B, rbd0 = h.hb, h.ctx, h.prm, h.B, h.rbd0
+    step_ahead, ramp_ahead = feature_distances(rbd0, h.feet)
     T_episode = TICKS * prm.period
 
-    def episode():
-        d_rbd = torch.from_numpy(rbd0).to(dev)
-        d_act = torch.zeros(B * C.sizeof(hb.HbActuationState), dtype=torch.uint8, device=dev)
-        d_estop = torch.zeros(B, dtype=torch.uint8, device=dev)
-        d_st = torch.from_numpy(hb.rollout_stats(B).view(np.uint8).copy()).to(dev)
-        if args.estimator:
-            d_est = torch.from_numpy(np.frombuffer(bytes(hb.estimation_states(B)), dtype=np.uint8).copy()).to(dev)
-        torch.cuda.synchronize(dev)
-        e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
-        l0 = ctx.launch_count
-        e0.record(stream)
-        if args.estimator:
-            rc = lib.hb_rollout_estimated_batch_dev(ctx._h, B, C.c_int64(0), TICKS, C.byref(prm), C.byref(ep), cmds, P(d_rbd), P(d_act), P(d_estop), P(d_st),
-                                                    P(d_est), None, None, None)
-        else:
-            rc = lib.hb_rollout_batch_dev(ctx._h, B, C.c_int64(0), TICKS, C.byref(prm), cmds, P(d_rbd), P(d_act), P(d_estop), P(d_st), None)
-        e1.record(stream)
-        assert rc == 0, rc
-        ctx.sync()
-        return e0.elapsed_time(e1), ctx.launch_count - l0, d_st.cpu().numpy().view(hb.ROLLOUT_STATS_DTYPE), d_rbd.cpu().numpy()
-
-    def cells(shift):
-        """(magnitude index, kind index) of every robot, assignment shifted by `shift`."""
-        c = (np.arange(B) + shift) % ncell
-        return c % len(MAGNITUDES), c // len(MAGNITUDES)
-
     def terrains(shift):
-        mi, ki = cells(shift)
+        mi, ki = cells(B, len(MAGNITUDES), len(KINDS), shift)
         origin, h = terrain_heights(rbd0, np.array(KINDS)[ki], np.array(MAGNITUDES)[mi], step_ahead, ramp_ahead)
         return hb.make_terrains(B, h, SPACING, origin)
 
@@ -146,11 +85,11 @@ def main():
     speed = np.zeros((len(KINDS), len(MAGNITUDES)))
     reasons = {name: 0 for name in hb.ROLLOUT_FAIL}
     ctx.set_terrains(terrains(0))
-    episode()                                   # warm-up episode
+    h.episode()                                 # warm-up episode
     for r in range(args.repeats):
         ctx.set_terrains(terrains(r))
-        _, _, st, rbd = episode()
-        mi, ki = cells(r)
+        _, _, st, rbd, _ = h.episode()
+        mi, ki = cells(B, len(MAGNITUDES), len(KINDS), r)
         ok = st["fail_tick"] < 0
         v = np.hypot(*(rbd[:, 3:5] - rbd0[:, 3:5]).T) / T_episode
         np.add.at(total, (ki, mi), 1)
@@ -171,30 +110,13 @@ def main():
     # terrain, flat-terrain and unset episodes alternate
     flat_origin, flat_h = terrain_heights(rbd0, np.full(B, "step_up"), np.zeros(B), step_ahead, ramp_ahead)
     flat = hb.make_terrains(B, flat_h, SPACING, flat_origin)
-    sampler = ClockSampler(args.device); sampler.start()
-    on_terrain, flats, unset = [], [], []
-    for _ in range(max(1, args.timed)):
-        ctx.set_terrains(terrains(0))
-        on_terrain.append(episode())
-        ctx.set_terrains(flat)
-        flats.append(episode())
-        ctx.set_terrains(None)
-        unset.append(episode())
-    clocks = sampler.stop()
-    tm, fm, um = [r[0] for r in on_terrain], [r[0] for r in flats], [r[0] for r in unset]
-    lt, lf, lu = on_terrain[-1][1], flats[-1][1], unset[-1][1]
+    runs, clocks, timing = h.alternate(ctx.set_terrains, [("terrain", terrains(0)), ("flat", flat), ("unset", None)], args.timed)
+    timing.update({"launches_" + n: int(runs[n][-1].launches) for n in runs})
     line = {"metric": "terrain: the highest step [cm] that >= 90 %% of the trotting robots cross blind within %.1f s; per kind (steps in cm, "
                       "slopes in degrees) under largest_magnitude_90pct" % T_episode, "value": largest["step_up"], "unit": "cm",
             "n_gpus": 1, "dtype": "f64", "data": "synthetic", "estimator": bool(args.estimator),
             "largest_magnitude_90pct": largest, "survival": survival, "mean_speed_of_survivors_m_per_s": mean_speed, "fail_reasons": reasons,
-            "upright_fraction_unset": float((unset[-1][2]["fail_tick"] < 0).mean()),
-            "timing": {"ms_per_episode_terrain": float(np.median(tm)), "ms_per_episode_terrain_range": [min(tm), max(tm)],
-                       "ms_per_episode_flat": float(np.median(fm)), "ms_per_episode_flat_range": [min(fm), max(fm)],
-                       "ms_per_episode_unset": float(np.median(um)), "ms_per_episode_unset_range": [min(um), max(um)],
-                       "terrain_minus_unset_ms": float(np.median(tm) - np.median(um)), "flat_minus_unset_ms": float(np.median(fm) - np.median(um)),
-                       "flat_same_outcome_as_unset": all(np.array_equal(f[2], u[2]) and np.array_equal(f[3], u[3]) for f, u in zip(flats, unset)),
-                       "episodes": len(tm), "launches_terrain": int(lt), "launches_flat": int(lf), "launches_unset": int(lu),
-                       "launches_equal": lt == lf == lu},
+            "upright_fraction_unset": float((runs["unset"][-1].stats["fail_tick"] < 0).mean()), "timing": timing,
             "config": {"workload": "%d robots, %.1f s simulated (%d ticks of %.0f ms), trot at 0.3 m/s from t = 0.1 s, initial poses of "
                                    "scenarios.random_initial_states(seed %d), N=%d dt=%.0f ms; %d kinds x %d magnitudes, %d episodes"
                                    % (B, T_episode, TICKS, 1e3 * prm.period, SEED, HORIZON_N, 1e3 * DT, len(KINDS), len(MAGNITUDES), args.repeats),
