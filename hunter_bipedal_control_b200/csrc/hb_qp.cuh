@@ -263,9 +263,11 @@ __device__ inline QpResult qp_solve_warp(int n, int m, const double* __restrict_
   }
   infeasible = __any_sync(HB_FULL_MASK, infeasible);
   QpResult res{1, 0};
-  if (infeasible || me > w.me_cap || mi > w.mi_cap || n > QP_MAX_N) {
+  // status 2: an all-zero row whose bounds exclude 0; status 4: more rows than the workspace holds (the problem itself may be feasible)
+  if (infeasible) res.status = 2;
+  else if (me > w.me_cap || mi > w.mi_cap || n > QP_MAX_N) res.status = 4;
+  if (res.status != 1) {
     for (int i = lane; i < n; i += 32) x_out[i] = 0.0;
-    res.status = 2;
     return res;
   }
   __syncwarp();

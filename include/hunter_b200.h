@@ -25,7 +25,8 @@
  *                               interpolation, evaluated on the node grid)   legged_interface/src/SwitchedModelReferenceManager.cpp:136-171
  *
  * Conventions: plain pointers and sizes only; no exceptions cross the ABI. Return 0 on success, <0 on misuse / CUDA error
- * (hb_strerror). Per-instance status words: 0 converged, 1 iteration cap, 2 infeasible / ill-posed, 3 NaN.
+ * (hb_strerror). Per-instance status words: 0 converged, 1 iteration cap, 2 infeasible / ill-posed, 3 NaN
+ * (the raw QP adds 4, beyond its row capacity: see hb_wbc_qp_batch_dev).
  * All arithmetic is IEEE float64 (the reference is all-double: ocs2::scalar_t).
  * Layouts (row-major, instance-major): state x[22] = [h_lin/m, h_ang/m, p, zyx, q_j]; input u[22] = [F0..F3, qj_dot];
  * rbd[32] = [zyx, p, q_j, omega_world, v, qj_dot]; WBC solution sol[38] = [qdd(16), F(12), tau(10)].
@@ -377,6 +378,14 @@ int hb_profile_read(hb_ctx* ctx, double* ms_per_kind /*7*/, int64_t* count_per_k
 void* hb_stream(hb_ctx* ctx);
 
 /* ---- device-pointer (asynchronous) entry points ---- */
+/* Batched dense QP, one problem per warp: min 1/2 x'(H + wbc_rho I) x + g'x  s.t.  lbA <= A x <= ubA, with 1 <= n <= 80 and 0 <= m <= 160
+ * (HB_EINVAL otherwise). H (n x n, row-major, exactly symmetric: the residuals read all of it, the factorisation its lower triangle).
+ * Rows: all-zero rows are dropped; |bound| >= 1e19 means no bound on that side; lbA == ubA (exactly) makes an equality row; a row with
+ * two finite bounds lbA < ubA is two-sided. Row capacity: at most 32 equality rows and 96 one-sided entries, where a two-sided row
+ * counts as two entries; zero rows and rows without finite bounds count towards neither.
+ * status[i] (nullable): 0 solved; 1 iteration cap (qp_max_iter) reached, x = last iterate; 2 an all-zero row whose bounds exclude 0
+ * (lbA > 1e-12 or ubA < -1e-12), or a failed factorisation; 3 non-finite iterate; 4 more rows than the capacity above.
+ * With status 2 from a zero row and with status 4, x = 0 and iters = 0. iters[i] (nullable): interior-point iterations. */
 int hb_wbc_qp_batch_dev(hb_ctx* ctx, int B, int n, int m, const double* H, const double* g, const double* A, const double* lbA,
                         const double* ubA, double* x, int32_t* status, int32_t* iters);
 int hb_wbc_solve_batch_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
