@@ -1,4 +1,4 @@
-// SQP iteration, version 2: the per-node work is split from the sequential recursion so that every SM runs many warps.
+// SQP iteration: the per-node work is split from the sequential recursion so that every SM runs many warps.
 //
 //   K0 lin_kernel      one warp = TWO horizon nodes (half-warp each). Lane-parallel unit / dual sweeps of the kinematic tree
 //                      give, per node and RK2 stage, the non-trivial rows of d f/dx, d f/du and the contact kinematics with
@@ -8,7 +8,7 @@
 //                      equations), projected LQ model. Output: "projected record" (PROJ_STRIDE doubles).
 //   K2 riccati_kernel  one warp = one instance, sequential in k, only the value-function recursion: S, s, K, k.
 //   K3 forward_ls      one warp = one instance: forward pass through the projected model, then the filter line search with
-//                      lanes = nodes (shared with version 1: flow_map_lane / node_values_lane in hb_mpc.cuh).
+//                      lanes = nodes (flow_map_lane / node_values_lane in hb_mpc.cuh).
 //
 // Block structure used throughout (x = [hbar(6) | p(3) | theta(3) | qj(10)], u = [F(12) | vj(10)]):
 //   d f/dx has non-zero rows 3..11 only; d f/dF is (1/m) I in rows 0..2, (r_c - com)x / m in rows 3..5;
