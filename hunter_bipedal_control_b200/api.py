@@ -31,6 +31,7 @@ EXPORTED_SYMBOLS = [
     "hb_rbd_to_centroidal_batch", "hb_reference_expand_batch", "hb_probe_flow_map",
     "hb_observer_reset", "hb_contact_force_estimate_batch_dev", "hb_contact_force_estimate_batch",
     "hb_default_wbc_settings", "hb_parse_task_info", "hb_wbc_get_settings", "hb_wbc_set_settings", "hb_wbc_set_kp_kd", "hb_load_task_info",
+    "hb_wbc_set_formulation", "hb_wbc_get_formulation",
     "hb_hoqp_solve_batch_dev", "hb_hierarchical_wbc_solve_batch_dev", "hb_hoqp_solve_batch", "hb_hierarchical_wbc_solve_batch", "hb_hierarchical_wbc_tasks_batch",
     "hb_default_sim_params", "hb_actuation_reset", "hb_actuation_batch_dev", "hb_actuation_batch", "hb_sim_step_batch_dev", "hb_sim_step_batch",
     "hb_resident_wbc_batch_dev", "hb_resident_wbc_batch",
@@ -108,6 +109,8 @@ def parse_task_info(path):
 
 
 HB_ACT_CAPACITY = 16
+HB_WBC_WEIGHTED, HB_WBC_HIERARCHICAL = 0, 1
+WBC_FORMULATIONS = {"weighted": HB_WBC_WEIGHTED, "hierarchical": HB_WBC_HIERARCHICAL}
 HB_HOQP_MAX_LEVELS, HB_HOQP_N, HB_HOQP_MAX_EQ, HB_HOQP_MAX_IN, HB_HOQP_MAX_STACKED = 3, 38, 32, 40, 80
 
 
@@ -570,6 +573,17 @@ class Context:
 
     def load_task_info(self, path):
         _check(self._lib.hb_load_task_info(self._h, str(path).encode()), "hb_load_task_info")
+
+    def set_wbc_formulation(self, name):
+        """The controller's WBC for every entry point that runs it: "weighted" (WeightedWbc, the default) or "hierarchical" (HierarchicalWbc)."""
+        if name not in WBC_FORMULATIONS:
+            raise ValueError("unknown WBC formulation %r (one of %s)" % (name, ", ".join(WBC_FORMULATIONS)))
+        _check(self._lib.hb_wbc_set_formulation(self._h, C.c_int32(WBC_FORMULATIONS[name])), "hb_wbc_set_formulation")
+
+    def wbc_formulation(self):
+        f = C.c_int32()
+        _check(self._lib.hb_wbc_get_formulation(self._h, C.byref(f)), "hb_wbc_get_formulation")
+        return {v: k for k, v in WBC_FORMULATIONS.items()}[f.value]
 
     @property
     def launch_count(self):

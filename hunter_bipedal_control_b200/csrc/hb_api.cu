@@ -45,6 +45,7 @@ template <class T> struct InstanceSetting {
 struct hb_ctx {
   hb_config cfg;
   hb_wbc_settings wbc;       // WBC gains / limits / weights in force (task.info values by default; hb_wbc_set_settings, hb_load_task_info)
+  int32_t wbc_form;          // the controller's WBC (HB_WBC_WEIGHTED, HB_WBC_HIERARCHICAL; hb_wbc_set_formulation)
   int device;
   cudaStream_t stream;
   cudaStream_t stream_main, stream_aux;   // the chunked host-pointer calls pipeline their chunks over these
@@ -57,7 +58,7 @@ struct hb_ctx {
   // WBC scratch: the control step's desired state / input / mode, the fused WBC's status and iterations when the caller passes none
   double *xdes, *udes;
   int32_t *wstatus, *witers, *wmode;
-  void* hoqp_mem; double* hoqp_scratch; hb_hoqp_problem* hoqp_prob;   // hierarchical WBC (allocated by its first call)
+  void* hoqp_mem; double* hoqp_scratch;   // hb_hoqp_solve_batch's lifted level problems (allocated by its first call)
   // hb_resident_cycle_batch_dev: references expanded over the horizon and, with event_nodes, the node grid they are expanded on
   double *cyc_xref, *cyc_swing, *cyc_tk;
   int32_t *cyc_mode, *cyc_nn;
@@ -418,6 +419,7 @@ int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
     attr((const void*)qp_batch_kernel, 200 * 1024);
     attr((const void*)wbc_fused_kernel, wbc_fused_doubles() * sizeof(double));
     attr((const void*)hoqp_kernel, hoqp_smem_bytes());
+    attr((const void*)hwbc_fused_kernel, hwbc_fused_bytes());
     attr((const void*)lin_kernel, 4 * sizeof(LinHalf) + sizeof(ChainModel));
     attr((const void*)lq_kernel, sizeof(LqShared));
     attr((const void*)riccati_kernel, sizeof(RicShared));
@@ -425,7 +427,7 @@ int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
     attr((const void*)warm_shift_kernel, sizeof(double) * ((N + 1) * NX + N * NU));
     // these kernels reach their blocks per SM (8 for the one-block-per-instance kernels, HB_LQ_MINB for lq_kernel) only with the full
     // shared-memory carveout; do not leave it to the driver
-    for (const void* fn : {(const void*)wbc_fused_kernel, (const void*)riccati_kernel, (const void*)lq_kernel})
+    for (const void* fn : {(const void*)wbc_fused_kernel, (const void*)riccati_kernel, (const void*)lq_kernel, (const void*)hwbc_fused_kernel})
       if (fe == cudaSuccess) fe = cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
     if (fe != cudaSuccess) { ctx->last_cuda = (int)fe; hb_destroy(ctx); return HB_ECUDA; }
   }
@@ -534,7 +536,7 @@ static int hoqp_reserve(hb_ctx* ctx) {
   const size_t Bc = ctx->cfg.max_batch;
   return reserve_group(&ctx->hoqp_mem, [&](void* m) {
     size_t off = 0;
-    ctx->hoqp_scratch = carve<double>(m, off, Bc * HQ_SCRATCH); ctx->hoqp_prob = carve<hb_hoqp_problem>(m, off, Bc);
+    ctx->hoqp_scratch = carve<double>(m, off, Bc * HQ_SCRATCH);
     return off;
   });
 }
@@ -553,11 +555,17 @@ static int hwbc_tasks_dev(hb_ctx* ctx, int B, const double* x_des, const double*
 int hb_hierarchical_wbc_solve_batch_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, double* sol,
                                         int32_t* status) {
   ENTER(ctx, B, x_des && u_des && rbd && mode && sol, CAPPED);
-  int rc = hoqp_reserve(ctx);
-  if (rc) return rc;
-  rc = hwbc_tasks_dev(ctx, B, x_des, u_des, rbd, mode, ctx->hoqp_prob);
-  if (rc) return rc;
-  return hb_hoqp_solve_batch_dev(ctx, B, ctx->hoqp_prob, sol, nullptr, status);
+  return launch(ctx, K_QP, hwbc_fused_kernel, B, 32, hwbc_fused_bytes(), B, ctx->wbc, x_des, u_des, rbd, mode, 2 * ctx->cfg.qp_max_iter, sol, status);
+}
+
+// The controller's WBC (LeggedController::wbc_) on device pointers: every entry point that runs it comes through here. stance_mode is read
+// by the weighted formulation only (WbcBase::setStanceMode reaches only WeightedWbc::formulateWeightedTasks). status: nullable, as for
+// hb_wbc_solve_batch_dev.
+static int controller_wbc_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
+                              const uint8_t* stance_mode, double* sol, int32_t* status) {
+  if (ctx->wbc_form == HB_WBC_HIERARCHICAL)
+    return hb_hierarchical_wbc_solve_batch_dev(ctx, B, x_des, u_des, rbd, mode, sol, status ? status : ctx->wstatus + ctx->base);
+  return hb_wbc_solve_batch_dev(ctx, B, x_des, u_des, rbd, mode, stance_mode, sol, status);
 }
 
 int hb_mpc_cold_start_batch_dev(hb_ctx* ctx, int B, const double* x0, const int32_t* mode, double* x_traj, double* u_traj) {
@@ -638,7 +646,7 @@ static int control_step_impl(hb_ctx* ctx, int B, double t_rel, const double* x0,
   double* xdes = ctx->xdes + (size_t)ctx->base * NX; double* udes = ctx->udes + (size_t)ctx->base * NU; int32_t* wmode = ctx->wmode + ctx->base;
   rc = policy_eval_impl(ctx, B, t_rel, x_traj, u_traj, mode, xdes, udes, wmode, tk, nn);
   if (rc) return rc;
-  rc = hb_wbc_solve_batch_dev(ctx, B, xdes, udes, rbd, wmode, nullptr, wbc_sol, wbc_status);
+  rc = controller_wbc_dev(ctx, B, xdes, udes, rbd, wmode, nullptr, wbc_sol, wbc_status);
   if (!rc && torque) rc = launch(ctx, K_UNPROFILED, torque_kernel, (B * NJ + 127) / 128, 128, 0, B, wbc_sol, torque);
   return rc;
 }
@@ -757,6 +765,18 @@ int hb_wbc_set_settings(hb_ctx* ctx, const hb_wbc_settings* s) {
   for (int j = 0; j < 5; ++j) if (!(s->torque_limits[j] > 0.0)) return HB_EINVAL;
   if (!(s->friction_coefficient > 0.0) || !(s->weight_swing_leg > 0.0) || !(s->weight_base_accel > 0.0) || s->weight_contact_force < 0.0) return HB_EINVAL;
   ctx->wbc = *s;      // passed by value with the next launch: nothing in flight is affected
+  return HB_OK;
+}
+
+int hb_wbc_set_formulation(hb_ctx* ctx, int32_t formulation) {
+  if (!ctx || (formulation != HB_WBC_WEIGHTED && formulation != HB_WBC_HIERARCHICAL)) return HB_EINVAL;
+  ctx->wbc_form = formulation;      // read on the host by the next launch: nothing in flight is affected
+  return HB_OK;
+}
+
+int hb_wbc_get_formulation(const hb_ctx* ctx, int32_t* formulation) {
+  if (!ctx || !formulation) return HB_EINVAL;
+  *formulation = ctx->wbc_form;
   return HB_OK;
 }
 
@@ -960,7 +980,7 @@ static int resident_wbc_impl(hb_ctx* ctx, int B, const double* t_now, const doub
   int rc = launch(ctx, K_UNPROFILED, policy_eval_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, (int)N, ctx->cfg.dt, 0.0, ctx->res_xt + o * (N + 1) * NX,
                   ctx->res_ut + o * N * NU, ctx->res_mode + o * (N + 1), x_des, u_des, mode_out, grid ? ctx->res_tk + o * (N + 1) : nullptr,
                   grid ? ctx->res_nn + o : nullptr, t_now, ctx->res_t0 + o);
-  if (!rc) rc = hb_wbc_solve_batch_dev(ctx, B, x_des, u_des, rbd, mode_out, stance_mode, wbc_sol, wbc_status);
+  if (!rc) rc = controller_wbc_dev(ctx, B, x_des, u_des, rbd, mode_out, stance_mode, wbc_sol, wbc_status);
   if (!rc && torque) rc = launch(ctx, K_UNPROFILED, torque_kernel, (B * NJ + 127) / 128, 128, 0, B, wbc_sol, torque);
   return rc ? rc : wbc_fallback(ctx, B, no_prev, wbc_status, wbc_sol, torque);
 }

@@ -8,9 +8,14 @@
 // exactly the (H, c, D, f) of HoQp::buildHMatrix / buildCVector / buildDMatrix / buildFVector, handed to the batched interior point
 // (qp_solve_warp replaces qpOASES as in the weighted WBC). Then Z <- Z kernel(A_k Z) (HoQp::buildZMatrix: Eigen FullPivLU::kernel; here a
 // Gauss-Jordan elimination with complete pivoting -- any basis of the same null space gives the same x).
+//
+// hwbc_fused_kernel runs HierarchicalWbc::update in one launch without materialising an hb_hoqp_problem: the tasks are built in shared
+// memory from the WBC terms and every level is solved at its real shape (hwbc_level0_warp for level 0, qp_solve_warp at <= 28 variables
+// for levels 1 and 2).
 #pragma once
 #include "hb_common.cuh"
 #include "hb_qp.cuh"
+#include "hb_wbc.cuh"
 #include "../../include/hunter_b200.h"
 
 namespace hb {
@@ -30,6 +35,65 @@ struct HoqpShared {
   int pcol[HQ_MA], prow[HQ_MA], isp[HQ_N], freec[HQ_N];
 };
 __host__ __device__ inline size_t hoqp_smem_bytes() { return sizeof(HoqpShared) + qp_workspace_doubles(HQ_NQ, 1, HQ_ROWS) * sizeof(double); }
+
+// Z <- Z kernel(A Z) (HoQp::buildZMatrix) for ma > 0, nx > 0: reduced row echelon form of AZ (ma x nx, leading dimension HQ_LDA, overwritten)
+// with complete pivoting, the new basis formed in Zn and copied back to Z (n x nfree, leading dimension HQ_LDZ). Returns nfree.
+__device__ inline int hoqp_null_space_step(double* Z, double* AZ, double* Zn, int* pcol, int* prow, int* isp, int* freec, int n, int ma, int nx) {
+  const int lane = lane_id();
+  double amax = 0.0;
+  for (int idx = lane; idx < ma * nx; idx += 32) amax = fmax(amax, fabs(AZ[(idx / nx) * HQ_LDA + idx % nx]));
+  amax = warp_max(amax);
+  const double tol = 1e-9 * fmax(amax, 1e-300);
+  for (int j = lane; j < nx; j += 32) isp[j] = 0;
+  __syncwarp();
+  int rank = 0;
+  unsigned long long rowused = 0ull;
+  for (int step = 0; step < min(ma, nx); ++step) {
+    double best = -1.0; int bi = 0, bj = 0;
+    for (int idx = lane; idx < ma * nx; idx += 32) {
+      const int i = idx / nx, j = idx - i * nx;
+      if (((rowused >> i) & 1ull) || isp[j]) continue;
+      const double a = fabs(AZ[i * HQ_LDA + j]);
+      if (a > best) { best = a; bi = i; bj = j; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const double ob = __shfl_xor_sync(HB_FULL_MASK, best, o);
+      const int oi = __shfl_xor_sync(HB_FULL_MASK, bi, o), oj = __shfl_xor_sync(HB_FULL_MASK, bj, o);
+      if (ob > best || (ob == best && (oi < bi || (oi == bi && oj < bj)))) { best = ob; bi = oi; bj = oj; }
+    }
+    if (!(best > tol)) break;
+    const double inv = 1.0 / AZ[bi * HQ_LDA + bj];
+    __syncwarp();
+    for (int j = lane; j < nx; j += 32) AZ[bi * HQ_LDA + j] *= inv;
+    __syncwarp();
+    for (int idx = lane; idx < ma * nx; idx += 32) {
+      const int i = idx / nx, j = idx - i * nx;
+      if (i == bi || j == bj) continue;
+      AZ[i * HQ_LDA + j] -= AZ[i * HQ_LDA + bj] * AZ[bi * HQ_LDA + j];
+    }
+    __syncwarp();
+    for (int i = lane; i < ma; i += 32) if (i != bi) AZ[i * HQ_LDA + bj] = 0.0;
+    if (lane == 0) { pcol[rank] = bj; prow[rank] = bi; isp[bj] = 1; }
+    rowused |= 1ull << bi;
+    ++rank;
+    __syncwarp();
+  }
+  int nfree = 0;
+  for (int j = 0; j < nx; ++j) if (!isp[j]) { if (lane == 0) freec[nfree] = j; ++nfree; }
+  __syncwarp();
+  // column c of the new basis: Z[:, f] - sum_i Z[:, pcol_i] R[prow_i][f]
+  for (int idx = lane; idx < n * nfree; idx += 32) {
+    const int k = idx / nfree, c = idx - k * nfree, fcol = freec[c];
+    double s = Z[k * HQ_LDZ + fcol];
+    for (int i = 0; i < rank; ++i) s = fma(-Z[k * HQ_LDZ + pcol[i]], AZ[prow[i] * HQ_LDA + fcol], s);
+    Zn[k * HQ_LDZ + c] = s;
+  }
+  __syncwarp();
+  for (int idx = lane; idx < n * nfree; idx += 32) { const int k = idx / nfree, c = idx - k * nfree; Z[k * HQ_LDZ + c] = Zn[k * HQ_LDZ + c]; }
+  __syncwarp();
+  return nfree;
+}
 
 // Solve one hierarchy. Returns 0, or the first failing level's QP status * 10 + level.
 __device__ inline int hoqp_solve_warp(const hb_hoqp_problem& pb, HoqpShared& sh, QpWorkspace& w, double* scratch, int max_iter, double* x_out,
@@ -109,65 +173,253 @@ __device__ inline int hoqp_solve_warp(const hb_hoqp_problem& pb, HoqpShared& sh,
     nstk += md;
     __syncwarp();
     // Z <- Z kernel(A Z): reduced row echelon form of AZ with complete pivoting
-    if (ma > 0 && nx > 0) {
-      double amax = 0.0;
-      for (int idx = lane; idx < ma * nx; idx += 32) amax = fmax(amax, fabs(sh.AZ[(idx / nx) * HQ_LDA + idx % nx]));
-      amax = warp_max(amax);
-      const double tol = 1e-9 * fmax(amax, 1e-300);
-      for (int j = lane; j < nx; j += 32) sh.isp[j] = 0;
-      __syncwarp();
-      int rank = 0;
-      unsigned long long rowused = 0ull;
-      for (int step = 0; step < min(ma, nx); ++step) {
-        double best = -1.0; int bi = 0, bj = 0;
-        for (int idx = lane; idx < ma * nx; idx += 32) {
-          const int i = idx / nx, j = idx - i * nx;
-          if (((rowused >> i) & 1ull) || sh.isp[j]) continue;
-          const double a = fabs(sh.AZ[i * HQ_LDA + j]);
-          if (a > best) { best = a; bi = i; bj = j; }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          const double ob = __shfl_xor_sync(HB_FULL_MASK, best, o);
-          const int oi = __shfl_xor_sync(HB_FULL_MASK, bi, o), oj = __shfl_xor_sync(HB_FULL_MASK, bj, o);
-          if (ob > best || (ob == best && (oi < bi || (oi == bi && oj < bj)))) { best = ob; bi = oi; bj = oj; }
-        }
-        if (!(best > tol)) break;
-        const double inv = 1.0 / sh.AZ[bi * HQ_LDA + bj];
-        __syncwarp();
-        for (int j = lane; j < nx; j += 32) sh.AZ[bi * HQ_LDA + j] *= inv;
-        __syncwarp();
-        for (int idx = lane; idx < ma * nx; idx += 32) {
-          const int i = idx / nx, j = idx - i * nx;
-          if (i == bi || j == bj) continue;
-          sh.AZ[i * HQ_LDA + j] -= sh.AZ[i * HQ_LDA + bj] * sh.AZ[bi * HQ_LDA + j];
-        }
-        __syncwarp();
-        for (int i = lane; i < ma; i += 32) if (i != bi) sh.AZ[i * HQ_LDA + bj] = 0.0;
-        if (lane == 0) { sh.pcol[rank] = bj; sh.prow[rank] = bi; sh.isp[bj] = 1; }
-        rowused |= 1ull << bi;
-        ++rank;
-        __syncwarp();
-      }
-      int nfree = 0;
-      for (int j = 0; j < nx; ++j) if (!sh.isp[j]) { if (lane == 0) sh.freec[nfree] = j; ++nfree; }
-      __syncwarp();
-      // column c of the new basis: Z[:, f] - sum_i Z[:, pcol_i] R[prow_i][f]
-      for (int idx = lane; idx < n * nfree; idx += 32) {
-        const int k = idx / nfree, c = idx - k * nfree, fcol = sh.freec[c];
-        double s = sh.Z[k * HQ_LDZ + fcol];
-        for (int i = 0; i < rank; ++i) s = fma(-sh.Z[k * HQ_LDZ + sh.pcol[i]], sh.AZ[sh.prow[i] * HQ_LDA + fcol], s);
-        sh.Zn[k * HQ_LDZ + c] = s;
-      }
-      __syncwarp();
-      for (int idx = lane; idx < n * nfree; idx += 32) { const int k = idx / nfree, c = idx - k * nfree; sh.Z[k * HQ_LDZ + c] = sh.Zn[k * HQ_LDZ + c]; }
-      nx = nfree;
-      __syncwarp();
-    }
+    if (ma > 0 && nx > 0) nx = hoqp_null_space_step(sh.Z, sh.AZ, sh.Zn, sh.pcol, sh.prow, sh.isp, sh.freec, n, ma, nx);
   }
   for (int i = lane; i < n; i += 32) x_out[i] = sh.x[i];
   if (slack_out) for (int i = lane; i < HQ_STK; i += 32) slack_out[i] = i < nstk ? stks[i] : 0.0;
   return status;
+}
+
+// ---- the three tasks of HierarchicalWbc::update (WbcBase.cpp:138-338), decision vector [qdd(16), F(12), tau(10)], rows of NWBC columns
+// at leading dimension lda. Rows of task0 after the 16 EoM rows come per contact in contact order: the swing contacts' first, then the
+// stance contacts'.
+
+// the k-th contact (contact order) whose contact flag is `stance`
+__device__ inline int hwbc_nth_contact(int mode, bool stance, int k) {
+  int c = 0;
+  for (; c < 3; ++c) if (contact_flag(mode, c) == stance && k-- == 0) break;
+  return c;
+}
+
+// task0 equalities (16 + 3 * 4 = 28 rows): EoM [M | -J' | -S'] x = -nle, zero force of each swing contact, no motion of each stance contact
+constexpr int HW_MA0 = 28;
+__device__ inline void hwbc_task0_eq(const WbcShared& sh, int mode, double* A, int lda, double* b) {
+  const int lane = lane_id();
+  int nsw = 0;
+  for (int c = 0; c < 4; ++c) nsw += !contact_flag(mode, c);
+  for (int idx = lane; idx < HW_MA0 * NWBC; idx += 32) {
+    const int i = idx / NWBC, j = idx - i * NWBC;
+    double a = 0.0;
+    if (i < 16) {
+      if (j < NQ) a = sh.M[i * 16 + j];
+      else if (j < NQ + 12) a = -sh.J[(j - NQ) * 16 + i];
+      else a = (i >= 6 && j - NQ - 12 == i - 6) ? -1.0 : 0.0;
+    } else if (i < 16 + 3 * nsw) {
+      const int k = i - 16, c = hwbc_nth_contact(mode, false, k / 3);
+      a = (j == NQ + 3 * c + k % 3) ? 1.0 : 0.0;
+    } else {
+      const int k = i - 16 - 3 * nsw, c = hwbc_nth_contact(mode, true, k / 3);
+      a = j < NQ ? sh.J[(3 * c + k % 3) * 16 + j] : 0.0;
+    }
+    A[i * lda + j] = a;
+  }
+  for (int i = lane; i < HW_MA0; i += 32) {
+    double v = 0.0;
+    if (i < 16) v = -sh.nle[i];
+    else if (i >= 16 + 3 * nsw) { const int k = i - 16 - 3 * nsw; v = -sh.dJv[3 * hwbc_nth_contact(mode, true, k / 3) + k % 3]; }
+    b[i] = v;
+  }
+}
+
+// task0 inequality row q (20 torque-limit rows, then 5 friction-pyramid rows per stance contact): its nonzeros are coef[0 .. len) from
+// column col0; returns its bound f
+__device__ inline double hwbc_task0_ineq(const hb_wbc_settings& ws, int mode, int q, int& col0, int& len, double* coef) {
+  if (q < 2 * NJ) {
+    const int j = q % NJ;
+    col0 = NQ + 12 + j; len = 1; coef[0] = q < NJ ? 1.0 : -1.0; coef[1] = 0.0; coef[2] = 0.0;
+    return ws.torque_limits[j % 5];
+  }
+  const int fr = q - 2 * NJ, k = fr % 5;
+  const double mu = ws.friction_coefficient;   // pyramid rows {0,0,-1}, {1,0,-mu}, {-1,0,-mu}, {0,1,-mu}, {0,-1,-mu}
+  col0 = NQ + 3 * hwbc_nth_contact(mode, true, fr / 5); len = 3;
+  coef[0] = k == 1 ? 1.0 : (k == 2 ? -1.0 : 0.0);
+  coef[1] = k == 3 ? 1.0 : (k == 4 ? -1.0 : 0.0);
+  coef[2] = k == 0 ? -1.0 : -mu;
+  return 0.0;
+}
+
+// task1 (lvl 1): the 6 base-acceleration rows; task2 (lvl 2): 0.1 * (F = F_des), then the 3 rows of each swing contact. Both are the
+// weighted formulation's rows (Aw, bw of WbcShared, stride 16) with the weight divided out. Returns the number of rows.
+__device__ inline int hwbc_task12_rows(int lvl, const double* Aw, const double* bw, const hb_wbc_settings& ws, const double* u_des, int nsw,
+                                       double* A, int lda, double* b) {
+  const int lane = lane_id(), nswr = 3 * nsw;
+  const int ma = lvl == 1 ? 6 : 12 + nswr;
+  for (int idx = lane; idx < ma * NWBC; idx += 32) {
+    const int i = idx / NWBC, j = idx - i * NWBC;
+    double a = 0.0;
+    if (lvl == 1) { if (j < NQ) a = Aw[(nswr + i) * 16 + j] / ws.weight_base_accel; }
+    else if (i < 12) a = (j == NQ + i) ? 0.1 : 0.0;
+    else if (j < NQ) a = Aw[(i - 12) * 16 + j] / ws.weight_swing_leg;
+    A[i * lda + j] = a;
+  }
+  for (int i = lane; i < ma; i += 32)
+    b[i] = lvl == 1 ? bw[nswr + i] / ws.weight_base_accel : (i < 12 ? 0.1 * u_des[i] : bw[i - 12] / ws.weight_swing_leg);
+  return ma;
+}
+
+// ---- the fused hierarchical WBC (hwbc_fused_kernel): one warp per instance, everything in shared memory
+// hwbc_fused_kernel calls level 0 and the null-space steps out of line: inlined into the kernel next to the WBC assembly, whose peak sits
+// at the 255-register ceiling, they made ptxas spill; hoqp_kernel keeps hoqp_null_space_step inline.
+__device__ __noinline__ int hwbc_null_space_step(double* Z, double* AZ, double* Zn, int* pcol, int* prow, int* isp, int* freec, int n, int ma, int nx) {
+  return hoqp_null_space_step(Z, AZ, Zn, pcol, prow, isp, freec, n, ma, nx);
+}
+constexpr int HW_NX = 28;   // free variables a level 1 / 2 QP holds (leading dimension 29: the register-window factorisation)
+constexpr int HW_LD0 = NWBC + 1;
+struct HwbcShared {
+  double Z[HQ_N * HQ_LDZ];        // null-space basis of the levels solved so far
+  double AZ[HW_MA0 * HQ_LDA];     // the level's task rows times Z, then their reduced row echelon form
+  double x[HQ_N], r[HW_MA0];      // solution so far; task residual A x - b
+  double dco[HQ_MD * 3], f0[HQ_MD], v0[HQ_MD];   // task0 inequality rows (nonzeros from column dc0), bounds, level-0 slack solution
+  double Aw[18 * 16], bw[18];     // the weighted rows of WbcShared that tasks 1 and 2 are built from
+  int pcol[HW_MA0], prow[HW_MA0], isp[HQ_N], freec[HQ_N], dc0[HQ_MD], dlen[HQ_MD];
+};
+// scratch shared by the phases: the assembly (WbcShared), level 0 (hwbc_level0_warp), a level-1/2 task and its QP, the next basis Zn
+__host__ __device__ constexpr size_t hw_level0_doubles() { return (size_t)tri_row(NWBC) + NWBC * HW_LD0 + 6 * NWBC + 6 * HQ_MD + 7 * 2 * HQ_MD; }
+__host__ __device__ constexpr size_t hw_level12_doubles() { return qp_workspace_doubles(HW_NX, 1, HQ_MD) + (size_t)HQ_MD * HW_NX + 2 * HQ_MD + 2 * HW_NX; }
+__host__ __device__ constexpr size_t hw_max(size_t a, size_t b) { return a > b ? a : b; }
+__host__ __device__ constexpr size_t hwbc_scratch_doubles() {
+  return hw_max(hw_max(hw_level0_doubles(), hw_level12_doubles()),
+                hw_max(hw_max(sizeof(WbcShared) / sizeof(double), (size_t)HQ_N * HQ_LDZ), (size_t)HW_MA0 * NWBC + HW_MA0));
+}
+__host__ __device__ constexpr size_t hwbc_fused_bytes() { return sizeof(HwbcShared) + hwbc_scratch_doubles() * sizeof(double); }
+// one warp per block: 4 blocks per SM put a 1024-instance batch in two waves on 132 SMs (the runtime reserves 1 KB per block)
+static_assert(4 * (hwbc_fused_bytes() + 1024) <= 228 * 1024, "hwbc_fused_kernel must fit 4 blocks per SM");
+
+// Level 0 of the cascade (Z = I, x_prev = 0) at its real shape. The lifted problem hoqp_solve_warp hands qp_solve_warp is, in x (38) and
+// one slack v_j per inequality row D_j of task0,
+//     min 1/2 x'G x + c'x + 1/2 v'v   s.t.  -v <= 0,  D x - v <= f,      G = A'A + 1e-12 I,  c = A'r  (r = -b)
+// This runs the same Mehrotra iteration as qp_solve_warp on it (start point, step rule, stopping test, status codes) without forming
+// the (38 + md)-square Newton matrix: its slack block is diagonal, d = 1 + rho + w_b + w_d (w = z / s of the two rows that hold v_j), so
+// the Newton step is the 38 x 38 Schur complement S = G + rho I + D' diag(w_d (1 + rho + w_b) / d) D, and D has at most 3 nonzeros per row.
+// x -> sh.x, v -> sh.v0.
+__device__ __noinline__ QpResult hwbc_level0_warp(HwbcShared& sh, int md, double rho, int max_iter, double* work) {
+  const int lane = lane_id();
+  constexpr int n = NWBC, ld = HW_LD0;
+  const int mi = 2 * md;                    // entries: 0 .. md-1 the bounds -v <= 0, md .. 2md-1 the rows D x - v <= f
+  double* G = work; double* K = G + tri_row(n); double* kdi = K + n * ld;
+  double* c = kdi + n; double* rdx = c + n; double* dx = rdx + n; double* t1 = dx + n; double* t2 = t1 + n;
+  double* v = t2 + n; double* dv = v + HQ_MD; double* rdv = dv + HQ_MD; double* dd = rdv + HQ_MD; double* wd = dd + HQ_MD; double* qv = wd + HQ_MD;
+  double* s = qv + HQ_MD; double* z = s + 2 * HQ_MD; double* ds = z + 2 * HQ_MD; double* dz = ds + 2 * HQ_MD; double* rs = dz + 2 * HQ_MD;
+  double* rc = rs + 2 * HQ_MD; double* cw = rc + 2 * HQ_MD;
+  const double* A = sh.AZ;
+  // row j of D times a vector
+  auto drow = [&](int j, const double* y) { double a = 0.0; for (int k = 0; k < sh.dlen[j]; ++k) a = fma(sh.dco[3 * j + k], y[sh.dc0[j] + k], a); return a; };
+  // sum_j q_j D_j[i] over the rows that touch column i
+  auto dtmul = [&](int i, const double* q, double a) {
+    for (int j = 0; j < md; ++j) { const int k = i - sh.dc0[j]; if (k >= 0 && k < sh.dlen[j]) a = fma(q[j], sh.dco[3 * j + k], a); }
+    return a;
+  };
+  for (int idx = lane; idx < n * n; idx += 32) {
+    const int i = idx / n, j = idx - i * n;
+    if (j > i) continue;
+    double a = 0.0;
+    for (int k = 0; k < HW_MA0; ++k) a = fma(A[k * HQ_LDA + i], A[k * HQ_LDA + j], a);
+    G[tri_row(i) + j] = a + (i == j ? 1e-12 : 0.0);
+  }
+  double gs = 1.0, bs = 1.0, fsum = 0.0;
+  for (int i = lane; i < n; i += 32) {
+    double a = 0.0;
+    for (int k = 0; k < HW_MA0; ++k) a = fma(A[k * HQ_LDA + i], sh.r[k], a);
+    c[i] = a; sh.x[i] = 0.0; gs = fmax(gs, 1.0 + fabs(a));
+  }
+  for (int j = lane; j < md; j += 32) { v[j] = 0.0; fsum += fabs(sh.f0[j]); bs = fmax(bs, 1.0 + fabs(sh.f0[j])); }
+  fsum = warp_sum(fsum);
+  const double theta = fmax(1.0, mi > 0 ? fsum / mi : 1.0);
+  for (int e = lane; e < mi; e += 32) { const double f = e < md ? 0.0 : sh.f0[e - md], se = fmax(theta, f); s[e] = se; z[e] = theta / se; }
+  gs = warp_max(gs); bs = warp_max(bs);
+  __syncwarp();
+  QpResult res{1, 0};
+  int it = 0;
+  for (; it < max_iter; ++it) {
+    // ---- residuals
+    for (int i = lane; i < n; i += 32) {
+      double a = c[i] + rho * sh.x[i];
+      for (int k = 0; k <= i; ++k) a += G[tri_row(i) + k] * sh.x[k];
+      for (int k = i + 1; k < n; ++k) a += G[tri_row(k) + i] * sh.x[k];
+      rdx[i] = dtmul(i, z + md, a);
+    }
+    double sz = 0.0, rpn = 0.0, rdn = 0.0;
+    for (int j = lane; j < md; j += 32) {
+      rdv[j] = rho * v[j] + v[j] - z[j] - z[md + j];
+      rs[j] = -v[j] + s[j];
+      rs[md + j] = drow(j, sh.x) - v[j] + s[md + j] - sh.f0[j];
+      sz += s[j] * z[j] + s[md + j] * z[md + j];
+      rdn = fmax(rdn, fabs(rdv[j])); rpn = fmax(rpn, fmax(fabs(rs[j]), fabs(rs[md + j])));
+    }
+    __syncwarp();
+    for (int i = lane; i < n; i += 32) rdn = fmax(rdn, fabs(rdx[i]));
+    rdn = warp_max(rdn); rpn = warp_max(rpn);
+    const double mu = mi > 0 ? warp_sum(sz) / mi : 0.0;
+    if (!(rdn == rdn) || !(rpn == rpn) || !(mu == mu) || rdn > 1e300 || rpn > 1e300) { res.status = 3; break; }
+    if (rdn < 1e-10 * gs && rpn < 1e-10 * bs && mu < 1e-12) { res.status = 0; break; }
+    // ---- Schur complement S (lower triangle): lane c owns column c, so the rows sharing a column block never collide
+    for (int j = lane; j < md; j += 32) {
+      const double wb = z[j] / s[j], w = z[md + j] / s[md + j], d = 1.0 + rho + wb + w;
+      dd[j] = d; wd[j] = w; cw[j] = w * (1.0 + rho + wb) / d;
+    }
+    for (int idx = lane; idx < n * ld; idx += 32) { const int i = idx / ld, k = idx - i * ld; if (k <= i && i < n) K[idx] = G[tri_row(i) + k] + (i == k ? rho : 0.0); }
+    __syncwarp();
+    for (int col = lane; col < n; col += 32)
+      for (int j = 0; j < md; ++j) {
+        const int k = col - sh.dc0[j];
+        if (k < 0 || k >= sh.dlen[j]) continue;
+        const double a = cw[j] * sh.dco[3 * j + k];
+        for (int m = k; m < sh.dlen[j]; ++m) K[(sh.dc0[j] + m) * ld + col] += a * sh.dco[3 * j + m];
+      }
+    __syncwarp();
+    if (!warp_chol_inv(K, n, ld, kdi, lane, 1e-10)) { res.status = 2; break; }
+    // ---- Newton step for the complementarity target rc: dx, dv, ds, dz
+    auto newton = [&]() {
+      for (int e = lane; e < mi; e += 32) cw[e] = (rc[e] - z[e] * rs[e]) / s[e];
+      __syncwarp();
+      for (int j = lane; j < md; j += 32) { const double rv = -rdv[j] - cw[j] - cw[md + j]; dv[j] = rv; qv[j] = cw[md + j] + wd[j] * rv / dd[j]; }
+      __syncwarp();
+      for (int i = lane; i < n; i += 32) t2[i] = dtmul(i, qv, -rdx[i]);
+      __syncwarp();
+      warp_li_mv(K, n, ld, kdi, t2, t1, lane);
+      warp_lit_mv(K, n, ld, kdi, t1, dx, lane);
+      for (int j = lane; j < md; j += 32) {
+        const double ddx = drow(j, dx), dvj = (dv[j] + wd[j] * ddx) / dd[j];
+        dv[j] = dvj;
+        ds[j] = -rs[j] + dvj;
+        ds[md + j] = -rs[md + j] - (ddx - dvj);
+        dz[j] = -(rc[j] + z[j] * ds[j]) / s[j];
+        dz[md + j] = -(rc[md + j] + z[md + j] * ds[md + j]) / s[md + j];
+      }
+      __syncwarp();
+    };
+    auto max_step = [&]() {
+      double a = 1.0;
+      for (int e = lane; e < mi; e += 32) {
+        if (ds[e] < 0.0) a = fmin(a, -s[e] / ds[e]);
+        if (dz[e] < 0.0) a = fmin(a, -z[e] / dz[e]);
+      }
+      return warp_min(a);
+    };
+    for (int e = lane; e < mi; e += 32) rc[e] = s[e] * z[e];
+    __syncwarp();
+    newton();
+    if (mi > 0) {
+      const double a_aff = max_step();
+      double ma = 0.0;
+      for (int e = lane; e < mi; e += 32) ma += (s[e] + a_aff * ds[e]) * (z[e] + a_aff * dz[e]);
+      ma = warp_sum(ma) / mi;
+      const double r = ma / mu;
+      const double sigma = r * r * r;
+      for (int e = lane; e < mi; e += 32) rc[e] = s[e] * z[e] + ds[e] * dz[e] - sigma * mu;
+      __syncwarp();
+      newton();
+    }
+    const double alpha = fmin(1.0, 0.995 * max_step());
+    for (int i = lane; i < n; i += 32) sh.x[i] += alpha * dx[i];
+    for (int j = lane; j < md; j += 32) v[j] += alpha * dv[j];
+    for (int e = lane; e < mi; e += 32) { s[e] += alpha * ds[e]; z[e] += alpha * dz[e]; }
+    __syncwarp();
+  }
+  for (int j = lane; j < md; j += 32) sh.v0[j] = v[j];
+  __syncwarp();
+  res.iters = it;
+  return res;
 }
 
 }  // namespace hb
@@ -197,45 +449,110 @@ __global__ void __launch_bounds__(32) hwbc_tasks_kernel(int B, hb_wbc_settings w
   int nw = 0;
   wbc_assemble_warp(x_des + (size_t)inst * NX, u_des + (size_t)inst * NU, rbd + (size_t)inst * 32, md_, false, ws, sh, nullptr, nullptr, nullptr, nullptr, nullptr, &nw);
   hb_hoqp_problem& pb = problems[inst];
-  bool fl[4]; int nc = 0;
-  for (int c = 0; c < 4; ++c) { fl[c] = contact_flag(md_, c); nc += fl[c]; }
+  int nc = 0;
+  for (int c = 0; c < 4; ++c) nc += contact_flag(md_, c);
   const int nsw = 4 - nc;
   const int ma0 = 16 + 3 * nsw + 3 * nc, md0 = 20 + 5 * nc, ma1 = 6, ma2 = 12 + 3 * nsw;
   if (lane == 0) { pb.n = NWBC; pb.levels = 3; pb.ma[0] = ma0; pb.md[0] = md0; pb.ma[1] = ma1; pb.md[1] = 0; pb.ma[2] = ma2; pb.md[2] = 0; }
   for (int idx = lane; idx < HB_HOQP_MAX_EQ * NWBC; idx += 32) { (&pb.a[0][0][0])[idx] = 0.0; (&pb.a[1][0][0])[idx] = 0.0; (&pb.a[2][0][0])[idx] = 0.0; }
   for (int idx = lane; idx < HB_HOQP_MAX_IN * NWBC; idx += 32) (&pb.d[0][0][0])[idx] = 0.0;
   __syncwarp();
-  // task0 equalities: EoM rows [M | -J' | -S'] x = -nle
-  for (int idx = lane; idx < 16 * NWBC; idx += 32) {
-    const int i = idx / NWBC, j = idx - i * NWBC;
-    double a;
-    if (j < NQ) a = sh.M[i * 16 + j];
-    else if (j < NQ + 12) a = -sh.J[(j - NQ) * 16 + i];
-    else a = (i >= 6 && j - NQ - 12 == i - 6) ? -1.0 : 0.0;
-    pb.a[0][i][j] = a;
+  hwbc_task0_eq(sh, md_, &pb.a[0][0][0], NWBC, pb.b[0]);
+  for (int q = lane; q < md0; q += 32) {
+    int c0, len; double coef[3];
+    pb.f[0][q] = hwbc_task0_ineq(ws, md_, q, c0, len, coef);
+    for (int k = 0; k < len; ++k) pb.d[0][q][c0 + k] = coef[k];
   }
-  if (lane < 16) pb.b[0][lane] = -sh.nle[lane];
-  if (lane == 0) {
-    int r = 16;
-    for (int c = 0; c < 4; ++c) if (!fl[c]) for (int a = 0; a < 3; ++a) { pb.a[0][r][NQ + 3 * c + a] = 1.0; pb.b[0][r] = 0.0; ++r; }      // zero swing force
-    for (int c = 0; c < 4; ++c) if (fl[c]) for (int a = 0; a < 3; ++a) {                                                                  // no contact motion
-      for (int j = 0; j < NQ; ++j) pb.a[0][r][j] = sh.J[(3 * c + a) * 16 + j];
-      pb.b[0][r] = -sh.dJv[3 * c + a]; ++r;
+  hwbc_task12_rows(1, sh.Aw, sh.bw, ws, u_des + (size_t)inst * NU, nsw, &pb.a[1][0][0], NWBC, pb.b[1]);
+  hwbc_task12_rows(2, sh.Aw, sh.bw, ws, u_des + (size_t)inst * NU, nsw, &pb.a[2][0][0], NWBC, pb.b[2]);
+}
+
+// HierarchicalWbc::update in one launch, one warp per instance (block): WBC terms (wbc_assemble_warp), the three tasks in shared memory,
+// level 0 by hwbc_level0_warp, levels 1 and 2 by qp_solve_warp at their real shape (n = the free variables level 0 leaves, rows = the
+// stacked task0 inequalities), the null-space steps of hoqp_solve_warp in between. sol = x (38), status as hoqp_kernel: 0,
+// 10 * (QP status) + level of the first failing level, or 20 + level when a level leaves more than HW_NX free variables.
+__global__ void __launch_bounds__(32, 4) hwbc_fused_kernel(int B, hb_wbc_settings ws, const double* x_des, const double* u_des, const double* rbd,
+                                                           const int32_t* mode, int max_iter, double* sol, int32_t* status) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int inst = blockIdx.x, lane = threadIdx.x;
+  if (inst >= B) return;
+  HwbcShared& sh = *reinterpret_cast<HwbcShared*>(smem_raw);
+  double* U = reinterpret_cast<double*>(smem_raw + sizeof(HwbcShared));     // scratch of the current phase
+  WbcShared& wsh = *reinterpret_cast<WbcShared*>(U);
+  const int md_ = mode[inst];
+  const double* ud = u_des + (size_t)inst * NU;
+  int nw = 0;
+  wbc_assemble_warp(x_des + (size_t)inst * NX, ud, rbd + (size_t)inst * 32, md_, false, ws, wsh, nullptr, nullptr, nullptr, nullptr, nullptr, &nw);
+  int nc = 0;
+  for (int c = 0; c < 4; ++c) nc += contact_flag(md_, c);
+  const int nsw = 4 - nc, md0 = 2 * NJ + 5 * nc;
+  // task0 (Z = I: AZ = A, r = -b), its inequality rows, the weighted rows tasks 1 and 2 are built from
+  hwbc_task0_eq(wsh, md_, sh.AZ, HQ_LDA, sh.r);
+  for (int q = lane; q < md0; q += 32) sh.f0[q] = hwbc_task0_ineq(ws, md_, q, sh.dc0[q], sh.dlen[q], &sh.dco[3 * q]);
+  for (int i = lane; i < 18 * 16; i += 32) sh.Aw[i] = wsh.Aw[i];
+  if (lane < 18) sh.bw[lane] = wsh.bw[lane];
+  for (int idx = lane; idx < HQ_N * HQ_LDZ; idx += 32) { const int i = idx / HQ_LDZ, j = idx - i * HQ_LDZ; sh.Z[idx] = (i == j) ? 1.0 : 0.0; }
+  __syncwarp();
+  for (int i = lane; i < HW_MA0; i += 32) sh.r[i] = -sh.r[i];
+  __syncwarp();
+  const QpResult r0 = hwbc_level0_warp(sh, md0, 1e-10, max_iter, U);
+  int status_ = r0.status != 0 ? 10 * r0.status : 0;
+  int nx = hwbc_null_space_step(sh.Z, sh.AZ, U, sh.pcol, sh.prow, sh.isp, sh.freec, HQ_N, HW_MA0, HQ_N);
+  for (int lvl = 1; lvl < 3; ++lvl) {
+    if (nx > HW_NX) { status_ = 20 + lvl; break; }
+    double* Ak = U; double* bk = U + HW_MA0 * NWBC;
+    const int ma = hwbc_task12_rows(lvl, sh.Aw, sh.bw, ws, ud, nsw, Ak, NWBC, bk);
+    __syncwarp();
+    if (nx == 0) continue;
+    // AZ = A Z, r = A x - b (the sums of hoqp_solve_warp)
+    for (int idx = lane; idx < ma * nx; idx += 32) {
+      const int i = idx / nx, j = idx - i * nx;
+      double s = 0.0;
+      for (int k = 0; k < HQ_N; ++k) s = fma(Ak[i * NWBC + k], sh.Z[k * HQ_LDZ + j], s);
+      sh.AZ[i * HQ_LDA + j] = s;
     }
-    // task0 inequalities: torque limits, friction pyramid
-    int q = 0;
-    for (int sgn = 0; sgn < 2; ++sgn) for (int j = 0; j < NJ; ++j) { pb.d[0][q][NQ + 12 + j] = sgn == 0 ? 1.0 : -1.0; pb.f[0][q] = ws.torque_limits[j % 5]; ++q; }
-    const double mu = ws.friction_coefficient;
-    const double pyr[5][3] = {{0, 0, -1}, {1, 0, -mu}, {-1, 0, -mu}, {0, 1, -mu}, {0, -1, -mu}};
-    for (int c = 0; c < 4; ++c) if (fl[c]) for (int k = 0; k < 5; ++k) { for (int a = 0; a < 3; ++a) pb.d[0][q][NQ + 3 * c + a] = pyr[k][a]; pb.f[0][q] = 0.0; ++q; }
-    // task2 first part: 0.1 * (F = F_des)
-    for (int j = 0; j < 12; ++j) { pb.a[2][j][NQ + j] = 0.1; pb.b[2][j] = 0.1 * u_des[(size_t)inst * NU + j]; }
+    for (int i = lane; i < ma; i += 32) { double s = -bk[i]; for (int k = 0; k < HQ_N; ++k) s = fma(Ak[i * NWBC + k], sh.x[k], s); sh.r[i] = s; }
+    __syncwarp();
+    // the level's QP: H = (AZ)'AZ + 1e-12 I, c = (AZ)'r, rows D0 Z <= f0 - D0 x + v0 (no slack of its own: tasks 1 and 2 have no inequalities)
+    QpWorkspace w;
+    qp_carve(U, HW_NX, w, 1, HQ_MD);
+    double* Dq = U + qp_workspace_doubles(HW_NX, 1, HQ_MD); double* lbq = Dq + HQ_MD * HW_NX; double* ubq = lbq + HQ_MD;
+    double* cq = ubq + HQ_MD; double* zq = cq + HW_NX;
+    for (int idx = lane; idx < nx * nx; idx += 32) {
+      const int i = idx / nx, j = idx - i * nx;
+      double s = 0.0;
+      for (int k = 0; k < ma; ++k) s = fma(sh.AZ[k * HQ_LDA + i], sh.AZ[k * HQ_LDA + j], s);
+      if (i == j) s += 1e-12;
+      w.H[i * w.ldn + j] = s;
+    }
+    for (int i = lane; i < nx; i += 32) { double s = 0.0; for (int k = 0; k < ma; ++k) s = fma(sh.AZ[k * HQ_LDA + i], sh.r[k], s); cq[i] = s; }
+    for (int idx = lane; idx < md0 * nx; idx += 32) {
+      const int i = idx / nx, j = idx - i * nx;
+      double s = 0.0;
+      for (int k = 0; k < sh.dlen[i]; ++k) s = fma(sh.dco[3 * i + k], sh.Z[(sh.dc0[i] + k) * HQ_LDZ + j], s);
+      Dq[idx] = s;
+    }
+    for (int i = lane; i < md0; i += 32) {
+      double s = 0.0;
+      for (int k = 0; k < sh.dlen[i]; ++k) s = fma(sh.dco[3 * i + k], sh.x[sh.dc0[i] + k], s);
+      lbq[i] = -1e20; ubq[i] = sh.f0[i] - s + sh.v0[i];
+    }
+    __syncwarp();
+    const QpResult qr = qp_solve_warp(nx, md0, nullptr, cq, Dq, lbq, ubq, 1e-10, max_iter, zq, w);
+    __syncwarp();
+    if (qr.status != 0 && status_ == 0) status_ = 10 * qr.status + lvl;
+    // x <- x + Z z
+    double xn = 0.0, xn2 = 0.0;
+    if (lane < HQ_N) { xn = sh.x[lane]; for (int j = 0; j < nx; ++j) xn = fma(sh.Z[lane * HQ_LDZ + j], zq[j], xn); }
+    if (lane + 32 < HQ_N) { xn2 = sh.x[lane + 32]; for (int j = 0; j < nx; ++j) xn2 = fma(sh.Z[(lane + 32) * HQ_LDZ + j], zq[j], xn2); }
+    __syncwarp();
+    if (lane < HQ_N) sh.x[lane] = xn;
+    if (lane + 32 < HQ_N) sh.x[lane + 32] = xn2;
+    __syncwarp();
+    if (ma > 0) nx = hwbc_null_space_step(sh.Z, sh.AZ, U, sh.pcol, sh.prow, sh.isp, sh.freec, HQ_N, ma, nx);
   }
-  // task1: base acceleration rows (the weighted formulation's base rows with the weight divided out); task2 second part: swing rows
-  const int nswr = 3 * nsw;
-  for (int idx = lane; idx < 6 * NQ; idx += 32) { const int i = idx / NQ, j = idx - i * NQ; pb.a[1][i][j] = sh.Aw[(nswr + i) * 16 + j] / ws.weight_base_accel; }
-  if (lane < 6) pb.b[1][lane] = sh.bw[nswr + lane] / ws.weight_base_accel;
-  for (int idx = lane; idx < nswr * NQ; idx += 32) { const int i = idx / NQ, j = idx - i * NQ; pb.a[2][12 + i][j] = sh.Aw[i * 16 + j] / ws.weight_swing_leg; }
-  if (lane < nswr) pb.b[2][12 + lane] = sh.bw[lane] / ws.weight_swing_leg;
+  double* out = sol + (size_t)inst * NWBC;
+  for (int i = lane; i < NWBC; i += 32) out[i] = sh.x[i];
+  if (status && lane == 0) status[inst] = status_;
 }
 }  // namespace

@@ -221,6 +221,8 @@ __device__ inline void warp_lit_mv(const double* M, int n, int ld, const double*
 struct QpResult { int status; int iters; };
 
 // A, lbA, ubA, H, g may live in global or shared memory (generic pointers). x_out: n doubles (generic).
+// hwbc_level0_warp (hb_hoqp.cuh) runs this same iteration on level 0 of the hierarchical WBC with a Schur-complement Newton step: a change
+// to the start point, the stopping test, the pivot floor or the step rule here belongs there too.
 // PACKED_H: the caller assembled H in w.H as its packed lower triangle (tri_row) and passes H == nullptr; H must be exactly symmetric.
 // The products read the same values in the same order as with the full matrix, so the iterates are bit-identical.
 template <bool PACKED_H = false>

@@ -166,6 +166,18 @@ int hb_parse_task_info(const char* path, hb_task_info* out);          /* host on
 int hb_wbc_get_settings(const hb_ctx* ctx, hb_wbc_settings* s);
 int hb_wbc_set_settings(hb_ctx* ctx, const hb_wbc_settings* s);
 int hb_wbc_set_kp_kd(hb_ctx* ctx, double swing_kp, double swing_kd);   /* WbcBase::setKpKd */
+/* The controller's whole-body controller (LeggedController::wbc_), per context. A new context is weighted.
+ * Entry points that run the controller's WBC follow it: hb_control_step_batch(_dev), hb_resident_cycle_batch(_dev),
+ * hb_resident_plan_cycle_batch, hb_resident_wbc_batch(_dev), hb_rollout_batch_dev and hb_rollout_estimated_batch_dev. Entry points named
+ * after one class ignore it: hb_wbc_solve_batch(_dev) is always WeightedWbc, hb_hierarchical_wbc_solve_batch(_dev) always HierarchicalWbc.
+ * Under HB_WBC_HIERARCHICAL, stance_mode arguments are accepted and have no effect (WbcBase::setStanceMode is read only by
+ * WeightedWbc::formulateWeightedTasks), and the previous-solution fallback of the weighted path applies to a status != 0 (the reference's
+ * HoQp applies whatever iterate qpOASES holds; see DESIGN §1 "Hierarchical WBC in the loop"). hb_wbc_set_settings, hb_wbc_set_kp_kd and
+ * hb_load_task_info apply to both formulations and leave the choice as it is. */
+#define HB_WBC_WEIGHTED 0       /* legged::WeightedWbc (default) */
+#define HB_WBC_HIERARCHICAL 1   /* legged::HierarchicalWbc       */
+int hb_wbc_set_formulation(hb_ctx* ctx, int32_t formulation);   /* -1 for any other value; the previous choice is kept */
+int hb_wbc_get_formulation(const hb_ctx* ctx, int32_t* formulation);
 int hb_load_task_info(hb_ctx* ctx, const char* path);                  /* hb_parse_task_info + hb_wbc_set_settings */
 
 /* ---- hierarchical QP (SURVEY 8f row N4): legged::HoQp / legged::HierarchicalWbc ---- */
@@ -404,7 +416,9 @@ int hb_wbc_qp_rows_batch_dev(hb_ctx* ctx, int B, int n, int m_alloc, const int32
  * slack (B x 80, nullable) = stacked slack solutions in level order, status[i] = 0 or 10 * (QP status) + level of the first failing level */
 int hb_hoqp_solve_batch_dev(hb_ctx* ctx, int B, const hb_hoqp_problem* problems, double* x, double* slack /*nullable*/, int32_t* status /*nullable*/);
 /* legged::HierarchicalWbc::update (legged_wbc/src/HierarchicalWbc.cpp:18-31): task0 = floating-base EoM + torque limits + friction cone +
- * no contact motion, task1 = base acceleration, task2 = 0.1 * contact force + swing leg; sol (B x 38) = [qdd, F, tau] */
+ * no contact motion, task1 = base acceleration, task2 = 0.1 * contact force + swing leg; sol (B x 38) = [qdd, F, tau]. One fused kernel per
+ * call: the tasks never leave the chip and each level is solved at its own shape. status[i] as hb_hoqp_solve_batch_dev's, plus 21 / 22
+ * when level 0 / 1 leaves more than 28 free variables to the next level (level 0 leaves at most 22 while its EoM rows have full rank). */
 int hb_hierarchical_wbc_solve_batch_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
                                         double* sol, int32_t* status /*nullable*/);
 int hb_mpc_cold_start_batch_dev(hb_ctx* ctx, int B, const double* x0, const int32_t* mode, double* x_traj, double* u_traj);

@@ -57,7 +57,7 @@ def main():
             "unit": "robot-s/s", "n_gpus": 1, "steps": len(runs), "warmup": 1, "higher_is_better": True, "dtype": "f64", "data": "synthetic",
             "ms_per_episode": med, "ms_per_episode_range": [min(ms), max(ms)], "ms_per_mpc_period": med / cycles,
             "launches_per_mpc_period": runs[-1].launches / cycles, "gpu_launches": int(runs[-1].launches),
-            "upright_fraction": float((st["fail_tick"] == -1).mean()), "fail_reasons": reasons,
+            "upright_fraction": float((st["fail_tick"] == -1).mean()), "fail_reasons": reasons, "wbc": args.wbc,
             "same_outcome_every_episode": all(np.array_equal(r.stats, st) for r in runs),
             "stats": {"mpc_bad": int(st["mpc_bad"].sum()), "wbc_fallbacks": int(st["wbc_fallbacks"].sum()), "plan_rejects": int(st["plan_rejects"].sum()),
                       "max_abs_torque": float(st["max_abs_torque"].max())},

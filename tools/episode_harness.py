@@ -40,6 +40,7 @@ def parser(batch_help="robots per episode"):
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--estimator", action="store_true", help="run the episodes through the state estimator")
     ap.add_argument("--sensor-noise", type=float, default=0.0, metavar="SCALE", help="with --estimator: sensor noise, SCALE x NOISE_SIGMAS")
+    ap.add_argument("--wbc", choices=("weighted", "hierarchical"), default="weighted", help="the controller's whole-body controller")
     return ap
 
 
@@ -76,6 +77,7 @@ class Episodes:
         torch.cuda.set_device(self.dev)
         self.B = B = args.batch
         self.ctx = hb.Context(horizon_N=HORIZON_N, dt=DT, max_batch=B, device=args.device)
+        self.ctx.set_wbc_formulation(args.wbc)
         x0 = S.random_initial_states(B, SEED)
         self.rbd0 = S.consistent_rbd(x0)
         self.feet = self.ctx.contact_positions(x0).reshape(B, 4, 3)

@@ -86,7 +86,7 @@ def main():
     timing.update({"launches_" + n: int(runs[n][-1].launches) for n in runs})
     line = {"metric": "model mismatch: the heaviest unmodelled payload (0.2 x 0.2 x 0.1 m box, CoM 0.1 m above the base) that >= 90 %% of the "
                       "trotting robots carry for %.1f s, per friction scale" % T_episode, "value": heaviest.get("1"), "unit": "kg",
-            "n_gpus": 1, "dtype": "f64", "data": "synthetic", "estimator": bool(args.estimator),
+            "n_gpus": 1, "dtype": "f64", "data": "synthetic", "estimator": bool(args.estimator), "wbc": args.wbc,
             "heaviest_payload_90pct": heaviest, "survival": survival, "mean_speed_of_survivors_m_per_s": mean_speed, "fail_reasons": reasons,
             "upright_fraction_unset": float((runs["unset"][-1].stats["fail_tick"] < 0).mean()), "timing": timing,
             "config": {"workload": "%d robots, %.1f s simulated (%d ticks of %.0f ms), trot at 0.3 m/s from t = 0.1 s, initial poses of "

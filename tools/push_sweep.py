@@ -89,7 +89,7 @@ def main():
     known = [v for v in largest.values() if v is not None]
     line = {"metric": "push recovery: the largest %.1f s world-frame push at the base, over the four horizontal directions, that >= 90 %% of the "
                       "trotting robots survive" % PUSH_DURATION, "value": min(known) if len(known) == len(names) else None, "unit": "N",
-            "n_gpus": 1, "dtype": "f64", "data": "synthetic", "estimator": bool(args.estimator),
+            "n_gpus": 1, "dtype": "f64", "data": "synthetic", "estimator": bool(args.estimator), "wbc": args.wbc,
             "largest_force_90pct": largest, "survival": survival, "robots_up_at_push": up, "fail_reasons_after_push": reasons,
             "upright_fraction_unpushed": float((runs["unpushed"][-1].stats["fail_tick"] < 0).mean()), "timing": timing,
             "config": {"workload": "%d robots, %.1f s simulated (%d ticks of %.0f ms), trot at 0.3 m/s from t = 0.1 s, initial poses of "

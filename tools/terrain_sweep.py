@@ -114,7 +114,7 @@ def main():
     timing.update({"launches_" + n: int(runs[n][-1].launches) for n in runs})
     line = {"metric": "terrain: the highest step [cm] that >= 90 %% of the trotting robots cross blind within %.1f s; per kind (steps in cm, "
                       "slopes in degrees) under largest_magnitude_90pct" % T_episode, "value": largest["step_up"], "unit": "cm",
-            "n_gpus": 1, "dtype": "f64", "data": "synthetic", "estimator": bool(args.estimator),
+            "n_gpus": 1, "dtype": "f64", "data": "synthetic", "estimator": bool(args.estimator), "wbc": args.wbc,
             "largest_magnitude_90pct": largest, "survival": survival, "mean_speed_of_survivors_m_per_s": mean_speed, "fail_reasons": reasons,
             "upright_fraction_unset": float((runs["unset"][-1].stats["fail_tick"] < 0).mean()), "timing": timing,
             "config": {"workload": "%d robots, %.1f s simulated (%d ticks of %.0f ms), trot at 0.3 m/s from t = 0.1 s, initial poses of "
