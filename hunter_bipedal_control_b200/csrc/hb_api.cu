@@ -58,7 +58,7 @@ struct hb_ctx {
   // WBC scratch: the control step's desired state / input / mode, the fused WBC's status and iterations when the caller passes none
   double *xdes, *udes;
   int32_t *wstatus, *witers, *wmode;
-  void* hoqp_mem; double* hoqp_scratch;   // hb_hoqp_solve_batch's lifted level problems (allocated by its first call)
+  void* hoqp_mem; double* hoqp_scratch;   // hb_hoqp_solve_batch's lifted inequality rows and bounds (allocated by its first call)
   // hb_resident_cycle_batch_dev: references expanded over the horizon and, with event_nodes, the node grid they are expanded on
   double *cyc_xref, *cyc_swing, *cyc_tk;
   int32_t *cyc_mode, *cyc_nn;

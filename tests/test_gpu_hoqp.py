@@ -30,7 +30,7 @@ def _oracle_chain(levels):
     return out
 
 
-def test_reference_unit_test_matrices_and_random_hierarchies(gpu_ctx):
+def _random_hierarchies():
     libc = ctypes.CDLL("libc.so.6")
     libc.srand(0)
     a0 = eigen_random(libc, 2, 4); d0 = eigen_random(libc, 2, 4)                      # HoQp_test.cpp:19-33 (TEST(HoQP, twoTask))
@@ -42,8 +42,21 @@ def test_reference_unit_test_matrices_and_random_hierarchies(gpu_ctx):
             t1 = (rng.normal(size=(2, n)), rng.normal(size=2), rng.normal(size=(3, n)), rng.normal(size=3))
             t2 = (rng.normal(size=(4, n)), rng.normal(size=4), None, None)
             hier.append([t0, t1, t2])
-    pbs = hb.make_hoqp_problems(hier)
-    x, sl, st = gpu_ctx.hoqp_solve(pbs)
+    return hier
+
+
+def _full_stack_hierarchies():
+    """Three levels with inequality rows at every level, 30 + 30 + 20 of them: the stack reaches its 80-row capacity at level 2."""
+    rng = np.random.default_rng(11)
+    hier = []
+    for n, ma in ((10, (4, 3, 4)), (10, (4, 3, 4)), (14, (3, 2, 4)), (14, (3, 2, 4))):
+        hier.append([(rng.normal(size=(m, n)), rng.normal(size=m), rng.normal(size=(md, n)), rng.normal(size=md) + 1.0)
+                     for m, md in zip(ma, (30, 30, 20))])
+    return hier
+
+
+def _check_hierarchies(hier, x, sl, st):
+    """Device cascades against the oracle's; returns how many hierarchies leave no freedom (x itself unique)."""
     assert (st == 0).all(), st
     n_unique = 0
     for i, levels in enumerate(hier):
@@ -64,9 +77,52 @@ def test_reference_unit_test_matrices_and_random_hierarchies(gpu_ctx):
         a_top, b_top, d_top, f_top = levels[0]
         assert np.abs(a_top @ x[i, :n] - a_top @ chain[0].solution()).max() < 1e-6
         assert np.all(d_top @ x[i, :n] <= f_top + chain[0].slack + 1e-6)
-        ns = sum(0 if l[2] is None else l[2].shape[0] for l in levels)
-        assert (sl[i, :ns] > -1e-8).all() and np.abs(sl[i, ns:]).max() == 0.0
-    assert n_unique >= 4
+        # each level's slack solution, stacked in level order
+        off = 0
+        for level, (a, b, d, f) in zip(chain, levels):
+            md = 0 if d is None else d.shape[0]
+            assert np.abs(sl[i, off:off + md] - level.slack).max(initial=0.0) < 1e-5, i
+            off += md
+        assert (sl[i, :off] > -1e-8).all() and np.abs(sl[i, off:]).max(initial=0.0) == 0.0
+    return n_unique
+
+
+def test_reference_unit_test_matrices_and_random_hierarchies(gpu_ctx):
+    hier = _random_hierarchies()
+    x, sl, st = gpu_ctx.hoqp_solve(hb.make_hoqp_problems(hier))
+    assert _check_hierarchies(hier, x, sl, st) >= 4
+
+
+def test_inequalities_at_every_level_fill_the_stack(gpu_ctx):
+    hier = _full_stack_hierarchies()
+    pbs = hb.make_hoqp_problems(hier)
+    assert all(sum(p.md) == 80 for p in pbs)
+    x, sl, st = gpu_ctx.hoqp_solve(pbs)
+    assert _check_hierarchies(hier, x, sl, st) == 2
+
+
+def test_device_call_without_slack_buffer(gpu_ctx):
+    """hb_hoqp_solve_batch_dev with slack = NULL gives the bits of the call with a slack buffer."""
+    import torch
+    hier = _random_hierarchies() + _full_stack_hierarchies()
+    pbs = hb.make_hoqp_problems(hier)
+    B, lib = len(hier), gpu_ctx._lib
+    d_pbs = torch.from_numpy(np.frombuffer(bytes(pbs), dtype=np.uint8).copy()).cuda()
+    P = lambda t: ctypes.c_void_p(t.data_ptr())      # noqa: E731
+
+    def run(with_slack):
+        x = torch.full((B, hb.api.HB_HOQP_N), np.nan, dtype=torch.float64, device="cuda")
+        st = torch.full((B,), -1, dtype=torch.int32, device="cuda")
+        sl = torch.full((B, hb.api.HB_HOQP_MAX_STACKED), np.nan, dtype=torch.float64, device="cuda")
+        torch.cuda.synchronize()
+        assert lib.hb_hoqp_solve_batch_dev(gpu_ctx._h, B, P(d_pbs), P(x), P(sl) if with_slack else None, P(st)) == 0
+        gpu_ctx.sync()
+        return x.cpu().numpy(), st.cpu().numpy(), sl.cpu().numpy()
+
+    x1, st1, sl1 = run(True)
+    x0, st0, _ = run(False)
+    assert (st1 == 0).all() and np.isfinite(sl1).all()
+    assert np.array_equal(x0.view(np.uint64), x1.view(np.uint64)) and np.array_equal(st0, st1)
 
 
 def _wbc_cases(B, seed):
