@@ -11,8 +11,9 @@
 //
 // hwbc_fused_kernel runs HierarchicalWbc::update in one launch without materialising an hb_hoqp_problem: the tasks are built in shared
 // memory from the WBC terms and every level is solved at its real shape (hwbc_level0_warp for level 0, qp_solve_warp at <= 28 variables
-// for levels 1 and 2). Both cascades take a level through the same steps: the task residual (hoqp_task_residual), the normal equations
-// of its objective (hoqp_normal_eq), the update x += Z z (hoqp_update_x) and the null-space step (hoqp_null_space_step).
+// for levels 1 and 2; both are qp_mehrotra_warp with their own Newton systems). Both cascades take a level through the same steps: the task
+// residual (hoqp_task_residual), the normal equations of its objective (hoqp_normal_eq), the update x += Z z (hoqp_update_x) and the
+// null-space step (hoqp_null_space_step).
 #pragma once
 #include "hb_common.cuh"
 #include "hb_qp.cuh"
@@ -312,10 +313,9 @@ static_assert(4 * (hwbc_fused_bytes() + 1024) <= 228 * 1024, "hwbc_fused_kernel 
 // Level 0 of the cascade (Z = I, x_prev = 0) at its real shape. The lifted problem hoqp_solve_warp hands qp_solve_warp is, in x (38) and
 // one slack v_j per inequality row D_j of task0,
 //     min 1/2 x'G x + c'x + 1/2 v'v   s.t.  -v <= 0,  D x - v <= f,      G = A'A + 1e-12 I,  c = A'r  (r = -b)
-// This runs the same Mehrotra iteration as qp_solve_warp on it (start point, step rule, stopping test, status codes) without forming
-// the (38 + md)-square Newton matrix: its slack block is diagonal, d = 1 + rho + w_b + w_d (w = z / s of the two rows that hold v_j), so
-// the Newton step is the 38 x 38 Schur complement S = G + rho I + D' diag(w_d (1 + rho + w_b) / d) D, and D has at most 3 nonzeros per row.
-// x -> sh.x, v -> sh.v0.
+// qp_mehrotra_warp solves it with this Newton system, which never forms the (38 + md)-square matrix: its slack block is diagonal,
+// d = 1 + rho + w_b + w_d (w = z / s of the two rows that hold v_j), so the Newton step is the 38 x 38 Schur complement
+// S = G + rho I + D' diag(w_d (1 + rho + w_b) / d) D, and D has at most 3 nonzeros per row. x -> sh.x, v -> sh.v0.
 __device__ __noinline__ QpResult hwbc_level0_warp(HwbcShared& sh, int md, double rho, int max_iter, double* work) {
   const int lane = lane_id();
   constexpr int n = NWBC, ld = HW_LD0;
@@ -333,25 +333,18 @@ __device__ __noinline__ QpResult hwbc_level0_warp(HwbcShared& sh, int md, double
     return a;
   };
   hoqp_normal_eq<true>(sh.AZ, sh.r, HW_MA0, n, G, 0, c);
+  // start point x = 0, v = 0; the bound sums run over f0 in row order (the bounds of -v <= 0 are 0 and add nothing)
   double gs = 1.0, bs = 1.0, fsum = 0.0;
   for (int i = lane; i < n; i += 32) { sh.x[i] = 0.0; gs = fmax(gs, 1.0 + fabs(c[i])); }
   for (int j = lane; j < md; j += 32) { v[j] = 0.0; fsum += fabs(sh.f0[j]); bs = fmax(bs, 1.0 + fabs(sh.f0[j])); }
-  fsum = warp_sum(fsum);
-  const double theta = fmax(1.0, mi > 0 ? fsum / mi : 1.0);
-  for (int e = lane; e < mi; e += 32) { const double f = e < md ? 0.0 : sh.f0[e - md], se = fmax(theta, f); s[e] = se; z[e] = theta / se; }
-  gs = warp_max(gs); bs = warp_max(bs);
-  __syncwarp();
-  QpResult res{1, 0};
-  int it = 0;
-  for (; it < max_iter; ++it) {
-    // ---- residuals
+  auto residuals = [&](double& rdn, double& rpn) {
     for (int i = lane; i < n; i += 32) {
       double a = c[i] + rho * sh.x[i];
       for (int k = 0; k <= i; ++k) a += G[tri_row(i) + k] * sh.x[k];
       for (int k = i + 1; k < n; ++k) a += G[tri_row(k) + i] * sh.x[k];
       rdx[i] = dtmul(i, z + md, a);
     }
-    double sz = 0.0, rpn = 0.0, rdn = 0.0;
+    double sz = 0.0;
     for (int j = lane; j < md; j += 32) {
       rdv[j] = rho * v[j] + v[j] - z[j] - z[md + j];
       rs[j] = -v[j] + s[j];
@@ -361,10 +354,9 @@ __device__ __noinline__ QpResult hwbc_level0_warp(HwbcShared& sh, int md, double
     }
     __syncwarp();
     for (int i = lane; i < n; i += 32) rdn = fmax(rdn, fabs(rdx[i]));
-    rdn = warp_max(rdn); rpn = warp_max(rpn);
-    const double mu = mi > 0 ? warp_sum(sz) / mi : 0.0;
-    if (!(rdn == rdn) || !(rpn == rpn) || !(mu == mu) || rdn > 1e300 || rpn > 1e300) { res.status = 3; break; }
-    if (rdn < 1e-10 * gs && rpn < 1e-10 * bs && mu < 1e-12) { res.status = 0; break; }
+    return sz;
+  };
+  auto factor = [&]() {
     // ---- Schur complement S (lower triangle): lane c owns column c, so the rows sharing a column block never collide
     for (int j = lane; j < md; j += 32) {
       const double wb = z[j] / s[j], w = z[md + j] / s[md + j], d = 1.0 + rho + wb + w;
@@ -380,58 +372,36 @@ __device__ __noinline__ QpResult hwbc_level0_warp(HwbcShared& sh, int md, double
         for (int m = k; m < sh.dlen[j]; ++m) K[(sh.dc0[j] + m) * ld + col] += a * sh.dco[3 * j + m];
       }
     __syncwarp();
-    if (!warp_chol_inv(K, n, ld, kdi, lane, 1e-10)) { res.status = 2; break; }
-    // ---- Newton step for the complementarity target rc: dx, dv, ds, dz
-    auto newton = [&]() {
-      for (int e = lane; e < mi; e += 32) cw[e] = (rc[e] - z[e] * rs[e]) / s[e];
-      __syncwarp();
-      for (int j = lane; j < md; j += 32) { const double rv = -rdv[j] - cw[j] - cw[md + j]; dv[j] = rv; qv[j] = cw[md + j] + wd[j] * rv / dd[j]; }
-      __syncwarp();
-      for (int i = lane; i < n; i += 32) t2[i] = dtmul(i, qv, -rdx[i]);
-      __syncwarp();
-      warp_li_mv(K, n, ld, kdi, t2, t1, lane);
-      warp_lit_mv(K, n, ld, kdi, t1, dx, lane);
-      for (int j = lane; j < md; j += 32) {
-        const double ddx = drow(j, dx), dvj = (dv[j] + wd[j] * ddx) / dd[j];
-        dv[j] = dvj;
-        ds[j] = -rs[j] + dvj;
-        ds[md + j] = -rs[md + j] - (ddx - dvj);
-        dz[j] = -(rc[j] + z[j] * ds[j]) / s[j];
-        dz[md + j] = -(rc[md + j] + z[md + j] * ds[md + j]) / s[md + j];
-      }
-      __syncwarp();
-    };
-    auto max_step = [&]() {
-      double a = 1.0;
-      for (int e = lane; e < mi; e += 32) {
-        if (ds[e] < 0.0) a = fmin(a, -s[e] / ds[e]);
-        if (dz[e] < 0.0) a = fmin(a, -z[e] / dz[e]);
-      }
-      return warp_min(a);
-    };
-    for (int e = lane; e < mi; e += 32) rc[e] = s[e] * z[e];
+    return warp_chol_inv(K, n, ld, kdi, lane, 1e-10);
+  };
+  // ---- Newton step for the complementarity target rc: dx, dv, ds, dz
+  auto newton = [&]() {
+    for (int e = lane; e < mi; e += 32) cw[e] = (rc[e] - z[e] * rs[e]) / s[e];
     __syncwarp();
-    newton();
-    if (mi > 0) {
-      const double a_aff = max_step();
-      double ma = 0.0;
-      for (int e = lane; e < mi; e += 32) ma += (s[e] + a_aff * ds[e]) * (z[e] + a_aff * dz[e]);
-      ma = warp_sum(ma) / mi;
-      const double r = ma / mu;
-      const double sigma = r * r * r;
-      for (int e = lane; e < mi; e += 32) rc[e] = s[e] * z[e] + ds[e] * dz[e] - sigma * mu;
-      __syncwarp();
-      newton();
+    for (int j = lane; j < md; j += 32) { const double rv = -rdv[j] - cw[j] - cw[md + j]; dv[j] = rv; qv[j] = cw[md + j] + wd[j] * rv / dd[j]; }
+    __syncwarp();
+    for (int i = lane; i < n; i += 32) t2[i] = dtmul(i, qv, -rdx[i]);
+    __syncwarp();
+    warp_li_mv(K, n, ld, kdi, t2, t1, lane);
+    warp_lit_mv(K, n, ld, kdi, t1, dx, lane);
+    for (int j = lane; j < md; j += 32) {
+      const double ddx = drow(j, dx), dvj = (dv[j] + wd[j] * ddx) / dd[j];
+      dv[j] = dvj;
+      ds[j] = -rs[j] + dvj;
+      ds[md + j] = -rs[md + j] - (ddx - dvj);
+      dz[j] = -(rc[j] + z[j] * ds[j]) / s[j];
+      dz[md + j] = -(rc[md + j] + z[md + j] * ds[md + j]) / s[md + j];
     }
-    const double alpha = fmin(1.0, 0.995 * max_step());
+    __syncwarp();
+  };
+  auto step = [&](double alpha) {
     for (int i = lane; i < n; i += 32) sh.x[i] += alpha * dx[i];
     for (int j = lane; j < md; j += 32) v[j] += alpha * dv[j];
-    for (int e = lane; e < mi; e += 32) { s[e] += alpha * ds[e]; z[e] += alpha * dz[e]; }
-    __syncwarp();
-  }
+  };
+  const QpResult res = qp_mehrotra_warp(mi, max_iter, gs, bs, fsum, s, z, ds, dz, rc, [&](int e) { return e < md ? 0.0 : sh.f0[e - md]; },
+                                        residuals, factor, newton, step);
   for (int j = lane; j < md; j += 32) sh.v0[j] = v[j];
   __syncwarp();
-  res.iters = it;
   return res;
 }
 
