@@ -92,15 +92,50 @@ def test_fused_equals_composition_and_oracle(oracle, settings):
     ctx.close()
 
 
+def _bits(a):
+    return np.ascontiguousarray(a, dtype=np.float64).view(np.uint64)
+
+
 def test_task_weights_do_not_change_the_hierarchical_solution():
+    """HierarchicalWbc has no task weights: its tasks are the unweighted rows, so the weighted formulation's weights leave its problems
+    and its solution bit for bit unchanged."""
     ctx = hb.Context(horizon_N=4, dt=0.01, max_batch=8, device=0)
     x, u, rbd, mode = _wbc_cases(8, 6)
     s0, st0 = ctx.hierarchical_wbc_solve(x, u, rbd, mode)
+    t0 = [hb.hoqp_tasks(p) for p in ctx.hierarchical_wbc_tasks(x, u, rbd, mode)]
     _settings(ctx, weight_swing_leg=ctx.wbc_settings().weight_swing_leg * 7.0, weight_base_accel=ctx.wbc_settings().weight_base_accel * 0.3)
     s1, st1 = ctx.hierarchical_wbc_solve(x, u, rbd, mode)
+    t1 = [hb.hoqp_tasks(p) for p in ctx.hierarchical_wbc_tasks(x, u, rbd, mode)]
     assert (st0 == 0).all() and (st1 == 0).all()
+    assert np.array_equal(_bits(s1), _bits(s0)) and np.array_equal(st1, st0)
     for i in range(8):
-        assert _rel(s1[i], s0[i]) < 1e-4, i
+        for lvl in range(3):
+            for k in range(4):
+                assert np.array_equal(_bits(t1[i][lvl][k]), _bits(t0[i][lvl][k])), (i, lvl, k)
+    ctx.close()
+
+
+@pytest.mark.parametrize("settings", ["default", "non_default"])
+def test_weighted_constraints_are_the_hierarchical_task0_rows(settings):
+    """WeightedWbc's constraints and HierarchicalWbc's task0 come from the same task functions: the equality rows of
+    hb_wbc_assemble_batch (EoM, zero swing forces) and its inequality rows (torque limits, friction pyramid) equal, bit for bit and in
+    order, the first 16 + 3 nsw equalities and all the inequalities of task0 of hb_hierarchical_wbc_tasks_batch, in every mode, with and
+    without stance mode."""
+    ctx = hb.Context(horizon_N=4, dt=0.01, max_batch=8, device=0)
+    if settings == "non_default":
+        _settings(ctx, **NON_DEFAULT)
+    x, u, rbd, mode = _wbc_cases(8, 9)
+    _, _, A, lb, ub, m = ctx.wbc_assemble(x, u, rbd, mode, stance_mode=(np.arange(8) // 4) % 2)
+    pbs = ctx.hierarchical_wbc_tasks(x, u, rbd, mode)
+    for i in range(8):
+        a0, b0, d0, f0 = hb.hoqp_tasks(pbs[i])[0]
+        nsw = 4 - sum(sc.mode_flags(int(mode[i])))
+        eq, md0 = 16 + 3 * nsw, d0.shape[0]
+        assert m[i] == eq + md0 + 3 * nsw, i
+        assert np.array_equal(_bits(A[i, :eq]), _bits(a0[:eq])), i
+        assert np.array_equal(_bits(lb[i, :eq]), _bits(b0[:eq])) and np.array_equal(_bits(ub[i, :eq]), _bits(b0[:eq])), i
+        assert np.array_equal(_bits(A[i, eq:eq + md0]), _bits(d0)), i
+        assert np.array_equal(_bits(ub[i, eq:eq + md0]), _bits(f0)) and (lb[i, eq:eq + md0] == -1e20).all(), i
     ctx.close()
 
 
