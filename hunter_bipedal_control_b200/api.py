@@ -40,6 +40,7 @@ EXPORTED_SYMBOLS = [
     "hb_default_rollout_params", "hb_rollout_batch_dev", "hb_rollout_set_pushes", "hb_sim_step_wrench",
     "hb_default_plant_variation", "hb_rollout_set_plant_variations", "hb_sim_step_varied", "hb_rollout_set_terrains", "hb_sim_step_terrain",
     "hb_default_estimation_params", "hb_estimation_reset", "hb_sim_read_sensors_batch_dev", "hb_sim_read_sensors", "hb_rollout_estimated_batch_dev",
+    "hb_plan_references_targets", "hb_goal_to_target", "hb_plan_set_targets", "hb_rollout_set_goals",
 ]
 
 
@@ -65,6 +66,42 @@ class HbReference(C.Structure):
 class HbPlanInput(C.Structure):
     _fields_ = [("t0", C.c_double), ("horizon", C.c_double), ("time_to_target", C.c_double), ("gait_start", C.c_double), ("prev_event", C.c_double),
                 ("x0", C.c_double * 22), ("cmd_vel", C.c_double * 4), ("feet_pos", C.c_double * 12), ("gait", C.c_int32), ("joint_ik", C.c_int32)]
+
+
+class HbTarget(C.Structure):
+    _fields_ = [("n", C.c_int32), ("time", C.c_double * HB_MAX_TARGETS), ("state", (C.c_double * 22) * HB_MAX_TARGETS)]
+
+
+def make_targets(times, states):
+    """ctypes array of HbTarget (plan_references(targets=...), Context.set_plan_targets): instance i has the samples (times[i][k],
+    states[i][k]), k < n_i. times: B sequences of strictly ascending absolute times (1..HB_MAX_TARGETS each); states: B sequences of
+    22-vectors of the same lengths."""
+    B = len(times)
+    out = (HbTarget * B)()
+    v = np.ctypeslib.as_array(out)
+    for i in range(B):
+        t, x = _f64(times[i]).reshape(-1), _f64(states[i]).reshape(-1, 22)
+        n = len(t)
+        if not 1 <= n <= HB_MAX_TARGETS or x.shape[0] != n:
+            raise ValueError("targets: 1..%d samples with one state each expected, got %d times and %d states" % (HB_MAX_TARGETS, n, x.shape[0]))
+        v["n"][i] = n; v["time"][i, :n] = t; v["state"][i, :n] = x
+    return out
+
+
+def reference_target(ref):
+    """The target trajectory an HbReference carries (its target samples) as an HbTarget."""
+    n = ref.n_targets
+    return make_targets([np.array(ref.target_times[:n])], [np.array([ref.target_states[k][:] for k in range(n)])])[0]
+
+
+def goal_to_target(t, x, goal):
+    """goalToTargetTrajectories (hb_goal_to_target) for a batch: t (B,) or a scalar, x (B, 22), goal (B, 3) = (x, y, yaw) or (3,).
+    Returns a ctypes array of B HbTarget."""
+    x = _f64(x).reshape(-1, NX); B = x.shape[0]
+    t = _f64(np.broadcast_to(_f64(t), (B,))); goal = _f64(np.broadcast_to(_f64(goal), (B, 3)))
+    out = (HbTarget * B)()
+    _check(load_library().hb_goal_to_target(B, _ptr(t), _ptr(x), _ptr(goal), out), "hb_goal_to_target")
+    return out
 
 
 class HbPdGains(C.Structure):
@@ -348,6 +385,38 @@ def make_terrains(B, heights, spacing, origin=(0.0, 0.0)):
     return out
 
 
+HB_MAX_GOALS = 8
+
+
+class HbGoalSchedule(C.Structure):
+    _fields_ = [("n_goal", C.c_int32), ("time", C.c_double * HB_MAX_GOALS), ("goal", (C.c_double * 3) * HB_MAX_GOALS)]
+
+
+def make_goal_schedules(B, times, goals):
+    """ctypes array of B HbGoalSchedule (Context.set_goals). Goal j of instance i, the world pose goals[i, j] = (x, y, yaw), comes into
+    force on the first MPC tick with t >= times[i, j]. times: (B, n), (n,) or a scalar, ascending; goals: (B, n, 3), (n, 3) or (3,);
+    n <= HB_MAX_GOALS (n = 0: no goals). Raises ValueError for what hb_rollout_set_goals rejects."""
+    tim, gol = _f64(times), _f64(goals)
+    dims = [tim.shape[-1]] if tim.ndim >= 1 else []
+    dims += [gol.shape[-2]] if gol.ndim >= 2 else []
+    n = max(dims) if dims else 1
+    if not 0 <= n <= HB_MAX_GOALS:
+        raise ValueError("goal schedules: at most %d goals per instance, got %d" % (HB_MAX_GOALS, n))
+    try:
+        tim = np.broadcast_to(tim, (B, n)); gol = np.broadcast_to(gol, (B, n, 3))
+    except ValueError as e:
+        raise ValueError("goal schedules: times (B, n), goals (B, n, 3) expected: %s" % e)
+    if not (np.isfinite(tim).all() and np.isfinite(gol).all()):
+        raise ValueError("goal schedules: times and goals must be finite")
+    if (np.diff(tim, axis=1) < 0).any():
+        raise ValueError("goal schedules: times must be ascending")
+    out = (HbGoalSchedule * B)()
+    v = np.ctypeslib.as_array(out)
+    v["n_goal"] = n
+    v["time"][:, :n] = tim; v["goal"][:, :n] = gol
+    return out
+
+
 class HbObserverState(C.Structure):
     _fields_ = [("p_filtered", C.c_double * 16)]
 
@@ -475,14 +544,19 @@ def plan_set_threads(n):
     _check(load_library().hb_plan_set_threads(int(n)), "hb_plan_set_threads")
 
 
-def plan_references(t0, horizon, x0, cmd_vel, feet_pos, gait, gait_start, prev_event=None, time_to_target=None, latest_stance=None, joint_ik=True):
-    """Host-side reference planner (hb_plan_references): returns (ctypes array of HbReference, latest_stance[B,12])."""
+def plan_references(t0, horizon, x0, cmd_vel, feet_pos, gait, gait_start, prev_event=None, time_to_target=None, latest_stance=None, joint_ik=True,
+                    targets=None):
+    """Host-side reference planner (hb_plan_references): returns (ctypes array of HbReference, latest_stance[B,12]). targets: B HbTarget
+    (make_targets, goal_to_target) planned on instead of the cmd_vel targets (hb_plan_references_targets); cmd_vel still drives the swing
+    planner."""
     lib = load_library()
     ins = make_plan_inputs(t0, horizon, x0, cmd_vel, feet_pos, gait, gait_start, prev_event, time_to_target, joint_ik)
     B = len(ins)
+    if targets is not None and len(targets) != B:
+        raise ValueError("plan_references: %d targets for %d instances" % (len(targets), B))
     ls = np.zeros((B, 12)) if latest_stance is None else _f64(latest_stance).copy()
     refs = (HbReference * B)()
-    _check(lib.hb_plan_references(B, ins, _ptr(ls), refs), "hb_plan_references")
+    _check(lib.hb_plan_references_targets(B, ins, targets, _ptr(ls), refs), "hb_plan_references_targets")
     return refs, ls
 
 
@@ -819,6 +893,17 @@ class Context:
         """Push schedules of this context's episodes (hb_rollout_set_pushes): schedules[i] (make_push_schedules) acts on instance i of every
         later rollout / rollout_estimated call, instances beyond len(schedules) are not pushed; None clears them."""
         self._set_instances("hb_rollout_set_pushes", schedules)
+
+    def set_goals(self, schedules):
+        """Goal schedules of this context's episodes (hb_rollout_set_goals): schedules[i] (make_goal_schedules) sends instance i of every
+        later rollout / rollout_estimated call to its goal poses, each converted once into a target (goal_to_target) on the MPC tick it comes
+        into force; instances beyond len(schedules) follow their cmd_vel; None clears them. Every call forgets the captured goals."""
+        self._set_instances("hb_rollout_set_goals", schedules)
+
+    def set_plan_targets(self, targets):
+        """Explicit planner targets of this context (hb_plan_set_targets): targets[i] (make_targets, goal_to_target) replaces the cmd_vel
+        target of instance i in plan_references_gpu and resident_plan_cycle (not in the episodes); None clears them."""
+        self._set_instances("hb_plan_set_targets", targets)
 
     def resident_wbc(self, t_now, rbd, stance_mode=None):
         """Policy of the resident solution at absolute time t_now + WeightedWbc: returns (x_des, u_des, mode, sol, torque, status)."""

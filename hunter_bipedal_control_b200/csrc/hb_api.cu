@@ -82,6 +82,13 @@ struct hb_ctx {
   InstanceSetting<hb_push_schedule> pushes;
   InstanceSetting<hb_plant_variation> variations;
   InstanceSetting<hb_terrain> terrains;
+  InstanceSetting<hb_goal_schedule> goals;
+  // the goal each instance of the episodes captured (index, -1: none) and its target, allocated at max_batch by the first
+  // hb_rollout_set_goals that sets schedules
+  void* goal_mem;
+  hb_target* goal_tg; int32_t* goal_idx;
+  // the planner's explicit targets (hb_plan_set_targets), read by the planner calls outside the episodes
+  InstanceSetting<hb_target> plan_targets;
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
   // hb_resident_cycle_batch's packed references / reference verdicts
   void* arena; size_t arena_cap;
@@ -441,7 +448,7 @@ int hb_destroy(hb_ctx* ctx) {
   void* ptrs[] = {ctx->sqp_mem, ctx->dxt, ctx->dut, ctx->perf, ctx->flags, ctx->xdes, ctx->udes, ctx->wstatus, ctx->witers, ctx->wmode,
                   ctx->hoqp_mem, ctx->cyc_xref, ctx->cyc_swing, ctx->cyc_tk, ctx->cyc_mode, ctx->cyc_nn, ctx->res_t0, ctx->res_xt,
                   ctx->res_ut, ctx->res_tk, ctx->res_mode, ctx->res_nn, ctx->res_sol, ctx->res_stance, ctx->arena, ctx->ro_mem, ctx->re_mem,
-                  ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev};
+                  ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->goal_mem, ctx->plan_targets.dev};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -711,11 +718,24 @@ int hb_resident_cycle_batch_dev(hb_ctx* ctx, int B, int cold_start, double t_rel
   return resident_cycle_impl(ctx, B, cold_start, t_rel, t0, x0, refs, rbd, info, wbc_sol, torque, wbc_status, true);
 }
 
+static const hbplan::PlanConsts& plan_consts() {
+  static const hbplan::PlanConsts pc = hbplan::make_consts();
+  return pc;
+}
+
+// The device planner after the entry checks: instance i < n_targets plans on targets[i] where captured is null or captured[i] >= 0
+static int plan_dev(hb_ctx* ctx, int B, const hb_plan_input* in, const double* feet, double* latest_stance, hb_reference* out, int32_t* status,
+                    const hb_target* targets, const int32_t* captured, int n_targets) {
+  return launch(ctx, K_UNPROFILED, plan_references_coop_kernel, (B + 7) / 8, 32, 0, B, in, feet, latest_stance, out, status, plan_consts(), targets,
+                captured, n_targets);
+}
+
 int hb_plan_references_batch_dev(hb_ctx* ctx, int B, const hb_plan_input* in, const double* feet, double* latest_stance, hb_reference* out,
                                  int32_t* status) {
   ENTER(ctx, B, in && latest_stance && out, UNCAPPED);
-  static const hbplan::PlanConsts pc = hbplan::make_consts();
-  return launch(ctx, K_UNPROFILED, plan_references_coop_kernel, (B + 7) / 8, 32, 0, B, in, feet, latest_stance, out, status, pc);
+  // the explicit targets of the instances this call plans (a chunk of a host-pointer call starts at instance ctx->base)
+  const int n_tg = ctx->plan_targets.n - ctx->base;
+  return plan_dev(ctx, B, in, feet, latest_stance, out, status, n_tg > 0 ? ctx->plan_targets.dev + ctx->base : nullptr, nullptr, n_tg);
 }
 
 int hb_default_kf_params(hb_kf_params* p) {
@@ -969,6 +989,42 @@ int hb_rollout_set_plant_variations(hb_ctx* ctx, int B, const hb_plant_variation
 }
 int hb_rollout_set_terrains(hb_ctx* ctx, int B, const hb_terrain* t) { return set_instances(ctx, B, t, terrain_ok, &hb_ctx::terrains); }
 
+// The ranges of hunter_b200.h's hb_goal_schedule: the count, finite times in ascending order, finite goals
+static bool goal_schedule_ok(const hb_goal_schedule& s) {
+  if (s.n_goal < 0 || s.n_goal > HB_MAX_GOALS) return false;
+  for (int j = 0; j < s.n_goal; ++j) {
+    if (!isfinite(s.time[j]) || (j > 0 && s.time[j] < s.time[j - 1])) return false;
+    for (int c = 0; c < 3; ++c) if (!isfinite(s.goal[j][c])) return false;
+  }
+  return true;
+}
+
+int hb_rollout_set_goals(hb_ctx* ctx, int B, const hb_goal_schedule* g) {
+  int rc = set_instances(ctx, B, g, goal_schedule_ok, &hb_ctx::goals);
+  if (rc || ctx->goals.n == 0) return rc;
+  const size_t Bc = ctx->cfg.max_batch;
+  rc = reserve_group(&ctx->goal_mem, [&](void* m) {
+    size_t off = 0;
+    ctx->goal_tg = carve<hb_target>(m, off, Bc); ctx->goal_idx = carve<int32_t>(m, off, Bc);
+    return off;
+  });
+  if (rc) { ctx->goals.n = 0; return rc; }
+  CK(cudaMemsetAsync(ctx->goal_idx, 0xff, sizeof(int32_t) * Bc, ctx->stream));     // every captured goal forgotten: index -1
+  return HB_OK;
+}
+
+// The ranges of hunter_b200.h's hb_target: the sample count, strictly ascending finite times, finite states in the used samples
+static bool target_ok(const hb_target& tg) {
+  if (tg.n < 1 || tg.n > HB_MAX_TARGETS) return false;
+  for (int k = 0; k < tg.n; ++k) {
+    if (!isfinite(tg.time[k]) || (k > 0 && !(tg.time[k] > tg.time[k - 1]))) return false;
+    for (int i = 0; i < 22; ++i) if (!isfinite(tg.state[k][i])) return false;
+  }
+  return true;
+}
+
+int hb_plan_set_targets(hb_ctx* ctx, int B, const hb_target* t) { return set_instances(ctx, B, t, target_ok, &hb_ctx::plan_targets); }
+
 // hb_resident_wbc_batch_dev; no_prev = true: the fallback has no previous solution yet (first tick after a cold start whose cycle ran no WBC)
 static int resident_wbc_impl(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
                              int32_t* mode_out, double* wbc_sol, double* torque, int32_t* wbc_status, bool no_prev) {
@@ -1064,6 +1120,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   const hb_plant_variation* var = ctx->variations.get();
   const hb_terrain* ter = ctx->terrains.get();
   double* wrench = push ? ctx->ro_wrench : nullptr;
+  const hb_goal_schedule* goals = ctx->goals.get();          // with goals, the plan-input kernel captures them and the planner reads the captures
   for (int k = 0; k < n_ticks && !rc; ++k) {
     const int64_t a = tick0 + k;
     const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
@@ -1082,9 +1139,11 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
     }
     if (!rc && mpc) {
       if (first_cold) CK(cudaMemsetAsync(ctx->res_stance, 0, sizeof(double) * B * 12, ctx->stream));   // latestStanceposition_ starts at zero
-      rc = launch(ctx, K_UNPROFILED, rollout_plan_inputs_kernel, grid, 64, 0, B, t, horizon, ctx->ro_cmd, meas, e ? e->est : nullptr, ctx->ro_in);
+      rc = launch(ctx, K_UNPROFILED, rollout_plan_inputs_kernel, grid, 64, 0, B, t, horizon, ctx->ro_cmd, meas, e ? e->est : nullptr, ctx->ro_in, goals,
+                  ctx->goals.n, first_cold ? 1 : 0, ctx->goal_tg, ctx->goal_idx, plan_consts());
       if (!rc) rc = launch(ctx, K_UNPROFILED, plan_prepare_kernel, grid, 64, 0, B, ctx->ro_in, ctx->ro_t0, ctx->ro_x0, ctx->ro_feet);
-      if (!rc) rc = hb_plan_references_batch_dev(ctx, B, ctx->ro_in, ctx->ro_feet, ctx->res_stance, ctx->ro_refs, ctx->ro_pstat);
+      if (!rc) rc = plan_dev(ctx, B, ctx->ro_in, ctx->ro_feet, ctx->res_stance, ctx->ro_refs, ctx->ro_pstat, goals ? ctx->goal_tg : nullptr, ctx->goal_idx,
+                             ctx->goals.n);
       if (!rc) rc = resident_cycle_impl(ctx, B, first_cold, 0.0, ctx->ro_t0, ctx->ro_x0, ctx->ro_refs, meas, ctx->ro_info, nullptr, nullptr, nullptr, false);
       if (!rc && e) rc = launch(ctx, K_UNPROFILED, est_schedule_kernel, grid, 64, 0, B, ctx->ro_refs, e->est);
     }
@@ -1565,10 +1624,10 @@ int hb_contact_positions_batch(hb_ctx* ctx, int B, const double* x, double* pos)
 }
 
 static std::atomic<int> g_plan_threads{0};   // 0 = hardware_concurrency (hb_plan_set_threads)
-static int plan_range(int lo, int hi, const hb_plan_input* in, double* latest_stance, hb_reference* out) {
-  static const hbplan::PlanConsts pc = hbplan::make_consts();
+static int plan_range(int lo, int hi, const hb_plan_input* in, const hb_target* targets, double* latest_stance, hb_reference* out) {
+  const hbplan::PlanConsts& pc = plan_consts();
   for (int i = lo; i < hi; ++i) {
-    const int rc = hbplan::plan_one(pc, in[i], latest_stance + (size_t)i * 12, out + i, true);
+    const int rc = hbplan::plan_one(pc, in[i], targets ? targets + i : nullptr, latest_stance + (size_t)i * 12, out + i, true);
     if (rc) return rc;
   }
   return HB_OK;
@@ -1581,20 +1640,39 @@ int hb_plan_set_threads(int n_threads) {
 }
 
 int hb_plan_references(int B, const hb_plan_input* in, double* latest_stance, hb_reference* out) {
-  if (B < 0 || !in || !latest_stance || !out) return HB_EINVAL;
+  return hb_plan_references_targets(B, in, nullptr, latest_stance, out);
+}
+
+int hb_plan_references_targets(int B, const hb_plan_input* in, const hb_target* targets, double* latest_stance, hb_reference* out) {
+  if (B < 0 || !in || !latest_stance || !out || !all_ok(B, targets, target_ok)) return HB_EINVAL;
   // instances are independent: spread them over the host cores (the planner feeds ~1e5 solves/s per GPU; one core plans ~2e4/s)
   unsigned hw = std::thread::hardware_concurrency();
   if (const int forced = g_plan_threads.load()) hw = (unsigned)forced;
   int nt = (int)std::min<unsigned>(hw ? hw : 1u, (unsigned)((B + 63) / 64));
-  if (nt <= 1) return plan_range(0, B, in, latest_stance, out);
+  if (nt <= 1) return plan_range(0, B, in, targets, latest_stance, out);
   std::vector<std::thread> pool;
   std::vector<int> rcs(nt, HB_OK);
   for (int t = 0; t < nt; ++t) {
     const int lo = (int)((long long)B * t / nt), hi = (int)((long long)B * (t + 1) / nt);
-    pool.emplace_back([=, &rcs]() { rcs[t] = plan_range(lo, hi, in, latest_stance, out); });
+    pool.emplace_back([=, &rcs]() { rcs[t] = plan_range(lo, hi, in, targets, latest_stance, out); });
   }
   for (auto& th : pool) th.join();
   for (int t = 0; t < nt; ++t) if (rcs[t]) return rcs[t];
+  return HB_OK;
+}
+
+int hb_goal_to_target(int B, const double* t, const double* x, const double* goal, hb_target* out) {
+  if (B < 0 || !t || !x || !goal || !out) return HB_EINVAL;
+  for (int i = 0; i < B; ++i) {
+    const double* xi = x + (size_t)i * NX; const double* gi = goal + (size_t)i * 3;
+    if (!isfinite(t[i]) || !isfinite(xi[6]) || !isfinite(xi[7]) || !isfinite(xi[8]) || !isfinite(xi[9]) || !isfinite(gi[0]) || !isfinite(gi[1]) ||
+        !isfinite(gi[2]))
+      return HB_EINVAL;
+  }
+  for (int i = 0; i < B; ++i) {
+    memset(&out[i], 0, sizeof(hb_target));
+    hbplan::goal_to_target(plan_consts(), t[i], x + (size_t)i * NX, goal + (size_t)i * 3, out[i]);
+  }
   return HB_OK;
 }
 

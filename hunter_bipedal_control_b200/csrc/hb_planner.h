@@ -134,6 +134,44 @@ HBP_HD inline Target cmd_vel_to_target(const PlanConsts& pc, const double* cmd /
   return tg;
 }
 
+// a product rounded on its own: never contracted into an fma by the device compiler, so host and device round alike
+HBP_HD inline double mul_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+
+// goalToTargetTrajectories with estimateTimeToTarget (TargetTrajectoriesPublisher.cpp:29-38, :83-100) and targetPoseToTargetTrajectories
+// (:41-62), written into a caller's hb_target (the device capture writes global memory, not a stack copy). The yaw difference is not
+// wrapped, as in the reference. A zero reaching time would give two samples at one time: the single target sample is kept instead.
+HBP_HD inline void goal_to_target(const PlanConsts& pc, double time, const double* state, const double* goal /*x, y, yaw*/, hb_target& tg) {
+  const double* pose = state + 6;
+  double dz = HB_COM_HEIGHT - pose[2];
+  dz = dz > 0 ? dmin(dz, 0.04) : dmax(dz, -0.04);      // changeLimit_[2] (TargetTrajectoriesPublisher.h:97)
+  const double z = pose[2] + dz;
+  const double dx = goal[0] - pose[0], dy = goal[1] - pose[1];
+  const double reach = dmax(fabs(goal[2] - pose[3]) / HB_TARGET_ROTATION_VELOCITY, sqrt(mul_rn(dx, dx) + mul_rn(dy, dy)) / HB_TARGET_DISPLACEMENT_VELOCITY);
+  const double cur[6] = {pose[0], pose[1], z, pose[3], 0.0, 0.0}, target[6] = {goal[0], goal[1], z, goal[2], 0.0, 0.0};
+  tg.n = reach > 0.0 ? 2 : 1;
+  tg.time[0] = time; tg.time[1] = time + reach;
+  for (int k = 0; k < tg.n; ++k) {
+    const double* p = (tg.n == 1 || k == 1) ? target : cur;
+    for (int i = 0; i < 6; ++i) { tg.state[k][i] = 0.0; tg.state[k][6 + i] = p[i]; }
+    for (int j = 0; j < 10; ++j) tg.state[k][12 + j] = pc.default_joints[j];
+  }
+}
+
+// the planner's copy of a caller's target (its n samples; n clamped to the capacity, so that a malformed record cannot index out of bounds)
+HBP_HD inline void target_from(const hb_target& src, Target& tg) {
+  tg.n = src.n < 1 ? 1 : (src.n > HB_MAX_TARGETS ? HB_MAX_TARGETS : src.n);
+  for (int k = 0; k < tg.n; ++k) {
+    tg.t[k] = src.time[k];
+    for (int i = 0; i < 22; ++i) tg.x[k][i] = src.state[k][i];
+  }
+}
+
 // TargetTrajectories::getDesiredState: piecewise-linear, clamped at both ends
 HBP_HD inline void target_state(const Target& tg, double t, double* x) {
   if (tg.n <= 1 || t <= tg.t[0]) { memcpy(x, tg.x[0], sizeof(double) * 22); return; }
@@ -584,16 +622,20 @@ HBP_HD inline int write_schedule_and_targets(const ModeSchedule& ms, const Targe
   return 0;
 }
 
-// One instance, start to finish: schedule, target, swing planner, IK joint references, compact output.
+// One instance, start to finish: schedule, target (the given one, or the cmd_vel target when target is null), swing planner, IK joint
+// references, compact output.
 // Returns 0, -1 (invalid input) or -5 (schedule / reference capacity exceeded, or a swing phase without take-off / touch-down time).
-HBP_HD inline int plan_one(const PlanConsts& pc, const hb_plan_input& p, double* latest_stance /*12, in/out*/, hb_reference* out, bool zero_fill) {
+HBP_HD inline int plan_one(const PlanConsts& pc, const hb_plan_input& p, const hb_target* target, double* latest_stance /*12, in/out*/, hb_reference* out,
+                           bool zero_fill) {
   if (!(p.horizon > 0.0) || !(p.prev_event < p.gait_start) || p.gait < 0 || p.gait > 3) return -1;
   const double tf = p.t0 + p.horizon;
   if (zero_fill) memset(out, 0, sizeof(*out));
   ModeSchedule ms;
   // the reference tiles over [t0 - T, tf + T] (SwitchedModelReferenceManager.cpp:147)
   if (!tile_gait(p.gait, p.prev_event, p.gait_start, p.t0 - p.horizon, tf + p.horizon, ms)) return -5;
-  Target tg = cmd_vel_to_target(pc, p.cmd_vel, p.t0, p.x0, p.time_to_target);
+  Target tg;
+  if (target) target_from(*target, tg);
+  else tg = cmd_vel_to_target(pc, p.cmd_vel, p.t0, p.x0, p.time_to_target);
   const double body_vel_cmd[6] = {p.cmd_vel[0], p.cmd_vel[1], p.cmd_vel[2], p.cmd_vel[3], 0.0, 0.0};
   SwingOut so{out, p.t0 - 1e-9, tf + 1e-9, false};
   for (int c = 0; c < 4; ++c) for (int a = 0; a < 3; ++a) out->n_segments[c][a] = 0;

@@ -13,8 +13,11 @@ namespace hb {
 // cmd_vel of the last command segment that has started (the first one before that), prev_event = min(t, gait_start) - 0.5, IK joint
 // references. feet_pos is left zero: plan_prepare_kernel computes the feet from x0. With est (estimated episodes) x0[9] is the unwrapped
 // observation yaw (LeggedController.cpp:335-337).
+// Goals (hb_goal_schedule, hunter_b200.h) of instances inst < n_goals: the goal in force at t is captured, target and index, when it differs
+// from the captured one (captured_idx -1: none); reset (an episode's tick 0) forgets the captured goal first. The planner reads them.
 __global__ void rollout_plan_inputs_kernel(int B, double t, double horizon, const hb_rollout_command* cmd, const double* rbd, const hb_estimation_state* est,
-                                           hb_plan_input* in) {
+                                           hb_plan_input* in, const hb_goal_schedule* goals, int n_goals, int reset, hb_target* captured,
+                                           int32_t* captured_idx, hbplan::PlanConsts pc) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
   const hb_rollout_command& c = cmd[inst];
@@ -28,6 +31,14 @@ __global__ void rollout_plan_inputs_kernel(int B, double t, double horizon, cons
   if (est) p.x0[9] = est[inst].yaw_obs;
   for (int i = 0; i < 12; ++i) p.feet_pos[i] = 0.0;
   p.gait = c.gait; p.joint_ik = 1;
+  if (goals && inst < n_goals) {
+    const hb_goal_schedule& s = goals[inst];
+    int g = -1;
+    for (int k = 0; k < s.n_goal; ++k) if (s.time[k] <= t) g = k;
+    const int had = reset ? -1 : captured_idx[inst];
+    if (g >= 0 && g != had) hbplan::goal_to_target(pc, t, p.x0, s.goal[g], captured[inst]);
+    captured_idx[inst] = g >= 0 ? g : had;
+  }
 }
 
 // One axis of a terrain lookup (terrain, hunter_b200.h): the grid coordinate of the world coordinate x, clamped to [0, n - 1], split into

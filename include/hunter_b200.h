@@ -99,6 +99,15 @@ typedef struct {
                              SwitchedModelReferenceManager.cpp:251-300); 0: keep the two-sample target with default joints */
 } hb_plan_input;
 
+/* A target trajectory of one instance (the TargetTrajectories the planner tracks: the two-sample target cmdVelToTargetTrajectories or
+ * goalToTargetTrajectories publishes, or any other): piecewise-linear in time between the samples, held before the first and after the
+ * last. The input trajectory is zero, as in every target the reference publishes. */
+typedef struct {
+  int32_t n;                              /* samples, 1..HB_MAX_TARGETS                                            */
+  double time[HB_MAX_TARGETS];            /* absolute times, strictly ascending                                    */
+  double state[HB_MAX_TARGETS][22];       /* state samples (layout of x)                                           */
+} hb_target;
+
 /* state of the speed-based gait selection of one instance (SwitchedModelReferenceManager velAbsHistory_/velAvg_/gaitLevel_);
  * zero-initialise, then set gait_level = -1 ("no template chosen yet") or the level in force */
 typedef struct {
@@ -334,6 +343,27 @@ typedef struct {                      /* the ground under one robot: a height fi
  * samples. */
 int hb_rollout_set_terrains(hb_ctx* ctx, int B, const hb_terrain* t);
 
+/* ---- goals: a schedule of goal poses per robot, the reference's /move_base_simple/goal command (goalToTargetTrajectories) ----
+ * Which goal is in force: on an MPC tick at time t, goal j is in force when j is the last index with time[j] <= t.
+ * Capture: when the goal in force differs from the one the instance last captured, that tick builds the target once,
+ * hb_goal_to_target(t, x0, goal[j]), with x0 the tick's plan-input state (the true state, or in estimated episodes the estimate with
+ * x0[9] = yaw_obs), and the instance captures it. This is the publisher's behaviour: it converts a goal once, on the observation it
+ * holds when the goal arrives.
+ * Later MPC ticks plan on the captured target until another goal comes into force (the swing planner still reads the command's cmd_vel,
+ * as the reference reads /cmd_vel_filtered apart from the target). Before its first goal an instance plans on its cmd_vel target.
+ * The captured target and goal index are per-instance context state, like the planner's latest stance positions: they are cleared by an
+ * episode call with tick0 == 0 and by every hb_rollout_set_goals call, so a split episode continues exactly. An instance without goals
+ * (n_goal == 0, or at or beyond B) runs exactly as with no goals set. Goals add no launch to an episode. */
+#define HB_MAX_GOALS 8
+typedef struct {                      /* the goal poses of one robot                                                          */
+  int32_t n_goal;                     /* 0..HB_MAX_GOALS                                                                       */
+  double time[HB_MAX_GOALS];          /* absolute time [s] the goal is given, ascending                                        */
+  double goal[HB_MAX_GOALS][3];       /* world x, y [m] and yaw [rad], the yaw in the unwrapped convention of x[9]             */
+} hb_goal_schedule;
+/* Sets the goal schedules of the context's episodes (a per-robot episode setting, above) and clears every captured goal. -1 also for
+ * n_goal outside 0..HB_MAX_GOALS, a non-finite time or goal entry, times that descend. */
+int hb_rollout_set_goals(hb_ctx* ctx, int B, const hb_goal_schedule* goals);
+
 /* ---- estimated episodes (hb_rollout_estimated_batch_dev): the controllers read the Kalman filter's estimate from synthesised, noisy
  * sensors instead of the plant's true state (LeggedController::updateStateEstimation, LeggedController.cpp:280-349) ---- */
 typedef struct {                 /* standard deviations of additive Gaussian sensor noise; 0 = that channel is exact and draws nothing */
@@ -463,6 +493,13 @@ int hb_resident_cycle_batch_dev(hb_ctx* ctx, int B, int cold_start, double t_rel
  * overrides in[i].feet_pos (B x 12, e.g. from hb_contact_positions_batch_dev); status[i] = 0, -1 or -5 like hb_plan_references. */
 int hb_plan_references_batch_dev(hb_ctx* ctx, int B, const hb_plan_input* in, const double* feet, double* latest_stance,
                                  hb_reference* out, int32_t* status /*nullable*/);
+/* Explicit planner targets of the context (hb_plan_references_targets on the device): while set, hb_plan_references_batch_dev,
+ * hb_plan_references_gpu and hb_resident_plan_cycle_batch plan instance i < B on targets[i] instead of its cmd_vel target; instances at
+ * or beyond B keep theirs. The episode calls do not read it (they take goals, hb_rollout_set_goals). Setting conventions of the
+ * per-robot episode settings (below): host array validated and copied in stream order, B == 0 clears, -4 for B > max_batch, a rejected
+ * call keeps the previous setting. -1 also for n outside 1..HB_MAX_TARGETS, times that are not strictly ascending, a non-finite
+ * time[k] or state[k][.] with k < n. */
+int hb_plan_set_targets(hb_ctx* ctx, int B, const hb_target* targets);
 /* One estimator update per instance (StateEstimateBase::updateJointStates / updateImu, StateEstimateBase.cpp:73-106, then
  * KalmanFilterEstimate::update): quat = (x, y, z, w); contact_flag: B x 4 (0 = the filter distrusts that foot, x100 noise);
  * rbd_out: B x 32 measured rbd state [zyx, p, q_j, omega_world, v, qd_j]. The odometry topic fusion (updateFromTopic) is ROS glue
@@ -625,6 +662,18 @@ int hb_contact_positions_batch(hb_ctx* ctx, int B, const double* x, double* pos 
  * throws there, SwingTrajectoryPlanner.cpp:421-458) or exceeds the capacity of hb_reference.
  * Instances are spread over std::thread::hardware_concurrency() host threads (hb_plan_set_threads overrides the count). */
 int hb_plan_references(int B, const hb_plan_input* in, double* latest_stance, hb_reference* out);
+/* hb_plan_references with an explicit target per instance: targets (B, nullable) replaces cmdVelToTargetTrajectories for every instance,
+ * everything else unchanged (the swing planner still reads cmd_vel as its body velocity command; with joint_ik the target is resampled and
+ * its joints filled by IK). NULL is hb_plan_references. -1 also for a record that hb_plan_set_targets rejects. */
+int hb_plan_references_targets(int B, const hb_plan_input* in, const hb_target* targets, double* latest_stance, hb_reference* out);
+/* goalToTargetTrajectories (TargetTrajectoriesPublisher.cpp:83-100, with estimateTimeToTarget :29-38 and
+ * targetPoseToTargetTrajectories :41-62) for the observation (t[i], x[i]) and goal[i] = (x, y, yaw), host only. With p = x[6:12] and
+ * z' = p[2] + clamp(HB_COM_HEIGHT - p[2], -0.04, 0.04): sample 0 = (t, [0 (6), p[0], p[1], z', p[3], 0, 0, default joints]), sample 1 =
+ * (t + T, [0 (6), goal x, goal y, z', goal yaw, 0, 0, default joints]) with T = max(|goal yaw - p[3]| / HB_TARGET_ROTATION_VELOCITY,
+ * sqrt(dx^2 + dy^2) / HB_TARGET_DISPLACEMENT_VELOCITY), each square rounded before the sum. The yaw difference is not wrapped, as in the
+ * reference: the goal yaw is absolute in the unwrapped convention of x[9]. T == 0 gives the single sample 1 at time t (n = 1) where the
+ * reference would publish two samples at the same time. -1 for a NULL pointer, B < 0 or a non-finite t, x[6:10] or goal. */
+int hb_goal_to_target(int B, const double* t, const double* x /*B x 22*/, const double* goal /*B x 3*/, hb_target* out);
 /* Host threads used by hb_plan_references (process-wide); 0 = hardware_concurrency. The result does not depend on the count. */
 int hb_plan_set_threads(int n_threads);
 /* speed-based gait selection (calculateVelAbs + walkGait / trotGait, src/SwitchedModelReferenceManager.cpp:185-249): updates the

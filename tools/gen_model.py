@@ -223,6 +223,8 @@ def main():
         ("HB_FEET_BIAS_Z", info_scalar(info_block(ts, "swing_trajectory_config"), "feet_bias_z")),
         ("HB_NEXT_POSITION_Z", 0.02),   # SwingTrajectoryPlanner.h:70 default (key mismatch in task.info, SURVEY App. A)
         ("HB_COM_HEIGHT", info_scalar(rs, "comHeight")),
+        ("HB_TARGET_DISPLACEMENT_VELOCITY", info_scalar(rs, "targetDisplacementVelocity")),   # goal reaching time (TargetTrajectoriesPublisher.cpp:29-38)
+        ("HB_TARGET_ROTATION_VELOCITY", info_scalar(rs, "targetRotationVelocity")),
     ]
     for k, v in scal:
         o.append("#define %s %.17g\n" % (k, v))
