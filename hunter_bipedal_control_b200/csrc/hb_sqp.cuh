@@ -966,18 +966,103 @@ __device__ __forceinline__ void rowmm_by(double* __restrict__ C, int ldc, int m,
   __syncwarp();
 }
 
-template <int N, bool TA, int MODE, bool TC = false>
-__device__ __forceinline__ void rowmm(double* __restrict__ C, int ldc, const double* __restrict__ A, int lda,
-                                      const double* __restrict__ B, int ldb, int m, int kdim) {
-  rowmm_by<N, MODE, TC>(C, ldc, m, [&](double (&c)[N], int i) { acc_rows(c, [&](int k) { return TA ? A[k * lda + i] : A[i * lda + k]; }, B, ldb, kdim); });
+// Tile products, for the 22 x 22 results of the node: the lanes form a grid of 32 / GJ x GJ, and lane (li, lj) owns the TI x TJ block
+// of the result at row li * TI, column lj * TJ. Both operands are k-major (L[k * ldl + i], R[k * ldr + j]), so per k a lane loads the
+// TI and TJ consecutive entries under its block (the right span with 128-bit loads when TJ is even) and issues TI * TJ DFMAs: 5 loads
+// for 12 DFMAs with 3 x 4 blocks, on every lane, where the row-owner form issues 12 loads for 22 DFMAs on 22 of 32 lanes. Each
+// accumulator still sees its operands in ascending k, so the values are the row-owner ones. Entries beyond the m x n result are loaded
+// as zeros and never stored.
+
+// acc_tile: c[r][j] = fma(L[k * ldl + r], R[k * ldr + j], c[r][j]) for k = 0 .. kn-1 in ascending order; L and R point at the lane's first
+// row and column, mi and nj are the rows and columns of its block that lie inside the result.
+template <int TI, int TJ>
+__device__ __forceinline__ void acc_tile(double (&c)[TI][TJ], const double* __restrict__ L, int ldl, int mi, const double* __restrict__ R, int ldr, int nj, int kn) {
+#pragma unroll 2
+  for (int k = 0; k < kn; ++k) {
+    double a[TI], b[TJ];
+#pragma unroll
+    for (int r = 0; r < TI; ++r) a[r] = (r < mi) ? L[k * ldl + r] : 0.0;
+    if constexpr (TJ % 2 == 0) {
+#pragma unroll
+      for (int j = 0; j < TJ; j += 2) {
+        const double2 b2 = (j < nj) ? *reinterpret_cast<const double2*>(R + k * ldr + j) : make_double2(0.0, 0.0);
+        b[j] = b2.x; b[j + 1] = b2.y;
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < TJ; ++j) b[j] = (j < nj) ? R[k * ldr + j] : 0.0;
+    }
+#pragma unroll
+    for (int r = 0; r < TI; ++r) {
+#pragma unroll
+      for (int j = 0; j < TJ; ++j) c[r][j] = fma(a[r], b[j], c[r][j]);
+    }
+  }
 }
 
+// Tile shell: c starts at 0, body(c, i0, j0, mi, nj) accumulates, the block is stored to C (row-major, m x n). An even TJ needs n, ldc
+// and C's offset even: its column pairs are then whole and 16-byte aligned.
+template <int TI, int TJ, int GJ, class Body>
+__device__ __forceinline__ void tilemm_by(double* __restrict__ C, int ldc, int m, int n, Body body) {
+  const int lane = lane_id(), i0 = (lane / GJ) * TI, j0 = (lane % GJ) * TJ;
+  const int mi = m - i0, nj = n - j0;
+  double c[TI][TJ];
+#pragma unroll
+  for (int r = 0; r < TI; ++r) {
+#pragma unroll
+    for (int j = 0; j < TJ; ++j) c[r][j] = 0.0;
+  }
+  body(c, i0, j0, mi, nj);
+#pragma unroll
+  for (int r = 0; r < TI; ++r) {
+    if (r < mi) {
+      double* cr = C + (i0 + r) * ldc + j0;
+      if constexpr (TJ % 2 == 0) {
+#pragma unroll
+        for (int j = 0; j < TJ; j += 2) if (j < nj) *reinterpret_cast<double2*>(cr + j) = make_double2(c[r][j], c[r][j + 1]);
+      } else {
+#pragma unroll
+        for (int j = 0; j < TJ; ++j) if (j < nj) cr[j] = c[r][j];
+      }
+    }
+  }
+  __syncwarp();
+}
+
+// Tile shell for the lower triangle of a symmetric NX x NX result: the TI x TJ blocks that hold an entry on or below the diagonal are
+// numbered row of blocks by row of blocks, and thread t takes block t (30 blocks of 3 x 4, 55 of 3 x 2). c starts at init(i, j),
+// body(c, i0, j0, mi, nj) accumulates, store(i, j, v) takes every entry with j <= i; the entries of a diagonal block above the diagonal
+// are computed and dropped.
+template <int TI, int TJ, class Init, class Body, class Store>
+__device__ __forceinline__ void tri_tile(int t, Init init, Body body, Store store) {
+  constexpr int NBI = (NX + TI - 1) / TI, NBJ = (NX + TJ - 1) / TJ;
+  int bi = 0;
+  for (; bi < NBI; ++bi) {
+    const int nb = min(NBJ, (TI * bi + TI - 1) / TJ + 1);      // blocks of block row bi that reach the diagonal
+    if (t < nb) break;
+    t -= nb;
+  }
+  const int i0 = bi * TI, j0 = t * TJ;
+  const int mi = bi < NBI ? NX - i0 : 0, nj = NX - j0;
+  double c[TI][TJ];
+#pragma unroll
+  for (int r = 0; r < TI; ++r) {
+#pragma unroll
+    for (int j = 0; j < TJ; ++j) c[r][j] = (r < mi && j0 + j <= i0 + r) ? init(i0 + r, j0 + j) : 0.0;
+  }
+  body(c, i0, j0, mi, nj);
+#pragma unroll
+  for (int r = 0; r < TI; ++r) {
+#pragma unroll
+    for (int j = 0; j < TJ; ++j) if (r < mi && j0 + j <= i0 + r) store(i0 + r, j0 + j, c[r][j]);
+  }
+  __syncwarp();
+}
 
 constexpr int SB_LD = 18;
 // Node inputs as staged in shared memory: the leading span of the projected record, one bulk copy. The rows of A~ and B~ that the record
 // does not store are closed-form values; the recursion multiplies only the support of each row and column of A~ and B~:
-//   A~ rows 0..2    the identity rows: adds (fma(a, 1.0, c) rounds as a + c), except in Qt + At' SA, where a lane-owned row would
-//                   cost registers below the 8-blocks/SM budget
+//   A~ rows 0..2    the identity rows: adds (fma(a, 1.0, c) rounds as a + c)
 //   A~ rows 12..21  [0 I] + dt P_xv, regenerated in place of the staged P_xv with the fma lq_node used for them
 //   B~ rows 0..2    dt/m (dt * (1/m)) at row c % 3 of each stance-force column c < nf
 //   B~ rows 12..21  dt N_v on the null-space columns nf .. nt-1
@@ -1055,11 +1140,15 @@ __device__ __forceinline__ void ric_prefetch_tma(RicNodeIn& n, const double* __r
 }
 
 // One node of the recursion, executed by the TWO warps of the block. The products that do not depend on each other are split
-// between the warps (by result columns, so that every row-owner product keeps its full lane utilisation); the Cholesky of Huu and
-// the gain solve (one warp, latency bound) overlap with the largest product At' S At of the other warp.
+// between the warps by result columns; the 22 x 22 results (SA, Qt + At' SA, S += Hux' K) are tile products over all 32 lanes, the
+// products with B~ (SB, Hux, Huu), which skip the zeros of its columns, are row-owner products. The Cholesky of Huu and the gain
+// solve (one warp, latency bound) overlap with the largest product At' S At of the other warp.
 template <int NTP, int NF>
 __device__ __noinline__ void riccati_node(RicShared& sh, RicNodeIn& in, const double* __restrict__ rec, double* __restrict__ rk, bool& fail,
-                                          int warp, unsigned ph) {
+                                          int warp_arg, unsigned ph) {
+  // the role as a value the compiler knows to be the same on every lane: taken as it arrives, it brackets each shuffle of the
+  // role's branch in a WARPSYNC / ENDCOLLECTIVE pair
+  const int warp = __shfl_sync(HB_FULL_MASK, warp_arg, 0);
   const int lane = lane_id();
   const NodeCols<NF> g(in.meta);
   double* SB = sh.SBK; double* K = sh.SBK;
@@ -1073,19 +1162,24 @@ __device__ __noinline__ void riccati_node(RicShared& sh, RicNodeIn& in, const do
     }
     __syncwarp();
   }
-  // ---- phase A: [SA | SB | sb] = S [At | Bt | bt] (+ s): 22 + NTP + 1 result columns, split SA_SPLIT / rest. S is exactly symmetric (both
-  // halves are written with the same value at the end of every node), so lane i reads its row as column i: consecutive addresses, no
+  // ---- phase A: [SA | SB | sb] = S [At | Bt | bt] (+ s): 22 + NTP + 1 result columns, split SA_SPLIT / rest. S is exactly symmetric (phase D
+  // writes both halves with the same value), so lane i reads its row as column i: consecutive addresses, no
   // bank conflicts (S^T: lane i reads S[k][i])
   if (warp == 0) {
-    rowmm_by<SA_SPLIT, 0>(sh.SA, NX, NX, [&](double (&c)[SA_SPLIT], int i) {
+    tilemm_by<3, 4, 4>(sh.SA, NX, NX, SA_SPLIT, [&](double (&c)[3][4], int i0, int j0, int mi, int nj) {
+      if (j0 == 0) {                          // columns 0..2: the identity rows of A~
 #pragma unroll
-      for (int j = 0; j < 3; ++j) c[j] = c[j] + sh.S[j * NX + i];
-      acc_rows(c, [&](int k) { return sh.S[(k + 3) * NX + i]; }, in.At3, NX, 19);
+        for (int r = 0; r < 3; ++r) {
+#pragma unroll
+          for (int j = 0; j < 3; ++j) if (r < mi) c[r][j] = c[r][j] + sh.S[j * NX + i0 + r];
+        }
+      }
+      acc_tile(c, sh.S + 3 * NX + i0, NX, mi, in.At3 + j0, NX, nj, 19);
     });
     mbar_wait(&sh.bar[2], ph);                // P~ / R~ staged by this warp at the top of the node
   } else {
-    rowmm_by<NX - SA_SPLIT, 0>(sh.SA + SA_SPLIT, NX, NX, [&](double (&c)[NX - SA_SPLIT], int i) {
-      acc_rows(c, [&](int k) { return sh.S[(k + 3) * NX + i]; }, in.At3 + SA_SPLIT, NX, 19);
+    tilemm_by<3, 2, 4>(sh.SA + SA_SPLIT, NX, NX, NX - SA_SPLIT, [&](double (&c)[3][2], int i0, int j0, int mi, int nj) {
+      acc_tile(c, sh.S + 3 * NX + i0, NX, mi, in.At3 + SA_SPLIT + j0, NX, nj, 19);
     });
     rowmm_by<NTP, 0>(SB, SB_LD, NX, [&](double (&c)[NTP], int i) { acc_bt(c, in, g, [&](int k) { return sh.S[k * NX + i]; }); });
     if (lane < NX) {
@@ -1140,12 +1234,15 @@ __device__ __noinline__ void riccati_node(RicShared& sh, RicNodeIn& in, const do
   // (Measured and rejected: factorising Huu in warp 1's phase-B slack and keeping the factor in registers across the barrier -- the
   // kernel needs 255 registers then, and capped for occupancy the factor lives in local memory, which is slower. 8 blocks/SM, which
   // puts 1024 instances in one wave, leave 128 registers per thread.)
+  // The identity rows of A~ are adds on the result rows 0..2 (result row i takes row i of SA; the other rows skip fma(0.0, SA, c) = c).
   if (warp == 0) {
     // Cholesky of the symmetrised Huu entirely in registers: lane i owns row i (right-looking, column by column, the pivot column is
     // broadcast with shuffles), then forward / backward substitution of the 22 + 1 right-hand sides, one per lane, with the factor
     // entries fetched from their owner lanes. No shared-memory round trips on this latency-bound stretch.
     {
-      double a[NTP], rinv[NTP];
+      // 1 / L[j][j] stays on lane j alone and is broadcast where a substitution divides by it (off the dependent chain): as a per-lane
+      // array of NTP equal values it would not leave room for 8 blocks per SM
+      double a[NTP], rinv = 0.0;
 #pragma unroll
       for (int c = 0; c < NTP; ++c) a[c] = (lane < NTP && c <= lane) ? 0.5 * (sh.Huu[lane * 18 + c] + sh.Huu[c * 18 + lane]) : 0.0;
 #pragma unroll
@@ -1153,7 +1250,7 @@ __device__ __noinline__ void riccati_node(RicShared& sh, RicNodeIn& in, const do
         double d = __shfl_sync(HB_FULL_MASK, a[j], j);
         if (!(d > 0.0)) { fail = true; d = 1.0; }
         const double r = rsqrt(d);
-        rinv[j] = r;
+        if (lane == j) rinv = r;
         const double l = a[j] * r;              // L[i][j] on lane i >= j
         a[j] = l;
 #pragma unroll
@@ -1165,14 +1262,14 @@ __device__ __noinline__ void riccati_node(RicShared& sh, RicNodeIn& in, const do
         double sacc = (lane < NX) ? sh.Hux[c * NX + lane] : ((lane == NX) ? sh.hu[c] : 0.0);
 #pragma unroll
         for (int kk = 0; kk < c; ++kk) sacc = fma(-__shfl_sync(HB_FULL_MASK, a[kk], c), y[kk], sacc);
-        y[c] = sacc * rinv[c];
+        y[c] = sacc * __shfl_sync(HB_FULL_MASK, rinv, c);
       }
 #pragma unroll
       for (int c = NTP - 1; c >= 0; --c) {
         double sacc = y[c];
 #pragma unroll
         for (int kk = c + 1; kk < NTP; ++kk) sacc = fma(-__shfl_sync(HB_FULL_MASK, a[c], kk), col[kk], sacc);
-        col[c] = sacc * rinv[c];                 // solution of Huu x = rhs; the gain is its negative
+        col[c] = sacc * __shfl_sync(HB_FULL_MASK, rinv, c);     // solution of Huu x = rhs; the gain is its negative
       }
       if (lane < NX) {
 #pragma unroll
@@ -1200,29 +1297,31 @@ __device__ __noinline__ void riccati_node(RicShared& sh, RicNodeIn& in, const do
   } else {
     mbar_wait(&sh.bar[3], ph);   // Qt has landed in S
     __syncwarp();
-    rowmm_by<NX, 1>(sh.S, NX, NX, [&](double (&c)[NX], int i) {          // At^T: lane i owns column i of At
-      acc_rows(c, [&](int k) { return (k == i) ? 1.0 : 0.0; }, sh.SA, NX, 3);
-      acc_rows(c, [&](int k) { return in.At3[k * NX + i]; }, sh.SA + 3 * NX, NX, 19);
-    });
+    // lower triangle only, started from the symmetric part of Qt (the record's halves differ in the last bits); the entries above the
+    // diagonal are read here and never written, so no lane reads what another stores
+    tri_tile<3, 4>(lane, [&](int i, int j) { return 0.5 * (sh.S[i * NX + j] + sh.S[j * NX + i]); },
+                   [&](double (&c)[3][4], int i0, int j0, int mi, int nj) {   // At^T: row i of the result takes column i of At
+#pragma unroll
+      for (int r = 0; r < 3; ++r) {             // rows 0..2 of A~ (identity): result row i < 3 takes row i of SA
+#pragma unroll
+        for (int j = 0; j < 4; ++j) if (i0 + r < 3 && j < nj) c[r][j] = c[r][j] + sh.SA[(i0 + r) * NX + j0 + j];
+      }
+      acc_tile(c, in.At3 + i0, NX, mi, sh.SA + 3 * NX + j0, NX, nj, 19);
+    }, [&](int i, int j, double v) { sh.S[i * NX + j] = v; });
   }
   __syncthreads();
-  // ---- phase D: S += Hux' K, result columns split 12 / 10
-  if (warp == 0) rowmm<12, true, 1>(sh.S, NX, sh.Hux, NX, K, NX, NX, NTP);
-  else rowmm<10, true, 1>(sh.S + 12, NX, sh.Hux, NX, K + 12, NX, NX, NTP);
-  __syncthreads();
-  // S <- (S + S') / 2: one (i, j) pair per thread and round, 231 pairs = 4 rounds of 64 threads. Pair t is (i, (i + d) mod 22) with
-  // i = t mod 22, d = t / 22 + 1: d = 1..10 gives every pair at cyclic distance 1..10 once, d = 11 (t = 220..230) the 11 pairs (i, i + 11)
-  for (int t = threadIdx.x; t < NX * (NX - 1) / 2; t += 64) {
-    const int d = t / NX + 1, i = t - (d - 1) * NX, j = (i + d) % NX;
-    const double v = 0.5 * (sh.S[i * NX + j] + sh.S[j * NX + i]);
-    sh.S[i * NX + j] = v; sh.S[j * NX + i] = v;
-  }
+  // ---- phase D: S += Hux' K on the lower triangle, its 55 blocks of 3 x 2 over the 64 threads; every value goes to both halves, so S is
+  // exactly symmetric with no averaging pass. The init reads entries on or below the diagonal only, the mirror stores go above it.
+  tri_tile<3, 2>((int)threadIdx.x, [&](int i, int j) { return sh.S[i * NX + j]; },
+                 [&](double (&c)[3][2], int i0, int j0, int mi, int nj) { acc_tile(c, sh.Hux + i0, NX, mi, K + j0, NX, nj, NTP); },
+                 [&](int i, int j, double v) { sh.S[i * NX + j] = v; if (j < i) sh.S[j * NX + i] = v; });
   __syncthreads();
 }
 
-// 128 registers x 64 threads also allow 8 blocks per SM. ptxas reaches 128 without spills on its own; a minimum-blocks bound of 8 (or
-// __maxnreg__(128)) makes it spill 40 B around the riccati_node calls at the same register count, so the bound is left out.
-__global__ void __launch_bounds__(64) riccati_kernel(SqpArgs a) {
+// 128 registers x 64 threads also allow 8 blocks per SM, and the bound says so: with the warp-uniform role ptxas schedules the node
+// more freely and takes 138 registers when left alone (6 blocks per SM, two waves at 1024 instances); bounded it uses 126 with the same
+// 8 B stack frame and no spills.
+__global__ void __launch_bounds__(64, 8) riccati_kernel(SqpArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   RicShared& sh = *reinterpret_cast<RicShared*>(smem_raw);
   const int inst = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1242,8 +1341,9 @@ __global__ void __launch_bounds__(64) riccati_kernel(SqpArgs a) {
     const double* rec = proj + (size_t)k * PJ_STRIDE;
     double* rk = a.rk + ((size_t)inst * a.N + k) * RK_STRIDE;
     const unsigned ph = (unsigned)(N - 1 - k) & 1u;      // phase of the once-per-node barriers
-    // every thread waits for the inputs of node k (prefetched one node ahead); the two block barriers that end the previous node already
-    // order the re-use of Hux / Huu / the other input buffer, so no barrier is needed here
+    // every thread waits for the inputs of node k (prefetched one node ahead); the block barrier that ends the previous node (after
+    // phase D, the last reader of Hux and K; the other input buffer was last read in phase C) already orders the re-use of Hux / Huu / that
+    // buffer, so no barrier is needed here
     if (k & 1) { mbar_wait(&sh.bar[1], ph_in1); ph_in1 ^= 1u; } else { mbar_wait(&sh.bar[0], ph_in0); ph_in0 ^= 1u; }
     RicNodeIn& in = sh.in[k & 1];
     const int nt = (int)in.meta[0], nf = (int)in.meta[1], nv = (int)in.meta[2];
