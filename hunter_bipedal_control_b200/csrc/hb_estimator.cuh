@@ -42,15 +42,14 @@ __global__ void __launch_bounds__(32) kf_update_kernel(int B, hb_kf_params prm, 
   sincos(zyx[0], &sz, &cz); sincos(zyx[1], &sy, &cy); sincos(zyx[2], &sx, &cx);
   const double wlx = angl[3 * inst], wly = angl[3 * inst + 1], wlz = angl[3 * inst + 2];
   const double dzr = (sx * wly + cx * wlz) / cy, dyr = cx * wly - sx * wlz, dxr = wlx + sy * dzr;   // yaw, pitch, roll rates
-  const double wg[3] = {-sz * dyr + cy * cz * dxr, cz * dyr + cy * sz * dxr, dzr - sy * dxr};
+  const double rates[3] = {dzr, dyr, dxr};
+  double wg[3];
+  world_omega_from_zyx_rates(sz, cz, sy, cy, rates, wg);
   // ---- contact kinematics with the base at the origin and zero base linear velocity (:84-100)
   double q[NQ], v[NQ];
   q[0] = q[1] = q[2] = 0.0; q[3] = zyx[0]; q[4] = zyx[1]; q[5] = zyx[2];
   v[0] = v[1] = v[2] = 0.0;
-  {
-    const double r = (cz * wg[0] + sz * wg[1]) / cy;      // getEulerAnglesZyxDerivativesFromGlobalAngularVelocity
-    v[5] = r; v[4] = -sz * wg[0] + cz * wg[1]; v[3] = wg[2] + sy * r;
-  }
+  zyx_rates_from_world_omega(sz, cz, sy, cy, wg, &v[3]);
   for (int j = 0; j < NJ; ++j) { q[6 + j] = jpos[(size_t)inst * NJ + j]; v[6 + j] = jvel[(size_t)inst * NJ + j]; }
   KinOut<double> ko;
   kin_pass<double>(q, v, ko);
@@ -168,14 +167,7 @@ __global__ void __launch_bounds__(32) contact_force_kernel(int B, double lambda,
   const double gama = exp(-lambda * dt), beta = (1.0 - gama) / (gama * dt);
   const double* r = rbd + (size_t)inst * 32;
   double q[NQ], v[NQ];
-  for (int i = 0; i < 3; ++i) { q[i] = r[3 + i]; q[3 + i] = r[i]; v[i] = r[NQ + 3 + i]; }
-  for (int j = 0; j < NJ; ++j) { q[6 + j] = r[6 + j]; v[6 + j] = r[NQ + 6 + j]; }
-  {
-    double sz, cz, sy, cy;
-    sincos(q[3], &sz, &cz); sincos(q[4], &sy, &cy);
-    const double dxr = (cz * r[NQ] + sz * r[NQ + 1]) / cy;      // getEulerAnglesZyxDerivativesFromGlobalAngularVelocity
-    v[5] = dxr; v[4] = -sz * r[NQ] + cz * r[NQ + 1]; v[3] = r[NQ + 2] + sy * dxr;
-  }
+  rbd_to_qv(r, q, v);
   if (lane < 3) sh.ctv[lane] = 0.0;                 // the kinetic energy does not depend on the base position
   else if (lane < NQ) {
     D1 qd[NQ], vd[NQ];

@@ -238,13 +238,9 @@ __global__ void plan_prepare_kernel(int B, const hb_plan_input* in, double* t0, 
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
   const hb_plan_input& p = in[inst];
-  double q[NQ], v[NQ];
   for (int i = 0; i < NX; ++i) x0[(size_t)inst * NX + i] = p.x0[i];
-  for (int i = 0; i < NQ; ++i) { q[i] = p.x0[6 + i]; v[i] = 0.0; }
   t0[inst] = p.t0;
-  KinOut<double> o;
-  kin_pass<double>(q, v, o);
-  for (int i = 0; i < 12; ++i) feet[(size_t)inst * 12 + i] = o.cpos[i];
+  contact_positions(p.x0 + 6, feet + (size_t)inst * 12);
 }
 
 // Device planner (row N1): the same source as the host planner (csrc/hb_planner.h), four threads per instance (eight instances per 32-thread block). Thread 0 of an

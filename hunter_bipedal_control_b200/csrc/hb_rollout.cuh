@@ -354,8 +354,8 @@ __global__ void actuation_kernel(int B, double delay, const double* time, hb_act
 // contact frames (normal spring-damper, viscous tangential friction clipped to the cone), semi-implicit Euler over `substeps` substeps.
 // Same rigid-body passes as the WBC assembly: lanes 0-15 unit-velocity sweeps -> J_c columns, lanes 0-15 RNEA with unit accelerations ->
 // M columns, lane 16 -> nle; 16 x 16 Cholesky in shared memory. One warp per instance. wrench (B x 6, nullable): an external world force at
-// the base origin and a world couple, which enter as the generalised forces Q_p = f, Q_zyx = T' tau with omega_world = T(zyx) zyx_dot (the
-// map of the world angular velocity written back below); null adds nothing. var (nullable): the plants of instances 0 .. n_var - 1 (varied
+// the base origin and a world couple, which enter as the generalised forces Q_p = f, Q_zyx = T' tau with omega_world = T(zyx) zyx_dot
+// (world_omega_from_zyx_rates, hb_rbd.cuh); null adds nothing. var (nullable): the plants of instances 0 .. n_var - 1 (varied
 // plants, hunter_b200.h); the others, and every instance with a null var, run the nominal plant. terrain (nullable): the ground under
 // instances 0 .. n_terrain - 1 (terrain, hunter_b200.h); the others stand on flat ground at prm.ground_height.
 struct SimShared { double q[NQ], v[NQ], J[12 * NQ], M[NQ * 17], nle[NQ], rhs[NQ], t1[NQ], t2[NQ], kdi[NQ], F[12], cpos[12], cvel[12]; };
@@ -404,14 +404,7 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
   const hb_terrain* ter = (terrain && inst < n_terrain) ? terrain + inst : nullptr;  // null: flat ground at prm.ground_height
   bool touch = false;                    // lanes 0-3: the normal force of their contact in the last substep is positive
   double* r = rbd_io + (size_t)inst * 32;
-  if (lane == 0) {
-    for (int i = 0; i < 3; ++i) { sh.q[i] = r[3 + i]; sh.q[3 + i] = r[i]; sh.v[i] = r[NQ + 3 + i]; }
-    for (int j = 0; j < NJ; ++j) { sh.q[6 + j] = r[6 + j]; sh.v[6 + j] = r[NQ + 6 + j]; }
-    double sz, cz, sy, cy;
-    sincos(sh.q[3], &sz, &cz); sincos(sh.q[4], &sy, &cy);
-    const double dxr = (cz * r[NQ] + sz * r[NQ + 1]) / cy;
-    sh.v[5] = dxr; sh.v[4] = -sz * r[NQ] + cz * r[NQ + 1]; sh.v[3] = r[NQ + 2] + sy * dxr;
-  }
+  if (lane == 0) rbd_to_qv(r, sh.q, sh.v);
   __syncwarp();
   const double h = prm.dt / (prm.substeps > 0 ? prm.substeps : 1);
   for (int sub = 0; sub < (prm.substeps > 0 ? prm.substeps : 1); ++sub) {
@@ -473,7 +466,8 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
         else {
           double sz, cz, sy, cy;
           sincos(sh.q[3], &sz, &cz); sincos(sh.q[4], &sy, &cy);
-          s += lane == 3 ? w[5] : (lane == 4 ? -sz * w[3] + cz * w[4] : cz * cy * w[3] + sz * cy * w[4] - sy * w[5]);   // yaw, pitch, roll
+          // rows yaw, pitch, roll of T' (couple), T the map of world_omega_from_zyx_rates
+          s += lane == 3 ? w[5] : (lane == 4 ? -sz * w[3] + cz * w[4] : cz * cy * w[3] + sz * cy * w[4] - sy * w[5]);
         }
       }
       sh.rhs[lane] = s;
@@ -487,14 +481,7 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
     if (lane < NQ) { const double vn = sh.v[lane] + h * sh.t2[lane]; sh.v[lane] = vn; sh.q[lane] += h * vn; }
     __syncwarp();
   }
-  if (lane == 0) {
-    for (int i = 0; i < 3; ++i) { r[3 + i] = sh.q[i]; r[i] = sh.q[3 + i]; r[NQ + 3 + i] = sh.v[i]; }
-    for (int j = 0; j < NJ; ++j) { r[6 + j] = sh.q[6 + j]; r[NQ + 6 + j] = sh.v[6 + j]; }
-    double sz, cz, sy, cy;
-    sincos(sh.q[3], &sz, &cz); sincos(sh.q[4], &sy, &cy);
-    const double d0 = sh.v[3], d1 = sh.v[4], d2 = sh.v[5];      // yaw, pitch, roll rates -> world angular velocity
-    r[NQ] = -sz * d1 + cz * cy * d2; r[NQ + 1] = cz * d1 + sz * cy * d2; r[NQ + 2] = d0 - sy * d2;
-  }
+  if (lane == 0) qv_to_rbd(sh.q, sh.v, r);
   if (lane < 12 && contact_force) contact_force[(size_t)inst * 12 + lane] = sh.F[lane];
   if (lane < 4 && contact_flag) contact_flag[(size_t)inst * 4 + lane] = touch ? 1 : 0;
 }

@@ -1,5 +1,5 @@
 // K5: WeightedWbc problem assembly on the device (legged_wbc/src/WbcBase.cpp:54-338, WeightedWbc.cpp:18-94),
-// one warp per instance. Lane-level parallelism (see hb_rbd.cuh):
+// one warp per instance. Lane-level parallelism (see hb_rbd.cuh; the measured q, v are its rbd_to_qv):
 //   pass A  lanes 0-15: unit velocities at the measured q -> contact Jacobian columns J_c (12x16)
 //           lanes 16-31: unit velocities at the planned q -> centroidal momentum matrix columns A(q_des) (6x16)
 //   pass B  lane 0: dual pass at (q_meas; direction v_meas)  -> p_c, v_c, dJ_c/dt v   (WbcBase.cpp:91-109)
@@ -75,13 +75,7 @@ __device__ inline int wbc_terms_warp(const double* __restrict__ x_des, const dou
   const Model& md = c_model;
   // ---- measured q, v (WbcBase.cpp:72-79)
   if (lane == 0) {
-    for (int i = 0; i < 3; ++i) { sh.q[i] = rbd[3 + i]; sh.q[3 + i] = rbd[i]; sh.v[i] = rbd[NQ + 3 + i]; }
-    for (int j = 0; j < NJ; ++j) { sh.q[6 + j] = rbd[6 + j]; sh.v[6 + j] = rbd[NQ + 6 + j]; }
-    double sz, cz, sy, cy;
-    sincos(sh.q[3], &sz, &cz); sincos(sh.q[4], &sy, &cy);
-    const double w0 = rbd[NQ], w1 = rbd[NQ + 1], w2 = rbd[NQ + 2];
-    const double dxr = (cz * w0 + sz * w1) / cy;
-    sh.v[5] = dxr; sh.v[4] = -sz * w0 + cz * w1; sh.v[3] = w2 + sy * dxr;
+    rbd_to_qv(rbd, sh.q, sh.v);
     for (int i = 0; i < NQ; ++i) sh.qd[i] = x_des[6 + i];
   }
   __syncwarp();
