@@ -18,6 +18,7 @@ _lib = None
 
 NX, NU, NQ, NJ, NWBC = 22, 22, 16, 10, 38
 HB_MAX_EVENTS, HB_MAX_TARGETS, HB_MAX_SEGMENTS = 32, 16, 24
+HB_MAX_HORIZON = 512       # longest horizon_N hb_create accepts
 
 EXPORTED_SYMBOLS = [
     "hb_shard_partition", "hb_shard_sort_by_schedule", "hb_shard_unique_id", "hb_shard_create", "hb_shard_destroy", "hb_shard_block", "hb_shard_gather_dev", "hb_shard_wait", "hb_shard_last_error",

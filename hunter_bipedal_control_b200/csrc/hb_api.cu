@@ -350,7 +350,8 @@ const char* hb_strerror(int code) {
 }
 
 int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
-  // horizon cap: the warm shift stages one instance's previous trajectories in shared memory ((2N+1) x 22 doubles <= 227 KB)
+  // horizon cap: the warm shift stages one instance's previous trajectories in shared memory ((2N+1) x 22 doubles <= 227 KB); its
+  // kernel is opted in once at the cap below, whatever this context's horizon
   if (!cfg || !out || cfg->horizon_N < 1 || cfg->horizon_N > HB_MAX_HORIZON || cfg->max_batch < 1 || !(cfg->dt > 0.0) || cfg->time_horizon < 0.0) return HB_EINVAL;
   hb_ctx* ctx = new (std::nothrow) hb_ctx();
   if (!ctx) return HB_ENOMEM;
@@ -431,7 +432,9 @@ int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
     attr((const void*)lq_kernel, sizeof(LqShared));
     attr((const void*)riccati_kernel, sizeof(RicShared));
     attr((const void*)forward_linesearch2_kernel, sizeof(Fw2Shared));
-    attr((const void*)warm_shift_kernel, sizeof(double) * ((N + 1) * NX + N * NU));
+    // the attribute is the kernel's, for the whole process, not this context's: opt in at the horizon cap so that a later context with a
+    // shorter horizon cannot lower it below what a longer one still needs (180 400 B + the 4 104 B static ptk, under the 227 KB limit)
+    attr((const void*)warm_shift_kernel, sizeof(double) * ((HB_MAX_HORIZON + 1) * NX + HB_MAX_HORIZON * NU));
     // these kernels reach their blocks per SM (8 for the one-block-per-instance kernels, HB_LQ_MINB for lq_kernel) only with the full
     // shared-memory carveout; do not leave it to the driver
     for (const void* fn : {(const void*)wbc_fused_kernel, (const void*)riccati_kernel, (const void*)lq_kernel, (const void*)hwbc_fused_kernel})

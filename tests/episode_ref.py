@@ -55,7 +55,7 @@ def params(log_every=0):
 
 
 def horizon(ctx):
-    return ctx.cfg.time_horizon if ctx.cfg.event_nodes else N * DT
+    return ctx.cfg.time_horizon if ctx.cfg.event_nodes else ctx.N * ctx.dt
 
 
 def noise(seed, scale=1.0):

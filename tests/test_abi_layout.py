@@ -27,7 +27,7 @@ def _struct_fields(body):
 
 STRUCTS = {name: _struct_fields(body) for body, name in re.findall(r"typedef\s+struct\s*\{(.*?)\}\s*(\w+)\s*;", HEADER, re.S)}
 MACROS = {k: int(v) for k, v in re.findall(r"^\s*#define\s+(HB_\w+)\s+(\d+)\s*$", HEADER, re.M)}
-PY_CONSTANTS = ["HB_MAX_EVENTS", "HB_MAX_TARGETS", "HB_MAX_SEGMENTS", "HB_HOQP_MAX_LEVELS", "HB_HOQP_N", "HB_HOQP_MAX_EQ", "HB_HOQP_MAX_IN",
+PY_CONSTANTS = ["HB_MAX_EVENTS", "HB_MAX_HORIZON", "HB_MAX_TARGETS", "HB_MAX_SEGMENTS", "HB_HOQP_MAX_LEVELS", "HB_HOQP_N", "HB_HOQP_MAX_EQ", "HB_HOQP_MAX_IN",
                 "HB_HOQP_MAX_STACKED", "HB_ACT_CAPACITY", "HB_ROLLOUT_MAX_CMDS", "HB_MAX_PUSHES"]
 
 PROBE = r"""#include "hunter_b200.h"

@@ -47,6 +47,16 @@ def test_no_cpu_fallback_without_gpu():
         hb.Context(max_batch=1)
 
 
+def test_horizon_outside_the_envelope_is_rejected_before_any_cuda_call():
+    """hb_create checks 1 <= horizon_N <= HB_MAX_HORIZON first: the rejection needs no GPU (the accepted ends run on one, in
+    test_gpu_horizon_envelope.py)."""
+    import hunter_bipedal_control_b200 as hb
+    from hunter_bipedal_control_b200.api import HB_MAX_HORIZON
+    for N in (0, -1, HB_MAX_HORIZON + 1):
+        with pytest.raises(hb.HunterB200Error, match=r"invalid argument \(-1\)"):
+            hb.Context(horizon_N=N, max_batch=1)
+
+
 def test_product_never_imports_oracle():
     pkg = os.path.join(ROOT, "hunter_bipedal_control_b200")
     for dp, _, fs in os.walk(pkg):
