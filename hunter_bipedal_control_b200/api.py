@@ -42,6 +42,7 @@ EXPORTED_SYMBOLS = [
     "hb_default_plant_variation", "hb_rollout_set_plant_variations", "hb_sim_step_varied", "hb_rollout_set_terrains", "hb_sim_step_terrain",
     "hb_default_estimation_params", "hb_estimation_reset", "hb_sim_read_sensors_batch_dev", "hb_sim_read_sensors", "hb_rollout_estimated_batch_dev",
     "hb_plan_references_targets", "hb_goal_to_target", "hb_plan_set_targets", "hb_rollout_set_goals",
+    "hb_rollout_set_mpc_latencies", "hb_policy_update", "hb_policy_wbc", "hb_policy_wbc_async",
 ]
 
 
@@ -901,6 +902,26 @@ class Context:
         into force; instances beyond len(schedules) follow their cmd_vel; None clears them. Every call forgets the captured goals."""
         self._set_instances("hb_rollout_set_goals", schedules)
 
+    def set_mpc_latencies(self, ticks):
+        """MPC latencies of this context's episodes (hb_rollout_set_mpc_latencies): instance i of every later rollout / rollout_estimated
+        call tracks the solution of an MPC cycle from ticks[i] ticks after the cycle (0 <= ticks[i] <= mpc_every; 0: from the cycle's own
+        tick), instances beyond len(ticks) run with latency 0; None clears them."""
+        if ticks is not None:
+            ticks = (C.c_int32 * len(ticks))(*[int(getattr(d, "value", d)) for d in ticks])      # ints, or c_int32 records
+        self._set_instances("hb_rollout_set_mpc_latencies", ticks)
+
+    def policy_update(self, B, update=None):
+        """MPC_MRT_Interface::updatePolicy of instances 0 .. B-1 (hb_policy_update): each with update[i] (None: every one) adopts the
+        resident solution as the policy policy_wbc evaluates."""
+        up = None if update is None else np.ascontiguousarray(update, dtype=np.uint8)
+        if up is not None and up.shape != (B,):
+            raise ValueError("policy_update: %d update flags for %d instances" % (up.size, B))
+        _check(self._lib.hb_policy_update(self._h, int(B), _ptr(up)), "hb_policy_update", self._h)
+
+    def policy_wbc(self, t_now, rbd, stance_mode=None):
+        """resident_wbc on each instance's adopted policy (hb_policy_wbc): returns (x_des, u_des, mode, sol, torque, status)."""
+        return self._wbc("hb_policy_wbc", t_now, rbd, stance_mode)
+
     def set_plan_targets(self, targets):
         """Explicit planner targets of this context (hb_plan_set_targets): targets[i] (make_targets, goal_to_target) replaces the cmd_vel
         target of instance i in plan_references_gpu and resident_plan_cycle (not in the episodes); None clears them."""
@@ -908,12 +929,16 @@ class Context:
 
     def resident_wbc(self, t_now, rbd, stance_mode=None):
         """Policy of the resident solution at absolute time t_now + WeightedWbc: returns (x_des, u_des, mode, sol, torque, status)."""
+        return self._wbc("hb_resident_wbc_batch", t_now, rbd, stance_mode)
+
+    def _wbc(self, symbol, t_now, rbd, stance_mode):
+        """The body of resident_wbc and policy_wbc, which differ only in the policy they evaluate."""
         rbd = _f64(rbd); B = rbd.shape[0]
         t_now = _f64(np.broadcast_to(_f64(t_now), (B,)))
         sm = None if stance_mode is None else np.ascontiguousarray(stance_mode, dtype=np.uint8)
         xd = np.zeros((B, NX)); ud = np.zeros((B, NU)); md = np.zeros(B, dtype=np.int32); sol = np.zeros((B, NWBC)); tau = np.zeros((B, NJ)); st = np.zeros(B, dtype=np.int32)
-        _check(self._lib.hb_resident_wbc_batch(self._h, B, _ptr(t_now), _ptr(rbd), _ptr(sm), _ptr(xd), _ptr(ud), _ptr(md), _ptr(sol), _ptr(tau), _ptr(st)),
-               "hb_resident_wbc_batch", self._h)
+        _check(getattr(self._lib, symbol)(self._h, B, _ptr(t_now), _ptr(rbd), _ptr(sm), _ptr(xd), _ptr(ud), _ptr(md), _ptr(sol), _ptr(tau), _ptr(st)),
+               symbol, self._h)
         return xd, ud, md, sol, tau, st
 
     def contact_force_estimate(self, dt, state, rbd, tau_cmd, cutoff_frequency=250.0):

@@ -13,6 +13,7 @@
 #include "hb_mpc.cuh"
 #include "hb_planner.h"
 #include <algorithm>
+#include <climits>
 #include <string>
 #include <utility>
 #include <atomic>
@@ -89,6 +90,12 @@ struct hb_ctx {
   hb_target* goal_tg; int32_t* goal_idx;
   // the planner's explicit targets (hb_plan_set_targets), read by the planner calls outside the episodes
   InstanceSetting<hb_target> plan_targets;
+  // the MPC latency of each instance of the episodes (hb_rollout_set_mpc_latencies), and the adopted policy of the MRT split
+  // (hb_policy_update, the episodes' adoptions), allocated at max_batch by its first use; pol_have[i]: instance i has adopted one
+  InstanceSetting<int32_t> latencies;
+  void* pol_mem;
+  SolutionRows pol;
+  std::vector<uint8_t> pol_have;
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
   // hb_resident_cycle_batch's packed references / reference verdicts
   void* arena; size_t arena_cap;
@@ -451,7 +458,8 @@ int hb_destroy(hb_ctx* ctx) {
   void* ptrs[] = {ctx->sqp_mem, ctx->dxt, ctx->dut, ctx->perf, ctx->flags, ctx->xdes, ctx->udes, ctx->wstatus, ctx->witers, ctx->wmode,
                   ctx->hoqp_mem, ctx->cyc_xref, ctx->cyc_swing, ctx->cyc_tk, ctx->cyc_mode, ctx->cyc_nn, ctx->res_t0, ctx->res_xt,
                   ctx->res_ut, ctx->res_tk, ctx->res_mode, ctx->res_nn, ctx->res_sol, ctx->res_stance, ctx->arena, ctx->ro_mem, ctx->re_mem,
-                  ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->goal_mem, ctx->plan_targets.dev};
+                  ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->goal_mem, ctx->plan_targets.dev,
+                  ctx->latencies.dev, ctx->pol_mem};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -627,7 +635,7 @@ static int policy_eval_impl(hb_ctx* ctx, int B, double t_rel, const double* x_tr
   ENTER(ctx, B, x_traj && u_traj && mode && x_des && u_des && (tk == nullptr) == (nn == nullptr), UNCAPPED);
   const int wpb = 4;
   return launch(ctx, K_UNPROFILED, policy_eval_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, ctx->cfg.horizon_N, ctx->cfg.dt, t_rel, x_traj, u_traj, mode,
-                x_des, u_des, mode_out, tk, nn, nullptr, nullptr);
+                x_des, u_des, mode_out, tk, nn, nullptr, nullptr, PolicyChoice{});
 }
 
 int hb_policy_eval_batch_dev(hb_ctx* ctx, int B, double t_rel, const double* x_traj, const double* u_traj, const int32_t* mode, double* x_des,
@@ -1028,17 +1036,72 @@ static bool target_ok(const hb_target& tg) {
 
 int hb_plan_set_targets(hb_ctx* ctx, int B, const hb_target* t) { return set_instances(ctx, B, t, target_ok, &hb_ctx::plan_targets); }
 
-// hb_resident_wbc_batch_dev; no_prev = true: the fallback has no previous solution yet (first tick after a cold start whose cycle ran no WBC)
-static int resident_wbc_impl(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
-                             int32_t* mode_out, double* wbc_sol, double* torque, int32_t* wbc_status, bool no_prev) {
-  ENTER(ctx, B, t_now && rbd && x_des && u_des && mode_out && wbc_sol, UNCAPPED,
-        [&] { return ctx->base + B <= ctx->res_valid; });             // a resident solution to evaluate
-  const size_t N = ctx->cfg.horizon_N, o = (size_t)ctx->base;
+static bool latency_ok(const int32_t& d) { return d >= 0; }     // the upper bound is the episode's mpc_every, checked by the episode call
+
+int hb_rollout_set_mpc_latencies(hb_ctx* ctx, int B, const int32_t* ticks) { return set_instances(ctx, B, ticks, latency_ok, &hb_ctx::latencies); }
+
+// the resident solution of instances [o, ...) as SolutionRows (grid rows only on event-node contexts)
+static SolutionRows resident_rows(hb_ctx* ctx, size_t o) {
+  const size_t N = ctx->cfg.horizon_N;
   const bool grid = ctx->cfg.event_nodes != 0;
+  return SolutionRows{ctx->res_t0 + o, ctx->res_xt + o * (N + 1) * NX, ctx->res_ut + o * N * NU, grid ? ctx->res_tk + o * (N + 1) : nullptr,
+                      ctx->res_mode + o * (N + 1), grid ? ctx->res_nn + o : nullptr};
+}
+
+// The adopted policy of instances [o, ...), allocated at max_batch by its first use (hb_policy_update, an episode with a latency set)
+static int policy_rows(hb_ctx* ctx, size_t o, SolutionRows* rows) {
+  const size_t Bc = ctx->cfg.max_batch, N = ctx->cfg.horizon_N;
+  const int rc = reserve_group(&ctx->pol_mem, [&](void* m) {
+    size_t off = 0;
+    SolutionRows& p = ctx->pol;
+    p.t0 = carve<double>(m, off, Bc); p.xt = carve<double>(m, off, Bc * (N + 1) * NX); p.ut = carve<double>(m, off, Bc * N * NU);
+    p.tk = carve<double>(m, off, Bc * (N + 1)); p.mode = carve<int32_t>(m, off, Bc * (N + 1)); p.nn = carve<int32_t>(m, off, Bc);
+    return off;
+  });
+  if (rc) return rc;
+  if (ctx->pol_have.size() != Bc) {
+    try { ctx->pol_have.assign(Bc, 0); } catch (const std::bad_alloc&) { return HB_ENOMEM; }
+  }
+  const bool grid = ctx->cfg.event_nodes != 0;
+  const SolutionRows& p = ctx->pol;
+  *rows = SolutionRows{p.t0 + o, p.xt + o * (N + 1) * NX, p.ut + o * N * NU, grid ? p.tk + o * (N + 1) : nullptr, p.mode + o * (N + 1),
+                       grid ? p.nn + o : nullptr};
+  return HB_OK;
+}
+
+// true when instances [lo, hi) have all adopted a policy
+static bool policies_adopted(const hb_ctx* ctx, size_t lo, size_t hi) {
+  if (hi > ctx->pol_have.size()) return false;
+  for (size_t i = lo; i < hi; ++i) if (!ctx->pol_have[i]) return false;
+  return true;
+}
+
+// policy_adopt_kernel on instances [0, B) after the entry checks: with lat the episodes' rule at `tick`, otherwise the update mask
+static int policy_adopt(hb_ctx* ctx, int B, const int32_t* lat, int n_lat, long long tick, int every, const uint8_t* update) {
+  SolutionRows to;
+  const int rc = policy_rows(ctx, (size_t)ctx->base, &to);
+  if (rc) return rc;
   const int wpb = 4;
-  int rc = launch(ctx, K_UNPROFILED, policy_eval_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, (int)N, ctx->cfg.dt, 0.0, ctx->res_xt + o * (N + 1) * NX,
-                  ctx->res_ut + o * N * NU, ctx->res_mode + o * (N + 1), x_des, u_des, mode_out, grid ? ctx->res_tk + o * (N + 1) : nullptr,
-                  grid ? ctx->res_nn + o : nullptr, t_now, ctx->res_t0 + o);
+  return launch(ctx, K_UNPROFILED, policy_adopt_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, (int)ctx->cfg.horizon_N, lat, n_lat, tick, every, update,
+                resident_rows(ctx, (size_t)ctx->base), to);
+}
+
+// hb_resident_wbc_batch_dev; no_prev = true: the fallback has no previous solution yet (first tick after a cold start whose cycle ran no WBC).
+// adopted: the adopted policy is evaluated instead of the resident solution (hb_policy_wbc_async); choice (the episodes): per instance one of
+// the two (PolicyChoice).
+static int resident_wbc_impl(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
+                             int32_t* mode_out, double* wbc_sol, double* torque, int32_t* wbc_status, bool no_prev, bool adopted = false,
+                             const PolicyChoice& choice = PolicyChoice{}) {
+  ENTER(ctx, B, t_now && rbd && x_des && u_des && mode_out && wbc_sol, UNCAPPED, [&] {   // a solution to evaluate
+    return adopted ? policies_adopted(ctx, (size_t)ctx->base, (size_t)ctx->base + B) : ctx->base + B <= ctx->res_valid;
+  });
+  const size_t N = ctx->cfg.horizon_N, o = (size_t)ctx->base;
+  SolutionRows s = resident_rows(ctx, o);
+  int rc = adopted ? policy_rows(ctx, o, &s) : HB_OK;
+  if (rc) return rc;
+  const int wpb = 4;
+  rc = launch(ctx, K_UNPROFILED, policy_eval_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, (int)N, ctx->cfg.dt, 0.0, s.xt, s.ut, s.mode, x_des, u_des,
+              mode_out, s.tk, s.nn, t_now, s.t0, choice);
   if (!rc) rc = controller_wbc_dev(ctx, B, x_des, u_des, rbd, mode_out, stance_mode, wbc_sol, wbc_status);
   if (!rc && torque) rc = launch(ctx, K_UNPROFILED, torque_kernel, (B * NJ + 127) / 128, 128, 0, B, wbc_sol, torque);
   return rc ? rc : wbc_fallback(ctx, B, no_prev, wbc_status, wbc_sol, torque);
@@ -1047,6 +1110,11 @@ static int resident_wbc_impl(hb_ctx* ctx, int B, const double* t_now, const doub
 int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
                               int32_t* mode_out, double* wbc_sol, double* torque, int32_t* wbc_status) {
   return resident_wbc_impl(ctx, B, t_now, rbd, stance_mode, x_des, u_des, mode_out, wbc_sol, torque, wbc_status, false);
+}
+
+int hb_policy_wbc_async(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
+                        int32_t* mode_out, double* wbc_sol, double* torque, int32_t* wbc_status) {
+  return resident_wbc_impl(ctx, B, t_now, rbd, stance_mode, x_des, u_des, mode_out, wbc_sol, torque, wbc_status, false, true);
 }
 
 int hb_default_rollout_params(hb_rollout_params* p) {
@@ -1099,18 +1167,40 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   const bool params_ok = p && p->mpc_every >= 1 && p->period > 0.0 && p->log_every >= 0 && delay_ok(p->actuation_delay) && sim_params_ok(p->sim) &&
                          tick0 + n_ticks <= INT32_MAX && (!e || (e->ep && e->est && sensor_noise_ok(e->ep->noise)));
   const bool cold = tick0 == 0;
+  // the MPC latencies of this batch's instances (hb_rollout_set_mpc_latencies): instances i < n_lat have one
+  const InstanceSetting<int32_t>& lat = ctx->latencies;
+  const int n_lat = std::min(lat.n, B);
   ENTER(ctx, B, n_ticks >= 0 && tick0 >= 0 && cmd && rbd && act && estop && stats && params_ok, CAPPED, [&] {
     for (int i = 0; i < B; ++i) {
       const hb_rollout_command& c = cmd[i];
       if (c.gait < 0 || c.gait > 3 || c.n_cmd < 1 || c.n_cmd > HB_ROLLOUT_MAX_CMDS || !(c.gait_start == c.gait_start)) return false;
       for (int k = 0; k < c.n_cmd; ++k) if (!(c.cmd_time[k] == c.cmd_time[k]) || (k > 0 && c.cmd_time[k] < c.cmd_time[k - 1])) return false;
     }
-    return cold || ctx->res_valid >= B;       // a warm start continues from the resident solution
+    for (int i = 0; i < lat.n; ++i) if (lat.host[i] > p->mpc_every) return false;     // latencies beyond one MPC period
+    // a warm start continues from the resident solution, and the instances with a latency from their adopted policies
+    for (int i = 0; i < n_lat && !cold; ++i) if (lat.host[i] >= 1 && !policies_adopted(ctx, i, i + 1)) return false;
+    return cold || ctx->res_valid >= B;
   });
   if (n_ticks == 0) return HB_OK;
   int rc = rollout_reserve(ctx);
   if (!rc && e) rc = estimation_reserve(ctx);
   if (rc) return rc;
+  // With a latency >= 1 in the batch: first_due[r] is the smallest latency d >= 1 with d % mpc_every == r (INT_MAX: none), so that some
+  // instance adopts on tick a iff a >= first_due[a % mpc_every]; the policy evaluation chooses per instance (PolicyChoice).
+  std::vector<int> first_due;
+  PolicyChoice choice{};
+  for (int i = 0; i < n_lat; ++i) {
+    const int d = lat.host[i];
+    if (d < 1) continue;
+    if (first_due.empty()) first_due.assign(p->mpc_every, INT_MAX);
+    first_due[d % p->mpc_every] = std::min(first_due[d % p->mpc_every], d);
+  }
+  const bool delayed = !first_due.empty();
+  if (delayed) {
+    rc = policy_rows(ctx, 0, &choice.adopted);
+    if (rc) return rc;
+    choice.lat = lat.dev; choice.n_lat = n_lat;
+  }
   CK(cudaMemcpyAsync(ctx->ro_cmd, cmd, sizeof(hb_rollout_command) * B, cudaMemcpyHostToDevice, ctx->stream));
   const double horizon = (ctx->cfg.event_nodes && ctx->cfg.time_horizon > 0.0) ? ctx->cfg.time_horizon : ctx->cfg.horizon_N * ctx->cfg.dt;
   const int n_log = (log && p->log_every > 0) ? (n_ticks + p->log_every - 1) / p->log_every : 0;
@@ -1140,6 +1230,8 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
                            ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag, meas);
       if (!rc) rc = launch(ctx, K_UNPROFILED, est_observe_kernel, grid, 64, 0, B, rbd, meas, stats, e->est, e->stats, est_row, (size_t)n_est_log * 32);
     }
+    // MPC_MRT_Interface::updatePolicy of the instances whose solution comes into force on this tick, before this tick's cycle
+    if (!rc && delayed && a >= first_due[a % p->mpc_every]) rc = policy_adopt(ctx, B, lat.dev, n_lat, a, p->mpc_every, nullptr);
     if (!rc && mpc) {
       if (first_cold) CK(cudaMemsetAsync(ctx->res_stance, 0, sizeof(double) * B * 12, ctx->stream));   // latestStanceposition_ starts at zero
       rc = launch(ctx, K_UNPROFILED, rollout_plan_inputs_kernel, grid, 64, 0, B, t, horizon, ctx->ro_cmd, meas, e ? e->est : nullptr, ctx->ro_in, goals,
@@ -1148,10 +1240,16 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
       if (!rc) rc = plan_dev(ctx, B, ctx->ro_in, ctx->ro_feet, ctx->res_stance, ctx->ro_refs, ctx->ro_pstat, goals ? ctx->goal_tg : nullptr, ctx->goal_idx,
                              ctx->goals.n);
       if (!rc) rc = resident_cycle_impl(ctx, B, first_cold, 0.0, ctx->ro_t0, ctx->ro_x0, ctx->ro_refs, meas, ctx->ro_info, nullptr, nullptr, nullptr, false);
+      // the cold tick: every instance with a latency starts with the policy of this first solve
+      if (!rc && delayed && first_cold) {
+        rc = policy_adopt(ctx, B, lat.dev, n_lat, -1, p->mpc_every, nullptr);
+        for (int i = 0; i < n_lat && !rc; ++i) if (lat.host[i] >= 1) ctx->pol_have[i] = 1;
+      }
       if (!rc && e) rc = launch(ctx, K_UNPROFILED, est_schedule_kernel, grid, 64, 0, B, ctx->ro_refs, e->est);
     }
     // the cycle ran no WBC, so after a cold start the first tick's fallback has no previous solution, as the cycle's own would not have
-    if (!rc) rc = resident_wbc_impl(ctx, B, ctx->ro_tnow, meas, nullptr, ctx->xdes, ctx->udes, ctx->wmode, ctx->ro_sol, nullptr, ctx->wstatus, first_cold);
+    if (!rc) rc = resident_wbc_impl(ctx, B, ctx->ro_tnow, meas, nullptr, ctx->xdes, ctx->udes, ctx->wmode, ctx->ro_sol, nullptr, ctx->wstatus, first_cold,
+                                    false, choice);
     if (!rc) rc = hb_joint_command_batch_dev(ctx, B, &p->gains, p->period, ctx->xdes, ctx->udes, ctx->ro_sol, ctx->wmode, meas, nullptr, estop, ctx->ro_jcmd,
                                              ctx->ro_jtau);
     if (!rc) rc = hb_actuation_batch_dev(ctx, B, p->actuation_delay, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau);
@@ -1592,6 +1690,29 @@ int hb_resident_wbc_batch(hb_ctx* ctx, int B, const double* t_now, const double*
   auto xd = s.out(x_des, NX); auto ud = s.out(u_des, NU); auto md = s.out(mode_out, 1); auto sol = s.out(wbc_sol, NWBC);
   auto tau = s.out(torque, NJ); auto st = s.out(wbc_status, 1);    // always passed: the fallback and its bookkeeping run on every call
   return s.run(1, [&](Chunk) { return hb_resident_wbc_batch_dev(ctx, B, tn, r, sm, xd, ud, md, sol, tau, st); });
+}
+
+int hb_policy_update(hb_ctx* ctx, int B, const uint8_t* update) {
+  ENTER(ctx, B, true, CAPPED, [&] {            // an instance that adopts needs a resident solution
+    for (int i = 0; i < B; ++i) if ((!update || update[i]) && i >= ctx->res_valid) return false;
+    return true;
+  });
+  Staging s(ctx, B);
+  auto up = s.in_or_null(update, 1);
+  const int rc = s.run(1, [&](Chunk) { return policy_adopt(ctx, B, nullptr, 0, 0, 1, up); });
+  if (rc) return rc;
+  for (int i = 0; i < B; ++i) if (!update || update[i]) ctx->pol_have[i] = 1;
+  return HB_OK;
+}
+
+int hb_policy_wbc(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des, int32_t* mode_out,
+                  double* wbc_sol, double* torque, int32_t* wbc_status) {
+  ENTER(ctx, B, t_now && rbd && x_des && u_des && mode_out && wbc_sol, CAPPED, [&] { return policies_adopted(ctx, 0, B); });
+  Staging s(ctx, B);
+  auto tn = s.in(t_now, 1); auto r = s.in(rbd, 32); auto sm = s.in_or_null(stance_mode, 1);
+  auto xd = s.out(x_des, NX); auto ud = s.out(u_des, NU); auto md = s.out(mode_out, 1); auto sol = s.out(wbc_sol, NWBC);
+  auto tau = s.out(torque, NJ); auto st = s.out(wbc_status, 1);    // always passed, as in hb_resident_wbc_batch
+  return s.run(1, [&](Chunk) { return hb_policy_wbc_async(ctx, B, tn, r, sm, xd, ud, md, sol, tau, st); });
 }
 
 int hb_contact_force_estimate_batch(hb_ctx* ctx, int B, double cutoff_frequency, double dt, hb_observer_state* state, const double* rbd,

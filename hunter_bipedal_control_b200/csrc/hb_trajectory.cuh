@@ -97,13 +97,60 @@ __global__ void __launch_bounds__(128) warm_shift_kernel(int B, int N, double dt
   if (grid) for (int i = threadIdx.x; i <= N; i += blockDim.x) tk_res[(size_t)inst * (N + 1) + i] = tn_[i];
 }
 
+// One solution of B instances as the kernels store it (the resident solution, or the adopted policy of the MRT split): solve time, node
+// times and interval counts (event-node grids; null on uniform ones), state / input trajectories, node modes
+struct SolutionRows {
+  double *t0, *xt, *ut, *tk;
+  int32_t *mode, *nn;
+};
+
+// The per-instance source choice of policy_eval_kernel: instance inst < n_lat with lat[inst] >= 1 (its MPC latency) evaluates `adopted`
+// instead of the solution the kernel was given. lat == null: every instance evaluates the given one.
+struct PolicyChoice {
+  const int32_t* lat;
+  int n_lat;
+  SolutionRows adopted;
+};
+
+// MPC_MRT_Interface::updatePolicy, one warp per instance: the resident solution `from` is copied into the adopted policy `to` of the
+// instances that adopt. With lat (the episodes), instance inst < n_lat with latency d = lat[inst] >= 1 adopts on tick `tick` iff
+// tick >= d and (tick - d) % every == 0, and every such instance adopts when tick < 0 (the cold tick's adoption after its cycle); without
+// lat, the instances with update[inst] != 0 adopt (update null: all).
+__global__ void policy_adopt_kernel(int B, int N, const int32_t* lat, int n_lat, long long tick, int every, const uint8_t* update, SolutionRows from,
+                                    SolutionRows to) {
+  const int inst = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (inst >= B) return;
+  const int lane = threadIdx.x & 31;
+  if (lat) {
+    const int d = inst < n_lat ? lat[inst] : 0;
+    if (d < 1 || (tick >= 0 && (tick < d || (tick - d) % every != 0))) return;
+  } else if (update && !update[inst]) {
+    return;
+  }
+  const size_t nx = (size_t)(N + 1) * NX, nu = (size_t)N * NU, i = (size_t)inst;
+  for (size_t k = lane; k < nx; k += 32) to.xt[i * nx + k] = from.xt[i * nx + k];
+  for (size_t k = lane; k < nu; k += 32) to.ut[i * nu + k] = from.ut[i * nu + k];
+  for (int k = lane; k <= N; k += 32) to.mode[i * (N + 1) + k] = from.mode[i * (N + 1) + k];
+  if (from.tk) for (int k = lane; k <= N; k += 32) to.tk[i * (N + 1) + k] = from.tk[i * (N + 1) + k];
+  if (lane == 0) {
+    to.t0[inst] = from.t0[inst];
+    if (from.nn) to.nn[inst] = from.nn[inst];
+  }
+}
+
 // MPC_MRT_Interface::evaluatePolicy with the feed-forward policy (LeggedController.cpp:154-156, task.info:93):
-// linear interpolation of the state / input trajectories at t0 + t_rel; mode = mode in force at that time.
+// linear interpolation of the state / input trajectories at t0 + t_rel; mode = mode in force at that time. choice: see PolicyChoice.
 __global__ void policy_eval_kernel(int B, int N, double dt, double t_rel, const double* xt, const double* ut, const int32_t* mode, double* x_des,
-                                   double* u_des, int32_t* mode_out, const double* tk, const int32_t* nn, const double* t_abs, const double* t0res) {
+                                   double* u_des, int32_t* mode_out, const double* tk, const int32_t* nn, const double* t_abs, const double* t0res,
+                                   PolicyChoice choice) {
   const int inst = blockIdx.x * blockDim.x / 32 + (threadIdx.x >> 5);
   if (inst >= B) return;
   const int lane = threadIdx.x & 31;
+  if (choice.lat && inst < choice.n_lat && choice.lat[inst] >= 1) {
+    const SolutionRows& a = choice.adopted;
+    xt = a.xt; ut = a.ut; mode = a.mode; t0res = a.t0;
+    if (tk) { tk = a.tk; nn = a.nn; }
+  }
   if (t_abs) t_rel = t_abs[inst] - t0res[inst];        // evaluation at an absolute time per instance (500 Hz WBC ticks between MPC updates)
   int k, na = N;
   double al;

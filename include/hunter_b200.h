@@ -364,6 +364,26 @@ typedef struct {                      /* the goal poses of one robot            
  * n_goal outside 0..HB_MAX_GOALS, a non-finite time or goal entry, times that descend. */
 int hb_rollout_set_goals(hb_ctx* ctx, int B, const hb_goal_schedule* goals);
 
+/* ---- MPC latency: the solve time of each robot's MPC cycle, as the MRT interface of the reference sees it (MPC_MRT_Interface) ----
+ * An instance with latency d >= 1 ticks tracks its own adopted policy: a copy of the resident solution (solve time, node times, interval
+ * count, state / input trajectories, node modes). Every MPC cycle still writes the resident solution, which stays the solver's warm start.
+ * Adoption (MPC_MRT_Interface::updatePolicy): on absolute tick a, before that tick's MPC cycle, the instance adopts the resident solution
+ * iff a >= d and (a - d) % mpc_every == 0, so the solution of the cycle at tick c comes into force at tick c + d (with d == mpc_every, just
+ * before the next cycle overwrites it). On the cold tick (tick0 == 0, first tick of the call) every instance with d >= 1 adopts right after
+ * the cycle, so the controller starts with a policy (the reference shows its stance override until the first solve; a deviation).
+ * The policy evaluation of every tick, and the WBC, joint command law and fallback after it, read the adopted policy for d >= 1 and the
+ * resident solution for d == 0; the joint command law takes its planned contact from the adopted policy's mode (the reference reads the
+ * reference manager's newest schedule there; a deviation). The plan inputs, the planner, the warm start, the estimator's contact flags
+ * and goal capture read the newest plan, as the reference's reference manager does.
+ * The adopted policy is per-instance context state like the captured goals, so a split episode continues exactly; snapshots
+ * (hb_resident_read_batch / hb_resident_write_batch) do not include it. Range: 0 <= d <= mpc_every; an episode call whose setting has an
+ * entry above its mpc_every returns -1 before any launch, and so does a warm call (tick0 > 0) in which an instance with d >= 1 has never
+ * adopted a policy. With no setting, or every latency 0, the episode calls issue exactly the launches they issue without one; with a
+ * latency set they add one launch on each tick where an instance within the setting adopts, and one on the cold tick. */
+/* Sets the MPC latencies of the context's episodes, ticks[i] for instance i (a per-robot episode setting, above; instances at or beyond B
+ * run with latency 0). -1 also for a negative entry. */
+int hb_rollout_set_mpc_latencies(hb_ctx* ctx, int B, const int32_t* ticks);
+
 /* ---- estimated episodes (hb_rollout_estimated_batch_dev): the controllers read the Kalman filter's estimate from synthesised, noisy
  * sensors instead of the plant's true state (LeggedController::updateStateEstimation, LeggedController.cpp:280-349) ---- */
 typedef struct {                 /* standard deviations of additive Gaussian sensor noise; 0 = that channel is exact and draws nothing */
@@ -530,7 +550,8 @@ int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const dou
  * cycle runs first: plan inputs built on the device from rbd (x0 = hb_rbd_to_centroidal, t0 = t, cmd_vel of the command segment in force,
  * horizon = time_to_target = horizon_N * dt or, for event_nodes contexts, the time horizon, prev_event = min(t, gait_start) - 0.5, IK
  * joint references), device planner, resident cycle without its WBC (cold start iff tick0 == 0). Every tick then runs
- * hb_resident_wbc_batch's policy + WeightedWbc at t, the joint command law (loaded, walking branch), the actuation model, saturation to
+ * hb_resident_wbc_batch's policy + WeightedWbc at t (the adopted policy's for instances with an MPC latency, hb_rollout_set_mpc_latencies),
+ * the joint command law (loaded, walking branch), the actuation model, saturation to
  * +-torque_limit and one plant step (with the tick's push wrench when hb_rollout_set_pushes has set schedules, on the instance's plant
  * when hb_rollout_set_plant_variations has set variations, on its ground when hb_rollout_set_terrains has set terrains). Failure checks run on the state entering each tick (finite, |roll| <= pi/2, base height) and on the
  * emergency stop the joint command raises; from its first failure on an instance is held (rbd put back to its last finite state after
@@ -647,6 +668,19 @@ int hb_sim_step_terrain(hb_ctx* ctx, int B, const hb_sim_params* params, double*
                         uint8_t* contact_flag /*nullable*/);
 int hb_resident_wbc_batch(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode /*nullable*/, double* x_des, double* u_des,
                           int32_t* mode_out, double* wbc_sol, double* torque /*nullable*/, int32_t* wbc_status /*nullable*/);
+
+/* ---- the MRT split outside the episodes: the adopted policy (MPC latency, above) through public calls ----
+ * hb_policy_update: MPC_MRT_Interface::updatePolicy of instances 0 .. B-1, each with update[i] != 0 (update NULL: every one) copying the
+ * resident solution into its adopted policy. -1 also when a flagged instance holds no resident solution. Synchronous. */
+int hb_policy_update(hb_ctx* ctx, int B, const uint8_t* update /*nullable*/);
+/* hb_resident_wbc_batch on the adopted policy: evaluatePolicy of each instance's adopted policy at t_now[i], the controller's WBC, torque
+ * law. It is the same WBC as hb_resident_wbc_batch and shares its per-instance previous-solution fallback. -1 when an instance of the batch
+ * has never adopted a policy. hb_policy_wbc takes host pointers (synchronous), hb_policy_wbc_async device pointers (asynchronous, on the
+ * context's stream). */
+int hb_policy_wbc(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode /*nullable*/, double* x_des, double* u_des,
+                  int32_t* mode_out, double* wbc_sol, double* torque /*nullable*/, int32_t* wbc_status /*nullable*/);
+int hb_policy_wbc_async(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode /*nullable*/, double* x_des,
+                        double* u_des, int32_t* mode_out, double* wbc_sol, double* torque /*nullable*/, int32_t* wbc_status /*nullable*/);
 int hb_rbd_to_centroidal_batch(hb_ctx* ctx, int B, const double* rbd, double* x);
 int hb_reference_expand_batch(hb_ctx* ctx, int B, const double* t0, const hb_reference* refs, double* x_ref, double* swing_ref,
                               int32_t* mode);
