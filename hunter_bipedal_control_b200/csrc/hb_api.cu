@@ -40,7 +40,8 @@ template <class T> struct InstanceSetting {
   T* dev;
   int n;
   std::vector<T> host;
-  const T* get() const { return n > 0 ? dev : nullptr; }   // what the kernels read: null while unset
+  // what the kernels of a call whose instances start at `base` (ctx->base in a chunk) read: the records from base on; unset, none
+  InstanceView<T> view(int base = 0) const { return n > base ? InstanceView<T>{dev + base, n - base} : InstanceView<T>{}; }
 };
 
 struct hb_ctx {
@@ -52,6 +53,7 @@ struct hb_ctx {
   cudaStream_t stream_main, stream_aux;   // the chunked host-pointer calls pipeline their chunks over these
   int base;                               // instance offset into the per-instance scratch (chunked calls)
   int64_t launches;
+  void* scratch_mem;   // the scratch every context has (dxt ... res_stance), carved by hb_create from this one allocation
   // MPC scratch
   double *dxt, *dut, *perf;
   void* sqp_mem; double *lin, *proj, *rk;   // node records of the SQP pipeline (K0 -> K1 -> K2/K3), allocated by the first MPC solve
@@ -64,9 +66,8 @@ struct hb_ctx {
   double *cyc_xref, *cyc_swing, *cyc_tk;
   int32_t *cyc_mode, *cyc_nn;
   // resident primal solution (hb_resident_cycle_batch): solve time, trajectories, node modes (policy evaluation between MPC solves),
-  // node times / interval counts (event-node grids)
-  double *res_t0, *res_xt, *res_ut, *res_tk;
-  int32_t *res_mode, *res_nn;
+  // node times / interval counts (event-node grids; allocated on every context)
+  SolutionRows res;
   int res_valid;                      // number of instances holding a previous solution
   double* res_sol; int res_sol_valid;   // last good WBC solution per instance (WeightedWbc fallback, W5)
   double* res_stance;                 // the device planner's latest stance positions (row N1)
@@ -236,6 +237,20 @@ template <class F> int reserve_group(void** mem, F&& layout) {
   if (cudaMalloc(mem, layout(nullptr)) != cudaSuccess) { cudaGetLastError(); *mem = nullptr; return HB_ENOMEM; }
   layout(*mem);
   return HB_OK;
+}
+
+// The six rows of a solution (SolutionRows) of n instances on a horizon of N intervals, carved from base as carve does
+SolutionRows carve_solution(void* base, size_t& off, size_t n, size_t N) {
+  SolutionRows r;
+  r.t0 = carve<double>(base, off, n); r.xt = carve<double>(base, off, n * (N + 1) * NX); r.ut = carve<double>(base, off, n * N * NU);
+  r.tk = carve<double>(base, off, n * (N + 1)); r.mode = carve<int32_t>(base, off, n * (N + 1)); r.nn = carve<int32_t>(base, off, n);
+  return r;
+}
+
+// Instances [o, ...) of a solution of horizon N stored at max_batch; the grid rows are null on uniform grids (grid false)
+SolutionRows rows_at(const SolutionRows& r, size_t o, size_t N, bool grid) {
+  return SolutionRows{r.t0 + o, r.xt + o * (N + 1) * NX, r.ut + o * N * NU, grid ? r.tk + o * (N + 1) : nullptr, r.mode + o * (N + 1),
+                      grid ? r.nn + o : nullptr};
 }
 
 // Device side of one staged argument. Converts to its device pointer once Staging::reserve has placed it (null for a null pass-through
@@ -413,20 +428,22 @@ int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
   delete m;
   if (e != cudaSuccess) { ctx->last_cuda = (int)e; hb_destroy(ctx); return HB_ECUDA; }
   const size_t B = cfg->max_batch, N = cfg->horizon_N;
-  bool ok = true;
   // the node records of the SQP pipeline (31 KB per instance and interval) are allocated by the first MPC solve: contexts that only run the
   // WBC / QP / planner / estimator entry points never pay for them
-  ok = ok && dalloc(&ctx->dxt, B * (N + 1) * NX) == cudaSuccess && dalloc(&ctx->dut, B * N * NU) == cudaSuccess;
-  ok = ok && dalloc(&ctx->perf, B * 4) == cudaSuccess && dalloc(&ctx->flags, B) == cudaSuccess;
-  ok = ok && dalloc(&ctx->xdes, B * NX) == cudaSuccess && dalloc(&ctx->udes, B * NU) == cudaSuccess;
-  ok = ok && dalloc(&ctx->wstatus, B) == cudaSuccess && dalloc(&ctx->witers, B) == cudaSuccess && dalloc(&ctx->wmode, B) == cudaSuccess;
-  ok = ok && dalloc(&ctx->cyc_xref, B * (N + 1) * NX) == cudaSuccess && dalloc(&ctx->cyc_swing, B * (N + 1) * 24) == cudaSuccess;
-  ok = ok && dalloc(&ctx->cyc_mode, B * (N + 1)) == cudaSuccess && dalloc(&ctx->cyc_tk, B * (N + 1)) == cudaSuccess && dalloc(&ctx->cyc_nn, B) == cudaSuccess;
-  ok = ok && dalloc(&ctx->res_xt, B * (N + 1) * NX) == cudaSuccess && dalloc(&ctx->res_ut, B * N * NU) == cudaSuccess && dalloc(&ctx->res_t0, B) == cudaSuccess;
-  ok = ok && dalloc(&ctx->res_mode, B * (N + 1)) == cudaSuccess && dalloc(&ctx->res_tk, B * (N + 1)) == cudaSuccess && dalloc(&ctx->res_nn, B) == cudaSuccess;
-  ok = ok && dalloc(&ctx->res_sol, B * NWBC) == cudaSuccess && dalloc(&ctx->res_stance, B * 12) == cudaSuccess;
+  const int rc = reserve_group(&ctx->scratch_mem, [&](void* m) {
+    size_t off = 0;
+    ctx->dxt = carve<double>(m, off, B * (N + 1) * NX); ctx->dut = carve<double>(m, off, B * N * NU);
+    ctx->perf = carve<double>(m, off, B * 4); ctx->flags = carve<int32_t>(m, off, B);
+    ctx->xdes = carve<double>(m, off, B * NX); ctx->udes = carve<double>(m, off, B * NU);
+    ctx->wstatus = carve<int32_t>(m, off, B); ctx->witers = carve<int32_t>(m, off, B); ctx->wmode = carve<int32_t>(m, off, B);
+    ctx->cyc_xref = carve<double>(m, off, B * (N + 1) * NX); ctx->cyc_swing = carve<double>(m, off, B * (N + 1) * 24);
+    ctx->cyc_mode = carve<int32_t>(m, off, B * (N + 1)); ctx->cyc_tk = carve<double>(m, off, B * (N + 1)); ctx->cyc_nn = carve<int32_t>(m, off, B);
+    ctx->res = carve_solution(m, off, B, N);
+    ctx->res_sol = carve<double>(m, off, B * NWBC); ctx->res_stance = carve<double>(m, off, B * 12);
+    return off;
+  });
   // host-pointer calls stage through ctx->arena, which the first such call sizes: contexts driven through device pointers never pay for it
-  if (!ok) { hb_destroy(ctx); return HB_ENOMEM; }
+  if (rc) { hb_destroy(ctx); return rc; }
   {
     cudaError_t fe = cudaSuccess;
     auto attr = [&](const void* fn, size_t bytes) { if (fe == cudaSuccess) fe = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); };
@@ -455,12 +472,9 @@ int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
 int hb_destroy(hb_ctx* ctx) {
   if (!ctx) return HB_EINVAL;
   cudaSetDevice(ctx->device);
-  void* ptrs[] = {ctx->sqp_mem, ctx->dxt, ctx->dut, ctx->perf, ctx->flags, ctx->xdes, ctx->udes, ctx->wstatus, ctx->witers, ctx->wmode,
-                  ctx->hoqp_mem, ctx->cyc_xref, ctx->cyc_swing, ctx->cyc_tk, ctx->cyc_mode, ctx->cyc_nn, ctx->res_t0, ctx->res_xt,
-                  ctx->res_ut, ctx->res_tk, ctx->res_mode, ctx->res_nn, ctx->res_sol, ctx->res_stance, ctx->arena, ctx->ro_mem, ctx->re_mem,
-                  ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->goal_mem, ctx->plan_targets.dev,
-                  ctx->latencies.dev, ctx->pol_mem};
-  for (void* p : ptrs) if (p) cudaFree(p);
+  void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->arena,
+                       ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev};
+  for (void* p : mem) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
   if (ctx->stream_aux) cudaStreamDestroy(ctx->stream_aux);
@@ -633,9 +647,12 @@ int hb_mpc_solve_grid_batch_dev(hb_ctx* ctx, int B, const double* x0, const doub
 static int policy_eval_impl(hb_ctx* ctx, int B, double t_rel, const double* x_traj, const double* u_traj, const int32_t* mode, double* x_des,
                             double* u_des, int32_t* mode_out, const double* tk, const int32_t* nn) {
   ENTER(ctx, B, x_traj && u_traj && mode && x_des && u_des && (tk == nullptr) == (nn == nullptr), UNCAPPED);
+  // the caller's solution, which the kernel only reads; no solve time: it is evaluated at t_rel
+  const SolutionRows s{nullptr, const_cast<double*>(x_traj), const_cast<double*>(u_traj), const_cast<double*>(tk), const_cast<int32_t*>(mode),
+                       const_cast<int32_t*>(nn)};
   const int wpb = 4;
-  return launch(ctx, K_UNPROFILED, policy_eval_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, ctx->cfg.horizon_N, ctx->cfg.dt, t_rel, x_traj, u_traj, mode,
-                x_des, u_des, mode_out, tk, nn, nullptr, nullptr, PolicyChoice{});
+  return launch(ctx, K_UNPROFILED, policy_eval_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, ctx->cfg.horizon_N, ctx->cfg.dt, t_rel, s, x_des, u_des,
+                mode_out, nullptr, PolicyChoice{});
 }
 
 int hb_policy_eval_batch_dev(hb_ctx* ctx, int B, double t_rel, const double* x_traj, const double* u_traj, const int32_t* mode, double* x_des,
@@ -694,11 +711,10 @@ static int resident_cycle_impl(hb_ctx* ctx, int B, int cold_start, double t_rel,
   ENTER(ctx, B, t0 && x0 && refs && rbd, CAPPED, [&] { return cold_start || ctx->res_valid >= ctx->base + B; });   // a warm start shifts the previous solution
   const size_t N = ctx->cfg.horizon_N, o = (size_t)ctx->base;
   double* xref = ctx->cyc_xref + o * (N + 1) * NX; double* swing = ctx->cyc_swing + o * (N + 1) * 24; int32_t* mode = ctx->cyc_mode + o * (N + 1);
-  double* xt = ctx->res_xt + o * (N + 1) * NX; double* ut = ctx->res_ut + o * N * NU; double* tres = ctx->res_t0 + o;
   // event-node grids (cfg.event_nodes): per-instance node times, kept resident beside the primal solution
   const bool grid = ctx->cfg.event_nodes != 0;
+  const SolutionRows res = rows_at(ctx->res, o, N, grid);
   double* tk = grid ? ctx->cyc_tk + o * (N + 1) : nullptr; int32_t* nn = grid ? ctx->cyc_nn + o : nullptr;
-  double* tkres = grid ? ctx->res_tk + o * (N + 1) : nullptr; int32_t* nnres = grid ? ctx->res_nn + o : nullptr;
   int rc = HB_OK;
   if (grid) {
     rc = hb_time_grid_batch_dev(ctx, B, t0, refs, tk, nn, nullptr);
@@ -709,17 +725,17 @@ static int resident_cycle_impl(hb_ctx* ctx, int B, int cold_start, double t_rel,
   }
   if (rc) return rc;
   if (cold_start) {
-    rc = hb_mpc_cold_start_batch_dev(ctx, B, x0, mode, xt, ut);
-    if (!rc) rc = launch(ctx, K_UNPROFILED, set_times_kernel, (B + 127) / 128, 128, 0, B, (int)N, t0, tres, tk, nn, tkres, nnres);
+    rc = hb_mpc_cold_start_batch_dev(ctx, B, x0, mode, res.xt, res.ut);
+    if (!rc) rc = launch(ctx, K_UNPROFILED, set_times_kernel, (B + 127) / 128, 128, 0, B, (int)N, t0, tk, nn, res);
   } else {
     const size_t smem = sizeof(double) * ((N + 1) * NX + N * NU);     // opted in at hb_create
-    rc = launch(ctx, K_UNPROFILED, warm_shift_kernel, B, 128, smem, B, (int)N, ctx->cfg.dt, t0, tres, x0, mode, xt, ut, tk, nn, tkres, nnres);
+    rc = launch(ctx, K_UNPROFILED, warm_shift_kernel, B, 128, smem, B, (int)N, ctx->cfg.dt, t0, x0, mode, tk, nn, res);
   }
   if (rc) return rc;
-  CK(cudaMemcpyAsync(ctx->res_mode + o * (N + 1), mode, sizeof(int32_t) * B * (N + 1), cudaMemcpyDeviceToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(res.mode, mode, sizeof(int32_t) * B * (N + 1), cudaMemcpyDeviceToDevice, ctx->stream));
   if (ctx->res_valid < ctx->base + B) ctx->res_valid = ctx->base + B;
-  if (!run_wbc) return mpc_solve_impl(ctx, B, x0, xref, swing, mode, xt, ut, info, tk, nn);
-  rc = control_step_impl(ctx, B, t_rel, x0, xref, swing, mode, rbd, xt, ut, info, wbc_sol, torque, wbc_status, tk, nn);
+  if (!run_wbc) return mpc_solve_impl(ctx, B, x0, xref, swing, mode, res.xt, res.ut, info, tk, nn);
+  rc = control_step_impl(ctx, B, t_rel, x0, xref, swing, mode, rbd, res.xt, res.ut, info, wbc_sol, torque, wbc_status, tk, nn);
   return rc ? rc : wbc_fallback(ctx, B, cold_start != 0, wbc_status, wbc_sol, torque);
 }
 
@@ -734,19 +750,17 @@ static const hbplan::PlanConsts& plan_consts() {
   return pc;
 }
 
-// The device planner after the entry checks: instance i < n_targets plans on targets[i] where captured is null or captured[i] >= 0
+// The device planner after the entry checks: an instance with a record in targets plans on it where captured is null or captured[i] >= 0
 static int plan_dev(hb_ctx* ctx, int B, const hb_plan_input* in, const double* feet, double* latest_stance, hb_reference* out, int32_t* status,
-                    const hb_target* targets, const int32_t* captured, int n_targets) {
+                    InstanceView<hb_target> targets, const int32_t* captured) {
   return launch(ctx, K_UNPROFILED, plan_references_coop_kernel, (B + 7) / 8, 32, 0, B, in, feet, latest_stance, out, status, plan_consts(), targets,
-                captured, n_targets);
+                captured);
 }
 
 int hb_plan_references_batch_dev(hb_ctx* ctx, int B, const hb_plan_input* in, const double* feet, double* latest_stance, hb_reference* out,
                                  int32_t* status) {
   ENTER(ctx, B, in && latest_stance && out, UNCAPPED);
-  // the explicit targets of the instances this call plans (a chunk of a host-pointer call starts at instance ctx->base)
-  const int n_tg = ctx->plan_targets.n - ctx->base;
-  return plan_dev(ctx, B, in, feet, latest_stance, out, status, n_tg > 0 ? ctx->plan_targets.dev + ctx->base : nullptr, nullptr, n_tg);
+  return plan_dev(ctx, B, in, feet, latest_stance, out, status, ctx->plan_targets.view(ctx->base), nullptr);
 }
 
 int hb_default_kf_params(hb_kf_params* p) {
@@ -934,16 +948,15 @@ int hb_actuation_batch_dev(hb_ctx* ctx, int B, double delay, const double* time,
   return launch(ctx, K_UNPROFILED, actuation_kernel, (B + 63) / 64, 64, 0, B, delay, time, state, command, rbd, tau);
 }
 
-// the plant step after the entry checks; wrench (B x 6) nullable; var (nullable): the plants of instances 0 .. n_var - 1; ter (nullable):
-// the ground under instances 0 .. n_ter - 1
-static int sim_step(hb_ctx* ctx, int B, const hb_sim_params& params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* var,
-                    int n_var, const hb_terrain* ter, int n_ter, double* contact_force, uint8_t* contact_flag) {
-  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, params, rbd, tau, wrench, var, n_var, ter, n_ter, contact_force, contact_flag);
+// the plant step after the entry checks; wrench (B x 6) nullable; var: the plants of the instances, ter: the ground under them
+static int sim_step(hb_ctx* ctx, int B, const hb_sim_params& params, double* rbd, const double* tau, const double* wrench,
+                    InstanceView<hb_plant_variation> var, InstanceView<hb_terrain> ter, double* contact_force, uint8_t* contact_flag) {
+  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, params, rbd, tau, wrench, var, ter, contact_force, contact_flag);
 }
 
 int hb_sim_step_batch_dev(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {
   ENTER(ctx, B, params && rbd && tau && sim_params_ok(*params), UNCAPPED);
-  return sim_step(ctx, B, *params, rbd, tau, nullptr, nullptr, 0, nullptr, 0, contact_force, contact_flag);
+  return sim_step(ctx, B, *params, rbd, tau, nullptr, {}, {}, contact_force, contact_flag);
 }
 
 int hb_default_plant_variation(hb_plant_variation* v) {
@@ -1040,32 +1053,18 @@ static bool latency_ok(const int32_t& d) { return d >= 0; }     // the upper bou
 
 int hb_rollout_set_mpc_latencies(hb_ctx* ctx, int B, const int32_t* ticks) { return set_instances(ctx, B, ticks, latency_ok, &hb_ctx::latencies); }
 
-// the resident solution of instances [o, ...) as SolutionRows (grid rows only on event-node contexts)
-static SolutionRows resident_rows(hb_ctx* ctx, size_t o) {
-  const size_t N = ctx->cfg.horizon_N;
-  const bool grid = ctx->cfg.event_nodes != 0;
-  return SolutionRows{ctx->res_t0 + o, ctx->res_xt + o * (N + 1) * NX, ctx->res_ut + o * N * NU, grid ? ctx->res_tk + o * (N + 1) : nullptr,
-                      ctx->res_mode + o * (N + 1), grid ? ctx->res_nn + o : nullptr};
-}
-
-// The adopted policy of instances [o, ...), allocated at max_batch by its first use (hb_policy_update, an episode with a latency set)
-static int policy_rows(hb_ctx* ctx, size_t o, SolutionRows* rows) {
-  const size_t Bc = ctx->cfg.max_batch, N = ctx->cfg.horizon_N;
+// The adopted policy ctx->pol, allocated at max_batch by its first use (hb_policy_update, an episode with a latency set)
+static int policy_reserve(hb_ctx* ctx) {
+  const size_t Bc = ctx->cfg.max_batch;
   const int rc = reserve_group(&ctx->pol_mem, [&](void* m) {
     size_t off = 0;
-    SolutionRows& p = ctx->pol;
-    p.t0 = carve<double>(m, off, Bc); p.xt = carve<double>(m, off, Bc * (N + 1) * NX); p.ut = carve<double>(m, off, Bc * N * NU);
-    p.tk = carve<double>(m, off, Bc * (N + 1)); p.mode = carve<int32_t>(m, off, Bc * (N + 1)); p.nn = carve<int32_t>(m, off, Bc);
+    ctx->pol = carve_solution(m, off, Bc, ctx->cfg.horizon_N);
     return off;
   });
   if (rc) return rc;
   if (ctx->pol_have.size() != Bc) {
     try { ctx->pol_have.assign(Bc, 0); } catch (const std::bad_alloc&) { return HB_ENOMEM; }
   }
-  const bool grid = ctx->cfg.event_nodes != 0;
-  const SolutionRows& p = ctx->pol;
-  *rows = SolutionRows{p.t0 + o, p.xt + o * (N + 1) * NX, p.ut + o * N * NU, grid ? p.tk + o * (N + 1) : nullptr, p.mode + o * (N + 1),
-                       grid ? p.nn + o : nullptr};
   return HB_OK;
 }
 
@@ -1076,14 +1075,15 @@ static bool policies_adopted(const hb_ctx* ctx, size_t lo, size_t hi) {
   return true;
 }
 
-// policy_adopt_kernel on instances [0, B) after the entry checks: with lat the episodes' rule at `tick`, otherwise the update mask
-static int policy_adopt(hb_ctx* ctx, int B, const int32_t* lat, int n_lat, long long tick, int every, const uint8_t* update) {
-  SolutionRows to;
-  const int rc = policy_rows(ctx, (size_t)ctx->base, &to);
+// policy_adopt_kernel on instances [0, B) after the entry checks: with lat set the episodes' rule at `tick`, otherwise the update mask
+static int policy_adopt(hb_ctx* ctx, int B, InstanceView<int32_t> lat, long long tick, int every, const uint8_t* update) {
+  const int rc = policy_reserve(ctx);
   if (rc) return rc;
+  const size_t N = ctx->cfg.horizon_N, o = (size_t)ctx->base;
+  const bool grid = ctx->cfg.event_nodes != 0;
   const int wpb = 4;
-  return launch(ctx, K_UNPROFILED, policy_adopt_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, (int)ctx->cfg.horizon_N, lat, n_lat, tick, every, update,
-                resident_rows(ctx, (size_t)ctx->base), to);
+  return launch(ctx, K_UNPROFILED, policy_adopt_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, (int)N, lat, tick, every, update, rows_at(ctx->res, o, N, grid),
+                rows_at(ctx->pol, o, N, grid));
 }
 
 // hb_resident_wbc_batch_dev; no_prev = true: the fallback has no previous solution yet (first tick after a cold start whose cycle ran no WBC).
@@ -1095,13 +1095,11 @@ static int resident_wbc_impl(hb_ctx* ctx, int B, const double* t_now, const doub
   ENTER(ctx, B, t_now && rbd && x_des && u_des && mode_out && wbc_sol, UNCAPPED, [&] {   // a solution to evaluate
     return adopted ? policies_adopted(ctx, (size_t)ctx->base, (size_t)ctx->base + B) : ctx->base + B <= ctx->res_valid;
   });
-  const size_t N = ctx->cfg.horizon_N, o = (size_t)ctx->base;
-  SolutionRows s = resident_rows(ctx, o);
-  int rc = adopted ? policy_rows(ctx, o, &s) : HB_OK;
-  if (rc) return rc;
+  const size_t N = ctx->cfg.horizon_N;   // adopted: policies_adopted() passed, so the adopted rows are allocated
+  const SolutionRows s = rows_at(adopted ? ctx->pol : ctx->res, (size_t)ctx->base, N, ctx->cfg.event_nodes != 0);
   const int wpb = 4;
-  rc = launch(ctx, K_UNPROFILED, policy_eval_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, (int)N, ctx->cfg.dt, 0.0, s.xt, s.ut, s.mode, x_des, u_des,
-              mode_out, s.tk, s.nn, t_now, s.t0, choice);
+  int rc = launch(ctx, K_UNPROFILED, policy_eval_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, (int)N, ctx->cfg.dt, 0.0, s, x_des, u_des, mode_out, t_now,
+                  choice);
   if (!rc) rc = controller_wbc_dev(ctx, B, x_des, u_des, rbd, mode_out, stance_mode, wbc_sol, wbc_status);
   if (!rc && torque) rc = launch(ctx, K_UNPROFILED, torque_kernel, (B * NJ + 127) / 128, 128, 0, B, wbc_sol, torque);
   return rc ? rc : wbc_fallback(ctx, B, no_prev, wbc_status, wbc_sol, torque);
@@ -1167,9 +1165,9 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   const bool params_ok = p && p->mpc_every >= 1 && p->period > 0.0 && p->log_every >= 0 && delay_ok(p->actuation_delay) && sim_params_ok(p->sim) &&
                          tick0 + n_ticks <= INT32_MAX && (!e || (e->ep && e->est && sensor_noise_ok(e->ep->noise)));
   const bool cold = tick0 == 0;
-  // the MPC latencies of this batch's instances (hb_rollout_set_mpc_latencies): instances i < n_lat have one
+  // the MPC latencies of this batch's instances (hb_rollout_set_mpc_latencies): instances i < with_lat have one
   const InstanceSetting<int32_t>& lat = ctx->latencies;
-  const int n_lat = std::min(lat.n, B);
+  const int with_lat = std::min(lat.n, B);
   ENTER(ctx, B, n_ticks >= 0 && tick0 >= 0 && cmd && rbd && act && estop && stats && params_ok, CAPPED, [&] {
     for (int i = 0; i < B; ++i) {
       const hb_rollout_command& c = cmd[i];
@@ -1178,7 +1176,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
     }
     for (int i = 0; i < lat.n; ++i) if (lat.host[i] > p->mpc_every) return false;     // latencies beyond one MPC period
     // a warm start continues from the resident solution, and the instances with a latency from their adopted policies
-    for (int i = 0; i < n_lat && !cold; ++i) if (lat.host[i] >= 1 && !policies_adopted(ctx, i, i + 1)) return false;
+    for (int i = 0; i < with_lat && !cold; ++i) if (lat.host[i] >= 1 && !policies_adopted(ctx, i, i + 1)) return false;
     return cold || ctx->res_valid >= B;
   });
   if (n_ticks == 0) return HB_OK;
@@ -1189,7 +1187,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   // instance adopts on tick a iff a >= first_due[a % mpc_every]; the policy evaluation chooses per instance (PolicyChoice).
   std::vector<int> first_due;
   PolicyChoice choice{};
-  for (int i = 0; i < n_lat; ++i) {
+  for (int i = 0; i < with_lat; ++i) {
     const int d = lat.host[i];
     if (d < 1) continue;
     if (first_due.empty()) first_due.assign(p->mpc_every, INT_MAX);
@@ -1197,9 +1195,9 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   }
   const bool delayed = !first_due.empty();
   if (delayed) {
-    rc = policy_rows(ctx, 0, &choice.adopted);
+    rc = policy_reserve(ctx);
     if (rc) return rc;
-    choice.lat = lat.dev; choice.n_lat = n_lat;
+    choice = PolicyChoice{lat.view(), rows_at(ctx->pol, 0, ctx->cfg.horizon_N, ctx->cfg.event_nodes != 0)};
   }
   CK(cudaMemcpyAsync(ctx->ro_cmd, cmd, sizeof(hb_rollout_command) * B, cudaMemcpyHostToDevice, ctx->stream));
   const double horizon = (ctx->cfg.event_nodes && ctx->cfg.time_horizon > 0.0) ? ctx->cfg.time_horizon : ctx->cfg.horizon_N * ctx->cfg.dt;
@@ -1208,19 +1206,16 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   const unsigned grid = (B + 63) / 64;
   // what the controllers measure: the true state, or the filter's estimate
   double* meas = e ? ctx->re_rbd : rbd;
-  // the episode settings (null while unset); the push wrench the begin kernel writes and the plant applies, none without schedules
-  const hb_push_schedule* push = ctx->pushes.get();
-  const hb_plant_variation* var = ctx->variations.get();
-  const hb_terrain* ter = ctx->terrains.get();
-  double* wrench = push ? ctx->ro_wrench : nullptr;
-  const hb_goal_schedule* goals = ctx->goals.get();          // with goals, the plan-input kernel captures them and the planner reads the captures
+  // the push wrench the begin kernel writes and the plant applies, none without schedules
+  double* wrench = ctx->pushes.n > 0 ? ctx->ro_wrench : nullptr;
+  const InstanceView<hb_target> goal_targets{ctx->goal_tg, ctx->goals.n};    // what the planner reads: the targets of the captured goals
   for (int k = 0; k < n_ticks && !rc; ++k) {
     const int64_t a = tick0 + k;
     const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
     const bool mpc = a % p->mpc_every == 0, first_cold = cold && k == 0;
     double* log_row = (n_log && k % p->log_every == 0) ? log + (size_t)(k / p->log_every) * 32 : nullptr;
     rc = launch(ctx, K_UNPROFILED, rollout_tick_begin_kernel, grid, 64, 0, B, (int)a, t, p->min_base_height, rbd, ctx->ro_held, stats, ctx->ro_tnow,
-                log_row, (size_t)n_log * 32, push, ctx->pushes.n, wrench, ter, ctx->terrains.n);
+                log_row, (size_t)n_log * 32, ctx->pushes.view(), wrench, ctx->terrains.view());
     if (!rc && e) {
       // LeggedController::updateStateEstimation: sensors and contact flags at the previous observation's time, filter, observation step
       double* est_row = (n_est_log && k % p->log_every == 0) ? e->log + (size_t)(k / p->log_every) * 32 : nullptr;
@@ -1231,19 +1226,18 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
       if (!rc) rc = launch(ctx, K_UNPROFILED, est_observe_kernel, grid, 64, 0, B, rbd, meas, stats, e->est, e->stats, est_row, (size_t)n_est_log * 32);
     }
     // MPC_MRT_Interface::updatePolicy of the instances whose solution comes into force on this tick, before this tick's cycle
-    if (!rc && delayed && a >= first_due[a % p->mpc_every]) rc = policy_adopt(ctx, B, lat.dev, n_lat, a, p->mpc_every, nullptr);
+    if (!rc && delayed && a >= first_due[a % p->mpc_every]) rc = policy_adopt(ctx, B, lat.view(), a, p->mpc_every, nullptr);
     if (!rc && mpc) {
       if (first_cold) CK(cudaMemsetAsync(ctx->res_stance, 0, sizeof(double) * B * 12, ctx->stream));   // latestStanceposition_ starts at zero
-      rc = launch(ctx, K_UNPROFILED, rollout_plan_inputs_kernel, grid, 64, 0, B, t, horizon, ctx->ro_cmd, meas, e ? e->est : nullptr, ctx->ro_in, goals,
-                  ctx->goals.n, first_cold ? 1 : 0, ctx->goal_tg, ctx->goal_idx, plan_consts());
+      rc = launch(ctx, K_UNPROFILED, rollout_plan_inputs_kernel, grid, 64, 0, B, t, horizon, ctx->ro_cmd, meas, e ? e->est : nullptr, ctx->ro_in,
+                  ctx->goals.view(), first_cold ? 1 : 0, ctx->goal_tg, ctx->goal_idx, plan_consts());
       if (!rc) rc = launch(ctx, K_UNPROFILED, plan_prepare_kernel, grid, 64, 0, B, ctx->ro_in, ctx->ro_t0, ctx->ro_x0, ctx->ro_feet);
-      if (!rc) rc = plan_dev(ctx, B, ctx->ro_in, ctx->ro_feet, ctx->res_stance, ctx->ro_refs, ctx->ro_pstat, goals ? ctx->goal_tg : nullptr, ctx->goal_idx,
-                             ctx->goals.n);
+      if (!rc) rc = plan_dev(ctx, B, ctx->ro_in, ctx->ro_feet, ctx->res_stance, ctx->ro_refs, ctx->ro_pstat, goal_targets, ctx->goal_idx);
       if (!rc) rc = resident_cycle_impl(ctx, B, first_cold, 0.0, ctx->ro_t0, ctx->ro_x0, ctx->ro_refs, meas, ctx->ro_info, nullptr, nullptr, nullptr, false);
       // the cold tick: every instance with a latency starts with the policy of this first solve
       if (!rc && delayed && first_cold) {
-        rc = policy_adopt(ctx, B, lat.dev, n_lat, -1, p->mpc_every, nullptr);
-        for (int i = 0; i < n_lat && !rc; ++i) if (lat.host[i] >= 1) ctx->pol_have[i] = 1;
+        rc = policy_adopt(ctx, B, lat.view(), -1, p->mpc_every, nullptr);
+        for (int i = 0; i < with_lat && !rc; ++i) if (lat.host[i] >= 1) ctx->pol_have[i] = 1;
       }
       if (!rc && e) rc = launch(ctx, K_UNPROFILED, est_schedule_kernel, grid, 64, 0, B, ctx->ro_refs, e->est);
     }
@@ -1254,7 +1248,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
                                              ctx->ro_jtau);
     if (!rc) rc = hb_actuation_batch_dev(ctx, B, p->actuation_delay, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, ctx->ro_tau);
-    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, var, ctx->variations.n, ter, ctx->terrains.n, nullptr, nullptr);
+    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, ctx->variations.view(), ctx->terrains.view(), nullptr, nullptr);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_tick_end_kernel, grid, 64, 0, B, (int)a, mpc ? 1 : 0, ctx->ro_info, ctx->ro_pstat, ctx->wstatus, estop, ctx->ro_tau, ctx->ro_held, rbd, stats);
   }
   return rc;
@@ -1484,9 +1478,10 @@ int hb_resident_write_batch(hb_ctx* ctx, int B, const double* t0, const double* 
   const bool grid = ctx->cfg.event_nodes != 0;
   const size_t N = ctx->cfg.horizon_N;
   const int rc = drain(ctx, [&]() -> int {
-    H2D(ctx->res_t0, t0, sizeof(double) * B); H2D(ctx->res_xt, x_traj, sizeof(double) * B * (N + 1) * NX); H2D(ctx->res_ut, u_traj, sizeof(double) * B * N * NU);
-    if (mode) H2D(ctx->res_mode, mode, sizeof(int32_t) * B * (N + 1));
-    if (grid) { H2D(ctx->res_tk, node_times, sizeof(double) * B * (N + 1)); H2D(ctx->res_nn, n_intervals, sizeof(int32_t) * B); }
+    const SolutionRows& r = ctx->res;
+    H2D(r.t0, t0, sizeof(double) * B); H2D(r.xt, x_traj, sizeof(double) * B * (N + 1) * NX); H2D(r.ut, u_traj, sizeof(double) * B * N * NU);
+    if (mode) H2D(r.mode, mode, sizeof(int32_t) * B * (N + 1));
+    if (grid) { H2D(r.tk, node_times, sizeof(double) * B * (N + 1)); H2D(r.nn, n_intervals, sizeof(int32_t) * B); }
     return HB_OK;
   }());
   if (rc) return rc;
@@ -1498,7 +1493,7 @@ int hb_resident_read_grid_batch(hb_ctx* ctx, int B, double* node_times, int32_t*
   ENTER(ctx, B, node_times && n_intervals, UNCAPPED, [&] { return B <= ctx->res_valid && ctx->cfg.event_nodes; });
   const size_t N = ctx->cfg.horizon_N;
   return drain(ctx, [&]() -> int {
-    D2H(node_times, ctx->res_tk, sizeof(double) * B * (N + 1)); D2H(n_intervals, ctx->res_nn, sizeof(int32_t) * B);
+    D2H(node_times, ctx->res.tk, sizeof(double) * B * (N + 1)); D2H(n_intervals, ctx->res.nn, sizeof(int32_t) * B);
     return HB_OK;
   }());
 }
@@ -1612,9 +1607,9 @@ int hb_resident_read_batch(hb_ctx* ctx, int B, double* t0, double* x_traj, doubl
   ENTER(ctx, B, true, UNCAPPED, [&] { return B <= ctx->res_valid; });
   const size_t N = ctx->cfg.horizon_N;
   return drain(ctx, [&]() -> int {
-    if (t0) D2H(t0, ctx->res_t0, sizeof(double) * B);
-    if (x_traj) D2H(x_traj, ctx->res_xt, sizeof(double) * B * (N + 1) * NX);
-    if (u_traj) D2H(u_traj, ctx->res_ut, sizeof(double) * B * N * NU);
+    if (t0) D2H(t0, ctx->res.t0, sizeof(double) * B);
+    if (x_traj) D2H(x_traj, ctx->res.xt, sizeof(double) * B * (N + 1) * NX);
+    if (u_traj) D2H(u_traj, ctx->res.ut, sizeof(double) * B * N * NU);
     return HB_OK;
   }());
 }
@@ -1679,7 +1674,7 @@ int hb_sim_step_terrain(hb_ctx* ctx, int B, const hb_sim_params* params, double*
   Staging s(ctx, B);
   auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto w = s.in_or_null(wrench, 6); auto pv = s.in_or_null(v, 1); auto pt = s.in_or_null(ter, 1);
   auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
-  return s.run(1, [&](Chunk) { return sim_step(ctx, B, *params, r, t, w, pv, v ? B : 0, pt, ter ? B : 0, cf, fl); });
+  return s.run(1, [&](Chunk) { return sim_step(ctx, B, *params, r, t, w, {pv, B}, {pt, B}, cf, fl); });
 }
 
 int hb_resident_wbc_batch(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
@@ -1699,7 +1694,7 @@ int hb_policy_update(hb_ctx* ctx, int B, const uint8_t* update) {
   });
   Staging s(ctx, B);
   auto up = s.in_or_null(update, 1);
-  const int rc = s.run(1, [&](Chunk) { return policy_adopt(ctx, B, nullptr, 0, 0, 1, up); });
+  const int rc = s.run(1, [&](Chunk) { return policy_adopt(ctx, B, {}, 0, 1, up); });
   if (rc) return rc;
   for (int i = 0; i < B; ++i) if (!update || update[i]) ctx->pol_have[i] = 1;
   return HB_OK;

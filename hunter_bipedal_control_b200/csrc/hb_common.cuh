@@ -56,4 +56,12 @@ __device__ __forceinline__ bool contact_flag(int mode, int c) {
   return (c & 1) ? (mode == 1 || mode == 3) : (mode == 2 || mode == 3);
 }
 
+// A per-robot setting as the kernels read it, passed by value: instances 0 .. n - 1 have a record. Default-constructed, it is unset.
+template <class T> struct InstanceView {
+  const T* recs;
+  int n;
+  // the record of instance i; null when the view is unset or i is beyond it
+  __host__ __device__ __forceinline__ const T* of(int i) const { return (recs && i < n) ? recs + i : nullptr; }
+};
+
 }  // namespace hb

@@ -247,11 +247,11 @@ __global__ void plan_prepare_kernel(int B, const hb_plan_input* in, double* t0, 
 // instance builds the two-sample target in shared memory, thread r plans foot r on it (the feet are independent), thread 0 resamples it,
 // then threads 0 and 1 run the IK of the left / right leg on the resampled target, then thread 0 writes the schedule and the targets.
 // Same functions as the host planner, so the plan is the same. The targets (2.9 KB each) live in shared memory only: no thread keeps
-// a copy on its stack. targets (nullable): instance inst < n_targets plans on targets[inst] instead of its cmd_vel target, where
-// captured (nullable: every such instance) has captured[inst] >= 0 (a goal an episode captured).
+// a copy on its stack. An instance with a record in targets plans on it instead of its cmd_vel target, where captured (nullable: every
+// such instance) has captured[inst] >= 0 (a goal an episode captured).
 __global__ void __launch_bounds__(32) plan_references_coop_kernel(int B, const hb_plan_input* in, const double* feet, double* latest_stance,
-                                                                  hb_reference* out, int32_t* status, hbplan::PlanConsts pc, const hb_target* targets,
-                                                                  const int32_t* captured, int n_targets) {
+                                                                  hb_reference* out, int32_t* status, hbplan::PlanConsts pc,
+                                                                  InstanceView<hb_target> targets, const int32_t* captured) {
   __shared__ hbplan::Target s_tg[8], s_old[8];
   __shared__ int s_rc[8];
   const int g = threadIdx.x >> 2, r = threadIdx.x & 3;
@@ -271,7 +271,8 @@ __global__ void __launch_bounds__(32) plan_references_coop_kernel(int B, const h
     tf = p.t0 + p.horizon; t_lo = p.t0 - 1e-9; t_hi = tf + 1e-9;
     if (rc == 0 && !hbplan::tile_gait(p.gait, p.prev_event, p.gait_start, p.t0 - p.horizon, tf + p.horizon, ms)) rc = -5;
     if (rc == 0 && r == 0) {
-      if (targets && inst < n_targets && (!captured || captured[inst] >= 0)) hbplan::target_from(targets[inst], s_tg[g]);
+      const hb_target* tg = targets.of(inst);
+      if (tg && (!captured || captured[inst] >= 0)) hbplan::target_from(*tg, s_tg[g]);
       else s_tg[g] = hbplan::cmd_vel_to_target(pc, p.cmd_vel, p.t0, p.x0, p.time_to_target);
     }
   }

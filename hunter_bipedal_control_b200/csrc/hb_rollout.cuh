@@ -13,10 +13,10 @@ namespace hb {
 // cmd_vel of the last command segment that has started (the first one before that), prev_event = min(t, gait_start) - 0.5, IK joint
 // references. feet_pos is left zero: plan_prepare_kernel computes the feet from x0. With est (estimated episodes) x0[9] is the unwrapped
 // observation yaw (LeggedController.cpp:335-337).
-// Goals (hb_goal_schedule, hunter_b200.h) of instances inst < n_goals: the goal in force at t is captured, target and index, when it differs
+// Goals (hb_goal_schedule, hunter_b200.h) of the instances that have one: the goal in force at t is captured, target and index, when it differs
 // from the captured one (captured_idx -1: none); reset (an episode's tick 0) forgets the captured goal first. The planner reads them.
 __global__ void rollout_plan_inputs_kernel(int B, double t, double horizon, const hb_rollout_command* cmd, const double* rbd, const hb_estimation_state* est,
-                                           hb_plan_input* in, const hb_goal_schedule* goals, int n_goals, int reset, hb_target* captured,
+                                           hb_plan_input* in, InstanceView<hb_goal_schedule> goals, int reset, hb_target* captured,
                                            int32_t* captured_idx, hbplan::PlanConsts pc) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
@@ -31,8 +31,8 @@ __global__ void rollout_plan_inputs_kernel(int B, double t, double horizon, cons
   if (est) p.x0[9] = est[inst].yaw_obs;
   for (int i = 0; i < 12; ++i) p.feet_pos[i] = 0.0;
   p.gait = c.gait; p.joint_ik = 1;
-  if (goals && inst < n_goals) {
-    const hb_goal_schedule& s = goals[inst];
+  if (const hb_goal_schedule* sp = goals.of(inst)) {
+    const hb_goal_schedule& s = *sp;
     int g = -1;
     for (int k = 0; k < s.n_goal; ++k) if (s.time[k] <= t) g = k;
     const int had = reset ? -1 : captured_idx[inst];
@@ -96,17 +96,17 @@ __device__ __forceinline__ void push_wrench(const hb_push_schedule& s, double t,
 // state every held instance is put back to, the tick time goes to every instance (policy evaluation, actuation stamp), and the state is
 // logged when log_row is set. A non-finite state can only enter the first tick of a call (the end kernel never leaves one behind); with no
 // finite state of that instance known, the nominal standing pose replaces it. With wrench set, the tick's push wrench (B x 6) is written
-// for the plant step: from pushes[inst] for inst < n_pushes, zeros for the others. The base height of instances inst < n_terrain is
-// measured above terrain[inst].
+// for the plant step: from the instance's push schedule, zeros without one. The base height of an instance with a terrain is measured
+// above it.
 __global__ void rollout_tick_begin_kernel(int B, int tick, double t, double min_base_height, double* rbd, double* held, hb_rollout_stats* stats,
-                                          double* t_now, double* log_row, size_t log_stride, const hb_push_schedule* pushes, int n_pushes,
-                                          double* wrench, const hb_terrain* terrain, int n_terrain) {
+                                          double* t_now, double* log_row, size_t log_stride, InstanceView<hb_push_schedule> pushes, double* wrench,
+                                          InstanceView<hb_terrain> terrain) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
   double* r = rbd + (size_t)inst * 32;
   double* h = held + (size_t)inst * 32;
   hb_rollout_stats& s = stats[inst];
-  const int why = rollout_state_check(r, min_base_height, (terrain && inst < n_terrain) ? terrain + inst : nullptr);
+  const int why = rollout_state_check(r, min_base_height, terrain.of(inst));
   if (why && s.fail_tick < 0) { s.fail_tick = tick; s.fail_reason = why; }
   if (why & HB_ROLLOUT_FAIL_NONFINITE) {
     const double nominal[NQ] = {0.0, 0.0, 0.0, 0.0, 0.0, HB_INITIAL_STATE[8], HB_INITIAL_STATE[12], HB_INITIAL_STATE[13], HB_INITIAL_STATE[14],
@@ -119,7 +119,7 @@ __global__ void rollout_tick_begin_kernel(int B, int tick, double t, double min_
   if (log_row) for (int i = 0; i < 32; ++i) log_row[inst * log_stride + i] = r[i];
   if (wrench) {
     double* w = wrench + (size_t)inst * 6;
-    if (inst < n_pushes) push_wrench(pushes[inst], t, w);
+    if (const hb_push_schedule* ps = pushes.of(inst)) push_wrench(*ps, t, w);
     else for (int c = 0; c < 6; ++c) w[c] = 0.0;
   }
 }
@@ -355,9 +355,9 @@ __global__ void actuation_kernel(int B, double delay, const double* time, hb_act
 // Same rigid-body passes as the WBC assembly: lanes 0-15 unit-velocity sweeps -> J_c columns, lanes 0-15 RNEA with unit accelerations ->
 // M columns, lane 16 -> nle; 16 x 16 Cholesky in shared memory. One warp per instance. wrench (B x 6, nullable): an external world force at
 // the base origin and a world couple, which enter as the generalised forces Q_p = f, Q_zyx = T' tau with omega_world = T(zyx) zyx_dot
-// (world_omega_from_zyx_rates, hb_rbd.cuh); null adds nothing. var (nullable): the plants of instances 0 .. n_var - 1 (varied
-// plants, hunter_b200.h); the others, and every instance with a null var, run the nominal plant. terrain (nullable): the ground under
-// instances 0 .. n_terrain - 1 (terrain, hunter_b200.h); the others stand on flat ground at prm.ground_height.
+// (world_omega_from_zyx_rates, hb_rbd.cuh); null adds nothing. var: the plants of the instances that have one (varied plants,
+// hunter_b200.h); the others run the nominal plant. terrain: the ground under the instances that have one (terrain, hunter_b200.h); the
+// others stand on flat ground at prm.ground_height.
 struct SimShared { double q[NQ], v[NQ], J[12 * NQ], M[NQ * 17], nle[NQ], rhs[NQ], t1[NQ], t2[NQ], kdi[NQ], F[12], cpos[12], cvel[12]; };
 
 // The payload of a varied plant in one RNEA lane: rnea_pass's base-body wrench for a rigid body fixed to the base with mass m, CoM c and
@@ -395,13 +395,14 @@ __device__ __forceinline__ double sloped_contact(const double* p, const double* 
   return fn;
 }
 
+// The views are __grid_constant__ (read in place, never copied): as plain by-value parameters they cost the kernel two registers.
 __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, double* rbd_io, const double* tau, const double* wrench,
-                                                      const hb_plant_variation* var, int n_var, const hb_terrain* terrain, int n_terrain,
-                                                      double* contact_force, uint8_t* contact_flag) {
+                                                      const __grid_constant__ InstanceView<hb_plant_variation> var,
+                                                      const __grid_constant__ InstanceView<hb_terrain> terrain, double* contact_force, uint8_t* contact_flag) {
   __shared__ SimShared sh;
   const int inst = blockIdx.x, lane = threadIdx.x;
-  const hb_plant_variation* pv = (var && inst < n_var) ? var + inst : nullptr;      // null: the nominal plant
-  const hb_terrain* ter = (terrain && inst < n_terrain) ? terrain + inst : nullptr;  // null: flat ground at prm.ground_height
+  const hb_plant_variation* pv = var.of(inst);      // null: the nominal plant
+  const hb_terrain* ter = terrain.of(inst);         // null: flat ground at prm.ground_height
   bool touch = false;                    // lanes 0-3: the normal force of their contact in the last substep is positive
   double* r = rbd_io + (size_t)inst * 32;
   if (lane == 0) rbd_to_qv(r, sh.q, sh.v);
