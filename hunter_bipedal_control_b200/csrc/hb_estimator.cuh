@@ -222,24 +222,58 @@ __global__ void __launch_bounds__(32) contact_force_kernel(int B, double lambda,
   __syncwarp();
   double* e = est + (size_t)inst * 16;
   if (lane < 2) {
-    // least-norm solution of A w = b, A = S J' (5 x 6): w = A' (A A')^-1 b (the reference takes the SVD solve; same result at full row rank)
+    // least-norm solution of A w = b, A = S J' (5 x 6), as the reference's SVD solve gives it: Householder QR of A' = Q [R; 0], then
+    // w = Q [R^-T b; 0]. A loses rank inside the joint limits (knee ~0.0208 rad, where the hip-pitch, knee and ankle origins line up,
+    // cond(A) ~ 1.8 / |knee - k*|); this solve is backward stable, so the error in w grows like cond(A) eps, where the normal equations
+    // A A' y = b it replaces squared the condition number.
     const double* A = sh.Jf + lane * 30;          // row j = joint j of the leg, 6 columns
-    double Gm[5][6];
+    double M[6][5], vd[5], bt[5], rd[5];          // M = A'; below the diagonal: Householder vectors (leading entries vd), rd = diag R
+#pragma unroll
+    for (int c = 0; c < 6; ++c)
+#pragma unroll
+      for (int j = 0; j < 5; ++j) M[c][j] = A[j * 6 + c];
+#pragma unroll
+    for (int k = 0; k < 5; ++k) {
+      double nn = 0.0;
+#pragma unroll
+      for (int i = k; i < 6; ++i) nn = fma(M[i][k], M[i][k], nn);
+      const double n = sqrt(nn), x0 = M[k][k];
+      const double alpha = x0 >= 0.0 ? -n : n;    // reflect onto -sign(x0) |x| e_k: v_0 = x0 - alpha has no cancellation
+      vd[k] = x0 - alpha;
+      bt[k] = n > 0.0 ? 1.0 / (n * (n + fabs(x0))) : 0.0;      // 2 / (v' v)
+      rd[k] = alpha;
+#pragma unroll
+      for (int j = k + 1; j < 5; ++j) {
+        double s = vd[k] * M[k][j];
+#pragma unroll
+        for (int i = k + 1; i < 6; ++i) s = fma(M[i][k], M[i][j], s);
+        s *= bt[k];
+        M[k][j] -= s * vd[k];
+#pragma unroll
+        for (int i = k + 1; i < 6; ++i) M[i][j] = fma(-s, M[i][k], M[i][j]);
+      }
+    }
+    double w[6];                                  // R' y = b (forward), then w = H_0 ... H_4 [y; 0]
+#pragma unroll
     for (int i = 0; i < 5; ++i) {
-      for (int j = 0; j < 5; ++j) { double s = 0.0; for (int c = 0; c < 6; ++c) s += A[i * 6 + c] * A[j * 6 + c]; Gm[i][j] = s; }
-      Gm[i][5] = sh.taud[6 + 5 * lane + i];
+      double s = sh.taud[6 + 5 * lane + i];
+#pragma unroll
+      for (int j = 0; j < i; ++j) s = fma(-M[j][i], w[j], s);
+      w[i] = s / rd[i];
     }
-    for (int c = 0; c < 5; ++c) {
-      int pv = c; double best = fabs(Gm[c][c]);
-      for (int rr = c + 1; rr < 5; ++rr) if (fabs(Gm[rr][c]) > best) { best = fabs(Gm[rr][c]); pv = rr; }
-      if (pv != c) for (int j = 0; j < 6; ++j) { const double t = Gm[c][j]; Gm[c][j] = Gm[pv][j]; Gm[pv][j] = t; }
-      const double inv = 1.0 / Gm[c][c];
-      for (int rr = c + 1; rr < 5; ++rr) { const double f = Gm[rr][c] * inv; for (int j = c; j < 6; ++j) Gm[rr][j] -= f * Gm[c][j]; }
+    w[5] = 0.0;
+#pragma unroll
+    for (int k = 4; k >= 0; --k) {
+      double s = vd[k] * w[k];
+#pragma unroll
+      for (int i = k + 1; i < 6; ++i) s = fma(M[i][k], w[i], s);
+      s *= bt[k];
+      w[k] -= s * vd[k];
+#pragma unroll
+      for (int i = k + 1; i < 6; ++i) w[i] = fma(-s, M[i][k], w[i]);
     }
-    double y[5];
-    for (int rr = 4; rr >= 0; --rr) { double s = Gm[rr][5]; for (int j = rr + 1; j < 5; ++j) s -= Gm[rr][j] * y[j]; y[rr] = s / Gm[rr][rr]; }
-    double w[6], n3 = 0.0, n6 = 0.0;
-    for (int c = 0; c < 6; ++c) { double s = 0.0; for (int j = 0; j < 5; ++j) s += A[j * 6 + c] * y[j]; w[c] = s; n6 += s * s; if (c < 3) n3 += s * s; }
+    double n3 = 0.0, n6 = 0.0;
+    for (int c = 0; c < 6; ++c) { n6 += w[c] * w[c]; if (c < 3) n3 += w[c] * w[c]; }
     for (int c = 0; c < 6; ++c) e[6 * lane + c] = w[c];
     e[12 + lane] = sqrt(n3);
     e[14 + lane] = sqrt(n6);

@@ -627,6 +627,33 @@ class ContactForceObserverRef:
         return self.est.copy()
 
 
+def foot_wrench_matrix(q, leg):
+    """S_l J_foot' of leg `leg` at the generalised coordinates q (5 x 6): the matrix of estContactForce's per-foot wrench solve."""
+    from . import hbo
+    J = hbo.observer_terms(q, np.zeros(16))[3]
+    return J[leg][:, 6 + 5 * leg:11 + 5 * leg].T
+
+
+def singular_knee(leg, q, lo=0.0, hi=0.05, tol=1e-14):
+    """The knee angle of leg `leg` in [lo, hi] that minimises sigma_min / sigma_max of foot_wrench_matrix, the other coordinates from q:
+    golden-section search (the ratio is unimodal there, |knee - k*| / 1.8 near its zero)."""
+    def ratio(k):
+        qk = np.array(q, dtype=float); qk[6 + 5 * leg + 3] = k
+        s = np.linalg.svd(foot_wrench_matrix(qk, leg), compute_uv=False)
+        return s[-1] / s[0]
+    g = (math.sqrt(5.0) - 1.0) / 2.0
+    c, d = hi - g * (hi - lo), lo + g * (hi - lo)
+    fc, fd = ratio(c), ratio(d)
+    while hi - lo > tol:
+        if fc < fd:
+            hi, d, fd = d, c, fc
+            c = hi - g * (hi - lo); fc = ratio(c)
+        else:
+            lo, c, fc = c, d, fd
+            d = lo + g * (hi - lo); fd = ratio(d)
+    return 0.5 * (lo + hi)
+
+
 class KalmanFilterRef:
     def __init__(self):
         self.x = np.zeros(18); self.P = 100.0 * np.eye(18); self.heights = np.zeros(4)
@@ -670,7 +697,8 @@ class KalmanFilterRef:
         self.x = self.x + pm @ self.c.T @ np.linalg.solve(s, ey)
         p = (np.eye(18) - pm @ self.c.T @ np.linalg.solve(s, self.c)) @ pm
         p = (p + p.T) / 2.0
-        if np.linalg.det(p[0:2, 0:2]) > 0.000001:
+        self.decoupled = bool(np.linalg.det(p[0:2, 0:2]) > 0.000001)        # the branch of :151-156 this update took
+        if self.decoupled:
             p[0:2, 2:18] = 0.0; p[2:18, 0:2] = 0.0; p[0:2, 0:2] /= 10.0
         self.P = p
         rbd = np.zeros(32)

@@ -52,6 +52,28 @@ def test_wbc_solution_satisfies_reference_constraints(oracle, seed, mode):
             assert np.abs(sol[16 + 3 * c:19 + 3 * c]).max() < 1e-8
 
 
+def test_foot_wrench_matrix_loses_rank_inside_the_knee_limits(oracle):
+    """The premise of the observer's near-singular sweep (test_gpu_estimator_envelope.py): each leg's S J_foot' (5 x 6) loses rank at one
+    knee angle k* strictly inside the knee's limits (the 5 mm forward offset of the ankle origin puts the hip-pitch, knee and ankle
+    origins in line there), and k* does not depend on the hip pitch or the ankle."""
+    from oracle import refs as R
+    q0 = np.r_[X0[6:9], X0[9:12], X0[12:]]
+    for leg in (0, 1):
+        ks = []
+        for hp, ank in ((X0[12 + 5 * leg + 2], X0[12 + 5 * leg + 4]), (-0.4, 0.6), (0.3, -0.5), (0.9, 0.0)):
+            q = q0.copy(); q[6 + 5 * leg + 2] = hp; q[6 + 5 * leg + 4] = ank
+            k = R.singular_knee(leg, q)
+            q[6 + 5 * leg + 3] = k
+            s = np.linalg.svd(R.foot_wrench_matrix(q, leg), compute_uv=False)
+            assert s[-1] / s[0] < 1e-10, (leg, hp, ank, s)
+            ks.append(k)
+        assert LO[5 * leg + 3] < min(ks) and max(ks) < HI[5 * leg + 3], ks
+        assert max(ks) - min(ks) < 1e-8, ks
+        # away from k* the matrix has full rank: cond ~ 20 at the default knee, ~ 880 at knee 0
+        q = q0.copy()
+        assert np.linalg.cond(R.foot_wrench_matrix(q, leg)) < 100
+
+
 def test_event_time_grid_restatement_properties():
     """scenarios.event_time_grid is the numpy side of row S1's parity test (ocs2::timeDiscretizationWithEvents with the event node pair collapsed):
     first node t0, last node t0 + T, strictly increasing, no step longer than dt, every mode switch strictly inside the horizon is a node, the grid
