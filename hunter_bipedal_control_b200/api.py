@@ -43,6 +43,7 @@ EXPORTED_SYMBOLS = [
     "hb_default_estimation_params", "hb_estimation_reset", "hb_sim_read_sensors_batch_dev", "hb_sim_read_sensors", "hb_rollout_estimated_batch_dev",
     "hb_plan_references_targets", "hb_goal_to_target", "hb_plan_set_targets", "hb_rollout_set_goals",
     "hb_rollout_set_mpc_latencies", "hb_policy_update", "hb_policy_wbc", "hb_policy_wbc_async",
+    "hb_rollout_set_odometry", "hb_sim_read_odometry", "hb_sim_read_odometry_async", "hb_estimator_fuse_odometry", "hb_estimator_fuse_odometry_async",
 ]
 
 
@@ -483,6 +484,35 @@ def estimation_stats(B):
     return np.zeros(B, dtype=ESTIMATION_STATS_DTYPE)
 
 
+HB_ODOM_MAX_DELAY = 15
+
+
+class HbOdometrySetting(C.Structure):
+    _fields_ = [("period_ticks", C.c_int32), ("delay_ticks", C.c_int32), ("sigma_position", C.c_double), ("sigma_drift", C.c_double)]
+
+
+def make_odometry_settings(B, period_ticks, delay_ticks=0, sigma_position=0.0, sigma_drift=0.0):
+    """ctypes array of B HbOdometrySetting (Context.set_odometry): the tracking camera of each robot of the estimated episodes, a message
+    every period_ticks ticks (0: no camera) carrying the base position of delay_ticks ticks earlier (0..HB_ODOM_MAX_DELAY), with white noise
+    sigma_position [m] and a bias whose random-walk increment per message is sigma_drift [m]. Each argument: (B,) or a scalar. Raises
+    ValueError for what hb_rollout_set_odometry rejects."""
+    try:
+        per, dly = (np.broadcast_to(np.asarray(a), (B,)) for a in (period_ticks, delay_ticks))
+        sp, sd = (np.broadcast_to(_f64(a), (B,)) for a in (sigma_position, sigma_drift))
+    except ValueError as e:
+        raise ValueError("odometry settings: (B,) or scalars expected: %s" % e)
+    if not (np.array_equal(per, np.rint(per)) and np.array_equal(dly, np.rint(dly))):
+        raise ValueError("odometry settings: period_ticks and delay_ticks must be integers")
+    if (per < 0).any() or (dly < 0).any() or (dly > HB_ODOM_MAX_DELAY).any():
+        raise ValueError("odometry settings: period_ticks >= 0 and 0 <= delay_ticks <= %d expected" % HB_ODOM_MAX_DELAY)
+    if not (np.isfinite(sp).all() and np.isfinite(sd).all() and (sp >= 0).all() and (sd >= 0).all()):
+        raise ValueError("odometry settings: the sigmas must be finite and >= 0")
+    out = (HbOdometrySetting * B)()
+    v = np.ctypeslib.as_array(out)
+    v["period_ticks"] = per; v["delay_ticks"] = dly; v["sigma_position"] = sp; v["sigma_drift"] = sd
+    return out
+
+
 class HbGaitSelector(C.Structure):
     _fields_ = [("history", C.c_double * 50), ("vel_avg", C.c_double), ("head", C.c_int32), ("count", C.c_int32), ("gait_level", C.c_int32),
                 ("reserved", C.c_int32)]
@@ -921,6 +951,35 @@ class Context:
     def policy_wbc(self, t_now, rbd, stance_mode=None):
         """resident_wbc on each instance's adopted policy (hb_policy_wbc): returns (x_des, u_des, mode, sol, torque, status)."""
         return self._wbc("hb_policy_wbc", t_now, rbd, stance_mode)
+
+    def set_odometry(self, settings):
+        """Tracking cameras of this context's estimated episodes (hb_rollout_set_odometry): settings[i] (make_odometry_settings) is the
+        camera of instance i of every later rollout_estimated call, whose messages the filter fuses (updateFromTopic); instances beyond
+        len(settings) have none; None clears them. Every call clears the cameras' history and bias."""
+        self._set_instances("hb_rollout_set_odometry", settings)
+
+    def read_odometry(self, rbd, est, tick, noise=None):
+        """The tracking cameras at absolute tick `tick` from the true rbd [B,32] (hb_sim_read_odometry), on this context's odometry setting
+        and camera state (advanced); `est` (ctypes array of HbEstimationState) gives the noise streams, noise (HbSensorNoise, None: seed 0)
+        the seed. Returns (pos [B,3], has_msg [B]): the message of each instance with one due, zeros for the others."""
+        rbd = _f64(rbd); B = rbd.shape[0]
+        noise = noise or HbSensorNoise()
+        pos = np.zeros((B, 3)); has = np.zeros(B, dtype=np.uint8)
+        _check(self._lib.hb_sim_read_odometry(self._h, B, C.byref(noise), C.c_int64(tick), _ptr(rbd), est, _ptr(pos), _ptr(has)),
+               "hb_sim_read_odometry", self._h)
+        return pos, has
+
+    def fuse_odometry(self, state, pos, has_msg, contact_flag, rbd, params=None):
+        """updateFromTopic after estimator_update (hb_estimator_fuse_odometry): each instance with has_msg[i] takes the message pos[i];
+        `state` (ctypes array of HbKfState) is updated in place. rbd: the estimated rbd [B,32] estimator_update returned. Returns the fused rbd."""
+        rbd = _f64(rbd).copy(); B = rbd.shape[0]
+        pos = _f64(pos).reshape(B, 3)
+        has = np.ascontiguousarray(has_msg, dtype=np.uint8).reshape(B)
+        flags = np.ascontiguousarray(contact_flag, dtype=np.uint8).reshape(B, 4)
+        params = params or default_kf_params()
+        _check(self._lib.hb_estimator_fuse_odometry(self._h, B, C.byref(params), state, _ptr(pos), _ptr(has), _ptr(flags), _ptr(rbd)),
+               "hb_estimator_fuse_odometry", self._h)
+        return rbd
 
     def set_plan_targets(self, targets):
         """Explicit planner targets of this context (hb_plan_set_targets): targets[i] (make_targets, goal_to_target) replaces the cmd_vel

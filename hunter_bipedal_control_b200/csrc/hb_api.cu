@@ -80,6 +80,7 @@ struct hb_ctx {
   void* re_mem;
   double *re_quat, *re_gyro, *re_acc, *re_jpos, *re_jvel, *re_rbd;
   uint8_t* re_flag;
+  double* re_opos; uint8_t* re_ohas;   // the tick's odometry messages (with hb_rollout_set_odometry)
   // the per-robot settings of the episodes (hb_rollout_set_pushes / _plant_variations / _terrains), set by set_instances
   InstanceSetting<hb_push_schedule> pushes;
   InstanceSetting<hb_plant_variation> variations;
@@ -97,6 +98,11 @@ struct hb_ctx {
   void* pol_mem;
   SolutionRows pol;
   std::vector<uint8_t> pol_have;
+  // the tracking camera of each instance of the estimated episodes (hb_rollout_set_odometry) and the cameras' state (history, bias),
+  // allocated at max_batch by the first call that sets cameras
+  InstanceSetting<hb_odometry_setting> odometry;
+  void* odom_mem;
+  OdomCamera* odom_cam;
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
   // hb_resident_cycle_batch's packed references / reference verdicts
   void* arena; size_t arena_cap;
@@ -472,8 +478,9 @@ int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
 int hb_destroy(hb_ctx* ctx) {
   if (!ctx) return HB_EINVAL;
   cudaSetDevice(ctx->device);
-  void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->arena,
-                       ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev};
+  void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->arena,
+                       ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
+                       ctx->odometry.dev};
   for (void* p : mem) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -783,8 +790,14 @@ int hb_estimator_update_batch_dev(hb_ctx* ctx, int B, const hb_kf_params* params
                                   const double* ang_vel_local, const double* lin_acc_local, const double* joint_pos, const double* joint_vel,
                                   const uint8_t* contact_flag, double* rbd_out) {
   ENTER(ctx, B, params && state && quat && ang_vel_local && lin_acc_local && joint_pos && joint_vel && contact_flag && rbd_out, UNCAPPED);
-  return launch(ctx, K_UNPROFILED, kf_update_kernel<hb_kf_state>, B, 32, sizeof(KfShared), B, *params, dt, state, quat, ang_vel_local, lin_acc_local,
-                joint_pos, joint_vel, contact_flag, rbd_out);
+  return launch(ctx, K_UNPROFILED, kf_update_kernel<hb_kf_state, false>, B, 32, sizeof(KfShared), B, *params, dt, state, quat, ang_vel_local, lin_acc_local,
+                joint_pos, joint_vel, contact_flag, rbd_out, (const double*)nullptr, (const uint8_t*)nullptr);
+}
+
+int hb_estimator_fuse_odometry_async(hb_ctx* ctx, int B, const hb_kf_params* params, hb_kf_state* state, const double* pos, const uint8_t* has_msg,
+                                     const uint8_t* contact_flag, double* rbd) {
+  ENTER(ctx, B, params && state && pos && has_msg && contact_flag && rbd, UNCAPPED);
+  return launch(ctx, K_UNPROFILED, odometry_fuse_kernel, (B + 63) / 64, 64, 0, B, params->foot_radius, state, pos, has_msg, contact_flag, rbd);
 }
 
 int hb_default_wbc_settings(hb_wbc_settings* s) {
@@ -1053,6 +1066,33 @@ static bool latency_ok(const int32_t& d) { return d >= 0; }     // the upper bou
 
 int hb_rollout_set_mpc_latencies(hb_ctx* ctx, int B, const int32_t* ticks) { return set_instances(ctx, B, ticks, latency_ok, &hb_ctx::latencies); }
 
+// The ranges of hunter_b200.h's hb_odometry_setting
+static bool odometry_ok(const hb_odometry_setting& s) {
+  if (s.period_ticks < 0 || s.delay_ticks < 0 || s.delay_ticks > HB_ODOM_MAX_DELAY) return false;
+  for (double sigma : {s.sigma_position, s.sigma_drift}) if (!(sigma >= 0.0) || !isfinite(sigma)) return false;
+  return true;
+}
+
+int hb_rollout_set_odometry(hb_ctx* ctx, int B, const hb_odometry_setting* s) {
+  int rc = set_instances(ctx, B, s, odometry_ok, &hb_ctx::odometry);
+  if (rc || ctx->odometry.n == 0) return rc;
+  const size_t Bc = ctx->cfg.max_batch;
+  rc = reserve_group(&ctx->odom_mem, [&](void* m) {
+    size_t off = 0;
+    ctx->odom_cam = carve<OdomCamera>(m, off, Bc);
+    return off;
+  });
+  if (rc) { ctx->odometry.n = 0; return rc; }
+  CK(cudaMemsetAsync(ctx->odom_cam, 0, sizeof(OdomCamera) * Bc, ctx->stream));     // every camera's history and bias cleared
+  return HB_OK;
+}
+
+// The camera read of a call whose instances start at ctx->base, on the context's odometry setting, its messages written to pos / has
+static OdomRead odometry_read(const hb_ctx* ctx, double* pos, uint8_t* has) {
+  const InstanceView<hb_odometry_setting> set = ctx->odometry.view(ctx->base);
+  return OdomRead{set, set.recs ? ctx->odom_cam + ctx->base : nullptr, pos, has};
+}
+
 // The adopted policy ctx->pol, allocated at max_batch by its first use (hb_policy_update, an episode with a latency set)
 static int policy_reserve(hb_ctx* ctx) {
   const size_t Bc = ctx->cfg.max_batch;
@@ -1147,6 +1187,7 @@ static int estimation_reserve(hb_ctx* ctx) {
     ctx->re_quat = carve<double>(m, off, Bc * 4); ctx->re_gyro = carve<double>(m, off, Bc * 3); ctx->re_acc = carve<double>(m, off, Bc * 3);
     ctx->re_jpos = carve<double>(m, off, Bc * NJ); ctx->re_jvel = carve<double>(m, off, Bc * NJ); ctx->re_rbd = carve<double>(m, off, Bc * 32);
     ctx->re_flag = carve<uint8_t>(m, off, Bc * 4);
+    ctx->re_opos = carve<double>(m, off, Bc * 3); ctx->re_ohas = carve<uint8_t>(m, off, Bc);
     return off;
   });
 }
@@ -1209,6 +1250,9 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   // the push wrench the begin kernel writes and the plant applies, none without schedules
   double* wrench = ctx->pushes.n > 0 ? ctx->ro_wrench : nullptr;
   const InstanceView<hb_target> goal_targets{ctx->goal_tg, ctx->goals.n};    // what the planner reads: the targets of the captured goals
+  // the cameras the sensor read reads and the messages the filter fuses, none without an odometry setting
+  const bool odom = e && ctx->odometry.n > 0;
+  const OdomRead odom_read = odom ? odometry_read(ctx, ctx->re_opos, ctx->re_ohas) : OdomRead{};
   for (int k = 0; k < n_ticks && !rc; ++k) {
     const int64_t a = tick0 + k;
     const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
@@ -1220,9 +1264,10 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
       // LeggedController::updateStateEstimation: sensors and contact flags at the previous observation's time, filter, observation step
       double* est_row = (n_est_log && k % p->log_every == 0) ? e->log + (size_t)(k / p->log_every) * 32 : nullptr;
       rc = launch(ctx, K_UNPROFILED, sensor_read_kernel, grid, 64, 0, B, e->ep->noise, (uint32_t)a, p->sim.dt, (double)(a - 1) * p->period, rbd, e->est,
-                  ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag);
-      if (!rc) rc = launch(ctx, K_UNPROFILED, kf_update_kernel<hb_estimation_state>, B, 32, sizeof(KfShared), B, e->ep->kf, p->period, e->est, ctx->re_quat,
-                           ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag, meas);
+                  ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag, odom_read);
+      if (!rc) rc = launch(ctx, K_UNPROFILED, odom ? kf_update_kernel<hb_estimation_state, true> : kf_update_kernel<hb_estimation_state, false>, B, 32,
+                           sizeof(KfShared), B, e->ep->kf, p->period, e->est, ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag,
+                           meas, (const double*)ctx->re_opos, (const uint8_t*)ctx->re_ohas);
       if (!rc) rc = launch(ctx, K_UNPROFILED, est_observe_kernel, grid, 64, 0, B, rbd, meas, stats, e->est, e->stats, est_row, (size_t)n_est_log * 32);
     }
     // MPC_MRT_Interface::updatePolicy of the instances whose solution comes into force on this tick, before this tick's cycle
@@ -1288,7 +1333,13 @@ int hb_sim_read_sensors_batch_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noi
   ENTER(ctx, B, noise && rbd && est && quat && ang_vel_local && lin_acc_local && joint_pos && joint_vel && sensor_noise_ok(*noise) && accel_dt > 0.0 &&
         tick >= 0 && tick <= UINT32_MAX, CAPPED);
   return launch(ctx, K_UNPROFILED, sensor_read_kernel, (B + 63) / 64, 64, 0, B, *noise, (uint32_t)tick, accel_dt, 0.0, rbd, est, quat, ang_vel_local,
-                lin_acc_local, joint_pos, joint_vel, (uint8_t*)nullptr);
+                lin_acc_local, joint_pos, joint_vel, (uint8_t*)nullptr, OdomRead{});
+}
+
+int hb_sim_read_odometry_async(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, const double* rbd, const hb_estimation_state* est,
+                               double* pos, uint8_t* has_msg) {
+  ENTER(ctx, B, noise && rbd && est && pos && has_msg && tick >= 0 && tick <= UINT32_MAX, CAPPED);
+  return launch(ctx, K_UNPROFILED, odometry_read_kernel, (B + 63) / 64, 64, 0, B, noise->seed, (uint32_t)tick, rbd, est, odometry_read(ctx, pos, has_msg));
 }
 
 int hb_observer_reset(int B, hb_observer_state* state) {
@@ -1642,6 +1693,22 @@ int hb_sim_read_sensors(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_
   auto r = s.in(rbd, 32); auto es = s.inout(est, 1); auto q = s.out(quat, 4); auto w = s.out(ang_vel_local, 3); auto a = s.out(lin_acc_local, 3);
   auto jp = s.out(joint_pos, NJ); auto jv = s.out(joint_vel, NJ);
   return s.run(1, [&](Chunk) { return hb_sim_read_sensors_batch_dev(ctx, B, noise, tick, accel_dt, r, es, q, w, a, jp, jv); });
+}
+
+int hb_sim_read_odometry(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, const double* rbd, const hb_estimation_state* est,
+                         double* pos, uint8_t* has_msg) {
+  ENTER(ctx, B, noise && rbd && est && pos && has_msg && tick >= 0 && tick <= UINT32_MAX, CAPPED);
+  Staging s(ctx, B);
+  auto r = s.in(rbd, 32); auto es = s.in(est, 1); auto p = s.out(pos, 3); auto h = s.out(has_msg, 1);
+  return s.run(1, [&](Chunk) { return hb_sim_read_odometry_async(ctx, B, noise, tick, r, es, p, h); });
+}
+
+int hb_estimator_fuse_odometry(hb_ctx* ctx, int B, const hb_kf_params* params, hb_kf_state* state, const double* pos, const uint8_t* has_msg,
+                               const uint8_t* contact_flag, double* rbd) {
+  ENTER(ctx, B, params && state && pos && has_msg && contact_flag && rbd, CAPPED);
+  Staging s(ctx, B);
+  auto st = s.inout(state, 1); auto p = s.in(pos, 3); auto h = s.in(has_msg, 1); auto fl = s.in(contact_flag, 4); auto r = s.inout(rbd, 32);
+  return s.run(1, [&](Chunk) { return hb_estimator_fuse_odometry_async(ctx, B, params, st, p, h, fl, r); });
 }
 
 int hb_actuation_batch(hb_ctx* ctx, int B, double delay, const double* time, hb_actuation_state* state, const double* command, const double* rbd,

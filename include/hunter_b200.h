@@ -384,6 +384,39 @@ int hb_rollout_set_goals(hb_ctx* ctx, int B, const hb_goal_schedule* goals);
  * run with latency 0). -1 also for a negative entry. */
 int hb_rollout_set_mpc_latencies(hb_ctx* ctx, int B, const int32_t* ticks);
 
+/* ---- odometry: a simulated tracking camera per robot, fused into the estimate (KalmanFilterEstimate::updateFromTopic) ----
+ * Only the estimated episodes read this setting; hb_rollout_batch_dev has no estimator and ignores it. An instance with period_ticks == 0,
+ * or at or beyond B, has no camera and runs exactly as with no setting.
+ * The camera of instance i at absolute tick a, in the tick's sensor read: at a == 0 its state (position history and bias) is cleared;
+ * the true base position entering the tick (rbd[3:6]) is recorded in history slot a % (HB_ODOM_MAX_DELAY + 1); a message is due iff
+ * a % period_ticks == 0 and a >= delay_ticks, and then bias += sigma_drift n_d and pos = p(a - delay_ticks) + bias + sigma_position n_p,
+ * each of the two terms added in that order. The normals are the sensor noise's Philox4x32-10 scheme (hb_sensor_noise, below): key
+ * hb_sensor_noise.seed, counter (block, tick, noise_stream), 3 normals of block 9 for n_d and of block 10 for n_p (blocks 0-8 are the
+ * sensors'); a sigma of 0 draws nothing. The history and bias are per-instance context state, allocated at max_batch by the first call that
+ * sets records, freed by hb_destroy and cleared by every such call and by a read at tick 0, so a split episode continues exactly, also
+ * between a reading and its delayed arrival.
+ * The fusion (updateFromTopic), after the filter's predict / correct step and its xy decoupling, on a tick with a message:
+ * x_hat[0:3] = pos; for each contact c, x_hat[6+3c : 9+3c] = pos + fk_c and then x_hat[8+3c] -= foot_radius, with fk_c the contact
+ * position at the filter's ZYX angles and joint readings with the base at the origin (the filter's own kinematics), and feet_heights[c] =
+ * x_hat[8+3c] where contact_flag[c]; the velocity x_hat[3:6] and P are left untouched. The estimated rbd then takes pos as its position,
+ * and everything downstream (est_stats, est_log, yaw_obs, planner, MPC, WBC, joint law, goal capture) sees the fused estimate. Once
+ * messages arrive, the filter's feet heights follow the camera instead of staying 0, as in the reference.
+ * Deviations from the reference: the camera is mounted at the base frame origin (base2sensor = identity: the robot's URDF has no camera
+ * link, and the tf lookup by stamp is not modelled); world2odom is the identity, which the reference never changes; messages arrive on whole
+ * ticks; the message's orientation is not used (with an identity mount the reference does not use it either). Pinocchio's kinematics at
+ * (pos, zyx, q) is restated as pos + fk_c: the same value, rounded as one more addition per coordinate.
+ * Odometry adds no launch to an episode. */
+#define HB_ODOM_MAX_DELAY 15
+typedef struct {            /* the tracking camera of one robot                                                                     */
+  int32_t period_ticks;     /* a message every period_ticks ticks, >= 0; 0 = no camera (the instance runs as with no setting)      */
+  int32_t delay_ticks;      /* 0..HB_ODOM_MAX_DELAY: a message carries the pose of delay_ticks ticks earlier                        */
+  double sigma_position;    /* white noise per message and axis [m], >= 0                                                           */
+  double sigma_drift;       /* random-walk increment of the camera's bias per message and axis [m], >= 0                            */
+} hb_odometry_setting;
+/* Sets the tracking cameras of the context's estimated episodes (a per-robot episode setting, above) and clears every camera's state. -1
+ * also for a negative period_ticks or delay_ticks, a delay_ticks above HB_ODOM_MAX_DELAY, or a sigma that is negative or not finite. */
+int hb_rollout_set_odometry(hb_ctx* ctx, int B, const hb_odometry_setting* s);
+
 /* ---- estimated episodes (hb_rollout_estimated_batch_dev): the controllers read the Kalman filter's estimate from synthesised, noisy
  * sensors instead of the plant's true state (LeggedController::updateStateEstimation, LeggedController.cpp:280-349) ---- */
 typedef struct {                 /* standard deviations of additive Gaussian sensor noise; 0 = that channel is exact and draws nothing */
@@ -522,8 +555,8 @@ int hb_plan_references_batch_dev(hb_ctx* ctx, int B, const hb_plan_input* in, co
 int hb_plan_set_targets(hb_ctx* ctx, int B, const hb_target* targets);
 /* One estimator update per instance (StateEstimateBase::updateJointStates / updateImu, StateEstimateBase.cpp:73-106, then
  * KalmanFilterEstimate::update): quat = (x, y, z, w); contact_flag: B x 4 (0 = the filter distrusts that foot, x100 noise);
- * rbd_out: B x 32 measured rbd state [zyx, p, q_j, omega_world, v, qd_j]. The odometry topic fusion (updateFromTopic) is ROS glue
- * and not part of it; zyxOffset_ is taken as zero. */
+ * rbd_out: B x 32 measured rbd state [zyx, p, q_j, omega_world, v, qd_j]. zyxOffset_ is taken as zero. The odometry fusion
+ * (updateFromTopic) is a call of its own, hb_estimator_fuse_odometry_async, applied after this one. */
 int hb_estimator_update_batch_dev(hb_ctx* ctx, int B, const hb_kf_params* params, double dt, hb_kf_state* state, const double* quat,
                                   const double* ang_vel_local, const double* lin_acc_local, const double* joint_pos,
                                   const double* joint_vel, const uint8_t* contact_flag, double* rbd_out);
@@ -576,7 +609,8 @@ int hb_sim_read_sensors_batch_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noi
  * and est_log. On MPC ticks the plan inputs come from the estimated rbd with x0[9] = yaw_obs, the planner and the cycle see the estimate,
  * and the schedule of the new plan is copied into est. The policy, the WeightedWbc and the joint command law see the estimated rbd;
  * actuation, saturation, the plant and the failure checks the true one. est (B) is in/out; est_stats (B, nullable) in/out; est_log
- * (nullable) the estimated rbd in log's layout. Arguments are checked before any launch (sigmas finite and >= 0). */
+ * (nullable) the estimated rbd in log's layout. Arguments are checked before any launch (sigmas finite and >= 0). With odometry set
+ * (hb_rollout_set_odometry), the sensor read also reads each camera and the filter fuses the messages due on the tick. */
 int hb_rollout_estimated_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb_rollout_params* p, const hb_estimation_params* ep,
                                    const hb_rollout_command* cmd, double* rbd, hb_actuation_state* act, uint8_t* estop, hb_rollout_stats* stats,
                                    hb_estimation_state* est, hb_estimation_stats* est_stats /*nullable*/, double* log /*nullable*/,
@@ -681,6 +715,24 @@ int hb_policy_wbc(hb_ctx* ctx, int B, const double* t_now, const double* rbd, co
                   int32_t* mode_out, double* wbc_sol, double* torque /*nullable*/, int32_t* wbc_status /*nullable*/);
 int hb_policy_wbc_async(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode /*nullable*/, double* x_des,
                         double* u_des, int32_t* mode_out, double* wbc_sol, double* torque /*nullable*/, int32_t* wbc_status /*nullable*/);
+
+/* ---- odometry outside the episodes: the camera read and the fusion of the estimated episodes (odometry, above) through public calls ----
+ * hb_sim_read_odometry: the camera read of instances 0 .. B-1 at absolute tick `tick` on the context's odometry setting and camera state
+ * (history and bias, updated), from the true rbd (B x 32); noise gives the seed, est (B) the noise streams (read only). has_msg[i] (B) = 1
+ * when a message is due, with pos (B x 3) its position; 0 and pos = 0 otherwise, and for instances without a camera. -1 also for a tick
+ * outside 0 .. 2^32 - 1.
+ * hb_estimator_fuse_odometry: the fusion on the filter state hb_estimator_update_batch advanced (state, in/out) and the estimated rbd it
+ * wrote (rbd, B x 32, in/out): instances with has_msg[i] != 0 take pos[i]; contact_flag (B x 4) as given to the filter, foot_radius from
+ * params. An instance with has_msg[i] == 0 is left bit for bit as it is. Both give bit for bit what the estimated episode computes.
+ * The plain names take host pointers (synchronous), the _async names device pointers (asynchronous, on the context's stream). */
+int hb_sim_read_odometry(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, const double* rbd, const hb_estimation_state* est,
+                         double* pos, uint8_t* has_msg);
+int hb_sim_read_odometry_async(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, const double* rbd, const hb_estimation_state* est,
+                               double* pos, uint8_t* has_msg);
+int hb_estimator_fuse_odometry(hb_ctx* ctx, int B, const hb_kf_params* params, hb_kf_state* state, const double* pos, const uint8_t* has_msg,
+                               const uint8_t* contact_flag, double* rbd);
+int hb_estimator_fuse_odometry_async(hb_ctx* ctx, int B, const hb_kf_params* params, hb_kf_state* state, const double* pos, const uint8_t* has_msg,
+                                     const uint8_t* contact_flag, double* rbd);
 int hb_rbd_to_centroidal_batch(hb_ctx* ctx, int B, const double* rbd, double* x);
 int hb_reference_expand_batch(hb_ctx* ctx, int B, const double* t0, const hb_reference* refs, double* x_ref, double* swing_ref,
                               int32_t* mode);
