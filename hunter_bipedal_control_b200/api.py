@@ -44,6 +44,7 @@ EXPORTED_SYMBOLS = [
     "hb_plan_references_targets", "hb_goal_to_target", "hb_plan_set_targets", "hb_rollout_set_goals",
     "hb_rollout_set_mpc_latencies", "hb_policy_update", "hb_policy_wbc", "hb_policy_wbc_async",
     "hb_rollout_set_odometry", "hb_sim_read_odometry", "hb_sim_read_odometry_async", "hb_estimator_fuse_odometry", "hb_estimator_fuse_odometry_async",
+    "hb_rollout_set_controller_settings",
 ]
 
 
@@ -482,6 +483,36 @@ def estimation_states(B, first_stream=0):
 def estimation_stats(B):
     """Estimation stats of B fresh episodes: zeros."""
     return np.zeros(B, dtype=ESTIMATION_STATS_DTYPE)
+
+
+class HbControllerSetting(C.Structure):
+    _fields_ = [("wbc", HbWbcSettings), ("gains", HbPdGains)]
+
+
+def make_controller_settings(B, wbc=None, gains=None, **fields):
+    """ctypes array of B HbControllerSetting (Context.set_controller_settings): each robot's WBC settings and joint PD gains in the episodes.
+    wbc (HbWbcSettings) and gains (HbPdGains) are the base of every record, default hb_default_wbc_settings and default_pd_gains(). Any field
+    of either struct can be given by name, as a scalar or a (B,) array; torque_limits as (5,) or (B, 5). Raises ValueError for an unknown
+    name or a shape that does not broadcast."""
+    lib = load_library()
+    if wbc is None:
+        wbc = HbWbcSettings()
+        _check(lib.hb_default_wbc_settings(C.byref(wbc)), "hb_default_wbc_settings")
+    gains = default_pd_gains() if gains is None else gains
+    out = (HbControllerSetting * B)()
+    v = np.ctypeslib.as_array(out)
+    v["wbc"] = np.frombuffer(bytes(wbc), dtype=v.dtype["wbc"])[0]
+    v["gains"] = np.frombuffer(bytes(gains), dtype=v.dtype["gains"])[0]
+    for name, value in fields.items():
+        part = "wbc" if name in v.dtype["wbc"].names else "gains" if name in v.dtype["gains"].names else None
+        if part is None:
+            raise ValueError("controller settings: unknown field %r" % name)
+        shape = (B, 5) if name == "torque_limits" else (B,)
+        try:
+            v[part][name] = np.broadcast_to(_f64(value), shape)
+        except ValueError as e:
+            raise ValueError("controller settings: %s: %s expected: %s" % (name, "(5,) or (B, 5)" if shape[1:] else "(B,) or a scalar", e))
+    return out
 
 
 HB_ODOM_MAX_DELAY = 15
@@ -957,6 +988,12 @@ class Context:
         camera of instance i of every later rollout_estimated call, whose messages the filter fuses (updateFromTopic); instances beyond
         len(settings) have none; None clears them. Every call clears the cameras' history and bias."""
         self._set_instances("hb_rollout_set_odometry", settings)
+
+    def set_controller_settings(self, settings):
+        """Controller settings of this context's episodes (hb_rollout_set_controller_settings): settings[i] (make_controller_settings) is the
+        WBC settings and joint PD gains of instance i of every later rollout / rollout_estimated call, in place of the context's WBC settings
+        and params.gains; instances beyond len(settings) run those; None clears them. No other call reads them."""
+        self._set_instances("hb_rollout_set_controller_settings", settings)
 
     def read_odometry(self, rbd, est, tick, noise=None):
         """The tracking cameras at absolute tick `tick` from the true rbd [B,32] (hb_sim_read_odometry), on this context's odometry setting

@@ -103,6 +103,8 @@ struct hb_ctx {
   InstanceSetting<hb_odometry_setting> odometry;
   void* odom_mem;
   OdomCamera* odom_cam;
+  // each instance's WBC settings and joint PD gains in the episodes (hb_rollout_set_controller_settings)
+  InstanceSetting<hb_controller_setting> controllers;
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
   // hb_resident_cycle_batch's packed references / reference verdicts
   void* arena; size_t arena_cap;
@@ -480,7 +482,7 @@ int hb_destroy(hb_ctx* ctx) {
   cudaSetDevice(ctx->device);
   void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->arena,
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
-                       ctx->odometry.dev};
+                       ctx->odometry.dev, ctx->controllers.dev};
   for (void* p : mem) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -550,11 +552,20 @@ int hb_wbc_qp_batch_dev(hb_ctx* ctx, int B, int n, int m, const double* H, const
   return launch_qp(ctx, B, n, m, H, g, A, lbA, ubA, (size_t)n * n, (size_t)m * n, (size_t)m, nullptr, x, status, iters);
 }
 
+// The instances' controller settings as the episode kernels read them; every other call passes an empty view
+using ControllerView = InstanceView<hb_controller_setting>;
+
+// hb_wbc_solve_batch_dev, with each instance of `cs` on its own WBC settings
+static int wbc_solve_impl(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
+                          const uint8_t* stance_mode, double* sol, int32_t* status, ControllerView cs) {
+  ENTER(ctx, B, x_des && u_des && rbd && mode && sol, CAPPED);
+  return launch(ctx, K_QP, wbc_fused_kernel, B, 32, wbc_fused_doubles() * sizeof(double), B, ctx->wbc, cs, x_des, u_des, rbd, mode, stance_mode,
+                ctx->cfg.wbc_rho, ctx->cfg.qp_max_iter, sol, status ? status : ctx->wstatus + ctx->base, ctx->witers + ctx->base);
+}
+
 int hb_wbc_solve_batch_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
                            const uint8_t* stance_mode, double* sol, int32_t* status) {
-  ENTER(ctx, B, x_des && u_des && rbd && mode && sol, CAPPED);
-  return launch(ctx, K_QP, wbc_fused_kernel, B, 32, wbc_fused_doubles() * sizeof(double), B, ctx->wbc, x_des, u_des, rbd, mode, stance_mode,
-                ctx->cfg.wbc_rho, ctx->cfg.qp_max_iter, sol, status ? status : ctx->wstatus + ctx->base, ctx->witers + ctx->base);
+  return wbc_solve_impl(ctx, B, x_des, u_des, rbd, mode, stance_mode, sol, status, ControllerView{});
 }
 
 int hb_wbc_assemble_batch_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
@@ -591,20 +602,27 @@ static int hwbc_tasks_dev(hb_ctx* ctx, int B, const double* x_des, const double*
   return launch(ctx, K_WBC_ASSEMBLE, hwbc_tasks_kernel, B, 32, 0, B, ctx->wbc, x_des, u_des, rbd, mode, problems);
 }
 
+// hb_hierarchical_wbc_solve_batch_dev, with each instance of `cs` on its own WBC settings
+static int hwbc_solve_impl(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, double* sol,
+                           int32_t* status, ControllerView cs) {
+  ENTER(ctx, B, x_des && u_des && rbd && mode && sol, CAPPED);
+  return launch(ctx, K_QP, hwbc_fused_kernel, B, 32, hwbc_fused_bytes(), B, ctx->wbc, cs, x_des, u_des, rbd, mode, 2 * ctx->cfg.qp_max_iter, sol,
+                status);
+}
+
 int hb_hierarchical_wbc_solve_batch_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, double* sol,
                                         int32_t* status) {
-  ENTER(ctx, B, x_des && u_des && rbd && mode && sol, CAPPED);
-  return launch(ctx, K_QP, hwbc_fused_kernel, B, 32, hwbc_fused_bytes(), B, ctx->wbc, x_des, u_des, rbd, mode, 2 * ctx->cfg.qp_max_iter, sol, status);
+  return hwbc_solve_impl(ctx, B, x_des, u_des, rbd, mode, sol, status, ControllerView{});
 }
 
 // The controller's WBC (LeggedController::wbc_) on device pointers: every entry point that runs it comes through here. stance_mode is read
 // by the weighted formulation only (WbcBase::setStanceMode reaches only WeightedWbc::formulateWeightedTasks). status: nullable, as for
-// hb_wbc_solve_batch_dev.
+// hb_wbc_solve_batch_dev. cs: the episodes' controller settings, empty for every other caller.
 static int controller_wbc_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
-                              const uint8_t* stance_mode, double* sol, int32_t* status) {
+                              const uint8_t* stance_mode, double* sol, int32_t* status, ControllerView cs = ControllerView{}) {
   if (ctx->wbc_form == HB_WBC_HIERARCHICAL)
-    return hb_hierarchical_wbc_solve_batch_dev(ctx, B, x_des, u_des, rbd, mode, sol, status ? status : ctx->wstatus + ctx->base);
-  return hb_wbc_solve_batch_dev(ctx, B, x_des, u_des, rbd, mode, stance_mode, sol, status);
+    return hwbc_solve_impl(ctx, B, x_des, u_des, rbd, mode, sol, status ? status : ctx->wstatus + ctx->base, cs);
+  return wbc_solve_impl(ctx, B, x_des, u_des, rbd, mode, stance_mode, sol, status, cs);
 }
 
 int hb_mpc_cold_start_batch_dev(hb_ctx* ctx, int B, const double* x0, const int32_t* mode, double* x_traj, double* u_traj) {
@@ -1087,6 +1105,26 @@ int hb_rollout_set_odometry(hb_ctx* ctx, int B, const hb_odometry_setting* s) {
   return HB_OK;
 }
 
+// The ranges of hunter_b200.h's hb_controller_setting: hb_wbc_set_settings' rules, every field finite, task gains and PD gains >= 0
+static bool controller_setting_ok(const hb_controller_setting& s) {
+  const double* f = reinterpret_cast<const double*>(&s);
+  static_assert(sizeof(hb_controller_setting) == 26 * sizeof(double), "hb_controller_setting holds 26 doubles");
+  for (int i = 0; i < 26; ++i) if (!isfinite(f[i])) return false;
+  const hb_wbc_settings& w = s.wbc;
+  for (double lim : w.torque_limits) if (!(lim > 0.0)) return false;
+  if (!(w.friction_coefficient > 0.0) || !(w.weight_swing_leg > 0.0) || !(w.weight_base_accel > 0.0) || !(w.weight_contact_force >= 0.0)) return false;
+  for (double k : {w.swing_kp, w.swing_kd, w.base_accel_kp, w.base_accel_kd, w.base_height_kp, w.base_height_kd, w.base_angular_kp, w.base_angular_kd})
+    if (!(k >= 0.0)) return false;
+  const hb_pd_gains& g = s.gains;
+  for (double k : {g.kp_position, g.kd_position, g.kp_big_stance, g.kp_big_swing, g.kd_big, g.kp_small_stance, g.kp_small_swing, g.kd_small, g.kd_feet})
+    if (!(k >= 0.0)) return false;
+  return true;
+}
+
+int hb_rollout_set_controller_settings(hb_ctx* ctx, int B, const hb_controller_setting* s) {
+  return set_instances(ctx, B, s, controller_setting_ok, &hb_ctx::controllers);
+}
+
 // The camera read of a call whose instances start at ctx->base, on the context's odometry setting, its messages written to pos / has
 static OdomRead odometry_read(const hb_ctx* ctx, double* pos, uint8_t* has) {
   const InstanceView<hb_odometry_setting> set = ctx->odometry.view(ctx->base);
@@ -1128,10 +1166,10 @@ static int policy_adopt(hb_ctx* ctx, int B, InstanceView<int32_t> lat, long long
 
 // hb_resident_wbc_batch_dev; no_prev = true: the fallback has no previous solution yet (first tick after a cold start whose cycle ran no WBC).
 // adopted: the adopted policy is evaluated instead of the resident solution (hb_policy_wbc_async); choice (the episodes): per instance one of
-// the two (PolicyChoice).
+// the two (PolicyChoice); cs (the episodes): each instance's controller setting.
 static int resident_wbc_impl(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
                              int32_t* mode_out, double* wbc_sol, double* torque, int32_t* wbc_status, bool no_prev, bool adopted = false,
-                             const PolicyChoice& choice = PolicyChoice{}) {
+                             const PolicyChoice& choice = PolicyChoice{}, ControllerView cs = ControllerView{}) {
   ENTER(ctx, B, t_now && rbd && x_des && u_des && mode_out && wbc_sol, UNCAPPED, [&] {   // a solution to evaluate
     return adopted ? policies_adopted(ctx, (size_t)ctx->base, (size_t)ctx->base + B) : ctx->base + B <= ctx->res_valid;
   });
@@ -1140,7 +1178,7 @@ static int resident_wbc_impl(hb_ctx* ctx, int B, const double* t_now, const doub
   const int wpb = 4;
   int rc = launch(ctx, K_UNPROFILED, policy_eval_kernel, (B + wpb - 1) / wpb, 32 * wpb, 0, B, (int)N, ctx->cfg.dt, 0.0, s, x_des, u_des, mode_out, t_now,
                   choice);
-  if (!rc) rc = controller_wbc_dev(ctx, B, x_des, u_des, rbd, mode_out, stance_mode, wbc_sol, wbc_status);
+  if (!rc) rc = controller_wbc_dev(ctx, B, x_des, u_des, rbd, mode_out, stance_mode, wbc_sol, wbc_status, cs);
   if (!rc && torque) rc = launch(ctx, K_UNPROFILED, torque_kernel, (B * NJ + 127) / 128, 128, 0, B, wbc_sol, torque);
   return rc ? rc : wbc_fallback(ctx, B, no_prev, wbc_status, wbc_sol, torque);
 }
@@ -1153,6 +1191,15 @@ int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const dou
 int hb_policy_wbc_async(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,
                         int32_t* mode_out, double* wbc_sol, double* torque, int32_t* wbc_status) {
   return resident_wbc_impl(ctx, B, t_now, rbd, stance_mode, x_des, u_des, mode_out, wbc_sol, torque, wbc_status, false, true);
+}
+
+// hb_joint_command_batch_dev, with each instance of `cs` on its own gains (the episodes)
+static int joint_command_dev(hb_ctx* ctx, int B, const hb_pd_gains* gains, double period, const double* x_des, const double* u_des,
+                             const double* wbc_sol, const int32_t* mode_cmd, const double* rbd, const uint8_t* loaded, uint8_t* estop, double* command,
+                             double* output_torque, ControllerView cs) {
+  ENTER(ctx, B, gains && x_des && u_des && wbc_sol && mode_cmd && rbd && command && output_torque, UNCAPPED);
+  return launch(ctx, K_UNPROFILED, joint_command_kernel, (B + 63) / 64, 64, 0, B, *gains, cs, period, x_des, u_des, wbc_sol, mode_cmd, rbd, loaded,
+                estop, command, output_torque);
 }
 
 int hb_default_rollout_params(hb_rollout_params* p) {
@@ -1253,6 +1300,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   // the cameras the sensor read reads and the messages the filter fuses, none without an odometry setting
   const bool odom = e && ctx->odometry.n > 0;
   const OdomRead odom_read = odom ? odometry_read(ctx, ctx->re_opos, ctx->re_ohas) : OdomRead{};
+  const ControllerView controllers = ctx->controllers.view();   // each instance's WBC settings and PD gains, none without a setting
   for (int k = 0; k < n_ticks && !rc; ++k) {
     const int64_t a = tick0 + k;
     const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
@@ -1288,9 +1336,9 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
     }
     // the cycle ran no WBC, so after a cold start the first tick's fallback has no previous solution, as the cycle's own would not have
     if (!rc) rc = resident_wbc_impl(ctx, B, ctx->ro_tnow, meas, nullptr, ctx->xdes, ctx->udes, ctx->wmode, ctx->ro_sol, nullptr, ctx->wstatus, first_cold,
-                                    false, choice);
-    if (!rc) rc = hb_joint_command_batch_dev(ctx, B, &p->gains, p->period, ctx->xdes, ctx->udes, ctx->ro_sol, ctx->wmode, meas, nullptr, estop, ctx->ro_jcmd,
-                                             ctx->ro_jtau);
+                                    false, choice, controllers);
+    if (!rc) rc = joint_command_dev(ctx, B, &p->gains, p->period, ctx->xdes, ctx->udes, ctx->ro_sol, ctx->wmode, meas, nullptr, estop, ctx->ro_jcmd,
+                                    ctx->ro_jtau, controllers);
     if (!rc) rc = hb_actuation_batch_dev(ctx, B, p->actuation_delay, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, ctx->ro_tau);
     if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, ctx->variations.view(), ctx->terrains.view(), nullptr, nullptr);
@@ -1366,9 +1414,7 @@ int hb_default_pd_gains(hb_pd_gains* g) {
 int hb_joint_command_batch_dev(hb_ctx* ctx, int B, const hb_pd_gains* gains, double period, const double* x_des, const double* u_des,
                                const double* wbc_sol, const int32_t* mode_cmd, const double* rbd, const uint8_t* loaded, uint8_t* estop,
                                double* command, double* output_torque) {
-  ENTER(ctx, B, gains && x_des && u_des && wbc_sol && mode_cmd && rbd && command && output_torque, UNCAPPED);
-  return launch(ctx, K_UNPROFILED, joint_command_kernel, (B + 63) / 64, 64, 0, B, *gains, period, x_des, u_des, wbc_sol, mode_cmd, rbd, loaded, estop,
-                command, output_torque);
+  return joint_command_dev(ctx, B, gains, period, x_des, u_des, wbc_sol, mode_cmd, rbd, loaded, estop, command, output_torque, ControllerView{});
 }
 
 int hb_rbd_to_centroidal_batch_dev(hb_ctx* ctx, int B, const double* rbd, double* x) {

@@ -227,7 +227,7 @@ __host__ __device__ constexpr size_t hw_level12_doubles() { return qp_workspace_
 __host__ __device__ constexpr size_t hw_max(size_t a, size_t b) { return a > b ? a : b; }
 __host__ __device__ constexpr size_t hwbc_scratch_doubles() {
   return hw_max(hw_max(hw_level0_doubles(), hw_level12_doubles()),
-                hw_max(hw_max(sizeof(WbcShared) / sizeof(double), (size_t)HQ_N * HQ_LDZ), (size_t)WBC_MA0 * NWBC + WBC_MA0));
+                hw_max(hw_max(sizeof(WbcStaged) / sizeof(double), (size_t)HQ_N * HQ_LDZ), (size_t)WBC_MA0 * NWBC + WBC_MA0));
 }
 __host__ __device__ constexpr size_t hwbc_fused_bytes() { return sizeof(HwbcShared) + hwbc_scratch_doubles() * sizeof(double); }
 // one warp per block: 4 blocks per SM put a 1024-instance batch in two waves on 132 SMs (the runtime reserves 1 KB per block)
@@ -373,14 +373,17 @@ __global__ void __launch_bounds__(32) hwbc_tasks_kernel(int B, hb_wbc_settings w
 // level 0 by hwbc_level0_warp, levels 1 and 2 by qp_solve_warp at their real shape (n = the free variables level 0 leaves, rows = the
 // stacked task0 inequalities), the null-space steps of hoqp_solve_warp in between. sol = x (38), status as hoqp_kernel: 0,
 // 10 * (QP status) + level of the first failing level, or 20 + level when a level leaves more than HW_NX free variables.
-__global__ void __launch_bounds__(32, 4) hwbc_fused_kernel(int B, hb_wbc_settings ws, const double* x_des, const double* u_des, const double* rbd,
-                                                           const int32_t* mode, int max_iter, double* sol, int32_t* status) {
+__global__ void __launch_bounds__(32, 4) hwbc_fused_kernel(int B, hb_wbc_settings ws_ctx, InstanceView<hb_controller_setting> cs, const double* x_des,
+                                                           const double* u_des, const double* rbd, const int32_t* mode, int max_iter, double* sol,
+                                                           int32_t* status) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int inst = blockIdx.x, lane = threadIdx.x;
   if (inst >= B) return;
   HwbcShared& sh = *reinterpret_cast<HwbcShared*>(smem_raw);
   double* U = reinterpret_cast<double*>(smem_raw + sizeof(HwbcShared));     // scratch of the current phase
-  WbcShared& wsh = *reinterpret_cast<WbcShared*>(U);
+  WbcStaged& stg = *reinterpret_cast<WbcStaged*>(U);
+  WbcShared& wsh = stg.sh;
+  const hb_wbc_settings& ws = wbc_select_settings(ws_ctx, cs, inst, stg.ws);   // read until level 0 takes over U
   const int md_ = mode[inst];
   const double* ud = u_des + (size_t)inst * NU;
   wbc_terms_warp(x_des + (size_t)inst * NX, ud, rbd + (size_t)inst * 32, md_, false, ws, wsh);

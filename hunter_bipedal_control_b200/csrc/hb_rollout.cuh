@@ -342,12 +342,16 @@ __global__ void est_schedule_kernel(int B, const hb_reference* refs, hb_estimati
 namespace {  // the kernels: internal linkage, the library exports only the hb_* entry points
 using namespace hb;
 // joint command law (LeggedController.cpp:186-257), one thread per instance; joints are visited in order because the limit
-// protection of joint j only affects the commands of joints >= j within the same cycle
-__global__ void joint_command_kernel(int B, hb_pd_gains g, double dt, const double* x_des, const double* u_des, const double* sol,
-                                     const int32_t* mode_cmd, const double* rbd, const uint8_t* loaded, uint8_t* estop, double* command,
-                                     double* out_tau) {
+// protection of joint j only affects the commands of joints >= j within the same cycle. An instance with a controller setting in `cs` runs
+// its gains in place of `gains`.
+__global__ void joint_command_kernel(int B, hb_pd_gains gains, InstanceView<hb_controller_setting> cs, double dt, const double* x_des,
+                                     const double* u_des, const double* sol, const int32_t* mode_cmd, const double* rbd, const uint8_t* loaded,
+                                     uint8_t* estop, double* command, double* out_tau) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
+  const hb_controller_setting* rec = cs.of(inst);
+  hb_pd_gains g = gains;
+  if (rec) g = rec->gains;
   const double* xd = x_des + (size_t)inst * NX; const double* ud = u_des + (size_t)inst * NU;
   const double* ws = sol + (size_t)inst * NWBC; const double* r = rbd + (size_t)inst * 32;
   const bool is_loaded = loaded ? loaded[inst] != 0 : true;

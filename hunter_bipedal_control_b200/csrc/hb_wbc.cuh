@@ -68,9 +68,10 @@ __device__ inline void rotation_error_world(const double* Rref, const double* Rm
 
 // The WBC terms of one instance in sh, and the motion task rows at unit weight in sh.At, sh.bt: formulateSwingLegTask (3 rows per swing
 // contact, in contact order), then formulateBaseAccelTask (6); in stance mode formulateStanceBaseAccelTask (6 identity rows, b = 0).
-// Returns the number of task rows.
+// Returns the number of task rows. stance_mode is read where it is used (wbc_fused_kernel passes its shared copy: held in a register
+// across the passes, it spilled).
 __device__ inline int wbc_terms_warp(const double* __restrict__ x_des, const double* __restrict__ u_des, const double* __restrict__ rbd,
-                                     int mode, bool stance_mode, const hb_wbc_settings& ws, WbcShared& sh) {
+                                     int mode, const bool& stance_mode, const hb_wbc_settings& ws, WbcShared& sh) {
   const int lane = lane_id();
   const Model& md = c_model;
   // ---- measured q, v (WbcBase.cpp:72-79)
@@ -215,6 +216,19 @@ __device__ inline void wbc_weight_rows(WbcShared& sh, const WbcRows& n, bool sta
   for (int idx = lane; idx < n.nt * 16; idx += 32) sh.At[idx] *= (idx >> 4) < nsr ? ws.weight_swing_leg : ws.weight_base_accel;
   for (int r = lane; r < n.nt; r += 32) sh.bt[r] *= r < nsr ? ws.weight_swing_leg : ws.weight_base_accel;
   __syncwarp();
+}
+
+// The WBC settings instance `inst` runs: its controller setting's (hb_rollout_set_controller_settings) when the view has one, the context's
+// `ws` otherwise. Lane 0 stages them in `dst`, shared memory of the warp, which every lane reads after the call.
+__device__ inline const hb_wbc_settings& wbc_select_settings(const hb_wbc_settings& ws, InstanceView<hb_controller_setting> cs, int inst,
+                                                             hb_wbc_settings& dst) {
+  if (lane_id() == 0) {
+    const hb_controller_setting* c = cs.of(inst);
+    if (c) dst = c->wbc;
+    else dst = ws;
+  }
+  __syncwarp();
+  return dst;
 }
 
 // ---- the tasks on the decision vector [qdd(16), F(12), tau(10)], rows of NWBC columns at leading dimension lda. Rows of task0 after the
@@ -409,7 +423,10 @@ __host__ __device__ constexpr size_t wbc_fused_doubles() { return qp_workspace_d
 // at 7 a tail wave of 100 blocks costs almost as much as the full one). The runtime reserves 1 KB of shared memory per block.
 static_assert(8 * (wbc_fused_doubles() * sizeof(double) + 1024) <= 228 * 1024, "wbc_fused_kernel must fit 8 blocks per SM");
 
-__global__ void __launch_bounds__(32, 8) wbc_fused_kernel(int B, hb_wbc_settings ws, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const uint8_t* stance_mode,
+// The assembly scratch and the WBC settings the warp's instance runs (wbc_select_settings), aliased over the QP's factorisation area
+struct WbcStaged { WbcShared sh; hb_wbc_settings ws; bool stance; };
+
+__global__ void __launch_bounds__(32, 8) wbc_fused_kernel(int B, hb_wbc_settings ws_ctx, InstanceView<hb_controller_setting> cs, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const uint8_t* stance_mode,
                                  double rho, int max_iter, double* sol, int32_t* status, int32_t* iters) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, wpb = blockDim.x >> 5, lane = threadIdx.x & 31;
@@ -426,11 +443,14 @@ __global__ void __launch_bounds__(32, 8) wbc_fused_kernel(int B, hb_wbc_settings
   double* xz = p; p += WZ_N;
   double* nlej = p; p += WZ_N;
   int* stcol = reinterpret_cast<int*>(p);
-  static_assert(sizeof(WbcShared) <= sizeof(double) * (WZ_N * 29 + WZ_N * 7 + WZ_ME * 7 + WZ_N + WZ_ME + 6 * WZ_N + 5 * WZ_ME + 8 * WZ_MI), "assembly scratch must fit in the aliased area");
-  WbcShared& sh = *reinterpret_cast<WbcShared*>(w.K);   // K, V, S, vectors: dead until the QP starts
+  static_assert(sizeof(WbcStaged) <= sizeof(double) * (WZ_N * 29 + WZ_N * 7 + WZ_ME * 7 + WZ_N + WZ_ME + 6 * WZ_N + 5 * WZ_ME + 8 * WZ_MI), "assembly scratch must fit in the aliased area");
+  WbcStaged& stg = *reinterpret_cast<WbcStaged*>(w.K);   // K, V, S, vectors: dead until the QP starts
+  WbcShared& sh = stg.sh;
+  if (lane == 0) stg.stance = stance_mode ? stance_mode[inst] != 0 : false;
+  const hb_wbc_settings& ws = wbc_select_settings(ws_ctx, cs, inst, stg.ws);
   const int md = mode[inst];
-  const bool stance = stance_mode ? stance_mode[inst] != 0 : false;
-  wbc_terms_warp(x_des + (size_t)inst * NX, u_des + (size_t)inst * NU, rbd + (size_t)inst * 32, md, stance, ws, sh);
+  wbc_terms_warp(x_des + (size_t)inst * NX, u_des + (size_t)inst * NU, rbd + (size_t)inst * 32, md, stg.stance, ws, sh);
+  const bool stance = stg.stance;
   const WbcRows n = wbc_rows(md, stance);
   wbc_weight_rows(sh, n, stance, ws);
   int m = 0;

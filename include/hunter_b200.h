@@ -417,6 +417,24 @@ typedef struct {            /* the tracking camera of one robot                 
  * also for a negative period_ticks or delay_ticks, a delay_ticks above HB_ODOM_MAX_DELAY, or a sigma that is negative or not finite. */
 int hb_rollout_set_odometry(hb_ctx* ctx, int B, const hb_odometry_setting* s);
 
+/* ---- controller settings: the controller's run-time tuning per robot (the WBC block of task.info, WbcBase::setKpKd, and the joint PD
+ * gains of LeggedController's dynamic_reconfigure, LeggedController.cpp:433-447) ----
+ * Record i acts on instance i of both episode calls: its wbc replaces the context's WBC settings (hb_wbc_set_settings, hb_wbc_set_kp_kd,
+ * hb_load_task_info) in the tick's WBC under both formulations (the three weights act only under HB_WBC_WEIGHTED, as the context's do), and
+ * its gains replace p->gains in the joint command law (the episodes run the loaded branch: kp_position / kd_position are carried and read
+ * by nothing, as those of p->gains). Instances at or beyond B keep the context's settings and p->gains, bit for bit as with no setting.
+ * Every other entry point ignores this setting: the control step, the resident cycle and tick, hb_wbc_solve_batch, hb_hierarchical_wbc_*,
+ * hb_joint_command_batch, hb_policy_wbc and the adapters run the context's settings and the gains they are given.
+ * The setting adds no launch to an episode; the fused WBC kernels and the joint command law read the record of their own instance. */
+typedef struct {
+  hb_wbc_settings wbc;   /* in place of the context's WBC settings, for this robot */
+  hb_pd_gains gains;     /* in place of hb_rollout_params.gains, for this robot     */
+} hb_controller_setting;
+/* Sets the controller settings of the context's episodes (a per-robot episode setting, above). -1 also for a field that is not finite, or
+ * for a record hb_wbc_set_settings would reject (a torque limit, friction_coefficient, weight_swing_leg or weight_base_accel <= 0,
+ * weight_contact_force < 0), a negative WBC task kp / kd, or a negative PD gain. */
+int hb_rollout_set_controller_settings(hb_ctx* ctx, int B, const hb_controller_setting* s);
+
 /* ---- estimated episodes (hb_rollout_estimated_batch_dev): the controllers read the Kalman filter's estimate from synthesised, noisy
  * sensors instead of the plant's true state (LeggedController::updateStateEstimation, LeggedController.cpp:280-349) ---- */
 typedef struct {                 /* standard deviations of additive Gaussian sensor noise; 0 = that channel is exact and draws nothing */

@@ -44,11 +44,13 @@ def parser(batch_help="robots per episode"):
     return ap
 
 
-def sweep_args(tool, timed_help, ncell):
-    """The command line of a sweep over ncell cells, validated: --repeats, --timed and the common arguments."""
+def sweep_args(tool, timed_help, ncell, extra=None):
+    """The command line of a sweep over ncell cells, validated: --repeats, --timed, the common arguments and what extra(parser) adds."""
     ap = parser("robots per episode (a multiple of %d)" % ncell)
     ap.add_argument("--repeats", type=int, default=4, help="episodes per grid (the robot -> cell assignment shifts between them)")
     ap.add_argument("--timed", type=int, default=3, help=timed_help)
+    if extra:
+        extra(ap)
     args = ap.parse_args()
     if args.batch < ncell or args.batch % ncell or args.repeats < 1 or args.sensor_noise < 0 or (args.sensor_noise and not args.estimator):
         raise SystemExit("%s: --batch a multiple of %d, --repeats >= 1, --sensor-noise takes a scale >= 0 and needs --estimator" % (tool, ncell))
@@ -93,19 +95,26 @@ class Episodes:
         self.stream = torch.cuda.ExternalStream(self.ctx.stream_handle, device=self.dev)
         self.lib = hb.load_library()
 
-    def episode(self, estimated=None, est_stats=False):
+    def episode(self, estimated=None, est_stats=False, rows=None):
         """One episode of self.ticks ticks from the start poses in one hb_rollout_batch_dev call, or hb_rollout_estimated_batch_dev when
-        estimated (default: --estimator), with device events around the call. est_stats: also collect the estimation stats."""
-        torch, hb, B, dev, ctx = self.torch, self.hb, self.B, self.dev, self.ctx
+        estimated (default: --estimator), with device events around the call. est_stats: also collect the estimation stats. rows: the
+        robots of a smaller batch (default: all), each with its start pose, command and noise stream, as instances 0 .. len(rows) - 1."""
+        torch, hb, dev, ctx = self.torch, self.hb, self.dev, self.ctx
+        rows = np.arange(self.B) if rows is None else np.asarray(rows)
+        B = len(rows)
+        cmds = self.cmds if B == self.B and (rows == np.arange(B)).all() else (hb.HbRolloutCommand * B)(*[self.cmds[i] for i in rows])
         estimated = self.args.estimator if estimated is None else estimated
         P = lambda t: C.c_void_p(t.data_ptr())
-        d_rbd = torch.from_numpy(self.rbd0).to(dev)
+        d_rbd = torch.from_numpy(np.ascontiguousarray(self.rbd0[rows])).to(dev)
         d_act = torch.zeros(B * C.sizeof(hb.HbActuationState), dtype=torch.uint8, device=dev)
         d_estop = torch.zeros(B, dtype=torch.uint8, device=dev)
         d_st = torch.from_numpy(hb.rollout_stats(B).view(np.uint8).copy()).to(dev)
         d_es = None
         if estimated:
-            d_est = torch.from_numpy(np.frombuffer(bytes(hb.estimation_states(B)), dtype=np.uint8).copy()).to(dev)
+            est = hb.estimation_states(B)
+            for k, i in enumerate(rows):
+                est[k].noise_stream = int(i)
+            d_est = torch.from_numpy(np.frombuffer(bytes(est), dtype=np.uint8).copy()).to(dev)
             if est_stats:
                 d_es = torch.from_numpy(hb.estimation_stats(B).view(np.uint8).copy()).to(dev)
         torch.cuda.synchronize(dev)
@@ -113,10 +122,10 @@ class Episodes:
         l0 = ctx.launch_count
         e0.record(self.stream)
         if estimated:
-            rc = self.lib.hb_rollout_estimated_batch_dev(ctx._h, B, C.c_int64(0), self.ticks, C.byref(self.prm), C.byref(self.ep), self.cmds, P(d_rbd),
+            rc = self.lib.hb_rollout_estimated_batch_dev(ctx._h, B, C.c_int64(0), self.ticks, C.byref(self.prm), C.byref(self.ep), cmds, P(d_rbd),
                                                          P(d_act), P(d_estop), P(d_st), P(d_est), None if d_es is None else P(d_es), None, None)
         else:
-            rc = self.lib.hb_rollout_batch_dev(ctx._h, B, C.c_int64(0), self.ticks, C.byref(self.prm), self.cmds, P(d_rbd), P(d_act), P(d_estop), P(d_st),
+            rc = self.lib.hb_rollout_batch_dev(ctx._h, B, C.c_int64(0), self.ticks, C.byref(self.prm), cmds, P(d_rbd), P(d_act), P(d_estop), P(d_st),
                                                None)
         e1.record(self.stream)
         assert rc == 0, rc
