@@ -45,6 +45,7 @@ EXPORTED_SYMBOLS = [
     "hb_rollout_set_mpc_latencies", "hb_policy_update", "hb_policy_wbc", "hb_policy_wbc_async",
     "hb_rollout_set_odometry", "hb_sim_read_odometry", "hb_sim_read_odometry_async", "hb_estimator_fuse_odometry", "hb_estimator_fuse_odometry_async",
     "hb_rollout_set_controller_settings",
+    "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
 ]
 
 
@@ -105,6 +106,85 @@ def goal_to_target(t, x, goal):
     t = _f64(np.broadcast_to(_f64(t), (B,))); goal = _f64(np.broadcast_to(_f64(goal), (B, 3)))
     out = (HbTarget * B)()
     _check(load_library().hb_goal_to_target(B, _ptr(t), _ptr(x), _ptr(goal), out), "hb_goal_to_target")
+    return out
+
+
+HB_GAIT_MAX_PHASES = 8
+MODE_NAMES = {"FLY": 0, "R": 1, "L": 2, "STANCE": 3}      # gait.info's mode names (string2ModeNumber)
+SWING_FIELDS = ("swing_height", "swing_time_scale", "next_stance_z", "feet_bias_x1", "feet_bias_x2", "feet_bias_y", "feet_bias_z")
+
+
+class HbGaitTemplate(C.Structure):
+    _fields_ = [("n_phase", C.c_int32), ("modes", C.c_int32 * HB_GAIT_MAX_PHASES), ("switching_times", C.c_double * (HB_GAIT_MAX_PHASES + 1))]
+
+
+class HbPlannerSettings(C.Structure):
+    _fields_ = [("gait", HbGaitTemplate * 4)] + [(k, C.c_double) for k in SWING_FIELDS]
+
+
+def gait_template(modes, switching_times):
+    """HbGaitTemplate of a ModeSequenceTemplate: modes (names FLY / R / L / STANCE or ids 0..3) and their n + 1 switching times, [0] = 0.
+    Raises ValueError for an unknown mode name, counts that do not match or more than HB_GAIT_MAX_PHASES phases; the library checks the
+    times (hb_plan_set_settings)."""
+    m = [MODE_NAMES[x] if isinstance(x, str) else int(x) for x in modes]
+    t = [float(x) for x in switching_times]
+    if not 1 <= len(m) <= HB_GAIT_MAX_PHASES or len(t) != len(m) + 1:
+        raise ValueError("gait template: 1..%d modes and one more switching time expected, got %d and %d" % (HB_GAIT_MAX_PHASES, len(m), len(t)))
+    g = HbGaitTemplate()
+    g.n_phase = len(m)
+    g.modes[:len(m)] = m
+    g.switching_times[:len(t)] = t
+    return g
+
+
+def default_planner_settings():
+    """hb_default_planner_settings: gait.info's four templates and task.info's swing_trajectory_config, the compiled-in planner values."""
+    s = HbPlannerSettings()
+    _check(load_library().hb_default_planner_settings(C.byref(s)), "hb_default_planner_settings")
+    return s
+
+
+def parse_planner_settings(task_info, gait_info):
+    """hb_parse_planner_settings: swing_trajectory_config of a task.info file and the templates of a gait.info file in its list order (host
+    only); absent keys and templates keep the defaults."""
+    s = HbPlannerSettings()
+    _check(load_library().hb_parse_planner_settings(str(task_info).encode(), str(gait_info).encode(), C.byref(s)), "hb_parse_planner_settings")
+    return s
+
+
+def _is_template(v):
+    """A single template: an HbGaitTemplate or a (modes, switching_times) pair whose modes are names or ids."""
+    if isinstance(v, HbGaitTemplate):
+        return True
+    return len(v) == 2 and all(isinstance(m, str) or np.ndim(m) == 0 for m in v[0])
+
+
+def make_planner_settings(B, base=None, gaits=None, **fields):
+    """ctypes array of B HbPlannerSettings (Context.set_planner_settings, plan_references(settings=...)): each robot's gait templates and
+    swing settings. base (HbPlannerSettings) is every record's start, default default_planner_settings(). gaits maps a gait (name of
+    GAIT_IDS or id) to a template, an HbGaitTemplate or (modes, switching_times) as gait_template takes, for every robot, or to a list of B
+    such templates, one per robot. The swing fields (SWING_FIELDS) can be given by name, as a scalar or a (B,) array. Raises ValueError for
+    an unknown name, a malformed template or a shape that does not broadcast."""
+    base = default_planner_settings() if base is None else base
+    out = (HbPlannerSettings * B)()
+    v = np.ctypeslib.as_array(out)
+    v[:] = np.frombuffer(bytes(base), dtype=v.dtype)[0]
+    for name, value in fields.items():
+        if name not in SWING_FIELDS:
+            raise ValueError("planner settings: unknown field %r" % name)
+        try:
+            v[name] = np.broadcast_to(_f64(value), (B,))
+        except ValueError as e:
+            raise ValueError("planner settings: %s: (B,) or a scalar expected: %s" % (name, e))
+    for gait, tmpl in (gaits or {}).items():
+        g = GAIT_IDS[gait] if isinstance(gait, str) else int(gait)
+        if not 0 <= g <= 3:
+            raise ValueError("planner settings: gait %r outside 0..3" % (gait,))
+        per = [tmpl] * B if _is_template(tmpl) else list(tmpl)
+        if len(per) != B:
+            raise ValueError("planner settings: gait %r: one template or %d expected, got %d" % (gait, B, len(per)))
+        for i, t in enumerate(per):
+            out[i].gait[g] = t if isinstance(t, HbGaitTemplate) else gait_template(*t)
     return out
 
 
@@ -608,18 +688,24 @@ def plan_set_threads(n):
 
 
 def plan_references(t0, horizon, x0, cmd_vel, feet_pos, gait, gait_start, prev_event=None, time_to_target=None, latest_stance=None, joint_ik=True,
-                    targets=None):
+                    targets=None, settings=None):
     """Host-side reference planner (hb_plan_references): returns (ctypes array of HbReference, latest_stance[B,12]). targets: B HbTarget
     (make_targets, goal_to_target) planned on instead of the cmd_vel targets (hb_plan_references_targets); cmd_vel still drives the swing
-    planner."""
+    planner. settings: B HbPlannerSettings (make_planner_settings) in place of the compiled-in templates and swing settings
+    (hb_plan_references_settings)."""
     lib = load_library()
     ins = make_plan_inputs(t0, horizon, x0, cmd_vel, feet_pos, gait, gait_start, prev_event, time_to_target, joint_ik)
     B = len(ins)
     if targets is not None and len(targets) != B:
         raise ValueError("plan_references: %d targets for %d instances" % (len(targets), B))
+    if settings is not None and len(settings) != B:
+        raise ValueError("plan_references: %d planner settings for %d instances" % (len(settings), B))
     ls = np.zeros((B, 12)) if latest_stance is None else _f64(latest_stance).copy()
     refs = (HbReference * B)()
-    _check(lib.hb_plan_references_targets(B, ins, targets, _ptr(ls), refs), "hb_plan_references_targets")
+    if settings is None:
+        _check(lib.hb_plan_references_targets(B, ins, targets, _ptr(ls), refs), "hb_plan_references_targets")
+    else:
+        _check(lib.hb_plan_references_settings(B, ins, targets, settings, _ptr(ls), refs), "hb_plan_references_settings")
     return refs, ls
 
 
@@ -1022,6 +1108,12 @@ class Context:
         """Explicit planner targets of this context (hb_plan_set_targets): targets[i] (make_targets, goal_to_target) replaces the cmd_vel
         target of instance i in plan_references_gpu and resident_plan_cycle (not in the episodes); None clears them."""
         self._set_instances("hb_plan_set_targets", targets)
+
+    def set_planner_settings(self, settings):
+        """Planner settings of this context (hb_plan_set_settings): settings[i] (make_planner_settings) gives the gait templates and swing
+        settings of instance i in every device planner path -- plan_references_gpu, resident_plan_cycle, rollout and rollout_estimated --
+        instances beyond len(settings) plan with the compiled-in ones; None clears them."""
+        self._set_instances("hb_plan_set_settings", settings)
 
     def resident_wbc(self, t_now, rbd, stance_mode=None):
         """Policy of the resident solution at absolute time t_now + WeightedWbc: returns (x_des, u_des, mode, sol, torque, status)."""

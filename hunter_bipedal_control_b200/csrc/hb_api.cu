@@ -105,6 +105,8 @@ struct hb_ctx {
   OdomCamera* odom_cam;
   // each instance's WBC settings and joint PD gains in the episodes (hb_rollout_set_controller_settings)
   InstanceSetting<hb_controller_setting> controllers;
+  // each instance's gait templates and swing settings in every device planner path (hb_plan_set_settings)
+  InstanceSetting<hb_planner_settings> plan_settings;
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
   // hb_resident_cycle_batch's packed references / reference verdicts
   void* arena; size_t arena_cap;
@@ -482,7 +484,7 @@ int hb_destroy(hb_ctx* ctx) {
   cudaSetDevice(ctx->device);
   void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->arena,
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
-                       ctx->odometry.dev, ctx->controllers.dev};
+                       ctx->odometry.dev, ctx->controllers.dev, ctx->plan_settings.dev};
   for (void* p : mem) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -775,17 +777,18 @@ static const hbplan::PlanConsts& plan_consts() {
   return pc;
 }
 
-// The device planner after the entry checks: an instance with a record in targets plans on it where captured is null or captured[i] >= 0
+// The device planner after the entry checks: an instance with a record in targets plans on it where captured is null or captured[i] >= 0;
+// an instance with a record in settings plans with it
 static int plan_dev(hb_ctx* ctx, int B, const hb_plan_input* in, const double* feet, double* latest_stance, hb_reference* out, int32_t* status,
-                    InstanceView<hb_target> targets, const int32_t* captured) {
+                    InstanceView<hb_target> targets, const int32_t* captured, InstanceView<hb_planner_settings> settings) {
   return launch(ctx, K_UNPROFILED, plan_references_coop_kernel, (B + 7) / 8, 32, 0, B, in, feet, latest_stance, out, status, plan_consts(), targets,
-                captured);
+                captured, settings);
 }
 
 int hb_plan_references_batch_dev(hb_ctx* ctx, int B, const hb_plan_input* in, const double* feet, double* latest_stance, hb_reference* out,
                                  int32_t* status) {
   ENTER(ctx, B, in && latest_stance && out, UNCAPPED);
-  return plan_dev(ctx, B, in, feet, latest_stance, out, status, ctx->plan_targets.view(ctx->base), nullptr);
+  return plan_dev(ctx, B, in, feet, latest_stance, out, status, ctx->plan_targets.view(ctx->base), nullptr, ctx->plan_settings.view(ctx->base));
 }
 
 int hb_default_kf_params(hb_kf_params* p) {
@@ -960,6 +963,76 @@ int hb_load_task_info(hb_ctx* ctx, const char* path) {
   return hb_wbc_set_settings(ctx, &ti.wbc);
 }
 
+// The ranges of hunter_b200.h's hb_planner_settings (NaN fails every test); the entries beyond n_phase are not read
+static bool planner_settings_ok(const hb_planner_settings& s) {
+  for (const hb_gait_template& g : s.gait) {
+    if (g.n_phase < 1 || g.n_phase > HB_GAIT_MAX_PHASES || !(g.switching_times[0] == 0.0)) return false;
+    for (int k = 0; k < g.n_phase; ++k) {
+      if (g.modes[k] < 0 || g.modes[k] > 3) return false;
+      if (!(g.switching_times[k + 1] > g.switching_times[k]) || !isfinite(g.switching_times[k + 1])) return false;
+    }
+  }
+  if (!isfinite(s.swing_height) || !(s.swing_height >= 0.0) || !isfinite(s.swing_time_scale) || !(s.swing_time_scale > 0.0)) return false;
+  for (double v : {s.next_stance_z, s.feet_bias_x1, s.feet_bias_x2, s.feet_bias_y, s.feet_bias_z}) if (!isfinite(v)) return false;
+  return true;
+}
+
+int hb_default_planner_settings(hb_planner_settings* s) {
+  if (!s) return HB_EINVAL;
+  hbplan::default_settings(*s);
+  return HB_OK;
+}
+
+namespace {
+// string2ModeNumber (MotionPhaseDefinition.h:57-60, :117-125) for the biped's modes; -1 for any other name
+int mode_number(const std::string& name) {
+  const char* names[4] = {"FLY", "R", "L", "STANCE"};
+  for (int m = 0; m < 4; ++m) if (name == names[m]) return m;
+  return -1;
+}
+// loadModeSequenceTemplate (ModeSequenceTemplate.cpp:59-83) of the template `name`: returns 1 with *t filled, 0 when the file has neither
+// of its lists, -1 when they are malformed (an unknown mode name, a non-numeric time, counts that are not n and n + 1, n > HB_GAIT_MAX_PHASES)
+int gait_template_from(const InfoMap& m, const std::string& name, hb_gait_template* t) {
+  memset(t, 0, sizeof(*t));
+  int nm = 0, nt = 0;
+  for (const std::string* v; (v = m.find(name + ".modeSequence.[" + std::to_string(nm) + "]")); ++nm) {
+    if (nm == HB_GAIT_MAX_PHASES) return -1;
+    if ((t->modes[nm] = mode_number(*v)) < 0) return -1;
+  }
+  for (std::string k; m.find(k = name + ".switchingTimes.[" + std::to_string(nt) + "]"); ++nt)
+    if (nt == HB_GAIT_MAX_PHASES + 1 || !m.number(k, &t->switching_times[nt])) return -1;
+  if (nm == 0 && nt == 0) return 0;
+  if (nm == 0 || nt != nm + 1) return -1;
+  t->n_phase = nm;
+  return 1;
+}
+}  // namespace
+
+int hb_parse_planner_settings(const char* task_info, const char* gait_info, hb_planner_settings* out) {
+  if (!task_info || !gait_info || !out) return HB_EINVAL;
+  InfoMap task, gait;
+  if (!info_parse(task_info, task) || !info_parse(gait_info, gait)) return HB_EINVAL;
+  hb_planner_settings s;
+  hbplan::default_settings(s);
+  // loadSwingTrajectorySettings (SwingTrajectoryPlanner.cpp:549-561): the fields the planner reads; an absent key keeps its default
+  const std::pair<const char*, double*> swing[] = {{"swingHeight", &s.swing_height}, {"swingTimeScale", &s.swing_time_scale},
+                                                   {"next_position_z", &s.next_stance_z}, {"feet_bias_x1", &s.feet_bias_x1},
+                                                   {"feet_bias_x2", &s.feet_bias_x2}, {"feet_bias_y", &s.feet_bias_y}, {"feet_bias_z", &s.feet_bias_z}};
+  for (const auto& f : swing) task.number(std::string("swing_trajectory_config.") + f.first, f.second);
+  // gait.info: gait g is the template named by list.[g]
+  for (int g = 0; g < 4; ++g) {
+    const std::string* name = gait.find("list.[" + std::to_string(g) + "]");
+    if (!name) continue;
+    hb_gait_template t;
+    const int rc = gait_template_from(gait, *name, &t);
+    if (rc < 0) return HB_EINVAL;
+    if (rc > 0) s.gait[g] = t;
+  }
+  if (!planner_settings_ok(s)) return HB_EINVAL;
+  *out = s;
+  return HB_OK;
+}
+
 int hb_default_sim_params(hb_sim_params* p) {
   if (!p) return HB_EINVAL;
   p->dt = 0.002; p->substeps = 4; p->ground_height = 0.0; p->ground_stiffness = 3.0e4; p->ground_damping = 3.0e2; p->tangential_damping = 3.0e2; p->friction_mu = 0.7;
@@ -1079,6 +1152,10 @@ static bool target_ok(const hb_target& tg) {
 }
 
 int hb_plan_set_targets(hb_ctx* ctx, int B, const hb_target* t) { return set_instances(ctx, B, t, target_ok, &hb_ctx::plan_targets); }
+
+int hb_plan_set_settings(hb_ctx* ctx, int B, const hb_planner_settings* s) {
+  return set_instances(ctx, B, s, planner_settings_ok, &hb_ctx::plan_settings);
+}
 
 static bool latency_ok(const int32_t& d) { return d >= 0; }     // the upper bound is the episode's mpc_every, checked by the episode call
 
@@ -1325,7 +1402,8 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
       rc = launch(ctx, K_UNPROFILED, rollout_plan_inputs_kernel, grid, 64, 0, B, t, horizon, ctx->ro_cmd, meas, e ? e->est : nullptr, ctx->ro_in,
                   ctx->goals.view(), first_cold ? 1 : 0, ctx->goal_tg, ctx->goal_idx, plan_consts());
       if (!rc) rc = launch(ctx, K_UNPROFILED, plan_prepare_kernel, grid, 64, 0, B, ctx->ro_in, ctx->ro_t0, ctx->ro_x0, ctx->ro_feet);
-      if (!rc) rc = plan_dev(ctx, B, ctx->ro_in, ctx->ro_feet, ctx->res_stance, ctx->ro_refs, ctx->ro_pstat, goal_targets, ctx->goal_idx);
+      if (!rc) rc = plan_dev(ctx, B, ctx->ro_in, ctx->ro_feet, ctx->res_stance, ctx->ro_refs, ctx->ro_pstat, goal_targets, ctx->goal_idx,
+                             ctx->plan_settings.view());
       if (!rc) rc = resident_cycle_impl(ctx, B, first_cold, 0.0, ctx->ro_t0, ctx->ro_x0, ctx->ro_refs, meas, ctx->ro_info, nullptr, nullptr, nullptr, false);
       // the cold tick: every instance with a latency starts with the policy of this first solve
       if (!rc && delayed && first_cold) {
@@ -1856,10 +1934,12 @@ int hb_contact_positions_batch(hb_ctx* ctx, int B, const double* x, double* pos)
 }
 
 static std::atomic<int> g_plan_threads{0};   // 0 = hardware_concurrency (hb_plan_set_threads)
-static int plan_range(int lo, int hi, const hb_plan_input* in, const hb_target* targets, double* latest_stance, hb_reference* out) {
+static int plan_range(int lo, int hi, const hb_plan_input* in, const hb_target* targets, const hb_planner_settings* settings, double* latest_stance,
+                      hb_reference* out) {
   const hbplan::PlanConsts& pc = plan_consts();
   for (int i = lo; i < hi; ++i) {
-    const int rc = hbplan::plan_one(pc, in[i], targets ? targets + i : nullptr, latest_stance + (size_t)i * 12, out + i, true);
+    const int rc = hbplan::plan_one(pc, in[i], targets ? targets + i : nullptr, settings ? settings + i : nullptr, latest_stance + (size_t)i * 12,
+                                    out + i, true);
     if (rc) return rc;
   }
   return HB_OK;
@@ -1876,17 +1956,22 @@ int hb_plan_references(int B, const hb_plan_input* in, double* latest_stance, hb
 }
 
 int hb_plan_references_targets(int B, const hb_plan_input* in, const hb_target* targets, double* latest_stance, hb_reference* out) {
-  if (B < 0 || !in || !latest_stance || !out || !all_ok(B, targets, target_ok)) return HB_EINVAL;
+  return hb_plan_references_settings(B, in, targets, nullptr, latest_stance, out);
+}
+
+int hb_plan_references_settings(int B, const hb_plan_input* in, const hb_target* targets, const hb_planner_settings* settings, double* latest_stance,
+                                hb_reference* out) {
+  if (B < 0 || !in || !latest_stance || !out || !all_ok(B, targets, target_ok) || !all_ok(B, settings, planner_settings_ok)) return HB_EINVAL;
   // instances are independent: spread them over the host cores (the planner feeds ~1e5 solves/s per GPU; one core plans ~2e4/s)
   unsigned hw = std::thread::hardware_concurrency();
   if (const int forced = g_plan_threads.load()) hw = (unsigned)forced;
   int nt = (int)std::min<unsigned>(hw ? hw : 1u, (unsigned)((B + 63) / 64));
-  if (nt <= 1) return plan_range(0, B, in, targets, latest_stance, out);
+  if (nt <= 1) return plan_range(0, B, in, targets, settings, latest_stance, out);
   std::vector<std::thread> pool;
   std::vector<int> rcs(nt, HB_OK);
   for (int t = 0; t < nt; ++t) {
     const int lo = (int)((long long)B * t / nt), hi = (int)((long long)B * (t + 1) / nt);
-    pool.emplace_back([=, &rcs]() { rcs[t] = plan_range(lo, hi, in, targets, latest_stance, out); });
+    pool.emplace_back([=, &rcs]() { rcs[t] = plan_range(lo, hi, in, targets, settings, latest_stance, out); });
   }
   for (auto& th : pool) th.join();
   for (int t = 0; t < nt; ++t) if (rcs[t]) return rcs[t];

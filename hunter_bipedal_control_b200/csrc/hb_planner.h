@@ -1,6 +1,6 @@
 // Host-side reference preprocessing of one MPC solve (SURVEY 8a rows P1, P3, P5), mirroring the reference's own objects:
 //   P1  GaitSchedule::{insertModeSequenceTemplate, tileModeSequenceTemplate}      legged_interface/src/gait/GaitSchedule.cpp:57-161
-//       gait templates                                                            legged_controllers/config/hunter/reference.info:54-118
+//       gait templates                                                            legged_controllers/config/hunter/gait.info (hb_planner_settings.gait)
 //   P3  SwingTrajectoryPlanner::{update, calNextFootPos, genSwingTrajs}           legged_interface/src/foot_planner/SwingTrajectoryPlanner.cpp:164-358
 //       CubicSpline nodes (time, position, velocity)                              legged_interface/src/foot_planner/CubicSpline.cpp:46-70
 //   P5  cmdVelToTargetTrajectories / targetPoseToTargetTrajectories               legged_controllers/src/TargetTrajectoriesPublisher.cpp:41-130
@@ -61,16 +61,49 @@ HBP_HD inline bool contact_flag(int mode, int c) { return (c & 1) ? (mode == 1 |
 
 struct ModeSchedule { int n_events; double events[MAX_PHASES]; int modes[MAX_PHASES + 1]; };   // n_events + 1 modes
 
-// reference.info:54-118; returns the number of phases of the template
-HBP_HD inline int gait_template(int gait, int* modes, double* times) {
+// The compiled-in template of gait 0..3 (legged_controllers/config/hunter/gait.info, ModeSequenceTemplate): hb_default_planner_settings.
+// The entries beyond n_phase are left as they are.
+HBP_HD inline void gait_template(int gait, hb_gait_template& g) {
+  int32_t* modes = g.modes; double* times = g.switching_times;
   switch (gait) {
-    case 1: modes[0] = 2; modes[1] = 1; times[0] = 0.0; times[1] = 0.3; times[2] = 0.6; return 2;                           // trot
+    case 1: modes[0] = 2; modes[1] = 1; times[0] = 0.0; times[1] = 0.3; times[2] = 0.6; g.n_phase = 2; break;                 // trot
     case 2: modes[0] = 2; modes[1] = 3; modes[2] = 1; modes[3] = 3;
-            times[0] = 0.0; times[1] = 0.25; times[2] = 0.3; times[3] = 0.55; times[4] = 0.6; return 4;                     // standing_trot
+            times[0] = 0.0; times[1] = 0.25; times[2] = 0.3; times[3] = 0.55; times[4] = 0.6; g.n_phase = 4; break;           // standing_trot
     case 3: modes[0] = 2; modes[1] = 0; modes[2] = 1; modes[3] = 0;
-            times[0] = 0.0; times[1] = 0.15; times[2] = 0.2; times[3] = 0.35; times[4] = 0.4; return 4;                     // flying_trot
-    default: modes[0] = 3; times[0] = 0.0; times[1] = 0.5; return 1;                                                          // stance
+            times[0] = 0.0; times[1] = 0.15; times[2] = 0.2; times[3] = 0.35; times[4] = 0.4; g.n_phase = 4; break;           // flying_trot
+    default: modes[0] = 3; times[0] = 0.0; times[1] = 0.5; g.n_phase = 1; break;                                                // stance
   }
+}
+
+// What one instance's plan reads of its hb_planner_settings: the template of its gait and swing_trajectory_config (168 B, staged per
+// instance in shared memory by the device planner).
+struct PlanSettings {
+  hb_gait_template tmpl;
+  double swing_height, swing_time_scale, next_stance_z, feet_bias_x1, feet_bias_x2, feet_bias_y, feet_bias_z;
+};
+
+// The settings of an instance planning gait `gait` (0..3): from its record s, or with s null the compiled-in values (task.info's
+// swing_trajectory_config, next_position_z at the loader's default), which hb_default_planner_settings records give as well.
+HBP_HD inline void plan_settings(const hb_planner_settings* s, int gait, PlanSettings& ps) {
+  if (s) {
+    ps.tmpl = s->gait[gait];
+    ps.swing_height = s->swing_height; ps.swing_time_scale = s->swing_time_scale; ps.next_stance_z = s->next_stance_z;
+    ps.feet_bias_x1 = s->feet_bias_x1; ps.feet_bias_x2 = s->feet_bias_x2; ps.feet_bias_y = s->feet_bias_y; ps.feet_bias_z = s->feet_bias_z;
+    return;
+  }
+  gait_template(gait, ps.tmpl);
+  ps.swing_height = HB_SWING_HEIGHT; ps.swing_time_scale = HB_SWING_TIME_SCALE; ps.next_stance_z = HB_NEXT_POSITION_Z;
+  ps.feet_bias_x1 = HB_FEET_BIAS_X1; ps.feet_bias_x2 = HB_FEET_BIAS_X2; ps.feet_bias_y = HB_FEET_BIAS_Y; ps.feet_bias_z = HB_FEET_BIAS_Z;
+}
+
+// hb_default_planner_settings: every gait's compiled-in template (unused entries zero) and the compiled-in swing settings
+inline void default_settings(hb_planner_settings& s) {
+  memset(&s, 0, sizeof(s));
+  for (int g = 0; g < 4; ++g) gait_template(g, s.gait[g]);
+  PlanSettings ps;
+  plan_settings(nullptr, 0, ps);
+  s.swing_height = ps.swing_height; s.swing_time_scale = ps.swing_time_scale; s.next_stance_z = ps.next_stance_z;
+  s.feet_bias_x1 = ps.feet_bias_x1; s.feet_bias_x2 = ps.feet_bias_x2; s.feet_bias_y = ps.feet_bias_y; s.feet_bias_z = ps.feet_bias_z;
 }
 
 // A schedule that is STANCE (two phases split at `prev_event`, like the reference's initialModeSchedule {STANCE, STANCE},
@@ -78,9 +111,9 @@ HBP_HD inline int gait_template(int gait, int* modes, double* times) {
 // GaitSchedule.cpp:57-93 (insert; the last mode before insertion is STANCE, so no extra transition phase) and :123-161 (tile).
 // Like GaitSchedule::getModeSchedule (:95-121), which drops the phases older than its lower bound, whole template periods that end
 // before `t_keep` are skipped; the schedule inside [t_keep, final_time] is unchanged. Returns false when MAX_PHASES is exceeded.
-HBP_HD inline bool tile_gait(int gait, double prev_event, double start, double t_keep, double final_time, ModeSchedule& ms) {
-  int tm[4]; double tt[5];
-  const int np = gait_template(gait, tm, tt);
+HBP_HD inline bool tile_gait(const hb_gait_template& g, double prev_event, double start, double t_keep, double final_time, ModeSchedule& ms) {
+  const int32_t* tm = g.modes; const double* tt = g.switching_times;
+  const int np = g.n_phase;
   const double period = tt[np];
   if (start < t_keep) start += floor((t_keep - start) / period) * period;
   int ne = 0;
@@ -205,11 +238,11 @@ HBP_HD inline void find_index(int index, const bool* stock, int n, int& start_id
 
 // SwingTrajectoryPlanner::calNextFootPos (:289-312). body_vel_cmd = [vx, vy, vz, wz, 0, 0] as set from /cmd_vel_filtered
 // (SwitchedModelReferenceManager.cpp:91-101): its tail(3) = (wz, 0, 0) is used as the commanded angular velocity, as the reference does.
-HBP_HD inline Vec3 next_foot_pos(int foot, double current_time, double stop_time, double next_middle_time, const double* next_middle_body_pos,
+HBP_HD inline Vec3 next_foot_pos(const PlanSettings& s, int foot, double current_time, double stop_time, double next_middle_time, const double* next_middle_body_pos,
                           const double* current_body_pos, Vec3 current_body_vel, const double* body_vel_cmd) {
-  const Vec3 bias[4] = {{HB_FEET_BIAS_X1, HB_FEET_BIAS_Y, HB_FEET_BIAS_Z}, {HB_FEET_BIAS_X1, -HB_FEET_BIAS_Y, HB_FEET_BIAS_Z},
-                        {HB_FEET_BIAS_X2, HB_FEET_BIAS_Y, HB_FEET_BIAS_Z}, {HB_FEET_BIAS_X2, -HB_FEET_BIAS_Y, HB_FEET_BIAS_Z}};
-  const Vec3 roted_bias = rot_zyx(next_middle_body_pos + 3, bias[foot]);
+  // feet_bias_ (SwingTrajectoryPlanner.cpp:76-79): toes x1, heels x2, +y on the left
+  const Vec3 bias{foot < 2 ? s.feet_bias_x1 : s.feet_bias_x2, (foot & 1) ? -s.feet_bias_y : s.feet_bias_y, s.feet_bias_z};
+  const Vec3 roted_bias = rot_zyx(next_middle_body_pos + 3, bias);
   const Vec3 vel_cmd_linear = rot_zyx(current_body_pos + 3, {body_vel_cmd[0], body_vel_cmd[1], body_vel_cmd[2]});
   const Vec3 vel_cmd_angular = rot_zyx(current_body_pos + 3, {body_vel_cmd[3], body_vel_cmd[4], body_vel_cmd[5]});
   Vec3 vel_linear = current_body_vel; vel_linear.z = 0.0;
@@ -218,12 +251,12 @@ HBP_HD inline Vec3 next_foot_pos(int foot, double current_time, double stop_time
   const Vec3 p_symmetry = (next_middle_time - stop_time) * vel_linear + k * (vel_linear - vel_cmd_linear);
   const Vec3 p_centrifugal = (0.5 * sqrt(current_body_pos[2] / 9.81)) * cross(vel_linear, vel_cmd_angular);
   Vec3 r = Vec3{current_body_pos[0], current_body_pos[1], current_body_pos[2]} + p_shoulder + p_symmetry + p_centrifugal;
-  r.z = HB_NEXT_POSITION_Z;
+  r.z = s.next_stance_z;
   return r;
 }
 
 // SwingTrajectoryPlanner::genSwingTrajs (:314-358): x/y three-node, z four-node Hermite splines with the reference's shape constants
-HBP_HD inline void gen_swing(SwingOut& sp, int foot, double t0, double t1, Vec3 a, Vec3 b) {
+HBP_HD inline void gen_swing(const PlanSettings& s, SwingOut& sp, int foot, double t0, double t1, Vec3 a, Vec3 b) {
   const double xy_a1 = 0.417, xy_l1 = 0.650, xy_k1 = 1.770;
   const double pa[3] = {a.x, a.y, a.z}, pb[3] = {b.x, b.y, b.z};
   for (int ax = 0; ax < 2; ++ax) {
@@ -231,8 +264,8 @@ HBP_HD inline void gen_swing(SwingOut& sp, int foot, double t0, double t1, Vec3 
     emit(sp, foot, ax, Seg{n0.t, n1.t, n0.p, n0.v, n1.p, n1.v});
     emit(sp, foot, ax, Seg{n1.t, n2.t, n1.p, n1.v, n2.p, n2.v});
   }
-  const double scaling = dmin(1.0, (t1 - t0) / HB_SWING_TIME_SCALE);
-  const double max_z = dmax(a.z, b.z) + scaling * HB_SWING_HEIGHT;
+  const double scaling = dmin(1.0, (t1 - t0) / s.swing_time_scale);
+  const double max_z = dmax(a.z, b.z) + scaling * s.swing_height;
   const double z_a1 = 0.251, z_l1 = 0.749, z_k1 = 1.338, z_a2 = 0.630, z_l2 = 0.570, z_k2 = 1.633, z_k3 = 0.0;
   const Node n0{t0, a.z, 0.0};
   const Node n1{(1 - z_a1) * t0 + z_a1 * t1, z_l1 * max_z, z_k1 * (z_l1 * (max_z - a.z)) / (z_a1 * (t1 - t0))};
@@ -247,13 +280,13 @@ HBP_HD inline void gen_swing(SwingOut& sp, int foot, double t0, double t1, Vec3 
 // Returns false where the reference would throw (swing phase without a defined take-off / touch-down, :421-458).
 // The feet are independent of each other: [j_begin, j_end) selects the ones this call plans (the host planner passes 0..4, the
 // cooperative device kernel one foot per thread).
-HBP_HD inline bool plan_swing(const ModeSchedule& ms, const Target& tg, double init_time, const double* current_feet /*12*/, const double* body_vel_cmd /*6*/,
+HBP_HD inline bool plan_swing(const PlanSettings& s, const ModeSchedule& ms, const Target& tg, double init_time, const double* current_feet /*12*/, const double* body_vel_cmd /*6*/,
                               double* latest_stance /*12*/, SwingOut& sp, int j_begin = 0, int j_end = 4) {
   const int np = ms.n_events + 1;
   const int mode_now = mode_at(ms, init_time + 0.001);
   for (int i = j_begin; i < j_end; ++i) {
     if (contact_flag(mode_now, i)) for (int a = 0; a < 3; ++a) latest_stance[3 * i + a] = current_feet[3 * i + a];
-    latest_stance[3 * i + 2] = HB_NEXT_POSITION_Z;
+    latest_stance[3 * i + 2] = s.next_stance_z;
   }
   for (int j = j_begin; j < j_end; ++j) {
     bool stock[MAX_PHASES + 1];
@@ -278,12 +311,12 @@ HBP_HD inline bool plan_swing(const ModeSchedule& ms, const Target& tg, double i
           target_state(tg, next_middle_time, xm);
           target_state(tg, init_time, xc);
           const Vec3 body_vel{tg.x[0][0], tg.x[0][1], tg.x[0][2]};
-          next = next_foot_pos(j, init_time, t_final, next_middle_time, xm + 6, xc + 6, body_vel, body_vel_cmd);
+          next = next_foot_pos(s, j, init_time, t_final, next_middle_time, xm + 6, xc + 6, body_vel, body_vel_cmd);
           last_final_idx = fi;
         }
         // every phase of a swing interval pushes the same spline set (one MultiCubicSpline per phase index in the reference);
         // only emit it once per swing interval
-        if (p == 0 || stock[p - 1]) gen_swing(sp, j, t_start, t_final, last, next);
+        if (p == 0 || stock[p - 1]) gen_swing(s, sp, j, t_start, t_final, last, next);
       } else {
         if (p == 0 || !stock[p - 1]) {
           const double t_start = ms.events[si], t_final = (fi >= 0 && fi < ms.n_events) ? ms.events[fi] : ms.events[ms.n_events - 1];
@@ -623,23 +656,25 @@ HBP_HD inline int write_schedule_and_targets(const ModeSchedule& ms, const Targe
 }
 
 // One instance, start to finish: schedule, target (the given one, or the cmd_vel target when target is null), swing planner, IK joint
-// references, compact output.
+// references, compact output; with the planner settings `settings` (null: the compiled-in ones).
 // Returns 0, -1 (invalid input) or -5 (schedule / reference capacity exceeded, or a swing phase without take-off / touch-down time).
-HBP_HD inline int plan_one(const PlanConsts& pc, const hb_plan_input& p, const hb_target* target, double* latest_stance /*12, in/out*/, hb_reference* out,
-                           bool zero_fill) {
+HBP_HD inline int plan_one(const PlanConsts& pc, const hb_plan_input& p, const hb_target* target, const hb_planner_settings* settings,
+                           double* latest_stance /*12, in/out*/, hb_reference* out, bool zero_fill) {
   if (!(p.horizon > 0.0) || !(p.prev_event < p.gait_start) || p.gait < 0 || p.gait > 3) return -1;
   const double tf = p.t0 + p.horizon;
   if (zero_fill) memset(out, 0, sizeof(*out));
+  PlanSettings ps;
+  plan_settings(settings, p.gait, ps);
   ModeSchedule ms;
   // the reference tiles over [t0 - T, tf + T] (SwitchedModelReferenceManager.cpp:147)
-  if (!tile_gait(p.gait, p.prev_event, p.gait_start, p.t0 - p.horizon, tf + p.horizon, ms)) return -5;
+  if (!tile_gait(ps.tmpl, p.prev_event, p.gait_start, p.t0 - p.horizon, tf + p.horizon, ms)) return -5;
   Target tg;
   if (target) target_from(*target, tg);
   else tg = cmd_vel_to_target(pc, p.cmd_vel, p.t0, p.x0, p.time_to_target);
   const double body_vel_cmd[6] = {p.cmd_vel[0], p.cmd_vel[1], p.cmd_vel[2], p.cmd_vel[3], 0.0, 0.0};
   SwingOut so{out, p.t0 - 1e-9, tf + 1e-9, false};
   for (int c = 0; c < 4; ++c) for (int a = 0; a < 3; ++a) out->n_segments[c][a] = 0;
-  if (!plan_swing(ms, tg, p.t0, p.feet_pos, body_vel_cmd, latest_stance, so) || so.overflow) return -5;
+  if (!plan_swing(ps, ms, tg, p.t0, p.feet_pos, body_vel_cmd, latest_stance, so) || so.overflow) return -5;
   if (p.joint_ik && !joint_references(pc, out, p.t0, tf, p.x0, tg)) return -5;
   return write_schedule_and_targets(ms, tg, so.t_lo, so.t_hi, out);
 }

@@ -248,11 +248,15 @@ __global__ void plan_prepare_kernel(int B, const hb_plan_input* in, double* t0, 
 // then threads 0 and 1 run the IK of the left / right leg on the resampled target, then thread 0 writes the schedule and the targets.
 // Same functions as the host planner, so the plan is the same. The targets (2.9 KB each) live in shared memory only: no thread keeps
 // a copy on its stack. An instance with a record in targets plans on it instead of its cmd_vel target, where captured (nullable: every
-// such instance) has captured[inst] >= 0 (a goal an episode captured).
+// such instance) has captured[inst] >= 0 (a goal an episode captured). Thread 0 of an instance stages what its plan reads of its record in
+// settings (hbplan::PlanSettings: its gait's template and the swing settings; the compiled-in values without a record) in shared memory,
+// where the four threads read it.
 __global__ void __launch_bounds__(32) plan_references_coop_kernel(int B, const hb_plan_input* in, const double* feet, double* latest_stance,
                                                                   hb_reference* out, int32_t* status, hbplan::PlanConsts pc,
-                                                                  InstanceView<hb_target> targets, const int32_t* captured) {
+                                                                  InstanceView<hb_target> targets, const int32_t* captured,
+                                                                  InstanceView<hb_planner_settings> settings) {
   __shared__ hbplan::Target s_tg[8], s_old[8];
+  __shared__ hbplan::PlanSettings s_set[8];
   __shared__ int s_rc[8];
   const int g = threadIdx.x >> 2, r = threadIdx.x & 3;
   const int inst = blockIdx.x * 8 + g;
@@ -269,7 +273,11 @@ __global__ void __launch_bounds__(32) plan_references_coop_kernel(int B, const h
     if (feet) for (int i = 0; i < 12; ++i) p.feet_pos[i] = feet[(size_t)inst * 12 + i];
     if (!(p.horizon > 0.0) || !(p.prev_event < p.gait_start) || p.gait < 0 || p.gait > 3) rc = -1;
     tf = p.t0 + p.horizon; t_lo = p.t0 - 1e-9; t_hi = tf + 1e-9;
-    if (rc == 0 && !hbplan::tile_gait(p.gait, p.prev_event, p.gait_start, p.t0 - p.horizon, tf + p.horizon, ms)) rc = -5;
+    if (rc == 0 && r == 0) hbplan::plan_settings(settings.of(inst), p.gait, s_set[g]);
+  }
+  __syncwarp();
+  if (active && rc == 0) {
+    if (!hbplan::tile_gait(s_set[g].tmpl, p.prev_event, p.gait_start, p.t0 - p.horizon, tf + p.horizon, ms)) rc = -5;
     if (rc == 0 && r == 0) {
       const hb_target* tg = targets.of(inst);
       if (tg && (!captured || captured[inst] >= 0)) hbplan::target_from(*tg, s_tg[g]);
@@ -282,7 +290,7 @@ __global__ void __launch_bounds__(32) plan_references_coop_kernel(int B, const h
     const double body_vel_cmd[6] = {p.cmd_vel[0], p.cmd_vel[1], p.cmd_vel[2], p.cmd_vel[3], 0.0, 0.0};
     hbplan::SwingOut so{o, t_lo, t_hi, false};
     for (int a = 0; a < 3; ++a) o->n_segments[r][a] = 0;
-    if (!hbplan::plan_swing(ms, s_tg[g], p.t0, p.feet_pos, body_vel_cmd, latest_stance + (size_t)inst * 12, so, r, r + 1) || so.overflow) rc = -5;
+    if (!hbplan::plan_swing(s_set[g], ms, s_tg[g], p.t0, p.feet_pos, body_vel_cmd, latest_stance + (size_t)inst * 12, so, r, r + 1) || so.overflow) rc = -5;
   }
   __syncwarp();                // every foot has read the two-sample target before thread 0 resamples it in place
   if (active) {

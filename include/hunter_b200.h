@@ -94,7 +94,7 @@ typedef struct {
   double x0[22];          /* current observation state                                                    */
   double cmd_vel[4];      /* filtered command: vx, vy, vz, yaw rate (body frame)                          */
   double feet_pos[12];    /* current contact positions in world (hb_contact_positions_batch)              */
-  int32_t gait;           /* 0 stance, 1 trot, 2 standing_trot, 3 flying_trot (reference.info:54-118)     */
+  int32_t gait;           /* 0 stance, 1 trot, 2 standing_trot, 3 flying_trot (gait.info; hb_planner_settings) */
   int32_t joint_ik;       /* 1: resample the target every 0.15 s and fill joint references by IK (calculateJointRef,
                              SwitchedModelReferenceManager.cpp:251-300); 0: keep the two-sample target with default joints */
 } hb_plan_input;
@@ -107,6 +107,41 @@ typedef struct {
   double time[HB_MAX_TARGETS];            /* absolute times, strictly ascending                                    */
   double state[HB_MAX_TARGETS][22];       /* state samples (layout of x)                                           */
 } hb_target;
+
+/* ---- planner settings: how each gait steps and swings, the reference's run-time planner configuration ----
+ * gait[g] is the ModeSequenceTemplate of gait g (hb_plan_input.gait, hb_rollout_command.gait), the templates of gait.info in its `list`
+ * order (legged_controllers/config/hunter/gait.info; loadModeSequenceTemplate, ModeSequenceTemplate.cpp:59-83); the swing fields are
+ * swing_trajectory_config (task.info:21-34; loadSwingTrajectorySettings, SwingTrajectoryPlanner.cpp:549-561). The template is tiled as
+ * the compiled-in one is: mode modes[k] holds for switching_times[k + 1] - switching_times[k], the period is switching_times[n_phase].
+ * Swing apex: max(lift-off z, touch-down z) + min(1, swing duration / swing_time_scale) * swing_height; every planned foothold and every
+ * stance foot stands at next_stance_z; the nominal foothold offset of foot c from the base is (x, +-feet_bias_y, feet_bias_z), with
+ * x = feet_bias_x1 for the toes (contacts 0, 1) and feet_bias_x2 for the heels (2, 3), +y for the left contacts (0, 2).
+ * Validity (the setters and hb_plan_references_settings return -1 otherwise): for each gait n_phase in 1..HB_GAIT_MAX_PHASES, modes[k] in
+ * 0..3 and switching_times[0..n_phase] finite, starting at 0 and strictly ascending (the entries beyond n_phase are not read);
+ * swing_height finite and >= 0, swing_time_scale finite and > 0, the other swing fields finite.
+ * A valid template may still be too short for the planner's capacities: more than 128 phases tiled over [t0 - T, t0 + 2T] (T the
+ * horizon), more than HB_MAX_EVENTS events inside the horizon or more than HB_MAX_SEGMENTS swing segments per foot and axis. Such a
+ * plan fails with status -5, like any plan over the capacities, and the episodes count it in plan_rejects. */
+#define HB_GAIT_MAX_PHASES 8
+typedef struct {                     /* ModeSequenceTemplate (gait.info)                                                          */
+  int32_t n_phase;                   /* 1..HB_GAIT_MAX_PHASES                                                                     */
+  int32_t modes[HB_GAIT_MAX_PHASES]; /* 0 FLY, 1 R, 2 L, 3 STANCE (MotionPhaseDefinition.h:57-60)                                 */
+  double switching_times[HB_GAIT_MAX_PHASES + 1];   /* [0] == 0, strictly ascending; the period is [n_phase]                      */
+} hb_gait_template;                  /* 112 B */
+typedef struct {
+  hb_gait_template gait[4];          /* indexed by hb_plan_input.gait / hb_rollout_command.gait                                   */
+  double swing_height, swing_time_scale, next_stance_z;           /* swing_trajectory_config                                       */
+  double feet_bias_x1, feet_bias_x2, feet_bias_y, feet_bias_z;
+} hb_planner_settings;               /* 504 B */
+/* The shipped settings (host only): gait.info's four templates and task.info's swing block, the values compiled into the planner. */
+int hb_default_planner_settings(hb_planner_settings* s);
+/* hb_planner_settings from a task.info and a gait.info file (host only), with the INFO reader of hb_parse_task_info: swing_trajectory_config's
+ * swingHeight, swingTimeScale, feet_bias_x1/x2/y/z and next_position_z (the key the reference loads; the shipped task.info names it
+ * next_stance_position_z, so the loader's default 0.02 applies, SwingTrajectoryPlanner.cpp:560), and for g = 0..3 the template named by
+ * `list.[g]` of gait_info (modeSequence names FLY, R, L, STANCE; switchingTimes). As in hb_parse_task_info, a key or template that is absent
+ * keeps its default (hb_default_planner_settings). -1: a NULL argument, a file missing or malformed, an unknown mode name, a template whose
+ * mode and time counts do not match (n modes, n + 1 times) or that has more than HB_GAIT_MAX_PHASES phases, or a result that is not valid. */
+int hb_parse_planner_settings(const char* task_info, const char* gait_info, hb_planner_settings* out);
 
 /* state of the speed-based gait selection of one instance (SwitchedModelReferenceManager velAbsHistory_/velAvg_/gaitLevel_);
  * zero-initialise, then set gait_level = -1 ("no template chosen yet") or the level in force */
@@ -571,6 +606,14 @@ int hb_plan_references_batch_dev(hb_ctx* ctx, int B, const hb_plan_input* in, co
  * call keeps the previous setting. -1 also for n outside 1..HB_MAX_TARGETS, times that are not strictly ascending, a non-finite
  * time[k] or state[k][.] with k < n. */
 int hb_plan_set_targets(hb_ctx* ctx, int B, const hb_target* targets);
+/* Planner settings of the context (hb_planner_settings, above): instance i < B of every device planner path -- hb_plan_references_batch_dev,
+ * hb_plan_references_gpu, hb_resident_plan_cycle_batch, hb_rollout_batch_dev and hb_rollout_estimated_batch_dev -- plans with settings[i]
+ * in place of the compiled-in templates and swing settings; instances at or beyond B, and every instance while none is set, plan with the
+ * compiled-in values bit for bit (hb_default_planner_settings gives the same plans). One setting serves every path, so an episode can be
+ * written as a loop of those calls. Setting conventions of the per-robot episode settings (below): host array validated and copied in
+ * stream order, B == 0 clears (settings may be NULL), -1 also for a record that is not valid, -4 for B > max_batch, a rejected call keeps
+ * the previous setting. The setting adds no launch to any call. */
+int hb_plan_set_settings(hb_ctx* ctx, int B, const hb_planner_settings* settings);
 /* One estimator update per instance (StateEstimateBase::updateJointStates / updateImu, StateEstimateBase.cpp:73-106, then
  * KalmanFilterEstimate::update): quat = (x, y, z, w); contact_flag: B x 4 (0 = the filter distrusts that foot, x100 noise);
  * rbd_out: B x 32 measured rbd state [zyx, p, q_j, omega_world, v, qd_j]. zyxOffset_ is taken as zero. The odometry fusion
@@ -770,6 +813,11 @@ int hb_plan_references(int B, const hb_plan_input* in, double* latest_stance, hb
  * everything else unchanged (the swing planner still reads cmd_vel as its body velocity command; with joint_ik the target is resampled and
  * its joints filled by IK). NULL is hb_plan_references. -1 also for a record that hb_plan_set_targets rejects. */
 int hb_plan_references_targets(int B, const hb_plan_input* in, const hb_target* targets, double* latest_stance, hb_reference* out);
+/* hb_plan_references_targets with planner settings per instance: settings (B, nullable) replaces the compiled-in templates and swing
+ * settings for every instance (hb_planner_settings). NULL settings, and hb_default_planner_settings records, give
+ * hb_plan_references_targets bit for bit. -1 also for a record that is not valid. */
+int hb_plan_references_settings(int B, const hb_plan_input* in, const hb_target* targets /*nullable*/, const hb_planner_settings* settings /*nullable*/,
+                                double* latest_stance, hb_reference* out);
 /* goalToTargetTrajectories (TargetTrajectoriesPublisher.cpp:83-100, with estimateTimeToTarget :29-38 and
  * targetPoseToTargetTrajectories :41-62) for the observation (t[i], x[i]) and goal[i] = (x, y, yaw), host only. With p = x[6:12] and
  * z' = p[2] + clamp(HB_COM_HEIGHT - p[2], -0.04, 0.04): sample 0 = (t, [0 (6), p[0], p[1], z', p[3], 0, 0, default joints]), sample 1 =

@@ -19,8 +19,9 @@ GROUND, MIN_HEIGHT = 0.02, 0.3
 # sensor noise at --sensor-noise 1 (standard deviations): orientation [rad], gyro [rad/s], accelerometer [m/s^2], encoders [rad], [rad/s]
 NOISE_SIGMAS = dict(orientation=0.005, angular_velocity=0.02, linear_acceleration=0.1, joint_position=0.001, joint_velocity=0.02)
 
-# one episode: device time [ms], launches, final hb_rollout_stats, final rbd (B x 32), and hb_estimation_stats when asked for
-Run = namedtuple("Run", "ms launches stats rbd est_stats")
+# one episode: device time [ms], launches, final hb_rollout_stats, final rbd (B x 32), hb_estimation_stats when asked for, and the log of
+# the true states (B x rows x 32) when asked for
+Run = namedtuple("Run", "ms launches stats rbd est_stats log", defaults=(None,))
 
 
 def gpu_identity(index):
@@ -95,10 +96,11 @@ class Episodes:
         self.stream = torch.cuda.ExternalStream(self.ctx.stream_handle, device=self.dev)
         self.lib = hb.load_library()
 
-    def episode(self, estimated=None, est_stats=False, rows=None):
+    def episode(self, estimated=None, est_stats=False, rows=None, log_every=0):
         """One episode of self.ticks ticks from the start poses in one hb_rollout_batch_dev call, or hb_rollout_estimated_batch_dev when
         estimated (default: --estimator), with device events around the call. est_stats: also collect the estimation stats. rows: the
-        robots of a smaller batch (default: all), each with its start pose, command and noise stream, as instances 0 .. len(rows) - 1."""
+        robots of a smaller batch (default: all), each with its start pose, command and noise stream, as instances 0 .. len(rows) - 1.
+        log_every: also log the true state every log_every ticks (0: no log)."""
         torch, hb, dev, ctx = self.torch, self.hb, self.dev, self.ctx
         rows = np.arange(self.B) if rows is None else np.asarray(rows)
         B = len(rows)
@@ -109,7 +111,10 @@ class Episodes:
         d_act = torch.zeros(B * C.sizeof(hb.HbActuationState), dtype=torch.uint8, device=dev)
         d_estop = torch.zeros(B, dtype=torch.uint8, device=dev)
         d_st = torch.from_numpy(hb.rollout_stats(B).view(np.uint8).copy()).to(dev)
-        d_es = None
+        d_es = d_log = None
+        if log_every:
+            d_log = torch.zeros(B * ((self.ticks + log_every - 1) // log_every) * 32, dtype=torch.float64, device=dev)
+        self.prm.log_every = log_every
         if estimated:
             est = hb.estimation_states(B)
             for k, i in enumerate(rows):
@@ -123,15 +128,17 @@ class Episodes:
         e0.record(self.stream)
         if estimated:
             rc = self.lib.hb_rollout_estimated_batch_dev(ctx._h, B, C.c_int64(0), self.ticks, C.byref(self.prm), C.byref(self.ep), cmds, P(d_rbd),
-                                                         P(d_act), P(d_estop), P(d_st), P(d_est), None if d_es is None else P(d_es), None, None)
+                                                         P(d_act), P(d_estop), P(d_st), P(d_est), None if d_es is None else P(d_es),
+                                                         None if d_log is None else P(d_log), None)
         else:
             rc = self.lib.hb_rollout_batch_dev(ctx._h, B, C.c_int64(0), self.ticks, C.byref(self.prm), cmds, P(d_rbd), P(d_act), P(d_estop), P(d_st),
-                                               None)
+                                               None if d_log is None else P(d_log))
         e1.record(self.stream)
         assert rc == 0, rc
         ctx.sync()
         return Run(e0.elapsed_time(e1), ctx.launch_count - l0, d_st.cpu().numpy().view(hb.ROLLOUT_STATS_DTYPE), d_rbd.cpu().numpy(),
-                   None if d_es is None else d_es.cpu().numpy().view(hb.ESTIMATION_STATS_DTYPE))
+                   None if d_es is None else d_es.cpu().numpy().view(hb.ESTIMATION_STATS_DTYPE),
+                   None if d_log is None else d_log.cpu().numpy().reshape(B, -1, 32))
 
     def alternate(self, set_, settings, timed):
         """Times a setting against its null setting and no setting: `timed` rounds (at least one), each setting the three of `settings`
