@@ -9,6 +9,7 @@ from .api import (HbWbcSettings, HbTaskInfo, parse_task_info, Context, WeightedW
                   HB_MAX_PUSHES, HbPushSchedule, make_push_schedules, HbPlantVariation, default_plant_variation, make_plant_variations, HB_TERRAIN_MAX, HbTerrain, make_terrains, HbSensorNoise, HbEstimationParams, HbEstimationState, HbEstimationStats, ESTIMATION_STATS_DTYPE, default_estimation_params, estimation_states, estimation_stats,
                   HbTarget, make_targets, reference_target, goal_to_target, HB_MAX_GOALS, HbGoalSchedule, make_goal_schedules,
                   HB_ODOM_MAX_DELAY, HbOdometrySetting, make_odometry_settings, HbControllerSetting, make_controller_settings,
+                  HbHardwareSetting, default_hardware_setting, make_hardware_settings,
                   HB_GAIT_MAX_PHASES, HbGaitTemplate, HbPlannerSettings, gait_template, default_planner_settings, parse_planner_settings, make_planner_settings)
 
 __all__ = ["HbWbcSettings", "HbTaskInfo", "parse_task_info", "Context", "WeightedWbc", "HierarchicalWbc", "HbHoqpProblem", "make_hoqp_problems", "hoqp_tasks", "SqpMpc", "HbReference", "HbSolveInfo", "HbConfig", "HunterB200Error", "load_library",
@@ -17,4 +18,5 @@ __all__ = ["HbWbcSettings", "HbTaskInfo", "parse_task_info", "Context", "Weighte
            "HB_MAX_PUSHES", "HbPushSchedule", "make_push_schedules", "HbPlantVariation", "default_plant_variation", "make_plant_variations", "HB_TERRAIN_MAX", "HbTerrain", "make_terrains", "HbSensorNoise", "HbEstimationParams", "HbEstimationState", "HbEstimationStats", "ESTIMATION_STATS_DTYPE", "default_estimation_params", "estimation_states", "estimation_stats",
            "HbTarget", "make_targets", "reference_target", "goal_to_target", "HB_MAX_GOALS", "HbGoalSchedule", "make_goal_schedules",
            "HB_ODOM_MAX_DELAY", "HbOdometrySetting", "make_odometry_settings", "HbControllerSetting", "make_controller_settings",
+           "HbHardwareSetting", "default_hardware_setting", "make_hardware_settings",
            "HB_GAIT_MAX_PHASES", "HbGaitTemplate", "HbPlannerSettings", "gait_template", "default_planner_settings", "parse_planner_settings", "make_planner_settings"]

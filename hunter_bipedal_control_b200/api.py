@@ -45,6 +45,7 @@ EXPORTED_SYMBOLS = [
     "hb_rollout_set_mpc_latencies", "hb_policy_update", "hb_policy_wbc", "hb_policy_wbc_async",
     "hb_rollout_set_odometry", "hb_sim_read_odometry", "hb_sim_read_odometry_async", "hb_estimator_fuse_odometry", "hb_estimator_fuse_odometry_async",
     "hb_rollout_set_controller_settings",
+    "hb_default_hardware_setting", "hb_rollout_set_hardware", "hb_actuation_hw", "hb_sim_read_sensors_hw",
     "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
 ]
 
@@ -595,6 +596,40 @@ def make_controller_settings(B, wbc=None, gains=None, **fields):
     return out
 
 
+class HbHardwareSetting(C.Structure):
+    _fields_ = [("actuation_delay", C.c_double), ("torque_limit", C.c_double * NJ)] + \
+        [(k, C.c_double) for k in ("sigma_orientation", "sigma_angular_velocity", "sigma_linear_acceleration", "sigma_joint_position",
+                                   "sigma_joint_velocity")] + \
+        [(k, C.c_double * 3) for k in ("orientation_offset", "gyro_bias", "accel_bias")] + [("encoder_offset", C.c_double * NJ)]
+
+
+def default_hardware_setting():
+    """hb_default_hardware_setting: the default episode's actuation delay and torque limits, no sensor noise, no offsets."""
+    s = HbHardwareSetting()
+    _check(load_library().hb_default_hardware_setting(C.byref(s)), "hb_default_hardware_setting")
+    return s
+
+
+def make_hardware_settings(B, base=None, **fields):
+    """ctypes array of B HbHardwareSetting (Context.set_hardware): each robot's simulated hardware in the episodes. base (HbHardwareSetting,
+    default default_hardware_setting()) is the base of every record. Any field can be given by name, as a scalar or a (B,) array;
+    torque_limit and encoder_offset as (10,) or (B, 10), orientation_offset, gyro_bias and accel_bias as (3,) or (B, 3). Raises ValueError
+    for an unknown name or a shape that does not broadcast; the ranges are checked by the setter."""
+    base = default_hardware_setting() if base is None else base
+    out = (HbHardwareSetting * B)()
+    v = np.ctypeslib.as_array(out)
+    v[:] = np.frombuffer(bytes(base), dtype=v.dtype)[0]
+    for name, value in fields.items():
+        if name not in v.dtype.names:
+            raise ValueError("hardware settings: unknown field %r" % name)
+        shape = (B,) + v.dtype[name].shape
+        try:
+            v[name] = np.broadcast_to(_f64(value), shape)
+        except ValueError as e:
+            raise ValueError("hardware settings: %s: %s expected: %s" % (name, "(%d,) or (B, %d)" % (shape[1], shape[1]) if shape[1:] else "(B,) or a scalar", e))
+    return out
+
+
 HB_ODOM_MAX_DELAY = 15
 
 
@@ -749,6 +784,11 @@ def _ptr(a):
 
 def _f64(a):
     return np.ascontiguousarray(a, dtype=np.float64)
+
+
+def _check_hardware(what, hardware, B):
+    if hardware is not None and len(hardware) != B:
+        raise ValueError("%s: %d hardware settings for %d robots" % (what, len(hardware), B))
 
 
 class Context:
@@ -985,23 +1025,29 @@ class Context:
                                                    _ptr(joint_pos), _ptr(joint_vel), _ptr(flags), _ptr(rbd)), "hb_estimator_update_batch", self._h)
         return rbd
 
-    def read_sensors(self, rbd, est, tick, noise=None, accel_dt=0.002):
-        """Sensors of the simulated robot at absolute tick `tick` from the true rbd [B,32] (hb_sim_read_sensors); `est` (ctypes array of
+    def read_sensors(self, rbd, est, tick, noise=None, accel_dt=0.002, hardware=None):
+        """Sensors of the simulated robot at absolute tick `tick` from the true rbd [B,32] (hb_sim_read_sensors_hw); `est` (ctypes array of
         HbEstimationState) gives the noise streams and the accelerometer's previous velocity and is updated in place. noise: HbSensorNoise
-        (None: exact). Returns (quat [B,4], ang_vel_local [B,3], lin_acc_local [B,3], joint_pos [B,10], joint_vel [B,10])."""
+        (None: exact). hardware: B HbHardwareSetting (make_hardware_settings), each robot's sensor offsets and sigmas in place of noise's
+        sigmas; None reads as hb_sim_read_sensors. Returns (quat [B,4], ang_vel_local [B,3], lin_acc_local [B,3], joint_pos [B,10],
+        joint_vel [B,10])."""
         rbd = _f64(rbd); B = rbd.shape[0]
         noise = noise or HbSensorNoise()
+        _check_hardware("read_sensors", hardware, B)
         quat = np.zeros((B, 4)); w = np.zeros((B, 3)); a = np.zeros((B, 3)); jp = np.zeros((B, NJ)); jv = np.zeros((B, NJ))
-        _check(self._lib.hb_sim_read_sensors(self._h, B, C.byref(noise), C.c_int64(tick), C.c_double(accel_dt), _ptr(rbd), est, _ptr(quat), _ptr(w), _ptr(a),
-                                             _ptr(jp), _ptr(jv)), "hb_sim_read_sensors", self._h)
+        _check(self._lib.hb_sim_read_sensors_hw(self._h, B, C.byref(noise), hardware, C.c_int64(tick), C.c_double(accel_dt), _ptr(rbd), est, _ptr(quat),
+                                                _ptr(w), _ptr(a), _ptr(jp), _ptr(jv)), "hb_sim_read_sensors_hw", self._h)
         return quat, w, a, jp, jv
 
-    def actuation(self, time, state, command, rbd, delay=0.009):
-        """LeggedHWSim::writeSim: delayed hybrid joint command -> applied joint torques [B,10]; `state` (ctypes array of HbActuationState) in place."""
+    def actuation(self, time, state, command, rbd, delay=0.009, hardware=None):
+        """LeggedHWSim::writeSim: delayed hybrid joint command -> applied joint torques [B,10]; `state` (ctypes array of HbActuationState) in place.
+        hardware: B HbHardwareSetting (make_hardware_settings), each robot's actuation_delay in place of delay (hb_actuation_hw)."""
         command, rbd = _f64(command), _f64(rbd); B = rbd.shape[0]
         time = _f64(np.broadcast_to(_f64(time), (B,)))
+        _check_hardware("actuation", hardware, B)
         tau = np.zeros((B, NJ))
-        _check(self._lib.hb_actuation_batch(self._h, B, C.c_double(delay), _ptr(time), state, _ptr(command), _ptr(rbd), _ptr(tau)), "hb_actuation_batch", self._h)
+        _check(self._lib.hb_actuation_hw(self._h, B, C.c_double(delay), hardware, _ptr(time), state, _ptr(command), _ptr(rbd), _ptr(tau)), "hb_actuation_hw",
+               self._h)
         return tau
 
     def sim_step(self, rbd, tau, params=None, wrench=None, variation=None, terrain=None):
@@ -1080,6 +1126,13 @@ class Context:
         WBC settings and joint PD gains of instance i of every later rollout / rollout_estimated call, in place of the context's WBC settings
         and params.gains; instances beyond len(settings) run those; None clears them. No other call reads them."""
         self._set_instances("hb_rollout_set_controller_settings", settings)
+
+    def set_hardware(self, settings):
+        """Simulated hardware of this context's episodes (hb_rollout_set_hardware): settings[i] (make_hardware_settings) is the actuation
+        delay and torque limits of instance i of every later rollout / rollout_estimated call, and in rollout_estimated its sensor sigmas
+        and offsets, in place of params' and est_params.noise's values; instances beyond len(settings) run those; None clears them. The
+        controllers are not told about it, and no other call reads it."""
+        self._set_instances("hb_rollout_set_hardware", settings)
 
     def read_odometry(self, rbd, est, tick, noise=None):
         """The tracking cameras at absolute tick `tick` from the true rbd [B,32] (hb_sim_read_odometry), on this context's odometry setting

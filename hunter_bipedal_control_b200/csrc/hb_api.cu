@@ -105,6 +105,8 @@ struct hb_ctx {
   OdomCamera* odom_cam;
   // each instance's WBC settings and joint PD gains in the episodes (hb_rollout_set_controller_settings)
   InstanceSetting<hb_controller_setting> controllers;
+  // each instance's simulated hardware in the episodes: actuation delay, torque limits, sensor noise and offsets (hb_rollout_set_hardware)
+  InstanceSetting<hb_hardware_setting> hardware;
   // each instance's gait templates and swing settings in every device planner path (hb_plan_set_settings)
   InstanceSetting<hb_planner_settings> plan_settings;
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
@@ -484,7 +486,7 @@ int hb_destroy(hb_ctx* ctx) {
   cudaSetDevice(ctx->device);
   void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->arena,
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
-                       ctx->odometry.dev, ctx->controllers.dev, ctx->plan_settings.dev};
+                       ctx->odometry.dev, ctx->controllers.dev, ctx->hardware.dev, ctx->plan_settings.dev};
   for (void* p : mem) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -1046,10 +1048,43 @@ int hb_actuation_reset(int B, hb_actuation_state* state) {
   return HB_OK;
 }
 
+// The instances' simulated hardware as the actuation, saturation and sensor kernels read it; the calls without records pass an empty view
+using HardwareView = InstanceView<hb_hardware_setting>;
+
+// The ranges of hunter_b200.h's hb_hardware_setting: every field finite, delay >= 0, limits > 0, sigmas >= 0
+static bool hardware_setting_ok(const hb_hardware_setting& s) {
+  const double* f = reinterpret_cast<const double*>(&s);
+  static_assert(sizeof(hb_hardware_setting) == 35 * sizeof(double), "hb_hardware_setting holds 35 doubles");
+  for (int i = 0; i < 35; ++i) if (!isfinite(f[i])) return false;
+  if (!delay_ok(s.actuation_delay)) return false;
+  for (double lim : s.torque_limit) if (!(lim > 0.0)) return false;
+  for (double sigma : {s.sigma_orientation, s.sigma_angular_velocity, s.sigma_linear_acceleration, s.sigma_joint_position, s.sigma_joint_velocity})
+    if (!(sigma >= 0.0)) return false;
+  return true;
+}
+
+int hb_default_hardware_setting(hb_hardware_setting* s) {
+  if (!s) return HB_EINVAL;
+  memset(s, 0, sizeof(*s));
+  hb_rollout_params p;            // the delay and limits of the default episode
+  hb_default_rollout_params(&p);
+  s->actuation_delay = p.actuation_delay;
+  for (int j = 0; j < NJ; ++j) s->torque_limit[j] = p.torque_limit[j];
+  return HB_OK;
+}
+
+int hb_rollout_set_hardware(hb_ctx* ctx, int B, const hb_hardware_setting* s) { return set_instances(ctx, B, s, hardware_setting_ok, &hb_ctx::hardware); }
+
+// hb_actuation_batch_dev, with each instance of `hw` on its own delay (the episodes, hb_actuation_hw)
+static int actuation_dev(hb_ctx* ctx, int B, double delay, HardwareView hw, const double* time, hb_actuation_state* state, const double* command,
+                         const double* rbd, double* tau) {
+  ENTER(ctx, B, time && state && command && rbd && tau && delay_ok(delay), UNCAPPED);
+  return launch(ctx, K_UNPROFILED, actuation_kernel, (B + 63) / 64, 64, 0, B, delay, hw, time, state, command, rbd, tau);
+}
+
 int hb_actuation_batch_dev(hb_ctx* ctx, int B, double delay, const double* time, hb_actuation_state* state, const double* command, const double* rbd,
                            double* tau) {
-  ENTER(ctx, B, time && state && command && rbd && tau && delay_ok(delay), UNCAPPED);
-  return launch(ctx, K_UNPROFILED, actuation_kernel, (B + 63) / 64, 64, 0, B, delay, time, state, command, rbd, tau);
+  return actuation_dev(ctx, B, delay, HardwareView{}, time, state, command, rbd, tau);
 }
 
 // the plant step after the entry checks; wrench (B x 6) nullable; var: the plants of the instances, ter: the ground under them
@@ -1378,6 +1413,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   const bool odom = e && ctx->odometry.n > 0;
   const OdomRead odom_read = odom ? odometry_read(ctx, ctx->re_opos, ctx->re_ohas) : OdomRead{};
   const ControllerView controllers = ctx->controllers.view();   // each instance's WBC settings and PD gains, none without a setting
+  const HardwareView hardware = ctx->hardware.view();           // each instance's actuators and sensors, none without a setting
   for (int k = 0; k < n_ticks && !rc; ++k) {
     const int64_t a = tick0 + k;
     const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
@@ -1388,8 +1424,8 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
     if (!rc && e) {
       // LeggedController::updateStateEstimation: sensors and contact flags at the previous observation's time, filter, observation step
       double* est_row = (n_est_log && k % p->log_every == 0) ? e->log + (size_t)(k / p->log_every) * 32 : nullptr;
-      rc = launch(ctx, K_UNPROFILED, sensor_read_kernel, grid, 64, 0, B, e->ep->noise, (uint32_t)a, p->sim.dt, (double)(a - 1) * p->period, rbd, e->est,
-                  ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag, odom_read);
+      rc = launch(ctx, K_UNPROFILED, sensor_read_kernel, grid, 64, 0, B, e->ep->noise, hardware, (uint32_t)a, p->sim.dt, (double)(a - 1) * p->period, rbd,
+                  e->est, ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag, odom_read);
       if (!rc) rc = launch(ctx, K_UNPROFILED, odom ? kf_update_kernel<hb_estimation_state, true> : kf_update_kernel<hb_estimation_state, false>, B, 32,
                            sizeof(KfShared), B, e->ep->kf, p->period, e->est, ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag,
                            meas, (const double*)ctx->re_opos, (const uint8_t*)ctx->re_ohas);
@@ -1417,8 +1453,8 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
                                     false, choice, controllers);
     if (!rc) rc = joint_command_dev(ctx, B, &p->gains, p->period, ctx->xdes, ctx->udes, ctx->ro_sol, ctx->wmode, meas, nullptr, estop, ctx->ro_jcmd,
                                     ctx->ro_jtau, controllers);
-    if (!rc) rc = hb_actuation_batch_dev(ctx, B, p->actuation_delay, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau);
-    if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, ctx->ro_tau);
+    if (!rc) rc = actuation_dev(ctx, B, p->actuation_delay, hardware, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau);
+    if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, hardware, ctx->ro_tau);
     if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, ctx->variations.view(), ctx->terrains.view(), nullptr, nullptr);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_tick_end_kernel, grid, 64, 0, B, (int)a, mpc ? 1 : 0, ctx->ro_info, ctx->ro_pstat, ctx->wstatus, estop, ctx->ro_tau, ctx->ro_held, rbd, stats);
   }
@@ -1453,13 +1489,19 @@ int hb_estimation_reset(int B, uint64_t first_stream, hb_estimation_state* state
   return HB_OK;
 }
 
+// hb_sim_read_sensors_batch_dev, with each instance of `hw` on its own sensors (hb_sim_read_sensors_hw)
+static int read_sensors_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noise, HardwareView hw, int64_t tick, double accel_dt, const double* rbd,
+                            hb_estimation_state* est, double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos, double* joint_vel) {
+  ENTER(ctx, B, noise && rbd && est && quat && ang_vel_local && lin_acc_local && joint_pos && joint_vel && sensor_noise_ok(*noise) && accel_dt > 0.0 &&
+        tick >= 0 && tick <= UINT32_MAX, CAPPED);
+  return launch(ctx, K_UNPROFILED, sensor_read_kernel, (B + 63) / 64, 64, 0, B, *noise, hw, (uint32_t)tick, accel_dt, 0.0, rbd, est, quat, ang_vel_local,
+                lin_acc_local, joint_pos, joint_vel, (uint8_t*)nullptr, OdomRead{});
+}
+
 int hb_sim_read_sensors_batch_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, double accel_dt, const double* rbd,
                                   hb_estimation_state* est, double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos,
                                   double* joint_vel) {
-  ENTER(ctx, B, noise && rbd && est && quat && ang_vel_local && lin_acc_local && joint_pos && joint_vel && sensor_noise_ok(*noise) && accel_dt > 0.0 &&
-        tick >= 0 && tick <= UINT32_MAX, CAPPED);
-  return launch(ctx, K_UNPROFILED, sensor_read_kernel, (B + 63) / 64, 64, 0, B, *noise, (uint32_t)tick, accel_dt, 0.0, rbd, est, quat, ang_vel_local,
-                lin_acc_local, joint_pos, joint_vel, (uint8_t*)nullptr, OdomRead{});
+  return read_sensors_dev(ctx, B, noise, HardwareView{}, tick, accel_dt, rbd, est, quat, ang_vel_local, lin_acc_local, joint_pos, joint_vel);
 }
 
 int hb_sim_read_odometry_async(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, const double* rbd, const hb_estimation_state* est,
@@ -1811,12 +1853,19 @@ int hb_estimator_update_batch(hb_ctx* ctx, int B, const hb_kf_params* params, do
 
 int hb_sim_read_sensors(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, double accel_dt, const double* rbd, hb_estimation_state* est,
                         double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos, double* joint_vel) {
+  return hb_sim_read_sensors_hw(ctx, B, noise, nullptr, tick, accel_dt, rbd, est, quat, ang_vel_local, lin_acc_local, joint_pos, joint_vel);
+}
+
+// the one host-pointer sensor read: hb_sim_read_sensors is it with null records
+int hb_sim_read_sensors_hw(hb_ctx* ctx, int B, const hb_sensor_noise* noise, const hb_hardware_setting* hw, int64_t tick, double accel_dt,
+                           const double* rbd, hb_estimation_state* est, double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos,
+                           double* joint_vel) {
   ENTER(ctx, B, noise && rbd && est && quat && ang_vel_local && lin_acc_local && joint_pos && joint_vel && sensor_noise_ok(*noise) && accel_dt > 0.0 &&
-        tick >= 0 && tick <= UINT32_MAX, CAPPED);
+        tick >= 0 && tick <= UINT32_MAX, CAPPED, [&] { return all_ok(B, hw, hardware_setting_ok); });
   Staging s(ctx, B);
-  auto r = s.in(rbd, 32); auto es = s.inout(est, 1); auto q = s.out(quat, 4); auto w = s.out(ang_vel_local, 3); auto a = s.out(lin_acc_local, 3);
-  auto jp = s.out(joint_pos, NJ); auto jv = s.out(joint_vel, NJ);
-  return s.run(1, [&](Chunk) { return hb_sim_read_sensors_batch_dev(ctx, B, noise, tick, accel_dt, r, es, q, w, a, jp, jv); });
+  auto r = s.in(rbd, 32); auto es = s.inout(est, 1); auto h = s.in_or_null(hw, 1); auto q = s.out(quat, 4); auto w = s.out(ang_vel_local, 3);
+  auto a = s.out(lin_acc_local, 3); auto jp = s.out(joint_pos, NJ); auto jv = s.out(joint_vel, NJ);
+  return s.run(1, [&](Chunk) { return read_sensors_dev(ctx, B, noise, {h, B}, tick, accel_dt, r, es, q, w, a, jp, jv); });
 }
 
 int hb_sim_read_odometry(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, const double* rbd, const hb_estimation_state* est,
@@ -1837,10 +1886,17 @@ int hb_estimator_fuse_odometry(hb_ctx* ctx, int B, const hb_kf_params* params, h
 
 int hb_actuation_batch(hb_ctx* ctx, int B, double delay, const double* time, hb_actuation_state* state, const double* command, const double* rbd,
                        double* tau) {
-  ENTER(ctx, B, time && state && command && rbd && tau, CAPPED, [&] { return delay_ok(delay); });
+  return hb_actuation_hw(ctx, B, delay, nullptr, time, state, command, rbd, tau);
+}
+
+// the one host-pointer actuation: hb_actuation_batch is it with null records
+int hb_actuation_hw(hb_ctx* ctx, int B, double delay, const hb_hardware_setting* hw, const double* time, hb_actuation_state* state, const double* command,
+                    const double* rbd, double* tau) {
+  ENTER(ctx, B, time && state && command && rbd && tau, CAPPED, [&] { return delay_ok(delay) && all_ok(B, hw, hardware_setting_ok); });
   Staging s(ctx, B);
-  auto st = s.inout(state, 1); auto tm = s.in(time, 1); auto cmd = s.in(command, NJ * 5); auto r = s.in(rbd, 32); auto t = s.out(tau, NJ);
-  return s.run(1, [&](Chunk) { return hb_actuation_batch_dev(ctx, B, delay, tm, st, cmd, r, t); });
+  auto st = s.inout(state, 1); auto tm = s.in(time, 1); auto cmd = s.in(command, NJ * 5); auto r = s.in(rbd, 32); auto h = s.in_or_null(hw, 1);
+  auto t = s.out(tau, NJ);
+  return s.run(1, [&](Chunk) { return actuation_dev(ctx, B, delay, {h, B}, tm, st, cmd, r, t); });
 }
 
 int hb_sim_step_batch(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {

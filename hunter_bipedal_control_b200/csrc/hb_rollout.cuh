@@ -124,11 +124,13 @@ __global__ void rollout_tick_begin_kernel(int B, int tick, double t, double min_
   }
 }
 
-// actuator saturation of the applied torques (B x 10); NaN passes through as in numpy.clip
-__global__ void rollout_saturate_kernel(int B, hb_rollout_params p, double* tau) {
+// actuator saturation of the applied torques (B x 10); NaN passes through as in numpy.clip. An instance with a hardware record in `hw`
+// saturates at its limits in place of p.torque_limit.
+__global__ void rollout_saturate_kernel(int B, hb_rollout_params p, InstanceView<hb_hardware_setting> hw, double* tau) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= B * NJ) return;
-  const double lim = p.torque_limit[idx % NJ], v = tau[idx];
+  const hb_hardware_setting* h = hw.of(idx / NJ);
+  const double lim = h ? h->torque_limit[idx % NJ] : p.torque_limit[idx % NJ], v = tau[idx];
   tau[idx] = v < -lim ? -lim : (v > lim ? lim : v);
 }
 
@@ -194,11 +196,17 @@ __device__ __forceinline__ void add_sensor_noise(double sigma, uint64_t seed, in
   }
 }
 
+// v[0..m) += off[0..m), skipping the entries equal to 0.0 so that a -0.0 reading keeps its sign (simulated hardware, hunter_b200.h)
+__device__ __forceinline__ void add_sensor_offset(const double* off, double* v, int m) {
+  for (int j = 0; j < m; ++j) if (off[j] != 0.0) v[j] += off[j];
+}
+
 // The simulated robot's sensors at absolute tick `tick` from the true rbd r (LeggedHWSim::readSim, LeggedHWSim.cpp:116-130, and the joint
 // encoders). The accelerometer differences the world base velocity over the last plant step (accel_dt) where Gazebo reads the instantaneous
-// acceleration; unprimed, it reads gravity only. Updates base_vel_prev / primed.
-__device__ __forceinline__ void read_sensors(const hb_sensor_noise& nz, uint32_t tick, double accel_dt, const double* r, hb_estimation_state& e,
-                                             double* quat, double* gyro, double* acc, double* jp, double* jv) {
+// acceleration; unprimed, it reads gravity only. Updates base_vel_prev / primed. hw (nullable): the robot's hardware record, whose offsets
+// are added before the noise and whose sigmas replace nz's.
+__device__ __forceinline__ void read_sensors(const hb_sensor_noise& nz, const hb_hardware_setting* hw, uint32_t tick, double accel_dt, const double* r,
+                                             hb_estimation_state& e, double* quat, double* gyro, double* acc, double* jp, double* jv) {
   double sz, cz, sy, cy, sx, cx;
   sincos(r[0], &sz, &cz); sincos(r[1], &sy, &cy); sincos(r[2], &sx, &cx);
   const double R[9] = {cz * cy, cz * sy * sx - sz * cx, cz * sy * cx + sz * sx, sz * cy, sz * sy * sx + cz * cx, sz * sy * cx - cz * sx, -sy, cy * sx, cy * cx};
@@ -213,12 +221,16 @@ __device__ __forceinline__ void read_sensors(const hb_sensor_noise& nz, uint32_t
   for (int j = 0; j < NJ; ++j) { q[j] = r[6 + j]; qd[j] = r[NQ + 6 + j]; }
   for (int i = 0; i < 3; ++i) { e.base_vel_prev[i] = r[NQ + 3 + i]; }
   e.primed = 1;
+  if (hw) {
+    add_sensor_offset(hw->orientation_offset, ang, 3); add_sensor_offset(hw->gyro_bias, g, 3); add_sensor_offset(hw->accel_bias, a, 3);
+    add_sensor_offset(hw->encoder_offset, q, NJ);
+  }
   const uint64_t st = e.noise_stream;
-  add_sensor_noise(nz.orientation, nz.seed, NOISE_BLOCK_ORIENTATION, tick, st, ang, 3);
-  add_sensor_noise(nz.angular_velocity, nz.seed, NOISE_BLOCK_GYRO, tick, st, g, 3);
-  add_sensor_noise(nz.linear_acceleration, nz.seed, NOISE_BLOCK_ACCEL, tick, st, a, 3);
-  add_sensor_noise(nz.joint_position, nz.seed, NOISE_BLOCK_JOINT_POS, tick, st, q, NJ);
-  add_sensor_noise(nz.joint_velocity, nz.seed, NOISE_BLOCK_JOINT_VEL, tick, st, qd, NJ);
+  add_sensor_noise(hw ? hw->sigma_orientation : nz.orientation, nz.seed, NOISE_BLOCK_ORIENTATION, tick, st, ang, 3);
+  add_sensor_noise(hw ? hw->sigma_angular_velocity : nz.angular_velocity, nz.seed, NOISE_BLOCK_GYRO, tick, st, g, 3);
+  add_sensor_noise(hw ? hw->sigma_linear_acceleration : nz.linear_acceleration, nz.seed, NOISE_BLOCK_ACCEL, tick, st, a, 3);
+  add_sensor_noise(hw ? hw->sigma_joint_position : nz.joint_position, nz.seed, NOISE_BLOCK_JOINT_POS, tick, st, q, NJ);
+  add_sensor_noise(hw ? hw->sigma_joint_velocity : nz.joint_velocity, nz.seed, NOISE_BLOCK_JOINT_VEL, tick, st, qd, NJ);
   // quaternion (x, y, z, w) of R = Rz(yaw) Ry(pitch) Rx(roll)
   double hsz, hcz, hsy, hcy, hsx, hcx;
   sincos(0.5 * ang[0], &hsz, &hcz); sincos(0.5 * ang[1], &hsy, &hcy); sincos(0.5 * ang[2], &hsx, &hcx);
@@ -269,13 +281,14 @@ __device__ __forceinline__ void read_odometry(const OdomRead& o, int inst, uint6
 
 // Sensor read of B instances, one thread each. With cflag (the episode tick) the filter's contact flags come from the stored schedule of the
 // latest plan at flag_time, the previous observation's time (LeggedController.cpp:296-297), all 1 before the first plan (:298-304). With odom
-// set (an estimated episode with odometry) each instance's camera is read too.
-__global__ void sensor_read_kernel(int B, hb_sensor_noise nz, uint32_t tick, double accel_dt, double flag_time, const double* rbd, hb_estimation_state* est,
-                                   double* quat, double* gyro, double* acc, double* jp, double* jv, uint8_t* cflag, OdomRead odom) {
+// set (an estimated episode with odometry) each instance's camera is read too. An instance with a record in `hw` reads its sensors on it.
+__global__ void sensor_read_kernel(int B, hb_sensor_noise nz, InstanceView<hb_hardware_setting> hw, uint32_t tick, double accel_dt, double flag_time,
+                                   const double* rbd, hb_estimation_state* est, double* quat, double* gyro, double* acc, double* jp, double* jv,
+                                   uint8_t* cflag, OdomRead odom) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
   hb_estimation_state& e = est[inst];
-  read_sensors(nz, tick, accel_dt, rbd + (size_t)inst * 32, e, quat + (size_t)inst * 4, gyro + (size_t)inst * 3, acc + (size_t)inst * 3,
+  read_sensors(nz, hw.of(inst), tick, accel_dt, rbd + (size_t)inst * 32, e, quat + (size_t)inst * 4, gyro + (size_t)inst * 3, acc + (size_t)inst * 3,
                jp + (size_t)inst * NJ, jv + (size_t)inst * NJ);
   if (cflag) {
     const int mode = e.has_plan ? hbplan::mode_at(e.n_events, e.event_times, e.modes, flag_time) : 3;
@@ -382,10 +395,14 @@ __global__ void joint_command_kernel(int B, hb_pd_gains gains, InstanceView<hb_c
 // Actuation model of the simulated hardware (legged_gazebo/src/LeggedHWSim.cpp:166-192): every write pushes the hybrid joint command
 // (posDes, velDes, kp, kd, ff) with its time stamp on a buffer, drops the entries older than `delay` from the far end, and applies the
 // OLDEST remaining one: tau = kp (posDes - q) + kd (velDes - qd) + ff with the CURRENT joint state. One thread per instance; the deque is a
-// ring of HB_ACT_CAPACITY entries (a full ring drops its oldest entry first).
-__global__ void actuation_kernel(int B, double delay, const double* time, hb_actuation_state* state, const double* command, const double* rbd, double* tau) {
+// ring of HB_ACT_CAPACITY entries (a full ring drops its oldest entry first). An instance with a hardware record in `hw` runs its delay in
+// place of `delay_all`.
+__global__ void actuation_kernel(int B, double delay_all, InstanceView<hb_hardware_setting> hw, const double* time, hb_actuation_state* state,
+                                 const double* command, const double* rbd, double* tau) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
+  const hb_hardware_setting* h = hw.of(inst);
+  const double delay = h ? h->actuation_delay : delay_all;
   hb_actuation_state& st = state[inst];
   const double t = time[inst];
   int cnt = st.count, head = st.head;             // head = newest entry; entries head, head+1, ... (mod capacity) are older and older

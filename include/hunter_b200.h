@@ -470,6 +470,44 @@ typedef struct {
  * weight_contact_force < 0), a negative WBC task kp / kd, or a negative PD gain. */
 int hb_rollout_set_controller_settings(hb_ctx* ctx, int B, const hb_controller_setting* s);
 
+/* ---- simulated hardware: each robot's actuators and sensors between the controller and the plant (LeggedHWSim) ----
+ * Like a plant variation, the setting acts on the simulated robot only; the planner, MPC, WBC, joint command law and estimator are not
+ * told about it. Record i acts on instance i of the episodes; instances at or beyond B run the call's values, bit for bit as with no
+ * setting. With r the record of an instance:
+ *  - actuation: the actuation model's drop rule (hb_actuation_batch_dev) runs with r.actuation_delay in place of p->actuation_delay: the
+ *    oldest entries with stamp + delay < t are dropped, and the oldest remaining one is applied. Everything else about the ring is unchanged,
+ *    so a delay of HB_ACT_CAPACITY - 1 periods or more applies the oldest entry of the full ring (the ring holds HB_ACT_CAPACITY commands), as
+ *    a per-call delay does.
+ *  - saturation: the applied torque of joint j is clipped to +-r.torque_limit[j] in place of p->torque_limit[j]; hb_rollout_stats'
+ *    max_abs_torque counts the clipped value, before a plant variation's motor_strength.
+ *  - sensors (hb_rollout_estimated_batch_dev only): each reading is formed as (1) the true value, as hb_sim_read_sensors_batch_dev forms it;
+ *    (2) plus its offset; (3) plus sigma x its Philox normals, with r's sigma in place of the call's hb_sensor_noise sigma of that channel,
+ *    and the call's seed, the instance's noise_stream and the same blocks. The offsets: orientation_offset is added to the ZYX angles
+ *    before the quaternion is formed; gyro_bias to R' omega_world; accel_bias to R' (a_world + (0, 0, 9.81)); encoder_offset to q_j; the
+ *    joint velocities get none. An offset entry equal to 0.0 (either sign) adds nothing, so a reading of -0.0 stays -0.0 and a record with
+ *    zero offsets reads bit for bit what the call's values read. The tracking camera (odometry) is unchanged.
+ * hb_rollout_batch_dev has no sensors and reads only the delay and the limits. Every other entry point ignores this setting: the control
+ * step, the resident cycle and tick, hb_actuation_batch(_dev), hb_sim_read_sensors(_batch_dev) and the adapters; hb_actuation_hw and
+ * hb_sim_read_sensors_hw take records explicitly. The setting adds no launch to an episode: the actuation, saturation and sensor kernels
+ * that run every tick read the record of their own instance. hb_default_hardware_setting's record, with the noise sigmas of the call,
+ * reproduces the unset episode bit for bit. */
+typedef struct {                 /* the simulated hardware of one robot (LeggedHWSim), which the controllers are not told about */
+  double actuation_delay;        /* [s], finite, >= 0: in place of hb_rollout_params.actuation_delay                       */
+  double torque_limit[10];       /* [N m], finite, > 0: in place of hb_rollout_params.torque_limit                          */
+  double sigma_orientation, sigma_angular_velocity, sigma_linear_acceleration,
+         sigma_joint_position, sigma_joint_velocity;   /* finite, >= 0: in place of the call's hb_sensor_noise sigmas (its seed stays the key) */
+  double orientation_offset[3];  /* IMU mounting error on the ZYX angles [rad]                                             */
+  double gyro_bias[3];           /* body frame [rad/s]                                                                      */
+  double accel_bias[3];          /* body frame [m/s^2]                                                                      */
+  double encoder_offset[10];     /* joint zero offsets [rad]                                                                */
+} hb_hardware_setting;           /* 280 B */
+/* host only: actuation_delay 0.009 s and torque_limit HB_WBC_TORQUE_LIMITS per leg (hb_default_rollout_params' values), every sigma and
+ * offset 0 */
+int hb_default_hardware_setting(hb_hardware_setting* s);
+/* Sets the simulated hardware of the context's episodes (a per-robot episode setting, above). -1 also for a field that is not finite, a
+ * negative actuation_delay, a torque_limit <= 0 or a negative sigma. */
+int hb_rollout_set_hardware(hb_ctx* ctx, int B, const hb_hardware_setting* s);
+
 /* ---- estimated episodes (hb_rollout_estimated_batch_dev): the controllers read the Kalman filter's estimate from synthesised, noisy
  * sensors instead of the plant's true state (LeggedController::updateStateEstimation, LeggedController.cpp:280-349) ---- */
 typedef struct {                 /* standard deviations of additive Gaussian sensor noise; 0 = that channel is exact and draws nothing */
@@ -646,7 +684,7 @@ int hb_resident_wbc_batch_dev(hb_ctx* ctx, int B, const double* t_now, const dou
  * joint references), device planner, resident cycle without its WBC (cold start iff tick0 == 0). Every tick then runs
  * hb_resident_wbc_batch's policy + WeightedWbc at t (the adopted policy's for instances with an MPC latency, hb_rollout_set_mpc_latencies),
  * the joint command law (loaded, walking branch), the actuation model, saturation to
- * +-torque_limit and one plant step (with the tick's push wrench when hb_rollout_set_pushes has set schedules, on the instance's plant
+ * +-torque_limit (each robot's own delay and limits when hb_rollout_set_hardware has set records) and one plant step (with the tick's push wrench when hb_rollout_set_pushes has set schedules, on the instance's plant
  * when hb_rollout_set_plant_variations has set variations, on its ground when hb_rollout_set_terrains has set terrains). Failure checks run on the state entering each tick (finite, |roll| <= pi/2, base height) and on the
  * emergency stop the joint command raises; from its first failure on an instance is held (rbd put back to its last finite state after
  * every plant step; a non-finite state entering the first tick of a call is replaced by the nominal standing pose) and its outputs no
@@ -671,7 +709,8 @@ int hb_sim_read_sensors_batch_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noi
  * and the schedule of the new plan is copied into est. The policy, the WeightedWbc and the joint command law see the estimated rbd;
  * actuation, saturation, the plant and the failure checks the true one. est (B) is in/out; est_stats (B, nullable) in/out; est_log
  * (nullable) the estimated rbd in log's layout. Arguments are checked before any launch (sigmas finite and >= 0). With odometry set
- * (hb_rollout_set_odometry), the sensor read also reads each camera and the filter fuses the messages due on the tick. */
+ * (hb_rollout_set_odometry), the sensor read also reads each camera and the filter fuses the messages due on the tick. With a hardware
+ * setting (hb_rollout_set_hardware), each robot's actuation, saturation and sensors run on its record. */
 int hb_rollout_estimated_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb_rollout_params* p, const hb_estimation_params* ep,
                                    const hb_rollout_command* cmd, double* rbd, hb_actuation_state* act, uint8_t* estop, hb_rollout_stats* stats,
                                    hb_estimation_state* est, hb_estimation_stats* est_stats /*nullable*/, double* log /*nullable*/,
@@ -744,6 +783,17 @@ int hb_contact_force_estimate_batch(hb_ctx* ctx, int B, double cutoff_frequency,
                                     const double* tau_cmd, double* est_contact_force, double* disturbance_torque /*nullable*/);
 int hb_actuation_batch(hb_ctx* ctx, int B, double delay, const double* time, hb_actuation_state* state, const double* command, const double* rbd,
                        double* tau);
+/* ---- the simulated hardware outside the episodes (simulated hardware, above): the episode's actuation and sensor read with explicit
+ * records, so that an episode with hb_rollout_set_hardware can be written as a loop of public calls ----
+ * hw (B, nullable): the record of each robot, validated as by hb_rollout_set_hardware (-1). hb_actuation_hw runs robot i's actuation with
+ * hw[i].actuation_delay in place of delay (the limits are the caller's clip); hb_sim_read_sensors_hw reads robot i's sensors with hw[i]'s
+ * offsets and sigmas in place of noise's sigmas. NULL hw is exactly hb_actuation_batch / hb_sim_read_sensors, which are these calls with
+ * hw = NULL. Host pointers, synchronous; the context's hardware setting is not read. */
+int hb_actuation_hw(hb_ctx* ctx, int B, double delay, const hb_hardware_setting* hw /*nullable*/, const double* time, hb_actuation_state* state,
+                    const double* command, const double* rbd, double* tau);
+int hb_sim_read_sensors_hw(hb_ctx* ctx, int B, const hb_sensor_noise* noise, const hb_hardware_setting* hw /*nullable*/, int64_t tick,
+                           double accel_dt, const double* rbd, hb_estimation_state* est, double* quat, double* ang_vel_local, double* lin_acc_local,
+                           double* joint_pos, double* joint_vel);
 int hb_sim_step_batch(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force /*nullable*/,
                       uint8_t* contact_flag /*nullable*/);
 /* hb_sim_step_batch with an external world wrench on each robot's base: wrench (B x 6) = force [N] at the base frame origin, then a couple
