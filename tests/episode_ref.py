@@ -1,6 +1,6 @@
-"""The batched closed-loop episode restated once for its tests (test_gpu_rollout_episodes.py, test_gpu_rollout_estimation.py,
-test_gpu_rollout_pushes.py, test_gpu_rollout.py): the shared setup, the plant in numpy, the episode as a loop of public calls, and the
-comparisons of episode outputs."""
+"""The batched closed-loop episode restated once for its tests (test_gpu_rollout*.py and the tests of the other per-robot settings): the
+shared setup, the plant in numpy, the episode with every per-robot setting as one loop of public calls (stepwise), the comparisons of
+episode outputs, and the checks and data shared by the settings."""
 import ctypes as C
 import math
 
@@ -222,27 +222,59 @@ def _mode_at(st, t):
     return st.modes[idx]
 
 
-def stepwise(ctx, rbd0, gaits, cmd_vels, n_ticks, prm, log_every, ep=None, est=None, pushes=None, variations=None, terrains=None):
+def latency_due(lat, a, every):
+    """The flags of the instances with MPC latencies lat (0 beyond the setting) whose solution comes into force on tick a: the MRT's
+    adoption d >= 1 ticks after each cycle."""
+    return (lat >= 1) & (a >= lat) & ((a - lat) % every == 0)
+
+
+def _padded(items, B, default):
+    """The B records of a per-robot setting: items, then `default` beyond them."""
+    return (type(default) * B)(*[items[i] if i < len(items) else default for i in range(B)])
+
+
+def stepwise(ctx, rbd0, gaits, cmd_vels, n_ticks, prm, log_every, ep=None, est=None, pushes=None, plant_variations=None, terrains=None,
+             goals=None, mpc_latencies=None, odometry=None, hardware=None):
     """The episode as a Python loop of public calls from tick 0, with the checks, holding and stats restated in numpy. It is the device
-    loop (rollout_impl) tick for tick: with ep and est (fresh estimation states, advanced in place) it is the estimated episode, whose
-    controllers read the filter's estimate, and the estimation steps sit where the device loop's estimation branches sit. pushes,
-    variations, terrains: the settings on ctx. Each tick's wrench comes from the pushes; every plant step runs on the variations and
-    terrains, padded as the setting is documented: the default variation, and flat ground at prm.sim.ground_height, beyond them. The
-    height check here is the absolute one, so with terrains it restates the episode only for prm.min_base_height = 0 (params()). Returns
-    the tuple of Context.rollout, or of Context.rollout_estimated with ep."""
+    loop (rollout_impl) tick for tick, each step in its place there: with ep and est (fresh estimation states, advanced in place) it is the
+    estimated episode, whose controllers read the filter's estimate. The per-robot settings are those on ctx, under the names of their
+    Context.set_<name>; one not given is unset. Each is restated by the public calls that take it, padded beyond its instances as the
+    setting is documented:
+    - pushes: each tick's wrench (wrench_numpy).
+    - plant_variations, terrains: every plant step, on the default variation and flat ground at prm.sim.ground_height beyond them. The
+      height check here is the absolute one, so with terrains this restates the episode only for prm.min_base_height = 0 (params()).
+    - goals: on each MPC tick the goal in force is converted by hb_goal_to_target on the tick's x0 when it differs from the captured one,
+      and every instance gets its target through hb_plan_set_targets: the captured one, or its cmd_vel target as the device planner
+      builds it. The cold tick 0 starts with no goal captured.
+    - mpc_latencies: the MRT split. The instances due adopt (hb_policy_update) before the tick's cycle, and on the cold tick every
+      instance with a latency adopts after it; the latency-0 instances adopt the resident solution on every tick, then the tick's WBC is
+      hb_policy_wbc. The public cycle runs its own WBC on the new solution, which the episodes do not, so the loop equals the episode
+      while no WBC falls back.
+    - odometry (estimated episodes; the cameras are ctx's): the camera read (hb_sim_read_odometry) after each sensor read, the fusion
+      (hb_estimator_fuse_odometry) after each filter update.
+    - hardware: the sensor read (hb_sim_read_sensors_hw) and the actuation (hb_actuation_hw) on the records, padded with the call's values
+      (call_hardware(prm, ep)), and each robot's torques clipped to its record's limits; unset, the call's delay and prm.torque_limit.
+    Controller and planner settings need no restating: the planner calls read ctx's planner settings, and the hardware test restates a
+    controller record as ctx's WBC settings and prm.gains. Returns the tuple of Context.rollout, or of Context.rollout_estimated with ep."""
     B = rbd0.shape[0]
-    var = None if variations is None else (hb.HbPlantVariation * B)(
-        *[variations[i] if i < len(variations) else hb.default_plant_variation() for i in range(B)])
+    var = None if plant_variations is None else _padded(plant_variations, B, hb.default_plant_variation())
     ter = None
     if terrains is not None:
         assert prm.min_base_height == 0
-        ter = (hb.HbTerrain * B)(*[terrains[i] if i < len(terrains) else flat_terrain(prm.sim.ground_height) for i in range(B)])
+        ter = _padded(terrains, B, flat_terrain(prm.sim.ground_height))
+    lat = None if mpc_latencies is None else np.array([mpc_latencies[i] if i < len(mpc_latencies) else 0 for i in range(B)])
+    captured = {}                                        # instance: (index of its captured goal, that goal's target)
+    hw = None
+    lim = np.array(prm.torque_limit[:])
+    if hardware is not None:
+        from hardware_ref import call_hardware           # hardware_ref imports this module
+        hw = _padded(hardware, B, call_hardware(prm, ep))
+        lim = np.array([h.torque_limit[:] for h in hw])
     rbd = rbd0.copy()
     act = hb.actuation_states(B)
     estop = np.zeros(B, dtype=np.uint8)
     st = hb.rollout_stats(B)
     held = rbd.copy()
-    lim = np.array(prm.torque_limit[:])
     times = np.array(CMD_TIMES)
     logs = []
     if ep is not None:
@@ -264,13 +296,17 @@ def stepwise(ctx, rbd0, gaits, cmd_vels, n_ticks, prm, log_every, ep=None, est=N
         meas = rbd                                       # what the controllers measure: the true state, or the filter's estimate
         if ep is not None:
             # sensors and contact flags at the previous observation's time, filter, observation step (yaw unwrap, estimation stats)
-            quat, w, acc, jp, jv = ctx.read_sensors(rbd, est, a, ep.noise, accel_dt=prm.sim.dt)
+            quat, w, acc, jp, jv = ctx.read_sensors(rbd, est, a, ep.noise, accel_dt=prm.sim.dt, hardware=hw)
+            if odometry is not None:
+                msg = ctx.read_odometry(rbd, est, a, ep.noise)
             flags = np.ones((B, 4), dtype=np.uint8)
             for i in range(B):
                 if est[i].has_plan:
                     m = _mode_at(est[i], (a - 1) * prm.period)
                     flags[i] = [1 if (m in (1, 3) if c & 1 else m in (2, 3)) else 0 for c in range(4)]
             meas = ctx.estimator_update(prm.period, kf, quat, w, acc, jp, jv, flags, params=ep.kf)
+            if odometry is not None:
+                meas = ctx.fuse_odometry(kf, *msg, flags, meas, params=ep.kf)
             for i in range(B):
                 est[i].yaw_obs = est[i].yaw_obs + shortest_angular_distance(est[i].yaw_obs, meas[i, 0])
                 if st["fail_tick"][i] < 0:
@@ -284,14 +320,34 @@ def stepwise(ctx, rbd0, gaits, cmd_vels, n_ticks, prm, log_every, ep=None, est=N
                     es["sum_sq_vel_err"][i] += sq; es["sum_sq_height_err"][i] += dz * dz; es["count"][i] += 1
             if log_every and a % log_every == 0:
                 est_logs.append(meas.copy())
+        if lat is not None:
+            due = latency_due(lat, a, prm.mpc_every)
+            if due.any():
+                ctx.policy_update(B, due)
         mpc = a % prm.mpc_every == 0
         if mpc:
             x0 = ctx.rbd_to_centroidal(meas)
             if ep is not None:
                 x0[:, 9] = [est[i].yaw_obs for i in range(B)]
             cmd = cmd_vels[:, max(np.searchsorted(times, t, side="right") - 1, 0)]      # the last segment that has started
+            if goals is not None:
+                ctx.set_plan_targets(None)
+                plain, _, pst = ctx.plan_references_gpu(hb.make_plan_inputs(np.full(B, t), horizon(ctx), x0, cmd, None, gaits, GAIT_START,
+                                                                            joint_ik=False), np.zeros((B, 12)))
+                assert (pst == 0).all()
+                targets = [hb.reference_target(r) for r in plain]
+                for i in range(min(B, len(goals))):
+                    s = goals[i]
+                    g = max([j for j in range(s.n_goal) if s.time[j] <= t], default=-1)
+                    if g >= 0 and captured.get(i, (-1,))[0] != g:
+                        captured[i] = (g, hb.goal_to_target(t, x0[i:i + 1], np.array(s.goal[g][:]))[0])
+                    if i in captured:
+                        targets[i] = captured[i][1]
+                ctx.set_plan_targets((hb.HbTarget * B)(*targets))
             ins = hb.make_plan_inputs(np.full(B, t), horizon(ctx), x0, cmd, None, gaits, GAIT_START)
             info, _, _, _, ps = ctx.resident_plan_cycle(a == 0, 0.0, ins, meas)
+            if lat is not None and a == 0 and (lat >= 1).any():
+                ctx.policy_update(B, lat >= 1)
             if ep is not None:
                 # the plan's schedule copied into the estimation state, for the next ticks' contact flags
                 refs, stance, _ = ctx.plan_references_gpu(hb.make_plan_inputs(np.full(B, t), horizon(ctx), x0, cmd, ctx.contact_positions(x0), gaits,
@@ -304,9 +360,13 @@ def stepwise(ctx, rbd0, gaits, cmd_vels, n_ticks, prm, log_every, ep=None, est=N
                     for k in range(n + 1):
                         est[i].modes[k] = refs[i].modes[k]
                     est[i].has_plan = 1
-        xd, ud, md, sol, _, wst = ctx.resident_wbc(t, meas)
+        if lat is None:
+            xd, ud, md, sol, _, wst = ctx.resident_wbc(t, meas)
+        else:
+            ctx.policy_update(B, lat == 0)
+            xd, ud, md, sol, _, wst = ctx.policy_wbc(t, meas)
         jcmd, _, estop = ctx.joint_command(prm.period, xd, ud, sol, md, meas, estop=estop, gains=prm.gains)
-        tau = ctx.actuation(t, act, jcmd, rbd, prm.actuation_delay)
+        tau = ctx.actuation(t, act, jcmd, rbd, prm.actuation_delay, hardware=hw)
         tau = np.clip(tau, -lim, lim)
         rbd, _, _ = ctx.sim_step(rbd, tau, prm.sim, wrench=None if pushes is None else wrench_numpy(pushes, t, B), variation=var, terrain=ter)
         for i in range(B):                               # after the plant step
@@ -417,8 +477,72 @@ def launch_coefficients(ctx, rbd0, gaits, cmd_vels, prm, ep=None):
 
 
 # ---------------------------------------------------------------------------------------------------------------- per-robot settings
-# Pushes, plant variations and terrains are per-robot settings of the episodes (Context.set_pushes / set_plant_variations / set_terrains,
-# hb_rollout_set_*), with one contract. The checks below take the setting's name and each test file's own data.
+# Every per-robot setting of the episodes (Context.set_<name>, hb_rollout_set_*) has one contract. The checks below take the setting's name
+# and each test file's own data.
+FRICTION = [1.0, 0.8, 1.0, 0.6, 1.0, 0.9]          # ground friction scales of six robots
+PUSH = [[25.0, -15.0, 0.0]]                         # one push of 25 N forward and 15 N to the right
+
+
+def small_terrains():
+    """Three flat terrains, at GROUND, 5 mm above and 4 mm below it: 2 x 2 grids at (-2, -2), beyond which the robots stand on the
+    clamped edge heights."""
+    return hb.make_terrains(3, np.full((3, 2, 2), [[[0.0]], [[0.005]], [[-0.004]]]) + GROUND, 0.5, (-2.0, -2.0))
+
+
+def random_goals(rbd0, B, seed):
+    """Goal schedules of the first B - 1 of the robots: a goal 0.15-0.4 m away in a random direction given between two MPC ticks, a second
+    one later for every other robot, and the goal at the start pose from the start for the robot at index 2."""
+    rng = np.random.default_rng(seed)
+    n = B - 1
+    d = rng.uniform(0.15, 0.4, n); th = rng.uniform(-np.pi, np.pi, n)
+    g1 = np.c_[rbd0[:n, 3] + d * np.cos(th), rbd0[:n, 4] + d * np.sin(th), rbd0[:n, 0] + rng.uniform(-0.6, 0.6, n)]
+    g2 = g1 + np.c_[rng.uniform(-0.2, 0.2, (n, 2)), rng.uniform(-0.3, 0.3, n)]
+    times = np.c_[np.full(n, 0.053), np.where(np.arange(n) % 2, 0.21, 1e9)]
+    s = hb.make_goal_schedules(n, times, np.stack([g1, g2], axis=1))
+    s[2].n_goal = 1; s[2].time[0] = 0.0
+    s[2].goal[0][0], s[2].goal[0][1], s[2].goal[0][2] = rbd0[2, 3], rbd0[2, 4], rbd0[2, 0]
+    return s
+
+
+def use(ctx, **settings):
+    """Sets each setting on ctx (Context.set_<name>(value)) and returns them: stepwise's keyword arguments for the same episode."""
+    for name, value in settings.items():
+        getattr(ctx, "set_" + name)(value)
+    return settings
+
+
+def array_of(records):
+    """A ctypes array of the records (all of one type)."""
+    return (type(records[0]) * len(records))(*records)
+
+
+def logged_episode(ctx, rbd0, prm, ep, n_ticks=100, streams=50):
+    """The episode of the instances rbd0 with GAITS and cmd_vels, logged every 10 ticks, as outputs(): estimated with ep (fresh estimation
+    states from noise stream `streams`), truth without."""
+    B = rbd0.shape[0]
+    est = hb.estimation_states(B, streams) if ep is not None else None
+    return outputs(device(ctx, rbd0, GAITS, cmd_vels(B), n_ticks, prm, 10, ep, est))
+
+
+def assert_records_act_as_their_values(ctx, name, records, values, rbd0, prm, ep, n_ticks=100, streams=50):
+    """The records of the setting cycled over the 2 len(records) instances rbd0 (logged_episode): instance i with record k gives bit for
+    bit what it gives with the setting cleared and record k's values given another way, `with values(ctx, record, prm, ep) as (prm_k,
+    ep_k)` (a context manager that undoes on exit what it changed on ctx); and every instance moves against the unset episode, so the
+    records really act."""
+    set_ = getattr(ctx, "set_" + name)
+    n = len(records)
+    set_(array_of([records[i % n] for i in range(2 * n)]))
+    got = logged_episode(ctx, rbd0, prm, ep, n_ticks, streams)
+    set_(None)
+    for k, rec in enumerate(records):
+        with values(ctx, rec, prm, ep) as (p, e):
+            want = logged_episode(ctx, rbd0, p, e, n_ticks, streams)
+        assert_episode_equal(got, want, rows_a=[k, k + n], rows_b=[k, k + n])
+    ref = logged_episode(ctx, rbd0, prm, ep, n_ticks, streams)
+    for i in range(2 * n):
+        assert not np.array_equal(got[0][i], ref[0][i]), i
+
+
 def _counted(ctx, run):
     c0 = ctx.launch_count
     out = run()

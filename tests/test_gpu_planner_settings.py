@@ -4,12 +4,15 @@ grids, truth and estimator, and alongside pushes, variations and a terrain), eac
 latency and controller settings also set, the shared setting contract (null settings, launch counts, continuation, independence,
 permutation, instances beyond the setting, clearing, argument checks), and what the records do to the robots on the plant: touchdowns at
 the template's period, clearance that grows with swing_height, a template with a flight phase planned and tracked."""
+from contextlib import contextmanager
+
 import numpy as np
 import pytest
 
 import hunter_bipedal_control_b200 as hb
-from episode_ref import (GAITS, GROUND, assert_episode_equal, assert_null_settings, assert_rejected_settings, assert_setting_episodes, cmd_vels,
-                         context, device, est_params, launch_coefficients, outputs, params, start_states, stepwise)
+from episode_ref import (FRICTION, GAITS, GROUND, PUSH, array_of, assert_episode_equal, assert_null_settings, assert_records_act_as_their_values,
+                         assert_rejected_settings, assert_setting_episodes, cmd_vels, context, device, est_params, launch_coefficients, outputs, params,
+                         small_terrains, start_states, stepwise, use)
 from planner_settings_ref import random_settings
 from test_planner_settings_host import T, _bad_records, _cases
 
@@ -54,14 +57,6 @@ def _records():
     ]
 
 
-def _array(recs):
-    return (hb.HbPlannerSettings * len(recs))(*recs)
-
-
-def _copy(rec):
-    return hb.HbPlannerSettings.from_buffer_copy(bytes(rec))
-
-
 def _ref_fields(r):
     ne, nt = r.n_events, r.n_targets
     segs = [[np.array([list(r.segments[c][a][k][:]) for k in range(r.n_segments[c][a])]).reshape(-1, 6) for a in range(3)] for c in range(4)]
@@ -92,8 +87,7 @@ def test_device_planner_matches_host_planner_with_settings():
                 assert a[6][c][ax].shape == b[6][c][ax].shape
                 np.testing.assert_allclose(a[6][c][ax], b[6][c][ax], rtol=0, atol=1e-11)
     # a template too short for the capacities: status -5 on the device as on the host, the others unaffected
-    short = _copy(settings[7]); short.gait[hb.GAIT_IDS[gaits[7]]] = hb.gait_template([3, 3], [0.0, 0.005, 0.01])
-    settings[7] = short
+    settings[7].gait[hb.GAIT_IDS[gaits[7]]] = hb.gait_template([3, 3], [0.0, 0.005, 0.01])
     ctx.set_planner_settings(settings)
     rd2, _, st2 = ctx.plan_references_gpu(ins, latest)
     assert st2[7] == -5 and (np.delete(st2, 7) == 0).all() and rd2[7].n_events == 0
@@ -127,9 +121,17 @@ def test_default_record_is_the_unset_device_planner_bitwise():
     ctx.close()
 
 
+@contextmanager
+def _on_every_robot(ctx, rec, prm, ep):
+    """rec as the planner settings of every robot, cleared on exit."""
+    ctx.set_planner_settings(array_of([rec] * B))
+    yield prm, ep
+    ctx.set_planner_settings(None)
+
+
 def _mixed(n=B):
     r = _records()
-    return _array([r[i % 3] for i in range(n)])
+    return array_of([r[i % 3] for i in range(n)])
 
 
 @pytest.mark.parametrize("wbc", ["weighted", "hierarchical"])
@@ -143,16 +145,14 @@ def test_episode_equals_the_stepwise_loop_bitwise(wbc, event_nodes, estimated):
     rbd0 = start_states(ctx, B, seed=81)
     vels = cmd_vels(B)
     prm = params(log_every)
-    extra = {}
+    kw = {}
     if wbc == "weighted" and not event_nodes:       # alongside pushes, plant variations and a terrain
-        extra = dict(terrains=hb.make_terrains(3, np.full((3, 2, 2), [[[0.0]], [[0.005]], [[-0.004]]]) + GROUND, 0.5, (-2.0, -2.0)),
-                     variations=hb.make_plant_variations(B, friction_scale=[1.0, 0.8, 1.0, 0.6, 1.0, 0.9]),
-                     pushes=hb.make_push_schedules(B, 0.15, 0.05, [[25.0, -15.0, 0.0]]))
-        ctx.set_terrains(extra["terrains"]); ctx.set_plant_variations(extra["variations"]); ctx.set_pushes(extra["pushes"])
+        kw = use(ctx, terrains=small_terrains(), plant_variations=hb.make_plant_variations(B, friction_scale=FRICTION),
+                 pushes=hb.make_push_schedules(B, 0.15, 0.05, PUSH))
     ep = est_params(seed=2031) if estimated else None
     ctx.set_planner_settings(_mixed())
     d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 30) if estimated else None)
-    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 30) if estimated else None, **extra)
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 30) if estimated else None, **kw)
     assert_episode_equal(d, r)
     ctx.set_planner_settings(None)
     u = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 30) if estimated else None)
@@ -167,28 +167,11 @@ def test_each_record_acts_on_its_robot_alone_with_every_other_setting(estimated)
     bit for bit robot i of the batch in which every robot has record k."""
     ctx = context()
     rbd0 = start_states(ctx, B, seed=82)
-    prm = params(10)
-    ep = est_params(seed=2032) if estimated else None
-    ctx.set_plant_variations(hb.make_plant_variations(B, friction_scale=[1.0, 0.8, 1.0, 0.6, 1.0, 0.9], motor_strength=0.95))
-    ctx.set_pushes(hb.make_push_schedules(B, 0.05, 0.05, [[25.0, -15.0, 0.0]]))
-    ctx.set_terrains(hb.make_terrains(3, np.full((3, 2, 2), [[[0.0]], [[0.005]], [[-0.004]]]) + GROUND, 0.5, (-2.0, -2.0)))
-    ctx.set_goals(hb.make_goal_schedules(B, 0.15, [0.2, 0.0, 0.1]))
-    ctx.set_mpc_latencies([0, 1, 2, 0, 3, 1])
-    ctx.set_controller_settings(hb.make_controller_settings(B, swing_kp=[150.0, 170.0, 160.0, 180.0, 140.0, 160.0]))
-
-    def run():
-        return outputs(device(ctx, rbd0, GAITS, cmd_vels(B), 150, prm, 10, ep, hb.estimation_states(B, 31) if estimated else None))
-
-    recs = _records()
-    ctx.set_planner_settings(_mixed())
-    got = run()
-    for k, rec in enumerate(recs):
-        ctx.set_planner_settings(_array([rec] * B))
-        assert_episode_equal(got, run(), rows_a=[k, k + 3], rows_b=[k, k + 3])
-    ctx.set_planner_settings(None)
-    ref = run()
-    for i in range(B):
-        assert not np.array_equal(got[0][i], ref[0][i]), i
+    use(ctx, plant_variations=hb.make_plant_variations(B, friction_scale=FRICTION, motor_strength=0.95), pushes=hb.make_push_schedules(B, 0.05, 0.05, PUSH),
+        terrains=small_terrains(), goals=hb.make_goal_schedules(B, 0.15, [0.2, 0.0, 0.1]), mpc_latencies=[0, 1, 2, 0, 3, 1],
+        controller_settings=hb.make_controller_settings(B, swing_kp=[150.0, 170.0, 160.0, 180.0, 140.0, 160.0]))
+    assert_records_act_as_their_values(ctx, "planner_settings", _records(), _on_every_robot, rbd0, params(10),
+                                       est_params(seed=2032) if estimated else None, n_ticks=150, streams=31)
     ctx.close()
 
 
@@ -216,13 +199,13 @@ def test_setting_contract():
     ctx = context()
     rbd0 = start_states(ctx, B, seed=84)
     r = _records()
-    full = _array([r[0], r[1], r[2], r[1], r[0], r[2]])
+    full = array_of([r[0], r[1], r[2], r[1], r[0], r[2]])
     one = hb.make_planner_settings(B)
-    one[0] = _copy(r[0])
-    other = _array([r[2], r[0], r[1], r[1], r[2], r[0]])       # instance 3 keeps its record
-    part = _array([r[1], r[2]])
+    one[0] = r[0]
+    other = array_of([r[2], r[0], r[1], r[1], r[2], r[0]])       # instance 3 keeps its record
+    part = array_of([r[1], r[2]])
     padded = hb.make_planner_settings(B)
-    padded[0], padded[1] = _copy(r[1]), _copy(r[2])
+    padded[0], padded[1] = r[1], r[2]
     assert_setting_episodes(_Ctx(ctx), "planner_settings", rbd0, params(10), full, one, other, 3, part, padded)
     ctx.close()
 

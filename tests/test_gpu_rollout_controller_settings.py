@@ -4,14 +4,16 @@ both time grids, with and without the estimator; then the setting's contract (nu
 permutation, instances beyond the setting, clearing, argument checks), the precedence over the context's settings, and the calls that
 ignore it."""
 import ctypes as C
+from contextlib import contextmanager
 
 import numpy as np
 import pytest
 
 import hunter_bipedal_control_b200 as hb
 from hunter_bipedal_control_b200 import scenarios as sc
-from episode_ref import (GAITS, assert_episode_equal, assert_null_settings, assert_rejected_settings, assert_setting_episodes, cmd_vels, context,
-                         device, est_params, outputs, params, start_states, stepwise)
+from episode_ref import (FRICTION, GAITS, PUSH, array_of, assert_episode_equal, assert_null_settings, assert_records_act_as_their_values,
+                         assert_rejected_settings, assert_setting_episodes, cmd_vels, context, device, est_params, logged_episode, outputs, params,
+                         small_terrains, start_states, stepwise, use)
 
 pytestmark = pytest.mark.gpu
 
@@ -37,26 +39,15 @@ def _records():
     ]
 
 
-def _array(recs):
-    return (hb.HbControllerSetting * len(recs))(*recs)
-
-
-def _copy(rec):
-    return hb.HbControllerSetting.from_buffer_copy(bytes(rec))
-
-
-def _run(ctx, rbd0, prm, ep, n_ticks=100, log_every=10):
-    est = hb.estimation_states(B, 50) if ep is not None else None
-    return outputs(device(ctx, rbd0, GAITS, cmd_vels(B), n_ticks, prm, log_every, ep, est))
-
-
-def _with_context(ctx, rec, prm):
-    """The context's WBC settings and a copy of prm carrying rec's values; returns the previous settings."""
+@contextmanager
+def _on_the_context(ctx, rec, prm, ep):
+    """The context's WBC settings and a copy of prm carrying rec's values; the previous settings restored on exit."""
     old = ctx.wbc_settings()
     ctx.set_wbc_settings(rec.wbc)
     p = hb.HbRolloutParams.from_buffer_copy(bytes(prm))
     p.gains = rec.gains
-    return old, p
+    yield p, ep
+    ctx.set_wbc_settings(old)
 
 
 @pytest.mark.parametrize("wbc", ["weighted", "hierarchical"])
@@ -67,28 +58,12 @@ def test_records_equal_per_context_runs_bitwise(wbc, event_nodes, estimated):
     ctx = context(event_nodes)
     ctx.set_wbc_formulation(wbc)
     rbd0 = start_states(ctx, B, seed=91)
-    prm = params(10)
-    ep = est_params(seed=2029) if estimated else None
     if wbc == "weighted" and not event_nodes:       # alongside pushes, variations, a terrain, goals and an MPC latency
-        ctx.set_plant_variations(hb.make_plant_variations(B, friction_scale=[1.0, 0.8, 1.0, 0.6, 1.0, 0.9], motor_strength=0.95))
-        ctx.set_pushes(hb.make_push_schedules(B, 0.05, 0.05, [[25.0, -15.0, 0.0]]))
-        ctx.set_terrains(hb.make_terrains(3, np.full((3, 2, 2), [[[0.0]], [[0.005]], [[-0.004]]]) + 0.02, 0.5, (-2.0, -2.0)))
-        ctx.set_goals(hb.make_goal_schedules(B, 0.05, [0.2, 0.0, 0.1]))
-        ctx.set_mpc_latencies([0, 1, 2, 0, 3, 1])
-    recs = _records()
-    ctx.set_controller_settings(_array([recs[i % 3] for i in range(B)]))
-    got = _run(ctx, rbd0, prm, ep)
-    ctx.set_controller_settings(None)
-    for k, rec in enumerate(recs):
-        old, p = _with_context(ctx, rec, prm)
-        want = _run(ctx, rbd0, p, ep)
-        ctx.set_wbc_settings(old)
-        rows = [k, k + 3]
-        assert_episode_equal(got, want, rows_a=rows, rows_b=rows)
-    # the records really act: each moves its robots away from the default controller
-    ref = _run(ctx, rbd0, prm, ep)
-    for i in range(B):
-        assert not np.array_equal(got[0][i], ref[0][i]), i
+        use(ctx, plant_variations=hb.make_plant_variations(B, friction_scale=FRICTION, motor_strength=0.95),
+            pushes=hb.make_push_schedules(B, 0.05, 0.05, PUSH), terrains=small_terrains(), goals=hb.make_goal_schedules(B, 0.05, [0.2, 0.0, 0.1]),
+            mpc_latencies=[0, 1, 2, 0, 3, 1])
+    assert_records_act_as_their_values(ctx, "controller_settings", _records(), _on_the_context, rbd0, params(10),
+                                       est_params(seed=2029) if estimated else None)
     ctx.close()
 
 
@@ -107,7 +82,7 @@ def test_null_settings(wbc, event_nodes, estimated):
     null = hb.make_controller_settings(B, wbc=ctx.wbc_settings(), gains=prm.gains)
     assert_null_settings(ctx, "controller_settings", lambda: device(ctx, rbd0, GAITS, cmd_vels(B), 60, prm, 5, ep,
                                                                     hb.estimation_states(B, 50) if estimated else None),
-                         (null, _array([null[0]] * 3)), _array(_records() * 2))
+                         (null, array_of([null[0]] * 3)), array_of(_records() * 2))
     ctx.close()
 
 
@@ -115,13 +90,13 @@ def test_setting_contract():
     ctx = context()
     rbd0 = start_states(ctx, B, seed=93)
     r = _records()
-    full = _array([r[0], r[1], r[2], r[1], r[0], r[2]])
+    full = array_of([r[0], r[1], r[2], r[1], r[0], r[2]])
     one = hb.make_controller_settings(B)
-    one[0] = _copy(r[0])
-    other = _array([r[2], r[0], r[1], r[1], r[2], r[0]])       # instance 3 keeps its record
-    part = _array([r[1], r[2]])
+    one[0] = r[0]
+    other = array_of([r[2], r[0], r[1], r[1], r[2], r[0]])       # instance 3 keeps its record
+    part = array_of([r[1], r[2]])
     padded = hb.make_controller_settings(B)
-    padded[0], padded[1] = _copy(r[1]), _copy(r[2])
+    padded[0], padded[1] = r[1], r[2]
     assert_setting_episodes(ctx, "controller_settings", rbd0, params(10), full, one, other, 3, part, padded)
     ctx.close()
 
@@ -145,7 +120,7 @@ def test_rejected_settings(estimated):
     ep = est_params(seed=8) if estimated else None
     assert_rejected_settings(ctx, "controller_settings",
                              lambda: device(ctx, rbd0, GAITS, cmd_vels(B), 40, params(5), 5, ep, hb.estimation_states(B, 50) if estimated else None),
-                             _array(_records() * 2), _bad(), hb.make_controller_settings(ctx.max_batch + 1))
+                             array_of(_records() * 2), _bad(), hb.make_controller_settings(ctx.max_batch + 1))
     ctx.close()
 
 
@@ -155,8 +130,8 @@ def test_precedence_over_the_context():
     ctx = context()
     rbd0 = start_states(ctx, B, seed=95)
     prm = params(10)
-    ctx.set_controller_settings(_array(_records()))
-    base = _run(ctx, rbd0, prm, None)
+    ctx.set_controller_settings(array_of(_records()))
+    base = logged_episode(ctx, rbd0, prm, None)
     w = ctx.wbc_settings()
     changes = []
     s = hb.HbWbcSettings.from_buffer_copy(bytes(w)); s.base_angular_kp *= 0.6
@@ -164,13 +139,13 @@ def test_precedence_over_the_context():
     changes.append(lambda: ctx.set_kp_kd(1.4 * w.swing_kp, w.swing_kd))
     for change in changes:
         change()
-        moved = _run(ctx, rbd0, prm, None)
+        moved = logged_episode(ctx, rbd0, prm, None)
         ctx.set_wbc_settings(w)
         assert_episode_equal(moved, base, rows_a=slice(0, 3), rows_b=slice(0, 3))
         assert any(not np.array_equal(moved[0][i], base[0][i]) for i in range(3, B))     # instance 5 stands: no swing task
     p = hb.HbRolloutParams.from_buffer_copy(bytes(prm))
     p.gains.kp_big_stance = 48.0
-    moved = _run(ctx, rbd0, p, None)
+    moved = logged_episode(ctx, rbd0, p, None)
     assert_episode_equal(moved, base, rows_a=slice(0, 3), rows_b=slice(0, 3))
     assert any(not np.array_equal(moved[0][i], base[0][i]) for i in range(3, B))
     ctx.close()
@@ -190,7 +165,7 @@ def test_other_calls_ignore_the_setting(wbc):
     x_ref, swing, cmode = (np.stack([r[j] for r in refs]) for j in range(3))
     rbd_cs = sc.consistent_rbd(x0)
     runs = []
-    for setting in (None, _array(_records() * 2)):
+    for setting in (None, array_of(_records() * 2)):
         ctx.set_controller_settings(setting)
         loop = stepwise(ctx, rbd0, GAITS, vels, 30, prm, 10)
         x = np.tile(sc.INITIAL_STATE, (B, 1)); u = np.zeros((B, hb.NU)); u[:, 2:12:3] = 9.81 * 2

@@ -1,8 +1,8 @@
-"""Goals (hb_rollout_set_goals) and explicit planner targets (hb_plan_set_targets) on the device. The device planner on explicit targets
-is checked against the host planner on the same targets; the goal episode bit for bit against the loop of public calls (hb_goal_to_target
-on the MPC tick a goal comes into force, hb_plan_set_targets, hb_resident_plan_cycle_batch), under both WBC formulations, truth and
-estimator, both time grids, together with pushes, plant variations and terrains; then the setting's contract (continuation across a split
-between a goal's time and its capture, independence, permutation, instances beyond the setting, re-capture on a new setting, zero-goal
+"""Goals (hb_rollout_set_goals) and explicit planner targets (hb_plan_set_targets) on the device. The device planner on explicit targets is
+checked against the host planner on the same targets; the goal episode bit for bit against the loop of public calls (episode_ref.stepwise:
+hb_goal_to_target on the MPC tick a goal comes into force, hb_plan_set_targets, hb_resident_plan_cycle_batch), under both WBC formulations,
+truth and estimator, both time grids, together with pushes, plant variations and terrains; then the setting's contract (continuation across a
+split between a goal's time and its capture, independence, permutation, instances beyond the setting, re-capture on a new setting, zero-goal
 schedules, launch counts, argument checks) and one closed-loop property of trotting robots sent to goals."""
 import ctypes as C
 
@@ -11,8 +11,9 @@ import pytest
 
 import hunter_bipedal_control_b200 as hb
 from hunter_bipedal_control_b200 import scenarios as sc
-from episode_ref import (GAITS, assert_continues, assert_episode_equal, assert_null_settings, assert_rejected_settings, assert_setting_episodes,
-                         cmd_vels, context, device, est_params, launch_coefficients, outputs, params, start_states, stepwise)
+from episode_ref import (FRICTION, GAITS, PUSH, assert_continues, assert_episode_equal, assert_null_settings, assert_rejected_settings,
+                         assert_setting_episodes, cmd_vels, context, device, est_params, launch_coefficients, outputs, params, random_goals, start_states,
+                         stepwise, use)
 
 pytestmark = pytest.mark.gpu
 
@@ -103,66 +104,6 @@ def test_the_cmd_vel_target_given_back_is_the_cmd_vel_plan_on_the_device():
 
 
 # ---------------------------------------------------------------------------------------------------------------- the goal episode
-class GoalLoop:
-    """A context whose resident_plan_cycle restates the goal capture of the episodes with public calls, for episode_ref.stepwise: on every
-    MPC cycle the goal in force at t is converted by hb_goal_to_target on the cycle's x0 when it differs from the captured one (a cold
-    cycle forgets the captured goals first), every instance gets its target through hb_plan_set_targets (the captured one, or its cmd_vel
-    target as the device planner builds it), then hb_resident_plan_cycle_batch runs. Everything else is the context's."""
-
-    def __init__(self, ctx, goals):
-        self._ctx, self._goals = ctx, goals
-        self._captured = {}
-
-    def __getattr__(self, name):
-        return getattr(self._ctx, name)
-
-    def resident_plan_cycle(self, cold_start, t_rel, ins, rbd):
-        ctx, B = self._ctx, len(ins)
-        if cold_start:
-            self._captured = {}
-        t = ins[0].t0
-        two = (hb.HbPlanInput * B)(*ins)
-        for p in two:
-            p.joint_ik = 0
-        ctx.set_plan_targets(None)
-        plain, _, st = ctx.plan_references_gpu(two, np.zeros((B, 12)))
-        assert (st == 0).all()
-        targets = [hb.reference_target(r) for r in plain]
-        for i in range(min(B, len(self._goals))):
-            s = self._goals[i]
-            g = max([j for j in range(s.n_goal) if s.time[j] <= t], default=-1)
-            if g >= 0 and self._captured.get(i, (-1,))[0] != g:
-                self._captured[i] = (g, hb.goal_to_target(t, np.array(ins[i].x0[:])[None], np.array(s.goal[g][:]))[0])
-            if i in self._captured:
-                targets[i] = self._captured[i][1]
-        ctx.set_plan_targets((hb.HbTarget * B)(*targets))
-        return ctx.resident_plan_cycle(cold_start, t_rel, ins, rbd)
-
-
-def _goals(rbd0, B, seed):
-    """Goal schedules of the first B - 1 of the robots: a goal 0.15-0.4 m away in a random direction given between two MPC ticks, a second
-    one later for every other robot, and the goal at the start pose from the start for the robot at index 2."""
-    rng = np.random.default_rng(seed)
-    n = B - 1
-    d = rng.uniform(0.15, 0.4, n); th = rng.uniform(-np.pi, np.pi, n)
-    g1 = np.c_[rbd0[:n, 3] + d * np.cos(th), rbd0[:n, 4] + d * np.sin(th), rbd0[:n, 0] + rng.uniform(-0.6, 0.6, n)]
-    g2 = g1 + np.c_[rng.uniform(-0.2, 0.2, (n, 2)), rng.uniform(-0.3, 0.3, n)]
-    times = np.c_[np.full(n, 0.053), np.where(np.arange(n) % 2, 0.21, 1e9)]
-    s = hb.make_goal_schedules(n, times, np.stack([g1, g2], axis=1))
-    s[2].n_goal = 1; s[2].time[0] = 0.0
-    s[2].goal[0][0], s[2].goal[0][1], s[2].goal[0][2] = rbd0[2, 3], rbd0[2, 4], rbd0[2, 0]
-    return s
-
-
-def _terrains_and_more(ctx, rbd0, B):
-    """Terrains (a 1 cm step), plant variations and pushes set on ctx, returned as stepwise's keyword arguments."""
-    kw = dict(terrains=hb.make_terrains(B, np.where(np.arange(8)[None, :, None] > 4, 0.03, 0.02) * np.ones((B, 8, 8)), 0.1, rbd0[:, 3:5] - 0.35),
-              variations=hb.make_plant_variations(B, friction_scale=[1.0, 0.8, 1.0, 0.6, 1.0, 0.9]),
-              pushes=hb.make_push_schedules(B, 0.15, 0.05, [[25.0, -15.0, 0.0]]))
-    ctx.set_terrains(kw["terrains"]); ctx.set_plant_variations(kw["variations"]); ctx.set_pushes(kw["pushes"])
-    return kw
-
-
 @pytest.mark.parametrize("wbc", ["weighted", "hierarchical"])
 @pytest.mark.parametrize("event_nodes", [False, True], ids=["uniform", "event_nodes"])
 @pytest.mark.parametrize("estimated", [False, True], ids=["truth", "estimator"])
@@ -174,12 +115,14 @@ def test_goal_episode_equals_the_stepwise_loop_bitwise(wbc, event_nodes, estimat
     rbd0 = start_states(ctx, B, seed=71)
     vels = cmd_vels(B)
     prm = params(log_every)
-    goals = _goals(rbd0, B, 71)
-    ctx.set_goals(goals)
-    extra = _terrains_and_more(ctx, rbd0, B) if wbc == "weighted" and not event_nodes else {}        # goals with the other settings
+    extra = {}
+    if wbc == "weighted" and not event_nodes:         # goals with terrains (a 1 cm step), plant variations and pushes
+        extra = dict(terrains=hb.make_terrains(B, np.where(np.arange(8)[None, :, None] > 4, 0.03, 0.02) * np.ones((B, 8, 8)), 0.1, rbd0[:, 3:5] - 0.35),
+                     plant_variations=hb.make_plant_variations(B, friction_scale=FRICTION), pushes=hb.make_push_schedules(B, 0.15, 0.05, PUSH))
+    kw = use(ctx, goals=random_goals(rbd0, B, 71), **extra)
     ep = est_params(seed=2026) if estimated else None
     d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40) if estimated else None)
-    r = stepwise(GoalLoop(ctx, goals), rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40) if estimated else None, **extra)
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40) if estimated else None, **kw)
     assert_episode_equal(d, r)
     ctx.set_goals(None)
     u = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40) if estimated else None)

@@ -1,30 +1,24 @@
 """Simulated hardware in the episodes (hb_rollout_set_hardware): each robot's actuation delay, torque limits, sensor noise and calibration
 offsets. The host calls with explicit records against numpy (hb_sim_read_sensors_hw, hb_actuation_hw); a record with zero offsets acts on
 its robot exactly as the same values in params / est_params act on an unset episode, under both WBCs, both time grids, truth and
-estimator; an episode with offsets equals the loop of public calls; then the setting's contract and two properties."""
+estimator; an episode with offsets equals the loop of public calls (episode_ref.stepwise); then the setting's contract and two properties."""
 import ctypes as C
 from collections import deque
+from contextlib import contextmanager
 
 import numpy as np
 import pytest
 
 import hunter_bipedal_control_b200 as hb
-from episode_ref import (GAITS, SIGMAS, assert_episode_equal, assert_null_settings, assert_rejected_settings, assert_setting_episodes, cmd_vels,
-                         context, device, est_params, outputs, params, start_states, stepwise)
-from hardware_ref import HardwareLoop, call_hardware, sensors_hw, unclipped
+from episode_ref import (FRICTION, GAITS, PUSH, SIGMAS, array_of, assert_episode_equal, assert_null_settings, assert_records_act_as_their_values,
+                         assert_rejected_settings, assert_setting_episodes, cmd_vels, context, device, est_params, outputs, params, random_goals,
+                         small_terrains, start_states, stepwise, use)
+from hardware_ref import call_hardware, sensors_hw
 
 pytestmark = pytest.mark.gpu
 
 B = 6
 DEFAULT_LIMITS = np.array(hb.default_rollout_params().torque_limit[:])
-
-
-def _array(recs):
-    return (hb.HbHardwareSetting * len(recs))(*recs)
-
-
-def _copy(rec):
-    return hb.HbHardwareSetting.from_buffer_copy(bytes(rec))
 
 
 def _sigmas(scale):
@@ -174,22 +168,18 @@ def test_actuation_without_records_is_the_plain_call_bitwise():
 
 
 # ---------------------------------------------------------------------------------------------------------------- 3. records = call values
-def _run(ctx, rbd0, prm, ep, n_ticks=100, log_every=10):
-    est = hb.estimation_states(B, 50) if ep is not None else None
-    return outputs(device(ctx, rbd0, GAITS, cmd_vels(B), n_ticks, prm, log_every, ep, est))
-
-
-def _with_values(rec, prm, ep):
+@contextmanager
+def _on_the_call(ctx, rec, prm, ep):
     """Copies of prm and ep carrying rec's delay, limits and sigmas."""
     p = hb.HbRolloutParams.from_buffer_copy(bytes(prm))
     p.actuation_delay = rec.actuation_delay
     p.torque_limit[:] = rec.torque_limit[:]
-    if ep is None:
-        return p, None
-    e = hb.HbEstimationParams.from_buffer_copy(bytes(ep))
-    for k in SIGMAS:
-        setattr(e.noise, k, getattr(rec, "sigma_" + k))
-    return p, e
+    e = None
+    if ep is not None:
+        e = hb.HbEstimationParams.from_buffer_copy(bytes(ep))
+        for k in SIGMAS:
+            setattr(e.noise, k, getattr(rec, "sigma_" + k))
+    yield p, e
 
 
 @pytest.mark.parametrize("wbc", ["weighted", "hierarchical"])
@@ -199,19 +189,7 @@ def test_records_equal_the_call_values_bitwise(wbc, event_nodes, estimated):
     ctx = context(event_nodes)
     ctx.set_wbc_formulation(wbc)
     rbd0 = start_states(ctx, B, seed=101)
-    prm = params(10)
-    ep = est_params(seed=2033) if estimated else None
-    recs = _records()
-    ctx.set_hardware(_array([recs[i % 3] for i in range(B)]))
-    got = _run(ctx, rbd0, prm, ep)
-    ctx.set_hardware(None)
-    for k, rec in enumerate(recs):
-        p, e = _with_values(rec, prm, ep)
-        rows = [k, k + 3]
-        assert_episode_equal(got, _run(ctx, rbd0, p, e), rows_a=rows, rows_b=rows)
-    ref = _run(ctx, rbd0, prm, ep)                      # the records really act
-    for i in range(B):
-        assert not np.array_equal(got[0][i], ref[0][i]), i
+    assert_records_act_as_their_values(ctx, "hardware", _records(), _on_the_call, rbd0, params(10), est_params(seed=2033) if estimated else None)
     ctx.close()
 
 
@@ -219,32 +197,23 @@ def test_records_equal_the_call_values_bitwise(wbc, event_nodes, estimated):
 def test_offset_episode_equals_the_stepwise_loop_bitwise():
     """An estimated episode with offsets, delays, limits and sigmas per robot and one robot beyond the setting, with pushes, plant
     variations, a terrain, goals, an MPC latency and controller settings set alongside."""
-    from test_gpu_rollout_goals import GoalLoop, _goals
-    from test_gpu_rollout_latency import LatencyLoop
     ctx = context()
     n_ticks, log_every = 120, 10
     rbd0 = start_states(ctx, B, seed=102)
     vels = cmd_vels(B)
     prm = params(log_every)
-    lat = [0, 2, 5, 1, 0, 3]
-    goals = _goals(rbd0, B, 102)
-    extra = dict(variations=hb.make_plant_variations(B, friction_scale=[1.0, 0.8, 1.0, 0.6, 1.0, 0.9], motor_strength=0.95),
-                 pushes=hb.make_push_schedules(B, 0.15, 0.05, [[25.0, -15.0, 0.0]]),
-                 terrains=hb.make_terrains(3, np.full((3, 2, 2), [[[0.0]], [[0.005]], [[-0.004]]]) + 0.02, 0.5, (-2.0, -2.0)))
-    ctx.set_plant_variations(extra["variations"]); ctx.set_pushes(extra["pushes"]); ctx.set_terrains(extra["terrains"])
-    ctx.set_goals(goals); ctx.set_mpc_latencies(lat)
+    kw = use(ctx, plant_variations=hb.make_plant_variations(B, friction_scale=FRICTION, motor_strength=0.95),
+             pushes=hb.make_push_schedules(B, 0.15, 0.05, PUSH), terrains=small_terrains(), goals=random_goals(rbd0, B, 102),
+             mpc_latencies=[0, 2, 5, 1, 0, 3], hardware=_offsets(B - 1))
     # one controller record for every robot, which the loop of public calls restates as the context's WBC settings and params.gains
     w = ctx.wbc_settings(); w.swing_kp *= 1.2
     g = hb.default_pd_gains(); g.kp_big_stance = 45.0
     ctx.set_controller_settings(hb.make_controller_settings(B, wbc=w, gains=g))
-    hw = _offsets(B - 1)
-    ctx.set_hardware(hw)
     ep = est_params(seed=2034)
     d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 70))
     ctx.set_wbc_settings(w)
-    p = unclipped(prm); p.gains = g
-    loop = HardwareLoop(GoalLoop(LatencyLoop(ctx, lat, p), goals), hw, prm, ep)
-    r = stepwise(loop, rbd0, GAITS, vels, n_ticks, p, log_every, ep, hb.estimation_states(B, 70), **extra)
+    prm.gains = g
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 70), **kw)
     assert_episode_equal(d, r)
     ctx.close()
 
@@ -260,15 +229,15 @@ def test_null_settings(wbc, estimated):
     rbd0 = start_states(ctx, B, seed=103)
     prm = params(5)
     ep = est_params(seed=9) if estimated else None
-    call = _array([call_hardware(prm, ep)] * B)
-    nulls = [call, _array([call_hardware(prm, ep)] * 3)]
+    call = array_of([call_hardware(prm, ep)] * B)
+    nulls = [call, array_of([call_hardware(prm, ep)] * 3)]
     if not estimated:
         nulls += [hb.make_hardware_settings(B), _offsets(B)]
         for r in nulls[-1]:
             r.actuation_delay = prm.actuation_delay
             r.torque_limit[:] = prm.torque_limit[:]
     assert_null_settings(ctx, "hardware", lambda: device(ctx, rbd0, GAITS, cmd_vels(B), 60, prm, 5, ep, hb.estimation_states(B, 50) if estimated else None),
-                         nulls, _array(_records() * 2))
+                         nulls, array_of(_records() * 2))
     ctx.close()
 
 
@@ -277,13 +246,13 @@ def test_setting_contract():
     ctx = context()
     rbd0 = start_states(ctx, B, seed=104)
     r = _records()
-    full = _array([r[0], r[1], r[2], r[1], r[0], r[2]])
+    full = array_of([r[0], r[1], r[2], r[1], r[0], r[2]])
     one = hb.make_hardware_settings(B)
-    one[0] = _copy(r[0])
-    other = _array([r[2], r[0], r[1], r[1], r[2], r[0]])       # instance 3 keeps its record
-    part = _array([r[1], r[2]])
+    one[0] = r[0]
+    other = array_of([r[2], r[0], r[1], r[1], r[2], r[0]])       # instance 3 keeps its record
+    part = array_of([r[1], r[2]])
     padded = hb.make_hardware_settings(B)
-    padded[0], padded[1] = _copy(r[1]), _copy(r[2])
+    padded[0], padded[1] = r[1], r[2]
     assert_setting_episodes(ctx, "hardware", rbd0, params(10), full, one, other, 3, part, padded)
     ctx.close()
 
@@ -311,7 +280,7 @@ def test_rejected_settings(estimated):
     ep = est_params(seed=10) if estimated else None
     assert_rejected_settings(ctx, "hardware",
                              lambda: device(ctx, rbd0, GAITS, cmd_vels(B), 40, params(5), 5, ep, hb.estimation_states(B, 50) if estimated else None),
-                             _array(_records() * 2), _bad(), hb.make_hardware_settings(ctx.max_batch + 1))
+                             array_of(_records() * 2), _bad(), hb.make_hardware_settings(ctx.max_batch + 1))
     # the host calls validate their records as the setter does
     rbd = _random_rbd(2, 1)
     for bad in _bad():

@@ -1,17 +1,18 @@
-"""MPC latency in the batched episodes (hb_rollout_set_mpc_latencies) and the MRT split behind it (hb_policy_update, hb_policy_wbc). The
-latency episode is checked bit for bit against the loop of public calls (the adoptions through hb_policy_update, the 500 Hz tick through
-hb_policy_wbc), with latencies 0, 1, 2, mpc_every - 1 and mpc_every and one instance beyond the setting, under both WBC formulations, truth
-and estimator, both time grids, and together with pushes and plant variations; then the setting's contract (null settings, continuation
-across a split between a cycle and its adoption, independence, permutation, instances beyond the setting, launch counts, argument checks)
-and the MRT entry points on their own (adoption, the mask, the held policy, the shared WBC fallback)."""
+"""MPC latency in the batched episodes (hb_rollout_set_mpc_latencies) and the MRT split behind it (hb_policy_update, hb_policy_wbc). The latency
+episode is checked bit for bit against the loop of public calls (episode_ref.stepwise: the adoptions through hb_policy_update, the 500 Hz tick
+through hb_policy_wbc), with latencies 0, 1, 2, mpc_every - 1 and mpc_every and one instance beyond the setting, under both WBC formulations,
+truth and estimator, both time grids, and together with pushes and plant variations; then the setting's contract (null settings, continuation
+across a split between a cycle and its adoption, independence, permutation, instances beyond the setting, launch counts, argument checks) and
+the MRT entry points on their own (adoption, the mask, the held policy, the shared WBC fallback)."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
 import hunter_bipedal_control_b200 as hb
-from episode_ref import (GAITS, GAIT_START, assert_continues, assert_episode_equal, assert_null_settings, assert_rejected_settings,
-                         assert_setting_episodes, cmd_vels, context, device, est_params, horizon, outputs, params, start_states, stepwise)
+from episode_ref import (FRICTION, GAITS, GAIT_START, PUSH, assert_continues, assert_episode_equal, assert_null_settings, assert_rejected_settings,
+                         assert_setting_episodes, cmd_vels, context, device, est_params, horizon, latency_due, outputs, params, start_states, stepwise,
+                         use)
 
 pytestmark = pytest.mark.gpu
 
@@ -19,53 +20,9 @@ EVERY = 5                                   # params()'s mpc_every (hb_default_r
 LATENCIES = [0, 1, 2, EVERY - 1, EVERY]                              # six robots: the sixth is beyond the setting
 
 
-class LatencyLoop:
-    """A context whose resident_plan_cycle and resident_wbc restate the MRT split of the episodes with public calls, for episode_ref.stepwise.
-    The cycle: the instances whose solution comes into force on this tick adopt (hb_policy_update with their flags), hb_resident_plan_cycle_batch
-    runs, and on the cold tick every instance with a latency adopts after it. The 500 Hz tick: on a tick without a cycle the instances due
-    adopt; the instances with latency 0 adopt the resident solution on every tick (so that their adopted policy is the resident one); then
-    hb_policy_wbc. Everything else is the context's. The public cycle runs its own WBC on the new solution, which the episodes do not, so the
-    loop equals the episode while no WBC falls back."""
-
-    def __init__(self, ctx, latencies, prm):
-        self._ctx, self._lat, self._prm = ctx, list(latencies), prm
-
-    def __getattr__(self, name):
-        return getattr(self._ctx, name)
-
-    def _d(self, B):
-        return np.array([self._lat[i] if i < len(self._lat) else 0 for i in range(B)])
-
-    def _due(self, a, B):
-        d = self._d(B)
-        return (d >= 1) & (a >= d) & ((a - d) % self._prm.mpc_every == 0)
-
-    def _tick(self, t):
-        return int(round(t / self._prm.period))
-
-    def resident_plan_cycle(self, cold_start, t_rel, ins, rbd):
-        ctx, B = self._ctx, len(ins)
-        due = self._due(self._tick(ins[0].t0), B)
-        if due.any():
-            ctx.policy_update(B, due)
-        out = ctx.resident_plan_cycle(cold_start, t_rel, ins, rbd)
-        if cold_start and (self._d(B) >= 1).any():
-            ctx.policy_update(B, self._d(B) >= 1)
-        return out
-
-    def resident_wbc(self, t, meas):
-        ctx, B = self._ctx, meas.shape[0]
-        a = self._tick(t)
-        adopt = self._d(B) == 0
-        if a % self._prm.mpc_every:
-            adopt |= self._due(a, B)
-        ctx.policy_update(B, adopt)
-        return ctx.policy_wbc(t, meas)
-
-
 def _due_ticks(latencies, ticks, every):
     """The ticks of `ticks` on which some instance of the setting adopts (one launch each)."""
-    return sum(1 for a in ticks if any(d >= 1 and a >= d and (a - d) % every == 0 for d in latencies))
+    return sum(1 for a in ticks if latency_due(np.array(latencies), a, every).any())
 
 
 @pytest.mark.parametrize("wbc", ["weighted", "hierarchical"])
@@ -79,16 +36,14 @@ def test_latency_episode_equals_the_stepwise_loop_bitwise(wbc, event_nodes, esti
     rbd0 = start_states(ctx, B, seed=81)
     vels = cmd_vels(B)
     prm = params(log_every)
-    ctx.set_mpc_latencies(LATENCIES)
     extra = {}
     if wbc == "weighted" and not event_nodes:         # the latency together with pushes and plant variations
-        extra = dict(variations=hb.make_plant_variations(B, friction_scale=[1.0, 0.8, 1.0, 0.6, 1.0, 0.9], motor_strength=0.95),
-                     pushes=hb.make_push_schedules(B, 0.15, 0.05, [[25.0, -15.0, 0.0]]))
-        ctx.set_plant_variations(extra["variations"]); ctx.set_pushes(extra["pushes"])
+        extra = dict(plant_variations=hb.make_plant_variations(B, friction_scale=FRICTION, motor_strength=0.95),
+                     pushes=hb.make_push_schedules(B, 0.15, 0.05, PUSH))
+    kw = use(ctx, mpc_latencies=LATENCIES, **extra)
     ep = est_params(seed=2027) if estimated else None
     d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 50) if estimated else None)
-    r = stepwise(LatencyLoop(ctx, LATENCIES, prm), rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 50) if estimated else None,
-                 **extra)
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 50) if estimated else None, **kw)
     assert (outputs(d)[3]["wbc_fallbacks"] == 0).all() and (r[3]["wbc_fallbacks"] == 0).all()
     assert_episode_equal(d, r)
     # the latency really delays: the instances with d >= 1 move, latency 0 and the instance beyond the setting do not

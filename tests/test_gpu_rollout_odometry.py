@@ -1,9 +1,10 @@
 """Odometry in the estimated episodes (hb_rollout_set_odometry): a simulated tracking camera per robot whose messages the Kalman filter fuses
-(KalmanFilterEstimate::updateFromTopic). The camera read (hb_sim_read_odometry) is checked against the numpy camera of odometry_ref.py and
-the fusion (hb_estimator_fuse_odometry) against its updateFromTopic; the episode bit for bit against the loop of public calls under both
-WBCs and both time grids, with pushes, plant variations, terrains and an MPC latency alongside; then the setting's contract (null
-settings, launch counts, continuation across a split between a reading and its arrival, independence, permutation, instances beyond the
-setting, clearing, argument checks), the truth episodes that ignore it, and the closed loop it is for: robots reach a goal closer."""
+(KalmanFilterEstimate::updateFromTopic). The camera read (hb_sim_read_odometry) is checked against the numpy camera of odometry_ref.py and the
+fusion (hb_estimator_fuse_odometry) against its updateFromTopic; the episode bit for bit against the loop of public calls
+(episode_ref.stepwise) under both WBCs and both time grids, with pushes, plant variations, terrains and an MPC latency alongside; then the
+setting's contract (null settings, launch counts, continuation across a split between a reading and its arrival, independence, permutation,
+instances beyond the setting, clearing, argument checks), the truth episodes that ignore it, and the closed loop it is for: robots reach a goal
+closer."""
 import ctypes as C
 
 import numpy as np
@@ -11,8 +12,8 @@ import pytest
 
 import hunter_bipedal_control_b200 as hb
 from hunter_bipedal_control_b200 import scenarios as sc
-from episode_ref import (GAITS, assert_continues, assert_episode_equal, assert_null_settings, assert_rejected_settings, cmd_vels, context, device,
-                         est_params, outputs, params, start_states, stepwise)
+from episode_ref import (FRICTION, GAITS, PUSH, assert_continues, assert_episode_equal, assert_null_settings, assert_rejected_settings, cmd_vels,
+                         context, device, est_params, outputs, params, small_terrains, start_states, stepwise, use)
 from odometry_ref import CameraRef, update_from_topic
 
 pytestmark = pytest.mark.gpu
@@ -24,27 +25,6 @@ SIGMA_P, SIGMA_D = [0.0, 0.005, 0.02, 0.005, 0.0, 0.01], [0.0, 0.0, 0.0, 0.001, 
 
 def _settings(n=len(PERIODS)):
     return hb.make_odometry_settings(n, PERIODS[:n], DELAYS[:n], SIGMA_P[:n], SIGMA_D[:n])
-
-
-class OdometryLoop:
-    """A context (or a wrapper of one, LatencyLoop) whose read_sensors and estimator_update restate the odometry of the estimated episodes
-    with public calls, for episode_ref.stepwise: each sensor read is followed by the camera read (hb_sim_read_odometry) of the same tick,
-    each filter update by the fusion of its messages (hb_estimator_fuse_odometry). Everything else is the wrapped object's."""
-
-    def __init__(self, ctx):
-        self._ctx = ctx
-
-    def __getattr__(self, name):
-        return getattr(self._ctx, name)
-
-    def read_sensors(self, rbd, est, tick, noise=None, accel_dt=0.002):
-        out = self._ctx.read_sensors(rbd, est, tick, noise, accel_dt)
-        self._msg = self._ctx.read_odometry(rbd, est, tick, noise)
-        return out
-
-    def estimator_update(self, dt, state, quat, w, a, jp, jv, flags, params=None):
-        rbd = self._ctx.estimator_update(dt, state, quat, w, a, jp, jv, flags, params=params)
-        return self._ctx.fuse_odometry(state, *self._msg, flags, rbd, params=params)
 
 
 def _streams(B, first=0, perm=None):
@@ -171,20 +151,14 @@ def test_odometry_episode_equals_the_stepwise_loop_bitwise(wbc, event_nodes):
     vels = cmd_vels(B)
     gaits = GAITS + ["trot"]
     prm = params(log_every)
-    ctx.set_odometry(_settings())
-    loop, extra = ctx, {}
+    extra = {}
     if wbc == "weighted" and not event_nodes:
-        from test_gpu_rollout_latency import LatencyLoop
-        lat = [0, 2, 5, 1, 0, 3]
-        extra = dict(variations=hb.make_plant_variations(B, friction_scale=[1.0, 0.8, 1.0, 0.6, 1.0, 0.9, 1.0], motor_strength=0.95),
-                     pushes=hb.make_push_schedules(B, 0.15, 0.05, [[25.0, -15.0, 0.0]]),
-                     terrains=hb.make_terrains(3, np.full((3, 2, 2), [[[0.0]], [[0.005]], [[-0.004]]]) + 0.02, 0.5, (-2.0, -2.0)))
-        ctx.set_plant_variations(extra["variations"]); ctx.set_pushes(extra["pushes"]); ctx.set_terrains(extra["terrains"])
-        ctx.set_mpc_latencies(lat)
-        loop = LatencyLoop(ctx, lat, prm)
+        extra = dict(plant_variations=hb.make_plant_variations(B, friction_scale=FRICTION + [1.0], motor_strength=0.95),
+                     pushes=hb.make_push_schedules(B, 0.15, 0.05, PUSH), terrains=small_terrains(), mpc_latencies=[0, 2, 5, 1, 0, 3])
+    kw = use(ctx, odometry=_settings(), **extra)
     ep = est_params(seed=2029)
     d = device(ctx, rbd0, gaits, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 60))
-    r = stepwise(OdometryLoop(loop), rbd0, gaits, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 60), **extra)
+    r = stepwise(ctx, rbd0, gaits, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 60), **kw)
     assert_episode_equal(d, r)
     # the cameras really move the estimate: the instances with one differ from the unset episode, period 0 and the instance beyond do not
     ctx.set_odometry(None)

@@ -10,7 +10,7 @@ import pytest
 import hunter_bipedal_control_b200 as hb
 from hunter_bipedal_control_b200 import scenarios as sc
 from episode_ref import (GAITS, assert_episode_equal, assert_null_settings, assert_rejected_settings, assert_setting_episodes, cmd_vels, context,
-                         device, est_params, launch_coefficients, params, plant_numpy, start_states, stepwise)
+                         device, est_params, launch_coefficients, params, plant_numpy, start_states, stepwise, use)
 from oracle import refs
 
 pytestmark = pytest.mark.gpu
@@ -238,11 +238,9 @@ def test_varied_episode_equals_the_stepwise_loop_bitwise(event_nodes):
     rbd0 = start_states(ctx, B, seed=11)
     vels = cmd_vels(B)
     prm = params(log_every)
-    V = _variations()
-    pushes = hb.make_push_schedules(B, 0.15, 0.05, [[30.0, -20.0, 0.0]])
-    ctx.set_plant_variations(V); ctx.set_pushes(pushes)
+    kw = use(ctx, plant_variations=_variations(), pushes=hb.make_push_schedules(B, 0.15, 0.05, [[30.0, -20.0, 0.0]]))
     d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
-    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, pushes=pushes, variations=V)
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, **kw)
     assert_episode_equal(d, r)
     ctx.set_plant_variations(None)
     u = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
@@ -258,11 +256,9 @@ def test_varied_estimated_episode_equals_the_stepwise_loop_bitwise():
     vels = cmd_vels(B)
     prm = params(log_every)
     ep = est_params(seed=2024)
-    V = _variations()
-    pushes = hb.make_push_schedules(B, 0.1, 0.04, [[0.0, 40.0, 0.0]])
-    ctx.set_plant_variations(V); ctx.set_pushes(pushes)
+    kw = use(ctx, plant_variations=_variations(), pushes=hb.make_push_schedules(B, 0.1, 0.04, [[0.0, 40.0, 0.0]]))
     d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40))
-    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40), pushes=pushes, variations=V)
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40), **kw)
     assert_episode_equal(d, r)
     ctx.close()
 

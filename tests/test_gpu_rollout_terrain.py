@@ -11,8 +11,9 @@ import pytest
 
 import hunter_bipedal_control_b200 as hb
 from hunter_bipedal_control_b200 import scenarios as sc
-from episode_ref import (GAITS, GROUND, assert_episode_equal, assert_null_settings, assert_rejected_settings, assert_setting_episodes, cmd_vels,
-                         context, device, est_params, launch_coefficients, outputs, params, plant_numpy, start_states, stepwise, terrain_height)
+from episode_ref import (FRICTION, GAITS, GROUND, PUSH, assert_episode_equal, assert_null_settings, assert_rejected_settings, assert_setting_episodes,
+                         cmd_vels, context, device, est_params, launch_coefficients, outputs, params, plant_numpy, start_states, stepwise, terrain_height,
+                         use)
 
 pytestmark = pytest.mark.gpu
 
@@ -305,12 +306,11 @@ def test_terrain_episode_equals_the_stepwise_loop_bitwise(event_nodes):
     rbd0 = start_states(ctx, B, seed=51)
     vels = cmd_vels(B)
     prm = params(log_every)
-    T = _profile_terrains(rbd0, PROFILES, np.random.default_rng(51))
-    V = hb.make_plant_variations(B, friction_scale=[1.0, 0.8, 1.0, 0.6, 1.0, 0.9], stiffness_scale=[1.0, 1.0, 1.3, 1.0, 0.8, 1.0])
-    pushes = hb.make_push_schedules(B, 0.15, 0.05, [[25.0, -15.0, 0.0]])
-    ctx.set_terrains(T); ctx.set_plant_variations(V); ctx.set_pushes(pushes)
+    kw = use(ctx, terrains=_profile_terrains(rbd0, PROFILES, np.random.default_rng(51)),
+             plant_variations=hb.make_plant_variations(B, friction_scale=FRICTION, stiffness_scale=[1.0, 1.0, 1.3, 1.0, 0.8, 1.0]),
+             pushes=hb.make_push_schedules(B, 0.15, 0.05, PUSH))
     d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
-    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, pushes=pushes, variations=V, terrains=T)
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, **kw)
     assert_episode_equal(d, r)
     ctx.set_terrains(None)
     u = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every)
@@ -326,12 +326,11 @@ def test_terrain_estimated_episode_equals_the_stepwise_loop_bitwise():
     vels = cmd_vels(B)
     prm = params(log_every)
     ep = est_params(seed=2025)
-    T = _profile_terrains(rbd0, PROFILES, np.random.default_rng(52))
-    V = hb.make_plant_variations(B, 1.5, [0.0, 0.0, 0.1], np.diag([0.01, 0.01, 0.01]))
-    pushes = hb.make_push_schedules(B, 0.1, 0.04, [[0.0, 30.0, 0.0]])
-    ctx.set_terrains(T); ctx.set_plant_variations(V); ctx.set_pushes(pushes)
+    kw = use(ctx, terrains=_profile_terrains(rbd0, PROFILES, np.random.default_rng(52)),
+             plant_variations=hb.make_plant_variations(B, 1.5, [0.0, 0.0, 0.1], np.diag([0.01, 0.01, 0.01])),
+             pushes=hb.make_push_schedules(B, 0.1, 0.04, [[0.0, 30.0, 0.0]]))
     d = device(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40))
-    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40), pushes=pushes, variations=V, terrains=T)
+    r = stepwise(ctx, rbd0, GAITS, vels, n_ticks, prm, log_every, ep, hb.estimation_states(B, 40), **kw)
     assert_episode_equal(d, r)
     ctx.close()
 
