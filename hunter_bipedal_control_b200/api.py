@@ -19,6 +19,9 @@ _lib = None
 NX, NU, NQ, NJ, NWBC = 22, 22, 16, 10, 38
 HB_MAX_EVENTS, HB_MAX_TARGETS, HB_MAX_SEGMENTS = 32, 16, 24
 HB_MAX_HORIZON = 512       # longest horizon_N hb_create accepts
+# hb_check_setting_records' kinds: the record type of each per-robot setting call
+HB_SETTING_PUSHES, HB_SETTING_PLANT_VARIATIONS, HB_SETTING_TERRAINS, HB_SETTING_GOALS, HB_SETTING_ODOMETRY = 0, 1, 2, 3, 4
+HB_SETTING_CONTROLLERS, HB_SETTING_HARDWARE, HB_SETTING_PLANNER, HB_SETTING_TARGETS, HB_SETTING_LATENCIES = 5, 6, 7, 8, 9
 
 EXPORTED_SYMBOLS = [
     "hb_shard_partition", "hb_shard_sort_by_schedule", "hb_shard_unique_id", "hb_shard_create", "hb_shard_destroy", "hb_shard_block", "hb_shard_gather_dev", "hb_shard_wait", "hb_shard_last_error",
@@ -47,6 +50,7 @@ EXPORTED_SYMBOLS = [
     "hb_rollout_set_controller_settings",
     "hb_default_hardware_setting", "hb_rollout_set_hardware", "hb_actuation_hw", "hb_sim_read_sensors_hw",
     "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
+    "hb_check_setting_records",
 ]
 
 
@@ -359,7 +363,8 @@ class HbPushSchedule(C.Structure):
 def make_push_schedules(B, t_start, duration, force, torque=None):
     """ctypes array of B HbPushSchedule (Context.set_pushes). Push j of instance i acts on the plant steps of the ticks with
     t_start[i, j] <= t < t_start[i, j] + duration[i, j]: a world force[i, j] [N] at the base origin plus a world couple torque[i, j] [N m]
-    (None: zero). t_start / duration: (B, n), (n,) or scalars; force / torque: (B, n, 3), (n, 3) or (3,); n <= HB_MAX_PUSHES."""
+    (None: zero). t_start / duration: (B, n), (n,) or scalars; force / torque: (B, n, 3), (n, 3) or (3,); n <= HB_MAX_PUSHES. Raises
+    ValueError for a shape that does not broadcast and for a record hb_rollout_set_pushes rejects (its own check)."""
     tim, dur, frc = _f64(t_start), _f64(duration), _f64(force)
     trq = np.zeros(3) if torque is None else _f64(torque)
     dims = [a.shape[-1] for a in (tim, dur) if a.ndim >= 1] + [a.shape[-2] for a in (frc, trq) if a.ndim >= 2]
@@ -371,15 +376,11 @@ def make_push_schedules(B, t_start, duration, force, torque=None):
         frc = np.broadcast_to(frc, (B, n, 3)); trq = np.broadcast_to(trq, (B, n, 3))
     except ValueError as e:
         raise ValueError("push schedules: t_start / duration (B, n), force / torque (B, n, 3) expected: %s" % e)
-    if not (np.isfinite(tim).all() and np.isfinite(frc).all() and np.isfinite(trq).all()):
-        raise ValueError("push schedules: t_start, force and torque must be finite")
-    if not (np.isfinite(dur).all() and (dur >= 0).all()):
-        raise ValueError("push schedules: durations must be finite and >= 0")
     out = (HbPushSchedule * B)()
     v = np.ctypeslib.as_array(out)
     v["n_push"] = n
     v["t_start"][:, :n] = tim; v["duration"][:, :n] = dur; v["force"][:, :n] = frc; v["torque"][:, :n] = trq
-    return out
+    return _check_records(HB_SETTING_PUSHES, out, "pushes")
 
 
 class HbPlantVariation(C.Structure):
@@ -394,24 +395,15 @@ def default_plant_variation():
     return v
 
 
-def _psd_by_minors(I):
-    """Sylvester's criterion for semidefiniteness of the symmetric 3 x 3 matrices I (..., 3, 3): no negative principal minor."""
-    d = [I[..., 0, 0], I[..., 1, 1], I[..., 2, 2],
-         I[..., 0, 0] * I[..., 1, 1] - I[..., 0, 1] * I[..., 1, 0], I[..., 0, 0] * I[..., 2, 2] - I[..., 0, 2] * I[..., 2, 0],
-         I[..., 1, 1] * I[..., 2, 2] - I[..., 1, 2] * I[..., 2, 1],
-         I[..., 0, 0] * (I[..., 1, 1] * I[..., 2, 2] - I[..., 1, 2] * I[..., 2, 1]) - I[..., 0, 1] * (I[..., 1, 0] * I[..., 2, 2] - I[..., 1, 2] * I[..., 2, 0])
-         + I[..., 0, 2] * (I[..., 1, 0] * I[..., 2, 1] - I[..., 1, 1] * I[..., 2, 0])]
-    return np.all([m >= 0 for m in d], axis=0)
-
-
 def make_plant_variations(B, payload_mass=0.0, payload_com=(0.0, 0.0, 0.0), payload_inertia=None, friction_scale=1.0, stiffness_scale=1.0,
                           damping_scale=1.0, motor_strength=1.0):
     """ctypes array of B HbPlantVariation (Context.set_plant_variations, Context.sim_step). Instance i carries a payload of payload_mass[i]
     [kg] with its CoM at payload_com[i] (base frame, from the base origin) and inertia payload_inertia[i] (3 x 3 about the CoM, base frame;
     None: zero), on ground of friction_scale[i] * mu, stiffness_scale[i] * k and damping_scale[i] * d, with motor_strength[i, j] scaling the
     torque of joint j. Scalars and per-instance arrays broadcast: masses and scales () or (B,), payload_com (3,) or (B, 3), payload_inertia
-    (3, 3) or (B, 3, 3), motor_strength (), (10,) or (B, 10) (per instance only: (B, 1)). Raises ValueError for what
-    hb_rollout_set_plant_variations rejects. The defaults give the nominal plant."""
+    (3, 3) or (B, 3, 3), motor_strength (), (10,) or (B, 10) (per instance only: (B, 1)). Raises ValueError for a
+    shape that does not broadcast and for a record hb_rollout_set_plant_variations rejects (its own check). The defaults give the nominal
+    plant."""
     try:
         m = np.broadcast_to(_f64(payload_mass), (B,)); c = np.broadcast_to(_f64(payload_com), (B, 3))
         I = np.broadcast_to(np.zeros((3, 3)) if payload_inertia is None else _f64(payload_inertia), (B, 3, 3))
@@ -420,20 +412,11 @@ def make_plant_variations(B, payload_mass=0.0, payload_com=(0.0, 0.0, 0.0), payl
     except ValueError as e:
         raise ValueError("plant variations: masses / scales (B,), payload_com (B, 3), payload_inertia (B, 3, 3), motor_strength (B, 10) expected: %s"
                          % e)
-    if not all(np.isfinite(a).all() for a in (m, c, I, fs, ks, ds, ms)):
-        raise ValueError("plant variations: every value must be finite")
-    if not ((m >= 0).all() and (fs >= 0).all() and (ks > 0).all() and (ds >= 0).all() and (ms >= 0).all()):
-        raise ValueError("plant variations: payload_mass, friction_scale, damping_scale and motor_strength must be >= 0, stiffness_scale > 0")
-    if not (np.array_equal(I, np.swapaxes(I, 1, 2)) and _psd_by_minors(I).all()):
-        raise ValueError("plant variations: payload_inertia must be exactly symmetric and positive semidefinite")
-    none = m == 0
-    if (c[none] != 0).any() or (I[none] != 0).any():
-        raise ValueError("plant variations: a zero payload_mass needs a zero payload_com and payload_inertia")
     out = (HbPlantVariation * B)()
     v = np.ctypeslib.as_array(out)
     v["payload_mass"] = m; v["payload_com"] = c; v["payload_inertia"] = I.reshape(B, 9)
     v["friction_scale"] = fs; v["stiffness_scale"] = ks; v["damping_scale"] = ds; v["motor_strength"] = ms
-    return out
+    return _check_records(HB_SETTING_PLANT_VARIATIONS, out, "plant_variations")
 
 
 HB_TERRAIN_MAX = 64
@@ -448,7 +431,8 @@ def make_terrains(B, heights, spacing, origin=(0.0, 0.0)):
     """ctypes array of B HbTerrain (Context.set_terrains, Context.sim_step). Instance i stands on the height field heights[i] (ny x nx,
     2..HB_TERRAIN_MAX each): heights[i][j, k] is the ground z at world (origin[i][0] + k spacing[i], origin[i][1] + j spacing[i]),
     interpolated bilinearly between the samples and continued flat beyond the grid's edges. heights (ny, nx) or (B, ny, nx), spacing () or
-    (B,), origin (2,) or (B, 2). Raises ValueError for what hb_rollout_set_terrains rejects."""
+    (B,), origin (2,) or (B, 2). Raises ValueError for a shape that does not broadcast and for a record hb_rollout_set_terrains rejects
+    (its own check)."""
     h = _f64(heights)
     if h.ndim not in (2, 3):
         raise ValueError("terrains: heights (ny, nx) or (B, ny, nx) expected, got shape %s" % (h.shape,))
@@ -459,15 +443,11 @@ def make_terrains(B, heights, spacing, origin=(0.0, 0.0)):
         h = np.broadcast_to(h, (B, ny, nx)); s = np.broadcast_to(_f64(spacing), (B,)); o = np.broadcast_to(_f64(origin), (B, 2))
     except ValueError as e:
         raise ValueError("terrains: heights (B, ny, nx), spacing (B,), origin (B, 2) expected: %s" % e)
-    if not (np.isfinite(h).all() and np.isfinite(o).all()):
-        raise ValueError("terrains: heights and origins must be finite")
-    if not (np.isfinite(s).all() and (s > 0).all()):
-        raise ValueError("terrains: spacings must be finite and > 0")
     out = (HbTerrain * B)()
     v = np.ctypeslib.as_array(out)
     v["nx"] = nx; v["ny"] = ny; v["origin"] = o; v["spacing"] = s
     v["height"][:, :ny, :nx] = h
-    return out
+    return _check_records(HB_SETTING_TERRAINS, out, "terrains")
 
 
 HB_MAX_GOALS = 8
@@ -480,7 +460,8 @@ class HbGoalSchedule(C.Structure):
 def make_goal_schedules(B, times, goals):
     """ctypes array of B HbGoalSchedule (Context.set_goals). Goal j of instance i, the world pose goals[i, j] = (x, y, yaw), comes into
     force on the first MPC tick with t >= times[i, j]. times: (B, n), (n,) or a scalar, ascending; goals: (B, n, 3), (n, 3) or (3,);
-    n <= HB_MAX_GOALS (n = 0: no goals). Raises ValueError for what hb_rollout_set_goals rejects."""
+    n <= HB_MAX_GOALS (n = 0: no goals). Raises ValueError for a shape that does not broadcast and for a record hb_rollout_set_goals
+    rejects (its own check)."""
     tim, gol = _f64(times), _f64(goals)
     dims = [tim.shape[-1]] if tim.ndim >= 1 else []
     dims += [gol.shape[-2]] if gol.ndim >= 2 else []
@@ -491,15 +472,11 @@ def make_goal_schedules(B, times, goals):
         tim = np.broadcast_to(tim, (B, n)); gol = np.broadcast_to(gol, (B, n, 3))
     except ValueError as e:
         raise ValueError("goal schedules: times (B, n), goals (B, n, 3) expected: %s" % e)
-    if not (np.isfinite(tim).all() and np.isfinite(gol).all()):
-        raise ValueError("goal schedules: times and goals must be finite")
-    if (np.diff(tim, axis=1) < 0).any():
-        raise ValueError("goal schedules: times must be ascending")
     out = (HbGoalSchedule * B)()
     v = np.ctypeslib.as_array(out)
     v["n_goal"] = n
     v["time"][:, :n] = tim; v["goal"][:, :n] = gol
-    return out
+    return _check_records(HB_SETTING_GOALS, out, "goals")
 
 
 class HbObserverState(C.Structure):
@@ -641,22 +618,21 @@ def make_odometry_settings(B, period_ticks, delay_ticks=0, sigma_position=0.0, s
     """ctypes array of B HbOdometrySetting (Context.set_odometry): the tracking camera of each robot of the estimated episodes, a message
     every period_ticks ticks (0: no camera) carrying the base position of delay_ticks ticks earlier (0..HB_ODOM_MAX_DELAY), with white noise
     sigma_position [m] and a bias whose random-walk increment per message is sigma_drift [m]. Each argument: (B,) or a scalar. Raises
-    ValueError for what hb_rollout_set_odometry rejects."""
+    ValueError for a shape that does not broadcast, a tick count that is not an int32 integer and a record hb_rollout_set_odometry rejects
+    (its own check)."""
     try:
         per, dly = (np.broadcast_to(np.asarray(a), (B,)) for a in (period_ticks, delay_ticks))
         sp, sd = (np.broadcast_to(_f64(a), (B,)) for a in (sigma_position, sigma_drift))
     except ValueError as e:
         raise ValueError("odometry settings: (B,) or scalars expected: %s" % e)
-    if not (np.array_equal(per, np.rint(per)) and np.array_equal(dly, np.rint(dly))):
-        raise ValueError("odometry settings: period_ticks and delay_ticks must be integers")
-    if (per < 0).any() or (dly < 0).any() or (dly > HB_ODOM_MAX_DELAY).any():
-        raise ValueError("odometry settings: period_ticks >= 0 and 0 <= delay_ticks <= %d expected" % HB_ODOM_MAX_DELAY)
-    if not (np.isfinite(sp).all() and np.isfinite(sd).all() and (sp >= 0).all() and (sd >= 0).all()):
-        raise ValueError("odometry settings: the sigmas must be finite and >= 0")
     out = (HbOdometrySetting * B)()
     v = np.ctypeslib.as_array(out)
-    v["period_ticks"] = per; v["delay_ticks"] = dly; v["sigma_position"] = sp; v["sigma_drift"] = sd
-    return out
+    with np.errstate(invalid="ignore"):                 # a NaN or out-of-range tick count casts to garbage, rejected below
+        v["period_ticks"] = per; v["delay_ticks"] = dly
+    if not (np.array_equal(v["period_ticks"], per) and np.array_equal(v["delay_ticks"], dly)):
+        raise ValueError("odometry settings: period_ticks and delay_ticks must be int32 integers")
+    v["sigma_position"] = sp; v["sigma_drift"] = sd
+    return _check_records(HB_SETTING_ODOMETRY, out, "odometry")
 
 
 class HbGaitSelector(C.Structure):
@@ -784,6 +760,14 @@ def _ptr(a):
 
 def _f64(a):
     return np.ascontiguousarray(a, dtype=np.float64)
+
+
+def _check_records(kind, records, setting):
+    """records, or ValueError naming the first that hb_rollout_set_<setting> rejects (hb_check_setting_records, its own check)."""
+    bad = C.c_int32()
+    if load_library().hb_check_setting_records(kind, len(records), records, C.byref(bad)) != 0:
+        raise ValueError("%s: record %d is rejected by hb_rollout_set_%s" % (setting, bad.value, setting))
+    return records
 
 
 def _check_hardware(what, hardware, B):

@@ -178,10 +178,14 @@ template <class F = bool (*)()> int enter(hb_ctx* ctx, int B, bool args, Cap cap
     if (rc__) return rc__ == EMPTY ? HB_OK : rc__;                   \
   } while (0)
 
-// true when every one of the B records passes ok (a null array holds none)
-template <class T> bool all_ok(int B, const T* src, bool (*ok)(const T&)) {
-  if (src) for (int i = 0; i < B; ++i) if (!ok(src[i])) return false;
+// true when every one of the B records passes ok (a null array holds none); otherwise false, with the index of the first that fails in *bad
+template <class T> bool all_ok(int B, const T* src, bool (*ok)(const T&), int32_t* bad = nullptr) {
+  if (src) for (int i = 0; i < B; ++i) if (!ok(src[i])) { if (bad) *bad = i; return false; }
   return true;
+}
+// The body of hb_check_setting_records for the records of one type, judged by the predicate their setter passes to set_instances
+template <class T> int check_records(int B, const void* records, bool (*ok)(const T&), int32_t* first_bad) {
+  return all_ok(B, static_cast<const T*>(records), ok, first_bad) ? HB_OK : HB_EINVAL;
 }
 
 // The body of the per-robot setting calls (hunter_b200.h, "per-robot episode settings"): the records are validated on the host, B == 0
@@ -1235,6 +1239,25 @@ static bool controller_setting_ok(const hb_controller_setting& s) {
 
 int hb_rollout_set_controller_settings(hb_ctx* ctx, int B, const hb_controller_setting* s) {
   return set_instances(ctx, B, s, controller_setting_ok, &hb_ctx::controllers);
+}
+
+int hb_check_setting_records(int32_t kind, int B, const void* records, int32_t* first_bad) {
+  if (!first_bad) return HB_EINVAL;
+  *first_bad = -1;
+  if (B < 0 || (B > 0 && !records)) return HB_EINVAL;
+  switch (kind) {
+    case HB_SETTING_PUSHES: return check_records(B, records, push_schedule_ok, first_bad);
+    case HB_SETTING_PLANT_VARIATIONS: return check_records(B, records, plant_variation_ok, first_bad);
+    case HB_SETTING_TERRAINS: return check_records(B, records, terrain_ok, first_bad);
+    case HB_SETTING_GOALS: return check_records(B, records, goal_schedule_ok, first_bad);
+    case HB_SETTING_ODOMETRY: return check_records(B, records, odometry_ok, first_bad);
+    case HB_SETTING_CONTROLLERS: return check_records(B, records, controller_setting_ok, first_bad);
+    case HB_SETTING_HARDWARE: return check_records(B, records, hardware_setting_ok, first_bad);
+    case HB_SETTING_PLANNER: return check_records(B, records, planner_settings_ok, first_bad);
+    case HB_SETTING_TARGETS: return check_records(B, records, target_ok, first_bad);
+    case HB_SETTING_LATENCIES: return check_records(B, records, latency_ok, first_bad);
+    default: return HB_EINVAL;
+  }
 }
 
 // The camera read of a call whose instances start at ctx->base, on the context's odometry setting, its messages written to pos / has

@@ -297,6 +297,26 @@ int hb_default_rollout_params(hb_rollout_params* p);       /* host only */
  * B run the nominal plant (no push, no variation) on the flat ground of sim.ground_height. The device copy is allocated at max_batch by
  * the first call that sets records and freed by hb_destroy. Settings add no launch to an episode. */
 
+/* The record type of each per-robot setting call, for hb_check_setting_records: hb_push_schedule for hb_rollout_set_pushes,
+ * hb_plant_variation for _plant_variations, hb_terrain for _terrains, hb_goal_schedule for _goals, hb_odometry_setting for _odometry,
+ * hb_controller_setting for _controller_settings, hb_hardware_setting for _hardware, hb_planner_settings for hb_plan_set_settings,
+ * hb_target for hb_plan_set_targets and int32_t latency ticks for hb_rollout_set_mpc_latencies. */
+#define HB_SETTING_PUSHES 0
+#define HB_SETTING_PLANT_VARIATIONS 1
+#define HB_SETTING_TERRAINS 2
+#define HB_SETTING_GOALS 3
+#define HB_SETTING_ODOMETRY 4
+#define HB_SETTING_CONTROLLERS 5
+#define HB_SETTING_HARDWARE 6
+#define HB_SETTING_PLANNER 7
+#define HB_SETTING_TARGETS 8
+#define HB_SETTING_LATENCIES 9
+/* The record check of the setting call of `kind`, without a context (host only, no GPU needed): records (B of the kind's type) are judged
+ * by that call's rules for a record, and a record passes iff the call accepts it (the call's other checks, such as B against max_batch,
+ * need its context). 0: every record passes, *first_bad = -1. -1: *first_bad is the index of the first record that fails, or -1 for an
+ * unknown kind, B < 0 or NULL records with B > 0; -1 also for a NULL first_bad. */
+int hb_check_setting_records(int32_t kind, int B, const void* records, int32_t* first_bad);
+
 /* ---- pushed episodes: scheduled external wrenches on the base, applied by the plant of both episode calls ----
  * Push j acts on the plant step of absolute tick a iff t_start[j] <= t && t < t_start[j] + duration[j], with t = (double)a * period (the
  * episode's tick time). During that step the wrench is constant over all substeps, so a push is quantised to whole ticks. Overlapping

@@ -20,9 +20,10 @@ def test_make_odometry_settings_layout():
 
 
 @pytest.mark.parametrize("kw", [dict(period_ticks=-1), dict(delay_ticks=-1), dict(delay_ticks=16), dict(sigma_position=-1e-3),
-                                dict(sigma_drift=np.nan), dict(sigma_position=np.inf), dict(period_ticks=1.5), dict(delay_ticks=[0, 1, 2])],
+                                dict(sigma_drift=np.nan), dict(sigma_position=np.inf), dict(period_ticks=1.5), dict(delay_ticks=[0, 1, 2]),
+                                dict(period_ticks=2**32 + 5), dict(period_ticks=np.inf)],
                          ids=["negative_period", "negative_delay", "delay_above_max", "negative_sigma", "nan_drift", "inf_sigma", "fractional_period",
-                              "wrong_shape"])
+                              "wrong_shape", "period_beyond_int32", "inf_period"])
 def test_make_odometry_settings_rejects(kw):
     args = dict(period_ticks=5)
     args.update(kw)
