@@ -22,6 +22,10 @@ HB_MAX_HORIZON = 512       # longest horizon_N hb_create accepts
 # hb_check_setting_records' kinds: the record type of each per-robot setting call
 HB_SETTING_PUSHES, HB_SETTING_PLANT_VARIATIONS, HB_SETTING_TERRAINS, HB_SETTING_GOALS, HB_SETTING_ODOMETRY = 0, 1, 2, 3, 4
 HB_SETTING_CONTROLLERS, HB_SETTING_HARDWARE, HB_SETTING_PLANNER, HB_SETTING_TARGETS, HB_SETTING_LATENCIES = 5, 6, 7, 8, 9
+# The recorded channels of the episodes (hb_rollout_set_channel, HB_CHANNEL_*): name -> (index, element type, elements per row)
+CHANNELS = {"torque": (0, np.float64, 10), "joint_command": (1, np.float64, 50), "x_des": (2, np.float64, 22), "u_des": (3, np.float64, 22),
+            "wbc_solution": (4, np.float64, 38), "mode": (5, np.int32, 1), "contact_force": (6, np.float64, 12), "contact_flag": (7, np.uint8, 4),
+            "sensors": (8, np.float64, 30), "status": (9, np.int32, 3)}
 
 EXPORTED_SYMBOLS = [
     "hb_shard_partition", "hb_shard_sort_by_schedule", "hb_shard_unique_id", "hb_shard_create", "hb_shard_destroy", "hb_shard_block", "hb_shard_gather_dev", "hb_shard_wait", "hb_shard_last_error",
@@ -50,7 +54,7 @@ EXPORTED_SYMBOLS = [
     "hb_rollout_set_controller_settings",
     "hb_default_hardware_setting", "hb_rollout_set_hardware", "hb_actuation_hw", "hb_sim_read_sensors_hw",
     "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
-    "hb_check_setting_records",
+    "hb_check_setting_records", "hb_rollout_set_channel",
 ]
 
 
@@ -283,6 +287,17 @@ class HbActuationState(C.Structure):
 class HbSimParams(C.Structure):
     _fields_ = [("dt", C.c_double), ("substeps", C.c_int32), ("ground_height", C.c_double), ("ground_stiffness", C.c_double), ("ground_damping", C.c_double),
                 ("tangential_damping", C.c_double), ("friction_mu", C.c_double), ("joint_armature", C.c_double), ("joint_damping", C.c_double)]
+
+
+def make_channels(B, rows, names=None, device="cuda"):
+    """Zeroed buffers for Context.set_channels: {name: torch tensor (B, rows, width) of the channel's type} for each name of `names`
+    (default: every channel of CHANNELS). rows = ceil(n_ticks / log_every) records an episode call of n_ticks ticks."""
+    import torch
+    names = list(CHANNELS) if names is None else list(names)
+    for n in names:
+        if n not in CHANNELS:
+            raise ValueError("unknown channel %r (one of %s)" % (n, ", ".join(CHANNELS)))
+    return {n: torch.zeros((B, rows, CHANNELS[n][2]), dtype=getattr(torch, np.dtype(CHANNELS[n][1]).name), device=device) for n in names}
 
 
 def default_sim_params():
@@ -1117,6 +1132,33 @@ class Context:
         and offsets, in place of params' and est_params.noise's values; instances beyond len(settings) run those; None clears them. The
         controllers are not told about it, and no other call reads it."""
         self._set_instances("hb_rollout_set_hardware", settings)
+
+    def set_channels(self, channels):
+        """Recorded channels of this context's episodes (hb_rollout_set_channel): channels maps names of CHANNELS to contiguous cuda
+        tensors (B, rows, width) of the channel's type (make_channels); every later rollout / rollout_estimated call with log_every > 0
+        writes tick r * log_every of the call to row r of each (the sensors only in rollout_estimated). The channels not named are cleared;
+        None clears all. The context keeps the tensors until they are replaced or cleared. A call with a set channel of fewer than its B
+        instances or fewer than its rows is rejected. On an error every channel is cleared."""
+        import torch
+        channels = dict(channels or {})
+        for name, t in channels.items():
+            if name not in CHANNELS:
+                raise ValueError("unknown channel %r (one of %s)" % (name, ", ".join(CHANNELS)))
+            _, dtype, width = CHANNELS[name]
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == getattr(torch, np.dtype(dtype).name) and t.dim() == 3
+                    and t.shape[2] == width and t.is_contiguous()):
+                raise ValueError("channel %s: a contiguous cuda %s tensor (B, rows, %d) is needed" % (name, np.dtype(dtype).name, width))
+        self._channels = {}
+        try:
+            for name, (c, _, _) in CHANNELS.items():
+                t = channels.get(name)
+                args = (0, 0, None) if t is None else (t.shape[0], t.shape[1], _ptr(t))
+                _check(self._lib.hb_rollout_set_channel(self._h, c, *args), "hb_rollout_set_channel", self._h)
+        except HunterB200Error:
+            for c, _, _ in CHANNELS.values():
+                self._lib.hb_rollout_set_channel(self._h, c, 0, 0, None)
+            raise
+        self._channels = channels
 
     def read_odometry(self, rbd, est, tick, noise=None):
         """The tracking cameras at absolute tick `tick` from the true rbd [B,32] (hb_sim_read_odometry), on this context's odometry setting

@@ -76,6 +76,7 @@ struct hb_ctx {
   void* ro_mem;
   hb_rollout_command* ro_cmd; hb_plan_input* ro_in; hb_reference* ro_refs; hb_solve_info* ro_info; int32_t* ro_pstat;
   double *ro_t0, *ro_x0, *ro_feet, *ro_sol, *ro_jcmd, *ro_jtau, *ro_tau, *ro_held, *ro_tnow, *ro_wrench;
+  double* ro_cforce; uint8_t* ro_cflag;   // the plant's contact forces and flags on a tick that records a contact channel
   // hb_rollout_estimated_batch_dev's own scratch (first such call, at max_batch): the tick's sensor readings, contact flags, estimated rbd
   void* re_mem;
   double *re_quat, *re_gyro, *re_acc, *re_jpos, *re_jvel, *re_rbd;
@@ -109,6 +110,8 @@ struct hb_ctx {
   InstanceSetting<hb_hardware_setting> hardware;
   // each instance's gait templates and swing settings in every device planner path (hb_plan_set_settings)
   InstanceSetting<hb_planner_settings> plan_settings;
+  // the recorded channels of the episodes (hb_rollout_set_channel): the caller's buffer, its instances and rows; B == 0: unset
+  struct { void* buf; int B, rows; } channels[HB_CHANNELS];
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
   // hb_resident_cycle_batch's packed references / reference verdicts
   void* arena; size_t arena_cap;
@@ -1357,6 +1360,7 @@ static int rollout_reserve(hb_ctx* ctx) {
     ctx->ro_x0 = carve<double>(m, off, Bc * NX); ctx->ro_feet = carve<double>(m, off, Bc * 12); ctx->ro_sol = carve<double>(m, off, Bc * NWBC);
     ctx->ro_jcmd = carve<double>(m, off, Bc * NJ * 5); ctx->ro_jtau = carve<double>(m, off, Bc * NJ); ctx->ro_tau = carve<double>(m, off, Bc * NJ);
     ctx->ro_held = carve<double>(m, off, Bc * 32); ctx->ro_tnow = carve<double>(m, off, Bc); ctx->ro_wrench = carve<double>(m, off, Bc * 6);
+    ctx->ro_cforce = carve<double>(m, off, Bc * 12); ctx->ro_cflag = carve<uint8_t>(m, off, Bc * 4);
     return off;
   });
 }
@@ -1391,7 +1395,9 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   // the MPC latencies of this batch's instances (hb_rollout_set_mpc_latencies): instances i < with_lat have one
   const InstanceSetting<int32_t>& lat = ctx->latencies;
   const int with_lat = std::min(lat.n, B);
+  const int n_rows = (p && p->log_every > 0) ? (n_ticks + p->log_every - 1) / p->log_every : 0;   // rows of log and of the channels
   ENTER(ctx, B, n_ticks >= 0 && tick0 >= 0 && cmd && rbd && act && estop && stats && params_ok, CAPPED, [&] {
+    for (const auto& ch : ctx->channels) if (p->log_every > 0 && ch.B > 0 && (ch.B < B || ch.rows < n_rows)) return false;
     for (int i = 0; i < B; ++i) {
       const hb_rollout_command& c = cmd[i];
       if (c.gait < 0 || c.gait > 3 || c.n_cmd < 1 || c.n_cmd > HB_ROLLOUT_MAX_CMDS || !(c.gait_start == c.gait_start)) return false;
@@ -1424,8 +1430,19 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   }
   CK(cudaMemcpyAsync(ctx->ro_cmd, cmd, sizeof(hb_rollout_command) * B, cudaMemcpyHostToDevice, ctx->stream));
   const double horizon = (ctx->cfg.event_nodes && ctx->cfg.time_horizon > 0.0) ? ctx->cfg.time_horizon : ctx->cfg.horizon_N * ctx->cfg.dt;
-  const int n_log = (log && p->log_every > 0) ? (n_ticks + p->log_every - 1) / p->log_every : 0;
-  const int n_est_log = (e && e->log && p->log_every > 0) ? (n_ticks + p->log_every - 1) / p->log_every : 0;
+  const int n_log = log ? n_rows : 0, n_est_log = (e && e->log) ? n_rows : 0;
+  // the channels this call records (hb_rollout_set_channel): every set one on the logged ticks, the sensors only in estimated episodes
+  RecordSlots rec{};
+  for (int c = 0; c < HB_CHANNELS && n_rows; ++c) {
+    if (ctx->channels[c].B == 0 || (c == HB_CHANNEL_SENSORS && !e)) continue;
+    rec.channel[rec.n] = c; rec.first[rec.n] = rec.width;
+    rec.stride[rec.n] = (size_t)ctx->channels[c].rows * CHANNEL_WIDTH[c];
+    rec.n++; rec.width += CHANNEL_WIDTH[c];
+  }
+  const bool contacts = ctx->channels[HB_CHANNEL_CONTACT_FORCE].B > 0 || ctx->channels[HB_CHANNEL_CONTACT_FLAG].B > 0;
+  RecordSources src{ctx->ro_tau, ctx->ro_jcmd, ctx->xdes, ctx->udes, ctx->ro_sol, ctx->ro_cforce, ctx->wmode, ctx->wstatus, ctx->ro_pstat,
+                    ctx->ro_cflag, ctx->ro_info};
+  if (e) { src.quat = ctx->re_quat; src.gyro = ctx->re_gyro; src.acc = ctx->re_acc; src.jpos = ctx->re_jpos; src.jvel = ctx->re_jvel; }
   const unsigned grid = (B + 63) / 64;
   // what the controllers measure: the true state, or the filter's estimate
   double* meas = e ? ctx->re_rbd : rbd;
@@ -1442,6 +1459,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
     const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
     const bool mpc = a % p->mpc_every == 0, first_cold = cold && k == 0;
     double* log_row = (n_log && k % p->log_every == 0) ? log + (size_t)(k / p->log_every) * 32 : nullptr;
+    const bool record = rec.n && k % p->log_every == 0;
     rc = launch(ctx, K_UNPROFILED, rollout_tick_begin_kernel, grid, 64, 0, B, (int)a, t, p->min_base_height, rbd, ctx->ro_held, stats, ctx->ro_tnow,
                 log_row, (size_t)n_log * 32, ctx->pushes.view(), wrench, ctx->terrains.view());
     if (!rc && e) {
@@ -1478,7 +1496,14 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
                                     ctx->ro_jtau, controllers);
     if (!rc) rc = actuation_dev(ctx, B, p->actuation_delay, hardware, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, hardware, ctx->ro_tau);
-    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, ctx->variations.view(), ctx->terrains.view(), nullptr, nullptr);
+    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, ctx->variations.view(), ctx->terrains.view(),
+                           record && contacts ? ctx->ro_cforce : nullptr, record && contacts ? ctx->ro_cflag : nullptr);
+    if (!rc && record) {
+      for (int j = 0; j < rec.n; ++j)
+        rec.dst[j] = static_cast<char*>(ctx->channels[rec.channel[j]].buf) + (size_t)(k / p->log_every) * CHANNEL_WIDTH[rec.channel[j]] * CHANNEL_BYTES[rec.channel[j]];
+      src.mpc = mpc ? 1 : 0;
+      rc = launch(ctx, K_UNPROFILED, rollout_record_kernel, (unsigned)(((size_t)B * rec.width + 127) / 128), 128, 0, B, rec, src);
+    }
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_tick_end_kernel, grid, 64, 0, B, (int)a, mpc ? 1 : 0, ctx->ro_info, ctx->ro_pstat, ctx->wstatus, estop, ctx->ro_tau, ctx->ro_held, rbd, stats);
   }
   return rc;
@@ -1494,6 +1519,14 @@ int hb_rollout_estimated_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_tick
                                    hb_estimation_state* est, hb_estimation_stats* est_stats, double* log, double* est_log) {
   const EstimationArgs e{ep, est, est_stats, est_log};
   return rollout_impl(ctx, B, tick0, n_ticks, p, cmd, rbd, act, estop, stats, log, &e);
+}
+
+int hb_rollout_set_channel(hb_ctx* ctx, int32_t channel, int B, int rows, void* buffer) {
+  const int rc = enter(ctx, B, channel >= 0 && channel < HB_CHANNELS && rows >= 0 && (B == 0 || buffer), CAPPED);
+  if (rc == EMPTY) { ctx->channels[channel] = {nullptr, 0, 0}; return HB_OK; }
+  if (rc) return rc;
+  ctx->channels[channel] = {buffer, B, rows};
+  return HB_OK;
 }
 
 int hb_default_estimation_params(hb_estimation_params* p) {

@@ -159,6 +159,59 @@ __global__ void rollout_tick_end_kernel(int B, int tick, int mpc_tick, const hb_
   if (restore) for (int i = 0; i < 32; ++i) r[i] = held[(size_t)inst * 32 + i];
 }
 
+// ---- recorded channels (hb_rollout_set_channel, hunter_b200.h)
+// Elements per row of each channel and the size of one element, by HB_CHANNEL_* index
+constexpr int CHANNEL_WIDTH[HB_CHANNELS] = {NJ, NJ * 5, NX, NU, NWBC, 1, 12, 4, 30, 3};
+constexpr int CHANNEL_BYTES[HB_CHANNELS] = {8, 8, 8, 8, 8, 4, 8, 1, 8, 4};
+// The channels one recorded tick writes, in ascending channel order: channel[k]'s elements are the instance's elements first[k] ..
+// first[k + 1] - 1 of width in all; dst[k] is that channel's row for the tick at instance 0, and stride[k] its elements per instance.
+struct RecordSlots {
+  int n, width;
+  int channel[HB_CHANNELS], first[HB_CHANNELS];
+  size_t stride[HB_CHANNELS];
+  void* dst[HB_CHANNELS];
+};
+// What the tick computed, in the episode's scratch (instance-major): sensors only in estimated episodes, contact forces only when a
+// contact channel is recorded, info and plan status only on an MPC tick.
+struct RecordSources {
+  const double *tau, *jcmd, *xdes, *udes, *sol, *cforce;
+  const int32_t *mode, *wstatus, *pstat;
+  const uint8_t* cflag;
+  const hb_solve_info* info;
+  const double *quat, *gyro, *acc, *jpos, *jvel;
+  int mpc;
+};
+
+// One recorded tick: one thread per recorded element of every instance, so that consecutive threads write consecutive addresses of an
+// instance's row. Reads only; the tick's values are copied as they are.
+__global__ void rollout_record_kernel(int B, const __grid_constant__ RecordSlots s, const __grid_constant__ RecordSources src) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (size_t)B * s.width) return;
+  const int inst = (int)(idx / s.width);
+  int e = (int)(idx % s.width), k = 0;
+  while (k + 1 < s.n && e >= s.first[k + 1]) ++k;
+  e -= s.first[k];
+  const size_t at = (size_t)inst * s.stride[k] + e;
+  double* d = static_cast<double*>(s.dst[k]);
+  switch (s.channel[k]) {
+    case HB_CHANNEL_TORQUE: d[at] = src.tau[(size_t)inst * NJ + e]; break;
+    case HB_CHANNEL_JOINT_COMMAND: d[at] = src.jcmd[(size_t)inst * NJ * 5 + e]; break;
+    case HB_CHANNEL_X_DES: d[at] = src.xdes[(size_t)inst * NX + e]; break;
+    case HB_CHANNEL_U_DES: d[at] = src.udes[(size_t)inst * NU + e]; break;
+    case HB_CHANNEL_WBC_SOLUTION: d[at] = src.sol[(size_t)inst * NWBC + e]; break;
+    case HB_CHANNEL_MODE: static_cast<int32_t*>(s.dst[k])[at] = src.mode[inst]; break;
+    case HB_CHANNEL_CONTACT_FORCE: d[at] = src.cforce[(size_t)inst * 12 + e]; break;
+    case HB_CHANNEL_CONTACT_FLAG: static_cast<uint8_t*>(s.dst[k])[at] = src.cflag[(size_t)inst * 4 + e]; break;
+    case HB_CHANNEL_SENSORS:
+      d[at] = e < 4 ? src.quat[(size_t)inst * 4 + e] : e < 7 ? src.gyro[(size_t)inst * 3 + e - 4] : e < 10 ? src.acc[(size_t)inst * 3 + e - 7]
+              : e < 20 ? src.jpos[(size_t)inst * NJ + e - 10] : src.jvel[(size_t)inst * NJ + e - 20];
+      break;
+    case HB_CHANNEL_STATUS:
+      static_cast<int32_t*>(s.dst[k])[at] = e == 0 ? src.wstatus[inst] : !src.mpc ? -1 : e == 1 ? src.info[inst].status : src.pstat[inst];
+      break;
+  }
+}
+
 // ---- estimated episodes (hb_rollout_estimated_batch_dev, hb_sim_read_sensors_batch_dev)
 
 // Philox4x32-10 (Salmon et al., SC'11): counter c encrypted under key (k0, k1), in place. Written out rather than taken from curand so that

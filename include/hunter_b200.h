@@ -735,6 +735,31 @@ int hb_rollout_estimated_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_tick
                                    const hb_rollout_command* cmd, double* rbd, hb_actuation_state* act, uint8_t* estop, hb_rollout_stats* stats,
                                    hb_estimation_state* est, hb_estimation_stats* est_stats /*nullable*/, double* log /*nullable*/,
                                    double* est_log /*nullable*/);
+/* ---- recorded channels: what the controllers did and what the plant felt on every logged tick of both episode calls ----
+ * A channel is one device buffer set on the context with hb_rollout_set_channel: B x rows x width elements of the channel's type,
+ * instance-major as log. Row r of an episode call holds tick r * log_every of that call (the same row as log, so the state log[:, r] and
+ * the action torque[:, r] are a pair), written after the tick's plant step from what the tick computed. A call with log_every == 0
+ * records nothing; a NULL log does not stop the recording. Rows of an instance after its fail_tick hold what the kernels computed for
+ * the held state (hb_rollout_stats says from which tick on). hb_rollout_estimated_batch_dev writes every set channel,
+ * hb_rollout_batch_dev every one but HB_CHANNEL_SENSORS, which it leaves untouched. Instances at or beyond the call's B and rows at or
+ * beyond its ceil(n_ticks / log_every) are not written. A call with log_every > 0 is rejected (-1, nothing enqueued) when a set channel
+ * has fewer than B instances or fewer than ceil(n_ticks / log_every) rows. With no channel set, or log_every == 0, an episode launches
+ * exactly what it launches without this feature; otherwise it adds one launch per recorded tick. */
+#define HB_CHANNEL_TORQUE 0          /* double x 10: applied torques after saturation (what the plant step receives, before a variation's motor_strength) */
+#define HB_CHANNEL_JOINT_COMMAND 1   /* double x 50: the joint command law's output per joint (pos_des, vel_des, kp, kd, ff), before the actuation delay */
+#define HB_CHANNEL_X_DES 2           /* double x 22: the policy's desired state at t (adopted policy with a latency) */
+#define HB_CHANNEL_U_DES 3           /* double x 22 */
+#define HB_CHANNEL_WBC_SOLUTION 4    /* double x 38: [qdd, F, tau] after the fallback, weighted or hierarchical */
+#define HB_CHANNEL_MODE 5            /* int32 x 1: the contact mode the WBC used */
+#define HB_CHANNEL_CONTACT_FORCE 6   /* double x 12: the plant's world-frame force at each contact point in the tick's last substep */
+#define HB_CHANNEL_CONTACT_FLAG 7    /* uint8 x 4: that normal force > 0 */
+#define HB_CHANNEL_SENSORS 8         /* double x 30: quat (x y z w), ang_vel_local, lin_acc_local, joint_pos, joint_vel as the filter read them (estimated episodes only) */
+#define HB_CHANNEL_STATUS 9          /* int32 x 3: wbc status; the MPC cycle's info.status and plan status on an MPC tick, -1 on other ticks */
+#define HB_CHANNELS 10
+/* Sets channel `channel` of the context's episodes to buffer (device memory, B x rows x the channel's width). B == 0 clears it (buffer may
+ * be NULL). -1: an unknown channel, B < 0, rows < 0, or a NULL buffer with B > 0; -4: B > max_batch. A rejected call keeps the previous
+ * channel. The call only stores the pointer: the caller keeps the buffer valid until the last episode call that writes it has completed. */
+int hb_rollout_set_channel(hb_ctx* ctx, int32_t channel, int B, int rows, void* buffer /*nullable with B == 0*/);
 int hb_rbd_to_centroidal_batch_dev(hb_ctx* ctx, int B, const double* rbd, double* x);
 int hb_reference_expand_batch_dev(hb_ctx* ctx, int B, const double* t0, const hb_reference* refs, double* x_ref, double* swing_ref,
                                   int32_t* mode);
