@@ -11,7 +11,7 @@ from .api import (HbWbcSettings, HbTaskInfo, parse_task_info, Context, WeightedW
                   HB_ODOM_MAX_DELAY, HbOdometrySetting, make_odometry_settings, HbControllerSetting, make_controller_settings,
                   HbHardwareSetting, default_hardware_setting, make_hardware_settings,
                   HB_GAIT_MAX_PHASES, HbGaitTemplate, HbPlannerSettings, gait_template, default_planner_settings, parse_planner_settings, make_planner_settings,
-                  CHANNELS, make_channels)
+                  CHANNELS, make_channels, EpisodeSnapshot, reseed)
 
 __all__ = ["HbWbcSettings", "HbTaskInfo", "parse_task_info", "Context", "WeightedWbc", "HierarchicalWbc", "HbHoqpProblem", "make_hoqp_problems", "hoqp_tasks", "SqpMpc", "HbReference", "HbSolveInfo", "HbConfig", "HunterB200Error", "load_library",
            "EXPORTED_SYMBOLS", "NX", "NU", "NQ", "NJ", "NWBC", "INFO_DTYPE", "HbPlanInput", "plan_references", "plan_set_threads", "make_plan_inputs", "GAIT_IDS", "GaitSelector", "HbPdGains", "default_pd_gains", "HbKfState", "HbKfParams", "default_kf_params", "kf_states", "HbObserverState", "observer_states", "HbActuationState", "HbSimParams", "default_sim_params", "actuation_states",
@@ -21,4 +21,4 @@ __all__ = ["HbWbcSettings", "HbTaskInfo", "parse_task_info", "Context", "Weighte
            "HB_ODOM_MAX_DELAY", "HbOdometrySetting", "make_odometry_settings", "HbControllerSetting", "make_controller_settings",
            "HbHardwareSetting", "default_hardware_setting", "make_hardware_settings",
            "HB_GAIT_MAX_PHASES", "HbGaitTemplate", "HbPlannerSettings", "gait_template", "default_planner_settings", "parse_planner_settings", "make_planner_settings",
-           "CHANNELS", "make_channels"]
+           "CHANNELS", "make_channels", "EpisodeSnapshot", "reseed"]

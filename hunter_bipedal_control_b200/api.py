@@ -26,6 +26,8 @@ HB_SETTING_CONTROLLERS, HB_SETTING_HARDWARE, HB_SETTING_PLANNER, HB_SETTING_TARG
 CHANNELS = {"torque": (0, np.float64, 10), "joint_command": (1, np.float64, 50), "x_des": (2, np.float64, 22), "u_des": (3, np.float64, 22),
             "wbc_solution": (4, np.float64, 38), "mode": (5, np.int32, 1), "contact_force": (6, np.float64, 12), "contact_flag": (7, np.uint8, 4),
             "sensors": (8, np.float64, 30), "status": (9, np.int32, 3)}
+# episode snapshot rows (hb_episode_save_async): the header's size and its flags
+HB_EPISODE_HEADER_BYTES, HB_EPISODE_HAS_SOLUTION, HB_EPISODE_HAS_FALLBACK, HB_EPISODE_HAS_POLICY = 32, 1, 2, 4
 
 EXPORTED_SYMBOLS = [
     "hb_shard_partition", "hb_shard_sort_by_schedule", "hb_shard_unique_id", "hb_shard_create", "hb_shard_destroy", "hb_shard_block", "hb_shard_gather_dev", "hb_shard_wait", "hb_shard_last_error",
@@ -55,6 +57,7 @@ EXPORTED_SYMBOLS = [
     "hb_default_hardware_setting", "hb_rollout_set_hardware", "hb_actuation_hw", "hb_sim_read_sensors_hw",
     "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
     "hb_check_setting_records", "hb_rollout_set_channel",
+    "hb_episode_state_bytes", "hb_episode_save_async", "hb_episode_restore",
 ]
 
 
@@ -751,6 +754,7 @@ def load_library():
         _lib.hb_last_cuda_error.restype = C.c_char_p
         _lib.hb_launch_count.restype = C.c_int64
         _lib.hb_last_reference_upload_bytes.restype = C.c_int64
+        _lib.hb_episode_state_bytes.restype = C.c_int64
         _lib.hb_stream.restype = C.c_void_p
         _lib.hb_shard_last_error.restype = C.c_char_p
     return _lib
@@ -783,6 +787,85 @@ def _check_records(kind, records, setting):
     if load_library().hb_check_setting_records(kind, len(records), records, C.byref(bad)) != 0:
         raise ValueError("%s: record %d is rejected by hb_rollout_set_%s" % (setting, bad.value, setting))
     return records
+
+
+def reseed(est, first_stream):
+    """Gives record i of the estimation states est (a tensor of B hb_estimation_state, as rollout_estimated takes) noise stream
+    first_stream + i, in place; returns est. Forked estimated copies share their source's stream, so without this their sensor and camera
+    noise stays identical. The noise an instance draws on absolute tick a is Philox4x32-10 under the key hb_sensor_noise.seed at the counter
+    (block, a, noise_stream) and depends on nothing else, so a copy reseeded at the fork tick draws from then on exactly what an instance
+    that had that stream from the start draws on those ticks."""
+    import torch
+    size, off = C.sizeof(HbEstimationState), HbEstimationState.noise_stream.offset
+    rec = est.view(-1, size)
+    streams = np.uint64(first_stream) + np.arange(rec.shape[0], dtype=np.uint64)
+    rec[:, off:off + 8] = torch.from_numpy(streams.view(np.uint8).reshape(-1, 8)).to(est.device)
+    return est
+
+
+def _episode_index(src, B, n, what):
+    """src as a list of B ints in [0, n) (None: 0 .. B-1), or ValueError."""
+    idx = list(range(B)) if src is None else [int(i) for i in src]
+    if len(idx) != B or not all(0 <= i < n for i in idx):
+        raise ValueError("%s: %d instances from %s of %d" % (what, B, "0 .. B-1" if src is None else "src %s" % idx, n))
+    return idx
+
+
+def _gather(idx, rbd, act, estop, stats, est=None, est_stats=None):
+    """Copies of instances idx of an episode's caller buffers: [rbd, act, estop, stats] and, with est, [est, est_stats]."""
+    import torch
+    t = torch.tensor(idx, dtype=torch.long, device=rbd.device)
+
+    def take(x, size):
+        return x.view(-1, size)[t].reshape(-1).clone()
+    out = [rbd[t].clone(), take(act, C.sizeof(HbActuationState)), estop[t].clone(), np.asarray(stats)[idx].copy()]
+    if est is not None:
+        out += [take(est, C.sizeof(HbEstimationState)), np.asarray(est_stats)[idx].copy()]
+    return out
+
+
+class EpisodeSnapshot:
+    """Episodes saved mid-way (Context.save_episodes): `rows`, the context state of each instance (a uint8 tensor (n, row bytes) on the
+    device, hb_episode_save_async), and clones of the caller's buffers of the same instances: rbd (n, 32), act (n hb_actuation_state
+    bytes), estop (n), stats (ROLLOUT_STATS_DTYPE), and for estimated episodes est (n hb_estimation_state bytes) and est_stats
+    (ESTIMATION_STATS_DTYPE), None otherwise. Context.restore_episodes continues them, in this or another context of the same
+    configuration; save / load keep them in an .npz file."""
+    _TENSORS = ("rows", "rbd", "act", "estop", "est")
+
+    def __init__(self, rows, rbd, act, estop, stats, est=None, est_stats=None):
+        n = rows.shape[0]
+        stats = np.asarray(stats, dtype=ROLLOUT_STATS_DTYPE)
+        ok = (rows.dim() == 2 and tuple(rbd.shape) == (n, 32) and act.numel() == n * C.sizeof(HbActuationState) and tuple(estop.shape) == (n,)
+              and stats.shape == (n,) and (est is None) == (est_stats is None))
+        if ok and est is not None:
+            est_stats = np.asarray(est_stats, dtype=ESTIMATION_STATS_DTYPE)
+            ok = est.numel() == n * C.sizeof(HbEstimationState) and est_stats.shape == (n,)
+        if not ok:
+            raise ValueError("EpisodeSnapshot: the rows and the caller's buffers must hold the same instances (estimated: est and est_stats both)")
+        self.rows, self.rbd, self.act, self.estop, self.stats, self.est, self.est_stats = rows, rbd, act, estop, stats, est, est_stats
+
+    def __len__(self):
+        return self.rows.shape[0]
+
+    @property
+    def estimated(self):
+        return self.est is not None
+
+    def save(self, path):
+        """Writes the snapshot to the .npz file `path`."""
+        arrays = {k: getattr(self, k).cpu().numpy() for k in self._TENSORS if getattr(self, k) is not None}
+        arrays["stats"] = self.stats
+        if self.estimated:
+            arrays["est_stats"] = self.est_stats
+        np.savez(path, **arrays)
+
+    @classmethod
+    def load(cls, path, device="cuda"):
+        """The snapshot save wrote to `path`, its tensors on `device`."""
+        import torch
+        with np.load(path) as f:
+            t = {k: torch.from_numpy(f[k]).to(device) for k in cls._TENSORS if k in f}
+            return cls(t["rows"], t["rbd"], t["act"], t["estop"], f["stats"], t.get("est"), f["est_stats"] if "est_stats" in f else None)
 
 
 def _check_hardware(what, hardware, B):
@@ -1329,6 +1412,42 @@ class Context:
         self.sync()
         out = (rbd, act, estop, d_st.cpu().numpy().view(ROLLOUT_STATS_DTYPE), log)
         return out + (est, d_es.cpu().numpy().view(ESTIMATION_STATS_DTYPE), est_log) if estimated else out
+
+    # ------------------------------------------------------------------ episode snapshots (hb_episode_save_async / hb_episode_restore)
+    @property
+    def episode_state_bytes(self):
+        """Bytes of one instance's snapshot row on this context (hb_episode_state_bytes)."""
+        return int(self._lib.hb_episode_state_bytes(self._h))
+
+    def save_episodes(self, B, rbd, act, estop, stats, est=None, est_stats=None, src=None):
+        """Snapshot of B episodes between two rollout / rollout_estimated calls: instance src[i] (None: i) of this context and of the caller's
+        buffers (rollout's tuple; est and est_stats for estimated episodes) becomes instance i of the returned EpisodeSnapshot."""
+        import torch
+        idx = _episode_index(src, B, rbd.shape[0], "save_episodes")
+        if (est is None) != (est_stats is None):
+            raise ValueError("save_episodes: est and est_stats go together")
+        dev = rbd.device
+        rows = torch.empty((B, self.episode_state_bytes), dtype=torch.uint8, device=dev)
+        torch.cuda.current_stream(dev).synchronize()          # the context's stream does not order itself after torch's
+        _check(self._lib.hb_episode_save_async(self._h, B, (C.c_int32 * B)(*idx), _ptr(rows)), "hb_episode_save_async", self._h)
+        self.sync()
+        out = [rows] + _gather(idx, rbd, act, estop, stats, est, est_stats)
+        return EpisodeSnapshot(*out)
+
+    def restore_episodes(self, snapshot, src=None):
+        """Instance i of this context from instance src[i] (None: i) of the EpisodeSnapshot, for B = len(src) (None: every instance).
+        Returns fresh buffers of the B instances to continue them with: (rbd, act, estop, stats) for rollout, followed by (est, est_stats)
+        for rollout_estimated, with tick0 the tick the episodes were saved at. Set goals and odometry before: both clear what this restores."""
+        import torch
+        n = len(snapshot)
+        B = n if src is None else len(src)
+        idx = _episode_index(src, B, n, "restore_episodes")
+        if snapshot.rows.shape[1] != self.episode_state_bytes:
+            raise ValueError("restore_episodes: rows of %d bytes, this context's hold %d" % (snapshot.rows.shape[1], self.episode_state_bytes))
+        rows = snapshot.rows.contiguous()
+        torch.cuda.current_stream(rows.device).synchronize()
+        _check(self._lib.hb_episode_restore(self._h, B, (C.c_int32 * B)(*idx), n, _ptr(rows)), "hb_episode_restore", self._h)
+        return tuple(_gather(idx, snapshot.rbd, snapshot.act, snapshot.estop, snapshot.stats, snapshot.est, snapshot.est_stats))
 
     def control_step_dev(self, t_rel, x0, x_ref, swing, mode, rbd, xt, ut, info, sol, tau, status=None):
         _check(self._lib.hb_control_step_batch_dev(self._h, x0.shape[0], C.c_double(t_rel), _ptr(x0), _ptr(x_ref), _ptr(swing), _ptr(mode), _ptr(rbd), _ptr(xt),

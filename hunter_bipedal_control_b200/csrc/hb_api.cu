@@ -112,6 +112,10 @@ struct hb_ctx {
   InstanceSetting<hb_planner_settings> plan_settings;
   // the recorded channels of the episodes (hb_rollout_set_channel): the caller's buffer, its instances and rows; B == 0: unset
   struct { void* buf; int B, rows; } channels[HB_CHANNELS];
+  // the episode snapshots' staging (hb_episode_save_async / hb_episode_restore), allocated at max_batch by their first call: the rows'
+  // context instances or source rows, and the headers a save writes
+  void* snap_mem;
+  int32_t* snap_src; int64_t* snap_head;
   // host-call staging, sized on demand by the calls that use it (grow): the device arena Staging carves, and the pinned host buffer of
   // hb_resident_cycle_batch's packed references / reference verdicts
   void* arena; size_t arena_cap;
@@ -491,7 +495,7 @@ int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
 int hb_destroy(hb_ctx* ctx) {
   if (!ctx) return HB_EINVAL;
   cudaSetDevice(ctx->device);
-  void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->arena,
+  void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->snap_mem, ctx->arena,
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
                        ctx->odometry.dev, ctx->controllers.dev, ctx->hardware.dev, ctx->plan_settings.dev};
   for (void* p : mem) if (p) cudaFree(p);
@@ -1169,17 +1173,22 @@ static bool goal_schedule_ok(const hb_goal_schedule& s) {
   return true;
 }
 
-int hb_rollout_set_goals(hb_ctx* ctx, int B, const hb_goal_schedule* g) {
-  int rc = set_instances(ctx, B, g, goal_schedule_ok, &hb_ctx::goals);
-  if (rc || ctx->goals.n == 0) return rc;
+// The captured goals, allocated at max_batch by their first use (hb_rollout_set_goals with schedules, hb_episode_restore)
+static int goal_reserve(hb_ctx* ctx) {
   const size_t Bc = ctx->cfg.max_batch;
-  rc = reserve_group(&ctx->goal_mem, [&](void* m) {
+  return reserve_group(&ctx->goal_mem, [&](void* m) {
     size_t off = 0;
     ctx->goal_tg = carve<hb_target>(m, off, Bc); ctx->goal_idx = carve<int32_t>(m, off, Bc);
     return off;
   });
+}
+
+int hb_rollout_set_goals(hb_ctx* ctx, int B, const hb_goal_schedule* g) {
+  int rc = set_instances(ctx, B, g, goal_schedule_ok, &hb_ctx::goals);
+  if (rc || ctx->goals.n == 0) return rc;
+  rc = goal_reserve(ctx);
   if (rc) { ctx->goals.n = 0; return rc; }
-  CK(cudaMemsetAsync(ctx->goal_idx, 0xff, sizeof(int32_t) * Bc, ctx->stream));     // every captured goal forgotten: index -1
+  CK(cudaMemsetAsync(ctx->goal_idx, 0xff, sizeof(int32_t) * ctx->cfg.max_batch, ctx->stream));     // every captured goal forgotten: index -1
   return HB_OK;
 }
 
@@ -1210,17 +1219,22 @@ static bool odometry_ok(const hb_odometry_setting& s) {
   return true;
 }
 
-int hb_rollout_set_odometry(hb_ctx* ctx, int B, const hb_odometry_setting* s) {
-  int rc = set_instances(ctx, B, s, odometry_ok, &hb_ctx::odometry);
-  if (rc || ctx->odometry.n == 0) return rc;
+// The cameras' state, allocated at max_batch by its first use (hb_rollout_set_odometry with cameras, hb_episode_restore)
+static int camera_reserve(hb_ctx* ctx) {
   const size_t Bc = ctx->cfg.max_batch;
-  rc = reserve_group(&ctx->odom_mem, [&](void* m) {
+  return reserve_group(&ctx->odom_mem, [&](void* m) {
     size_t off = 0;
     ctx->odom_cam = carve<OdomCamera>(m, off, Bc);
     return off;
   });
+}
+
+int hb_rollout_set_odometry(hb_ctx* ctx, int B, const hb_odometry_setting* s) {
+  int rc = set_instances(ctx, B, s, odometry_ok, &hb_ctx::odometry);
+  if (rc || ctx->odometry.n == 0) return rc;
+  rc = camera_reserve(ctx);
   if (rc) { ctx->odometry.n = 0; return rc; }
-  CK(cudaMemsetAsync(ctx->odom_cam, 0, sizeof(OdomCamera) * Bc, ctx->stream));     // every camera's history and bias cleared
+  CK(cudaMemsetAsync(ctx->odom_cam, 0, sizeof(OdomCamera) * ctx->cfg.max_batch, ctx->stream));     // every camera's history and bias cleared
   return HB_OK;
 }
 
@@ -1526,6 +1540,119 @@ int hb_rollout_set_channel(hb_ctx* ctx, int32_t channel, int B, int rows, void* 
   if (rc == EMPTY) { ctx->channels[channel] = {nullptr, 0, 0}; return HB_OK; }
   if (rc) return rc;
   ctx->channels[channel] = {buffer, B, rows};
+  return HB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- episode snapshots
+// The segments of a snapshot row (hunter_b200.h, "episode snapshots") over this context's buffers, in the row's order; head: the headers
+// a save writes (null: a restore, which keeps the headers out of the context)
+struct EpisodeTable {
+  EpisodeSegments t{};
+  uint32_t words = 0;
+  void add(void* buf, size_t bytes, uint32_t fill = 0, bool by_row = false) {
+    t.seg[t.n++] = EpisodeSegment{static_cast<char*>(buf), (uint32_t)bytes, words, fill, by_row ? 1 : 0};
+    words += (uint32_t)((bytes + 7) / 8);
+  }
+  // the rows of a solution that the layout of this grid holds, in SolutionRows' order
+  void add_solution(const SolutionRows& r, size_t N, bool grid) {
+    add(r.t0, sizeof(double)); add(r.xt, sizeof(double) * (N + 1) * NX); add(r.ut, sizeof(double) * N * NU);
+    if (grid) add(r.tk, sizeof(double) * (N + 1));
+    add(r.mode, sizeof(int32_t) * (N + 1));
+    if (grid) add(r.nn, sizeof(int32_t));
+  }
+};
+static_assert(sizeof(hb_target) % 4 == 0 && sizeof(OdomCamera) % 4 == 0, "snapshot segments are copied in 4-byte units");
+
+static EpisodeSegments episode_segments(const hb_ctx* ctx, int64_t* head) {
+  const size_t N = ctx->cfg.horizon_N;
+  const bool grid = ctx->cfg.event_nodes != 0;
+  EpisodeTable e;
+  e.add(head, HB_EPISODE_HEADER_BYTES, 0, true);
+  e.add_solution(rows_at(ctx->res, 0, N, grid), N, grid);
+  e.add(ctx->res_sol, sizeof(double) * NWBC);
+  e.add(ctx->res_stance, sizeof(double) * 12);
+  e.add(ctx->goal_idx, sizeof(int32_t), 0xffffffffu);       // unallocated: no goal captured
+  e.add(ctx->goal_tg, sizeof(hb_target));
+  e.add_solution(ctx->pol_mem ? rows_at(ctx->pol, 0, N, grid) : SolutionRows{}, N, grid);
+  e.add(ctx->odom_cam, sizeof(OdomCamera));
+  e.t.row_words = e.words;
+  return e.t;
+}
+
+// The staging of the snapshot calls, at max_batch
+static int snapshot_reserve(hb_ctx* ctx) {
+  const size_t Bc = ctx->cfg.max_batch;
+  return reserve_group(&ctx->snap_mem, [&](void* m) {
+    size_t off = 0;
+    ctx->snap_src = carve<int32_t>(m, off, Bc); ctx->snap_head = carve<int64_t>(m, off, Bc * 4);
+    return off;
+  });
+}
+
+// episode_copy_kernel over B rows, after the entry checks. src (host) is staged in stream order, so a later call's staging cannot overtake
+// this call's kernel.
+static int episode_copy(hb_ctx* ctx, int B, const int32_t* src, bool restore, const void* rows, int64_t* head) {
+  if (src) CK(cudaMemcpyAsync(ctx->snap_src, src, sizeof(int32_t) * B, cudaMemcpyHostToDevice, ctx->stream));
+  const EpisodeSegments t = episode_segments(ctx, head);
+  const size_t n = (size_t)B * t.row_words;
+  return launch(ctx, K_UNPROFILED, episode_copy_kernel, (unsigned)((n + 127) / 128), 128, 0, B, t, src ? (const int32_t*)ctx->snap_src : nullptr,
+                restore ? 1 : 0, static_cast<uint32_t*>(const_cast<void*>(rows)));
+}
+
+int64_t hb_episode_state_bytes(const hb_ctx* ctx) { return ctx ? (int64_t)episode_segments(ctx, nullptr).row_words * 8 : HB_EINVAL; }
+
+int hb_episode_save_async(hb_ctx* ctx, int B, const int32_t* src, void* rows) {
+  ENTER(ctx, B, B == 0 || rows, CAPPED, [&] { return !src || std::all_of(src, src + B, [&](int32_t s) { return s >= 0 && s < ctx->cfg.max_batch; }); });
+  int rc = snapshot_reserve(ctx);
+  if (rc) return rc;
+  std::vector<int64_t> head;
+  try { head.resize((size_t)B * 4); } catch (const std::bad_alloc&) { return HB_ENOMEM; }
+  const int64_t bytes = hb_episode_state_bytes(ctx);
+  for (int i = 0; i < B; ++i) {
+    const int s = src ? src[i] : i;
+    const bool pol = (size_t)s < ctx->pol_have.size() && ctx->pol_have[s];
+    int64_t* h = &head[(size_t)i * 4];
+    h[0] = ctx->cfg.horizon_N; h[1] = ctx->cfg.event_nodes; h[2] = bytes;
+    h[3] = (s < ctx->res_valid ? HB_EPISODE_HAS_SOLUTION : 0) | (s < ctx->res_sol_valid ? HB_EPISODE_HAS_FALLBACK : 0) | (pol ? HB_EPISODE_HAS_POLICY : 0);
+  }
+  CK(cudaMemcpyAsync(ctx->snap_head, head.data(), sizeof(int64_t) * head.size(), cudaMemcpyHostToDevice, ctx->stream));
+  return episode_copy(ctx, B, src, false, rows, ctx->snap_head);
+}
+
+int hb_episode_restore(hb_ctx* ctx, int B, const int32_t* src, int n_rows, const void* rows) {
+  ENTER(ctx, B, B == 0 || (rows && n_rows >= 1), CAPPED, [&] {
+    return src ? std::all_of(src, src + B, [&](int32_t s) { return s >= 0 && s < n_rows; }) : B <= n_rows;
+  });
+  // the headers of the rows up to the last one restored, read back before anything changes
+  const int n_head = src ? *std::max_element(src, src + B) + 1 : B;
+  const int64_t bytes = hb_episode_state_bytes(ctx);
+  std::vector<int64_t> head;
+  try { head.resize((size_t)n_head * 4); } catch (const std::bad_alloc&) { return HB_ENOMEM; }
+  CK(cudaMemcpy2DAsync(head.data(), HB_EPISODE_HEADER_BYTES, rows, (size_t)bytes, HB_EPISODE_HEADER_BYTES, n_head, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  // every row of this layout with a solution; k: the first restored instance without a fallback solution, after which none may have one
+  int k = B;
+  bool any_policy = false;
+  for (int i = 0; i < B; ++i) {
+    const int64_t* h = &head[(size_t)(src ? src[i] : i) * 4];
+    if (h[0] != ctx->cfg.horizon_N || h[1] != ctx->cfg.event_nodes || h[2] != bytes || !(h[3] & HB_EPISODE_HAS_SOLUTION)) return HB_EINVAL;
+    const bool fallback = (h[3] & HB_EPISODE_HAS_FALLBACK) != 0;
+    if (!fallback && k == B) k = i;
+    if (fallback && k < B) return HB_EINVAL;
+    any_policy |= (h[3] & HB_EPISODE_HAS_POLICY) != 0;
+  }
+  if (k < B && ctx->res_sol_valid > B) return HB_EINVAL;     // instances beyond B keep a previous solution that instance k lacks
+  // the buffers the rows write: the goal and camera state, and the adopted policy when a row holds one or the context has one
+  int rc = snapshot_reserve(ctx);
+  if (!rc) rc = goal_reserve(ctx);
+  if (!rc) rc = camera_reserve(ctx);
+  if (!rc && (any_policy || ctx->pol_mem)) rc = policy_reserve(ctx);
+  if (!rc) rc = episode_copy(ctx, B, src, true, rows, nullptr);
+  if (rc) return rc;
+  ctx->res_valid = std::max(ctx->res_valid, B);
+  ctx->res_sol_valid = k < B ? k : std::max(ctx->res_sol_valid, B);
+  for (int i = 0; i < B && !ctx->pol_have.empty(); ++i) ctx->pol_have[i] = (head[(size_t)(src ? src[i] : i) * 4 + 3] & HB_EPISODE_HAS_POLICY) ? 1 : 0;
+  CK(cudaStreamSynchronize(ctx->stream));
   return HB_OK;
 }
 

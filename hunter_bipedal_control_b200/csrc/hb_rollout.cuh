@@ -212,6 +212,51 @@ __global__ void rollout_record_kernel(int B, const __grid_constant__ RecordSlots
   }
 }
 
+// ---- episode snapshots (hb_episode_save_async / hb_episode_restore, hunter_b200.h)
+constexpr int EPISODE_MAX_SEGMENTS = 20;
+// One per-instance buffer of a snapshot row: the context's buffer (instance-major, `bytes` per instance, a multiple of 4) and the row's
+// 8-byte words first .. first + ceil(bytes / 8) - 1 that hold it. A null buffer is one the context never allocated: a save writes `fill`
+// in each of its 4-byte units, a restore skips it. by_row: the buffer is indexed by the row instead of the context instance (the headers a
+// save stages).
+struct EpisodeSegment {
+  char* buf;
+  uint32_t bytes, first, fill;
+  int32_t by_row;
+};
+struct EpisodeSegments {
+  int n;
+  uint32_t row_words;
+  EpisodeSegment seg[EPISODE_MAX_SEGMENTS];
+};
+
+// Save (restore == 0): row i <- instance src[i] of every segment. Restore: instance i <- row src[i]. src null: i. One thread per 8-byte
+// word of the B rows written or read, so that consecutive threads touch consecutive addresses of a row and of a segment; the copy goes in
+// 4-byte units because int32 segments (node modes, interval counts, goal index) leave the context's per-instance strides 4-byte aligned.
+// The padding of a row is written as zeros.
+__global__ void episode_copy_kernel(int B, const __grid_constant__ EpisodeSegments t, const int32_t* src, int restore, uint32_t* rows) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (size_t)B * t.row_words) return;
+  const int i = (int)(idx / t.row_words);
+  const uint32_t w = (uint32_t)(idx % t.row_words);
+  int k = 0;
+  while (k + 1 < t.n && w >= t.seg[k + 1].first) ++k;
+  const EpisodeSegment& s = t.seg[k];
+  const uint32_t off = (w - s.first) * 8;
+  const bool two = off + 4 < s.bytes;
+  const int other = src ? src[i] : i;
+  uint32_t* row = rows + ((size_t)(restore ? other : i) * t.row_words + w) * 2;
+  if (restore) {
+    if (!s.buf) return;
+    uint32_t* c = reinterpret_cast<uint32_t*>(s.buf + (size_t)i * s.bytes + off);
+    c[0] = row[0];
+    if (two) c[1] = row[1];
+  } else {
+    const uint32_t* c = s.buf ? reinterpret_cast<const uint32_t*>(s.buf + (size_t)(s.by_row ? i : other) * s.bytes + off) : nullptr;
+    row[0] = c ? c[0] : s.fill;
+    row[1] = !two ? 0u : c ? c[1] : s.fill;
+  }
+}
+
 // ---- estimated episodes (hb_rollout_estimated_batch_dev, hb_sim_read_sensors_batch_dev)
 
 // Philox4x32-10 (Salmon et al., SC'11): counter c encrypted under key (k0, k1), in place. Written out rather than taken from curand so that

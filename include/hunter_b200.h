@@ -430,8 +430,9 @@ int hb_rollout_set_goals(hb_ctx* ctx, int B, const hb_goal_schedule* goals);
  * resident solution for d == 0; the joint command law takes its planned contact from the adopted policy's mode (the reference reads the
  * reference manager's newest schedule there; a deviation). The plan inputs, the planner, the warm start, the estimator's contact flags
  * and goal capture read the newest plan, as the reference's reference manager does.
- * The adopted policy is per-instance context state like the captured goals, so a split episode continues exactly; snapshots
- * (hb_resident_read_batch / hb_resident_write_batch) do not include it. Range: 0 <= d <= mpc_every; an episode call whose setting has an
+ * The adopted policy is per-instance context state like the captured goals, so a split episode continues exactly; the resident
+ * snapshots (hb_resident_read_batch / hb_resident_write_batch) do not include it, the episode snapshots (hb_episode_save_async, below)
+ * do. Range: 0 <= d <= mpc_every; an episode call whose setting has an
  * entry above its mpc_every returns -1 before any launch, and so does a warm call (tick0 > 0) in which an instance with d >= 1 has never
  * adopted a policy. With no setting, or every latency 0, the episode calls issue exactly the launches they issue without one; with a
  * latency set they add one launch on each tick where an instance within the setting adopts, and one on the cold tick. */
@@ -889,6 +890,44 @@ int hb_estimator_fuse_odometry(hb_ctx* ctx, int B, const hb_kf_params* params, h
                                const uint8_t* contact_flag, double* rbd);
 int hb_estimator_fuse_odometry_async(hb_ctx* ctx, int B, const hb_kf_params* params, hb_kf_state* state, const double* pos, const uint8_t* has_msg,
                                      const uint8_t* contact_flag, double* rbd);
+
+/* ---- episode snapshots: each robot's whole closed-loop state in one device row (checkpoint, resume, fork) ----
+ * The episode calls continue across calls because part of an episode's state stays on the context between them. A snapshot row holds all
+ * of that state for one instance, so that an episode can stop and continue in another context or process, and so that many instances can
+ * start from one instance's exact mid-episode state (a fork).
+ * In a row: every per-instance buffer an episode call reads from an earlier call: the resident MPC solution (the warm start), the
+ * WeightedWbc fallback's previous solution, the planner's latest stance positions, the captured goal index and target, the adopted policy
+ * of the MRT split and the tracking camera's history and bias. Not in a row: the caller's buffers (rbd, act, estop, stats and, in estimated
+ * episodes, est and est_stats), which the caller saves itself, and configuration: the per-robot settings, the WBC settings and
+ * formulation, loaded task settings and recorded channels.
+ * Row layout (treated as opaque; hb_episode_state_bytes gives its size): a header of four int64 (horizon_N, event_nodes, the row's size in
+ * bytes, HB_EPISODE_HAS_* flags), then these segments, each padded to a multiple of 8 bytes: the resident solution (t0 double; x_traj
+ * (N+1) x 22 double; u_traj N x 22 double; on event-node contexts node_times (N+1) double; node modes (N+1) int32; on event-node contexts
+ * n_intervals int32, each of these padded), the fallback's previous solution (38 double), the stance positions (12 double), the captured
+ * goal index (int32, -1: none), the captured target (hb_target), the adopted policy (as the resident solution) and the camera state
+ * ((HB_ODOM_MAX_DELAY + 1) x 3 double history, 3 double bias). A segment whose buffer the context never allocated (no goals set, no odometry
+ * set, no policy adopted) saves as its cleared value: goal index -1, zeros elsewhere.
+ * hb_episode_save_async writes row i (device memory, B rows) from instance src[i] of the context (src NULL: instance i), flags from the
+ * context's bookkeeping. Asynchronous on the context's stream: src (host) is consumed when the call returns.
+ * hb_episode_restore sets instance i of the context from row src[i] of the n_rows rows (src NULL: row i). It reads the rows' headers back
+ * with one small synchronous copy before anything changes, and returns when the rows are written: a setting-like call, not a per-tick one.
+ * After it, instances [0, B) hold the rows' solution, fallback solution and adopted policy as their flags say, so that a warm episode call
+ * (tick0 > 0) passes its entry checks exactly when the rows would have passed them in the context that saved them. A restore writes the
+ * goal and camera state whether or not goals or odometry are set, allocating their buffers as their setting calls do; hb_rollout_set_goals
+ * and hb_rollout_set_odometry clear that state, so a restore must come after them.
+ * Return codes: -1 for a null context, B < 0, NULL rows with B > 0, a src entry outside [0, max_batch) (save) or [0, n_rows) (restore), a
+ * B > n_rows restore with src NULL, and on restore a row whose fingerprint (horizon_N, event_nodes, size) differs from this context's, a row
+ * without HB_EPISODE_HAS_SOLUTION, or fallback flags that would leave instances with a previous WBC solution that are not a prefix
+ * [0, k) of the context; -4 for B > max_batch. B == 0 does nothing. A rejected call changes nothing and launches nothing. Each call is one
+ * launch; without them an episode launches exactly what it launches without this feature. */
+#define HB_EPISODE_HEADER_BYTES 32
+#define HB_EPISODE_HAS_SOLUTION 1      /* the instance holds a resident MPC solution                                         */
+#define HB_EPISODE_HAS_FALLBACK 2      /* the WeightedWbc fallback holds a previous solution                                 */
+#define HB_EPISODE_HAS_POLICY 4        /* the instance has adopted a policy (MPC latency)                                    */
+/* bytes of one instance's row for this context's configuration; -1 for a null context */
+int64_t hb_episode_state_bytes(const hb_ctx* ctx);
+int hb_episode_save_async(hb_ctx* ctx, int B, const int32_t* src /*host, nullable*/, void* rows /*device, B rows*/);
+int hb_episode_restore(hb_ctx* ctx, int B, const int32_t* src /*host, nullable*/, int n_rows, const void* rows /*device, n_rows rows*/);
 int hb_rbd_to_centroidal_batch(hb_ctx* ctx, int B, const double* rbd, double* x);
 int hb_reference_expand_batch(hb_ctx* ctx, int B, const double* t0, const hb_reference* refs, double* x_ref, double* swing_ref,
                               int32_t* mode);
