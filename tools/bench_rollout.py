@@ -19,7 +19,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from episode_harness import MIN_HEIGHT, NOISE_SIGMAS, Episodes, gpu_identity, parser  # noqa: E402
+from episode_harness import Episodes, failure_checks, noise_ok, parser, report, sensor_noise  # noqa: E402
 from bench import DT, HORIZON_N, SEED, ClockSampler  # noqa: E402  (episode_harness put the repository root on the path)
 
 TICKS = 500
@@ -29,7 +29,7 @@ def main():
     ap = parser()
     ap.add_argument("--steps", type=int, default=5, help="timed episodes")
     args = ap.parse_args()
-    if args.sensor_noise < 0 or (args.sensor_noise and not args.estimator):
+    if not noise_ok(args):
         raise SystemExit("bench_rollout.py: --sensor-noise takes a scale >= 0 and needs --estimator")
     h = Episodes("bench_rollout.py", args, TICKS)
     hb, prm, B = h.hb, h.prm, h.B
@@ -54,18 +54,17 @@ def main():
     sim_s = TICKS * prm.period
     reasons = {name: int(((st["fail_reason"] & bit) != 0).sum()) for name, bit in hb.ROLLOUT_FAIL.items()}
     line = {"metric": "closed-loop episodes: simulated robot-seconds per wall-second (Hunter, MPC 100 Hz + WBC 500 Hz + plant)", "value": B * sim_s / (med * 1e-3),
-            "unit": "robot-s/s", "n_gpus": 1, "steps": len(runs), "warmup": 1, "higher_is_better": True, "dtype": "f64", "data": "synthetic",
+            "unit": "robot-s/s", **report(args, clocks, estimator=False), "steps": len(runs), "warmup": 1, "higher_is_better": True,
             "ms_per_episode": med, "ms_per_episode_range": [min(ms), max(ms)], "ms_per_mpc_period": med / cycles,
             "launches_per_mpc_period": runs[-1].launches / cycles, "gpu_launches": int(runs[-1].launches),
-            "upright_fraction": float((st["fail_tick"] == -1).mean()), "fail_reasons": reasons, "wbc": args.wbc,
+            "upright_fraction": float((st["fail_tick"] == -1).mean()), "fail_reasons": reasons,
             "same_outcome_every_episode": all(np.array_equal(r.stats, st) for r in runs),
             "stats": {"mpc_bad": int(st["mpc_bad"].sum()), "wbc_fallbacks": int(st["wbc_fallbacks"].sum()), "plan_rejects": int(st["plan_rejects"].sum()),
                       "max_abs_torque": float(st["max_abs_torque"].max())},
             "config": {"workload": "%d robots, %.1f s simulated (%d ticks of %.0f ms, %d MPC cycles), trot at 0.3 m/s from t = 0.1 s, initial poses of "
                                    "scenarios.random_initial_states(seed %d), N=%d dt=%.0f ms, one hb_rollout_batch_dev call per episode, device events "
                                    "around it" % (B, sim_s, TICKS, 1e3 * prm.period, cycles, SEED, HORIZON_N, 1e3 * DT),
-                       "failure_checks": "non-finite state, |roll| > pi/2, base z < %.2f m, emergency stop" % MIN_HEIGHT},
-            "gpu": gpu_identity(args.device), "clocks": clocks}
+                       "failure_checks": failure_checks()}}
     if args.estimator:
         ems = [r.ms for r in est_runs]
         est_st, es = est_runs[-1].stats, est_runs[-1].est_stats
@@ -81,7 +80,7 @@ def main():
             "stats": {"mpc_bad": int(est_st["mpc_bad"].sum()), "wbc_fallbacks": int(est_st["wbc_fallbacks"].sum()),
                       "plan_rejects": int(est_st["plan_rejects"].sum()), "max_abs_torque": float(est_st["max_abs_torque"].max())},
             "same_outcome_every_episode": all(np.array_equal(r.stats, est_st) and np.array_equal(r.est_stats, es) for r in est_runs),
-            "sensor_noise": {k: args.sensor_noise * v for k, v in NOISE_SIGMAS.items()}, "noise_seed": SEED,
+            **sensor_noise(args),
             "errors": "filter output against the true state entering each tick, counted while the robot is up: |v_hat - v| world base "
                       "velocity [m/s], |z_hat - z| [m]; rms over robots and ticks"}
     print(json.dumps(line))

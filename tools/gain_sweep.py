@@ -21,15 +21,13 @@ with the setting in force and without, with the card's name and power limit.
 import json
 import os
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from episode_harness import MIN_HEIGHT, NOISE_SIGMAS, Episodes, cells, gpu_identity, sweep_args  # noqa: E402
-from push_sweep import PUSH_DURATION, PUSH_T  # noqa: E402
-from bench import DT, HORIZON_N, SEED, ClockSampler  # noqa: E402
+from episode_harness import PUSH_DURATION, PUSH_T, Episodes, Tally, cell_members, cells, failure_checks, report, sweep_args, workload  # noqa: E402
+from bench import ClockSampler  # noqa: E402  (episode_harness put the repository root on the path)
 
 TICKS, NX, NY = 750, 8, 8
 DEFAULT_X, DEFAULT_Y = "swing_kp", "base_angular_kp"
@@ -72,64 +70,36 @@ def main():
     n_per = B // (NX * NY)
 
     def grid(shift):
-        """The records of every robot and, per cell (row-major), its robots, for the assignment shifted by `shift`."""
+        """The records of every robot for the assignment shifted by `shift`."""
         col, row = cells(B, NX, NY, shift)
-        recs = hb.make_controller_settings(B, **{xf: xs[col], yf: ys[row]})
-        members = [np.nonzero(row * NX + col == k)[0] for k in range(NX * NY)]
-        return recs, members
+        return hb.make_controller_settings(B, **{xf: xs[col], yf: ys[row]})
 
     # the grid, episode r on assignment shift r
-    surv, fb, n = np.zeros(NX * NY), np.zeros(NX * NY), np.zeros(NX * NY)
-    ctx.set_controller_settings(grid(0)[0])
-    h.episode()                                 # warm-up episode
-    for r in range(args.repeats):
-        recs, members = grid(r)
-        ctx.set_controller_settings(recs)
-        st = h.episode().stats
-        for k, m in enumerate(members):
-            surv[k] += (st["fail_tick"][m] < 0).sum(); fb[k] += st["wbc_fallbacks"][m].sum(); n[k] += len(m)
-    survival, fallbacks = surv / n, fb / n
+    tally = Tally(NX, NY)
+    for r, run in h.sweep(ctx.set_controller_settings, grid):
+        tally.add(*cells(B, NX, NY, r), run.stats)
+    survival, fallbacks = tally.survival().ravel(), (tally.fallbacks / tally.total).ravel()
     at = lambda k: {"cell": [int(k % NX), int(k // NX)], xf: float(xs[k % NX]), yf: float(ys[k // NX]), "survival": float(survival[k]),
                     "wbc_fallbacks_per_robot": float(fallbacks[k])}
     order = sorted(range(NX * NY), key=lambda k: (-survival[k], fallbacks[k], k))
     shipped_cell = [int(np.argmin(np.abs(np.log(xs / shipped[xf])))), int(np.argmin(np.abs(np.log(ys / shipped[yf]))))]
 
     # one call against 64 calls of B / 64 robots on the context's settings, alternated; assignment shift 0
-    recs, members = grid(0)
+    recs, members = grid(0), cell_members(B, NX, NY, 0)
     wbc0, gains0 = ctx.wbc_settings(), hb.HbPdGains.from_buffer_copy(bytes(prm.gains))
 
-    def one_call():
-        ctx.set_controller_settings(recs)
-        t0 = time.perf_counter()
-        run = h.episode()
-        return run, time.perf_counter() - t0
+    def set_cell(k):                            # with --push, a call's robots take the first B / 64 push schedules, which are all alike
+        ctx.set_wbc_settings(recs[members[k][0]].wbc)
+        prm.gains = recs[members[k][0]].gains
 
-    def per_cell_calls():
-        ctx.set_controller_settings(None)
-        runs, t0 = [], time.perf_counter()      # with --push, a call's robots take the first B / 64 push schedules, which are all alike
-        for k, m in enumerate(members):
-            ctx.set_wbc_settings(recs[m[0]].wbc)
-            prm.gains = recs[m[0]].gains
-            runs.append(h.episode(rows=m))
-        wall = time.perf_counter() - t0
+    def restore():
         ctx.set_wbc_settings(wbc0); prm.gains = gains0
-        return runs, wall
 
-    times = {"one_call_ms": [], "one_call_wall_ms": [], "per_cell_calls_ms": [], "per_cell_calls_wall_ms": []}
-    equal = True
     sampler = ClockSampler(args.device); sampler.start()
-    for _ in range(max(1, args.timed)):
-        one, w1 = one_call()
-        many, w64 = per_cell_calls()
-        times["one_call_ms"].append(one.ms); times["one_call_wall_ms"].append(1e3 * w1)
-        times["per_cell_calls_ms"].append(sum(r.ms for r in many)); times["per_cell_calls_wall_ms"].append(1e3 * w64)
-        for m, r in zip(members, many):
-            equal &= bool(np.array_equal(one.stats[m], r.stats) and np.array_equal(one.rbd[m], r.rbd))
+    timing = h.one_call_against_per_cell_calls(ctx.set_controller_settings, recs, set_cell, restore, members)
     clocks = sampler.stop()
-    timing = {k: float(np.median(v)) for k, v in times.items()}
-    timing.update({k + "_range": [min(v), max(v)] for k, v in times.items()})
-    timing.update(rounds=max(1, args.timed), launches_one_call=int(one.launches), launches_per_cell_calls=int(sum(r.launches for r in many)),
-                  cells_bitwise_equal=equal)
+    # workload() reads h.ticks, which the WBC kernel profile below sets to 50
+    sentence = workload(h, "; %d robots per cell, %d episodes (assignment shifted)" % (n_per, args.repeats))
 
     # the fused WBC kernel (hb_profile kind qp_ipm) per call on the whole batch, with the grid's setting in force and without
     h.ticks, wbc_ms = 50, {}
@@ -144,22 +114,14 @@ def main():
     ctx.set_controller_settings(None)
     timing.update(wbc_kernel_ms_per_call_set=wbc_ms["set"], wbc_kernel_ms_per_call_unset=wbc_ms["unset"])
 
-    line = {"metric": "controller gain sweep: survival of %d robots per cell over an 8 x 8 grid of %s x %s" % (n_per * args.repeats, xf, yf),
-            "value": float(survival[order[0]]), "unit": "fraction surviving (best cell)", "n_gpus": 1, "dtype": "f64", "data": "synthetic",
-            "estimator": bool(args.estimator), "wbc": args.wbc, "push_N": args.push,
-            "x": {"field": xf, "values": [float(v) for v in xs]}, "y": {"field": yf, "values": [float(v) for v in ys]},
-            "survival": survival.reshape(NY, NX).tolist(), "wbc_fallbacks_per_robot": fallbacks.reshape(NY, NX).tolist(),
-            "shipped_cell": at(shipped_cell[1] * NX + shipped_cell[0]), "best_cell": at(order[0]), "timing": timing,
-            "config": {"workload": "%d robots, %.1f s simulated (%d ticks of %.0f ms), trot at 0.3 m/s from t = 0.1 s, initial poses of "
-                                   "scenarios.random_initial_states(seed %d), N=%d dt=%.0f ms; %d robots per cell, %d episodes (assignment shifted)"
-                                   % (B, TICKS * prm.period, TICKS, 1e3 * prm.period, SEED, HORIZON_N, 1e3 * DT, n_per, args.repeats),
-                       "survival": "robots up at the end of the episode",
-                       "failure_checks": "non-finite state, |roll| > pi/2, base z < %.2f m, emergency stop" % MIN_HEIGHT},
-            "gpu": gpu_identity(args.device), "clocks": clocks}
-    if args.estimator:
-        line["sensor_noise"] = {k: args.sensor_noise * v for k, v in NOISE_SIGMAS.items()}
-        line["noise_seed"] = SEED
-    print(json.dumps(line))
+    print(json.dumps({
+        "metric": "controller gain sweep: survival of %d robots per cell over an 8 x 8 grid of %s x %s" % (n_per * args.repeats, xf, yf),
+        "value": float(survival[order[0]]), "unit": "fraction surviving (best cell)", **report(args, clocks), "push_N": args.push,
+        "x": {"field": xf, "values": [float(v) for v in xs]}, "y": {"field": yf, "values": [float(v) for v in ys]},
+        "survival": survival.reshape(NY, NX).tolist(), "wbc_fallbacks_per_robot": fallbacks.reshape(NY, NX).tolist(),
+        "shipped_cell": at(shipped_cell[1] * NX + shipped_cell[0]), "best_cell": at(order[0]), "timing": timing,
+        "config": {"workload": sentence,
+                   "survival": "robots up at the end of the episode", "failure_checks": failure_checks()}}))
 
 
 if __name__ == "__main__":

@@ -26,8 +26,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from episode_harness import GROUND, MIN_HEIGHT, NOISE_SIGMAS, Episodes, cells, gpu_identity, parser  # noqa: E402
-from bench import DT, HORIZON_N, SEED  # noqa: E402
+from episode_harness import GROUND, Episodes, cells, failure_checks, noise_ok, parser, report, workload  # noqa: E402
 
 TICKS, LOG_EVERY, V_CMD = 1000, 5, 0.3
 T_VEL, T_CLEAR = 0.5, 0.3
@@ -58,7 +57,7 @@ def main():
     args = ap.parse_args()
     periods, heights = axis(args.periods, "0.4:0.8:5", "periods"), axis(args.heights, "0.02:0.10:5", "heights")
     nx, ny = len(periods), len(heights)
-    if args.batch < nx * ny or args.repeats < 1 or args.sensor_noise < 0 or (args.sensor_noise and not args.estimator):
+    if args.batch < nx * ny or args.repeats < 1 or not noise_ok(args):
         raise SystemExit("gait_sweep.py: --batch >= %d, --repeats >= 1, --sensor-noise takes a scale >= 0 and needs --estimator" % (nx * ny))
     h = Episodes("gait_sweep.py", args, TICKS)
     hb, ctx, prm, B = h.hb, h.ctx, h.prm, h.B
@@ -102,26 +101,19 @@ def main():
                                     args.timed)
     ctx.set_planner_settings(None)
 
-    line = {"metric": "gait sweep: survival, velocity tracking and foot clearance over a %d x %d grid of trot period x swing height" % (nx, ny),
-            "value": float(survival[order[0]]), "unit": "fraction surviving (best cell)", "n_gpus": 1, "dtype": "f64", "data": "synthetic",
-            "estimator": bool(args.estimator), "wbc": args.wbc,
-            "periods_s": [float(p) for p in periods], "swing_heights_m": [float(v) for v in heights],
-            "survival": survival.reshape(ny, nx).tolist(), "velocity_error_rms_mps": vel_err.reshape(ny, nx).tolist(),
-            "clearance_m": clearance.reshape(ny, nx).tolist(), "plan_rejects": rejects.reshape(ny, nx).astype(int).tolist(),
-            "shipped_cell": at(shipped), "best_cell": at(order[0]), "timing": timing,
-            "config": {"workload": "%d robots, %.1f s simulated (%d ticks of %.0f ms), trot at %.1f m/s from t = 0.1 s, initial poses of "
-                                   "scenarios.random_initial_states(seed %d), N=%d dt=%.0f ms; %d or %d robots per cell, %d episodes (assignment shifted)"
-                                   % (B, TICKS * prm.period, TICKS, 1e3 * prm.period, V_CMD, SEED, HORIZON_N, 1e3 * DT, B // (nx * ny),
-                                      -(-B // (nx * ny)), args.repeats),
-                       "survival": "robots up at the end of the episode",
-                       "velocity_error": "RMS of the horizontal base velocity error in the heading frame, surviving robots, t >= %.1f s" % T_VEL,
-                       "clearance": "mean over surviving robots of the highest contact point above the ground, t >= %.1f s" % T_CLEAR,
-                       "failure_checks": "non-finite state, |roll| > pi/2, base z < %.2f m, emergency stop" % MIN_HEIGHT},
-            "gpu": gpu_identity(args.device), "clocks": clocks}
-    if args.estimator:
-        line["sensor_noise"] = {k: args.sensor_noise * v for k, v in NOISE_SIGMAS.items()}
-        line["noise_seed"] = SEED
-    print(json.dumps(line))
+    print(json.dumps({
+        "metric": "gait sweep: survival, velocity tracking and foot clearance over a %d x %d grid of trot period x swing height" % (nx, ny),
+        "value": float(survival[order[0]]), "unit": "fraction surviving (best cell)", **report(args, clocks),
+        "periods_s": [float(p) for p in periods], "swing_heights_m": [float(v) for v in heights],
+        "survival": survival.reshape(ny, nx).tolist(), "velocity_error_rms_mps": vel_err.reshape(ny, nx).tolist(),
+        "clearance_m": clearance.reshape(ny, nx).tolist(), "plan_rejects": rejects.reshape(ny, nx).astype(int).tolist(),
+        "shipped_cell": at(shipped), "best_cell": at(order[0]), "timing": timing,
+        "config": {"workload": workload(h, "; %d or %d robots per cell, %d episodes (assignment shifted)" % (B // (nx * ny), -(-B // (nx * ny)), args.repeats),
+                                        "trot at %.1f m/s from t = 0.1 s" % V_CMD),
+                   "survival": "robots up at the end of the episode",
+                   "velocity_error": "RMS of the horizontal base velocity error in the heading frame, surviving robots, t >= %.1f s" % T_VEL,
+                   "clearance": "mean over surviving robots of the highest contact point above the ground, t >= %.1f s" % T_CLEAR,
+                   "failure_checks": failure_checks()}}))
 
 
 if __name__ == "__main__":

@@ -27,8 +27,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from episode_harness import GROUND, MIN_HEIGHT, NOISE_SIGMAS, Episodes, cells, gpu_identity, parser  # noqa: E402
-from bench import DT, HORIZON_N, SEED  # noqa: E402  (episode_harness put the repository root on the path)
+from episode_harness import GROUND, Episodes, Tally, cells, failure_checks, report, sweep_args, workload  # noqa: E402
 
 DISTANCES = [0.25, 0.5, 1.0, 2.0]                        # [m]
 HEADINGS = [k * 45.0 for k in range(8)]                  # [deg], world frame
@@ -37,17 +36,11 @@ V_DISP, V_ROT = 0.5, 1.57                                # targetDisplacementVel
 
 
 def main():
-    ncell = len(DISTANCES) * len(HEADINGS)
-    ap = parser("robots per episode (a multiple of %d)" % ncell)
-    ap.add_argument("--repeats", type=int, default=1, help="episodes per grid (the robot -> cell assignment shifts between them)")
-    ap.add_argument("--timed", type=int, default=2, help="timed goal / zero-goal / unset episode triples")
-    ap.add_argument("--yaw-change", type=float, default=0.0, metavar="RAD", help="goal yaw - start yaw")
-    ap.add_argument("--settle", type=float, default=2.0, metavar="S", help="seconds after the longest reaching time")
-    args = ap.parse_args()
-    if (args.batch < ncell or args.batch % ncell or args.repeats < 1 or args.sensor_noise < 0 or (args.sensor_noise and not args.estimator)
-            or not args.settle >= 0.0 or not math.isfinite(args.yaw_change)):
-        raise SystemExit("goal_sweep.py: --batch a multiple of %d, --repeats >= 1, --settle >= 0, a finite --yaw-change, --sensor-noise takes a "
-                         "scale >= 0 and needs --estimator" % ncell)
+    def extra(ap):
+        ap.add_argument("--yaw-change", type=float, default=0.0, metavar="RAD", help="goal yaw - start yaw")
+        ap.add_argument("--settle", type=float, default=2.0, metavar="S", help="seconds after the longest reaching time")
+    args = sweep_args("goal_sweep.py", "timed goal / zero-goal / unset episode triples", len(DISTANCES) * len(HEADINGS), extra, repeats=1,
+                      timed=2, valid=lambda a: a.settle >= 0.0 and math.isfinite(a.yaw_change), needs="--settle >= 0, a finite --yaw-change, ")
     yaw_change, settle = args.yaw_change, args.settle
     reach_max = max(max(DISTANCES) / V_DISP, abs(yaw_change) / V_ROT)
     T_episode = GOAL_TIME + reach_max + settle
@@ -62,31 +55,21 @@ def main():
         g = np.c_[rbd0[:, 3] + d * np.cos(th), rbd0[:, 4] + d * np.sin(th), rbd0[:, 0] + yaw_change]
         return g, di, hi
 
-    def schedules(g):
-        return hb.make_goal_schedules(B, GOAL_TIME, g[:, None, :])
+    def schedules(shift):
+        return hb.make_goal_schedules(B, GOAL_TIME, goals_of(shift)[0][:, None, :])
 
     nd, nh = len(DISTANCES), len(HEADINGS)
     pos_err = [[[] for _ in range(nh)] for _ in range(nd)]
     yaw_err = [[[] for _ in range(nh)] for _ in range(nd)]
-    up = np.zeros((nd, nh), dtype=int)
-    total = np.zeros_like(up)
-    reasons = {name: 0 for name in hb.ROLLOUT_FAIL}
-    g0, _, _ = goals_of(0)
-    ctx.set_goals(schedules(g0))
-    h.episode()                                 # warm-up episode
-    for r in range(args.repeats):
+    tally = Tally(nh, nd)                       # [distance, heading]
+    for r, run in h.sweep(ctx.set_goals, schedules):
         g, di, hi = goals_of(r)
-        ctx.set_goals(schedules(g))
-        _, _, st, rbd, _ = h.episode()
-        ok = st["fail_tick"] < 0
-        pe = np.hypot(rbd[:, 3] - g[:, 0], rbd[:, 4] - g[:, 1])
-        ye = np.abs(np.mod(rbd[:, 0] - g[:, 2] + np.pi, 2 * np.pi) - np.pi)
-        np.add.at(total, (di, hi), 1)
-        np.add.at(up, (di, hi), ok.astype(int))
+        ok = run.stats["fail_tick"] < 0
+        pe = np.hypot(run.rbd[:, 3] - g[:, 0], run.rbd[:, 4] - g[:, 1])
+        ye = np.abs(np.mod(run.rbd[:, 0] - g[:, 2] + np.pi, 2 * np.pi) - np.pi)
+        tally.add(hi, di, run.stats)
         for i in np.nonzero(ok)[0]:
             pos_err[di[i]][hi[i]].append(float(pe[i])); yaw_err[di[i]][hi[i]].append(float(ye[i]))
-        for name, bit in hb.ROLLOUT_FAIL.items():
-            reasons[name] += int(((st["fail_reason"] & bit) != 0)[~ok].sum())
 
     def summary(p, y, n_up, n_total):
         p, y = np.array(p), np.array(y)
@@ -97,31 +80,25 @@ def main():
                         "within_5cm_0.1rad": float(((p < 0.05) & (y < 0.1)).mean())})
         return out
 
+    up, total = tally.up, tally.total
     per_distance = {str(d): summary(sum(pos_err[a], []), sum(yaw_err[a], []), up[a].sum(), total[a].sum()) for a, d in enumerate(DISTANCES)}
     per_cell = {"%g m / %g deg" % (d, hd): summary(pos_err[a][b], yaw_err[a][b], up[a, b], total[a, b])
                 for a, d in enumerate(DISTANCES) for b, hd in enumerate(HEADINGS)}
 
     # goal, zero-goal and unset episodes alternate
     none = hb.make_goal_schedules(B, np.zeros((B, 0)), np.zeros((B, 0, 3)))
-    runs, clocks, timing = h.alternate(ctx.set_goals, [("goals", schedules(g0)), ("zero_goals", none), ("unset", None)], args.timed)
-    timing.update({"launches_" + n: int(runs[n][-1].launches) for n in runs})
-    line = {"metric": "goals: fraction of the trotting robots within 5 cm and 0.1 rad of a goal 0.5 m away, %.1f s after it is given"
-                      % (T_episode - GOAL_TIME), "value": per_distance["0.5"].get("within_5cm_0.1rad"), "unit": "fraction",
-            "n_gpus": 1, "dtype": "f64", "data": "synthetic", "estimator": bool(args.estimator), "wbc": args.wbc,
-            "per_distance": per_distance, "per_cell": per_cell, "fail_reasons": reasons, "timing": timing,
-            "config": {"workload": "%d robots, %.2f s simulated (%d ticks of %.0f ms), trot with cmd_vel 0 from t = 0.1 s, initial poses of "
-                                   "scenarios.random_initial_states(seed %d), N=%d dt=%.0f ms; %d distances x %d headings, %d episodes"
-                                   % (B, T_episode, h.ticks, 1e3 * prm.period, SEED, HORIZON_N, 1e3 * DT, nd, nh, args.repeats),
-                       "goal": "given at t = %g s: start position + d (cos h, sin h), start yaw %+g rad; settle %g s after the longest reaching "
-                               "time (%g s)" % (GOAL_TIME, yaw_change, settle, reach_max),
-                       "errors": "over the robots still up at the end: |base xy - goal xy|, |wrap(base yaw - goal yaw)|",
-                       "failure_checks": "non-finite state, |roll| > pi/2, base z < %.2f m, emergency stop" % MIN_HEIGHT,
-                       "ground_m": GROUND},
-            "gpu": gpu_identity(args.device), "clocks": clocks}
-    if args.estimator:
-        line["sensor_noise"] = {k: args.sensor_noise * v for k, v in NOISE_SIGMAS.items()}
-        line["noise_seed"] = SEED
-    print(json.dumps(line))
+    runs, clocks, timing = h.alternate(ctx.set_goals, [("goals", schedules(0)), ("zero_goals", none), ("unset", None)], args.timed,
+                                       launches=True)
+    print(json.dumps({
+        "metric": "goals: fraction of the trotting robots within 5 cm and 0.1 rad of a goal 0.5 m away, %.1f s after it is given"
+                  % (T_episode - GOAL_TIME), "value": per_distance["0.5"].get("within_5cm_0.1rad"), "unit": "fraction",
+        **report(args, clocks), "per_distance": per_distance, "per_cell": per_cell, "fail_reasons": tally.reasons, "timing": timing,
+        "config": {"workload": workload(h, "; %d distances x %d headings, %d episodes" % (nd, nh, args.repeats), "trot with cmd_vel 0 from t = 0.1 s",
+                                        T_episode, 2),
+                   "goal": "given at t = %g s: start position + d (cos h, sin h), start yaw %+g rad; settle %g s after the longest reaching "
+                           "time (%g s)" % (GOAL_TIME, yaw_change, settle, reach_max),
+                   "errors": "over the robots still up at the end: |base xy - goal xy|, |wrap(base yaw - goal yaw)|",
+                   "failure_checks": failure_checks(), "ground_m": GROUND}}))
 
 
 if __name__ == "__main__":

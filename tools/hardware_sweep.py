@@ -25,14 +25,13 @@ offset, so this mode makes no comparison.
 import json
 import os
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from episode_harness import MIN_HEIGHT, NOISE_SIGMAS, Episodes, cells, gpu_identity, sweep_args  # noqa: E402
-from bench import DT, HORIZON_N, SEED, ClockSampler  # noqa: E402
+from episode_harness import NOISE_SIGMAS, Episodes, Tally, cell_members, cells, failure_checks, report, sweep_args, workload  # noqa: E402
+from bench import SEED, ClockSampler  # noqa: E402  (episode_harness put the repository root on the path)
 
 TICKS, NX, NY = 750, 8, 8
 DELAYS = 0.004 * np.arange(NX)                                      # [s]
@@ -54,45 +53,32 @@ def main():
         return {"sigma_" + k: scale * v for k, v in NOISE_SIGMAS.items()}
 
     def grid(shift):
-        """The records of every robot and, per cell (row-major), its robots, for the assignment shifted by `shift`."""
+        """The records of every robot for the assignment shifted by `shift`."""
         col, row = cells(B, NX, NY, shift)
         if args.offsets:
-            recs = hb.make_hardware_settings(B, accel_bias=np.c_[ACCEL_BIAS[col], np.zeros((B, 2))], orientation_offset=np.c_[np.zeros((B, 2)), ROLL_OFFSET[row]])
-        else:
-            recs = hb.make_hardware_settings(B, actuation_delay=DELAYS[col], **{k: SCALES[row] * v for k, v in sigmas(1.0).items()})
-        members = [np.nonzero(row * NX + col == k)[0] for k in range(NX * NY)]
-        return recs, members
-
-    def episode():
-        return h.episode(True, est_stats=True)
+            return hb.make_hardware_settings(B, accel_bias=np.c_[ACCEL_BIAS[col], np.zeros((B, 2))], orientation_offset=np.c_[np.zeros((B, 2)), ROLL_OFFSET[row]])
+        return hb.make_hardware_settings(B, actuation_delay=DELAYS[col], **{k: SCALES[row] * v for k, v in sigmas(1.0).items()})
 
     ref = None
     if args.offsets:
         ctx.set_hardware(None)
-        ref = episode()                          # ideal hardware: where each robot ends without offsets
-    surv, fb, n = np.zeros(NX * NY), np.zeros(NX * NY), np.zeros(NX * NY)
+        ref = h.episode(True, est_stats=True)   # ideal hardware: where each robot ends without offsets
+    tally = Tally(NX, NY)
     vel, hgt, cnt, perr = np.zeros(NX * NY), np.zeros(NX * NY), np.zeros(NX * NY), [[] for _ in range(NX * NY)]
-    ctx.set_hardware(grid(0)[0])
-    episode()                                    # warm-up episode
-    for r in range(args.repeats):
-        recs, members = grid(r)
-        ctx.set_hardware(recs)
-        run = episode()
+    for r, run in h.sweep(ctx.set_hardware, grid, estimated=True, est_stats=True):
         st, es = run.stats, run.est_stats
-        for k, m in enumerate(members):
-            up = m[st["fail_tick"][m] < 0]
-            surv[k] += len(up); fb[k] += st["wbc_fallbacks"][m].sum(); n[k] += len(m)
+        tally.add(*cells(B, NX, NY, r), st)
+        for k, m in enumerate(cell_members(B, NX, NY, r)):
             vel[k] += es["sum_sq_vel_err"][m].sum(); hgt[k] += es["sum_sq_height_err"][m].sum(); cnt[k] += es["count"][m].sum()
             if ref is not None:
+                up = m[st["fail_tick"][m] < 0]
                 perr[k] += list(np.hypot(*(run.rbd[up, 3:5] - ref.rbd[up, 3:5]).T))
-    survival, fallbacks = surv / n, fb / n
-    cnt = np.maximum(cnt, 1)
+    survival, cnt = tally.survival().ravel(), np.maximum(cnt, 1)
     axes = ({"field": "accel_bias[0]", "unit": "m/s^2", "values": ACCEL_BIAS.tolist()}, {"field": "orientation_offset[2]", "unit": "rad", "values": ROLL_OFFSET.tolist()}) \
         if args.offsets else ({"field": "actuation_delay", "unit": "s", "values": DELAYS.tolist()}, {"field": "sensor noise scale", "unit": "x NOISE_SIGMAS", "values": SCALES.tolist()})
     line = {"metric": "simulated hardware sweep: survival of %d robots per cell over an 8 x 8 grid of %s x %s" % (n_per * args.repeats, axes[0]["field"], axes[1]["field"]),
-            "value": float(survival.mean()), "unit": "fraction surviving (mean over cells)", "n_gpus": 1, "dtype": "f64", "data": "synthetic",
-            "wbc": args.wbc, "x": axes[0], "y": axes[1],
-            "survival": survival.reshape(NY, NX).tolist(), "wbc_fallbacks_per_robot": fallbacks.reshape(NY, NX).tolist()}
+            "value": float(survival.mean()), "unit": "fraction surviving (mean over cells)", "x": axes[0], "y": axes[1],
+            "survival": survival.reshape(NY, NX).tolist(), "wbc_fallbacks_per_robot": (tally.fallbacks / tally.total).tolist()}
     if args.offsets:
         line["final_position_error_m"] = {"median": [float(np.median(p)) if p else None for p in perr], "max": [float(np.max(p)) if p else None for p in perr]}
         for key in ("median", "max"):
@@ -105,54 +91,27 @@ def main():
     timing = {}
     if not args.offsets:
         # one call against 64 calls of B / 64 robots on the call's values, alternated; assignment shift 0
-        recs, members = grid(0)
         delay0, noise0 = prm.actuation_delay, hb.HbSensorNoise.from_buffer_copy(bytes(ep.noise))
 
-        def one_call():
-            ctx.set_hardware(recs)
-            t0 = time.perf_counter()
-            run = episode()
-            return run, time.perf_counter() - t0
+        def set_cell(k):
+            prm.actuation_delay = DELAYS[k % NX]
+            for name, v in NOISE_SIGMAS.items():
+                setattr(ep.noise, name, SCALES[k // NX] * v)
 
-        def per_cell_calls():
-            ctx.set_hardware(None)
-            runs, t0 = [], time.perf_counter()
-            for k, m in enumerate(members):
-                prm.actuation_delay = DELAYS[k % NX]
-                for name, v in NOISE_SIGMAS.items():
-                    setattr(ep.noise, name, SCALES[k // NX] * v)
-                runs.append(h.episode(True, est_stats=True, rows=m))
-            wall = time.perf_counter() - t0
+        def restore():
             prm.actuation_delay, ep.noise = delay0, noise0
-            return runs, wall
 
-        times = {"one_call_ms": [], "one_call_wall_ms": [], "per_cell_calls_ms": [], "per_cell_calls_wall_ms": []}
-        equal = True
-        for _ in range(max(1, args.timed)):
-            one, w1 = one_call()
-            many, w64 = per_cell_calls()
-            times["one_call_ms"].append(one.ms); times["one_call_wall_ms"].append(1e3 * w1)
-            times["per_cell_calls_ms"].append(sum(r.ms for r in many)); times["per_cell_calls_wall_ms"].append(1e3 * w64)
-            for m, r in zip(members, many):
-                equal &= bool(np.array_equal(one.stats[m], r.stats) and np.array_equal(one.rbd[m], r.rbd) and np.array_equal(one.est_stats[m], r.est_stats))
-        timing = {k: float(np.median(v)) for k, v in times.items()}
-        timing.update({k + "_range": [min(v), max(v)] for k, v in times.items()})
-        timing.update(rounds=max(1, args.timed), launches_one_call=int(one.launches), launches_per_cell_calls=int(sum(r.launches for r in many)),
-                      cells_bitwise_equal=equal)
+        timing = h.one_call_against_per_cell_calls(ctx.set_hardware, grid(0), set_cell, restore, cell_members(B, NX, NY, 0), est_stats=True)
     # the grid's records, records of the call's values on every robot and no setting, alternated, at 1 x NOISE_SIGMAS
     for name, v in NOISE_SIGMAS.items():
         setattr(ep.noise, name, v)
     call = hb.make_hardware_settings(B, actuation_delay=prm.actuation_delay, torque_limit=prm.torque_limit[:], **sigmas(1.0))
-    _, _, alt = h.alternate(ctx.set_hardware, [("grid_records", grid(0)[0]), ("call_value_records", call), ("unset", None)], args.timed)
-    timing["episode"] = alt
+    _, _, timing["episode"] = h.alternate(ctx.set_hardware, [("grid_records", grid(0)), ("call_value_records", call), ("unset", None)], args.timed)
     line["timing"] = timing
-    line["clocks"] = sampler.stop()
-    line["config"] = {"workload": "%d robots through the estimator, %.1f s simulated (%d ticks of %.0f ms), trot at 0.3 m/s from t = 0.1 s, initial poses of "
-                                  "scenarios.random_initial_states(seed %d), N=%d dt=%.0f ms; %d robots per cell, %d episodes (assignment shifted)"
-                                  % (B, TICKS * prm.period, TICKS, 1e3 * prm.period, SEED, HORIZON_N, 1e3 * DT, n_per, args.repeats),
+    line.update(report(args, sampler.stop(), estimator=False))
+    line["config"] = {"workload": workload(h, "; %d robots per cell, %d episodes (assignment shifted)" % (n_per, args.repeats), robots="robots through the estimator"),
                       "noise_sigmas_at_scale_1": NOISE_SIGMAS, "noise_seed": SEED, "survival": "robots up at the end of the episode",
-                      "failure_checks": "non-finite state, |roll| > pi/2, base z < %.2f m, emergency stop" % MIN_HEIGHT}
-    line["gpu"] = gpu_identity(args.device)
+                      "failure_checks": failure_checks()}
     print(json.dumps(line))
 
 

@@ -21,8 +21,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from episode_harness import GROUND, MIN_HEIGHT, NOISE_SIGMAS, Episodes, gpu_identity, parser  # noqa: E402
-from bench import DT, HORIZON_N, SEED  # noqa: E402  (episode_harness put the repository root on the path)
+from episode_harness import GROUND, Episodes, failure_checks, noise_ok, parser, report, workload  # noqa: E402
 
 LATENCIES = [0, 1, 2, 3, 4, 5]          # [ticks]
 TIMED_LATENCY = 4                       # about the 7.8 ms of one 1024-robot MPC step in README
@@ -35,7 +34,7 @@ def main():
     ap.add_argument("--push", type=float, default=0.0, metavar="N", help="world-y push on every robot [N], 0: none")
     ap.add_argument("--timed", type=int, default=3, help="timed latency / zero / unset episode triples")
     args = ap.parse_args()
-    if args.ticks < 1 or args.sensor_noise < 0 or (args.sensor_noise and not args.estimator) or not np.isfinite(args.push):
+    if args.ticks < 1 or not noise_ok(args) or not np.isfinite(args.push):
         raise SystemExit("latency_sweep.py: --ticks >= 1, a finite --push, --sensor-noise takes a scale >= 0 and needs --estimator")
     h = Episodes("latency_sweep.py", args, args.ticks)
     hb, ctx, prm, B = h.hb, h.ctx, h.prm, h.B
@@ -57,22 +56,16 @@ def main():
             "mpc_bad": int(st["mpc_bad"].sum()), "wbc_fallbacks": int(st["wbc_fallbacks"].sum()), "plan_rejects": int(st["plan_rejects"].sum()),
             "max_abs_torque": float(st["max_abs_torque"].max()), "ms_per_episode": run.ms}
     runs, clocks, timing = h.alternate(ctx.set_mpc_latencies, [("latency_%d" % TIMED_LATENCY, np.full(B, TIMED_LATENCY)),
-                                                               ("zero_latency", np.zeros(B)), ("unset", None)], args.timed)
-    timing.update({"launches_" + n: int(runs[n][-1].launches) for n in runs})
-    line = {"metric": "MPC latency: share of trotting robots that survive %.1f s with a %d-tick (%.0f ms) MPC latency"
-                      % (args.ticks * prm.period, TIMED_LATENCY, TIMED_LATENCY * 1e3 * prm.period),
-            "value": per_latency[str(TIMED_LATENCY)]["survival"], "unit": "fraction", "n_gpus": 1, "dtype": "f64", "data": "synthetic",
-            "estimator": bool(args.estimator), "wbc": args.wbc, "push_n": args.push, "per_latency": per_latency, "timing": timing,
-            "config": {"workload": "%d robots, %.2f s simulated (%d ticks of %.0f ms), trot at 0.3 m/s from t = 0.1 s, MPC every %d ticks, initial "
-                                   "poses of scenarios.random_initial_states(seed %d), N=%d dt=%.0f ms"
-                                   % (B, args.ticks * prm.period, args.ticks, 1e3 * prm.period, prm.mpc_every, SEED, HORIZON_N, 1e3 * DT),
-                       "push": ("world-y %g N at the base from t = %g s for %g s" % (args.push, PUSH_TIME, PUSH_DURATION)) if args.push else None,
-                       "failure_checks": "non-finite state, |roll| > pi/2, base z < %.2f m, emergency stop" % MIN_HEIGHT, "ground_m": GROUND},
-            "gpu": gpu_identity(args.device), "clocks": clocks}
-    if args.estimator:
-        line["sensor_noise"] = {k: args.sensor_noise * v for k, v in NOISE_SIGMAS.items()}
-        line["noise_seed"] = SEED
-    print(json.dumps(line))
+                                                               ("zero_latency", np.zeros(B)), ("unset", None)], args.timed,
+                                       launches=True)
+    print(json.dumps({
+        "metric": "MPC latency: share of trotting robots that survive %.1f s with a %d-tick (%.0f ms) MPC latency"
+                  % (args.ticks * prm.period, TIMED_LATENCY, TIMED_LATENCY * 1e3 * prm.period),
+        "value": per_latency[str(TIMED_LATENCY)]["survival"], "unit": "fraction", **report(args, clocks), "push_n": args.push,
+        "per_latency": per_latency, "timing": timing,
+        "config": {"workload": workload(h, "", "trot at 0.3 m/s from t = 0.1 s, MPC every %d ticks" % prm.mpc_every, digits=2),
+                   "push": ("world-y %g N at the base from t = %g s for %g s" % (args.push, PUSH_TIME, PUSH_DURATION)) if args.push else None,
+                   "failure_checks": failure_checks(), "ground_m": GROUND}}))
 
 
 if __name__ == "__main__":

@@ -16,7 +16,6 @@ The line also times, in the same invocation, a camera (100 Hz, 5 mm) against all
 events around the episode call, and reports the launch counts of the three (odometry adds no launch), whether the period-0 records give
 the outcome of no setting, and the card's name and power limit and the clocks sampled during the timed episodes.
 """
-import ctypes as C
 import json
 import os
 import sys
@@ -25,8 +24,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from episode_harness import MIN_HEIGHT, NOISE_SIGMAS, Episodes, cells, gpu_identity, parser  # noqa: E402
-from bench import DT, HORIZON_N, SEED  # noqa: E402  (episode_harness put the repository root on the path)
+from episode_harness import Episodes, cells, failure_checks, parser, report, sensor_noise, workload  # noqa: E402
 
 DISTANCES = [0.5, 1.0]                                   # [m]
 HEADINGS = [k * 45.0 for k in range(8)]                  # [deg], world frame
@@ -51,7 +49,7 @@ def main():
     args.estimator = True
     T_episode = GOAL_TIME + max(DISTANCES) / V_DISP + args.settle
     h = Episodes("odometry_sweep.py", args, 0)
-    hb, ctx, prm, B, rbd0, torch = h.hb, h.ctx, h.prm, h.B, h.rbd0, h.torch
+    hb, ctx, prm, B, rbd0 = h.hb, h.ctx, h.prm, h.B, h.rbd0
     h.ticks = int(round(T_episode / prm.period))
     h.cmds = hb.make_rollout_commands("trot", np.full(B, 0.1), [0.0], [[0.0, 0.0, 0.0, 0.0]])
     di, hi = cells(B, len(DISTANCES), len(HEADINGS), 0)
@@ -60,28 +58,10 @@ def main():
     ctx.set_goals(hb.make_goal_schedules(B, GOAL_TIME, goal[:, None, :]))
     n_log = -(-h.ticks // LOG_EVERY)
 
-    def logged_episode():
-        """One estimated episode with the true and estimated states logged every LOG_EVERY ticks: (stats, final rbd, log, est_log)."""
-        P = lambda t: C.c_void_p(t.data_ptr())             # noqa: E731
-        prm.log_every = LOG_EVERY
-        d_rbd = torch.from_numpy(rbd0).to(h.dev)
-        d_act = torch.zeros(B * C.sizeof(hb.HbActuationState), dtype=torch.uint8, device=h.dev)
-        d_estop = torch.zeros(B, dtype=torch.uint8, device=h.dev)
-        d_st = torch.from_numpy(hb.rollout_stats(B).view(np.uint8).copy()).to(h.dev)
-        d_est = torch.from_numpy(np.frombuffer(bytes(hb.estimation_states(B)), dtype=np.uint8).copy()).to(h.dev)
-        log = torch.zeros((B, n_log, 32), dtype=torch.float64, device=h.dev)
-        est_log = torch.zeros_like(log)
-        torch.cuda.synchronize(h.dev)
-        rc = h.lib.hb_rollout_estimated_batch_dev(ctx._h, B, C.c_int64(0), h.ticks, C.byref(prm), C.byref(h.ep), h.cmds, P(d_rbd), P(d_act), P(d_estop),
-                                                  P(d_st), P(d_est), None, P(log), P(est_log))
-        assert rc == 0, rc
-        ctx.sync()
-        prm.log_every = 0
-        return d_st.cpu().numpy().view(hb.ROLLOUT_STATS_DTYPE), d_rbd.cpu().numpy(), log.cpu().numpy(), est_log.cpu().numpy()
-
     def summary(setting):
         ctx.set_odometry(setting)
-        st, rbd, log, est_log = logged_episode()
+        run = h.episode(log_every=LOG_EVERY, est_log=True)
+        st, rbd, log, est_log = run.stats, run.rbd, run.log, run.est_log
         up = st["fail_tick"] < 0
         pe = np.hypot(rbd[:, 3] - goal[:, 0], rbd[:, 4] - goal[:, 1])
         ye = np.abs(np.mod(rbd[:, 0] - goal[:, 2] + np.pi, 2 * np.pi) - np.pi)
@@ -112,20 +92,17 @@ def main():
 
     # camera, period-0 records and no setting alternate
     runs, clocks, timing = h.alternate(ctx.set_odometry, [("odometry", hb.make_odometry_settings(B, 5, 0, 0.005)),
-                                                          ("zero_periods", hb.make_odometry_settings(B, 0)), ("unset", None)], args.timed)
-    timing.update({"launches_" + n: int(runs[n][-1].launches) for n in runs})
-    line = {"metric": "odometry: fraction of the surviving robots within 5 cm and 0.1 rad of a goal 0.5 m away through the estimator with a "
-                      "100 Hz, 5 mm tracking camera", "value": results["period 5 / delay 0 / noise 0.005 m"]["0.5"].get("within_5cm_0.1rad"),
-            "unit": "fraction", "n_gpus": 1, "dtype": "f64", "data": "synthetic", "wbc": args.wbc, "cameras": results, "timing": timing,
-            "config": {"workload": "%d robots, %.2f s simulated (%d ticks of %.0f ms), trot with cmd_vel 0 from t = 0.1 s, initial poses of "
-                                   "scenarios.random_initial_states(seed %d), N=%d dt=%.0f ms, through the estimator"
-                                   % (B, T_episode, h.ticks, 1e3 * prm.period, SEED, HORIZON_N, 1e3 * DT),
-                       "goal": "given at t = %g s: start position + d (cos h, sin h), d in %s m, h in 8 headings, start yaw" % (GOAL_TIME, DISTANCES),
-                       "errors": "goal: over the robots still up at the end; estimate: |est xy - true xy| every %d ticks while up" % LOG_EVERY,
-                       "failure_checks": "non-finite state, |roll| > pi/2, base z < %.2f m, emergency stop" % MIN_HEIGHT},
-            "sensor_noise": {k: args.sensor_noise * v for k, v in NOISE_SIGMAS.items()}, "noise_seed": SEED,
-            "gpu": gpu_identity(args.device), "clocks": clocks}
-    print(json.dumps(line))
+                                                          ("zero_periods", hb.make_odometry_settings(B, 0)), ("unset", None)], args.timed,
+                                       launches=True)
+    print(json.dumps({
+        "metric": "odometry: fraction of the surviving robots within 5 cm and 0.1 rad of a goal 0.5 m away through the estimator with a "
+                  "100 Hz, 5 mm tracking camera", "value": results["period 5 / delay 0 / noise 0.005 m"]["0.5"].get("within_5cm_0.1rad"),
+        "unit": "fraction", **report(args, clocks, estimator=False), "cameras": results, "timing": timing,
+        "config": {"workload": workload(h, ", through the estimator", "trot with cmd_vel 0 from t = 0.1 s", T_episode, 2),
+                   "goal": "given at t = %g s: start position + d (cos h, sin h), d in %s m, h in 8 headings, start yaw" % (GOAL_TIME, DISTANCES),
+                   "errors": "goal: over the robots still up at the end; estimate: |est xy - true xy| every %d ticks while up" % LOG_EVERY,
+                   "failure_checks": failure_checks()},
+        **sensor_noise(args)}))
 
 
 if __name__ == "__main__":

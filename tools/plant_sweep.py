@@ -26,8 +26,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from episode_harness import MIN_HEIGHT, NOISE_SIGMAS, Episodes, cells, gpu_identity, sweep_args  # noqa: E402
-from bench import DT, HORIZON_N, SEED  # noqa: E402  (episode_harness put the repository root on the path)
+from episode_harness import Episodes, Tally, cells, failure_checks, keyed, report, sweep_args, workload  # noqa: E402
 
 TICKS = 750
 MASSES = [0.5 * k for k in range(16)]                   # [kg]
@@ -52,55 +51,26 @@ def main():
         return hb.make_plant_variations(B, m, np.where(m[:, None] > 0, COM, 0.0), np.stack([box_inertia(x) for x in m]),
                                         friction_scale=np.array(FRICTION)[fi])
 
-    up = np.zeros((len(FRICTION), len(MASSES)), dtype=int)
-    total = np.zeros_like(up)
-    speed = np.zeros((len(FRICTION), len(MASSES)))
-    reasons = {name: 0 for name in hb.ROLLOUT_FAIL}
-    ctx.set_plant_variations(variations(0))
-    h.episode()                                 # warm-up episode
-    for r in range(args.repeats):
-        ctx.set_plant_variations(variations(r))
-        _, _, st, rbd, _ = h.episode()
-        mi, fi = cells(B, len(MASSES), len(FRICTION), r)
-        ok = st["fail_tick"] < 0
-        v = np.hypot(*(rbd[:, 3:5] - rbd0[:, 3:5]).T) / T_episode
-        np.add.at(total, (fi, mi), 1)
-        np.add.at(up, (fi, mi), ok.astype(int))
-        np.add.at(speed, (fi, mi), np.where(ok, v, 0.0))
-        for name, bit in hb.ROLLOUT_FAIL.items():
-            reasons[name] += int(((st["fail_reason"] & bit) != 0)[~ok].sum())
-    survival = {"%g" % f: {"%g" % m: float(up[a, b] / total[a, b]) for b, m in enumerate(MASSES)} for a, f in enumerate(FRICTION)}
-    mean_speed = {"%g" % f: {"%g" % m: (float(speed[a, b] / up[a, b]) if up[a, b] else None) for b, m in enumerate(MASSES)}
-                  for a, f in enumerate(FRICTION)}
-    heaviest = {}                               # per friction scale: the heaviest payload up to which every cell keeps >= 90 % survival
-    for a, f in enumerate(FRICTION):
-        heaviest["%g" % f] = None
-        for b, m in enumerate(MASSES):
-            if up[a, b] < 0.9 * total[a, b]:
-                break
-            heaviest["%g" % f] = m
+    tally = Tally(len(MASSES), len(FRICTION))
+    for r, run in h.sweep(ctx.set_plant_variations, variations):
+        tally.add(*cells(B, len(MASSES), len(FRICTION), r), run.stats, value=np.hypot(*(run.rbd[:, 3:5] - rbd0[:, 3:5]).T) / T_episode)
+    fk, mk = ["%g" % f for f in FRICTION], ["%g" % m for m in MASSES]
+    # per friction scale: the heaviest payload up to which every cell keeps >= 90 % survival
+    heaviest = dict(zip(fk, tally.largest(MASSES)))
 
     # varied, all-default and unset episodes alternate
     runs, clocks, timing = h.alternate(ctx.set_plant_variations, [("varied", variations(0)), ("default", hb.make_plant_variations(B)),
-                                                                  ("unset", None)], args.timed)
-    timing.update({"launches_" + n: int(runs[n][-1].launches) for n in runs})
-    line = {"metric": "model mismatch: the heaviest unmodelled payload (0.2 x 0.2 x 0.1 m box, CoM 0.1 m above the base) that >= 90 %% of the "
-                      "trotting robots carry for %.1f s, per friction scale" % T_episode, "value": heaviest.get("1"), "unit": "kg",
-            "n_gpus": 1, "dtype": "f64", "data": "synthetic", "estimator": bool(args.estimator), "wbc": args.wbc,
-            "heaviest_payload_90pct": heaviest, "survival": survival, "mean_speed_of_survivors_m_per_s": mean_speed, "fail_reasons": reasons,
-            "upright_fraction_unset": float((runs["unset"][-1].stats["fail_tick"] < 0).mean()), "timing": timing,
-            "config": {"workload": "%d robots, %.1f s simulated (%d ticks of %.0f ms), trot at 0.3 m/s from t = 0.1 s, initial poses of "
-                                   "scenarios.random_initial_states(seed %d), N=%d dt=%.0f ms; %d payload masses x %d friction scales, %d episodes"
-                                   % (B, T_episode, TICKS, 1e3 * prm.period, SEED, HORIZON_N, 1e3 * DT, len(MASSES), len(FRICTION), args.repeats),
-                       "payload": "solid box %g x %g x %g m, CoM (%g, %g, %g) m in the base frame" % (BOX + COM),
-                       "friction": "plant mu = scale x %g; the WBC's friction cone keeps its nominal coefficient" % prm.sim.friction_mu,
-                       "survival": "robots still up at the end of the episode",
-                       "failure_checks": "non-finite state, |roll| > pi/2, base z < %.2f m, emergency stop" % MIN_HEIGHT},
-            "gpu": gpu_identity(args.device), "clocks": clocks}
-    if args.estimator:
-        line["sensor_noise"] = {k: args.sensor_noise * v for k, v in NOISE_SIGMAS.items()}
-        line["noise_seed"] = SEED
-    print(json.dumps(line))
+                                                                  ("unset", None)], args.timed, launches=True)
+    print(json.dumps({
+        "metric": "model mismatch: the heaviest unmodelled payload (0.2 x 0.2 x 0.1 m box, CoM 0.1 m above the base) that >= 90 %% of the "
+                  "trotting robots carry for %.1f s, per friction scale" % T_episode, "value": heaviest.get("1"), "unit": "kg",
+        **report(args, clocks), "heaviest_payload_90pct": heaviest, "survival": keyed(fk, mk, tally.survival().tolist()),
+        "mean_speed_of_survivors_m_per_s": keyed(fk, mk, tally.mean()), "fail_reasons": tally.reasons,
+        "upright_fraction_unset": float((runs["unset"][-1].stats["fail_tick"] < 0).mean()), "timing": timing,
+        "config": {"workload": workload(h, "; %d payload masses x %d friction scales, %d episodes" % (len(MASSES), len(FRICTION), args.repeats)),
+                   "payload": "solid box %g x %g x %g m, CoM (%g, %g, %g) m in the base frame" % (BOX + COM),
+                   "friction": "plant mu = scale x %g; the WBC's friction cone keeps its nominal coefficient" % prm.sim.friction_mu,
+                   "survival": "robots still up at the end of the episode", "failure_checks": failure_checks()}}))
 
 
 if __name__ == "__main__":

@@ -26,12 +26,12 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from episode_harness import MIN_HEIGHT, NOISE_SIGMAS, Episodes, cells, gpu_identity, sweep_args  # noqa: E402
-from bench import DT, HORIZON_N, SEED  # noqa: E402  (episode_harness put the repository root on the path)
+from episode_harness import PUSH_DURATION, PUSH_T, Episodes, Tally, cells, failure_checks, report, sweep_args, workload  # noqa: E402
 
-TICKS, PUSH_T, PUSH_DURATION = 750, 0.5, 0.1
+TICKS = 750
 DIRECTIONS = {"+x": (1.0, 0.0, 0.0), "-x": (-1.0, 0.0, 0.0), "+y": (0.0, 1.0, 0.0), "-y": (0.0, -1.0, 0.0)}
 STEP_N, BLOCK, MAX_FORCE, SURVIVE = 10.0, 16, 1000.0, 0.9
+BLOCKS = int(MAX_FORCE // (BLOCK * STEP_N)) + 1          # grid blocks up to the first one that ends above MAX_FORCE
 
 
 def main():
@@ -41,44 +41,34 @@ def main():
     push_tick = int(round(PUSH_T / prm.period))
 
     def push_cells(block, shift):
-        """(direction index, magnitude) of every robot for grid block `block`, assignment shifted by `shift`."""
+        """(magnitude index, direction index) of every robot for grid block `block`, assignment shifted by `shift`."""
         c, d = cells(B, BLOCK, len(DIRECTIONS), shift)
-        return d, (block * BLOCK + c) * STEP_N
+        return block * BLOCK + c, d
 
     def schedules(block, shift):
-        d, mag = push_cells(block, shift)
+        k, d = push_cells(block, shift)
         dirs = np.array(list(DIRECTIONS.values()))
-        return hb.make_push_schedules(B, PUSH_T, PUSH_DURATION, (dirs[d] * mag[:, None])[:, None, :])
+        return hb.make_push_schedules(B, PUSH_T, PUSH_DURATION, (dirs[d] * (k * STEP_N)[:, None])[:, None, :])
 
     names = list(DIRECTIONS)
-    up = {n: {} for n in names}
-    survived = {n: {} for n in names}
-    reasons = {name: 0 for name in hb.ROLLOUT_FAIL}
+    tally = Tally(BLOCKS * BLOCK, len(names))
     ctx.set_pushes(schedules(0, 0))
     h.episode()                                 # warm-up episode
-    block = 0
-    while True:
+    for block in range(BLOCKS):
         for r in range(args.repeats):
             ctx.set_pushes(schedules(block, r))
             st = h.episode().stats
-            d, mag = push_cells(block, r)
-            was_up = (st["fail_tick"] < 0) | (st["fail_tick"] > push_tick)
-            ok = st["fail_tick"] < 0
-            for i in np.nonzero(was_up)[0]:
-                key = "%g" % mag[i]
-                up[names[d[i]]][key] = up[names[d[i]]].get(key, 0) + 1
-                survived[names[d[i]]][key] = survived[names[d[i]]].get(key, 0) + int(ok[i])
-                for name, bit in hb.ROLLOUT_FAIL.items():
-                    reasons[name] += int(not ok[i] and (st["fail_reason"][i] & bit) != 0)
-        top = "%g" % ((block + 1) * BLOCK * STEP_N - STEP_N)
-        if (block + 1) * BLOCK * STEP_N > MAX_FORCE or all(survived[n].get(top, 0) < SURVIVE * max(up[n].get(top, 0), 1) for n in names):
+            tally.add(*push_cells(block, r), st, counts=(st["fail_tick"] < 0) | (st["fail_tick"] > push_tick))
+        top = (block + 1) * BLOCK - 1
+        if all(tally.up[:, top] < SURVIVE * np.maximum(tally.total[:, top], 1)):
             break
-        block += 1
 
-    survival = {n: {k: survived[n][k] / up[n][k] for k in sorted(up[n], key=float)} for n in names}
-    largest = {}
-    for n in names:
-        good = [float(k) for k, f in survival[n].items() if f >= SURVIVE]
+    fractions, survival, up, largest = tally.survival(), {}, {}, {}
+    for a, n in enumerate(names):                # the magnitudes at which some robot was up when the push began
+        ks = np.nonzero(tally.total[a])[0]
+        survival[n] = {"%g" % (k * STEP_N): float(fractions[a, k]) for k in ks}
+        up[n] = {"%g" % (k * STEP_N): int(tally.total[a, k]) for k in ks}
+        good = [float(k * STEP_N) for k in ks if fractions[a, k] >= SURVIVE]
         largest[n] = max(good) if good else None
 
     # pushed, zero-force (schedules set, the trajectories of the unpushed batch: the cost of the wrench path alone) and unpushed episodes
@@ -87,22 +77,16 @@ def main():
     runs, clocks, timing = h.alternate(ctx.set_pushes, [("pushed", schedules(0, 0)), ("zero_force", zero), ("unpushed", None)], args.timed)
     timing.update(launches_pushed=int(runs["pushed"][-1].launches), launches_unpushed=int(runs["unpushed"][-1].launches))
     known = [v for v in largest.values() if v is not None]
-    line = {"metric": "push recovery: the largest %.1f s world-frame push at the base, over the four horizontal directions, that >= 90 %% of the "
-                      "trotting robots survive" % PUSH_DURATION, "value": min(known) if len(known) == len(names) else None, "unit": "N",
-            "n_gpus": 1, "dtype": "f64", "data": "synthetic", "estimator": bool(args.estimator), "wbc": args.wbc,
-            "largest_force_90pct": largest, "survival": survival, "robots_up_at_push": up, "fail_reasons_after_push": reasons,
-            "upright_fraction_unpushed": float((runs["unpushed"][-1].stats["fail_tick"] < 0).mean()), "timing": timing,
-            "config": {"workload": "%d robots, %.1f s simulated (%d ticks of %.0f ms), trot at 0.3 m/s from t = 0.1 s, initial poses of "
-                                   "scenarios.random_initial_states(seed %d), N=%d dt=%.0f ms; one push per robot at t = %.1f s for %.1f s, %d "
-                                   "episodes per grid block of %d magnitudes x 4 directions" % (B, TICKS * prm.period, TICKS, 1e3 * prm.period, SEED,
-                                                                                                HORIZON_N, 1e3 * DT, PUSH_T, PUSH_DURATION, args.repeats, BLOCK),
-                       "survival": "robots up when the push began (fail_tick < 0 or after tick %d) that are still up at the end" % push_tick,
-                       "failure_checks": "non-finite state, |roll| > pi/2, base z < %.2f m, emergency stop" % MIN_HEIGHT},
-            "gpu": gpu_identity(args.device), "clocks": clocks}
-    if args.estimator:
-        line["sensor_noise"] = {k: args.sensor_noise * v for k, v in NOISE_SIGMAS.items()}
-        line["noise_seed"] = SEED
-    print(json.dumps(line))
+    print(json.dumps({
+        "metric": "push recovery: the largest %.1f s world-frame push at the base, over the four horizontal directions, that >= 90 %% of the "
+                  "trotting robots survive" % PUSH_DURATION, "value": min(known) if len(known) == len(names) else None, "unit": "N",
+        **report(args, clocks), "largest_force_90pct": largest, "survival": survival,
+        "robots_up_at_push": up, "fail_reasons_after_push": tally.reasons,
+        "upright_fraction_unpushed": float((runs["unpushed"][-1].stats["fail_tick"] < 0).mean()), "timing": timing,
+        "config": {"workload": workload(h, "; one push per robot at t = %.1f s for %.1f s, %d episodes per grid block of %d magnitudes x 4 directions"
+                                        % (PUSH_T, PUSH_DURATION, args.repeats, BLOCK)),
+                   "survival": "robots up when the push began (fail_tick < 0 or after tick %d) that are still up at the end" % push_tick,
+                   "failure_checks": failure_checks()}}))
 
 
 if __name__ == "__main__":

@@ -22,8 +22,8 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from episode_harness import MIN_HEIGHT, Episodes, gpu_identity, parser  # noqa: E402
-from bench import DT, HORIZON_N, SEED, ClockSampler  # noqa: E402
+from episode_harness import Episodes, failure_checks, parser, report, workload  # noqa: E402
+from bench import ClockSampler  # noqa: E402  (episode_harness put the repository root on the path)
 
 TICKS = 750
 SPEEDS = np.array([0.1, 0.2, 0.3, 0.4, 0.5])      # commanded forward speed [m/s]
@@ -43,7 +43,7 @@ def main():
     per_tick = {call: sum(w * np.dtype(t).itemsize for n, (_, t, w) in hb.CHANNELS.items() if call == "estimated" or n != "sensors")
                 for call in ("truth", "estimated")}
     line = {"metric": "recorded channels: overhead of recording every channel on every tick of %d robots over %.1f s" % (B, TICKS * prm.period),
-            "unit": "ms per episode", "n_gpus": 1, "dtype": "f64", "data": "synthetic", "wbc": args.wbc}
+            "unit": "ms per episode"}
     saved = {}
     sampler = ClockSampler(args.device); sampler.start()
     for call, estimated in (("truth", False), ("estimated", True)):
@@ -85,14 +85,11 @@ def main():
         if args.out:
             saved.update({"%s/%s" % (call, n): t.cpu().numpy() for n, t in bufs.items() if estimated or n != "sensors"})
             saved["%s/log" % call] = rec.log
-    line["clocks"] = sampler.stop()
-    line["value"] = line["truth"]["recording_overhead_ms"]
-    line["config"] = {"workload": "%d robots, %.1f s simulated (%d ticks of %.0f ms), trot from t = 0.1 s at SPEEDS[i %% 5] = %s m/s, initial poses of "
-                                  "scenarios.random_initial_states(seed %d), N=%d dt=%.0f ms, no sensor noise; every channel and the log on every tick"
-                                  % (B, TICKS * prm.period, TICKS, 1e3 * prm.period, SPEEDS.tolist(), SEED, HORIZON_N, 1e3 * DT),
-                      "failure_checks": "non-finite state, |roll| > pi/2, base z < %.2f m, emergency stop" % MIN_HEIGHT,
+    line.update(report(args, sampler.stop(), estimator=False), value=line["truth"]["recording_overhead_ms"])
+    line["config"] = {"workload": workload(h, ", no sensor noise; every channel and the log on every tick",
+                                           "trot from t = 0.1 s at SPEEDS[i %% 5] = %s m/s" % SPEEDS.tolist()),
+                      "failure_checks": failure_checks(),
                       "cost_of_transport": "sum over ticks and joints of |tau q_dot| dt / (m g horizontal distance), robots that stayed up"}
-    line["gpu"] = gpu_identity(args.device)
     if args.out:
         np.savez(args.out, **saved)
     print(json.dumps(line))

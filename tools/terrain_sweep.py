@@ -35,8 +35,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from episode_harness import GROUND, MIN_HEIGHT, NOISE_SIGMAS, Episodes, cells, gpu_identity, sweep_args  # noqa: E402
-from bench import DT, HORIZON_N, SEED  # noqa: E402  (episode_harness put the repository root on the path)
+from episode_harness import GROUND, Episodes, Tally, cells, failure_checks, keyed, report, sweep_args, workload  # noqa: E402
 
 TICKS = 750
 KINDS = ["step_up", "step_down", "incline", "decline"]
@@ -80,58 +79,30 @@ def main():
         origin, h = terrain_heights(rbd0, np.array(KINDS)[ki], np.array(MAGNITUDES)[mi], step_ahead, ramp_ahead)
         return hb.make_terrains(B, h, SPACING, origin)
 
-    up = np.zeros((len(KINDS), len(MAGNITUDES)), dtype=int)
-    total = np.zeros_like(up)
-    speed = np.zeros((len(KINDS), len(MAGNITUDES)))
-    reasons = {name: 0 for name in hb.ROLLOUT_FAIL}
-    ctx.set_terrains(terrains(0))
-    h.episode()                                 # warm-up episode
-    for r in range(args.repeats):
-        ctx.set_terrains(terrains(r))
-        _, _, st, rbd, _ = h.episode()
-        mi, ki = cells(B, len(MAGNITUDES), len(KINDS), r)
-        ok = st["fail_tick"] < 0
-        v = np.hypot(*(rbd[:, 3:5] - rbd0[:, 3:5]).T) / T_episode
-        np.add.at(total, (ki, mi), 1)
-        np.add.at(up, (ki, mi), ok.astype(int))
-        np.add.at(speed, (ki, mi), np.where(ok, v, 0.0))
-        for name, bit in hb.ROLLOUT_FAIL.items():
-            reasons[name] += int(((st["fail_reason"] & bit) != 0)[~ok].sum())
-    survival = {k: {str(m): float(up[a, b] / total[a, b]) for b, m in enumerate(MAGNITUDES)} for a, k in enumerate(KINDS)}
-    mean_speed = {k: {str(m): (float(speed[a, b] / up[a, b]) if up[a, b] else None) for b, m in enumerate(MAGNITUDES)} for a, k in enumerate(KINDS)}
-    largest = {}                                # per kind: the largest magnitude up to which every cell keeps >= 90 % survival
-    for a, k in enumerate(KINDS):
-        largest[k] = None
-        for b, m in enumerate(MAGNITUDES):
-            if up[a, b] < 0.9 * total[a, b]:
-                break
-            largest[k] = m
+    tally = Tally(len(MAGNITUDES), len(KINDS))
+    for r, run in h.sweep(ctx.set_terrains, terrains):
+        tally.add(*cells(B, len(MAGNITUDES), len(KINDS), r), run.stats, value=np.hypot(*(run.rbd[:, 3:5] - rbd0[:, 3:5]).T) / T_episode)
+    mk = [str(m) for m in MAGNITUDES]
+    largest = dict(zip(KINDS, tally.largest(MAGNITUDES)))   # per kind: the largest magnitude up to which every cell keeps >= 90 % survival
 
     # terrain, flat-terrain and unset episodes alternate
     flat_origin, flat_h = terrain_heights(rbd0, np.full(B, "step_up"), np.zeros(B), step_ahead, ramp_ahead)
     flat = hb.make_terrains(B, flat_h, SPACING, flat_origin)
-    runs, clocks, timing = h.alternate(ctx.set_terrains, [("terrain", terrains(0)), ("flat", flat), ("unset", None)], args.timed)
-    timing.update({"launches_" + n: int(runs[n][-1].launches) for n in runs})
-    line = {"metric": "terrain: the highest step [cm] that >= 90 %% of the trotting robots cross blind within %.1f s; per kind (steps in cm, "
-                      "slopes in degrees) under largest_magnitude_90pct" % T_episode, "value": largest["step_up"], "unit": "cm",
-            "n_gpus": 1, "dtype": "f64", "data": "synthetic", "estimator": bool(args.estimator), "wbc": args.wbc,
-            "largest_magnitude_90pct": largest, "survival": survival, "mean_speed_of_survivors_m_per_s": mean_speed, "fail_reasons": reasons,
-            "upright_fraction_unset": float((runs["unset"][-1].stats["fail_tick"] < 0).mean()), "timing": timing,
-            "config": {"workload": "%d robots, %.1f s simulated (%d ticks of %.0f ms), trot at 0.3 m/s from t = 0.1 s, initial poses of "
-                                   "scenarios.random_initial_states(seed %d), N=%d dt=%.0f ms; %d kinds x %d magnitudes, %d episodes"
-                                   % (B, T_episode, TICKS, 1e3 * prm.period, SEED, HORIZON_N, 1e3 * DT, len(KINDS), len(MAGNITUDES), args.repeats),
-                       "terrain": "%d x %d height field at %g m centred on the start, ground %g m under the start; steps with the edge %g m "
-                                  "ahead (a ramp one cell wide), slopes starting %g m ahead, across the initial heading"
-                                  % (GRID, GRID, SPACING, GROUND, STEP_AHEAD, RAMP_AHEAD),
-                       "robots_with_features_moved_ahead": {"step": int((step_ahead > STEP_AHEAD).sum()), "ramp": int((ramp_ahead > RAMP_AHEAD).sum()),
-                                                            "max_step_ahead_m": float(step_ahead.max()), "max_ramp_ahead_m": float(ramp_ahead.max())},
-                       "survival": "robots still up at the end of the episode",
-                       "failure_checks": "non-finite state, |roll| > pi/2, base z above the terrain < %.2f m, emergency stop" % MIN_HEIGHT},
-            "gpu": gpu_identity(args.device), "clocks": clocks}
-    if args.estimator:
-        line["sensor_noise"] = {k: args.sensor_noise * v for k, v in NOISE_SIGMAS.items()}
-        line["noise_seed"] = SEED
-    print(json.dumps(line))
+    runs, clocks, timing = h.alternate(ctx.set_terrains, [("terrain", terrains(0)), ("flat", flat), ("unset", None)], args.timed, launches=True)
+    print(json.dumps({
+        "metric": "terrain: the highest step [cm] that >= 90 %% of the trotting robots cross blind within %.1f s; per kind (steps in cm, "
+                  "slopes in degrees) under largest_magnitude_90pct" % T_episode, "value": largest["step_up"], "unit": "cm",
+        **report(args, clocks), "largest_magnitude_90pct": largest, "survival": keyed(KINDS, mk, tally.survival().tolist()),
+        "mean_speed_of_survivors_m_per_s": keyed(KINDS, mk, tally.mean()), "fail_reasons": tally.reasons,
+        "upright_fraction_unset": float((runs["unset"][-1].stats["fail_tick"] < 0).mean()), "timing": timing,
+        "config": {"workload": workload(h, "; %d kinds x %d magnitudes, %d episodes" % (len(KINDS), len(MAGNITUDES), args.repeats)),
+                   "terrain": "%d x %d height field at %g m centred on the start, ground %g m under the start; steps with the edge %g m "
+                              "ahead (a ramp one cell wide), slopes starting %g m ahead, across the initial heading"
+                              % (GRID, GRID, SPACING, GROUND, STEP_AHEAD, RAMP_AHEAD),
+                   "robots_with_features_moved_ahead": {"step": int((step_ahead > STEP_AHEAD).sum()), "ramp": int((ramp_ahead > RAMP_AHEAD).sum()),
+                                                        "max_step_ahead_m": float(step_ahead.max()), "max_ramp_ahead_m": float(ramp_ahead.max())},
+                   "survival": "robots still up at the end of the episode",
+                   "failure_checks": failure_checks("base z above the terrain")}}))
 
 
 if __name__ == "__main__":
