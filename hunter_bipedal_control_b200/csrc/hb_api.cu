@@ -397,7 +397,8 @@ const char* hb_strerror(int code) {
 int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
   // horizon cap: the warm shift stages one instance's previous trajectories in shared memory ((2N+1) x 22 doubles <= 227 KB); its
   // kernel is opted in once at the cap below, whatever this context's horizon
-  if (!cfg || !out || cfg->horizon_N < 1 || cfg->horizon_N > HB_MAX_HORIZON || cfg->max_batch < 1 || !(cfg->dt > 0.0) || cfg->time_horizon < 0.0) return HB_EINVAL;
+  if (!cfg || !out || cfg->horizon_N < 1 || cfg->horizon_N > HB_MAX_HORIZON || cfg->max_batch < 1 || !(cfg->dt > 0.0) || cfg->time_horizon < 0.0 ||
+      cfg->line_search_max_trials < 1) return HB_EINVAL;
   hb_ctx* ctx = new (std::nothrow) hb_ctx();
   if (!ctx) return HB_ENOMEM;
   memset(ctx, 0, sizeof(*ctx));

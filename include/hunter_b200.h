@@ -50,7 +50,9 @@ typedef struct {
   int32_t max_batch;     /* capacity of the context's scratch buffers                             */
   double wbc_rho;        /* Tikhonov weight that defines the least-norm WBC optimum (qpOASES setToMPC regularisation) */
   int32_t qp_max_iter;   /* interior-point iteration cap                                          */
-  int32_t line_search_max_trials; /* alpha = 1, 1/2, ... >= 1e-4 -> 14                            */
+  int32_t line_search_max_trials; /* trials of the filter line search, alpha = 1, 1/2, ...; >= 1 (hb_create rejects less:
+                                     a line search of no trials never steps). Default 14; alpha >= 1e-4 ends the search at
+                                     14 trials, so caps above 14 act as 14                                               */
   double time_horizon;   /* mpc.timeHorizon [s] (task.info:144 0.8); 0 = horizon_N * dt. Used by the event-node grid */
   int32_t event_nodes;   /* 1: the resident cycle discretises [t0, t0 + time_horizon] like ocs2::timeDiscretizationWithEvents
                             (steps of dt, a node on every mode switch, grid re-anchored there, last node = final time); horizon_N is

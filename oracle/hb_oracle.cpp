@@ -480,8 +480,9 @@ Perf performance(const hbo_horizon& hz, const double* xt, const double* ut, cons
   return pf;
 }
 
+// max_trials caps the line search's trials like hb_config.line_search_max_trials; record (nullable) receives one row per trial evaluated
 void mpc_iteration(const hbo_horizon& hz, const double* x0, const double* x_ref, const double* swing, const int32_t* mode,
-                   double* xt, double* ut, hbo_solve_info* info) {
+                   double* xt, double* ut, hbo_solve_info* info, int max_trials = 14, hbo_ls_trial* record = nullptr) {
   const int N = hz.N;
   for (int i = 0; i < NX; ++i) xt[i] = x0[i];
   std::vector<NodeGain> gains(N);
@@ -521,20 +522,23 @@ void mpc_iteration(const hbo_horizon& hz, const double* x0, const double* x_ref,
   for (double v : dx) finite = finite && std::isfinite(v);
   for (double v : du) finite = finite && std::isfinite(v);
   if (finite) {
-    do {
+    while (alpha >= alpha_min && trials < max_trials) {
       for (size_t i = 0; i < xn.size(); ++i) xn[i] = xt[i] + alpha * dx[i];
       for (size_t i = 0; i < un.size(); ++i) un[i] = ut[i] + alpha * du[i];
       pn = performance(hz, xn.data(), un.data(), x_ref, swing, mode);
-      ++trials;
       const double v1 = total_violation(pn);
       const double am = alpha * armijo;
       bool acc;
-      if (v1 > HB_SQP_G_MAX) acc = v1 < (1.0 - gamma_c) * v0;
-      else if (v1 < HB_SQP_G_MIN && v0 < HB_SQP_G_MIN && am < 0.0) acc = pn.merit < base.merit + armijoFactor * am;
-      else acc = pn.merit < (base.merit - gamma_c * v0) || v1 < (1.0 - gamma_c) * v0;
-      if (std::isfinite(pn.merit) && std::isfinite(v1) && acc) { accepted = true; break; }
+      int branch;
+      if (v1 > HB_SQP_G_MAX) { branch = HBO_LS_VIOLATION; acc = v1 < (1.0 - gamma_c) * v0; }
+      else if (v1 < HB_SQP_G_MIN && v0 < HB_SQP_G_MIN && am < 0.0) { branch = HBO_LS_ARMIJO; acc = pn.merit < base.merit + armijoFactor * am; }
+      else { branch = HBO_LS_FILTER; acc = pn.merit < (base.merit - gamma_c * v0) || v1 < (1.0 - gamma_c) * v0; }
+      acc = std::isfinite(pn.merit) && std::isfinite(v1) && acc;
+      if (record) record[trials] = hbo_ls_trial{alpha, pn.merit, v1, branch, acc ? 1 : 0};
+      ++trials;
+      if (acc) { accepted = true; break; }
       alpha *= alpha_decay;
-    } while (alpha >= alpha_min);
+    }
   }
   if (accepted) {
     std::copy(xn.begin(), xn.end(), xt);
@@ -986,10 +990,10 @@ void hbo_node_lq(double dt, const double* x, const double* u, const double* xn, 
   *m = lq.m; *cost = lq.cost;
 }
 
-void hbo_mpc_iteration(const hbo_horizon* hz, const double* x0, const double* x_ref, const double* swing, const int32_t* mode,
-                       double* x_traj, double* u_traj, hbo_solve_info* info) {
+void hbo_mpc_iteration(const hbo_horizon* hz, int max_trials, const double* x0, const double* x_ref, const double* swing, const int32_t* mode,
+                       double* x_traj, double* u_traj, hbo_solve_info* info, hbo_ls_trial* trials) {
   hbo_init();
-  mpc_iteration(*hz, x0, x_ref, swing, mode, x_traj, u_traj, info);
+  mpc_iteration(*hz, x0, x_ref, swing, mode, x_traj, u_traj, info, max_trials, trials);
 }
 
 // LeggedRobotInitializer::compute (initialization/LeggedRobotInitializer.cpp:67-77): x_{k+1} = x_k, u = weight compensation

@@ -34,6 +34,14 @@ typedef struct {
   int n_trials;
 } hbo_solve_info;
 
+// one trial of the filter line search (App. C.5 step 4): the branch that decided it and the decision
+enum { HBO_LS_VIOLATION = 0, HBO_LS_ARMIJO = 1, HBO_LS_FILTER = 2 };
+typedef struct {
+  double alpha, merit, viol;  // step length, merit and total violation of the trial
+  int branch;                 // HBO_LS_*: violation (viol > g_max), Armijo (viol, viol0 < g_min and a descent metric < 0), filter
+  int accepted;               // 1: the step was taken at this trial
+} hbo_ls_trial;
+
 void hbo_init(void);
 // rigid-body probes (for pinning against MuJoCo / finite differences)
 void hbo_rbd(const double* q, const double* v, double* M /*16x16*/, double* nle /*16*/, double* J /*12x16*/,
@@ -49,9 +57,11 @@ void hbo_set_wbc_settings(const double* s /*17 doubles, order of hb_wbc_settings
 void hbo_node_lq(double t_dt, const double* x, const double* u, const double* xn, const double* xref, const double* swing,
                  int mode, double* Ad, double* Bd, double* b, double* Q, double* R, double* P, double* q, double* r,
                  double* C, double* D, double* e, int* m, double* cost);
-// one SQP iteration (S1-S7) on one instance; x_traj[(N+1)x22], u_traj[Nx22] in/out
-void hbo_mpc_iteration(const hbo_horizon* hz, const double* x0, const double* x_ref, const double* swing, const int32_t* mode,
-                       double* x_traj, double* u_traj, hbo_solve_info* info);
+// one SQP iteration (S1-S7) on one instance; x_traj[(N+1)x22], u_traj[Nx22] in/out. max_trials (>= 1) caps the line search like
+// hb_config.line_search_max_trials (14: alpha = 1, 1/2, ... >= 1e-4, the cap alpha_min reaches first); trials (nullable, max_trials rows)
+// receives one row per trial evaluated, info->n_trials in all
+void hbo_mpc_iteration(const hbo_horizon* hz, int max_trials, const double* x0, const double* x_ref, const double* swing, const int32_t* mode,
+                       double* x_traj, double* u_traj, hbo_solve_info* info, hbo_ls_trial* trials);
 void hbo_mpc_cold_start(const hbo_horizon* hz, const double* x0, const int32_t* mode, double* x_traj, double* u_traj);
 // WBC (W1-W4)
 void hbo_wbc_terms(const double* x_des, const double* u_des, const double* rbd, int mode, double* Aw, double* bw, int* rw, double* J, double* dJv);

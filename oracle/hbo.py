@@ -30,6 +30,14 @@ class SolveInfo(C.Structure):
                 ("viol1", C.c_double), ("armijo", C.c_double), ("status", C.c_int), ("n_trials", C.c_int)]
 
 
+class LsTrial(C.Structure):
+    _fields_ = [("alpha", C.c_double), ("merit", C.c_double), ("viol", C.c_double), ("branch", C.c_int), ("accepted", C.c_int)]
+
+
+LS_BRANCHES = ("violation", "armijo", "filter")      # HBO_LS_VIOLATION, HBO_LS_ARMIJO, HBO_LS_FILTER
+LS_MAX_TRIALS = 14                                   # hb_config.line_search_max_trials by default: alpha = 1, 1/2, ... >= 1e-4
+
+
 def build():
     subprocess.check_call(["make", "-s", "-C", _HERE])
 
@@ -122,14 +130,22 @@ def mpc_cold_start(N, dt, x0, mode):
     return xt, ut
 
 
-def mpc_iteration(N, dt, x0, x_ref, swing, mode, xt, ut):
+def mpc_iteration(N, dt, x0, x_ref, swing, mode, xt, ut, max_trials=LS_MAX_TRIALS, record=False):
+    """One SQP iteration with at most max_trials line-search trials. record: also return the line search's trials, one dict per trial
+    (alpha, merit, viol, branch: one of LS_BRANCHES, accepted: bool), as a fourth result."""
     hz, _keep = _horizon(N, dt)
     x0, x_ref, swing = _d(x0), _d(x_ref), _d(swing)
     mode = np.ascontiguousarray(mode, dtype=np.int32)
     xt = _d(xt).copy(); ut = _d(ut).copy()
     info = SolveInfo()
-    lib().hbo_mpc_iteration(C.byref(hz), _p(x0), _p(x_ref), _p(swing), _p(mode), _p(xt), _p(ut), C.byref(info))
-    return xt, ut, {k: getattr(info, k) for k, _ in SolveInfo._fields_}
+    rows = (LsTrial * max(1, max_trials))()
+    lib().hbo_mpc_iteration(C.byref(hz), C.c_int(max_trials), _p(x0), _p(x_ref), _p(swing), _p(mode), _p(xt), _p(ut), C.byref(info), rows)
+    info = {k: getattr(info, k) for k, _ in SolveInfo._fields_}
+    if not record:
+        return xt, ut, info
+    trials = [dict(alpha=r.alpha, merit=r.merit, viol=r.viol, branch=LS_BRANCHES[r.branch], accepted=bool(r.accepted))
+              for r in rows[:info["n_trials"]]]
+    return xt, ut, info, trials
 
 
 def mpc_iteration_batch(N, dt, x0, x_ref, swing, mode, xt, ut, threads=1):
