@@ -10,6 +10,7 @@ from .api import (HbWbcSettings, HbTaskInfo, parse_task_info, Context, WeightedW
                   HbTarget, make_targets, reference_target, goal_to_target, HB_MAX_GOALS, HbGoalSchedule, make_goal_schedules,
                   HB_ODOM_MAX_DELAY, HbOdometrySetting, make_odometry_settings, HbControllerSetting, make_controller_settings,
                   HbHardwareSetting, default_hardware_setting, make_hardware_settings,
+                  HbMotorBridge, default_motor_bridge, make_motor_bridges, bridge_encode, bridge_feedback,
                   HB_GAIT_MAX_PHASES, HbGaitTemplate, HbPlannerSettings, gait_template, default_planner_settings, parse_planner_settings, make_planner_settings,
                   CHANNELS, make_channels, EpisodeSnapshot, reseed)
 
@@ -20,5 +21,6 @@ __all__ = ["HbWbcSettings", "HbTaskInfo", "parse_task_info", "Context", "Weighte
            "HbTarget", "make_targets", "reference_target", "goal_to_target", "HB_MAX_GOALS", "HbGoalSchedule", "make_goal_schedules",
            "HB_ODOM_MAX_DELAY", "HbOdometrySetting", "make_odometry_settings", "HbControllerSetting", "make_controller_settings",
            "HbHardwareSetting", "default_hardware_setting", "make_hardware_settings",
+           "HbMotorBridge", "default_motor_bridge", "make_motor_bridges", "bridge_encode", "bridge_feedback",
            "HB_GAIT_MAX_PHASES", "HbGaitTemplate", "HbPlannerSettings", "gait_template", "default_planner_settings", "parse_planner_settings", "make_planner_settings",
            "CHANNELS", "make_channels", "EpisodeSnapshot", "reseed"]

@@ -55,6 +55,8 @@ EXPORTED_SYMBOLS = [
     "hb_rollout_set_odometry", "hb_sim_read_odometry", "hb_sim_read_odometry_async", "hb_estimator_fuse_odometry", "hb_estimator_fuse_odometry_async",
     "hb_rollout_set_controller_settings",
     "hb_default_hardware_setting", "hb_rollout_set_hardware", "hb_actuation_hw", "hb_sim_read_sensors_hw",
+    "hb_default_motor_bridge", "hb_rollout_set_motor_bridge", "hb_motor_bridge_encode", "hb_motor_bridge_feedback", "hb_actuation_bridge",
+    "hb_sim_step_bridge", "hb_sim_read_sensors_bridge",
     "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
     "hb_check_setting_records", "hb_rollout_set_channel",
     "hb_episode_state_bytes", "hb_episode_save_async", "hb_episode_restore",
@@ -625,6 +627,73 @@ def make_hardware_settings(B, base=None, **fields):
     return out
 
 
+class HbMotorBridge(C.Structure):
+    SETTING_KIND = 11        # HB_SETTING_MOTOR_BRIDGE, the record's kind for hb_check_setting_records
+    _fields_ = [("command_scale", C.c_double * NJ), ("direction", C.c_int32 * NJ), ("zero", C.c_double * NJ)] + \
+        [(k, C.c_double * NJ) for k in ("kp_max", "kd_max", "pos_max", "vel_max", "ff_max")] + [("quantise", C.c_int32)]
+
+
+def default_motor_bridge():
+    """hb_default_motor_bridge: the real Hunter's joint path (legged_bridge_hw): the 0.7 command scale on joints 0, 1, 5, 6, its motor
+    directions, zero offsets 0, the protocol ranges of each joint's X or D motor, and the protocol's quantisation."""
+    r = HbMotorBridge()
+    _check(load_library().hb_default_motor_bridge(C.byref(r)), "hb_default_motor_bridge")
+    return r
+
+
+def make_motor_bridges(B, base=None, **fields):
+    """ctypes array of B HbMotorBridge (Context.set_motor_bridge): each robot's joint path through the motor driver in the episodes. base
+    (HbMotorBridge, default default_motor_bridge()) is the base of every record. Any field can be given by name: quantise as a scalar or
+    a (B,) array, the others as a scalar, (10,) or (B, 10). Raises ValueError for an unknown name, a shape that does not broadcast, a
+    direction or quantise that is not an integer, and a record hb_rollout_set_motor_bridge rejects."""
+    base = default_motor_bridge() if base is None else base
+    out = (HbMotorBridge * B)()
+    v = np.ctypeslib.as_array(out)
+    v[:] = np.frombuffer(bytes(base), dtype=v.dtype)[0]
+    for name, value in fields.items():
+        if name not in v.dtype.names:
+            raise ValueError("motor bridges: unknown field %r" % name)
+        shape = (B,) + v.dtype[name].shape
+        try:
+            x = np.broadcast_to(np.asarray(value, dtype=np.float64), shape)
+        except ValueError as e:
+            raise ValueError("motor bridges: %s: %s expected: %s" % (name, "(10,) or (B, 10)" if shape[1:] else "(B,) or a scalar", e))
+        if v.dtype[name].base.kind == "i" and not (np.isfinite(x).all() and (x == np.rint(x)).all() and (np.abs(x) < 2 ** 31).all()):
+            raise ValueError("motor bridges: %s: int32 integers expected" % name)
+        v[name] = x
+    return _check_records(HbMotorBridge.SETTING_KIND, out, "motor_bridge")
+
+
+def _bridge_records(bridge, B, what):
+    """bridge (a ctypes array or a sequence of B HbMotorBridge) as a ctypes array (None stays None), or ValueError."""
+    if bridge is None:
+        return None
+    if len(bridge) != B:
+        raise ValueError("%s: %d motor bridges for %d robots" % (what, len(bridge), B))
+    return bridge if isinstance(bridge, C.Array) else (HbMotorBridge * B)(*bridge)
+
+
+def bridge_encode(bridge, command):
+    """The motor bridge's command codec on the host (hb_motor_bridge_encode): command [B,10,5] (joint frame: pos_des, vel_des, kp, kd, ff)
+    -> the decoded motor command [B,10,5] (motor frame: pos, vel, kp, kd, ff) of the records bridge (B HbMotorBridge)."""
+    command = _f64(command).reshape(-1, NJ, 5)
+    B = command.shape[0]
+    out = np.zeros((B, NJ, 5))
+    _check(load_library().hb_motor_bridge_encode(B, _bridge_records(bridge, B, "bridge_encode"), _ptr(command), _ptr(out)), "hb_motor_bridge_encode")
+    return out
+
+
+def bridge_feedback(bridge, q, qd):
+    """The motor bridge's encoders on the host (hb_motor_bridge_feedback): joint readings q, qd [B,10] -> what the driver reports back in
+    the joint frame, (q_out, qd_out)."""
+    q, qd = _f64(q).reshape(-1, NJ), _f64(qd).reshape(-1, NJ)
+    B = q.shape[0]
+    q_out, qd_out = np.zeros((B, NJ)), np.zeros((B, NJ))
+    _check(load_library().hb_motor_bridge_feedback(B, _bridge_records(bridge, B, "bridge_feedback"), _ptr(q), _ptr(qd), _ptr(q_out), _ptr(qd_out)),
+           "hb_motor_bridge_feedback")
+    return q_out, qd_out
+
+
 HB_ODOM_MAX_DELAY = 15
 
 
@@ -1107,36 +1176,43 @@ class Context:
                                                    _ptr(joint_pos), _ptr(joint_vel), _ptr(flags), _ptr(rbd)), "hb_estimator_update_batch", self._h)
         return rbd
 
-    def read_sensors(self, rbd, est, tick, noise=None, accel_dt=0.002, hardware=None):
-        """Sensors of the simulated robot at absolute tick `tick` from the true rbd [B,32] (hb_sim_read_sensors_hw); `est` (ctypes array of
-        HbEstimationState) gives the noise streams and the accelerometer's previous velocity and is updated in place. noise: HbSensorNoise
+    def read_sensors(self, rbd, est, tick, noise=None, accel_dt=0.002, hardware=None, bridge=None):
+        """Sensors of the simulated robot at absolute tick `tick` from the true rbd [B,32] (hb_sim_read_sensors_bridge); `est` (ctypes array
+        of HbEstimationState) gives the noise streams and the accelerometer's previous velocity and is updated in place. noise: HbSensorNoise
         (None: exact). hardware: B HbHardwareSetting (make_hardware_settings), each robot's sensor offsets and sigmas in place of noise's
-        sigmas; None reads as hb_sim_read_sensors. Returns (quat [B,4], ang_vel_local [B,3], lin_acc_local [B,3], joint_pos [B,10],
-        joint_vel [B,10])."""
+        sigmas; bridge: B HbMotorBridge (make_motor_bridges), each robot's joint encoders; None reads as hb_sim_read_sensors. Returns
+        (quat [B,4], ang_vel_local [B,3], lin_acc_local [B,3], joint_pos [B,10], joint_vel [B,10])."""
         rbd = _f64(rbd); B = rbd.shape[0]
         noise = noise or HbSensorNoise()
         _check_hardware("read_sensors", hardware, B)
+        bridge = _bridge_records(bridge, B, "read_sensors")
         quat = np.zeros((B, 4)); w = np.zeros((B, 3)); a = np.zeros((B, 3)); jp = np.zeros((B, NJ)); jv = np.zeros((B, NJ))
-        _check(self._lib.hb_sim_read_sensors_hw(self._h, B, C.byref(noise), hardware, C.c_int64(tick), C.c_double(accel_dt), _ptr(rbd), est, _ptr(quat),
-                                                _ptr(w), _ptr(a), _ptr(jp), _ptr(jv)), "hb_sim_read_sensors_hw", self._h)
+        _check(self._lib.hb_sim_read_sensors_bridge(self._h, B, C.byref(noise), hardware, bridge, C.c_int64(tick), C.c_double(accel_dt), _ptr(rbd), est,
+                                                    _ptr(quat), _ptr(w), _ptr(a), _ptr(jp), _ptr(jv)), "hb_sim_read_sensors_bridge", self._h)
         return quat, w, a, jp, jv
 
-    def actuation(self, time, state, command, rbd, delay=0.009, hardware=None):
+    def actuation(self, time, state, command, rbd, delay=0.009, hardware=None, bridge=None):
         """LeggedHWSim::writeSim: delayed hybrid joint command -> applied joint torques [B,10]; `state` (ctypes array of HbActuationState) in place.
-        hardware: B HbHardwareSetting (make_hardware_settings), each robot's actuation_delay in place of delay (hb_actuation_hw)."""
+        hardware: B HbHardwareSetting (make_hardware_settings), each robot's actuation_delay in place of delay. bridge: B HbMotorBridge
+        (make_motor_bridges): each robot's applied entry is encoded instead, and the decoded motor commands [B,10,5] (pos, vel, kp, kd, ff,
+        motor frame) are returned in place of the torques, for sim_step(bridge=...) (hb_actuation_bridge)."""
         command, rbd = _f64(command), _f64(rbd); B = rbd.shape[0]
         time = _f64(np.broadcast_to(_f64(time), (B,)))
         _check_hardware("actuation", hardware, B)
-        tau = np.zeros((B, NJ))
-        _check(self._lib.hb_actuation_hw(self._h, B, C.c_double(delay), hardware, _ptr(time), state, _ptr(command), _ptr(rbd), _ptr(tau)), "hb_actuation_hw",
-               self._h)
-        return tau
+        bridge = _bridge_records(bridge, B, "actuation")
+        tau = np.zeros((B, NJ)) if bridge is None else None
+        mcmd = None if bridge is None else np.zeros((B, NJ, 5))
+        _check(self._lib.hb_actuation_bridge(self._h, B, C.c_double(delay), hardware, bridge, _ptr(time), state, _ptr(command), _ptr(rbd), _ptr(tau),
+                                             _ptr(mcmd)), "hb_actuation_bridge", self._h)
+        return tau if bridge is None else mcmd
 
-    def sim_step(self, rbd, tau, params=None, wrench=None, variation=None, terrain=None):
+    def sim_step(self, rbd, tau, params=None, wrench=None, variation=None, terrain=None, bridge=None, limits=None):
         """One control period of the batched rigid-body plant: returns (rbd_next [B,32], contact_force [B,12], contact_flag [B,4]).
         wrench [B,6]: an external world force at the base origin, then a world couple, held over the period. variation: B HbPlantVariation
-        (make_plant_variations), the plant of each robot. terrain: B HbTerrain (make_terrains), the ground under each robot. Every step is
-        hb_sim_step_terrain; without any of the three it is the plain plant step of hb_sim_step_batch."""
+        (make_plant_variations), the plant of each robot. terrain: B HbTerrain (make_terrains), the ground under each robot. bridge: B
+        HbMotorBridge (make_motor_bridges): tau is then the decoded motor commands [B,10,5] of actuation(bridge=...), whose motor PD runs on
+        every substep, clipped to limits ([10] or [B,10]), and the mean clipped torque [B,10] is returned fourth. Every step is
+        hb_sim_step_bridge; without any of the four it is the plain plant step of hb_sim_step_batch."""
         rbd = _f64(rbd).copy(); tau = _f64(tau); B = rbd.shape[0]
         params = params or default_sim_params()
         cf = np.zeros((B, 12)); fl = np.zeros((B, 4), dtype=np.uint8)
@@ -1145,9 +1221,15 @@ class Context:
             raise ValueError("sim_step: %d plant variations for %d robots" % (len(variation), B))
         if terrain is not None and len(terrain) != B:
             raise ValueError("sim_step: %d terrains for %d robots" % (len(terrain), B))
-        _check(self._lib.hb_sim_step_terrain(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), variation, terrain, _ptr(cf), _ptr(fl)),
-               "hb_sim_step_terrain", self._h)
-        return rbd, cf, fl
+        bridge = _bridge_records(bridge, B, "sim_step")
+        mcmd, lim, applied = None, None, None
+        if bridge is not None:
+            mcmd, tau = tau.reshape(B, NJ, 5), None
+            lim = _f64(np.broadcast_to(_f64(limits), (B, NJ)))
+            applied = np.zeros((B, NJ))
+        _check(self._lib.hb_sim_step_bridge(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), variation, terrain, bridge, _ptr(mcmd), _ptr(lim),
+                                            _ptr(applied), _ptr(cf), _ptr(fl)), "hb_sim_step_bridge", self._h)
+        return (rbd, cf, fl) if bridge is None else (rbd, cf, fl, applied)
 
     def _set_instances(self, symbol, items):
         """One per-robot episode setting (hb_rollout_set_*): items[i] for instance i, None clears the setting."""
@@ -1215,6 +1297,13 @@ class Context:
         and offsets, in place of params' and est_params.noise's values; instances beyond len(settings) run those; None clears them. The
         controllers are not told about it, and no other call reads it."""
         self._set_instances("hb_rollout_set_hardware", settings)
+
+    def set_motor_bridge(self, bridges):
+        """Motor bridges of this context's episodes (hb_rollout_set_motor_bridge): bridges[i] (make_motor_bridges) is the joint path of
+        instance i of every later rollout / rollout_estimated call through the real robot's motor driver: scaled, quantised commands, the
+        motor's PD on every plant substep and, in rollout_estimated, quantised encoders; instances beyond len(bridges) run the simulated
+        hardware's torque law; None clears them. The controllers are not told about it, and no other call reads it."""
+        self._set_instances("hb_rollout_set_motor_bridge", bridges)
 
     def set_channels(self, channels):
         """Recorded channels of this context's episodes (hb_rollout_set_channel): channels maps names of CHANNELS to contiguous cuda

@@ -77,6 +77,7 @@ struct hb_ctx {
   hb_rollout_command* ro_cmd; hb_plan_input* ro_in; hb_reference* ro_refs; hb_solve_info* ro_info; int32_t* ro_pstat;
   double *ro_t0, *ro_x0, *ro_feet, *ro_sol, *ro_jcmd, *ro_jtau, *ro_tau, *ro_held, *ro_tnow, *ro_wrench;
   double* ro_cforce; uint8_t* ro_cflag;   // the plant's contact forces and flags on a tick that records a contact channel
+  double* ro_mcmd;                        // the decoded motor commands of the instances with a motor bridge (B x 50)
   // hb_rollout_estimated_batch_dev's own scratch (first such call, at max_batch): the tick's sensor readings, contact flags, estimated rbd
   void* re_mem;
   double *re_quat, *re_gyro, *re_acc, *re_jpos, *re_jvel, *re_rbd;
@@ -108,6 +109,8 @@ struct hb_ctx {
   InstanceSetting<hb_controller_setting> controllers;
   // each instance's simulated hardware in the episodes: actuation delay, torque limits, sensor noise and offsets (hb_rollout_set_hardware)
   InstanceSetting<hb_hardware_setting> hardware;
+  // each instance's joint path through the real robot's motor driver in the episodes (hb_rollout_set_motor_bridge)
+  InstanceSetting<hb_motor_bridge> bridges;
   // each instance's gait templates and swing settings in every device planner path (hb_plan_set_settings)
   InstanceSetting<hb_planner_settings> plan_settings;
   // the recorded channels of the episodes (hb_rollout_set_channel): the caller's buffer, its instances and rows; B == 0: unset
@@ -498,7 +501,8 @@ int hb_destroy(hb_ctx* ctx) {
   cudaSetDevice(ctx->device);
   void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->snap_mem, ctx->arena,
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
-                       ctx->odometry.dev, ctx->controllers.dev, ctx->hardware.dev, ctx->plan_settings.dev};
+                       ctx->odometry.dev, ctx->controllers.dev, ctx->hardware.dev, ctx->plan_settings.dev,
+                       ctx->bridges.dev};
   for (void* p : mem) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -1087,27 +1091,78 @@ int hb_default_hardware_setting(hb_hardware_setting* s) {
 
 int hb_rollout_set_hardware(hb_ctx* ctx, int B, const hb_hardware_setting* s) { return set_instances(ctx, B, s, hardware_setting_ok, &hb_ctx::hardware); }
 
-// hb_actuation_batch_dev, with each instance of `hw` on its own delay (the episodes, hb_actuation_hw)
-static int actuation_dev(hb_ctx* ctx, int B, double delay, HardwareView hw, const double* time, hb_actuation_state* state, const double* command,
-                         const double* rbd, double* tau) {
+// The instances' motor bridges as the actuation, plant and sensor kernels read them; the calls without records pass an empty view
+using BridgeView = InstanceView<hb_motor_bridge>;
+
+// The ranges of hunter_b200.h's hb_motor_bridge: directions +-1, every value finite, scales >= 0, maxima > 0, quantise 0 or 1
+static bool motor_bridge_ok(const hb_motor_bridge& r) {
+  if (r.quantise != 0 && r.quantise != 1) return false;
+  for (int j = 0; j < NJ; ++j) {
+    if (r.direction[j] != 1 && r.direction[j] != -1) return false;
+    if (!isfinite(r.command_scale[j]) || !(r.command_scale[j] >= 0.0) || !isfinite(r.zero[j])) return false;
+    for (double m : {r.kp_max[j], r.kd_max[j], r.pos_max[j], r.vel_max[j], r.ff_max[j]}) if (!isfinite(m) || !(m > 0.0)) return false;
+  }
+  return true;
+}
+
+int hb_default_motor_bridge(hb_motor_bridge* r) {
+  if (!r) return HB_EINVAL;
+  memset(r, 0, sizeof(*r));
+  static const int32_t dir[NJ] = {1, -1, 1, 1, 1, 1, -1, 1, -1, 1};            // BridgeHW.h:118
+  for (int j = 0; j < NJ; ++j) {
+    const int k = j % 5;
+    r->command_scale[j] = (k == 0 || k == 1) ? 0.7 : 1.0;                       // BridgeHW.cpp:74-85
+    r->direction[j] = dir[j];
+    r->kp_max[j] = 500.0; r->kd_max[j] = 5.0; r->pos_max[j] = 12.5; r->vel_max[j] = 18.0;   // motor_control.c:11-35
+    r->ff_max[j] = (k == 2 || k == 3) ? 90.0 : 30.0;                            // D motors (ids 3, 4: joints 2, 3 of a leg), X motors
+  }
+  r->quantise = 1;
+  return HB_OK;
+}
+
+int hb_rollout_set_motor_bridge(hb_ctx* ctx, int B, const hb_motor_bridge* r) { return set_instances(ctx, B, r, motor_bridge_ok, &hb_ctx::bridges); }
+
+int hb_motor_bridge_encode(int B, const hb_motor_bridge* r, const double* command, double* out) {
+  if (B < 0 || (B > 0 && !(r && command && out)) || !all_ok(B, r, motor_bridge_ok)) return HB_EINVAL;
+  for (int i = 0; i < B; ++i)
+    for (int j = 0; j < NJ; ++j) bridge_command(r[i], j, command + ((size_t)i * NJ + j) * 5, out + ((size_t)i * NJ + j) * 5);
+  return HB_OK;
+}
+
+int hb_motor_bridge_feedback(int B, const hb_motor_bridge* r, const double* q, const double* qd, double* q_out, double* qd_out) {
+  if (B < 0 || (B > 0 && !(r && q && qd && q_out && qd_out)) || !all_ok(B, r, motor_bridge_ok)) return HB_EINVAL;
+  for (size_t k = 0; k < (size_t)B * NJ; ++k) {
+    double a = q[k], v = qd[k];
+    bridge_feedback(r[k / NJ], (int)(k % NJ), &a, &v);
+    q_out[k] = a; qd_out[k] = v;
+  }
+  return HB_OK;
+}
+
+// hb_actuation_batch_dev, with each instance of `hw` on its own delay and each instance of `bridge` writing its motor command to mcmd (the
+// episodes, hb_actuation_bridge)
+static int actuation_dev(hb_ctx* ctx, int B, double delay, HardwareView hw, BridgeView bridge, const double* time, hb_actuation_state* state,
+                         const double* command, const double* rbd, double* tau, double* mcmd) {
   ENTER(ctx, B, time && state && command && rbd && tau && delay_ok(delay), UNCAPPED);
-  return launch(ctx, K_UNPROFILED, actuation_kernel, (B + 63) / 64, 64, 0, B, delay, hw, time, state, command, rbd, tau);
+  return launch(ctx, K_UNPROFILED, actuation_kernel, (B + 63) / 64, 64, 0, B, delay, hw, bridge, time, state, command, rbd, tau, mcmd);
 }
 
 int hb_actuation_batch_dev(hb_ctx* ctx, int B, double delay, const double* time, hb_actuation_state* state, const double* command, const double* rbd,
                            double* tau) {
-  return actuation_dev(ctx, B, delay, HardwareView{}, time, state, command, rbd, tau);
+  return actuation_dev(ctx, B, delay, HardwareView{}, BridgeView{}, time, state, command, rbd, tau, nullptr);
 }
 
-// the plant step after the entry checks; wrench (B x 6) nullable; var: the plants of the instances, ter: the ground under them
+// the plant step after the entry checks; wrench (B x 6) nullable; var: the plants of the instances, ter: the ground under them, drive: the
+// motors of the bridged ones
 static int sim_step(hb_ctx* ctx, int B, const hb_sim_params& params, double* rbd, const double* tau, const double* wrench,
-                    InstanceView<hb_plant_variation> var, InstanceView<hb_terrain> ter, double* contact_force, uint8_t* contact_flag) {
-  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, params, rbd, tau, wrench, var, ter, contact_force, contact_flag);
+                    InstanceView<hb_plant_variation> var, InstanceView<hb_terrain> ter, const MotorDrive& drive, double* contact_force,
+                    uint8_t* contact_flag) {
+  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, params, rbd, tau, wrench, var, ter, drive, contact_force, contact_flag);
 }
 
 int hb_sim_step_batch_dev(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {
   ENTER(ctx, B, params && rbd && tau && sim_params_ok(*params), UNCAPPED);
-  return sim_step(ctx, B, *params, rbd, tau, nullptr, {}, {}, contact_force, contact_flag);
+  return sim_step(ctx, B, *params, rbd, tau, nullptr, {}, {}, MotorDrive{}, contact_force, contact_flag);
 }
 
 int hb_default_plant_variation(hb_plant_variation* v) {
@@ -1274,6 +1329,7 @@ int hb_check_setting_records(int32_t kind, int B, const void* records, int32_t* 
     case HB_SETTING_PLANNER: return check_records(B, records, planner_settings_ok, first_bad);
     case HB_SETTING_TARGETS: return check_records(B, records, target_ok, first_bad);
     case HB_SETTING_LATENCIES: return check_records(B, records, latency_ok, first_bad);
+    case HB_SETTING_MOTOR_BRIDGE: return check_records(B, records, motor_bridge_ok, first_bad);
     default: return HB_EINVAL;
   }
 }
@@ -1376,6 +1432,7 @@ static int rollout_reserve(hb_ctx* ctx) {
     ctx->ro_jcmd = carve<double>(m, off, Bc * NJ * 5); ctx->ro_jtau = carve<double>(m, off, Bc * NJ); ctx->ro_tau = carve<double>(m, off, Bc * NJ);
     ctx->ro_held = carve<double>(m, off, Bc * 32); ctx->ro_tnow = carve<double>(m, off, Bc); ctx->ro_wrench = carve<double>(m, off, Bc * 6);
     ctx->ro_cforce = carve<double>(m, off, Bc * 12); ctx->ro_cflag = carve<uint8_t>(m, off, Bc * 4);
+    ctx->ro_mcmd = carve<double>(m, off, Bc * NJ * 5);
     return off;
   });
 }
@@ -1469,6 +1526,9 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   const OdomRead odom_read = odom ? odometry_read(ctx, ctx->re_opos, ctx->re_ohas) : OdomRead{};
   const ControllerView controllers = ctx->controllers.view();   // each instance's WBC settings and PD gains, none without a setting
   const HardwareView hardware = ctx->hardware.view();           // each instance's actuators and sensors, none without a setting
+  const BridgeView bridges = ctx->bridges.view();               // each instance's motor bridge, none without a setting
+  MotorDrive drive{bridges, ctx->ro_mcmd, nullptr, hardware, {}, ctx->ro_tau};
+  for (int j = 0; j < NJ; ++j) drive.lim[j] = p->torque_limit[j];
   for (int k = 0; k < n_ticks && !rc; ++k) {
     const int64_t a = tick0 + k;
     const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
@@ -1480,7 +1540,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
     if (!rc && e) {
       // LeggedController::updateStateEstimation: sensors and contact flags at the previous observation's time, filter, observation step
       double* est_row = (n_est_log && k % p->log_every == 0) ? e->log + (size_t)(k / p->log_every) * 32 : nullptr;
-      rc = launch(ctx, K_UNPROFILED, sensor_read_kernel, grid, 64, 0, B, e->ep->noise, hardware, (uint32_t)a, p->sim.dt, (double)(a - 1) * p->period, rbd,
+      rc = launch(ctx, K_UNPROFILED, sensor_read_kernel, grid, 64, 0, B, e->ep->noise, hardware, bridges, (uint32_t)a, p->sim.dt, (double)(a - 1) * p->period, rbd,
                   e->est, ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag, odom_read);
       if (!rc) rc = launch(ctx, K_UNPROFILED, odom ? kf_update_kernel<hb_estimation_state, true> : kf_update_kernel<hb_estimation_state, false>, B, 32,
                            sizeof(KfShared), B, e->ep->kf, p->period, e->est, ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag,
@@ -1509,9 +1569,9 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
                                     false, choice, controllers);
     if (!rc) rc = joint_command_dev(ctx, B, &p->gains, p->period, ctx->xdes, ctx->udes, ctx->ro_sol, ctx->wmode, meas, nullptr, estop, ctx->ro_jcmd,
                                     ctx->ro_jtau, controllers);
-    if (!rc) rc = actuation_dev(ctx, B, p->actuation_delay, hardware, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau);
+    if (!rc) rc = actuation_dev(ctx, B, p->actuation_delay, hardware, bridges, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau, ctx->ro_mcmd);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, hardware, ctx->ro_tau);
-    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, ctx->variations.view(), ctx->terrains.view(),
+    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, ctx->variations.view(), ctx->terrains.view(), drive,
                            record && contacts ? ctx->ro_cforce : nullptr, record && contacts ? ctx->ro_cflag : nullptr);
     if (!rc && record) {
       for (int j = 0; j < rec.n; ++j)
@@ -1673,19 +1733,20 @@ int hb_estimation_reset(int B, uint64_t first_stream, hb_estimation_state* state
   return HB_OK;
 }
 
-// hb_sim_read_sensors_batch_dev, with each instance of `hw` on its own sensors (hb_sim_read_sensors_hw)
-static int read_sensors_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noise, HardwareView hw, int64_t tick, double accel_dt, const double* rbd,
-                            hb_estimation_state* est, double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos, double* joint_vel) {
+// hb_sim_read_sensors_batch_dev, with each instance of `hw` on its own sensors and each of `bridge` on its encoders (hb_sim_read_sensors_bridge)
+static int read_sensors_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noise, HardwareView hw, BridgeView bridge, int64_t tick, double accel_dt,
+                            const double* rbd, hb_estimation_state* est, double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos,
+                            double* joint_vel) {
   ENTER(ctx, B, noise && rbd && est && quat && ang_vel_local && lin_acc_local && joint_pos && joint_vel && sensor_noise_ok(*noise) && accel_dt > 0.0 &&
         tick >= 0 && tick <= UINT32_MAX, CAPPED);
-  return launch(ctx, K_UNPROFILED, sensor_read_kernel, (B + 63) / 64, 64, 0, B, *noise, hw, (uint32_t)tick, accel_dt, 0.0, rbd, est, quat, ang_vel_local,
+  return launch(ctx, K_UNPROFILED, sensor_read_kernel, (B + 63) / 64, 64, 0, B, *noise, hw, bridge, (uint32_t)tick, accel_dt, 0.0, rbd, est, quat, ang_vel_local,
                 lin_acc_local, joint_pos, joint_vel, (uint8_t*)nullptr, OdomRead{});
 }
 
 int hb_sim_read_sensors_batch_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, double accel_dt, const double* rbd,
                                   hb_estimation_state* est, double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos,
                                   double* joint_vel) {
-  return read_sensors_dev(ctx, B, noise, HardwareView{}, tick, accel_dt, rbd, est, quat, ang_vel_local, lin_acc_local, joint_pos, joint_vel);
+  return read_sensors_dev(ctx, B, noise, HardwareView{}, BridgeView{}, tick, accel_dt, rbd, est, quat, ang_vel_local, lin_acc_local, joint_pos, joint_vel);
 }
 
 int hb_sim_read_odometry_async(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, const double* rbd, const hb_estimation_state* est,
@@ -2040,16 +2101,22 @@ int hb_sim_read_sensors(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_
   return hb_sim_read_sensors_hw(ctx, B, noise, nullptr, tick, accel_dt, rbd, est, quat, ang_vel_local, lin_acc_local, joint_pos, joint_vel);
 }
 
-// the one host-pointer sensor read: hb_sim_read_sensors is it with null records
 int hb_sim_read_sensors_hw(hb_ctx* ctx, int B, const hb_sensor_noise* noise, const hb_hardware_setting* hw, int64_t tick, double accel_dt,
                            const double* rbd, hb_estimation_state* est, double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos,
                            double* joint_vel) {
+  return hb_sim_read_sensors_bridge(ctx, B, noise, hw, nullptr, tick, accel_dt, rbd, est, quat, ang_vel_local, lin_acc_local, joint_pos, joint_vel);
+}
+
+// the one host-pointer sensor read: hb_sim_read_sensors and hb_sim_read_sensors_hw are it with null records
+int hb_sim_read_sensors_bridge(hb_ctx* ctx, int B, const hb_sensor_noise* noise, const hb_hardware_setting* hw, const hb_motor_bridge* bridge, int64_t tick,
+                               double accel_dt, const double* rbd, hb_estimation_state* est, double* quat, double* ang_vel_local, double* lin_acc_local,
+                               double* joint_pos, double* joint_vel) {
   ENTER(ctx, B, noise && rbd && est && quat && ang_vel_local && lin_acc_local && joint_pos && joint_vel && sensor_noise_ok(*noise) && accel_dt > 0.0 &&
-        tick >= 0 && tick <= UINT32_MAX, CAPPED, [&] { return all_ok(B, hw, hardware_setting_ok); });
+        tick >= 0 && tick <= UINT32_MAX, CAPPED, [&] { return all_ok(B, hw, hardware_setting_ok) && all_ok(B, bridge, motor_bridge_ok); });
   Staging s(ctx, B);
-  auto r = s.in(rbd, 32); auto es = s.inout(est, 1); auto h = s.in_or_null(hw, 1); auto q = s.out(quat, 4); auto w = s.out(ang_vel_local, 3);
-  auto a = s.out(lin_acc_local, 3); auto jp = s.out(joint_pos, NJ); auto jv = s.out(joint_vel, NJ);
-  return s.run(1, [&](Chunk) { return read_sensors_dev(ctx, B, noise, {h, B}, tick, accel_dt, r, es, q, w, a, jp, jv); });
+  auto r = s.in(rbd, 32); auto es = s.inout(est, 1); auto h = s.in_or_null(hw, 1); auto mb = s.in_or_null(bridge, 1); auto q = s.out(quat, 4);
+  auto w = s.out(ang_vel_local, 3); auto a = s.out(lin_acc_local, 3); auto jp = s.out(joint_pos, NJ); auto jv = s.out(joint_vel, NJ);
+  return s.run(1, [&](Chunk) { return read_sensors_dev(ctx, B, noise, {h, B}, {mb, B}, tick, accel_dt, r, es, q, w, a, jp, jv); });
 }
 
 int hb_sim_read_odometry(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, const double* rbd, const hb_estimation_state* est,
@@ -2073,14 +2140,20 @@ int hb_actuation_batch(hb_ctx* ctx, int B, double delay, const double* time, hb_
   return hb_actuation_hw(ctx, B, delay, nullptr, time, state, command, rbd, tau);
 }
 
-// the one host-pointer actuation: hb_actuation_batch is it with null records
 int hb_actuation_hw(hb_ctx* ctx, int B, double delay, const hb_hardware_setting* hw, const double* time, hb_actuation_state* state, const double* command,
                     const double* rbd, double* tau) {
-  ENTER(ctx, B, time && state && command && rbd && tau, CAPPED, [&] { return delay_ok(delay) && all_ok(B, hw, hardware_setting_ok); });
+  return hb_actuation_bridge(ctx, B, delay, hw, nullptr, time, state, command, rbd, tau, nullptr);
+}
+
+// the one host-pointer actuation: hb_actuation_batch and hb_actuation_hw are it with null records
+int hb_actuation_bridge(hb_ctx* ctx, int B, double delay, const hb_hardware_setting* hw, const hb_motor_bridge* bridge, const double* time,
+                        hb_actuation_state* state, const double* command, const double* rbd, double* tau, double* motor_cmd) {
+  ENTER(ctx, B, time && state && command && rbd && (bridge ? motor_cmd : tau), CAPPED,
+        [&] { return delay_ok(delay) && all_ok(B, hw, hardware_setting_ok) && all_ok(B, bridge, motor_bridge_ok); });
   Staging s(ctx, B);
   auto st = s.inout(state, 1); auto tm = s.in(time, 1); auto cmd = s.in(command, NJ * 5); auto r = s.in(rbd, 32); auto h = s.in_or_null(hw, 1);
-  auto t = s.out(tau, NJ);
-  return s.run(1, [&](Chunk) { return actuation_dev(ctx, B, delay, {h, B}, tm, st, cmd, r, t); });
+  auto mb = s.in_or_null(bridge, 1); auto t = s.out(bridge ? nullptr : tau, NJ); auto m = s.out(bridge ? motor_cmd : nullptr, NJ * 5);
+  return s.run(1, [&](Chunk) { return actuation_dev(ctx, B, delay, {h, B}, {mb, B}, tm, st, cmd, r, t, m); });
 }
 
 int hb_sim_step_batch(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {
@@ -2097,15 +2170,29 @@ int hb_sim_step_varied(hb_ctx* ctx, int B, const hb_sim_params* params, double* 
   return hb_sim_step_terrain(ctx, B, params, rbd, tau, wrench, v, nullptr, contact_force, contact_flag);
 }
 
-// the one host-pointer plant step: the three above are it with null terrains, variations and wrench
 int hb_sim_step_terrain(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* v,
                         const hb_terrain* ter, double* contact_force, uint8_t* contact_flag) {
-  ENTER(ctx, B, params && rbd && tau, CAPPED,
-        [&] { return sim_params_ok(*params) && all_ok(B, v, plant_variation_ok) && all_ok(B, ter, terrain_ok); });
+  return hb_sim_step_bridge(ctx, B, params, rbd, tau, wrench, v, ter, nullptr, nullptr, nullptr, nullptr, contact_force, contact_flag);
+}
+
+// the one host-pointer plant step: the four above are it with null bridges, terrains, variations and wrench
+int hb_sim_step_bridge(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* v,
+                       const hb_terrain* ter, const hb_motor_bridge* bridge, const double* motor_cmd, const double* limits, double* applied,
+                       double* contact_force, uint8_t* contact_flag) {
+  ENTER(ctx, B, params && rbd && (bridge ? motor_cmd && limits : tau != nullptr), CAPPED, [&] {
+    if (bridge) for (size_t k = 0; k < (size_t)B * NJ; ++k) if (!(limits[k] > 0.0)) return false;
+    return sim_params_ok(*params) && all_ok(B, v, plant_variation_ok) && all_ok(B, ter, terrain_ok) && all_ok(B, bridge, motor_bridge_ok);
+  });
+  const bool br = bridge != nullptr;
   Staging s(ctx, B);
-  auto r = s.inout(rbd, 32); auto t = s.in(tau, NJ); auto w = s.in_or_null(wrench, 6); auto pv = s.in_or_null(v, 1); auto pt = s.in_or_null(ter, 1);
+  auto r = s.inout(rbd, 32); auto t = s.in_or_null(br ? nullptr : tau, NJ); auto w = s.in_or_null(wrench, 6); auto pv = s.in_or_null(v, 1);
+  auto pt = s.in_or_null(ter, 1); auto mb = s.in_or_null(bridge, 1); auto mc = s.in_or_null(br ? motor_cmd : nullptr, NJ * 5);
+  auto lim = s.in_or_null(br ? limits : nullptr, NJ); auto ap = s.out(br ? applied : nullptr, NJ);
   auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
-  return s.run(1, [&](Chunk) { return sim_step(ctx, B, *params, r, t, w, {pv, B}, {pt, B}, cf, fl); });
+  return s.run(1, [&](Chunk) {
+    const MotorDrive drive{{mb, B}, mc, lim, {}, {}, br ? (double*)ap : nullptr};
+    return sim_step(ctx, B, *params, r, t, w, {pv, B}, {pt, B}, drive, cf, fl);
+  });
 }
 
 int hb_resident_wbc_batch(hb_ctx* ctx, int B, const double* t_now, const double* rbd, const uint8_t* stance_mode, double* x_des, double* u_des,

@@ -1,6 +1,7 @@
 // Closed-loop episodes (hb_rollout_batch_dev, SURVEY 8f row N2): the joint command law, the actuation model and the plant, and the
 // per-instance kernels the episode loop adds around them, the device planner, the resident cycle and the 500 Hz WBC tick.
 #pragma once
+#include "hb_bridge.cuh"
 #include "hb_common.cuh"
 #include "hb_planner.h"
 #include "hb_qp.cuh"
@@ -302,9 +303,11 @@ __device__ __forceinline__ void add_sensor_offset(const double* off, double* v, 
 // The simulated robot's sensors at absolute tick `tick` from the true rbd r (LeggedHWSim::readSim, LeggedHWSim.cpp:116-130, and the joint
 // encoders). The accelerometer differences the world base velocity over the last plant step (accel_dt) where Gazebo reads the instantaneous
 // acceleration; unprimed, it reads gravity only. Updates base_vel_prev / primed. hw (nullable): the robot's hardware record, whose offsets
-// are added before the noise and whose sigmas replace nz's.
-__device__ __forceinline__ void read_sensors(const hb_sensor_noise& nz, const hb_hardware_setting* hw, uint32_t tick, double accel_dt, const double* r,
-                                             hb_estimation_state& e, double* quat, double* gyro, double* acc, double* jp, double* jv) {
+// are added before the noise and whose sigmas replace nz's. mb (nullable): the robot's motor bridge, whose encoders the joint readings pass
+// after the noise.
+__device__ __forceinline__ void read_sensors(const hb_sensor_noise& nz, const hb_hardware_setting* hw, const hb_motor_bridge* mb, uint32_t tick,
+                                             double accel_dt, const double* r, hb_estimation_state& e, double* quat, double* gyro, double* acc,
+                                             double* jp, double* jv) {
   double sz, cz, sy, cy, sx, cx;
   sincos(r[0], &sz, &cz); sincos(r[1], &sy, &cy); sincos(r[2], &sx, &cx);
   const double R[9] = {cz * cy, cz * sy * sx - sz * cx, cz * sy * cx + sz * sx, sz * cy, sz * sy * sx + cz * cx, sz * sy * cx - cz * sx, -sy, cy * sx, cy * cx};
@@ -329,6 +332,7 @@ __device__ __forceinline__ void read_sensors(const hb_sensor_noise& nz, const hb
   add_sensor_noise(hw ? hw->sigma_linear_acceleration : nz.linear_acceleration, nz.seed, NOISE_BLOCK_ACCEL, tick, st, a, 3);
   add_sensor_noise(hw ? hw->sigma_joint_position : nz.joint_position, nz.seed, NOISE_BLOCK_JOINT_POS, tick, st, q, NJ);
   add_sensor_noise(hw ? hw->sigma_joint_velocity : nz.joint_velocity, nz.seed, NOISE_BLOCK_JOINT_VEL, tick, st, qd, NJ);
+  if (mb) for (int j = 0; j < NJ; ++j) bridge_feedback(*mb, j, &q[j], &qd[j]);
   // quaternion (x, y, z, w) of R = Rz(yaw) Ry(pitch) Rx(roll)
   double hsz, hcz, hsy, hcy, hsx, hcx;
   sincos(0.5 * ang[0], &hsz, &hcz); sincos(0.5 * ang[1], &hsy, &hcy); sincos(0.5 * ang[2], &hsx, &hcx);
@@ -379,14 +383,15 @@ __device__ __forceinline__ void read_odometry(const OdomRead& o, int inst, uint6
 
 // Sensor read of B instances, one thread each. With cflag (the episode tick) the filter's contact flags come from the stored schedule of the
 // latest plan at flag_time, the previous observation's time (LeggedController.cpp:296-297), all 1 before the first plan (:298-304). With odom
-// set (an estimated episode with odometry) each instance's camera is read too. An instance with a record in `hw` reads its sensors on it.
-__global__ void sensor_read_kernel(int B, hb_sensor_noise nz, InstanceView<hb_hardware_setting> hw, uint32_t tick, double accel_dt, double flag_time,
-                                   const double* rbd, hb_estimation_state* est, double* quat, double* gyro, double* acc, double* jp, double* jv,
-                                   uint8_t* cflag, OdomRead odom) {
+// set (an estimated episode with odometry) each instance's camera is read too. An instance with a record in `hw` reads its sensors on it,
+// and one with a record in `bridge` its joints through the bridge's encoders.
+__global__ void sensor_read_kernel(int B, hb_sensor_noise nz, InstanceView<hb_hardware_setting> hw, InstanceView<hb_motor_bridge> bridge, uint32_t tick,
+                                   double accel_dt, double flag_time, const double* rbd, hb_estimation_state* est, double* quat, double* gyro,
+                                   double* acc, double* jp, double* jv, uint8_t* cflag, OdomRead odom) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
   hb_estimation_state& e = est[inst];
-  read_sensors(nz, hw.of(inst), tick, accel_dt, rbd + (size_t)inst * 32, e, quat + (size_t)inst * 4, gyro + (size_t)inst * 3, acc + (size_t)inst * 3,
+  read_sensors(nz, hw.of(inst), bridge.of(inst), tick, accel_dt, rbd + (size_t)inst * 32, e, quat + (size_t)inst * 4, gyro + (size_t)inst * 3, acc + (size_t)inst * 3,
                jp + (size_t)inst * NJ, jv + (size_t)inst * NJ);
   if (cflag) {
     const int mode = e.has_plan ? hbplan::mode_at(e.n_events, e.event_times, e.modes, flag_time) : 3;
@@ -490,13 +495,21 @@ __global__ void joint_command_kernel(int B, hb_pd_gains gains, InstanceView<hb_c
   if (estop) estop[inst] = stop ? 1 : 0;
 }
 
+// The hybrid joint command's PD law (LeggedHWSim.cpp:181-186): one body for the actuation model and the motor bridge's motor PD, so that a
+// neutral bridge reproduces the actuation model bit for bit. The roundings are written out, as the compiler contracts
+// kp (pos - q) + kd (vel - qd) + ff: otherwise the contraction could differ between the call sites.
+__device__ __forceinline__ double hybrid_pd(double pos, double vel, double kp, double kd, double ff, double q, double qd) {
+  return __dadd_rn(__fma_rn(kp, __dsub_rn(pos, q), __dmul_rn(kd, __dsub_rn(vel, qd))), ff);
+}
+
 // Actuation model of the simulated hardware (legged_gazebo/src/LeggedHWSim.cpp:166-192): every write pushes the hybrid joint command
 // (posDes, velDes, kp, kd, ff) with its time stamp on a buffer, drops the entries older than `delay` from the far end, and applies the
 // OLDEST remaining one: tau = kp (posDes - q) + kd (velDes - qd) + ff with the CURRENT joint state. One thread per instance; the deque is a
 // ring of HB_ACT_CAPACITY entries (a full ring drops its oldest entry first). An instance with a hardware record in `hw` runs its delay in
-// place of `delay_all`.
-__global__ void actuation_kernel(int B, double delay_all, InstanceView<hb_hardware_setting> hw, const double* time, hb_actuation_state* state,
-                                 const double* command, const double* rbd, double* tau) {
+// place of `delay_all`. An instance with a record in `bridge` writes the oldest entry's decoded motor command to its row of mcmd (B x 50)
+// instead of a torque to tau; the plant runs its PD.
+__global__ void actuation_kernel(int B, double delay_all, InstanceView<hb_hardware_setting> hw, InstanceView<hb_motor_bridge> bridge, const double* time,
+                                 hb_actuation_state* state, const double* command, const double* rbd, double* tau, double* mcmd) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
   const hb_hardware_setting* h = hw.of(inst);
@@ -512,8 +525,12 @@ __global__ void actuation_kernel(int B, double delay_all, InstanceView<hb_hardwa
   ++cnt;
   st.count = cnt; st.head = head;
   const double* c = st.cmd[(head + cnt - 1) % HB_ACT_CAPACITY];
+  if (const hb_motor_bridge* mb = bridge.of(inst)) {
+    for (int j = 0; j < NJ; ++j) bridge_command(*mb, j, c + 5 * j, mcmd + ((size_t)inst * NJ + j) * 5);
+    return;
+  }
   const double* r = rbd + (size_t)inst * 32;
-  for (int j = 0; j < NJ; ++j) tau[(size_t)inst * NJ + j] = c[5 * j + 2] * (c[5 * j] - r[6 + j]) + c[5 * j + 3] * (c[5 * j + 1] - r[NQ + 6 + j]) + c[5 * j + 4];
+  for (int j = 0; j < NJ; ++j) tau[(size_t)inst * NJ + j] = hybrid_pd(c[5 * j], c[5 * j + 1], c[5 * j + 2], c[5 * j + 3], c[5 * j + 4], r[6 + j], r[NQ + 6 + j]);
 }
 
 // One step of a batched rigid-body simulation of the robot on the ground (stands in for the Gazebo / MuJoCo plant of the reference's
@@ -562,15 +579,40 @@ __device__ __forceinline__ double sloped_contact(const double* p, const double* 
   return fn;
 }
 
+// The motor bridge's side of a plant step (motor bridge, hunter_b200.h): the bridged instances (rec; an empty view bridges none), their
+// decoded motor commands (cmd, B x 50), their torque limits (lim_rows, B x 10, when given; otherwise the hardware record's, or lim) and
+// where the mean over the substeps of the clipped torque goes (applied, B x 10, nullable).
+struct MotorDrive {
+  InstanceView<hb_motor_bridge> rec;
+  const double* cmd;
+  const double* lim_rows;
+  InstanceView<hb_hardware_setting> hw;
+  double lim[NJ];
+  double* applied;
+};
+
+// The torque the motor of joint j of bridged instance inst applies at joint state q, qd: the hybrid PD law in the motor frame, back to the
+// joint frame, clipped to the instance's limit. Not inlined, as payload_rnea, to keep sim_step_kernel without spills.
+__device__ __noinline__ double bridge_motor_torque(const MotorDrive& d, const hb_motor_bridge& b, int inst, int j, double q, double qd) {
+  const double* m = d.cmd + ((size_t)inst * NJ + j) * 5;
+  const hb_hardware_setting* h = d.hw.of(inst);
+  const double lim = d.lim_rows ? d.lim_rows[(size_t)inst * NJ + j] : h ? h->torque_limit[j] : d.lim[j], dir = (double)b.direction[j];
+  const double t = dir * hybrid_pd(m[0], m[1], m[2], m[3], m[4], dir * q + b.zero[j], dir * qd);
+  return t < -lim ? -lim : (t > lim ? lim : t);
+}
+
 // The views are __grid_constant__ (read in place, never copied): as plain by-value parameters they cost the kernel two registers.
 __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, double* rbd_io, const double* tau, const double* wrench,
                                                       const __grid_constant__ InstanceView<hb_plant_variation> var,
-                                                      const __grid_constant__ InstanceView<hb_terrain> terrain, double* contact_force, uint8_t* contact_flag) {
+                                                      const __grid_constant__ InstanceView<hb_terrain> terrain, const __grid_constant__ MotorDrive drive,
+                                                      double* contact_force, uint8_t* contact_flag) {
   __shared__ SimShared sh;
   const int inst = blockIdx.x, lane = threadIdx.x;
   const hb_plant_variation* pv = var.of(inst);      // null: the nominal plant
   const hb_terrain* ter = terrain.of(inst);         // null: flat ground at prm.ground_height
+  const hb_motor_bridge* mb = drive.rec.of(inst);   // null: the joints receive tau
   bool touch = false;                    // lanes 0-3: the normal force of their contact in the last substep is positive
+  double applied = 0.0;                  // lanes 6-15 of a bridged instance: the sum over the substeps of the motor's clipped torque
   double* r = rbd_io + (size_t)inst * 32;
   if (lane == 0) rbd_to_qv(r, sh.q, sh.v);
   __syncwarp();
@@ -623,8 +665,14 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
     if (lane < NQ) {
       // joint side of the plant as in the reference's MuJoCo model (mujoco/model/hunter/hunter.xml:6): rotor armature on the diagonal of M,
       // viscous joint damping. A varied plant's motor strength scales the torque first, as one rounded product (never contracted into
-      // the damping term), so that strength s on tau is strength 1 on s * tau.
-      double tj = lane >= 6 ? tau[(size_t)inst * NJ + lane - 6] : 0.0;
+      // the damping term), so that strength s on tau is strength 1 on s * tau. A bridged joint's motor runs its PD on this substep's state.
+      double tj = 0.0;
+      if (lane >= 6 && mb) {
+        tj = bridge_motor_torque(drive, *mb, inst, lane - 6, sh.q[lane], sh.v[lane]);
+        applied = sub ? applied + tj : tj;
+      } else if (lane >= 6) {
+        tj = tau[(size_t)inst * NJ + lane - 6];
+      }
       if (pv && lane >= 6) tj = __dmul_rn(pv->motor_strength[lane - 6], tj);
       double s = -sh.nle[lane] + (lane >= 6 ? tj - prm.joint_damping * sh.v[lane] : 0.0);
       for (int rr = 0; rr < 12; ++rr) s += sh.J[rr * NQ + lane] * sh.F[rr];
@@ -650,6 +698,7 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
     __syncwarp();
   }
   if (lane == 0) qv_to_rbd(sh.q, sh.v, r);
+  if (lane >= 6 && lane < NQ && mb && drive.applied) drive.applied[(size_t)inst * NJ + lane - 6] = applied / (prm.substeps > 0 ? prm.substeps : 1);
   if (lane < 12 && contact_force) contact_force[(size_t)inst * 12 + lane] = sh.F[lane];
   if (lane < 4 && contact_flag) contact_flag[(size_t)inst * 4 + lane] = touch ? 1 : 0;
 }

@@ -287,7 +287,8 @@ typedef struct {                 /* per-instance outcome, in/out: start an episo
   int32_t fail_tick;             /* absolute tick of the first failure, -1: never failed                                          */
   int32_t fail_reason;           /* HB_ROLLOUT_FAIL_* bits of that tick                                                           */
   int32_t mpc_bad, wbc_fallbacks, plan_rejects;   /* counts of info.status != 0, wbc_status != 0, plan_status != 0                */
-  double max_abs_torque;         /* over the applied (saturated) torques, before a plant variation's motor_strength scales them  */
+  double max_abs_torque;         /* over the applied (saturated) torques, before a plant variation's motor_strength scales them
+                                    (with a motor bridge: the mean over the tick's substeps of the motor's clipped torque)        */
 } hb_rollout_stats;
 int hb_default_rollout_params(hb_rollout_params* p);       /* host only */
 
@@ -313,6 +314,7 @@ int hb_default_rollout_params(hb_rollout_params* p);       /* host only */
 #define HB_SETTING_PLANNER 7
 #define HB_SETTING_TARGETS 8
 #define HB_SETTING_LATENCIES 9
+#define HB_SETTING_MOTOR_BRIDGE 11     /* hb_motor_bridge for hb_rollout_set_motor_bridge (10 stays unassigned: callers have used it as an unknown kind) */
 /* The record check of the setting call of `kind`, without a context (host only, no GPU needed): records (B of the kind's type) are judged
  * by that call's rules for a record, and a record passes iff the call accepts it (the call's other checks, such as B against max_batch,
  * need its context). 0: every record passes, *first_bad = -1. -1: *first_bad is the index of the first record that fails, or -1 for an
@@ -531,6 +533,58 @@ int hb_default_hardware_setting(hb_hardware_setting* s);
  * negative actuation_delay, a torque_limit <= 0 or a negative sigma. */
 int hb_rollout_set_hardware(hb_ctx* ctx, int B, const hb_hardware_setting* s);
 
+/* ---- motor bridge: each robot's joint path through the real Hunter's driver (legged_bridge_hw) in place of LeggedHWSim's torque law ----
+ * Like the hardware setting, it acts on the simulated robot only; the planner, MPC, WBC, joint command law and estimator are not told
+ * about it. Record i acts on instance i of the episodes; instances at or beyond B run the unbridged path bit for bit. The bridge has no
+ * state of its own (hb_episode_state_bytes does not count it). With r the record of an instance, joint j:
+ *  - command (BridgeHW::write, BridgeHW.cpp:67-88, then the motor protocol, motor_control.c:146-225): the actuation model's drop rule is
+ *    unchanged (the hardware record's delay included); the oldest remaining entry (posDes, velDes, kp, kd, ff) is mapped to the motor frame
+ *    in double: kp_m = s kp, kd_m = s kd, pos_m = d posDes + z, vel_m = d velDes, ff_m = (s ff) d, with s = command_scale[j],
+ *    d = direction[j], z = zero[j]. Each is clamped to its range: kp_m to [0, kp_max], kd_m to [0, kd_max], pos_m, vel_m and ff_m to
+ *    +-pos_max, +-vel_max, +-ff_max. With quantise = 1 each is first rounded to float32, clamped in float32, encoded as the protocol does,
+ *    code = (int)((x - min) * (2^bits - 1) / span), truncated, with 12 / 9 / 16 / 12 / 12 bits for kp / kd / pos / vel / ff, and decoded
+ *    as (float)code * span / (2^bits - 1) + min, every float32 operation rounded on its own (span = max - min in float32). Deviation: the
+ *    firmware's decode is not public; it is assumed to be the map the driver uses for feedback. A NaN value encodes as code 0 (what a
+ *    float-to-int truncation on the GPU gives); +-inf clamps to the range's end. With quantise = 0 the values are clamped in double and
+ *    neither rounded nor encoded (a NaN stays NaN).
+ *  - motor PD (on the motor, at its own rate): on every plant substep, the joint receives tau = d (kp_m (pos_m - (d q + z)) + kd_m
+ *    (vel_m - d qd) + ff_m) with that substep's q, qd: the same PD law as the unbridged actuation, evaluated in the motor frame. Deviation:
+ *    the driver's loop runs at the plant's substep rate (sim.dt / sim.substeps, 2 kHz by default). tau is clipped to the instance's torque
+ *    limit (the hardware record's, or hb_rollout_params.torque_limit) and then scaled by a plant variation's motor_strength, as unbridged.
+ *    The episode's saturation step does not act on the instance: the plant clips. The applied torque that HB_CHANNEL_TORQUE records and
+ *    hb_rollout_stats.max_abs_torque counts is the mean over the tick's substeps of the clipped tau, before motor_strength.
+ *  - encoders (hb_rollout_estimated_batch_dev only; motor_control.c:484-500, BridgeHW.cpp:35-43): the joint readings are formed as (1) the
+ *    true q, qd; (2) plus the hardware record's encoder offset and the noise, as unbridged; (3) to the motor frame, d q + z and d qd; (4)
+ *    clamped to +-pos_max / +-vel_max and, with quantise = 1, rounded to float32, encoded in 16 / 12 bits and decoded as above; (5) back to
+ *    the joint frame, (p - z) d: in float32 with quantise = 1 (the driver's values are float32), in double without. Deviation: no current
+ *    or torque feedback, which nothing in the episode loop reads.
+ * A record with scale 1, directions +-1, zero 0, quantise 0 and ranges that never bind, on a plant with one substep, gives the unbridged
+ * episode bit for bit. hb_rollout_batch_dev has no sensors and reads only the command side. The setting adds no launch to an episode:
+ * the actuation, plant and sensor kernels that run every tick read the record of their own instance. Every other entry point ignores it;
+ * hb_actuation_bridge, hb_sim_step_bridge and hb_sim_read_sensors_bridge take records explicitly. */
+typedef struct {                 /* one robot's joint path through legged_bridge_hw, which the controllers are not told about   */
+  double command_scale[10];      /* multiplies kp, kd and ff, >= 0 (BridgeHW.cpp:74-85: 0.7 on joints 0, 1, 5, 6; 1 elsewhere)    */
+  int32_t direction[10];         /* +1 or -1: motor angle = direction * q + zero (BridgeHW.h:118)                                */
+  double zero[10];               /* motor angle of joint angle 0 [rad] (baseMotor_, BridgeHW.h:120: 0)                           */
+  double kp_max[10];             /* protocol range of kp: [0, kp_max], > 0 (motor_control.c:11-35: 500)                          */
+  double kd_max[10];             /* [0, kd_max], > 0 (5)                                                                         */
+  double pos_max[10];            /* +-pos_max [rad], > 0 (12.5)                                                                  */
+  double vel_max[10];            /* +-vel_max [rad/s], > 0 (18)                                                                  */
+  double ff_max[10];             /* +-ff_max [N m], > 0 (30 on X motors, 90 on D motors: joints 2, 3, 7, 8, transmit.cpp:434-500) */
+  int32_t quantise;              /* 1: the protocol's float32 codes; 0: clamps only, in double                                  */
+} hb_motor_bridge;               /* 608 B */
+/* host only: the reference's record: the scales, directions and zeros above, each joint's X or D motor ranges, quantise = 1 */
+int hb_default_motor_bridge(hb_motor_bridge* r);
+/* Sets the motor bridges of the context's episodes (a per-robot episode setting, above). -1 also for a direction other than +-1, a
+ * non-finite value, a negative command_scale, a maximum <= 0, or quantise outside {0, 1}. */
+int hb_rollout_set_motor_bridge(hb_ctx* ctx, int B, const hb_motor_bridge* r);
+/* The bridge's codec on the host, the same functions the kernels run (host only, no context, no GPU): hb_motor_bridge_encode maps
+ * command (B x 10 x 5, joint frame, as hb_joint_command_batch writes it) to the decoded motor command out (B x 10 x 5: pos_m, vel_m,
+ * kp_m, kd_m, ff_m in the motor frame) of records r (B); hb_motor_bridge_feedback maps joint readings q, qd (B x 10) through steps (3) to
+ * (5) of the encoders to q_out, qd_out. -1: B < 0, a NULL pointer with B > 0, or a record hb_rollout_set_motor_bridge rejects. */
+int hb_motor_bridge_encode(int B, const hb_motor_bridge* r, const double* command, double* out);
+int hb_motor_bridge_feedback(int B, const hb_motor_bridge* r, const double* q, const double* qd, double* q_out, double* qd_out);
+
 /* ---- estimated episodes (hb_rollout_estimated_batch_dev): the controllers read the Kalman filter's estimate from synthesised, noisy
  * sensors instead of the plant's true state (LeggedController::updateStateEstimation, LeggedController.cpp:280-349) ---- */
 typedef struct {                 /* standard deviations of additive Gaussian sensor noise; 0 = that channel is exact and draws nothing */
@@ -748,7 +802,8 @@ int hb_rollout_estimated_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_tick
  * beyond its ceil(n_ticks / log_every) are not written. A call with log_every > 0 is rejected (-1, nothing enqueued) when a set channel
  * has fewer than B instances or fewer than ceil(n_ticks / log_every) rows. With no channel set, or log_every == 0, an episode launches
  * exactly what it launches without this feature; otherwise it adds one launch per recorded tick. */
-#define HB_CHANNEL_TORQUE 0          /* double x 10: applied torques after saturation (what the plant step receives, before a variation's motor_strength) */
+#define HB_CHANNEL_TORQUE 0          /* double x 10: applied torques after saturation (what the plant step receives, before a variation's motor_strength;
+                                        with a motor bridge, the mean over the tick's substeps of the motor's clipped torque) */
 #define HB_CHANNEL_JOINT_COMMAND 1   /* double x 50: the joint command law's output per joint (pos_des, vel_des, kp, kd, ff), before the actuation delay */
 #define HB_CHANNEL_X_DES 2           /* double x 22: the policy's desired state at t (adopted policy with a latency) */
 #define HB_CHANNEL_U_DES 3           /* double x 22 */
@@ -842,6 +897,29 @@ int hb_actuation_hw(hb_ctx* ctx, int B, double delay, const hb_hardware_setting*
 int hb_sim_read_sensors_hw(hb_ctx* ctx, int B, const hb_sensor_noise* noise, const hb_hardware_setting* hw /*nullable*/, int64_t tick,
                            double accel_dt, const double* rbd, hb_estimation_state* est, double* quat, double* ang_vel_local, double* lin_acc_local,
                            double* joint_pos, double* joint_vel);
+/* ---- the motor bridge outside the episodes (motor bridge, above): the episode's actuation, plant step and sensor read with explicit
+ * records, so that an episode with hb_rollout_set_motor_bridge can be written as a loop of public calls ----
+ * bridge (B, nullable): the record of every robot of the call, validated as by hb_rollout_set_motor_bridge (-1). Host pointers,
+ * synchronous; the context's settings are not read.
+ * hb_actuation_bridge: hb_actuation_hw, and with bridge, robot i's oldest entry is encoded on bridge[i] and written to motor_cmd (B x 10 x
+ * 5: pos_m, vel_m, kp_m, kd_m, ff_m) in place of a torque to tau. Without bridge, tau is required and motor_cmd is not written (nullable);
+ * with it, motor_cmd is required and tau is not written (nullable). hb_actuation_hw and hb_actuation_batch are it with bridge = NULL. */
+int hb_actuation_bridge(hb_ctx* ctx, int B, double delay, const hb_hardware_setting* hw /*nullable*/, const hb_motor_bridge* bridge /*nullable*/,
+                        const double* time, hb_actuation_state* state, const double* command, const double* rbd, double* tau /*nullable with bridge*/,
+                        double* motor_cmd /*nullable without bridge*/);
+/* hb_sim_step_terrain, and with bridge, each robot's joints run the motor PD on motor_cmd (B x 10 x 5, hb_actuation_bridge's) on every
+ * substep, clipped to limits (B x 10, > 0); tau is then not read (nullable) and applied (B x 10, nullable) receives the mean over the
+ * substeps of the clipped torque. Without bridge, tau is required and motor_cmd, limits and applied are not read or written.
+ * hb_sim_step_terrain is it with bridge, motor_cmd, limits and applied NULL. */
+int hb_sim_step_bridge(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau /*nullable with bridge*/,
+                       const double* wrench /*nullable*/, const hb_plant_variation* v /*nullable*/, const hb_terrain* t /*nullable*/,
+                       const hb_motor_bridge* bridge /*nullable*/, const double* motor_cmd, const double* limits, double* applied /*nullable*/,
+                       double* contact_force /*nullable*/, uint8_t* contact_flag /*nullable*/);
+/* hb_sim_read_sensors_hw, and with bridge, each robot's joint readings pass its encoders (steps (3) to (5) of the motor bridge, above)
+ * after the offsets and the noise. hb_sim_read_sensors_hw is it with bridge = NULL. */
+int hb_sim_read_sensors_bridge(hb_ctx* ctx, int B, const hb_sensor_noise* noise, const hb_hardware_setting* hw /*nullable*/,
+                               const hb_motor_bridge* bridge /*nullable*/, int64_t tick, double accel_dt, const double* rbd, hb_estimation_state* est,
+                               double* quat, double* ang_vel_local, double* lin_acc_local, double* joint_pos, double* joint_vel);
 int hb_sim_step_batch(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force /*nullable*/,
                       uint8_t* contact_flag /*nullable*/);
 /* hb_sim_step_batch with an external world wrench on each robot's base: wrench (B x 6) = force [N] at the base frame origin, then a couple
@@ -854,8 +932,8 @@ int hb_sim_step_wrench(hb_ctx* ctx, int B, const hb_sim_params* params, double* 
 int hb_sim_step_varied(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench /*nullable*/,
                        const hb_plant_variation* v /*nullable*/, double* contact_force /*nullable*/, uint8_t* contact_flag /*nullable*/);
 /* hb_sim_step_varied on terrains: t (B, nullable) = the ground under each robot (terrain, above), validated as by hb_rollout_set_terrains
- * (-1). NULL t is exactly hb_sim_step_varied. This is the one host-pointer plant step: hb_sim_step_batch, hb_sim_step_wrench and
- * hb_sim_step_varied are it with the arguments they lack passed as NULL. */
+ * (-1). NULL t is exactly hb_sim_step_varied. hb_sim_step_batch, hb_sim_step_wrench and hb_sim_step_varied are it with the arguments
+ * they lack passed as NULL, and it is hb_sim_step_bridge (the motor bridge, above) without a bridge. */
 int hb_sim_step_terrain(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench /*nullable*/,
                         const hb_plant_variation* v /*nullable*/, const hb_terrain* t /*nullable*/, double* contact_force /*nullable*/,
                         uint8_t* contact_flag /*nullable*/);
