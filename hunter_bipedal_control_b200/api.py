@@ -57,6 +57,7 @@ EXPORTED_SYMBOLS = [
     "hb_default_hardware_setting", "hb_rollout_set_hardware", "hb_actuation_hw", "hb_sim_read_sensors_hw",
     "hb_default_motor_bridge", "hb_rollout_set_motor_bridge", "hb_motor_bridge_encode", "hb_motor_bridge_feedback", "hb_actuation_bridge",
     "hb_sim_step_bridge", "hb_sim_read_sensors_bridge",
+    "hb_default_teleop_setting", "hb_rollout_set_teleop", "hb_cmd_vel_to_target",
     "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
     "hb_check_setting_records", "hb_rollout_set_channel",
     "hb_episode_state_bytes", "hb_episode_save_async", "hb_episode_restore",
@@ -111,6 +112,17 @@ def reference_target(ref):
     """The target trajectory an HbReference carries (its target samples) as an HbTarget."""
     n = ref.n_targets
     return make_targets([np.array(ref.target_times[:n])], [np.array([ref.target_states[k][:] for k in range(n)])])[0]
+
+
+def cmd_vel_to_target(t, horizon, x, cmd_vel):
+    """cmdVelToTargetTrajectories (hb_cmd_vel_to_target) for a batch: the two-sample target the planner builds from cmd_vel (vx, vy, vz, yaw
+    rate) at time t on the observation x with time_to_target = horizon. t (B,) or a scalar, x (B, 22), cmd_vel (B, 4) or (4,). Returns a
+    ctypes array of B HbTarget."""
+    x = _f64(x).reshape(-1, NX); B = x.shape[0]
+    t = _f64(np.broadcast_to(_f64(t), (B,))); cmd = _f64(np.broadcast_to(_f64(cmd_vel), (B, 4)))
+    out = (HbTarget * B)()
+    _check(load_library().hb_cmd_vel_to_target(B, _ptr(t), C.c_double(horizon), _ptr(x), _ptr(cmd), out), "hb_cmd_vel_to_target")
+    return out
 
 
 def goal_to_target(t, x, goal):
@@ -692,6 +704,74 @@ def bridge_feedback(bridge, q, qd):
     _check(load_library().hb_motor_bridge_feedback(B, _bridge_records(bridge, B, "bridge_feedback"), _ptr(q), _ptr(qd), _ptr(q_out), _ptr(qd_out)),
            "hb_motor_bridge_feedback")
     return q_out, qd_out
+
+
+HB_MAX_TELEOP_WINDOWS = 4
+TELEOP_ALWAYS = 2 ** 31 - 1      # an off_tick that never comes (INT32_MAX)
+
+
+class HbTeleopSetting(C.Structure):
+    SETTING_KIND = 12        # HB_SETTING_TELEOP, the record's kind for hb_check_setting_records
+    _fields_ = [("period_ticks", C.c_int32), ("n_window", C.c_int32), ("on_tick", C.c_int32 * HB_MAX_TELEOP_WINDOWS),
+                ("off_tick", C.c_int32 * HB_MAX_TELEOP_WINDOWS), ("change_limit", C.c_double * 3)]
+
+
+HbTeleop = HbTeleopSetting
+
+
+def default_teleop_setting():
+    """hb_default_teleop_setting: the reference's joystick and publisher: a message every 50 ticks (10 Hz), the deadman held from tick 0
+    on, the change per message limited to 0.1 m/s, 0.05 m/s and 0.3 rad/s."""
+    r = HbTeleopSetting()
+    _check(load_library().hb_default_teleop_setting(C.byref(r)), "hb_default_teleop_setting")
+    return r
+
+
+def make_teleop_settings(B, period_ticks=50, windows=((0, TELEOP_ALWAYS),), change_limit=(0.1, 0.05, 0.3)):
+    """ctypes array of B HbTeleopSetting (Context.set_teleop): each robot's joystick and target publisher in the episodes. period_ticks:
+    (B,) or a scalar; windows: the absolute ticks [on, off) the deadman is held, (n, 2) for every robot, (B, n, 2), or a sequence of B
+    (n_i, 2) sequences, n <= HB_MAX_TELEOP_WINDOWS (n = 0: no message ever); change_limit: the per-message change of vx, vy and yaw rate,
+    (3,) or (B, 3) (inf: no limit). Raises ValueError for a shape that does not broadcast, a tick that is not an int32 integer and a record
+    hb_rollout_set_teleop rejects (its own check)."""
+    def ticks(a, shape, what):
+        x = np.asarray(a, dtype=np.float64)
+        try:
+            x = np.broadcast_to(x, shape)
+        except ValueError as e:
+            raise ValueError("teleop settings: %s: %s expected: %s" % (what, shape, e))
+        if not (np.isfinite(x).all() and (x == np.rint(x)).all() and (np.abs(x) < 2 ** 31).all()):
+            raise ValueError("teleop settings: %s: int32 integers expected" % what)
+        return x.astype(np.int32)
+    w = None
+    try:
+        w = np.asarray(windows, dtype=np.float64)
+    except ValueError:
+        pass
+    shape_error = ValueError("teleop settings: windows: (n, 2), (B, n, 2) or B sequences of (n_i, 2) expected")
+    if w is not None and w.size == 0:                   # no window: no message ever
+        per = [np.zeros((0, 2))] * B
+    elif w is not None and w.ndim == 2 and w.shape[1] == 2:
+        per = [w] * B
+    elif w is not None and w.ndim == 3 and w.shape[0] == B and w.shape[2] == 2:
+        per = list(w)
+    elif w is None and len(windows) == B:
+        per = [np.asarray(x, dtype=np.float64).reshape(-1, 2) for x in windows]
+    else:
+        raise shape_error
+    if any(len(x) > HB_MAX_TELEOP_WINDOWS for x in per):
+        raise ValueError("teleop settings: at most %d windows per robot" % HB_MAX_TELEOP_WINDOWS)
+    out = (HbTeleopSetting * B)()
+    v = np.ctypeslib.as_array(out)
+    v["period_ticks"] = ticks(period_ticks, (B,), "period_ticks")
+    for i, x in enumerate(per):
+        x = ticks(x, x.shape, "windows")
+        v["n_window"][i] = len(x)
+        v["on_tick"][i, :len(x)] = x[:, 0]; v["off_tick"][i, :len(x)] = x[:, 1]
+    try:
+        v["change_limit"] = np.broadcast_to(_f64(change_limit), (B, 3))
+    except ValueError as e:
+        raise ValueError("teleop settings: change_limit: (3,) or (B, 3) expected: %s" % e)
+    return _check_records(HbTeleopSetting.SETTING_KIND, out, "teleop")
 
 
 HB_ODOM_MAX_DELAY = 15
@@ -1304,6 +1384,14 @@ class Context:
         motor's PD on every plant substep and, in rollout_estimated, quantised encoders; instances beyond len(bridges) run the simulated
         hardware's torque law; None clears them. The controllers are not told about it, and no other call reads it."""
         self._set_instances("hb_rollout_set_motor_bridge", bridges)
+
+    def set_teleop(self, settings):
+        """Teleoperation of this context's episodes (hb_rollout_set_teleop): settings[i] (make_teleop_settings) is the joystick and target
+        publisher of instance i of every later rollout / rollout_estimated call: rate-limited cmd_vel messages at the teleop rate while the
+        deadman is held, each converted once into a target (cmd_vel_to_target), the filtered command as the planner's cmd_vel; instances
+        beyond len(settings) follow their cmd_vel segments directly; None clears them. Every call clears the publishers and the captured
+        targets. An episode call rejects a record whose period or window starts are not multiples of its mpc_every."""
+        self._set_instances("hb_rollout_set_teleop", settings)
 
     def set_channels(self, channels):
         """Recorded channels of this context's episodes (hb_rollout_set_channel): channels maps names of CHANNELS to contiguous cuda

@@ -111,6 +111,11 @@ struct hb_ctx {
   InstanceSetting<hb_hardware_setting> hardware;
   // each instance's joint path through the real robot's motor driver in the episodes (hb_rollout_set_motor_bridge)
   InstanceSetting<hb_motor_bridge> bridges;
+  // each instance's joystick and target publisher in the episodes (hb_rollout_set_teleop), and the publishers' state, allocated at
+  // max_batch by the first call that sets records
+  InstanceSetting<hb_teleop_setting> teleop;
+  void* tele_mem;
+  TeleopState* tele_state;
   // each instance's gait templates and swing settings in every device planner path (hb_plan_set_settings)
   InstanceSetting<hb_planner_settings> plan_settings;
   // the recorded channels of the episodes (hb_rollout_set_channel): the caller's buffer, its instances and rows; B == 0: unset
@@ -499,7 +504,7 @@ int hb_create(const hb_config* cfg, int device, hb_ctx** out) {
 int hb_destroy(hb_ctx* ctx) {
   if (!ctx) return HB_EINVAL;
   cudaSetDevice(ctx->device);
-  void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->snap_mem, ctx->arena,
+  void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->tele_mem, ctx->snap_mem, ctx->arena,
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
                        ctx->odometry.dev, ctx->controllers.dev, ctx->hardware.dev, ctx->plan_settings.dev,
                        ctx->bridges.dev};
@@ -1245,6 +1250,10 @@ int hb_rollout_set_goals(hb_ctx* ctx, int B, const hb_goal_schedule* g) {
   rc = goal_reserve(ctx);
   if (rc) { ctx->goals.n = 0; return rc; }
   CK(cudaMemsetAsync(ctx->goal_idx, 0xff, sizeof(int32_t) * ctx->cfg.max_batch, ctx->stream));     // every captured goal forgotten: index -1
+  // and the goal each teleop publisher last saw (goal_seen 0: none), so that teleoperated instances capture the new goals as the others do
+  if (ctx->tele_mem)
+    CK(cudaMemset2DAsync(reinterpret_cast<char*>(ctx->tele_state) + offsetof(TeleopState, goal_seen), sizeof(TeleopState), 0, sizeof(int32_t),
+                         ctx->cfg.max_batch, ctx->stream));
   return HB_OK;
 }
 
@@ -1283,6 +1292,50 @@ static int camera_reserve(hb_ctx* ctx) {
     ctx->odom_cam = carve<OdomCamera>(m, off, Bc);
     return off;
   });
+}
+
+// The ranges of hunter_b200.h's hb_teleop_setting: a period, windows that ascend without overlapping, limits > 0 (+inf: none). The
+// multiples of the episode's mpc_every are checked by the episode call.
+static bool teleop_setting_ok(const hb_teleop_setting& s) {
+  if (s.period_ticks < 1 || s.n_window < 0 || s.n_window > HB_MAX_TELEOP_WINDOWS) return false;
+  for (int w = 0; w < s.n_window; ++w)
+    if (s.on_tick[w] < 0 || !(s.on_tick[w] < s.off_tick[w]) || (w > 0 && s.on_tick[w] < s.off_tick[w - 1])) return false;
+  for (double lim : s.change_limit) if (!(lim > 0.0)) return false;
+  return true;
+}
+
+int hb_default_teleop_setting(hb_teleop_setting* s) {
+  if (!s) return HB_EINVAL;
+  memset(s, 0, sizeof(*s));
+  s->period_ticks = 50;                                     // joy_node autorepeat_rate 10 Hz (joy_teleop.launch) at the 500 Hz tick
+  s->n_window = 1; s->on_tick[0] = 0; s->off_tick[0] = INT32_MAX;
+  s->change_limit[0] = 0.1; s->change_limit[1] = 0.05; s->change_limit[2] = 0.3;     // changeLimit_ (TargetTrajectoriesPublisher.h:97)
+  return HB_OK;
+}
+
+// The publishers' state, allocated at max_batch by its first use (hb_rollout_set_teleop with records), with the captured targets it writes
+static int teleop_reserve(hb_ctx* ctx) {
+  const size_t Bc = ctx->cfg.max_batch;
+  int rc = goal_reserve(ctx);
+  if (!rc) rc = reserve_group(&ctx->tele_mem, [&](void* m) {
+    size_t off = 0;
+    ctx->tele_state = carve<TeleopState>(m, off, Bc);
+    return off;
+  });
+  return rc;
+}
+
+int hb_rollout_set_teleop(hb_ctx* ctx, int B, const hb_teleop_setting* s) {
+  int rc = set_instances(ctx, B, s, teleop_setting_ok, &hb_ctx::teleop);
+  if (rc) return rc;
+  if (ctx->teleop.n > 0) rc = teleop_reserve(ctx);
+  if (rc) { ctx->teleop.n = 0; return rc; }
+  if (!ctx->tele_mem) return HB_OK;          // cleared, never set: no publisher and no message target exist
+  // every publisher and captured target cleared, by a clearing call too (no target of a message outlives the setting): last 0, no goal
+  // seen, source -1
+  CK(cudaMemsetAsync(ctx->tele_state, 0, sizeof(TeleopState) * ctx->cfg.max_batch, ctx->stream));
+  CK(cudaMemsetAsync(ctx->goal_idx, 0xff, sizeof(int32_t) * ctx->cfg.max_batch, ctx->stream));
+  return HB_OK;
 }
 
 int hb_rollout_set_odometry(hb_ctx* ctx, int B, const hb_odometry_setting* s) {
@@ -1330,6 +1383,7 @@ int hb_check_setting_records(int32_t kind, int B, const void* records, int32_t* 
     case HB_SETTING_TARGETS: return check_records(B, records, target_ok, first_bad);
     case HB_SETTING_LATENCIES: return check_records(B, records, latency_ok, first_bad);
     case HB_SETTING_MOTOR_BRIDGE: return check_records(B, records, motor_bridge_ok, first_bad);
+    case HB_SETTING_TELEOP: return check_records(B, records, teleop_setting_ok, first_bad);
     default: return HB_EINVAL;
   }
 }
@@ -1476,6 +1530,11 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
       for (int k = 0; k < c.n_cmd; ++k) if (!(c.cmd_time[k] == c.cmd_time[k]) || (k > 0 && c.cmd_time[k] < c.cmd_time[k - 1])) return false;
     }
     for (int i = 0; i < lat.n; ++i) if (lat.host[i] > p->mpc_every) return false;     // latencies beyond one MPC period
+    for (int i = 0; i < ctx->teleop.n; ++i) {                                          // teleop messages off the MPC ticks
+      const hb_teleop_setting& s = ctx->teleop.host[i];
+      if (s.period_ticks < 1 || s.period_ticks % p->mpc_every != 0) return false;
+      for (int w = 0; w < s.n_window; ++w) if (s.on_tick[w] % p->mpc_every != 0) return false;
+    }
     // a warm start continues from the resident solution, and the instances with a latency from their adopted policies
     for (int i = 0; i < with_lat && !cold; ++i) if (lat.host[i] >= 1 && !policies_adopted(ctx, i, i + 1)) return false;
     return cold || ctx->res_valid >= B;
@@ -1520,7 +1579,8 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   double* meas = e ? ctx->re_rbd : rbd;
   // the push wrench the begin kernel writes and the plant applies, none without schedules
   double* wrench = ctx->pushes.n > 0 ? ctx->ro_wrench : nullptr;
-  const InstanceView<hb_target> goal_targets{ctx->goal_tg, ctx->goals.n};    // what the planner reads: the targets of the captured goals
+  // what the planner reads: the captured targets of the goals and the teleop messages
+  const InstanceView<hb_target> goal_targets{ctx->goal_tg, std::max(ctx->goals.n, ctx->teleop.n)};
   // the cameras the sensor read reads and the messages the filter fuses, none without an odometry setting
   const bool odom = e && ctx->odometry.n > 0;
   const OdomRead odom_read = odom ? odometry_read(ctx, ctx->re_opos, ctx->re_ohas) : OdomRead{};
@@ -1551,8 +1611,8 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
     if (!rc && delayed && a >= first_due[a % p->mpc_every]) rc = policy_adopt(ctx, B, lat.view(), a, p->mpc_every, nullptr);
     if (!rc && mpc) {
       if (first_cold) CK(cudaMemsetAsync(ctx->res_stance, 0, sizeof(double) * B * 12, ctx->stream));   // latestStanceposition_ starts at zero
-      rc = launch(ctx, K_UNPROFILED, rollout_plan_inputs_kernel, grid, 64, 0, B, t, horizon, ctx->ro_cmd, meas, e ? e->est : nullptr, ctx->ro_in,
-                  ctx->goals.view(), first_cold ? 1 : 0, ctx->goal_tg, ctx->goal_idx, plan_consts());
+      rc = launch(ctx, K_UNPROFILED, rollout_plan_inputs_kernel, grid, 64, 0, B, (int)a, t, horizon, ctx->ro_cmd, meas, e ? e->est : nullptr,
+                  ctx->ro_in, ctx->goals.view(), ctx->teleop.view(), ctx->tele_state, first_cold ? 1 : 0, ctx->goal_tg, ctx->goal_idx, plan_consts());
       if (!rc) rc = launch(ctx, K_UNPROFILED, plan_prepare_kernel, grid, 64, 0, B, ctx->ro_in, ctx->ro_t0, ctx->ro_x0, ctx->ro_feet);
       if (!rc) rc = plan_dev(ctx, B, ctx->ro_in, ctx->ro_feet, ctx->res_stance, ctx->ro_refs, ctx->ro_pstat, goal_targets, ctx->goal_idx,
                              ctx->plan_settings.view());
@@ -1622,7 +1682,7 @@ struct EpisodeTable {
     if (grid) add(r.nn, sizeof(int32_t));
   }
 };
-static_assert(sizeof(hb_target) % 4 == 0 && sizeof(OdomCamera) % 4 == 0, "snapshot segments are copied in 4-byte units");
+static_assert(sizeof(hb_target) % 4 == 0 && sizeof(OdomCamera) % 4 == 0 && sizeof(TeleopState) % 4 == 0, "snapshot segments are copied in 4-byte units");
 
 static EpisodeSegments episode_segments(const hb_ctx* ctx, int64_t* head) {
   const size_t N = ctx->cfg.horizon_N;
@@ -1636,6 +1696,7 @@ static EpisodeSegments episode_segments(const hb_ctx* ctx, int64_t* head) {
   e.add(ctx->goal_tg, sizeof(hb_target));
   e.add_solution(ctx->pol_mem ? rows_at(ctx->pol, 0, N, grid) : SolutionRows{}, N, grid);
   e.add(ctx->odom_cam, sizeof(OdomCamera));
+  if (ctx->teleop.n > 0) e.add(ctx->tele_state, sizeof(TeleopState));     // only with a teleop setting: other rows keep their size
   e.t.row_words = e.words;
   return e.t;
 }
@@ -2316,6 +2377,20 @@ int hb_goal_to_target(int B, const double* t, const double* x, const double* goa
   for (int i = 0; i < B; ++i) {
     memset(&out[i], 0, sizeof(hb_target));
     hbplan::goal_to_target(plan_consts(), t[i], x + (size_t)i * NX, goal + (size_t)i * 3, out[i]);
+  }
+  return HB_OK;
+}
+
+int hb_cmd_vel_to_target(int B, const double* t, double horizon, const double* x, const double* cmd_vel, hb_target* out) {
+  if (B < 0 || !t || !x || !cmd_vel || !out || !isfinite(horizon)) return HB_EINVAL;
+  for (int i = 0; i < B; ++i) {
+    if (!isfinite(t[i])) return HB_EINVAL;
+    for (int k = 6; k < 12; ++k) if (!isfinite(x[(size_t)i * NX + k])) return HB_EINVAL;
+    for (int k = 0; k < 4; ++k) if (!isfinite(cmd_vel[(size_t)i * 4 + k])) return HB_EINVAL;
+  }
+  for (int i = 0; i < B; ++i) {
+    memset(&out[i], 0, sizeof(hb_target));
+    hbplan::cmd_vel_to_target(plan_consts(), cmd_vel + (size_t)i * 4, t[i], x + (size_t)i * NX, horizon, out[i]);
   }
   return HB_OK;
 }

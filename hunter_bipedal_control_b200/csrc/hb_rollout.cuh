@@ -10,14 +10,31 @@
 
 namespace hb {
 
+// The publisher state of a teleoperated instance (teleoperation, hunter_b200.h; per-instance context state, zero when cleared): the
+// filtered command last (vx, vy, vz, yaw rate) and 1 + the index of the goal in force it last saw (0: none), so that a goal a message
+// replaced is not captured again
+struct TeleopState { double last[4]; int32_t goal_seen, pad; };
+// The captured-target source of an instance whose target a teleop message wrote: beyond every goal index, so the planner plans on it
+constexpr int32_t TELEOP_CAPTURED = HB_MAX_GOALS;
+
+// whether the joystick of record s sends a message on absolute tick a: inside a window, on its period from the window's start
+__device__ __forceinline__ bool teleop_message(const hb_teleop_setting& s, int a) {
+  for (int w = 0; w < s.n_window && w < HB_MAX_TELEOP_WINDOWS; ++w)
+    if (s.on_tick[w] <= a && a < s.off_tick[w] && (a - s.on_tick[w]) % s.period_ticks == 0) return true;
+  return false;
+}
+
 // Plan inputs of the MPC cycle at time t, with the defaults of api.make_plan_inputs: x0 = the centroidal restatement of the measured rbd,
 // cmd_vel of the last command segment that has started (the first one before that), prev_event = min(t, gait_start) - 0.5, IK joint
 // references. feet_pos is left zero: plan_prepare_kernel computes the feet from x0. With est (estimated episodes) x0[9] is the unwrapped
 // observation yaw (LeggedController.cpp:335-337).
 // Goals (hb_goal_schedule, hunter_b200.h) of the instances that have one: the goal in force at t is captured, target and index, when it differs
 // from the captured one (captured_idx -1: none); reset (an episode's tick 0) forgets the captured goal first. The planner reads them.
-__global__ void rollout_plan_inputs_kernel(int B, double t, double horizon, const hb_rollout_command* cmd, const double* rbd, const hb_estimation_state* est,
-                                           hb_plan_input* in, InstanceView<hb_goal_schedule> goals, int reset, hb_target* captured,
+// Teleoperated instances (a record in teleop; publisher state pub): the goal capture compares with the goal they last saw, then a message
+// due on tick a runs the publisher step and captures the cmd_vel target of last (source TELEOP_CAPTURED); they plan with cmd_vel = last.
+__global__ void rollout_plan_inputs_kernel(int B, int a, double t, double horizon, const hb_rollout_command* cmd, const double* rbd,
+                                           const hb_estimation_state* est, hb_plan_input* in, InstanceView<hb_goal_schedule> goals,
+                                           InstanceView<hb_teleop_setting> teleop, TeleopState* pub, int reset, hb_target* captured,
                                            int32_t* captured_idx, hbplan::PlanConsts pc) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
@@ -32,13 +49,39 @@ __global__ void rollout_plan_inputs_kernel(int B, double t, double horizon, cons
   if (est) p.x0[9] = est[inst].yaw_obs;
   for (int i = 0; i < 12; ++i) p.feet_pos[i] = 0.0;
   p.gait = c.gait; p.joint_ik = 1;
+  const hb_teleop_setting* tp = teleop.of(inst);
+  TeleopState* ts = tp ? pub + inst : nullptr;
+  if (ts && reset) {
+    for (int i = 0; i < 4; ++i) ts->last[i] = 0.0;
+    ts->goal_seen = 0;
+    captured_idx[inst] = -1;
+  }
   if (const hb_goal_schedule* sp = goals.of(inst)) {
     const hb_goal_schedule& s = *sp;
     int g = -1;
     for (int k = 0; k < s.n_goal; ++k) if (s.time[k] <= t) g = k;
-    const int had = reset ? -1 : captured_idx[inst];
-    if (g >= 0 && g != had) hbplan::goal_to_target(pc, t, p.x0, s.goal[g], captured[inst]);
-    captured_idx[inst] = g >= 0 ? g : had;
+    const int had = ts ? ts->goal_seen - 1 : reset ? -1 : captured_idx[inst];
+    if (g >= 0 && g != had) {
+      hbplan::goal_to_target(pc, t, p.x0, s.goal[g], captured[inst]);
+      if (ts) captured_idx[inst] = g;
+    }
+    if (ts) ts->goal_seen = (g >= 0 ? g : had) + 1;
+    else captured_idx[inst] = g >= 0 ? g : had;
+  }
+  if (ts) {
+    if (teleop_message(*tp, a)) {     // TargetTrajectoriesPublisher's cmdVelCallback
+      double* last = ts->last;
+      for (int k : {0, 1, 3}) {
+        const double lim = tp->change_limit[k == 3 ? 2 : k];
+        double d = p.cmd_vel[k] - last[k];
+        d = d > 0 ? fmin(d, lim) : fmax(d, -lim);
+        last[k] += d;
+      }
+      last[2] = 0.0;
+      hbplan::cmd_vel_to_target(pc, last, t, p.x0, horizon, captured[inst]);
+      captured_idx[inst] = TELEOP_CAPTURED;
+    }
+    for (int i = 0; i < 4; ++i) p.cmd_vel[i] = ts->last[i];
   }
 }
 

@@ -585,6 +585,45 @@ int hb_rollout_set_motor_bridge(hb_ctx* ctx, int B, const hb_motor_bridge* r);
 int hb_motor_bridge_encode(int B, const hb_motor_bridge* r, const double* command, double* out);
 int hb_motor_bridge_feedback(int B, const hb_motor_bridge* r, const double* q, const double* qd, double* q_out, double* qd_out);
 
+/* ---- teleoperation: each robot driven as the joystick drives the reference (joy_teleop.launch, TargetTrajectoriesPublisher) ----
+ * The operator's velocity command reaches the robot as /cmd_vel messages at the teleop rate while the deadman button is held, and the
+ * publisher limits the change per message and converts each message once into a target. Record i acts on instance i of both episode
+ * calls; instances at or beyond B run without it: the cmd_vel segment in force, and the cmd_vel target rebuilt on every MPC tick.
+ * Messages: instance i receives a message on absolute MPC tick a iff on_tick[w] <= a < off_tick[w] and (a - on_tick[w]) % period_ticks
+ * == 0 for some window w < n_window. An episode call returns -1 before any launch when a record's period_ticks or any on_tick[w] is not a
+ * multiple of its mpc_every, so messages fall on MPC ticks only.
+ * Publisher step (TargetTrajectoriesPublisher.h:97-131), on each message with cmd the cmd_vel segment in force at t: for k = vx, vy, yaw
+ * rate in that order, d = cmd[k] - last[k], d = d > 0 ? min(d, change_limit) : max(d, -change_limit), last[k] += d; last[vz] = 0; then the
+ * target is hb_cmd_vel_to_target(t, x0, last) with x0 the tick's plan-input state (the true state, or in estimated episodes the estimate
+ * with x0[9] = yaw_obs), as goal capture uses it.
+ * Planning: a teleoperated instance plans with cmd_vel = last (its swing planner's body velocity command, /cmd_vel_filtered) on its
+ * captured target. Before its first message last = 0 and it plans on the cmd_vel target of last, rebuilt each MPC tick (deviation: the
+ * reference's starting() target is the zero state). The latest message wins: the goal capture (goals, above) and the messages write one
+ * captured target; on one tick the goal is captured first and the message second; a goal a message has replaced is not captured again;
+ * outside the windows the last target stays in force, as when the operator lets go of the stick.
+ * last, the goal last seen, the captured target and its source are per-instance context state: they are cleared by an episode call with
+ * tick0 == 0 and by every hb_rollout_set_teleop call, the clearing call (B == 0) included, so a split episode continues exactly and no
+ * message's target outlives the setting. hb_rollout_set_goals with schedules forgets the captured target and the goal last seen, and keeps
+ * last: a teleoperated instance then captures the new goal in force as an instance without teleop does. Teleop adds no launch to an
+ * episode.
+ * Deviations: joy_node also publishes when an axis changes (coalesced to 50 ms), here messages come at the autorepeat rate only; the
+ * reference drops messages while its observation time is 0, here the controller has published from tick 0. */
+#define HB_MAX_TELEOP_WINDOWS 4
+typedef struct {                              /* the joystick and the target publisher of one robot                                   */
+  int32_t period_ticks;                       /* message period [ticks], >= 1 (50: autorepeat_rate 10 Hz at the 500 Hz tick)          */
+  int32_t n_window;                           /* 0..HB_MAX_TELEOP_WINDOWS; 0: no message ever (the instance keeps last = 0)           */
+  int32_t on_tick[HB_MAX_TELEOP_WINDOWS];     /* the deadman is held over absolute ticks [on_tick[w], off_tick[w]): on_tick >= 0,     */
+  int32_t off_tick[HB_MAX_TELEOP_WINDOWS];    /* on_tick < off_tick, and off_tick[w] <= on_tick[w + 1] (ascending, not overlapping)   */
+  double change_limit[3];                     /* per-message change of vx, vy [m/s] and yaw rate [rad/s], > 0; +inf: no limit         */
+} hb_teleop_setting;                          /* 64 B */
+#define HB_SETTING_TELEOP 12                  /* hb_teleop_setting for hb_rollout_set_teleop (hb_check_setting_records)                */
+/* host only: period_ticks 50, one window [0, INT32_MAX), change_limit (0.1, 0.05, 0.3) (changeLimit_, TargetTrajectoriesPublisher.h:97) */
+int hb_default_teleop_setting(hb_teleop_setting* s);
+/* Sets the teleoperation of the context's episodes (a per-robot episode setting, above) and clears every instance's publisher state and
+ * captured target (also with B == 0, once a setting has been made). -1 also for a period_ticks < 1, n_window outside 0..HB_MAX_TELEOP_WINDOWS, a window outside the rules above, or a
+ * change_limit that is not > 0 (NaN). */
+int hb_rollout_set_teleop(hb_ctx* ctx, int B, const hb_teleop_setting* s);
+
 /* ---- estimated episodes (hb_rollout_estimated_batch_dev): the controllers read the Kalman filter's estimate from synthesised, noisy
  * sensors instead of the plant's true state (LeggedController::updateStateEstimation, LeggedController.cpp:280-349) ---- */
 typedef struct {                 /* standard deviations of additive Gaussian sensor noise; 0 = that channel is exact and draws nothing */
@@ -985,16 +1024,18 @@ int hb_estimator_fuse_odometry_async(hb_ctx* ctx, int B, const hb_kf_params* par
  * (N+1) x 22 double; u_traj N x 22 double; on event-node contexts node_times (N+1) double; node modes (N+1) int32; on event-node contexts
  * n_intervals int32, each of these padded), the fallback's previous solution (38 double), the stance positions (12 double), the captured
  * goal index (int32, -1: none), the captured target (hb_target), the adopted policy (as the resident solution) and the camera state
- * ((HB_ODOM_MAX_DELAY + 1) x 3 double history, 3 double bias). A segment whose buffer the context never allocated (no goals set, no odometry
- * set, no policy adopted) saves as its cleared value: goal index -1, zeros elsewhere.
+ * ((HB_ODOM_MAX_DELAY + 1) x 3 double history, 3 double bias), and only on a context with a teleop setting the publisher state (4 double
+ * filtered command, int32 1 + the goal last seen, int32 padding; teleoperation, above), so that rows of a context without one keep their
+ * size. A segment whose buffer the context never allocated (no goals set, no odometry set, no policy adopted) saves as its cleared value:
+ * goal index -1 (the source of the captured target: a goal's index, HB_MAX_GOALS for a teleop message), zeros elsewhere.
  * hb_episode_save_async writes row i (device memory, B rows) from instance src[i] of the context (src NULL: instance i), flags from the
  * context's bookkeeping. Asynchronous on the context's stream: src (host) is consumed when the call returns.
  * hb_episode_restore sets instance i of the context from row src[i] of the n_rows rows (src NULL: row i). It reads the rows' headers back
  * with one small synchronous copy before anything changes, and returns when the rows are written: a setting-like call, not a per-tick one.
  * After it, instances [0, B) hold the rows' solution, fallback solution and adopted policy as their flags say, so that a warm episode call
  * (tick0 > 0) passes its entry checks exactly when the rows would have passed them in the context that saved them. A restore writes the
- * goal and camera state whether or not goals or odometry are set, allocating their buffers as their setting calls do; hb_rollout_set_goals
- * and hb_rollout_set_odometry clear that state, so a restore must come after them.
+ * goal and camera state whether or not goals or odometry are set, allocating their buffers as their setting calls do; hb_rollout_set_goals,
+ * hb_rollout_set_odometry and hb_rollout_set_teleop clear that state, so a restore must come after them.
  * Return codes: -1 for a null context, B < 0, NULL rows with B > 0, a src entry outside [0, max_batch) (save) or [0, n_rows) (restore), a
  * B > n_rows restore with src NULL, and on restore a row whose fingerprint (horizon_N, event_nodes, size) differs from this context's, a row
  * without HB_EPISODE_HAS_SOLUTION, or fallback flags that would leave instances with a previous WBC solution that are not a prefix
@@ -1040,6 +1081,11 @@ int hb_plan_references_settings(int B, const hb_plan_input* in, const hb_target*
  * reference: the goal yaw is absolute in the unwrapped convention of x[9]. T == 0 gives the single sample 1 at time t (n = 1) where the
  * reference would publish two samples at the same time. -1 for a NULL pointer, B < 0 or a non-finite t, x[6:10] or goal. */
 int hb_goal_to_target(int B, const double* t, const double* x /*B x 22*/, const double* goal /*B x 3*/, hb_target* out);
+/* cmdVelToTargetTrajectories (TargetTrajectoriesPublisher.cpp:102-130) for the observation (t[i], x[i]) and cmd_vel[i] = (vx, vy, vz, yaw
+ * rate), host only: the two-sample target the planner builds from cmd_vel with time_to_target = horizon (hb_plan_references with joint_ik
+ * = 0 carries it bit for bit), the unused samples zero. The teleop messages' target (teleoperation, above). -1 for a NULL pointer, B < 0, a
+ * non-finite t, horizon, x[6:12] or cmd_vel. */
+int hb_cmd_vel_to_target(int B, const double* t, double horizon, const double* x /*B x 22*/, const double* cmd_vel /*B x 4*/, hb_target* out);
 /* Host threads used by hb_plan_references (process-wide); 0 = hardware_concurrency. The result does not depend on the count. */
 int hb_plan_set_threads(int n_threads);
 /* speed-based gait selection (calculateVelAbs + walkGait / trotGait, src/SwitchedModelReferenceManager.cpp:185-249): updates the

@@ -1,6 +1,6 @@
 """The closed-loop episode harness of the tools that run batched episodes: bench_rollout.py, record_episodes.py, latency_sweep.py and the
 sweeps push_sweep.py, plant_sweep.py, terrain_sweep.py, goal_sweep.py, odometry_sweep.py, gain_sweep.py, hardware_sweep.py,
-gait_sweep.py and bridge_sweep.py. It holds their shared command line, the workload (bench.py's configs[1] start poses trotting at 0.3 m/s on ground at
+gait_sweep.py, bridge_sweep.py and teleop_sweep.py. It holds their shared command line, the workload (bench.py's configs[1] start poses trotting at 0.3 m/s on ground at
 GROUND, failure below MIN_HEIGHT), one timed episode call, the robot -> cell assignment of the sweeps and their per-cell tally, the timed
 alternation of a per-robot setting, its null setting and no setting, the timing of a grid in one call against one call per cell, and the
 fields and sentences the tools' JSON lines share."""
