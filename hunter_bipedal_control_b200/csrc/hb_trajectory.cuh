@@ -137,7 +137,8 @@ __global__ void policy_adopt_kernel(int B, int N, InstanceView<int32_t> lat, lon
 }
 
 // MPC_MRT_Interface::evaluatePolicy with the feed-forward policy (LeggedController.cpp:154-156, task.info:93): linear interpolation of
-// the state / input trajectories of s at t0 + t_rel (s.t0 read only with t_abs); mode = mode in force at that time. choice: see PolicyChoice.
+// the state / input trajectories of s at t0 + t_rel (s.t0 read only with t_abs); mode = the node mode of the interval holding that time
+// (the interval ending there at a node where the mode changes). choice: see PolicyChoice.
 __global__ void policy_eval_kernel(int B, int N, double dt, double t_rel, SolutionRows s, double* x_des, double* u_des, int32_t* mode_out,
                                    const double* t_abs, PolicyChoice choice) {
   const int inst = blockIdx.x * blockDim.x / 32 + (threadIdx.x >> 5);
@@ -162,7 +163,12 @@ __global__ void policy_eval_kernel(int B, int N, double dt, double t_rel, Soluti
     const int k1 = (k + 1 < na) ? k + 1 : na - 1;   // the input trajectory repeats its last sample at the final node
     u_des[(size_t)inst * NU + lane] = (1.0 - al) * u[k * NU + lane] + al * u[k1 * NU + lane];
   }
-  if (lane == 0 && mode_out) mode_out[inst] = s.mode[(size_t)inst * (N + 1) + k];
+  // mode in force at t: ModeSchedule::modeAtTime finds a switch at t by lower_bound, so the earlier mode holds AT a switching time; a node
+  // whose mode differs from its predecessor's starts a new mode, and exactly at that node the interval ending there still holds
+  if (lane == 0 && mode_out) {
+    const int32_t* md = s.mode + (size_t)inst * (N + 1);
+    mode_out[inst] = (al == 0.0 && k > 0 && md[k] != md[k - 1]) ? md[k - 1] : md[k];
+  }
 }
 
 // store the solve time (and, with tk_new, the node grid) of a cold-started resident solution res

@@ -202,7 +202,9 @@ def test_warm_cycle_and_policy_at_long_horizons(N, contexts, oracle):
             xe = (1 - al[i]) * xres[i, k[i]] + al[i] * xres[i, k[i] + 1]
             ue = (1 - al[i]) * ures[i, k[i]] + al[i] * ures[i, min(k[i] + 1, N - 1)]
             assert _rel(xd[i], xe) < 1e-13 and _rel(ud[i], ue) < 1e-13, (off, i)
-            assert mode[i] == md[i, k[i]], (off, i)
+            # on a node where the mode changes the interval ending there holds (modeAtTime's earlier mode at a switch)
+            ki = k[i] - 1 if al[i] == 0.0 and k[i] > 0 and md[i, k[i]] != md[i, k[i] - 1] else k[i]
+            assert mode[i] == md[i, ki], (off, i)
     # beyond the horizon: the last state node and the last input sample, exactly
     assert np.array_equal(xd, xres[:, N]) and np.array_equal(ud, ures[:, N - 1])
 
