@@ -57,6 +57,7 @@ EXPORTED_SYMBOLS = [
     "hb_default_hardware_setting", "hb_rollout_set_hardware", "hb_actuation_hw", "hb_sim_read_sensors_hw",
     "hb_default_motor_bridge", "hb_rollout_set_motor_bridge", "hb_motor_bridge_encode", "hb_motor_bridge_feedback", "hb_actuation_bridge",
     "hb_sim_step_bridge", "hb_sim_read_sensors_bridge",
+    "hb_default_link_variation", "hb_rollout_set_link_variations", "hb_sim_step_links",
     "hb_default_teleop_setting", "hb_rollout_set_teleop", "hb_cmd_vel_to_target",
     "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
     "hb_check_setting_records", "hb_rollout_set_channel",
@@ -449,6 +450,37 @@ def make_plant_variations(B, payload_mass=0.0, payload_com=(0.0, 0.0, 0.0), payl
     v["payload_mass"] = m; v["payload_com"] = c; v["payload_inertia"] = I.reshape(B, 9)
     v["friction_scale"] = fs; v["stiffness_scale"] = ks; v["damping_scale"] = ds; v["motor_strength"] = ms
     return _check_records(HB_SETTING_PLANT_VARIATIONS, out, "plant_variations")
+
+
+NBODY = 11             # the model's bodies: 0 base (+imu), 1-5 leg_l1..l5, 6-10 leg_r1..r5 (l5, r5 with their toe and heel)
+
+
+class HbLinkVariation(C.Structure):
+    SETTING_KIND = 13        # HB_SETTING_LINK_VARIATIONS, the record's kind for hb_check_setting_records
+    _fields_ = [("mass_scale", C.c_double * NBODY), ("com_shift", (C.c_double * 3) * NBODY), ("inertia_scale", C.c_double * NBODY)]
+
+
+def default_link_variation():
+    """hb_default_link_variation: the nominal bodies (every scale 1, every shift 0)."""
+    r = HbLinkVariation()
+    _check(load_library().hb_default_link_variation(C.byref(r)), "hb_default_link_variation")
+    return r
+
+
+def make_link_variations(B, mass_scale=1.0, com_shift=0.0, inertia_scale=1.0):
+    """ctypes array of B HbLinkVariation (Context.set_link_variations, Context.sim_step): body b of robot i has mass mass_scale[i, b] m_b,
+    CoM c_b + com_shift[i, b] (body frame [m]) and inertia inertia_scale[i, b] I_b about it. Scalars and arrays broadcast over robot x body:
+    the scales (), (11,) or (B, 11) (per robot only: (B, 1)), com_shift (), (3,), (11, 3) or (B, 11, 3). Raises ValueError for a shape that
+    does not broadcast and for a record hb_rollout_set_link_variations rejects (its own check). The defaults give the nominal bodies."""
+    try:
+        ms = np.broadcast_to(_f64(mass_scale), (B, NBODY)); cs = np.broadcast_to(_f64(com_shift), (B, NBODY, 3))
+        js = np.broadcast_to(_f64(inertia_scale), (B, NBODY))
+    except ValueError as e:
+        raise ValueError("link variations: mass_scale / inertia_scale (B, 11), com_shift (B, 11, 3) expected: %s" % e)
+    out = (HbLinkVariation * B)()
+    v = np.ctypeslib.as_array(out)
+    v["mass_scale"] = ms; v["com_shift"] = cs; v["inertia_scale"] = js
+    return _check_records(HbLinkVariation.SETTING_KIND, out, "link_variations")
 
 
 HB_TERRAIN_MAX = 64
@@ -1286,13 +1318,14 @@ class Context:
                                              _ptr(mcmd)), "hb_actuation_bridge", self._h)
         return tau if bridge is None else mcmd
 
-    def sim_step(self, rbd, tau, params=None, wrench=None, variation=None, terrain=None, bridge=None, limits=None):
+    def sim_step(self, rbd, tau, params=None, wrench=None, variation=None, terrain=None, bridge=None, limits=None, links=None):
         """One control period of the batched rigid-body plant: returns (rbd_next [B,32], contact_force [B,12], contact_flag [B,4]).
         wrench [B,6]: an external world force at the base origin, then a world couple, held over the period. variation: B HbPlantVariation
         (make_plant_variations), the plant of each robot. terrain: B HbTerrain (make_terrains), the ground under each robot. bridge: B
         HbMotorBridge (make_motor_bridges): tau is then the decoded motor commands [B,10,5] of actuation(bridge=...), whose motor PD runs on
-        every substep, clipped to limits ([10] or [B,10]), and the mean clipped torque [B,10] is returned fourth. Every step is
-        hb_sim_step_bridge; without any of the four it is the plain plant step of hb_sim_step_batch."""
+        every substep, clipped to limits ([10] or [B,10]), and the mean clipped torque [B,10] is returned fourth. links: B
+        HbLinkVariation (make_link_variations), the bodies of each robot. Every step is hb_sim_step_links; without any of the five it is the
+        plain plant step of hb_sim_step_batch."""
         rbd = _f64(rbd).copy(); tau = _f64(tau); B = rbd.shape[0]
         params = params or default_sim_params()
         cf = np.zeros((B, 12)); fl = np.zeros((B, 4), dtype=np.uint8)
@@ -1301,14 +1334,16 @@ class Context:
             raise ValueError("sim_step: %d plant variations for %d robots" % (len(variation), B))
         if terrain is not None and len(terrain) != B:
             raise ValueError("sim_step: %d terrains for %d robots" % (len(terrain), B))
+        if links is not None and len(links) != B:
+            raise ValueError("sim_step: %d link variations for %d robots" % (len(links), B))
         bridge = _bridge_records(bridge, B, "sim_step")
         mcmd, lim, applied = None, None, None
         if bridge is not None:
             mcmd, tau = tau.reshape(B, NJ, 5), None
             lim = _f64(np.broadcast_to(_f64(limits), (B, NJ)))
             applied = np.zeros((B, NJ))
-        _check(self._lib.hb_sim_step_bridge(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), variation, terrain, bridge, _ptr(mcmd), _ptr(lim),
-                                            _ptr(applied), _ptr(cf), _ptr(fl)), "hb_sim_step_bridge", self._h)
+        _check(self._lib.hb_sim_step_links(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), variation, terrain, bridge, _ptr(mcmd), _ptr(lim),
+                                           _ptr(applied), links, _ptr(cf), _ptr(fl)), "hb_sim_step_links", self._h)
         return (rbd, cf, fl) if bridge is None else (rbd, cf, fl, applied)
 
     def _set_instances(self, symbol, items):
@@ -1327,6 +1362,12 @@ class Context:
         of instance i of every later rollout / rollout_estimated call, instances beyond len(variations) run the nominal plant; None clears
         them."""
         self._set_instances("hb_rollout_set_plant_variations", variations)
+
+    def set_link_variations(self, variations):
+        """Link variations of this context's episodes (hb_rollout_set_link_variations): variations[i] (make_link_variations) is the
+        masses, CoMs and inertias of the bodies of instance i's plant in every later rollout / rollout_estimated call; instances beyond
+        len(variations) run the nominal bodies; None clears them. The controllers are not told about it, and no other call reads it."""
+        self._set_instances("hb_rollout_set_link_variations", variations)
 
     def set_pushes(self, schedules):
         """Push schedules of this context's episodes (hb_rollout_set_pushes): schedules[i] (make_push_schedules) acts on instance i of every

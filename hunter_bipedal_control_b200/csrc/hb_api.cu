@@ -111,6 +111,8 @@ struct hb_ctx {
   InstanceSetting<hb_hardware_setting> hardware;
   // each instance's joint path through the real robot's motor driver in the episodes (hb_rollout_set_motor_bridge)
   InstanceSetting<hb_motor_bridge> bridges;
+  // each instance's own bodies in the episodes' plant (hb_rollout_set_link_variations)
+  InstanceSetting<hb_link_variation> links;
   // each instance's joystick and target publisher in the episodes (hb_rollout_set_teleop), and the publishers' state, allocated at
   // max_batch by the first call that sets records
   InstanceSetting<hb_teleop_setting> teleop;
@@ -507,7 +509,7 @@ int hb_destroy(hb_ctx* ctx) {
   void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->tele_mem, ctx->snap_mem, ctx->arena,
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
                        ctx->odometry.dev, ctx->controllers.dev, ctx->hardware.dev, ctx->plan_settings.dev,
-                       ctx->bridges.dev};
+                       ctx->bridges.dev, ctx->links.dev};
   for (void* p : mem) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -1160,14 +1162,14 @@ int hb_actuation_batch_dev(hb_ctx* ctx, int B, double delay, const double* time,
 // the plant step after the entry checks; wrench (B x 6) nullable; var: the plants of the instances, ter: the ground under them, drive: the
 // motors of the bridged ones
 static int sim_step(hb_ctx* ctx, int B, const hb_sim_params& params, double* rbd, const double* tau, const double* wrench,
-                    InstanceView<hb_plant_variation> var, InstanceView<hb_terrain> ter, const MotorDrive& drive, double* contact_force,
-                    uint8_t* contact_flag) {
-  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, params, rbd, tau, wrench, var, ter, drive, contact_force, contact_flag);
+                    InstanceView<hb_plant_variation> var, InstanceView<hb_terrain> ter, const MotorDrive& drive, InstanceView<hb_link_variation> links,
+                    double* contact_force, uint8_t* contact_flag) {
+  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, params, rbd, tau, wrench, var, ter, drive, links, contact_force, contact_flag);
 }
 
 int hb_sim_step_batch_dev(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {
   ENTER(ctx, B, params && rbd && tau && sim_params_ok(*params), UNCAPPED);
-  return sim_step(ctx, B, *params, rbd, tau, nullptr, {}, {}, MotorDrive{}, contact_force, contact_flag);
+  return sim_step(ctx, B, *params, rbd, tau, nullptr, {}, {}, MotorDrive{}, {}, contact_force, contact_flag);
 }
 
 int hb_default_plant_variation(hb_plant_variation* v) {
@@ -1223,6 +1225,26 @@ int hb_rollout_set_plant_variations(hb_ctx* ctx, int B, const hb_plant_variation
   return set_instances(ctx, B, v, plant_variation_ok, &hb_ctx::variations);
 }
 int hb_rollout_set_terrains(hb_ctx* ctx, int B, const hb_terrain* t) { return set_instances(ctx, B, t, terrain_ok, &hb_ctx::terrains); }
+
+int hb_default_link_variation(hb_link_variation* r) {
+  if (!r) return HB_EINVAL;
+  memset(r, 0, sizeof(*r));
+  for (int b = 0; b < NBODY; ++b) { r->mass_scale[b] = 1.0; r->inertia_scale[b] = 1.0; }
+  return HB_OK;
+}
+
+// The ranges of hunter_b200.h's hb_link_variation: every value finite, the scales > 0
+static bool link_variation_ok(const hb_link_variation& r) {
+  for (int b = 0; b < NBODY; ++b) {
+    if (!isfinite(r.mass_scale[b]) || !(r.mass_scale[b] > 0.0) || !isfinite(r.inertia_scale[b]) || !(r.inertia_scale[b] > 0.0)) return false;
+    for (int i = 0; i < 3; ++i) if (!isfinite(r.com_shift[b][i])) return false;
+  }
+  return true;
+}
+
+int hb_rollout_set_link_variations(hb_ctx* ctx, int B, const hb_link_variation* r) {
+  return set_instances(ctx, B, r, link_variation_ok, &hb_ctx::links);
+}
 
 // The ranges of hunter_b200.h's hb_goal_schedule: the count, finite times in ascending order, finite goals
 static bool goal_schedule_ok(const hb_goal_schedule& s) {
@@ -1384,6 +1406,7 @@ int hb_check_setting_records(int32_t kind, int B, const void* records, int32_t* 
     case HB_SETTING_LATENCIES: return check_records(B, records, latency_ok, first_bad);
     case HB_SETTING_MOTOR_BRIDGE: return check_records(B, records, motor_bridge_ok, first_bad);
     case HB_SETTING_TELEOP: return check_records(B, records, teleop_setting_ok, first_bad);
+    case HB_SETTING_LINK_VARIATIONS: return check_records(B, records, link_variation_ok, first_bad);
     default: return HB_EINVAL;
   }
 }
@@ -1631,7 +1654,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
                                     ctx->ro_jtau, controllers);
     if (!rc) rc = actuation_dev(ctx, B, p->actuation_delay, hardware, bridges, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau, ctx->ro_mcmd);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, hardware, ctx->ro_tau);
-    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, ctx->variations.view(), ctx->terrains.view(), drive,
+    if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, ctx->variations.view(), ctx->terrains.view(), drive, ctx->links.view(),
                            record && contacts ? ctx->ro_cforce : nullptr, record && contacts ? ctx->ro_cflag : nullptr);
     if (!rc && record) {
       for (int j = 0; j < rec.n; ++j)
@@ -2236,23 +2259,30 @@ int hb_sim_step_terrain(hb_ctx* ctx, int B, const hb_sim_params* params, double*
   return hb_sim_step_bridge(ctx, B, params, rbd, tau, wrench, v, ter, nullptr, nullptr, nullptr, nullptr, contact_force, contact_flag);
 }
 
-// the one host-pointer plant step: the four above are it with null bridges, terrains, variations and wrench
 int hb_sim_step_bridge(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* v,
                        const hb_terrain* ter, const hb_motor_bridge* bridge, const double* motor_cmd, const double* limits, double* applied,
                        double* contact_force, uint8_t* contact_flag) {
+  return hb_sim_step_links(ctx, B, params, rbd, tau, wrench, v, ter, bridge, motor_cmd, limits, applied, nullptr, contact_force, contact_flag);
+}
+
+// the one host-pointer plant step: the five above are it with null link variations, bridges, terrains, variations and wrench
+int hb_sim_step_links(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* v,
+                      const hb_terrain* ter, const hb_motor_bridge* bridge, const double* motor_cmd, const double* limits, double* applied,
+                      const hb_link_variation* links, double* contact_force, uint8_t* contact_flag) {
   ENTER(ctx, B, params && rbd && (bridge ? motor_cmd && limits : tau != nullptr), CAPPED, [&] {
     if (bridge) for (size_t k = 0; k < (size_t)B * NJ; ++k) if (!(limits[k] > 0.0)) return false;
-    return sim_params_ok(*params) && all_ok(B, v, plant_variation_ok) && all_ok(B, ter, terrain_ok) && all_ok(B, bridge, motor_bridge_ok);
+    return sim_params_ok(*params) && all_ok(B, v, plant_variation_ok) && all_ok(B, ter, terrain_ok) && all_ok(B, bridge, motor_bridge_ok) &&
+           all_ok(B, links, link_variation_ok);
   });
   const bool br = bridge != nullptr;
   Staging s(ctx, B);
   auto r = s.inout(rbd, 32); auto t = s.in_or_null(br ? nullptr : tau, NJ); auto w = s.in_or_null(wrench, 6); auto pv = s.in_or_null(v, 1);
   auto pt = s.in_or_null(ter, 1); auto mb = s.in_or_null(bridge, 1); auto mc = s.in_or_null(br ? motor_cmd : nullptr, NJ * 5);
-  auto lim = s.in_or_null(br ? limits : nullptr, NJ); auto ap = s.out(br ? applied : nullptr, NJ);
+  auto lim = s.in_or_null(br ? limits : nullptr, NJ); auto ap = s.out(br ? applied : nullptr, NJ); auto lk = s.in_or_null(links, 1);
   auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
   return s.run(1, [&](Chunk) {
     const MotorDrive drive{{mb, B}, mc, lim, {}, {}, br ? (double*)ap : nullptr};
-    return sim_step(ctx, B, *params, r, t, w, {pv, B}, {pt, B}, drive, cf, fl);
+    return sim_step(ctx, B, *params, r, t, w, {pv, B}, {pt, B}, drive, {lk, B}, cf, fl);
   });
 }
 

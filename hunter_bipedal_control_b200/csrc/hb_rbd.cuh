@@ -422,14 +422,31 @@ __device__ __forceinline__ void rigid_body_wrench(const double* R, const double*
   for (int i = 0; i < 3; ++i) n[i] = N[i] + rxF[i];
 }
 
-// Recursive Newton-Euler in the coordinates above: tau = M(q) a + C(q,v) v + g(q)   (float64, per lane).
+// The inertial parameters rnea_pass reads for body b: its mass, its CoM and its inertia about the CoM (body frame, row-major).
+// NominalBodies reads the model; LinkBodies reads a table of 13 doubles per body, [m, c(3), I(9)] (a varied robot's bodies, sim_step_kernel).
+struct NominalBodies {
+  __device__ __forceinline__ double mass(int b) const { return c_model.mass[b]; }
+  __device__ __forceinline__ const double* com(int b) const { return &c_model.com[3 * b]; }
+  __device__ __forceinline__ const double* inertia(int b) const { return &c_model.inertia[9 * b]; }
+};
+constexpr int LINK_BODY = 13;
+struct LinkBodies {
+  const double* t;
+  __device__ __forceinline__ double mass(int b) const { return t[LINK_BODY * b]; }
+  __device__ __forceinline__ const double* com(int b) const { return t + LINK_BODY * b + 1; }
+  __device__ __forceinline__ const double* inertia(int b) const { return t + LINK_BODY * b + 4; }
+};
+
+// Recursive Newton-Euler in the coordinates above: tau = M(q) a + C(q,v) v + g(q)   (float64, per lane), with the bodies' inertial
+// parameters from `bodies` (the model's by default; the kinematics are always the model's).
 // Also returns the classical acceleration of the four contact points (= J_c a + dJ_c/dt v).
-__device__ void rnea_pass(const double* q, const double* v, const double* a, bool gravity, double* tau, double* cacc) {
+template <class Bodies = NominalBodies>
+__device__ void rnea_pass(const double* q, const double* v, const double* a, bool gravity, double* tau, double* cacc, Bodies bodies = Bodies()) {
   const Model& md = c_model;
   double R0[9], ax0[9], w0[3], wd0[3], pd0[3];
   rnea_base_motion(q, v, a, R0, ax0, w0, wd0, pd0);
   auto body_wrench = [&](int b, const double* R, const double* w, const double* wd, const double* pd, double* F, double* n) {
-    rigid_body_wrench(R, w, wd, pd, md.mass[b], &md.com[3 * b], &md.inertia[9 * b], gravity, F, n);
+    rigid_body_wrench(R, w, wd, pd, bodies.mass(b), bodies.com(b), bodies.inertia(b), gravity, F, n);
   };
   double f0[3], n0[3];
   body_wrench(0, R0, w0, wd0, pd0, f0, n0);

@@ -584,8 +584,28 @@ __global__ void actuation_kernel(int B, double delay_all, InstanceView<hb_hardwa
 // the base origin and a world couple, which enter as the generalised forces Q_p = f, Q_zyx = T' tau with omega_world = T(zyx) zyx_dot
 // (world_omega_from_zyx_rates, hb_rbd.cuh); null adds nothing. var: the plants of the instances that have one (varied plants,
 // hunter_b200.h); the others run the nominal plant. terrain: the ground under the instances that have one (terrain, hunter_b200.h); the
-// others stand on flat ground at prm.ground_height.
-struct SimShared { double q[NQ], v[NQ], J[12 * NQ], M[NQ * 17], nle[NQ], rhs[NQ], t1[NQ], t2[NQ], kdi[NQ], F[12], cpos[12], cvel[12]; };
+// others stand on flat ground at prm.ground_height. links: the bodies of the instances that have them (link variations, hunter_b200.h),
+// formed once per call into `body` (LinkBodies' table); the others read the model's.
+struct SimShared {
+  double q[NQ], v[NQ], J[12 * NQ], M[NQ * 17], nle[NQ], rhs[NQ], t1[NQ], t2[NQ], kdi[NQ], F[12], cpos[12], cvel[12], body[NBODY * LINK_BODY];
+};
+
+// Body b of a link variation l as LinkBodies reads it (out: 13 doubles): m' = s_m m, c' = c + shift, I' = s_I I, each one rounded operation.
+// Returns whether the body equals the model's.
+__device__ __forceinline__ bool link_body(const hb_link_variation& l, int b, double* out) {
+  const Model& md = c_model;
+  out[0] = __dmul_rn(l.mass_scale[b], md.mass[b]);
+  bool same = out[0] == md.mass[b];
+  for (int i = 0; i < 3; ++i) { out[1 + i] = __dadd_rn(md.com[3 * b + i], l.com_shift[b][i]); same &= out[1 + i] == md.com[3 * b + i]; }
+  for (int i = 0; i < 9; ++i) { out[4 + i] = __dmul_rn(l.inertia_scale[b], md.inertia[9 * b + i]); same &= out[4 + i] == md.inertia[9 * b + i]; }
+  return same;
+}
+
+// One RNEA lane of a varied robot on the body table t (LinkBodies). Not inlined, as payload_rnea: the nominal lanes keep their code. Its
+// roundings can differ from the inlined nominal pass's, so a robot whose bodies all equal the model's runs the nominal pass.
+__device__ __noinline__ void link_rnea(const double* q, const double* v, const double* a, bool gravity, const double* t, double* tau) {
+  rnea_pass(q, v, a, gravity, tau, nullptr, LinkBodies{t});
+}
 
 // The payload of a varied plant in one RNEA lane: rnea_pass's base-body wrench for a rigid body fixed to the base with mass m, CoM c and
 // inertia I (base frame), added to the base rows of tau (the joint rows get nothing from a body on the base). Not inlined: inlined after
@@ -648,16 +668,19 @@ __device__ __noinline__ double bridge_motor_torque(const MotorDrive& d, const hb
 __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, double* rbd_io, const double* tau, const double* wrench,
                                                       const __grid_constant__ InstanceView<hb_plant_variation> var,
                                                       const __grid_constant__ InstanceView<hb_terrain> terrain, const __grid_constant__ MotorDrive drive,
-                                                      double* contact_force, uint8_t* contact_flag) {
+                                                      const __grid_constant__ InstanceView<hb_link_variation> links, double* contact_force,
+                                                      uint8_t* contact_flag) {
   __shared__ SimShared sh;
   const int inst = blockIdx.x, lane = threadIdx.x;
   const hb_plant_variation* pv = var.of(inst);      // null: the nominal plant
   const hb_terrain* ter = terrain.of(inst);         // null: flat ground at prm.ground_height
   const hb_motor_bridge* mb = drive.rec.of(inst);   // null: the joints receive tau
+  const hb_link_variation* lv = links.of(inst);     // null: the model's bodies (also for a record whose bodies equal the model's)
   bool touch = false;                    // lanes 0-3: the normal force of their contact in the last substep is positive
   double applied = 0.0;                  // lanes 6-15 of a bridged instance: the sum over the substeps of the motor's clipped torque
   double* r = rbd_io + (size_t)inst * 32;
   if (lane == 0) rbd_to_qv(r, sh.q, sh.v);
+  if (lv && !__any_sync(HB_FULL_MASK, lane < NBODY && !link_body(*lv, lane, &sh.body[LINK_BODY * lane]))) lv = nullptr;
   __syncwarp();
   const double h = prm.dt / (prm.substeps > 0 ? prm.substeps : 1);
   for (int sub = 0; sub < (prm.substeps > 0 ? prm.substeps : 1); ++sub) {
@@ -698,7 +721,8 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
     if (lane < 17) {
       double q[NQ], v[NQ], a[NQ], tq[NQ];
       for (int i = 0; i < NQ; ++i) { q[i] = sh.q[i]; v[i] = lane == 16 ? sh.v[i] : 0.0; a[i] = (i == lane) ? 1.0 : 0.0; }
-      rnea_pass(q, v, a, lane == 16, tq, nullptr);
+      if (lv) link_rnea(q, v, a, lane == 16, sh.body, tq);
+      else rnea_pass(q, v, a, lane == 16, tq, nullptr);
       if (pv && (lane < 6 || lane == 16) && pv->payload_mass > 0.0)
         payload_rnea(q, v, a, lane == 16, pv->payload_mass, pv->payload_com, pv->payload_inertia, tq);
       if (lane < 16) { for (int rr = 0; rr < NQ; ++rr) sh.M[rr * 17 + lane] = tq[rr]; }

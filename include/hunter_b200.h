@@ -372,6 +372,31 @@ int hb_default_plant_variation(hb_plant_variation* v);      /* host only: no pay
  * zero mass with a nonzero CoM or inertia. */
 int hb_rollout_set_plant_variations(hb_ctx* ctx, int B, const hb_plant_variation* v);
 
+/* ---- link variations: each robot's own bodies in the episodes (link masses, centres of mass and inertias) ----
+ * Like a plant variation, the setting acts on the simulated plant only; the planner, MPC, WBC, joint command law, actuation model and
+ * estimator keep the nominal model and are not told about it. Record i acts on instance i of both episode calls; instances at or beyond B
+ * run the nominal bodies bit for bit. The bodies are those of the model (HB_NBODY = 11): 0 is the base with the imu merged in, 1-5 are
+ * leg_l1 .. leg_l5 and 6-10 leg_r1 .. leg_r5, l5 and r5 carrying their welded toe and heel bodies. With r the record of an instance and
+ * m_b, c_b, I_b the model's mass, CoM (body frame) and rotational inertia about the CoM (body frame) of body b, the plant's body b has
+ *   m' = mass_scale[b] m_b,   c' = c_b + com_shift[b],   I' = inertia_scale[b] I_b (every entry),
+ * each value formed once, as one rounded product or sum, so that scale 1 and shift 0 give the nominal value exactly. These values enter
+ * every rigid-body term of the plant's dynamics: the 16 columns of M(q) and nle(q, v). The kinematics (contact points, J_c), the armature,
+ * the joint damping, the contacts, the wrench path and a plant variation's payload (which adds on top) are unchanged.
+ * hb_default_link_variation's record (every scale 1, every shift 0) is the unvaried plant bit for bit, as is an instance with no record.
+ * The setting has no state of its own (hb_episode_state_bytes does not count it) and adds no launch to an episode: the plant kernel forms
+ * a varied instance's bodies once per step and reads the model's for the others, and for a record whose bodies all equal the model's. Every other entry point ignores it; hb_sim_step_links
+ * takes records explicitly. */
+typedef struct {                 /* the bodies of one robot, relative to the nominal model                                        */
+  double mass_scale[11];         /* m' = mass_scale[b] m_b, finite, > 0                                                            */
+  double com_shift[11][3];       /* c' = c_b + com_shift[b], body frame [m], finite                                                */
+  double inertia_scale[11];      /* I' = inertia_scale[b] I_b, finite, > 0                                                         */
+} hb_link_variation;             /* 440 B */
+#define HB_SETTING_LINK_VARIATIONS 13         /* hb_link_variation for hb_rollout_set_link_variations (hb_check_setting_records)     */
+int hb_default_link_variation(hb_link_variation* r);      /* host only: every scale 1, every shift 0 */
+/* Sets the link variations of the context's episodes (a per-robot episode setting, above). -1 also for a value that is not finite, a
+ * mass_scale <= 0 or an inertia_scale <= 0. */
+int hb_rollout_set_link_variations(hb_ctx* ctx, int B, const hb_link_variation* r);
+
 /* ---- terrain: the ground under each robot of the episodes, a height field on a regular world-frame grid ----
  * The terrain acts on the simulated plant and on the height failure check only; the planner, MPC, WBC, joint command law, actuation
  * model and estimator keep assuming flat ground at z = 0 and are not told about it (the estimator's feet_heights included).
@@ -954,6 +979,13 @@ int hb_sim_step_bridge(hb_ctx* ctx, int B, const hb_sim_params* params, double* 
                        const double* wrench /*nullable*/, const hb_plant_variation* v /*nullable*/, const hb_terrain* t /*nullable*/,
                        const hb_motor_bridge* bridge /*nullable*/, const double* motor_cmd, const double* limits, double* applied /*nullable*/,
                        double* contact_force /*nullable*/, uint8_t* contact_flag /*nullable*/);
+/* hb_sim_step_bridge on each robot's own bodies: links (B, nullable) = the bodies of every robot of the call (link variations, above),
+ * validated as by hb_rollout_set_link_variations (-1). This is the one host-pointer plant step; hb_sim_step_bridge is it with links =
+ * NULL. */
+int hb_sim_step_links(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau /*nullable with bridge*/,
+                      const double* wrench /*nullable*/, const hb_plant_variation* v /*nullable*/, const hb_terrain* t /*nullable*/,
+                      const hb_motor_bridge* bridge /*nullable*/, const double* motor_cmd, const double* limits, double* applied /*nullable*/,
+                      const hb_link_variation* links /*nullable*/, double* contact_force /*nullable*/, uint8_t* contact_flag /*nullable*/);
 /* hb_sim_read_sensors_hw, and with bridge, each robot's joint readings pass its encoders (steps (3) to (5) of the motor bridge, above)
  * after the offsets and the noise. hb_sim_read_sensors_hw is it with bridge = NULL. */
 int hb_sim_read_sensors_bridge(hb_ctx* ctx, int B, const hb_sensor_noise* noise, const hb_hardware_setting* hw /*nullable*/,
