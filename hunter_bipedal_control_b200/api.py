@@ -60,6 +60,7 @@ EXPORTED_SYMBOLS = [
     "hb_default_link_variation", "hb_rollout_set_link_variations", "hb_sim_step_links",
     "hb_default_teleop_setting", "hb_rollout_set_teleop", "hb_cmd_vel_to_target",
     "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
+    "hb_plan_set_maps", "hb_plan_references_maps", "hb_goal_to_target_maps", "hb_cmd_vel_to_target_maps",
     "hb_check_setting_records", "hb_rollout_set_channel",
     "hb_episode_state_bytes", "hb_episode_save_async", "hb_episode_restore",
 ]
@@ -115,24 +116,32 @@ def reference_target(ref):
     return make_targets([np.array(ref.target_times[:n])], [np.array([ref.target_states[k][:] for k in range(n)])])[0]
 
 
-def cmd_vel_to_target(t, horizon, x, cmd_vel):
+def _maps_of(maps, B, what):
+    """The height maps argument of a host planner call: None, or B HbTerrain (make_terrains)."""
+    if maps is not None and len(maps) != B:
+        raise ValueError("%s: %d height maps for %d instances" % (what, len(maps), B))
+    return maps
+
+
+def cmd_vel_to_target(t, horizon, x, cmd_vel, maps=None):
     """cmdVelToTargetTrajectories (hb_cmd_vel_to_target) for a batch: the two-sample target the planner builds from cmd_vel (vx, vy, vz, yaw
-    rate) at time t on the observation x with time_to_target = horizon. t (B,) or a scalar, x (B, 22), cmd_vel (B, 4) or (4,). Returns a
-    ctypes array of B HbTarget."""
+    rate) at time t on the observation x with time_to_target = horizon. t (B,) or a scalar, x (B, 22), cmd_vel (B, 4) or (4,). maps: B
+    HbTerrain (make_terrains), the height map of each instance (hb_cmd_vel_to_target_maps). Returns a ctypes array of B HbTarget."""
     x = _f64(x).reshape(-1, NX); B = x.shape[0]
     t = _f64(np.broadcast_to(_f64(t), (B,))); cmd = _f64(np.broadcast_to(_f64(cmd_vel), (B, 4)))
     out = (HbTarget * B)()
-    _check(load_library().hb_cmd_vel_to_target(B, _ptr(t), C.c_double(horizon), _ptr(x), _ptr(cmd), out), "hb_cmd_vel_to_target")
+    _check(load_library().hb_cmd_vel_to_target_maps(B, _ptr(t), C.c_double(horizon), _ptr(x), _ptr(cmd), _maps_of(maps, B, "cmd_vel_to_target"), out),
+           "hb_cmd_vel_to_target_maps")
     return out
 
 
-def goal_to_target(t, x, goal):
-    """goalToTargetTrajectories (hb_goal_to_target) for a batch: t (B,) or a scalar, x (B, 22), goal (B, 3) = (x, y, yaw) or (3,).
-    Returns a ctypes array of B HbTarget."""
+def goal_to_target(t, x, goal, maps=None):
+    """goalToTargetTrajectories (hb_goal_to_target) for a batch: t (B,) or a scalar, x (B, 22), goal (B, 3) = (x, y, yaw) or (3,). maps: B
+    HbTerrain (make_terrains), the height map of each instance (hb_goal_to_target_maps). Returns a ctypes array of B HbTarget."""
     x = _f64(x).reshape(-1, NX); B = x.shape[0]
     t = _f64(np.broadcast_to(_f64(t), (B,))); goal = _f64(np.broadcast_to(_f64(goal), (B, 3)))
     out = (HbTarget * B)()
-    _check(load_library().hb_goal_to_target(B, _ptr(t), _ptr(x), _ptr(goal), out), "hb_goal_to_target")
+    _check(load_library().hb_goal_to_target_maps(B, _ptr(t), _ptr(x), _ptr(goal), _maps_of(maps, B, "goal_to_target"), out), "hb_goal_to_target_maps")
     return out
 
 
@@ -484,6 +493,9 @@ def make_link_variations(B, mass_scale=1.0, com_shift=0.0, inertia_scale=1.0):
 
 
 HB_TERRAIN_MAX = 64
+
+
+HEIGHT_MAPS_SETTING_KIND = 14     # HB_SETTING_HEIGHT_MAPS: HbTerrain records as planner height maps (Context.set_height_maps), for hb_check_setting_records
 
 
 class HbTerrain(C.Structure):
@@ -898,11 +910,11 @@ def plan_set_threads(n):
 
 
 def plan_references(t0, horizon, x0, cmd_vel, feet_pos, gait, gait_start, prev_event=None, time_to_target=None, latest_stance=None, joint_ik=True,
-                    targets=None, settings=None):
+                    targets=None, settings=None, maps=None):
     """Host-side reference planner (hb_plan_references): returns (ctypes array of HbReference, latest_stance[B,12]). targets: B HbTarget
     (make_targets, goal_to_target) planned on instead of the cmd_vel targets (hb_plan_references_targets); cmd_vel still drives the swing
     planner. settings: B HbPlannerSettings (make_planner_settings) in place of the compiled-in templates and swing settings
-    (hb_plan_references_settings)."""
+    (hb_plan_references_settings). maps: B HbTerrain (make_terrains), the height map each instance plans on (hb_plan_references_maps)."""
     lib = load_library()
     ins = make_plan_inputs(t0, horizon, x0, cmd_vel, feet_pos, gait, gait_start, prev_event, time_to_target, joint_ik)
     B = len(ins)
@@ -912,7 +924,9 @@ def plan_references(t0, horizon, x0, cmd_vel, feet_pos, gait, gait_start, prev_e
         raise ValueError("plan_references: %d planner settings for %d instances" % (len(settings), B))
     ls = np.zeros((B, 12)) if latest_stance is None else _f64(latest_stance).copy()
     refs = (HbReference * B)()
-    if settings is None:
+    if maps is not None:
+        _check(lib.hb_plan_references_maps(B, ins, targets, settings, _maps_of(maps, B, "plan_references"), _ptr(ls), refs), "hb_plan_references_maps")
+    elif settings is None:
         _check(lib.hb_plan_references_targets(B, ins, targets, _ptr(ls), refs), "hb_plan_references_targets")
     else:
         _check(lib.hb_plan_references_settings(B, ins, targets, settings, _ptr(ls), refs), "hb_plan_references_settings")
@@ -1494,6 +1508,13 @@ class Context:
         settings of instance i in every device planner path -- plan_references_gpu, resident_plan_cycle, rollout and rollout_estimated --
         instances beyond len(settings) plan with the compiled-in ones; None clears them."""
         self._set_instances("hb_plan_set_settings", settings)
+
+    def set_height_maps(self, maps):
+        """Height maps of this context (hb_plan_set_maps): maps[i] (make_terrains) is the ground the planner of instance i is told about in
+        every device planner path -- plan_references_gpu, resident_plan_cycle, rollout and rollout_estimated, their goal and teleop targets
+        included -- measured from the flat ground the planner otherwise assumes (a terrain H under a plant at sim.ground_height g is the map
+        H - g); instances beyond len(maps) plan without one; None clears them."""
+        self._set_instances("hb_plan_set_maps", maps)
 
     def resident_wbc(self, t_now, rbd, stance_mode=None):
         """Policy of the resident solution at absolute time t_now + WeightedWbc: returns (x_des, u_des, mode, sol, torque, status)."""

@@ -120,6 +120,8 @@ struct hb_ctx {
   TeleopState* tele_state;
   // each instance's gait templates and swing settings in every device planner path (hb_plan_set_settings)
   InstanceSetting<hb_planner_settings> plan_settings;
+  // each instance's height map in every device planner path (hb_plan_set_maps)
+  InstanceSetting<hb_terrain> height_maps;
   // the recorded channels of the episodes (hb_rollout_set_channel): the caller's buffer, its instances and rows; B == 0: unset
   struct { void* buf; int B, rows; } channels[HB_CHANNELS];
   // the episode snapshots' staging (hb_episode_save_async / hb_episode_restore), allocated at max_batch by their first call: the rows'
@@ -509,7 +511,7 @@ int hb_destroy(hb_ctx* ctx) {
   void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->tele_mem, ctx->snap_mem, ctx->arena,
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
                        ctx->odometry.dev, ctx->controllers.dev, ctx->hardware.dev, ctx->plan_settings.dev,
-                       ctx->bridges.dev, ctx->links.dev};
+                       ctx->bridges.dev, ctx->links.dev, ctx->height_maps.dev};
   for (void* p : mem) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -803,17 +805,19 @@ static const hbplan::PlanConsts& plan_consts() {
 }
 
 // The device planner after the entry checks: an instance with a record in targets plans on it where captured is null or captured[i] >= 0;
-// an instance with a record in settings plans with it
+// an instance with a record in settings plans with it, and one with a record in maps on that height map
 static int plan_dev(hb_ctx* ctx, int B, const hb_plan_input* in, const double* feet, double* latest_stance, hb_reference* out, int32_t* status,
-                    InstanceView<hb_target> targets, const int32_t* captured, InstanceView<hb_planner_settings> settings) {
+                    InstanceView<hb_target> targets, const int32_t* captured, InstanceView<hb_planner_settings> settings,
+                    InstanceView<hb_terrain> maps) {
   return launch(ctx, K_UNPROFILED, plan_references_coop_kernel, (B + 7) / 8, 32, 0, B, in, feet, latest_stance, out, status, plan_consts(), targets,
-                captured, settings);
+                captured, settings, maps);
 }
 
 int hb_plan_references_batch_dev(hb_ctx* ctx, int B, const hb_plan_input* in, const double* feet, double* latest_stance, hb_reference* out,
                                  int32_t* status) {
   ENTER(ctx, B, in && latest_stance && out, UNCAPPED);
-  return plan_dev(ctx, B, in, feet, latest_stance, out, status, ctx->plan_targets.view(ctx->base), nullptr, ctx->plan_settings.view(ctx->base));
+  return plan_dev(ctx, B, in, feet, latest_stance, out, status, ctx->plan_targets.view(ctx->base), nullptr, ctx->plan_settings.view(ctx->base),
+                  ctx->height_maps.view(ctx->base));
 }
 
 int hb_default_kf_params(hb_kf_params* p) {
@@ -1295,6 +1299,8 @@ int hb_plan_set_settings(hb_ctx* ctx, int B, const hb_planner_settings* s) {
   return set_instances(ctx, B, s, planner_settings_ok, &hb_ctx::plan_settings);
 }
 
+int hb_plan_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps) { return set_instances(ctx, B, maps, terrain_ok, &hb_ctx::height_maps); }
+
 static bool latency_ok(const int32_t& d) { return d >= 0; }     // the upper bound is the episode's mpc_every, checked by the episode call
 
 int hb_rollout_set_mpc_latencies(hb_ctx* ctx, int B, const int32_t* ticks) { return set_instances(ctx, B, ticks, latency_ok, &hb_ctx::latencies); }
@@ -1407,6 +1413,7 @@ int hb_check_setting_records(int32_t kind, int B, const void* records, int32_t* 
     case HB_SETTING_MOTOR_BRIDGE: return check_records(B, records, motor_bridge_ok, first_bad);
     case HB_SETTING_TELEOP: return check_records(B, records, teleop_setting_ok, first_bad);
     case HB_SETTING_LINK_VARIATIONS: return check_records(B, records, link_variation_ok, first_bad);
+    case HB_SETTING_HEIGHT_MAPS: return check_records(B, records, terrain_ok, first_bad);
     default: return HB_EINVAL;
   }
 }
@@ -1635,10 +1642,11 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
     if (!rc && mpc) {
       if (first_cold) CK(cudaMemsetAsync(ctx->res_stance, 0, sizeof(double) * B * 12, ctx->stream));   // latestStanceposition_ starts at zero
       rc = launch(ctx, K_UNPROFILED, rollout_plan_inputs_kernel, grid, 64, 0, B, (int)a, t, horizon, ctx->ro_cmd, meas, e ? e->est : nullptr,
-                  ctx->ro_in, ctx->goals.view(), ctx->teleop.view(), ctx->tele_state, first_cold ? 1 : 0, ctx->goal_tg, ctx->goal_idx, plan_consts());
+                  ctx->ro_in, ctx->goals.view(), ctx->teleop.view(), ctx->tele_state, first_cold ? 1 : 0, ctx->goal_tg, ctx->goal_idx, plan_consts(),
+                  ctx->height_maps.view());
       if (!rc) rc = launch(ctx, K_UNPROFILED, plan_prepare_kernel, grid, 64, 0, B, ctx->ro_in, ctx->ro_t0, ctx->ro_x0, ctx->ro_feet);
       if (!rc) rc = plan_dev(ctx, B, ctx->ro_in, ctx->ro_feet, ctx->res_stance, ctx->ro_refs, ctx->ro_pstat, goal_targets, ctx->goal_idx,
-                             ctx->plan_settings.view());
+                             ctx->plan_settings.view(), ctx->height_maps.view());
       if (!rc) rc = resident_cycle_impl(ctx, B, first_cold, 0.0, ctx->ro_t0, ctx->ro_x0, ctx->ro_refs, meas, ctx->ro_info, nullptr, nullptr, nullptr, false);
       // the cold tick: every instance with a latency starts with the policy of this first solve
       if (!rc && delayed && first_cold) {
@@ -2352,12 +2360,12 @@ int hb_contact_positions_batch(hb_ctx* ctx, int B, const double* x, double* pos)
 }
 
 static std::atomic<int> g_plan_threads{0};   // 0 = hardware_concurrency (hb_plan_set_threads)
-static int plan_range(int lo, int hi, const hb_plan_input* in, const hb_target* targets, const hb_planner_settings* settings, double* latest_stance,
-                      hb_reference* out) {
+static int plan_range(int lo, int hi, const hb_plan_input* in, const hb_target* targets, const hb_planner_settings* settings,
+                      const hb_terrain* maps, double* latest_stance, hb_reference* out) {
   const hbplan::PlanConsts& pc = plan_consts();
   for (int i = lo; i < hi; ++i) {
-    const int rc = hbplan::plan_one(pc, in[i], targets ? targets + i : nullptr, settings ? settings + i : nullptr, latest_stance + (size_t)i * 12,
-                                    out + i, true);
+    const int rc = hbplan::plan_one(pc, in[i], targets ? targets + i : nullptr, settings ? settings + i : nullptr, maps ? maps + i : nullptr,
+                                    latest_stance + (size_t)i * 12, out + i, true);
     if (rc) return rc;
   }
   return HB_OK;
@@ -2379,17 +2387,24 @@ int hb_plan_references_targets(int B, const hb_plan_input* in, const hb_target* 
 
 int hb_plan_references_settings(int B, const hb_plan_input* in, const hb_target* targets, const hb_planner_settings* settings, double* latest_stance,
                                 hb_reference* out) {
-  if (B < 0 || !in || !latest_stance || !out || !all_ok(B, targets, target_ok) || !all_ok(B, settings, planner_settings_ok)) return HB_EINVAL;
+  return hb_plan_references_maps(B, in, targets, settings, nullptr, latest_stance, out);
+}
+
+int hb_plan_references_maps(int B, const hb_plan_input* in, const hb_target* targets, const hb_planner_settings* settings, const hb_terrain* maps,
+                            double* latest_stance, hb_reference* out) {
+  if (B < 0 || !in || !latest_stance || !out || !all_ok(B, targets, target_ok) || !all_ok(B, settings, planner_settings_ok) ||
+      !all_ok(B, maps, terrain_ok))
+    return HB_EINVAL;
   // instances are independent: spread them over the host cores (the planner feeds ~1e5 solves/s per GPU; one core plans ~2e4/s)
   unsigned hw = std::thread::hardware_concurrency();
   if (const int forced = g_plan_threads.load()) hw = (unsigned)forced;
   int nt = (int)std::min<unsigned>(hw ? hw : 1u, (unsigned)((B + 63) / 64));
-  if (nt <= 1) return plan_range(0, B, in, targets, settings, latest_stance, out);
+  if (nt <= 1) return plan_range(0, B, in, targets, settings, maps, latest_stance, out);
   std::vector<std::thread> pool;
   std::vector<int> rcs(nt, HB_OK);
   for (int t = 0; t < nt; ++t) {
     const int lo = (int)((long long)B * t / nt), hi = (int)((long long)B * (t + 1) / nt);
-    pool.emplace_back([=, &rcs]() { rcs[t] = plan_range(lo, hi, in, targets, settings, latest_stance, out); });
+    pool.emplace_back([=, &rcs]() { rcs[t] = plan_range(lo, hi, in, targets, settings, maps, latest_stance, out); });
   }
   for (auto& th : pool) th.join();
   for (int t = 0; t < nt; ++t) if (rcs[t]) return rcs[t];
@@ -2397,7 +2412,11 @@ int hb_plan_references_settings(int B, const hb_plan_input* in, const hb_target*
 }
 
 int hb_goal_to_target(int B, const double* t, const double* x, const double* goal, hb_target* out) {
-  if (B < 0 || !t || !x || !goal || !out) return HB_EINVAL;
+  return hb_goal_to_target_maps(B, t, x, goal, nullptr, out);
+}
+
+int hb_goal_to_target_maps(int B, const double* t, const double* x, const double* goal, const hb_terrain* maps, hb_target* out) {
+  if (B < 0 || !t || !x || !goal || !out || !all_ok(B, maps, terrain_ok)) return HB_EINVAL;
   for (int i = 0; i < B; ++i) {
     const double* xi = x + (size_t)i * NX; const double* gi = goal + (size_t)i * 3;
     if (!isfinite(t[i]) || !isfinite(xi[6]) || !isfinite(xi[7]) || !isfinite(xi[8]) || !isfinite(xi[9]) || !isfinite(gi[0]) || !isfinite(gi[1]) ||
@@ -2406,13 +2425,17 @@ int hb_goal_to_target(int B, const double* t, const double* x, const double* goa
   }
   for (int i = 0; i < B; ++i) {
     memset(&out[i], 0, sizeof(hb_target));
-    hbplan::goal_to_target(plan_consts(), t[i], x + (size_t)i * NX, goal + (size_t)i * 3, out[i]);
+    hbplan::goal_to_target(plan_consts(), t[i], x + (size_t)i * NX, goal + (size_t)i * 3, out[i], maps ? maps + i : nullptr);
   }
   return HB_OK;
 }
 
 int hb_cmd_vel_to_target(int B, const double* t, double horizon, const double* x, const double* cmd_vel, hb_target* out) {
-  if (B < 0 || !t || !x || !cmd_vel || !out || !isfinite(horizon)) return HB_EINVAL;
+  return hb_cmd_vel_to_target_maps(B, t, horizon, x, cmd_vel, nullptr, out);
+}
+
+int hb_cmd_vel_to_target_maps(int B, const double* t, double horizon, const double* x, const double* cmd_vel, const hb_terrain* maps, hb_target* out) {
+  if (B < 0 || !t || !x || !cmd_vel || !out || !isfinite(horizon) || !all_ok(B, maps, terrain_ok)) return HB_EINVAL;
   for (int i = 0; i < B; ++i) {
     if (!isfinite(t[i])) return HB_EINVAL;
     for (int k = 6; k < 12; ++k) if (!isfinite(x[(size_t)i * NX + k])) return HB_EINVAL;
@@ -2420,7 +2443,7 @@ int hb_cmd_vel_to_target(int B, const double* t, double horizon, const double* x
   }
   for (int i = 0; i < B; ++i) {
     memset(&out[i], 0, sizeof(hb_target));
-    hbplan::cmd_vel_to_target(plan_consts(), cmd_vel + (size_t)i * 4, t[i], x + (size_t)i * NX, horizon, out[i]);
+    hbplan::cmd_vel_to_target(plan_consts(), cmd_vel + (size_t)i * 4, t[i], x + (size_t)i * NX, horizon, out[i], maps ? maps + i : nullptr);
   }
   return HB_OK;
 }

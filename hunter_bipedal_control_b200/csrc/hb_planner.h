@@ -20,8 +20,10 @@
 
 #if defined(__CUDACC__)
 #define HBP_HD __host__ __device__
+#define HBP_HDI __host__ __device__ __forceinline__
 #else
 #define HBP_HD
+#define HBP_HDI inline
 #endif
 
 namespace hbplan {
@@ -42,6 +44,53 @@ inline PlanConsts make_consts() {
 
 HBP_HD inline double dmin(double a, double b) { return a < b ? a : b; }
 HBP_HD inline double dmax(double a, double b) { return a > b ? a : b; }
+
+// a product rounded on its own: never contracted into an fma by the device compiler, so host and device round alike
+HBP_HD inline double mul_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+
+// The one terrain lookup (terrain, hunter_b200.h) of the plant, the height check and the planner's height maps. RN: every product of
+// the interpolation is rounded on its own (mul_rn), so that the host and the device get the same bits (the planner); without it the
+// device compiler contracts them as it always has (the plant and the height check, whose instructions this form leaves unchanged).
+template <bool RN> HBP_HDI double terrain_mul(double a, double b) { return RN ? mul_rn(a, b) : a * b; }
+
+// One axis of a terrain lookup: the grid coordinate of the world coordinate x, clamped to [0, n - 1], split into the cell index
+// i <= n - 2 and the fraction a of the cell. Returns whether x was clamped (off the grid, where the gradient along this axis is zero).
+// A NaN coordinate clamps to 0, so no index leaves the grid.
+HBP_HDI bool terrain_axis(double x, double origin, double spacing, int n, int* i, double* a) {
+  double u = (x - origin) / spacing;
+  bool clamped = false;
+  if (!(u >= 0.0)) { u = 0.0; clamped = true; }
+  else if (u > (double)(n - 1)) { u = (double)(n - 1); clamped = true; }
+  int c = (int)floor(u);
+  if (c > n - 2) c = n - 2;
+  *i = c; *a = u - (double)c;
+  return clamped;
+}
+
+// Height h of the terrain at world (x, y) and its gradient (gx, gy), bilinear on the cell, as hunter_b200.h documents it
+template <bool RN> HBP_HDI double terrain_height(const hb_terrain& t, double x, double y, double* gx, double* gy) {
+  int i, j;
+  double a, b;
+  const bool cx = terrain_axis(x, t.origin[0], t.spacing, t.nx, &i, &a), cy = terrain_axis(y, t.origin[1], t.spacing, t.ny, &j, &b);
+  const double h00 = t.height[j][i], h01 = t.height[j][i + 1], h10 = t.height[j + 1][i], h11 = t.height[j + 1][i + 1];
+  const double h0 = h00 + terrain_mul<RN>(a, h01 - h00), h1 = h10 + terrain_mul<RN>(a, h11 - h10);
+  const double d0 = h01 - h00, d1 = h11 - h10;
+  *gx = cx ? 0.0 : (d0 + terrain_mul<RN>(b, d1 - d0)) / t.spacing;
+  *gy = cy ? 0.0 : (h1 - h0) / t.spacing;
+  return h0 + terrain_mul<RN>(b, h1 - h0);
+}
+
+// h(x, y) of a planner height map (height maps, hunter_b200.h): the terrain lookup with its products rounded on their own
+HBP_HD inline double map_height(const hb_terrain* m, double x, double y) {
+  double gx, gy;
+  return terrain_height<true>(*m, x, y, &gx, &gy);
+}
 
 struct Vec3 { double x, y, z; };
 HBP_HD inline Vec3 operator+(Vec3 a, Vec3 b) { return {a.x + b.x, a.y + b.y, a.z + b.z}; }
@@ -146,16 +195,18 @@ struct Target { int n; double t[HB_MAX_TARGETS]; double x[HB_MAX_TARGETS][22]; }
 
 // cmdVelToTargetTrajectories (TargetTrajectoriesPublisher.cpp:102-130) with targetPoseToTargetTrajectories (:41-62), written into the
 // sample count n, times tm and states x of a target: the planner's Target, or a caller's hb_target (the teleop capture writes global
-// memory, not a stack copy)
+// memory, not a stack copy). With a height map (nullable) both samples' body heights are taken above the map (height maps, hunter_b200.h).
 HBP_HD inline void cmd_vel_target(const PlanConsts& pc, const double* cmd /*vx,vy,vz,wz*/, double time, const double* state, double time_to_target,
-                                  int& n, double* tm, double (*x)[22]) {
+                                  int& n, double* tm, double (*x)[22], const hb_terrain* map) {
   const double* pose = state + 6;
   Vec3 v = rot_zyx(pose + 3, {cmd[0], cmd[1], cmd[2]});
   if (fabs(v.x) < 0.06) v.x = 0.0;
   else if (fabs(v.y) < 0.06) v.y = 0.0;
   double target[6] = {pose[0] + v.x * time_to_target, pose[1] + v.y * time_to_target, HB_COM_HEIGHT, pose[3] + cmd[3] * time_to_target, 0.0, 0.0};
   double cur[6] = {pose[0], pose[1], pose[2], pose[3], 0.0, 0.0};
-  double dz = HB_COM_HEIGHT - pose[2];
+  double com = HB_COM_HEIGHT;
+  if (map) { com = HB_COM_HEIGHT + map_height(map, pose[0], pose[1]); target[2] = HB_COM_HEIGHT + map_height(map, target[0], target[1]); }
+  double dz = com - pose[2];
   dz = dz > 0 ? dmin(dz, 0.04) : dmax(dz, -0.04);      // changeLimit_[2] (TargetTrajectoriesPublisher.h:97)
   cur[2] = pose[2] + dz;
   n = 2;
@@ -167,35 +218,32 @@ HBP_HD inline void cmd_vel_target(const PlanConsts& pc, const double* cmd /*vx,v
     x[k][0] = v.x; x[k][1] = v.y; x[k][2] = v.z;    // stateTrajectory[.].head(3) = cmdVelRot (:127-128)
   }
 }
-HBP_HD inline Target cmd_vel_to_target(const PlanConsts& pc, const double* cmd, double time, const double* state, double time_to_target) {
+HBP_HD inline Target cmd_vel_to_target(const PlanConsts& pc, const double* cmd, double time, const double* state, double time_to_target,
+                                        const hb_terrain* map = nullptr) {
   Target tg;
-  cmd_vel_target(pc, cmd, time, state, time_to_target, tg.n, tg.t, tg.x);
+  cmd_vel_target(pc, cmd, time, state, time_to_target, tg.n, tg.t, tg.x, map);
   return tg;
 }
-HBP_HD inline void cmd_vel_to_target(const PlanConsts& pc, const double* cmd, double time, const double* state, double time_to_target, hb_target& tg) {
-  cmd_vel_target(pc, cmd, time, state, time_to_target, tg.n, tg.time, tg.state);
-}
-
-// a product rounded on its own: never contracted into an fma by the device compiler, so host and device round alike
-HBP_HD inline double mul_rn(double a, double b) {
-#if defined(__CUDA_ARCH__)
-  return __dmul_rn(a, b);
-#else
-  return a * b;
-#endif
+HBP_HD inline void cmd_vel_to_target(const PlanConsts& pc, const double* cmd, double time, const double* state, double time_to_target, hb_target& tg,
+                                     const hb_terrain* map = nullptr) {
+  cmd_vel_target(pc, cmd, time, state, time_to_target, tg.n, tg.time, tg.state, map);
 }
 
 // goalToTargetTrajectories with estimateTimeToTarget (TargetTrajectoriesPublisher.cpp:29-38, :83-100) and targetPoseToTargetTrajectories
 // (:41-62), written into a caller's hb_target (the device capture writes global memory, not a stack copy). The yaw difference is not
 // wrapped, as in the reference. A zero reaching time would give two samples at one time: the single target sample is kept instead.
-HBP_HD inline void goal_to_target(const PlanConsts& pc, double time, const double* state, const double* goal /*x, y, yaw*/, hb_target& tg) {
+// With a height map (nullable) the body height is taken above the map, and the goal sample's differs by the map's rise to the goal.
+HBP_HD inline void goal_to_target(const PlanConsts& pc, double time, const double* state, const double* goal /*x, y, yaw*/, hb_target& tg,
+                                  const hb_terrain* map = nullptr) {
   const double* pose = state + 6;
-  double dz = HB_COM_HEIGHT - pose[2];
+  const double h = map ? map_height(map, pose[0], pose[1]) : 0.0;
+  double dz = (map ? HB_COM_HEIGHT + h : HB_COM_HEIGHT) - pose[2];
   dz = dz > 0 ? dmin(dz, 0.04) : dmax(dz, -0.04);      // changeLimit_[2] (TargetTrajectoriesPublisher.h:97)
   const double z = pose[2] + dz;
+  const double zg = map ? z + (map_height(map, goal[0], goal[1]) - h) : z;
   const double dx = goal[0] - pose[0], dy = goal[1] - pose[1];
   const double reach = dmax(fabs(goal[2] - pose[3]) / HB_TARGET_ROTATION_VELOCITY, sqrt(mul_rn(dx, dx) + mul_rn(dy, dy)) / HB_TARGET_DISPLACEMENT_VELOCITY);
-  const double cur[6] = {pose[0], pose[1], z, pose[3], 0.0, 0.0}, target[6] = {goal[0], goal[1], z, goal[2], 0.0, 0.0};
+  const double cur[6] = {pose[0], pose[1], z, pose[3], 0.0, 0.0}, target[6] = {goal[0], goal[1], zg, goal[2], 0.0, 0.0};
   tg.n = reach > 0.0 ? 2 : 1;
   tg.time[0] = time; tg.time[1] = time + reach;
   for (int k = 0; k < tg.n; ++k) {
@@ -247,8 +295,9 @@ HBP_HD inline void find_index(int index, const bool* stock, int n, int& start_id
 
 // SwingTrajectoryPlanner::calNextFootPos (:289-312). body_vel_cmd = [vx, vy, vz, wz, 0, 0] as set from /cmd_vel_filtered
 // (SwitchedModelReferenceManager.cpp:91-101): its tail(3) = (wz, 0, 0) is used as the commanded angular velocity, as the reference does.
+// With a height map (nullable) the centrifugal term reads the body height above the map, and the foothold stands on the map.
 HBP_HD inline Vec3 next_foot_pos(const PlanSettings& s, int foot, double current_time, double stop_time, double next_middle_time, const double* next_middle_body_pos,
-                          const double* current_body_pos, Vec3 current_body_vel, const double* body_vel_cmd) {
+                          const double* current_body_pos, Vec3 current_body_vel, const double* body_vel_cmd, const hb_terrain* map) {
   // feet_bias_ (SwingTrajectoryPlanner.cpp:76-79): toes x1, heels x2, +y on the left
   const Vec3 bias{foot < 2 ? s.feet_bias_x1 : s.feet_bias_x2, (foot & 1) ? -s.feet_bias_y : s.feet_bias_y, s.feet_bias_z};
   const Vec3 roted_bias = rot_zyx(next_middle_body_pos + 3, bias);
@@ -258,14 +307,17 @@ HBP_HD inline Vec3 next_foot_pos(const PlanSettings& s, int foot, double current
   const double k = 0.03;
   const Vec3 p_shoulder = (stop_time - current_time) * (0.5 * vel_linear + 0.5 * vel_cmd_linear) + roted_bias;
   const Vec3 p_symmetry = (next_middle_time - stop_time) * vel_linear + k * (vel_linear - vel_cmd_linear);
-  const Vec3 p_centrifugal = (0.5 * sqrt(current_body_pos[2] / 9.81)) * cross(vel_linear, vel_cmd_angular);
+  const double body_z = map ? current_body_pos[2] - map_height(map, current_body_pos[0], current_body_pos[1]) : current_body_pos[2];
+  const Vec3 p_centrifugal = (0.5 * sqrt(body_z / 9.81)) * cross(vel_linear, vel_cmd_angular);
   Vec3 r = Vec3{current_body_pos[0], current_body_pos[1], current_body_pos[2]} + p_shoulder + p_symmetry + p_centrifugal;
-  r.z = s.next_stance_z;
+  r.z = map ? s.next_stance_z + map_height(map, r.x, r.y) : s.next_stance_z;
   return r;
 }
 
-// SwingTrajectoryPlanner::genSwingTrajs (:314-358): x/y three-node, z four-node Hermite splines with the reference's shape constants
-HBP_HD inline void gen_swing(const PlanSettings& s, SwingOut& sp, int foot, double t0, double t1, Vec3 a, Vec3 b) {
+// SwingTrajectoryPlanner::genSwingTrajs (:314-358): x/y three-node, z four-node Hermite splines with the reference's shape constants.
+// The z shape is that of ground at z = 0 (its node heights are fractions of the absolute apex). With a height map (nullable) it is built
+// on ends lowered by h_lo = min(a.z, b.z) - next_stance_z, the lower end's ground, and h_lo is added back to the node positions.
+HBP_HD inline void gen_swing(const PlanSettings& s, SwingOut& sp, int foot, double t0, double t1, Vec3 a, Vec3 b, const hb_terrain* map) {
   const double xy_a1 = 0.417, xy_l1 = 0.650, xy_k1 = 1.770;
   const double pa[3] = {a.x, a.y, a.z}, pb[3] = {b.x, b.y, b.z};
   for (int ax = 0; ax < 2; ++ax) {
@@ -273,13 +325,16 @@ HBP_HD inline void gen_swing(const PlanSettings& s, SwingOut& sp, int foot, doub
     emit(sp, foot, ax, Seg{n0.t, n1.t, n0.p, n0.v, n1.p, n1.v});
     emit(sp, foot, ax, Seg{n1.t, n2.t, n1.p, n1.v, n2.p, n2.v});
   }
+  double h_lo = 0.0;
+  if (map) { h_lo = dmin(a.z, b.z) - s.next_stance_z; a.z = a.z - h_lo; b.z = b.z - h_lo; }
   const double scaling = dmin(1.0, (t1 - t0) / s.swing_time_scale);
   const double max_z = dmax(a.z, b.z) + scaling * s.swing_height;
   const double z_a1 = 0.251, z_l1 = 0.749, z_k1 = 1.338, z_a2 = 0.630, z_l2 = 0.570, z_k2 = 1.633, z_k3 = 0.0;
-  const Node n0{t0, a.z, 0.0};
-  const Node n1{(1 - z_a1) * t0 + z_a1 * t1, z_l1 * max_z, z_k1 * (z_l1 * (max_z - a.z)) / (z_a1 * (t1 - t0))};
-  const Node n2{(1 - z_a2) * t0 + z_a2 * t1, z_l2 * max_z + (1 - z_l2) * b.z, z_k2 * z_l2 * (b.z - max_z) / ((1 - z_a2) * (t1 - t0))};
-  const Node n3{t1, b.z, z_k3 * z_l2 * (b.z - max_z) / ((1 - z_a2) * (t1 - t0))};
+  Node n0{t0, a.z, 0.0};
+  Node n1{(1 - z_a1) * t0 + z_a1 * t1, z_l1 * max_z, z_k1 * (z_l1 * (max_z - a.z)) / (z_a1 * (t1 - t0))};
+  Node n2{(1 - z_a2) * t0 + z_a2 * t1, z_l2 * max_z + (1 - z_l2) * b.z, z_k2 * z_l2 * (b.z - max_z) / ((1 - z_a2) * (t1 - t0))};
+  Node n3{t1, b.z, z_k3 * z_l2 * (b.z - max_z) / ((1 - z_a2) * (t1 - t0))};
+  if (map) { n0.p = n0.p + h_lo; n1.p = n1.p + h_lo; n2.p = n2.p + h_lo; n3.p = n3.p + h_lo; }
   emit(sp, foot, 2, Seg{n0.t, n1.t, n0.p, n0.v, n1.p, n1.v});
   emit(sp, foot, 2, Seg{n1.t, n2.t, n1.p, n1.v, n2.p, n2.v});
   emit(sp, foot, 2, Seg{n2.t, n3.t, n2.p, n2.v, n3.p, n3.v});
@@ -288,14 +343,15 @@ HBP_HD inline void gen_swing(const PlanSettings& s, SwingOut& sp, int foot, doub
 // SwingTrajectoryPlanner::update (:164-286). latest_stance (4x3) is the planner's state (in/out).
 // Returns false where the reference would throw (swing phase without a defined take-off / touch-down, :421-458).
 // The feet are independent of each other: [j_begin, j_end) selects the ones this call plans (the host planner passes 0..4, the
-// cooperative device kernel one foot per thread).
+// cooperative device kernel one foot per thread). With a height map (nullable) every lift-off point stands on the map: its z is
+// next_stance_z + h at its (x, y).
 HBP_HD inline bool plan_swing(const PlanSettings& s, const ModeSchedule& ms, const Target& tg, double init_time, const double* current_feet /*12*/, const double* body_vel_cmd /*6*/,
-                              double* latest_stance /*12*/, SwingOut& sp, int j_begin = 0, int j_end = 4) {
+                              double* latest_stance /*12*/, SwingOut& sp, const hb_terrain* map, int j_begin = 0, int j_end = 4) {
   const int np = ms.n_events + 1;
   const int mode_now = mode_at(ms, init_time + 0.001);
   for (int i = j_begin; i < j_end; ++i) {
     if (contact_flag(mode_now, i)) for (int a = 0; a < 3; ++a) latest_stance[3 * i + a] = current_feet[3 * i + a];
-    latest_stance[3 * i + 2] = s.next_stance_z;
+    latest_stance[3 * i + 2] = map ? s.next_stance_z + map_height(map, latest_stance[3 * i], latest_stance[3 * i + 1]) : s.next_stance_z;
   }
   for (int j = j_begin; j < j_end; ++j) {
     bool stock[MAX_PHASES + 1];
@@ -320,12 +376,12 @@ HBP_HD inline bool plan_swing(const PlanSettings& s, const ModeSchedule& ms, con
           target_state(tg, next_middle_time, xm);
           target_state(tg, init_time, xc);
           const Vec3 body_vel{tg.x[0][0], tg.x[0][1], tg.x[0][2]};
-          next = next_foot_pos(s, j, init_time, t_final, next_middle_time, xm + 6, xc + 6, body_vel, body_vel_cmd);
+          next = next_foot_pos(s, j, init_time, t_final, next_middle_time, xm + 6, xc + 6, body_vel, body_vel_cmd, map);
           last_final_idx = fi;
         }
         // every phase of a swing interval pushes the same spline set (one MultiCubicSpline per phase index in the reference);
         // only emit it once per swing interval
-        if (p == 0 || stock[p - 1]) gen_swing(s, sp, j, t_start, t_final, last, next);
+        if (p == 0 || stock[p - 1]) gen_swing(s, sp, j, t_start, t_final, last, next, map);
       } else {
         if (p == 0 || !stock[p - 1]) {
           const double t_start = ms.events[si], t_final = (fi >= 0 && fi < ms.n_events) ? ms.events[fi] : ms.events[ms.n_events - 1];
@@ -665,10 +721,10 @@ HBP_HD inline int write_schedule_and_targets(const ModeSchedule& ms, const Targe
 }
 
 // One instance, start to finish: schedule, target (the given one, or the cmd_vel target when target is null), swing planner, IK joint
-// references, compact output; with the planner settings `settings` (null: the compiled-in ones).
+// references, compact output; with the planner settings `settings` (null: the compiled-in ones) and the height map `map` (null: none).
 // Returns 0, -1 (invalid input) or -5 (schedule / reference capacity exceeded, or a swing phase without take-off / touch-down time).
 HBP_HD inline int plan_one(const PlanConsts& pc, const hb_plan_input& p, const hb_target* target, const hb_planner_settings* settings,
-                           double* latest_stance /*12, in/out*/, hb_reference* out, bool zero_fill) {
+                           const hb_terrain* map, double* latest_stance /*12, in/out*/, hb_reference* out, bool zero_fill) {
   if (!(p.horizon > 0.0) || !(p.prev_event < p.gait_start) || p.gait < 0 || p.gait > 3) return -1;
   const double tf = p.t0 + p.horizon;
   if (zero_fill) memset(out, 0, sizeof(*out));
@@ -679,11 +735,11 @@ HBP_HD inline int plan_one(const PlanConsts& pc, const hb_plan_input& p, const h
   if (!tile_gait(ps.tmpl, p.prev_event, p.gait_start, p.t0 - p.horizon, tf + p.horizon, ms)) return -5;
   Target tg;
   if (target) target_from(*target, tg);
-  else tg = cmd_vel_to_target(pc, p.cmd_vel, p.t0, p.x0, p.time_to_target);
+  else tg = cmd_vel_to_target(pc, p.cmd_vel, p.t0, p.x0, p.time_to_target, map);
   const double body_vel_cmd[6] = {p.cmd_vel[0], p.cmd_vel[1], p.cmd_vel[2], p.cmd_vel[3], 0.0, 0.0};
   SwingOut so{out, p.t0 - 1e-9, tf + 1e-9, false};
   for (int c = 0; c < 4; ++c) for (int a = 0; a < 3; ++a) out->n_segments[c][a] = 0;
-  if (!plan_swing(ps, ms, tg, p.t0, p.feet_pos, body_vel_cmd, latest_stance, so) || so.overflow) return -5;
+  if (!plan_swing(ps, ms, tg, p.t0, p.feet_pos, body_vel_cmd, latest_stance, so, map) || so.overflow) return -5;
   if (p.joint_ik && !joint_references(pc, out, p.t0, tf, p.x0, tg)) return -5;
   return write_schedule_and_targets(ms, tg, so.t_lo, so.t_hi, out);
 }

@@ -250,17 +250,19 @@ __global__ void plan_prepare_kernel(int B, const hb_plan_input* in, double* t0, 
 // a copy on its stack. An instance with a record in targets plans on it instead of its cmd_vel target, where captured (nullable: every
 // such instance) has captured[inst] >= 0 (a goal an episode captured). Thread 0 of an instance stages what its plan reads of its record in
 // settings (hbplan::PlanSettings: its gait's template and the swing settings; the compiled-in values without a record) in shared memory,
-// where the four threads read it.
+// where the four threads read it. An instance with a record in maps plans on that height map (height maps, hunter_b200.h), which every
+// thread reads where it is (a map is 32.8 KB, read at a few points per foot).
 __global__ void __launch_bounds__(32) plan_references_coop_kernel(int B, const hb_plan_input* in, const double* feet, double* latest_stance,
                                                                   hb_reference* out, int32_t* status, hbplan::PlanConsts pc,
                                                                   InstanceView<hb_target> targets, const int32_t* captured,
-                                                                  InstanceView<hb_planner_settings> settings) {
+                                                                  InstanceView<hb_planner_settings> settings, InstanceView<hb_terrain> maps) {
   __shared__ hbplan::Target s_tg[8], s_old[8];
   __shared__ hbplan::PlanSettings s_set[8];
   __shared__ int s_rc[8];
   const int g = threadIdx.x >> 2, r = threadIdx.x & 3;
   const int inst = blockIdx.x * 8 + g;
   const bool active = inst < B;
+  const hb_terrain* map = active ? maps.of(inst) : nullptr;
   hb_plan_input p;
   hbplan::ModeSchedule ms;
   hb_reference* o = out + (active ? inst : 0);
@@ -281,7 +283,7 @@ __global__ void __launch_bounds__(32) plan_references_coop_kernel(int B, const h
     if (rc == 0 && r == 0) {
       const hb_target* tg = targets.of(inst);
       if (tg && (!captured || captured[inst] >= 0)) hbplan::target_from(*tg, s_tg[g]);
-      else s_tg[g] = hbplan::cmd_vel_to_target(pc, p.cmd_vel, p.t0, p.x0, p.time_to_target);
+      else s_tg[g] = hbplan::cmd_vel_to_target(pc, p.cmd_vel, p.t0, p.x0, p.time_to_target, map);
     }
   }
   __syncwarp();
@@ -290,7 +292,7 @@ __global__ void __launch_bounds__(32) plan_references_coop_kernel(int B, const h
     const double body_vel_cmd[6] = {p.cmd_vel[0], p.cmd_vel[1], p.cmd_vel[2], p.cmd_vel[3], 0.0, 0.0};
     hbplan::SwingOut so{o, t_lo, t_hi, false};
     for (int a = 0; a < 3; ++a) o->n_segments[r][a] = 0;
-    if (!hbplan::plan_swing(s_set[g], ms, s_tg[g], p.t0, p.feet_pos, body_vel_cmd, latest_stance + (size_t)inst * 12, so, r, r + 1) || so.overflow) rc = -5;
+    if (!hbplan::plan_swing(s_set[g], ms, s_tg[g], p.t0, p.feet_pos, body_vel_cmd, latest_stance + (size_t)inst * 12, so, map, r, r + 1) || so.overflow) rc = -5;
   }
   __syncwarp();                // every foot has read the two-sample target before thread 0 resamples it in place
   if (active) {

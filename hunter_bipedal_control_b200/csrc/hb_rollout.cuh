@@ -32,10 +32,11 @@ __device__ __forceinline__ bool teleop_message(const hb_teleop_setting& s, int a
 // from the captured one (captured_idx -1: none); reset (an episode's tick 0) forgets the captured goal first. The planner reads them.
 // Teleoperated instances (a record in teleop; publisher state pub): the goal capture compares with the goal they last saw, then a message
 // due on tick a runs the publisher step and captures the cmd_vel target of last (source TELEOP_CAPTURED); they plan with cmd_vel = last.
+// Both captures of an instance with a record in maps build their targets on that height map (height maps, hunter_b200.h).
 __global__ void rollout_plan_inputs_kernel(int B, int a, double t, double horizon, const hb_rollout_command* cmd, const double* rbd,
                                            const hb_estimation_state* est, hb_plan_input* in, InstanceView<hb_goal_schedule> goals,
                                            InstanceView<hb_teleop_setting> teleop, TeleopState* pub, int reset, hb_target* captured,
-                                           int32_t* captured_idx, hbplan::PlanConsts pc) {
+                                           int32_t* captured_idx, hbplan::PlanConsts pc, InstanceView<hb_terrain> maps) {
   const int inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= B) return;
   const hb_rollout_command& c = cmd[inst];
@@ -62,7 +63,7 @@ __global__ void rollout_plan_inputs_kernel(int B, int a, double t, double horizo
     for (int k = 0; k < s.n_goal; ++k) if (s.time[k] <= t) g = k;
     const int had = ts ? ts->goal_seen - 1 : reset ? -1 : captured_idx[inst];
     if (g >= 0 && g != had) {
-      hbplan::goal_to_target(pc, t, p.x0, s.goal[g], captured[inst]);
+      hbplan::goal_to_target(pc, t, p.x0, s.goal[g], captured[inst], maps.of(inst));
       if (ts) captured_idx[inst] = g;
     }
     if (ts) ts->goal_seen = (g >= 0 ? g : had) + 1;
@@ -78,38 +79,11 @@ __global__ void rollout_plan_inputs_kernel(int B, int a, double t, double horizo
         last[k] += d;
       }
       last[2] = 0.0;
-      hbplan::cmd_vel_to_target(pc, last, t, p.x0, horizon, captured[inst]);
+      hbplan::cmd_vel_to_target(pc, last, t, p.x0, horizon, captured[inst], maps.of(inst));
       captured_idx[inst] = TELEOP_CAPTURED;
     }
     for (int i = 0; i < 4; ++i) p.cmd_vel[i] = ts->last[i];
   }
-}
-
-// One axis of a terrain lookup (terrain, hunter_b200.h): the grid coordinate of the world coordinate x, clamped to [0, n - 1], split into
-// the cell index i <= n - 2 and the fraction a of the cell. Returns whether x was clamped (off the grid, where the gradient along this
-// axis is zero). A NaN coordinate clamps to 0, so no index leaves the grid.
-__device__ __forceinline__ bool terrain_axis(double x, double origin, double spacing, int n, int* i, double* a) {
-  double u = (x - origin) / spacing;
-  bool clamped = false;
-  if (!(u >= 0.0)) { u = 0.0; clamped = true; }
-  else if (u > (double)(n - 1)) { u = (double)(n - 1); clamped = true; }
-  int c = (int)floor(u);
-  if (c > n - 2) c = n - 2;
-  *i = c; *a = u - (double)c;
-  return clamped;
-}
-
-// Height h of the terrain at world (x, y) and its gradient (gx, gy), bilinear on the cell, as hunter_b200.h documents it
-__device__ __forceinline__ double terrain_height(const hb_terrain& t, double x, double y, double* gx, double* gy) {
-  int i, j;
-  double a, b;
-  const bool cx = terrain_axis(x, t.origin[0], t.spacing, t.nx, &i, &a), cy = terrain_axis(y, t.origin[1], t.spacing, t.ny, &j, &b);
-  const double h00 = t.height[j][i], h01 = t.height[j][i + 1], h10 = t.height[j + 1][i], h11 = t.height[j + 1][i + 1];
-  const double h0 = h00 + a * (h01 - h00), h1 = h10 + a * (h11 - h10);
-  const double d0 = h01 - h00, d1 = h11 - h10;
-  *gx = cx ? 0.0 : (d0 + b * (d1 - d0)) / t.spacing;
-  *gy = cy ? 0.0 : (h1 - h0) / t.spacing;
-  return h0 + b * (h1 - h0);
 }
 
 // failure bits of a state entering a tick; the orientation and height checks are only meaningful on a finite state. ter (nullable): the
@@ -120,7 +94,7 @@ __device__ __forceinline__ int rollout_state_check(const double* r, double min_b
   if (r[2] > M_PI_2 || r[2] < -M_PI_2) why |= HB_ROLLOUT_FAIL_ORIENTATION;     // zyx[2] = roll: SafetyChecker::checkOrientation
   if (min_base_height != 0.0) {
     double z = r[5];
-    if (ter) { double gx, gy; z -= terrain_height(*ter, r[3], r[4], &gx, &gy); }
+    if (ter) { double gx, gy; z -= hbplan::terrain_height<false>(*ter, r[3], r[4], &gx, &gy); }
     if (z < min_base_height) why |= HB_ROLLOUT_FAIL_HEIGHT;
   }
   return why;
@@ -697,7 +671,7 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
     __syncwarp();
     if (lane < 4) {
       double gh = prm.ground_height, gx = 0.0, gy = 0.0;
-      if (ter) gh = terrain_height(*ter, sh.cpos[3 * lane], sh.cpos[3 * lane + 1], &gx, &gy);
+      if (ter) gh = hbplan::terrain_height<false>(*ter, sh.cpos[3 * lane], sh.cpos[3 * lane + 1], &gx, &gy);
       if (gx == 0.0 && gy == 0.0) {      // flat ground, or a level patch of the terrain: the flat contact at its height
         const double depth = gh - sh.cpos[3 * lane + 2];
         double fz = 0.0, fx = 0.0, fy = 0.0;

@@ -145,6 +145,25 @@ int hb_default_planner_settings(hb_planner_settings* s);
  * mode and time counts do not match (n modes, n + 1 times) or that has more than HB_GAIT_MAX_PHASES phases, or a result that is not valid. */
 int hb_parse_planner_settings(const char* task_info, const char* gait_info, hb_planner_settings* out);
 
+/* ---- height maps: the ground the planner is told about, the reference's terrainHeight as a function of (x, y) ----
+ * A height map is an hb_terrain record (terrain, below) that the planner reads; the reference plans with terrainHeight = 0 everywhere
+ * (SwitchedModelReferenceManager.cpp:152). For an instance with a map m, h(x, y) is the terrain lookup of m (the grid, clamping and
+ * bilinear rules of terrain, below) with each of its products rounded on its own, so the host and the device get the same bits. Map
+ * heights are measured from the ground the planner otherwise assumes: an all-zero map is the planner without one, and over a plant whose
+ * flat ground is at sim.ground_height = g the map of a terrain H is H - g. With a map the planner changes in these places only:
+ *  - lift-off: every stance foot's latest stance point has z = next_stance_z + h at its (x, y);
+ *  - touch-down: every planned foothold r has r.z = next_stance_z + h(r.x, r.y);
+ *  - swing z: the four-node z spline is built on its ends lowered by h_lo = min(lift-off z, touch-down z) - next_stance_z, with the shape
+ *    of swing_trajectory_config, and h_lo is added back to its node positions (velocities are differences and stay);
+ *  - centrifugal term of the foothold: sqrt((z - h(x, y)) / g) with (x, y, z) the body position it reads;
+ *  - body height of the targets: with the pose p = x[6:12] and z' = p[2] + clamp(HB_COM_HEIGHT + h(p[0], p[1]) - p[2], -0.04, 0.04), the
+ *    cmd_vel target's sample 0 has height z' and its sample 1 HB_COM_HEIGHT + h at sample 1's (x, y); the goal target's sample 0 has z'
+ *    and its goal sample z' + (h(goal x, y) - h(p[0], p[1])), also when it is the only sample. The teleop messages' target is the cmd_vel
+ *    target.
+ * A map of zeros gives the plans and targets of no map bit for bit; an instance without a map plans as before. The IK joint references
+ * follow the swing splines and the targets. Maps are read by every device planner path (hb_plan_set_maps) and by the host calls
+ * hb_plan_references_maps, hb_goal_to_target_maps and hb_cmd_vel_to_target_maps. The MPC, WBC, joint law and estimator do not read them. */
+
 /* state of the speed-based gait selection of one instance (SwitchedModelReferenceManager velAbsHistory_/velAvg_/gaitLevel_);
  * zero-initialise, then set gait_level = -1 ("no template chosen yet") or the level in force */
 typedef struct {
@@ -392,6 +411,7 @@ typedef struct {                 /* the bodies of one robot, relative to the nom
   double inertia_scale[11];      /* I' = inertia_scale[b] I_b, finite, > 0                                                         */
 } hb_link_variation;             /* 440 B */
 #define HB_SETTING_LINK_VARIATIONS 13         /* hb_link_variation for hb_rollout_set_link_variations (hb_check_setting_records)     */
+#define HB_SETTING_HEIGHT_MAPS 14             /* hb_terrain for hb_plan_set_maps (hb_check_setting_records), the rules of _TERRAINS  */
 int hb_default_link_variation(hb_link_variation* r);      /* host only: every scale 1, every shift 0 */
 /* Sets the link variations of the context's episodes (a per-robot episode setting, above). -1 also for a value that is not finite, a
  * mass_scale <= 0 or an inertia_scale <= 0. */
@@ -399,7 +419,8 @@ int hb_rollout_set_link_variations(hb_ctx* ctx, int B, const hb_link_variation* 
 
 /* ---- terrain: the ground under each robot of the episodes, a height field on a regular world-frame grid ----
  * The terrain acts on the simulated plant and on the height failure check only; the planner, MPC, WBC, joint command law, actuation
- * model and estimator keep assuming flat ground at z = 0 and are not told about it (the estimator's feet_heights included).
+ * model and estimator keep assuming flat ground at z = 0 and are not told about it (the estimator's feet_heights included). The planner
+ * can be told where the ground is by a height map (height maps, above; hb_plan_set_maps), a record of this type set on its own.
  * Height and gradient at a world point (x, y): u = (x - origin[0]) / spacing clamped to [0, nx - 1], i = min(floor(u), nx - 2),
  * a = u - i; the same for y gives w, j and b. With lerp(p, q, s) = p + s (q - p): h0 = lerp(h[j][i], h[j][i+1], a),
  * h1 = lerp(h[j+1][i], h[j+1][i+1], a), h = lerp(h0, h1, b); g_x = lerp(h[j][i+1] - h[j][i], h[j+1][i+1] - h[j+1][i], b) / spacing,
@@ -793,6 +814,13 @@ int hb_plan_set_targets(hb_ctx* ctx, int B, const hb_target* targets);
  * stream order, B == 0 clears (settings may be NULL), -1 also for a record that is not valid, -4 for B > max_batch, a rejected call keeps
  * the previous setting. The setting adds no launch to any call. */
 int hb_plan_set_settings(hb_ctx* ctx, int B, const hb_planner_settings* settings);
+/* Height maps of the context (height maps, above): instance i < B of every device planner path -- hb_plan_references_batch_dev,
+ * hb_plan_references_gpu, hb_resident_plan_cycle_batch, hb_rollout_batch_dev and hb_rollout_estimated_batch_dev, the goal and teleop
+ * captures of the episodes included -- plans on maps[i]; instances at or beyond B, and every instance while none is set, plan without a
+ * map. The contract of hb_plan_set_settings: host array validated and copied in stream order, B == 0 clears (maps may be NULL), -1 for a
+ * record hb_rollout_set_terrains rejects, -4 for B > max_batch, a rejected call keeps the previous setting, no launch added. Maps are a
+ * setting, not episode state: snapshots do not hold them. */
+int hb_plan_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
 /* One estimator update per instance (StateEstimateBase::updateJointStates / updateImu, StateEstimateBase.cpp:73-106, then
  * KalmanFilterEstimate::update): quat = (x, y, z, w); contact_flag: B x 4 (0 = the filter distrusts that foot, x100 noise);
  * rbd_out: B x 32 measured rbd state [zyx, p, q_j, omega_world, v, qd_j]. zyxOffset_ is taken as zero. The odometry fusion
@@ -1105,6 +1133,10 @@ int hb_plan_references_targets(int B, const hb_plan_input* in, const hb_target* 
  * hb_plan_references_targets bit for bit. -1 also for a record that is not valid. */
 int hb_plan_references_settings(int B, const hb_plan_input* in, const hb_target* targets /*nullable*/, const hb_planner_settings* settings /*nullable*/,
                                 double* latest_stance, hb_reference* out);
+/* hb_plan_references_settings on height maps (height maps, above): maps (B, nullable), instance i plans on maps[i]. NULL maps is
+ * hb_plan_references_settings, and all-zero maps give it bit for bit. -1 also for a map hb_plan_set_maps rejects. */
+int hb_plan_references_maps(int B, const hb_plan_input* in, const hb_target* targets /*nullable*/, const hb_planner_settings* settings /*nullable*/,
+                            const hb_terrain* maps /*nullable*/, double* latest_stance, hb_reference* out);
 /* goalToTargetTrajectories (TargetTrajectoriesPublisher.cpp:83-100, with estimateTimeToTarget :29-38 and
  * targetPoseToTargetTrajectories :41-62) for the observation (t[i], x[i]) and goal[i] = (x, y, yaw), host only. With p = x[6:12] and
  * z' = p[2] + clamp(HB_COM_HEIGHT - p[2], -0.04, 0.04): sample 0 = (t, [0 (6), p[0], p[1], z', p[3], 0, 0, default joints]), sample 1 =
@@ -1113,11 +1145,19 @@ int hb_plan_references_settings(int B, const hb_plan_input* in, const hb_target*
  * reference: the goal yaw is absolute in the unwrapped convention of x[9]. T == 0 gives the single sample 1 at time t (n = 1) where the
  * reference would publish two samples at the same time. -1 for a NULL pointer, B < 0 or a non-finite t, x[6:10] or goal. */
 int hb_goal_to_target(int B, const double* t, const double* x /*B x 22*/, const double* goal /*B x 3*/, hb_target* out);
+/* hb_goal_to_target on height maps (B, nullable; height maps, above): the body heights of instance i's target are taken above maps[i].
+ * NULL is hb_goal_to_target; -1 also for a map hb_plan_set_maps rejects. */
+int hb_goal_to_target_maps(int B, const double* t, const double* x /*B x 22*/, const double* goal /*B x 3*/, const hb_terrain* maps /*nullable*/,
+                           hb_target* out);
 /* cmdVelToTargetTrajectories (TargetTrajectoriesPublisher.cpp:102-130) for the observation (t[i], x[i]) and cmd_vel[i] = (vx, vy, vz, yaw
  * rate), host only: the two-sample target the planner builds from cmd_vel with time_to_target = horizon (hb_plan_references with joint_ik
  * = 0 carries it bit for bit), the unused samples zero. The teleop messages' target (teleoperation, above). -1 for a NULL pointer, B < 0, a
  * non-finite t, horizon, x[6:12] or cmd_vel. */
 int hb_cmd_vel_to_target(int B, const double* t, double horizon, const double* x /*B x 22*/, const double* cmd_vel /*B x 4*/, hb_target* out);
+/* hb_cmd_vel_to_target on height maps (B, nullable; height maps, above): the body heights of instance i's target are taken above maps[i].
+ * NULL is hb_cmd_vel_to_target; -1 also for a map hb_plan_set_maps rejects. */
+int hb_cmd_vel_to_target_maps(int B, const double* t, double horizon, const double* x /*B x 22*/, const double* cmd_vel /*B x 4*/,
+                              const hb_terrain* maps /*nullable*/, hb_target* out);
 /* Host threads used by hb_plan_references (process-wide); 0 = hardware_concurrency. The result does not depend on the count. */
 int hb_plan_set_threads(int n_threads);
 /* speed-based gait selection (calculateVelAbs + walkGait / trotGait, src/SwitchedModelReferenceManager.cpp:185-249): updates the

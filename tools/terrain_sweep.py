@@ -26,6 +26,12 @@ flat and unset give the same outcome, and the card's name and power limit and th
 
 --estimator runs everything through hb_rollout_estimated_batch_dev (controllers on the Kalman filter's estimate from simulated sensors,
 noise = SCALE x episode_harness's NOISE_SIGMAS).
+
+--height-maps tells the planner where the ground is (hb_plan_set_maps): each robot's height map is its terrain minus the flat ground of
+0.02 m, so the planner plans on the terrain the plant stands on. The line then reports the blind and the mapped survival tables over the
+same cells and start poses, each with its largest magnitude at >= 90 % per kind, and times mapped episodes against the same terrain
+episodes with all-zero maps and blind (no map), alternately, with the launch counts of the three and whether zero maps gave the blind
+outcome.
 """
 import json
 import os
@@ -67,12 +73,63 @@ def terrain_heights(rbd0, kind, magnitude, step_ahead, ramp_ahead):
     return origin, GROUND + h
 
 
+def height_map_sweep(h, args, grid):
+    """--height-maps: the blind and the mapped sweep over the same cells, then mapped / zero-map / blind terrain episodes timed alternately.
+    grid(shift) gives the (origin, heights) of the terrains of assignment shift."""
+    hb, ctx, prm, B, rbd0 = h.hb, h.ctx, h.prm, h.B, h.rbd0
+    T_episode = TICKS * prm.period
+
+    def set_both(value):
+        terrains, maps = value
+        ctx.set_terrains(terrains)
+        ctx.set_height_maps(maps)
+
+    def settings(shift, mapped):
+        origin, heights = grid(shift)
+        return hb.make_terrains(B, heights, SPACING, origin), hb.make_terrains(B, heights - GROUND, SPACING, origin) if mapped else None
+
+    out, mk = {}, [str(m) for m in MAGNITUDES]
+    for name, mapped in (("blind", False), ("mapped", True)):
+        tally = Tally(len(MAGNITUDES), len(KINDS))
+        for r, run in h.sweep(set_both, lambda shift: settings(shift, mapped)):
+            tally.add(*cells(B, len(MAGNITUDES), len(KINDS), r), run.stats, value=np.hypot(*(run.rbd[:, 3:5] - rbd0[:, 3:5]).T) / T_episode)
+        out[name] = {"largest_magnitude_90pct": dict(zip(KINDS, tally.largest(MAGNITUDES))), "survival": keyed(KINDS, mk, tally.survival().tolist()),
+                     "mean_speed_of_survivors_m_per_s": keyed(KINDS, mk, tally.mean()), "fail_reasons": tally.reasons}
+    terrains, maps = settings(0, True)
+    origin, heights = grid(0)
+    zero = hb.make_terrains(B, np.zeros_like(heights), SPACING, origin)
+    _, clocks, timing = h.alternate(set_both, [("mapped", (terrains, maps)), ("zero_maps", (terrains, zero)), ("blind", (terrains, None))],
+                                    args.timed, launches=True)
+    set_both((None, None))
+    return out, clocks, timing
+
+
 def main():
-    args = sweep_args("terrain_sweep.py", "timed terrain / flat / unset episode triples", len(KINDS) * len(MAGNITUDES))
+    args = sweep_args("terrain_sweep.py", "timed terrain / flat / unset episode triples (with --height-maps: mapped / zero-map / blind)",
+                      len(KINDS) * len(MAGNITUDES),
+                      extra=lambda ap: ap.add_argument("--height-maps", action="store_true", help="also plan on maps of the terrains"))
     h = Episodes("terrain_sweep.py", args, TICKS)
     hb, ctx, prm, B, rbd0 = h.hb, h.ctx, h.prm, h.B, h.rbd0
     step_ahead, ramp_ahead = feature_distances(rbd0, h.feet)
     T_episode = TICKS * prm.period
+
+    if args.height_maps:
+        def grid(shift):
+            mi, ki = cells(B, len(MAGNITUDES), len(KINDS), shift)
+            return terrain_heights(rbd0, np.array(KINDS)[ki], np.array(MAGNITUDES)[mi], step_ahead, ramp_ahead)
+
+        out, clocks, timing = height_map_sweep(h, args, grid)
+        print(json.dumps({
+            "metric": "height maps: the highest step [cm] that >= 90 %% of the trotting robots cross within %.1f s when the planner is told "
+                      "the terrain; blind and mapped tables per kind (steps in cm, slopes in degrees)" % T_episode,
+            "value": out["mapped"]["largest_magnitude_90pct"]["step_up"], "unit": "cm", **report(args, clocks), **out, "timing": timing,
+            "config": {"workload": workload(h, "; %d kinds x %d magnitudes, %d episodes per table" % (len(KINDS), len(MAGNITUDES), args.repeats)),
+                       "terrain": "%d x %d height field at %g m centred on the start, ground %g m under the start; steps with the edge %g m "
+                                  "ahead (a ramp one cell wide), slopes starting %g m ahead, across the initial heading"
+                                  % (GRID, GRID, SPACING, GROUND, STEP_AHEAD, RAMP_AHEAD),
+                       "height_maps": "each robot's terrain minus %g m (hb_plan_set_maps); blind: no map" % GROUND,
+                       "survival": "robots still up at the end of the episode", "failure_checks": failure_checks("base z above the terrain")}}))
+        return
 
     def terrains(shift):
         mi, ki = cells(B, len(MAGNITUDES), len(KINDS), shift)
