@@ -60,7 +60,7 @@ EXPORTED_SYMBOLS = [
     "hb_default_link_variation", "hb_rollout_set_link_variations", "hb_sim_step_links",
     "hb_default_teleop_setting", "hb_rollout_set_teleop", "hb_cmd_vel_to_target",
     "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
-    "hb_plan_set_maps", "hb_plan_references_maps", "hb_goal_to_target_maps", "hb_cmd_vel_to_target_maps",
+    "hb_plan_set_maps", "hb_plan_references_maps", "hb_goal_to_target_maps", "hb_cmd_vel_to_target_maps", "hb_estimator_set_maps",
     "hb_check_setting_records", "hb_rollout_set_channel",
     "hb_episode_state_bytes", "hb_episode_save_async", "hb_episode_restore",
 ]
@@ -496,6 +496,7 @@ HB_TERRAIN_MAX = 64
 
 
 HEIGHT_MAPS_SETTING_KIND = 14     # HB_SETTING_HEIGHT_MAPS: HbTerrain records as planner height maps (Context.set_height_maps), for hb_check_setting_records
+ESTIMATOR_MAPS_SETTING_KIND = 15  # HB_SETTING_ESTIMATOR_MAPS: HbTerrain records as estimator maps (Context.set_estimator_maps), for hb_check_setting_records
 
 
 class HbTerrain(C.Structure):
@@ -1292,7 +1293,8 @@ class Context:
         return info, sol, tau, st, ps
 
     def estimator_update(self, dt, state, quat, ang_vel_local, lin_acc_local, joint_pos, joint_vel, contact_flag, params=None):
-        """KalmanFilterEstimate::update for a batch; `state` (ctypes array of HbKfState) is updated in place. Returns rbd [B,32]."""
+        """KalmanFilterEstimate::update for a batch; `state` (ctypes array of HbKfState) is updated in place. Instance i measures its feet
+        heights on this context's estimator map i (set_estimator_maps) when it has one, on state[i].feet_heights otherwise. Returns rbd [B,32]."""
         quat, ang_vel_local, lin_acc_local, joint_pos, joint_vel = map(_f64, (quat, ang_vel_local, lin_acc_local, joint_pos, joint_vel))
         B = quat.shape[0]
         flags = np.ascontiguousarray(contact_flag, dtype=np.uint8).reshape(B, 4)
@@ -1515,6 +1517,13 @@ class Context:
         included -- measured from the flat ground the planner otherwise assumes (a terrain H under a plant at sim.ground_height g is the map
         H - g); instances beyond len(maps) plan without one; None clears them."""
         self._set_instances("hb_plan_set_maps", maps)
+
+    def set_estimator_maps(self, maps):
+        """Estimator maps of this context (hb_estimator_set_maps): maps[i] (make_terrains) is the ground the Kalman filter of instance i
+        measures its feet heights on, in estimator_update and rollout_estimated, in place of its feet_heights; measured from the flat ground
+        the filter otherwise assumes, as height maps are (a terrain H under a plant at sim.ground_height g is the map H - g). Instances
+        beyond len(maps) run the filter without one; None clears them."""
+        self._set_instances("hb_estimator_set_maps", maps)
 
     def resident_wbc(self, t_now, rbd, stance_mode=None):
         """Policy of the resident solution at absolute time t_now + WeightedWbc: returns (x_des, u_des, mode, sol, torque, status)."""

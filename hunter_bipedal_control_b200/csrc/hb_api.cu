@@ -122,6 +122,8 @@ struct hb_ctx {
   InstanceSetting<hb_planner_settings> plan_settings;
   // each instance's height map in every device planner path (hb_plan_set_maps)
   InstanceSetting<hb_terrain> height_maps;
+  // each instance's estimator map in every estimator path: the Kalman filter's foot heights (hb_estimator_set_maps)
+  InstanceSetting<hb_terrain> estimator_maps;
   // the recorded channels of the episodes (hb_rollout_set_channel): the caller's buffer, its instances and rows; B == 0: unset
   struct { void* buf; int B, rows; } channels[HB_CHANNELS];
   // the episode snapshots' staging (hb_episode_save_async / hb_episode_restore), allocated at max_batch by their first call: the rows'
@@ -511,7 +513,7 @@ int hb_destroy(hb_ctx* ctx) {
   void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->tele_mem, ctx->snap_mem, ctx->arena,
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
                        ctx->odometry.dev, ctx->controllers.dev, ctx->hardware.dev, ctx->plan_settings.dev,
-                       ctx->bridges.dev, ctx->links.dev, ctx->height_maps.dev};
+                       ctx->bridges.dev, ctx->links.dev, ctx->height_maps.dev, ctx->estimator_maps.dev};
   for (void* p : mem) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -841,7 +843,7 @@ int hb_estimator_update_batch_dev(hb_ctx* ctx, int B, const hb_kf_params* params
                                   const uint8_t* contact_flag, double* rbd_out) {
   ENTER(ctx, B, params && state && quat && ang_vel_local && lin_acc_local && joint_pos && joint_vel && contact_flag && rbd_out, UNCAPPED);
   return launch(ctx, K_UNPROFILED, kf_update_kernel<hb_kf_state, false>, B, 32, sizeof(KfShared), B, *params, dt, state, quat, ang_vel_local, lin_acc_local,
-                joint_pos, joint_vel, contact_flag, rbd_out, (const double*)nullptr, (const uint8_t*)nullptr);
+                joint_pos, joint_vel, contact_flag, rbd_out, (const double*)nullptr, (const uint8_t*)nullptr, ctx->estimator_maps.view(ctx->base));
 }
 
 int hb_estimator_fuse_odometry_async(hb_ctx* ctx, int B, const hb_kf_params* params, hb_kf_state* state, const double* pos, const uint8_t* has_msg,
@@ -1301,6 +1303,8 @@ int hb_plan_set_settings(hb_ctx* ctx, int B, const hb_planner_settings* s) {
 
 int hb_plan_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps) { return set_instances(ctx, B, maps, terrain_ok, &hb_ctx::height_maps); }
 
+int hb_estimator_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps) { return set_instances(ctx, B, maps, terrain_ok, &hb_ctx::estimator_maps); }
+
 static bool latency_ok(const int32_t& d) { return d >= 0; }     // the upper bound is the episode's mpc_every, checked by the episode call
 
 int hb_rollout_set_mpc_latencies(hb_ctx* ctx, int B, const int32_t* ticks) { return set_instances(ctx, B, ticks, latency_ok, &hb_ctx::latencies); }
@@ -1414,6 +1418,7 @@ int hb_check_setting_records(int32_t kind, int B, const void* records, int32_t* 
     case HB_SETTING_TELEOP: return check_records(B, records, teleop_setting_ok, first_bad);
     case HB_SETTING_LINK_VARIATIONS: return check_records(B, records, link_variation_ok, first_bad);
     case HB_SETTING_HEIGHT_MAPS: return check_records(B, records, terrain_ok, first_bad);
+    case HB_SETTING_ESTIMATOR_MAPS: return check_records(B, records, terrain_ok, first_bad);
     default: return HB_EINVAL;
   }
 }
@@ -1634,7 +1639,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
                   e->est, ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag, odom_read);
       if (!rc) rc = launch(ctx, K_UNPROFILED, odom ? kf_update_kernel<hb_estimation_state, true> : kf_update_kernel<hb_estimation_state, false>, B, 32,
                            sizeof(KfShared), B, e->ep->kf, p->period, e->est, ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag,
-                           meas, (const double*)ctx->re_opos, (const uint8_t*)ctx->re_ohas);
+                           meas, (const double*)ctx->re_opos, (const uint8_t*)ctx->re_ohas, ctx->estimator_maps.view());
       if (!rc) rc = launch(ctx, K_UNPROFILED, est_observe_kernel, grid, 64, 0, B, rbd, meas, stats, e->est, e->stats, est_row, (size_t)n_est_log * 32);
     }
     // MPC_MRT_Interface::updatePolicy of the instances whose solution comes into force on this tick, before this tick's cycle

@@ -2,6 +2,7 @@
 // contact-force observer of StateEstimateBase. One warp per instance.
 #pragma once
 #include "hb_common.cuh"
+#include "hb_planner.h"
 #include "hb_qp.cuh"
 #include "hb_rbd.cuh"
 #include "../../include/hunter_b200.h"
@@ -46,10 +47,13 @@ __device__ __forceinline__ double odom_fused_state(int i, const double* pos, con
 // Odom (estimated episodes with hb_rollout_set_odometry): odom_pos / odom_has (B x 3 / B) are the odometry messages of the tick, and an
 // instance with odom_has[i] != 0 is fused after the filter step (odom_fused_state; feet heights of the contact feet follow, velocity and P
 // stay). Without Odom the pointers are not read and the kernel has no call to odom_contact_positions, whose call site costs registers.
+// maps: the estimator maps (hb_estimator_set_maps). An instance with a map measures foot c's height (row 24 + c) as the map's height under
+// the predicted foot, hbplan::map_height at x[6 + 3c], x[7 + 3c], in place of feet_heights[c], which it then does not read; the fusion
+// above still writes it.
 template <class State, bool Odom>
 __global__ void __launch_bounds__(32) kf_update_kernel(int B, hb_kf_params prm, double dt, State* state, const double* quat, const double* angl,
                                                        const double* accl, const double* jpos, const double* jvel, const uint8_t* cflag, double* rbd_out,
-                                                       const double* odom_pos, const uint8_t* odom_has) {
+                                                       const double* odom_pos, const uint8_t* odom_has, InstanceView<hb_terrain> maps) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   KfShared& sh = *reinterpret_cast<KfShared*>(smem_raw);
   const int inst = blockIdx.x, lane = threadIdx.x;
@@ -114,11 +118,13 @@ __global__ void __launch_bounds__(32) kf_update_kernel(int B, hb_kf_params prm, 
     if (r == c) s += sh.qd[r];
     sh.Pm[idx] = s;
   }
-  // innovation y - C x (:137-143): ps = -eePos (+ footRadius on z), vs = -eeVel, feet heights
+  // innovation y - C x (:137-143): ps = -eePos (+ footRadius on z), vs = -eeVel, feet heights (on a map: the ground under the predicted foot)
+  const hb_terrain* map = maps.of(inst);
   if (lane < 28) {
     double y;
     if (lane < 12) y = -ko.cpos[lane] + ((lane % 3) == 2 ? prm.foot_radius : 0.0);
     else if (lane < 24) y = -ko.cvel[lane - 12];
+    else if (map) y = hbplan::map_height(map, sh.x[6 + 3 * (lane - 24)], sh.x[7 + 3 * (lane - 24)]);
     else y = st.feet_heights[lane - 24];
     sh.ey[lane] = y - kf_c_row(sh.x, 1, lane, 0);
   }

@@ -162,7 +162,22 @@ int hb_parse_planner_settings(const char* task_info, const char* gait_info, hb_p
  *    target.
  * A map of zeros gives the plans and targets of no map bit for bit; an instance without a map plans as before. The IK joint references
  * follow the swing splines and the targets. Maps are read by every device planner path (hb_plan_set_maps) and by the host calls
- * hb_plan_references_maps, hb_goal_to_target_maps and hb_cmd_vel_to_target_maps. The MPC, WBC, joint law and estimator do not read them. */
+ * hb_plan_references_maps, hb_goal_to_target_maps and hb_cmd_vel_to_target_maps. The MPC, WBC, joint law and estimator do not read them;
+ * the estimator is told about the ground by estimator maps (below), records of this type set on their own. */
+
+/* ---- estimator maps: the ground the Kalman filter is told about, its feet heights as a function of (x, y) ----
+ * An estimator map is an hb_terrain record that the filter reads; the reference measures each foot's height as feetHeights_, zero unless
+ * updateFromTopic writes it (LinearKalmanFilter.cpp:62, 143, 227). For an instance with a map m, the update's measurement row 24 + c is
+ * y = h_m(x[6 + 3c], x[7 + 3c]) at the predicted state x (the prediction does not move the feet: the previous estimate's foot xy), with h_m
+ * the height-map lookup (height maps, above; the same bits on the host and the device). C, R, Q and the decoupling do not change, and the
+ * row stays the foot's z: it has no -grad h . (x, y) coupling (no linearisation of the ground; the foot xy is measured kinematically by
+ * rows 0..11, and a step of the map is a one-cell ramp whose gradient would make such a row jump between ticks). Map heights are measured
+ * from the ground the filter otherwise assumes (z = 0), as a height map's: over a plant whose flat ground is at g the map of a terrain H is
+ * H - g, so one record serves both settings. A mapped update does not read feet_heights; the odometry fusion still writes it, and with a
+ * camera and a map the map wins. An all-zero map is the filter without one bit for bit while feet_heights is +0 (every episode without
+ * odometry: hb_kf_reset sets +0 and only the fusion writes it). Maps are read by hb_estimator_update_batch_dev, hb_estimator_update_batch
+ * and hb_rollout_estimated_batch_dev (hb_estimator_set_maps); the truth episodes, the planner, the plant and hb_estimator_fuse_odometry
+ * do not read them. */
 
 /* state of the speed-based gait selection of one instance (SwitchedModelReferenceManager velAbsHistory_/velAvg_/gaitLevel_);
  * zero-initialise, then set gait_level = -1 ("no template chosen yet") or the level in force */
@@ -187,7 +202,7 @@ typedef struct {
 typedef struct {
   double x_hat[18];        /* base position(3), base linear velocity(3), four contact positions(12), world frame */
   double P[18 * 18];       /* covariance, row-major                                                              */
-  double feet_heights[4];  /* terrain height under each contact (measurement rows 24..27)                        */
+  double feet_heights[4];  /* terrain height under each contact (measurement rows 24..27; not read on an estimator map) */
 } hb_kf_state;
 
 typedef struct {           /* task.info:336-345 */
@@ -412,6 +427,7 @@ typedef struct {                 /* the bodies of one robot, relative to the nom
 } hb_link_variation;             /* 440 B */
 #define HB_SETTING_LINK_VARIATIONS 13         /* hb_link_variation for hb_rollout_set_link_variations (hb_check_setting_records)     */
 #define HB_SETTING_HEIGHT_MAPS 14             /* hb_terrain for hb_plan_set_maps (hb_check_setting_records), the rules of _TERRAINS  */
+#define HB_SETTING_ESTIMATOR_MAPS 15          /* hb_terrain for hb_estimator_set_maps (hb_check_setting_records), as _TERRAINS      */
 int hb_default_link_variation(hb_link_variation* r);      /* host only: every scale 1, every shift 0 */
 /* Sets the link variations of the context's episodes (a per-robot episode setting, above). -1 also for a value that is not finite, a
  * mass_scale <= 0 or an inertia_scale <= 0. */
@@ -419,8 +435,9 @@ int hb_rollout_set_link_variations(hb_ctx* ctx, int B, const hb_link_variation* 
 
 /* ---- terrain: the ground under each robot of the episodes, a height field on a regular world-frame grid ----
  * The terrain acts on the simulated plant and on the height failure check only; the planner, MPC, WBC, joint command law, actuation
- * model and estimator keep assuming flat ground at z = 0 and are not told about it (the estimator's feet_heights included). The planner
- * can be told where the ground is by a height map (height maps, above; hb_plan_set_maps), a record of this type set on its own.
+ * model and estimator keep assuming flat ground at z = 0 and are not told about it. The planner can be told where the ground is by a
+ * height map (height maps, above; hb_plan_set_maps) and the estimator's feet heights by an estimator map (estimator maps, above;
+ * hb_estimator_set_maps), records of this type each set on its own.
  * Height and gradient at a world point (x, y): u = (x - origin[0]) / spacing clamped to [0, nx - 1], i = min(floor(u), nx - 2),
  * a = u - i; the same for y gives w, j and b. With lerp(p, q, s) = p + s (q - p): h0 = lerp(h[j][i], h[j][i+1], a),
  * h1 = lerp(h[j+1][i], h[j+1][i+1], a), h = lerp(h0, h1, b); g_x = lerp(h[j][i+1] - h[j][i], h[j+1][i+1] - h[j+1][i], b) / spacing,
@@ -821,10 +838,18 @@ int hb_plan_set_settings(hb_ctx* ctx, int B, const hb_planner_settings* settings
  * record hb_rollout_set_terrains rejects, -4 for B > max_batch, a rejected call keeps the previous setting, no launch added. Maps are a
  * setting, not episode state: snapshots do not hold them. */
 int hb_plan_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
+/* Estimator maps of the context (estimator maps, above): instance i < B of every estimator path -- hb_estimator_update_batch_dev,
+ * hb_estimator_update_batch and hb_rollout_estimated_batch_dev -- measures its feet heights on maps[i]; instances at or beyond B, and every
+ * instance while none is set, run the filter without a map. One setting serves the public filter call and the episode, so an estimated
+ * episode can be written as a loop of public calls. The contract of hb_plan_set_maps: host array validated and copied in stream order,
+ * B == 0 clears (maps may be NULL), -1 for a record hb_rollout_set_terrains rejects, -4 for B > max_batch, a rejected call keeps the
+ * previous setting, no launch added. Maps are a setting, not episode state: hb_episode_state_bytes and snapshots do not count them. */
+int hb_estimator_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
 /* One estimator update per instance (StateEstimateBase::updateJointStates / updateImu, StateEstimateBase.cpp:73-106, then
  * KalmanFilterEstimate::update): quat = (x, y, z, w); contact_flag: B x 4 (0 = the filter distrusts that foot, x100 noise);
  * rbd_out: B x 32 measured rbd state [zyx, p, q_j, omega_world, v, qd_j]. zyxOffset_ is taken as zero. The odometry fusion
- * (updateFromTopic) is a call of its own, hb_estimator_fuse_odometry_async, applied after this one. */
+ * (updateFromTopic) is a call of its own, hb_estimator_fuse_odometry_async, applied after this one. Instance i measures its feet heights
+ * on the context's estimator map i (hb_estimator_set_maps) when it has one, and on state[i].feet_heights otherwise. */
 int hb_estimator_update_batch_dev(hb_ctx* ctx, int B, const hb_kf_params* params, double dt, hb_kf_state* state, const double* quat,
                                   const double* ang_vel_local, const double* lin_acc_local, const double* joint_pos,
                                   const double* joint_vel, const uint8_t* contact_flag, double* rbd_out);
@@ -879,7 +904,8 @@ int hb_sim_read_sensors_batch_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noi
  * actuation, saturation, the plant and the failure checks the true one. est (B) is in/out; est_stats (B, nullable) in/out; est_log
  * (nullable) the estimated rbd in log's layout. Arguments are checked before any launch (sigmas finite and >= 0). With odometry set
  * (hb_rollout_set_odometry), the sensor read also reads each camera and the filter fuses the messages due on the tick. With a hardware
- * setting (hb_rollout_set_hardware), each robot's actuation, saturation and sensors run on its record. */
+ * setting (hb_rollout_set_hardware), each robot's actuation, saturation and sensors run on its record. The filter measures each robot's
+ * feet heights on its estimator map (hb_estimator_set_maps) when it has one, as hb_estimator_update_batch_dev does. */
 int hb_rollout_estimated_batch_dev(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb_rollout_params* p, const hb_estimation_params* ep,
                                    const hb_rollout_command* cmd, double* rbd, hb_actuation_state* act, uint8_t* estop, hb_rollout_stats* stats,
                                    hb_estimation_state* est, hb_estimation_stats* est_stats /*nullable*/, double* log /*nullable*/,

@@ -32,6 +32,12 @@ noise = SCALE x episode_harness's NOISE_SIGMAS).
 same cells and start poses, each with its largest magnitude at >= 90 % per kind, and times mapped episodes against the same terrain
 episodes with all-zero maps and blind (no map), alternately, with the launch counts of the three and whether zero maps gave the blind
 outcome.
+
+--estimator-maps (with --height-maps --estimator) also tells the Kalman filter where the ground is (hb_estimator_set_maps), with the same
+maps, so that it measures each foot's height on the terrain instead of at z = 0. Planner maps and estimator maps are separate settings:
+the line reports four tables over the same cells and start poses -- blind, planner maps only, estimator maps only, both -- and times
+episodes with both maps against planner maps with all-zero estimator maps and planner maps only, alternately; the tool asserts that
+all-zero estimator maps give the outcome of planner maps only bit for bit.
 """
 import json
 import os
@@ -74,40 +80,55 @@ def terrain_heights(rbd0, kind, magnitude, step_ahead, ramp_ahead):
 
 
 def height_map_sweep(h, args, grid):
-    """--height-maps: the blind and the mapped sweep over the same cells, then mapped / zero-map / blind terrain episodes timed alternately.
+    """--height-maps: the blind and the mapped sweep over the same cells, then mapped / zero-map / blind terrain episodes timed alternately;
+    with --estimator-maps the four tables (blind, planner maps, estimator maps, both), then both / zero estimator maps / planner maps only.
     grid(shift) gives the (origin, heights) of the terrains of assignment shift."""
     hb, ctx, prm, B, rbd0 = h.hb, h.ctx, h.prm, h.B, h.rbd0
     T_episode = TICKS * prm.period
 
-    def set_both(value):
-        terrains, maps = value
+    def set_all(value):
+        terrains, maps, est_maps = value
         ctx.set_terrains(terrains)
         ctx.set_height_maps(maps)
+        ctx.set_estimator_maps(est_maps)
 
-    def settings(shift, mapped):
+    def settings(shift, planner, estimator):
         origin, heights = grid(shift)
-        return hb.make_terrains(B, heights, SPACING, origin), hb.make_terrains(B, heights - GROUND, SPACING, origin) if mapped else None
+        maps = hb.make_terrains(B, heights - GROUND, SPACING, origin)
+        return hb.make_terrains(B, heights, SPACING, origin), maps if planner else None, maps if estimator else None
 
+    tables = [("blind", False, False), ("mapped", True, False)]
+    if args.estimator_maps:
+        tables = [("blind", False, False), ("planner_maps", True, False), ("estimator_maps", False, True), ("both_maps", True, True)]
     out, mk = {}, [str(m) for m in MAGNITUDES]
-    for name, mapped in (("blind", False), ("mapped", True)):
+    for name, planner, estimator in tables:
         tally = Tally(len(MAGNITUDES), len(KINDS))
-        for r, run in h.sweep(set_both, lambda shift: settings(shift, mapped)):
+        for r, run in h.sweep(set_all, lambda shift: settings(shift, planner, estimator)):
             tally.add(*cells(B, len(MAGNITUDES), len(KINDS), r), run.stats, value=np.hypot(*(run.rbd[:, 3:5] - rbd0[:, 3:5]).T) / T_episode)
         out[name] = {"largest_magnitude_90pct": dict(zip(KINDS, tally.largest(MAGNITUDES))), "survival": keyed(KINDS, mk, tally.survival().tolist()),
                      "mean_speed_of_survivors_m_per_s": keyed(KINDS, mk, tally.mean()), "fail_reasons": tally.reasons}
-    terrains, maps = settings(0, True)
+    terrains, maps, _ = settings(0, True, True)
     origin, heights = grid(0)
     zero = hb.make_terrains(B, np.zeros_like(heights), SPACING, origin)
-    _, clocks, timing = h.alternate(set_both, [("mapped", (terrains, maps)), ("zero_maps", (terrains, zero)), ("blind", (terrains, None))],
-                                    args.timed, launches=True)
-    set_both((None, None))
+    if args.estimator_maps:
+        _, clocks, timing = h.alternate(set_all, [("both_maps", (terrains, maps, maps)), ("zero_estimator_maps", (terrains, maps, zero)),
+                                                  ("planner_maps", (terrains, maps, None))], args.timed, launches=True)
+        assert timing["zero_estimator_maps_same_outcome_as_planner_maps"], "all-zero estimator maps changed the outcome of planner maps only"
+    else:
+        _, clocks, timing = h.alternate(set_all, [("mapped", (terrains, maps, None)), ("zero_maps", (terrains, zero, None)),
+                                                  ("blind", (terrains, None, None))], args.timed, launches=True)
+    set_all((None, None, None))
     return out, clocks, timing
 
 
 def main():
+    def extra(ap):
+        ap.add_argument("--height-maps", action="store_true", help="also plan on maps of the terrains")
+        ap.add_argument("--estimator-maps", action="store_true", help="with --height-maps --estimator: also give the Kalman filter the maps")
+
     args = sweep_args("terrain_sweep.py", "timed terrain / flat / unset episode triples (with --height-maps: mapped / zero-map / blind)",
-                      len(KINDS) * len(MAGNITUDES),
-                      extra=lambda ap: ap.add_argument("--height-maps", action="store_true", help="also plan on maps of the terrains"))
+                      len(KINDS) * len(MAGNITUDES), extra=extra, valid=lambda a: not a.estimator_maps or (a.height_maps and a.estimator),
+                      needs="--estimator-maps needs --height-maps --estimator, ")
     h = Episodes("terrain_sweep.py", args, TICKS)
     hb, ctx, prm, B, rbd0 = h.hb, h.ctx, h.prm, h.B, h.rbd0
     step_ahead, ramp_ahead = feature_distances(rbd0, h.feet)
@@ -119,15 +140,23 @@ def main():
             return terrain_heights(rbd0, np.array(KINDS)[ki], np.array(MAGNITUDES)[mi], step_ahead, ramp_ahead)
 
         out, clocks, timing = height_map_sweep(h, args, grid)
+        if args.estimator_maps:
+            metric = ("estimator maps: the highest step [cm] that >= 90 %% of the trotting robots cross within %.1f s through the estimator "
+                      "when the planner and the Kalman filter are told the terrain; blind, planner-map, estimator-map and both-map tables per "
+                      "kind (steps in cm, slopes in degrees)" % T_episode)
+            value = out["both_maps"]["largest_magnitude_90pct"]["step_up"]
+        else:
+            metric = ("height maps: the highest step [cm] that >= 90 %% of the trotting robots cross within %.1f s when the planner is told "
+                      "the terrain; blind and mapped tables per kind (steps in cm, slopes in degrees)" % T_episode)
+            value = out["mapped"]["largest_magnitude_90pct"]["step_up"]
         print(json.dumps({
-            "metric": "height maps: the highest step [cm] that >= 90 %% of the trotting robots cross within %.1f s when the planner is told "
-                      "the terrain; blind and mapped tables per kind (steps in cm, slopes in degrees)" % T_episode,
-            "value": out["mapped"]["largest_magnitude_90pct"]["step_up"], "unit": "cm", **report(args, clocks), **out, "timing": timing,
+            "metric": metric, "value": value, "unit": "cm", **report(args, clocks), **out, "timing": timing,
             "config": {"workload": workload(h, "; %d kinds x %d magnitudes, %d episodes per table" % (len(KINDS), len(MAGNITUDES), args.repeats)),
                        "terrain": "%d x %d height field at %g m centred on the start, ground %g m under the start; steps with the edge %g m "
                                   "ahead (a ramp one cell wide), slopes starting %g m ahead, across the initial heading"
                                   % (GRID, GRID, SPACING, GROUND, STEP_AHEAD, RAMP_AHEAD),
-                       "height_maps": "each robot's terrain minus %g m (hb_plan_set_maps); blind: no map" % GROUND,
+                       "height_maps": "each robot's terrain minus %g m (hb_plan_set_maps%s); blind: no map"
+                                      % (GROUND, ", and the same maps with hb_estimator_set_maps" if args.estimator_maps else ""),
                        "survival": "robots still up at the end of the episode", "failure_checks": failure_checks("base z above the terrain")}}))
         return
 
