@@ -61,6 +61,7 @@ EXPORTED_SYMBOLS = [
     "hb_default_teleop_setting", "hb_rollout_set_teleop", "hb_cmd_vel_to_target",
     "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
     "hb_plan_set_maps", "hb_plan_references_maps", "hb_goal_to_target_maps", "hb_cmd_vel_to_target_maps", "hb_estimator_set_maps",
+    "hb_mpc_set_maps",
     "hb_check_setting_records", "hb_rollout_set_channel",
     "hb_episode_state_bytes", "hb_episode_save_async", "hb_episode_restore",
 ]
@@ -497,6 +498,7 @@ HB_TERRAIN_MAX = 64
 
 HEIGHT_MAPS_SETTING_KIND = 14     # HB_SETTING_HEIGHT_MAPS: HbTerrain records as planner height maps (Context.set_height_maps), for hb_check_setting_records
 ESTIMATOR_MAPS_SETTING_KIND = 15  # HB_SETTING_ESTIMATOR_MAPS: HbTerrain records as estimator maps (Context.set_estimator_maps), for hb_check_setting_records
+MPC_MAPS_SETTING_KIND = 17        # HB_SETTING_MPC_MAPS: HbTerrain records as MPC maps (Context.set_mpc_maps), for hb_check_setting_records
 
 
 class HbTerrain(C.Structure):
@@ -1524,6 +1526,13 @@ class Context:
         the filter otherwise assumes, as height maps are (a terrain H under a plant at sim.ground_height g is the map H - g). Instances
         beyond len(maps) run the filter without one; None clears them."""
         self._set_instances("hb_estimator_set_maps", maps)
+
+    def set_mpc_maps(self, maps):
+        """MPC maps of this context (hb_mpc_set_maps): maps[i] (make_terrains) is the ground the MPC of instance i holds its stance feet on,
+        in every MPC path (mpc_solve, control_step, the resident cycles, rollout and rollout_estimated): the stance z row pulls each stance
+        contact to 0.02 + h at its swing reference's (x, y). Measured from the flat ground the MPC otherwise assumes, as height maps are.
+        Instances beyond len(maps) solve without one; None clears them."""
+        self._set_instances("hb_mpc_set_maps", maps)
 
     def resident_wbc(self, t_now, rbd, stance_mode=None):
         """Policy of the resident solution at absolute time t_now + WeightedWbc: returns (x_des, u_des, mode, sol, torque, status)."""

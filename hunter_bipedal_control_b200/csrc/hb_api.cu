@@ -124,6 +124,10 @@ struct hb_ctx {
   InstanceSetting<hb_terrain> height_maps;
   // each instance's estimator map in every estimator path: the Kalman filter's foot heights (hb_estimator_set_maps)
   InstanceSetting<hb_terrain> estimator_maps;
+  // each instance's MPC map in every MPC path: the ground under the stance feet (hb_mpc_set_maps), and the heights a solve looks up on
+  // them (B x (N+1) x 4, allocated at max_batch by the first solve with a map set)
+  InstanceSetting<hb_terrain> mpc_maps;
+  void* sth_mem; double* sth;
   // the recorded channels of the episodes (hb_rollout_set_channel): the caller's buffer, its instances and rows; B == 0: unset
   struct { void* buf; int B, rows; } channels[HB_CHANNELS];
   // the episode snapshots' staging (hb_episode_save_async / hb_episode_restore), allocated at max_batch by their first call: the rows'
@@ -513,7 +517,8 @@ int hb_destroy(hb_ctx* ctx) {
   void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->tele_mem, ctx->snap_mem, ctx->arena,
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
                        ctx->odometry.dev, ctx->controllers.dev, ctx->hardware.dev, ctx->plan_settings.dev,
-                       ctx->bridges.dev, ctx->links.dev, ctx->height_maps.dev, ctx->estimator_maps.dev};
+                       ctx->bridges.dev, ctx->links.dev, ctx->height_maps.dev, ctx->estimator_maps.dev,
+                       ctx->mpc_maps.dev, ctx->sth_mem};
   for (void* p : mem) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -672,8 +677,15 @@ static int mpc_solve_impl(hb_ctx* ctx, int B, const double* x0, const double* x_
     return off;
   });
   if (rc) return rc;
+  // the stance heights on the MPC maps, which K1 looks up and K3 reads: their storage, only while a map is set (no launch)
+  const InstanceView<hb_terrain> maps = ctx->mpc_maps.view(ctx->base);
+  if (maps.recs) {
+    rc = reserve_group(&ctx->sth_mem, [&](void* m) { size_t off = 0; ctx->sth = carve<double>(m, off, Bc * (Nc + 1) * 4); return off; });
+    if (rc) return rc;
+  }
   SqpArgs a;
   a.tk = tk; a.nn = nn;
+  a.maps = maps; a.sth = maps.recs ? ctx->sth + (size_t)ctx->base * (Nc + 1) * 4 : nullptr;
   a.B = B; a.N = ctx->cfg.horizon_N; a.dt = ctx->cfg.dt; a.x_ref = x_ref; a.swing = swing_ref; a.mode = mode; a.xt = x_traj; a.ut = u_traj;
   {
     const size_t o = (size_t)ctx->base, Nn = (size_t)ctx->cfg.horizon_N;
@@ -1305,6 +1317,8 @@ int hb_plan_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps) { return set_in
 
 int hb_estimator_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps) { return set_instances(ctx, B, maps, terrain_ok, &hb_ctx::estimator_maps); }
 
+int hb_mpc_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps) { return set_instances(ctx, B, maps, terrain_ok, &hb_ctx::mpc_maps); }
+
 static bool latency_ok(const int32_t& d) { return d >= 0; }     // the upper bound is the episode's mpc_every, checked by the episode call
 
 int hb_rollout_set_mpc_latencies(hb_ctx* ctx, int B, const int32_t* ticks) { return set_instances(ctx, B, ticks, latency_ok, &hb_ctx::latencies); }
@@ -1419,6 +1433,7 @@ int hb_check_setting_records(int32_t kind, int B, const void* records, int32_t* 
     case HB_SETTING_LINK_VARIATIONS: return check_records(B, records, link_variation_ok, first_bad);
     case HB_SETTING_HEIGHT_MAPS: return check_records(B, records, terrain_ok, first_bad);
     case HB_SETTING_ESTIMATOR_MAPS: return check_records(B, records, terrain_ok, first_bad);
+    case HB_SETTING_MPC_MAPS: return check_records(B, records, terrain_ok, first_bad);
     default: return HB_EINVAL;
   }
 }

@@ -200,9 +200,10 @@ struct BarrierSum {
   __device__ __forceinline__ double value(double mu) const { return mu * (quad - log(prod)); }
 };
 
-// Stage cost (unscaled) and equality-constraint values of one node, one lane = one node (values only).
+// Stage cost (unscaled) and equality-constraint values of one node, one lane = one node (values only). sth (nullable): the node's four
+// stance heights on an MPC map (SqpArgs::sth), which the stance z rows subtract as K1's do.
 __device__ inline void node_values_lane(const double* x, const double* u, const double* xref, const double* swing, int mode,
-                                        const double* epos, const double* evel, double& cost, double& eq_sq) {
+                                        const double* epos, const double* evel, const double* sth, double& cost, double& eq_sq) {
   const Model& md = c_model;
   bool fl[4]; int ns = 0;
   for (int c = 0; c < 4; ++c) { fl[c] = contact_flag(mode, c); ns += fl[c]; }
@@ -220,7 +221,9 @@ __device__ inline void node_values_lane(const double* x, const double* u, const 
       const double Fx = u[3 * c], Fy = u[3 * c + 1], Fz = u[3 * c + 2];
       const double h = HB_FRICTION_MU * Fz - sqrt(Fx * Fx + Fy * Fy + HB_FRICTION_REGULARIZATION);
       fric.add(h, HB_FRICTION_BARRIER_DELTA);
-      const double e0 = evel[3 * c], e1 = evel[3 * c + 1], e2z = evel[3 * c + 2] + HB_ZEROVEL_Z_GAIN * epos[3 * c + 2] + HB_ZEROVEL_Z_OFFSET;
+      const double e0 = evel[3 * c], e1 = evel[3 * c + 1];
+      double e2z = evel[3 * c + 2] + HB_ZEROVEL_Z_GAIN * epos[3 * c + 2] + HB_ZEROVEL_Z_OFFSET;
+      if (sth) e2z -= HB_ZEROVEL_Z_GAIN * sth[c];
       e2 += e0 * e0 + e1 * e1 + e2z * e2z;
     } else {
       for (int a = 0; a < 2; ++a) {

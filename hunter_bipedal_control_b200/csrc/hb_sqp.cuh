@@ -18,6 +18,7 @@
 #pragma once
 #include "hb_common.cuh"
 #include "hb_mpc.cuh"
+#include "hb_planner.h"
 #include "hb_rbd.cuh"
 
 namespace hb {
@@ -301,7 +302,25 @@ struct SqpArgs {
   // time discretisation (row S1): node times tk (B x (N+1)) and active interval counts nn (B) of a grid with event nodes; both null =
   // uniform grid of N intervals of length dt. N stays the capacity (stride) of every per-node array.
   const double* tk; const int32_t* nn;
+  // MPC maps (hb_mpc_set_maps): each instance's map, and sth, B x (N+1) x 4 ground heights under the stance contacts of each node. K1
+  // looks the heights up (stance_height_lane) and writes them for K3; both stance z rows subtract them. sth is null while no map is set,
+  // and then no kernel reads either.
+  InstanceView<hb_terrain> maps;
+  double* sth;
 };
+
+// The ground under stance contact `lane` (< 4) of node k on the instance's MPC map: hbplan::map_height at the swing reference's (x, y);
+// +0 for a swing contact or an instance without a map (a +0 height leaves the stance z row's bits as they are without one). Stored to
+// sth for K3's stance z rows; lanes >= 4 return 0 and store nothing. Read only while a.sth is set.
+__device__ __forceinline__ double stance_height_lane(const SqpArgs& a, int inst, int k, int lane, unsigned flm, const double* swing) {
+  double h = 0.0;
+  if (lane < 4) {
+    const hb_terrain* m = a.maps.of(inst);
+    if (m && ((flm >> lane) & 1u)) h = hbplan::map_height(m, swing[6 * lane], swing[6 * lane + 1]);
+    a.sth[((size_t)inst * (a.N + 1) + k) * 4 + lane] = h;
+  }
+  return h;
+}
 __device__ __forceinline__ int sqp_nn(const SqpArgs& a, int inst) { return a.nn ? a.nn[inst] : a.N; }
 __device__ __forceinline__ double sqp_dt(const SqpArgs& a, int inst, int k) {
   if (!a.tk) return a.dt;
@@ -615,12 +634,16 @@ __device__ __forceinline__ void lq_node(LqShared& sh, const SqpArgs& a, int inst
     }
   }
   __syncwarp();
+  double hrow = 0.0;      // on an MPC map: the ground under the contact of this lane's row (lane < MR)
+  if (a.sth) hrow = __shfl_sync(HB_FULL_MASK, stance_height_lane(a, inst, k, lane, flm, sh.swing), lane < MR ? sh.rowi[lane] / 3 : 0);
   double e2 = 0.0;
   if (lane < MR) {
     const int row = sh.rowi[lane], c = row / 3, ax = row - 3 * c;
     double evv;
-    if ((flm >> c) & 1u) evv = evel[row] + (ax == 2 ? HB_ZEROVEL_Z_GAIN * epos[row] + HB_ZEROVEL_Z_OFFSET : 0.0);
-    else evv = evel[row] - sh.swing[6 * c + 5] + HB_POSITION_ERROR_GAIN * (epos[row] - sh.swing[6 * c + 2]);
+    if ((flm >> c) & 1u) {
+      evv = evel[row] + (ax == 2 ? HB_ZEROVEL_Z_GAIN * epos[row] + HB_ZEROVEL_Z_OFFSET : 0.0);
+      if (ax == 2 && a.sth) evv -= HB_ZEROVEL_Z_GAIN * hrow;       // held at 0.02 + h on a map
+    } else evv = evel[row] - sh.swing[6 * c + 5] + HB_POSITION_ERROR_GAIN * (epos[row] - sh.swing[6 * c + 2]);
     sh.ev[lane] = evv;
     e2 = evv * evv;
   }
@@ -1506,7 +1529,7 @@ __global__ void __launch_bounds__(32) forward_linesearch2_kernel(SqpArgs a, int 
         double d2 = 0.0;
         for (int i = 0; i < NX; ++i) { const double d = x[i] + 0.5 * dt * (f1[i] + f2[i]) - xn[i]; d2 += d * d; }
         double cost, e2;
-        node_values_lane(x, u, xr, sw, mode[k], ep, ev, cost, e2);
+        node_values_lane(x, u, xr, sw, mode[k], ep, ev, a.sth ? a.sth + ((size_t)inst * (NS + 1) + k) * 4 : nullptr, cost, e2);
         ms += dt * cost; ds += dt * d2; es += dt * e2;
       }
       ms = warp_sum(ms); ds = warp_sum(ds); es = warp_sum(es);

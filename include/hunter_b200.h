@@ -179,6 +179,18 @@ int hb_parse_planner_settings(const char* task_info, const char* gait_info, hb_p
  * and hb_rollout_estimated_batch_dev (hb_estimator_set_maps); the truth episodes, the planner, the plant and hb_estimator_fuse_odometry
  * do not read them. */
 
+/* ---- MPC maps: the ground the MPC's stance feet are held on ----
+ * An MPC map is an hb_terrain record that the MPC's stance-foot equality reads. The reference's row (LeggedInterface.cpp:436-446) is
+ * v_c + diag(0, 0, 3) p_c + (0, 0, -0.06) = 0: its z row pulls every stance contact towards z = 0.02, flat ground. For an instance with a
+ * map m, at node k and each contact c in stance there, h = h_m(x, y) at the swing reference's position of c at the node (swing_ref[k][6c],
+ * [6c + 1]: for a stance phase the planner's stance position, the foot's current position for the current stance and the planned foothold
+ * for later ones), with h_m the height-map lookup (height maps, above; one record means the same ground to the planner, the filter and
+ * the MPC). The z row is then (v_z + 3 p_z - 0.06) - 3 h, so the stance foot is held at 0.02 + h; the linearisation's row and the line
+ * search's violation use the same h. h depends on the reference, not on the iterate: the row's Jacobian is unchanged and has no grad h
+ * coupling (a step of the map is a one-cell ramp, as for estimator maps). Swing rows, friction cones, costs, the WBC, the planner, the
+ * filter and the plant do not read MPC maps. An all-zero map (h = +0) is the solve without one bit for bit. Map heights are measured
+ * from the flat ground the MPC otherwise assumes (z = 0), as height maps' are. Maps are read by every MPC path (hb_mpc_set_maps). */
+
 /* state of the speed-based gait selection of one instance (SwitchedModelReferenceManager velAbsHistory_/velAvg_/gaitLevel_);
  * zero-initialise, then set gait_level = -1 ("no template chosen yet") or the level in force */
 typedef struct {
@@ -428,6 +440,7 @@ typedef struct {                 /* the bodies of one robot, relative to the nom
 #define HB_SETTING_LINK_VARIATIONS 13         /* hb_link_variation for hb_rollout_set_link_variations (hb_check_setting_records)     */
 #define HB_SETTING_HEIGHT_MAPS 14             /* hb_terrain for hb_plan_set_maps (hb_check_setting_records), the rules of _TERRAINS  */
 #define HB_SETTING_ESTIMATOR_MAPS 15          /* hb_terrain for hb_estimator_set_maps (hb_check_setting_records), as _TERRAINS      */
+#define HB_SETTING_MPC_MAPS 17                /* hb_terrain for hb_mpc_set_maps (hb_check_setting_records), as _TERRAINS; 16 unused */
 int hb_default_link_variation(hb_link_variation* r);      /* host only: every scale 1, every shift 0 */
 /* Sets the link variations of the context's episodes (a per-robot episode setting, above). -1 also for a value that is not finite, a
  * mass_scale <= 0 or an inertia_scale <= 0. */
@@ -436,8 +449,9 @@ int hb_rollout_set_link_variations(hb_ctx* ctx, int B, const hb_link_variation* 
 /* ---- terrain: the ground under each robot of the episodes, a height field on a regular world-frame grid ----
  * The terrain acts on the simulated plant and on the height failure check only; the planner, MPC, WBC, joint command law, actuation
  * model and estimator keep assuming flat ground at z = 0 and are not told about it. The planner can be told where the ground is by a
- * height map (height maps, above; hb_plan_set_maps) and the estimator's feet heights by an estimator map (estimator maps, above;
- * hb_estimator_set_maps), records of this type each set on its own.
+ * height map (height maps, above; hb_plan_set_maps), the estimator's feet heights by an estimator map (estimator maps, above;
+ * hb_estimator_set_maps) and the MPC's stance feet by an MPC map (MPC maps, above; hb_mpc_set_maps), records of this type each set on
+ * its own.
  * Height and gradient at a world point (x, y): u = (x - origin[0]) / spacing clamped to [0, nx - 1], i = min(floor(u), nx - 2),
  * a = u - i; the same for y gives w, j and b. With lerp(p, q, s) = p + s (q - p): h0 = lerp(h[j][i], h[j][i+1], a),
  * h1 = lerp(h[j+1][i], h[j+1][i+1], a), h = lerp(h0, h1, b); g_x = lerp(h[j][i+1] - h[j][i], h[j+1][i+1] - h[j+1][i], b) / spacing,
@@ -845,6 +859,15 @@ int hb_plan_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
  * B == 0 clears (maps may be NULL), -1 for a record hb_rollout_set_terrains rejects, -4 for B > max_batch, a rejected call keeps the
  * previous setting, no launch added. Maps are a setting, not episode state: hb_episode_state_bytes and snapshots do not count them. */
 int hb_estimator_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
+/* MPC maps of the context (MPC maps, above): instance i < B of every MPC path -- hb_mpc_solve_batch(_dev), hb_mpc_solve_grid_batch(_dev),
+ * hb_control_step_batch(_dev), hb_resident_cycle_batch(_dev), hb_resident_plan_cycle_batch (the MRT split's solves included),
+ * hb_rollout_batch_dev and hb_rollout_estimated_batch_dev -- holds its stance feet on maps[i]; instances at or beyond B, and every
+ * instance while none is set, solve without a map. One setting serves every path, so an episode can be written as a loop of public
+ * calls. The contract of hb_plan_set_maps: host array validated and copied in stream order, B == 0 clears (maps may be NULL), -1 for a
+ * record hb_rollout_set_terrains rejects, -4 for B > max_batch, a rejected call keeps the previous setting. While a map is set, each solve
+ * runs one more launch (the stance heights, once per solve); unset, the launches are those without the setting. Maps are a setting, not
+ * episode state: hb_episode_state_bytes and snapshots do not count them. */
+int hb_mpc_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
 /* One estimator update per instance (StateEstimateBase::updateJointStates / updateImu, StateEstimateBase.cpp:73-106, then
  * KalmanFilterEstimate::update): quat = (x, y, z, w); contact_flag: B x 4 (0 = the filter distrusts that foot, x100 noise);
  * rbd_out: B x 32 measured rbd state [zyx, p, q_j, omega_world, v, qd_j]. zyxOffset_ is taken as zero. The odometry fusion

@@ -38,6 +38,12 @@ maps, so that it measures each foot's height on the terrain instead of at z = 0.
 the line reports four tables over the same cells and start poses -- blind, planner maps only, estimator maps only, both -- and times
 episodes with both maps against planner maps with all-zero estimator maps and planner maps only, alternately; the tool asserts that
 all-zero estimator maps give the outcome of planner maps only bit for bit.
+
+--mpc-maps (with --height-maps) also holds the MPC's stance feet on the ground (hb_mpc_set_maps), with the same maps: the stance-foot
+constraint pulls each stance contact to 0.02 m above the map instead of z = 0.02. The line reports the tables above plus one with MPC maps
+added to every map the run gives (planner + MPC maps; with --estimator-maps all three), and times episodes with MPC maps against the same
+episodes with all-zero MPC maps and without MPC maps, alternately; the tool asserts that all-zero MPC maps give the outcome of no MPC maps
+bit for bit.
 """
 import json
 import os
@@ -87,37 +93,46 @@ def height_map_sweep(h, args, grid):
     T_episode = TICKS * prm.period
 
     def set_all(value):
-        terrains, maps, est_maps = value
+        terrains, maps, est_maps, mpc_maps = value
         ctx.set_terrains(terrains)
         ctx.set_height_maps(maps)
         ctx.set_estimator_maps(est_maps)
+        ctx.set_mpc_maps(mpc_maps)
 
-    def settings(shift, planner, estimator):
+    def settings(shift, planner, estimator, mpc=False):
         origin, heights = grid(shift)
         maps = hb.make_terrains(B, heights - GROUND, SPACING, origin)
-        return hb.make_terrains(B, heights, SPACING, origin), maps if planner else None, maps if estimator else None
+        return hb.make_terrains(B, heights, SPACING, origin), maps if planner else None, maps if estimator else None, maps if mpc else None
 
     tables = [("blind", False, False), ("mapped", True, False)]
     if args.estimator_maps:
         tables = [("blind", False, False), ("planner_maps", True, False), ("estimator_maps", False, True), ("both_maps", True, True)]
+    tables = [t + (False,) for t in tables]
+    if args.mpc_maps:
+        tables.append(("all_maps", True, True, True) if args.estimator_maps else ("planner_mpc_maps", True, False, True))
     out, mk = {}, [str(m) for m in MAGNITUDES]
-    for name, planner, estimator in tables:
+    for name, planner, estimator, mpc in tables:
         tally = Tally(len(MAGNITUDES), len(KINDS))
-        for r, run in h.sweep(set_all, lambda shift: settings(shift, planner, estimator)):
+        for r, run in h.sweep(set_all, lambda shift: settings(shift, planner, estimator, mpc)):
             tally.add(*cells(B, len(MAGNITUDES), len(KINDS), r), run.stats, value=np.hypot(*(run.rbd[:, 3:5] - rbd0[:, 3:5]).T) / T_episode)
         out[name] = {"largest_magnitude_90pct": dict(zip(KINDS, tally.largest(MAGNITUDES))), "survival": keyed(KINDS, mk, tally.survival().tolist()),
                      "mean_speed_of_survivors_m_per_s": keyed(KINDS, mk, tally.mean()), "fail_reasons": tally.reasons}
-    terrains, maps, _ = settings(0, True, True)
+    terrains, maps, _, _ = settings(0, True, True)
     origin, heights = grid(0)
     zero = hb.make_terrains(B, np.zeros_like(heights), SPACING, origin)
-    if args.estimator_maps:
-        _, clocks, timing = h.alternate(set_all, [("both_maps", (terrains, maps, maps)), ("zero_estimator_maps", (terrains, maps, zero)),
-                                                  ("planner_maps", (terrains, maps, None))], args.timed, launches=True)
+    if args.mpc_maps:
+        est = maps if args.estimator_maps else None
+        _, clocks, timing = h.alternate(set_all, [("mpc_maps", (terrains, maps, est, maps)), ("zero_mpc_maps", (terrains, maps, est, zero)),
+                                                  ("no_mpc_maps", (terrains, maps, est, None))], args.timed, launches=True)
+        assert timing["zero_mpc_maps_same_outcome_as_no_mpc_maps"], "all-zero MPC maps changed the outcome of no MPC maps"
+    elif args.estimator_maps:
+        _, clocks, timing = h.alternate(set_all, [("both_maps", (terrains, maps, maps, None)), ("zero_estimator_maps", (terrains, maps, zero, None)),
+                                                  ("planner_maps", (terrains, maps, None, None))], args.timed, launches=True)
         assert timing["zero_estimator_maps_same_outcome_as_planner_maps"], "all-zero estimator maps changed the outcome of planner maps only"
     else:
-        _, clocks, timing = h.alternate(set_all, [("mapped", (terrains, maps, None)), ("zero_maps", (terrains, zero, None)),
-                                                  ("blind", (terrains, None, None))], args.timed, launches=True)
-    set_all((None, None, None))
+        _, clocks, timing = h.alternate(set_all, [("mapped", (terrains, maps, None, None)), ("zero_maps", (terrains, zero, None, None)),
+                                                  ("blind", (terrains, None, None, None))], args.timed, launches=True)
+    set_all((None, None, None, None))
     return out, clocks, timing
 
 
@@ -125,10 +140,12 @@ def main():
     def extra(ap):
         ap.add_argument("--height-maps", action="store_true", help="also plan on maps of the terrains")
         ap.add_argument("--estimator-maps", action="store_true", help="with --height-maps --estimator: also give the Kalman filter the maps")
+        ap.add_argument("--mpc-maps", action="store_true", help="with --height-maps: also hold the MPC's stance feet on the maps")
 
     args = sweep_args("terrain_sweep.py", "timed terrain / flat / unset episode triples (with --height-maps: mapped / zero-map / blind)",
-                      len(KINDS) * len(MAGNITUDES), extra=extra, valid=lambda a: not a.estimator_maps or (a.height_maps and a.estimator),
-                      needs="--estimator-maps needs --height-maps --estimator, ")
+                      len(KINDS) * len(MAGNITUDES), extra=extra,
+                      valid=lambda a: (not a.estimator_maps or (a.height_maps and a.estimator)) and (not a.mpc_maps or a.height_maps),
+                      needs="--estimator-maps needs --height-maps --estimator, --mpc-maps needs --height-maps, ")
     h = Episodes("terrain_sweep.py", args, TICKS)
     hb, ctx, prm, B, rbd0 = h.hb, h.ctx, h.prm, h.B, h.rbd0
     step_ahead, ramp_ahead = feature_distances(rbd0, h.feet)
@@ -140,7 +157,14 @@ def main():
             return terrain_heights(rbd0, np.array(KINDS)[ki], np.array(MAGNITUDES)[mi], step_ahead, ramp_ahead)
 
         out, clocks, timing = height_map_sweep(h, args, grid)
-        if args.estimator_maps:
+        if args.mpc_maps:
+            last = "all_maps" if args.estimator_maps else "planner_mpc_maps"
+            metric = ("MPC maps: the highest step [cm] that >= 90 %% of the trotting robots cross within %.1f s%s when the planner%s and the "
+                      "MPC are told the terrain; %s tables per kind (steps in cm, slopes in degrees)"
+                      % (T_episode, " through the estimator" if args.estimator else "", ", the Kalman filter" if args.estimator_maps else "",
+                         ", ".join(out)))
+            value = out[last]["largest_magnitude_90pct"]["step_up"]
+        elif args.estimator_maps:
             metric = ("estimator maps: the highest step [cm] that >= 90 %% of the trotting robots cross within %.1f s through the estimator "
                       "when the planner and the Kalman filter are told the terrain; blind, planner-map, estimator-map and both-map tables per "
                       "kind (steps in cm, slopes in degrees)" % T_episode)
@@ -155,8 +179,9 @@ def main():
                        "terrain": "%d x %d height field at %g m centred on the start, ground %g m under the start; steps with the edge %g m "
                                   "ahead (a ramp one cell wide), slopes starting %g m ahead, across the initial heading"
                                   % (GRID, GRID, SPACING, GROUND, STEP_AHEAD, RAMP_AHEAD),
-                       "height_maps": "each robot's terrain minus %g m (hb_plan_set_maps%s); blind: no map"
-                                      % (GROUND, ", and the same maps with hb_estimator_set_maps" if args.estimator_maps else ""),
+                       "height_maps": "each robot's terrain minus %g m (hb_plan_set_maps%s%s); blind: no map"
+                                      % (GROUND, ", and the same maps with hb_estimator_set_maps" if args.estimator_maps else "",
+                                         ", and the same maps with hb_mpc_set_maps in the last table" if args.mpc_maps else ""),
                        "survival": "robots still up at the end of the episode", "failure_checks": failure_checks("base z above the terrain")}}))
         return
 
