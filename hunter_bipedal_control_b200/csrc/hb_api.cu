@@ -128,6 +128,8 @@ struct hb_ctx {
   // them (B x (N+1) x 4, allocated at max_batch by the first solve with a map set)
   InstanceSetting<hb_terrain> mpc_maps;
   void* sth_mem; double* sth;
+  // each instance's WBC map in every WBC path: the surface normals of the friction pyramids (hb_wbc_set_maps)
+  InstanceSetting<hb_terrain> wbc_maps;
   // the recorded channels of the episodes (hb_rollout_set_channel): the caller's buffer, its instances and rows; B == 0: unset
   struct { void* buf; int B, rows; } channels[HB_CHANNELS];
   // the episode snapshots' staging (hb_episode_save_async / hb_episode_restore), allocated at max_batch by their first call: the rows'
@@ -518,7 +520,7 @@ int hb_destroy(hb_ctx* ctx) {
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
                        ctx->odometry.dev, ctx->controllers.dev, ctx->hardware.dev, ctx->plan_settings.dev,
                        ctx->bridges.dev, ctx->links.dev, ctx->height_maps.dev, ctx->estimator_maps.dev,
-                       ctx->mpc_maps.dev, ctx->sth_mem};
+                       ctx->mpc_maps.dev, ctx->sth_mem, ctx->wbc_maps.dev};
   for (void* p : mem) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -595,7 +597,8 @@ using ControllerView = InstanceView<hb_controller_setting>;
 static int wbc_solve_impl(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
                           const uint8_t* stance_mode, double* sol, int32_t* status, ControllerView cs) {
   ENTER(ctx, B, x_des && u_des && rbd && mode && sol, CAPPED);
-  return launch(ctx, K_QP, wbc_fused_kernel, B, 32, wbc_fused_doubles() * sizeof(double), B, ctx->wbc, cs, x_des, u_des, rbd, mode, stance_mode,
+  return launch(ctx, K_QP, wbc_fused_kernel, B, 32, wbc_fused_doubles() * sizeof(double), B, ctx->wbc, cs, ctx->wbc_maps.view(ctx->base), x_des,
+                u_des, rbd, mode, stance_mode,
                 ctx->cfg.wbc_rho, ctx->cfg.qp_max_iter, sol, status ? status : ctx->wstatus + ctx->base, ctx->witers + ctx->base);
 }
 
@@ -608,8 +611,8 @@ int hb_wbc_assemble_batch_dev(hb_ctx* ctx, int B, const double* x_des, const dou
                               const uint8_t* stance_mode, double* H, double* g, double* A, double* lbA, double* ubA, int32_t* m_rows) {
   ENTER(ctx, B, x_des && u_des && rbd && mode && H && g && A && lbA && ubA && m_rows, UNCAPPED);
   const int wpb = 4;
-  return launch(ctx, K_WBC_ASSEMBLE, wbc_assemble_kernel, (B + wpb - 1) / wpb, 32 * wpb, sizeof(WbcShared) * wpb, B, ctx->wbc, x_des, u_des, rbd, mode,
-                stance_mode, H, g, A, lbA, ubA, m_rows);
+  return launch(ctx, K_WBC_ASSEMBLE, wbc_assemble_kernel, (B + wpb - 1) / wpb, 32 * wpb, sizeof(WbcShared) * wpb, B, ctx->wbc,
+                ctx->wbc_maps.view(ctx->base), x_des, u_des, rbd, mode, stance_mode, H, g, A, lbA, ubA, m_rows);
 }
 
 int hb_wbc_qp_rows_batch_dev(hb_ctx* ctx, int B, int n, int m_alloc, const int32_t* m_rows, const double* H, const double* g, const double* A,
@@ -635,15 +638,15 @@ int hb_hoqp_solve_batch_dev(hb_ctx* ctx, int B, const hb_hoqp_problem* problems,
 }
 
 static int hwbc_tasks_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, hb_hoqp_problem* problems) {
-  return launch(ctx, K_WBC_ASSEMBLE, hwbc_tasks_kernel, B, 32, 0, B, ctx->wbc, x_des, u_des, rbd, mode, problems);
+  return launch(ctx, K_WBC_ASSEMBLE, hwbc_tasks_kernel, B, 32, 0, B, ctx->wbc, ctx->wbc_maps.view(ctx->base), x_des, u_des, rbd, mode, problems);
 }
 
 // hb_hierarchical_wbc_solve_batch_dev, with each instance of `cs` on its own WBC settings
 static int hwbc_solve_impl(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, double* sol,
                            int32_t* status, ControllerView cs) {
   ENTER(ctx, B, x_des && u_des && rbd && mode && sol, CAPPED);
-  return launch(ctx, K_QP, hwbc_fused_kernel, B, 32, hwbc_fused_bytes(), B, ctx->wbc, cs, x_des, u_des, rbd, mode, 2 * ctx->cfg.qp_max_iter, sol,
-                status);
+  return launch(ctx, K_QP, hwbc_fused_kernel, B, 32, hwbc_fused_bytes(), B, ctx->wbc, cs, ctx->wbc_maps.view(ctx->base), x_des, u_des, rbd, mode,
+                2 * ctx->cfg.qp_max_iter, sol, status);
 }
 
 int hb_hierarchical_wbc_solve_batch_dev(hb_ctx* ctx, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, double* sol,
@@ -1319,6 +1322,8 @@ int hb_estimator_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps) { return s
 
 int hb_mpc_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps) { return set_instances(ctx, B, maps, terrain_ok, &hb_ctx::mpc_maps); }
 
+int hb_wbc_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps) { return set_instances(ctx, B, maps, terrain_ok, &hb_ctx::wbc_maps); }
+
 static bool latency_ok(const int32_t& d) { return d >= 0; }     // the upper bound is the episode's mpc_every, checked by the episode call
 
 int hb_rollout_set_mpc_latencies(hb_ctx* ctx, int B, const int32_t* ticks) { return set_instances(ctx, B, ticks, latency_ok, &hb_ctx::latencies); }
@@ -1434,6 +1439,7 @@ int hb_check_setting_records(int32_t kind, int B, const void* records, int32_t* 
     case HB_SETTING_HEIGHT_MAPS: return check_records(B, records, terrain_ok, first_bad);
     case HB_SETTING_ESTIMATOR_MAPS: return check_records(B, records, terrain_ok, first_bad);
     case HB_SETTING_MPC_MAPS: return check_records(B, records, terrain_ok, first_bad);
+    case HB_SETTING_WBC_MAPS: return check_records(B, records, terrain_ok, first_bad);
     default: return HB_EINVAL;
   }
 }

@@ -346,13 +346,14 @@ __global__ void __launch_bounds__(32) hoqp_kernel(int B, const hb_hoqp_problem* 
 // The three tasks of HierarchicalWbc::update from the WBC terms of one instance (decision vector [qdd(16), F(12), tau(10)]):
 //   task0 = formulateFloatingBaseEomTask + formulateTorqueLimitsTask + formulateFrictionConeTask + formulateNoContactMotionTask
 //   task1 = formulateBaseAccelTask          task2 = formulateContactForceTask * 0.1 + formulateSwingLegTask * 1     (WbcBase.cpp:138-338)
-__global__ void __launch_bounds__(32) hwbc_tasks_kernel(int B, hb_wbc_settings ws, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
+__global__ void __launch_bounds__(32) hwbc_tasks_kernel(int B, hb_wbc_settings ws, const __grid_constant__ InstanceView<hb_terrain> maps,
+                                                        const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
                                                         hb_hoqp_problem* problems) {
   __shared__ WbcShared sh;
   const int inst = blockIdx.x, lane = threadIdx.x;
   if (inst >= B) return;
   const int md_ = mode[inst];
-  wbc_terms_warp(x_des + (size_t)inst * NX, u_des + (size_t)inst * NU, rbd + (size_t)inst * 32, md_, false, ws, sh);
+  wbc_terms_warp(x_des + (size_t)inst * NX, u_des + (size_t)inst * NU, rbd + (size_t)inst * 32, md_, false, ws, maps, inst, sh);
   const WbcRows n = wbc_rows(md_, false);
   hb_hoqp_problem& pb = problems[inst];
   if (lane == 0) { pb.n = NWBC; pb.levels = 3; pb.ma[0] = WBC_MA0; pb.md[0] = n.md0; pb.ma[1] = 6; pb.md[1] = 0; pb.ma[2] = n.ma2; pb.md[2] = 0; }
@@ -362,7 +363,7 @@ __global__ void __launch_bounds__(32) hwbc_tasks_kernel(int B, hb_wbc_settings w
   wbc_task0_eq(sh, md_, n, WBC_MA0, &pb.a[0][0][0], NWBC, pb.b[0]);
   for (int q = lane; q < n.md0; q += 32) {
     int c0, len; double coef[3];
-    pb.f[0][q] = wbc_task0_ineq(ws, md_, q, c0, len, coef);
+    pb.f[0][q] = wbc_task0_ineq(ws, md_, q, c0, len, coef, wbc_frames(maps, inst, sh));
     for (int k = 0; k < len; ++k) pb.d[0][q][c0 + k] = coef[k];
   }
   wbc_task12_rows(1, sh.At, sh.bt, n, u_des + (size_t)inst * NU, &pb.a[1][0][0], NWBC, pb.b[1]);
@@ -373,7 +374,8 @@ __global__ void __launch_bounds__(32) hwbc_tasks_kernel(int B, hb_wbc_settings w
 // level 0 by hwbc_level0_warp, levels 1 and 2 by qp_solve_warp at their real shape (n = the free variables level 0 leaves, rows = the
 // stacked task0 inequalities), the null-space steps of hoqp_solve_warp in between. sol = x (38), status as hoqp_kernel: 0,
 // 10 * (QP status) + level of the first failing level, or 20 + level when a level leaves more than HW_NX free variables.
-__global__ void __launch_bounds__(32, 4) hwbc_fused_kernel(int B, hb_wbc_settings ws_ctx, InstanceView<hb_controller_setting> cs, const double* x_des,
+__global__ void __launch_bounds__(32, 4) hwbc_fused_kernel(int B, hb_wbc_settings ws_ctx, InstanceView<hb_controller_setting> cs,
+                                                           const __grid_constant__ InstanceView<hb_terrain> maps, const double* x_des,
                                                            const double* u_des, const double* rbd, const int32_t* mode, int max_iter, double* sol,
                                                            int32_t* status) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -386,11 +388,12 @@ __global__ void __launch_bounds__(32, 4) hwbc_fused_kernel(int B, hb_wbc_setting
   const hb_wbc_settings& ws = wbc_select_settings(ws_ctx, cs, inst, stg.ws);   // read until level 0 takes over U
   const int md_ = mode[inst];
   const double* ud = u_des + (size_t)inst * NU;
-  wbc_terms_warp(x_des + (size_t)inst * NX, ud, rbd + (size_t)inst * 32, md_, false, ws, wsh);
+  wbc_terms_warp(x_des + (size_t)inst * NX, ud, rbd + (size_t)inst * 32, md_, false, ws, maps, inst, wsh);
   const WbcRows n = wbc_rows(md_, false);
-  // task0 (Z = I: AZ = A, r = -b), its inequality rows, the motion rows tasks 1 and 2 are built from
+  // task0 (Z = I: AZ = A, r = -b), its inequality rows (the frames are read here, before level 0 takes over U), the motion rows tasks 1
+  // and 2 are built from
   wbc_task0_eq(wsh, md_, n, WBC_MA0, sh.AZ, HQ_LDA, sh.r);
-  for (int q = lane; q < n.md0; q += 32) sh.f0[q] = wbc_task0_ineq(ws, md_, q, sh.dc0[q], sh.dlen[q], &sh.dco[3 * q]);
+  for (int q = lane; q < n.md0; q += 32) sh.f0[q] = wbc_task0_ineq(ws, md_, q, sh.dc0[q], sh.dlen[q], &sh.dco[3 * q], wbc_frames(maps, inst, wsh));
   for (int i = lane; i < 18 * 16; i += 32) sh.At[i] = wsh.At[i];
   if (lane < 18) sh.bt[lane] = wsh.bt[lane];
   for (int idx = lane; idx < HQ_N * HQ_LDZ; idx += 32) { const int i = idx / HQ_LDZ, j = idx - i * HQ_LDZ; sh.Z[idx] = (i == j) ? 1.0 : 0.0; }

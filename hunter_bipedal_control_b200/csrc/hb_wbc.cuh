@@ -11,6 +11,7 @@
 // fused path (wbc_reduced_build); HierarchicalWbc stacks the unweighted tasks by priority (hb_hoqp.cuh).
 #pragma once
 #include "hb_common.cuh"
+#include "hb_planner.h"
 #include "hb_qp.cuh"
 #include "hb_rbd.cuh"
 #include "../../include/hunter_b200.h"
@@ -31,6 +32,7 @@ struct WbcShared {
   double At[18 * 16];   // motion task rows acting on qdd (swing: <=12, base: 6), at unit weight until wbc_weight_rows
   double bt[18];
   double misc[32];
+  double frame[36];     // WBC maps: contact c's surface frame n, t1, t2 at frame[9c ..]; n_z = 0 marks flat ground (wbc_contact_frames)
 };
 
 // row counts of the tasks for one contact mode
@@ -66,12 +68,41 @@ __device__ inline void rotation_error_world(const double* Rref, const double* Rm
   for (int i = 0; i < 3; ++i) err[i] = f * sk[i];
 }
 
+// The surface frame of each contact on WBC map m (WBC maps, hunter_b200.h), lane c < 4 for contact c at its measured position sh.pos_m:
+// n = (-gx, -gy, 1) / L, t1 = (1, 0, gx) / sqrt(1 + gx^2), t2 = n x t1, with each product rounded on its own (mul_rn) as the map lookup's,
+// so that a restatement gets the same bits. Where the gradient is zero the contact keeps the flat rows: its n_z is written 0, which no
+// frame has (n_z = 1 / L > 0).
+__device__ inline void wbc_contact_frames(const hb_terrain& m, WbcShared& sh) {
+  using hbplan::mul_rn;
+  const int c = lane_id();
+  if (c >= 4) return;
+  double gx, gy;
+  hbplan::terrain_height<true>(m, sh.pos_m[3 * c], sh.pos_m[3 * c + 1], &gx, &gy);
+  double* f = sh.frame + 9 * c;
+  if (gx == 0.0 && gy == 0.0) { f[2] = 0.0; return; }
+  const double L = sqrt(1.0 + mul_rn(gx, gx) + mul_rn(gy, gy)), Lt = sqrt(1.0 + mul_rn(gx, gx));
+  const double n0 = -gx / L, n1 = -gy / L, n2 = 1.0 / L, t0 = 1.0 / Lt, t2 = gx / Lt;
+  f[0] = n0; f[1] = n1; f[2] = n2;
+  f[3] = t0; f[4] = 0.0; f[5] = t2;
+  f[6] = mul_rn(n1, t2) - mul_rn(n2, 0.0);
+  f[7] = mul_rn(n2, t0) - mul_rn(n0, t2);
+  f[8] = mul_rn(n0, 0.0) - mul_rn(n1, t0);
+}
+
+// The surface frames the friction rows of instance `inst` read (wbc_task0_ineq): sh.frame when the instance has a WBC map, null (flat
+// rows) otherwise
+__device__ __forceinline__ const double* wbc_frames(const InstanceView<hb_terrain>& maps, int inst, const WbcShared& sh) {
+  return maps.of(inst) ? sh.frame : nullptr;
+}
+
 // The WBC terms of one instance in sh, and the motion task rows at unit weight in sh.At, sh.bt: formulateSwingLegTask (3 rows per swing
 // contact, in contact order), then formulateBaseAccelTask (6); in stance mode formulateStanceBaseAccelTask (6 identity rows, b = 0).
 // Returns the number of task rows. stance_mode is read where it is used (wbc_fused_kernel passes its shared copy: held in a register
-// across the passes, it spilled).
+// across the passes, it spilled). maps: the WBC maps (the kernels' __grid_constant__ parameter); with a map, instance inst's contact
+// frames go to sh.frame after pass C.
 __device__ inline int wbc_terms_warp(const double* __restrict__ x_des, const double* __restrict__ u_des, const double* __restrict__ rbd,
-                                     int mode, const bool& stance_mode, const hb_wbc_settings& ws, WbcShared& sh) {
+                                     int mode, const bool& stance_mode, const hb_wbc_settings& ws, const InstanceView<hb_terrain>& maps, int inst,
+                                     WbcShared& sh) {
   const int lane = lane_id();
   const Model& md = c_model;
   // ---- measured q, v (WbcBase.cpp:72-79)
@@ -131,6 +162,8 @@ __device__ inline int wbc_terms_warp(const double* __restrict__ x_des, const dou
     else { for (int r = 0; r < NQ; ++r) sh.nle[r] = tau[r]; }
   }
   __syncwarp();
+  // ---- contact frames on the WBC map (pass B's measured contact positions)
+  if (const hb_terrain* m = maps.of(inst)) wbc_contact_frames(*m, sh);
   // symmetrise M (WbcBase.cpp:88-89 copies the upper triangle; numerically the same matrix)
   for (int idx = lane; idx < 256; idx += 32) {
     const int i = idx >> 4, j = idx & 15;
@@ -269,8 +302,9 @@ __device__ inline void wbc_task0_eq(const WbcShared& sh, int mode, const WbcRows
 }
 
 // task0 inequality row q (formulateTorqueLimitsTask: 20 rows, then formulateFrictionConeTask: 5 pyramid rows per stance contact): its
-// nonzeros are coef[0 .. len) from column col0; returns its bound f
-__device__ inline double wbc_task0_ineq(const hb_wbc_settings& ws, int mode, int q, int& col0, int& len, double* coef) {
+// nonzeros are coef[0 .. len) from column col0; returns its bound f. frames (nullable: flat): the contacts' surface frames on a WBC map
+// (WbcShared::frame); a contact with a frame gets the pyramid about its normal, -n, +-t1 - mu n, +-t2 - mu n.
+__device__ inline double wbc_task0_ineq(const hb_wbc_settings& ws, int mode, int q, int& col0, int& len, double* coef, const double* frames) {
   if (q < 2 * NJ) {
     const int j = q % NJ;
     col0 = NQ + 12 + j; len = 1; coef[0] = q < NJ ? 1.0 : -1.0; coef[1] = 0.0; coef[2] = 0.0;
@@ -278,7 +312,14 @@ __device__ inline double wbc_task0_ineq(const hb_wbc_settings& ws, int mode, int
   }
   const int fr = q - 2 * NJ, k = fr % 5;
   const double mu = ws.friction_coefficient;   // pyramid rows {0,0,-1}, {1,0,-mu}, {-1,0,-mu}, {0,1,-mu}, {0,-1,-mu}
-  col0 = NQ + 3 * wbc_nth_contact(mode, true, fr / 5); len = 3;
+  const int c = wbc_nth_contact(mode, true, fr / 5);
+  col0 = NQ + 3 * c; len = 3;
+  const double* f = frames ? frames + 9 * c : nullptr;
+  if (f && f[2] != 0.0) {
+    const double* t = f + (k < 3 ? 3 : 6);
+    for (int a = 0; a < 3; ++a) coef[a] = k == 0 ? -f[a] : (k & 1 ? t[a] : -t[a]) - hbplan::mul_rn(mu, f[a]);
+    return 0.0;
+  }
   coef[0] = k == 1 ? 1.0 : (k == 2 ? -1.0 : 0.0);
   coef[1] = k == 3 ? 1.0 : (k == 4 ? -1.0 : 0.0);
   coef[2] = k == 0 ? -1.0 : -mu;
@@ -307,10 +348,10 @@ __device__ inline int wbc_task12_rows(int lvl, const double* At, const double* b
 // stance contact (their limits and pyramid coefficients from wbc_task0_ineq). The Tikhonov term rho ||[qdd, F, tau]||^2 of the full
 // problem is carried over exactly (rho I + rho T'T).
 // Hz is written into `Hw` as its packed lower triangle (tri_row; Hz is exactly symmetric: entry (i, j) and (j, i) are the same products
-// summed in the same order), rows of Az have stride nz. Returns nz; m_out = number of rows.
+// summed in the same order), rows of Az have stride nz. Returns nz; m_out = number of rows. frames: as wbc_task0_ineq's.
 __device__ inline int wbc_reduced_build(const WbcShared& sh, const WbcRows& n, int mode, bool stance_mode, double rho, const hb_wbc_settings& ws,
-                                        const double* __restrict__ u_des, double* Hw, double* gz, double* Az, double* lbz, double* ubz,
-                                        int* stcol /*12*/, int& m_out) {
+                                        const double* frames, const double* __restrict__ u_des, double* Hw, double* gz, double* Az, double* lbz,
+                                        double* ubz, int* stcol /*12*/, int& m_out) {
   const int lane = lane_id();
   if (lane == 0) for (int j = 0, k = 0; j < 12; ++j) if (contact_flag(mode, j / 3)) stcol[k++] = j;
   const int nz = NQ + 3 * n.nc, m = 6 + NJ + 5 * n.nc, nw = n.nt;
@@ -323,15 +364,15 @@ __device__ inline int wbc_reduced_build(const WbcShared& sh, const WbcRows& n, i
     else {
       const int fr = r - 6 - NJ, ci = fr / 5;     // stance contact ci occupies columns NQ+3ci .. NQ+3ci+2
       const int cc = c - NQ - 3 * ci;
-      if (cc >= 0 && cc < 3) { int c0, len; double coef[3]; wbc_task0_ineq(ws, mode, 2 * NJ + fr, c0, len, coef); v = coef[cc]; }
+      if (cc >= 0 && cc < 3) { int c0, len; double coef[3]; wbc_task0_ineq(ws, mode, 2 * NJ + fr, c0, len, coef, frames); v = coef[cc]; }
     }
     Az[idx] = v;
   }
   for (int r = lane; r < m; r += 32) {
     int c0, len; double coef[3];
     if (r < 6) { lbz[r] = -sh.nle[r]; ubz[r] = -sh.nle[r]; }
-    else if (r < 6 + NJ) { const int j = r - 6; const double lim = wbc_task0_ineq(ws, mode, j, c0, len, coef); lbz[r] = -lim - sh.nle[6 + j]; ubz[r] = lim - sh.nle[6 + j]; }
-    else { lbz[r] = -QP_INFTY; ubz[r] = wbc_task0_ineq(ws, mode, NJ + r - 6, c0, len, coef); }
+    else if (r < 6 + NJ) { const int j = r - 6; const double lim = wbc_task0_ineq(ws, mode, j, c0, len, coef, nullptr); lbz[r] = -lim - sh.nle[6 + j]; ubz[r] = lim - sh.nle[6 + j]; }
+    else { lbz[r] = -QP_INFTY; ubz[r] = wbc_task0_ineq(ws, mode, NJ + r - 6, c0, len, coef, frames); }
   }
   __syncwarp();
   const double* Tm = Az + 6 * nz;   // torque rows double as the map tau = T z + nle_j
@@ -365,8 +406,9 @@ namespace {  // the kernels: internal linkage, the library exports only the hb_*
 using namespace hb;
 constexpr int QP_STRIDE_H = NWBC * NWBC, QP_STRIDE_A = WBC_ROWS * NWBC;
 
-__global__ void wbc_assemble_kernel(int B, hb_wbc_settings ws, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode,
-                                    const uint8_t* stance_mode, double* H, double* g, double* A, double* lbA, double* ubA, int32_t* m_out) {
+__global__ void wbc_assemble_kernel(int B, hb_wbc_settings ws, const __grid_constant__ InstanceView<hb_terrain> maps, const double* x_des,
+                                    const double* u_des, const double* rbd, const int32_t* mode, const uint8_t* stance_mode, double* H, double* g,
+                                    double* A, double* lbA, double* ubA, int32_t* m_out) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
   const int inst = blockIdx.x * wpb + warp;
@@ -375,7 +417,7 @@ __global__ void wbc_assemble_kernel(int B, hb_wbc_settings ws, const double* x_d
   const int md = mode[inst];
   const bool stance = stance_mode ? stance_mode[inst] != 0 : false;
   const double* ud = u_des + (size_t)inst * NU;
-  wbc_terms_warp(x_des + (size_t)inst * NX, ud, rbd + (size_t)inst * 32, md, stance, ws, sh);
+  wbc_terms_warp(x_des + (size_t)inst * NX, ud, rbd + (size_t)inst * 32, md, stance, ws, maps, inst, sh);
   const WbcRows n = wbc_rows(md, stance);
   wbc_weight_rows(sh, n, stance, ws);
   const int lane = lane_id();
@@ -404,7 +446,7 @@ __global__ void wbc_assemble_kernel(int B, hb_wbc_settings ws, const double* x_d
   for (int q = lane; q < n.md0; q += 32) {
     int c0, len; double coef[3];
     const int r = n.eq + q;
-    ubA[r] = wbc_task0_ineq(ws, md, q, c0, len, coef);
+    ubA[r] = wbc_task0_ineq(ws, md, q, c0, len, coef, wbc_frames(maps, inst, sh));
     lbA[r] = -QP_INFTY;
     for (int k = 0; k < len; ++k) A[r * NWBC + c0 + k] = coef[k];
   }
@@ -426,8 +468,9 @@ static_assert(8 * (wbc_fused_doubles() * sizeof(double) + 1024) <= 228 * 1024, "
 // The assembly scratch and the WBC settings the warp's instance runs (wbc_select_settings), aliased over the QP's factorisation area
 struct WbcStaged { WbcShared sh; hb_wbc_settings ws; bool stance; };
 
-__global__ void __launch_bounds__(32, 8) wbc_fused_kernel(int B, hb_wbc_settings ws_ctx, InstanceView<hb_controller_setting> cs, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const uint8_t* stance_mode,
-                                 double rho, int max_iter, double* sol, int32_t* status, int32_t* iters) {
+__global__ void __launch_bounds__(32, 8) wbc_fused_kernel(int B, hb_wbc_settings ws_ctx, InstanceView<hb_controller_setting> cs,
+                                 const __grid_constant__ InstanceView<hb_terrain> maps, const double* x_des, const double* u_des, const double* rbd,
+                                 const int32_t* mode, const uint8_t* stance_mode, double rho, int max_iter, double* sol, int32_t* status, int32_t* iters) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, wpb = blockDim.x >> 5, lane = threadIdx.x & 31;
   const int inst = blockIdx.x * wpb + warp;
@@ -449,12 +492,13 @@ __global__ void __launch_bounds__(32, 8) wbc_fused_kernel(int B, hb_wbc_settings
   if (lane == 0) stg.stance = stance_mode ? stance_mode[inst] != 0 : false;
   const hb_wbc_settings& ws = wbc_select_settings(ws_ctx, cs, inst, stg.ws);
   const int md = mode[inst];
-  wbc_terms_warp(x_des + (size_t)inst * NX, u_des + (size_t)inst * NU, rbd + (size_t)inst * 32, md, stg.stance, ws, sh);
+  wbc_terms_warp(x_des + (size_t)inst * NX, u_des + (size_t)inst * NU, rbd + (size_t)inst * 32, md, stg.stance, ws, maps, inst, sh);
   const bool stance = stg.stance;
   const WbcRows n = wbc_rows(md, stance);
   wbc_weight_rows(sh, n, stance, ws);
   int m = 0;
-  const int nz = wbc_reduced_build(sh, n, md, stance, rho, ws, u_des + (size_t)inst * NU, w.H, gz, Az, lbz, ubz, stcol, m);
+  // the frames are read here, before the QP takes over the aliased area
+  const int nz = wbc_reduced_build(sh, n, md, stance, rho, ws, wbc_frames(maps, inst, sh), u_des + (size_t)inst * NU, w.H, gz, Az, lbz, ubz, stcol, m);
   if (lane < NJ) nlej[lane] = sh.nle[6 + lane];
   __syncwarp();
   // the workspace is carved for n = 28 (leading dimension 29); smaller problems (nz = 22, 16) use the same leading dimension

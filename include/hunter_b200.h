@@ -191,6 +191,21 @@ int hb_parse_planner_settings(const char* task_info, const char* gait_info, hb_p
  * filter and the plant do not read MPC maps. An all-zero map (h = +0) is the solve without one bit for bit. Map heights are measured
  * from the flat ground the MPC otherwise assumes (z = 0), as height maps' are. Maps are read by every MPC path (hb_mpc_set_maps). */
 
+/* ---- WBC maps: the ground the WBC's friction pyramids stand on ----
+ * A WBC map is an hb_terrain record that the WBC's friction constraint reads. The reference's pyramid (WbcBase::formulateFrictionConeTask,
+ * WbcBase.cpp:205-221) is about the world z axis: rows (0, 0, -1), (+-1, 0, -mu), (0, +-1, -mu) on each stance contact's force. For an
+ * instance with a map m, each stance contact c gets the frame of m at its measured position (the contact position of the forward
+ * kinematics at the rbd state the WBC is given: in estimated episodes the estimate, so the lookup drifts with the estimate unless
+ * odometry is set): with (gx, gy) the gradient of the height-map lookup (height maps, above) at (x_c, y_c),
+ *   L = sqrt(1 + gx^2 + gy^2),  n = (-gx, -gy, 1) / L,  t1 = (1, 0, gx) / sqrt(1 + gx^2),  t2 = n x t1,
+ * every product rounded on its own as the lookup's. The contact's five rows become -n, t1 - mu n, -t1 - mu n, t2 - mu n, -t2 - mu n, each
+ * with bound 0, mu the instance's friction_coefficient (the context's hb_wbc_settings or its controller setting). Where gx == 0 and
+ * gy == 0 (a zero map, a plateau cell, a point off the grid on both axes) the rows are the flat rows unchanged, the plant's own flat-path
+ * rule, so an all-zero map is the WBC without one bit for bit. The normal is the bilinear gradient the plant's sloped contact pushes along:
+ * a foot on a step's one-cell ramp gets the ramp's steep normal, as it does in the plant; there is no smoothing over the foot. Every other
+ * WBC row (EoM, torque limits, zero swing forces, no contact motion, swing-leg, base and contact-force tasks), the MPC's friction cone,
+ * the planner, the filter and the plant do not read WBC maps. Maps are read by every WBC path (hb_wbc_set_maps). */
+
 /* state of the speed-based gait selection of one instance (SwitchedModelReferenceManager velAbsHistory_/velAvg_/gaitLevel_);
  * zero-initialise, then set gait_level = -1 ("no template chosen yet") or the level in force */
 typedef struct {
@@ -441,6 +456,7 @@ typedef struct {                 /* the bodies of one robot, relative to the nom
 #define HB_SETTING_HEIGHT_MAPS 14             /* hb_terrain for hb_plan_set_maps (hb_check_setting_records), the rules of _TERRAINS  */
 #define HB_SETTING_ESTIMATOR_MAPS 15          /* hb_terrain for hb_estimator_set_maps (hb_check_setting_records), as _TERRAINS      */
 #define HB_SETTING_MPC_MAPS 17                /* hb_terrain for hb_mpc_set_maps (hb_check_setting_records), as _TERRAINS; 16 unused */
+#define HB_SETTING_WBC_MAPS 18                /* hb_terrain for hb_wbc_set_maps (hb_check_setting_records), as _TERRAINS            */
 int hb_default_link_variation(hb_link_variation* r);      /* host only: every scale 1, every shift 0 */
 /* Sets the link variations of the context's episodes (a per-robot episode setting, above). -1 also for a value that is not finite, a
  * mass_scale <= 0 or an inertia_scale <= 0. */
@@ -450,8 +466,8 @@ int hb_rollout_set_link_variations(hb_ctx* ctx, int B, const hb_link_variation* 
  * The terrain acts on the simulated plant and on the height failure check only; the planner, MPC, WBC, joint command law, actuation
  * model and estimator keep assuming flat ground at z = 0 and are not told about it. The planner can be told where the ground is by a
  * height map (height maps, above; hb_plan_set_maps), the estimator's feet heights by an estimator map (estimator maps, above;
- * hb_estimator_set_maps) and the MPC's stance feet by an MPC map (MPC maps, above; hb_mpc_set_maps), records of this type each set on
- * its own.
+ * hb_estimator_set_maps), the MPC's stance feet by an MPC map (MPC maps, above; hb_mpc_set_maps) and the WBC's friction pyramids by a
+ * WBC map (WBC maps, above; hb_wbc_set_maps), records of this type each set on its own.
  * Height and gradient at a world point (x, y): u = (x - origin[0]) / spacing clamped to [0, nx - 1], i = min(floor(u), nx - 2),
  * a = u - i; the same for y gives w, j and b. With lerp(p, q, s) = p + s (q - p): h0 = lerp(h[j][i], h[j][i+1], a),
  * h1 = lerp(h[j+1][i], h[j+1][i+1], a), h = lerp(h0, h1, b); g_x = lerp(h[j][i+1] - h[j][i], h[j+1][i+1] - h[j+1][i], b) / spacing,
@@ -868,6 +884,15 @@ int hb_estimator_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
  * runs one more launch (the stance heights, once per solve); unset, the launches are those without the setting. Maps are a setting, not
  * episode state: hb_episode_state_bytes and snapshots do not count them. */
 int hb_mpc_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
+/* WBC maps of the context (WBC maps, above): instance i < B of every WBC path -- hb_wbc_solve_batch(_dev), hb_wbc_assemble_batch(_dev),
+ * hb_hierarchical_wbc_solve_batch(_dev), hb_hierarchical_wbc_tasks_batch, hb_control_step_batch(_dev), hb_resident_cycle_batch(_dev),
+ * hb_resident_plan_cycle_batch, hb_resident_wbc_batch(_dev), hb_policy_wbc(_async), hb_rollout_batch_dev and hb_rollout_estimated_batch_dev
+ * -- tilts its stance contacts' friction pyramids on maps[i]; instances at or beyond B, and every instance while none is set, keep the
+ * flat pyramids. One setting serves every path, so an episode can be written as a loop of public calls. The contract of hb_plan_set_maps:
+ * host array validated and copied in stream order, B == 0 clears (maps may be NULL), -1 for a record hb_rollout_set_terrains rejects, -4
+ * for B > max_batch, a rejected call keeps the previous setting. No launch is added, set or not. Maps are a setting, not episode state:
+ * hb_episode_state_bytes and snapshots do not count them. */
+int hb_wbc_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
 /* One estimator update per instance (StateEstimateBase::updateJointStates / updateImu, StateEstimateBase.cpp:73-106, then
  * KalmanFilterEstimate::update): quat = (x, y, z, w); contact_flag: B x 4 (0 = the filter distrusts that foot, x100 noise);
  * rbd_out: B x 32 measured rbd state [zyx, p, q_j, omega_world, v, qd_j]. zyxOffset_ is taken as zero. The odometry fusion

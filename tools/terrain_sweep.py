@@ -44,6 +44,16 @@ constraint pulls each stance contact to 0.02 m above the map instead of z = 0.02
 added to every map the run gives (planner + MPC maps; with --estimator-maps all three), and times episodes with MPC maps against the same
 episodes with all-zero MPC maps and without MPC maps, alternately; the tool asserts that all-zero MPC maps give the outcome of no MPC maps
 bit for bit.
+
+--wbc-maps (with --height-maps) also tilts the WBC's friction pyramids on the ground (hb_wbc_set_maps), with the same maps: each stance
+contact's pyramid is about the map's normal at the contact's measured position instead of the world z axis. The line reports the tables
+above plus one, with_wbc_maps, with WBC maps added to every map the run gives, and times episodes with WBC maps against the same episodes
+with all-zero WBC maps and without WBC maps, alternately; the tool asserts that all-zero WBC maps give the outcome of no WBC maps bit for
+bit.
+
+--friction-scale S scales every robot's ground friction by S in every table (hb_rollout_set_plant_variations, friction_scale) and runs its
+WBC with friction_coefficient S times the context's (task.info's) value (hb_rollout_set_controller_settings): the slope's direction
+matters most to the friction pyramids where friction is short.
 """
 import json
 import os
@@ -93,46 +103,56 @@ def height_map_sweep(h, args, grid):
     T_episode = TICKS * prm.period
 
     def set_all(value):
-        terrains, maps, est_maps, mpc_maps = value
+        terrains, maps, est_maps, mpc_maps, wbc_maps = value
         ctx.set_terrains(terrains)
         ctx.set_height_maps(maps)
         ctx.set_estimator_maps(est_maps)
         ctx.set_mpc_maps(mpc_maps)
+        ctx.set_wbc_maps(wbc_maps)
 
-    def settings(shift, planner, estimator, mpc=False):
+    def settings(shift, planner, estimator, mpc=False, wbc=False):
         origin, heights = grid(shift)
         maps = hb.make_terrains(B, heights - GROUND, SPACING, origin)
-        return hb.make_terrains(B, heights, SPACING, origin), maps if planner else None, maps if estimator else None, maps if mpc else None
+        return (hb.make_terrains(B, heights, SPACING, origin), maps if planner else None, maps if estimator else None, maps if mpc else None,
+                maps if wbc else None)
 
     tables = [("blind", False, False), ("mapped", True, False)]
     if args.estimator_maps:
         tables = [("blind", False, False), ("planner_maps", True, False), ("estimator_maps", False, True), ("both_maps", True, True)]
-    tables = [t + (False,) for t in tables]
+    tables = [t + (False, False) for t in tables]
     if args.mpc_maps:
-        tables.append(("all_maps", True, True, True) if args.estimator_maps else ("planner_mpc_maps", True, False, True))
+        tables.append(("all_maps", True, True, True, False) if args.estimator_maps else ("planner_mpc_maps", True, False, True, False))
+    if args.wbc_maps:
+        tables.append(("with_wbc_maps", True, args.estimator_maps, args.mpc_maps, True))
     out, mk = {}, [str(m) for m in MAGNITUDES]
-    for name, planner, estimator, mpc in tables:
+    for name, planner, estimator, mpc, wbc in tables:
         tally = Tally(len(MAGNITUDES), len(KINDS))
-        for r, run in h.sweep(set_all, lambda shift: settings(shift, planner, estimator, mpc)):
+        for r, run in h.sweep(set_all, lambda shift: settings(shift, planner, estimator, mpc, wbc)):
             tally.add(*cells(B, len(MAGNITUDES), len(KINDS), r), run.stats, value=np.hypot(*(run.rbd[:, 3:5] - rbd0[:, 3:5]).T) / T_episode)
         out[name] = {"largest_magnitude_90pct": dict(zip(KINDS, tally.largest(MAGNITUDES))), "survival": keyed(KINDS, mk, tally.survival().tolist()),
                      "mean_speed_of_survivors_m_per_s": keyed(KINDS, mk, tally.mean()), "fail_reasons": tally.reasons}
-    terrains, maps, _, _ = settings(0, True, True)
+    terrains, maps, _, _, _ = settings(0, True, True)
     origin, heights = grid(0)
     zero = hb.make_terrains(B, np.zeros_like(heights), SPACING, origin)
-    if args.mpc_maps:
-        est = maps if args.estimator_maps else None
-        _, clocks, timing = h.alternate(set_all, [("mpc_maps", (terrains, maps, est, maps)), ("zero_mpc_maps", (terrains, maps, est, zero)),
-                                                  ("no_mpc_maps", (terrains, maps, est, None))], args.timed, launches=True)
+    est = maps if args.estimator_maps else None
+    if args.wbc_maps:
+        mpc = maps if args.mpc_maps else None
+        _, clocks, timing = h.alternate(set_all, [("wbc_maps", (terrains, maps, est, mpc, maps)), ("zero_wbc_maps", (terrains, maps, est, mpc, zero)),
+                                                  ("no_wbc_maps", (terrains, maps, est, mpc, None))], args.timed, launches=True)
+        assert timing["zero_wbc_maps_same_outcome_as_no_wbc_maps"], "all-zero WBC maps changed the outcome of no WBC maps"
+    elif args.mpc_maps:
+        _, clocks, timing = h.alternate(set_all, [("mpc_maps", (terrains, maps, est, maps, None)), ("zero_mpc_maps", (terrains, maps, est, zero, None)),
+                                                  ("no_mpc_maps", (terrains, maps, est, None, None))], args.timed, launches=True)
         assert timing["zero_mpc_maps_same_outcome_as_no_mpc_maps"], "all-zero MPC maps changed the outcome of no MPC maps"
     elif args.estimator_maps:
-        _, clocks, timing = h.alternate(set_all, [("both_maps", (terrains, maps, maps, None)), ("zero_estimator_maps", (terrains, maps, zero, None)),
-                                                  ("planner_maps", (terrains, maps, None, None))], args.timed, launches=True)
+        _, clocks, timing = h.alternate(set_all, [("both_maps", (terrains, maps, maps, None, None)),
+                                                  ("zero_estimator_maps", (terrains, maps, zero, None, None)),
+                                                  ("planner_maps", (terrains, maps, None, None, None))], args.timed, launches=True)
         assert timing["zero_estimator_maps_same_outcome_as_planner_maps"], "all-zero estimator maps changed the outcome of planner maps only"
     else:
-        _, clocks, timing = h.alternate(set_all, [("mapped", (terrains, maps, None, None)), ("zero_maps", (terrains, zero, None, None)),
-                                                  ("blind", (terrains, None, None, None))], args.timed, launches=True)
-    set_all((None, None, None, None))
+        _, clocks, timing = h.alternate(set_all, [("mapped", (terrains, maps, None, None, None)), ("zero_maps", (terrains, zero, None, None, None)),
+                                                  ("blind", (terrains, None, None, None, None))], args.timed, launches=True)
+    set_all((None, None, None, None, None))
     return out, clocks, timing
 
 
@@ -141,15 +161,23 @@ def main():
         ap.add_argument("--height-maps", action="store_true", help="also plan on maps of the terrains")
         ap.add_argument("--estimator-maps", action="store_true", help="with --height-maps --estimator: also give the Kalman filter the maps")
         ap.add_argument("--mpc-maps", action="store_true", help="with --height-maps: also hold the MPC's stance feet on the maps")
+        ap.add_argument("--wbc-maps", action="store_true", help="with --height-maps: also tilt the WBC's friction pyramids on the maps")
+        ap.add_argument("--friction-scale", type=float, default=1.0, help="scale of every robot's ground friction and WBC friction coefficient")
 
     args = sweep_args("terrain_sweep.py", "timed terrain / flat / unset episode triples (with --height-maps: mapped / zero-map / blind)",
                       len(KINDS) * len(MAGNITUDES), extra=extra,
-                      valid=lambda a: (not a.estimator_maps or (a.height_maps and a.estimator)) and (not a.mpc_maps or a.height_maps),
-                      needs="--estimator-maps needs --height-maps --estimator, --mpc-maps needs --height-maps, ")
+                      valid=lambda a: ((not a.estimator_maps or (a.height_maps and a.estimator)) and (not a.mpc_maps or a.height_maps)
+                                       and (not a.wbc_maps or a.height_maps) and a.friction_scale > 0),
+                      needs="--estimator-maps needs --height-maps --estimator, --mpc-maps needs --height-maps, "
+                            "--wbc-maps needs --height-maps, --friction-scale takes a scale > 0, ")
     h = Episodes("terrain_sweep.py", args, TICKS)
     hb, ctx, prm, B, rbd0 = h.hb, h.ctx, h.prm, h.B, h.rbd0
     step_ahead, ramp_ahead = feature_distances(rbd0, h.feet)
     T_episode = TICKS * prm.period
+    if args.friction_scale != 1.0:         # short friction on both sides of the loop: the plant's ground and the WBC's pyramids
+        ctx.set_plant_variations(hb.make_plant_variations(B, friction_scale=args.friction_scale))
+        ctx.set_controller_settings(hb.make_controller_settings(B, wbc=ctx.wbc_settings(),
+                                                                friction_coefficient=args.friction_scale * ctx.wbc_settings().friction_coefficient))
 
     if args.height_maps:
         def grid(shift):
@@ -157,7 +185,13 @@ def main():
             return terrain_heights(rbd0, np.array(KINDS)[ki], np.array(MAGNITUDES)[mi], step_ahead, ramp_ahead)
 
         out, clocks, timing = height_map_sweep(h, args, grid)
-        if args.mpc_maps:
+        if args.wbc_maps:
+            metric = ("WBC maps: the highest step [cm] that >= 90 %% of the trotting robots cross within %.1f s%s when the planner%s%s and "
+                      "the WBC are told the terrain; %s tables per kind (steps in cm, slopes in degrees)"
+                      % (T_episode, " through the estimator" if args.estimator else "", ", the Kalman filter" if args.estimator_maps else "",
+                         ", the MPC" if args.mpc_maps else "", ", ".join(out)))
+            value = out["with_wbc_maps"]["largest_magnitude_90pct"]["step_up"]
+        elif args.mpc_maps:
             last = "all_maps" if args.estimator_maps else "planner_mpc_maps"
             metric = ("MPC maps: the highest step [cm] that >= 90 %% of the trotting robots cross within %.1f s%s when the planner%s and the "
                       "MPC are told the terrain; %s tables per kind (steps in cm, slopes in degrees)"
@@ -181,7 +215,9 @@ def main():
                                   % (GRID, GRID, SPACING, GROUND, STEP_AHEAD, RAMP_AHEAD),
                        "height_maps": "each robot's terrain minus %g m (hb_plan_set_maps%s%s); blind: no map"
                                       % (GROUND, ", and the same maps with hb_estimator_set_maps" if args.estimator_maps else "",
-                                         ", and the same maps with hb_mpc_set_maps in the last table" if args.mpc_maps else ""),
+                                         ", and the same maps with hb_mpc_set_maps in the last table" if args.mpc_maps else "")
+                                      + (", and the same maps with hb_wbc_set_maps in with_wbc_maps" if args.wbc_maps else ""),
+                       "friction_scale": args.friction_scale,
                        "survival": "robots still up at the end of the episode", "failure_checks": failure_checks("base z above the terrain")}}))
         return
 
