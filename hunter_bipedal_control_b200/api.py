@@ -61,7 +61,7 @@ EXPORTED_SYMBOLS = [
     "hb_default_teleop_setting", "hb_rollout_set_teleop", "hb_cmd_vel_to_target",
     "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
     "hb_plan_set_maps", "hb_plan_references_maps", "hb_goal_to_target_maps", "hb_cmd_vel_to_target_maps", "hb_estimator_set_maps",
-    "hb_mpc_set_maps", "hb_wbc_set_maps",
+    "hb_mpc_set_maps", "hb_wbc_set_maps", "hb_mpc_set_cone_maps",
     "hb_check_setting_records", "hb_rollout_set_channel",
     "hb_episode_state_bytes", "hb_episode_save_async", "hb_episode_restore",
 ]
@@ -500,6 +500,7 @@ HEIGHT_MAPS_SETTING_KIND = 14     # HB_SETTING_HEIGHT_MAPS: HbTerrain records as
 ESTIMATOR_MAPS_SETTING_KIND = 15  # HB_SETTING_ESTIMATOR_MAPS: HbTerrain records as estimator maps (Context.set_estimator_maps), for hb_check_setting_records
 MPC_MAPS_SETTING_KIND = 17        # HB_SETTING_MPC_MAPS: HbTerrain records as MPC maps (Context.set_mpc_maps), for hb_check_setting_records
 WBC_MAPS_SETTING_KIND = 18        # HB_SETTING_WBC_MAPS: HbTerrain records as WBC maps (Context.set_wbc_maps), for hb_check_setting_records
+MPC_CONE_MAPS_SETTING_KIND = 19   # HB_SETTING_MPC_CONE_MAPS: HbTerrain records as MPC cone maps (Context.set_mpc_cone_maps), for hb_check_setting_records
 
 
 class HbTerrain(C.Structure):
@@ -1541,6 +1542,13 @@ class Context:
         resident_wbc, policy_wbc, rollout and rollout_estimated): each stance contact's pyramid is about the map's normal at its measured
         position. Instances beyond len(maps) keep the flat pyramids; None clears them."""
         self._set_instances("hb_wbc_set_maps", maps)
+
+    def set_mpc_cone_maps(self, maps):
+        """MPC cone maps of this context (hb_mpc_set_cone_maps): maps[i] (make_terrains) is the ground the MPC of instance i stands its
+        friction cones on, in every MPC path (those of set_mpc_maps): each stance contact's cone bounds its force in the map's surface frame
+        at its swing reference's (x, y). A setting of its own, apart from set_mpc_maps. Instances beyond len(maps) keep the cones about
+        world z; None clears them."""
+        self._set_instances("hb_mpc_set_cone_maps", maps)
 
     def resident_wbc(self, t_now, rbd, stance_mode=None):
         """Policy of the resident solution at absolute time t_now + WeightedWbc: returns (x_des, u_des, mode, sol, torque, status)."""

@@ -128,6 +128,10 @@ struct hb_ctx {
   // them (B x (N+1) x 4, allocated at max_batch by the first solve with a map set)
   InstanceSetting<hb_terrain> mpc_maps;
   void* sth_mem; double* sth;
+  // each instance's MPC cone map in every MPC path: the ground the friction cones stand on (hb_mpc_set_cone_maps), and the gradients a
+  // solve looks up on them (B x (N+1) x 4 x 2, allocated at max_batch by the first solve with a cone map set)
+  InstanceSetting<hb_terrain> cone_maps;
+  void* cgr_mem; double* cgr;
   // each instance's WBC map in every WBC path: the surface normals of the friction pyramids (hb_wbc_set_maps)
   InstanceSetting<hb_terrain> wbc_maps;
   // the recorded channels of the episodes (hb_rollout_set_channel): the caller's buffer, its instances and rows; B == 0: unset
@@ -520,7 +524,7 @@ int hb_destroy(hb_ctx* ctx) {
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
                        ctx->odometry.dev, ctx->controllers.dev, ctx->hardware.dev, ctx->plan_settings.dev,
                        ctx->bridges.dev, ctx->links.dev, ctx->height_maps.dev, ctx->estimator_maps.dev,
-                       ctx->mpc_maps.dev, ctx->sth_mem, ctx->wbc_maps.dev};
+                       ctx->mpc_maps.dev, ctx->sth_mem, ctx->wbc_maps.dev, ctx->cone_maps.dev, ctx->cgr_mem};
   for (void* p : mem) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -686,9 +690,16 @@ static int mpc_solve_impl(hb_ctx* ctx, int B, const double* x0, const double* x_
     rc = reserve_group(&ctx->sth_mem, [&](void* m) { size_t off = 0; ctx->sth = carve<double>(m, off, Bc * (Nc + 1) * 4); return off; });
     if (rc) return rc;
   }
+  // the ground gradients on the MPC cone maps, which K1 looks up and K3 reads: their storage, only while a cone map is set (no launch)
+  const InstanceView<hb_terrain> cone_maps = ctx->cone_maps.view(ctx->base);
+  if (cone_maps.recs) {
+    rc = reserve_group(&ctx->cgr_mem, [&](void* m) { size_t off = 0; ctx->cgr = carve<double>(m, off, Bc * (Nc + 1) * 8); return off; });
+    if (rc) return rc;
+  }
   SqpArgs a;
   a.tk = tk; a.nn = nn;
   a.maps = maps; a.sth = maps.recs ? ctx->sth + (size_t)ctx->base * (Nc + 1) * 4 : nullptr;
+  a.cone_maps = cone_maps; a.cgr = cone_maps.recs ? ctx->cgr + (size_t)ctx->base * (Nc + 1) * 8 : nullptr;
   a.B = B; a.N = ctx->cfg.horizon_N; a.dt = ctx->cfg.dt; a.x_ref = x_ref; a.swing = swing_ref; a.mode = mode; a.xt = x_traj; a.ut = u_traj;
   {
     const size_t o = (size_t)ctx->base, Nn = (size_t)ctx->cfg.horizon_N;
@@ -1322,6 +1333,8 @@ int hb_estimator_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps) { return s
 
 int hb_mpc_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps) { return set_instances(ctx, B, maps, terrain_ok, &hb_ctx::mpc_maps); }
 
+int hb_mpc_set_cone_maps(hb_ctx* ctx, int B, const hb_terrain* maps) { return set_instances(ctx, B, maps, terrain_ok, &hb_ctx::cone_maps); }
+
 int hb_wbc_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps) { return set_instances(ctx, B, maps, terrain_ok, &hb_ctx::wbc_maps); }
 
 static bool latency_ok(const int32_t& d) { return d >= 0; }     // the upper bound is the episode's mpc_every, checked by the episode call
@@ -1439,6 +1452,7 @@ int hb_check_setting_records(int32_t kind, int B, const void* records, int32_t* 
     case HB_SETTING_HEIGHT_MAPS: return check_records(B, records, terrain_ok, first_bad);
     case HB_SETTING_ESTIMATOR_MAPS: return check_records(B, records, terrain_ok, first_bad);
     case HB_SETTING_MPC_MAPS: return check_records(B, records, terrain_ok, first_bad);
+    case HB_SETTING_MPC_CONE_MAPS: return check_records(B, records, terrain_ok, first_bad);
     case HB_SETTING_WBC_MAPS: return check_records(B, records, terrain_ok, first_bad);
     default: return HB_EINVAL;
   }

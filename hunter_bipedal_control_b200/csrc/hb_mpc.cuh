@@ -4,6 +4,7 @@
 //   horizon node: the centroidal flow map (flow_map_lane) and the stage cost / equality-constraint values (node_values_lane).
 #pragma once
 #include "hb_common.cuh"
+#include "hb_planner.h"
 #include "hb_rbd.cuh"
 
 namespace hb {
@@ -200,10 +201,19 @@ struct BarrierSum {
   __device__ __forceinline__ double value(double mu) const { return mu * (quad - log(prod)); }
 };
 
+// Stance force (Fx, Fy, Fz) in the surface frame f = (n, t1, t2) of hbplan::surface_frame: the local force t_R_w F = (t1.F, t2.F, n.F)
+// of FrictionConeConstraint.cpp:82, which the friction cone bounds on an MPC cone map
+__device__ __forceinline__ void cone_local_force(const double* f, double& Fx, double& Fy, double& Fz) {
+  const double lx = f[3] * Fx + f[4] * Fy + f[5] * Fz, ly = f[6] * Fx + f[7] * Fy + f[8] * Fz, lz = f[0] * Fx + f[1] * Fy + f[2] * Fz;
+  Fx = lx; Fy = ly; Fz = lz;
+}
+
 // Stage cost (unscaled) and equality-constraint values of one node, one lane = one node (values only). sth (nullable): the node's four
-// stance heights on an MPC map (SqpArgs::sth), which the stance z rows subtract as K1's do.
+// stance heights on an MPC map (SqpArgs::sth), which the stance z rows subtract as K1's do. cgr (nullable): the node's four ground
+// gradients on an MPC cone map (SqpArgs::cgr); a stance contact on sloped ground has its cone about that ground's frame, as K1's has.
 __device__ inline void node_values_lane(const double* x, const double* u, const double* xref, const double* swing, int mode,
-                                        const double* epos, const double* evel, const double* sth, double& cost, double& eq_sq) {
+                                        const double* epos, const double* evel, const double* sth, const double* cgr, double& cost,
+                                        double& eq_sq) {
   const Model& md = c_model;
   bool fl[4]; int ns = 0;
   for (int c = 0; c < 4; ++c) { fl[c] = contact_flag(mode, c); ns += fl[c]; }
@@ -219,7 +229,13 @@ __device__ inline void node_values_lane(const double* x, const double* u, const 
   for (int c = 0; c < 4; ++c) {
     if (fl[c]) {
       const double Fx = u[3 * c], Fy = u[3 * c + 1], Fz = u[3 * c + 2];
-      const double h = HB_FRICTION_MU * Fz - sqrt(Fx * Fx + Fy * Fy + HB_FRICTION_REGULARIZATION);
+      double h, f[9];
+      if (cgr && hbplan::surface_frame(cgr[2 * c], cgr[2 * c + 1], f)) {
+        // the cone on the local force; written apart from the flat statement, which keeps its own instructions
+        double lx = Fx, ly = Fy, lz = Fz;
+        cone_local_force(f, lx, ly, lz);
+        h = fma(HB_FRICTION_MU, lz, -sqrt(fma(lx, lx, fma(ly, ly, (double)HB_FRICTION_REGULARIZATION))));
+      } else h = HB_FRICTION_MU * Fz - sqrt(Fx * Fx + Fy * Fy + HB_FRICTION_REGULARIZATION);
       fric.add(h, HB_FRICTION_BARRIER_DELTA);
       const double e0 = evel[3 * c], e1 = evel[3 * c + 1];
       double e2z = evel[3 * c + 2] + HB_ZEROVEL_Z_GAIN * epos[3 * c + 2] + HB_ZEROVEL_Z_OFFSET;

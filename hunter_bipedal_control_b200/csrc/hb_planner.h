@@ -92,6 +92,29 @@ HBP_HD inline double map_height(const hb_terrain* m, double x, double y) {
   return terrain_height<true>(*m, x, y, &gx, &gy);
 }
 
+// The surface frame of ground with gradient (gx, gy): f = (n, t1, t2) with n = (-gx, -gy, 1) / L, L = sqrt(1 + gx^2 + gy^2),
+// t1 = (1, 0, gx) / sqrt(1 + gx^2) and t2 = n x t1, each product rounded on its own (mul_rn) as the map lookup's, so that host and device
+// frames have the same bits. Returns whether the ground is sloped; a zero gradient is flat ground, and f is then left as it is.
+HBP_HD inline bool surface_frame(double gx, double gy, double* f) {
+  if (gx == 0.0 && gy == 0.0) return false;
+  const double L = sqrt(1.0 + mul_rn(gx, gx) + mul_rn(gy, gy)), Lt = sqrt(1.0 + mul_rn(gx, gx));
+  const double n0 = -gx / L, n1 = -gy / L, n2 = 1.0 / L, t0 = 1.0 / Lt, t2 = gx / Lt;
+  f[0] = n0; f[1] = n1; f[2] = n2;
+  f[3] = t0; f[4] = 0.0; f[5] = t2;
+  f[6] = mul_rn(n1, t2) - mul_rn(n2, 0.0);
+  f[7] = mul_rn(n2, t0) - mul_rn(n0, t2);
+  f[8] = mul_rn(n0, 0.0) - mul_rn(n1, t0);
+  return true;
+}
+
+// The surface frame of map m at world (x, y) (surface_frame of the lookup's gradient): the friction cones of the WBC maps and the MPC
+// cone maps (hunter_b200.h) are about it. Returns whether the ground is sloped there; f is written only then.
+HBP_HD inline bool map_frame(const hb_terrain& m, double x, double y, double* f) {
+  double gx, gy;
+  terrain_height<true>(m, x, y, &gx, &gy);
+  return surface_frame(gx, gy, f);
+}
+
 struct Vec3 { double x, y, z; };
 HBP_HD inline Vec3 operator+(Vec3 a, Vec3 b) { return {a.x + b.x, a.y + b.y, a.z + b.z}; }
 HBP_HD inline Vec3 operator-(Vec3 a, Vec3 b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }

@@ -307,6 +307,11 @@ struct SqpArgs {
   // and then no kernel reads either.
   InstanceView<hb_terrain> maps;
   double* sth;
+  // MPC cone maps (hb_mpc_set_cone_maps): each instance's map, and cgr, B x (N+1) x 4 x 2 ground gradients (gx, gy) under the stance
+  // contacts of each node. K1 looks them up (cone_gradient) and writes them for K3; both friction cones are about the surface frame
+  // hbplan::surface_frame builds from them. cgr is null while no cone map is set, and then no kernel reads either.
+  InstanceView<hb_terrain> cone_maps;
+  double* cgr;
 };
 
 // The ground under stance contact `lane` (< 4) of node k on the instance's MPC map: hbplan::map_height at the swing reference's (x, y);
@@ -320,6 +325,16 @@ __device__ __forceinline__ double stance_height_lane(const SqpArgs& a, int inst,
     a.sth[((size_t)inst * (a.N + 1) + k) * 4 + lane] = h;
   }
   return h;
+}
+
+// The ground's gradient under stance contact c of node k on the instance's MPC cone map, at the swing reference's (x, y) as for
+// stance_height_lane; (+0, +0), flat, for a swing contact or an instance without a cone map. Stored to cgr for K3's cones.
+__device__ __forceinline__ void cone_gradient(const SqpArgs& a, int inst, int k, int c, unsigned flm, const double* swing, double& gx, double& gy) {
+  gx = 0.0; gy = 0.0;
+  const hb_terrain* m = a.cone_maps.of(inst);
+  if (m && ((flm >> c) & 1u)) hbplan::terrain_height<true>(*m, swing[6 * c], swing[6 * c + 1], &gx, &gy);
+  double* g = a.cgr + (((size_t)inst * (a.N + 1) + k) * 4 + c) * 2;
+  g[0] = gx; g[1] = gy;
 }
 __device__ __forceinline__ int sqp_nn(const SqpArgs& a, int inst) { return a.nn ? a.nn[inst] : a.N; }
 __device__ __forceinline__ double sqp_dt(const SqpArgs& a, int inst, int k) {
@@ -466,7 +481,8 @@ static_assert((LQ_T % 2) == 0 && (sizeof(double) * LIN_STRIDE) % 16 == 0, "T is 
 // RK2 sensitivities (S2) and the stage cost (M2, M6, M8) of one node: the part of the LQ approximation that does not depend on the number
 // of swing contacts, so one copy of its code serves every lq_node<NSW>. Leaves the discrete A / B rows 3..11 in the record and q, Qd, r,
 // b, RFF, dvd in shared memory; returns this lane's share of the cost and the warp's squared dynamics defect.
-__device__ __forceinline__ void lq_model(LqShared& sh, int lane, unsigned flm, int nsw, double dt, double xn_l, double xref_l, double& cost_l, double& d2_w) {
+__device__ __forceinline__ void lq_model(LqShared& sh, const SqpArgs& a, int inst, int k, int lane, unsigned flm, int nsw, double dt, double xn_l,
+                                         double xref_l, double& cost_l, double& d2_w) {
   const Model& md = c_model;
   const double im = 1.0 / md.total_mass;
   const double* A1c = sh.rec + LIN_A1; const double* A2c = sh.rec + LIN_A2;
@@ -555,21 +571,24 @@ __device__ __forceinline__ void lq_model(LqShared& sh, int lane, unsigned flm, i
   __syncwarp();
   if (lane < 12) { const int c = lane / 3, ax = lane - 3 * c; sh.RFF[c * 9 + ax * 4] = ltab[1]; }
   // all scalar penalties in ONE pass: lanes 0-9 joint position limits, 10-19 joint velocity limits, 20-23 normal-force limits
-  // (double sided), 24-27 friction cones of stance contacts (one sided)
+  // (double sided), 24-27 friction cones of stance contacts (one sided); on sloped ground of an MPC cone map the cone bounds the local
+  // force in the surface frame fr (tilt)
   double shiftsum = 0.0;
   {
     double h = 1.0, lo = 0.0, hi = 2.0, pmu = 0.0, pdl = 1.0;
-    bool two = true, on = false;
-    double Fx = 0.0, Fy = 0.0, tn = 1.0, t2 = 1.0;
+    bool two = true, on = false, tilt = false;
+    double Fx = 0.0, Fy = 0.0, Fz = 0.0, tn = 1.0, t2 = 1.0, fr[9];
     if (lane < 10) { h = sh.x[12 + lane]; lo = ltab[12]; hi = ltab[13]; pmu = HB_LIMIT_POS_MU; pdl = HB_LIMIT_POS_DELTA; on = true; }
     else if (lane < 20) { const int j = lane - 10; h = sh.u[12 + j]; lo = ltab[12]; hi = ltab[13]; pmu = HB_LIMIT_VEL_MU; pdl = HB_LIMIT_VEL_DELTA; on = true; }
     else if (lane < 24) { const int c = lane - 20; h = sh.u[3 * c + 2]; lo = 0.0; hi = HB_LIMIT_FORCE_MAX; pmu = HB_LIMIT_FORCE_MU; pdl = HB_LIMIT_FORCE_DELTA; on = true; }
     else if (lane < 28) {
       const int c = lane - 24;
+      if (a.cgr) { double gx, gy; cone_gradient(a, inst, k, c, flm, sh.swing, gx, gy); tilt = hbplan::surface_frame(gx, gy, fr); }
       if ((flm >> c) & 1u) {
-        Fx = sh.u[3 * c]; Fy = sh.u[3 * c + 1];
+        Fx = sh.u[3 * c]; Fy = sh.u[3 * c + 1]; Fz = sh.u[3 * c + 2];
+        if (tilt) cone_local_force(fr, Fx, Fy, Fz);
         t2 = Fx * Fx + Fy * Fy + HB_FRICTION_REGULARIZATION; tn = sqrt(t2);
-        h = HB_FRICTION_MU * sh.u[3 * c + 2] - tn; lo = 0.0; pmu = HB_FRICTION_BARRIER_MU; pdl = HB_FRICTION_BARRIER_DELTA; two = false; on = true;
+        h = HB_FRICTION_MU * Fz - tn; lo = 0.0; pmu = HB_FRICTION_BARRIER_MU; pdl = HB_FRICTION_BARRIER_DELTA; two = false; on = true;
       }
     }
     const Pen pa = relaxed_barrier(h - lo, pmu, pdl);
@@ -589,10 +608,27 @@ __device__ __forceinline__ void lq_model(LqShared& sh, int lane, unsigned flm, i
       const double g0 = -Fx * it, g1 = -Fy * it, g2 = HB_FRICTION_MU;
       const double h00 = -(Fy * Fy + HB_FRICTION_REGULARIZATION) * it32, h01 = Fx * Fy * it32, h11 = -(Fx * Fx + HB_FRICTION_REGULARIZATION) * it32;
       double* Rc = sh.RFF + c * 9;
-      sh.r[3 * c] += p1 * g0; sh.r[3 * c + 1] += p1 * g1; sh.r[3 * c + 2] += p1 * g2;
-      Rc[0] += p2 * g0 * g0 + p1 * h00; Rc[1] += p2 * g0 * g1 + p1 * h01; Rc[2] += p2 * g0 * g2;
-      Rc[3] += p2 * g1 * g0 + p1 * h01; Rc[4] += p2 * g1 * g1 + p1 * h11; Rc[5] += p2 * g1 * g2;
-      Rc[6] += p2 * g2 * g0;            Rc[7] += p2 * g2 * g1;            Rc[8] += p2 * g2 * g2;
+      if (tilt) {
+        // chained through dF_du = t_R_w, whose rows are t1, t2, n (FrictionConeConstraint.cpp:185-196): g = t_R_w' g_l and
+        // H = t_R_w' H_l t_R_w = t1 (h00 t1 + h01 t2)' + t2 (h01 t1 + h11 t2)', H_l having no n row or column
+        double gw[3], m1[3], m2[3];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+          gw[i] = g0 * fr[3 + i] + g1 * fr[6 + i] + g2 * fr[i];
+          m1[i] = h00 * fr[3 + i] + h01 * fr[6 + i]; m2[i] = h01 * fr[3 + i] + h11 * fr[6 + i];
+        }
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+          sh.r[3 * c + i] += p1 * gw[i];
+#pragma unroll
+          for (int j = 0; j < 3; ++j) Rc[3 * i + j] += p2 * gw[i] * gw[j] + p1 * (fr[3 + i] * m1[j] + fr[6 + i] * m2[j]);
+        }
+      } else {
+        sh.r[3 * c] += p1 * g0; sh.r[3 * c + 1] += p1 * g1; sh.r[3 * c + 2] += p1 * g2;
+        Rc[0] += p2 * g0 * g0 + p1 * h00; Rc[1] += p2 * g0 * g1 + p1 * h01; Rc[2] += p2 * g0 * g2;
+        Rc[3] += p2 * g1 * g0 + p1 * h01; Rc[4] += p2 * g1 * g1 + p1 * h11; Rc[5] += p2 * g1 * g2;
+        Rc[6] += p2 * g2 * g0;            Rc[7] += p2 * g2 * g1;            Rc[8] += p2 * g2 * g2;
+      }
       shiftsum = -p1 * HB_FRICTION_HESSIAN_SHIFT;
     }
   }
@@ -944,7 +980,7 @@ __global__ void __launch_bounds__(32, HB_LQ_MINB) lq_kernel(SqpArgs a) {
   const double dt = sqp_dt(a, inst, k);
   const unsigned flm = (contact_flag(mode, 0) ? 1u : 0u) | (contact_flag(mode, 1) ? 2u : 0u) | (contact_flag(mode, 2) ? 4u : 0u) | (contact_flag(mode, 3) ? 8u : 0u);
   double cost, d2;
-  lq_model(sh, lane, flm, nsw, dt, xn_l, xref_l, cost, d2);
+  lq_model(sh, a, inst, k, lane, flm, nsw, dt, xn_l, xref_l, cost, d2);
   if (nsw == 2) lq_node<2>(sh, a, inst, k, lane, flm, dt, cost, d2);
   else if (nsw == 0) lq_node<0>(sh, a, inst, k, lane, flm, dt, cost, d2);
   else lq_node<4>(sh, a, inst, k, lane, flm, dt, cost, d2);
@@ -1529,7 +1565,8 @@ __global__ void __launch_bounds__(32) forward_linesearch2_kernel(SqpArgs a, int 
         double d2 = 0.0;
         for (int i = 0; i < NX; ++i) { const double d = x[i] + 0.5 * dt * (f1[i] + f2[i]) - xn[i]; d2 += d * d; }
         double cost, e2;
-        node_values_lane(x, u, xr, sw, mode[k], ep, ev, a.sth ? a.sth + ((size_t)inst * (NS + 1) + k) * 4 : nullptr, cost, e2);
+        node_values_lane(x, u, xr, sw, mode[k], ep, ev, a.sth ? a.sth + ((size_t)inst * (NS + 1) + k) * 4 : nullptr,
+                         a.cgr ? a.cgr + ((size_t)inst * (NS + 1) + k) * 8 : nullptr, cost, e2);
         ms += dt * cost; ds += dt * d2; es += dt * e2;
       }
       ms = warp_sum(ms); ds = warp_sum(ds); es = warp_sum(es);

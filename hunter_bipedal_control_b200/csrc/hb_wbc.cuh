@@ -68,25 +68,14 @@ __device__ inline void rotation_error_world(const double* Rref, const double* Rm
   for (int i = 0; i < 3; ++i) err[i] = f * sk[i];
 }
 
-// The surface frame of each contact on WBC map m (WBC maps, hunter_b200.h), lane c < 4 for contact c at its measured position sh.pos_m:
-// n = (-gx, -gy, 1) / L, t1 = (1, 0, gx) / sqrt(1 + gx^2), t2 = n x t1, with each product rounded on its own (mul_rn) as the map lookup's,
-// so that a restatement gets the same bits. Where the gradient is zero the contact keeps the flat rows: its n_z is written 0, which no
-// frame has (n_z = 1 / L > 0).
+// The surface frame (n, t1, t2) of each contact on WBC map m (WBC maps, hunter_b200.h; hbplan::map_frame), lane c < 4 for contact c at its
+// measured position sh.pos_m. Where the ground is flat the contact keeps the flat rows: its n_z is written 0, which no frame has
+// (n_z = 1 / L > 0).
 __device__ inline void wbc_contact_frames(const hb_terrain& m, WbcShared& sh) {
-  using hbplan::mul_rn;
   const int c = lane_id();
   if (c >= 4) return;
-  double gx, gy;
-  hbplan::terrain_height<true>(m, sh.pos_m[3 * c], sh.pos_m[3 * c + 1], &gx, &gy);
   double* f = sh.frame + 9 * c;
-  if (gx == 0.0 && gy == 0.0) { f[2] = 0.0; return; }
-  const double L = sqrt(1.0 + mul_rn(gx, gx) + mul_rn(gy, gy)), Lt = sqrt(1.0 + mul_rn(gx, gx));
-  const double n0 = -gx / L, n1 = -gy / L, n2 = 1.0 / L, t0 = 1.0 / Lt, t2 = gx / Lt;
-  f[0] = n0; f[1] = n1; f[2] = n2;
-  f[3] = t0; f[4] = 0.0; f[5] = t2;
-  f[6] = mul_rn(n1, t2) - mul_rn(n2, 0.0);
-  f[7] = mul_rn(n2, t0) - mul_rn(n0, t2);
-  f[8] = mul_rn(n0, 0.0) - mul_rn(n1, t0);
+  if (!hbplan::map_frame(m, sh.pos_m[3 * c], sh.pos_m[3 * c + 1], f)) f[2] = 0.0;
 }
 
 // The surface frames the friction rows of instance `inst` read (wbc_task0_ineq): sh.frame when the instance has a WBC map, null (flat

@@ -187,8 +187,8 @@ int hb_parse_planner_settings(const char* task_info, const char* gait_info, hb_p
  * for later ones), with h_m the height-map lookup (height maps, above; one record means the same ground to the planner, the filter and
  * the MPC). The z row is then (v_z + 3 p_z - 0.06) - 3 h, so the stance foot is held at 0.02 + h; the linearisation's row and the line
  * search's violation use the same h. h depends on the reference, not on the iterate: the row's Jacobian is unchanged and has no grad h
- * coupling (a step of the map is a one-cell ramp, as for estimator maps). Swing rows, friction cones, costs, the WBC, the planner, the
- * filter and the plant do not read MPC maps. An all-zero map (h = +0) is the solve without one bit for bit. Map heights are measured
+ * coupling (a step of the map is a one-cell ramp, as for estimator maps). Swing rows, friction cones (MPC cone maps, below), costs, the
+ * WBC, the planner, the filter and the plant do not read MPC maps. An all-zero map (h = +0) is the solve without one bit for bit. Map heights are measured
  * from the flat ground the MPC otherwise assumes (z = 0), as height maps' are. Maps are read by every MPC path (hb_mpc_set_maps). */
 
 /* ---- WBC maps: the ground the WBC's friction pyramids stand on ----
@@ -203,8 +203,22 @@ int hb_parse_planner_settings(const char* task_info, const char* gait_info, hb_p
  * gy == 0 (a zero map, a plateau cell, a point off the grid on both axes) the rows are the flat rows unchanged, the plant's own flat-path
  * rule, so an all-zero map is the WBC without one bit for bit. The normal is the bilinear gradient the plant's sloped contact pushes along:
  * a foot on a step's one-cell ramp gets the ramp's steep normal, as it does in the plant; there is no smoothing over the foot. Every other
- * WBC row (EoM, torque limits, zero swing forces, no contact motion, swing-leg, base and contact-force tasks), the MPC's friction cone,
- * the planner, the filter and the plant do not read WBC maps. Maps are read by every WBC path (hb_wbc_set_maps). */
+ * WBC row (EoM, torque limits, zero swing forces, no contact motion, swing-leg, base and contact-force tasks), the MPC's friction cone
+ * (MPC cone maps, below), the planner, the filter and the plant do not read WBC maps. Maps are read by every WBC path (hb_wbc_set_maps). */
+
+/* ---- MPC cone maps: the ground the MPC's friction cones stand on ----
+ * An MPC cone map is an hb_terrain record that the MPC's friction cone (FrictionConeConstraint) reads. The reference's cone is
+ * h = mu F_z - sqrt(F_x^2 + F_y^2 + reg) on the local force t_R_w F of each stance contact (FrictionConeConstraint.cpp:78-233), with
+ * t_R_w the identity: a cone about the world z axis. For an instance with a cone map m, at node k and each contact c in stance there,
+ * t_R_w has the rows t1, t2 and n of the WBC maps' frame (above) at the swing reference's position of c at the node (swing_ref[k][6c],
+ * [6c + 1], where MPC maps look up the stance height). The cone is then h = mu Fl_z - sqrt(Fl_x^2 + Fl_y^2 + reg) with
+ * Fl = (t1.F, t2.F, n.F), its input gradient t_R_w' g_l and its input Hessian t_R_w' H_l t_R_w, the reference's chain through
+ * dF_du = t_R_w; the linearisation and the line search's trial cost use the same frame. mu, reg, the relaxed barrier and the Hessian
+ * diagonal shift are unchanged. Where gx == 0 and gy == 0 (a zero map, a plateau cell, a point off the grid on both axes) and for a swing
+ * contact the cone's statements are those without a map, so an all-zero map is the solve without one bit for bit. The frame depends on
+ * the reference, not on the iterate. The normal-force limits on u[3c + 2] stay on world z: they are the reference's box on that input,
+ * and the tilted cone itself keeps the force's normal component positive (mu Fl_z >= sqrt(reg)). The stance z row (MPC maps, above), the
+ * swing rows, the costs, the WBC, the planner, the filter and the plant do not read cone maps. Cone maps are read by every MPC path (hb_mpc_set_cone_maps). */
 
 /* state of the speed-based gait selection of one instance (SwitchedModelReferenceManager velAbsHistory_/velAvg_/gaitLevel_);
  * zero-initialise, then set gait_level = -1 ("no template chosen yet") or the level in force */
@@ -457,6 +471,7 @@ typedef struct {                 /* the bodies of one robot, relative to the nom
 #define HB_SETTING_ESTIMATOR_MAPS 15          /* hb_terrain for hb_estimator_set_maps (hb_check_setting_records), as _TERRAINS      */
 #define HB_SETTING_MPC_MAPS 17                /* hb_terrain for hb_mpc_set_maps (hb_check_setting_records), as _TERRAINS; 16 unused */
 #define HB_SETTING_WBC_MAPS 18                /* hb_terrain for hb_wbc_set_maps (hb_check_setting_records), as _TERRAINS            */
+#define HB_SETTING_MPC_CONE_MAPS 19           /* hb_terrain for hb_mpc_set_cone_maps (hb_check_setting_records), as _TERRAINS       */
 int hb_default_link_variation(hb_link_variation* r);      /* host only: every scale 1, every shift 0 */
 /* Sets the link variations of the context's episodes (a per-robot episode setting, above). -1 also for a value that is not finite, a
  * mass_scale <= 0 or an inertia_scale <= 0. */
@@ -466,8 +481,9 @@ int hb_rollout_set_link_variations(hb_ctx* ctx, int B, const hb_link_variation* 
  * The terrain acts on the simulated plant and on the height failure check only; the planner, MPC, WBC, joint command law, actuation
  * model and estimator keep assuming flat ground at z = 0 and are not told about it. The planner can be told where the ground is by a
  * height map (height maps, above; hb_plan_set_maps), the estimator's feet heights by an estimator map (estimator maps, above;
- * hb_estimator_set_maps), the MPC's stance feet by an MPC map (MPC maps, above; hb_mpc_set_maps) and the WBC's friction pyramids by a
- * WBC map (WBC maps, above; hb_wbc_set_maps), records of this type each set on its own.
+ * hb_estimator_set_maps), the MPC's stance feet by an MPC map (MPC maps, above; hb_mpc_set_maps), the WBC's friction pyramids by a
+ * WBC map (WBC maps, above; hb_wbc_set_maps) and the MPC's friction cones by an MPC cone map (MPC cone maps, above;
+ * hb_mpc_set_cone_maps), records of this type each set on its own.
  * Height and gradient at a world point (x, y): u = (x - origin[0]) / spacing clamped to [0, nx - 1], i = min(floor(u), nx - 2),
  * a = u - i; the same for y gives w, j and b. With lerp(p, q, s) = p + s (q - p): h0 = lerp(h[j][i], h[j][i+1], a),
  * h1 = lerp(h[j+1][i], h[j+1][i+1], a), h = lerp(h0, h1, b); g_x = lerp(h[j][i+1] - h[j][i], h[j+1][i+1] - h[j+1][i], b) / spacing,
@@ -893,6 +909,13 @@ int hb_mpc_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
  * for B > max_batch, a rejected call keeps the previous setting. No launch is added, set or not. Maps are a setting, not episode state:
  * hb_episode_state_bytes and snapshots do not count them. */
 int hb_wbc_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
+/* MPC cone maps of the context (MPC cone maps, above): instance i < B of every MPC path -- the paths of hb_mpc_set_maps -- has its stance
+ * contacts' friction cones about maps[i]'s surface frames; instances at or beyond B, and every instance while none is set, keep the cones
+ * about world z. A setting of its own, apart from the MPC maps, so that either can be measured alone. The contract of hb_plan_set_maps:
+ * host array validated and copied in stream order, B == 0 clears (maps may be NULL), -1 for a record hb_rollout_set_terrains rejects, -4
+ * for B > max_batch, a rejected call keeps the previous setting. No launch is added, set or not. Maps are a setting, not episode state:
+ * hb_episode_state_bytes and snapshots do not count them. */
+int hb_mpc_set_cone_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
 /* One estimator update per instance (StateEstimateBase::updateJointStates / updateImu, StateEstimateBase.cpp:73-106, then
  * KalmanFilterEstimate::update): quat = (x, y, z, w); contact_flag: B x 4 (0 = the filter distrusts that foot, x100 noise);
  * rbd_out: B x 32 measured rbd state [zyx, p, q_j, omega_world, v, qd_j]. zyxOffset_ is taken as zero. The odometry fusion

@@ -51,6 +51,12 @@ above plus one, with_wbc_maps, with WBC maps added to every map the run gives, a
 with all-zero WBC maps and without WBC maps, alternately; the tool asserts that all-zero WBC maps give the outcome of no WBC maps bit for
 bit.
 
+--mpc-cone-maps (with --height-maps) also stands the MPC's friction cones on the ground (hb_mpc_set_cone_maps), with the same maps: each
+stance contact's cone bounds its force in the map's surface frame at its swing reference instead of about the world z axis. The line
+reports the tables above plus one, with_cone_maps, with MPC cone maps added to every map the run gives, and times episodes with cone maps
+against the same episodes with all-zero cone maps and without cone maps, alternately; the tool asserts that all-zero cone maps give the
+outcome of no cone maps bit for bit.
+
 --friction-scale S scales every robot's ground friction by S in every table (hb_rollout_set_plant_variations, friction_scale) and runs its
 WBC with friction_coefficient S times the context's (task.info's) value (hb_rollout_set_controller_settings): the slope's direction
 matters most to the friction pyramids where friction is short.
@@ -103,56 +109,65 @@ def height_map_sweep(h, args, grid):
     T_episode = TICKS * prm.period
 
     def set_all(value):
-        terrains, maps, est_maps, mpc_maps, wbc_maps = value
+        terrains, maps, est_maps, mpc_maps, wbc_maps, cone_maps = value
         ctx.set_terrains(terrains)
         ctx.set_height_maps(maps)
         ctx.set_estimator_maps(est_maps)
         ctx.set_mpc_maps(mpc_maps)
         ctx.set_wbc_maps(wbc_maps)
+        ctx.set_mpc_cone_maps(cone_maps)
 
-    def settings(shift, planner, estimator, mpc=False, wbc=False):
+    def settings(shift, planner, estimator, mpc=False, wbc=False, cone=False):
         origin, heights = grid(shift)
         maps = hb.make_terrains(B, heights - GROUND, SPACING, origin)
         return (hb.make_terrains(B, heights, SPACING, origin), maps if planner else None, maps if estimator else None, maps if mpc else None,
-                maps if wbc else None)
+                maps if wbc else None, maps if cone else None)
 
     tables = [("blind", False, False), ("mapped", True, False)]
     if args.estimator_maps:
         tables = [("blind", False, False), ("planner_maps", True, False), ("estimator_maps", False, True), ("both_maps", True, True)]
-    tables = [t + (False, False) for t in tables]
+    tables = [t + (False, False, False) for t in tables]
     if args.mpc_maps:
-        tables.append(("all_maps", True, True, True, False) if args.estimator_maps else ("planner_mpc_maps", True, False, True, False))
+        tables.append(("all_maps", True, True, True, False, False) if args.estimator_maps else ("planner_mpc_maps", True, False, True, False, False))
     if args.wbc_maps:
-        tables.append(("with_wbc_maps", True, args.estimator_maps, args.mpc_maps, True))
+        tables.append(("with_wbc_maps", True, args.estimator_maps, args.mpc_maps, True, False))
+    if args.mpc_cone_maps:
+        tables.append(("with_cone_maps", True, args.estimator_maps, args.mpc_maps, args.wbc_maps, True))
     out, mk = {}, [str(m) for m in MAGNITUDES]
-    for name, planner, estimator, mpc, wbc in tables:
+    for name, planner, estimator, mpc, wbc, cone in tables:
         tally = Tally(len(MAGNITUDES), len(KINDS))
-        for r, run in h.sweep(set_all, lambda shift: settings(shift, planner, estimator, mpc, wbc)):
+        for r, run in h.sweep(set_all, lambda shift: settings(shift, planner, estimator, mpc, wbc, cone)):
             tally.add(*cells(B, len(MAGNITUDES), len(KINDS), r), run.stats, value=np.hypot(*(run.rbd[:, 3:5] - rbd0[:, 3:5]).T) / T_episode)
         out[name] = {"largest_magnitude_90pct": dict(zip(KINDS, tally.largest(MAGNITUDES))), "survival": keyed(KINDS, mk, tally.survival().tolist()),
                      "mean_speed_of_survivors_m_per_s": keyed(KINDS, mk, tally.mean()), "fail_reasons": tally.reasons}
-    terrains, maps, _, _, _ = settings(0, True, True)
+    terrains, maps, _, _, _, _ = settings(0, True, True)
     origin, heights = grid(0)
     zero = hb.make_terrains(B, np.zeros_like(heights), SPACING, origin)
     est = maps if args.estimator_maps else None
-    if args.wbc_maps:
+    if args.mpc_cone_maps:
+        mpc, wbc = (maps if args.mpc_maps else None), (maps if args.wbc_maps else None)
+        _, clocks, timing = h.alternate(set_all, [("cone_maps", (terrains, maps, est, mpc, wbc, maps)),
+                                                  ("zero_cone_maps", (terrains, maps, est, mpc, wbc, zero)),
+                                                  ("no_cone_maps", (terrains, maps, est, mpc, wbc, None))], args.timed, launches=True)
+        assert timing["zero_cone_maps_same_outcome_as_no_cone_maps"], "all-zero MPC cone maps changed the outcome of no cone maps"
+    elif args.wbc_maps:
         mpc = maps if args.mpc_maps else None
-        _, clocks, timing = h.alternate(set_all, [("wbc_maps", (terrains, maps, est, mpc, maps)), ("zero_wbc_maps", (terrains, maps, est, mpc, zero)),
-                                                  ("no_wbc_maps", (terrains, maps, est, mpc, None))], args.timed, launches=True)
+        _, clocks, timing = h.alternate(set_all, [("wbc_maps", (terrains, maps, est, mpc, maps, None)), ("zero_wbc_maps", (terrains, maps, est, mpc, zero, None)),
+                                                  ("no_wbc_maps", (terrains, maps, est, mpc, None, None))], args.timed, launches=True)
         assert timing["zero_wbc_maps_same_outcome_as_no_wbc_maps"], "all-zero WBC maps changed the outcome of no WBC maps"
     elif args.mpc_maps:
-        _, clocks, timing = h.alternate(set_all, [("mpc_maps", (terrains, maps, est, maps, None)), ("zero_mpc_maps", (terrains, maps, est, zero, None)),
-                                                  ("no_mpc_maps", (terrains, maps, est, None, None))], args.timed, launches=True)
+        _, clocks, timing = h.alternate(set_all, [("mpc_maps", (terrains, maps, est, maps, None, None)), ("zero_mpc_maps", (terrains, maps, est, zero, None, None)),
+                                                  ("no_mpc_maps", (terrains, maps, est, None, None, None))], args.timed, launches=True)
         assert timing["zero_mpc_maps_same_outcome_as_no_mpc_maps"], "all-zero MPC maps changed the outcome of no MPC maps"
     elif args.estimator_maps:
-        _, clocks, timing = h.alternate(set_all, [("both_maps", (terrains, maps, maps, None, None)),
-                                                  ("zero_estimator_maps", (terrains, maps, zero, None, None)),
-                                                  ("planner_maps", (terrains, maps, None, None, None))], args.timed, launches=True)
+        _, clocks, timing = h.alternate(set_all, [("both_maps", (terrains, maps, maps, None, None, None)),
+                                                  ("zero_estimator_maps", (terrains, maps, zero, None, None, None)),
+                                                  ("planner_maps", (terrains, maps, None, None, None, None))], args.timed, launches=True)
         assert timing["zero_estimator_maps_same_outcome_as_planner_maps"], "all-zero estimator maps changed the outcome of planner maps only"
     else:
-        _, clocks, timing = h.alternate(set_all, [("mapped", (terrains, maps, None, None, None)), ("zero_maps", (terrains, zero, None, None, None)),
-                                                  ("blind", (terrains, None, None, None, None))], args.timed, launches=True)
-    set_all((None, None, None, None, None))
+        _, clocks, timing = h.alternate(set_all, [("mapped", (terrains, maps, None, None, None, None)), ("zero_maps", (terrains, zero, None, None, None, None)),
+                                                  ("blind", (terrains, None, None, None, None, None))], args.timed, launches=True)
+    set_all((None, None, None, None, None, None))
     return out, clocks, timing
 
 
@@ -162,14 +177,15 @@ def main():
         ap.add_argument("--estimator-maps", action="store_true", help="with --height-maps --estimator: also give the Kalman filter the maps")
         ap.add_argument("--mpc-maps", action="store_true", help="with --height-maps: also hold the MPC's stance feet on the maps")
         ap.add_argument("--wbc-maps", action="store_true", help="with --height-maps: also tilt the WBC's friction pyramids on the maps")
+        ap.add_argument("--mpc-cone-maps", action="store_true", help="with --height-maps: also stand the MPC's friction cones on the maps")
         ap.add_argument("--friction-scale", type=float, default=1.0, help="scale of every robot's ground friction and WBC friction coefficient")
 
     args = sweep_args("terrain_sweep.py", "timed terrain / flat / unset episode triples (with --height-maps: mapped / zero-map / blind)",
                       len(KINDS) * len(MAGNITUDES), extra=extra,
                       valid=lambda a: ((not a.estimator_maps or (a.height_maps and a.estimator)) and (not a.mpc_maps or a.height_maps)
-                                       and (not a.wbc_maps or a.height_maps) and a.friction_scale > 0),
+                                       and (not a.wbc_maps or a.height_maps) and (not a.mpc_cone_maps or a.height_maps) and a.friction_scale > 0),
                       needs="--estimator-maps needs --height-maps --estimator, --mpc-maps needs --height-maps, "
-                            "--wbc-maps needs --height-maps, --friction-scale takes a scale > 0, ")
+                            "--wbc-maps needs --height-maps, --mpc-cone-maps needs --height-maps, --friction-scale takes a scale > 0, ")
     h = Episodes("terrain_sweep.py", args, TICKS)
     hb, ctx, prm, B, rbd0 = h.hb, h.ctx, h.prm, h.B, h.rbd0
     step_ahead, ramp_ahead = feature_distances(rbd0, h.feet)
@@ -185,7 +201,13 @@ def main():
             return terrain_heights(rbd0, np.array(KINDS)[ki], np.array(MAGNITUDES)[mi], step_ahead, ramp_ahead)
 
         out, clocks, timing = height_map_sweep(h, args, grid)
-        if args.wbc_maps:
+        if args.mpc_cone_maps:
+            metric = ("MPC cone maps: the highest step [cm] that >= 90 %% of the trotting robots cross within %.1f s%s when the planner%s%s%s "
+                      "and the MPC's friction cones are told the terrain; %s tables per kind (steps in cm, slopes in degrees)"
+                      % (T_episode, " through the estimator" if args.estimator else "", ", the Kalman filter" if args.estimator_maps else "",
+                         ", the MPC's stance feet" if args.mpc_maps else "", ", the WBC" if args.wbc_maps else "", ", ".join(out)))
+            value = out["with_cone_maps"]["largest_magnitude_90pct"]["step_up"]
+        elif args.wbc_maps:
             metric = ("WBC maps: the highest step [cm] that >= 90 %% of the trotting robots cross within %.1f s%s when the planner%s%s and "
                       "the WBC are told the terrain; %s tables per kind (steps in cm, slopes in degrees)"
                       % (T_episode, " through the estimator" if args.estimator else "", ", the Kalman filter" if args.estimator_maps else "",
@@ -216,7 +238,8 @@ def main():
                        "height_maps": "each robot's terrain minus %g m (hb_plan_set_maps%s%s); blind: no map"
                                       % (GROUND, ", and the same maps with hb_estimator_set_maps" if args.estimator_maps else "",
                                          ", and the same maps with hb_mpc_set_maps in the last table" if args.mpc_maps else "")
-                                      + (", and the same maps with hb_wbc_set_maps in with_wbc_maps" if args.wbc_maps else ""),
+                                      + (", and the same maps with hb_wbc_set_maps in with_wbc_maps" if args.wbc_maps else "")
+                                      + (", and the same maps with hb_mpc_set_cone_maps in with_cone_maps" if args.mpc_cone_maps else ""),
                        "friction_scale": args.friction_scale,
                        "survival": "robots still up at the end of the episode", "failure_checks": failure_checks("base z above the terrain")}}))
         return
