@@ -14,7 +14,8 @@ from .api import (HbWbcSettings, HbTaskInfo, parse_task_info, Context, WeightedW
                   NBODY, HbLinkVariation, default_link_variation, make_link_variations,
                   HB_MAX_TELEOP_WINDOWS, TELEOP_ALWAYS, HbTeleop, HbTeleopSetting, default_teleop_setting, make_teleop_settings, cmd_vel_to_target,
                   HB_GAIT_MAX_PHASES, HbGaitTemplate, HbPlannerSettings, gait_template, default_planner_settings, parse_planner_settings, make_planner_settings,
-                  CHANNELS, make_channels, EpisodeSnapshot, reseed)
+                  CHANNELS, make_channels, EpisodeSnapshot, reseed,
+                  HbContactDetection, default_contact_detection, make_contact_detection_settings, contact_state_host)
 
 __all__ = ["HbWbcSettings", "HbTaskInfo", "parse_task_info", "Context", "WeightedWbc", "HierarchicalWbc", "HbHoqpProblem", "make_hoqp_problems", "hoqp_tasks", "SqpMpc", "HbReference", "HbSolveInfo", "HbConfig", "HunterB200Error", "load_library",
            "EXPORTED_SYMBOLS", "NX", "NU", "NQ", "NJ", "NWBC", "INFO_DTYPE", "HbPlanInput", "plan_references", "plan_set_threads", "make_plan_inputs", "GAIT_IDS", "GaitSelector", "HbPdGains", "default_pd_gains", "HbKfState", "HbKfParams", "default_kf_params", "kf_states", "HbObserverState", "observer_states", "HbActuationState", "HbSimParams", "default_sim_params", "actuation_states",
@@ -27,4 +28,5 @@ __all__ = ["HbWbcSettings", "HbTaskInfo", "parse_task_info", "Context", "Weighte
            "NBODY", "HbLinkVariation", "default_link_variation", "make_link_variations",
            "HB_MAX_TELEOP_WINDOWS", "TELEOP_ALWAYS", "HbTeleop", "HbTeleopSetting", "default_teleop_setting", "make_teleop_settings", "cmd_vel_to_target",
            "HB_GAIT_MAX_PHASES", "HbGaitTemplate", "HbPlannerSettings", "gait_template", "default_planner_settings", "parse_planner_settings", "make_planner_settings",
-           "CHANNELS", "make_channels", "EpisodeSnapshot", "reseed"]
+           "CHANNELS", "make_channels", "EpisodeSnapshot", "reseed",
+           "HbContactDetection", "default_contact_detection", "make_contact_detection_settings", "contact_state_host"]

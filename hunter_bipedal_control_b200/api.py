@@ -62,6 +62,8 @@ EXPORTED_SYMBOLS = [
     "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
     "hb_plan_set_maps", "hb_plan_references_maps", "hb_goal_to_target_maps", "hb_cmd_vel_to_target_maps", "hb_estimator_set_maps",
     "hb_mpc_set_maps", "hb_wbc_set_maps", "hb_mpc_set_cone_maps",
+    "hb_default_contact_detection", "hb_rollout_set_contact_detection", "hb_contact_state_estimate_async", "hb_contact_state_estimate",
+    "hb_rollout_contact_estimates", "hb_contact_state_host",
     "hb_check_setting_records", "hb_rollout_set_channel",
     "hb_episode_state_bytes", "hb_episode_save_async", "hb_episode_restore",
 ]
@@ -264,6 +266,61 @@ def parse_task_info(path):
     ti = HbTaskInfo()
     _check(load_library().hb_parse_task_info(str(path).encode(), C.byref(ti)), "hb_parse_task_info")
     return ti
+
+
+class HbContactDetection(C.Structure):
+    SETTING_KIND = 20        # HB_SETTING_CONTACT_DETECTION, the record's kind for hb_check_setting_records
+    _fields_ = [("cutoff_frequency", C.c_double), ("threshold", C.c_double), ("swing_fraction", C.c_double), ("stance_fraction", C.c_double)]
+
+
+def default_contact_detection(task=None):
+    """hb_default_contact_detection: the observer's cutoff and the contact threshold of task (an HbTaskInfo, or the path of a task.info
+    file; None: 250 and 75), with the reference's fractions 0.75 and 0.25."""
+    if task is not None and not isinstance(task, HbTaskInfo):
+        task = parse_task_info(task)
+    r = HbContactDetection()
+    _check(load_library().hb_default_contact_detection(None if task is None else C.byref(task), C.byref(r)), "hb_default_contact_detection")
+    return r
+
+
+def make_contact_detection_settings(B, base=None, **fields):
+    """ctypes array of B HbContactDetection (Context.set_contact_detection): each robot's contact detection in rollout_estimated. base
+    (HbContactDetection, default default_contact_detection()) is the base of every record; any field can be given by name as a scalar or a
+    (B,) array. Raises ValueError for an unknown name, a shape that does not broadcast, and a record the setter rejects, naming the first."""
+    base = default_contact_detection() if base is None else base
+    out = (HbContactDetection * B)()
+    v = np.ctypeslib.as_array(out)
+    v[:] = np.frombuffer(bytes(base), dtype=v.dtype)[0]
+    for name, value in fields.items():
+        if name not in v.dtype.names:
+            raise ValueError("contact detection: unknown field %r" % name)
+        try:
+            v[name] = np.broadcast_to(_f64(value), (B,))
+        except ValueError as e:
+            raise ValueError("contact detection: %s: (B,) or a scalar expected: %s" % (name, e))
+    return _check_records(HbContactDetection.SETTING_KIND, out, "contact_detection")
+
+
+def _contact_records(records, B, what):
+    """records (None, a ctypes array or a sequence of B HbContactDetection) as a ctypes array or None, or ValueError."""
+    if records is None:
+        return None
+    if len(records) != B:
+        raise ValueError("%s: %d records for %d instances" % (what, len(records), B))
+    return records if isinstance(records, C.Array) else (HbContactDetection * B)(*records)
+
+
+def contact_state_host(t, est, est_force, records, flags):
+    """The contact detection rule on the host (hb_contact_state_host): est (ctypes array of B HbEstimationState, the stored schedules),
+    est_force [B,16] (the observer's output), records (B HbContactDetection, or None: flags unchanged) and the schedule's flags [B,4] at
+    time t. Returns (the detected flags [B,4] uint8, the phase times [B,4,2]: start and stop of each contact's run around t)."""
+    B = len(est)
+    force = _f64(est_force).reshape(B, 16)
+    fl = np.ascontiguousarray(flags, dtype=np.uint8).reshape(B, 4).copy()
+    times = np.zeros((B, 4, 2))
+    _check(load_library().hb_contact_state_host(B, C.c_double(t), est, _ptr(force), _contact_records(records, B, "contact_state_host"), _ptr(fl),
+                                                _ptr(times)), "hb_contact_state_host")
+    return fl, times
 
 
 HB_ACT_CAPACITY = 16
@@ -1549,6 +1606,30 @@ class Context:
         at its swing reference's (x, y). A setting of its own, apart from set_mpc_maps. Instances beyond len(maps) keep the cones about
         world z; None clears them."""
         self._set_instances("hb_mpc_set_cone_maps", maps)
+
+    def set_contact_detection(self, records):
+        """Contact detection of this context's estimated episodes (hb_rollout_set_contact_detection): records[i]
+        (make_contact_detection_settings) makes instance i of every later rollout_estimated call run the momentum observer on each tick and
+        hand its Kalman filter the flags of estContactState instead of the schedule's; instances beyond len(records), rollout and every
+        other call run without it; None clears it. Every call clears the detection state (observer, effort, flags)."""
+        self._set_instances("hb_rollout_set_contact_detection", records)
+
+    def contact_state_estimate(self, t, est, est_force, records, flags):
+        """The detection rule on the device (hb_contact_state_estimate): est (ctypes array of B HbEstimationState), est_force [B,16],
+        records (B HbContactDetection, or None: flags unchanged) and the schedule's flags [B,4] at time t. Returns the detected flags [B,4]."""
+        B = len(est)
+        force = _f64(est_force).reshape(B, 16)
+        fl = np.ascontiguousarray(flags, dtype=np.uint8).reshape(B, 4).copy()
+        _check(self._lib.hb_contact_state_estimate(self._h, B, C.c_double(t), est, _ptr(force), _contact_records(records, B, "contact_state_estimate"),
+                                                   _ptr(fl)), "hb_contact_state_estimate", self._h)
+        return fl
+
+    def contact_estimates(self, B):
+        """The detection state of instances 0 .. B-1 (hb_rollout_contact_estimates): (the last observer output [B,16], the flags the filter
+        last used [B,4])."""
+        force = np.zeros((B, 16)); fl = np.zeros((B, 4), dtype=np.uint8)
+        _check(self._lib.hb_rollout_contact_estimates(self._h, B, _ptr(force), _ptr(fl)), "hb_rollout_contact_estimates", self._h)
+        return force, fl
 
     def resident_wbc(self, t_now, rbd, stance_mode=None):
         """Policy of the resident solution at absolute time t_now + WeightedWbc: returns (x_des, u_des, mode, sol, torque, status)."""

@@ -134,6 +134,11 @@ struct hb_ctx {
   void* cgr_mem; double* cgr;
   // each instance's WBC map in every WBC path: the surface normals of the friction pyramids (hb_wbc_set_maps)
   InstanceSetting<hb_terrain> wbc_maps;
+  // each instance's contact detection in the estimated episodes (hb_rollout_set_contact_detection) and its state, allocated at max_batch
+  // by the first call that sets records; the staged records of the last hb_contact_state_estimate_async
+  InstanceSetting<hb_contact_detection> contact_detection, contact_call;
+  void* cd_mem;
+  ContactDetectState* cd_state;
   // the recorded channels of the episodes (hb_rollout_set_channel): the caller's buffer, its instances and rows; B == 0: unset
   struct { void* buf; int B, rows; } channels[HB_CHANNELS];
   // the episode snapshots' staging (hb_episode_save_async / hb_episode_restore), allocated at max_batch by their first call: the rows'
@@ -524,7 +529,8 @@ int hb_destroy(hb_ctx* ctx) {
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
                        ctx->odometry.dev, ctx->controllers.dev, ctx->hardware.dev, ctx->plan_settings.dev,
                        ctx->bridges.dev, ctx->links.dev, ctx->height_maps.dev, ctx->estimator_maps.dev,
-                       ctx->mpc_maps.dev, ctx->sth_mem, ctx->wbc_maps.dev, ctx->cone_maps.dev, ctx->cgr_mem};
+                       ctx->mpc_maps.dev, ctx->sth_mem, ctx->wbc_maps.dev, ctx->cone_maps.dev, ctx->cgr_mem,
+                       ctx->contact_detection.dev, ctx->contact_call.dev, ctx->cd_mem};
   for (void* p : mem) if (p) cudaFree(p);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->prof_ev) { for (int i = 0; i < 2 * PROF_MAX; ++i) cudaEventDestroy(ctx->prof_ev[i]); delete[] ctx->prof_ev; delete[] ctx->prof_kind; }
@@ -1431,6 +1437,81 @@ int hb_rollout_set_controller_settings(hb_ctx* ctx, int B, const hb_controller_s
   return set_instances(ctx, B, s, controller_setting_ok, &hb_ctx::controllers);
 }
 
+// The ranges of hunter_b200.h's hb_contact_detection: the observer's cutoff as hb_contact_force_estimate_batch takes it, a finite
+// threshold, fractions in [0, 1]
+static bool contact_detection_ok(const hb_contact_detection& r) {
+  return cutoff_ok(r.cutoff_frequency, 1.0) && isfinite(r.threshold) && r.swing_fraction >= 0.0 && r.swing_fraction <= 1.0 &&
+         r.stance_fraction >= 0.0 && r.stance_fraction <= 1.0;
+}
+
+int hb_default_contact_detection(const hb_task_info* task, hb_contact_detection* out) {
+  if (!out) return HB_EINVAL;
+  out->cutoff_frequency = task ? task->contact_force_cutoff_frequency : 250.0;
+  out->threshold = task ? task->contact_threshold : 75.0;
+  out->swing_fraction = 0.75; out->stance_fraction = 0.25;
+  return HB_OK;
+}
+
+int hb_rollout_set_contact_detection(hb_ctx* ctx, int B, const hb_contact_detection* records) {
+  // Whatever can fail runs before the setting changes, so that a failed call keeps the previous one: the checks, the state's allocation
+  // (at max_batch, by the first call that sets records) and the host image of the cleared state.
+  int rc = enter(ctx, B, B == 0 || records, CAPPED, [&] { return all_ok(B, records, contact_detection_ok); });
+  if (rc && rc != EMPTY) return rc;
+  const size_t Bc = ctx->cfg.max_batch;
+  if (B > 0 && reserve_group(&ctx->cd_mem, [&](void* m) {
+        size_t off = 0;
+        ctx->cd_state = carve<ContactDetectState>(m, off, Bc);
+        return off;
+      })) return HB_ENOMEM;
+  // every instance's state cleared, by a clearing call too (once a setting has been made); a pageable copy, consumed when cudaMemcpyAsync
+  // returns
+  std::vector<ContactDetectState> clear;
+  if (ctx->cd_mem) {
+    try { clear.resize(Bc); } catch (const std::bad_alloc&) { return HB_ENOMEM; }
+    for (ContactDetectState& d : clear) contact_detect_clear(d);
+  }
+  rc = set_instances(ctx, B, records, contact_detection_ok, &hb_ctx::contact_detection);
+  if (rc || !ctx->cd_mem) return rc;         // rejected, or cleared and never set: no state exists
+  if (set_device(ctx)) return HB_ECUDA;      // a clearing call does not pass set_instances' switch to the device
+  CK(cudaMemcpyAsync(ctx->cd_state, clear.data(), sizeof(ContactDetectState) * Bc, cudaMemcpyHostToDevice, ctx->stream));
+  return HB_OK;
+}
+
+int hb_contact_state_estimate_async(hb_ctx* ctx, int B, double t, const hb_estimation_state* est, const double* est_force,
+                                    const hb_contact_detection* records, uint8_t* flags) {
+  ENTER(ctx, B, est && est_force && flags, CAPPED, [&] { return all_ok(B, records, contact_detection_ok); });
+  if (!records) return HB_OK;                // no record: the flags stay the schedule's
+  const int rc = set_instances(ctx, B, records, contact_detection_ok, &hb_ctx::contact_call);
+  if (rc) return rc;
+  return launch(ctx, K_UNPROFILED, contact_state_kernel, (B + 63) / 64, 64, 0, B, t, est, est_force, ctx->contact_call.view(), flags);
+}
+
+int hb_contact_state_host(int B, double t, const hb_estimation_state* est, const double* est_force, const hb_contact_detection* records,
+                          uint8_t* flags, double* phase_times) {
+  if (B < 0 || (B > 0 && !(est && est_force && flags)) || !all_ok(B, records, contact_detection_ok)) return HB_EINVAL;
+  for (int i = 0; i < B; ++i) {
+    const hb_estimation_state& e = est[i];
+    double s[4], en[4];
+    hbplan::contact_phase_times(e.has_plan, e.n_events, e.event_times, e.modes, t, s, en);
+    if (phase_times) for (int c = 0; c < 4; ++c) { phase_times[8 * i + 2 * c] = s[c]; phase_times[8 * i + 2 * c + 1] = en[c]; }
+    if (records) hbplan::contact_state(records[i], t, s, en, est_force + 16 * (size_t)i, flags + 4 * (size_t)i);
+  }
+  return HB_OK;
+}
+
+int hb_rollout_contact_estimates(hb_ctx* ctx, int B, double* est_force, uint8_t* flags) {
+  ENTER(ctx, B, true, CAPPED, [&] { return ctx->cd_mem != nullptr; });
+  const size_t pitch = sizeof(ContactDetectState);
+  const char* st = reinterpret_cast<const char*>(ctx->cd_state);
+  int rc = HB_OK;
+  if (est_force && cudaMemcpy2DAsync(est_force, sizeof(double) * 16, st + offsetof(ContactDetectState, force), pitch, sizeof(double) * 16, B,
+                                     cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) rc = HB_ECUDA;
+  if (!rc && flags && cudaMemcpy2DAsync(flags, 4, st + offsetof(ContactDetectState, flags), pitch, 4, B, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess)
+    rc = HB_ECUDA;
+  if (rc) { ctx->last_cuda = (int)cudaGetLastError(); }
+  return drain(ctx, rc);
+}
+
 int hb_check_setting_records(int32_t kind, int B, const void* records, int32_t* first_bad) {
   if (!first_bad) return HB_EINVAL;
   *first_bad = -1;
@@ -1454,6 +1535,7 @@ int hb_check_setting_records(int32_t kind, int B, const void* records, int32_t* 
     case HB_SETTING_MPC_MAPS: return check_records(B, records, terrain_ok, first_bad);
     case HB_SETTING_MPC_CONE_MAPS: return check_records(B, records, terrain_ok, first_bad);
     case HB_SETTING_WBC_MAPS: return check_records(B, records, terrain_ok, first_bad);
+    case HB_SETTING_CONTACT_DETECTION: return check_records(B, records, contact_detection_ok, first_bad);
     default: return HB_EINVAL;
   }
 }
@@ -1659,6 +1741,9 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
   const BridgeView bridges = ctx->bridges.view();               // each instance's motor bridge, none without a setting
   MotorDrive drive{bridges, ctx->ro_mcmd, nullptr, hardware, {}, ctx->ro_tau};
   for (int j = 0; j < NJ; ++j) drive.lim[j] = p->torque_limit[j];
+  // each instance's contact detection and its state, none without a setting or in a truth episode
+  const bool detect = e && ctx->contact_detection.n > 0;
+  const ContactDetect det = detect ? ContactDetect{ctx->contact_detection.view(), ctx->cd_state} : ContactDetect{};
   for (int k = 0; k < n_ticks && !rc; ++k) {
     const int64_t a = tick0 + k;
     const double t = (double)a * p->period;           // a product, never an accumulated sum: a stepwise caller reproduces it exactly
@@ -1671,10 +1756,11 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
       // LeggedController::updateStateEstimation: sensors and contact flags at the previous observation's time, filter, observation step
       double* est_row = (n_est_log && k % p->log_every == 0) ? e->log + (size_t)(k / p->log_every) * 32 : nullptr;
       rc = launch(ctx, K_UNPROFILED, sensor_read_kernel, grid, 64, 0, B, e->ep->noise, hardware, bridges, (uint32_t)a, p->sim.dt, (double)(a - 1) * p->period, rbd,
-                  e->est, ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag, odom_read);
+                  e->est, ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag, odom_read, det);
       if (!rc) rc = launch(ctx, K_UNPROFILED, odom ? kf_update_kernel<hb_estimation_state, true> : kf_update_kernel<hb_estimation_state, false>, B, 32,
                            sizeof(KfShared), B, e->ep->kf, p->period, e->est, ctx->re_quat, ctx->re_gyro, ctx->re_acc, ctx->re_jpos, ctx->re_jvel, ctx->re_flag,
                            meas, (const double*)ctx->re_opos, (const uint8_t*)ctx->re_ohas, ctx->estimator_maps.view());
+      if (!rc && detect) rc = launch(ctx, K_UNPROFILED, contact_observe_kernel, B, 32, 0, B, p->period, det.set, det.st, (const double*)meas);
       if (!rc) rc = launch(ctx, K_UNPROFILED, est_observe_kernel, grid, 64, 0, B, rbd, meas, stats, e->est, e->stats, est_row, (size_t)n_est_log * 32);
     }
     // MPC_MRT_Interface::updatePolicy of the instances whose solution comes into force on this tick, before this tick's cycle
@@ -1710,7 +1796,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
       src.mpc = mpc ? 1 : 0;
       rc = launch(ctx, K_UNPROFILED, rollout_record_kernel, (unsigned)(((size_t)B * rec.width + 127) / 128), 128, 0, B, rec, src);
     }
-    if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_tick_end_kernel, grid, 64, 0, B, (int)a, mpc ? 1 : 0, ctx->ro_info, ctx->ro_pstat, ctx->wstatus, estop, ctx->ro_tau, ctx->ro_held, rbd, stats);
+    if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_tick_end_kernel, grid, 64, 0, B, (int)a, mpc ? 1 : 0, ctx->ro_info, ctx->ro_pstat, ctx->wstatus, estop, ctx->ro_tau, ctx->ro_held, rbd, stats, det);
   }
   return rc;
 }
@@ -1753,7 +1839,8 @@ struct EpisodeTable {
     if (grid) add(r.nn, sizeof(int32_t));
   }
 };
-static_assert(sizeof(hb_target) % 4 == 0 && sizeof(OdomCamera) % 4 == 0 && sizeof(TeleopState) % 4 == 0, "snapshot segments are copied in 4-byte units");
+static_assert(sizeof(hb_target) % 4 == 0 && sizeof(OdomCamera) % 4 == 0 && sizeof(TeleopState) % 4 == 0 && sizeof(ContactDetectState) % 4 == 0,
+              "snapshot segments are copied in 4-byte units");
 
 static EpisodeSegments episode_segments(const hb_ctx* ctx, int64_t* head) {
   const size_t N = ctx->cfg.horizon_N;
@@ -1768,6 +1855,7 @@ static EpisodeSegments episode_segments(const hb_ctx* ctx, int64_t* head) {
   e.add_solution(ctx->pol_mem ? rows_at(ctx->pol, 0, N, grid) : SolutionRows{}, N, grid);
   e.add(ctx->odom_cam, sizeof(OdomCamera));
   if (ctx->teleop.n > 0) e.add(ctx->tele_state, sizeof(TeleopState));     // only with a teleop setting: other rows keep their size
+  if (ctx->contact_detection.n > 0) e.add(ctx->cd_state, sizeof(ContactDetectState));     // only with contact detection, as teleop
   e.t.row_words = e.words;
   return e.t;
 }
@@ -1872,7 +1960,7 @@ static int read_sensors_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noise, Ha
   ENTER(ctx, B, noise && rbd && est && quat && ang_vel_local && lin_acc_local && joint_pos && joint_vel && sensor_noise_ok(*noise) && accel_dt > 0.0 &&
         tick >= 0 && tick <= UINT32_MAX, CAPPED);
   return launch(ctx, K_UNPROFILED, sensor_read_kernel, (B + 63) / 64, 64, 0, B, *noise, hw, bridge, (uint32_t)tick, accel_dt, 0.0, rbd, est, quat, ang_vel_local,
-                lin_acc_local, joint_pos, joint_vel, (uint8_t*)nullptr, OdomRead{});
+                lin_acc_local, joint_pos, joint_vel, (uint8_t*)nullptr, OdomRead{}, ContactDetect{});
 }
 
 int hb_sim_read_sensors_batch_dev(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64_t tick, double accel_dt, const double* rbd,
@@ -2257,6 +2345,14 @@ int hb_sim_read_odometry(hb_ctx* ctx, int B, const hb_sensor_noise* noise, int64
   Staging s(ctx, B);
   auto r = s.in(rbd, 32); auto es = s.in(est, 1); auto p = s.out(pos, 3); auto h = s.out(has_msg, 1);
   return s.run(1, [&](Chunk) { return hb_sim_read_odometry_async(ctx, B, noise, tick, r, es, p, h); });
+}
+
+int hb_contact_state_estimate(hb_ctx* ctx, int B, double t, const hb_estimation_state* est, const double* est_force,
+                              const hb_contact_detection* records, uint8_t* flags) {
+  ENTER(ctx, B, est && est_force && flags, CAPPED, [&] { return all_ok(B, records, contact_detection_ok); });
+  Staging s(ctx, B);
+  auto es = s.in(est, 1); auto f = s.in(est_force, 16); auto fl = s.inout(flags, 4);
+  return s.run(1, [&](Chunk) { return hb_contact_state_estimate_async(ctx, B, t, es, f, records, fl); });
 }
 
 int hb_estimator_fuse_odometry(hb_ctx* ctx, int B, const hb_kf_params* params, hb_kf_state* state, const double* pos, const uint8_t* has_msg,

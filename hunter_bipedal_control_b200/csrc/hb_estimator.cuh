@@ -5,6 +5,7 @@
 #include "hb_planner.h"
 #include "hb_qp.cuh"
 #include "hb_rbd.cuh"
+#include "hb_rollout.cuh"
 #include "../../include/hunter_b200.h"
 
 namespace {  // the kernels: internal linkage, the library exports only the hb_* entry points
@@ -214,14 +215,14 @@ __global__ void odometry_fuse_kernel(int B, double foot_radius, hb_kf_state* sta
 // One warp per instance; the terms Pinocchio provides are obtained as
 //   M v  = inverse dynamics with acceleration v at zero velocity, no gravity;   g = inverse dynamics at rest with gravity;
 //   C' v = d/dq (1/2 v' M(q) v) at fixed v (lane i = dual sweep seeded on q_i; valid for any C with dM/dt = C + C', as Pinocchio's).
+// One observer step of one instance on its warp (every lane calls it): p_filtered (16) advanced, est (16) and disturbance (16, nullable)
+// written, from the rbd r (32) and the torques tau (10). Not inlined: contact_force_kernel and the estimated episodes' contact_observe_kernel
+// run this one compiled body, so that the episode and hb_contact_force_estimate_batch give the same bits (as odom_contact_positions).
 struct ObsShared { double p[NQ], g[NQ], ctv[NQ], taud[NQ], Jf[2 * 5 * 6]; };
-__global__ void __launch_bounds__(32) contact_force_kernel(int B, double lambda, double dt_in, hb_observer_state* state, const double* rbd, const double* tau_cmd,
-                                                           double* est, double* disturbance) {
-  __shared__ ObsShared sh;
-  const int inst = blockIdx.x, lane = threadIdx.x;
+__device__ __noinline__ void observer_step(ObsShared& sh, int lane, double lambda, double dt_in, double* p_filtered, const double* r, const double* tau,
+                                           double* e, double* disturbance) {
   const double dt = dt_in > 1.0 ? 0.002 : dt_in;
   const double gama = exp(-lambda * dt), beta = (1.0 - gama) / (gama * dt);
-  const double* r = rbd + (size_t)inst * 32;
   double q[NQ], v[NQ];
   rbd_to_qv(r, q, v);
   if (lane < 3) sh.ctv[lane] = 0.0;                 // the kinetic energy does not depend on the base position
@@ -265,18 +266,16 @@ __global__ void __launch_bounds__(32) contact_force_kernel(int B, double lambda,
     }
   }
   __syncwarp();
-  hb_observer_state& st = state[inst];
   if (lane < NQ) {
     const double p = sh.p[lane];
-    const double pscg = beta * p + (lane >= 6 ? tau_cmd[(size_t)inst * NJ + lane - 6] : 0.0) + sh.ctv[lane] - sh.g[lane];
-    const double filt = (1.0 - gama) * pscg + gama * st.p_filtered[lane];
-    st.p_filtered[lane] = filt;
+    const double pscg = beta * p + (lane >= 6 ? tau[lane - 6] : 0.0) + sh.ctv[lane] - sh.g[lane];
+    const double filt = (1.0 - gama) * pscg + gama * p_filtered[lane];
+    p_filtered[lane] = filt;
     const double td = beta * p - filt;
     sh.taud[lane] = td;
-    if (disturbance) disturbance[(size_t)inst * NQ + lane] = td;
+    if (disturbance) disturbance[lane] = td;
   }
   __syncwarp();
-  double* e = est + (size_t)inst * 16;
   if (lane < 2) {
     // least-norm solution of A w = b, A = S J' (5 x 6), as the reference's SVD solve gives it: Householder QR of A' = Q [R; 0], then
     // w = Q [R^-T b; 0]. A loses rank inside the joint limits (knee ~0.0208 rad, where the hip-pitch, knee and ankle origins line up,
@@ -334,5 +333,24 @@ __global__ void __launch_bounds__(32) contact_force_kernel(int B, double lambda,
     e[12 + lane] = sqrt(n3);
     e[14 + lane] = sqrt(n6);
   }
+}
+__global__ void __launch_bounds__(32) contact_force_kernel(int B, double lambda, double dt_in, hb_observer_state* state, const double* rbd, const double* tau_cmd,
+                                                           double* est, double* disturbance) {
+  __shared__ ObsShared sh;
+  const int inst = blockIdx.x;
+  observer_step(sh, threadIdx.x, lambda, dt_in, state[inst].p_filtered, rbd + (size_t)inst * 32, tau_cmd + (size_t)inst * NJ, est + (size_t)inst * 16,
+                disturbance ? disturbance + (size_t)inst * NQ : nullptr);
+}
+
+// Step (4) of an estimated tick with contact detection (hunter_b200.h): the observer of each instance with a record, on its estimated rbd
+// with its stored effort, into its stored output. One warp per instance; the others return.
+__global__ void __launch_bounds__(32) contact_observe_kernel(int B, double dt, InstanceView<hb_contact_detection> set, ContactDetectState* st,
+                                                             const double* rbd) {
+  __shared__ ObsShared sh;
+  const int inst = blockIdx.x;
+  const hb_contact_detection* r = set.of(inst);
+  if (!r) return;
+  ContactDetectState& d = st[inst];
+  observer_step(sh, threadIdx.x, r->cutoff_frequency, dt, d.p_filtered, rbd + (size_t)inst * 32, d.effort, d.force, nullptr);
 }
 }  // namespace

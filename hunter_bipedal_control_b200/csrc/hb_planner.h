@@ -316,6 +316,40 @@ HBP_HD inline void find_index(int index, const bool* stock, int n, int& start_id
   for (int ip = index + 1; ip < n; ++ip) if (stock[ip] != stock[index]) { final_idx = ip - 1; break; }
 }
 
+// SwingTrajectoryPlanner::threadSaftyGetStartStopTime (:510-532) on a stored schedule (n_events, events, modes): for each contact c the start
+// and stop [s[c], e[c]] of the run of equal contact flags around t, as update (:164-260) stores them per phase: events[find_index(p)]. The
+// phase is lookup::findIndexInTimeArray's (mode_at's: an event time belongs to the earlier phase), clamped to n_events - 1. Without a plan,
+// or with a schedule of one phase (where the reference indexes events[-1]), both are t. n_events is clamped to HB_MAX_EVENTS.
+HBP_HD inline void contact_phase_times(int has_plan, int n_events, const double* events, const int* modes, double t, double* s, double* e) {
+  const int n = n_events < HB_MAX_EVENTS ? n_events : HB_MAX_EVENTS;
+  if (!has_plan || n < 1) {
+    for (int c = 0; c < 4; ++c) s[c] = e[c] = t;
+    return;
+  }
+  int idx = 0;
+  while (idx < n && events[idx] < t) ++idx;
+  if (idx > n - 1) idx = n - 1;
+  for (int c = 0; c < 4; ++c) {
+    bool stock[HB_MAX_EVENTS + 1];
+    for (int p = 0; p <= n; ++p) stock[p] = contact_flag(modes[p], c);
+    int si, fi;
+    find_index(idx, stock, n + 1, si, fi);
+    s[c] = events[si]; e[c] = events[fi];
+  }
+}
+
+// StateEstimateBase::estContactState (StateEstimateBase.cpp:208-226) with the record r: flags (in: the schedule's, out: the detected ones)
+// at time t, phase times s, e (contact_phase_times) and the observer's output force (16, hb_contact_force_estimate_batch's layout), whose
+// F_z of leg c % 2 decides a swing foot late in its phase and a stance foot early in its phase. The comparisons are strict.
+HBP_HD inline void contact_state(const hb_contact_detection& r, double t, const double* s, const double* e, const double* force, uint8_t* flags) {
+  for (int c = 0; c < 4; ++c) {
+    const bool cmd = flags[c] != 0;
+    const double P = e[c] - s[c], fz = force[6 * (c % 2) + 2];
+    if (!cmd && t - s[c] > r.swing_fraction * P) flags[c] = fz > r.threshold ? 1 : 0;
+    if (cmd && t - s[c] < r.stance_fraction * P) flags[c] = fz > r.threshold ? 1 : 0;
+  }
+}
+
 // SwingTrajectoryPlanner::calNextFootPos (:289-312). body_vel_cmd = [vx, vy, vz, wz, 0, 0] as set from /cmd_vel_filtered
 // (SwitchedModelReferenceManager.cpp:91-101): its tail(3) = (wz, 0, 0) is used as the commanded angular velocity, as the reference does.
 // With a height map (nullable) the centrifugal term reads the body height above the map, and the foothold stands on the map.

@@ -916,6 +916,59 @@ int hb_wbc_set_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
  * for B > max_batch, a rejected call keeps the previous setting. No launch is added, set or not. Maps are a setting, not episode state:
  * hb_episode_state_bytes and snapshots do not count them. */
 int hb_mpc_set_cone_maps(hb_ctx* ctx, int B, const hb_terrain* maps);
+
+/* ---- contact detection: the Kalman filter's contact flags from the momentum observer instead of the plan's schedule alone ----
+ * Without it an estimated episode tells the filter the schedule's flags (LeggedController.cpp:296-304), which are wrong where a foot
+ * lands late (a step down) or early (a step up). With a record r for an instance, each estimated tick runs StateEstimateBase::
+ * estContactForce (the observer of hb_contact_force_estimate_batch) and replaces the schedule's flags by StateEstimateBase::estContactState
+ * (StateEstimateBase.cpp:208-226), which the reference computes every input of and never calls. At time t with the schedule's flag
+ * cmd[c] of contact c (ordered l_f1, r_f1, l_f2, r_f2, so c % 2 is the leg) and the run [s_c, e_c] of equal flags of c around t
+ * (SwingTrajectoryPlanner::threadSaftyGetStartStopTime on the stored schedule: the phase of t, an event time belonging to the earlier
+ * phase, clamped to n_events - 1; [t, t] without a plan or with a one-phase schedule), P = e_c - s_c and Fz = force[6 (c % 2) + 2] of
+ * the last observer output:
+ *   flag[c] = Fz > threshold   if !cmd[c] && t - s_c > swing_fraction P     (a swing foot late in its phase)
+ *   flag[c] = Fz > threshold   if  cmd[c] && t - s_c < stance_fraction P    (a stance foot early in its phase)
+ *   flag[c] = cmd[c]           otherwise.
+ * Order of one estimated tick of an instance with a record: (1) the schedule's flags at the previous observation's time, as without the
+ * setting; (2) the rule above at that time on the stored observer output; (3) the filter on the detected flags (the odometry fusion too);
+ * (4) the observer on the filter's estimated rbd with the stored effort and dt = period, its output stored; (5) after the plant step the
+ * tick's applied torque (what HB_CHANNEL_TORQUE records) is stored as the next tick's effort. The detected flags reach the filter only:
+ * the planner, MPC and WBC read the schedule's flags, as the reference's do. */
+typedef struct {                 /* one robot's contact detection                                                                   */
+  double cutoff_frequency;       /* the observer's [rad/s], > 0 as hb_contact_force_estimate_batch takes it (cutoffFrequency: 250) */
+  double threshold;              /* F_z above which a foot counts as loaded [N], finite (contactForceEsimation.contactThreshold: 75) */
+  double swing_fraction;         /* share of a swing phase after which the force decides, in [0, 1] (0.75)                         */
+  double stance_fraction;        /* share of a stance phase before which the force decides, in [0, 1] (0.25)                        */
+} hb_contact_detection;          /* 32 B */
+#define HB_SETTING_CONTACT_DETECTION 20   /* hb_contact_detection for hb_rollout_set_contact_detection (hb_check_setting_records)         */
+/* host only: task's contactForceEsimation cutoff and threshold (task NULL: 250 and 75, hb_parse_task_info's defaults), fractions 0.75 and
+ * 0.25 (StateEstimateBase.cpp:215-221). -1 for a NULL out. */
+int hb_default_contact_detection(const hb_task_info* task /*nullable*/, hb_contact_detection* out);
+/* Contact detection of the context's estimated episodes: record i acts on instance i of hb_rollout_estimated_batch_dev; instances at or
+ * beyond B, hb_rollout_batch_dev and every other entry point run without it. The contract of a per-robot episode setting (above): -1 also
+ * for a record outside its documented range, -4 for B > max_batch, a rejected call keeps the previous setting. Per-instance context state:
+ * the observer's filtered momentum, its last output (16, 50 each before the first: StateEstimateBase.cpp:61-62), the effort (10) and the
+ * flags the filter last used (4). Every call that is not rejected clears that state (B == 0 included), so a restore comes after it; an
+ * episode call with tick0 == 0 clears it too. The state is part of a snapshot row while a setting is made, adding 344 bytes to
+ * hb_episode_state_bytes; unset, the row keeps its size. While a setting is made, each estimated tick runs one more launch (the observer). */
+int hb_rollout_set_contact_detection(hb_ctx* ctx, int B, const hb_contact_detection* records);
+/* The detection rule alone, as the episode's step (2) runs it: for each instance i, flags[i] (B x 4, in: the schedule's, out: detected)
+ * at time t on the schedule of est[i] (has_plan, n_events, event_times, modes) and the observer output est_force[i] (B x 16) with
+ * records[i]; records NULL leaves the flags unchanged. hb_contact_state_estimate_async takes device pointers (records on the host), and
+ * hb_contact_state_estimate host pointers. -1: B < 0, a NULL pointer other than records, a record the setter rejects; -4: B > max_batch. */
+int hb_contact_state_estimate_async(hb_ctx* ctx, int B, double t, const hb_estimation_state* est, const double* est_force,
+                                    const hb_contact_detection* records /*nullable*/, uint8_t* flags);
+int hb_contact_state_estimate(hb_ctx* ctx, int B, double t, const hb_estimation_state* est, const double* est_force,
+                              const hb_contact_detection* records /*nullable*/, uint8_t* flags);
+/* The detection state of instances 0 .. B-1 of the context (host pointers): est_force (B x 16, nullable), the last observer output, and
+ * flags (B x 4, nullable), the flags the filter last used; an instance beyond the setting reads the cleared state (50 each, flags 0).
+ * -1: B < 0 or no setting made since the context was created; -4: B > max_batch. */
+int hb_rollout_contact_estimates(hb_ctx* ctx, int B, double* est_force /*nullable*/, uint8_t* flags /*nullable*/);
+/* The rule on the host, the body the kernels run (host only, no context, no GPU): phase_times (B x 4 x 2, nullable) receives [s_c, e_c];
+ * flags as hb_contact_state_estimate. -1 as there, without the capacity. */
+int hb_contact_state_host(int B, double t, const hb_estimation_state* est, const double* est_force, const hb_contact_detection* records /*nullable*/,
+                          uint8_t* flags, double* phase_times /*nullable*/);
+
 /* One estimator update per instance (StateEstimateBase::updateJointStates / updateImu, StateEstimateBase.cpp:73-106, then
  * KalmanFilterEstimate::update): quat = (x, y, z, w); contact_flag: B x 4 (0 = the filter distrusts that foot, x100 noise);
  * rbd_out: B x 32 measured rbd state [zyx, p, q_j, omega_world, v, qd_j]. zyxOffset_ is taken as zero. The odometry fusion

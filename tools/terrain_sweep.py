@@ -57,6 +57,14 @@ reports the tables above plus one, with_cone_maps, with MPC cone maps added to e
 against the same episodes with all-zero cone maps and without cone maps, alternately; the tool asserts that all-zero cone maps give the
 outcome of no cone maps bit for bit.
 
+--contact-detection (with --estimator) hands each robot's Kalman filter the contact flags of the momentum observer
+(hb_rollout_set_contact_detection, default_contact_detection: task.info's threshold, fractions 0.75 and 0.25) instead of the schedule's.
+The line reports four tables over the same cells and start poses -- blind, blind with detection, estimator maps (each robot's terrain
+minus 0.02 m, hb_estimator_set_maps) and estimator maps with detection -- each with its largest magnitude at >= 90 % per kind and, per
+kind and magnitude, the mean over the cell's robots of the estimation stats' largest base-height error and RMS base-velocity error. It
+times episodes with detection against the same episodes with the setting made and cleared and without it, alternately; the tool asserts
+that the cleared setting gives the outcome of none bit for bit.
+
 --friction-scale S scales every robot's ground friction by S in every table (hb_rollout_set_plant_variations, friction_scale) and runs its
 WBC with friction_coefficient S times the context's (task.info's) value (hb_rollout_set_controller_settings): the slope's direction
 matters most to the friction pyramids where friction is short.
@@ -171,6 +179,50 @@ def height_map_sweep(h, args, grid):
     return out, clocks, timing
 
 
+def contact_detection_sweep(h, args, grid):
+    """--contact-detection: blind, blind with detection, estimator maps and estimator maps with detection over the same cells, each with its
+    estimation errors; then detection / cleared / unset episodes timed alternately."""
+    hb, ctx, prm, B, rbd0 = h.hb, h.ctx, h.prm, h.B, h.rbd0
+    records = hb.make_contact_detection_settings(B)
+    mk = [str(m) for m in MAGNITUDES]
+
+    def set_all(value):
+        terrains, est_maps, detection = value
+        ctx.set_terrains(terrains)
+        ctx.set_estimator_maps(est_maps)
+        if detection == "cleared":
+            ctx.set_contact_detection(records)
+            detection = None
+        ctx.set_contact_detection(detection)
+
+    def settings(shift, maps, detection):
+        origin, heights = grid(shift)
+        return hb.make_terrains(B, heights, SPACING, origin), hb.make_terrains(B, heights - GROUND, SPACING, origin) if maps else None, \
+            records if detection else None
+
+    out = {}
+    for name, maps, detection in [("blind", False, False), ("blind_detection", False, True), ("estimator_maps", True, False),
+                                  ("estimator_maps_detection", True, True)]:
+        tally = Tally(len(MAGNITUDES), len(KINDS))
+        height, vel = np.zeros((len(KINDS), len(MAGNITUDES))), np.zeros((len(KINDS), len(MAGNITUDES)))
+        for r, run in h.sweep(set_all, lambda shift: settings(shift, maps, detection), est_stats=True):
+            mi, ki = cells(B, len(MAGNITUDES), len(KINDS), r)
+            tally.add(mi, ki, run.stats, value=np.hypot(*(run.rbd[:, 3:5] - rbd0[:, 3:5]).T) / (TICKS * prm.period))
+            es = run.est_stats
+            rms = np.sqrt(es["sum_sq_vel_err"] / np.maximum(es["count"], 1))
+            np.add.at(height, (ki, mi), es["max_height_err"] / (args.repeats * B / (len(KINDS) * len(MAGNITUDES))))
+            np.add.at(vel, (ki, mi), rms / (args.repeats * B / (len(KINDS) * len(MAGNITUDES))))
+        out[name] = {"largest_magnitude_90pct": dict(zip(KINDS, tally.largest(MAGNITUDES))), "survival": keyed(KINDS, mk, tally.survival().tolist()),
+                     "mean_max_height_err_m": keyed(KINDS, mk, height.tolist()), "mean_rms_vel_err_m_per_s": keyed(KINDS, mk, vel.tolist()),
+                     "fail_reasons": tally.reasons}
+    terrains, _, _ = settings(0, False, True)
+    _, clocks, timing = h.alternate(set_all, [("detection", (terrains, None, records)), ("cleared", (terrains, None, "cleared")),
+                                              ("no_detection", (terrains, None, None))], args.timed, launches=True)
+    assert timing["cleared_same_outcome_as_no_detection"], "a cleared contact detection changed the outcome of none"
+    set_all((None, None, None))
+    return out, clocks, timing
+
+
 def main():
     def extra(ap):
         ap.add_argument("--height-maps", action="store_true", help="also plan on maps of the terrains")
@@ -179,13 +231,16 @@ def main():
         ap.add_argument("--wbc-maps", action="store_true", help="with --height-maps: also tilt the WBC's friction pyramids on the maps")
         ap.add_argument("--mpc-cone-maps", action="store_true", help="with --height-maps: also stand the MPC's friction cones on the maps")
         ap.add_argument("--friction-scale", type=float, default=1.0, help="scale of every robot's ground friction and WBC friction coefficient")
+        ap.add_argument("--contact-detection", action="store_true", help="with --estimator: also run the filter on detected contact flags")
 
     args = sweep_args("terrain_sweep.py", "timed terrain / flat / unset episode triples (with --height-maps: mapped / zero-map / blind)",
                       len(KINDS) * len(MAGNITUDES), extra=extra,
                       valid=lambda a: ((not a.estimator_maps or (a.height_maps and a.estimator)) and (not a.mpc_maps or a.height_maps)
-                                       and (not a.wbc_maps or a.height_maps) and (not a.mpc_cone_maps or a.height_maps) and a.friction_scale > 0),
+                                       and (not a.wbc_maps or a.height_maps) and (not a.mpc_cone_maps or a.height_maps) and a.friction_scale > 0
+                                       and (not a.contact_detection or (a.estimator and not a.height_maps))),
                       needs="--estimator-maps needs --height-maps --estimator, --mpc-maps needs --height-maps, "
-                            "--wbc-maps needs --height-maps, --mpc-cone-maps needs --height-maps, --friction-scale takes a scale > 0, ")
+                            "--wbc-maps needs --height-maps, --mpc-cone-maps needs --height-maps, --friction-scale takes a scale > 0, "
+                            "--contact-detection needs --estimator and no --height-maps, ")
     h = Episodes("terrain_sweep.py", args, TICKS)
     hb, ctx, prm, B, rbd0 = h.hb, h.ctx, h.prm, h.B, h.rbd0
     step_ahead, ramp_ahead = feature_distances(rbd0, h.feet)
@@ -195,11 +250,27 @@ def main():
         ctx.set_controller_settings(hb.make_controller_settings(B, wbc=ctx.wbc_settings(),
                                                                 friction_coefficient=args.friction_scale * ctx.wbc_settings().friction_coefficient))
 
-    if args.height_maps:
-        def grid(shift):
-            mi, ki = cells(B, len(MAGNITUDES), len(KINDS), shift)
-            return terrain_heights(rbd0, np.array(KINDS)[ki], np.array(MAGNITUDES)[mi], step_ahead, ramp_ahead)
+    def grid(shift):
+        mi, ki = cells(B, len(MAGNITUDES), len(KINDS), shift)
+        return terrain_heights(rbd0, np.array(KINDS)[ki], np.array(MAGNITUDES)[mi], step_ahead, ramp_ahead)
 
+    if args.contact_detection:
+        out, clocks, timing = contact_detection_sweep(h, args, grid)
+        print(json.dumps({
+            "metric": "contact detection: the highest step [cm] that >= 90 %% of the trotting robots cross within %.1f s through the estimator "
+                      "when the Kalman filter's contact flags come from the momentum observer; %s tables per kind (steps in cm, slopes in "
+                      "degrees)" % (T_episode, ", ".join(out)), "value": out["blind_detection"]["largest_magnitude_90pct"]["step_up"], "unit": "cm",
+            **report(args, clocks), **out, "timing": timing,
+            "config": {"workload": workload(h, "; %d kinds x %d magnitudes, %d episodes per table" % (len(KINDS), len(MAGNITUDES), args.repeats)),
+                       "terrain": "%d x %d height field at %g m centred on the start, ground %g m under the start; steps with the edge %g m "
+                                  "ahead (a ramp one cell wide), slopes starting %g m ahead, across the initial heading"
+                                  % (GRID, GRID, SPACING, GROUND, STEP_AHEAD, RAMP_AHEAD),
+                       "contact_detection": "default_contact_detection() for every robot: threshold 75 N, fractions 0.75 / 0.25, cutoff 250",
+                       "estimator_maps": "each robot's terrain minus %g m (hb_estimator_set_maps)" % GROUND,
+                       "survival": "robots still up at the end of the episode", "failure_checks": failure_checks("base z above the terrain")}}))
+        return
+
+    if args.height_maps:
         out, clocks, timing = height_map_sweep(h, args, grid)
         if args.mpc_cone_maps:
             metric = ("MPC cone maps: the highest step [cm] that >= 90 %% of the trotting robots cross within %.1f s%s when the planner%s%s%s "
