@@ -11,7 +11,7 @@ from .api import (HbWbcSettings, HbTaskInfo, parse_task_info, Context, WeightedW
                   HB_ODOM_MAX_DELAY, HbOdometrySetting, make_odometry_settings, HbControllerSetting, make_controller_settings,
                   HbHardwareSetting, default_hardware_setting, make_hardware_settings,
                   HbMotorBridge, default_motor_bridge, make_motor_bridges, bridge_encode, bridge_feedback,
-                  NBODY, HbLinkVariation, default_link_variation, make_link_variations,
+                  NBODY, HbLinkVariation, default_link_variation, make_link_variations, HbJointModel, default_joint_model, make_joint_models,
                   HB_MAX_TELEOP_WINDOWS, TELEOP_ALWAYS, HbTeleop, HbTeleopSetting, default_teleop_setting, make_teleop_settings, cmd_vel_to_target,
                   HB_GAIT_MAX_PHASES, HbGaitTemplate, HbPlannerSettings, gait_template, default_planner_settings, parse_planner_settings, make_planner_settings,
                   CHANNELS, make_channels, EpisodeSnapshot, reseed,
@@ -25,7 +25,7 @@ __all__ = ["HbWbcSettings", "HbTaskInfo", "parse_task_info", "Context", "Weighte
            "HB_ODOM_MAX_DELAY", "HbOdometrySetting", "make_odometry_settings", "HbControllerSetting", "make_controller_settings",
            "HbHardwareSetting", "default_hardware_setting", "make_hardware_settings",
            "HbMotorBridge", "default_motor_bridge", "make_motor_bridges", "bridge_encode", "bridge_feedback",
-           "NBODY", "HbLinkVariation", "default_link_variation", "make_link_variations",
+           "NBODY", "HbLinkVariation", "default_link_variation", "make_link_variations", "HbJointModel", "default_joint_model", "make_joint_models",
            "HB_MAX_TELEOP_WINDOWS", "TELEOP_ALWAYS", "HbTeleop", "HbTeleopSetting", "default_teleop_setting", "make_teleop_settings", "cmd_vel_to_target",
            "HB_GAIT_MAX_PHASES", "HbGaitTemplate", "HbPlannerSettings", "gait_template", "default_planner_settings", "parse_planner_settings", "make_planner_settings",
            "CHANNELS", "make_channels", "EpisodeSnapshot", "reseed",

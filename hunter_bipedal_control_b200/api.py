@@ -58,6 +58,7 @@ EXPORTED_SYMBOLS = [
     "hb_default_motor_bridge", "hb_rollout_set_motor_bridge", "hb_motor_bridge_encode", "hb_motor_bridge_feedback", "hb_actuation_bridge",
     "hb_sim_step_bridge", "hb_sim_read_sensors_bridge",
     "hb_default_link_variation", "hb_rollout_set_link_variations", "hb_sim_step_links",
+    "hb_default_joint_model", "hb_rollout_set_joint_models", "hb_sim_step_joints",
     "hb_default_teleop_setting", "hb_rollout_set_teleop", "hb_cmd_vel_to_target",
     "hb_default_planner_settings", "hb_parse_planner_settings", "hb_plan_references_settings", "hb_plan_set_settings",
     "hb_plan_set_maps", "hb_plan_references_maps", "hb_goal_to_target_maps", "hb_cmd_vel_to_target_maps", "hb_estimator_set_maps",
@@ -548,6 +549,40 @@ def make_link_variations(B, mass_scale=1.0, com_shift=0.0, inertia_scale=1.0):
     v = np.ctypeslib.as_array(out)
     v["mass_scale"] = ms; v["com_shift"] = cs; v["inertia_scale"] = js
     return _check_records(HbLinkVariation.SETTING_KIND, out, "link_variations")
+
+
+class HbJointModel(C.Structure):
+    SETTING_KIND = 21        # HB_SETTING_JOINT_MODELS, the record's kind for hb_check_setting_records
+    _fields_ = [("friction_loss", C.c_double * NJ), ("friction_velocity", C.c_double), ("lower", C.c_double * NJ), ("upper", C.c_double * NJ),
+                ("stop_stiffness", C.c_double), ("stop_damping", C.c_double)]
+
+
+def default_joint_model():
+    """hb_default_joint_model: the reference's joints (friction loss 0.2 N m, range stops at HB_JOINT_LOWER / HB_JOINT_UPPER) with
+    v_s = 0.01 rad/s and the stop gains of MuJoCo's default solref and solimp."""
+    r = HbJointModel()
+    _check(load_library().hb_default_joint_model(C.byref(r)), "hb_default_joint_model")
+    return r
+
+
+def make_joint_models(B, friction_loss=None, friction_velocity=None, lower=None, upper=None, stop_stiffness=None, stop_damping=None):
+    """ctypes array of B HbJointModel (Context.set_joint_models, Context.sim_step): each robot's friction loss f [N m] and regularisation
+    velocity v_s [rad/s], its stop range [lower, upper] [rad] (+-inf: no stop on that side) and the stop's gains k [1/s^2], b [1/s]. A
+    field not given is default_joint_model()'s. Per-joint fields broadcast from (), (10,) or (B, 10) (per robot only: (B, 1)), the others
+    from () or (B,). Raises ValueError for a shape that does not broadcast and for a record hb_rollout_set_joint_models rejects (its own
+    check); the stability rule against the plant's params is checked by the plant step and the episode calls."""
+    d = np.ctypeslib.as_array(default_joint_model())
+    fields = dict(friction_loss=friction_loss, friction_velocity=friction_velocity, lower=lower, upper=upper, stop_stiffness=stop_stiffness,
+                  stop_damping=stop_damping)
+    out = (HbJointModel * B)()
+    v = np.ctypeslib.as_array(out)
+    for name, x in fields.items():
+        shape = (B,) + d[name].shape
+        try:
+            v[name] = np.broadcast_to(d[name] if x is None else _f64(x), shape)
+        except ValueError as e:
+            raise ValueError("joint models: %s %s expected: %s" % (name, shape, e))
+    return _check_records(HbJointModel.SETTING_KIND, out, "joint_models")
 
 
 HB_TERRAIN_MAX = 64
@@ -1395,14 +1430,15 @@ class Context:
                                              _ptr(mcmd)), "hb_actuation_bridge", self._h)
         return tau if bridge is None else mcmd
 
-    def sim_step(self, rbd, tau, params=None, wrench=None, variation=None, terrain=None, bridge=None, limits=None, links=None):
+    def sim_step(self, rbd, tau, params=None, wrench=None, variation=None, terrain=None, bridge=None, limits=None, links=None, joints=None):
         """One control period of the batched rigid-body plant: returns (rbd_next [B,32], contact_force [B,12], contact_flag [B,4]).
         wrench [B,6]: an external world force at the base origin, then a world couple, held over the period. variation: B HbPlantVariation
         (make_plant_variations), the plant of each robot. terrain: B HbTerrain (make_terrains), the ground under each robot. bridge: B
         HbMotorBridge (make_motor_bridges): tau is then the decoded motor commands [B,10,5] of actuation(bridge=...), whose motor PD runs on
         every substep, clipped to limits ([10] or [B,10]), and the mean clipped torque [B,10] is returned fourth. links: B
-        HbLinkVariation (make_link_variations), the bodies of each robot. Every step is hb_sim_step_links; without any of the five it is the
-        plain plant step of hb_sim_step_batch."""
+        HbLinkVariation (make_link_variations), the bodies of each robot. joints: B HbJointModel (make_joint_models), the range stops and
+        friction loss of each robot's joints. Every step is hb_sim_step_joints; without any of the six it is the plain plant step of
+        hb_sim_step_batch."""
         rbd = _f64(rbd).copy(); tau = _f64(tau); B = rbd.shape[0]
         params = params or default_sim_params()
         cf = np.zeros((B, 12)); fl = np.zeros((B, 4), dtype=np.uint8)
@@ -1413,14 +1449,16 @@ class Context:
             raise ValueError("sim_step: %d terrains for %d robots" % (len(terrain), B))
         if links is not None and len(links) != B:
             raise ValueError("sim_step: %d link variations for %d robots" % (len(links), B))
+        if joints is not None and len(joints) != B:
+            raise ValueError("sim_step: %d joint models for %d robots" % (len(joints), B))
         bridge = _bridge_records(bridge, B, "sim_step")
         mcmd, lim, applied = None, None, None
         if bridge is not None:
             mcmd, tau = tau.reshape(B, NJ, 5), None
             lim = _f64(np.broadcast_to(_f64(limits), (B, NJ)))
             applied = np.zeros((B, NJ))
-        _check(self._lib.hb_sim_step_links(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), variation, terrain, bridge, _ptr(mcmd), _ptr(lim),
-                                           _ptr(applied), links, _ptr(cf), _ptr(fl)), "hb_sim_step_links", self._h)
+        _check(self._lib.hb_sim_step_joints(self._h, B, C.byref(params), _ptr(rbd), _ptr(tau), _ptr(w), variation, terrain, bridge, _ptr(mcmd), _ptr(lim),
+                                            _ptr(applied), links, joints, _ptr(cf), _ptr(fl)), "hb_sim_step_joints", self._h)
         return (rbd, cf, fl) if bridge is None else (rbd, cf, fl, applied)
 
     def _set_instances(self, symbol, items):
@@ -1445,6 +1483,13 @@ class Context:
         masses, CoMs and inertias of the bodies of instance i's plant in every later rollout / rollout_estimated call; instances beyond
         len(variations) run the nominal bodies; None clears them. The controllers are not told about it, and no other call reads it."""
         self._set_instances("hb_rollout_set_link_variations", variations)
+
+    def set_joint_models(self, models):
+        """Joint models of this context's episodes (hb_rollout_set_joint_models): models[i] (make_joint_models) gives the joints of instance
+        i's plant range stops and friction loss in every later rollout / rollout_estimated call; instances beyond len(models) run without
+        them; None clears them. The controllers are not told about it, and no other call reads it. An episode call whose params.sim break
+        the models' stability rule, h (joint_damping + f_j / v_s) <= joint_armature, raises before it runs."""
+        self._set_instances("hb_rollout_set_joint_models", models)
 
     def set_pushes(self, schedules):
         """Push schedules of this context's episodes (hb_rollout_set_pushes): schedules[i] (make_push_schedules) acts on instance i of every

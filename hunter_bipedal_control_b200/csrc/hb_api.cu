@@ -113,6 +113,8 @@ struct hb_ctx {
   InstanceSetting<hb_motor_bridge> bridges;
   // each instance's own bodies in the episodes' plant (hb_rollout_set_link_variations)
   InstanceSetting<hb_link_variation> links;
+  // each instance's joint range stops and friction loss in the episodes' plant (hb_rollout_set_joint_models)
+  InstanceSetting<hb_joint_model> joints;
   // each instance's joystick and target publisher in the episodes (hb_rollout_set_teleop), and the publishers' state, allocated at
   // max_batch by the first call that sets records
   InstanceSetting<hb_teleop_setting> teleop;
@@ -528,7 +530,7 @@ int hb_destroy(hb_ctx* ctx) {
   void* const mem[] = {ctx->scratch_mem, ctx->sqp_mem, ctx->hoqp_mem, ctx->ro_mem, ctx->re_mem, ctx->goal_mem, ctx->pol_mem, ctx->odom_mem, ctx->tele_mem, ctx->snap_mem, ctx->arena,
                        ctx->pushes.dev, ctx->variations.dev, ctx->terrains.dev, ctx->goals.dev, ctx->plan_targets.dev, ctx->latencies.dev,
                        ctx->odometry.dev, ctx->controllers.dev, ctx->hardware.dev, ctx->plan_settings.dev,
-                       ctx->bridges.dev, ctx->links.dev, ctx->height_maps.dev, ctx->estimator_maps.dev,
+                       ctx->bridges.dev, ctx->links.dev, ctx->joints.dev, ctx->height_maps.dev, ctx->estimator_maps.dev,
                        ctx->mpc_maps.dev, ctx->sth_mem, ctx->wbc_maps.dev, ctx->cone_maps.dev, ctx->cgr_mem,
                        ctx->contact_detection.dev, ctx->contact_call.dev, ctx->cd_mem};
   for (void* p : mem) if (p) cudaFree(p);
@@ -1198,16 +1200,16 @@ int hb_actuation_batch_dev(hb_ctx* ctx, int B, double delay, const double* time,
 }
 
 // the plant step after the entry checks; wrench (B x 6) nullable; var: the plants of the instances, ter: the ground under them, drive: the
-// motors of the bridged ones
+// motors of the bridged ones, links: their bodies, joints: their joint models
 static int sim_step(hb_ctx* ctx, int B, const hb_sim_params& params, double* rbd, const double* tau, const double* wrench,
                     InstanceView<hb_plant_variation> var, InstanceView<hb_terrain> ter, const MotorDrive& drive, InstanceView<hb_link_variation> links,
-                    double* contact_force, uint8_t* contact_flag) {
-  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, params, rbd, tau, wrench, var, ter, drive, links, contact_force, contact_flag);
+                    InstanceView<hb_joint_model> joints, double* contact_force, uint8_t* contact_flag) {
+  return launch(ctx, K_UNPROFILED, sim_step_kernel, B, 32, 0, B, params, rbd, tau, wrench, var, ter, drive, links, joints, contact_force, contact_flag);
 }
 
 int hb_sim_step_batch_dev(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, double* contact_force, uint8_t* contact_flag) {
   ENTER(ctx, B, params && rbd && tau && sim_params_ok(*params), UNCAPPED);
-  return sim_step(ctx, B, *params, rbd, tau, nullptr, {}, {}, MotorDrive{}, {}, contact_force, contact_flag);
+  return sim_step(ctx, B, *params, rbd, tau, nullptr, {}, {}, MotorDrive{}, {}, {}, contact_force, contact_flag);
 }
 
 int hb_default_plant_variation(hb_plant_variation* v) {
@@ -1283,6 +1285,38 @@ static bool link_variation_ok(const hb_link_variation& r) {
 int hb_rollout_set_link_variations(hb_ctx* ctx, int B, const hb_link_variation* r) {
   return set_instances(ctx, B, r, link_variation_ok, &hb_ctx::links);
 }
+
+int hb_default_joint_model(hb_joint_model* r) {
+  if (!r) return HB_EINVAL;
+  memset(r, 0, sizeof(*r));
+  const double tc = 0.02, zeta = 1.0, d_max = 0.95;     // MuJoCo's default solref (timeconst, dampratio) and solimp's d_max
+  for (int j = 0; j < NJ; ++j) { r->friction_loss[j] = 0.2; r->lower[j] = HB_JOINT_LOWER[j]; r->upper[j] = HB_JOINT_UPPER[j]; }
+  r->friction_velocity = 0.01;
+  r->stop_stiffness = 1.0 / (d_max * tc * tc * zeta * zeta);
+  r->stop_damping = 2.0 / (d_max * tc);
+  return HB_OK;
+}
+
+// The ranges of hunter_b200.h's hb_joint_model: finite f_j >= 0 and v_s > 0, bounds not NaN with lower < upper, finite gains >= 0
+static bool joint_model_ok(const hb_joint_model& r) {
+  for (int j = 0; j < NJ; ++j) {
+    if (!isfinite(r.friction_loss[j]) || !(r.friction_loss[j] >= 0.0)) return false;
+    if (isnan(r.lower[j]) || isnan(r.upper[j]) || !(r.lower[j] < r.upper[j])) return false;
+  }
+  return isfinite(r.friction_velocity) && r.friction_velocity > 0.0 && isfinite(r.stop_stiffness) && r.stop_stiffness >= 0.0 &&
+         isfinite(r.stop_damping) && r.stop_damping >= 0.0;
+}
+
+// The stability rule of hunter_b200.h's joint models for the plant params p: h (joint_damping + f_j / v_s) <= joint_armature on every joint
+// of the n records
+static bool joint_models_stable(const hb_sim_params& p, const hb_joint_model* r, int n) {
+  const double h = p.dt / p.substeps;
+  for (int i = 0; i < n; ++i)
+    for (int j = 0; j < NJ; ++j) if (!(h * (p.joint_damping + r[i].friction_loss[j] / r[i].friction_velocity) <= p.joint_armature)) return false;
+  return true;
+}
+
+int hb_rollout_set_joint_models(hb_ctx* ctx, int B, const hb_joint_model* r) { return set_instances(ctx, B, r, joint_model_ok, &hb_ctx::joints); }
 
 // The ranges of hunter_b200.h's hb_goal_schedule: the count, finite times in ascending order, finite goals
 static bool goal_schedule_ok(const hb_goal_schedule& s) {
@@ -1530,6 +1564,7 @@ int hb_check_setting_records(int32_t kind, int B, const void* records, int32_t* 
     case HB_SETTING_MOTOR_BRIDGE: return check_records(B, records, motor_bridge_ok, first_bad);
     case HB_SETTING_TELEOP: return check_records(B, records, teleop_setting_ok, first_bad);
     case HB_SETTING_LINK_VARIATIONS: return check_records(B, records, link_variation_ok, first_bad);
+    case HB_SETTING_JOINT_MODELS: return check_records(B, records, joint_model_ok, first_bad);
     case HB_SETTING_HEIGHT_MAPS: return check_records(B, records, terrain_ok, first_bad);
     case HB_SETTING_ESTIMATOR_MAPS: return check_records(B, records, terrain_ok, first_bad);
     case HB_SETTING_MPC_MAPS: return check_records(B, records, terrain_ok, first_bad);
@@ -1682,6 +1717,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
       for (int k = 0; k < c.n_cmd; ++k) if (!(c.cmd_time[k] == c.cmd_time[k]) || (k > 0 && c.cmd_time[k] < c.cmd_time[k - 1])) return false;
     }
     for (int i = 0; i < lat.n; ++i) if (lat.host[i] > p->mpc_every) return false;     // latencies beyond one MPC period
+    if (!joint_models_stable(p->sim, ctx->joints.host.data(), std::min(ctx->joints.n, B))) return false;   // joint models too stiff for the substep
     for (int i = 0; i < ctx->teleop.n; ++i) {                                          // teleop messages off the MPC ticks
       const hb_teleop_setting& s = ctx->teleop.host[i];
       if (s.period_ticks < 1 || s.period_ticks % p->mpc_every != 0) return false;
@@ -1789,7 +1825,7 @@ static int rollout_impl(hb_ctx* ctx, int B, int64_t tick0, int n_ticks, const hb
     if (!rc) rc = actuation_dev(ctx, B, p->actuation_delay, hardware, bridges, ctx->ro_tnow, act, ctx->ro_jcmd, rbd, ctx->ro_tau, ctx->ro_mcmd);
     if (!rc) rc = launch(ctx, K_UNPROFILED, rollout_saturate_kernel, (B * NJ + 127) / 128, 128, 0, B, *p, hardware, ctx->ro_tau);
     if (!rc) rc = sim_step(ctx, B, p->sim, rbd, ctx->ro_tau, wrench, ctx->variations.view(), ctx->terrains.view(), drive, ctx->links.view(),
-                           record && contacts ? ctx->ro_cforce : nullptr, record && contacts ? ctx->ro_cflag : nullptr);
+                           ctx->joints.view(), record && contacts ? ctx->ro_cforce : nullptr, record && contacts ? ctx->ro_cflag : nullptr);
     if (!rc && record) {
       for (int j = 0; j < rec.n; ++j)
         rec.dst[j] = static_cast<char*>(ctx->channels[rec.channel[j]].buf) + (size_t)(k / p->log_every) * CHANNEL_WIDTH[rec.channel[j]] * CHANNEL_BYTES[rec.channel[j]];
@@ -2409,24 +2445,30 @@ int hb_sim_step_bridge(hb_ctx* ctx, int B, const hb_sim_params* params, double* 
   return hb_sim_step_links(ctx, B, params, rbd, tau, wrench, v, ter, bridge, motor_cmd, limits, applied, nullptr, contact_force, contact_flag);
 }
 
-// the one host-pointer plant step: the five above are it with null link variations, bridges, terrains, variations and wrench
 int hb_sim_step_links(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* v,
                       const hb_terrain* ter, const hb_motor_bridge* bridge, const double* motor_cmd, const double* limits, double* applied,
                       const hb_link_variation* links, double* contact_force, uint8_t* contact_flag) {
+  return hb_sim_step_joints(ctx, B, params, rbd, tau, wrench, v, ter, bridge, motor_cmd, limits, applied, links, nullptr, contact_force, contact_flag);
+}
+
+// the one host-pointer plant step: the six above are it with null joint models, link variations, bridges, terrains, variations and wrench
+int hb_sim_step_joints(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau, const double* wrench, const hb_plant_variation* v,
+                       const hb_terrain* ter, const hb_motor_bridge* bridge, const double* motor_cmd, const double* limits, double* applied,
+                       const hb_link_variation* links, const hb_joint_model* joints, double* contact_force, uint8_t* contact_flag) {
   ENTER(ctx, B, params && rbd && (bridge ? motor_cmd && limits : tau != nullptr), CAPPED, [&] {
     if (bridge) for (size_t k = 0; k < (size_t)B * NJ; ++k) if (!(limits[k] > 0.0)) return false;
     return sim_params_ok(*params) && all_ok(B, v, plant_variation_ok) && all_ok(B, ter, terrain_ok) && all_ok(B, bridge, motor_bridge_ok) &&
-           all_ok(B, links, link_variation_ok);
+           all_ok(B, links, link_variation_ok) && all_ok(B, joints, joint_model_ok) && (!joints || joint_models_stable(*params, joints, B));
   });
   const bool br = bridge != nullptr;
   Staging s(ctx, B);
   auto r = s.inout(rbd, 32); auto t = s.in_or_null(br ? nullptr : tau, NJ); auto w = s.in_or_null(wrench, 6); auto pv = s.in_or_null(v, 1);
   auto pt = s.in_or_null(ter, 1); auto mb = s.in_or_null(bridge, 1); auto mc = s.in_or_null(br ? motor_cmd : nullptr, NJ * 5);
   auto lim = s.in_or_null(br ? limits : nullptr, NJ); auto ap = s.out(br ? applied : nullptr, NJ); auto lk = s.in_or_null(links, 1);
-  auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
+  auto jm = s.in_or_null(joints, 1); auto cf = s.out(contact_force, 12); auto fl = s.out(contact_flag, 4);
   return s.run(1, [&](Chunk) {
     const MotorDrive drive{{mb, B}, mc, lim, {}, {}, br ? (double*)ap : nullptr};
-    return sim_step(ctx, B, *params, r, t, w, {pv, B}, {pt, B}, drive, {lk, B}, cf, fl);
+    return sim_step(ctx, B, *params, r, t, w, {pv, B}, {pt, B}, drive, {lk, B}, {jm, B}, cf, fl);
   });
 }
 

@@ -681,11 +681,27 @@ __device__ __noinline__ double bridge_motor_torque(const MotorDrive& d, const hb
   return t < -lim ? -lim : (t > lim ? lim : t);
 }
 
+// Friction loss of joint j of a joint model (joint models, hunter_b200.h) at velocity v: -f_j clamp(v / v_s, -1, 1)
+__device__ __forceinline__ double joint_friction(const hb_joint_model& m, int j, double v) {
+  const double x = v / m.friction_velocity;
+  return -m.friction_loss[j] * (x < -1.0 ? -1.0 : (x > 1.0 ? 1.0 : x));
+}
+
+// The range stop of joint j of a joint model at q, v with m_jj the joint's diagonal of M + armature: 0 inside the range (and at a bound),
+// min(0, -m_jj (k r + b v)) past the upper end, max(0, m_jj (k r - b v)) past the lower end; it never pulls the joint towards the stop.
+__device__ __forceinline__ double joint_stop(const hb_joint_model& m, int j, double q, double v, double mjj) {
+  if (q > m.upper[j]) { const double t = -mjj * (m.stop_stiffness * (q - m.upper[j]) + m.stop_damping * v); return t < 0.0 ? t : 0.0; }
+  if (q < m.lower[j]) { const double t = mjj * (m.stop_stiffness * (m.lower[j] - q) - m.stop_damping * v); return t > 0.0 ? t : 0.0; }
+  return 0.0;
+}
+
 // The views are __grid_constant__ (read in place, never copied): as plain by-value parameters they cost the kernel two registers.
+// joints: the joint models of the instances that have one (joint models, hunter_b200.h); the others have no stops and no friction loss.
 __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, double* rbd_io, const double* tau, const double* wrench,
                                                       const __grid_constant__ InstanceView<hb_plant_variation> var,
                                                       const __grid_constant__ InstanceView<hb_terrain> terrain, const __grid_constant__ MotorDrive drive,
-                                                      const __grid_constant__ InstanceView<hb_link_variation> links, double* contact_force,
+                                                      const __grid_constant__ InstanceView<hb_link_variation> links,
+                                                      const __grid_constant__ InstanceView<hb_joint_model> joints, double* contact_force,
                                                       uint8_t* contact_flag) {
   __shared__ SimShared sh;
   const int inst = blockIdx.x, lane = threadIdx.x;
@@ -758,7 +774,12 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
         tj = tau[(size_t)inst * NJ + lane - 6];
       }
       if (pv && lane >= 6) tj = __dmul_rn(pv->motor_strength[lane - 6], tj);
-      double s = -sh.nle[lane] + (lane >= 6 ? tj - prm.joint_damping * sh.v[lane] : 0.0);
+      // a joint model's terms (joint models, hunter_b200.h), skipped where they do not act: the friction loss after the damping, the stop
+      // after the armature
+      const hb_joint_model* jm = lane >= 6 ? joints.of(inst) : nullptr;
+      double jt = lane >= 6 ? tj - prm.joint_damping * sh.v[lane] : 0.0;
+      if (jm && jm->friction_loss[lane - 6] != 0.0) jt += joint_friction(*jm, lane - 6, sh.v[lane]);
+      double s = -sh.nle[lane] + jt;
       for (int rr = 0; rr < 12; ++rr) s += sh.J[rr * NQ + lane] * sh.F[rr];
       if (wrench && lane < 6) {
         const double* w = wrench + (size_t)inst * 6;
@@ -770,8 +791,10 @@ __global__ void __launch_bounds__(32) sim_step_kernel(int B, hb_sim_params prm, 
           s += lane == 3 ? w[5] : (lane == 4 ? -sz * w[3] + cz * w[4] : cz * cy * w[3] + sz * cy * w[4] - sy * w[5]);
         }
       }
-      sh.rhs[lane] = s;
       if (lane >= 6) sh.M[lane * 17 + lane] += prm.joint_armature;
+      if (jm && (sh.q[lane] > jm->upper[lane - 6] || sh.q[lane] < jm->lower[lane - 6]))
+        s += joint_stop(*jm, lane - 6, sh.q[lane], sh.v[lane], sh.M[lane * 17 + lane]);
+      sh.rhs[lane] = s;
       for (int j = lane + 1; j < NQ; ++j) { const double a = 0.5 * (sh.M[lane * 17 + j] + sh.M[j * 17 + lane]); sh.M[j * 17 + lane] = a; }   // lower triangle, symmetrised
     }
     __syncwarp();

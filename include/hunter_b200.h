@@ -477,6 +477,50 @@ int hb_default_link_variation(hb_link_variation* r);      /* host only: every sc
  * mass_scale <= 0 or an inertia_scale <= 0. */
 int hb_rollout_set_link_variations(hb_ctx* ctx, int B, const hb_link_variation* r);
 
+/* ---- joint models: each robot's joint range stops and friction loss in the episodes' plant ----
+ * The reference's plants give every leg joint a range and a friction loss: mujoco/model/hunter/hunter.xml:59-124 (range, which MuJoCo 3's
+ * autolimits makes a limit constraint, and frictionloss="0.2") and legged_hunter_description/urdf/hunter_sim.urdf (<limit lower upper>,
+ * enforced by Gazebo's ODE, and <dynamics friction="0.2">). A joint model adds both to the simulated plant, per robot. Like a link
+ * variation it acts on the plant only: the planner, MPC, WBC, joint command law, actuation model, estimator and the emergency-stop check
+ * keep their behaviour and are not told about it. Record i acts on instance i of both episode calls; instances at or beyond B, and
+ * instances without a record, run the plant without these terms bit for bit.
+ * For joint j (lanes 6-15 of the plant step, coordinate 6 + j) in each substep, at the substep's q_j and v_j, after the joint torque and
+ * the viscous damping have been summed into the joint's right-hand side, s = tau_j - joint_damping v_j:
+ *   (1) friction loss, when f_j != 0: s -= f_j clamp(v_j / v_s, -1, 1), regularised Coulomb friction (the bridged joints' motor torque
+ *       takes the place of tau_j, and the term follows in the same place);
+ *   (2) the contact Jacobian's forces and the wrench are added as without a record; joint_armature is added to the diagonal of M;
+ *   (3) range stop, with m_jj the joint's diagonal entry of M + armature in this substep (a link variation's bodies included; a payload
+ *       only changes the base block): past the upper end, r = q_j - upper_j > 0, s += min(0, -m_jj (k r + b v_j)); past the lower end,
+ *       r = lower_j - q_j > 0, s += max(0, m_jj (k r - b v_j)). The stop never pulls a joint towards it (as the ground's normal force is
+ *       clipped at 0). A joint at its bound exactly (r = 0) gets no stop term.
+ * Then the step solves (M + A) qdd = rhs and integrates as before. A term whose condition is false is skipped, not added as zero, so a
+ * record with every f_j = 0 and every bound infinite (any k, b) is the plant without a record bit for bit.
+ * Stability rule: the plant integrates explicitly (semi-implicit Euler, h = sim.dt / sim.substeps), and the effective inertia of a joint is
+ * at least joint_armature (the joint block's Schur complement of M + A is at least A). Each joint's total viscous gain must therefore
+ * satisfy h (sim.joint_damping + f_j / v_s) <= sim.joint_armature. A plant step or an episode call whose sim params break this rule for
+ * any record it reads returns -1 before any launch. The stop's gains are not part of the rule: they scale with m_jj.
+ * Deviations from the reference's simulators: MuJoCo solves friction loss and limits as soft constraints in its solver, scaled by 1/A_jj of
+ * the constraint's inverse inertia; here they are explicit penalty terms scaled by m_jj. No parity with MuJoCo's solver is claimed.
+ * The setting has no state of its own (hb_episode_state_bytes does not count it) and adds no launch to an episode. */
+typedef struct {                 /* the joints of one robot's plant                                                                */
+  double friction_loss[10];      /* f_j [N m], finite, >= 0                                            (hunter.xml frictionloss: 0.2) */
+  double friction_velocity;      /* v_s [rad/s], finite, > 0: the regularisation velocity                                          */
+  double lower[10], upper[10];   /* stop range [rad], not NaN, lower < upper; -inf / +inf: no stop on that side                     */
+  double stop_stiffness;         /* k [1/s^2], finite, >= 0                                                                        */
+  double stop_damping;           /* b [1/s], finite, >= 0                                                                          */
+} hb_joint_model;                /* 264 B */
+#define HB_SETTING_JOINT_MODELS 21            /* hb_joint_model for hb_rollout_set_joint_models (hb_check_setting_records)          */
+/* host only: f_j = 0.2 (hunter.xml, hunter_sim.urdf), v_s = 0.01 rad/s, the ranges HB_JOINT_LOWER / HB_JOINT_UPPER (those of hunter.xml
+ * and hunter_sim.urdf), and k, b from MuJoCo's default solref (timeconst tc = 0.02, dampratio zeta = 1) and solimp (d_max = 0.95) past the
+ * impedance width, where MuJoCo's reference acceleration is a_ref = -b v - k r with b = 2 / (d_max tc) and k = 1 / (d_max tc^2 zeta^2)
+ * (MuJoCo documentation, Computation > Constraint model > Reference acceleration, and Modeling > Solver parameters): b = 105.26.. 1/s,
+ * k = 2631.57.. 1/s^2. At hb_default_sim_params, h (1 + 0.2 / 0.01) = 0.0105 <= 0.1. */
+int hb_default_joint_model(hb_joint_model* r);
+/* Sets the joint models of the context's episodes (a per-robot episode setting, above). -1 also for a friction loss that is not finite
+ * and >= 0, a friction_velocity that is not finite and > 0, a NaN bound, lower >= upper, a stop gain that is not finite and >= 0. The
+ * stability rule above is checked by each episode call against its params. */
+int hb_rollout_set_joint_models(hb_ctx* ctx, int B, const hb_joint_model* r);
+
 /* ---- terrain: the ground under each robot of the episodes, a height field on a regular world-frame grid ----
  * The terrain acts on the simulated plant and on the height failure check only; the planner, MPC, WBC, joint command law, actuation
  * model and estimator keep assuming flat ground at z = 0 and are not told about it. The planner can be told where the ground is by a
@@ -1158,12 +1202,19 @@ int hb_sim_step_bridge(hb_ctx* ctx, int B, const hb_sim_params* params, double* 
                        const hb_motor_bridge* bridge /*nullable*/, const double* motor_cmd, const double* limits, double* applied /*nullable*/,
                        double* contact_force /*nullable*/, uint8_t* contact_flag /*nullable*/);
 /* hb_sim_step_bridge on each robot's own bodies: links (B, nullable) = the bodies of every robot of the call (link variations, above),
- * validated as by hb_rollout_set_link_variations (-1). This is the one host-pointer plant step; hb_sim_step_bridge is it with links =
- * NULL. */
+ * validated as by hb_rollout_set_link_variations (-1). hb_sim_step_bridge is it with links = NULL. */
 int hb_sim_step_links(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau /*nullable with bridge*/,
                       const double* wrench /*nullable*/, const hb_plant_variation* v /*nullable*/, const hb_terrain* t /*nullable*/,
                       const hb_motor_bridge* bridge /*nullable*/, const double* motor_cmd, const double* limits, double* applied /*nullable*/,
                       const hb_link_variation* links /*nullable*/, double* contact_force /*nullable*/, uint8_t* contact_flag /*nullable*/);
+/* hb_sim_step_links with each robot's joint model: joints (B, nullable) = the joints of every robot of the call (joint models, above),
+ * validated as by hb_rollout_set_joint_models, and against params by the stability rule (-1 for either). This is the one host-pointer
+ * plant step; hb_sim_step_links is it with joints = NULL. */
+int hb_sim_step_joints(hb_ctx* ctx, int B, const hb_sim_params* params, double* rbd, const double* tau /*nullable with bridge*/,
+                       const double* wrench /*nullable*/, const hb_plant_variation* v /*nullable*/, const hb_terrain* t /*nullable*/,
+                       const hb_motor_bridge* bridge /*nullable*/, const double* motor_cmd, const double* limits, double* applied /*nullable*/,
+                       const hb_link_variation* links /*nullable*/, const hb_joint_model* joints /*nullable*/, double* contact_force /*nullable*/,
+                       uint8_t* contact_flag /*nullable*/);
 /* hb_sim_read_sensors_hw, and with bridge, each robot's joint readings pass its encoders (steps (3) to (5) of the motor bridge, above)
  * after the offsets and the noise. hb_sim_read_sensors_hw is it with bridge = NULL. */
 int hb_sim_read_sensors_bridge(hb_ctx* ctx, int B, const hb_sensor_noise* noise, const hb_hardware_setting* hw /*nullable*/,
